@@ -1,6 +1,6 @@
 """Same-box comparator: GPT-2 pre-training step in plain PyTorch, the way a competent user would write it today.
 
-NOT the reference (that needs OneFlow, see DESIGN.md §4) and nothing from ``libai_b200`` — only stock PyTorch pieces:
+NOT the reference (that needs OneFlow) and nothing from ``libai_b200`` — only stock PyTorch pieces:
 ``F.scaled_dot_product_attention`` (flash / cuDNN backend picked by PyTorch), ``F.layer_norm``, ``F.gelu``, cuBLAS
 matmuls under bf16 autocast, ``torch.optim.AdamW(fused=True)`` on fp32 parameters, ``DistributedDataParallel`` over
 NCCL (bucketed all-reduce overlapped with backward) when world > 1.  ``bench.py`` runs it in the same process launch

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Headline benchmark: GPT-2 pre-training throughput (tokens/s) on N B200 GPUs of one node.
+"""Headline benchmark: GPT-2 pre-training throughput (tokens/s) on N H100 GPUs of one node.
 
 Model/config = the reference's published GPT-2 benchmark (docs Benchmark.md:20-26, BASELINE.md rows
 6-8: 24 layers, hidden 1024, 16 heads, seq 1024, data parallel, micro-batch per GPU fixed → weak
@@ -18,13 +18,17 @@ the device→host loss read.
 from __future__ import annotations
 
 import argparse
+import atexit
 import json
 import os
+import shutil
 import statistics
 import subprocess
 import sys
+import tempfile
 import threading
 import time
+import zlib
 
 REPO = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, REPO)
@@ -51,6 +55,9 @@ def parse_args():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
     ap.add_argument("--steps", type=int, default=10)
+    ap.add_argument("--dump-outputs", default="", metavar="DIR",
+                    help="after the timed steps, write what the last one computed (the loss and a fixed, seeded sample of "
+                         "every updated parameter) as DIR/<name>.npy in float32")
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", default="native", choices=["native", "ref", "reference"])
     ap.add_argument("--model", default="gpt2", choices=sorted(MODELS),
@@ -117,7 +124,7 @@ def run_reference(args):
         try:
             import libai  # noqa: F401
 
-            why = "reference import succeeded but no OneFlow CUDA runtime path is wired for sm_100"
+            why = "reference import succeeded but no OneFlow CUDA runtime path is wired for sm_90a"
         except Exception as e:  # noqa
             why = f"import libai failed: {type(e).__name__}: {e}"
     print(json.dumps({"impl": "reference", "unavailable": why.replace("\n", " ")[:300]}))
@@ -260,7 +267,9 @@ def build_cfg(args, lay):
     cfg.train.amp.enabled = True
     cfg.train.evaluation.enabled = False
     cfg.train.checkpointer.period = 10 ** 9
-    cfg.train.output_dir = os.path.join(REPO, "output", "bench")
+    # the trainer writes its config dump and log there; the source tree may be read-only
+    cfg.train.output_dir = tempfile.mkdtemp(prefix="libai_b200_bench_")
+    atexit.register(shutil.rmtree, cfg.train.output_dir, ignore_errors=True)
     cfg.train.cuda_graphs.enabled = bool(args.graphs)
     cfg.train.dist.tensor_parallel_size = lay["tp"]
     cfg.train.dist.pipeline_parallel_size = lay["pp"]
@@ -276,9 +285,33 @@ def build_cfg(args, lay):
     return cfg
 
 
-def measure_native(args, lay, world, rank, local_rank, steps, warmup, with_e2e, clock_sampler=None):
+DUMP_SAMPLE = 16384   # elements per parameter in --dump-outputs (all of a smaller one); ~20 MB for GPT-2 medium
+
+
+def dump_outputs(out_dir, model, loss, rank):
+    """The arrays the timed path produced in its last step: the loss terms and, from every parameter the optimizer
+    updated, the same seeded random sample of elements on every run (float32 .npy, one file per array)."""
+    import numpy as np
+    import torch
+
+    if rank != 0:
+        return
+    os.makedirs(out_dir, exist_ok=True)
+    for k, v in sorted((loss or {}).items()):
+        np.save(os.path.join(out_dir, f"{k}.npy"), np.asarray([float(v)], dtype=np.float32))
+    for name, p in model.named_parameters():
+        flat = p.detach().reshape(-1)
+        if flat.numel() > DUMP_SAMPLE:
+            g = torch.Generator(device="cpu").manual_seed(zlib.crc32(name.encode()))
+            idx = torch.randperm(flat.numel(), generator=g)[:DUMP_SAMPLE].sort().values.to(flat.device)
+            flat = flat[idx]
+        np.save(os.path.join(out_dir, f"param.{name}.npy"), flat.float().cpu().numpy())
+
+
+def measure_native(args, lay, world, rank, local_rank, steps, warmup, with_e2e, clock_sampler=None, dump_dir=""):
     """Build the trainer for ``lay`` through the public API, time ``steps`` optimizer steps on the device (CUDA events,
-    max over ranks) and optionally the end-to-end loop through ``trainer.run_step()``."""
+    max over ranks) and optionally the end-to-end loop through ``trainer.run_step()``.  With ``dump_dir`` the outputs of
+    the last timed step are written there (before the end-to-end loop trains further)."""
     import gc
     import logging
 
@@ -388,6 +421,8 @@ def measure_native(args, lay, world, rank, local_rank, steps, warmup, with_e2e, 
     if world > 1:
         dist.all_reduce(lv, op=dist.ReduceOp.MAX)
     res["final_loss"] = float(lv) if float(lv) > -1e29 else None
+    if dump_dir:
+        dump_outputs(dump_dir, trainer.model, loss, rank)
 
     # ---- end to end through the trainer API: loader (pinned host) → H2D → step → loss D2H, every step ---------------
     if with_e2e:
@@ -581,7 +616,8 @@ def main():
 
     primary = layout_of(args, world)
     sampler = ClockSampler(local_rank) if rank == 0 else None
-    main_res = measure_native(args, primary, world, rank, local_rank, args.steps, args.warmup, not args.no_e2e, sampler)
+    main_res = measure_native(args, primary, world, rank, local_rank, args.steps, args.warmup, not args.no_e2e, sampler,
+                              args.dump_outputs)
 
     layouts = {main_res["parallelism"]: {k: main_res[k] for k in ("value", "ms_per_step", "cuda_graphs", "gpu_launches",
                                                                   "host_enqueue_ms_per_step", "global_batch")}}
@@ -616,7 +652,7 @@ def main():
                 "micro_batch_per_gpu": args.micro_batch,
                 "seq_len": args.seq,
                 "parallelism": main_res["parallelism"],
-                "l2_policy": "working set (weights+activations+optimizer state >> 126MB L2) exceeds L2 every step",
+                "l2_policy": "working set (weights+activations+optimizer state >> 50 MB L2) exceeds L2 every step",
                 "cuda_graphs": main_res["cuda_graphs"],
             },
             "clocks": main_res["clocks"],

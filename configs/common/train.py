@@ -32,7 +32,7 @@ train = dict(
     # (≈800 kernel launches per step become 48 graph launches; data-parallel and fused tensor-parallel layouts, static
     # shapes; anything else silently keeps eager launches)
     cuda_graphs=dict(enabled=True),
-    # NEW: forward GEMMs of the linear layers with E4M3 operands (per-tensor dynamic scaling, tcgen05 kind::f8f6f4,
+    # NEW: forward GEMMs of the linear layers with E4M3 operands (per-tensor dynamic scaling, wgmma e4m3,
     # fp32 accumulation, bf16 outputs); backward GEMMs stay bf16.  Opt-in: see docs/source/tutorials/basics/Kernels.md
     fp8=dict(enabled=False),
     # NEW: SIGTERM → write a resumable checkpoint at the next step boundary and stop (all ranks agree via all-reduce)

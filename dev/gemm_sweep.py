@@ -1,7 +1,6 @@
 """Tile-N sweep of the forward (NT) and dgrad (NN) GEMMs on the benchmark model's shapes: does the heuristic of
-gemm_sm100.cu (bn = 0) pick the fastest tile?  Run once per LIBAI_B200_GEMM_2CTA setting (read at first use)."""
+gemm_sm90.cu (bn = 0) pick the fastest tile?"""
 import json
-import os
 import sys
 
 import torch
@@ -30,7 +29,7 @@ def timeit(fn, iters=40, warmup=8):
 
 def main():
     ext = load_ext()
-    out = {"gemm_2cta": os.environ.get("LIBAI_B200_GEMM_2CTA", "2")}
+    out = {}
     shapes = [("fwd_qkv", 0, 8192, 3072, 1024), ("fwd_proj", 0, 8192, 1024, 1024), ("fwd_fc1", 0, 8192, 4096, 1024),
               ("fwd_fc2", 0, 8192, 1024, 4096), ("dgrad_qkv", 1, 8192, 1024, 3072), ("dgrad_proj", 1, 8192, 1024, 1024),
               ("dgrad_fc2", 1, 8192, 4096, 1024), ("dgrad_fc1", 1, 8192, 1024, 4096)]

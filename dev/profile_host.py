@@ -1,7 +1,7 @@
 """Host-side profile (cProfile) of a few training steps of a bench layout: where does the enqueue time go?
 
     python -m torch.distributed.run --nproc-per-node 2 --master-addr 127.0.0.1 dev/profile_host.py --layout tp2
-writes gpurun_out/host_profile_<layout>_rank<r>.txt"""
+writes output/host_profile_<layout>_rank<r>.txt"""
 import argparse
 import cProfile
 import io
@@ -61,15 +61,15 @@ def main():
     bench.time = types.SimpleNamespace(perf_counter=hooked, sleep=_time.sleep, time=_time.time)
     res = bench.measure_native(args, lay, world, rank, local_rank, a.steps, 4, False)
     bench.time = _time
-    os.makedirs(os.path.join(REPO, "gpurun_out"), exist_ok=True)
+    os.makedirs(os.path.join(REPO, "output"), exist_ok=True)
     if tprof is not None:
         table = tprof.key_averages().table(sort_by="cuda_time_total", row_limit=45, max_name_column_width=90)
-        with open(os.path.join(REPO, "gpurun_out", f"device_profile_{a.layout}_rank{rank}.txt"), "w") as f:
+        with open(os.path.join(REPO, "output", f"device_profile_{a.layout}_rank{rank}.txt"), "w") as f:
             f.write(f"{res}\nsteps profiled: {a.steps}\n\n{table}")
     else:
         buf = io.StringIO()
         pstats.Stats(prof, stream=buf).sort_stats("cumulative").print_stats(70)
-        with open(os.path.join(REPO, "gpurun_out", f"host_profile_{a.layout}_rank{rank}.txt"), "w") as f:
+        with open(os.path.join(REPO, "output", f"host_profile_{a.layout}_rank{rank}.txt"), "w") as f:
             f.write(f"{res}\n\n{buf.getvalue()}")
     if rank == 0:
         print(res)

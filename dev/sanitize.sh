@@ -1,5 +1,5 @@
 #!/usr/bin/env bash
-# compute-sanitizer passes over the native kernels (needs a B200; run through gpurun).
+# compute-sanitizer passes over the native kernels (needs an H100).
 #   bash dev/sanitize.sh [memcheck|racecheck|synccheck|initcheck] [kernel-check name prefixes, comma separated]
 # Each tool runs tests/gpu_kernel_check.py (every kernel against its fp32 reference) in --quick mode; racecheck and
 # synccheck look at the shared-memory pipelines (mbarrier / TMA rings, epilogue staging slots), memcheck at global and
@@ -7,9 +7,9 @@
 set -euo pipefail
 TOOL=${1:-memcheck}
 ONLY=${2:-}
-OUT=gpurun_out/sanitize_${TOOL}.log
-mkdir -p gpurun_out
-ARGS=(--quick --out gpurun_out/sanitize_kernel_check.json)
+OUT=output/sanitize_${TOOL}.log
+mkdir -p output
+ARGS=(--quick --out output/sanitize_kernel_check.json)
 if [ -n "$ONLY" ]; then ARGS+=(--only "$ONLY"); fi
 timeout 1500 compute-sanitizer --tool "$TOOL" --error-exitcode 9 --print-limit 20 \
   python tests/gpu_kernel_check.py "${ARGS[@]}" > "$OUT" 2>&1 || echo "compute-sanitizer exit code $?"

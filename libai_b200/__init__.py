@@ -1,4 +1,4 @@
-"""libai_b200 — a Blackwell (sm_100a) native large-model training toolbox.
+"""libai_b200 — a Hopper (sm_90a) native large-model training toolbox.
 
 Same user-facing surface as LiBai (LazyConfig configs, DefaultTrainer, parallel layers, model
 zoo) on PyTorch + hand-written CUDA kernels + NCCL/NVLink.

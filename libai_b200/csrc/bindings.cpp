@@ -40,16 +40,19 @@ int lb_rope_qkv(const void* x, const float* cosv, const float* sinv, void* y, lo
                 int pos_offset, int backward, cudaStream_t s);
 int lb_rope(const void* x, const float* cosv, const float* sinv, void* y, long rows, int S, int D, int backward,
             cudaStream_t s);
-int lb_colsum(const void* x, float* out, int M, int N, int accumulate, cudaStream_t s);
+int lb_colsum_workspace_rows(int M, int N);
+int lb_colsum(const void* x, float* out, int M, int N, int accumulate, float* workspace, cudaStream_t s);
 int lb_embedding_fwd(const int64_t* ids, const void* table, void* out, long T, int H, long vocab_start, long rows, cudaStream_t s);
-int lb_embedding_bwd(const int64_t* ids, const void* gy, float* grad, long T, int H, long vocab_start, long rows, cudaStream_t s);
+int lb_embedding_bwd(const int64_t* sorted_ids, const int64_t* order, const void* gy, float* grad, long T, int H,
+                     long vocab_start, long rows, cudaStream_t s);
 int lb_ce_stats(const void* logits, const int64_t* labels, float* mx, float* se, float* tgt, int T, int V,
                 long vocab_start, int dtype, cudaStream_t s);
 int lb_ce_bwd(const void* logits, const int64_t* labels, const float* lse, const float* gloss, void* dlogits, int T,
               int V, long vocab_start, int dtype, cudaStream_t s);
 int lb_adamw(float* master, const float* grad, float* m, float* v, void* lp_out, const float* scale, long n, float lr,
              float b1, float b2, float eps, float wd, float bc1, float bc2, int decoupled, cudaStream_t s);
-int lb_sqnorm(const float* x, float* out, long n, cudaStream_t s);
+int lb_sqnorm_workspace(long n);
+int lb_sqnorm(const float* x, float* out, long n, float* workspace, cudaStream_t s);
 int lb_gemm_bf16_comm(const void* a, const void* b, void* out, int M, int N, int K, int layout, int epi,
                       const void* bias, int act, void* pre_out, const void* pre_in, float* colsum, int mode,
                       int world, int rank, const long* peer_buf, const long* peer_flags, const long* peer_done,
@@ -81,7 +84,7 @@ int lb_attn_bwd(const void* dout, const void* q, const void* k, const void* v, c
                 void* dq, void* dk, void* dv, float* delta, float* dq_accum, int B, int A, int S, int D,
                 const long* q_strides, const long* k_strides, const long* v_strides, const long* do_strides, int causal,
                 float scale, const int* kv_lens, const void* bias, const long* bias_strides, const float* alibi_slopes,
-                float* dbias, float p_drop, const long long* rng_state, cudaStream_t s);
+                float* dbias, float p_drop, const long long* rng_state, unsigned* dq_order, cudaStream_t s);
 int lb_bias_dropout_residual(const void* x, const void* bias, const void* res, void* y, long rows, int N, float p,
                              const LbRngArgs* rng, const long long* rng_in, long long* rng_out, cudaStream_t s);
 }
@@ -162,8 +165,14 @@ Tensor dgrad_actgrad(const Tensor& gy, const Tensor& w, const Tensor& pre, int64
     colsum = bias_grad->data_ptr<float>();
   }
   check(lb_gemm_bf16_actgrad(gy.data_ptr(), w.data_ptr(), out.data_ptr(), (int)M, (int)N, (int)K, (int)gy.stride(0),
-                             (int)w.stride(0), (int)N, 1, (int)act, pre.data_ptr(), colsum, cur_stream()),
+                             (int)w.stride(0), (int)N, 1, (int)act, pre.data_ptr(), nullptr, cur_stream()),
         "dgrad_actgrad");
+  // the bias gradient = column sums of the stored output, in a fixed summation order (the GEMM epilogue's per-tile
+  // reductions would arrive in scheduling order)
+  if (colsum != nullptr) {
+    Tensor ws = at::empty({(int64_t)lb_colsum_workspace_rows((int)M, (int)N) * N}, gy.options().dtype(at::kFloat));
+    check(lb_colsum(out.data_ptr(), colsum, (int)M, (int)N, 1, ws.data_ptr<float>(), cur_stream()), "dgrad_actgrad colsum");
+  }
   return out;
 }
 
@@ -307,8 +316,10 @@ void embedding_bwd(const Tensor& ids, const Tensor& gy, Tensor grad, int64_t voc
               "embedding_bwd: gy must be contiguous bf16 [ids.numel(), H]");
   TORCH_CHECK(grad.dim() == 2 && grad.is_contiguous() && grad.scalar_type() == at::kFloat && grad.size(1) == gy.size(1),
               "embedding_bwd: grad must be contiguous fp32 [rows, H]");
-  check(lb_embedding_bwd(ids.data_ptr<int64_t>(), gy.data_ptr(), grad.data_ptr<float>(), (long)ids.numel(), (int)gy.size(1),
-                         (long)vocab_start, (long)grad.size(0), cur_stream()),
+  const auto sorted = at::sort(ids.reshape({-1}), /*stable=*/true, /*dim=*/0, /*descending=*/false);
+  check(lb_embedding_bwd(std::get<0>(sorted).data_ptr<int64_t>(), std::get<1>(sorted).data_ptr<int64_t>(), gy.data_ptr(),
+                         grad.data_ptr<float>(), (long)ids.numel(), (int)gy.size(1), (long)vocab_start, (long)grad.size(0),
+                         cur_stream()),
         "embedding_bwd");
 }
 
@@ -318,11 +329,18 @@ Tensor colsum(const Tensor& x, const c10::optional<Tensor>& accum) {
   if (accum.has_value() && accum->defined()) {
     TORCH_CHECK(accum->scalar_type() == at::kFloat && accum->numel() == x.size(1) && accum->is_contiguous(),
                 "colsum: accum must be contiguous fp32 [N]");
-    check(lb_colsum(x.data_ptr(), accum->data_ptr<float>(), (int)x.size(0), (int)x.size(1), 1, cur_stream()), "colsum");
+    Tensor ws = at::empty({(int64_t)lb_colsum_workspace_rows((int)x.size(0), (int)x.size(1)) * x.size(1)},
+                          x.options().dtype(at::kFloat));
+    check(lb_colsum(x.data_ptr(), accum->data_ptr<float>(), (int)x.size(0), (int)x.size(1), 1, ws.data_ptr<float>(),
+                    cur_stream()),
+          "colsum");
     return at::empty({0}, x.options());
   }
   Tensor out = at::empty({x.size(1)}, x.options().dtype(at::kFloat));
-  check(lb_colsum(x.data_ptr(), out.data_ptr<float>(), (int)x.size(0), (int)x.size(1), 0, cur_stream()), "colsum");
+  Tensor ws = at::empty({(int64_t)lb_colsum_workspace_rows((int)x.size(0), (int)x.size(1)) * x.size(1)},
+                        x.options().dtype(at::kFloat));
+  check(lb_colsum(x.data_ptr(), out.data_ptr<float>(), (int)x.size(0), (int)x.size(1), 0, ws.data_ptr<float>(), cur_stream()),
+        "colsum");
   return out.to(at::kBFloat16);
 }
 
@@ -503,7 +521,8 @@ void fused_adamw(Tensor master, const Tensor& grad, Tensor m, Tensor v, const c1
 Tensor sqnorm(const Tensor& x) {
   c10::cuda::CUDAGuard guard(x.device());
   Tensor out = at::zeros({1}, x.options().dtype(at::kFloat));
-  check(lb_sqnorm(x.data_ptr<float>(), out.data_ptr<float>(), x.numel(), cur_stream()), "sqnorm");
+  Tensor ws = at::empty({(int64_t)lb_sqnorm_workspace(x.numel())}, x.options().dtype(at::kFloat));
+  check(lb_sqnorm(x.data_ptr<float>(), out.data_ptr<float>(), x.numel(), ws.data_ptr<float>(), cur_stream()), "sqnorm");
   return out;
 }
 
@@ -635,6 +654,8 @@ std::tuple<Tensor, Tensor, Tensor, Tensor> attn_bwd(const Tensor& dout, const Te
   Tensor dv = dqkv.select(3, 2).permute({0, 2, 1, 3});
   Tensor delta = at::empty({B, A, S}, q.options().dtype(at::kFloat));
   Tensor dq_acc = at::empty({B, A, S, D}, q.options().dtype(at::kFloat));   // cleared by the delta kernel
+  // per (batch, head, 64-query block): key blocks that have added their dQ contribution
+  Tensor dq_order = at::zeros({B * A * ((S + 63) / 64)}, q.options().dtype(at::kInt));
   TORCH_CHECK(o.stride(3) == 1, "attn_bwd: o must have contiguous D");
   Tensor dout_c = dout;
   if (dout.strides() != o.strides()) {  // bring dout into the [B, S, A, D]-backed layout of o
@@ -659,7 +680,8 @@ std::tuple<Tensor, Tensor, Tensor, Tensor> attn_bwd(const Tensor& dout, const Te
                     (kv_lens.has_value() && kv_lens->defined()) ? kv_lens->data_ptr<int>() : nullptr, bd.ptr, bd.strides,
                     (alibi_slopes.has_value() && alibi_slopes->defined()) ? alibi_slopes->data_ptr<float>() : nullptr, dbp,
                     (float)(has_rng ? p_drop : 0.0),
-                    has_rng ? reinterpret_cast<const long long*>(rng_state->data_ptr<int64_t>()) : nullptr, cur_stream()),
+                    has_rng ? reinterpret_cast<const long long*>(rng_state->data_ptr<int64_t>()) : nullptr,
+                    reinterpret_cast<unsigned*>(dq_order.data_ptr<int>()), cur_stream()),
         "attn_bwd");
   return std::make_tuple(dq, dk, dv, dqkv);
 }

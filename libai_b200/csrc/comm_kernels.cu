@@ -213,7 +213,7 @@ p2p_allgather_push_kernel(const uint4* __restrict__ shard, PeerPtrs outs, PeerPt
 
 namespace {
 int comm_grid(size_t work) {
-  int dev = 0, sms = 148;
+  int dev = 0, sms = 132;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   size_t need = (work + 255) / 256;

@@ -1,4 +1,4 @@
-// Shared device helpers for the sm_100a kernels: mbarrier, TMA, tcgen05 / TMEM PTX wrappers.
+// Shared device helpers for the sm_90a kernels: mbarrier, TMA, wgmma PTX wrappers.
 // Everything is inline PTX (no CUTLASS dependency) so the kernels compile in seconds.
 #pragma once
 #include <cuda.h>
@@ -6,6 +6,8 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdio.h>
+
+#include "wgmma.cuh"
 
 namespace lb {
 
@@ -28,7 +30,7 @@ LB_DEVICE bool elect_one() {
 
 // ---------------------------------------------------------------------------------------------
 // cross-GPU flag waits (NVLink peer memory).  Every wait is BOUNDED: a dead or wedged peer must not hang the GPU
-// forever (SURVEY §5.3) — after `timeout_ns` the waiter prints who/what it was waiting for and traps, which surfaces
+// forever — after `timeout_ns` the waiter prints who/what it was waiting for and traps, which surfaces
 // as a CUDA error on the host (the trainer's emergency path / the launcher's restart then take over).
 // ---------------------------------------------------------------------------------------------
 LB_DEVICE unsigned long long globaltimer_ns() {
@@ -184,185 +186,34 @@ LB_DEVICE void tma_store_wait() {
 }
 
 // ---------------------------------------------------------------------------------------------
-// tcgen05 / TMEM
+// wgmma (warpgroup MMA, accumulators in registers)
 // ---------------------------------------------------------------------------------------------
-template <uint32_t kCols>
-LB_DEVICE void tmem_alloc(uint32_t* smem_result) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;\n" ::"r"(smem_u32(smem_result)),
-               "n"(kCols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;\n" ::: "memory");
+LB_DEVICE void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;\n" ::: "memory"); }
+LB_DEVICE void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;\n" ::: "memory"); }
+template <int N>
+LB_DEVICE void wgmma_wait() {
+  asm volatile("wgmma.wait_group.sync.aligned %0;\n" ::"n"(N) : "memory");
 }
-template <uint32_t kCols>
-LB_DEVICE void tmem_dealloc(uint32_t taddr) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;\n" ::"r"(taddr), "n"(kCols) : "memory");
+// keeps the compiler from moving accumulator reads / writes across an in-flight wgmma
+template <int R>
+LB_DEVICE void wgmma_fence_regs(float (&d)[R]) {
+#pragma unroll
+  for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
-LB_DEVICE void tc_fence_before_sync() { asm volatile("tcgen05.fence::before_thread_sync;\n" ::: "memory"); }
-LB_DEVICE void tc_fence_after_sync() { asm volatile("tcgen05.fence::after_thread_sync;\n" ::: "memory"); }
+// named barrier over the 128 threads of one warpgroup (ids 1..4 are reserved for this)
+LB_DEVICE void warpgroup_sync(int wg) { asm volatile("bar.sync %0, 128;\n" ::"r"(wg + 1) : "memory"); }
 
-// ---- CTA pair (cta_group::2): two SMs of one TPC work on one 256-row tile.  Each CTA stages its own 128 rows of A and
-// HALF of the B tile in shared memory; the MMA (issued by the leader CTA only) reads both halves, each CTA's TMEM
-// receives the accumulator rows of its own 128 rows.  PTX forms as in cute/arch/{mma_sm100_umma,copy_sm100_tma,
-// tmem_allocator_sm100}.hpp and cutlass/arch/barrier.h of the vendored CUTLASS headers.
-LB_DEVICE uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;\n" : "=r"(r));
-  return r;
-}
-LB_DEVICE void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;\n" ::: "memory");
-  asm volatile("barrier.cluster.wait.acquire.aligned;\n" ::: "memory");
-}
-template <uint32_t kCols>
-LB_DEVICE void tmem_alloc_2cta(uint32_t* smem_result) {
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;\n" ::"r"(smem_u32(smem_result)),
-               "n"(kCols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;\n" ::: "memory");
-}
-template <uint32_t kCols>
-LB_DEVICE void tmem_dealloc_2cta(uint32_t taddr) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;\n" ::"r"(taddr), "n"(kCols) : "memory");
-}
-// arrive (count 1) on the mbarrier at the same shared-memory offset in CTA `cta` of the cluster (the form CUTLASS'
-// ClusterBarrier::arrive(cta_id) uses; an explicit `.release.cluster` compiles to MEMBAR.ALL.GPU + ERRBAR per arrival,
-// which throttled the peer's TMA producer to one k-block per fence: profiles/r2_10_ncu_gemm_2cta_first.txt)
-LB_DEVICE void mbar_arrive_cluster(uint64_t* bar, uint32_t cta) {
-  asm volatile(
-      "{\n\t.reg .b32 ra;\n\t"
-      "mapa.shared::cluster.u32 ra, %0, %1;\n\t"
-      "mbarrier.arrive.shared::cluster.b64 _, [ra];\n\t}\n" ::"r"(smem_u32(bar)),
-      "r"(cta)
-      : "memory");
-}
-// 2-D tiled TMA load issued by either CTA of a pair; the transaction bytes are credited to the mbarrier of the EVEN
-// (leader) CTA at the same offset (peer bit of the shared::cluster address cleared)
-LB_DEVICE void tma_load_2d_2cta(void* smem_dst, const CUtensorMap* map, uint64_t* bar, int32_t c0, int32_t c1) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];\n" ::"r"(
-          smem_u32(smem_dst)),
-      "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar) & 0xFEFFFFFFu), "r"(c0), "r"(c1)
-      : "memory");
-}
-LB_DEVICE void umma_f16_ss_2cta(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, {%5, %5, %5, %5, %5, %5, %5, %5}, p;\n\t}\n" ::"r"(tmem_d),
-      "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate), "r"(0u)
-      : "memory");
-}
-// arrive on the mbarrier at this offset in BOTH CTAs of the pair once all previously issued MMAs have completed
-LB_DEVICE void umma_commit_2cta(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;\n" ::"r"(
-                   smem_u32(bar)),
-               "h"(static_cast<uint16_t>(3))
-               : "memory");
-}
-
-// D[tmem] (+)= A[smem desc] * B[smem desc], bf16/fp16 inputs, fp32 accumulate; one thread issues.
-LB_DEVICE void umma_f16_ss(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}\n" ::"r"(tmem_d),
-      "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// 8-bit float operands (E4M3/E5M2 selected by the instruction descriptor), 32 elements of K per instruction
-LB_DEVICE void umma_f8_ss(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f8f6f4 [%0], %1, %2, %3, p;\n\t}\n" ::"r"(tmem_d),
-      "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// A operand from TMEM (used by attention: P stays in tensor memory)
-LB_DEVICE void umma_f16_ts(uint32_t tmem_d, uint32_t tmem_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t}\n" ::"r"(tmem_d),
-      "r"(tmem_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// arrive on an mbarrier once all previously issued tcgen05.mma of this thread have completed
-LB_DEVICE void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];\n" ::"r"(smem_u32(bar))
-               : "memory");
-}
-
-// 32 lanes x 32 consecutive 32-bit columns -> 32 registers per thread (thread i <-> TMEM lane base+i)
-LB_DEVICE void tmem_ld_32x32b_x32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];\n"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
-LB_DEVICE void tmem_ld_32x32b_x16(uint32_t taddr, uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];\n"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-}
-LB_DEVICE void tmem_st_32x32b_x16(uint32_t taddr, const uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};\n" ::"r"(taddr),
-      "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]), "r"(r[9]),
-      "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15])
-      : "memory");
-}
-LB_DEVICE void tmem_st_32x32b_x32(uint32_t taddr, const uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-      "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};\n" ::"r"(taddr),
-      "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]), "r"(r[9]),
-      "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15]), "r"(r[16]), "r"(r[17]), "r"(r[18]),
-      "r"(r[19]), "r"(r[20]), "r"(r[21]), "r"(r[22]), "r"(r[23]), "r"(r[24]), "r"(r[25]), "r"(r[26]), "r"(r[27]),
-      "r"(r[28]), "r"(r[29]), "r"(r[30]), "r"(r[31])
-      : "memory");
-}
-LB_DEVICE void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;\n" ::: "memory"); }
-LB_DEVICE void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;\n" ::: "memory"); }
-
-// ---------------------------------------------------------------------------------------------
-// UMMA descriptors (bit layout: cute/arch/mma_sm100_desc.hpp)
-// ---------------------------------------------------------------------------------------------
-// shared-memory matrix descriptor, 128-byte swizzle, dense tiles whose rows are 128 bytes:
-//   start address [0,14) (>>4), LBO [16,30) (>>4), SBO [32,46) (>>4), version=1 [46,48), layout=2 (SW128) [61,64)
+// shared-memory matrix descriptor for wgmma, 128-byte swizzle (bit layout: PTX ISA "Matrix Descriptor Format"):
+//   start address [0,14) (>>4), LBO [16,30) (>>4), SBO [32,46) (>>4), layout = 1 (128B swizzle) [62,64)
+// K-major tiles (rows of 64 bf16 = 128 bytes): SBO = 1024 (8-row groups), advance 32 bytes per 16 elements of K.
+// MN-major tiles (64-element MN atoms, one 128-byte row per k): LBO = distance between MN atoms, SBO = 1024.
 LB_DEVICE uint64_t make_smem_desc_sw128(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
   uint64_t d = 0;
   d |= static_cast<uint64_t>((smem_addr & 0x3FFFF) >> 4);
   d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFF) << 16;
   d |= static_cast<uint64_t>((sbo_bytes >> 4) & 0x3FFF) << 32;
-  d |= static_cast<uint64_t>(1) << 46;
-  d |= static_cast<uint64_t>(2) << 61;
+  d |= static_cast<uint64_t>(1) << 62;
   return d;
-}
-
-// instruction descriptor for kind::f16 with bf16 inputs and fp32 accumulation
-//   c_format=F32 (1) [4,6), a_format=BF16 (1) [7,10), b_format=BF16 (1) [10,13),
-//   a_major [15], b_major [16] (0 = K-major, 1 = MN-major), N>>3 [17,23), M>>4 [24,29)
-__host__ __device__ constexpr uint32_t make_idesc_bf16(uint32_t m, uint32_t n, bool a_mn_major, bool b_mn_major) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | ((a_mn_major ? 1u : 0u) << 15) | ((b_mn_major ? 1u : 0u) << 16) |
-         ((n >> 3) << 17) | ((m >> 4) << 24);
-}
-
-// kind::f8f6f4 with E4M3 x E4M3 inputs (a_format = b_format = 0), fp32 accumulation, both operands K-major
-__host__ __device__ constexpr uint32_t make_idesc_e4m3(uint32_t m, uint32_t n) {
-  return (1u << 4) | ((n >> 3) << 17) | ((m >> 4) << 24);
 }
 
 // ---------------------------------------------------------------------------------------------

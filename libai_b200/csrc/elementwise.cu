@@ -1,4 +1,4 @@
-// Bandwidth-bound fused kernels for sm_100a: bias+activation (fwd/bwd), bias+residual, SwiGLU,
+// Bandwidth-bound fused kernels for sm_90a: bias+activation (fwd/bwd), bias+residual, SwiGLU,
 // RoPE, column sums (bias gradients), vocab-parallel softmax cross entropy (stats + backward),
 // fused AdamW over flat buffers, squared-norm reduction.  All use 128-bit accesses and grid-stride
 // loops sized to the SM count.
@@ -260,10 +260,10 @@ __global__ void rope_qkv_kernel(const __nv_bfloat16* __restrict__ x, const float
   }
 }
 
-// out[c] += sum_r x[r, c]: block = 32 column lanes (8 columns each, 16-byte loads) x 8 row stripes; the stripes are
-// combined in shared memory so that a block issues one atomic per column (the first version issued one per thread
-// and serialised on 256-way contended addresses).
-__global__ void __launch_bounds__(256) colsum_vec_kernel(const __nv_bfloat16* __restrict__ x, float* __restrict__ out,
+// part[blockIdx.y, c] = sum over the block's rows of x[r, c]: block = 32 column lanes (8 columns each, 16-byte loads) x
+// 8 row stripes combined in shared memory.  The partials are summed in a fixed order by colsum_partials_kernel, so the
+// result does not depend on the order in which blocks finish.
+__global__ void __launch_bounds__(256) colsum_vec_kernel(const __nv_bfloat16* __restrict__ x, float* __restrict__ part,
                                                          int M, int N, int rows_per_block) {
   __shared__ float sm[8][32][9];
   const int tx = threadIdx.x % 32, ty = threadIdx.x / 32;
@@ -301,12 +301,12 @@ __global__ void __launch_bounds__(256) colsum_vec_kernel(const __nv_bfloat16* __
     float t = 0.f;
 #pragma unroll
     for (int j = 0; j < 8; ++j) t += sm[j][col / 8][col % 8];
-    atomicAdd(out + gcol, t);
+    part[static_cast<size_t>(blockIdx.y) * N + gcol] = t;
   }
 }
 
-// out[c] += sum_r x[r, c]   (out fp32, zero-initialised by the caller)
-__global__ void colsum_kernel(const __nv_bfloat16* __restrict__ x, float* __restrict__ out, int M, int N,
+// part[blockIdx.y, c] = sum over the block's rows of x[r, c]  (any even N)
+__global__ void colsum_kernel(const __nv_bfloat16* __restrict__ x, float* __restrict__ part, int M, int N,
                               int rows_per_block) {
   const int c2 = blockIdx.x * blockDim.x + threadIdx.x;  // pair of columns
   if (c2 * 2 >= N) return;
@@ -318,8 +318,26 @@ __global__ void colsum_kernel(const __nv_bfloat16* __restrict__ x, float* __rest
     a0 += v.x;
     a1 += v.y;
   }
-  atomicAdd(out + c2 * 2, a0);
-  atomicAdd(out + c2 * 2 + 1, a1);
+  part[static_cast<size_t>(blockIdx.y) * N + c2 * 2] = a0;
+  part[static_cast<size_t>(blockIdx.y) * N + c2 * 2 + 1] = a1;
+}
+
+// out[c] (+)= sum_b part[b, c], b in increasing order (one thread per column: coalesced, deterministic)
+__global__ void __launch_bounds__(256) colsum_partials_kernel(const float* __restrict__ part, float* __restrict__ out,
+                                                              int nparts, int N, int accumulate) {
+  const int c = blockIdx.x * blockDim.x + threadIdx.x;
+  if (c >= N) return;
+  float t = 0.f;
+  for (int b = 0; b < nparts; ++b) t += part[static_cast<size_t>(b) * N + c];
+  out[c] = accumulate ? out[c] + t : t;
+}
+
+// out[0] += sum of part[0, n): each lane sums a fixed stride, then a fixed shuffle tree (one warp)
+__global__ void sum_partials_kernel(const float* __restrict__ part, int n, float* __restrict__ out) {
+  float acc = 0.f;
+  for (int i = threadIdx.x; i < n; i += 32) acc += part[i];
+  acc = warp_sum(acc);
+  if (threadIdx.x == 0) out[0] += acc;
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -477,7 +495,8 @@ __global__ void adamw_kernel(float* __restrict__ master, const float* __restrict
 }
 
 // out[0] += sum x^2
-__global__ void sqnorm_kernel(const float* __restrict__ x, float* __restrict__ out, size_t n) {
+// part[blockIdx.x] = sum of x[i]^2 over the block's grid-stride slice (summed in order by sum_partials_kernel)
+__global__ void sqnorm_kernel(const float* __restrict__ x, float* __restrict__ part, size_t n) {
   __shared__ float sm[32];
   float acc = 0.f;
   const size_t nvec = n / 4;
@@ -494,7 +513,7 @@ __global__ void sqnorm_kernel(const float* __restrict__ x, float* __restrict__ o
   if (threadIdx.x < 32) {
     float t = threadIdx.x < blockDim.x / 32 ? sm[threadIdx.x] : 0.f;
     t = warp_sum(t);
-    if (threadIdx.x == 0) atomicAdd(out, t);
+    if (threadIdx.x == 0) part[blockIdx.x] = t;
   }
 }
 
@@ -510,20 +529,31 @@ __global__ void __launch_bounds__(128) embedding_fwd_kernel(const int64_t* __res
   for (int i = threadIdx.x; i < H / 8; i += blockDim.x) dst[i] = inside ? src[i] : make_uint4(0, 0, 0, 0);
 }
 
-// grad_table[ids[t] - vocab_start, :] += gy[t, :]   (fp32 main-grad buffer, vector reductions: no sort, no temporary,
-// and the tied LM-head wgrad accumulates into the same buffer)
-__global__ void __launch_bounds__(128) embedding_bwd_kernel(const int64_t* __restrict__ ids, const __nv_bfloat16* __restrict__ gy,
-                                                            float* __restrict__ grad, int H, long vocab_start, long rows) {
+// grad_table[ids[t] - vocab_start, :] += gy[t, :]   (fp32 main-grad buffer; the tied LM-head wgrad accumulates into the
+// same buffer).  The ids arrive sorted (stable) with their token positions: the block of the first token of every run
+// of equal ids sums the run in token order and is the only writer of that row, so the result is deterministic.
+__global__ void __launch_bounds__(128) embedding_bwd_kernel(const int64_t* __restrict__ sorted_ids,
+                                                            const int64_t* __restrict__ order,
+                                                            const __nv_bfloat16* __restrict__ gy, float* __restrict__ grad,
+                                                            long T, int H, long vocab_start, long rows) {
   const long t = blockIdx.x;
-  const long r = ids[t] - vocab_start;
+  const int64_t id = sorted_ids[t];
+  if (t > 0 && sorted_ids[t - 1] == id) return;
+  const long r = id - vocab_start;
   if (r < 0 || r >= rows) return;
-  const uint4* src = reinterpret_cast<const uint4*>(gy + t * H);
   float* dst = grad + r * H;
   for (int i = threadIdx.x; i < H / 8; i += blockDim.x) {
-    const uint4 q = src[i];
-    const float2 a = unpack_bf16(q.x), b = unpack_bf16(q.y), c = unpack_bf16(q.z), d = unpack_bf16(q.w);
-    asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};\n" ::"l"(dst + i * 8), "f"(a.x), "f"(a.y), "f"(b.x), "f"(b.y) : "memory");
-    asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};\n" ::"l"(dst + i * 8 + 4), "f"(c.x), "f"(c.y), "f"(d.x), "f"(d.y) : "memory");
+    float acc[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+    for (long u = t; u < T && sorted_ids[u] == id; ++u) {
+      const uint4 q = reinterpret_cast<const uint4*>(gy + order[u] * H)[i];
+      const float2 a = unpack_bf16(q.x), b = unpack_bf16(q.y), c = unpack_bf16(q.z), d = unpack_bf16(q.w);
+      acc[0] += a.x; acc[1] += a.y; acc[2] += b.x; acc[3] += b.y;
+      acc[4] += c.x; acc[5] += c.y; acc[6] += d.x; acc[7] += d.y;
+    }
+    float4* d4 = reinterpret_cast<float4*>(dst + i * 8);
+    const float4 o0 = d4[0], o1 = d4[1];
+    d4[0] = make_float4(o0.x + acc[0], o0.y + acc[1], o0.z + acc[2], o0.w + acc[3]);
+    d4[1] = make_float4(o1.x + acc[4], o1.y + acc[5], o1.z + acc[6], o1.w + acc[7]);
   }
 }
 
@@ -531,7 +561,7 @@ __global__ void __launch_bounds__(128) embedding_bwd_kernel(const int64_t* __res
 
 namespace {
 int ew_grid(size_t work, int block) {
-  int dev = 0, sms = 148;
+  int dev = 0, sms = 132;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   size_t need = (work + block - 1) / block;
@@ -626,23 +656,38 @@ extern "C" int lb_rope_qkv(const void* x, const float* cosv, const float* sinv, 
       (const bf16*)x, cosv, sinv, (bf16*)y, (size_t)heads, S, A, D, pos_offset, backward, copy_v);
   return (int)cudaGetLastError();
 }
-extern "C" int lb_colsum(const void* x, float* out, int M, int N, int accumulate, cudaStream_t s) {
+// rows per block of the column-sum pass; the number of row blocks is the row count of its fp32 workspace [.., N]
+static int colsum_rows_per_block(int M, int N) {
+  if (N % 8) return 128;
+  int dev = 0, sms = 0;
+  cudaGetDevice(&dev);
+  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+  const int col_blocks = (N + 255) / 256;
+  int row_blocks = (2 * sms + col_blocks - 1) / col_blocks;  // ~2 blocks per SM
+  if (row_blocks > (M + 63) / 64) row_blocks = (M + 63) / 64;
+  if (row_blocks < 1) row_blocks = 1;
+  return (M + row_blocks - 1) / row_blocks;
+}
+extern "C" int lb_colsum_workspace_rows(int M, int N) {
+  if (M <= 0) return 1;
+  const int rpb = colsum_rows_per_block(M, N);
+  return (M + rpb - 1) / rpb;
+}
+// out[c] (+)= sum_r x[r, c]; workspace: fp32 [lb_colsum_workspace_rows(M, N), N]
+extern "C" int lb_colsum(const void* x, float* out, int M, int N, int accumulate, float* workspace, cudaStream_t s) {
   if (N % 2) return -1;
-  if (!accumulate) cudaMemsetAsync(out, 0, sizeof(float) * N, s);
-  if (M == 0) return 0;
-  if (N % 8 == 0) {
-    const int col_blocks = (N + 255) / 256;
-    int row_blocks = (2 * 148 + col_blocks - 1) / col_blocks;  // ~2 blocks per SM
-    if (row_blocks > (M + 63) / 64) row_blocks = (M + 63) / 64;
-    if (row_blocks < 1) row_blocks = 1;
-    const int rpb = (M + row_blocks - 1) / row_blocks;
-    dim3 grid(col_blocks, (M + rpb - 1) / rpb);
-    lb::colsum_vec_kernel<<<grid, 256, 0, s>>>((const bf16*)x, out, M, N, rpb);
-    return (int)cudaGetLastError();
+  if (M == 0) {
+    if (!accumulate) cudaMemsetAsync(out, 0, sizeof(float) * N, s);
+    return 0;
   }
-  const int rpb = 128;
-  dim3 grid((N / 2 + 127) / 128, (M + rpb - 1) / rpb);
-  lb::colsum_kernel<<<grid, 128, 0, s>>>((const bf16*)x, out, M, N, rpb);
+  const int rpb = colsum_rows_per_block(M, N);
+  const int row_blocks = (M + rpb - 1) / rpb;
+  if (N % 8 == 0) {
+    lb::colsum_vec_kernel<<<dim3((N + 255) / 256, row_blocks), 256, 0, s>>>((const bf16*)x, workspace, M, N, rpb);
+  } else {
+    lb::colsum_kernel<<<dim3((N / 2 + 127) / 128, row_blocks), 128, 0, s>>>((const bf16*)x, workspace, M, N, rpb);
+  }
+  lb::colsum_partials_kernel<<<(N + 255) / 256, 256, 0, s>>>(workspace, out, row_blocks, N, accumulate);
   return (int)cudaGetLastError();
 }
 extern "C" int lb_ce_stats(const void* logits, const int64_t* labels, float* mx, float* se, float* tgt, int T, int V,
@@ -680,16 +725,21 @@ extern "C" int lb_embedding_fwd(const int64_t* ids, const void* table, void* out
   lb::embedding_fwd_kernel<<<(unsigned)T, 128, 0, s>>>(ids, (const bf16*)table, (bf16*)out, H, vocab_start, rows);
   return (int)cudaGetLastError();
 }
-extern "C" int lb_embedding_bwd(const int64_t* ids, const void* gy, float* grad, long T, int H, long vocab_start, long rows,
-                                cudaStream_t s) {
+// sorted_ids / order: the ids sorted stably and their token positions
+extern "C" int lb_embedding_bwd(const int64_t* sorted_ids, const int64_t* order, const void* gy, float* grad, long T, int H,
+                                long vocab_start, long rows, cudaStream_t s) {
   if (T == 0) return 0;
   if (H % 8) return -1;
-  lb::embedding_bwd_kernel<<<(unsigned)T, 128, 0, s>>>(ids, (const bf16*)gy, grad, H, vocab_start, rows);
+  lb::embedding_bwd_kernel<<<(unsigned)T, 128, 0, s>>>(sorted_ids, order, (const bf16*)gy, grad, T, H, vocab_start, rows);
   return (int)cudaGetLastError();
 }
-extern "C" int lb_sqnorm(const float* x, float* out, long n, cudaStream_t s) {
+extern "C" int lb_sqnorm_workspace(long n) { return ew_grid(n / 4, 256); }
+// out[0] += sum x^2; workspace: fp32 [lb_sqnorm_workspace(n)]
+extern "C" int lb_sqnorm(const float* x, float* out, long n, float* workspace, cudaStream_t s) {
   if (n == 0) return 0;  // (the kernel handles the n % 4 tail)
-  lb::sqnorm_kernel<<<ew_grid(n / 4, 256), 256, 0, s>>>(x, out, (size_t)n);
+  const int grid = ew_grid(n / 4, 256);
+  lb::sqnorm_kernel<<<grid, 256, 0, s>>>(x, workspace, (size_t)n);
+  lb::sum_partials_kernel<<<1, 32, 0, s>>>(workspace, grid, out);
   return (int)cudaGetLastError();
 }
 
@@ -753,7 +803,8 @@ extern "C" int lb_quant_e4m3(const void* x, void* q, void* amax_scratch, float* 
   const __nv_bfloat16* tail = reinterpret_cast<const __nv_bfloat16*>(x) + n8 * 8;
   long blocks = (n8 + 255) / 256;
   if (blocks < 1) blocks = 1;
-  if (blocks > 148 * 8) blocks = 148 * 8;
+  const long cap = ew_grid(~size_t(0) >> 1, 1);   // 8 blocks per SM
+  if (blocks > cap) blocks = cap;
   amax_bf16_kernel<<<(int)blocks, 256, 0, s>>>(reinterpret_cast<const uint4*>(x), n8, tail, ntail,
                                               reinterpret_cast<unsigned*>(amax_scratch));
   quant_e4m3_kernel<<<(int)blocks, 256, 0, s>>>(reinterpret_cast<const uint4*>(x), n8, tail, ntail,

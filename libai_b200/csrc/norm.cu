@@ -1,4 +1,4 @@
-// Fused LayerNorm / RMSNorm forward + backward for sm_100a (bandwidth-bound: one warp per row,
+// Fused LayerNorm / RMSNorm forward + backward for sm_90a (bandwidth-bound: one warp per row,
 // 128-bit vector accesses, statistics in fp32, row cached in registers between the passes).
 // Replaces flow._C.layer_norm_affine / rms_norm (reference libai/layers/layer_norm.py:78-131).
 //
@@ -163,8 +163,8 @@ norm_bwd_kernel(const T* __restrict__ gy, const T* __restrict__ x, const W* __re
 
 // bf16 activations, bandwidth-oriented variant of the kernel above (same maths, same outputs).  The first version kept
 // x̂ and g·γ of a row as 2 x VPL x 8 floats across the two warp reductions and fetched the residual gradient afterwards:
-// 191 registers → one 8-warp block per SM, and three dependent memory phases per row — 19 µs for [8192, 1024] where
-// the 64 MB it moves take 9 µs (profiles/r2_20_step_breakdown.md).  Here a row's x, gy and residual gradient are
+// 191 registers → one 8-warp block per SM, and three dependent memory phases per row, about twice the time its memory
+// traffic needs.  Here a row's x, gy and residual gradient are
 // fetched together as raw 16-byte vectors (3 x VPL x 4 registers), unpacked twice (before and after the reductions:
 // ALU is free here), and blocks are 4 warps at <= 168 registers → 12 warps per SM with 12 loads each in flight.
 constexpr int NORM_BWD_WARPS = 4;
@@ -174,7 +174,7 @@ __global__ void __launch_bounds__(NORM_BWD_WARPS * 32, 3)
 norm_bwd_bf16_kernel(const __nv_bfloat16* __restrict__ gy, const __nv_bfloat16* __restrict__ x, const W* __restrict__ gamma,
                      const float* __restrict__ mean_in, const float* __restrict__ rstd_in, __nv_bfloat16* __restrict__ gx,
                      float* __restrict__ part_dgamma, float* __restrict__ part_dbeta, int rows,
-                     const __nv_bfloat16* __restrict__ gadd, float* __restrict__ acc_dgamma, float* __restrict__ acc_dbeta) {
+                     const __nv_bfloat16* __restrict__ gadd) {
   constexpr int H = VPL * 256;
   __shared__ float red[NORM_BWD_WARPS][32 * 8 + 8];
   const int warp = threadIdx.x / 32, lane = threadIdx.x % 32;
@@ -253,14 +253,8 @@ norm_bwd_bf16_kernel(const __nv_bfloat16* __restrict__ gy, const __nv_bfloat16* 
         float acc = 0.f;
 #pragma unroll
         for (int w = 0; w < NORM_BWD_WARPS; ++w) acc += red[w][c];
-        if (acc_dgamma != nullptr) {
-          // accumulate mode (training: dγ/dβ live in the fp32 main_grad buffer): one red.add per block and column
-          // straight into the gradient instead of a [blocks, H] partial matrix + a second reduction kernel
-          atomicAdd((which == 0 ? acc_dgamma : acc_dbeta) + i * 256 + c, acc);
-        } else {
-          float* dst = (which == 0 ? part_dgamma : part_dbeta) + static_cast<size_t>(blockIdx.x) * H + i * 256 + c;
-          *dst = acc;
-        }
+        float* dst = (which == 0 ? part_dgamma : part_dbeta) + static_cast<size_t>(blockIdx.x) * H + i * 256 + c;
+        *dst = acc;
       }
     }
   }
@@ -408,11 +402,10 @@ bool fwd_dispatch(int vpl, const T* x, const W* g, const W* b, T* y, float* mean
 template <typename W, bool RMS>
 bool bwd_dispatch_bf16(int vpl, const __nv_bfloat16* gy, const __nv_bfloat16* x, const W* g, const float* mean,
                        const float* rstd, __nv_bfloat16* gx, float* pdg, float* pdb, int rows, int grid, cudaStream_t s,
-                       const __nv_bfloat16* gadd, float* acc_dg, float* acc_db) {
+                       const __nv_bfloat16* gadd) {
 #define LB_CASE(V)                                                                                                        \
   case V:                                                                                                                 \
-    lb::norm_bwd_bf16_kernel<W, V, RMS><<<grid, lb::NORM_BWD_WARPS * 32, 0, s>>>(gy, x, g, mean, rstd, gx, pdg, pdb, rows, gadd, \
-                                                                                 acc_dg, acc_db);                         \
+    lb::norm_bwd_bf16_kernel<W, V, RMS><<<grid, lb::NORM_BWD_WARPS * 32, 0, s>>>(gy, x, g, mean, rstd, gx, pdg, pdb, rows, gadd); \
     return true;
   switch (vpl) {
     LB_CASE(1) LB_CASE(2) LB_CASE(3) LB_CASE(4)
@@ -426,11 +419,10 @@ bool norm_bwd_uses_bf16_kernel(int H, int dtype) { return dtype == 0 && H % 256 
 
 template <typename T, typename W, bool RMS>
 bool bwd_dispatch(int vpl, const T* gy, const T* x, const W* g, const float* mean, const float* rstd, T* gx, float* pdg,
-                  float* pdb, int rows, int grid, cudaStream_t s, const T* gadd, float* acc_dg = nullptr,
-                  float* acc_db = nullptr) {
+                  float* pdb, int rows, int grid, cudaStream_t s, const T* gadd) {
   if constexpr (std::is_same<T, __nv_bfloat16>::value) {
     if (norm_bwd_uses_bf16_kernel(vpl * 256, 0))
-      return bwd_dispatch_bf16<W, RMS>(vpl, gy, x, g, mean, rstd, gx, pdg, pdb, rows, grid, s, gadd, acc_dg, acc_db);
+      return bwd_dispatch_bf16<W, RMS>(vpl, gy, x, g, mean, rstd, gx, pdg, pdb, rows, grid, s, gadd);
   }
 #define LB_CASE(V)                                                                                                   \
   case V:                                                                                                            \
@@ -500,19 +492,14 @@ extern "C" int lb_norm_bwd(const void* gy, const void* x, const void* gamma, con
   bool done = false;
   float* pdg = workspace;
   float* pdb = dbeta != nullptr ? workspace + static_cast<size_t>(grid) * H : nullptr;
-  // accumulate mode + bandwidth-oriented bf16 kernel: the blocks add their column partials straight into dgamma / dbeta
-  const bool direct = accumulate && norm_bwd_uses_bf16_kernel(H, dtype);
-  float* direct_dg = direct ? dgamma : nullptr;
-  float* direct_db = (direct && dbeta != nullptr) ? dbeta : nullptr;
-  if (direct && dbeta == nullptr) pdb = nullptr;
 #define LB_GO(T, W)                                                                                                  \
   {                                                                                                                  \
     if (fast) {                                                                                                      \
       done = rms ? bwd_dispatch<T, W, true>(H / 256, (const T*)gy, (const T*)x, (const W*)gamma, mean, rstd, (T*)gx, \
-                                            pdg, pdb, rows, grid, s, (const T*)gadd, direct_dg, direct_db)           \
+                                            pdg, pdb, rows, grid, s, (const T*)gadd)           \
                  : bwd_dispatch<T, W, false>(H / 256, (const T*)gy, (const T*)x, (const W*)gamma, mean, rstd,        \
-                                             (T*)gx, pdg, pdb, rows, grid, s, (const T*)gadd, direct_dg, direct_db); \
-      if (done && direct_dg == nullptr) {                                                                            \
+                                             (T*)gx, pdg, pdb, rows, grid, s, (const T*)gadd); \
+      if (done) {                                                                            \
         lb::colreduce_kernel<<<dim3((H + 31) / 32, dbeta != nullptr ? 2 : 1), 256, 0, s>>>(pdg, dgamma, pdb, dbeta, grid, \
                                                                                            H, accumulate);           \
       }                                                                                                              \

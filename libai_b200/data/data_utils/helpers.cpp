@@ -1,6 +1,6 @@
 // Native index builders for the Megatron-style datasets (C ABI, loaded through ctypes).
 //
-// Behavioural contract = reference libai/data/data_utils/helpers.cpp (N1-N4 in SURVEY.md §2.2):
+// Behavioural contract = reference libai/data/data_utils/helpers.cpp:
 //   * lb_build_sample_idx      – GPT sample index over the flattened document stream      (:86-169)
 //   * lb_build_mapping_{count,fill}  – BERT/T5 sentence-span samples, mt19937(seed) target lengths,
 //                                 Fisher-Yates shuffle with mt19937_64(seed + 1)           (:180-391)

@@ -1,8 +1,7 @@
 """CUDA-graph capture of the transformer blocks.
 
-A training step of the 24-layer benchmark model issues ≈820 kernels; the host needs ≈25 ms to enqueue them against
-≈29 ms of device time, so the step is within ~15 % of being launch-bound (``bench.py`` reports
-``host_enqueue_ms_per_step``).  The blocks are where the launches are (≈14 forward + ≈20 backward kernels each), they
+A training step of the 24-layer benchmark model issues ≈820 kernels, so the time the host needs to enqueue them is
+comparable to the device time of a small step (``bench.py`` reports ``host_enqueue_ms_per_step``).  The blocks are where the launches are (≈14 forward + ≈20 backward kernels each), they
 have static shapes and no host synchronisation, so each block's forward and backward are captured once into CUDA graphs
 (``torch.cuda.make_graphed_callables``) and replayed: 48 graph launches replace ≈800 kernel launches per step.
 

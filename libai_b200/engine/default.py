@@ -110,7 +110,7 @@ def _compile_dependencies():
 def _resolve_auto_tensor_parallel_mode(cfg):
     """``train.dist.sequence_parallel / fused_tp_comm = "auto"``: on for models that declare
     ``supports_sequence_parallel`` (GPT-2, BERT, Llama family) — their tensor-parallel blocks then run on token shards
-    with the collectives inside the GEMM kernels (the B200 product path) — off for the others, which keep the
+    with the collectives inside the GEMM kernels (the H100 product path) — off for the others, which keep the
     reference's replicated-activation form (libai/layers/linear.py:123-149)."""
     d = try_get_key(cfg, "train.dist")
     if d is None:

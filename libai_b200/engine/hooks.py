@@ -269,7 +269,7 @@ class LRScheduler(HookBase):
 
 
 # ---------------------------------------------------------------------------------------------------------------
-# NEW (not in the reference, SURVEY §5.1 / §5.3): preemption-safe stop and a profiling window
+# NEW (not in the reference): preemption-safe stop and a profiling window
 # ---------------------------------------------------------------------------------------------------------------
 class EmergencyCheckpointHook(HookBase):
     """SIGTERM (schedulers send it before killing a job) → write a resumable checkpoint at the next step boundary and
@@ -378,7 +378,7 @@ class ProfilerHook(HookBase):
 
 
 class FaultInjectionHook(HookBase):
-    """Test facility for the failure-recovery path (SURVEY §5.3): ``LIBAI_B200_FAULT_INJECT="<rank>:<iteration>"`` makes
+    """Test facility for the failure-recovery path: ``LIBAI_B200_FAULT_INJECT="<rank>:<iteration>"`` makes
     that rank die abruptly (``os._exit``, no cleanup, no checkpoint) right after the given iteration — the launcher
     (``torchrun``) then tears the job down and a relaunch with ``--resume`` must continue from the last periodic
     checkpoint (``tests/test_fault_recovery_cpu.py``)."""

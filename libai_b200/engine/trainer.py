@@ -173,10 +173,9 @@ class StepTrainer(TrainerBase):
     def _arm_grad_overlap(self, last_micro_batch: bool):
         """Opt-in (``LIBAI_B200_OVERLAP_GRAD_SYNC=1``): overlap the data-parallel gradient reduction with the backward
         pass of the last micro-batch (the fused NVLink reduce-scatter of the already-final part of the gradient buffer
-        starts at a few block boundaries).  Measured on B200 it does NOT pay for the 345M benchmark model: the
-        end-of-step reduction costs ~1 ms at 8 GPUs (97 % weak scaling without overlap), while the extra side-stream
-        kernels, their flag exchanges and the added host work cost more (2 GPUs 29.4 → 30.0 ms, 8 GPUs 29.9 → 35.3 ms;
-        `profiles/r20_*`, `profiles/r21_*`).  Kept for models whose gradient volume per step is much larger."""
+        starts at a few block boundaries).  Off by default: for a model of the benchmark's size the end-of-step
+        reduction is short, while the extra side-stream kernels, their flag exchanges and the added host work are paid
+        on every step.  Meant for models whose gradient volume per step is much larger."""
         if not hasattr(self, "_overlap_layers"):
             self._overlap_layers = ()
             model = self.model.module if hasattr(self.model, "module") else self.model

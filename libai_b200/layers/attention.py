@@ -8,7 +8,7 @@ multiplying it back (``apply_query_key_layer_scaling``, :87-91, numerically the 
 exact arithmetic) — masked positions filled with −10000 (:223-245), row-parallel output
 projection, bias+dropout fused with the residual add.
 
-The softmax(QKᵀ)V core runs in the sm_100a flash-attention kernel (no ``[b,a,s,s]`` tensor, no
+The softmax(QKᵀ)V core runs in the sm_90a flash-attention kernel (no ``[b,a,s,s]`` tensor, no
 materialised masks) whenever the mask is purely causal or absent; padding-mask / bias / dropout
 variants fall back to the reference math in :func:`libai_b200.ops.functional.attention_ref`.
 """

@@ -138,7 +138,7 @@ class SinePositionalEmbedding(nn.Module):
 class PatchEmbedding(nn.Module):
     """2-D image → patch tokens: a stride-``patch`` convolution == patchify + GEMM.
 
-    Implemented as unfold-free reshape + the tcgen05 GEMM (``[b·n_patches, c·p·p] × [c·p·p, h]``)
+    Implemented as unfold-free reshape + the wgmma GEMM (``[b·n_patches, c·p·p] × [c·p·p, h]``)
     instead of cuDNN; the parameter keeps the Conv2d layout ``[embed_dim, in_chans, p, p]`` so HF
     / reference checkpoints load unchanged."""
 

@@ -1,4 +1,4 @@
-"""LayerNorm / RMSLayerNorm backed by the fused sm_100a norm kernels.
+"""LayerNorm / RMSLayerNorm backed by the fused sm_90a norm kernels.
 
 Spec: reference libai/layers/layer_norm.py:22-131 — parameters are replicated, normalisation is
 over the trailing ``normalized_shape`` dims, ``elementwise_affine`` / ``bias`` switches, ``eps``.

@@ -12,7 +12,7 @@ Communication (explicit, instead of SBP boxing):
 * row: fwd all-reduce(y) over TP; with sequence parallelism fwd reduce-scatter(y) /
   bwd all-gather(dy).
 
-On B200 the sequence-parallel pairs run as single fused kernels (AG→GEMM, GEMM→RS over NVLink
+On H100 the sequence-parallel pairs run as single fused kernels (AG→GEMM, GEMM→RS over NVLink
 peer memory, ``libai_b200/ops/comm_gemm.py``) when ``train.dist.fused_tp_comm`` is on.
 """
 from __future__ import annotations
@@ -98,7 +98,7 @@ class Linear1D(nn.Module):
         return y
 
     def _forward_fused(self, x, bias_now, act, topo, residual=None):
-        """AG->GEMM / GEMM->RS with the collective inside the tcgen05 kernel (None = shape unsupported)."""
+        """AG->GEMM / GEMM->RS with the collective inside the wgmma kernel (None = shape unsupported)."""
         from libai_b200.ops import comm_gemm, use_native
 
         if not use_native(x) or x.dtype != torch.bfloat16:

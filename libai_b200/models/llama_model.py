@@ -7,7 +7,7 @@ per-head ``[q|k|v]`` ``query_key_value`` (col) + ``o_proj`` (row) and a KV cache
 ``SFTLoss`` = CE ignoring label 0 / negative labels (:497-520), ``LlamaForCausalLM`` (:523-649).  Parameter names
 follow the reference so its HF loader mapping (projects/Llama/utils/llama_loader.py) carries over.
 
-B200 path: rotary runs as one pass over the packed QKV projection (``rope_qkv`` kernel, v copied) feeding the
+H100 path: rotary runs as one pass over the packed QKV projection (``rope_qkv`` kernel, v copied) feeding the
 flash-attention kernel; SwiGLU and RMSNorm are native kernels; the LM head is vocab-parallel with the fused
 vocab-parallel cross entropy (the reference replicates ``lm_head``).
 """

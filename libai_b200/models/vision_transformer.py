@@ -4,7 +4,7 @@ Spec: reference libai/models/vision_transformer.py:25-267 — ``PatchEmbedding``
 ``cls_token`` / ``pos_embed`` (trunc-normal 0.02, no weight decay), ``depth`` pre-LN
 ``TransformerLayer`` blocks with linearly increasing DropPath, final LN, linear head on the class
 token; ``{"losses"}`` when training with labels, else ``{"prediction_scores"}``.
-The patch stem runs as patchify + tcgen05 GEMM (``layers/embedding.py``).
+The patch stem runs as patchify + wgmma GEMM (``layers/embedding.py``).
 """
 from __future__ import annotations
 

@@ -2,7 +2,7 @@
 
 Spec: reference libai/onnx_export/{gpt2_to_onnx.py,t5_to_onnx.py} — wrap the eager model, trace it with example
 inputs and write an ONNX file (there through ``oneflow_onnx``).  Here ``torch.onnx.export`` does the conversion of
-the PyTorch reference path of the model (``LIBAI_B200_IMPL=ref``: the hand-written sm_100a kernels have no ONNX
+the PyTorch reference path of the model (``LIBAI_B200_IMPL=ref``: the hand-written sm_90a kernels have no ONNX
 symbolics, the exported graph uses the mathematically identical library ops).  When the ``onnx`` package is not
 installed the model is exported as a TorchScript trace instead (``.pt``), which serves the same deployment role.
 """

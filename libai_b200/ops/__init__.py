@@ -2,7 +2,7 @@
 
 Every operator has two implementations:
 
-* ``native`` – hand-written sm_100a CUDA kernels in ``libai_b200/csrc`` (tcgen05/TMEM/TMA GEMMs,
+* ``native`` – hand-written sm_90a CUDA kernels in ``libai_b200/csrc`` (wgmma/TMA GEMMs,
   fused norms, flash attention, fused optimizer, vocab-parallel cross entropy, in-kernel
   NVLink collectives).  This is the product and the only path GPU training takes.
 * ``ref`` – plain PyTorch (+ ``torch.distributed``).  Test oracle, CPU/gloo plumbing path and the
@@ -38,7 +38,7 @@ def impl() -> str:
 class _FastOps:
     """``torch.ops.libai_b200`` with every operator resolved once to its ``.default`` overload.  Calling the
     ``OpOverloadPacket`` (what ``torch.ops.ns.name(...)`` is) re-resolves the overload on every call — a few
-    microseconds of Python per kernel launch, ~600 times per training step (``profiles/r23_host_profile.txt``)."""
+    microseconds of Python per kernel launch, several hundred times per training step."""
 
     def __init__(self, namespace):
         self._ns = namespace
@@ -77,7 +77,7 @@ def load_ext(required: bool = True):
 
 
 def use_native(*tensors) -> bool:
-    """True when the native sm_100a kernel must be used for these tensors."""
+    """True when the native sm_90a kernel must be used for these tensors."""
     if impl() != "native":
         return False
     for t in tensors:
@@ -113,7 +113,7 @@ _FP8_EPOCH = 0
 
 def set_fp8(enabled: bool) -> None:
     """Run the forward GEMMs of the linear layers with E4M3 operands (per-tensor dynamic scaling, fp32 accumulation
-    in TMEM, bf16 outputs); backward GEMMs stay bf16 on the saved bf16 operands."""
+    in registers, bf16 outputs); backward GEMMs stay bf16 on the saved bf16 operands."""
     global _FP8
     _FP8 = bool(enabled)
 
@@ -134,9 +134,11 @@ def bump_fp8_weight_epoch() -> None:
 
 
 # --------------------------------------------------------------------------------------
-# bias gradient of the MLP's first linear inside the dgrad epilogue (GEMM column sums via red.add)
+# bias gradient of the MLP's first linear accumulated by the dgrad call straight into the bias' fp32 main_grad: on one
+# GPU an ordered column-sum pass launched with the dgrad GEMM, under tensor parallelism inside the all-gather GEMM's
+# epilogue.  Off: the layer returns the column sums as a separate bf16 gradient.
 # --------------------------------------------------------------------------------------
-_FUSED_BIAS_GRAD = os.environ.get("LIBAI_B200_FUSED_BIAS_GRAD", "1") == "1"   # +0.8 % on the step in a same-box A/B (profiles/r2_28_*)
+_FUSED_BIAS_GRAD = os.environ.get("LIBAI_B200_FUSED_BIAS_GRAD", "1") == "1"
 
 
 def fused_bias_grad() -> bool:

@@ -2,7 +2,7 @@
 
     python -m libai_b200.ops.build [--force] [--verbose]
 
-CUDA sources are compiled for sm_100a only (``-gencode arch=compute_100a,code=sm_100a -lineinfo``);
+CUDA sources are compiled for sm_90a only (``-gencode arch=compute_90a,code=sm_90a -lineinfo``);
 nvcc cross-compiles without a GPU.  Objects are cached under ``libai_b200/csrc/build`` keyed by
 source mtime.  ``--sass`` additionally dumps ``cuobjdump -sass`` listings into ``profiles/sass``.
 """
@@ -22,11 +22,11 @@ SO_PATH = os.path.join(ROOT, "_C.so")
 CUDA_HOME = os.environ.get("CUDA_HOME", "/usr/local/cuda")
 NVCC = os.path.join(CUDA_HOME, "bin", "nvcc")
 
-CU_SOURCES = ["gemm_sm100.cu", "norm.cu", "elementwise.cu", "attention_sm100.cu", "comm_kernels.cu"]
+CU_SOURCES = ["gemm_sm90.cu", "norm.cu", "elementwise.cu", "attention_sm90.cu", "comm_kernels.cu"]
 CPP_SOURCES = ["bindings.cpp", "symm_mem.cpp"]
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "--use_fast_math", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "--use_fast_math", "-std=c++17",
     "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr", "-Xptxas", "-v",
 ]
 
@@ -91,7 +91,7 @@ def build(force: bool = False, verbose: bool = False, sass: bool = False) -> str
 
 
 def dump_sass():
-    """Write SASS listings + a mnemonic summary (UTC*MMA / LDTM / UTMALDG ...) to profiles/sass."""
+    """Write SASS listings + a mnemonic summary (HGMMA / UTMALDG ...) to profiles/sass."""
     out_dir = os.path.join(os.path.dirname(ROOT), "profiles", "sass")
     os.makedirs(out_dir, exist_ok=True)
     summary = []
@@ -102,18 +102,18 @@ def dump_sass():
         text = subprocess.run([os.path.join(CUDA_HOME, "bin", "cuobjdump"), "-sass", obj], stdout=subprocess.PIPE,
                               text=True).stdout
         counts = {}
-        # UTCHMMA / UTCQMMA = tcgen05.mma (bf16 / fp8), .2CTA = cta_group::2 pairs; LDTM/STTM = tcgen05.ld/st; UTMALDG /
-        # UTMASTG / UTMAREDG / UBLKCP = TMA tensor + bulk copies and reductions; LDGMC = multimem.ld_reduce (NVLS in-switch
-        # reduction; multimem.st is a STG.*.STRONG.SYS on a multicast address); USETMAXREG = setmaxnreg
-        for key in ("UTCHMMA", "UTCHMMA.2CTA", "UTCQMMA", "UTCBAR", "LDTM", "STTM", "UTMALDG", "UTMALDG.2D.2CTA", "UTMASTG",
-                    "UTMAREDG", "UBLKCP", "SYNCS", "LDGMC", "USETMAXREG", "RED.E", "REDG", "LDG.E", "STG.E"):
+        # HGMMA / QGMMA = wgmma (bf16 / fp8); UTMALDG / UTMASTG / UTMAREDG / UBLKCP = TMA tensor + bulk copies and
+        # reductions; LDGMC = multimem.ld_reduce (NVLS in-switch reduction; multimem.st is a STG.*.STRONG.SYS on a
+        # multicast address); USETMAXREG = setmaxnreg
+        for key in ("HGMMA", "QGMMA", "UTMALDG", "UTMASTG", "UTMAREDG", "UBLKCP", "SYNCS", "LDGMC", "USETMAXREG", "RED.E",
+                    "REDG", "LDG.E", "STG.E"):
             counts[key] = text.count(key)
         summary.append((s, counts))
-        keep = [ln for ln in text.splitlines() if "Function :" in ln or any(k in ln for k in ("UTC", "LDTM", "STTM", "UTMA", "UBLKCP", "LDGMC", "USETMAXREG"))]
+        keep = [ln for ln in text.splitlines() if "Function :" in ln or any(k in ln for k in ("GMMA", "UTMA", "UBLKCP", "LDGMC", "USETMAXREG"))]
         with open(os.path.join(out_dir, s + ".sass.txt"), "w") as f:
             f.write("\n".join(keep) + "\n")
     with open(os.path.join(out_dir, "SUMMARY.md"), "w") as f:
-        f.write("# SASS mnemonic counts per translation unit (cuobjdump -sass, sm_100a)\n\n")
+        f.write("# SASS mnemonic counts per translation unit (cuobjdump -sass, sm_90a)\n\n")
         for s, c in summary:
             f.write(f"* `{s}`: " + ", ".join(f"{k}={v}" for k, v in c.items() if v) + "\n")
     return summary

@@ -4,8 +4,8 @@
     row parallel    (sequence-parallel output):  y_shard  = reduce_scatter(x · Wᵀ)        → GEMM→RS
     column wgrad:                                dW       = dyᵀ · all_gather(x_shard)     → AG→GEMM (gathered B, TN)
 
-One kernel does both the math and the transfer (``csrc/gemm_sm100.cu`` COMM_AG / COMM_RS): copy CTAs push the local
-shard to the peers with TMA bulk copies while tcgen05 tiles that only need local rows are already running; the RS
+One kernel does both the math and the transfer (``csrc/gemm_sm90.cu`` COMM_AG / COMM_RS): copy CTAs push the local
+shard to the peers with TMA bulk copies while wgmma tiles that only need local rows are already running; the RS
 epilogue stores partial tiles straight into the owner's staging slot over NVLink and the owners reduce as arrivals are
 counted.  The whole handshake state (call counters, arrival targets, "done reading" credits) lives in device memory and
 is advanced by the kernels themselves: a call site always launches with the same parameters, so transformer blocks
@@ -28,8 +28,11 @@ _BM = 128
 
 
 def _n_comm_ctas(world: int) -> int:
-    """Copy CTAs of the AG kernels: each streams ~200 KB in flight through its TMA ring; more destinations → more CTAs."""
-    return 24 if world <= 4 else 32      # measured: profiles/r2_04_comm_bench_2gpu.json (8: 132 us, 16: 71, 24: 69, 32: 65, 48: 73)
+    """Copy CTAs of the AG kernels: each streams ~200 KB in flight through its TMA ring; more destinations → more CTAs.
+    A fixed share of the SMs (a sixth up to 4 ranks, two ninths beyond: 22 / 29 of an H100's 132); not yet tuned on
+    H100 (``tests/gpu_comm_bench.py`` sweeps it on two or more GPUs)."""
+    sms = torch.cuda.get_device_properties(torch.cuda.current_device()).multi_processor_count
+    return sms // 6 if world <= 4 else (2 * sms) // 9
 
 
 class _TPState:
@@ -88,8 +91,8 @@ def fused_supported(M: int, N: int, K: int, world: int) -> bool:
 
 # Keep all_gather(x) of the forward for the weight gradient (one device copy of [tokens, h] per column-parallel linear
 # and layer) instead of gathering x a second time inside the wgrad kernel: trades b·s·h·2 bytes of activation memory per
-# column-parallel linear for ~35 us of exposed NVLink synchronisation per wgrad (profiles/r2_06_comm_bench_2gpu.json:
-# AG->wgrad 80 us vs plain wgrad 42 us at 16k tokens).  ``LIBAI_B200_SP_SAVE_GATHERED=0`` restores the re-gather
+# column-parallel linear for the exposed NVLink synchronisation of a gathering wgrad.  ``LIBAI_B200_SP_SAVE_GATHERED=0``
+# restores the re-gather
 # (Megatron's sequence-parallel memory profile).
 import os as _os
 
@@ -138,8 +141,8 @@ def ag_gemm(x_shard: torch.Tensor, w: torch.Tensor, bias, act, group, layout: in
     gathered = s["buf"].view(torch.bfloat16, (2, M, K))[par]
     if fill_local:
         # the local rows of the gathered buffer are only needed by LATER kernels of this stream (the wgrad that reuses
-        # all_gather(dy)): a plain device copy at HBM speed (~6 us per 16 MB) instead of a second job for the copy
-        # CTAs, whose throughput is what the kernel waits for (profiles/r2_04_comm_bench_2gpu.json)
+        # all_gather(dy)): a plain device copy at HBM speed instead of a second job for the copy
+        # CTAs, whose throughput is what the kernel waits for
         gathered[st.rank * rows : (st.rank + 1) * rows].copy_(x_shard)
         count_launch()
     y, pre = ext.ag_gemm(

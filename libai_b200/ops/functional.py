@@ -1,8 +1,8 @@
 """Functional front-end of the hot operators (autograd wrappers).
 
-Each function dispatches to the native sm_100a kernels for CUDA tensors and to the PyTorch
+Each function dispatches to the native sm_90a kernels for CUDA tensors and to the PyTorch
 reference otherwise (see :mod:`libai_b200.ops`).  The reference call sites these replace are the
-OneFlow fused ops listed in SURVEY.md §2.4: ``flow._C.layer_norm_affine`` / ``rms_norm``
+OneFlow fused ops: ``flow._C.layer_norm_affine`` / ``rms_norm``
 (libai/layers/layer_norm.py:78-131), ``fused_bias_add_gelu`` (libai/layers/mlp.py:95),
 ``fused_bias_add_dropout`` (libai/layers/mlp.py:104, attention.py:265),
 ``fused_scale_mask_softmax_dropout`` / ``fused_scale_tril_softmax_mask_scale``
@@ -63,7 +63,7 @@ def _act_ref(x, act):
 # GEMM: y = x @ w^T (+ bias) (+ activation)
 # --------------------------------------------------------------------------------------
 def _gemm_ok(x: torch.Tensor, w: torch.Tensor) -> bool:
-    """Shapes/dtypes the tcgen05 kernel accepts (TMA needs 16-byte aligned rows)."""
+    """Shapes/dtypes the wgmma kernel accepts (TMA needs 16-byte aligned rows)."""
     return (
         x.dtype == torch.bfloat16
         and w.dtype == torch.bfloat16
@@ -213,8 +213,8 @@ class _MLPFn(torch.autograd.Function):
         g2 = gy.reshape(-1, gy.shape[-1])
         if not g2.is_contiguous():
             g2 = g2.contiguous()
-        # bias gradient of the first linear = column sums of dpre: accumulated into b1.main_grad by the dgrad epilogue
-        # (red.add from the staged chunk) instead of a separate pass over the [tokens, ffn] tensor
+        # bias gradient of the first linear = column sums of dpre, accumulated into b1.main_grad by the dgrad call (a
+        # column-sum pass with a fixed summation order, launched right behind the GEMM)
         b1 = ctx.bias_param
         fused_gb1 = None
         if ctx.has_bias and ctx.needs_input_grad[2] and ops.fused_bias_grad():
@@ -423,7 +423,7 @@ def bias_gelu(x, bias):
 
 
 def tp_rng_salt(sharded: bool) -> int:
-    """Salt of the dropout RNG stream (TP-aware RNG, SURVEY K21).  All tensor-parallel ranks of a model replica share
+    """Salt of the dropout RNG stream (TP-aware RNG).  All tensor-parallel ranks of a model replica share
     one (seed, offset) sequence (``dutil.model_parallel_seed``); activations that are *sharded* over the TP group
     (attention heads, token shards under sequence parallelism) must see different masks on different ranks → the TP
     rank is mixed into the Philox key; *replicated* activations (salt 0) get identical masks everywhere."""
@@ -550,7 +550,7 @@ def _prep_bias(bias, q):
 
 class _FlashAttnFn(torch.autograd.Function):
     """Flash attention on ``[b, a, s, d]`` views with optional additive bias (dense or ALiBi slopes), key-padding
-    lengths and Philox dropout on the probabilities — all inside the tcgen05 kernels."""
+    lengths and Philox dropout on the probabilities — all inside the wgmma kernels."""
 
     @staticmethod
     def forward(ctx, q, k, v, causal, scale, bias, alibi_slopes, p_drop, kv_lens):

@@ -1,7 +1,7 @@
 """Gated MLP (SwiGLU) with the gate and up projections as ONE GEMM.
 
 Reference: projects/Llama/llama.py:81-113 — ``down(silu(gate(x)) * up(x))`` with two separate column-parallel linears and an
-unfused elementwise product (SURVEY K1d / K16: "fuse gate/up as one 2f/t GEMM").  The two weights stay separate
+unfused elementwise product ("fuse gate/up as one 2f/t GEMM").  The two weights stay separate
 ``Parameter``s (checkpoints, HF loaders and the reference's module names are unchanged); once the optimizer has moved the
 parameters into its flat buffer they are adjacent in memory, so a ``[2F, K]`` view over both — and over their fp32
 ``main_grad`` slices — costs nothing:

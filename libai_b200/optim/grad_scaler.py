@@ -1,4 +1,4 @@
-"""Dynamic loss scaling for fp16 training (bf16 – the B200 default – needs none).
+"""Dynamic loss scaling for fp16 training (bf16 – the H100 default – needs none).
 
 Spec: reference libai/models/utils/graph_base.py:53-61 – ``GradScaler(init_scale=65536·D,
 growth_factor=2, backoff_factor=0.5, growth_interval=2000)``.

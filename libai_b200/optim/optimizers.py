@@ -4,10 +4,10 @@ clipping and mixed precision (bf16 params + fp32 master).
 What the reference gets from OneFlow (``flow.optim.AdamW`` + nn.Graph switches: ZeRO
 ``graph_base.py:69-70``, fused model update ``:75``, fused cast+scale ``:76``, grad clipping stored
 in the param groups ``optim/build.py:86-88`` and applied by ``optimizer.clip_grad()``
-``engine/trainer.py:284``) is provided explicitly here, designed around B200:
+``engine/trainer.py:284``) is provided explicitly here, designed around H100:
 
 * every param group lives in ONE contiguous buffer: low-precision params (``param_flat``), fp32
-  gradients (``grad_flat`` – the tcgen05 wgrad kernels accumulate into it directly through
+  gradients (``grad_flat`` – the wgmma wgrad kernels accumulate into it directly through
   ``param.main_grad``), fp32 master weights and Adam moments.  One fused kernel launch updates a
   whole group (K18), the gradient norm is one reduction over the flat buffer (K19).
 * ``zero_stage >= 1`` partitions master/moments (and the update) over the DP group: the gradient
@@ -62,8 +62,7 @@ class _Group:
             # LIBAI_B200_NVLS=1 (opt-in): bind the buffers to an NVSwitch multicast object — the reduce-scatter then reads
             # in-switch sums (multimem.ld_reduce), the parameter all-gather is one multimem.st per vector.  Off by default:
             # a reduce-SCATTER through the switch still has every GPU send its whole buffer (only the inbound side
-            # shrinks), so it cannot beat the unicast pull on full-duplex links; measured on 2 GPUs 26.9 vs 26.2 ms per
-            # step (profiles/r2_26_*), bit-identical results.
+            # shrinks), so it cannot beat the unicast pull on full-duplex links; results are bit-identical.
             nvls = os.environ.get("LIBAI_B200_NVLS", "0") == "1" and self.dtype == torch.bfloat16
             pbuf = symm_ws.buffer(("zero_param", index, self.numel, nvls), self.numel * params[0].element_size(), multicast=nvls)
             gbuf = symm_ws.buffer(("zero_grad", index, self.numel, nvls), self.numel * 4, multicast=nvls)

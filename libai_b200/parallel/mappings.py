@@ -15,7 +15,7 @@ gather_from_tp    all-gather (last dim)    take local slice
 ================  =======================  =======================
 
 "sp" = Megatron-style sequence parallelism: activations outside the TP region are sharded over
-the *flattened token* dimension (dim 0).  On B200 the GEMM-adjacent pairs (all-gather→GEMM,
+the *flattened token* dimension (dim 0).  On H100 the GEMM-adjacent pairs (all-gather→GEMM,
 GEMM→reduce-scatter) are replaced by fused kernels (see ``libai_b200/ops/comm_gemm.py``); these
 NCCL versions are the oracle and the baseline.
 """

@@ -3,7 +3,7 @@
 Each rank of a process group allocates the same number of bytes with ``cudaMalloc`` (outside the
 caching allocator), the 64-byte CUDA IPC handles are exchanged through ``torch.distributed``, and
 every rank maps all peers' buffers.  Kernels receive the table of peer pointers and use plain
-``ld/st/red`` on them – the traffic goes over NVLink 5 / NVSwitch.  (SURVEY §5.8 item 2.)
+``ld/st/red`` on them – the traffic goes over NVLink 5 / NVSwitch. 
 """
 from __future__ import annotations
 

@@ -5,7 +5,7 @@ rank mesh "PP outermost, DP middle, TP innermost" (:149-159, :246-252), the laye
 the "middle stages get more layers" rule (:161-195), ``custom_pipeline_stage_id`` (:115-130),
 helpers (:366-494).
 
-Design (B200-first, not a port): the reference expresses placement through OneFlow SBP/placement
+Design (H100-first, not a port): the reference expresses placement through OneFlow SBP/placement
 objects and lets the runtime insert collectives.  Here the topology is a plain object that owns
 ``torch.distributed`` process groups (NCCL for device collectives, gloo for host objects) built
 from the same rank formula
@@ -131,7 +131,7 @@ class DistributedTopology:
         self._device_type = try_get_key(cfg, "device_type", default="cuda")
         if self._device_type not in ("cuda", "cpu"):
             raise NotImplementedError(
-                f"Unsupported device {self._device_type}: this framework targets B200 ('cuda'); "
+                f"Unsupported device {self._device_type}: this framework targets H100 ('cuda'); "
                 "'cpu' is kept for gloo plumbing tests"
             )
         if self._device_type == "cuda" and not torch.cuda.is_available():

@@ -4,7 +4,7 @@ Spec: reference projects/CLIP/clip/model.py — ``Bottleneck`` / ``AttentionPool
 ``LayerNorm`` (fp32 compute), ``QuickGELU``, ``ResidualAttentionBlock``, ``Transformer``, ``VisionTransformer``,
 ``CLIP`` (``encode_image``, ``encode_text`` taking the features at the EOT token, cosine logits scaled by
 ``exp(logit_scale)``), ``convert_weights``, ``build_model`` (infers the architecture from a state dict).
-Attention runs through ``libai_b200.ops.attention`` (flash kernel for mask-free / causal shapes on B200).
+Attention runs through ``libai_b200.ops.attention`` (flash kernel for mask-free / causal shapes on H100).
 """
 from collections import OrderedDict
 from typing import Tuple, Union
@@ -238,7 +238,7 @@ class CLIP(nn.Module):
 
 
 def convert_weights(model: nn.Module, dtype=torch.bfloat16):
-    """Cast the matmul / conv weights to half precision (bf16 on B200), keep norms in fp32."""
+    """Cast the matmul / conv weights to half precision (bf16 on H100), keep norms in fp32."""
 
     def _convert(layer):
         if isinstance(layer, (nn.Conv1d, nn.Conv2d, nn.Linear)):

@@ -5,8 +5,8 @@ Spec: reference projects/ConvNeXT/modeling/{convnext_layers.py,convnext_model.py
 scale → drop path`` blocks with 2×2 strided down-sampling between stages, global average pooling, LayerNorm,
 classifier with the ``problem_type`` dependent loss (:138-170).
 
-B200 mapping: the depth-wise 7×7 convolution stays on cuDNN (channels-last), everything after it runs on the token
-layout ``[N·H·W, C]`` through the native LayerNorm and the tcgen05 GEMM with the GELU epilogue (the 1×1 "pwconv"
+H100 mapping: the depth-wise 7×7 convolution stays on cuDNN (channels-last), everything after it runs on the token
+layout ``[N·H·W, C]`` through the native LayerNorm and the wgmma GEMM with the GELU epilogue (the 1×1 "pwconv"
 layers are the column/row-parallel linears of the fused MLP node).
 """
 import torch

@@ -5,7 +5,7 @@ Spec: reference projects/Llama/adapter/adapter_model.py — ``adapter_query`` em
 ``query_key_value`` projection (:219-228, no rotary), per-head ``gate`` with
 ``softmax(scores_adapter)·tanh(gate)`` concatenated to the ordinary softmax (:252-266).
 
-B200 decomposition: ``softmax([A | S])`` is never formed — the sequence part stays on the flash-attention kernel
+H100 decomposition: ``softmax([A | S])`` is never formed — the sequence part stays on the flash-attention kernel
 (``attention_qkvpacked``) and the adapter part (``adapter_len`` ≈ 10 keys) is a small dense attention added on
 top: ``ctx = flash(q, k, v) + tanh(gate) · softmax(q·k_aᵀ) · v_a``.
 """

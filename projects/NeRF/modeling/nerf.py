@@ -1,7 +1,7 @@
 """NeRF positional encoding and MLP (spec: reference projects/NeRF/modeling/NeRF.py:22-146).
 
 The MLP is eight 256-wide GEMMs over ``rays × samples`` points (≈200k rows per step at the default batch) — GEMM
-shaped work, so the layers are this framework's ``Linear`` with the ReLU fused into the tcgen05 GEMM epilogue.
+shaped work, so the layers are this framework's ``Linear`` with the ReLU fused into the wgmma GEMM epilogue.
 The first layer's input (63 channels) and the skip layer's input (319) are zero-padded to multiples of 8 so the
 operand rows satisfy TMA's 16-byte alignment; the padding columns of the weights receive zero inputs and therefore
 zero gradients."""

@@ -6,7 +6,7 @@ Spec: reference projects/PaLM/palm_model.py — ``RotaryEmbedding`` / ``apply_ro
 reference feeds the un-normalised ``x`` to the feed-forward, :189), ``PalmHead`` tied to the embedding with the LM
 loss (:193-208), ``PaLM`` (:211-300).
 
-B200 mapping: queries are column-parallel over heads; the single KV head is replicated (it is tiny:
+H100 mapping: queries are column-parallel over heads; the single KV head is replicated (it is tiny:
 ``2·dim_head`` columns); attention runs through ``ops.attention`` (flash kernel when shapes allow: the KV head is
 expanded as a zero-copy stride-0 view → falls back to the library path, the GEMMs stay native).
 """

@@ -5,8 +5,8 @@ package; this framework carries its own implementation so the project has no dep
 and parameter names follow the public diffusers checkpoint layout (``down_blocks.0.attentions.1.transformer_blocks.0
 .attn2.to_k.weight`` ...) so released Stable Diffusion weights load by name (``modules/loader.py``).
 
-B200 notes: the transformer blocks are where the time goes at 64×64 latents (4096 tokens): their projections and
-the GEGLU feed-forward are ``libai_b200.layers.Linear`` (tcgen05 GEMM), attention goes through ``ops.attention``
+H100 notes: the transformer blocks are where the time goes at 64×64 latents (4096 tokens): their projections and
+the GEGLU feed-forward are ``libai_b200.layers.Linear`` (wgmma GEMM), attention goes through ``ops.attention``
 (flash kernel for head_dim 64/128, which covers SD2.x; SD1.x head dims 40/80/160 use the reference math), and
 tensors stay channels-last through the convolutions.
 """

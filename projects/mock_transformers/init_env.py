@@ -7,7 +7,7 @@ modelling code (and ``model.generate``) runs tensor-parallel.
 Here the HF model already is a torch model, so nothing needs mocking.  What remains is the real feature: *rewrite a
 loaded HF model in place into a tensor-parallel one*.  ``parallelize`` walks a plan of
 ``(module-name regex → "col" | "row")`` rules, replaces each matched ``nn.Linear``/``Conv1D`` by this framework's
-:class:`Linear1D` (so the GEMM runs on the tcgen05 kernels, and — with ``fused_tp_comm`` — the all-gather /
+:class:`Linear1D` (so the GEMM runs on the wgmma kernels, and — with ``fused_tp_comm`` — the all-gather /
 reduce-scatter runs inside the GEMM), copies this rank's shard of the checkpoint weights into it, and divides the
 per-module head counts by the TP size.  Fused QKV projections are sharded per section so every rank gets whole heads
 of q, k and v.

@@ -1,6 +1,6 @@
 """Packaging (reference setup.py:24-117): version file, the native extensions, and the packaged configs.
 
-    pip install -e .            # builds the C++ data helpers and the sm_100a CUDA extension in-tree
+    pip install -e .            # builds the C++ data helpers and the sm_90a CUDA extension in-tree
 
 Both native pieces are compiled by the same code the runtime uses (``libai_b200.data.data_utils.helpers_build`` and
 ``libai_b200.ops.build``), so an installed tree and a source checkout produce identical binaries.  ``configs/`` is
@@ -50,11 +50,11 @@ def build_native():
     from libai_b200.ops import build as ops_build
 
     helpers_build.ensure_built()
-    ops_build.build()          # nvcc -gencode arch=compute_100a,code=sm_100a (cross-compiles without a GPU)
+    ops_build.build()          # nvcc -gencode arch=compute_90a,code=sm_90a (cross-compiles without a GPU)
 
 
 class BuildNative(Command):
-    description = "compile the C++ data helpers and the sm_100a CUDA extension in-tree"
+    description = "compile the C++ data helpers and the sm_90a CUDA extension in-tree"
     user_options = []
 
     def initialize_options(self):
@@ -85,7 +85,7 @@ if __name__ == "__main__":
     setup(
         name="libai_b200",
         version=version,
-        description="Blackwell-native toolbox for large-scale distributed parallel training",
+        description="Hopper-native toolbox for large-scale distributed parallel training",
         packages=find_packages(exclude=("tests", "tests.*", "projects", "projects.*")),
         package_data={"libai_b200": ["*.so", "csrc/*", "data/data_utils/*.so", "data/data_utils/*.cpp",
                                      "config/configs/**/*.py"]},

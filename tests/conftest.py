@@ -9,7 +9,7 @@ if REPO not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: test needs a CUDA device (run on a B200 via gpurun)")
+    config.addinivalue_line("markers", "gpu: test needs a CUDA device (an H100)")
 
 
 def pytest_collection_modifyitems(config, items):

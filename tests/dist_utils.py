@@ -1,5 +1,5 @@
 """Spawn ``world`` CPU processes with a gloo process group and run ``fn(rank, world, *args)`` in each
-("multi-node without a cluster", SURVEY §4).  Return values of all ranks are collected."""
+("multi-node without a cluster").  Return values of all ranks are collected."""
 import os
 import socket
 import traceback

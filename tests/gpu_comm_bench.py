@@ -1,6 +1,6 @@
 """Steady-state cost of the fused comm+GEMM kernels at the benchmark model's tensor-parallel shapes: every op is issued
 back to back (no host barrier between iterations, like inside a training step) and compared with the plain GEMM of the
-same shape.  Run under torchrun with 2+ GPUs; rank 0 writes gpurun_out/comm_bench.json."""
+same shape.  Run under torchrun with 2+ GPUs; rank 0 writes output/comm_bench.json."""
 import json
 import os
 import sys
@@ -23,7 +23,7 @@ def main():
     topo = dutil.setup_dist_util(DictConfig(dict(data_parallel_size=1, tensor_parallel_size=world, pipeline_parallel_size=1,
                                                  sequence_parallel=True, fused_tp_comm=True)))
     g = topo.tp_group
-    out_path = sys.argv[sys.argv.index("--out") + 1] if "--out" in sys.argv else "gpurun_out/comm_bench.json"
+    out_path = sys.argv[sys.argv.index("--out") + 1] if "--out" in sys.argv else "output/comm_bench.json"
     tag = os.environ.get("LIBAI_B200_DEBUG_COMM_NO_PAYLOAD", "0")
 
     def bench(fn, iters=40):

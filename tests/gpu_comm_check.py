@@ -282,8 +282,8 @@ def main():
         # lr * g / (|g| + 1e-8), i.e. by +-lr with the SIGN of the reduced gradient, and among 4 M elements there is
         # (with these fixed seeds: at 8 ranks) one whose 8-term sum is ~1e-8 — the rotated summation order of the pull
         # kernel, NCCL's ring order and the sequential local reference then disagree by half a step on that element
-        # (0.5 * lr = 0.005 against max|p| = 0.13 is exactly the 0.0385 max-norm "error" of profiles/r18_comm_check_8gpu.json
-        # and of the first 8-GPU run of round 2; commutative at 2 ranks, hence bitwise equal there).
+        # (0.5 * lr = 0.005 against max|p| = 0.13, a 0.0385 max-norm "error"; commutative at 2 ranks, hence bitwise equal
+        # there).
         return (x * 1024.0).round() / 1024.0
 
     def zero():
@@ -396,7 +396,7 @@ def main():
     record("overlapped grad reduce-scatter == end-of-step", overlap)
 
     if rank == 0:
-        out = "gpurun_out/comm_check.json"
+        out = "output/comm_check.json"
         if "--out" in sys.argv:
             out = sys.argv[sys.argv.index("--out") + 1]
         os.makedirs(os.path.dirname(out) or ".", exist_ok=True)

@@ -1,6 +1,6 @@
 """Numerics + timing report of every native kernel against fp32 PyTorch references.
 
-Run on a B200:  python tests/gpu_kernel_check.py [--out gpurun_out/kernel_check.json]
+Run on an H100:  python tests/gpu_kernel_check.py [--out output/kernel_check.json]
 Never aborts on the first failure: every case is recorded (ok / max error / device time / achieved
 TFLOP/s or GB/s) so one GPU call yields the full picture.
 """
@@ -26,7 +26,7 @@ def timeit(fn, iters=20, warmup=5):
     flush = torch.empty(256 * 1024 * 1024, dtype=torch.uint8, device="cuda")
     times = []
     for _ in range(iters):
-        flush.zero_()  # evict L2 (126 MB)
+        flush.zero_()  # evict L2 (50 MB on H100)
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         e0.record()
         fn()
@@ -59,6 +59,7 @@ def record(name, fn):
     RESULTS.append({"name": name, **info})
     print(json.dumps({k: v for k, v in RESULTS[-1].items() if k != "trace"}), flush=True)
     if OUT_PATH:
+        os.makedirs(os.path.dirname(OUT_PATH) or ".", exist_ok=True)
         with open(OUT_PATH, "w") as f:
             json.dump(RESULTS, f, indent=1)
 
@@ -99,7 +100,7 @@ def check_gemm(ext, layout, M, N, K, bn=0, splits=1, fp32_out=False, time_it=Fal
 
 def main():
     ap = argparse.ArgumentParser()
-    ap.add_argument("--out", default="gpurun_out/kernel_check.json")
+    ap.add_argument("--out", default="output/kernel_check.json")
     ap.add_argument("--quick", action="store_true")
     ap.add_argument("--only", default="", help="comma separated name prefixes")
     args = ap.parse_args()
@@ -302,7 +303,7 @@ def main():
     record("embedding gather / scatter-add", embedding_native)
 
     def fp8_forward_gemm():
-        """E4M3 forward GEMM (tcgen05 kind::f8f6f4): exact against an fp32 matmul of the *dequantised* operands (the
+        """E4M3 forward GEMM (wgmma e4m3): exact against an fp32 matmul of the *dequantised* operands (the
         only error left is the bf16 rounding of the output), close to the bf16 GEMM, plus quantiser checks and timing."""
         e = {}
         x = torch.randn(777, 1040, device="cuda").bfloat16() * 3
@@ -746,6 +747,7 @@ def main():
 
         record("attention speed B8 A16 S1024 D64 causal", att_speed)
 
+    os.makedirs(os.path.dirname(args.out) or ".", exist_ok=True)
     with open(args.out, "w") as f:
         json.dump(RESULTS, f, indent=1)
     bad = [r["name"] for r in RESULTS if not r.get("ok", False)]

@@ -4,8 +4,8 @@ import os
 import re
 
 REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-DOCS = ["DESIGN.md", "README.md", "COVERAGE.md", "profiles/README.md", "docs/source/tutorials/get_started/Benchmark.md",
-        "profiles/r2_19_ncu_attention_backward.md", "profiles/sanitizer/README.md"]
+DOCS = ["README.md", "BASELINE.md"] + sorted(
+    os.path.relpath(p, REPO) for p in glob.glob(os.path.join(REPO, "docs", "source", "**", "*.md"), recursive=True))
 
 
 def _expand(text):
@@ -20,10 +20,11 @@ def test_cited_profile_files_exist():
     missing = []
     for doc in DOCS:
         path = os.path.join(REPO, doc)
-        if not os.path.exists(path):
-            continue
+        assert os.path.exists(path), doc
         text = _expand(open(path).read())
-        for name in set(re.findall(r"\b(r2?_?\d+_[\w\-.]+\.(?:json|md|txt|log))\b", text)):
+        names = set(re.findall(r"\b(r2?_?\d+_[\w\-.]+\.(?:json|md|txt|log))\b", text))
+        names |= set(re.findall(r"\bprofiles/([\w\-./*]+)", text))
+        for name in names:
             hits = glob.glob(os.path.join(REPO, "profiles", name)) + glob.glob(os.path.join(REPO, "profiles", "sanitizer", name))
             if not hits:
                 missing.append((doc, name))

@@ -1,4 +1,4 @@
-"""GPU tier (run on a B200 with ``pytest -m gpu``): every sm_100a kernel against fp32 PyTorch references, the native
+"""GPU tier (run on an H100 with ``pytest -m gpu``): every sm_90a kernel against fp32 PyTorch references, the native
 training step against the PyTorch/cuBLAS reference path, the fused NVLink collectives (when ≥ 2 GPUs are visible) and
 the bench / smoke contracts.  The native extension must be the code that runs: tests fail if it is not loaded."""
 import json
@@ -134,8 +134,54 @@ def test_cuda_graph_blocks_match_eager():
     assert abs(n_graph - n_eager) <= 0.1 * n_eager, (n_eager, n_graph)     # replayed kernels are still counted
 
 
+
+def test_training_steps_are_bit_identical_run_to_run():
+    """Two trainings from the same seeds and batches end with bit-identical losses and parameters: every reduction on
+    the single-GPU path (split-free wgrad, column sums, norm γ/β, gradient norm, embedding backward, attention dQ)
+    sums in a fixed order."""
+    from libai_b200 import ops
+    from libai_b200.config import DictConfig
+    from libai_b200.layers._param import param_defaults
+    from libai_b200.models import GPTForPreTraining
+    from libai_b200.optim import AdamW, get_default_optimizer_params
+    from libai_b200.utils import distributed as dutil
+
+    os.environ["LIBAI_B200_IMPL"] = "native"
+    cfg = DictConfig(dict(
+        hidden_layers=2, vocab_size=512, hidden_size=256, ffn_hidden_size=1024, num_attention_heads=4, max_seq_length=512,
+        embedding_dropout_prob=0.1, attention_dropout_prob=0.1, output_dropout_prob=0.1, layernorm_epsilon=1e-5,
+        initializer_range=0.02, use_scaled_init_for_output_weights=True, bias_gelu_fusion=True, bias_dropout_fusion=True,
+        scale_mask_softmax_fusion=True, apply_query_key_layer_scaling=False, apply_residual_post_layernorm=False,
+        amp_enabled=True))
+    runs = []
+    for _ in range(2):
+        dutil.reset_dist_util()
+        dutil.setup_dist_util(DictConfig(dict(data_parallel_size=1, tensor_parallel_size=1, pipeline_parallel_size=1)))
+        torch.manual_seed(11)
+        torch.cuda.manual_seed(11)
+        with param_defaults(dtype=torch.bfloat16, device="cuda", seed=5):
+            model = GPTForPreTraining(cfg).train()
+        opt = AdamW(get_default_optimizer_params(model, clip_grad_max_norm=1.0, clip_grad_norm_type=2.0), lr=1e-3)
+        opt.configure(param_names={id(p): n for n, p in model.named_parameters()})
+        opt.setup()
+        g = torch.Generator(device="cuda").manual_seed(9)
+        n0 = ops.launch_count()
+        losses = []
+        for _ in range(4):
+            ids = torch.randint(0, 512, (8, 512), device="cuda", generator=g)   # 4096 tokens: repeated ids, 8 key blocks
+            opt.zero_grad()
+            loss = model(ids, ids)["lm_loss"]
+            loss.backward()
+            opt.step()
+            losses.append(loss.item())
+        assert ops.launch_count() - n0 > 50, "the native kernels did not run"
+        runs.append((losses, [p.detach().float().cpu() for p in model.parameters()]))
+    (l0, p0), (l1, p1) = runs
+    assert l0 == l1, (l0, l1)
+    assert all(torch.equal(a, b) for a, b in zip(p0, p1))
+
 def test_fp8_forward_gemms_train_like_bf16():
-    """``ops.set_fp8(True)``: the linear layers' forward GEMMs take E4M3 operands (quantise + tcgen05 kind::f8f6f4
+    """``ops.set_fp8(True)``: the linear layers' forward GEMMs take E4M3 operands (quantise + wgmma e4m3
     kernel); losses track the bf16 run, eagerly (cached weight copies refreshed per optimizer step) and under CUDA
     graphs (quantisation captured)."""
     from libai_b200 import ops

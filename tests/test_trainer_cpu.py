@@ -1,5 +1,5 @@
 """End-to-end: `tools/train_net.py` flow on CPU — training, periodic checkpoints, exact resume, evaluation, and
-2-rank data-parallel training over gloo (the reference's model tests train real configs on 4 GPUs; SURVEY §4)."""
+2-rank data-parallel training over gloo (the reference's model tests train real configs on 4 GPUs)."""
 import json
 import os
 import sys
@@ -89,7 +89,7 @@ def test_two_rank_data_parallel(tmp_path):
 
 
 def test_sigterm_writes_checkpoint_and_resume_matches(tmp_path):
-    """SURVEY §5.3 (new): SIGTERM mid-run → emergency checkpoint at the step boundary + clean stop; ``--resume`` then
+    """SIGTERM mid-run → emergency checkpoint at the step boundary + clean stop; ``--resume`` then
     finishes with exactly the weights of an uninterrupted run.  Also exercises the profiling window hook."""
     import signal
 

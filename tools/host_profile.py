@@ -1,6 +1,6 @@
 """Where does the HOST time of a training step go?  Runs the benchmark model for a few steps under cProfile (1 GPU)
-and prints the functions with the largest own time.  (The step is within ~15 % of being launch-bound, so Python /
-dispatcher overhead per kernel matters: `bench.py` reports `host_enqueue_ms_per_step`.)
+and prints the functions with the largest own time.  (Python / dispatcher overhead per kernel
+matters when the step comes close to being launch-bound: `bench.py` reports `host_enqueue_ms_per_step`.)
 
     python tools/host_profile.py [--steps 6]
 """
