@@ -1,5 +1,11 @@
-"""Tile-N sweep of the forward (NT) and dgrad (NN) GEMMs on the benchmark model's shapes: does the heuristic of
-gemm_sm90.cu (bn = 0) pick the fastest tile?"""
+"""Tile-N sweep of every GEMM of the benchmark model's training step (GPT-2 medium, micro-batch 8 x 1024 tokens): does
+the heuristic of gemm_sm90.cu (bn = 0) pick the fastest tile, and how far is each shape from cuBLAS?
+
+Shapes: forward NT and dgrad NN of the four transformer linears, their wgrad TN with the fp32 `red.add` epilogue into
+a main_grad buffer, and the LM head's forward, dgrad and wgrad.  Prints one JSON line: per shape the median time (ms)
+and TFLOP/s (2·M·N·K over time) of each tile width and of torch.matmul (cuBLAS) on the same operands.  The forced tile
+widths of the wgrad go through `gemm_tuned`, which also zero-fills the fp32 output (M·N·4 bytes) inside the timed
+region; `bn0` of the wgrad accumulates into an existing buffer, as the training step does.  cuBLAS writes bf16."""
 import json
 import sys
 
@@ -7,6 +13,16 @@ import torch
 
 sys.path.insert(0, ".")
 from libai_b200.ops import load_ext  # noqa: E402
+
+T, H, FFN, VOCAB = 8192, 1024, 4096, 50304
+
+# (name, layout, M, N, K); layout 0 = NT (A[M,K], B[N,K]), 1 = NN (A[M,K], B[K,N]), 2 = TN (A[K,M], B[K,N])
+SHAPES = [
+    ("fwd_qkv", 0, T, 3 * H, H), ("fwd_proj", 0, T, H, H), ("fwd_fc1", 0, T, FFN, H), ("fwd_fc2", 0, T, H, FFN),
+    ("dgrad_qkv", 1, T, H, 3 * H), ("dgrad_proj", 1, T, H, H), ("dgrad_fc2", 1, T, FFN, H), ("dgrad_fc1", 1, T, H, FFN),
+    ("wgrad_qkv", 2, 3 * H, H, T), ("wgrad_proj", 2, H, H, T), ("wgrad_fc1", 2, FFN, H, T), ("wgrad_fc2", 2, H, FFN, T),
+    ("lmhead_fwd", 0, T, VOCAB, H), ("lmhead_dgrad", 1, T, H, VOCAB), ("lmhead_wgrad", 2, VOCAB, H, T),
+]
 
 
 def timeit(fn, iters=40, warmup=8):
@@ -27,23 +43,41 @@ def timeit(fn, iters=40, warmup=8):
     return ts[len(ts) // 2]
 
 
+def operands(layout, M, N, K):
+    a = (torch.randn(K, M, device="cuda") if layout == 2 else torch.randn(M, K, device="cuda")).bfloat16()
+    b = (torch.randn(N, K, device="cuda") if layout == 0 else torch.randn(K, N, device="cuda")).bfloat16()
+    return a, b
+
+
 def main():
     ext = load_ext()
+    torch.manual_seed(0)
     out = {}
-    shapes = [("fwd_qkv", 0, 8192, 3072, 1024), ("fwd_proj", 0, 8192, 1024, 1024), ("fwd_fc1", 0, 8192, 4096, 1024),
-              ("fwd_fc2", 0, 8192, 1024, 4096), ("dgrad_qkv", 1, 8192, 1024, 3072), ("dgrad_proj", 1, 8192, 1024, 1024),
-              ("dgrad_fc2", 1, 8192, 4096, 1024), ("dgrad_fc1", 1, 8192, 1024, 4096)]
-    for name, layout, M, N, K in shapes:
-        a = torch.randn(M, K, device="cuda").bfloat16()
-        b = (torch.randn(N, K, device="cuda") if layout == 0 else torch.randn(K, N, device="cuda")).bfloat16()
-        res = {}
-        for bn in (0, 128, 192, 256):
+    for name, layout, M, N, K in SHAPES:
+        a, b = operands(layout, M, N, K)
+        flop = 2.0 * M * N * K
+        res = {"shape": [M, N, K]}
+
+        def record(key, ms):
+            res[key] = {"ms": round(ms, 4), "tflops": round(flop / (ms * 1e-3) / 1e12, 1)}
+
+        if layout == 2:
+            main_grad = torch.zeros(M, N, device="cuda")
+            record("bn0", timeit(lambda: ext.gemm(a, b, 2, None, main_grad, True, torch.float32)))
+        for bn in (0, 64, 128, 192, 256) if layout != 2 else (64, 128, 192, 256):
             try:
-                res[f"bn{bn}"] = round(timeit(lambda: ext.gemm_tuned(a, b, layout, bn, 1, False)), 4)
+                record(f"bn{bn}", timeit(lambda: ext.gemm_tuned(a, b, layout, bn, 0 if layout == 2 else 1, False)))
             except Exception as e:  # noqa: BLE001
                 res[f"bn{bn}"] = f"{type(e).__name__}"
-        res["cublas"] = round(timeit(lambda: torch.matmul(a, b.t() if layout == 0 else b)), 4)
+        if layout == 0:
+            record("cublas", timeit(lambda: torch.matmul(a, b.t())))
+        elif layout == 1:
+            record("cublas", timeit(lambda: torch.matmul(a, b)))
+        else:
+            record("cublas", timeit(lambda: torch.matmul(a.t(), b)))
         out[name] = res
+        del a, b
+        torch.cuda.empty_cache()
     print(json.dumps(out))
 
 

@@ -419,6 +419,7 @@ struct AttnBwdParams {
   float inv_keep;
   const long long* rng_state;
   unsigned* dq_order;   // [B * A * query blocks]: key blocks whose dQ contribution has landed (zeroed by the caller)
+  SpinTimeout* timeout_rec;  // where a timed-out dq_order wait leaves its diagnostic (host-mapped)
 };
 
 template <int D, int BIAS, bool DROP>
@@ -609,7 +610,7 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
     const int q_blk = i_begin + it;
     unsigned* order = p.dq_order + bh * nq + q_blk;
     const int last_kb = p.causal ? q_blk : static_cast<int>(gridDim.x) - 1;
-    if (t == 0) spin_wait_ge_sys(order, static_cast<uint32_t>(last_kb - kv_blk), 0, /*what=*/5, kv_blk);
+    if (t == 0) spin_wait_ge_sys(order, static_cast<uint32_t>(last_kb - kv_blk), 0, p.timeout_rec, /*what=*/5, kv_blk);
     warpgroup_sync(0);
     // ---- dQ_i = dS·K, 64 columns at a time: A = dSᵀ read transposed, B = the K tile read MN-major
 #pragma unroll
@@ -829,6 +830,7 @@ extern "C" int lb_attn_bwd(const void* dout, const void* q, const void* k, const
   p.inv_keep = 256.0f / (256.0f - (float)p.drop_thresh);
   p.rng_state = rng_state;
   p.dq_order = dq_order;
+  p.timeout_rec = lb_host::spin_timeout_record(s);
   cudaError_t e = (D == 64) ? launch_bwd<64>(tq, tk, tv, tdo, p, s) : launch_bwd<128>(tq, tk, tv, tdo, p, s);
   if (e != cudaSuccess) return (int)e;
   const long nvec = rows * D / 8;

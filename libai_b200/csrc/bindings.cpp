@@ -87,6 +87,7 @@ int lb_attn_bwd(const void* dout, const void* q, const void* k, const void* v, c
                 float* dbias, float p_drop, const long long* rng_state, unsigned* dq_order, cudaStream_t s);
 int lb_bias_dropout_residual(const void* x, const void* bias, const void* res, void* y, long rows, int N, float p,
                              const LbRngArgs* rng, const long long* rng_in, long long* rng_out, cudaStream_t s);
+int lb_spin_timeout_report(char* buf, int n);
 }
 
 namespace {
@@ -95,9 +96,18 @@ using at::Tensor;
 
 cudaStream_t cur_stream() { return at::cuda::getCurrentCUDAStream().stream(); }
 
+// description of the device flag wait that timed out and trapped in this process, or "" when none did
+std::string spin_timeout_report() {
+  char buf[256];
+  return std::string(buf, lb_spin_timeout_report(buf, sizeof(buf)));
+}
+
 void check(int code, const char* what) {
-  TORCH_CHECK(code == 0, "libai_b200 kernel '", what, "' failed with code ", code,
-              code > 0 ? std::string(" (") + cudaGetErrorString(static_cast<cudaError_t>(code)) + ")" : std::string());
+  if (code == 0) return;
+  const std::string timeout = spin_timeout_report();
+  TORCH_CHECK(false, "libai_b200 kernel '", what, "' failed with code ", code,
+              code > 0 ? std::string(" (") + cudaGetErrorString(static_cast<cudaError_t>(code)) + ")" : std::string(),
+              timeout.empty() ? std::string() : "; " + timeout);
 }
 
 int dtype_code(const Tensor& t) {
@@ -798,6 +808,7 @@ void p2p_allgather(const Tensor& shard, at::IntArrayRef out_ptrs, at::IntArrayRe
 }  // namespace
 
 TORCH_LIBRARY(libai_b200, m) {
+  m.def("spin_timeout_report() -> str", &spin_timeout_report);
   m.def("ag_gemm(Tensor gathered, Tensor shard, Tensor w, int layout, Tensor? bias, int act, bool need_pre, Tensor? pre_in, Tensor(a!)? colsum, bool fill_local, int world, int rank, int[] peer_buf, int[] peer_flags, int[] peer_done, Tensor(b!) state, int n_comm) -> (Tensor, Tensor)", &ag_gemm);
   m.def("ag_wgrad(Tensor gy, Tensor gathered, Tensor shard, Tensor(a!) out, bool accumulate, int world, int rank, int[] peer_buf, int[] peer_flags, int[] peer_done, Tensor(b!) state, int n_comm) -> ()", &ag_wgrad);
   m.def("gemm_rs(Tensor x, Tensor w, int layout, Tensor? bias, Tensor? residual, int world, int rank, int[] peer_buf, int[] peer_flags, int[] peer_done, Tensor(a!) state, int staging_parity_off) -> Tensor", &gemm_rs);

@@ -66,10 +66,10 @@ LB_DEVICE void signal_peers(const PeerPtrs& flags, int world, int rank, int slot
   for (int q = 0; q < world; ++q)
     st_release_sys(reinterpret_cast<uint32_t*>(flags.p[q]) + slot * world + rank, epoch);
 }
-LB_DEVICE void wait_peers(const PeerPtrs& flags, int world, int rank, int slot, uint32_t epoch) {
+LB_DEVICE void wait_peers(const PeerPtrs& flags, int world, int rank, int slot, uint32_t epoch, SpinTimeout* rec) {
   const uint32_t* mine = reinterpret_cast<const uint32_t*>(flags.p[rank]) + slot * world;
   // bounded (common.cuh): a dead peer turns into a device trap with a diagnostic instead of a hung GPU
-  for (int q = 0; q < world; ++q) spin_wait_ge_sys(mine + q, epoch, 0ull, /*what=*/10 + slot, q);
+  for (int q = 0; q < world; ++q) spin_wait_ge_sys(mine + q, epoch, 0ull, rec, /*what=*/10 + slot, q);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -78,10 +78,11 @@ LB_DEVICE void wait_peers(const PeerPtrs& flags, int world, int rank, int slot, 
 __global__ void __launch_bounds__(256)
 zero_reduce_scatter_kernel(PeerPtrs grads, PeerPtrs flags, float* __restrict__ red, float* __restrict__ sqnorm,
                            size_t lo, size_t n, float scale, int world, int rank, uint32_t epoch,
-                           const float* __restrict__ mc_grad /* multicast address of the gradient buffers, or null */) {
+                           const float* __restrict__ mc_grad /* multicast address of the gradient buffers, or null */,
+                           SpinTimeout* timeout_rec) {
   __shared__ float sm[8];
   if (blockIdx.x == 0 && threadIdx.x == 0) signal_peers(flags, world, rank, /*slot=*/0, epoch);
-  if (threadIdx.x == 0) wait_peers(flags, world, rank, 0, epoch);
+  if (threadIdx.x == 0) wait_peers(flags, world, rank, 0, epoch, timeout_rec);
   __syncthreads();
   const size_t nvec = n / 4;
   float acc_sq = 0.f;
@@ -129,7 +130,8 @@ zero_adam_allgather_kernel(float* __restrict__ master, const float* __restrict__
                            unsigned int* __restrict__ done_counter, const float* __restrict__ clip_ptr, size_t lo,
                            size_t n, float lr, float b1, float b2, float eps, float wd, float bc1, float bc2,
                            int decoupled, int world, int rank, uint32_t epoch,
-                           __nv_bfloat16* __restrict__ mc_param /* multicast address of the parameter buffers, or null */) {
+                           __nv_bfloat16* __restrict__ mc_param /* multicast address of the parameter buffers, or null */,
+                           SpinTimeout* timeout_rec) {
   const float clip = clip_ptr != nullptr ? *clip_ptr : 1.0f;
   const size_t nvec = n / 4;
   for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < nvec; i += (size_t)gridDim.x * blockDim.x) {
@@ -172,23 +174,23 @@ zero_adam_allgather_kernel(float* __restrict__ master, const float* __restrict__
     if (prev == gridDim.x - 1) {
       *done_counter = 0;
       signal_peers(flags, world, rank, /*slot=*/1, epoch);
-      wait_peers(flags, world, rank, 1, epoch);
+      wait_peers(flags, world, rank, 1, epoch, timeout_rec);
     }
   }
 }
 
 // plain device-side barrier (used by tests and between phases that have no data dependency flag)
-__global__ void device_barrier_kernel(PeerPtrs flags, int world, int rank, int slot, uint32_t epoch) {
+__global__ void device_barrier_kernel(PeerPtrs flags, int world, int rank, int slot, uint32_t epoch, SpinTimeout* timeout_rec) {
   if (threadIdx.x == 0) {
     signal_peers(flags, world, rank, slot, epoch);
-    wait_peers(flags, world, rank, slot, epoch);
+    wait_peers(flags, world, rank, slot, epoch, timeout_rec);
   }
 }
 
 // all-gather by P2P stores: every rank pushes its shard into slot `rank` of every peer's buffer
 __global__ void __launch_bounds__(256)
 p2p_allgather_push_kernel(const uint4* __restrict__ shard, PeerPtrs outs, PeerPtrs flags, unsigned int* done_counter,
-                          size_t nvec, int world, int rank, uint32_t epoch) {
+                          size_t nvec, int world, int rank, uint32_t epoch, SpinTimeout* timeout_rec) {
   for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < nvec; i += (size_t)gridDim.x * blockDim.x) {
     const uint4 v = shard[i];
 #pragma unroll 8
@@ -204,7 +206,7 @@ p2p_allgather_push_kernel(const uint4* __restrict__ shard, PeerPtrs outs, PeerPt
     if (prev == gridDim.x - 1) {
       *done_counter = 0;
       signal_peers(flags, world, rank, 2, epoch);
-      wait_peers(flags, world, rank, 2, epoch);
+      wait_peers(flags, world, rank, 2, epoch, timeout_rec);
     }
   }
 }
@@ -233,7 +235,8 @@ extern "C" int lb_zero_reduce_scatter(const long* grad_ptrs, const long* flag_pt
   if (world > lb::MAX_RANKS || (n % 4) || (lo % 4)) return -1;
   lb::zero_reduce_scatter_kernel<<<comm_grid(n / 4), 256, 0, s>>>(to_peers(grad_ptrs, world), to_peers(flag_ptrs, world),
                                                                  red, sqnorm, (size_t)lo, (size_t)n, scale, world, rank,
-                                                                 epoch, reinterpret_cast<const float*>(mc_grad));
+                                                                 epoch, reinterpret_cast<const float*>(mc_grad),
+                                                                 lb_host::spin_timeout_record(s));
   return (int)cudaGetLastError();
 }
 
@@ -245,12 +248,13 @@ extern "C" int lb_zero_adam_allgather(float* master, const float* red, float* m,
   lb::zero_adam_allgather_kernel<<<comm_grid(n / 4), 256, 0, s>>>(
       master, red, m, v, to_peers(param_ptrs, world), to_peers(flag_ptrs, world), done_counter, clip, (size_t)lo,
       (size_t)n, lr, b1, b2, eps, wd, bc1, bc2, decoupled, world, rank, epoch,
-      reinterpret_cast<__nv_bfloat16*>(mc_param));
+      reinterpret_cast<__nv_bfloat16*>(mc_param), lb_host::spin_timeout_record(s));
   return (int)cudaGetLastError();
 }
 
 extern "C" int lb_device_barrier(const long* flag_ptrs, int world, int rank, int slot, unsigned epoch, cudaStream_t s) {
-  lb::device_barrier_kernel<<<1, 32, 0, s>>>(to_peers(flag_ptrs, world), world, rank, slot, epoch);
+  lb::device_barrier_kernel<<<1, 32, 0, s>>>(to_peers(flag_ptrs, world), world, rank, slot, epoch,
+                                             lb_host::spin_timeout_record(s));
   return (int)cudaGetLastError();
 }
 
@@ -259,6 +263,6 @@ extern "C" int lb_p2p_allgather(const void* shard, const long* out_ptrs, const l
   if (nbytes % 16) return -1;
   lb::p2p_allgather_push_kernel<<<comm_grid(nbytes / 16), 256, 0, s>>>(
       (const uint4*)shard, to_peers(out_ptrs, world), to_peers(flag_ptrs, world), done_counter, (size_t)(nbytes / 16),
-      world, rank, epoch);
+      world, rank, epoch, lb_host::spin_timeout_record(s));
   return (int)cudaGetLastError();
 }

@@ -30,9 +30,21 @@ LB_DEVICE bool elect_one() {
 
 // ---------------------------------------------------------------------------------------------
 // cross-GPU flag waits (NVLink peer memory).  Every wait is BOUNDED: a dead or wedged peer must not hang the GPU
-// forever — after `timeout_ns` the waiter prints who/what it was waiting for and traps, which surfaces
+// forever — after `timeout_ns` the waiter records who/what it was waiting for and traps, which surfaces
 // as a CUDA error on the host (the trainer's emergency path / the launcher's restart then take over).
+//
+// The timeout path makes no function call (no printf, no assert, no __noinline__ helper): a call anywhere in a kernel
+// that issues wgmma makes ptxas wait for every wgmma to complete before the next one issues (warning C7510), which
+// the build treats as an error.  The diagnostic goes to a record in host-mapped pinned memory instead, which the host
+// can still read after the trap has destroyed the context (lb_host::spin_timeout_record, read by lb_spin_timeout_report).
 // ---------------------------------------------------------------------------------------------
+struct SpinTimeout {
+  uint32_t claimed;            // the first waiter to time out owns the record
+  uint32_t set;                // the fields below are complete
+  int kind, who, block;
+  uint32_t value, target;
+  unsigned long long flag;     // address of the flag that was waited on
+};
 LB_DEVICE unsigned long long globaltimer_ns() {
   unsigned long long t;
   asm volatile("mov.u64 %0, %%globaltimer;\n" : "=l"(t));
@@ -44,19 +56,29 @@ LB_DEVICE uint32_t ld_acquire_sys_u32(const uint32_t* a) {
   return v;
 }
 constexpr unsigned long long kDefaultSpinTimeoutNs = 120ull * 1000ull * 1000ull * 1000ull;  // 2 min
-// wait until *addr >= target (wrap-safe signed distance); `what`/`who` only label the diagnostic
-static __device__ __noinline__ void spin_timeout_trap(const uint32_t* addr, uint32_t target, int what, int who) {
-  printf("[libai_b200] device spin-wait timed out: kind=%d rank/peer=%d flag=%p value=%u target=%u (block %d)\n", what, who,
-         (const void*)addr, ld_acquire_sys_u32(addr), target, (int)blockIdx.x);
-  __trap();
-}
-LB_DEVICE void spin_wait_ge_sys(const uint32_t* addr, uint32_t target, unsigned long long timeout_ns, int what, int who) {
+// wait until *addr >= target (wrap-safe signed distance); `what`/`who` only label the diagnostic written to `rec`
+// (may be null: then the waiter traps without a record)
+LB_DEVICE void spin_wait_ge_sys(const uint32_t* addr, uint32_t target, unsigned long long timeout_ns, SpinTimeout* rec,
+                                int what, int who) {
   if (static_cast<int32_t>(ld_acquire_sys_u32(addr) - target) >= 0) return;
   const unsigned long long t0 = globaltimer_ns();
   const unsigned long long budget = timeout_ns ? timeout_ns : kDefaultSpinTimeoutNs;
   uint32_t polls = 0;
   while (static_cast<int32_t>(ld_acquire_sys_u32(addr) - target) < 0) {
-    if ((++polls & 1023u) == 0 && globaltimer_ns() - t0 > budget) spin_timeout_trap(addr, target, what, who);
+    if ((++polls & 1023u) == 0 && globaltimer_ns() - t0 > budget) {
+      if (rec != nullptr && atomicCAS(&rec->claimed, 0u, 1u) == 0u) {
+        rec->kind = what;
+        rec->who = who;
+        rec->block = static_cast<int>(blockIdx.x);
+        rec->value = ld_acquire_sys_u32(addr);
+        rec->target = target;
+        rec->flag = reinterpret_cast<unsigned long long>(addr);
+        __threadfence_system();
+        *reinterpret_cast<volatile uint32_t*>(&rec->set) = 1u;
+        __threadfence_system();
+      }
+      asm volatile("trap;");
+    }
   }
 }
 
@@ -345,4 +367,7 @@ bool make_tmap_typed(CUtensorMap* out, CUtensorMapDataType dtype, const void* ba
                      const uint64_t* strides_bytes, const uint32_t* box, CUtensorMapSwizzle swizzle);
 bool make_tmap_bf16(CUtensorMap* out, const void* base, int rank, const uint64_t* dims, const uint64_t* strides_bytes,
                     const uint32_t* box, CUtensorMapSwizzle swizzle);
+// the process-wide lb::SpinTimeout record (host-mapped pinned memory, allocated on first use); null when it does not
+// exist yet and `s` is being captured into a CUDA graph, or when the allocation failed
+lb::SpinTimeout* spin_timeout_record(cudaStream_t s);
 }  // namespace lb_host

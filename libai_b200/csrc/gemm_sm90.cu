@@ -86,6 +86,7 @@ struct CommParams {
   __nv_bfloat16* rs_out;        // RS: [rows_per_rank, N]
   long staging_parity_off;      // RS: element offset of the staging half used by this call
   unsigned long long timeout_ns;  // bound of every cross-GPU flag wait (0 = default)
+  SpinTimeout* timeout_rec;       // where a timed-out wait leaves its diagnostic (host-mapped)
 };
 
 // streaming (non-volatile, L1 no-allocate) 128-bit load: many of these stay in flight per thread over NVLink
@@ -257,7 +258,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
         mbar_wait(&bars[slot], (stored / NSLOT) & 1);
         const int dst = dst_of(q_st);
         if (!((dst_ok_mask >> dst) & 1u)) {
-          spin_wait_ge_sys(cp.peer_done[cp.rank] + dst, call_idx, cp.timeout_ns, /*what=*/3, dst);
+          spin_wait_ge_sys(cp.peer_done[cp.rank] + dst, call_idx, cp.timeout_ns, cp.timeout_rec, /*what=*/3, dst);
           dst_ok_mask |= 1u << dst;
         }
         uint8_t* dp = reinterpret_cast<uint8_t*>(cp.peer_buf[dst]) + static_cast<size_t>(blk_of(q_st)) * blk_bytes +
@@ -301,7 +302,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
         // from the gathered buffer once that peer's copy CTAs have pushed the row block (arrival counter)
         const bool a_local = cp.mode == COMM_AG && !ag_b && m_blk / mbpr == cp.rank;
         if (cp.mode == COMM_AG && !ag_b && !a_local) {
-          spin_wait_ge_sys(cp.peer_flags[cp.rank] + m_blk, arrive_target, cp.timeout_ns, /*what=*/1, m_blk / mbpr);
+          spin_wait_ge_sys(cp.peer_flags[cp.rank] + m_blk, arrive_target, cp.timeout_ns, cp.timeout_rec, /*what=*/1, m_blk / mbpr);
           asm volatile("fence.proxy.async.global;\n" ::: "memory");
         }
         const CUtensorMap* map_a = a_local ? &tmap_g : &tmap_a;
@@ -315,7 +316,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
             const int blk = (kb * BLOCK_K) / BLOCK_M;
             b_local = blk / mbpr == cp.rank;
             if (!b_local && blk != waited_blk) {
-              spin_wait_ge_sys(cp.peer_flags[cp.rank] + blk, arrive_target, cp.timeout_ns, /*what=*/1, blk / mbpr);
+              spin_wait_ge_sys(cp.peer_flags[cp.rank] + blk, arrive_target, cp.timeout_ns, cp.timeout_rec, /*what=*/1, blk / mbpr);
               asm volatile("fence.proxy.async.global;\n" ::: "memory");
               waited_blk = blk;
             }
@@ -360,7 +361,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
       // buffer set (its reduce phase read what we stored then) before the first partial tile of this call lands
       if (lane == 0) {
         for (int q = 0; q < cp.world; ++q)
-          if (q != cp.rank) spin_wait_ge_sys(cp.peer_done[cp.rank] + q, call_idx, cp.timeout_ns, /*what=*/4, q);
+          if (q != cp.rank) spin_wait_ge_sys(cp.peer_done[cp.rank] + q, call_idx, cp.timeout_ns, cp.timeout_rec, /*what=*/4, q);
       }
       __syncwarp();
     }
@@ -524,7 +525,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
     };
     for (int u = blockIdx.x; u < units; u += gridDim.x) {
       const int lm = u / col_groups, cg = u % col_groups;
-      if (threadIdx.x == 0) spin_wait_ge_sys(cp.peer_flags[cp.rank] + lm, arrive_target, cp.timeout_ns, /*what=*/2, lm);
+      if (threadIdx.x == 0) spin_wait_ge_sys(cp.peer_flags[cp.rank] + lm, arrive_target, cp.timeout_ns, cp.timeout_rec, /*what=*/2, lm);
       __syncthreads();
       const int c_lo = cg * 256;
       const int c_n = min(256, p.N - c_lo) / 8;  // vectors of 8 per row in this column group
@@ -663,7 +664,42 @@ bool make_tmap_bf16(CUtensorMap* out, const void* base, int rank, const uint64_t
   return make_tmap_typed(out, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, base, rank, dims, strides_bytes, box, swizzle);
 }
 
+static lb::SpinTimeout* g_spin_timeout = nullptr;
+
+lb::SpinTimeout* spin_timeout_record(cudaStream_t s) {
+  static std::mutex mu;
+  std::lock_guard<std::mutex> lock(mu);
+  if (g_spin_timeout != nullptr) return g_spin_timeout;
+  cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
+  if (cudaStreamIsCapturing(s, &cap) != cudaSuccess || cap != cudaStreamCaptureStatusNone) return nullptr;
+  void* host = nullptr;
+  if (cudaHostAlloc(&host, sizeof(lb::SpinTimeout), cudaHostAllocMapped | cudaHostAllocPortable) != cudaSuccess) {
+    cudaGetLastError();
+    return nullptr;
+  }
+  memset(host, 0, sizeof(lb::SpinTimeout));
+  void* dev = nullptr;
+  if (cudaHostGetDevicePointer(&dev, host, 0) != cudaSuccess) {
+    cudaGetLastError();
+    cudaFreeHost(host);
+    return nullptr;
+  }
+  g_spin_timeout = static_cast<lb::SpinTimeout*>(dev);
+  return g_spin_timeout;
+}
+
 }  // namespace lb_host
+
+// Writes a one-line description of the flag wait that timed out into buf (n bytes) and returns its length, or 0 when
+// no wait has timed out.  Reads host memory only, so it works after the trap has left the CUDA context unusable.
+extern "C" int lb_spin_timeout_report(char* buf, int n) {
+  const volatile lb::SpinTimeout* r = lb_host::g_spin_timeout;
+  if (r == nullptr || r->set == 0u || n <= 0) return 0;
+  const int len = snprintf(buf, n,
+                           "device flag wait timed out: kind=%d rank/peer=%d flag=0x%llx value=%u target=%u (block %d)",
+                           r->kind, r->who, r->flag, r->value, r->target, r->block);
+  return len < n ? len : n - 1;
+}
 
 namespace {
 
@@ -747,7 +783,7 @@ static int gemm_impl(const void* a, const void* b, void* out, int M, int N, int 
   const bool b_mn = (layout != 0);
   const int sms = num_sms();
   const int m_blocks = (M + lb::BLOCK_M - 1) / lb::BLOCK_M;
-  // ---- tile-N heuristic: fewest waves, ties -> wider tile (less smem traffic per flop)
+  // ---- tile-N heuristic: least estimated time (waves x per-tile time), ties -> wider tile
   int bn = force_bn;
   if (bn == 0 && epi == 2 && cp.mode == lb::COMM_AG && cp.gathered_is_b) {
     // gathered-B wgrad: split-K fills the machine, so take the widest tile that fits N
@@ -756,14 +792,19 @@ static int gemm_impl(const void* a, const void* b, void* out, int M, int N, int 
   if (bn == 0) {
     double best = 1e30;
     const int cands[4] = {256, 192, 128, 64};
+    const double k_blocks = (double)((K + lb::BLOCK_K - 1) / lb::BLOCK_K);
     for (int c : cands) {
       if (c > 64 && N <= c / 2) continue;
       const long tiles = (long)m_blocks * ((N + c - 1) / c);
       const long waves = (tiles + sms - 1) / sms;
-      // cost ~ waves * per-tile time (proportional to c, narrower tiles pay more shared-memory traffic per
-      // flop, plus a fixed prologue/epilogue overhead per tile)
-      const double eff = c == 256 ? 1.0 : (c == 192 ? 1.03 : (c == 128 ? 1.08 : 1.2));
-      const double cost = (double)waves * (c * eff + 24.0);
+      // cost ~ waves * per-tile time in microseconds = main loop (c * k-blocks * per-column cost: narrower tiles pay
+      // more shared-memory traffic per flop) + epilogue.  The bf16 epilogue grows faster than the tile width, so with
+      // a short K (1024: the forward and most dgrad GEMMs of a transformer) narrow tiles win and only a long K pays
+      // for a wide one; the fp32 epilogues (wgrad) are cheap at every width.  Fitted to dev/gemm_sweep.py on an
+      // H100 SXM (700 W).
+      const double per_col = c == 256 ? 0.00286 : (c == 192 ? 0.00272 : (c == 128 ? 0.00332 : 0.00414));
+      const double epilogue = epi != 0 ? 4.0 : (c == 256 ? 54.0 : (c == 192 ? 24.4 : (c == 128 ? 11.6 : 4.2)));
+      const double cost = (double)waves * (c * k_blocks * per_col + epilogue);
       if (cost < best - 1e-9) {
         best = cost;
         bn = c;
@@ -963,6 +1004,7 @@ extern "C" int lb_gemm_bf16_comm(const void* a, const void* b, void* out, int M,
   cp.rs_out = reinterpret_cast<__nv_bfloat16*>(rs_out);
   cp.staging_parity_off = staging_parity_off;
   cp.timeout_ns = spin_timeout_ns();
+  cp.timeout_rec = lb_host::spin_timeout_record(stream);
   {
     static int rings = -1;
     if (rings < 0) {

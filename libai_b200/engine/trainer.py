@@ -91,6 +91,11 @@ class TrainerBase:
                 self.interrupted = True
             except Exception:
                 logger.exception("Exception during training:")
+                from libai_b200.ops import spin_timeout_report
+
+                timeout = spin_timeout_report()
+                if timeout:
+                    logger.error("%s", timeout)
                 raise
             finally:
                 self.after_train()

@@ -76,6 +76,13 @@ def load_ext(required: bool = True):
     return _EXT
 
 
+def spin_timeout_report() -> str:
+    """Who and what the device flag wait that timed out (and trapped) in this process was waiting for; ``""`` when
+    none did or the extension is not loaded.  The record lives in host memory, so this works after the trap has made
+    the CUDA context unusable."""
+    return _EXT.spin_timeout_report() if _EXT is not None else ""
+
+
 def use_native(*tensors) -> bool:
     """True when the native sm_90a kernel must be used for these tensors."""
     if impl() != "native":

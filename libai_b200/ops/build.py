@@ -40,6 +40,20 @@ def _run(cmd, verbose):
     return res.stdout
 
 
+def serialized_wgmma(log: str) -> list:
+    """ptxas warning C7510 means that it made every wgmma of a kernel wait for the previous one to complete (for
+    example because the kernel contains a function call), which turns the asynchronous tensor-core pipeline into a
+    serial one.  Returns the distinct such warnings of a ptxas log, demangled; each names the function it blames."""
+    lines = list(dict.fromkeys(ln.split("(C7510)", 1)[-1].strip() for ln in log.splitlines() if "C7510" in ln))
+    if lines:
+        try:
+            lines = subprocess.run(["c++filt"], input="\n".join(lines), stdout=subprocess.PIPE, text=True,
+                                   check=True).stdout.splitlines()
+        except (OSError, subprocess.CalledProcessError):
+            pass
+    return lines
+
+
 def _stale(src, obj, deps=()):
     if not os.path.exists(obj):
         return True
@@ -80,6 +94,14 @@ def build(force: bool = False, verbose: bool = False, sass: bool = False) -> str
         with open(os.path.join(BUILD, "ptxas.log"), "w") as f:
             for name, out in logs.items():
                 f.write(f"==== {name}\n{out}\n")
+        serialized = {name: serialized_wgmma(out) for name, out in logs.items()}
+        serialized = {name: lines for name, lines in serialized.items() if lines}
+        if serialized:
+            for name in serialized:   # the next build must compile them again, not link the serialized objects
+                os.remove(os.path.join(BUILD, name + ".o"))
+            raise RuntimeError("ptxas serialized wgmma (C7510); kernels that issue wgmma must not contain a function "
+                               "call:\n" + "\n".join(f"{name}: {ln}" for name, lines in serialized.items()
+                                                    for ln in lines))
     if jobs or force or not os.path.exists(SO_PATH):
         tlib = os.path.join(os.path.dirname(torch.__file__), "lib")
         _run(["g++", "-shared", "-o", SO_PATH, *objs, f"-L{tlib}", "-lc10", "-ltorch_cpu", "-ltorch", "-lc10_cuda",
