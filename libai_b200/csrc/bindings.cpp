@@ -88,6 +88,12 @@ int lb_attn_bwd(const void* dout, const void* q, const void* k, const void* v, c
 int lb_bias_dropout_residual(const void* x, const void* bias, const void* res, void* y, long rows, int N, float p,
                              const LbRngArgs* rng, const long long* rng_in, long long* rng_out, cudaStream_t s);
 int lb_spin_timeout_report(char* buf, int n);
+int lb_decode_splits(int B, int A, int C, int D);
+int lb_decode_attn(const void* q, const long* q_strides, const void* k, const void* v, void* o, float* part_o,
+                   float* part_ml, const int* seqlens, const int* kv_start, int B, int Sq, int A, int C, int D, float scale,
+                   int nsplit, cudaStream_t s);
+int lb_kv_append(const void* qkv, const float* cosv, const float* sinv, void* q_out, void* k_cache, void* v_cache,
+                 const int* seqlens, int B, int Sq, int A, int C, int D, cudaStream_t s);
 }
 
 namespace {
@@ -649,6 +655,86 @@ std::tuple<Tensor, Tensor, Tensor> attn_fwd(const Tensor& q, const Tensor& k, co
   return std::make_tuple(o.permute({0, 2, 1, 3}), lse, rng_state);
 }
 
+// ---- KV-cache decoding ------------------------------------------------------------------------------
+// The cache capacity C (rows per head) cannot be checked against the device-side lengths without a host sync: the
+// caller (libai_b200.inference.kv_cache.StaticKVCache) guarantees cache_seqlens[b] + Sq <= C before every call.
+void check_cache(const Tensor& k_cache, const Tensor& v_cache, const char* what) {
+  TORCH_CHECK(k_cache.is_cuda() && k_cache.scalar_type() == at::kBFloat16 && v_cache.scalar_type() == at::kBFloat16,
+              what, ": bf16 CUDA cache expected");
+  TORCH_CHECK(k_cache.dim() == 4 && k_cache.sizes() == v_cache.sizes() && k_cache.is_contiguous() && v_cache.is_contiguous(),
+              what, ": K and V caches must be contiguous [B, A, C, D] of the same shape");
+  TORCH_CHECK(k_cache.size(3) == 64 || k_cache.size(3) == 128, what, ": head dim must be 64 or 128");
+  TORCH_CHECK(reinterpret_cast<uintptr_t>(k_cache.data_ptr()) % 16 == 0 &&
+              reinterpret_cast<uintptr_t>(v_cache.data_ptr()) % 16 == 0, what, ": caches must be 16-byte aligned");
+}
+void check_lengths(const Tensor& t, int64_t B, const char* what) {
+  TORCH_CHECK(t.is_cuda() && t.scalar_type() == at::kInt && t.dim() == 1 && t.size(0) == B && t.is_contiguous(), what,
+              ": int32 CUDA [B] expected");
+}
+
+// k, v of the packed projection qkv [B, Sq, A, 3D] go to rows cache_seqlens[b] + i of the caches; with cos/sin (fp32
+// [>= positions, D]) q and k are rotated first.  Returns the (rotated) q as [B, Sq, A, D] when write_q, else empty.
+Tensor kv_append(const Tensor& qkv, const Tensor& k_cache, const Tensor& v_cache, const Tensor& cache_seqlens,
+                 const c10::optional<Tensor>& cosv, const c10::optional<Tensor>& sinv, bool write_q) {
+  c10::cuda::CUDAGuard guard(qkv.device());
+  check_cache(k_cache, v_cache, "kv_append");
+  const int B = (int)k_cache.size(0), A = (int)k_cache.size(1), C = (int)k_cache.size(2), D = (int)k_cache.size(3);
+  TORCH_CHECK(qkv.is_cuda() && qkv.scalar_type() == at::kBFloat16 && qkv.dim() == 4 && qkv.is_contiguous(),
+              "kv_append: contiguous bf16 qkv [B, Sq, A, 3D] expected");
+  TORCH_CHECK(qkv.size(0) == B && qkv.size(2) == A && qkv.size(3) == 3 * D, "kv_append: qkv does not match the cache");
+  const int Sq = (int)qkv.size(1);
+  TORCH_CHECK(Sq >= 1 && Sq <= C, "kv_append: 1 <= Sq <= capacity");
+  check_lengths(cache_seqlens, B, "kv_append: cache_seqlens");
+  const float* cp = nullptr;
+  const float* sp = nullptr;
+  if (cosv.has_value() && cosv->defined()) {
+    TORCH_CHECK(sinv.has_value() && sinv->defined(), "kv_append: cos and sin go together");
+    TORCH_CHECK(cosv->scalar_type() == at::kFloat && sinv->scalar_type() == at::kFloat && cosv->is_contiguous() &&
+                sinv->is_contiguous() && cosv->dim() == 2 && cosv->size(1) == D && cosv->sizes() == sinv->sizes() &&
+                cosv->is_cuda(), "kv_append: cos/sin fp32 contiguous [positions, D]");
+    // like the capacity, the rows of the tables (positions up to cache_seqlens[b] + Sq - 1) are the caller's guarantee
+    cp = cosv->data_ptr<float>();
+    sp = sinv->data_ptr<float>();
+  }
+  Tensor q_out = write_q ? at::empty({B, Sq, A, D}, qkv.options()) : at::empty({0}, qkv.options());
+  check(lb_kv_append(qkv.data_ptr(), cp, sp, write_q ? q_out.data_ptr() : nullptr, k_cache.data_ptr(),
+                     v_cache.data_ptr(), cache_seqlens.data_ptr<int>(), B, Sq, A, C, D, cur_stream()),
+        "kv_append");
+  return q_out;
+}
+
+// q [B, Sq, A, D] (any strides with D contiguous, e.g. a view of the packed projection) against the caches; query i of
+// sample b sees keys kv_start[b] .. cache_seqlens[b] + i.  Returns o [B, Sq, A, D] contiguous.  splits = 0: automatic.
+Tensor decode_attn(const Tensor& q, const Tensor& k_cache, const Tensor& v_cache, const Tensor& cache_seqlens,
+                   const Tensor& kv_start, double scale, int64_t splits) {
+  c10::cuda::CUDAGuard guard(q.device());
+  check_cache(k_cache, v_cache, "decode_attn");
+  const int B = (int)k_cache.size(0), A = (int)k_cache.size(1), C = (int)k_cache.size(2), D = (int)k_cache.size(3);
+  TORCH_CHECK(q.is_cuda() && q.scalar_type() == at::kBFloat16 && q.dim() == 4 && q.stride(3) == 1,
+              "decode_attn: bf16 q [B, Sq, A, D] with D contiguous expected");
+  TORCH_CHECK(q.size(0) == B && q.size(2) == A && q.size(3) == D, "decode_attn: q does not match the cache");
+  const int Sq = (int)q.size(1);
+  TORCH_CHECK(Sq >= 1 && Sq <= 16, "decode_attn: 1 <= Sq <= 16 new queries");
+  TORCH_CHECK(reinterpret_cast<uintptr_t>(q.data_ptr()) % 16 == 0 && q.stride(0) % 8 == 0 && q.stride(1) % 8 == 0 &&
+              q.stride(2) % 8 == 0, "decode_attn: q must be 16-byte aligned with strides that are multiples of 8");
+  check_lengths(cache_seqlens, B, "decode_attn: cache_seqlens");
+  check_lengths(kv_start, B, "decode_attn: kv_start");
+  const int nsplit = splits > 0 ? (int)std::min<int64_t>(splits, 32) : lb_decode_splits(B, A, C, D);
+  Tensor o = at::empty({B, Sq, A, D}, q.options());
+  Tensor part_o, part_ml;
+  if (nsplit > 1) {
+    part_o = at::empty({(int64_t)B * A * nsplit * Sq * D}, q.options().dtype(at::kFloat));
+    part_ml = at::empty({(int64_t)B * A * nsplit * Sq * 2}, q.options().dtype(at::kFloat));
+  }
+  long qs[3] = {q.stride(0), q.stride(1), q.stride(2)};
+  check(lb_decode_attn(q.data_ptr(), qs, k_cache.data_ptr(), v_cache.data_ptr(), o.data_ptr(),
+                       nsplit > 1 ? part_o.data_ptr<float>() : nullptr, nsplit > 1 ? part_ml.data_ptr<float>() : nullptr,
+                       cache_seqlens.data_ptr<int>(), kv_start.data_ptr<int>(), B, Sq, A, C, D, (float)scale, nsplit,
+                       cur_stream()),
+        "decode_attn");
+  return o;
+}
+
 // `dbias` (optional, fp32, same shape as `bias`): the gradient of a learned bias is accumulated into it
 std::tuple<Tensor, Tensor, Tensor, Tensor> attn_bwd(const Tensor& dout, const Tensor& q, const Tensor& k, const Tensor& v,
                                             const Tensor& o, const Tensor& lse, bool causal, double scale,
@@ -844,5 +930,7 @@ TORCH_LIBRARY(libai_b200, m) {
   m.def("sqnorm(Tensor x) -> Tensor", &sqnorm);
   m.def("attn_fwd(Tensor q, Tensor k, Tensor v, bool causal, float scale, Tensor? kv_lens, Tensor? bias=None, Tensor? alibi_slopes=None, float p_drop=0.0, int salt=0) -> (Tensor, Tensor, Tensor)", &attn_fwd);
   m.def("attn_bwd(Tensor dout, Tensor q, Tensor k, Tensor v, Tensor o, Tensor lse, bool causal, float scale, Tensor? kv_lens, Tensor? bias=None, Tensor? alibi_slopes=None, Tensor(a!)? dbias=None, float p_drop=0.0, Tensor? rng_state=None) -> (Tensor, Tensor, Tensor, Tensor)", &attn_bwd);
+  m.def("kv_append(Tensor qkv, Tensor(a!) k_cache, Tensor(b!) v_cache, Tensor cache_seqlens, Tensor? cos, Tensor? sin, bool write_q) -> Tensor", &kv_append);
+  m.def("decode_attn(Tensor q, Tensor k_cache, Tensor v_cache, Tensor cache_seqlens, Tensor kv_start, float scale, int splits=0) -> Tensor", &decode_attn);
   m.def("bias_dropout_residual(Tensor x, Tensor? bias, Tensor? res, float p, int salt, Tensor? rng_state=None) -> (Tensor, Tensor)", &bias_dropout_residual);
 }

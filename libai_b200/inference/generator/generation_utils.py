@@ -22,6 +22,7 @@ import torch
 from libai_b200.utils import distributed as dutil
 import torch.distributed as dist
 
+from ..kv_cache import StaticKVCache
 from .generation_beam_search import BeamScorer, BeamSearchScorer
 from .generation_logits_processor import (
     EncoderNoRepeatNGramLogitsProcessor,
@@ -163,10 +164,13 @@ class Generator:
             model_kwargs["past"] = outputs["past_key_values"]
         else:
             past = getattr(self, "past_key_values", None)
-            # under pipeline parallelism a rank only holds the caches of its own layers (possibly none at all): the
-            # model's `past_length` says whether a cache exists somewhere
-            cached = bool(past) and (any(p is not None for p in past) or (
-                dutil.get_dist_util().pipeline_parallel_size > 1 and getattr(self, "past_length", 0) > 0))
+            if isinstance(past, StaticKVCache):
+                cached = past.length > 0   # the host mirror: valid on stages that own no layer, too
+            else:
+                # under pipeline parallelism a rank only holds the caches of its own layers (possibly none at all): the
+                # model's `past_length` says whether a cache exists somewhere
+                cached = bool(past) and (any(p is not None for p in past) or (
+                    dutil.get_dist_util().pipeline_parallel_size > 1 and getattr(self, "past_length", 0) > 0))
             model_kwargs["past"] = past if cached else None
         key = "decoder_attn_mask" if is_encoder_decoder else "attention_mask"
         if model_kwargs.get(key) is not None:
@@ -175,9 +179,13 @@ class Generator:
         return model_kwargs
 
     def _reorder_cache(self, past, beam_idx):
-        """Default: every cached tensor is batch-major; models with another layout override this."""
+        """Default: every cached tensor is batch-major; models with another layout override this.  A
+        :class:`StaticKVCache` is gathered in place."""
         if past is None:
             return None
+        if isinstance(past, StaticKVCache):
+            past.reorder_(beam_idx)
+            return past
 
         def reorder(x):
             if torch.is_tensor(x):
@@ -553,6 +561,11 @@ class Generator:
             renormalize_logits=renormalize_logits,
         )
         stopping_criteria = self._get_stopping_criteria(max_length, max_time, stopping_criteria)
+        # models with a preallocated cache size it once for every sequence the search runs
+        allocate = getattr(self, "allocate_kv_cache", None)
+        if allocate is not None and model_kwargs.get("use_cache") and stopping_criteria.max_length is not None:
+            rows = batch_size * (num_beams if is_beam else num_return_sequences if is_sample else 1)
+            allocate(rows, stopping_criteria.max_length)
 
         was_training = self.training
         self.eval()

@@ -8,6 +8,8 @@ The pipeline hand-off the reference performs inside ``forward`` (``to_global(pla
 """
 from torch import nn
 
+from libai_b200.inference.kv_cache import KVCacheLayer
+
 from ._param import xavier_normal_
 from .attention import AttnMaskType, MultiheadAttention
 from .droppath import DropPath
@@ -90,7 +92,9 @@ class TransformerLayer(nn.Module):
         """``past_key_value``: ``(self_k, self_v[, cross_k, cross_v])``; returns hidden states, and
         the updated cache tuple when ``use_cache``."""
         self_past = cross_past = None
-        if past_key_value is not None:
+        if isinstance(past_key_value, KVCacheLayer):   # preallocated self-attention cache (decoder-only models)
+            self_past = past_key_value
+        elif past_key_value is not None:
             self_past = past_key_value[:2]
             cross_past = past_key_value[2:] if len(past_key_value) > 2 else None
             cross_past = cross_past or None

@@ -29,6 +29,7 @@ from libai_b200.parallel import mappings
 from libai_b200.utils import distributed as dutil
 
 from libai_b200.inference.generator.generation_utils import Generator
+from libai_b200.inference.kv_cache import KVCacheLayer, KVCacheOwner, StaticKVCache, left_padding
 
 from .utils.pipeline_model import PipelineStageMixin
 from .utils.weight_init import init_method_normal, scaled_init_method_normal
@@ -132,6 +133,11 @@ class LlamaAttention(nn.Module):
         a, d = self.local_heads, self.head_size
         bsz, tgt_len = get_sp_shape() if sp else hidden_states.shape[:2]
         qkv = self.query_key_value(hidden_states).view(bsz, -1, a, 3 * d)
+        if isinstance(past_key_value, KVCacheLayer):
+            context = self._cached_attention(qkv, attention_mask, past_key_value, cos_cached, sin_cached)
+            context = context.reshape(-1, a * d) if sp else context.reshape(bsz, -1, a * d)
+            output = self.o_proj(context)
+            return (output, past_key_value) if use_cache else output
         past_len = 0 if past_key_value is None else past_key_value[0].shape[2]
         qkv = OF.apply_rotary_qkv(qkv, cos_cached, sin_cached, past_len)
         if (
@@ -157,6 +163,22 @@ class LlamaAttention(nn.Module):
             context = context.reshape(-1, a * d)
         output = self.o_proj(context)
         return (output, past_key_value) if use_cache else output
+
+    def _cached_attention(self, qkv, attention_mask, cache, cos, sin):
+        """Rotary + append into the layer's cache, then attention over it → ``[b, s, a, d]``.  Steps after the prefill
+        (padding carried by ``cache.kv_start``) go to :func:`OF.decode_attention`: the split-KV kernel for bf16 with head
+        dim 64 / 128 and up to 16 new tokens, the reference math otherwise.  The prefill runs the usual dispatch (flash
+        kernel for a causal prompt) on views of the cache, and a dense ``attention_mask`` keeps the reference math."""
+        past, s_len = cache.length, qkv.shape[1]
+        q = OF.kv_cache_append(qkv, cache.k, cache.v, cache.seqlens, cos, sin)
+        if past > 0 and attention_mask is None:
+            return OF.decode_attention(q, cache.k, cache.v, cache.seqlens, cache.kv_start, scale=self.norm_factor)
+        L = past + s_len
+        key, value = cache.k[:, :, :L], cache.v[:, :, :L]
+        causal = attention_mask is None   # prefill of an unpadded prompt
+        context = OF.attention(q.permute(0, 2, 1, 3), key, value, causal=causal, scale=self.norm_factor,
+                               mask=attention_mask)
+        return context.transpose(1, 2)
 
 
 class CasualMask(nn.Module):
@@ -245,6 +267,17 @@ class LlamaModel(nn.Module):
         return self.embed_tokens(input_ids)
 
     def forward(self, input_ids, attention_mask=None, past_key_values=None, use_cache=False, set_cache=None):
+        if isinstance(past_key_values, StaticKVCache):
+            # the layers append in place; the lengths advance once every layer has seen this step's tokens
+            cache = past_key_values
+            if self.cos_cached.device != input_ids.device:   # tables built on the CPU for a model built on the GPU
+                self.cos_cached, self.sin_cached = self.cos_cached.to(input_ids.device), self.sin_cached.to(input_ids.device)
+            hidden_states = self.embed(input_ids)
+            for i, layer in enumerate(self.layers):
+                hidden_states = layer(hidden_states, attention_mask=attention_mask, past_key_value=cache.layer(i),
+                                      cos_cached=self.cos_cached, sin_cached=self.sin_cached, use_cache=False)
+            cache.advance(input_ids.shape[1])
+            return self.norm(hidden_states)
         presents = [] if use_cache else None
         hidden_states = self.embed(input_ids)
         past_key_values = past_key_values or [None] * len(self.layers)
@@ -286,7 +319,7 @@ class SFTLoss(nn.Module):
         return {"lm_loss": (loss * keep).sum() / keep.sum().clamp(min=1.0)}
 
 
-class LlamaForCausalLM(nn.Module, PipelineStageMixin, Generator):
+class LlamaForCausalLM(nn.Module, PipelineStageMixin, Generator, KVCacheOwner):
 
     # `train.dist.sequence_parallel = "auto"` resolves to True for this model (token-sharded activations between
     # the tensor-parallel blocks are handled by its embeddings / heads)
@@ -312,7 +345,7 @@ class LlamaForCausalLM(nn.Module, PipelineStageMixin, Generator):
         self.lm_head = Linear(hidden_size, vocab_size, bias=False, parallel="col",
                               init_method=init_method_normal(initializer_range), layer_idx=-1)
         self.loss_func = SFTLoss()
-        self.past_key_values: List[Optional[Tuple[torch.Tensor, torch.Tensor]]] = [None] * hidden_layers
+        self.kv_cache: Optional[StaticKVCache] = None
         self.past_length = 0
 
     @classmethod
@@ -354,27 +387,32 @@ class LlamaForCausalLM(nn.Module, PipelineStageMixin, Generator):
         if not use_cache and attention_mask is None:
             return self.forward_stage({"input_ids": input_ids, "labels": labels})
         # generation / padded batches: explicit masks and the KV cache (single pipeline stage)
-        self.past_length = self.past_key_values[0][0].size(-2) if use_cache and self.past_key_values[0] is not None else 0
-        mask = None
-        if attention_mask is not None or self.past_length == 0:
-            mask = self.casual_mask(input_ids, past_length=self.past_length, attention_mask=attention_mask)
-            if attention_mask is None:
-                mask = None  # pure causal prefill: let the kernel apply causality
-        output = self.model(input_ids, attention_mask=mask, past_key_values=self.past_key_values if use_cache else None,
-                            use_cache=use_cache, set_cache=self.set_cache)
+        if not use_cache:
+            mask = None if attention_mask is None else self.casual_mask(input_ids, attention_mask=attention_mask)
+            output = self.model(input_ids, attention_mask=mask)
+        else:
+            cache = self._prepare_cache(input_ids, max_positions=self.model.cos_cached.shape[0])
+            self.past_length = past = cache.length
+            mask = None
+            if attention_mask is not None:
+                if past == 0:
+                    kv_start = left_padding(attention_mask) if attention_mask.dim() == 2 else None
+                    cache.dense_mask = kv_start is None
+                    if kv_start is not None:
+                        cache.kv_start.copy_(kv_start)
+                if past == 0 or cache.dense_mask:
+                    # the prefill of a padded prompt (and every step of a mask kv_start cannot express) is dense
+                    mask = self.casual_mask(input_ids, past_length=past, attention_mask=attention_mask)
+            output = self.model(input_ids, attention_mask=mask, past_key_values=cache)
+            self.past_length = cache.length
         logits = self.lm_head(output)
         if labels is not None:
             return self.loss_func(logits, labels)
         return {"logits": self._full_logits(logits)}
 
-    def set_cache(self, past_key_values):
-        self.past_length = 0 if past_key_values is None else past_key_values[0][0].shape[2]
-        if past_key_values is None:
-            past_key_values = [None] * self.hidden_layers
-        assert len(past_key_values) == self.hidden_layers, (
-            f"past_key_values's length {len(past_key_values)} doesn't match num_layers:' {self.hidden_layers}"
-        )
-        self.past_key_values = list(past_key_values)
+    # ---- KV cache (KVCacheOwner) ----------------------------------------------------------------
+    def _cache_attention_modules(self):
+        return [layer.self_attn for layer in self.model.layers]
 
     def prepare_inputs_for_generation(self, input_ids, past=None, attention_mask=None, use_cache=None, **kwargs):
         """With a warm cache only the newest token is fed; the padding mask always covers cache + new tokens."""

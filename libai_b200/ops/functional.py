@@ -663,6 +663,82 @@ def attention(q, k, v, *, causal: bool = False, scale: Optional[float] = None, m
 
 
 # --------------------------------------------------------------------------------------
+# KV-cache decoding: caches are [b, a, C, d] buffers (libai_b200.inference.kv_cache.StaticKVCache); ``cache_seqlens``
+# (int32 [b]) is the number of rows already held, ``kv_start`` (int32 [b]) the left padding of each sample
+# --------------------------------------------------------------------------------------
+def _decode_native(x, k_cache) -> bool:
+    """The decode kernels take bf16 projections and caches with head dim 64 or 128; other dtypes and head dims run the
+    reference math (as :func:`attention` does)."""
+    return (
+        use_native(x)
+        and x.dtype == torch.bfloat16
+        and k_cache.dtype == torch.bfloat16
+        and k_cache.shape[-1] in (64, 128)
+    )
+
+
+def kv_cache_append(qkv, k_cache, v_cache, cache_seqlens, cos=None, sin=None, return_q: bool = True):
+    """Write k, v of the packed projection ``qkv [b, s, a, 3d]`` into rows ``cache_seqlens[b] + i`` of the caches.  With
+    ``cos/sin`` (fp32 ``[positions, d]``) q and k are first rotated at those positions, exactly as
+    :func:`apply_rotary_qkv` with ``pos_offset = cache_seqlens[b]`` does.  Returns q ``[b, s, a, d]`` (rotated when the
+    tables are given) when ``return_q``, else None."""
+    if _decode_native(qkv, k_cache) and (cos is None or cos.dtype == torch.float32):
+        ext = load_ext()
+        q = ext.kv_append(qkv if qkv.is_contiguous() else qkv.contiguous(), k_cache, v_cache, cache_seqlens, cos, sin,
+                          bool(return_q))
+        count_launch()
+        return q if return_q else None
+    q = kv_cache_append_ref(qkv, k_cache, v_cache, cache_seqlens, cos, sin)
+    return q if return_q else None
+
+
+def kv_cache_append_ref(qkv, k_cache, v_cache, cache_seqlens, cos=None, sin=None):
+    d = qkv.shape[-1] // 3
+    s_len = qkv.shape[1]
+    q, k, v = qkv[..., :d], qkv[..., d : 2 * d], qkv[..., 2 * d :]
+    starts = [int(x) for x in cache_seqlens.tolist()]
+    if cos is not None:
+        pos = torch.tensor(starts, device=cos.device)[:, None] + torch.arange(s_len, device=cos.device)[None]
+        c = cos[pos][:, :, None, :].to(qkv.dtype)
+        sn = sin[pos][:, :, None, :].to(qkv.dtype)
+        q = q * c + rotate_half(q) * sn
+        k = k * c + rotate_half(k) * sn
+    for b, st in enumerate(starts):
+        k_cache[b, :, st : st + s_len] = k[b].transpose(0, 1)
+        v_cache[b, :, st : st + s_len] = v[b].transpose(0, 1)
+    return q
+
+
+def decode_attention(q, k_cache, v_cache, cache_seqlens, kv_start, *, scale: float, splits: int = 0):
+    """Attention of ``q [b, s, a, d]`` (new tokens, already appended to the caches; any strides with d contiguous) over
+    the caches: query ``i`` of sample ``b`` sees exactly the keys ``kv_start[b] <= j <= cache_seqlens[b] + i``.  Returns
+    ``[b, s, a, d]`` contiguous; a query without a visible key gets zeros.  The native kernel takes up to 16 new tokens
+    and reads lengths on the device (no host sync; one CUDA-graph capture replays after the lengths change); ``splits``
+    > 0 fixes its number of key-range splits."""
+    if _decode_native(q, k_cache) and q.shape[1] <= 16:
+        ext = load_ext()
+        o = ext.decode_attn(q, k_cache, v_cache, cache_seqlens, kv_start, float(scale), int(splits))
+        count_launch(2)
+        return o
+    return decode_attention_ref(q, k_cache, v_cache, cache_seqlens, kv_start, scale=scale)
+
+
+def decode_attention_ref(q, k_cache, v_cache, cache_seqlens, kv_start, *, scale: float):
+    """:func:`attention_ref` over the window ``[:L]`` of the caches (``L = max(cache_seqlens) + s``) with the mask built
+    from ``kv_start`` and causality among the new tokens."""
+    s_len = q.shape[1]
+    lens = cache_seqlens.long()
+    L = int(lens.max()) + s_len
+    j = torch.arange(L, device=q.device)[None, None, :]
+    i = torch.arange(s_len, device=q.device)[None, :, None]
+    visible = (j >= kv_start.long()[:, None, None]) & (j <= lens[:, None, None] + i)          # [b, s, L]
+    o = attention_ref(q.permute(0, 2, 1, 3), k_cache[:, :, :L], v_cache[:, :, :L], causal=False, scale=scale,
+                      mask=visible[:, None])
+    o = o.masked_fill(~visible.any(-1)[:, None, :, None], 0)
+    return o.permute(0, 2, 1, 3).contiguous()
+
+
+# --------------------------------------------------------------------------------------
 # vocab-parallel softmax cross entropy
 # --------------------------------------------------------------------------------------
 class _VocabParallelCE(torch.autograd.Function):

@@ -13,6 +13,7 @@ import torch
 from torch import nn
 
 from libai_b200.config import configurable
+from libai_b200.inference.kv_cache import KVCacheLayer
 from libai_b200.layers import Embedding
 from libai_b200.layers._param import create_parameter, zeros_
 from libai_b200.models.llama_model import LlamaAttention, LlamaForCausalLM as _BaseLlama
@@ -37,7 +38,12 @@ class AdapterAttention(LlamaAttention):
         bsz = hidden_states.shape[0]
         # queries need the same rotary phase as in the main path
         qkv = self.query_key_value(hidden_states).view(bsz, -1, a, 3 * d)
-        past_len = 0 if past_key_value is None else past_key_value[0].shape[2]
+        if past_key_value is None:
+            past_len = 0
+        elif isinstance(past_key_value, KVCacheLayer):
+            past_len = past_key_value.length   # rows before this step: the lengths advance after the last layer
+        else:
+            past_len = past_key_value[0].shape[2]
         q = OF.apply_rotary_qkv(qkv, cos_cached, sin_cached, past_len)[..., :d].permute(0, 2, 1, 3)
         akv = self.query_key_value(self.adapter.to(hidden_states.dtype)).view(1, -1, a, 3 * d).permute(0, 2, 1, 3)
         ak, av = akv[..., d : 2 * d], akv[..., 2 * d :]

@@ -1,22 +1,22 @@
 """GPT-2 with a KV cache and ``generate`` (reference projects/MagicPrompt/gpt2.py: the library GPT-2 extended with
 ``past_key_values`` / ``use_cache`` and the ``Generator`` mixin for prompt completion)."""
-import torch
 from torch import nn
 
 from libai_b200.config import configurable
 from libai_b200.inference.generator.generation_utils import Generator
+from libai_b200.inference.kv_cache import KVCacheOwner
 from libai_b200.models import gpt_model as core
 from libai_b200.models.gpt_model import GPTEmbedding, Transformer  # noqa: F401  (building blocks, same names as the reference module)
 from libai_b200.parallel import mappings
 from libai_b200.utils import distributed as dutil
 
 
-class GPTModel(core.GPTModel, Generator):
+class GPTModel(core.GPTModel, Generator, KVCacheOwner):
     @configurable
     def __init__(self, *args, cfg=None, **kwargs):
         super().__init__(*args, **kwargs)
         self.cfg = cfg
-        self.past_key_values = [None] * len(self.transformer.layers)
+        self.kv_cache = None
         self.past_length = 0
 
     @classmethod
@@ -28,30 +28,23 @@ class GPTModel(core.GPTModel, Generator):
     def forward(self, input_ids, use_cache=False):
         if not use_cache and self.training:
             return {"logits": super().forward(input_ids)}
-        past_len = self.past_key_values[0][0].shape[2] if use_cache and self.past_key_values[0] is not None else 0
+        cache = self._prepare_cache(input_ids) if use_cache else None
+        past_len = cache.length if use_cache else 0
         hidden = self.embeddings(input_ids, past_len)
-        presents = []
-        for layer, past in zip(self.transformer.layers, self.past_key_values if use_cache else [None] * len(self.past_key_values)):
-            mask = None
-            if past is not None:  # new tokens see the whole cache and the causal part of themselves
-                q, k = input_ids.shape[1], past_len + input_ids.shape[1]
-                mask = torch.ones(k, k, dtype=torch.bool, device=input_ids.device).tril()[k - q :][None, None]
-            out = layer(hidden, mask, past_key_value=past, use_cache=use_cache)
-            if use_cache:
-                hidden, present = out
-                presents.append(present)
-            else:
-                hidden = out
+        for i, layer in enumerate(self.transformer.layers):
+            # causal prefill, then decoding steps over the cache (every cached token is visible)
+            hidden = layer(hidden, None, past_key_value=cache.layer(i) if use_cache else None)
         if use_cache:
-            self.set_cache(presents)
+            cache.advance(input_ids.shape[1])
+            self.past_length = cache.length
         logits = self.lm_head(self.transformer.layernorm_f(hidden), self.word_embeddings_weight())
         if dutil.get_dist_util().tensor_parallel_size > 1:
             logits = mappings.gather_from_tp(logits)
         return {"logits": logits}
 
-    def set_cache(self, past_key_values):
-        self.past_length = 0 if past_key_values is None else past_key_values[0][0].shape[2]
-        self.past_key_values = [None] * len(self.transformer.layers) if past_key_values is None else list(past_key_values)
+    # ---- KV cache (KVCacheOwner) ----------------------------------------------------------------
+    def _cache_attention_modules(self):
+        return [layer.self_attention for layer in self.transformer.layers]
 
     def prepare_inputs_for_generation(self, input_ids, past=None, use_cache=None, **kwargs):
         if past is not None and use_cache:
