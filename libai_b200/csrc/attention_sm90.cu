@@ -2,10 +2,16 @@
 //
 // Replaces the score GEMM + fused_scale_(tril_)softmax(_mask)_dropout + context GEMM sequence of the
 // reference (libai/layers/attention.py:211-253): no [b, a, s, s] tensor and no materialised mask.
-// Q/K/V are read straight out of the packed QKV projection through strided 4-D TMA tensor maps
-// ([B, A, S, D] views), O is written in [B, S, A, D] so the output projection consumes it as-is.
+// Q/K/V are read straight out of the packed QKV projection through strided TMA tensor maps, O is written in
+// [B, S, A, D] so the output projection consumes it as-is.
 //
-// Forward, one CTA per (batch, head, 128-query block), 384 threads:
+// Grouped-query attention: A query heads share G = A / r key/value heads, query head h reading K/V head h / r.  Q is
+// described by (batch, group, in-group, seq) strides and read through a 5-D map ({D, S, r, G, B}), so both a plain
+// [B, A, S, D] q and the q slots of the grouped packed projection [B, S, G, r + 2, D] (per group q_0 .. q_{r-1}, k, v;
+// r = 1 is the per-head [q|k|v] layout) are read without a copy.  K/V use 4-D maps over the G heads.  Everything else
+// (O, lse, bias, ALiBi slope, dropout stream, kv_lens) stays per query head.
+//
+// Forward, one CTA per (batch, query head, 128-query block), 384 threads:
 //   warpgroup 0  TMA producer (one elected thread): Q once, then K/V tiles of 128 keys (double buffered); it gives
 //                its registers to the consumers (setmaxnreg)
 //   warpgroups 1, 2  consumers, 64 query rows each: S = Q·K_jᵀ (wgmma, accumulators in registers) →
@@ -28,6 +34,7 @@ struct AttnFwdParams {
   __nv_bfloat16* o;   // [B, S, A, D]
   float* lse;         // [B, A, S]
   int B, A, S;
+  int r;              // query heads per K/V head
   int causal;
   float scale_log2;   // scale * log2(e)
   float scale;
@@ -92,6 +99,7 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
   // heavy (late) query blocks first: better tail behaviour under the causal mask
   const int q_blk = static_cast<int>(gridDim.x) - 1 - static_cast<int>(blockIdx.x);
   const int head = blockIdx.y, batch = blockIdx.z;
+  const int kv_head = head / p.r;
   const int q0 = q_blk * ATT_BM;
   const int kv_len = p.kv_lens != nullptr ? max(1, min(p.S, p.kv_lens[batch])) : p.S;
   int nkv = (kv_len + ATT_BN - 1) / ATT_BN;
@@ -119,7 +127,7 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
       mbar_arrive_expect_tx(q_full, Cfg::TILE_BYTES);
 #pragma unroll
       for (int c = 0; c < Cfg::CHUNKS; ++c)
-        tma_load_4d(sQ + c * (ATT_BM * 128), &tmap_q, q_full, c * 64, q0, head, batch);
+        tma_load_5d(sQ + c * (ATT_BM * 128), &tmap_q, q_full, c * 64, q0, head - kv_head * p.r, kv_head, batch);
       for (int j = 0; j < nkv; ++j) {
         const int b = j & 1;
         const uint32_t par = ((j >> 1) & 1) ^ 1;
@@ -127,12 +135,12 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
         mbar_arrive_expect_tx(&k_full[b], Cfg::TILE_BYTES);
 #pragma unroll
         for (int c = 0; c < Cfg::CHUNKS; ++c)
-          tma_load_4d(sK + b * Cfg::TILE_BYTES + c * (ATT_BN * 128), &tmap_k, &k_full[b], c * 64, j * ATT_BN, head, batch);
+          tma_load_4d(sK + b * Cfg::TILE_BYTES + c * (ATT_BN * 128), &tmap_k, &k_full[b], c * 64, j * ATT_BN, kv_head, batch);
         mbar_wait(&v_empty[b], par);
         mbar_arrive_expect_tx(&v_full[b], Cfg::TILE_BYTES);
 #pragma unroll
         for (int c = 0; c < Cfg::CHUNKS; ++c)
-          tma_load_4d(sV + b * Cfg::TILE_BYTES + c * (ATT_BN * 128), &tmap_v, &v_full[b], c * 64, j * ATT_BN, head, batch);
+          tma_load_4d(sV + b * Cfg::TILE_BYTES + c * (ATT_BN * 128), &tmap_v, &v_full[b], c * 64, j * ATT_BN, kv_head, batch);
       }
     }
     return;
@@ -305,6 +313,14 @@ bool make_qkv_tmap(CUtensorMap* m, const void* ptr, int B, int A, int S, int D, 
   uint32_t box[4] = {64, (uint32_t)rows, 1, 1};
   return lb_host::make_tmap_bf16(m, ptr, 4, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B);
 }
+// query-head tensors of grouped-query attention, dims innermost first {D, S, r, G, B}; st = {batch, group, in-group,
+// seq} strides in elements
+bool make_q_tmap(CUtensorMap* m, const void* ptr, int B, int G, int r, int S, int D, const long* st, int rows) {
+  uint64_t dims[5] = {(uint64_t)D, (uint64_t)S, (uint64_t)r, (uint64_t)G, (uint64_t)B};
+  uint64_t strides[5] = {2, (uint64_t)st[3] * 2, (uint64_t)st[2] * 2, (uint64_t)st[1] * 2, (uint64_t)st[0] * 2};
+  uint32_t box[5] = {64, (uint32_t)rows, 1, 1, 1};
+  return lb_host::make_tmap_bf16(m, ptr, 5, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B);
+}
 
 template <int D, int BIAS, bool DROP>
 cudaError_t launch_fwd_t(const CUtensorMap& tq, const CUtensorMap& tk, const CUtensorMap& tv, const lb::AttnFwdParams& p,
@@ -332,25 +348,30 @@ cudaError_t launch_fwd(const CUtensorMap& tq, const CUtensorMap& tk, const CUten
   return drop ? launch_fwd_t<D, lb::BIAS_ALIBI, true>(tq, tk, tv, p, s) : launch_fwd_t<D, lb::BIAS_ALIBI, false>(tq, tk, tv, p, s);
 }
 }  // namespace
+// A query heads in G groups (A % G == 0); q_strides = {batch, group, in-group, seq}, k/v_strides = {batch, head, seq}
+// over the G K/V heads (elements).
 // p_drop in [0, 1): attention dropout probability (quantised to 1/256 like the byte-threshold test of the kernel);
 // bias (optional, bf16): dense additive score bias with (batch, head, query-row) strides in elements, key stride 1;
 // alibi_slopes (optional, fp32 [A]).
-extern "C" int lb_attn_fwd(const void* q, const void* k, const void* v, void* o, float* lse, int B, int A, int S, int D,
-                           const long* q_strides, const long* k_strides, const long* v_strides, int causal, float scale,
+extern "C" int lb_attn_fwd(const void* q, const void* k, const void* v, void* o, float* lse, int B, int A, int G, int S,
+                           int D, const long* q_strides, const long* k_strides, const long* v_strides, int causal, float scale,
                            const int* kv_lens, const void* bias, const long* bias_strides, const float* alibi_slopes,
                            float p_drop, const lb::RngArgs* rng, long long* rng_out, cudaStream_t s) {
   if (D != 64 && D != 128) return -1;
+  if (G <= 0 || A % G) return -4;
   for (int i = 0; i < 3; ++i)
     if ((q_strides[i] % 8) || (k_strides[i] % 8) || (v_strides[i] % 8)) return -3;
+  if (q_strides[3] % 8) return -3;
   CUtensorMap tq, tk, tv;
-  if (!make_qkv_tmap(&tq, q, B, A, S, D, q_strides, 128)) return -2;
-  if (!make_qkv_tmap(&tk, k, B, A, S, D, k_strides, 128)) return -2;
-  if (!make_qkv_tmap(&tv, v, B, A, S, D, v_strides, 128)) return -2;
+  if (!make_q_tmap(&tq, q, B, G, A / G, S, D, q_strides, 128)) return -2;
+  if (!make_qkv_tmap(&tk, k, B, G, S, D, k_strides, 128)) return -2;
+  if (!make_qkv_tmap(&tv, v, B, G, S, D, v_strides, 128)) return -2;
   lb::AttnFwdParams p;
   p.o = reinterpret_cast<__nv_bfloat16*>(o);
   p.lse = lse;
   p.B = B;
   p.A = A;
+  p.r = A / G;
   p.S = S;
   p.causal = causal;
   p.scale = scale;
@@ -372,15 +393,17 @@ extern "C" int lb_attn_fwd(const void* q, const void* k, const void* v, void* o,
   return (int)e;
 }
 // =================================================================================================
-// Backward.  One CTA per (batch, head, 64-key block); one consumer warpgroup loops over the 64-query blocks that
-// attend to it (warp 4 = TMA producer, Q / dO double buffered):
+// Backward.  One CTA per (batch, K/V head, 64-key block); one consumer warpgroup loops over the r query heads of the
+// group and, for each, over the 64-query blocks that attend to it (warp 4 = TMA producer, Q / dO double buffered):
 //   Sᵀ = K·Q_iᵀ , dPᵀ = V·dO_iᵀ                  (wgmma, registers)
 //   Pᵀ = exp(Sᵀ·scale − lse) , dSᵀ = Pᵀ ∘ (dPᵀ − δ) · scale
 //   dV += Pᵀ·dO_i , dK += dSᵀ·Q_i                 (A operands straight from the registers, accumulators stay in
-//                                                  registers for the whole CTA)
+//                                                  registers for the whole CTA: the group's sum is formed in a fixed
+//                                                  order and written once, no atomics)
 //   dQ_i += dS·K                                  (dSᵀ through shared memory, read as a transposed A operand; fp32
 //                                                  red.add into dq_accum, key block after key block in decreasing
-//                                                  order: a per-query-block counter orders the CTAs, so the sums are
+//                                                  order: a per-(query head, query block) counter orders the CTAs, so
+//                                                  the sums are
 //                                                  deterministic.  CTA kb at step `it` needs what kb + 1 added at step
 //                                                  it - 1, so the CTAs do not stall each other, and the highest key
 //                                                  blocks are launched first so that a waiter's predecessor is resident)
@@ -403,10 +426,11 @@ struct AttnBwdParams {
   const float* lse;     // [B, A, S]
   const float* delta;   // [B, A, S]
   float* dq_accum;      // [B, A, S, D] fp32
-  __nv_bfloat16* dk;    // strided [B, A, S, D] views
+  __nv_bfloat16* dk;    // strided [B, G, S, D] views
   __nv_bfloat16* dv;
   long g_strides[3];    // batch, head, seq strides (elements) of dk / dv
   int B, A, S;
+  int r;                // query heads per K/V head (G = A / r)
   int causal;
   float scale, scale_log2;
   const int* kv_lens;   // optional [B]
@@ -441,12 +465,13 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
 
   const int warp_idx = threadIdx.x / 32;
   const int kv_blk = static_cast<int>(gridDim.x) - 1 - static_cast<int>(blockIdx.x);
-  const int head = blockIdx.y, batch = blockIdx.z;
+  const int kv_head = blockIdx.y, batch = blockIdx.z;
   const int k0 = kv_blk * ATT_BWD_BN;
   const int kv_len = p.kv_lens != nullptr ? max(1, min(p.S, p.kv_lens[batch])) : p.S;
   const int nq = (p.S + ATT_BWD_BM - 1) / ATT_BWD_BM;
   const int i_begin = p.causal ? (k0 / ATT_BWD_BM) : 0;
-  const int iters = nq - i_begin;
+  const int iters = nq - i_begin;   // query blocks per query head
+  const int steps = p.r * iters;    // step = (query head in group) * iters + query block - i_begin
 
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmap_q);
@@ -468,18 +493,19 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
       mbar_arrive_expect_tx(kv_full, 2 * Cfg::TILE_BYTES);
 #pragma unroll
       for (int c = 0; c < Cfg::CHUNKS; ++c) {
-        tma_load_4d(sK + c * (64 * 128), &tmap_k, kv_full, c * 64, k0, head, batch);
-        tma_load_4d(sV + c * (64 * 128), &tmap_v, kv_full, c * 64, k0, head, batch);
+        tma_load_4d(sK + c * (64 * 128), &tmap_k, kv_full, c * 64, k0, kv_head, batch);
+        tma_load_4d(sV + c * (64 * 128), &tmap_v, kv_full, c * 64, k0, kv_head, batch);
       }
-      for (int it = 0; it < iters; ++it) {
-        const int st = it & 1;
-        const int q0 = (i_begin + it) * ATT_BWD_BM;
-        mbar_wait(&qdo_empty[st], ((it >> 1) & 1) ^ 1);
+      for (int step = 0; step < steps; ++step) {
+        const int hi = step / iters;
+        const int st = step & 1;
+        const int q0 = (i_begin + step - hi * iters) * ATT_BWD_BM;
+        mbar_wait(&qdo_empty[st], ((step >> 1) & 1) ^ 1);
         mbar_arrive_expect_tx(&qdo_full[st], 2 * Cfg::TILE_BYTES);
 #pragma unroll
         for (int c = 0; c < Cfg::CHUNKS; ++c) {
-          tma_load_4d(sQ + st * Cfg::TILE_BYTES + c * (64 * 128), &tmap_q, &qdo_full[st], c * 64, q0, head, batch);
-          tma_load_4d(sDO + st * Cfg::TILE_BYTES + c * (64 * 128), &tmap_do, &qdo_full[st], c * 64, q0, head, batch);
+          tma_load_5d(sQ + st * Cfg::TILE_BYTES + c * (64 * 128), &tmap_q, &qdo_full[st], c * 64, q0, hi, kv_head, batch);
+          tma_load_5d(sDO + st * Cfg::TILE_BYTES + c * (64 * 128), &tmap_do, &qdo_full[st], c * 64, q0, hi, kv_head, batch);
         }
       }
     }
@@ -489,16 +515,12 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
   const int t = threadIdx.x;                              // 0..127
   const int r_loc = 16 * (t / 32) + (t % 32) / 4;         // fragment rows r_loc, r_loc + 8
   const int cq = 2 * (t % 4);
-  const size_t bh = static_cast<size_t>(batch) * p.A + head;
   constexpr float LOG2E = 1.4426950408889634f;
   unsigned long long rng_seed = 0, rng_offset = 0;
   if constexpr (DROP) {
     rng_seed = static_cast<unsigned long long>(p.rng_state[0]);
     rng_offset = static_cast<unsigned long long>(p.rng_state[1]);
   }
-  float slope2 = 0.f;
-  if constexpr (BIAS == BIAS_ALIBI) slope2 = p.alibi_slopes[head] * LOG2E;
-  const long bias_bh = batch * p.bias_strides[0] + head * p.bias_strides[1];
   const float inv_scale = 1.0f / p.scale;
   const uint32_t k_addr = smem_u32(sK), v_addr = smem_u32(sV), ds_addr = smem_u32(sDS);
 
@@ -510,11 +532,18 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
   }
   mbar_wait(kv_full, 0);
 
-  for (int it = 0; it < iters; ++it) {
-    const int st = it & 1;
+  for (int step = 0; step < steps; ++step) {
+    const int hi = step / iters;
+    const int it = step - hi * iters;
+    const int head = kv_head * p.r + hi;   // query head
+    const size_t bh = static_cast<size_t>(batch) * p.A + head;
+    float slope2 = 0.f;
+    if constexpr (BIAS == BIAS_ALIBI) slope2 = p.alibi_slopes[head] * LOG2E;
+    const long bias_bh = batch * p.bias_strides[0] + head * p.bias_strides[1];
+    const int st = step & 1;
     const int q0 = (i_begin + it) * ATT_BWD_BM;
     const uint32_t q_addr = smem_u32(sQ + st * Cfg::TILE_BYTES), do_addr = smem_u32(sDO + st * Cfg::TILE_BYTES);
-    mbar_wait(&qdo_full[st], (it >> 1) & 1);
+    mbar_wait(&qdo_full[st], (step >> 1) & 1);
     // ---- Sᵀ = K·Q_iᵀ, dPᵀ = V·dO_iᵀ (64 keys x 64 queries each)
     float sT[32], dpT[32];
     wgmma_fence();
@@ -651,7 +680,7 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
   for (int h = 0; h < 2; ++h) {
     const int k_idx = k0 + r_loc + 8 * h;
     if (k_idx >= p.S) continue;
-    const long off = batch * p.g_strides[0] + head * p.g_strides[1] + static_cast<long>(k_idx) * p.g_strides[2];
+    const long off = batch * p.g_strides[0] + kv_head * p.g_strides[1] + static_cast<long>(k_idx) * p.g_strides[2];
 #pragma unroll
     for (int jj = 0; jj < D / 8; ++jj) {
       *reinterpret_cast<uint32_t*>(p.dv + off + 8 * jj + cq) = pack_bf16(dv[4 * jj + 2 * h], dv[4 * jj + 2 * h + 1]);
@@ -703,10 +732,11 @@ attn_delta_kernel(const __nv_bfloat16* __restrict__ dout, const __nv_bfloat16* _
   }
 }
 
-// dq (strided bf16) = dq_accum (fp32 [B, A, S, D]); 8 elements per thread (two 16-byte loads, one 16-byte store)
+// dq (strided bf16, query head a = group a / r, slot a % r) = dq_accum (fp32 [B, A, S, D]); 8 elements per thread (two
+// 16-byte loads, one 16-byte store)
 __global__ void __launch_bounds__(256)
-attn_dq_convert_kernel(const float* __restrict__ acc, __nv_bfloat16* __restrict__ dq, int B, int A, int S, int D, long sb,
-                       long sa, long ss) {
+attn_dq_convert_kernel(const float* __restrict__ acc, __nv_bfloat16* __restrict__ dq, int B, int A, int S, int D, int r,
+                       long sb, long sg, long si, long ss) {
   const long nvec = static_cast<long>(B) * A * S * D / 8;
   const long stride = static_cast<long>(gridDim.x) * blockDim.x;
   for (long i0 = blockIdx.x * static_cast<long>(blockDim.x) + threadIdx.x; i0 < nvec; i0 += 2 * stride) {
@@ -728,7 +758,7 @@ attn_dq_convert_kernel(const float* __restrict__ acc, __nv_bfloat16* __restrict_
         const long row = e / D;
         const int sq = static_cast<int>(row % S), a = static_cast<int>((row / S) % A);
         const long b = row / (static_cast<long>(S) * A);
-        *reinterpret_cast<uint4*>(dq + b * sb + a * sa + sq * ss + d) =
+        *reinterpret_cast<uint4*>(dq + b * sb + (a / r) * sg + (a % r) * si + sq * ss + d) =
             make_uint4(pack_bf16(lo[u].x, lo[u].y), pack_bf16(lo[u].z, lo[u].w), pack_bf16(hi[u].x, hi[u].y), pack_bf16(hi[u].z, hi[u].w));
       }
     }
@@ -759,7 +789,7 @@ cudaError_t launch_bwd_t(const CUtensorMap& tq, const CUtensorMap& tk, const CUt
     if (e != cudaSuccess) return e;
     configured = true;
   }
-  dim3 grid((p.S + lb::ATT_BWD_BN - 1) / lb::ATT_BWD_BN, p.A, p.B);
+  dim3 grid((p.S + lb::ATT_BWD_BN - 1) / lb::ATT_BWD_BN, p.A / p.r, p.B);
   kern<<<grid, lb::ATT_BWD_THREADS, Cfg::SMEM_BYTES, s>>>(tq, tk, tv, tdo, p);
   return cudaGetLastError();
 }
@@ -773,20 +803,27 @@ cudaError_t launch_bwd(const CUtensorMap& tq, const CUtensorMap& tk, const CUten
   return drop ? launch_bwd_t<D, lb::BIAS_ALIBI, true>(tq, tk, tv, tdo, p, s) : launch_bwd_t<D, lb::BIAS_ALIBI, false>(tq, tk, tv, tdo, p, s);
 }
 }  // namespace
+// A query heads in G groups; q_strides = {batch, group, in-group, seq}, k/v_strides = {batch, head, seq} over the G K/V
+// heads, do_strides = {batch, head, seq} over the A query heads.  dq, dk, dv point into one packed [B, S, G, r + 2, D]
+// gradient (slots 0 .. r - 1, r and r + 1 of each group).
 extern "C" int lb_attn_bwd(const void* dout, const void* q, const void* k, const void* v, const void* o,
                            const float* lse, void* dq, void* dk, void* dv, float* delta, float* dq_accum, int B, int A,
-                           int S, int D, const long* q_strides, const long* k_strides, const long* v_strides,
+                           int G, int S, int D, const long* q_strides, const long* k_strides, const long* v_strides,
                            const long* do_strides, int causal, float scale, const int* kv_lens, const void* bias,
                            const long* bias_strides, const float* alibi_slopes, float* dbias, float p_drop,
                            const long long* rng_state, unsigned* dq_order, cudaStream_t s) {
   if (D != 64 && D != 128) return -1;
+  if (G <= 0 || A % G) return -4;
+  const int r = A / G;
   for (int i = 0; i < 3; ++i)
     if ((q_strides[i] % 8) || (k_strides[i] % 8) || (v_strides[i] % 8) || (do_strides[i] % 8)) return -3;
+  if (q_strides[3] % 8) return -3;
+  const long do_strides4[4] = {do_strides[0], r * do_strides[1], do_strides[1], do_strides[2]};
   CUtensorMap tq, tk, tv, tdo;
-  if (!make_qkv_tmap(&tq, q, B, A, S, D, q_strides, 64)) return -2;
-  if (!make_qkv_tmap(&tk, k, B, A, S, D, k_strides, 64)) return -2;
-  if (!make_qkv_tmap(&tv, v, B, A, S, D, v_strides, 64)) return -2;
-  if (!make_qkv_tmap(&tdo, dout, B, A, S, D, do_strides, 64)) return -2;
+  if (!make_q_tmap(&tq, q, B, G, r, S, D, q_strides, 64)) return -2;
+  if (!make_qkv_tmap(&tk, k, B, G, S, D, k_strides, 64)) return -2;
+  if (!make_qkv_tmap(&tv, v, B, G, S, D, v_strides, 64)) return -2;
+  if (!make_q_tmap(&tdo, dout, B, G, r, S, D, do_strides4, 64)) return -2;
   const long rows = (long)B * A * S;
   {
     // 4 rows per thread-group and iteration; cap the grid at a few waves
@@ -809,12 +846,13 @@ extern "C" int lb_attn_bwd(const void* dout, const void* q, const void* k, const
   p.dq_accum = dq_accum;
   p.dk = (__nv_bfloat16*)dk;
   p.dv = (__nv_bfloat16*)dv;
-  // dq / dk / dv are views of one packed [B, S, A, 3, D] tensor: same strides as the packed q view
-  p.g_strides[0] = (long)S * A * 3 * D;
-  p.g_strides[1] = 3L * D;
-  p.g_strides[2] = (long)A * 3 * D;
+  // dq / dk / dv are views of one packed [B, S, G, r + 2, D] tensor
+  p.g_strides[0] = (long)S * G * (r + 2) * D;
+  p.g_strides[1] = (long)(r + 2) * D;
+  p.g_strides[2] = (long)G * (r + 2) * D;
   p.B = B;
   p.A = A;
+  p.r = r;
   p.S = S;
   p.causal = causal;
   p.scale = scale;
@@ -836,7 +874,7 @@ extern "C" int lb_attn_bwd(const void* dout, const void* q, const void* k, const
   const long nvec = rows * D / 8;
   int blocks = (int)((nvec + 511) / 512);
   if (blocks > sm_count() * 8) blocks = sm_count() * 8;
-  lb::attn_dq_convert_kernel<<<blocks, 256, 0, s>>>(dq_accum, (__nv_bfloat16*)dq, B, A, S, D, p.g_strides[0],
-                                                    p.g_strides[1], p.g_strides[2]);
+  lb::attn_dq_convert_kernel<<<blocks, 256, 0, s>>>(dq_accum, (__nv_bfloat16*)dq, B, A, S, D, r, p.g_strides[0],
+                                                    p.g_strides[1], (long)D, p.g_strides[2]);
   return (int)cudaGetLastError();
 }

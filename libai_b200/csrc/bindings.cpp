@@ -36,7 +36,7 @@ int lb_swiglu_fwd(const void* gate, const void* up, void* y, long n, cudaStream_
 int lb_swiglu_bwd(const void* gy, const void* gate, const void* up, void* dgate, void* dup, long n, cudaStream_t s);
 int lb_swiglu_packed_fwd(const void* gu, void* y, long rows, long F, cudaStream_t s);
 int lb_swiglu_packed_bwd(const void* gy, const void* gu, void* dgu, long rows, long F, cudaStream_t s);
-int lb_rope_qkv(const void* x, const float* cosv, const float* sinv, void* y, long heads, int S, int A, int D,
+int lb_rope_qkv(const void* x, const float* cosv, const float* sinv, void* y, long groups, int S, int G, int r, int D,
                 int pos_offset, int backward, cudaStream_t s);
 int lb_rope(const void* x, const float* cosv, const float* sinv, void* y, long rows, int S, int D, int backward,
             cudaStream_t s);
@@ -76,24 +76,24 @@ struct LbRngArgs {
   int captured;
   unsigned long long salt;
 };
-int lb_attn_fwd(const void* q, const void* k, const void* v, void* o, float* lse, int B, int A, int S, int D,
+int lb_attn_fwd(const void* q, const void* k, const void* v, void* o, float* lse, int B, int A, int G, int S, int D,
                 const long* q_strides, const long* k_strides, const long* v_strides, int causal, float scale,
                 const int* kv_lens, const void* bias, const long* bias_strides, const float* alibi_slopes, float p_drop,
                 const LbRngArgs* rng, long long* rng_out, cudaStream_t s);
 int lb_attn_bwd(const void* dout, const void* q, const void* k, const void* v, const void* o, const float* lse,
-                void* dq, void* dk, void* dv, float* delta, float* dq_accum, int B, int A, int S, int D,
+                void* dq, void* dk, void* dv, float* delta, float* dq_accum, int B, int A, int G, int S, int D,
                 const long* q_strides, const long* k_strides, const long* v_strides, const long* do_strides, int causal,
                 float scale, const int* kv_lens, const void* bias, const long* bias_strides, const float* alibi_slopes,
                 float* dbias, float p_drop, const long long* rng_state, unsigned* dq_order, cudaStream_t s);
 int lb_bias_dropout_residual(const void* x, const void* bias, const void* res, void* y, long rows, int N, float p,
                              const LbRngArgs* rng, const long long* rng_in, long long* rng_out, cudaStream_t s);
 int lb_spin_timeout_report(char* buf, int n);
-int lb_decode_splits(int B, int A, int C, int D);
+int lb_decode_splits(int B, int blocks, int C, int D);
 int lb_decode_attn(const void* q, const long* q_strides, const void* k, const void* v, void* o, float* part_o,
-                   float* part_ml, const int* seqlens, const int* kv_start, int B, int Sq, int A, int C, int D, float scale,
-                   int nsplit, cudaStream_t s);
+                   float* part_ml, const int* seqlens, const int* kv_start, int B, int Sq, int A, int G, int C, int D,
+                   float scale, int nsplit, cudaStream_t s);
 int lb_kv_append(const void* qkv, const float* cosv, const float* sinv, void* q_out, void* k_cache, void* v_cache,
-                 const int* seqlens, int B, int Sq, int A, int C, int D, cudaStream_t s);
+                 const int* seqlens, int B, int Sq, int G, int r, int C, int D, cudaStream_t s);
 }
 
 namespace {
@@ -469,21 +469,46 @@ Tensor swiglu_packed_bwd(const Tensor& gy, const Tensor& gu) {
         "swiglu_packed_bwd");
   return dgu;
 }
-// qkv [b, s, a, 3d] packed projection; rotates q and k (v copied).  inplace=true rewrites qkv itself.
+// Geometry of a packed projection: [b, s, a, 3d] (per-head [q|k|v], G = a, r = 1) or the grouped [b, s, g, r + 2, d]
+// (per K/V group q_0 .. q_{r-1}, k, v).
+struct PackedQKV {
+  int B, S, G, r, D;
+};
+PackedQKV packed_qkv(const Tensor& qkv, const char* what) {
+  TORCH_CHECK(qkv.dim() == 4 || qkv.dim() == 5, what, ": packed projection [b, s, a, 3d] or [b, s, g, r + 2, d] expected");
+  PackedQKV g;
+  g.B = (int)qkv.size(0);
+  g.S = (int)qkv.size(1);
+  g.G = (int)qkv.size(2);
+  if (qkv.dim() == 4) {
+    g.r = 1;
+    g.D = (int)qkv.size(3) / 3;
+    TORCH_CHECK(qkv.size(3) == 3 * g.D, what, ": last dim must be 3*d");
+  } else {
+    g.r = (int)qkv.size(3) - 2;
+    g.D = (int)qkv.size(4);
+    TORCH_CHECK(g.r >= 1, what, ": a group holds r >= 1 query heads, k and v");
+  }
+  return g;
+}
+
+// packed projection [b, s, a, 3d] or [b, s, g, r + 2, d]; rotates every q and k (v copied).  inplace=true rewrites qkv
+// itself.
 Tensor rope_qkv(const Tensor& qkv, const Tensor& cosv, const Tensor& sinv, int64_t pos_offset, bool backward,
                 bool inplace) {
   c10::cuda::CUDAGuard guard(qkv.device());
-  TORCH_CHECK(qkv.dim() == 4 && qkv.is_contiguous() && qkv.scalar_type() == at::kBFloat16,
-              "rope_qkv: contiguous bf16 [b,s,a,3d]");
-  const int S = qkv.size(1), A = qkv.size(2), D = qkv.size(3) / 3;
-  TORCH_CHECK(qkv.size(3) == 3 * D && D % 2 == 0, "rope_qkv: last dim must be 3*d");
+  TORCH_CHECK(qkv.is_contiguous() && qkv.scalar_type() == at::kBFloat16, "rope_qkv: contiguous bf16 packed projection");
+  const PackedQKV g = packed_qkv(qkv, "rope_qkv");
+  const int S = g.S, D = g.D;
+  TORCH_CHECK(D % 2 == 0, "rope_qkv: head dim must be even");
   TORCH_CHECK(cosv.scalar_type() == at::kFloat && sinv.scalar_type() == at::kFloat && cosv.is_contiguous() &&
                   sinv.is_contiguous() && cosv.size(0) >= S + pos_offset && cosv.size(1) == D &&
                   sinv.sizes() == cosv.sizes(),
               "rope_qkv: cos/sin fp32 [>=S+offset, D]");
+  TORCH_CHECK(cosv.device() == qkv.device() && sinv.device() == qkv.device(), "rope_qkv: cos/sin must be on qkv's device");
   Tensor y = inplace ? qkv : at::empty_like(qkv);
   check(lb_rope_qkv(qkv.data_ptr(), cosv.data_ptr<float>(), sinv.data_ptr<float>(), y.data_ptr(),
-                    qkv.numel() / (3 * D), S, A, D, (int)pos_offset, backward ? 1 : 0, cur_stream()),
+                    qkv.numel() / ((g.r + 2) * D), S, g.G, g.r, D, (int)pos_offset, backward ? 1 : 0, cur_stream()),
         "rope_qkv");
   return y;
 }
@@ -594,7 +619,8 @@ std::tuple<Tensor, Tensor> bias_dropout_residual(const Tensor& x, const c10::opt
 }
 
 // ---- attention ----------------------------------------------------------------------------------------------
-// q, k, v: [B, A, S, D] views with arbitrary batch/head/seq strides (D contiguous). Output o is allocated as
+// q: [B, A, S, D] or, grouped, [B, G, r, S, D]; k, v: [B, G, S, D] with A = G * r (grouped-query attention: query head
+// h reads K/V head h / r); views with arbitrary batch/head/seq strides (D contiguous).  Output o is allocated as
 // [B, S, A, D] and returned as the [B, A, S, D] view, lse fp32 [B, A, S].
 struct BiasDesc {
   const void* ptr = nullptr;
@@ -615,16 +641,51 @@ BiasDesc bias_desc(const c10::optional<Tensor>& bias, int B, int A, int S) {
   return d;
 }
 
+// shapes of an attention call: q [B, A, S, D] / [B, G, r, S, D] against k, v [B, G, S, D]; qs = q's {batch, group,
+// in-group, seq} strides
+struct QGeom {
+  int B, A, G, S, D;
+  long qs[4];
+};
+QGeom q_geom(const Tensor& q, const Tensor& k, const Tensor& v, const char* what) {
+  TORCH_CHECK(q.dim() == 4 || q.dim() == 5, what, ": q must be [B, A, S, D] or [B, G, r, S, D]");
+  TORCH_CHECK(k.dim() == 4 && k.sizes() == v.sizes(), what, ": k, v must be [B, G, S, D] of one shape");
+  TORCH_CHECK(q.stride(-1) == 1 && k.stride(3) == 1 && v.stride(3) == 1, what, ": D must be contiguous");
+  QGeom g;
+  g.B = (int)q.size(0);
+  g.G = (int)k.size(1);
+  g.S = (int)q.size(-2);
+  g.D = (int)q.size(-1);
+  if (q.dim() == 4) {
+    g.A = (int)q.size(1);
+    TORCH_CHECK(g.G > 0 && g.A % g.G == 0, what, ": the query heads must be a multiple of the K/V heads");
+    const long r = g.A / g.G;
+    g.qs[0] = q.stride(0);
+    g.qs[1] = r * q.stride(1);
+    g.qs[2] = q.stride(1);
+    g.qs[3] = q.stride(2);
+  } else {
+    TORCH_CHECK(q.size(1) == g.G, what, ": grouped q [B, G, r, S, D] must have the K/V heads' G");
+    g.A = g.G * (int)q.size(2);
+    g.qs[0] = q.stride(0);
+    g.qs[1] = q.stride(1);
+    g.qs[2] = q.stride(2);
+    g.qs[3] = q.stride(3);
+  }
+  TORCH_CHECK(k.size(0) == g.B && k.size(2) == g.S && k.size(3) == g.D, what, ": k, v do not match q");
+  return g;
+}
+
 // returns (o, lse, rng_state): rng_state int64[2] = (seed, offset) of the dropout mask (empty without dropout)
 std::tuple<Tensor, Tensor, Tensor> attn_fwd(const Tensor& q, const Tensor& k, const Tensor& v, bool causal, double scale,
                                             const c10::optional<Tensor>& kv_lens, const c10::optional<Tensor>& bias,
                                             const c10::optional<Tensor>& alibi_slopes, double p_drop, int64_t salt) {
   c10::cuda::CUDAGuard guard(q.device());
-  TORCH_CHECK(q.dim() == 4 && q.stride(3) == 1 && k.stride(3) == 1 && v.stride(3) == 1, "attn_fwd: [B,A,S,D], D contiguous");
-  const int B = (int)q.size(0), A = (int)q.size(1), S = (int)q.size(2), D = (int)q.size(3);
+  const QGeom g = q_geom(q, k, v, "attn_fwd");
+  const int B = g.B, A = g.A, S = g.S, D = g.D;
   Tensor o = at::empty({B, S, A, D}, q.options());
   Tensor lse = at::empty({B, A, S}, q.options().dtype(at::kFloat));
-  long qs[3] = {q.stride(0), q.stride(1), q.stride(2)};
+  const long* qs = g.qs;
   long ks[3] = {k.stride(0), k.stride(1), k.stride(2)};
   long vs[3] = {v.stride(0), v.stride(1), v.stride(2)};
   const int* kvl = nullptr;
@@ -648,7 +709,7 @@ std::tuple<Tensor, Tensor, Tensor> attn_fwd(const Tensor& q, const Tensor& k, co
   } else {
     rng_state = at::empty({0}, q.options().dtype(at::kLong));
   }
-  check(lb_attn_fwd(q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(), lse.data_ptr<float>(), B, A, S, D, qs, ks,
+  check(lb_attn_fwd(q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(), lse.data_ptr<float>(), B, A, g.G, S, D, qs, ks,
                     vs, causal ? 1 : 0, (float)scale, kvl, bd.ptr, bd.strides, slopes, (float)p_drop, drop ? &a : nullptr,
                     drop ? reinterpret_cast<long long*>(rng_state.data_ptr<int64_t>()) : nullptr, cur_stream()),
         "attn_fwd");
@@ -662,7 +723,7 @@ void check_cache(const Tensor& k_cache, const Tensor& v_cache, const char* what)
   TORCH_CHECK(k_cache.is_cuda() && k_cache.scalar_type() == at::kBFloat16 && v_cache.scalar_type() == at::kBFloat16,
               what, ": bf16 CUDA cache expected");
   TORCH_CHECK(k_cache.dim() == 4 && k_cache.sizes() == v_cache.sizes() && k_cache.is_contiguous() && v_cache.is_contiguous(),
-              what, ": K and V caches must be contiguous [B, A, C, D] of the same shape");
+              what, ": K and V caches must be contiguous [B, G, C, D] of the same shape");
   TORCH_CHECK(k_cache.size(3) == 64 || k_cache.size(3) == 128, what, ": head dim must be 64 or 128");
   TORCH_CHECK(reinterpret_cast<uintptr_t>(k_cache.data_ptr()) % 16 == 0 &&
               reinterpret_cast<uintptr_t>(v_cache.data_ptr()) % 16 == 0, what, ": caches must be 16-byte aligned");
@@ -672,17 +733,19 @@ void check_lengths(const Tensor& t, int64_t B, const char* what) {
               ": int32 CUDA [B] expected");
 }
 
-// k, v of the packed projection qkv [B, Sq, A, 3D] go to rows cache_seqlens[b] + i of the caches; with cos/sin (fp32
-// [>= positions, D]) q and k are rotated first.  Returns the (rotated) q as [B, Sq, A, D] when write_q, else empty.
+// k, v of the packed projection qkv ([B, Sq, A, 3D] or grouped [B, Sq, G, r + 2, D]) go to rows cache_seqlens[b] + i
+// of the caches [B, G, C, D]; with cos/sin (fp32 [>= positions, D]) q and k are rotated first.  Returns the (rotated) q
+// as [B, Sq, G * r, D] when write_q, else empty.
 Tensor kv_append(const Tensor& qkv, const Tensor& k_cache, const Tensor& v_cache, const Tensor& cache_seqlens,
                  const c10::optional<Tensor>& cosv, const c10::optional<Tensor>& sinv, bool write_q) {
   c10::cuda::CUDAGuard guard(qkv.device());
   check_cache(k_cache, v_cache, "kv_append");
-  const int B = (int)k_cache.size(0), A = (int)k_cache.size(1), C = (int)k_cache.size(2), D = (int)k_cache.size(3);
-  TORCH_CHECK(qkv.is_cuda() && qkv.scalar_type() == at::kBFloat16 && qkv.dim() == 4 && qkv.is_contiguous(),
-              "kv_append: contiguous bf16 qkv [B, Sq, A, 3D] expected");
-  TORCH_CHECK(qkv.size(0) == B && qkv.size(2) == A && qkv.size(3) == 3 * D, "kv_append: qkv does not match the cache");
-  const int Sq = (int)qkv.size(1);
+  const int B = (int)k_cache.size(0), G = (int)k_cache.size(1), C = (int)k_cache.size(2), D = (int)k_cache.size(3);
+  TORCH_CHECK(qkv.is_cuda() && qkv.scalar_type() == at::kBFloat16 && qkv.is_contiguous(),
+              "kv_append: contiguous bf16 packed projection expected");
+  const PackedQKV g = packed_qkv(qkv, "kv_append");
+  TORCH_CHECK(g.B == B && g.G == G && g.D == D, "kv_append: qkv does not match the cache");
+  const int Sq = g.S, A = G * g.r;
   TORCH_CHECK(Sq >= 1 && Sq <= C, "kv_append: 1 <= Sq <= capacity");
   check_lengths(cache_seqlens, B, "kv_append: cache_seqlens");
   const float* cp = nullptr;
@@ -698,28 +761,31 @@ Tensor kv_append(const Tensor& qkv, const Tensor& k_cache, const Tensor& v_cache
   }
   Tensor q_out = write_q ? at::empty({B, Sq, A, D}, qkv.options()) : at::empty({0}, qkv.options());
   check(lb_kv_append(qkv.data_ptr(), cp, sp, write_q ? q_out.data_ptr() : nullptr, k_cache.data_ptr(),
-                     v_cache.data_ptr(), cache_seqlens.data_ptr<int>(), B, Sq, A, C, D, cur_stream()),
+                     v_cache.data_ptr(), cache_seqlens.data_ptr<int>(), B, Sq, G, g.r, C, D, cur_stream()),
         "kv_append");
   return q_out;
 }
 
-// q [B, Sq, A, D] (any strides with D contiguous, e.g. a view of the packed projection) against the caches; query i of
-// sample b sees keys kv_start[b] .. cache_seqlens[b] + i.  Returns o [B, Sq, A, D] contiguous.  splits = 0: automatic.
+// q [B, Sq, A, D] (any strides with D contiguous, e.g. a view of the packed projection) against the caches [B, G, C, D]
+// (query head h reads cache head h / (A / G)); query i of sample b sees keys kv_start[b] .. cache_seqlens[b] + i.
+// Returns o [B, Sq, A, D] contiguous.  splits = 0: automatic.
 Tensor decode_attn(const Tensor& q, const Tensor& k_cache, const Tensor& v_cache, const Tensor& cache_seqlens,
                    const Tensor& kv_start, double scale, int64_t splits) {
   c10::cuda::CUDAGuard guard(q.device());
   check_cache(k_cache, v_cache, "decode_attn");
-  const int B = (int)k_cache.size(0), A = (int)k_cache.size(1), C = (int)k_cache.size(2), D = (int)k_cache.size(3);
+  const int B = (int)k_cache.size(0), G = (int)k_cache.size(1), C = (int)k_cache.size(2), D = (int)k_cache.size(3);
   TORCH_CHECK(q.is_cuda() && q.scalar_type() == at::kBFloat16 && q.dim() == 4 && q.stride(3) == 1,
               "decode_attn: bf16 q [B, Sq, A, D] with D contiguous expected");
-  TORCH_CHECK(q.size(0) == B && q.size(2) == A && q.size(3) == D, "decode_attn: q does not match the cache");
+  const int A = (int)q.size(2);
+  TORCH_CHECK(q.size(0) == B && A % G == 0 && q.size(3) == D, "decode_attn: q does not match the cache");
   const int Sq = (int)q.size(1);
   TORCH_CHECK(Sq >= 1 && Sq <= 16, "decode_attn: 1 <= Sq <= 16 new queries");
   TORCH_CHECK(reinterpret_cast<uintptr_t>(q.data_ptr()) % 16 == 0 && q.stride(0) % 8 == 0 && q.stride(1) % 8 == 0 &&
               q.stride(2) % 8 == 0, "decode_attn: q must be 16-byte aligned with strides that are multiples of 8");
   check_lengths(cache_seqlens, B, "decode_attn: cache_seqlens");
   check_lengths(kv_start, B, "decode_attn: kv_start");
-  const int nsplit = splits > 0 ? (int)std::min<int64_t>(splits, 32) : lb_decode_splits(B, A, C, D);
+  const int row_blocks = ((A / G) * Sq + 15) / 16;   // (query head, token) rows of one cache head, 16 per CTA
+  const int nsplit = splits > 0 ? (int)std::min<int64_t>(splits, 32) : lb_decode_splits(B, G * row_blocks, C, D);
   Tensor o = at::empty({B, Sq, A, D}, q.options());
   Tensor part_o, part_ml;
   if (nsplit > 1) {
@@ -729,7 +795,7 @@ Tensor decode_attn(const Tensor& q, const Tensor& k_cache, const Tensor& v_cache
   long qs[3] = {q.stride(0), q.stride(1), q.stride(2)};
   check(lb_decode_attn(q.data_ptr(), qs, k_cache.data_ptr(), v_cache.data_ptr(), o.data_ptr(),
                        nsplit > 1 ? part_o.data_ptr<float>() : nullptr, nsplit > 1 ? part_ml.data_ptr<float>() : nullptr,
-                       cache_seqlens.data_ptr<int>(), kv_start.data_ptr<int>(), B, Sq, A, C, D, (float)scale, nsplit,
+                       cache_seqlens.data_ptr<int>(), kv_start.data_ptr<int>(), B, Sq, A, G, C, D, (float)scale, nsplit,
                        cur_stream()),
         "decode_attn");
   return o;
@@ -742,12 +808,14 @@ std::tuple<Tensor, Tensor, Tensor, Tensor> attn_bwd(const Tensor& dout, const Te
                                             const c10::optional<Tensor>& alibi_slopes, c10::optional<Tensor> dbias,
                                             double p_drop, const c10::optional<Tensor>& rng_state) {
   c10::cuda::CUDAGuard guard(q.device());
-  const int B = (int)q.size(0), A = (int)q.size(1), S = (int)q.size(2), D = (int)q.size(3);
-  // gradients are produced in the packed [B, S, A, 3, D] layout so that the QKV dgrad/wgrad GEMMs read them directly
-  Tensor dqkv = at::empty({B, S, A, 3, D}, q.options());
-  Tensor dq = dqkv.select(3, 0).permute({0, 2, 1, 3});
-  Tensor dk = dqkv.select(3, 1).permute({0, 2, 1, 3});
-  Tensor dv = dqkv.select(3, 2).permute({0, 2, 1, 3});
+  const QGeom g = q_geom(q, k, v, "attn_bwd");
+  const int B = g.B, A = g.A, G = g.G, S = g.S, D = g.D, r = A / G;
+  // gradients are produced in the packed [B, S, G, r + 2, D] layout (r = 1: [B, S, A, 3, D]) so that the QKV
+  // dgrad/wgrad GEMMs read them directly; dq comes back in q's shape (a copy only for a 4-D q with r > 1)
+  Tensor dqkv = at::empty({B, S, G, r + 2, D}, q.options());
+  Tensor dq5 = dqkv.narrow(3, 0, r).permute({0, 2, 3, 1, 4});
+  Tensor dk = dqkv.select(3, r).permute({0, 2, 1, 3});
+  Tensor dv = dqkv.select(3, r + 1).permute({0, 2, 1, 3});
   Tensor delta = at::empty({B, A, S}, q.options().dtype(at::kFloat));
   Tensor dq_acc = at::empty({B, A, S, D}, q.options().dtype(at::kFloat));   // cleared by the delta kernel
   // per (batch, head, 64-query block): key blocks that have added their dQ contribution
@@ -758,7 +826,7 @@ std::tuple<Tensor, Tensor, Tensor, Tensor> attn_bwd(const Tensor& dout, const Te
     dout_c = at::empty_strided(o.sizes(), o.strides(), o.options());
     dout_c.copy_(dout);
   }
-  long qs[3] = {q.stride(0), q.stride(1), q.stride(2)};
+  const long* qs = g.qs;
   long ks[3] = {k.stride(0), k.stride(1), k.stride(2)};
   long vs[3] = {v.stride(0), v.stride(1), v.stride(2)};
   long ds[3] = {dout_c.stride(0), dout_c.stride(1), dout_c.stride(2)};
@@ -771,14 +839,15 @@ std::tuple<Tensor, Tensor, Tensor, Tensor> attn_bwd(const Tensor& dout, const Te
   }
   const bool has_rng = p_drop > 0.0 && rng_state.has_value() && rng_state->defined() && rng_state->numel() == 2;
   check(lb_attn_bwd(dout_c.data_ptr(), q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(), lse.data_ptr<float>(),
-                    dq.data_ptr(), dk.data_ptr(), dv.data_ptr(), delta.data_ptr<float>(), dq_acc.data_ptr<float>(), B, A,
-                    S, D, qs, ks, vs, ds, causal ? 1 : 0, (float)scale,
+                    dq5.data_ptr(), dk.data_ptr(), dv.data_ptr(), delta.data_ptr<float>(), dq_acc.data_ptr<float>(), B, A,
+                    G, S, D, qs, ks, vs, ds, causal ? 1 : 0, (float)scale,
                     (kv_lens.has_value() && kv_lens->defined()) ? kv_lens->data_ptr<int>() : nullptr, bd.ptr, bd.strides,
                     (alibi_slopes.has_value() && alibi_slopes->defined()) ? alibi_slopes->data_ptr<float>() : nullptr, dbp,
                     (float)(has_rng ? p_drop : 0.0),
                     has_rng ? reinterpret_cast<const long long*>(rng_state->data_ptr<int64_t>()) : nullptr,
                     reinterpret_cast<unsigned*>(dq_order.data_ptr<int>()), cur_stream()),
         "attn_bwd");
+  Tensor dq = q.dim() == 5 ? dq5 : dq5.reshape({B, A, S, D});   // after the kernel: for r > 1 this copies
   return std::make_tuple(dq, dk, dv, dqkv);
 }
 

@@ -183,6 +183,14 @@ LB_DEVICE void tma_load_4d(void* smem_dst, const CUtensorMap* map, uint64_t* bar
       "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
       : "memory");
 }
+LB_DEVICE void tma_load_5d(void* smem_dst, const CUtensorMap* map, uint64_t* bar, int32_t c0, int32_t c1, int32_t c2,
+                           int32_t c3, int32_t c4) {
+  asm volatile(
+      "cp.async.bulk.tensor.5d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6, %7}], "
+      "[%2];\n" ::"r"(smem_u32(smem_dst)),
+      "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(c4)
+      : "memory");
+}
 // shared -> global tiled store (bulk async group completion)
 LB_DEVICE void tma_store_2d(const CUtensorMap* map, const void* smem_src, int32_t c0, int32_t c1) {
   asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];\n" ::"l"(

@@ -1,26 +1,32 @@
 // KV-cache decoding on sm_90a: the cache append (with rotary embedding) and split-KV ("flash-decoding") attention.
 //
-// lb_kv_append: one pass over the packed projection qkv [B, Sq, A, 3D] (per-head [q|k|v]).  q and k are rotated with
-//   the fp32 cos/sin tables in the rotate-half convention of rope_qkv_kernel (same expressions, so the rotated values are
-//   bit-identical), k and v are written into the layer's cache K, V [B, A, C, D] at rows cache_seqlens[b] + i, and the
-//   rotated q goes to q_out [B, Sq, A, D].  Without tables (GPT-2) the values are copied unrotated.
+// Grouped-query attention: the A query heads share G = A / r cache heads.  The packed projection is grouped,
+// [B, Sq, G, r + 2, D] with q_0 .. q_{r-1}, k, v per group (r = 1: per-head [q|k|v]), and the caches hold the G heads.
+//
+// lb_kv_append: one pass over the packed projection.  q and k are rotated with the fp32 cos/sin tables in the
+//   rotate-half convention of rope_qkv_kernel (same expressions, so the rotated values are bit-identical), k and v are
+//   written into the layer's cache K, V [B, G, C, D] at rows cache_seqlens[b] + i, and the rotated q goes to
+//   q_out [B, Sq, A, D].  Without tables (GPT-2) the values are copied unrotated.
 //
 // lb_decode_attn: o [B, Sq, A, D] for 1 <= Sq <= 16 new queries per (sample, head).  Query i of sample b sees exactly the
 //   keys j with kv_start[b] <= j <= cache_seqlens[b] + i (kv_start = left padding, cache_seqlens = length before this
 //   step's append); every other key is excluded outright, and a query without a visible key writes zeros.
-//   Grid (splits, A, B), 160 threads: the key window of each (b, h) is cut into `splits` contiguous ranges of 64-key
-//   tiles so that small batches still fill the SMs.  Warp 4 streams the K/V tiles of its range through a ring of
+//   The MMA rows of a CTA are (query head in group, new token) pairs of one cache head: row = j * Sq + i for query head
+//   g * r + j and token i, r * Sq rows cut into blocks of 16.  A group with r * Sq <= 16 therefore reads each K/V tile
+//   once for all its query heads.
+//   Grid (splits, G * row blocks, B), 160 threads: the key window of each (b, g) is cut into `splits` contiguous ranges
+//   of 64-key tiles so that small batches still fill the SMs.  Warp 4 streams the K/V tiles of its range through a ring of
 //   shared-memory stages with cp.async.bulk (one bulk copy per key row, into rows padded by 16 bytes so the ldmatrix
 //   reads below are free of bank conflicts; the non-tensor bulk copy has no swizzle), completion on mbarriers.  Warps
 //   0-3 each take 16 keys of every tile: S = Q·Kᵀ and O += P·V on mma.sync m16n8k16 (bf16 in, fp32 accumulators), the
-//   16 query rows of the MMA being the Sq new tokens, and keep their own online-softmax state.  The four warps are
+//   16 rows of the MMA being (query head, new token) pairs, and keep their own online-softmax state.  The four warps are
 //   merged in warp order in shared memory; with one split that is the output, otherwise the CTA writes its fp32 partial
 //   (m, l, O) and decode_combine_kernel reduces the partials in split order.  No atomics: results are bit-identical from
 //   run to run.
 //   mma.sync rather than wgmma: the kernel moves ~2 bytes of K/V per multiply-add, so it is bound by HBM bandwidth, not
 //   by the tensor cores; wgmma's 64-row minimum M would be 4-64x wasted work for Sq <= 16 and would need swizzled
 //   (TMA tensor-map) tiles, while mma.sync's M = 16 matches Sq exactly and reads plain row-major tiles.
-//   Lengths are read on the device and the grid depends only on (B, A, splits): one captured launch replays correctly
+//   Lengths are read on the device and the grid depends only on (B, G, r, Sq, splits): one captured launch replays correctly
 //   after cache_seqlens has been bumped on the device.
 //   Known limit (docs/source/tutorials/get_started/Benchmark.md, "Decoding"): at large batches the kernel tops out near
 //   the same rate of key rows per second at both head dims (about 2.1 TB/s at 128, 1.0 TB/s at 64 on an H100), which
@@ -34,7 +40,7 @@ namespace dec {
 constexpr int kTile = 64;                  // keys per pipeline stage
 constexpr int kWarps = 4;                  // consumer warps, 16 keys of every tile each
 constexpr int kThreads = (kWarps + 1) * 32;
-constexpr int kMaxQ = 16;                  // query rows of the m16n8k16 MMA
+constexpr int kMaxQ = 16;                  // rows of the m16n8k16 MMA: (query head, new token) pairs
 constexpr int kMaxSplits = 32;
 
 template <int D>
@@ -50,14 +56,16 @@ struct Cfg {
 struct Params {
   const __nv_bfloat16* q;      // [B, Sq, A, D] view: strides below (elements), D contiguous
   long q_sb, q_si, q_sh;
-  const __nv_bfloat16* k;      // [B, A, C, D] contiguous
+  const __nv_bfloat16* k;      // [B, G, C, D] contiguous
   const __nv_bfloat16* v;
   __nv_bfloat16* o;            // [B, Sq, A, D] contiguous
-  float* part_o;               // [B, A, splits, Sq, D] (splits > 1)
-  float2* part_ml;             // [B, A, splits, Sq]: (max, sum) in log2 units
+  float* part_o;               // [B, G, splits, r * Sq, D] (splits > 1)
+  float2* part_ml;             // [B, G, splits, r * Sq]: (max, sum) in log2 units
   const int* seqlens;          // [B]
   const int* kv_start;         // [B]
-  int A, C, Sq;
+  int A, G, C, Sq;
+  int rows;                    // r * Sq
+  int row_blocks;              // ceil(rows / 16)
   float scale_log2;
 };
 
@@ -93,11 +101,12 @@ __global__ void __launch_bounds__(kThreads) decode_attn_kernel(const Params p) {
   uint64_t* full = reinterpret_cast<uint64_t*>(smem + (C::kRingBytes > C::kMergeBytes ? C::kRingBytes : C::kMergeBytes));
   uint64_t* empty = full + C::kStages;
 
-  const int split = blockIdx.x, nsplit = gridDim.x, h = blockIdx.y, b = blockIdx.z;
+  const int split = blockIdx.x, nsplit = gridDim.x, b = blockIdx.z;
+  const int kvh = blockIdx.y / p.row_blocks;                  // cache head
+  const int row0 = (blockIdx.y - kvh * p.row_blocks) * kMaxQ; // first (query head in group, token) row of this CTA
+  const int nrows = min(kMaxQ, p.rows - row0);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  // the one place that maps a query head to its cache head (grouped-query attention: h / (A / A_kv))
-  const int kvh = h;
-  const long head_off = ((long)b * p.A + kvh) * p.C * D;
+  const long head_off = ((long)b * p.G + kvh) * p.C * D;
   const int len = p.seqlens[b];
   const int lo = max(p.kv_start[b], 0);
   const int hi = min(len + p.Sq, p.C);   // exclusive; the cache object keeps len + Sq <= C, this only guards memory
@@ -142,13 +151,21 @@ __global__ void __launch_bounds__(kThreads) decode_attn_kernel(const Params p) {
       }
     }
   } else if (my > 0) {
-    // Q fragments (A operand, rows = new tokens; rows >= Sq are zero), loaded once
+    // Q fragments (A operand, rows = (query head, new token) pairs; rows past the last pair are zero), loaded once.
+    // lim: the last visible key of each of this thread's two rows (causal among the new tokens)
     uint32_t qf[D / 16][4];
+    int lim[2];
     {
-      const __nv_bfloat16* qb = p.q + (long)b * p.q_sb + (long)h * p.q_sh;
-      const bool v0 = r0 < p.Sq, v1 = r0 + 8 < p.Sq;
-      const uint32_t* q0 = reinterpret_cast<const uint32_t*>(qb + (long)r0 * p.q_si + c0);
-      const uint32_t* q1 = reinterpret_cast<const uint32_t*>(qb + (long)(r0 + 8) * p.q_si + c0);
+      const int hr = kvh * (p.rows / p.Sq);   // first query head of the group
+      const bool v0 = r0 < nrows, v1 = r0 + 8 < nrows;
+      const int t0 = (row0 + r0) % p.Sq, t1 = (row0 + r0 + 8) % p.Sq;
+      lim[0] = len + t0;
+      lim[1] = len + t1;
+      const __nv_bfloat16* qb = p.q + (long)b * p.q_sb + c0;
+      const uint32_t* q0 = reinterpret_cast<const uint32_t*>(
+          qb + (long)t0 * p.q_si + (long)(hr + (row0 + r0) / p.Sq) * p.q_sh);
+      const uint32_t* q1 = reinterpret_cast<const uint32_t*>(
+          qb + (long)t1 * p.q_si + (long)(hr + (row0 + r0 + 8) / p.Sq) * p.q_sh);
 #pragma unroll
       for (int ks = 0; ks < D / 16; ++ks) {
         qf[ks][0] = v0 ? q0[ks * 8] : 0u;
@@ -182,8 +199,7 @@ __global__ void __launch_bounds__(kThreads) decode_attn_kernel(const Params p) {
 #pragma unroll
         for (int j = 0; j < 4; ++j) {
           const int key = key0 + n * 8 + (j & 1);
-          const int qi = r0 + (j >> 1) * 8;
-          const bool vis = key < hi && key <= len + qi;
+          const bool vis = key < hi && key <= lim[j >> 1];
           s[n][j] = vis ? s[n][j] * p.scale_log2 : -INFINITY;
           mx[j >> 1] = fmaxf(mx[j >> 1], s[n][j]);
         }
@@ -252,9 +268,9 @@ __global__ void __launch_bounds__(kThreads) decode_attn_kernel(const Params p) {
   }
   __syncthreads();
 
-  const long bh = (long)b * p.A + h;
-  for (int e = threadIdx.x; e < p.Sq * D; e += kThreads) {
-    const int i = e / D, d = e % D;
+  const long bg = (long)b * p.G + kvh;
+  for (int e = threadIdx.x; e < nrows * D; e += kThreads) {
+    const int i = e / D, d = e % D;   // row row0 + i: query head kvh * r + (row0 + i) / Sq, token (row0 + i) % Sq
     float M = -INFINITY;
 #pragma unroll
     for (int w = 0; w < kWarps; ++w) M = fmaxf(M, mm[w * kMaxQ + i]);
@@ -267,76 +283,84 @@ __global__ void __launch_bounds__(kThreads) decode_attn_kernel(const Params p) {
       O += mo[(w * kMaxQ + i) * D + d] * f;
     }
     if (nsplit == 1) {
-      p.o[(((long)b * p.Sq + i) * p.A + h) * D + d] = __float2bfloat16(L > 0.f ? O / L : 0.f);
+      const int row = row0 + i, tok = row % p.Sq;
+      const int h = kvh * (p.rows / p.Sq) + row / p.Sq;
+      p.o[(((long)b * p.Sq + tok) * p.A + h) * D + d] = __float2bfloat16(L > 0.f ? O / L : 0.f);
     } else {
-      const long row = (bh * nsplit + split) * p.Sq + i;
+      const long row = (bg * nsplit + split) * p.rows + row0 + i;
       p.part_o[row * D + d] = O;
       if (d == 0) p.part_ml[row] = make_float2(M, L);
     }
   }
 }
 
-// o[b, i, h, :] from the per-split partials, summed in split order
+// o[b, i, h, :] from the per-split partials, summed in split order; one CTA per (cache head, row block, sample)
 template <int D>
 __global__ void __launch_bounds__(128) decode_combine_kernel(const Params p, int nsplit) {
-  const int h = blockIdx.x, b = blockIdx.y;
-  const long bh = (long)b * p.A + h;
-  for (int e = threadIdx.x; e < p.Sq * D; e += blockDim.x) {
-    const int i = e / D, d = e % D;
+  const int b = blockIdx.y;
+  const int kvh = blockIdx.x / p.row_blocks;
+  const int row0 = (blockIdx.x - kvh * p.row_blocks) * kMaxQ;
+  const int nrows = min(kMaxQ, p.rows - row0);
+  const long bg = (long)b * p.G + kvh;
+  for (int e = threadIdx.x; e < nrows * D; e += blockDim.x) {
+    const int i = row0 + e / D, d = e % D;
     float M = -INFINITY;
-    for (int s = 0; s < nsplit; ++s) M = fmaxf(M, p.part_ml[(bh * nsplit + s) * p.Sq + i].x);
+    for (int s = 0; s < nsplit; ++s) M = fmaxf(M, p.part_ml[(bg * nsplit + s) * p.rows + i].x);
     const float base = M == -INFINITY ? 0.f : M;
     float L = 0.f, O = 0.f;
     for (int s = 0; s < nsplit; ++s) {
-      const long row = (bh * nsplit + s) * p.Sq + i;
+      const long row = (bg * nsplit + s) * p.rows + i;
       const float2 ml = p.part_ml[row];
       const float f = fast_exp2(ml.x - base);
       L += ml.y * f;
       O += p.part_o[row * D + d] * f;
     }
-    p.o[(((long)b * p.Sq + i) * p.A + h) * D + d] = __float2bfloat16(L > 0.f ? O / L : 0.f);
+    const int h = kvh * (p.rows / p.Sq) + i / p.Sq;
+    p.o[(((long)b * p.Sq + i % p.Sq) * p.A + h) * D + d] = __float2bfloat16(L > 0.f ? O / L : 0.f);
   }
 }
 
-// one thread per (b, i, head, c < D/2): q and k pairs (c, c + D/2) rotated exactly like rope_qkv_kernel, v copied
+// one thread per (b, i, group, c < D/2): the r q pairs and the k pair (c, c + D/2) rotated exactly like rope_qkv_kernel,
+// v copied
 __global__ void kv_append_kernel(const __nv_bfloat16* __restrict__ qkv, const float* __restrict__ cosv,
                                  const float* __restrict__ sinv, __nv_bfloat16* __restrict__ q_out,
                                  __nv_bfloat16* __restrict__ kc, __nv_bfloat16* __restrict__ vc,
-                                 const int* __restrict__ seqlens, int B, int Sq, int A, int C, int D) {
+                                 const int* __restrict__ seqlens, int B, int Sq, int G, int r, int C, int D) {
   const int half = D / 2;
-  const size_t total = (size_t)B * Sq * A * half;
+  const size_t total = (size_t)B * Sq * G * half;
   for (size_t idx = blockIdx.x * (size_t)blockDim.x + threadIdx.x; idx < total; idx += (size_t)gridDim.x * blockDim.x) {
     const int c = static_cast<int>(idx % half);
-    const size_t head = idx / half;              // (b * Sq + i) * A + a
-    const int a = static_cast<int>(head % A);
-    const int i = static_cast<int>((head / A) % Sq);
-    const int b = static_cast<int>(head / ((size_t)A * Sq));
+    const size_t grp = idx / half;               // (b * Sq + i) * G + g
+    const int g = static_cast<int>(grp % G);
+    const int i = static_cast<int>((grp / G) % Sq);
+    const int b = static_cast<int>(grp / ((size_t)G * Sq));
     const int pos = seqlens[b] + i;
-    const size_t in = head * 3 * D;
-    const size_t crow = (((size_t)b * A + a) * C + pos) * D;
-    float yq1, yq2, yk1, yk2;
-    {
-      const float x1 = __bfloat162float(qkv[in + c]), x2 = __bfloat162float(qkv[in + c + half]);
-      const float k1 = __bfloat162float(qkv[in + D + c]), k2 = __bfloat162float(qkv[in + D + c + half]);
+    const size_t in = grp * (r + 2) * D;
+    const size_t crow = (((size_t)b * G + g) * C + pos) * D;
+    float c1 = 1.f, c2 = 1.f, s1 = 0.f, s2 = 0.f;
+    if (cosv != nullptr) {
+      c1 = cosv[pos * D + c], c2 = cosv[pos * D + c + half];
+      s1 = sinv[pos * D + c], s2 = sinv[pos * D + c + half];
+    }
+    for (int j = 0; j <= r; ++j) {   // slots 0 .. r - 1: q of query head g * r + j; slot r: k
+      const size_t src = in + (size_t)j * D;
+      const float x1 = __bfloat162float(qkv[src + c]), x2 = __bfloat162float(qkv[src + c + half]);
+      float y1 = x1, y2 = x2;
       if (cosv != nullptr) {
-        const float c1 = cosv[pos * D + c], c2 = cosv[pos * D + c + half];
-        const float s1 = sinv[pos * D + c], s2 = sinv[pos * D + c + half];
-        yq1 = x1 * c1 - x2 * s1;
-        yq2 = x2 * c2 + x1 * s2;
-        yk1 = k1 * c1 - k2 * s1;
-        yk2 = k2 * c2 + k1 * s2;
-      } else {
-        yq1 = x1, yq2 = x2, yk1 = k1, yk2 = k2;
+        y1 = x1 * c1 - x2 * s1;
+        y2 = x2 * c2 + x1 * s2;
+      }
+      if (j == r) {
+        kc[crow + c] = __float2bfloat16(y1);
+        kc[crow + c + half] = __float2bfloat16(y2);
+      } else if (q_out != nullptr) {
+        const size_t qrow = (grp * r + j) * D;    // [B, Sq, A, D] with A = G * r
+        q_out[qrow + c] = __float2bfloat16(y1);
+        q_out[qrow + c + half] = __float2bfloat16(y2);
       }
     }
-    if (q_out != nullptr) {
-      q_out[head * D + c] = __float2bfloat16(yq1);
-      q_out[head * D + c + half] = __float2bfloat16(yq2);
-    }
-    kc[crow + c] = __float2bfloat16(yk1);
-    kc[crow + c + half] = __float2bfloat16(yk2);
-    vc[crow + c] = qkv[in + 2 * D + c];
-    vc[crow + c + half] = qkv[in + 2 * D + c + half];
+    vc[crow + c] = qkv[in + (size_t)(r + 1) * D + c];
+    vc[crow + c + half] = qkv[in + (size_t)(r + 1) * D + c + half];
   }
 }
 
@@ -373,18 +397,18 @@ cudaError_t launch_decode(const lb::dec::Params& p, int B, int nsplit, cudaStrea
   using Cfg = lb::dec::Cfg<D>;
   auto kern = lb::dec::decode_attn_kernel<D>;
   if (configure_decode<D>() == 0) return cudaErrorInvalidConfiguration;   // the shared memory opt-in failed
-  kern<<<dim3(nsplit, p.A, B), lb::dec::kThreads, Cfg::kSmem, s>>>(p);
-  if (nsplit > 1) lb::dec::decode_combine_kernel<D><<<dim3(p.A, B), 128, 0, s>>>(p, nsplit);
+  kern<<<dim3(nsplit, p.G * p.row_blocks, B), lb::dec::kThreads, Cfg::kSmem, s>>>(p);
+  if (nsplit > 1) lb::dec::decode_combine_kernel<D><<<dim3(p.G * p.row_blocks, B), 128, 0, s>>>(p, nsplit);
   return cudaGetLastError();
 }
 }  // namespace
 
-// Number of key-range splits per (sample, head): as many as fill the resident CTA slots of the GPU in one wave (a
-// second, partial wave would only add a tail), at most one split per 128 keys of the capacity.  Depends on the
-// shapes only, never on the current lengths.
-extern "C" int lb_decode_splits(int B, int A, int C, int D) {
+// Number of key-range splits per (sample, cache head, row block): as many as fill the resident CTA slots of the GPU in
+// one wave (a second, partial wave would only add a tail), at most one split per 128 keys of the capacity.  `blocks` =
+// G * ceil(r * Sq / 16) CTAs per sample and split.  Depends on the shapes only, never on the current lengths.
+extern "C" int lb_decode_splits(int B, int blocks, int C, int D) {
   const int resident = D == 64 ? configure_decode<64>() : configure_decode<128>();
-  int n = dec_sm_count() * (resident > 0 ? resident : 1) / (B * A);
+  int n = dec_sm_count() * (resident > 0 ? resident : 1) / (B * blocks);
   n = n < (C + 127) / 128 ? n : (C + 127) / 128;
   n = n < lb::dec::kMaxSplits ? n : lb::dec::kMaxSplits;
   return n > 1 ? n : 1;
@@ -392,8 +416,9 @@ extern "C" int lb_decode_splits(int B, int A, int C, int D) {
 
 extern "C" int lb_decode_attn(const void* q, const long* q_strides, const void* k, const void* v, void* o,
                               float* part_o, float* part_ml, const int* seqlens, const int* kv_start, int B, int Sq,
-                              int A, int C, int D, float scale, int nsplit, cudaStream_t s) {
+                              int A, int G, int C, int D, float scale, int nsplit, cudaStream_t s) {
   if (B == 0 || A == 0) return 0;
+  if (G <= 0 || A % G) return -4;
   lb::dec::Params p;
   p.q = static_cast<const __nv_bfloat16*>(q);
   p.q_sb = q_strides[0];
@@ -407,21 +432,24 @@ extern "C" int lb_decode_attn(const void* q, const long* q_strides, const void* 
   p.seqlens = seqlens;
   p.kv_start = kv_start;
   p.A = A;
+  p.G = G;
   p.C = C;
   p.Sq = Sq;
+  p.rows = (A / G) * Sq;
+  p.row_blocks = (p.rows + lb::dec::kMaxQ - 1) / lb::dec::kMaxQ;
   p.scale_log2 = scale * 1.4426950408889634f;
   cudaError_t e = D == 64 ? launch_decode<64>(p, B, nsplit, s) : launch_decode<128>(p, B, nsplit, s);
   return (int)e;
 }
 
 extern "C" int lb_kv_append(const void* qkv, const float* cosv, const float* sinv, void* q_out, void* k_cache,
-                            void* v_cache, const int* seqlens, int B, int Sq, int A, int C, int D, cudaStream_t s) {
-  const size_t total = (size_t)B * Sq * A * (D / 2);
+                            void* v_cache, const int* seqlens, int B, int Sq, int G, int r, int C, int D, cudaStream_t s) {
+  const size_t total = (size_t)B * Sq * G * (D / 2);
   if (total == 0) return 0;
   const int threads = 256;
   const int blocks = (int)((total + threads - 1) / threads < 4096 ? (total + threads - 1) / threads : 4096);
   lb::dec::kv_append_kernel<<<blocks, threads, 0, s>>>(
       static_cast<const __nv_bfloat16*>(qkv), cosv, sinv, static_cast<__nv_bfloat16*>(q_out),
-      static_cast<__nv_bfloat16*>(k_cache), static_cast<__nv_bfloat16*>(v_cache), seqlens, B, Sq, A, C, D);
+      static_cast<__nv_bfloat16*>(k_cache), static_cast<__nv_bfloat16*>(v_cache), seqlens, B, Sq, G, r, C, D);
   return (int)cudaGetLastError();
 }

@@ -225,26 +225,27 @@ __global__ void rope_kernel(const __nv_bfloat16* __restrict__ x, const float* __
   }
 }
 
-// Rotary embedding on the packed QKV projection [tokens(b*s), A, 3*D] (per-head [q|k|v]): q and k are rotated
-// with the position (s + pos_offset), v is copied.  `y` may alias `x` (in-place, used by the backward).
+// Rotary embedding on the grouped packed QKV projection [tokens(b*s), G, r + 2, D] (per K/V group q_0 .. q_{r-1}, k, v;
+// r = 1 is the per-head [q|k|v] layout): the r + 1 q/k slots are rotated with the position (s + pos_offset), v is
+// copied.  `y` may alias `x` (in-place, used by the backward).
 __global__ void rope_qkv_kernel(const __nv_bfloat16* __restrict__ x, const float* __restrict__ cosv,
-                                const float* __restrict__ sinv, __nv_bfloat16* __restrict__ y, size_t heads, int S,
-                                int A, int D, int pos_offset, int backward, int copy_v) {
+                                const float* __restrict__ sinv, __nv_bfloat16* __restrict__ y, size_t groups, int S,
+                                int G, int r, int D, int pos_offset, int backward, int copy_v) {
   const int half = D / 2;
-  const int parts = copy_v ? 3 : 2;
-  const size_t total = heads * parts * half;
+  const int parts = copy_v ? r + 2 : r + 1;
+  const size_t total = groups * parts * half;
   for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
     const int c = static_cast<int>(i % half);
     const int part = static_cast<int>((i / half) % parts);
-    const size_t head = i / (static_cast<size_t>(half) * parts);
-    const size_t base = head * 3 * D + static_cast<size_t>(part) * D;
+    const size_t head = i / (static_cast<size_t>(half) * parts);   // token * G + group
+    const size_t base = head * (r + 2) * D + static_cast<size_t>(part) * D;
     const float x1 = __bfloat162float(x[base + c]), x2 = __bfloat162float(x[base + c + half]);
-    if (part == 2) {
+    if (part == r + 1) {
       y[base + c] = x[base + c];
       y[base + c + half] = x[base + c + half];
       continue;
     }
-    const int s = static_cast<int>((head / A) % S) + pos_offset;
+    const int s = static_cast<int>((head / G) % S) + pos_offset;
     const float c1 = cosv[s * D + c], c2 = cosv[s * D + c + half];
     const float s1 = sinv[s * D + c], s2 = sinv[s * D + c + half];
     float y1, y2;
@@ -648,12 +649,13 @@ extern "C" int lb_rope(const void* x, const float* cosv, const float* sinv, void
                                                                      (size_t)rows, S, D, backward);
   return (int)cudaGetLastError();
 }
-extern "C" int lb_rope_qkv(const void* x, const float* cosv, const float* sinv, void* y, long heads, int S, int A, int D,
-                           int pos_offset, int backward, cudaStream_t s) {
-  if (heads == 0) return 0;
+// groups = tokens * G; r query heads per group
+extern "C" int lb_rope_qkv(const void* x, const float* cosv, const float* sinv, void* y, long groups, int S, int G, int r,
+                           int D, int pos_offset, int backward, cudaStream_t s) {
+  if (groups == 0) return 0;
   const int copy_v = (x != y);
-  lb::rope_qkv_kernel<<<ew_grid((size_t)heads * (copy_v ? 3 : 2) * D / 2, 256), 256, 0, s>>>(
-      (const bf16*)x, cosv, sinv, (bf16*)y, (size_t)heads, S, A, D, pos_offset, backward, copy_v);
+  lb::rope_qkv_kernel<<<ew_grid((size_t)groups * (copy_v ? r + 2 : r + 1) * D / 2, 256), 256, 0, s>>>(
+      (const bf16*)x, cosv, sinv, (bf16*)y, (size_t)groups, S, G, r, D, pos_offset, backward, copy_v);
   return (int)cudaGetLastError();
 }
 // rows per block of the column-sum pass; the number of row blocks is the row count of its fp32 workspace [.., N]

@@ -1,7 +1,8 @@
 """Preallocated KV cache for incremental decoding.
 
 ``StaticKVCache`` keeps one K and one V buffer ``[batch, heads, capacity, head_dim]`` per layer this pipeline stage owns
-(under tensor parallelism: the rank's local heads).  New tokens are written in place at rows ``seqlens[b] + i``
+(``heads`` = the key/value heads, fewer than the query heads under grouped-query attention; under tensor parallelism the
+rank's local ones).  New tokens are written in place at rows ``seqlens[b] + i``
 (:func:`libai_b200.ops.functional.kv_cache_append`) and the decode attention reads the buffers directly, so a decoding
 step copies nothing but the new rows.  ``seqlens`` and ``kv_start`` (the left padding of each sample) are int32 device
 tensors read inside the kernels; ``length`` is their host-side mirror (every sample holds the same number of rows, the
@@ -122,7 +123,8 @@ class StaticKVCache:
 class KVCacheOwner:
     """The model side of a :class:`StaticKVCache` for decoder-only models: ``generate`` sizes it through
     ``allocate_kv_cache``, ``set_cache`` / ``past_key_values`` / ``past_length`` keep the generator's cache protocol.
-    The model lists its self-attention modules (``query_key_value``, ``local_heads``, ``head_size``)."""
+    The model lists its self-attention modules (``query_key_value``, ``head_size``, and ``local_kv_heads`` — the rank's
+    key/value heads — or, for modules without grouped-query attention, ``local_heads``)."""
 
     kv_cache: Optional[StaticKVCache] = None
     past_length = 0
@@ -143,8 +145,8 @@ class KVCacheOwner:
         w = mods[0].query_key_value.weight
         c = self.kv_cache
         if c is None or not c.matches(batch, w.dtype, w.device) or c.capacity < max_length:
-            c = StaticKVCache(len(mods), batch, mods[0].local_heads, mods[0].head_size, max_length, w.dtype, w.device,
-                              owned)
+            heads = getattr(mods[0], "local_kv_heads", mods[0].local_heads)
+            c = StaticKVCache(len(mods), batch, heads, mods[0].head_size, max_length, w.dtype, w.device, owned)
         c.reset()
         self.kv_cache, self.past_length = c, 0
         return c

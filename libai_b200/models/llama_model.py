@@ -7,6 +7,11 @@ per-head ``[q|k|v]`` ``query_key_value`` (col) + ``o_proj`` (row) and a KV cache
 ``SFTLoss`` = CE ignoring label 0 / negative labels (:497-520), ``LlamaForCausalLM`` (:523-649).  Parameter names
 follow the reference so its HF loader mapping (projects/Llama/utils/llama_loader.py) carries over.
 
+Grouped-query attention (``num_key_value_heads`` < ``num_attention_heads``, Llama-2-70B / Llama-3 / Mistral / Qwen2): the
+``query_key_value`` outputs are laid out per key/value group, ``[g, r + 2, d]`` = ``q_0 .. q_{r-1}, k, v`` (Megatron's
+grouped layout; ``r = 1`` is the per-head ``[q|k|v]`` layout), so a column-parallel split by tensor-parallel rank hands
+every rank whole groups.  The kernels read the ``g`` K/V heads directly and the KV cache holds ``g`` heads.
+
 H100 path: rotary runs as one pass over the packed QKV projection (``rope_qkv`` kernel, v copied) feeding the
 flash-attention kernel; SwiGLU and RMSNorm are native kernels; the LM head is vocab-parallel with the fused
 vocab-parallel cross entropy (the reference replicates ``lm_head``).
@@ -112,17 +117,27 @@ class LlamaMLP(nn.Module):
 class LlamaAttention(nn.Module):
     def __init__(self, hidden_size, num_attention_heads, max_position_embeddings, init_method=xavier_normal_,
                  output_layer_init_method=None, scale_mask_softmax_fusion=False, attn_mask_type=AttnMaskType.causal,
-                 qkv_bias=False, *, layer_idx=0):
+                 qkv_bias=False, num_key_value_heads=None, *, layer_idx=0):
         super().__init__()
         output_layer_init_method = output_layer_init_method or init_method
         topo = dutil.get_dist_util()
-        self.hidden_size, self.num_heads = hidden_size, num_attention_heads
+        tp = topo.tensor_parallel_size
+        kv_heads = num_attention_heads if num_key_value_heads is None else int(num_key_value_heads)
+        if kv_heads <= 0 or num_attention_heads % kv_heads:
+            raise ValueError(f"num_attention_heads={num_attention_heads} must be a multiple of "
+                             f"num_key_value_heads={kv_heads}")
+        if kv_heads % tp:
+            raise ValueError(f"num_key_value_heads={kv_heads} must be divisible by the tensor-parallel size {tp} "
+                             "(every rank holds whole key/value groups)")
+        self.hidden_size, self.num_heads, self.num_kv_heads = hidden_size, num_attention_heads, kv_heads
         self.head_size = hidden_size // num_attention_heads
-        assert num_attention_heads % topo.tensor_parallel_size == 0
-        self.local_heads = num_attention_heads // topo.tensor_parallel_size
+        assert num_attention_heads % tp == 0
+        self.local_heads = num_attention_heads // tp
+        self.local_kv_heads = kv_heads // tp
         self.norm_factor = 1.0 / math.sqrt(float(self.head_size))
         self.attn_mask_type = attn_mask_type
-        self.query_key_value = Linear(hidden_size, hidden_size * 3, bias=qkv_bias, parallel="col",
+        qkv_out = hidden_size * 3 if kv_heads == num_attention_heads else (num_attention_heads + 2 * kv_heads) * self.head_size
+        self.query_key_value = Linear(hidden_size, qkv_out, bias=qkv_bias, parallel="col",
                                       init_method=init_method, layer_idx=layer_idx)
         self.o_proj = Linear(hidden_size, hidden_size, bias=False, parallel="row",
                              init_method=output_layer_init_method, layer_idx=layer_idx)
@@ -130,9 +145,10 @@ class LlamaAttention(nn.Module):
     def forward(self, hidden_states, attention_mask=None, past_key_value=None, cos_cached=None, sin_cached=None,
                 use_cache=False):
         sp = dutil.get_dist_util().sequence_parallel and hidden_states.dim() == 2
-        a, d = self.local_heads, self.head_size
+        a, d, g = self.local_heads, self.head_size, self.local_kv_heads
         bsz, tgt_len = get_sp_shape() if sp else hidden_states.shape[:2]
-        qkv = self.query_key_value(hidden_states).view(bsz, -1, a, 3 * d)
+        qkv = self.query_key_value(hidden_states)
+        qkv = qkv.view(bsz, -1, a, 3 * d) if g == a else qkv.view(bsz, -1, g, a // g + 2, d)
         if isinstance(past_key_value, KVCacheLayer):
             context = self._cached_attention(qkv, attention_mask, past_key_value, cos_cached, sin_cached)
             context = context.reshape(-1, a * d) if sp else context.reshape(bsz, -1, a * d)
@@ -146,8 +162,7 @@ class LlamaAttention(nn.Module):
         ):
             context = OF.attention_qkvpacked(qkv, causal=True, scale=self.norm_factor).reshape(bsz, -1, a * d)
         else:
-            q4 = qkv.permute(0, 2, 1, 3)
-            query, key, value = q4[..., :d], q4[..., d : 2 * d], q4[..., 2 * d :]
+            query, key, value = (t.permute(0, 2, 1, 3) for t in OF.split_qkv(qkv))   # key, value: g heads
             if past_key_value is not None:
                 key = torch.cat((past_key_value[0].type_as(key), key), dim=2)
                 value = torch.cat((past_key_value[1].type_as(value), value), dim=2)
@@ -203,14 +218,16 @@ class CasualMask(nn.Module):
 class LlamaDecoderLayer(nn.Module):
     def __init__(self, hidden_size, intermediate_size, num_attention_heads, is_decoder=False, rms_norm_eps=1e-5,
                  max_position_embeddings=None, init_method=xavier_normal_, output_layer_init_method=None,
-                 scale_mask_softmax_fusion=False, attn_mask_type=AttnMaskType.causal, qkv_bias=False, *, layer_idx=0):
+                 scale_mask_softmax_fusion=False, attn_mask_type=AttnMaskType.causal, qkv_bias=False,
+                 num_key_value_heads=None, *, layer_idx=0):
         super().__init__()
         self.layer_idx, self.is_decoder = layer_idx, is_decoder
         self.input_layernorm = RMSLayerNorm(hidden_size, eps=rms_norm_eps, layer_idx=layer_idx)
         self.self_attn = LlamaAttention(hidden_size, num_attention_heads, max_position_embeddings,
                                         init_method=init_method, output_layer_init_method=output_layer_init_method,
                                         scale_mask_softmax_fusion=scale_mask_softmax_fusion,
-                                        attn_mask_type=attn_mask_type, qkv_bias=qkv_bias, layer_idx=layer_idx)
+                                        attn_mask_type=attn_mask_type, qkv_bias=qkv_bias,
+                                        num_key_value_heads=num_key_value_heads, layer_idx=layer_idx)
         self.post_attention_layernorm = RMSLayerNorm(hidden_size, eps=rms_norm_eps, layer_idx=layer_idx)
         self.mlp = LlamaMLP(hidden_size, intermediate_size, init_method, output_layer_init_method, layer_idx=layer_idx)
 
@@ -231,7 +248,7 @@ class LlamaModel(nn.Module):
     def __init__(self, hidden_layers, vocab_size, hidden_size, intermediate_size, num_attention_heads,
                  max_position_embeddings=1024, rms_norm_eps=1e-5, initializer_range=0.02,
                  use_scaled_init_for_output_weights=True, scale_mask_softmax_fusion=False, amp_enabled=False,
-                 qkv_bias=False, rope_base=10000.0):
+                 qkv_bias=False, rope_base=10000.0, num_key_value_heads=None):
         super().__init__()
         init_method = init_method_normal(sigma=initializer_range)
         output_layer_init_method = (
@@ -245,7 +262,8 @@ class LlamaModel(nn.Module):
                                   max_position_embeddings=max_position_embeddings, init_method=init_method,
                                   output_layer_init_method=output_layer_init_method,
                                   scale_mask_softmax_fusion=scale_mask_softmax_fusion,
-                                  attn_mask_type=AttnMaskType.causal, qkv_bias=qkv_bias, layer_idx=i)
+                                  attn_mask_type=AttnMaskType.causal, qkv_bias=qkv_bias,
+                                  num_key_value_heads=num_key_value_heads, layer_idx=i)
                 for i in range(hidden_layers)
             ]
         )
@@ -328,7 +346,7 @@ class LlamaForCausalLM(nn.Module, PipelineStageMixin, Generator, KVCacheOwner):
     def __init__(self, hidden_layers, vocab_size, hidden_size, intermediate_size, num_attention_heads,
                  max_position_embeddings=1024, rms_norm_eps=1e-5, initializer_range=0.02,
                  use_scaled_init_for_output_weights=True, scale_mask_softmax_fusion=False, amp_enabled=False,
-                 qkv_bias=False, rope_base=10000.0, cfg=None):
+                 qkv_bias=False, rope_base=10000.0, num_key_value_heads=None, cfg=None):
         super().__init__()
         self.cfg = cfg
         self.hidden_layers = hidden_layers
@@ -339,7 +357,7 @@ class LlamaForCausalLM(nn.Module, PipelineStageMixin, Generator, KVCacheOwner):
             initializer_range=initializer_range,
             use_scaled_init_for_output_weights=use_scaled_init_for_output_weights,
             scale_mask_softmax_fusion=scale_mask_softmax_fusion, amp_enabled=amp_enabled, qkv_bias=qkv_bias,
-            rope_base=rope_base,
+            rope_base=rope_base, num_key_value_heads=num_key_value_heads,
         )
         self.casual_mask = CasualMask(max_position_embeddings, layer_idx=0)
         self.lm_head = Linear(hidden_size, vocab_size, bias=False, parallel="col",
@@ -354,7 +372,7 @@ class LlamaForCausalLM(nn.Module, PipelineStageMixin, Generator, KVCacheOwner):
                 "rms_norm_eps initializer_range use_scaled_init_for_output_weights scale_mask_softmax_fusion "
                 "amp_enabled").split()
         out = {k: cfg[k] for k in keys}
-        for k in ("qkv_bias", "rope_base"):
+        for k in ("qkv_bias", "rope_base", "num_key_value_heads"):
             if k in cfg:
                 out[k] = cfg[k]
         out["cfg"] = cfg

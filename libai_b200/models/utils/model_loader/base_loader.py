@@ -187,9 +187,18 @@ class ModelLoaderHuggerFace(LoadPretrainedBase):
         return state_dict
 
     @staticmethod
-    def _fix_qkv_ordering(qkv, head_size, num_heads, hidden_size=None, checkpoint_version=0.0):
+    def _fix_qkv_ordering(qkv, head_size, num_heads, hidden_size=None, checkpoint_version=0.0, num_kv_heads=None):
         """``[q; k; v]`` blocks (each ``[a·d, …]``) → per-head interleaved ``[a, (q|k|v), d, …]`` rows, the layout
-        the fused ``query_key_value`` projection (and its tensor-parallel split over heads) expects."""
+        the fused ``query_key_value`` projection (and its tensor-parallel split over heads) expects.  With
+        ``num_kv_heads`` = g < a (grouped-query attention: q ``[a·d, …]``, k and v ``[g·d, …]``) the rows are grouped
+        ``[g, (q_0 .. q_{r-1}|k|v), d, …]``, ``r = a / g``."""
+        if num_kv_heads is not None and num_kv_heads != num_heads:
+            g, r = num_kv_heads, num_heads // num_kv_heads
+            rest = tuple(qkv.shape[1:])
+            q, k, v = qkv.split([num_heads * head_size, g * head_size, g * head_size])
+            out = torch.cat([q.reshape(g, r, head_size, *rest), k.reshape(g, 1, head_size, *rest),
+                             v.reshape(g, 1, head_size, *rest)], dim=1)
+            return out.reshape(-1, *rest).contiguous()
         n = qkv.shape[0] // (head_size * num_heads)
         if qkv.dim() > 1:
             hidden_size = qkv.shape[1] if hidden_size is None else hidden_size
@@ -202,8 +211,9 @@ class ModelLoaderHuggerFace(LoadPretrainedBase):
         """Checkpoint tensors are kept in their stored dtype on CPU; the copy into the parameter casts."""
         return tensor.contiguous() if torch.is_tensor(tensor) else torch.as_tensor(tensor)
 
-    def _fuse_qkv(self, sd, q, k, v, out, head_size, num_heads, transpose=False):
-        """Pop q/k/v entries (weight + optional bias) and store the fused, re-ordered tensor under ``out``."""
+    def _fuse_qkv(self, sd, q, k, v, out, head_size, num_heads, transpose=False, num_kv_heads=None):
+        """Pop q/k/v entries (weight + optional bias) and store the fused, re-ordered tensor under ``out``
+        (``num_kv_heads``: see :meth:`_fix_qkv_ordering`)."""
         for suffix in ("weight", "bias"):
             keys = [f"{n}.{suffix}" for n in (q, k, v)]
             if not all(kk in sd for kk in keys):
@@ -211,7 +221,8 @@ class ModelLoaderHuggerFace(LoadPretrainedBase):
             parts = [sd.pop(kk) for kk in keys]
             if transpose and suffix == "weight":
                 parts = [p.t() for p in parts]
-            sd[f"{out}.{suffix}"] = self._fix_qkv_ordering(torch.cat(parts, dim=0), head_size, num_heads)
+            sd[f"{out}.{suffix}"] = self._fix_qkv_ordering(torch.cat(parts, dim=0), head_size, num_heads,
+                                                           num_kv_heads=num_kv_heads)
 
     @staticmethod
     def _rename(sd, rules: Sequence[Tuple[str, str]]):

@@ -1,5 +1,6 @@
 """Llama loaders (reference projects/Llama/utils/llama_loader.py): HF ``q_proj/k_proj/v_proj`` → fused per-head
-interleaved ``query_key_value``; everything else keeps its name."""
+interleaved ``query_key_value`` (grouped per key/value head for grouped-query checkpoints); everything else keeps its
+name."""
 import collections
 
 from .base_loader import ModelLoaderHuggerFace, ModelLoaderLiBai
@@ -14,11 +15,12 @@ class LlamaLoaderHuggerFace(ModelLoaderHuggerFace):
     def _convert_state_dict(self, sd, cfg):
         sd = collections.OrderedDict(sd)
         heads, hidden, layers = cfg.get("num_attention_heads"), cfg.get("hidden_size"), cfg.get("hidden_layers")
+        kv_heads = cfg.get("num_key_value_heads") or heads
         prefix = "model." if any(k.startswith("model.") for k in sd) else ""
         for i in range(layers):
             base = f"{prefix}layers.{i}.self_attn"
             self._fuse_qkv(sd, f"{base}.q_proj", f"{base}.k_proj", f"{base}.v_proj", f"{base}.query_key_value",
-                           hidden // heads, heads)
+                           hidden // heads, heads, num_kv_heads=kv_heads)
         out = collections.OrderedDict()
         for k, v in sd.items():
             if k.endswith("rotary_emb.inv_freq"):
@@ -35,11 +37,8 @@ class LlamaLoaderHuggerFace(ModelLoaderHuggerFace):
             "max_position_embeddings": "max_position_embeddings", "intermediate_size": "intermediate_size",
             "rms_norm_eps": "rms_norm_eps", "vocab_size": "vocab_size", "initializer_range": "initializer_range",
             "rope_theta": "rope_base", "bos_token_id": "bos_token_id", "eos_token_id": "eos_token_id",
-            "pad_token_id": "pad_token_id",
+            "pad_token_id": "pad_token_id", "num_key_value_heads": "num_key_value_heads",
         })
-        kv = cfg.get("num_key_value_heads")
-        if kv is not None and kv != cfg.get("num_attention_heads"):
-            raise NotImplementedError("grouped-query checkpoints need num_key_value_heads == num_attention_heads")
 
 
 class LlamaLoaderLiBai(ModelLoaderLiBai):

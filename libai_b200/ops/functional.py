@@ -515,11 +515,53 @@ class _BiasAddFn(torch.autograd.Function):
 
 # --------------------------------------------------------------------------------------
 # attention
+#
+# Grouped-query attention (GQA): ``a`` query heads share ``g`` key/value heads (``a % g == 0``), query head ``h`` reading
+# K/V head ``h // (a // g)``.  The packed projection of a grouped model is ``[b, s, g, r + 2, d]`` with ``q_0 .. q_{r-1},
+# k, v`` per group (``r = a // g``); the 4-D ``[b, s, a, 3d]`` (per-head ``[q|k|v]``) keeps meaning MHA and is the
+# same memory as the grouped view with ``r = 1``.
 # --------------------------------------------------------------------------------------
+def _expand_kv(x, heads: int):
+    """K/V ``[.., g, s, d]`` repeated to ``heads`` query heads (reference math only: the kernels read the g heads)."""
+    g = x.shape[-3]
+    if g == heads:
+        return x
+    if heads % g:
+        raise ValueError(f"{heads} query heads cannot share {g} key/value heads")
+    return x.repeat_interleave(heads // g, dim=-3)
+
+
+def split_qkv(qkv):
+    """q ``[b, s, a, d]`` and k, v ``[b, s, g, d]`` of a packed projection ``[b, s, a, 3d]`` or ``[b, s, g, r + 2, d]``."""
+    if qkv.dim() == 4:
+        d = qkv.shape[-1] // 3
+        return qkv[..., :d], qkv[..., d : 2 * d], qkv[..., 2 * d :]
+    b, s, g, r2, d = qkv.shape
+    return qkv[..., : r2 - 2, :].reshape(b, s, g * (r2 - 2), d), qkv[..., r2 - 2, :], qkv[..., r2 - 1, :]
+
+
+def _packed_views(qkv):
+    """The attention kernels' operands, read in place: q ``[b, a, s, d]`` (from ``[b, s, a, 3d]``) or ``[b, g, r, s, d]``
+    (from ``[b, s, g, r + 2, d]``), k and v ``[b, g, s, d]``."""
+    if qkv.dim() == 4:
+        d = qkv.shape[-1] // 3
+        v4 = qkv.permute(0, 2, 1, 3)
+        return v4[..., :d], v4[..., d : 2 * d], v4[..., 2 * d :]
+    r = qkv.shape[3] - 2
+    return (qkv[:, :, :, :r].permute(0, 2, 3, 1, 4), qkv[:, :, :, r].permute(0, 2, 1, 3),
+            qkv[:, :, :, r + 1].permute(0, 2, 1, 3))
+
+
+def packed_head_dim(qkv) -> int:
+    return qkv.shape[-1] // 3 if qkv.dim() == 4 else qkv.shape[-1]
+
+
 def attention_ref(q, k, v, *, causal: bool, scale: float, mask=None, bias=None, dropout_p: float = 0.0,
                   training: bool = False, fill: float = -10000.0):
-    """Unfused attention on ``[b, a, s, d]`` tensors. ``mask``: 1 = keep, 0 = masked
+    """Unfused attention on ``[b, a, s, d]`` queries and ``[b, g, s, d]`` keys / values (``g`` divides ``a``; the K/V
+    heads are repeated here). ``mask``: 1 = keep, 0 = masked
     (filled with ``fill`` like the reference: libai/layers/attention.py:223-245)."""
+    k, v = _expand_kv(k, q.shape[-3]), _expand_kv(v, q.shape[-3])
     scores = torch.matmul(q.float(), k.float().transpose(-1, -2)) * scale
     if bias is not None:
         scores = scores + bias.float()
@@ -584,16 +626,14 @@ class _FlashAttnFn(torch.autograd.Function):
 
 
 class _FlashAttnPackedFn(torch.autograd.Function):
-    """Self-attention straight from the packed QKV projection ``[b, s, a, 3d]`` (per-head ``[q|k|v]``):
-    the kernels read q/k/v through strided TMA maps and the backward writes one packed ``dqkv`` – no
-    slicing, no gradient accumulation kernels around the attention."""
+    """Self-attention straight from the packed QKV projection ``[b, s, a, 3d]`` (per-head ``[q|k|v]``) or
+    ``[b, s, g, r + 2, d]`` (grouped): the kernels read q/k/v through strided TMA maps and the backward writes one packed
+    ``dqkv`` of the same layout – no slicing, no expanded K/V, no gradient accumulation kernels around the attention."""
 
     @staticmethod
     def forward(ctx, qkv, causal, scale, kv_lens, p_drop=0.0, alibi_slopes=None):
         ext = load_ext()
-        d = qkv.shape[-1] // 3
-        v4 = qkv.permute(0, 2, 1, 3)
-        q, k, v = v4[..., :d], v4[..., d : 2 * d], v4[..., 2 * d :]
+        q, k, v = _packed_views(qkv)
         o, lse, rng_state = ext.attn_fwd(q, k, v, causal, scale, kv_lens, None, alibi_slopes, p_drop,
                                          tp_rng_salt(True) if p_drop > 0 else 0)
         count_launch()
@@ -605,9 +645,7 @@ class _FlashAttnPackedFn(torch.autograd.Function):
     def backward(ctx, go):
         ext = load_ext()
         qkv, o, lse, kv_lens, rng_state, slopes = ctx.saved_tensors
-        d = qkv.shape[-1] // 3
-        v4 = qkv.permute(0, 2, 1, 3)
-        q, k, v = v4[..., :d], v4[..., d : 2 * d], v4[..., 2 * d :]
+        q, k, v = _packed_views(qkv)
         _, _, _, dqkv = ext.attn_bwd(go.permute(0, 2, 1, 3), q, k, v, o, lse, ctx.causal, ctx.scale, kv_lens, None, slopes,
                                      None, ctx.p_drop, rng_state if ctx.p_drop > 0 else None)
         count_launch(3)
@@ -619,14 +657,14 @@ def attention_qkvpacked_supported(qkv, mask, dropout_p, training) -> bool:
         use_native(qkv)
         and qkv.dtype == torch.bfloat16
         and mask is None
-        and qkv.shape[-1] // 3 in (64, 128)
+        and packed_head_dim(qkv) in (64, 128)
         and qkv.is_contiguous()
     )
 
 
 def attention_qkvpacked(qkv, *, causal: bool, scale: float, kv_lens=None, dropout_p: float = 0.0, training: bool = False,
                         alibi_slopes=None):
-    """qkv ``[b, s, a, 3d]`` → context ``[b, s, a, d]``; ``kv_lens`` (int32 ``[b]``): valid keys per sample
+    """qkv ``[b, s, a, 3d]`` or grouped ``[b, s, g, r + 2, d]`` → context ``[b, s, a, d]``; ``kv_lens`` (int32 ``[b]``): valid keys per sample
     of a right-padded batch (keys beyond it are masked inside the kernel); ``dropout_p`` > 0 in training drops
     attention probabilities inside the kernel (Philox, TP-rank salted)."""
     p = float(dropout_p) if training else 0.0
@@ -635,7 +673,8 @@ def attention_qkvpacked(qkv, *, causal: bool, scale: float, kv_lens=None, dropou
 
 def attention(q, k, v, *, causal: bool = False, scale: Optional[float] = None, mask=None, bias=None,
               dropout_p: float = 0.0, training: bool = False, alibi_slopes=None, kv_lens=None):
-    """Softmax attention on ``[b, a, s, d]``.  The native flash kernels handle causal / full / key-padding
+    """Softmax attention of q ``[b, a, s, d]`` over k, v ``[b, g, s, d]`` (``g = a`` or, grouped-query, a divisor of
+    ``a``).  The native flash kernels handle causal / full / key-padding
     (``kv_lens``) masking, an additive score bias (dense ``[b|1, a|1, s, s]`` — T5 relative positions — or
     ``alibi_slopes`` ``[a]``) and dropout on the probabilities; arbitrary dense 0/1 masks and cross attention with
     different query / key lengths use the reference math."""
@@ -663,7 +702,7 @@ def attention(q, k, v, *, causal: bool = False, scale: Optional[float] = None, m
 
 
 # --------------------------------------------------------------------------------------
-# KV-cache decoding: caches are [b, a, C, d] buffers (libai_b200.inference.kv_cache.StaticKVCache); ``cache_seqlens``
+# KV-cache decoding: caches are [b, g, C, d] buffers (g = the key/value heads) (libai_b200.inference.kv_cache.StaticKVCache); ``cache_seqlens``
 # (int32 [b]) is the number of rows already held, ``kv_start`` (int32 [b]) the left padding of each sample
 # --------------------------------------------------------------------------------------
 def _decode_native(x, k_cache) -> bool:
@@ -678,7 +717,8 @@ def _decode_native(x, k_cache) -> bool:
 
 
 def kv_cache_append(qkv, k_cache, v_cache, cache_seqlens, cos=None, sin=None, return_q: bool = True):
-    """Write k, v of the packed projection ``qkv [b, s, a, 3d]`` into rows ``cache_seqlens[b] + i`` of the caches.  With
+    """Write k, v of the packed projection ``qkv`` (``[b, s, a, 3d]``, or grouped ``[b, s, g, r + 2, d]``) into rows
+    ``cache_seqlens[b] + i`` of the caches ``[b, g, C, d]``.  With
     ``cos/sin`` (fp32 ``[positions, d]``) q and k are first rotated at those positions, exactly as
     :func:`apply_rotary_qkv` with ``pos_offset = cache_seqlens[b]`` does.  Returns q ``[b, s, a, d]`` (rotated when the
     tables are given) when ``return_q``, else None."""
@@ -693,9 +733,8 @@ def kv_cache_append(qkv, k_cache, v_cache, cache_seqlens, cos=None, sin=None, re
 
 
 def kv_cache_append_ref(qkv, k_cache, v_cache, cache_seqlens, cos=None, sin=None):
-    d = qkv.shape[-1] // 3
     s_len = qkv.shape[1]
-    q, k, v = qkv[..., :d], qkv[..., d : 2 * d], qkv[..., 2 * d :]
+    q, k, v = split_qkv(qkv)
     starts = [int(x) for x in cache_seqlens.tolist()]
     if cos is not None:
         pos = torch.tensor(starts, device=cos.device)[:, None] + torch.arange(s_len, device=cos.device)[None]
@@ -711,7 +750,7 @@ def kv_cache_append_ref(qkv, k_cache, v_cache, cache_seqlens, cos=None, sin=None
 
 def decode_attention(q, k_cache, v_cache, cache_seqlens, kv_start, *, scale: float, splits: int = 0):
     """Attention of ``q [b, s, a, d]`` (new tokens, already appended to the caches; any strides with d contiguous) over
-    the caches: query ``i`` of sample ``b`` sees exactly the keys ``kv_start[b] <= j <= cache_seqlens[b] + i``.  Returns
+    the caches ``[b, g, C, d]`` (query head ``h`` reads cache head ``h // (a // g)``): query ``i`` of sample ``b`` sees exactly the keys ``kv_start[b] <= j <= cache_seqlens[b] + i``.  Returns
     ``[b, s, a, d]`` contiguous; a query without a visible key gets zeros.  The native kernel takes up to 16 new tokens
     and reads lengths on the device (no host sync; one CUDA-graph capture replays after the lengths change); ``splits``
     > 0 fixes its number of key-range splits."""
@@ -886,7 +925,8 @@ def apply_rotary(x, cos, sin):
 
 
 class _RopeQKVFn(torch.autograd.Function):
-    """Rotary embedding on q and k of the packed projection ``[b, s, a, 3d]`` in one pass (v copied);
+    """Rotary embedding on every q and k of the packed projection (``[b, s, a, 3d]`` or ``[b, s, g, r + 2, d]``) in one
+    pass (v copied);
     the backward rotates the packed ``dqkv`` of the attention kernel in place with the inverse rotation."""
 
     @staticmethod
@@ -907,12 +947,18 @@ class _RopeQKVFn(torch.autograd.Function):
 
 
 def apply_rotary_qkv(qkv, cos, sin, pos_offset: int = 0):
-    """qkv ``[b, s, a, 3d]`` (per-head ``[q|k|v]``); cos/sin fp32 ``[max_pos, d]``; token ``i`` of the
-    sequence uses position ``i + pos_offset``."""
+    """qkv ``[b, s, a, 3d]`` (per-head ``[q|k|v]``) or grouped ``[b, s, g, r + 2, d]`` (per group ``q_0 .. q_{r-1}, k,
+    v``); cos/sin fp32 ``[max_pos, d]``; token ``i`` of the sequence uses position ``i + pos_offset``."""
     if use_native(qkv) and qkv.dtype == torch.bfloat16 and cos.dtype == torch.float32 and qkv.is_contiguous():
         return _RopeQKVFn.apply(qkv, cos, sin, int(pos_offset))
-    d = qkv.shape[-1] // 3
     s_len = qkv.shape[1]
+    if qkv.dim() == 5:
+        r = qkv.shape[3] - 2
+        c = cos[pos_offset : pos_offset + s_len, None, None, :].to(qkv.dtype)
+        sn = sin[pos_offset : pos_offset + s_len, None, None, :].to(qkv.dtype)
+        qk = qkv[..., : r + 1, :]
+        return torch.cat([qk * c + rotate_half(qk) * sn, qkv[..., r + 1 :, :]], dim=3)
+    d = qkv.shape[-1] // 3
     c = cos[pos_offset : pos_offset + s_len, None, :].to(qkv.dtype)
     sn = sin[pos_offset : pos_offset + s_len, None, :].to(qkv.dtype)
     q, k, v = qkv[..., :d], qkv[..., d : 2 * d], qkv[..., 2 * d :]

@@ -66,6 +66,9 @@ class LlamaForCausalLM(_BaseLlama):
         # swap in the gated attention for the adapted layers (weights are shared with the originals)
         for layer in self.model.layers[-self.adapter_layer:]:
             old = layer.self_attn
+            if old.num_kv_heads != old.num_heads:
+                # the adapter keys / values are read from the per-head [q|k|v] view of query_key_value
+                raise ValueError("LLaMA-Adapter needs num_key_value_heads == num_attention_heads")
             new = AdapterAttention(old.hidden_size, old.num_heads, None, layer_idx=layer.layer_idx)
             new.query_key_value, new.o_proj = old.query_key_value, old.o_proj
             layer.self_attn = new
