@@ -11,6 +11,11 @@
 // r = 1 is the per-head [q|k|v] layout) are read without a copy.  K/V use 4-D maps over the G heads.  Everything else
 // (O, lse, bias, ALiBi slope, dropout stream, kv_lens) stays per query head.
 //
+// Rectangular problems: Sq queries against Sk keys.  Key j is visible to query i of sample b iff
+// kv_start[b] <= j < kv_lens[b] (defaults 0 and Sk; kv_lens is clamped to >= 1 as it always was) and, when causal,
+// j <= i + (Sk - Sq) (bottom-right alignment, as in decode attention).  A query without a visible key gets O = 0,
+// lse = 0 and dQ = 0, and adds nothing to dK / dV.
+//
 // Forward, one CTA per (batch, query head, 128-query block), 384 threads:
 //   warpgroup 0  TMA producer (one elected thread): Q once, then K/V tiles of 128 keys (double buffered); it gives
 //                its registers to the consumers (setmaxnreg)
@@ -31,16 +36,17 @@ constexpr int ATT_BWD_BM = 64;   // queries per step (backward)
 constexpr int ATT_BWD_THREADS = 160;
 
 struct AttnFwdParams {
-  __nv_bfloat16* o;   // [B, S, A, D]
-  float* lse;         // [B, A, S]
-  int B, A, S;
+  __nv_bfloat16* o;   // [B, Sq, A, D]
+  float* lse;         // [B, A, Sq]
+  int B, A, Sq, Sk;
   int r;              // query heads per K/V head
   int causal;
   float scale_log2;   // scale * log2(e)
   float scale;
-  const int* kv_lens; // optional [B]: number of valid keys per sample (right-padded batches)
-  // additive score bias (v2 kernel): dense bf16 [.., S, S] with (batch, head, query) strides in elements (0 = broadcast;
-  // T5 relative-position bias, Swin/BERT style masks) or ALiBi slopes per head (bias = slope * (key - query))
+  const int* kv_lens; // optional [B]: end of the visible keys per sample (right-padded batches)
+  const int* kv_start;   // optional [B]: start of the visible keys per sample (left-padded batches)
+  // additive score bias (v2 kernel): dense bf16 [.., Sq, Sk] with (batch, head, query) strides in elements (0 = broadcast;
+  // T5 relative-position bias, Swin/BERT style masks) or ALiBi slopes per head (bias = slope * (key - query - (Sk - Sq)))
   const __nv_bfloat16* bias;
   long bias_strides[3];
   const float* alibi_slopes;
@@ -101,9 +107,13 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
   const int head = blockIdx.y, batch = blockIdx.z;
   const int kv_head = head / p.r;
   const int q0 = q_blk * ATT_BM;
-  const int kv_len = p.kv_lens != nullptr ? max(1, min(p.S, p.kv_lens[batch])) : p.S;
-  int nkv = (kv_len + ATT_BN - 1) / ATT_BN;
-  if (p.causal) nkv = min(nkv, q_blk + 1);
+  const int kv_len = p.kv_lens != nullptr ? max(1, min(p.Sk, p.kv_lens[batch])) : p.Sk;
+  const int kv_beg = p.kv_start != nullptr ? min(max(p.kv_start[batch], 0), p.Sk) : 0;
+  const int off = p.Sk - p.Sq;   // causal offset: query i sees keys j <= i + off
+  // key tiles j0 .. j0 + nkv - 1 hold every key some row of this block can see; the others are not loaded
+  const int key_end = p.causal ? min(kv_len, min(q0 + ATT_BM, p.Sq) + off) : kv_len;
+  const int j0 = kv_beg / ATT_BN;
+  const int nkv = max(0, (key_end + ATT_BN - 1) / ATT_BN - j0);
 
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmap_q);
@@ -128,9 +138,9 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
 #pragma unroll
       for (int c = 0; c < Cfg::CHUNKS; ++c)
         tma_load_5d(sQ + c * (ATT_BM * 128), &tmap_q, q_full, c * 64, q0, head - kv_head * p.r, kv_head, batch);
-      for (int j = 0; j < nkv; ++j) {
-        const int b = j & 1;
-        const uint32_t par = ((j >> 1) & 1) ^ 1;
+      for (int it = 0; it < nkv; ++it) {
+        const int j = j0 + it, b = it & 1;
+        const uint32_t par = ((it >> 1) & 1) ^ 1;
         mbar_wait(&k_empty[b], par);
         mbar_arrive_expect_tx(&k_full[b], Cfg::TILE_BYTES);
 #pragma unroll
@@ -151,11 +161,12 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
   const int t = threadIdx.x % 128;
   const int r_loc = 64 * wg + 16 * (t / 32) + (t % 32) / 4;   // this thread's rows: r_loc and r_loc + 8
   const int cq = 2 * (t % 4);                                  // its columns inside every 8-column group: cq, cq + 1
-  int q_idx[2], key_lim[2];
+  // keys kv_beg + [0, vis_len) are visible to row h: one unsigned comparison of key - kv_beg per element tests both ends
+  int q_idx[2], vis_len[2];
 #pragma unroll
   for (int h = 0; h < 2; ++h) {
     q_idx[h] = q0 + r_loc + 8 * h;
-    key_lim[h] = p.causal ? min(kv_len, q_idx[h] + 1) : kv_len;   // keys [0, key_lim) are visible to this row
+    vis_len[h] = max(0, (p.causal ? min(kv_len, q_idx[h] + off + 1) : kv_len) - kv_beg);
   }
   constexpr float LOG2E = 1.4426950408889634f;
   unsigned long long rng_seed = 0, rng_offset = 0;
@@ -173,7 +184,7 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
 #pragma unroll
     for (int h = 0; h < 2; ++h)
       bias_row[h] = p.bias + batch * p.bias_strides[0] + head * p.bias_strides[1] +
-                    static_cast<long>(min(q_idx[h], p.S - 1)) * p.bias_strides[2];
+                    static_cast<long>(min(q_idx[h], p.Sq - 1)) * p.bias_strides[2];
   }
   if constexpr (BIAS == BIAS_ALIBI) slope2 = p.alibi_slopes[head] * LOG2E;
 
@@ -184,9 +195,9 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
   const uint32_t q_addr = smem_u32(sQ) + wg * (64 * 128);
   mbar_wait(q_full, 0);
 
-  for (int j = 0; j < nkv; ++j) {
-    const int b = j & 1;
-    const uint32_t par = (j >> 1) & 1;
+  for (int it = 0; it < nkv; ++it) {
+    const int j = j0 + it, b = it & 1;
+    const uint32_t par = (it >> 1) & 1;
     // ---- S = Q·K_jᵀ (64 x 128 per warpgroup)
     float s[ATT_BN / 2];
     mbar_wait(&k_full[b], par);
@@ -205,8 +216,8 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
     mbar_arrive(&k_empty[b]);
 
     // ---- scores in the log2 domain, masked
-    const int kbase = j * ATT_BN;
-    const bool need_mask = (p.causal && j == q_blk) || (kbase + ATT_BN > kv_len);
+    const int kbase = j * ATT_BN, krel = kbase - kv_beg;
+    const bool need_mask = kbase < kv_beg || kbase + ATT_BN > kv_len || (p.causal && kbase + ATT_BN - 1 > q0 + off);
 #pragma unroll
     for (int jj = 0; jj < ATT_BN / 8; ++jj) {
 #pragma unroll
@@ -217,13 +228,27 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
           float x = s[4 * jj + 2 * h + c] * p.scale_log2;
           if constexpr (BIAS == BIAS_DENSE) {
             const int kb = kbase + 8 * jj + cq;
-            const float2 f = kb < p.S ? unpack_bf16(*reinterpret_cast<const uint32_t*>(bias_row[h] + kb)) : make_float2(0.f, 0.f);
+            // a pair load never reads past the row's last key (Sk may be odd)
+            const float2 f = kb + 1 < p.Sk ? unpack_bf16(*reinterpret_cast<const uint32_t*>(bias_row[h] + kb))
+                             : make_float2(kb < p.Sk ? __bfloat162float(bias_row[h][kb]) : 0.f, 0.f);
             x = fmaf(c ? f.y : f.x, LOG2E, x);
           } else if constexpr (BIAS == BIAS_ALIBI) {
-            x = fmaf(slope2, static_cast<float>(kidx - q_idx[h]), x);
+            x = fmaf(slope2, static_cast<float>(kidx - q_idx[h] - off), x);
+            // (ALiBi keeps the test inline: the separate pass below costs the head-dim-128 dropout variant a spill)
+            if (need_mask && static_cast<unsigned>(krel + 8 * jj + cq + c) >= static_cast<unsigned>(vis_len[h])) x = -INFINITY;
           }
-          if (need_mask && kidx >= key_lim[h]) x = -INFINITY;
           s[4 * jj + 2 * h + c] = x;
+        }
+      }
+    }
+    if (BIAS != BIAS_ALIBI && need_mask) {   // uniform per tile: tiles inside every row's window skip the element test
+#pragma unroll
+      for (int jj = 0; jj < ATT_BN / 8; ++jj) {
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+#pragma unroll
+          for (int c = 0; c < 2; ++c)
+            if (static_cast<unsigned>(krel + 8 * jj + cq + c) >= static_cast<unsigned>(vis_len[h])) s[4 * jj + 2 * h + c] = -INFINITY;
         }
       }
     }
@@ -284,21 +309,21 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
     mbar_arrive(&v_empty[b]);
   }
 
-  // ---- epilogue: O / l  →  [B, S, A, D]; lse in natural log
+  // ---- epilogue: O / l  →  [B, Sq, A, D]; lse in natural log (0 for a row without a visible key)
 #pragma unroll
   for (int h = 0; h < 2; ++h) {
     float l = l_run[h];
     l += __shfl_xor_sync(0xffffffffu, l, 1);
     l += __shfl_xor_sync(0xffffffffu, l, 2);
     const float inv = l > 0.f ? (DROP ? p.inv_keep : 1.0f) / l : 0.f;
-    if (q_idx[h] < p.S) {
-      __nv_bfloat16* orow = p.o + ((static_cast<size_t>(batch) * p.S + q_idx[h]) * p.A + head) * D;
+    if (q_idx[h] < p.Sq) {
+      __nv_bfloat16* orow = p.o + ((static_cast<size_t>(batch) * p.Sq + q_idx[h]) * p.A + head) * D;
 #pragma unroll
       for (int jj = 0; jj < D / 8; ++jj)
         *reinterpret_cast<uint32_t*>(orow + 8 * jj + cq) = pack_bf16(o[4 * jj + 2 * h] * inv, o[4 * jj + 2 * h + 1] * inv);
       if (t % 4 == 0)
-        p.lse[(static_cast<size_t>(batch) * p.A + head) * p.S + q_idx[h]] =
-            (m_run[h] == -INFINITY) ? -INFINITY : (m_run[h] + log2f(l)) * 0.6931471805599453f;
+        p.lse[(static_cast<size_t>(batch) * p.A + head) * p.Sq + q_idx[h]] =
+            (m_run[h] == -INFINITY) ? 0.f : (m_run[h] + log2f(l)) * 0.6931471805599453f;
     }
   }
 }
@@ -333,7 +358,7 @@ cudaError_t launch_fwd_t(const CUtensorMap& tq, const CUtensorMap& tk, const CUt
     if (e != cudaSuccess) return e;
     configured = true;
   }
-  dim3 grid((p.S + lb::ATT_BM - 1) / lb::ATT_BM, p.A, p.B);
+  dim3 grid((p.Sq + lb::ATT_BM - 1) / lb::ATT_BM, p.A, p.B);
   kern<<<grid, lb::ATT_FWD_THREADS, Cfg::SMEM_BYTES, s>>>(tq, tk, tv, p);
   return cudaGetLastError();
 }
@@ -348,35 +373,39 @@ cudaError_t launch_fwd(const CUtensorMap& tq, const CUtensorMap& tk, const CUten
   return drop ? launch_fwd_t<D, lb::BIAS_ALIBI, true>(tq, tk, tv, p, s) : launch_fwd_t<D, lb::BIAS_ALIBI, false>(tq, tk, tv, p, s);
 }
 }  // namespace
-// A query heads in G groups (A % G == 0); q_strides = {batch, group, in-group, seq}, k/v_strides = {batch, head, seq}
-// over the G K/V heads (elements).
+// A query heads in G groups (A % G == 0); Sq queries, Sk keys; q_strides = {batch, group, in-group, seq}, k/v_strides =
+// {batch, head, seq} over the G K/V heads (elements).  kv_lens / kv_start (optional, int32 [B], device): per-sample key
+// window.
 // p_drop in [0, 1): attention dropout probability (quantised to 1/256 like the byte-threshold test of the kernel);
 // bias (optional, bf16): dense additive score bias with (batch, head, query-row) strides in elements, key stride 1;
 // alibi_slopes (optional, fp32 [A]).
-extern "C" int lb_attn_fwd(const void* q, const void* k, const void* v, void* o, float* lse, int B, int A, int G, int S,
-                           int D, const long* q_strides, const long* k_strides, const long* v_strides, int causal, float scale,
-                           const int* kv_lens, const void* bias, const long* bias_strides, const float* alibi_slopes,
-                           float p_drop, const lb::RngArgs* rng, long long* rng_out, cudaStream_t s) {
+extern "C" int lb_attn_fwd(const void* q, const void* k, const void* v, void* o, float* lse, int B, int A, int G, int Sq,
+                           int Sk, int D, const long* q_strides, const long* k_strides, const long* v_strides, int causal,
+                           float scale, const int* kv_lens, const int* kv_start, const void* bias, const long* bias_strides,
+                           const float* alibi_slopes, float p_drop, const lb::RngArgs* rng, long long* rng_out, cudaStream_t s) {
   if (D != 64 && D != 128) return -1;
+  if (Sq <= 0 || Sk <= 0) return -5;
   if (G <= 0 || A % G) return -4;
   for (int i = 0; i < 3; ++i)
     if ((q_strides[i] % 8) || (k_strides[i] % 8) || (v_strides[i] % 8)) return -3;
   if (q_strides[3] % 8) return -3;
   CUtensorMap tq, tk, tv;
-  if (!make_q_tmap(&tq, q, B, G, A / G, S, D, q_strides, 128)) return -2;
-  if (!make_qkv_tmap(&tk, k, B, G, S, D, k_strides, 128)) return -2;
-  if (!make_qkv_tmap(&tv, v, B, G, S, D, v_strides, 128)) return -2;
+  if (!make_q_tmap(&tq, q, B, G, A / G, Sq, D, q_strides, 128)) return -2;
+  if (!make_qkv_tmap(&tk, k, B, G, Sk, D, k_strides, 128)) return -2;
+  if (!make_qkv_tmap(&tv, v, B, G, Sk, D, v_strides, 128)) return -2;
   lb::AttnFwdParams p;
   p.o = reinterpret_cast<__nv_bfloat16*>(o);
   p.lse = lse;
   p.B = B;
   p.A = A;
   p.r = A / G;
-  p.S = S;
+  p.Sq = Sq;
+  p.Sk = Sk;
   p.causal = causal;
   p.scale = scale;
   p.scale_log2 = scale * 1.4426950408889634f;
   p.kv_lens = kv_lens;
+  p.kv_start = kv_start;
   p.bias = reinterpret_cast<const __nv_bfloat16*>(bias);
   for (int i = 0; i < 3; ++i) p.bias_strides[i] = (bias != nullptr && bias_strides != nullptr) ? bias_strides[i] : 0;
   if (bias != nullptr && ((p.bias_strides[0] | p.bias_strides[1] | p.bias_strides[2]) % 8 || (reinterpret_cast<uintptr_t>(bias) & 15)))
@@ -394,7 +423,10 @@ extern "C" int lb_attn_fwd(const void* q, const void* k, const void* v, void* o,
 }
 // =================================================================================================
 // Backward.  One CTA per (batch, K/V head, 64-key block); one consumer warpgroup loops over the r query heads of the
-// group and, for each, over the 64-query blocks that attend to it (warp 4 = TMA producer, Q / dO double buffered):
+// group and, for each, over the 64-query blocks that attend to it (warp 4 = TMA producer, Q / dO double buffered).
+// Which query blocks a key block visits depends on the shapes only (Sq, Sk, causal): under the causal mask query block
+// i and key block kb meet iff 64 kb <= 64 i + 63 + (Sk - Sq).  Keys outside a sample's kv_start / kv_lens window are
+// masked element-wise, so every visit happens and the dQ ordering below counts the same visits on both sides.
 //   Sᵀ = K·Q_iᵀ , dPᵀ = V·dO_iᵀ                  (wgmma, registers)
 //   Pᵀ = exp(Sᵀ·scale − lse) , dSᵀ = Pᵀ ∘ (dPᵀ − δ) · scale
 //   dV += Pᵀ·dO_i , dK += dSᵀ·Q_i                 (A operands straight from the registers, accumulators stay in
@@ -423,17 +455,18 @@ struct AttnBwdCfg {
 };
 
 struct AttnBwdParams {
-  const float* lse;     // [B, A, S]
-  const float* delta;   // [B, A, S]
-  float* dq_accum;      // [B, A, S, D] fp32
-  __nv_bfloat16* dk;    // strided [B, G, S, D] views
+  const float* lse;     // [B, A, Sq]
+  const float* delta;   // [B, A, Sq]
+  float* dq_accum;      // [B, A, Sq, D] fp32
+  __nv_bfloat16* dk;    // strided [B, G, Sk, D] views
   __nv_bfloat16* dv;
   long g_strides[3];    // batch, head, seq strides (elements) of dk / dv
-  int B, A, S;
+  int B, A, Sq, Sk;
   int r;                // query heads per K/V head (G = A / r)
   int causal;
   float scale, scale_log2;
   const int* kv_lens;   // optional [B]
+  const int* kv_start;  // optional [B]
   // same additive bias / dropout description as the forward; `rng_state` = the (seed, offset) pair the forward used
   const __nv_bfloat16* bias;
   long bias_strides[3];
@@ -467,9 +500,13 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
   const int kv_blk = static_cast<int>(gridDim.x) - 1 - static_cast<int>(blockIdx.x);
   const int kv_head = blockIdx.y, batch = blockIdx.z;
   const int k0 = kv_blk * ATT_BWD_BN;
-  const int kv_len = p.kv_lens != nullptr ? max(1, min(p.S, p.kv_lens[batch])) : p.S;
-  const int nq = (p.S + ATT_BWD_BM - 1) / ATT_BWD_BM;
-  const int i_begin = p.causal ? (k0 / ATT_BWD_BM) : 0;
+  const int kv_len = p.kv_lens != nullptr ? max(1, min(p.Sk, p.kv_lens[batch])) : p.Sk;
+  const int kv_beg = p.kv_start != nullptr ? min(max(p.kv_start[batch], 0), p.Sk) : 0;
+  const int off = p.Sk - p.Sq;
+  const int nq = (p.Sq + ATT_BWD_BM - 1) / ATT_BWD_BM;
+  // first query block whose last row (64 i + 63) sees key k0: floor((k0 - off) / 64), at least 0 (C division truncates
+  // a negative quotient towards 0, which the max turns into the same 0).  It is at most nq - 1, since k0 <= Sk - 1.
+  const int i_begin = p.causal ? max(0, (k0 - off) / ATT_BWD_BM) : 0;
   const int iters = nq - i_begin;   // query blocks per query head
   const int steps = p.r * iters;    // step = (query head in group) * iters + query block - i_begin
 
@@ -523,6 +560,11 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
   }
   const float inv_scale = 1.0f / p.scale;
   const uint32_t k_addr = smem_u32(sK), v_addr = smem_u32(sV), ds_addr = smem_u32(sDS);
+  // this thread's key rows are fixed for the CTA: a row before kv_start is never visible, which folds into the one
+  // comparison against key_lim per element (INT_MAX is never below it)
+  int kvis[2];
+#pragma unroll
+  for (int h = 0; h < 2; ++h) kvis[h] = k0 + r_loc + 8 * h >= kv_beg ? k0 + r_loc + 8 * h : INT_MAX;
 
   float dv[D / 2], dk[D / 2];
 #pragma unroll
@@ -570,10 +612,10 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
 #pragma unroll
       for (int c = 0; c < 2; ++c) {
         const int q_idx = q0 + 8 * jj + cq + c;
-        const bool q_ok = q_idx < p.S;
-        const float lse2 = q_ok ? p.lse[bh * p.S + q_idx] * LOG2E : 0.f;
-        const float delta_s = q_ok ? p.delta[bh * p.S + q_idx] * p.scale : 0.f;
-        const int key_lim = !q_ok ? 0 : (p.causal ? min(kv_len, q_idx + 1) : kv_len);
+        const bool q_ok = q_idx < p.Sq;
+        const float lse2 = q_ok ? p.lse[bh * p.Sq + q_idx] * LOG2E : 0.f;
+        const float delta_s = q_ok ? p.delta[bh * p.Sq + q_idx] * p.scale : 0.f;
+        const int key_lim = !q_ok ? 0 : (p.causal ? min(kv_len, q_idx + off + 1) : kv_len);
         uint4 rnd;
         if constexpr (DROP)   // both rows of this thread lie in the same 16-key group
           rnd = attn_dropout_bytes(static_cast<uint32_t>(q_idx), static_cast<uint32_t>((k0 + 16 * (t / 32)) >> 4),
@@ -585,12 +627,12 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
           float x = sT[i] * p.scale_log2;
           long boff = 0;
           if constexpr (BIAS == BIAS_DENSE) {
-            boff = bias_bh + static_cast<long>(min(q_idx, p.S - 1)) * p.bias_strides[2] + min(kidx, p.S - 1);
+            boff = bias_bh + static_cast<long>(min(q_idx, p.Sq - 1)) * p.bias_strides[2] + min(kidx, p.Sk - 1);
             x = fmaf(__bfloat162float(p.bias[boff]), LOG2E, x);
           } else if constexpr (BIAS == BIAS_ALIBI) {
-            x = fmaf(slope2, static_cast<float>(kidx - q_idx), x);
+            x = fmaf(slope2, static_cast<float>(kidx - q_idx - off), x);
           }
-          const float pv = kidx < key_lim ? fast_exp2(x - lse2) : 0.f;
+          const float pv = kvis[h] < key_lim ? fast_exp2(x - lse2) : 0.f;
           float g = dpT[i], pd = pv;   // dP w.r.t. the dropped, rescaled P; what multiplied V in the forward
           if constexpr (DROP) {
             const bool keep = rnd_byte(rnd, (r_loc + 8 * h) & 15) >= p.drop_thresh;
@@ -600,7 +642,7 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
           const float ds = pv * fmaf(g, p.scale, -delta_s);
           if constexpr (BIAS == BIAS_DENSE) {
             // d bias = P ∘ (dP − δ): fp32 reductions (broadcast dims sum over CTAs)
-            if (p.dbias != nullptr && q_ok && kidx < p.S) atomicAdd(p.dbias + boff, ds * inv_scale);
+            if (p.dbias != nullptr && q_ok && kidx < p.Sk) atomicAdd(p.dbias + boff, ds * inv_scale);
           }
           sT[i] = pd;
           dpT[i] = ds;
@@ -635,10 +677,12 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
       wgmma_bf16_rs<D, 1>(dk, da[kk], make_smem_desc_sw128(q_addr + kk * (16 * 128), 64 * 128, 1024), 1u);
     wgmma_commit();
     // ---- dQ_i is accumulated by the key blocks in decreasing order: wait until the key blocks above this one that
-    // contribute to query block i (all of them, or those up to i under the causal mask) have added theirs
+    // visit query block i (all of them, or under the causal mask kb <= (64 i + 63 + off) / 64, a non-negative quotient
+    // since this block visits i) have added theirs
     const int q_blk = i_begin + it;
     unsigned* order = p.dq_order + bh * nq + q_blk;
-    const int last_kb = p.causal ? q_blk : static_cast<int>(gridDim.x) - 1;
+    const int last_kb = p.causal ? min(static_cast<int>(gridDim.x) - 1, (q_blk * ATT_BWD_BM + ATT_BWD_BM - 1 + off) / ATT_BWD_BN)
+                                 : static_cast<int>(gridDim.x) - 1;
     if (t == 0) spin_wait_ge_sys(order, static_cast<uint32_t>(last_kb - kv_blk), 0, p.timeout_rec, /*what=*/5, kv_blk);
     warpgroup_sync(0);
     // ---- dQ_i = dS·K, 64 columns at a time: A = dSᵀ read transposed, B = the K tile read MN-major
@@ -657,8 +701,8 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
         const int q_idx = q0 + r_loc + 8 * h;
-        if (q_idx < p.S) {
-          float* dq_row = p.dq_accum + (bh * p.S + q_idx) * D + n * 64;
+        if (q_idx < p.Sq) {
+          float* dq_row = p.dq_accum + (bh * p.Sq + q_idx) * D + n * 64;
 #pragma unroll
           for (int jj = 0; jj < 8; ++jj)
             asm volatile("red.global.add.v2.f32 [%0], {%1, %2};\n" ::"l"(dq_row + 8 * jj + cq), "f"(dq[4 * jj + 2 * h]),
@@ -679,7 +723,7 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
 #pragma unroll
   for (int h = 0; h < 2; ++h) {
     const int k_idx = k0 + r_loc + 8 * h;
-    if (k_idx >= p.S) continue;
+    if (k_idx >= p.Sk) continue;
     const long off = batch * p.g_strides[0] + kv_head * p.g_strides[1] + static_cast<long>(k_idx) * p.g_strides[2];
 #pragma unroll
     for (int jj = 0; jj < D / 8; ++jj) {
@@ -789,7 +833,7 @@ cudaError_t launch_bwd_t(const CUtensorMap& tq, const CUtensorMap& tk, const CUt
     if (e != cudaSuccess) return e;
     configured = true;
   }
-  dim3 grid((p.S + lb::ATT_BWD_BN - 1) / lb::ATT_BWD_BN, p.A / p.r, p.B);
+  dim3 grid((p.Sk + lb::ATT_BWD_BN - 1) / lb::ATT_BWD_BN, p.A / p.r, p.B);
   kern<<<grid, lb::ATT_BWD_THREADS, Cfg::SMEM_BYTES, s>>>(tq, tk, tv, tdo, p);
   return cudaGetLastError();
 }
@@ -804,15 +848,18 @@ cudaError_t launch_bwd(const CUtensorMap& tq, const CUtensorMap& tk, const CUten
 }
 }  // namespace
 // A query heads in G groups; q_strides = {batch, group, in-group, seq}, k/v_strides = {batch, head, seq} over the G K/V
-// heads, do_strides = {batch, head, seq} over the A query heads.  dq, dk, dv point into one packed [B, S, G, r + 2, D]
-// gradient (slots 0 .. r - 1, r and r + 1 of each group).
+// heads, do_strides = {batch, head, seq} over the A query heads.  dq is written with dq_strides = {batch, group,
+// in-group, seq}, dk and dv with dkv_strides = {batch, head, seq} (for Sq == Sk the caller passes views of one packed
+// [B, S, G, r + 2, D] gradient).
 extern "C" int lb_attn_bwd(const void* dout, const void* q, const void* k, const void* v, const void* o,
-                           const float* lse, void* dq, void* dk, void* dv, float* delta, float* dq_accum, int B, int A,
-                           int G, int S, int D, const long* q_strides, const long* k_strides, const long* v_strides,
-                           const long* do_strides, int causal, float scale, const int* kv_lens, const void* bias,
-                           const long* bias_strides, const float* alibi_slopes, float* dbias, float p_drop,
-                           const long long* rng_state, unsigned* dq_order, cudaStream_t s) {
+                           const float* lse, void* dq, void* dk, void* dv, const long* dq_strides, const long* dkv_strides,
+                           float* delta, float* dq_accum, int B, int A, int G, int Sq, int Sk, int D, const long* q_strides,
+                           const long* k_strides, const long* v_strides, const long* do_strides, int causal, float scale,
+                           const int* kv_lens, const int* kv_start, const void* bias, const long* bias_strides,
+                           const float* alibi_slopes, float* dbias, float p_drop, const long long* rng_state,
+                           unsigned* dq_order, cudaStream_t s) {
   if (D != 64 && D != 128) return -1;
+  if (Sq <= 0 || Sk <= 0) return -5;
   if (G <= 0 || A % G) return -4;
   const int r = A / G;
   for (int i = 0; i < 3; ++i)
@@ -820,11 +867,11 @@ extern "C" int lb_attn_bwd(const void* dout, const void* q, const void* k, const
   if (q_strides[3] % 8) return -3;
   const long do_strides4[4] = {do_strides[0], r * do_strides[1], do_strides[1], do_strides[2]};
   CUtensorMap tq, tk, tv, tdo;
-  if (!make_q_tmap(&tq, q, B, G, r, S, D, q_strides, 64)) return -2;
-  if (!make_qkv_tmap(&tk, k, B, G, S, D, k_strides, 64)) return -2;
-  if (!make_qkv_tmap(&tv, v, B, G, S, D, v_strides, 64)) return -2;
-  if (!make_q_tmap(&tdo, dout, B, G, r, S, D, do_strides4, 64)) return -2;
-  const long rows = (long)B * A * S;
+  if (!make_q_tmap(&tq, q, B, G, r, Sq, D, q_strides, 64)) return -2;
+  if (!make_qkv_tmap(&tk, k, B, G, Sk, D, k_strides, 64)) return -2;
+  if (!make_qkv_tmap(&tv, v, B, G, Sk, D, v_strides, 64)) return -2;
+  if (!make_q_tmap(&tdo, dout, B, G, r, Sq, D, do_strides4, 64)) return -2;
+  const long rows = (long)B * A * Sq;
   {
     // 4 rows per thread-group and iteration; cap the grid at a few waves
     const long groups = (rows + 3) / 4;
@@ -833,11 +880,11 @@ extern "C" int lb_attn_bwd(const void* dout, const void* q, const void* k, const
     if (blocks > sm_count() * 16L) blocks = sm_count() * 16L;
     if (D == 64)
       lb::attn_delta_kernel<64><<<(unsigned)blocks, 256, 0, s>>>((const __nv_bfloat16*)dout, (const __nv_bfloat16*)o, delta, B,
-                                                                   A, S, do_strides[0], do_strides[1], do_strides[2],
+                                                                   A, Sq, do_strides[0], do_strides[1], do_strides[2],
                                                                    reinterpret_cast<float4*>(dq_accum), rows * D / 4);
     else
       lb::attn_delta_kernel<128><<<(unsigned)blocks, 256, 0, s>>>((const __nv_bfloat16*)dout, (const __nv_bfloat16*)o, delta, B,
-                                                                    A, S, do_strides[0], do_strides[1], do_strides[2],
+                                                                    A, Sq, do_strides[0], do_strides[1], do_strides[2],
                                                                     reinterpret_cast<float4*>(dq_accum), rows * D / 4);
   }
   lb::AttnBwdParams p;
@@ -846,18 +893,17 @@ extern "C" int lb_attn_bwd(const void* dout, const void* q, const void* k, const
   p.dq_accum = dq_accum;
   p.dk = (__nv_bfloat16*)dk;
   p.dv = (__nv_bfloat16*)dv;
-  // dq / dk / dv are views of one packed [B, S, G, r + 2, D] tensor
-  p.g_strides[0] = (long)S * G * (r + 2) * D;
-  p.g_strides[1] = (long)(r + 2) * D;
-  p.g_strides[2] = (long)G * (r + 2) * D;
+  for (int i = 0; i < 3; ++i) p.g_strides[i] = dkv_strides[i];
   p.B = B;
   p.A = A;
   p.r = r;
-  p.S = S;
+  p.Sq = Sq;
+  p.Sk = Sk;
   p.causal = causal;
   p.scale = scale;
   p.scale_log2 = scale * 1.4426950408889634f;
   p.kv_lens = kv_lens;
+  p.kv_start = kv_start;
   p.bias = reinterpret_cast<const __nv_bfloat16*>(bias);
   for (int i = 0; i < 3; ++i) p.bias_strides[i] = (bias != nullptr && bias_strides != nullptr) ? bias_strides[i] : 0;
   p.alibi_slopes = bias != nullptr ? nullptr : alibi_slopes;
@@ -874,7 +920,7 @@ extern "C" int lb_attn_bwd(const void* dout, const void* q, const void* k, const
   const long nvec = rows * D / 8;
   int blocks = (int)((nvec + 511) / 512);
   if (blocks > sm_count() * 8) blocks = sm_count() * 8;
-  lb::attn_dq_convert_kernel<<<blocks, 256, 0, s>>>(dq_accum, (__nv_bfloat16*)dq, B, A, S, D, r, p.g_strides[0],
-                                                    p.g_strides[1], (long)D, p.g_strides[2]);
+  lb::attn_dq_convert_kernel<<<blocks, 256, 0, s>>>(dq_accum, (__nv_bfloat16*)dq, B, A, Sq, D, r, dq_strides[0],
+                                                    dq_strides[1], dq_strides[2], dq_strides[3]);
   return (int)cudaGetLastError();
 }

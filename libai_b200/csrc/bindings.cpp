@@ -76,15 +76,16 @@ struct LbRngArgs {
   int captured;
   unsigned long long salt;
 };
-int lb_attn_fwd(const void* q, const void* k, const void* v, void* o, float* lse, int B, int A, int G, int S, int D,
-                const long* q_strides, const long* k_strides, const long* v_strides, int causal, float scale,
-                const int* kv_lens, const void* bias, const long* bias_strides, const float* alibi_slopes, float p_drop,
-                const LbRngArgs* rng, long long* rng_out, cudaStream_t s);
+int lb_attn_fwd(const void* q, const void* k, const void* v, void* o, float* lse, int B, int A, int G, int Sq, int Sk,
+                int D, const long* q_strides, const long* k_strides, const long* v_strides, int causal, float scale,
+                const int* kv_lens, const int* kv_start, const void* bias, const long* bias_strides,
+                const float* alibi_slopes, float p_drop, const LbRngArgs* rng, long long* rng_out, cudaStream_t s);
 int lb_attn_bwd(const void* dout, const void* q, const void* k, const void* v, const void* o, const float* lse,
-                void* dq, void* dk, void* dv, float* delta, float* dq_accum, int B, int A, int G, int S, int D,
-                const long* q_strides, const long* k_strides, const long* v_strides, const long* do_strides, int causal,
-                float scale, const int* kv_lens, const void* bias, const long* bias_strides, const float* alibi_slopes,
-                float* dbias, float p_drop, const long long* rng_state, unsigned* dq_order, cudaStream_t s);
+                void* dq, void* dk, void* dv, const long* dq_strides, const long* dkv_strides, float* delta,
+                float* dq_accum, int B, int A, int G, int Sq, int Sk, int D, const long* q_strides, const long* k_strides,
+                const long* v_strides, const long* do_strides, int causal, float scale, const int* kv_lens,
+                const int* kv_start, const void* bias, const long* bias_strides, const float* alibi_slopes, float* dbias,
+                float p_drop, const long long* rng_state, unsigned* dq_order, cudaStream_t s);
 int lb_bias_dropout_residual(const void* x, const void* bias, const void* res, void* y, long rows, int N, float p,
                              const LbRngArgs* rng, const long long* rng_in, long long* rng_out, cudaStream_t s);
 int lb_spin_timeout_report(char* buf, int n);
@@ -619,20 +620,21 @@ std::tuple<Tensor, Tensor> bias_dropout_residual(const Tensor& x, const c10::opt
 }
 
 // ---- attention ----------------------------------------------------------------------------------------------
-// q: [B, A, S, D] or, grouped, [B, G, r, S, D]; k, v: [B, G, S, D] with A = G * r (grouped-query attention: query head
-// h reads K/V head h / r); views with arbitrary batch/head/seq strides (D contiguous).  Output o is allocated as
-// [B, S, A, D] and returned as the [B, A, S, D] view, lse fp32 [B, A, S].
+// q: [B, A, Sq, D] or, grouped, [B, G, r, Sq, D]; k, v: [B, G, Sk, D] with A = G * r (grouped-query attention: query
+// head h reads K/V head h / r); views with arbitrary batch/head/seq strides (D contiguous).  Output o is allocated as
+// [B, Sq, A, D] and returned as the [B, A, Sq, D] view, lse fp32 [B, A, Sq].  Key j is visible to query i of sample b
+// iff kv_start[b] <= j < kv_lens[b] (defaults 0 and Sk) and, when causal, j <= i + Sk - Sq.
 struct BiasDesc {
   const void* ptr = nullptr;
   long strides[3] = {0, 0, 0};
 };
-// bias [Bb, Ab, S, S] (Bb in {1, B}, Ab in {1, A}), bf16, key dimension contiguous; broadcast dims get stride 0
-BiasDesc bias_desc(const c10::optional<Tensor>& bias, int B, int A, int S) {
+// bias [Bb, Ab, Sq, Sk] (Bb in {1, B}, Ab in {1, A}), bf16, key dimension contiguous; broadcast dims get stride 0
+BiasDesc bias_desc(const c10::optional<Tensor>& bias, int B, int A, int Sq, int Sk) {
   BiasDesc d;
   if (!(bias.has_value() && bias->defined())) return d;
   const Tensor& b = *bias;
-  TORCH_CHECK(b.dim() == 4 && b.scalar_type() == at::kBFloat16 && b.stride(3) == 1 && b.size(2) == S && b.size(3) == S,
-              "attention bias: bf16 [B|1, A|1, S, S] with contiguous keys");
+  TORCH_CHECK(b.dim() == 4 && b.scalar_type() == at::kBFloat16 && b.stride(3) == 1 && b.size(2) == Sq && b.size(3) == Sk,
+              "attention bias: bf16 [B|1, A|1, Sq, Sk] with contiguous keys");
   TORCH_CHECK((b.size(0) == 1 || b.size(0) == B) && (b.size(1) == 1 || b.size(1) == A), "attention bias: bad broadcast shape");
   d.ptr = b.data_ptr();
   d.strides[0] = b.size(0) == 1 ? 0 : b.stride(0);
@@ -641,10 +643,10 @@ BiasDesc bias_desc(const c10::optional<Tensor>& bias, int B, int A, int S) {
   return d;
 }
 
-// shapes of an attention call: q [B, A, S, D] / [B, G, r, S, D] against k, v [B, G, S, D]; qs = q's {batch, group,
+// shapes of an attention call: q [B, A, Sq, D] / [B, G, r, Sq, D] against k, v [B, G, Sk, D]; qs = q's {batch, group,
 // in-group, seq} strides
 struct QGeom {
-  int B, A, G, S, D;
+  int B, A, G, Sq, Sk, D;
   long qs[4];
 };
 QGeom q_geom(const Tensor& q, const Tensor& k, const Tensor& v, const char* what) {
@@ -654,7 +656,8 @@ QGeom q_geom(const Tensor& q, const Tensor& k, const Tensor& v, const char* what
   QGeom g;
   g.B = (int)q.size(0);
   g.G = (int)k.size(1);
-  g.S = (int)q.size(-2);
+  g.Sq = (int)q.size(-2);
+  g.Sk = (int)k.size(2);
   g.D = (int)q.size(-1);
   if (q.dim() == 4) {
     g.A = (int)q.size(1);
@@ -672,28 +675,37 @@ QGeom q_geom(const Tensor& q, const Tensor& k, const Tensor& v, const char* what
     g.qs[2] = q.stride(2);
     g.qs[3] = q.stride(3);
   }
-  TORCH_CHECK(k.size(0) == g.B && k.size(2) == g.S && k.size(3) == g.D, what, ": k, v do not match q");
+  TORCH_CHECK(k.size(0) == g.B && k.size(3) == g.D, what, ": k, v do not match q");
+  TORCH_CHECK(g.Sq >= 1 && g.Sk >= 1, what, ": empty query or key sequence");
   return g;
+}
+
+// optional per-sample key bound (kv_lens: end, kv_start: start of the visible keys) → device pointer or nullptr
+const int* key_bound(const c10::optional<Tensor>& t, const Tensor& q, int B, const char* what) {
+  if (!(t.has_value() && t->defined())) return nullptr;
+  TORCH_CHECK(t->scalar_type() == at::kInt, what, ": int32 expected, got ", t->scalar_type());
+  TORCH_CHECK(t->numel() == B, what, ": ", B, " elements (one per sample) expected, got shape ", t->sizes());
+  TORCH_CHECK(t->is_cuda() && t->device() == q.device(), what, ": must be on ", q.device(), ", got ", t->device());
+  TORCH_CHECK(t->is_contiguous(), what, ": must be contiguous");
+  return t->data_ptr<int>();
 }
 
 // returns (o, lse, rng_state): rng_state int64[2] = (seed, offset) of the dropout mask (empty without dropout)
 std::tuple<Tensor, Tensor, Tensor> attn_fwd(const Tensor& q, const Tensor& k, const Tensor& v, bool causal, double scale,
                                             const c10::optional<Tensor>& kv_lens, const c10::optional<Tensor>& bias,
-                                            const c10::optional<Tensor>& alibi_slopes, double p_drop, int64_t salt) {
+                                            const c10::optional<Tensor>& alibi_slopes, double p_drop, int64_t salt,
+                                            const c10::optional<Tensor>& kv_start) {
   c10::cuda::CUDAGuard guard(q.device());
   const QGeom g = q_geom(q, k, v, "attn_fwd");
-  const int B = g.B, A = g.A, S = g.S, D = g.D;
-  Tensor o = at::empty({B, S, A, D}, q.options());
-  Tensor lse = at::empty({B, A, S}, q.options().dtype(at::kFloat));
+  const int B = g.B, A = g.A, Sq = g.Sq, Sk = g.Sk, D = g.D;
+  Tensor o = at::empty({B, Sq, A, D}, q.options());
+  Tensor lse = at::empty({B, A, Sq}, q.options().dtype(at::kFloat));
   const long* qs = g.qs;
   long ks[3] = {k.stride(0), k.stride(1), k.stride(2)};
   long vs[3] = {v.stride(0), v.stride(1), v.stride(2)};
-  const int* kvl = nullptr;
-  if (kv_lens.has_value() && kv_lens->defined()) {
-    TORCH_CHECK(kv_lens->scalar_type() == at::kInt && kv_lens->numel() == B && kv_lens->is_cuda(), "kv_lens: int32 cuda [B]");
-    kvl = kv_lens->data_ptr<int>();
-  }
-  BiasDesc bd = bias_desc(bias, B, A, S);
+  const int* kvl = key_bound(kv_lens, q, B, "attn_fwd: kv_lens");
+  const int* kvs = key_bound(kv_start, q, B, "attn_fwd: kv_start");
+  BiasDesc bd = bias_desc(bias, B, A, Sq, Sk);
   const float* slopes = nullptr;
   if (alibi_slopes.has_value() && alibi_slopes->defined()) {
     TORCH_CHECK(alibi_slopes->scalar_type() == at::kFloat && alibi_slopes->numel() == A && alibi_slopes->is_cuda(), "alibi_slopes: fp32 cuda [A]");
@@ -709,8 +721,9 @@ std::tuple<Tensor, Tensor, Tensor> attn_fwd(const Tensor& q, const Tensor& k, co
   } else {
     rng_state = at::empty({0}, q.options().dtype(at::kLong));
   }
-  check(lb_attn_fwd(q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(), lse.data_ptr<float>(), B, A, g.G, S, D, qs, ks,
-                    vs, causal ? 1 : 0, (float)scale, kvl, bd.ptr, bd.strides, slopes, (float)p_drop, drop ? &a : nullptr,
+  check(lb_attn_fwd(q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(), lse.data_ptr<float>(), B, A, g.G, Sq, Sk, D, qs,
+                    ks, vs, causal ? 1 : 0, (float)scale, kvl, kvs, bd.ptr, bd.strides, slopes, (float)p_drop,
+                    drop ? &a : nullptr,
                     drop ? reinterpret_cast<long long*>(rng_state.data_ptr<int64_t>()) : nullptr, cur_stream()),
         "attn_fwd");
   return std::make_tuple(o.permute({0, 2, 1, 3}), lse, rng_state);
@@ -806,20 +819,33 @@ std::tuple<Tensor, Tensor, Tensor, Tensor> attn_bwd(const Tensor& dout, const Te
                                             const Tensor& o, const Tensor& lse, bool causal, double scale,
                                             const c10::optional<Tensor>& kv_lens, const c10::optional<Tensor>& bias,
                                             const c10::optional<Tensor>& alibi_slopes, c10::optional<Tensor> dbias,
-                                            double p_drop, const c10::optional<Tensor>& rng_state) {
+                                            double p_drop, const c10::optional<Tensor>& rng_state,
+                                            const c10::optional<Tensor>& kv_start) {
   c10::cuda::CUDAGuard guard(q.device());
   const QGeom g = q_geom(q, k, v, "attn_bwd");
-  const int B = g.B, A = g.A, G = g.G, S = g.S, D = g.D, r = A / G;
-  // gradients are produced in the packed [B, S, G, r + 2, D] layout (r = 1: [B, S, A, 3, D]) so that the QKV
-  // dgrad/wgrad GEMMs read them directly; dq comes back in q's shape (a copy only for a 4-D q with r > 1)
-  Tensor dqkv = at::empty({B, S, G, r + 2, D}, q.options());
-  Tensor dq5 = dqkv.narrow(3, 0, r).permute({0, 2, 3, 1, 4});
-  Tensor dk = dqkv.select(3, r).permute({0, 2, 1, 3});
-  Tensor dv = dqkv.select(3, r + 1).permute({0, 2, 1, 3});
-  Tensor delta = at::empty({B, A, S}, q.options().dtype(at::kFloat));
-  Tensor dq_acc = at::empty({B, A, S, D}, q.options().dtype(at::kFloat));   // cleared by the delta kernel
+  const int B = g.B, A = g.A, G = g.G, Sq = g.Sq, Sk = g.Sk, D = g.D, r = A / G;
+  // Sq == Sk: gradients are produced in the packed [B, S, G, r + 2, D] layout (r = 1: [B, S, A, 3, D]) so that the QKV
+  // dgrad/wgrad GEMMs read them directly; dq comes back in q's shape (a copy only for a 4-D q with r > 1).
+  // Sq != Sk: dq is [B, Sq, G, r, D] and dk, dv are packed as [B, Sk, G, 2, D]; the returned dqkv is empty.
+  Tensor dqkv, dq5, dk, dv;
+  if (Sq == Sk) {
+    dqkv = at::empty({B, Sq, G, r + 2, D}, q.options());
+    dq5 = dqkv.narrow(3, 0, r).permute({0, 2, 3, 1, 4});
+    dk = dqkv.select(3, r).permute({0, 2, 1, 3});
+    dv = dqkv.select(3, r + 1).permute({0, 2, 1, 3});
+  } else {
+    dqkv = at::empty({0}, q.options());
+    dq5 = at::empty({B, Sq, G, r, D}, q.options()).permute({0, 2, 3, 1, 4});
+    Tensor dkv = at::empty({B, Sk, G, 2, D}, q.options());
+    dk = dkv.select(3, 0).permute({0, 2, 1, 3});
+    dv = dkv.select(3, 1).permute({0, 2, 1, 3});
+  }
+  const long dqs[4] = {dq5.stride(0), dq5.stride(1), dq5.stride(2), dq5.stride(3)};
+  const long dkvs[3] = {dk.stride(0), dk.stride(1), dk.stride(2)};
+  Tensor delta = at::empty({B, A, Sq}, q.options().dtype(at::kFloat));
+  Tensor dq_acc = at::empty({B, A, Sq, D}, q.options().dtype(at::kFloat));   // cleared by the delta kernel
   // per (batch, head, 64-query block): key blocks that have added their dQ contribution
-  Tensor dq_order = at::zeros({B * A * ((S + 63) / 64)}, q.options().dtype(at::kInt));
+  Tensor dq_order = at::zeros({B * A * ((Sq + 63) / 64)}, q.options().dtype(at::kInt));
   TORCH_CHECK(o.stride(3) == 1, "attn_bwd: o must have contiguous D");
   Tensor dout_c = dout;
   if (dout.strides() != o.strides()) {  // bring dout into the [B, S, A, D]-backed layout of o
@@ -830,7 +856,9 @@ std::tuple<Tensor, Tensor, Tensor, Tensor> attn_bwd(const Tensor& dout, const Te
   long ks[3] = {k.stride(0), k.stride(1), k.stride(2)};
   long vs[3] = {v.stride(0), v.stride(1), v.stride(2)};
   long ds[3] = {dout_c.stride(0), dout_c.stride(1), dout_c.stride(2)};
-  BiasDesc bd = bias_desc(bias, B, A, S);
+  BiasDesc bd = bias_desc(bias, B, A, Sq, Sk);
+  const int* kvl = key_bound(kv_lens, q, B, "attn_bwd: kv_lens");
+  const int* kvs = key_bound(kv_start, q, B, "attn_bwd: kv_start");
   float* dbp = nullptr;
   if (dbias.has_value() && dbias->defined()) {
     TORCH_CHECK(bd.ptr != nullptr && dbias->scalar_type() == at::kFloat && dbias->sizes() == bias->sizes() &&
@@ -839,15 +867,15 @@ std::tuple<Tensor, Tensor, Tensor, Tensor> attn_bwd(const Tensor& dout, const Te
   }
   const bool has_rng = p_drop > 0.0 && rng_state.has_value() && rng_state->defined() && rng_state->numel() == 2;
   check(lb_attn_bwd(dout_c.data_ptr(), q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(), lse.data_ptr<float>(),
-                    dq5.data_ptr(), dk.data_ptr(), dv.data_ptr(), delta.data_ptr<float>(), dq_acc.data_ptr<float>(), B, A,
-                    G, S, D, qs, ks, vs, ds, causal ? 1 : 0, (float)scale,
-                    (kv_lens.has_value() && kv_lens->defined()) ? kv_lens->data_ptr<int>() : nullptr, bd.ptr, bd.strides,
+                    dq5.data_ptr(), dk.data_ptr(), dv.data_ptr(), dqs, dkvs, delta.data_ptr<float>(),
+                    dq_acc.data_ptr<float>(), B, A, G, Sq, Sk, D, qs, ks, vs, ds, causal ? 1 : 0, (float)scale, kvl, kvs,
+                    bd.ptr, bd.strides,
                     (alibi_slopes.has_value() && alibi_slopes->defined()) ? alibi_slopes->data_ptr<float>() : nullptr, dbp,
                     (float)(has_rng ? p_drop : 0.0),
                     has_rng ? reinterpret_cast<const long long*>(rng_state->data_ptr<int64_t>()) : nullptr,
                     reinterpret_cast<unsigned*>(dq_order.data_ptr<int>()), cur_stream()),
         "attn_bwd");
-  Tensor dq = q.dim() == 5 ? dq5 : dq5.reshape({B, A, S, D});   // after the kernel: for r > 1 this copies
+  Tensor dq = q.dim() == 5 ? dq5 : dq5.reshape({B, A, Sq, D});   // after the kernel: for r > 1 this copies
   return std::make_tuple(dq, dk, dv, dqkv);
 }
 
@@ -997,8 +1025,8 @@ TORCH_LIBRARY(libai_b200, m) {
   m.def("ce_bwd(Tensor(a!) logits, Tensor labels, Tensor lse, Tensor gloss, int vocab_start) -> Tensor(a!)", &ce_bwd);
   m.def("fused_adamw(Tensor(a!) master, Tensor grad, Tensor(b!) m, Tensor(c!) v, Tensor? lp_out, Tensor scale, float lr, float b1, float b2, float eps, float wd, float bc1, float bc2, bool decoupled) -> ()", &fused_adamw);
   m.def("sqnorm(Tensor x) -> Tensor", &sqnorm);
-  m.def("attn_fwd(Tensor q, Tensor k, Tensor v, bool causal, float scale, Tensor? kv_lens, Tensor? bias=None, Tensor? alibi_slopes=None, float p_drop=0.0, int salt=0) -> (Tensor, Tensor, Tensor)", &attn_fwd);
-  m.def("attn_bwd(Tensor dout, Tensor q, Tensor k, Tensor v, Tensor o, Tensor lse, bool causal, float scale, Tensor? kv_lens, Tensor? bias=None, Tensor? alibi_slopes=None, Tensor(a!)? dbias=None, float p_drop=0.0, Tensor? rng_state=None) -> (Tensor, Tensor, Tensor, Tensor)", &attn_bwd);
+  m.def("attn_fwd(Tensor q, Tensor k, Tensor v, bool causal, float scale, Tensor? kv_lens, Tensor? bias=None, Tensor? alibi_slopes=None, float p_drop=0.0, int salt=0, Tensor? kv_start=None) -> (Tensor, Tensor, Tensor)", &attn_fwd);
+  m.def("attn_bwd(Tensor dout, Tensor q, Tensor k, Tensor v, Tensor o, Tensor lse, bool causal, float scale, Tensor? kv_lens, Tensor? bias=None, Tensor? alibi_slopes=None, Tensor(a!)? dbias=None, float p_drop=0.0, Tensor? rng_state=None, Tensor? kv_start=None) -> (Tensor, Tensor, Tensor, Tensor)", &attn_bwd);
   m.def("kv_append(Tensor qkv, Tensor(a!) k_cache, Tensor(b!) v_cache, Tensor cache_seqlens, Tensor? cos, Tensor? sin, bool write_q) -> Tensor", &kv_append);
   m.def("decode_attn(Tensor q, Tensor k_cache, Tensor v_cache, Tensor cache_seqlens, Tensor kv_start, float scale, int splits=0) -> Tensor", &decode_attn);
   m.def("bias_dropout_residual(Tensor x, Tensor? bias, Tensor? res, float p, int salt, Tensor? rng_state=None) -> (Tensor, Tensor)", &bias_dropout_residual);

@@ -199,8 +199,12 @@ class MultiheadAttention(nn.Module):
         if use_cache:
             past_key_value = (key, value)
 
+        key_lens = None
         if isinstance(attention_mask, KeyPaddingMask):
-            attention_mask = attention_mask.dense()
+            if self.is_cross_attention and attention_mask.is_prefix() and OF.attention_supported(query, key):
+                key_lens, attention_mask = attention_mask.lengths, None   # right-padded encoder keys, in the kernel
+            else:
+                attention_mask = attention_mask.dense()
         causal = (
             self.attn_mask_type == AttnMaskType.causal
             and attention_mask is None
@@ -213,6 +217,7 @@ class MultiheadAttention(nn.Module):
             mask=attention_mask,
             dropout_p=self.attention_dropout_prob,
             training=self.training,
+            kv_lens=key_lens,
         )  # [b, a, s, d]
         context = context.transpose(1, 2).reshape(bsz, -1, a * d)
         if sp and hidden_states.dim() == 2:
@@ -225,14 +230,16 @@ class MultiheadAttention(nn.Module):
 
     def _cached_attention(self, qkv, attention_mask, cache):
         """Self-attention with a :class:`KVCacheLayer`: append k, v in place, then :func:`OF.decode_attention` for the
-        steps after the prefill (split-KV kernel for bf16 with head dim 64 / 128 and up to 16 new tokens) or the usual
-        dispatch on views of the cache → ``[b, s, a, d]``."""
+        steps after the prefill (split-KV kernel for bf16 with head dim 64 / 128 and up to 16 new tokens, the causal
+        flash kernel over the cache window for longer continuations) or the usual dispatch on views of the cache →
+        ``[b, s, a, d]``."""
         d = self.head_size
         past, s_len = cache.length, qkv.shape[1]
         OF.kv_cache_append(qkv, cache.k, cache.v, cache.seqlens, return_q=False)
         q = qkv[..., :d]
         if past > 0 and attention_mask is None and self.attn_mask_type == AttnMaskType.causal:
-            return OF.decode_attention(q, cache.k, cache.v, cache.seqlens, cache.kv_start, scale=self.softmax_scale)
+            return OF.decode_attention(q, cache.k, cache.v, cache.seqlens, cache.kv_start, scale=self.softmax_scale,
+                                       past=past)
         if isinstance(attention_mask, KeyPaddingMask):
             attention_mask = attention_mask.dense()
         L = past + s_len

@@ -182,17 +182,21 @@ class LlamaAttention(nn.Module):
     def _cached_attention(self, qkv, attention_mask, cache, cos, sin):
         """Rotary + append into the layer's cache, then attention over it → ``[b, s, a, d]``.  Steps after the prefill
         (padding carried by ``cache.kv_start``) go to :func:`OF.decode_attention`: the split-KV kernel for bf16 with head
-        dim 64 / 128 and up to 16 new tokens, the reference math otherwise.  The prefill runs the usual dispatch (flash
-        kernel for a causal prompt) on views of the cache, and a dense ``attention_mask`` keeps the reference math."""
+        dim 64 / 128 and up to 16 new tokens, the causal flash kernel over the cache window for longer continuations,
+        the reference math otherwise.  The prefill runs the usual dispatch on views of the cache: the flash kernel for
+        a causal prompt, left padding included (``cache.kv_start``), and the reference math for a dense
+        ``attention_mask``."""
         past, s_len = cache.length, qkv.shape[1]
         q = OF.kv_cache_append(qkv, cache.k, cache.v, cache.seqlens, cos, sin)
         if past > 0 and attention_mask is None:
-            return OF.decode_attention(q, cache.k, cache.v, cache.seqlens, cache.kv_start, scale=self.norm_factor)
+            return OF.decode_attention(q, cache.k, cache.v, cache.seqlens, cache.kv_start, scale=self.norm_factor,
+                                       past=past)
         L = past + s_len
-        key, value = cache.k[:, :, :L], cache.v[:, :, :L]
-        causal = attention_mask is None   # prefill of an unpadded prompt
-        context = OF.attention(q.permute(0, 2, 1, 3), key, value, causal=causal, scale=self.norm_factor,
-                               mask=attention_mask)
+        query, key, value = q.permute(0, 2, 1, 3), cache.k[:, :, :L], cache.v[:, :, :L]
+        causal = attention_mask is None   # prefill of an unpadded or left-padded prompt
+        kv_start = cache.kv_start if causal and OF.attention_supported(query, key) else None
+        context = OF.attention(query, key, value, causal=causal, scale=self.norm_factor, mask=attention_mask,
+                               kv_start=kv_start)
         return context.transpose(1, 2)
 
 
@@ -418,8 +422,10 @@ class LlamaForCausalLM(nn.Module, PipelineStageMixin, Generator, KVCacheOwner):
                     cache.dense_mask = kv_start is None
                     if kv_start is not None:
                         cache.kv_start.copy_(kv_start)
-                if past == 0 or cache.dense_mask:
-                    # the prefill of a padded prompt (and every step of a mask kv_start cannot express) is dense
+                # the flash kernel reads a left-padded prompt's padding from cache.kv_start; the reference math and
+                # every step of a mask kv_start cannot express take the dense mask
+                c_k = cache.k[cache.owned[0]]
+                if cache.dense_mask or (past == 0 and not OF.attention_supported(c_k, c_k)):
                     mask = self.casual_mask(input_ids, past_length=past, attention_mask=attention_mask)
             output = self.model(input_ids, attention_mask=mask, past_key_values=cache)
             self.past_length = cache.length

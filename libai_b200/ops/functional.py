@@ -576,8 +576,25 @@ def attention_ref(q, k, v, *, causal: bool, scale: float, mask=None, bias=None, 
     return torch.matmul(probs, v.float()).to(q.dtype)
 
 
+def visible_keys(sq: int, sk: int, *, causal: bool, kv_start=None, kv_lens=None, device=None):
+    """Boolean ``[b|1, 1, sq, sk]`` visibility of the flash kernels: key ``j`` is visible to query ``i`` of sample ``b``
+    iff ``kv_start[b] <= j < max(1, kv_lens[b])`` (defaults ``0`` and ``sk``) and, when ``causal``,
+    ``j <= i + sk - sq`` (bottom-right alignment)."""
+    j = torch.arange(sk, device=device)
+    vis = torch.ones(1, sq, sk, dtype=torch.bool, device=device)
+    if causal:
+        vis = vis & (j[None, :] <= torch.arange(sq, device=device)[:, None] + (sk - sq))[None]
+    if kv_start is not None:
+        vis = vis & (j[None, None, :] >= kv_start.to(device=device, dtype=torch.long)[:, None, None])
+    if kv_lens is not None:
+        end = kv_lens.to(device=device, dtype=torch.long).clamp(min=1)
+        vis = vis & (j[None, None, :] < end[:, None, None])
+    return vis[:, None]
+
+
 def _prep_bias(bias, q):
-    """Additive score bias for the flash kernel: bf16 ``[B|1, A|1, S, S]`` with contiguous keys."""
+    """Additive score bias for the flash kernel: bf16 ``[B|1, A|1, Sq, Sk]`` with contiguous keys and rows whose stride
+    is a multiple of 8 elements (a key length that is not gets its rows padded)."""
     if bias is None:
         return None
     b = bias
@@ -586,22 +603,29 @@ def _prep_bias(bias, q):
     if b.dtype != torch.bfloat16:
         b = b.to(torch.bfloat16)
     if b.stride(-1) != 1 or b.stride(-2) % 8 or b.stride(0) % 8 or b.stride(1) % 8 or b.data_ptr() % 16:
-        b = b.contiguous()
+        sk = b.shape[-1]
+        if sk % 8 == 0:
+            b = b.contiguous()
+        else:
+            padded = b.new_zeros(*b.shape[:-1], sk + (-sk % 8))
+            padded[..., :sk] = b
+            b = padded[..., :sk]
     return b
 
 
 class _FlashAttnFn(torch.autograd.Function):
-    """Flash attention on ``[b, a, s, d]`` views with optional additive bias (dense or ALiBi slopes), key-padding
-    lengths and Philox dropout on the probabilities — all inside the wgmma kernels."""
+    """Flash attention on ``[b, a, sq, d]`` / ``[b, g, sk, d]`` views with optional additive bias (dense or ALiBi
+    slopes), per-sample key windows (``kv_start`` / ``kv_lens``) and Philox dropout on the probabilities — all inside
+    the wgmma kernels."""
 
     @staticmethod
-    def forward(ctx, q, k, v, causal, scale, bias, alibi_slopes, p_drop, kv_lens):
+    def forward(ctx, q, k, v, causal, scale, bias, alibi_slopes, p_drop, kv_lens, kv_start=None):
         ext = load_ext()
         b = _prep_bias(bias, q)
         o, lse, rng_state = ext.attn_fwd(q, k, v, causal, scale, kv_lens, b, alibi_slopes, p_drop,
-                                         tp_rng_salt(True) if p_drop > 0 else 0)
+                                         tp_rng_salt(True) if p_drop > 0 else 0, kv_start)
         count_launch()
-        ctx.save_for_backward(q, k, v, o, lse, b, alibi_slopes, rng_state, kv_lens)
+        ctx.save_for_backward(q, k, v, o, lse, b, alibi_slopes, rng_state, kv_lens, kv_start)
         ctx.causal, ctx.scale, ctx.p_drop = causal, scale, p_drop
         ctx.bias_shape = None if bias is None else (bias.shape, bias.dtype)
         return o
@@ -609,20 +633,20 @@ class _FlashAttnFn(torch.autograd.Function):
     @staticmethod
     def backward(ctx, go):
         ext = load_ext()
-        q, k, v, o, lse, b, slopes, rng_state, kv_lens = ctx.saved_tensors
+        q, k, v, o, lse, b, slopes, rng_state, kv_lens, kv_start = ctx.saved_tensors
         dbias = None
         if b is not None and ctx.needs_input_grad[5]:
             dbias = torch.zeros(b.shape, dtype=torch.float32, device=b.device)
             if dbias.stride() != b.stride():
                 dbias = torch.empty_strided(b.shape, b.stride(), dtype=torch.float32, device=b.device).zero_()
         dq, dk, dv, _ = ext.attn_bwd(go, q, k, v, o, lse, ctx.causal, ctx.scale, kv_lens, b, slopes, dbias, ctx.p_drop,
-                                     rng_state if ctx.p_drop > 0 else None)
+                                     rng_state if ctx.p_drop > 0 else None, kv_start)
         count_launch(3)
         gb = None
         if dbias is not None:
             shape, dtype = ctx.bias_shape
             gb = dbias.to(dtype).reshape(shape)
-        return dq, dk, dv, None, None, gb, None, None, None
+        return dq, dk, dv, None, None, gb, None, None, None, None
 
 
 class _FlashAttnPackedFn(torch.autograd.Function):
@@ -671,27 +695,42 @@ def attention_qkvpacked(qkv, *, causal: bool, scale: float, kv_lens=None, dropou
     return _FlashAttnPackedFn.apply(qkv, causal, float(scale), kv_lens, p, alibi_slopes)
 
 
-def attention(q, k, v, *, causal: bool = False, scale: Optional[float] = None, mask=None, bias=None,
-              dropout_p: float = 0.0, training: bool = False, alibi_slopes=None, kv_lens=None):
-    """Softmax attention of q ``[b, a, s, d]`` over k, v ``[b, g, s, d]`` (``g = a`` or, grouped-query, a divisor of
-    ``a``).  The native flash kernels handle causal / full / key-padding
-    (``kv_lens``) masking, an additive score bias (dense ``[b|1, a|1, s, s]`` — T5 relative positions — or
-    ``alibi_slopes`` ``[a]``) and dropout on the probabilities; arbitrary dense 0/1 masks and cross attention with
-    different query / key lengths use the reference math."""
-    if scale is None:
-        scale = 1.0 / math.sqrt(q.shape[-1])
-    if (
+def attention_supported(q, k, mask=None, bias=None) -> bool:
+    """True when :func:`attention` of ``q`` over ``k`` runs the native flash kernels: bf16 on the GPU, head dim 64 or
+    128, no dense 0/1 ``mask`` and a dense ``bias`` (if any) of shape ``[.., sq, sk]``.  Query and key lengths are free.
+    Otherwise :func:`attention` runs the reference math."""
+    return (
         use_native(q)
         and q.dtype == torch.bfloat16
         and mask is None
         and q.shape[-1] in (64, 128)
-        and q.shape[-2] == k.shape[-2]
-        and q.shape[-2] % 8 == 0
         and (bias is None or (bias.shape[-1] == k.shape[-2] and bias.shape[-2] == q.shape[-2]))
-    ):
+    )
+
+
+def attention(q, k, v, *, causal: bool = False, scale: Optional[float] = None, mask=None, bias=None,
+              dropout_p: float = 0.0, training: bool = False, alibi_slopes=None, kv_lens=None, kv_start=None):
+    """Softmax attention of q ``[b, a, sq, d]`` over k, v ``[b, g, sk, d]`` (``g = a`` or, grouped-query, a divisor of
+    ``a``; ``sq`` and ``sk`` independent).  Key ``j`` is visible to query ``i`` of sample ``b`` iff
+    ``kv_start[b] <= j < kv_lens[b]`` (int32 ``[b]`` device tensors, defaults ``0`` and ``sk``; ``kv_lens`` is clamped to
+    at least 1) and, when ``causal``, ``j <= i + sk - sq`` (bottom-right alignment).  A query without a visible key
+    gets zeros.  The native flash kernels (see :func:`attention_supported`) handle this masking, an additive score bias
+    (dense ``[b|1, a|1, sq, sk]`` — T5 relative positions — or ``alibi_slopes`` ``[a]``, ``slope·(j − i − (sk − sq))``)
+    and dropout on the probabilities; arbitrary dense 0/1 masks use the reference math.  The reference applies
+    ``kv_lens`` only together with ``kv_start``."""
+    if scale is None:
+        scale = 1.0 / math.sqrt(q.shape[-1])
+    if attention_supported(q, k, mask, bias):
         # strided [b, a, s, d] views of the packed QKV projection are consumed directly (TMA strides)
         return _FlashAttnFn.apply(q, k, v, causal, float(scale), bias, alibi_slopes,
-                                  float(dropout_p) if training else 0.0, kv_lens)
+                                  float(dropout_p) if training else 0.0, kv_lens, kv_start)
+    if kv_start is not None:
+        vis = visible_keys(q.shape[-2], k.shape[-2], causal=causal, kv_start=kv_start, kv_lens=kv_lens, device=q.device)
+        if mask is not None:
+            vis = vis & mask.bool()
+        o = attention(q, k, v, causal=False, scale=scale, mask=vis, bias=bias, dropout_p=dropout_p, training=training,
+                      alibi_slopes=alibi_slopes)
+        return o.masked_fill(~vis.any(-1, keepdim=True), 0)
     if alibi_slopes is not None:
         sq, sk = q.shape[-2], k.shape[-2]
         rel = torch.arange(sk, device=q.device)[None, :] - torch.arange(sk - sq, sk, device=q.device)[:, None]
@@ -748,17 +787,26 @@ def kv_cache_append_ref(qkv, k_cache, v_cache, cache_seqlens, cos=None, sin=None
     return q
 
 
-def decode_attention(q, k_cache, v_cache, cache_seqlens, kv_start, *, scale: float, splits: int = 0):
+def decode_attention(q, k_cache, v_cache, cache_seqlens, kv_start, *, scale: float, splits: int = 0,
+                     past: Optional[int] = None):
     """Attention of ``q [b, s, a, d]`` (new tokens, already appended to the caches; any strides with d contiguous) over
     the caches ``[b, g, C, d]`` (query head ``h`` reads cache head ``h // (a // g)``): query ``i`` of sample ``b`` sees exactly the keys ``kv_start[b] <= j <= cache_seqlens[b] + i``.  Returns
     ``[b, s, a, d]`` contiguous; a query without a visible key gets zeros.  The native kernel takes up to 16 new tokens
     and reads lengths on the device (no host sync; one CUDA-graph capture replays after the lengths change); ``splits``
-    > 0 fixes its number of key-range splits."""
-    if _decode_native(q, k_cache) and q.shape[1] <= 16:
-        ext = load_ext()
-        o = ext.decode_attn(q, k_cache, v_cache, cache_seqlens, kv_start, float(scale), int(splits))
-        count_launch(2)
-        return o
+    > 0 fixes its number of key-range splits.  ``past`` (host int): the rows every sample held before these tokens
+    (``cache_seqlens`` all equal to it, as in a :class:`~libai_b200.inference.kv_cache.StaticKVCache`); with it, more
+    than 16 new tokens run the causal flash kernel over the cache window ``[:past + s]`` (chunked prefill)."""
+    if _decode_native(q, k_cache):
+        if q.shape[1] <= 16:
+            ext = load_ext()
+            o = ext.decode_attn(q, k_cache, v_cache, cache_seqlens, kv_start, float(scale), int(splits))
+            count_launch(2)
+            return o
+        if past is not None:
+            L = past + q.shape[1]
+            o = attention(q.permute(0, 2, 1, 3), k_cache[:, :, :L], v_cache[:, :, :L], causal=True, scale=scale,
+                          kv_start=kv_start)
+            return o.transpose(1, 2)   # the kernel's [b, s, a, d] output
     return decode_attention_ref(q, k_cache, v_cache, cache_seqlens, kv_start, scale=scale)
 
 
