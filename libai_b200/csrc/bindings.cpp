@@ -149,7 +149,8 @@ Tensor gemm(const Tensor& a, const Tensor& b, int64_t layout, const c10::optiona
     epi = 0;
   } else {
     TORCH_CHECK(out.scalar_type() == at::kFloat, "gemm: out must be bf16 or fp32");
-    epi = (accumulate || layout == 2) ? 2 : 1;
+    // a freshly zeroed wgrad output takes the accumulating epilogue too; a given `out` is added to only on request
+    epi = (accumulate || (layout == 2 && !out_opt.has_value())) ? 2 : 1;
   }
   const void* bias_ptr = nullptr;
   if (bias.has_value() && bias->defined()) {
@@ -362,15 +363,34 @@ Tensor colsum(const Tensor& x, const c10::optional<Tensor>& accum) {
 }
 
 // ---- norms ----------------------------------------------------------------------------------------
+// The kernels read H elements of γ (and β) with no bounds of their own and are built for the (x, γ) dtype pairs
+// (bf16, bf16), (bf16, fp32) and (fp32, fp32).
+void check_norm_params(const char* what, const Tensor& x, const Tensor& gamma, const Tensor* beta) {
+  TORCH_CHECK(x.is_cuda() && x.dim() == 2 && x.is_contiguous(), what, ": x must be a contiguous CUDA tensor [rows, H]");
+  const bool pair_ok = (x.scalar_type() == at::kBFloat16 &&
+                        (gamma.scalar_type() == at::kBFloat16 || gamma.scalar_type() == at::kFloat)) ||
+                       (x.scalar_type() == at::kFloat && gamma.scalar_type() == at::kFloat);
+  TORCH_CHECK(pair_ok, what, ": unsupported dtypes x ", x.scalar_type(), " with gamma ", gamma.scalar_type(),
+              " (supported: bf16/bf16, bf16/fp32, fp32/fp32)");
+  TORCH_CHECK(gamma.is_contiguous() && gamma.numel() == x.size(1) && gamma.device() == x.device(), what,
+              ": gamma must be contiguous with H = ", x.size(1), " elements on x's device");
+  if (beta != nullptr) {
+    TORCH_CHECK(beta->scalar_type() == gamma.scalar_type(), what, ": beta must have gamma's dtype");
+    TORCH_CHECK(beta->is_contiguous() && beta->numel() == x.size(1) && beta->device() == x.device(), what,
+                ": beta must be contiguous with H = ", x.size(1), " elements on x's device");
+  }
+}
+
 std::tuple<Tensor, Tensor, Tensor> norm_fwd(const Tensor& x, const Tensor& gamma, const c10::optional<Tensor>& beta,
                                             double eps, bool rms) {
   c10::cuda::CUDAGuard guard(x.device());
-  TORCH_CHECK(x.dim() == 2 && x.is_contiguous(), "norm_fwd: contiguous [rows, H]");
+  const bool has_beta = beta.has_value() && beta->defined();
+  check_norm_params("norm_fwd", x, gamma, has_beta ? &beta.value() : nullptr);
   const int rows = (int)x.size(0), H = (int)x.size(1);
   Tensor y = at::empty_like(x);
   Tensor mean = rms ? at::empty({0}, x.options().dtype(at::kFloat)) : at::empty({rows}, x.options().dtype(at::kFloat));
   Tensor rstd = at::empty({rows}, x.options().dtype(at::kFloat));
-  const void* b = (beta.has_value() && beta->defined()) ? beta->data_ptr() : nullptr;
+  const void* b = has_beta ? beta->data_ptr() : nullptr;
   check(lb_norm_fwd(x.data_ptr(), gamma.data_ptr(), b, y.data_ptr(), rms ? nullptr : mean.data_ptr<float>(),
                     rstd.data_ptr<float>(), rows, H, (float)eps, rms ? 1 : 0, dtype_code(x), dtype_code(gamma),
                     cur_stream()),
@@ -384,7 +404,12 @@ std::tuple<Tensor, Tensor, Tensor> norm_bwd(const Tensor& gy, const Tensor& x, c
                                             const c10::optional<Tensor>& dbeta_accum,
                                             const c10::optional<Tensor>& gadd) {
   c10::cuda::CUDAGuard guard(x.device());
+  check_norm_params("norm_bwd", x, gamma, nullptr);
+  TORCH_CHECK(gy.sizes() == x.sizes() && gy.scalar_type() == x.scalar_type() && gy.is_contiguous() &&
+                  gy.device() == x.device(),
+              "norm_bwd: gy must be contiguous with x's shape, dtype and device");
   const int rows = (int)x.size(0), H = (int)x.size(1);
+  TORCH_CHECK(rstd.numel() == rows && (rms || mean.numel() == rows), "norm_bwd: mean / rstd must hold one value per row");
   Tensor gx = at::empty_like(x);
   auto fopt = x.options().dtype(at::kFloat);
   // accumulate mode: dgamma / dbeta are added straight into the fp32 main-grad slices of the parameters

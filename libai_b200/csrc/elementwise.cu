@@ -387,6 +387,7 @@ __global__ void __launch_bounds__(256) ce_stats_kernel(const T* __restrict__ log
       float cm = x[0];
 #pragma unroll
       for (int j = 1; j < 8; ++j) cm = fmaxf(cm, x[j]);
+      if (cm == -INFINITY) continue;  // adds exp(-inf) = 0; with m = -inf the update below would add exp(-inf + inf)
       if (cm > m) {
         s *= __expf(m - cm);
         m = cm;
@@ -397,6 +398,7 @@ __global__ void __launch_bounds__(256) ce_stats_kernel(const T* __restrict__ log
   } else {
     for (int c = threadIdx.x; c < V; c += blockDim.x) {
       const float x = ld_logit<T>(lr + c);
+      if (x == -INFINITY) continue;
       if (x > m) {
         s = s * __expf(m - x) + 1.0f;
         m = x;

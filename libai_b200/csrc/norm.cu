@@ -321,11 +321,11 @@ __global__ void norm_fwd_generic(const T* __restrict__ x, const W* __restrict__ 
   }
 }
 
+// gx only; dγ / dβ come from norm_bwd_colpart_generic + colreduce_kernel
 template <typename T, typename W, bool RMS>
 __global__ void norm_bwd_generic(const T* __restrict__ gy, const T* __restrict__ x, const W* __restrict__ gamma,
                                  const float* __restrict__ mean_in, const float* __restrict__ rstd_in,
-                                 T* __restrict__ gx, float* __restrict__ dgamma, float* __restrict__ dbeta, int rows,
-                                 int H) {
+                                 T* __restrict__ gx, int rows, int H) {
   const int warp = threadIdx.x / 32, lane = threadIdx.x % 32;
   const int row = blockIdx.x * (blockDim.x / 32) + warp;
   if (row >= rows) return;
@@ -335,12 +335,9 @@ __global__ void norm_bwd_generic(const T* __restrict__ gy, const T* __restrict__
   float s1 = 0.f, s2 = 0.f;
   for (int c = lane; c < H; c += 32) {
     const float xh = (static_cast<float>(xr[c]) - mean) * rstd;
-    const float g = static_cast<float>(gr[c]);
-    const float gw = g * static_cast<float>(gamma[c]);
+    const float gw = static_cast<float>(gr[c]) * static_cast<float>(gamma[c]);
     s1 += gw;
     s2 += gw * xh;
-    atomicAdd(&dgamma[c], g * xh);
-    if (dbeta != nullptr) atomicAdd(&dbeta[c], g);
   }
   s1 = RMS ? 0.f : warp_sum(s1) / H;
   s2 = warp_sum(s2) / H;
@@ -350,6 +347,29 @@ __global__ void norm_bwd_generic(const T* __restrict__ gy, const T* __restrict__
     const float gw = static_cast<float>(gr[c]) * static_cast<float>(gamma[c]);
     gxr[c] = static_cast<T>(rstd * (gw - s1 - xh * s2));
   }
+}
+
+// part_dgamma[blockIdx.y, c] = Σ g·x̂ and part_dbeta[blockIdx.y, c] = Σ g over rows [blockIdx.y * rows_per_block, +
+// rows_per_block): one thread per column, rows in increasing order, so the sums colreduce_kernel makes of the partials
+// do not depend on scheduling (atomics would make dγ / dβ differ from run to run in the last bits)
+template <typename T, bool RMS>
+__global__ void __launch_bounds__(256)
+norm_bwd_colpart_generic(const T* __restrict__ gy, const T* __restrict__ x, const float* __restrict__ mean_in,
+                         const float* __restrict__ rstd_in, float* __restrict__ part_dgamma,
+                         float* __restrict__ part_dbeta, int rows, int H, int rows_per_block) {
+  const int c = blockIdx.x * blockDim.x + threadIdx.x;
+  if (c >= H) return;
+  const int r0 = blockIdx.y * rows_per_block;
+  const int r1 = min(rows, r0 + rows_per_block);
+  float dg = 0.f, db = 0.f;
+  for (int r = r0; r < r1; ++r) {
+    const float mean = RMS ? 0.f : mean_in[r];
+    const float g = static_cast<float>(gy[static_cast<size_t>(r) * H + c]);
+    dg += g * ((static_cast<float>(x[static_cast<size_t>(r) * H + c]) - mean) * rstd_in[r]);
+    db += g;
+  }
+  part_dgamma[static_cast<size_t>(blockIdx.y) * H + c] = dg;
+  if (part_dbeta != nullptr) part_dbeta[static_cast<size_t>(blockIdx.y) * H + c] = db;
 }
 
 }  // namespace lb
@@ -505,18 +525,25 @@ extern "C" int lb_norm_bwd(const void* gy, const void* x, const void* gamma, con
       }                                                                                                              \
     }                                                                                                                \
     if (!done) {                                                                                                     \
-      if (!accumulate) {                                                                                             \
-        cudaMemsetAsync(dgamma, 0, sizeof(float) * H, s);                                                            \
-        if (dbeta != nullptr) cudaMemsetAsync(dbeta, 0, sizeof(float) * H, s);                                       \
-      }                                                                                                              \
       const int wpb = 8;                                                                                             \
       const int g2 = (rows + wpb - 1) / wpb;                                                                         \
-      if (rms)                                                                                                       \
+      /* column partials over `grid` (<= workspace rows) fixed row blocks */                                         \
+      const int rpb = (rows + grid - 1) / grid;                                                                      \
+      const int nparts = (rows + rpb - 1) / rpb;                                                                     \
+      const dim3 pgrid((H + 255) / 256, nparts);                                                                     \
+      if (rms) {                                                                                                     \
         lb::norm_bwd_generic<T, W, true><<<g2, wpb * 32, 0, s>>>((const T*)gy, (const T*)x, (const W*)gamma, mean,   \
-                                                                 rstd, (T*)gx, dgamma, dbeta, rows, H);              \
-      else                                                                                                           \
+                                                                 rstd, (T*)gx, rows, H);                             \
+        lb::norm_bwd_colpart_generic<T, true><<<pgrid, 256, 0, s>>>((const T*)gy, (const T*)x, mean, rstd, pdg, pdb, \
+                                                                    rows, H, rpb);                                   \
+      } else {                                                                                                       \
         lb::norm_bwd_generic<T, W, false><<<g2, wpb * 32, 0, s>>>((const T*)gy, (const T*)x, (const W*)gamma, mean,  \
-                                                                  rstd, (T*)gx, dgamma, dbeta, rows, H);             \
+                                                                  rstd, (T*)gx, rows, H);                            \
+        lb::norm_bwd_colpart_generic<T, false><<<pgrid, 256, 0, s>>>((const T*)gy, (const T*)x, mean, rstd, pdg,     \
+                                                                     pdb, rows, H, rpb);                             \
+      }                                                                                                              \
+      lb::colreduce_kernel<<<dim3((H + 31) / 32, dbeta != nullptr ? 2 : 1), 256, 0, s>>>(pdg, dgamma, pdb, dbeta,    \
+                                                                                         nparts, H, accumulate);     \
     }                                                                                                                \
   }
   if (dtype == 0 && wdtype == 0) LB_GO(__nv_bfloat16, __nv_bfloat16)

@@ -359,15 +359,24 @@ class _LayerNormFn(torch.autograd.Function):
                 None)
 
 
+_NORM_DTYPES = {(torch.bfloat16, torch.bfloat16), (torch.bfloat16, torch.float32), (torch.float32, torch.float32)}
+
+
+def _norm_native(x, weight, bias=None) -> bool:
+    """The native norm kernels take these (activation, γ) dtype pairs, with β of γ's dtype."""
+    return (use_native(x) and weight is not None and (x.dtype, weight.dtype) in _NORM_DTYPES
+            and (bias is None or bias.dtype == weight.dtype))
+
+
 def layer_norm_with_skip(x, weight, bias, eps: float = 1e-5):
     """``(layer_norm(x), x)`` where the second output carries the skip connection (see ``_LayerNormFn``)."""
-    if use_native(x) and x.dtype in (torch.bfloat16, torch.float32) and weight is not None and x.requires_grad:
+    if _norm_native(x, weight, bias) and x.requires_grad:
         return _LayerNormFn.apply(x, weight, bias, eps, False, True)
     return layer_norm(x, weight, bias, eps), x
 
 
 def layer_norm(x, weight, bias, eps: float = 1e-5):
-    if use_native(x) and x.dtype in (torch.bfloat16, torch.float32) and weight is not None:
+    if _norm_native(x, weight, bias):
         return _LayerNormFn.apply(x, weight, bias, eps, False)
     w = None if weight is None else weight.float()
     b = None if bias is None else bias.float()
@@ -375,7 +384,7 @@ def layer_norm(x, weight, bias, eps: float = 1e-5):
 
 
 def rms_norm(x, weight, eps: float = 1e-6):
-    if use_native(x) and x.dtype in (torch.bfloat16, torch.float32):
+    if _norm_native(x, weight):
         return _LayerNormFn.apply(x, weight, None, eps, True)
     xf = x.float()
     y = xf * torch.rsqrt(xf.pow(2).mean(-1, keepdim=True) + eps)
