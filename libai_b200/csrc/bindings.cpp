@@ -543,7 +543,11 @@ Tensor rope(const Tensor& x, const Tensor& cosv, const Tensor& sinv, bool backwa
   c10::cuda::CUDAGuard guard(x.device());
   TORCH_CHECK(x.dim() == 4 && x.is_contiguous() && x.scalar_type() == at::kBFloat16, "rope: contiguous bf16 [b,a,s,d]");
   const int S = (int)x.size(2), D = (int)x.size(3);
-  TORCH_CHECK(cosv.is_contiguous() && sinv.is_contiguous() && cosv.size(0) >= S && cosv.size(1) == D, "rope: cos/sin [S,D]");
+  TORCH_CHECK(cosv.scalar_type() == at::kFloat && sinv.scalar_type() == at::kFloat && cosv.is_contiguous() &&
+                  sinv.is_contiguous() && cosv.dim() == 2 && cosv.size(0) >= S && cosv.size(1) == D &&
+                  sinv.sizes() == cosv.sizes(),
+              "rope: cos/sin fp32 contiguous [>=S, D] of one shape");
+  TORCH_CHECK(cosv.device() == x.device() && sinv.device() == x.device(), "rope: cos/sin must be on x's device");
   Tensor y = at::empty_like(x);
   check(lb_rope(x.data_ptr(), cosv.data_ptr<float>(), sinv.data_ptr<float>(), y.data_ptr(), x.numel() / D, S, D,
                 backward ? 1 : 0, cur_stream()),
