@@ -19,7 +19,7 @@ int lb_norm_fwd(const void* x, const void* gamma, const void* beta, void* y, flo
 int lb_gemm_bf16_bias_residual(const void* x, const void* w, void* out, int M, int N, int K, int lda, int ldb,
                                const void* bias, const void* residual, cudaStream_t s);
 int lb_gemm_fp8(const void* xq, const void* wq, void* out, int M, int N, int K, const void* bias, int act, void* pre_out,
-                const void* residual, const float* deq_x, const float* deq_w, cudaStream_t s);
+                const void* residual, const float* deq_x, const float* deq_w, int force_bn, cudaStream_t s);
 int lb_quant_e4m3(const void* x, void* q, void* amax_scratch, float* deq, long n, cudaStream_t s);
 int lb_norm_bwd_workspace_rows(int rows);
 int lb_norm_bwd_supports_gadd(int H);
@@ -49,8 +49,8 @@ int lb_ce_stats(const void* logits, const int64_t* labels, float* mx, float* se,
                 long vocab_start, int dtype, cudaStream_t s);
 int lb_ce_bwd(const void* logits, const int64_t* labels, const float* lse, const float* gloss, void* dlogits, int T,
               int V, long vocab_start, int dtype, cudaStream_t s);
-int lb_adamw(float* master, const float* grad, float* m, float* v, void* lp_out, const float* scale, long n, float lr,
-             float b1, float b2, float eps, float wd, float bc1, float bc2, int decoupled, cudaStream_t s);
+int lb_adamw(float* master, const float* grad, float* m, float* v, void* lp_out, int lp_dtype, const float* scale, long n,
+             float lr, float b1, float b2, float eps, float wd, float bc1, float bc2, int decoupled, cudaStream_t s);
 int lb_sqnorm_workspace(long n);
 int lb_sqnorm(const float* x, float* out, long n, float* workspace, cudaStream_t s);
 int lb_gemm_bf16_comm(const void* a, const void* b, void* out, int M, int N, int K, int layout, int epi,
@@ -251,10 +251,16 @@ std::tuple<Tensor, Tensor> quantize_e4m3(const Tensor& x) {
   return std::make_tuple(q, scratch.narrow(0, 0, 1));
 }
 
-// fp8 forward: y = act((xq @ wqᵀ) * deq_x * deq_w + bias) in bf16, optional bf16 pre-activation copy
+// fp8 forward: y = act((xq @ wqᵀ) * deq_x * deq_w + bias) in bf16, optional bf16 pre-activation copy; with a residual
+// y = (xq @ wqᵀ) * deq_x * deq_w + bias + residual (no activation, no pre-activation copy).  bn: tile width (0 = the
+// heuristic; 64 / 128 / 192 / 256 for tests and tuning)
 std::tuple<Tensor, Tensor> linear_fp8_fwd(const Tensor& xq, const Tensor& wq, const Tensor& deq_x, const Tensor& deq_w,
                                           const c10::optional<Tensor>& bias, int64_t act, bool want_pre,
-                                          const c10::optional<Tensor>& residual) {
+                                          const c10::optional<Tensor>& residual, int64_t bn) {
+  TORCH_CHECK(bn == 0 || bn == 64 || bn == 128 || bn == 192 || bn == 256, "linear_fp8_fwd: bn must be 0, 64, 128, 192 or 256");
+  const bool has_res = residual.has_value() && residual->defined();
+  TORCH_CHECK(!has_res || (act == 0 && !want_pre),
+              "linear_fp8_fwd: a residual epilogue takes no activation and no pre-activation copy");
   TORCH_CHECK(xq.is_cuda() && xq.dim() == 2 && wq.dim() == 2 && xq.size(1) == wq.size(1), "linear_fp8_fwd: shape mismatch");
   TORCH_CHECK(xq.scalar_type() == at::kFloat8_e4m3fn && wq.scalar_type() == at::kFloat8_e4m3fn, "linear_fp8_fwd: e4m3 operands");
   TORCH_CHECK(xq.is_contiguous() && wq.is_contiguous(), "linear_fp8_fwd: contiguous operands");
@@ -279,7 +285,7 @@ std::tuple<Tensor, Tensor> linear_fp8_fwd(const Tensor& xq, const Tensor& wq, co
   }
   check(lb_gemm_fp8(xq.data_ptr(), wq.data_ptr(), y.data_ptr(), (int)M, (int)N, (int)K, bias_ptr, (int)act,
                     pre.defined() ? pre.data_ptr() : nullptr, res_ptr, deq_x.data_ptr<float>(), deq_w.data_ptr<float>(),
-                    cur_stream()),
+                    (int)bn, cur_stream()),
         "linear_fp8_fwd");
   return std::make_tuple(y, pre.defined() ? pre : at::empty({0}, opts));
 }
@@ -330,6 +336,8 @@ Tensor embedding_fwd(const Tensor& ids, const Tensor& table, int64_t vocab_start
 void embedding_bwd(const Tensor& ids, const Tensor& gy, Tensor grad, int64_t vocab_start) {
   c10::cuda::CUDAGuard guard(gy.device());
   TORCH_CHECK(ids.scalar_type() == at::kLong && ids.is_contiguous(), "embedding_bwd: contiguous int64 ids");
+  TORCH_CHECK(gy.is_cuda() && ids.device() == gy.device() && grad.device() == gy.device(),
+              "embedding_bwd: ids, gy and grad must be on one CUDA device");
   TORCH_CHECK(gy.dim() == 2 && gy.is_contiguous() && gy.scalar_type() == at::kBFloat16 && gy.size(0) == ids.numel(),
               "embedding_bwd: gy must be contiguous bf16 [ids.numel(), H]");
   TORCH_CHECK(grad.dim() == 2 && grad.is_contiguous() && grad.scalar_type() == at::kFloat && grad.size(1) == gy.size(1),
@@ -582,9 +590,31 @@ Tensor ce_bwd(const Tensor& logits, const Tensor& labels, const Tensor& lse, con
 void fused_adamw(Tensor master, const Tensor& grad, Tensor m, Tensor v, const c10::optional<Tensor>& lp_out,
                  const Tensor& scale, double lr, double b1, double b2, double eps, double wd, double bc1, double bc2,
                  bool decoupled) {
-  c10::cuda::CUDAGuard guard(master.device());
-  void* lp = (lp_out.has_value() && lp_out->defined()) ? lp_out->data_ptr() : nullptr;
-  check(lb_adamw(master.data_ptr<float>(), grad.data_ptr<float>(), m.data_ptr<float>(), v.data_ptr<float>(), lp,
+  // float4 loads and stores over master.numel() elements of every buffer
+  const auto dev = master.device();
+  for (const Tensor* t : {static_cast<const Tensor*>(&master), &grad, static_cast<const Tensor*>(&m),
+                          static_cast<const Tensor*>(&v)}) {
+    TORCH_CHECK(t->is_cuda() && t->device() == dev && t->scalar_type() == at::kFloat && t->is_contiguous() &&
+                    t->numel() == master.numel(),
+                "fused_adamw: master, grad, m and v must be contiguous fp32 tensors of one size on one CUDA device");
+    TORCH_CHECK(reinterpret_cast<uintptr_t>(t->data_ptr()) % 16 == 0, "fused_adamw: buffers must be 16-byte aligned");
+  }
+  TORCH_CHECK(master.numel() % 4 == 0, "fused_adamw: numel must be a multiple of 4");
+  TORCH_CHECK(scale.is_cuda() && scale.device() == dev && scale.scalar_type() == at::kFloat && scale.numel() == 1,
+              "fused_adamw: scale must be a one-element fp32 tensor on the buffers' device");
+  void* lp = nullptr;
+  int lp_dtype = 0;
+  if (lp_out.has_value() && lp_out->defined()) {
+    TORCH_CHECK(lp_out->scalar_type() == at::kBFloat16 || lp_out->scalar_type() == at::kHalf,
+                "fused_adamw: lp_out must be bf16 or fp16");
+    TORCH_CHECK(lp_out->is_cuda() && lp_out->device() == dev && lp_out->is_contiguous() &&
+                    lp_out->numel() == master.numel() && reinterpret_cast<uintptr_t>(lp_out->data_ptr()) % 8 == 0,
+                "fused_adamw: lp_out must be contiguous, 8-byte aligned, of master's size and on its device");
+    lp = lp_out->data_ptr();
+    lp_dtype = lp_out->scalar_type() == at::kHalf ? 1 : 0;
+  }
+  c10::cuda::CUDAGuard guard(dev);
+  check(lb_adamw(master.data_ptr<float>(), grad.data_ptr<float>(), m.data_ptr<float>(), v.data_ptr<float>(), lp, lp_dtype,
                  scale.data_ptr<float>(), master.numel(), (float)lr, (float)b1, (float)b2, (float)eps, (float)wd,
                  (float)bc1, (float)bc2, decoupled ? 1 : 0, cur_stream()),
         "fused_adamw");
@@ -1035,7 +1065,7 @@ TORCH_LIBRARY(libai_b200, m) {
   m.def("gemm_tuned(Tensor a, Tensor b, int layout, int bn, int splits, bool fp32_out) -> Tensor", &gemm_tuned);
   m.def("linear_fwd(Tensor x, Tensor w, Tensor? bias, int act, bool need_pre) -> (Tensor, Tensor)", &linear_fwd);
   m.def("quantize_e4m3(Tensor x) -> (Tensor, Tensor)", &quantize_e4m3);
-  m.def("linear_fp8_fwd(Tensor xq, Tensor wq, Tensor deq_x, Tensor deq_w, Tensor? bias, int act, bool need_pre, Tensor? residual=None) -> (Tensor, Tensor)", &linear_fp8_fwd);
+  m.def("linear_fp8_fwd(Tensor xq, Tensor wq, Tensor deq_x, Tensor deq_w, Tensor? bias, int act, bool need_pre, Tensor? residual=None, int bn=0) -> (Tensor, Tensor)", &linear_fp8_fwd);
   m.def("act_bwd(Tensor gy, Tensor pre, int act) -> Tensor", &act_bwd);
   m.def("colsum(Tensor x, Tensor(a!)? accum=None) -> Tensor", &colsum);
   m.def("norm_fwd(Tensor x, Tensor gamma, Tensor? beta, float eps, bool rms) -> (Tensor, Tensor, Tensor)", &norm_fwd);

@@ -142,15 +142,7 @@ zero_adam_allgather_kernel(float* __restrict__ master, const float* __restrict__
     float pp[4] = {p4.x, p4.y, p4.z, p4.w}, gg[4] = {g4.x, g4.y, g4.z, g4.w};
     float mm[4] = {m4.x, m4.y, m4.z, m4.w}, vv[4] = {v4.x, v4.y, v4.z, v4.w};
 #pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      float g = gg[j] * clip;
-      if (!decoupled) g += wd * pp[j];
-      mm[j] = b1 * mm[j] + (1.0f - b1) * g;
-      vv[j] = b2 * vv[j] + (1.0f - b2) * g * g;
-      float upd = (mm[j] / bc1) / (sqrtf(vv[j] / bc2) + eps);
-      if (decoupled) upd += wd * pp[j];
-      pp[j] -= lr * upd;
-    }
+    for (int j = 0; j < 4; ++j) adam_element(pp[j], mm[j], vv[j], gg[j], clip, lr, b1, b2, eps, wd, bc1, bc2, decoupled);
     reinterpret_cast<float4*>(master)[i] = make_float4(pp[0], pp[1], pp[2], pp[3]);
     reinterpret_cast<float4*>(m)[i] = make_float4(mm[0], mm[1], mm[2], mm[3]);
     reinterpret_cast<float4*>(v)[i] = make_float4(vv[0], vv[1], vv[2], vv[3]);

@@ -259,6 +259,19 @@ LB_DEVICE float2 unpack_bf16(uint32_t u) {
   return make_float2(__uint_as_float(u << 16), __uint_as_float(u & 0xffff0000u));
 }
 
+// one Adam step of one element, shared by fused_adamw and the ZeRO update: g = grad * scale (+ wd * p when the weight
+// decay is coupled), fp32 moments m, v, bias corrections bc1, bc2; decoupled weight decay adds wd * p to the update
+LB_DEVICE void adam_element(float& p, float& m, float& v, float grad, float scale, float lr, float b1, float b2, float eps,
+                            float wd, float bc1, float bc2, int decoupled) {
+  float g = grad * scale;
+  if (!decoupled) g += wd * p;
+  m = b1 * m + (1.0f - b1) * g;
+  v = b2 * v + (1.0f - b2) * g * g;
+  float upd = (m / bc1) / (sqrtf(v / bc2) + eps);
+  if (decoupled) upd += wd * p;
+  p -= lr * upd;
+}
+
 enum Act : int { ACT_NONE = 0, ACT_GELU = 1, ACT_GELU_TANH = 2, ACT_RELU = 3, ACT_SILU = 4, ACT_QUICK_GELU = 5,
                  ACT_RESADD = 6 /* GEMM epilogue only: out = acc (+ bias) + pre_in, i.e. the residual add */ };
 

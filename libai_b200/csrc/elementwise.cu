@@ -8,7 +8,9 @@
 // apply_rotary_pos_emb (projects/Llama/llama.py:31-43), sparse_softmax_cross_entropy
 // (libai/layers/cross_entropy.py:44), flow.optim.AdamW multi-tensor update (configs/common/optim.py).
 #include "common.cuh"
+#include <cuda_fp16.h>
 #include <cuda_fp8.h>
+#include <type_traits>
 
 namespace lb {
 
@@ -463,10 +465,21 @@ __global__ void __launch_bounds__(256) ce_bwd_kernel(const T* __restrict__ logit
 }
 
 // ------------------------------------------------------------------------------------------------
-// fused AdamW over flat fp32 buffers (+ optional low-precision parameter copy)
+// fused AdamW over flat fp32 buffers (+ optional low-precision parameter copy, bf16 or fp16: LP)
 // ------------------------------------------------------------------------------------------------
+template <typename LP>
+__device__ __forceinline__ uint32_t pack_lp(float a, float b) {
+  if constexpr (std::is_same<LP, __half>::value) {
+    __half2 h = __floats2half2_rn(a, b);
+    return *reinterpret_cast<uint32_t*>(&h);
+  } else {
+    return pack_bf16(a, b);
+  }
+}
+
+template <typename LP>
 __global__ void adamw_kernel(float* __restrict__ master, const float* __restrict__ grad, float* __restrict__ m,
-                             float* __restrict__ v, __nv_bfloat16* __restrict__ lp_out,
+                             float* __restrict__ v, LP* __restrict__ lp_out,
                              const float* __restrict__ scale_ptr, size_t n, float lr, float b1, float b2, float eps,
                              float wd, float bc1, float bc2, int decoupled) {
   const float scale = scale_ptr != nullptr ? *scale_ptr : 1.0f;
@@ -479,20 +492,12 @@ __global__ void adamw_kernel(float* __restrict__ master, const float* __restrict
     float pp[4] = {p4.x, p4.y, p4.z, p4.w}, gg[4] = {g4.x, g4.y, g4.z, g4.w};
     float mm[4] = {m4.x, m4.y, m4.z, m4.w}, vv[4] = {v4.x, v4.y, v4.z, v4.w};
 #pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      float g = gg[j] * scale;
-      if (!decoupled) g += wd * pp[j];
-      mm[j] = b1 * mm[j] + (1.0f - b1) * g;
-      vv[j] = b2 * vv[j] + (1.0f - b2) * g * g;
-      float upd = (mm[j] / bc1) / (sqrtf(vv[j] / bc2) + eps);
-      if (decoupled) upd += wd * pp[j];
-      pp[j] -= lr * upd;
-    }
+    for (int j = 0; j < 4; ++j) adam_element(pp[j], mm[j], vv[j], gg[j], scale, lr, b1, b2, eps, wd, bc1, bc2, decoupled);
     reinterpret_cast<float4*>(master)[i] = make_float4(pp[0], pp[1], pp[2], pp[3]);
     reinterpret_cast<float4*>(m)[i] = make_float4(mm[0], mm[1], mm[2], mm[3]);
     reinterpret_cast<float4*>(v)[i] = make_float4(vv[0], vv[1], vv[2], vv[3]);
     if (lp_out != nullptr) {
-      reinterpret_cast<uint2*>(lp_out)[i] = make_uint2(pack_bf16(pp[0], pp[1]), pack_bf16(pp[2], pp[3]));
+      reinterpret_cast<uint2*>(lp_out)[i] = make_uint2(pack_lp<LP>(pp[0], pp[1]), pack_lp<LP>(pp[2], pp[3]));
     }
   }
 }
@@ -713,13 +718,18 @@ extern "C" int lb_ce_bwd(const void* logits, const int64_t* labels, const float*
                                                vocab_start);
   return (int)cudaGetLastError();
 }
-extern "C" int lb_adamw(float* master, const float* grad, float* m, float* v, void* lp_out, const float* scale,
-                        long n, float lr, float b1, float b2, float eps, float wd, float bc1, float bc2, int decoupled,
-                        cudaStream_t s) {
+// lp_dtype: 0 = bf16, 1 = fp16 (the type of lp_out, when given)
+extern "C" int lb_adamw(float* master, const float* grad, float* m, float* v, void* lp_out, int lp_dtype,
+                        const float* scale, long n, float lr, float b1, float b2, float eps, float wd, float bc1,
+                        float bc2, int decoupled, cudaStream_t s) {
   if (n % 4) return -1;
   if (n == 0) return 0;
-  lb::adamw_kernel<<<ew_grid(n / 4, 256), 256, 0, s>>>(master, grad, m, v, (bf16*)lp_out, scale, (size_t)n, lr, b1, b2,
-                                                       eps, wd, bc1, bc2, decoupled);
+  if (lp_dtype == 1)
+    lb::adamw_kernel<__half><<<ew_grid(n / 4, 256), 256, 0, s>>>(master, grad, m, v, (__half*)lp_out, scale, (size_t)n,
+                                                                 lr, b1, b2, eps, wd, bc1, bc2, decoupled);
+  else
+    lb::adamw_kernel<bf16><<<ew_grid(n / 4, 256), 256, 0, s>>>(master, grad, m, v, (bf16*)lp_out, scale, (size_t)n, lr,
+                                                               b1, b2, eps, wd, bc1, bc2, decoupled);
   return (int)cudaGetLastError();
 }
 extern "C" int lb_embedding_fwd(const int64_t* ids, const void* table, void* out, long T, int H, long vocab_start, long rows,
@@ -778,7 +788,8 @@ __global__ void quant_e4m3_kernel(const uint4* __restrict__ x, long n8, const __
                                   const unsigned* __restrict__ amax_bits, uint2* __restrict__ q, uint8_t* __restrict__ qtail,
                                   float* __restrict__ deq) {
   const float amax = fmaxf(__uint_as_float(*amax_bits), 1e-12f);
-  const float scale = 448.0f / amax;
+  // correctly rounded: under --use_fast_math a plain `/` is div.approx, which returns 0 for amax > 2^126
+  const float scale = __fdiv_rn(448.0f, amax);
   if (blockIdx.x == 0 && threadIdx.x == 0) deq[0] = amax / 448.0f;
   for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < n8; i += (long)gridDim.x * blockDim.x) {
     const uint4 v = x[i];

@@ -921,19 +921,18 @@ extern "C" int lb_gemm_bf16(const void* a, const void* b, void* out, int M, int 
 
 // fp8 forward GEMM: y[M,N] (bf16) = act((xq[M,K] · wq[N,K]ᵀ) * deq_x * deq_w + bias); xq / wq hold E4M3 bytes, K % 16 == 0.
 // The operands are handed to the kernel as bf16 matrices with K/2 columns (identical bytes, see GemmParams::fp8).
-// With `residual` ([M, N] bf16) the epilogue is bias + residual add instead of an activation.
+// With `residual` ([M, N] bf16) the epilogue is bias + residual add instead of an activation, and neither an activation
+// nor a pre-activation copy may be asked for.  force_bn: tile width 64 / 128 / 192 / 256, or 0 for the heuristic.
 extern "C" int lb_gemm_fp8(const void* xq, const void* wq, void* out, int M, int N, int K, const void* bias, int act,
-                           void* pre_out, const void* residual, const float* deq_x, const float* deq_w,
+                           void* pre_out, const void* residual, const float* deq_x, const float* deq_w, int force_bn,
                            cudaStream_t stream) {
   if ((K % 16) != 0 || deq_x == nullptr || deq_w == nullptr) return -7;
+  if (residual != nullptr && (act != lb::ACT_NONE || pre_out != nullptr)) return -7;
   lb::CommParams cp;
   memset(&cp, 0, sizeof(cp));
-  if (residual != nullptr) {
-    act = lb::ACT_RESADD;
-    pre_out = nullptr;
-  }
-  return gemm_impl(xq, wq, out, M, N, K / 2, K / 2, K / 2, N, 0, 0, bias, act, pre_out, residual, 0, 0, cp, stream, deq_x,
-                   deq_w);
+  if (residual != nullptr) act = lb::ACT_RESADD;
+  return gemm_impl(xq, wq, out, M, N, K / 2, K / 2, K / 2, N, 0, 0, bias, act, pre_out, residual, force_bn, 0, cp, stream,
+                   deq_x, deq_w);
 }
 
 // dgrad fused with the activation backward: out[M,N] = (A·B) * act'(pre_in[M,N])   (bf16 output, ldo = row stride

@@ -494,7 +494,13 @@ class FlatOptimizer(torch.optim.Optimizer):
             if fg is None:
                 continue
             g = self.param_groups[gi]
-            scale = coef * self.grad_scale if coef is not None else None
+            # the gradient multiplier: clip coefficient times 1/loss-scale; without clipping the loss scale alone
+            if coef is not None:
+                scale = coef * self.grad_scale
+            elif self.grad_scale != 1.0:
+                scale = torch.full((), float(self.grad_scale), dtype=torch.float32, device=fg.device)
+            else:
+                scale = None
             if fg.symm is not None and hasattr(self, "_fused_zero_update"):
                 self._fused_zero_update(g, fg, self._step_count, scale)
                 continue

@@ -106,18 +106,20 @@ def gemm_operands(a, b, layout):
     return a.t(), b.t()
 
 
-def check_gemm(out, A, B, what, *, bias=None, act=0, pre=None, residual=None, base=None, dpre=None, chunk=1024):
+def check_gemm(out, A, B, what, *, bias=None, act=0, pre=None, residual=None, base=None, dpre=None, chunk=1024,
+               acc_bound=None):
     """``out`` against ``A @ B^T`` in fp64, in row chunks of ``chunk``.
 
     ``bias`` [N] and ``act`` apply the epilogue act(acc + bias); ``pre`` is then the bf16 copy of acc + bias.
     ``residual`` [M, N]: out = acc + bias + residual.  ``base`` [M, N]: out = base + acc (fp32 accumulation; base is the
-    content of the buffer before the call).  ``dpre`` [M, N]: out = acc * act'(dpre)."""
+    content of the buffer before the call).  ``dpre`` [M, N]: out = acc * act'(dpre).  ``acc_bound``: a function of the
+    row slice giving the accumulation error bound of those rows, for accumulators that are not fp32."""
     M, K = A.shape
     for r0 in range(0, M, chunk):
         a = A[r0:r0 + chunk].double()
         acc = a @ B.double().t()
-        kterm = K * ACC * (a.abs() @ B.double().abs().t())
         rows = slice(r0, r0 + chunk)
+        kterm = K * ACC * (a.abs() @ B.double().abs().t()) if acc_bound is None else acc_bound(rows)
         v, vbound = acc, kterm
         if bias is not None:
             v = v + bias.double()

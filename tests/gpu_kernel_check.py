@@ -303,8 +303,9 @@ def main():
     record("embedding gather / scatter-add", embedding_native)
 
     def fp8_forward_gemm():
-        """E4M3 forward GEMM (wgmma e4m3): exact against an fp32 matmul of the *dequantised* operands (the
-        only error left is the bf16 rounding of the output), close to the bf16 GEMM, plus quantiser checks and timing."""
+        """E4M3 forward GEMM (wgmma e4m3): close to an fp32 matmul of the *dequantised* operands (the errors left are
+        the fp8 accumulator, which keeps about 12-13 bits rather than fp32's 24 (dev/measure_fp8_acc.py), and the bf16
+        rounding of the output), close to the bf16 GEMM, plus quantiser checks and timing."""
         e = {}
         x = torch.randn(777, 1040, device="cuda").bfloat16() * 3
         xq, dx = ext.quantize_e4m3(x)
@@ -338,8 +339,8 @@ def main():
                 msq = timeit(lambda: ext.quantize_e4m3(x))
                 res[f"{M}x{N}x{K}"] = {"fp8_ms": ms8, "fp8_pflops": flops / ms8 / 1e12, "bf16_ms": ms16,
                                        "bf16_pflops": flops / ms16 / 1e12, "quantize_x_ms": msq}
-        exact = [v for k, v in e.items() if "x" in k and "vs_bf16" not in k and not k.startswith("quant")]
-        ok = (max(exact) < 1e-2 and e["deq_scale"] < 1e-5 and e["quant_vs_torch"] < 1e-6 and e["quant_tail"] < 1e-6
+        vs_dequant = [v for k, v in e.items() if "x" in k and "vs_bf16" not in k and not k.startswith("quant")]
+        ok = (max(vs_dequant) < 1e-2 and e["deq_scale"] < 1e-5 and e["quant_vs_torch"] < 1e-6 and e["quant_tail"] < 1e-6
               and e["quant_roundtrip"] < 0.06 and all(v < 0.08 for k, v in e.items() if "vs_bf16" in k))
         return {"ok": ok, "errs": e, "timing": res}
 
