@@ -1,4 +1,9 @@
-// Flash attention for sm_90a on wgmma / TMA / mbarrier (head dim 64 or 128, causal or full, bf16).
+// Flash attention for sm_90a on wgmma / TMA / mbarrier (bf16, causal or full, head dim d a multiple of 8 in [8, 128]).
+//
+// Head dim: d runs on a tile of D = 64 (d <= 64) or D = 128 (64 < d <= 128) columns.  The Q/K/V/dO tensor maps have
+// d columns, so TMA fills columns d .. D of every 64-column box with zeros (the transaction byte counts stay at the full
+// box): the padded columns add nothing to S = Q·Kᵀ or dPᵀ = V·dOᵀ and stay zero in the O, dK, dV and dQ accumulators.
+// Every store stops at column d: in the packed projections the columns past a q slot's d are the k slot of the head.
 //
 // Replaces the score GEMM + fused_scale_(tril_)softmax(_mask)_dropout + context GEMM sequence of the
 // reference (libai/layers/attention.py:211-253): no [b, a, s, s] tensor and no materialised mask.
@@ -36,9 +41,10 @@ constexpr int ATT_BWD_BM = 64;   // queries per step (backward)
 constexpr int ATT_BWD_THREADS = 160;
 
 struct AttnFwdParams {
-  __nv_bfloat16* o;   // [B, Sq, A, D]
+  __nv_bfloat16* o;   // [B, Sq, A, d]
   float* lse;         // [B, A, Sq]
   int B, A, Sq, Sk;
+  int d;              // head dim (d <= D, a multiple of 8)
   int r;              // query heads per K/V head
   int causal;
   float scale_log2;   // scale * log2(e)
@@ -75,6 +81,12 @@ LB_DEVICE void acc_to_a_frag(const float* d, uint32_t (&a)[4]) {
   a[1] = pack_bf16(d[2], d[3]);
   a[2] = pack_bf16(d[4], d[5]);
   a[3] = pack_bf16(d[6], d[7]);
+}
+// column c (a compile-time constant in the unrolled store loops) of a D-wide tile lies inside head dim d; the 128-wide
+// tile runs d > 64 only, so its first 64 columns need no run-time test
+template <int D>
+LB_DEVICE bool col_in_head(int c, int d) {
+  return (D == 128 && c < 64) || c < d;
 }
 
 template <int D>
@@ -309,7 +321,7 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
     mbar_arrive(&v_empty[b]);
   }
 
-  // ---- epilogue: O / l  →  [B, Sq, A, D]; lse in natural log (0 for a row without a visible key)
+  // ---- epilogue: O / l  →  [B, Sq, A, d]; lse in natural log (0 for a row without a visible key)
 #pragma unroll
   for (int h = 0; h < 2; ++h) {
     float l = l_run[h];
@@ -317,10 +329,11 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
     l += __shfl_xor_sync(0xffffffffu, l, 2);
     const float inv = l > 0.f ? (DROP ? p.inv_keep : 1.0f) / l : 0.f;
     if (q_idx[h] < p.Sq) {
-      __nv_bfloat16* orow = p.o + ((static_cast<size_t>(batch) * p.Sq + q_idx[h]) * p.A + head) * D;
+      __nv_bfloat16* orow = p.o + ((static_cast<size_t>(batch) * p.Sq + q_idx[h]) * p.A + head) * p.d;
 #pragma unroll
       for (int jj = 0; jj < D / 8; ++jj)
-        *reinterpret_cast<uint32_t*>(orow + 8 * jj + cq) = pack_bf16(o[4 * jj + 2 * h] * inv, o[4 * jj + 2 * h + 1] * inv);
+        if (col_in_head<D>(8 * jj, p.d))
+          *reinterpret_cast<uint32_t*>(orow + 8 * jj + cq) = pack_bf16(o[4 * jj + 2 * h] * inv, o[4 * jj + 2 * h + 1] * inv);
       if (t % 4 == 0)
         p.lse[(static_cast<size_t>(batch) * p.A + head) * p.Sq + q_idx[h]] =
             (m_run[h] == -INFINITY) ? 0.f : (m_run[h] + log2f(l)) * 0.6931471805599453f;
@@ -331,14 +344,20 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
 }  // namespace lb
 
 namespace {
-// dims innermost first: {D, S, A, B}; st = {batch, head, seq} strides in elements; boxes of 64 columns x `rows` rows
+// the tile width a head dim runs on: 64 or 128, 0 for an unsupported head dim
+int head_dim_tile(int d) {
+  if (d % 8 || d < 8 || d > 128) return 0;
+  return d <= 64 ? 64 : 128;
+}
+// dims innermost first: {d, S, A, B}; st = {batch, head, seq} strides in elements; boxes of 64 columns x `rows` rows
+// (columns past d are zero-filled)
 bool make_qkv_tmap(CUtensorMap* m, const void* ptr, int B, int A, int S, int D, const long* st, int rows) {
   uint64_t dims[4] = {(uint64_t)D, (uint64_t)S, (uint64_t)A, (uint64_t)B};
   uint64_t strides[4] = {2, (uint64_t)st[2] * 2, (uint64_t)st[1] * 2, (uint64_t)st[0] * 2};
   uint32_t box[4] = {64, (uint32_t)rows, 1, 1};
   return lb_host::make_tmap_bf16(m, ptr, 4, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B);
 }
-// query-head tensors of grouped-query attention, dims innermost first {D, S, r, G, B}; st = {batch, group, in-group,
+// query-head tensors of grouped-query attention, dims innermost first {d, S, r, G, B}; st = {batch, group, in-group,
 // seq} strides in elements
 bool make_q_tmap(CUtensorMap* m, const void* ptr, int B, int G, int r, int S, int D, const long* st, int rows) {
   uint64_t dims[5] = {(uint64_t)D, (uint64_t)S, (uint64_t)r, (uint64_t)G, (uint64_t)B};
@@ -373,9 +392,9 @@ cudaError_t launch_fwd(const CUtensorMap& tq, const CUtensorMap& tk, const CUten
   return drop ? launch_fwd_t<D, lb::BIAS_ALIBI, true>(tq, tk, tv, p, s) : launch_fwd_t<D, lb::BIAS_ALIBI, false>(tq, tk, tv, p, s);
 }
 }  // namespace
-// A query heads in G groups (A % G == 0); Sq queries, Sk keys; q_strides = {batch, group, in-group, seq}, k/v_strides =
-// {batch, head, seq} over the G K/V heads (elements).  kv_lens / kv_start (optional, int32 [B], device): per-sample key
-// window.
+// A query heads in G groups (A % G == 0); Sq queries, Sk keys; head dim D a multiple of 8 in [8, 128]; q_strides =
+// {batch, group, in-group, seq}, k/v_strides = {batch, head, seq} over the G K/V heads (elements).  kv_lens / kv_start
+// (optional, int32 [B], device): per-sample key window.
 // p_drop in [0, 1): attention dropout probability (quantised to 1/256 like the byte-threshold test of the kernel);
 // bias (optional, bf16): dense additive score bias with (batch, head, query-row) strides in elements, key stride 1;
 // alibi_slopes (optional, fp32 [A]).
@@ -383,7 +402,8 @@ extern "C" int lb_attn_fwd(const void* q, const void* k, const void* v, void* o,
                            int Sk, int D, const long* q_strides, const long* k_strides, const long* v_strides, int causal,
                            float scale, const int* kv_lens, const int* kv_start, const void* bias, const long* bias_strides,
                            const float* alibi_slopes, float p_drop, const lb::RngArgs* rng, long long* rng_out, cudaStream_t s) {
-  if (D != 64 && D != 128) return -1;
+  const int tile = head_dim_tile(D);
+  if (tile == 0) return -1;
   if (Sq <= 0 || Sk <= 0) return -5;
   if (G <= 0 || A % G) return -4;
   for (int i = 0; i < 3; ++i)
@@ -401,6 +421,7 @@ extern "C" int lb_attn_fwd(const void* q, const void* k, const void* v, void* o,
   p.r = A / G;
   p.Sq = Sq;
   p.Sk = Sk;
+  p.d = D;
   p.causal = causal;
   p.scale = scale;
   p.scale_log2 = scale * 1.4426950408889634f;
@@ -418,7 +439,7 @@ extern "C" int lb_attn_fwd(const void* q, const void* k, const void* v, void* o,
   memset(&p.rng, 0, sizeof(p.rng));
   if (rng != nullptr) p.rng = *rng;
   p.rng_out = rng_out;
-  cudaError_t e = (D == 64) ? launch_fwd<64>(tq, tk, tv, p, s) : launch_fwd<128>(tq, tk, tv, p, s);
+  cudaError_t e = (tile == 64) ? launch_fwd<64>(tq, tk, tv, p, s) : launch_fwd<128>(tq, tk, tv, p, s);
   return (int)e;
 }
 // =================================================================================================
@@ -457,11 +478,12 @@ struct AttnBwdCfg {
 struct AttnBwdParams {
   const float* lse;     // [B, A, Sq]
   const float* delta;   // [B, A, Sq]
-  float* dq_accum;      // [B, A, Sq, D] fp32
-  __nv_bfloat16* dk;    // strided [B, G, Sk, D] views
+  float* dq_accum;      // [B, A, Sq, d] fp32
+  __nv_bfloat16* dk;    // strided [B, G, Sk, d] views
   __nv_bfloat16* dv;
   long g_strides[3];    // batch, head, seq strides (elements) of dk / dv
   int B, A, Sq, Sk;
+  int d;                // head dim (d <= D, a multiple of 8)
   int r;                // query heads per K/V head (G = A / r)
   int causal;
   float scale, scale_log2;
@@ -702,12 +724,13 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
       for (int h = 0; h < 2; ++h) {
         const int q_idx = q0 + r_loc + 8 * h;
         if (q_idx < p.Sq) {
-          float* dq_row = p.dq_accum + (bh * p.Sq + q_idx) * D + n * 64;
+          float* dq_row = p.dq_accum + (bh * p.Sq + q_idx) * p.d + n * 64;
 #pragma unroll
           for (int jj = 0; jj < 8; ++jj)
-            asm volatile("red.global.add.v2.f32 [%0], {%1, %2};\n" ::"l"(dq_row + 8 * jj + cq), "f"(dq[4 * jj + 2 * h]),
-                         "f"(dq[4 * jj + 2 * h + 1])
-                         : "memory");
+            if (col_in_head<D>(n * 64 + 8 * jj, p.d))
+              asm volatile("red.global.add.v2.f32 [%0], {%1, %2};\n" ::"l"(dq_row + 8 * jj + cq), "f"(dq[4 * jj + 2 * h]),
+                           "f"(dq[4 * jj + 2 * h + 1])
+                           : "memory");
         }
       }
     }
@@ -727,19 +750,20 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
     const long off = batch * p.g_strides[0] + kv_head * p.g_strides[1] + static_cast<long>(k_idx) * p.g_strides[2];
 #pragma unroll
     for (int jj = 0; jj < D / 8; ++jj) {
+      if (!col_in_head<D>(8 * jj, p.d)) continue;
       *reinterpret_cast<uint32_t*>(p.dv + off + 8 * jj + cq) = pack_bf16(dv[4 * jj + 2 * h], dv[4 * jj + 2 * h + 1]);
       *reinterpret_cast<uint32_t*>(p.dk + off + 8 * jj + cq) = pack_bf16(dk[4 * jj + 2 * h], dk[4 * jj + 2 * h + 1]);
     }
   }
 }
 
-// delta[b, a, s] = sum_d dO[b, a, s, d] * O[b, a, s, d]
-// D / 8 lanes per row, 16-byte loads; rows are visited in (b, s, a) order = memory order of the [b, s, a, d] tensors, so
-// a warp reads 32 x 16 contiguous bytes per tensor, and every thread keeps 4 rows (8 loads) in flight.
+// delta[b, a, s] = sum_d dO[b, a, s, d] * O[b, a, s, d] over the head dim d <= D
+// D / 8 lanes per row (lanes past d add zeros), 16-byte loads; rows are visited in (b, s, a) order = memory order of the
+// [b, s, a, d] tensors, so a warp reads contiguous bytes per tensor, and every thread keeps 4 rows (8 loads) in flight.
 template <int D>
 __global__ void __launch_bounds__(256)
 attn_delta_kernel(const __nv_bfloat16* __restrict__ dout, const __nv_bfloat16* __restrict__ o, float* __restrict__ delta,
-                  int B, int A, int S, long sb, long sa, long ss, float4* __restrict__ zero_fill, long zero_n4) {
+                  int B, int A, int S, int d, long sb, long sa, long ss, float4* __restrict__ zero_fill, long zero_n4) {
   constexpr int LPR = D / 8;  // lanes per row
   const long total = static_cast<long>(B) * A * S;
   const long gid = blockIdx.x * static_cast<long>(blockDim.x) + threadIdx.x;
@@ -747,6 +771,7 @@ attn_delta_kernel(const __nv_bfloat16* __restrict__ dout, const __nv_bfloat16* _
   for (long z = gid; z < zero_n4; z += static_cast<long>(gridDim.x) * blockDim.x) zero_fill[z] = make_float4(0.f, 0.f, 0.f, 0.f);
   const long gstride = static_cast<long>(gridDim.x) * blockDim.x / LPR;
   const int sub = static_cast<int>(gid % LPR);
+  const bool col_ok = sub * 8 < d;
   const long warp_r0 = (gid - (threadIdx.x % 32)) / LPR;  // loop bound is warp-uniform (the shuffles below need all lanes)
   for (long base = 0; warp_r0 + base < total; base += 4 * gstride) {
     const long r0 = gid / LPR + base;
@@ -761,8 +786,8 @@ attn_delta_kernel(const __nv_bfloat16* __restrict__ dout, const __nv_bfloat16* _
       const long b = rr / (static_cast<long>(A) * S);
       const long off = b * sb + a * sa + sq * ss + sub * 8;
       drow[u] = ok ? (b * A + a) * static_cast<long>(S) + sq : -1;
-      x[u] = ok ? *reinterpret_cast<const uint4*>(dout + off) : make_uint4(0, 0, 0, 0);
-      y[u] = ok ? *reinterpret_cast<const uint4*>(o + off) : make_uint4(0, 0, 0, 0);
+      x[u] = ok && col_ok ? *reinterpret_cast<const uint4*>(dout + off) : make_uint4(0, 0, 0, 0);
+      y[u] = ok && col_ok ? *reinterpret_cast<const uint4*>(o + off) : make_uint4(0, 0, 0, 0);
     }
 #pragma unroll
     for (int u = 0; u < 4; ++u) {
@@ -858,7 +883,8 @@ extern "C" int lb_attn_bwd(const void* dout, const void* q, const void* k, const
                            const int* kv_lens, const int* kv_start, const void* bias, const long* bias_strides,
                            const float* alibi_slopes, float* dbias, float p_drop, const long long* rng_state,
                            unsigned* dq_order, cudaStream_t s) {
-  if (D != 64 && D != 128) return -1;
+  const int tile = head_dim_tile(D);
+  if (tile == 0) return -1;
   if (Sq <= 0 || Sk <= 0) return -5;
   if (G <= 0 || A % G) return -4;
   const int r = A / G;
@@ -875,16 +901,16 @@ extern "C" int lb_attn_bwd(const void* dout, const void* q, const void* k, const
   {
     // 4 rows per thread-group and iteration; cap the grid at a few waves
     const long groups = (rows + 3) / 4;
-    const long lpr = D / 8;
+    const long lpr = tile / 8;
     long blocks = (groups * lpr + 255) / 256;
     if (blocks > sm_count() * 16L) blocks = sm_count() * 16L;
-    if (D == 64)
+    if (tile == 64)
       lb::attn_delta_kernel<64><<<(unsigned)blocks, 256, 0, s>>>((const __nv_bfloat16*)dout, (const __nv_bfloat16*)o, delta, B,
-                                                                   A, Sq, do_strides[0], do_strides[1], do_strides[2],
+                                                                   A, Sq, D, do_strides[0], do_strides[1], do_strides[2],
                                                                    reinterpret_cast<float4*>(dq_accum), rows * D / 4);
     else
       lb::attn_delta_kernel<128><<<(unsigned)blocks, 256, 0, s>>>((const __nv_bfloat16*)dout, (const __nv_bfloat16*)o, delta, B,
-                                                                    A, Sq, do_strides[0], do_strides[1], do_strides[2],
+                                                                    A, Sq, D, do_strides[0], do_strides[1], do_strides[2],
                                                                     reinterpret_cast<float4*>(dq_accum), rows * D / 4);
   }
   lb::AttnBwdParams p;
@@ -899,6 +925,7 @@ extern "C" int lb_attn_bwd(const void* dout, const void* q, const void* k, const
   p.r = r;
   p.Sq = Sq;
   p.Sk = Sk;
+  p.d = D;
   p.causal = causal;
   p.scale = scale;
   p.scale_log2 = scale * 1.4426950408889634f;
@@ -915,7 +942,7 @@ extern "C" int lb_attn_bwd(const void* dout, const void* q, const void* k, const
   p.rng_state = rng_state;
   p.dq_order = dq_order;
   p.timeout_rec = lb_host::spin_timeout_record(s);
-  cudaError_t e = (D == 64) ? launch_bwd<64>(tq, tk, tv, tdo, p, s) : launch_bwd<128>(tq, tk, tv, tdo, p, s);
+  cudaError_t e = (tile == 64) ? launch_bwd<64>(tq, tk, tv, tdo, p, s) : launch_bwd<128>(tq, tk, tv, tdo, p, s);
   if (e != cudaSuccess) return (int)e;
   const long nvec = rows * D / 8;
   int blocks = (int)((nvec + 511) / 512);

@@ -680,9 +680,10 @@ std::tuple<Tensor, Tensor> bias_dropout_residual(const Tensor& x, const c10::opt
 
 // ---- attention ----------------------------------------------------------------------------------------------
 // q: [B, A, Sq, D] or, grouped, [B, G, r, Sq, D]; k, v: [B, G, Sk, D] with A = G * r (grouped-query attention: query
-// head h reads K/V head h / r); views with arbitrary batch/head/seq strides (D contiguous).  Output o is allocated as
-// [B, Sq, A, D] and returned as the [B, A, Sq, D] view, lse fp32 [B, A, Sq].  Key j is visible to query i of sample b
-// iff kv_start[b] <= j < kv_lens[b] (defaults 0 and Sk) and, when causal, j <= i + Sk - Sq.
+// head h reads K/V head h / r) and head dim D a multiple of 8 in [8, 128]; views with arbitrary batch/head/seq strides
+// (D contiguous).  Output o is allocated as [B, Sq, A, D] and returned as the [B, A, Sq, D] view, lse fp32 [B, A, Sq].
+// Key j is visible to query i of sample b iff kv_start[b] <= j < kv_lens[b] (defaults 0 and Sk) and, when causal,
+// j <= i + Sk - Sq.
 struct BiasDesc {
   const void* ptr = nullptr;
   long strides[3] = {0, 0, 0};
@@ -735,6 +736,7 @@ QGeom q_geom(const Tensor& q, const Tensor& k, const Tensor& v, const char* what
     g.qs[3] = q.stride(3);
   }
   TORCH_CHECK(k.size(0) == g.B && k.size(3) == g.D, what, ": k, v do not match q");
+  TORCH_CHECK(g.D % 8 == 0 && g.D >= 8 && g.D <= 128, what, ": head dim must be a multiple of 8 in [8, 128], got ", g.D);
   TORCH_CHECK(g.Sq >= 1 && g.Sk >= 1, what, ": empty query or key sequence");
   return g;
 }

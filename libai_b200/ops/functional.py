@@ -685,12 +685,20 @@ class _FlashAttnPackedFn(torch.autograd.Function):
         return dqkv.view(qkv.shape), None, None, None, None, None
 
 
+def flash_head_dim_supported(d: int) -> bool:
+    """True for the head dims the flash kernels take: multiples of 8 from 8 to 128 (a head dim up to 64 runs on the
+    64-wide tile, a larger one on the 128-wide tile, with the columns past ``d`` zero-filled)."""
+    return d % 8 == 0 and 8 <= d <= 128
+
+
 def attention_qkvpacked_supported(qkv, mask, dropout_p, training) -> bool:
+    """True when :func:`attention_qkvpacked` runs the native flash kernels: a contiguous bf16 projection on the GPU
+    whose head dim :func:`flash_head_dim_supported` accepts, and no dense ``mask``."""
     return (
         use_native(qkv)
         and qkv.dtype == torch.bfloat16
         and mask is None
-        and packed_head_dim(qkv) in (64, 128)
+        and flash_head_dim_supported(packed_head_dim(qkv))
         and qkv.is_contiguous()
     )
 
@@ -705,14 +713,15 @@ def attention_qkvpacked(qkv, *, causal: bool, scale: float, kv_lens=None, dropou
 
 
 def attention_supported(q, k, mask=None, bias=None) -> bool:
-    """True when :func:`attention` of ``q`` over ``k`` runs the native flash kernels: bf16 on the GPU, head dim 64 or
-    128, no dense 0/1 ``mask`` and a dense ``bias`` (if any) of shape ``[.., sq, sk]``.  Query and key lengths are free.
-    Otherwise :func:`attention` runs the reference math."""
+    """True when :func:`attention` of ``q`` over ``k`` runs the native flash kernels: bf16 on the GPU, a head dim
+    :func:`flash_head_dim_supported` accepts (a multiple of 8 from 8 to 128), no dense 0/1 ``mask`` and a dense
+    ``bias`` (if any) of shape ``[.., sq, sk]``.  Query and key lengths are free.  Otherwise :func:`attention` runs the
+    reference math."""
     return (
         use_native(q)
         and q.dtype == torch.bfloat16
         and mask is None
-        and q.shape[-1] in (64, 128)
+        and flash_head_dim_supported(q.shape[-1])
         and (bias is None or (bias.shape[-1] == k.shape[-2] and bias.shape[-2] == q.shape[-2]))
     )
 
