@@ -1,6 +1,11 @@
 """Tile-N sweep of every GEMM of the benchmark model's training step (GPT-2 medium, micro-batch 8 x 1024 tokens): does
 the heuristic of gemm_sm90.cu (bn = 0) pick the fastest tile, and how far is each shape from cuBLAS?
 
+For the NT and NN layouts `pingpong` is the ping-pong kernel (128 x 128 tiles, what the dispatch runs for bf16 outputs)
+and `bn*` the 288-thread kernel at each width, forced with `gemm_schedule(1)`.  `epilogues` times the fused epilogues
+the step runs at K = 1024 (fc1 forward with bias + GELU + pre-activation copy, attention-out and fc2 forward with bias
++ residual, the fc2 dgrad fused with GELU') with both kernels.
+
 Shapes: forward NT and dgrad NN of the four transformer linears, their wgrad TN with the fp32 `red.add` epilogue into
 a main_grad buffer, and the LM head's forward, dgrad and wgrad.  Prints one JSON line: per shape the median time (ms)
 and TFLOP/s (2·M·N·K over time) of each tile width and of torch.matmul (cuBLAS) on the same operands.  The forced tile
@@ -64,11 +69,15 @@ def main():
         if layout == 2:
             main_grad = torch.zeros(M, N, device="cuda")
             record("bn0", timeit(lambda: ext.gemm(a, b, 2, None, main_grad, True, torch.float32)))
+        if layout != 2:
+            record("pingpong", timeit(lambda: ext.gemm_tuned(a, b, layout, 128, 1, False)))
+        prev = ext.gemm_schedule(1)
         for bn in (0, 64, 128, 192, 256) if layout != 2 else (64, 128, 192, 256):
             try:
                 record(f"bn{bn}", timeit(lambda: ext.gemm_tuned(a, b, layout, bn, 0 if layout == 2 else 1, False)))
             except Exception as e:  # noqa: BLE001
                 res[f"bn{bn}"] = f"{type(e).__name__}"
+        ext.gemm_schedule(prev)
         if layout == 0:
             record("cublas", timeit(lambda: torch.matmul(a, b.t())))
         elif layout == 1:
@@ -78,7 +87,33 @@ def main():
         out[name] = res
         del a, b
         torch.cuda.empty_cache()
+    out["epilogues"] = epilogues(ext)
     print(json.dumps(out))
+
+
+def epilogues(ext):
+    x, x4 = torch.randn(T, H, device="cuda").bfloat16(), torch.randn(T, FFN, device="cuda").bfloat16()
+    w_fc1, w_proj = torch.randn(FFN, H, device="cuda").bfloat16(), torch.randn(H, H, device="cuda").bfloat16()
+    w_fc2 = torch.randn(H, FFN, device="cuda").bfloat16()
+    b_fc1, b_h = torch.randn(FFN, device="cuda").bfloat16(), torch.randn(H, device="cuda").bfloat16()
+    res, gy = torch.randn(T, H, device="cuda").bfloat16(), torch.randn(T, H, device="cuda").bfloat16()
+    cases = {
+        "fwd_fc1_bias_gelu_pre": ([T, FFN, H], lambda: ext.linear_fwd(x, w_fc1, b_fc1, 1, True)),
+        "fwd_proj_bias_residual": ([T, H, H], lambda: ext.linear_bias_residual(x, w_proj, b_h, res)),
+        "fwd_fc2_bias_residual": ([T, H, FFN], lambda: ext.linear_bias_residual(x4, w_fc2, b_h, res)),
+        "dgrad_fc2_gelu_grad": ([T, FFN, H], lambda: ext.dgrad_actgrad(gy, w_fc2, x4, 1, None)),
+    }
+    out = {}
+    for name, ((M, N, K), fn) in cases.items():
+        flop = 2.0 * M * N * K
+        res_ = {"shape": [M, N, K]}
+        for key, schedule in (("pingpong", 0), ("old", 1)):
+            prev = ext.gemm_schedule(schedule)
+            ms = timeit(fn)
+            ext.gemm_schedule(prev)
+            res_[key] = {"ms": round(ms, 4), "tflops": round(flop / (ms * 1e-3) / 1e12, 1)}
+        out[name] = res_
+    return out
 
 
 if __name__ == "__main__":

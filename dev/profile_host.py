@@ -30,6 +30,9 @@ def kernel_class(name: str) -> str:
     m = re.search(r"gemm_kernel<\d+, (true|false), (true|false), \d+, (true|false)>", name)
     if m:
         return ("fp8 " if m.group(3) == "true" else "") + "gemm " + _GEMM_LAYOUT[(m.group(1), m.group(2))]
+    m = re.search(r"gemm_pingpong_kernel<(true|false)>", name)
+    if m:
+        return "gemm " + _GEMM_LAYOUT[("false", m.group(1))]
     if "attn_fwd" in name:
         return "attention fwd"
     if "attn_" in name:          # attn_bwd_kernel and its delta / dQ-convert kernels

@@ -14,6 +14,7 @@
 extern "C" {
 int lb_gemm_bf16(const void* a, const void* b, void* out, int M, int N, int K, int lda, int ldb, int ldo, int layout,
                  int epi, const void* bias, int act, void* pre_out, int force_bn, int force_splits, cudaStream_t s);
+int lb_gemm_set_schedule(int schedule);
 int lb_norm_fwd(const void* x, const void* gamma, const void* beta, void* y, float* mean, float* rstd, int rows, int H,
                 float eps, int rms, int dtype, int wdtype, cudaStream_t s);
 int lb_gemm_bf16_bias_residual(const void* x, const void* w, void* out, int M, int N, int K, int lda, int ldb,
@@ -306,6 +307,13 @@ Tensor gemm_tuned(const Tensor& a, const Tensor& b, int64_t layout, int64_t bn, 
                      cur_stream()),
         "gemm_tuned");
   return out;
+}
+
+// GEMM schedule of later calls, for comparing the kernels in one process: 0 = automatic (the ping-pong kernel for bf16
+// outputs of NT / NN GEMMs with a 128-wide or heuristic tile), 1 = the 288-thread kernel only.  Returns the previous one.
+int64_t gemm_schedule(int64_t schedule) {
+  TORCH_CHECK(schedule == 0 || schedule == 1, "gemm_schedule: 0 (automatic) or 1 (288-thread kernel only)");
+  return lb_gemm_set_schedule((int)schedule);
 }
 
 // gx = gy * act'(pre)
@@ -1065,6 +1073,7 @@ TORCH_LIBRARY(libai_b200, m) {
   m.def("embedding_fwd(Tensor ids, Tensor table, int vocab_start) -> Tensor", &embedding_fwd);
   m.def("embedding_bwd(Tensor ids, Tensor gy, Tensor(a!) grad, int vocab_start) -> ()", &embedding_bwd);
   m.def("gemm_tuned(Tensor a, Tensor b, int layout, int bn, int splits, bool fp32_out) -> Tensor", &gemm_tuned);
+  m.def("gemm_schedule(int schedule) -> int", &gemm_schedule);
   m.def("linear_fwd(Tensor x, Tensor w, Tensor? bias, int act, bool need_pre) -> (Tensor, Tensor)", &linear_fwd);
   m.def("quantize_e4m3(Tensor x) -> (Tensor, Tensor)", &quantize_e4m3);
   m.def("linear_fp8_fwd(Tensor xq, Tensor wq, Tensor deq_x, Tensor deq_w, Tensor? bias, int act, bool need_pre, Tensor? residual=None, int bn=0) -> (Tensor, Tensor)", &linear_fp8_fwd);

@@ -12,10 +12,14 @@
 // Warp roles (288 threads): warps 0..7 = two consumer warpgroups (rows [0, 64) and [64, 128) of the 128-row tile; each
 // issues m64nBLOCK_Nk16 wgmma over the shared stage and runs the epilogue of its rows), warp 8 = TMA producer.  One CTA
 // per SM, static round-robin tile scheduler over (m_blk, n_blk, k_split).
+//
+// The bf16-output NT / NN GEMMs without a collective run gemm_pingpong_kernel below instead (384 threads, whole tiles
+// per consumer warpgroup, TMA-store epilogue); gemm_impl decides which kernel a call takes.
 #include "common.cuh"
 
 #include <cstdio>
 #include <cstdlib>
+#include <atomic>
 #include <cstring>
 #include <mutex>
 
@@ -596,6 +600,286 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
   }
 }
 
+// ---------------------------------------------------------------------------------------------------------------------
+// Ping-pong schedule for bf16 outputs (NT forward and NN dgrad, one K partition, no collective).
+//
+// Warp roles (384 threads): warpgroup 0 = TMA producer (one elected thread; registers lowered with setmaxnreg),
+// warpgroups 1 and 2 = consumers, each owning WHOLE 128 x 128 output tiles (two m64n128k16 wgmmas per k-step, 128 fp32
+// accumulators per thread).  The CTA's tiles cta + k * stride go to consumer k % 2.  Two named barriers hand the
+// tensor cores from one consumer to the other: consumer A's k-loop of tile k issues before consumer B's k-loop of
+// tile k + 1, and A's epilogue runs under B's k-loop.  With short K (1024: most forward and dgrad GEMMs of a
+// transformer) the epilogue of the 288-thread kernel above took as long as the main loop with the tensor cores idle.
+//
+// Epilogue: the bf16 tile goes through a per-consumer 32 KB shared staging buffer (two 64-column boxes, 128-byte
+// swizzle) and leaves with TMA stores, which clip at M and N.  The store completes while the consumer runs its next
+// k-loop; it waits for the read of the staging buffer only before the buffer is written again.  `pre_out` uses the same
+// buffer first.  `pre_in` (GELU' input, or the residual of ACT_RESADD) is loaded by the producer with TMA into the
+// staging buffer when the tile's k-loop starts, and each thread overwrites its own elements with the result.
+//
+// Numerics are those of gemm_kernel<.., EPI_BF16>: the same k-blocks in increasing order, the same wgmma k16 steps,
+// the same epilogue arithmetic and RNE rounding, so every output element is bit-identical.
+constexpr int PP_BLOCK_N = 128;
+constexpr int PP_THREADS = 384;
+constexpr int PP_STAGES = 5;
+constexpr int PP_STAGE_BYTES = (BLOCK_M + PP_BLOCK_N) * BLOCK_K * 2;       // 32 KB
+constexpr int PP_STAGING_BYTES = BLOCK_M * PP_BLOCK_N * 2;                 // 32 KB per consumer
+constexpr int PP_BOX_BYTES = BLOCK_M * 64 * 2;                             // one 64-column box of the staging tile
+constexpr int PP_SMEM_BYTES = PP_STAGES * PP_STAGE_BYTES + 2 * PP_STAGING_BYTES + 1024 /*align*/ + 256 /*barriers*/;
+static_assert(PP_SMEM_BYTES <= 227 * 1024, "ping-pong GEMM exceeds the shared memory of an SM");
+
+// named barriers: 1, 2 = warpgroup_sync of consumer 0 / 1; 3, 4 = "consumer 0 / 1 may issue its k-loop"
+LB_DEVICE void pp_order_wait(int c) { asm volatile("bar.sync %0, 256;\n" ::"r"(3 + c) : "memory"); }
+LB_DEVICE void pp_order_signal(int c) { asm volatile("bar.arrive %0, 256;\n" ::"r"(3 + c) : "memory"); }
+
+// last epilogue pass of the ping-pong kernel for one activation: act(acc) or acc * act'(pre_in) or acc + residual, in
+// the arithmetic of gemm_kernel's bf16 epilogue (act_fwd(GELU) is gelu_fast, act_grad(GELU) is gelu_grad_fast), packed
+// to bf16 into the staging tile.  `row0`: this thread's slot in row 16 * warp + r, column 0; r = lane / 4 is also the
+// row's swizzle phase.  With PRE_IN the slot holds the pre_in element on entry.
+template <int ACT, bool PRE_IN>
+LB_DEVICE void pp_finish(float (&acc)[2][PP_BLOCK_N / 2], uint32_t row0, int r) {
+#pragma unroll
+  for (int j = 0; j < PP_BLOCK_N / 8; ++j) {
+    const uint32_t col_off = (j / 8) * PP_BOX_BYTES + (((j % 8) ^ r) << 4);
+#pragma unroll
+    for (int hm = 0; hm < 2; ++hm)
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const uint32_t addr = row0 + (64 * hm + 8 * h) * 128 + col_off;
+        float v0 = acc[hm][4 * j + 2 * h], v1 = acc[hm][4 * j + 2 * h + 1];
+        if constexpr (PRE_IN) {
+          uint32_t u;
+          asm volatile("ld.shared.u32 %0, [%1];\n" : "=r"(u) : "r"(addr) : "memory");
+          const float2 a = unpack_bf16(u);
+          if constexpr (ACT == ACT_RESADD) {
+            v0 += a.x;
+            v1 += a.y;
+          } else {
+            v0 *= act_grad(a.x, ACT);
+            v1 *= act_grad(a.y, ACT);
+          }
+        } else if constexpr (ACT != ACT_NONE) {
+          v0 = act_fwd(v0, ACT);
+          v1 = act_fwd(v1, ACT);
+        }
+        asm volatile("st.shared.u32 [%0], %1;\n" ::"r"(addr), "r"(pack_bf16(v0, v1)) : "memory");
+      }
+  }
+}
+
+template <bool B_MN>
+__global__ void __launch_bounds__(PP_THREADS, 1)
+gemm_pingpong_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
+                     const __grid_constant__ CUtensorMap tmap_out, const __grid_constant__ CUtensorMap tmap_pre_out,
+                     const __grid_constant__ CUtensorMap tmap_pre_in, GemmParams p) {
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  uint8_t* staging = smem + PP_STAGES * PP_STAGE_BYTES;   // [2][PP_STAGING_BYTES]
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(staging + 2 * PP_STAGING_BYTES);
+  uint64_t* empty_bar = full_bar + PP_STAGES;
+  uint64_t* pre_full = empty_bar + PP_STAGES;    // [2] pre_in tile of consumer c landed in its staging buffer
+  uint64_t* stg_free = pre_full + 2;             // [2] consumer c's previous TMA store has read its staging buffer
+
+  const int m_blocks = (p.M + BLOCK_M - 1) / BLOCK_M;
+  const int n_blocks = (p.N + PP_BLOCK_N - 1) / PP_BLOCK_N;
+  const int k_blocks = (p.K + BLOCK_K - 1) / BLOCK_K;
+  const int num_tiles = m_blocks * n_blocks;
+  const int cta = blockIdx.x, cta_stride = gridDim.x;
+  const bool use_pre = p.pre_in != nullptr;
+
+  if (threadIdx.x == 0) {
+    tma_prefetch_desc(&tmap_a);
+    tma_prefetch_desc(&tmap_b);
+#pragma unroll
+    for (int i = 0; i < PP_STAGES; ++i) {
+      mbar_init(&full_bar[i], 1);
+      mbar_init(&empty_bar[i], 128);
+    }
+#pragma unroll
+    for (int c = 0; c < 2; ++c) {
+      mbar_init(&pre_full[c], 1);
+      mbar_init(&stg_free[c], 1);
+    }
+    fence_barrier_init();
+    fence_proxy_async();
+  }
+  __syncthreads();
+
+  const int wg = threadIdx.x / 128;
+  if (wg == 0) {
+    // ======================= TMA producer: tiles in the consumers' interleaved order =======================
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;\n" ::: "memory");
+    if (threadIdx.x < 32 && elect_one()) {
+      int stage = 0;
+      uint32_t phase = 0;
+      for (int k = 0, tile = cta; tile < num_tiles; ++k, tile += cta_stride) {
+        const int m_blk = tile / n_blocks, n_blk = tile % n_blocks;
+        if (use_pre) {
+          const int c = k & 1;
+          mbar_wait(&stg_free[c], (k >> 1) & 1);
+          uint8_t* dst = staging + c * PP_STAGING_BYTES;
+          mbar_arrive_expect_tx(&pre_full[c], PP_STAGING_BYTES);
+          tma_load_2d(dst, &tmap_pre_in, &pre_full[c], n_blk * PP_BLOCK_N, m_blk * BLOCK_M);
+          tma_load_2d(dst + PP_BOX_BYTES, &tmap_pre_in, &pre_full[c], n_blk * PP_BLOCK_N + 64, m_blk * BLOCK_M);
+        }
+        for (int kb = 0; kb < k_blocks; ++kb) {
+          mbar_wait(&empty_bar[stage], phase ^ 1);
+          uint8_t* sa = smem + stage * PP_STAGE_BYTES;
+          uint8_t* sb = sa + BLOCK_M * BLOCK_K * 2;
+          mbar_arrive_expect_tx(&full_bar[stage], PP_STAGE_BYTES);
+          tma_load_2d(sa, &tmap_a, &full_bar[stage], kb * BLOCK_K, m_blk * BLOCK_M);
+          if constexpr (!B_MN) {
+            tma_load_2d(sb, &tmap_b, &full_bar[stage], kb * BLOCK_K, n_blk * PP_BLOCK_N);
+          } else {
+#pragma unroll
+            for (int a = 0; a < PP_BLOCK_N / 64; ++a)
+              tma_load_2d(sb + a * (BLOCK_K * 128), &tmap_b, &full_bar[stage], n_blk * PP_BLOCK_N + a * 64, kb * BLOCK_K);
+          }
+          if (++stage == PP_STAGES) {
+            stage = 0;
+            phase ^= 1;
+          }
+        }
+      }
+    }
+    return;
+  }
+
+  // ======================= consumers: whole tiles, alternately =======================
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 232;\n" ::: "memory");
+  const int c = wg - 1;
+  const int t = threadIdx.x % 128;
+  const int warp = t / 32, lane = t % 32;
+  uint8_t* stg = staging + c * PP_STAGING_BYTES;
+  const uint32_t stg_u32 = smem_u32(stg);
+  // this thread's 4-byte slot of (m64 half hm, 8-column group j, row offset 8h) in the swizzled staging tile
+  auto stg_off = [&](int hm, int j, int h) -> uint32_t {
+    const int row = 64 * hm + 16 * warp + lane / 4 + 8 * h;
+    return (j / 8) * PP_BOX_BYTES + row * 128 + (((j % 8) ^ (lane / 4)) << 4) + 4 * (lane % 4);
+  };
+  auto tile_of = [&](int k) { return cta + k * cta_stride; };
+  // consumer 1's first k-loop waits for consumer 0's; consumer 0 goes first
+  if (c == 1) pp_order_signal(0);
+
+  float acc[2][PP_BLOCK_N / 2];
+  for (int k = c; tile_of(k) < num_tiles; k += 2) {
+    const int tile = tile_of(k);
+    const int m_blk = tile / n_blocks, n_blk = tile % n_blocks;
+    if (use_pre && t == 0) {
+      // the producer loads this tile's pre_in into the staging buffer once the previous store has read it
+      tma_store_wait_read<0>();
+      mbar_arrive(&stg_free[c]);
+    }
+    pp_order_wait(c);
+    const long g0 = static_cast<long>(k) * k_blocks;   // k-blocks the ring delivered before this tile
+    int stage = static_cast<int>(g0 % PP_STAGES);
+    uint32_t phase = static_cast<uint32_t>((g0 / PP_STAGES) & 1);
+    int prev_stage = -1;
+    for (int kb = 0; kb < k_blocks; ++kb) {
+      mbar_wait(&full_bar[stage], phase);
+      const uint32_t sa = smem_u32(smem + stage * PP_STAGE_BYTES);
+      const uint32_t sb = sa + BLOCK_M * BLOCK_K * 2;
+      wgmma_fence();
+#pragma unroll
+      for (int kk = 0; kk < BLOCK_K / WGMMA_K; ++kk) {
+        const uint64_t db = B_MN ? make_smem_desc_sw128(sb + kk * (WGMMA_K * 128), BLOCK_K * 128, 1024)
+                                 : make_smem_desc_sw128(sb + kk * (WGMMA_K * 2), 0, 1024);
+        const uint32_t accumulate = (kb > 0 || kk > 0) ? 1u : 0u;
+#pragma unroll
+        for (int hm = 0; hm < 2; ++hm) {
+          const uint64_t da = make_smem_desc_sw128(sa + hm * (64 * 128) + kk * (WGMMA_K * 2), 0, 1024);
+          wgmma_bf16_ss<PP_BLOCK_N, 0, B_MN ? 1 : 0>(acc[hm], da, db, accumulate);
+        }
+      }
+      wgmma_commit();
+      wgmma_wait<1>();
+      if (prev_stage >= 0) mbar_arrive(&empty_bar[prev_stage]);
+      prev_stage = stage;
+      if (++stage == PP_STAGES) {
+        stage = 0;
+        phase ^= 1;
+      }
+    }
+    // the other consumer's next tile may issue now (its wgmmas queue behind ours)
+    if (tile_of(k + 1) < num_tiles) pp_order_signal(c ^ 1);
+    wgmma_wait<0>();
+    wgmma_fence_regs(acc[0]);
+    wgmma_fence_regs(acc[1]);
+    if (prev_stage >= 0) mbar_arrive(&empty_bar[prev_stage]);
+
+    // ---------------- epilogue ----------------
+    if (use_pre) {
+      mbar_wait(&pre_full[c], (k >> 1) & 1);
+    } else {
+      if (t == 0) tma_store_wait_read<0>();
+      warpgroup_sync(c);
+    }
+    const int col_base = n_blk * PP_BLOCK_N + 2 * (lane % 4);
+    // bias (and the pre-activation copy, which passes through the staging buffer first)
+#pragma unroll
+    for (int j = 0; j < PP_BLOCK_N / 8; ++j) {
+      const int col = col_base + 8 * j;
+      float2 b2 = make_float2(0.f, 0.f);
+      if (p.bias != nullptr && col < p.N) b2 = unpack_bf16(*reinterpret_cast<const uint32_t*>(p.bias + col));
+#pragma unroll
+      for (int hm = 0; hm < 2; ++hm)
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          acc[hm][4 * j + 2 * h] += b2.x;
+          acc[hm][4 * j + 2 * h + 1] += b2.y;
+          if (p.pre_out != nullptr)
+            asm volatile("st.shared.u32 [%0], %1;\n" ::"r"(stg_u32 + stg_off(hm, j, h)),
+                         "r"(pack_bf16(acc[hm][4 * j + 2 * h], acc[hm][4 * j + 2 * h + 1]))
+                         : "memory");
+        }
+    }
+    if (p.pre_out != nullptr) {
+      fence_proxy_async();
+      warpgroup_sync(c);
+      if (t == 0) {
+        tma_store_2d(&tmap_pre_out, stg, n_blk * PP_BLOCK_N, m_blk * BLOCK_M);
+        tma_store_2d(&tmap_pre_out, stg + PP_BOX_BYTES, n_blk * PP_BLOCK_N + 64, m_blk * BLOCK_M);
+        tma_store_commit();
+        tma_store_wait_read<0>();
+      }
+      warpgroup_sync(c);
+    }
+    // one unrolled pass per (activation, pre_in) pair: a runtime switch inside the 64 unrolled steps would spread the
+    // executed instructions over a code region that evicts the other consumer's k-loop from the instruction cache
+    const uint32_t row0 = stg_u32 + (16 * warp + lane / 4) * 128 + 4 * (lane % 4);   // row 16 warp + lane / 4, column 0
+    const int r = lane / 4;
+    switch (p.act) {
+      case ACT_GELU:
+        use_pre ? pp_finish<ACT_GELU, true>(acc, row0, r) : pp_finish<ACT_GELU, false>(acc, row0, r);
+        break;
+      case ACT_GELU_TANH:
+        use_pre ? pp_finish<ACT_GELU_TANH, true>(acc, row0, r) : pp_finish<ACT_GELU_TANH, false>(acc, row0, r);
+        break;
+      case ACT_RELU:
+        use_pre ? pp_finish<ACT_RELU, true>(acc, row0, r) : pp_finish<ACT_RELU, false>(acc, row0, r);
+        break;
+      case ACT_SILU:
+        use_pre ? pp_finish<ACT_SILU, true>(acc, row0, r) : pp_finish<ACT_SILU, false>(acc, row0, r);
+        break;
+      case ACT_QUICK_GELU:
+        use_pre ? pp_finish<ACT_QUICK_GELU, true>(acc, row0, r) : pp_finish<ACT_QUICK_GELU, false>(acc, row0, r);
+        break;
+      case ACT_RESADD:
+        pp_finish<ACT_RESADD, true>(acc, row0, r);
+        break;
+      default:
+        use_pre ? pp_finish<ACT_NONE, true>(acc, row0, r) : pp_finish<ACT_NONE, false>(acc, row0, r);
+    }
+    fence_proxy_async();
+    warpgroup_sync(c);
+    if (t == 0) {
+      tma_store_2d(&tmap_out, stg, n_blk * PP_BLOCK_N, m_blk * BLOCK_M);
+      tma_store_2d(&tmap_out, stg + PP_BOX_BYTES, n_blk * PP_BLOCK_N + 64, m_blk * BLOCK_M);
+      tma_store_commit();
+    }
+  }
+  if (t == 0) tma_store_wait<0>();
+}
+
 }  // namespace lb
 
 // =================================================================================================
@@ -758,7 +1042,40 @@ cudaError_t launch_bn(int bn, const CUtensorMap& ta, const CUtensorMap& tb, cons
   }
 }
 
+// bf16 [M, N] matrix with row stride ld, in 64-column x 128-row boxes (128-byte swizzle): the ping-pong kernel's
+// epilogue stores (out, pre_out) and pre_in loads
+bool epilogue_tmap(CUtensorMap* m, const void* ptr, int M, int N, int ld) {
+  uint64_t dims[2] = {(uint64_t)N, (uint64_t)M};
+  uint64_t strides[2] = {2, (uint64_t)ld * 2};
+  uint32_t box[2] = {64u, (uint32_t)lb::BLOCK_M};
+  return lb_host::make_tmap_bf16(m, ptr, 2, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B);
+}
+
+template <bool BMN>
+cudaError_t launch_pingpong(const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& to, const CUtensorMap& tpo,
+                            const CUtensorMap& tpi, const lb::GemmParams& p, int grid, cudaStream_t stream) {
+  auto kern = lb::gemm_pingpong_kernel<BMN>;
+  static bool configured = false;
+  if (!configured) {
+    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, lb::PP_SMEM_BYTES);
+    if (e != cudaSuccess) return e;
+    configured = true;
+  }
+  kern<<<grid, lb::PP_THREADS, lb::PP_SMEM_BYTES, stream>>>(ta, tb, to, tpo, tpi, p);
+  return cudaGetLastError();
+}
+
+// 0: the ping-pong kernel where it applies (bf16 output, NT / NN, no collective); 1: always the 288-thread kernel
+std::atomic<int> g_gemm_schedule{0};
+
+bool aligned16(const void* ptr) { return (reinterpret_cast<uintptr_t>(ptr) & 15) == 0; }
+
 }  // namespace
+
+// Selects the GEMM schedule of later calls (0 = automatic, 1 = the 288-thread kernel only) and returns the previous
+// one: for in-process comparisons of the two kernels.  Decided on the host at launch, so a CUDA graph keeps the kernel
+// that was selected when it was captured.
+extern "C" int lb_gemm_set_schedule(int schedule) { return g_gemm_schedule.exchange(schedule == 1 ? 1 : 0); }
 
 // layout: 0 = NT (A[M,K], B[N,K]); 1 = NN (A[M,K], B[K,N]); 2 = TN (A[K,M], B[K,N])
 // epi:    0 = bf16 store (+bias, act, optional pre-activation copy); 1 = fp32 store; 2 = fp32 atomic accumulate
@@ -783,6 +1100,40 @@ static int gemm_impl(const void* a, const void* b, void* out, int M, int N, int 
   const bool b_mn = (layout != 0);
   const int sms = num_sms();
   const int m_blocks = (M + lb::BLOCK_M - 1) / lb::BLOCK_M;
+  // ---- ping-pong schedule: bf16 output of NT / NN without a collective, 128 x 128 tiles.  Its epilogue goes through
+  // TMA (16-byte aligned bases, ldo % 8 == 0); pre_out and pre_in share its staging buffer, so not both at once; the
+  // column-sum epilogue stays with the 288-thread kernel.  Explicit tile widths other than 128 select that kernel too.
+  const bool pingpong = g_gemm_schedule.load(std::memory_order_relaxed) == 0 && cp.mode == lb::COMM_NONE && epi == 0 &&
+                        deq_a == nullptr && layout != 2 && colsum == nullptr && !(pre_out != nullptr && pre_in != nullptr) &&
+                        (force_bn == 0 || force_bn == lb::PP_BLOCK_N) && ldo % 8 == 0 && aligned16(out) &&
+                        aligned16(pre_out) && aligned16(pre_in);
+  if (pingpong) {
+    lb::GemmParams p;
+    memset(&p, 0, sizeof(p));
+    p.M = M;
+    p.N = N;
+    p.K = K;
+    p.k_splits = 1;
+    p.k_per_split = (K + lb::BLOCK_K - 1) / lb::BLOCK_K;
+    p.bias = reinterpret_cast<const __nv_bfloat16*>(bias);
+    p.act = act;
+    p.out = out;
+    p.pre_out = reinterpret_cast<__nv_bfloat16*>(pre_out);
+    p.pre_in = reinterpret_cast<const __nv_bfloat16*>(pre_in);
+    p.ldo = ldo;
+    CUtensorMap ta, tb, to, tpo, tpi;
+    if (!operand_tmap(&ta, a, false, M, K, lda, lb::BLOCK_M)) return -2;
+    if (!operand_tmap(&tb, b, b_mn, N, K, ldb, lb::PP_BLOCK_N)) return -2;
+    if (!epilogue_tmap(&to, out, M, N, ldo)) return -2;
+    tpo = to;
+    tpi = to;
+    if (pre_out != nullptr && !epilogue_tmap(&tpo, pre_out, M, N, ldo)) return -2;
+    if (pre_in != nullptr && !epilogue_tmap(&tpi, pre_in, M, N, ldo)) return -2;
+    const long tiles = (long)m_blocks * ((N + lb::PP_BLOCK_N - 1) / lb::PP_BLOCK_N);
+    const int grid = (int)(tiles < sms ? tiles : sms);
+    return (int)(b_mn ? launch_pingpong<true>(ta, tb, to, tpo, tpi, p, grid, stream)
+                      : launch_pingpong<false>(ta, tb, to, tpo, tpi, p, grid, stream));
+  }
   // ---- tile-N heuristic: least estimated time (waves x per-tile time), ties -> wider tile
   int bn = force_bn;
   if (bn == 0 && epi == 2 && cp.mode == lb::COMM_AG && cp.gathered_is_b) {
