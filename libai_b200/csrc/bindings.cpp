@@ -96,6 +96,12 @@ int lb_decode_attn(const void* q, const long* q_strides, const void* k, const vo
                    float scale, int nsplit, cudaStream_t s);
 int lb_kv_append(const void* qkv, const float* cosv, const float* sinv, void* q_out, void* k_cache, void* v_cache,
                  const int* seqlens, int B, int Sq, int G, int r, int C, int D, cudaStream_t s);
+int lb_window_attn_groups(int B, int H, int W, int ws, int heads);
+int lb_window_attn_fwd(const void* qkv, void* out, float* lse, const float* table, const float* tau, int B, int H, int W,
+                       int ws, int shift, int heads, int d, float scale, cudaStream_t s);
+int lb_window_attn_bwd(const void* dout, const void* qkv, const float* lse, const float* table,
+                       const float* tau, void* dqkv, float* dtable, float* dtau, float* dt_part, float* dtau_part, int B,
+                       int H, int W, int ws, int shift, int heads, int d, float scale, cudaStream_t s);
 }
 
 namespace {
@@ -883,6 +889,84 @@ Tensor decode_attn(const Tensor& q, const Tensor& k_cache, const Tensor& v_cache
   return o;
 }
 
+// ---- shifted-window attention -----------------------------------------------------------------------
+// qkv [B, H*W, 3*C] in image order (per token [3, heads, d]), an H x W map of ws x ws windows cyclically shifted by
+// `shift`; table fp32 [(2ws - 1)^2, heads]; tau fp32 [heads] selects cosine attention (SwinV2).  Returns the head dim.
+int64_t check_window_args(const Tensor& qkv, int64_t H, int64_t W, int64_t ws, int64_t shift, int64_t heads,
+                          const Tensor& table, const c10::optional<Tensor>& tau, const char* what) {
+  TORCH_CHECK(qkv.is_cuda() && qkv.scalar_type() == at::kBFloat16 && qkv.dim() == 3 && qkv.is_contiguous(), what,
+              ": contiguous bf16 CUDA qkv [B, H*W, 3*C] expected");
+  TORCH_CHECK(reinterpret_cast<uintptr_t>(qkv.data_ptr()) % 16 == 0, what, ": qkv must be 16-byte aligned");
+  TORCH_CHECK(heads >= 1 && heads <= 65535 && qkv.size(2) % (3 * heads) == 0, what, ": qkv width ", qkv.size(2),
+              " is not 3 * heads * d for ", heads, " heads");
+  const int64_t d = qkv.size(2) / (3 * heads);
+  TORCH_CHECK(d % 8 == 0 && d >= 8 && d <= 64, what, ": head dim ", d,
+              " not supported (supported: multiples of 8 from 8 to 64)");
+  TORCH_CHECK(ws >= 1 && ws <= 16, what, ": window ", ws, " not supported (supported: 1 to 16)");
+  TORCH_CHECK(H >= 1 && W >= 1 && H % ws == 0 && W % ws == 0, what, ": the ", H, " x ", W,
+              " map must be a whole number of ", ws, " x ", ws, " windows");
+  TORCH_CHECK(qkv.size(1) == H * W, what, ": qkv has ", qkv.size(1), " tokens, the map ", H * W);
+  TORCH_CHECK(qkv.size(0) * H * W <= INT32_MAX, what, ": more than 2^31 - 1 tokens");
+  TORCH_CHECK(shift >= 0 && shift < ws, what, ": shift ", shift, " not supported (supported: 0 <= shift < window)");
+  TORCH_CHECK(table.is_cuda() && table.scalar_type() == at::kFloat && table.is_contiguous() && table.dim() == 2 &&
+                  table.size(0) == (2 * ws - 1) * (2 * ws - 1) && table.size(1) == heads,
+              what, ": table must be contiguous fp32 CUDA [(2 * window - 1)^2, heads]");
+  if (tau.has_value() && tau->defined())
+    TORCH_CHECK(tau->is_cuda() && tau->scalar_type() == at::kFloat && tau->is_contiguous() && tau->numel() == heads,
+                what, ": tau must be contiguous fp32 CUDA [heads]");
+  return d;
+}
+
+std::tuple<Tensor, Tensor> window_attn_fwd(const Tensor& qkv, int64_t H, int64_t W, int64_t window, int64_t shift,
+                                           int64_t heads, double scale, const Tensor& table,
+                                           const c10::optional<Tensor>& tau) {
+  c10::cuda::CUDAGuard guard(qkv.device());
+  const int64_t d = check_window_args(qkv, H, W, window, shift, heads, table, tau, "window_attn_fwd");
+  const int64_t B = qkv.size(0), nwin = B * (H / window) * (W / window);
+  Tensor o = at::empty({B, H * W, heads * d}, qkv.options());
+  Tensor lse = at::empty({nwin, heads, window * window}, qkv.options().dtype(at::kFloat));
+  const bool cos = tau.has_value() && tau->defined();
+  check(lb_window_attn_fwd(qkv.data_ptr(), o.data_ptr(), lse.data_ptr<float>(), table.data_ptr<float>(),
+                           cos ? tau->data_ptr<float>() : nullptr, (int)B, (int)H, (int)W, (int)window, (int)shift,
+                           (int)heads, (int)d, (float)scale, cur_stream()),
+        "window_attn_fwd");
+  return {o, lse};
+}
+
+// returns (dqkv [B, H*W, 3*C] bf16, dtable fp32 like table, dtau fp32 [heads] (empty without tau))
+std::tuple<Tensor, Tensor, Tensor> window_attn_bwd(const Tensor& dout, const Tensor& qkv, const Tensor& lse, int64_t H, int64_t W, int64_t window,
+                                                   int64_t shift, int64_t heads, double scale, const Tensor& table,
+                                                   const c10::optional<Tensor>& tau) {
+  c10::cuda::CUDAGuard guard(qkv.device());
+  const int64_t d = check_window_args(qkv, H, W, window, shift, heads, table, tau, "window_attn_bwd");
+  const int64_t B = qkv.size(0), N = window * window, nwin = B * (H / window) * (W / window);
+  TORCH_CHECK(dout.is_cuda() && dout.scalar_type() == at::kBFloat16 && dout.is_contiguous() &&
+                  dout.sizes() == at::IntArrayRef({B, H * W, heads * d}) &&
+                  reinterpret_cast<uintptr_t>(dout.data_ptr()) % 16 == 0,
+              "window_attn_bwd: dout must be a contiguous 16-byte aligned bf16 [B, H*W, C]");
+  TORCH_CHECK(lse.is_cuda() && lse.scalar_type() == at::kFloat && lse.is_contiguous() &&
+                  lse.sizes() == at::IntArrayRef({nwin, heads, N}),
+              "window_attn_bwd: lse must be the forward's fp32 [windows, heads, window^2]");
+  const bool cos = tau.has_value() && tau->defined();
+  const int G = lb_window_attn_groups((int)B, (int)H, (int)W, (int)window, (int)heads);
+  Tensor dqkv = at::empty_like(qkv);
+  Tensor dtable = at::empty_like(table);
+  Tensor dtau = at::empty({cos ? heads : 0}, table.options());
+  Tensor part = at::empty({std::max<int64_t>(G, 1) * heads * N * N}, table.options());
+  Tensor tau_part = at::empty({cos ? std::max<int64_t>(G, 1) * heads : 0}, table.options());
+  check(lb_window_attn_bwd(dout.data_ptr(), qkv.data_ptr(), lse.data_ptr<float>(),
+                           table.data_ptr<float>(), cos ? tau->data_ptr<float>() : nullptr, dqkv.data_ptr(),
+                           dtable.data_ptr<float>(), cos ? dtau.data_ptr<float>() : nullptr, part.data_ptr<float>(),
+                           cos ? tau_part.data_ptr<float>() : nullptr, (int)B, (int)H, (int)W, (int)window, (int)shift,
+                           (int)heads, (int)d, (float)scale, cur_stream()),
+        "window_attn_bwd");
+  if (nwin == 0) {
+    dtable.zero_();
+    dtau.zero_();
+  }
+  return {dqkv, dtable, dtau};
+}
+
 // `dbias` (optional, fp32, same shape as `bias`): the gradient of a learned bias is accumulated into it
 std::tuple<Tensor, Tensor, Tensor, Tensor> attn_bwd(const Tensor& dout, const Tensor& q, const Tensor& k, const Tensor& v,
                                             const Tensor& o, const Tensor& lse, bool causal, double scale,
@@ -1098,6 +1182,8 @@ TORCH_LIBRARY(libai_b200, m) {
   m.def("attn_fwd(Tensor q, Tensor k, Tensor v, bool causal, float scale, Tensor? kv_lens, Tensor? bias=None, Tensor? alibi_slopes=None, float p_drop=0.0, int salt=0, Tensor? kv_start=None) -> (Tensor, Tensor, Tensor)", &attn_fwd);
   m.def("attn_bwd(Tensor dout, Tensor q, Tensor k, Tensor v, Tensor o, Tensor lse, bool causal, float scale, Tensor? kv_lens, Tensor? bias=None, Tensor? alibi_slopes=None, Tensor(a!)? dbias=None, float p_drop=0.0, Tensor? rng_state=None, Tensor? kv_start=None) -> (Tensor, Tensor, Tensor, Tensor)", &attn_bwd);
   m.def("kv_append(Tensor qkv, Tensor(a!) k_cache, Tensor(b!) v_cache, Tensor cache_seqlens, Tensor? cos, Tensor? sin, bool write_q) -> Tensor", &kv_append);
+  m.def("window_attn_fwd(Tensor qkv, int H, int W, int window, int shift, int heads, float scale, Tensor table, Tensor? tau) -> (Tensor, Tensor)", &window_attn_fwd);
+  m.def("window_attn_bwd(Tensor dout, Tensor qkv, Tensor lse, int H, int W, int window, int shift, int heads, float scale, Tensor table, Tensor? tau) -> (Tensor, Tensor, Tensor)", &window_attn_bwd);
   m.def("decode_attn(Tensor q, Tensor k_cache, Tensor v_cache, Tensor cache_seqlens, Tensor kv_start, float scale, int splits=0) -> Tensor", &decode_attn);
   m.def("bias_dropout_residual(Tensor x, Tensor? bias, Tensor? res, float p, int salt, Tensor? rng_state=None) -> (Tensor, Tensor)", &bias_dropout_residual);
 }

@@ -16,6 +16,7 @@ from torch import nn
 from libai_b200.config import configurable
 from libai_b200.layers import MLP, DropPath, LayerNorm, Linear
 from libai_b200.layers._param import create_parameter, trunc_normal_, zeros_
+from libai_b200.ops import functional as OF
 
 from .utils.pipeline_model import PipelineStageMixin
 
@@ -97,6 +98,14 @@ class WindowAttention(nn.Module):
         x = torch.matmul(attn, v).transpose(1, 2).reshape(B_, N, C)
         return self.proj_drop(self.proj(x))
 
+    def forward_image(self, x, H, W, shift):
+        """The whole shifted-window attention of the image-ordered tokens ``x`` ``[B, H·W, C]`` in one kernel (see
+        :func:`OF.window_attention`): qkv and proj act per token, so they run on the image order and no roll, partition
+        or reverse copy is made."""
+        o = OF.window_attention(self.qkv(x), H=H, W=W, window=self.window_size[0], shift=shift, heads=self.num_heads,
+                                scale=self.scale, table=self.relative_position_bias_table.float())
+        return self.proj_drop(self.proj(o))
+
 
 class SwinTransformerBlock(nn.Module):
     def __init__(self, dim, input_resolution, num_heads, window_size=7, shift_size=0, mlp_ratio=4.0, qkv_bias=True,
@@ -132,6 +141,10 @@ class SwinTransformerBlock(nn.Module):
         H, W = self.input_resolution
         B, L, C = x.shape
         assert L == H * W, "input feature has wrong size"
+        if OF.window_attention_supported(x, H=H, W=W, window=self.window_size, shift=self.shift_size,
+                                         head_dim=C // self.num_heads, attn_drop=self.attn.attn_drop.p,
+                                         training=self.training):
+            return self.attn.forward_image(x, H, W, self.shift_size)
         x = x.view(B, H, W, C)
         if self.shift_size > 0:
             x = torch.roll(x, shifts=(-self.shift_size, -self.shift_size), dims=(1, 2))

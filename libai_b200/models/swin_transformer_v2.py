@@ -18,6 +18,7 @@ from torch import nn
 from libai_b200.config import configurable
 from libai_b200.layers import MLP, DropPath, LayerNorm, Linear
 from libai_b200.layers._param import create_parameter, zeros_
+from libai_b200.ops import functional as OF
 
 from .swin_transformer import (
     PatchEmbed,
@@ -93,6 +94,20 @@ class WindowAttention(nn.Module):
         x = torch.matmul(attn, v).transpose(1, 2).reshape(B_, N, C)
         return self.proj_drop(self.proj(x))
 
+    def forward_image(self, x, H, W, shift):
+        """The whole shifted-window cosine attention of the image-ordered tokens ``x`` ``[B, H·W, C]`` in one kernel
+        (see :func:`OF.window_attention`).  The fp32 table ``16·sigmoid(cpb_mlp(coords))`` and ``tau = exp(min(logit_scale,
+        ln 100))`` are formed here, so autograd carries their gradients to ``cpb_mlp`` and ``logit_scale``."""
+        qkv = self.qkv(x)
+        if self.q_bias is not None:
+            qkv = qkv + torch.cat([self.q_bias, torch.zeros_like(self.v_bias), self.v_bias]).to(qkv.dtype)
+        table = self.cpb_mlp(self.relative_coords_table.to(self.qkv.weight.dtype)).view(-1, self.num_heads)
+        table = 16.0 * torch.sigmoid(table.float())
+        tau = torch.clamp(self.logit_scale.float(), max=math.log(1.0 / 0.01)).exp().view(-1)
+        o = OF.window_attention(qkv, H=H, W=W, window=self.window_size[0], shift=shift, heads=self.num_heads, scale=1.0,
+                                table=table, tau=tau)
+        return self.proj_drop(self.proj(o))
+
 
 class SwinTransformerBlock(nn.Module):
     def __init__(self, dim, input_resolution, num_heads, window_size=7, shift_size=0, mlp_ratio=4.0, qkv_bias=True,
@@ -130,14 +145,19 @@ class SwinTransformerBlock(nn.Module):
         B, L, C = x.shape
         assert L == H * W, "input feature has wrong size"
         shortcut = x
-        x = x.view(B, H, W, C)
-        if self.shift_size > 0:
-            x = torch.roll(x, shifts=(-self.shift_size, -self.shift_size), dims=(1, 2))
-        win = window_partition(x, self.window_size).view(-1, self.window_size * self.window_size, C)
-        win = self.attn(win, mask=self._attn_mask(x.device)).view(-1, self.window_size, self.window_size, C)
-        x = window_reverse(win, self.window_size, H, W)
-        if self.shift_size > 0:
-            x = torch.roll(x, shifts=(self.shift_size, self.shift_size), dims=(1, 2))
+        if OF.window_attention_supported(x, H=H, W=W, window=self.window_size, shift=self.shift_size,
+                                         head_dim=C // self.num_heads, attn_drop=self.attn.attn_drop.p,
+                                         training=self.training):
+            x = self.attn.forward_image(x, H, W, self.shift_size)
+        else:
+            x = x.view(B, H, W, C)
+            if self.shift_size > 0:
+                x = torch.roll(x, shifts=(-self.shift_size, -self.shift_size), dims=(1, 2))
+            win = window_partition(x, self.window_size).view(-1, self.window_size * self.window_size, C)
+            win = self.attn(win, mask=self._attn_mask(x.device)).view(-1, self.window_size, self.window_size, C)
+            x = window_reverse(win, self.window_size, H, W)
+            if self.shift_size > 0:
+                x = torch.roll(x, shifts=(self.shift_size, self.shift_size), dims=(1, 2))
         x = shortcut + self.drop_path(self.norm1(x.view(B, H * W, C)))  # res-post-norm
         return x + self.drop_path(self.norm2(self.mlp(x)))
 

@@ -23,7 +23,7 @@ CUDA_HOME = os.environ.get("CUDA_HOME", "/usr/local/cuda")
 NVCC = os.path.join(CUDA_HOME, "bin", "nvcc")
 
 CU_SOURCES = ["gemm_sm90.cu", "norm.cu", "elementwise.cu", "attention_sm90.cu", "comm_kernels.cu",
-              "decode_attention_sm90.cu"]
+              "decode_attention_sm90.cu", "window_attention_sm90.cu"]
 CPP_SOURCES = ["bindings.cpp", "symm_mem.cpp"]
 
 NVCC_FLAGS = [

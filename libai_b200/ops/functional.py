@@ -759,6 +759,62 @@ def attention(q, k, v, *, causal: bool = False, scale: Optional[float] = None, m
 
 
 # --------------------------------------------------------------------------------------
+# shifted-window attention (Swin, SwinV2)
+# --------------------------------------------------------------------------------------
+def window_attention_supported(x, *, H: int, W: int, window: int, shift: int, head_dim: int, attn_drop: float = 0.0,
+                               training: bool = False) -> bool:
+    """True when a Swin block on the tokens ``x`` ``[B, H·W, C]`` runs :func:`window_attention`: bf16 on the GPU, a head
+    dim that is a multiple of 8 from 8 to 64, a window of 1 to 16 that tiles the ``H × W`` map, ``0 <= shift < window``,
+    and no attention dropout in training (the kernel has none).  Otherwise the block keeps its PyTorch window path."""
+    return (
+        use_native(x)
+        and x.dtype == torch.bfloat16
+        and head_dim % 8 == 0
+        and 8 <= head_dim <= 64
+        and 1 <= window <= 16
+        and H % window == 0
+        and W % window == 0
+        and 0 <= shift < window
+        and not (training and attn_drop > 0.0)
+    )
+
+
+class _WindowAttnFn(torch.autograd.Function):
+    """Shifted-window attention read straight from the image-ordered qkv projection; the backward writes one ``dqkv`` of
+    the same layout and the table (and ``tau``) gradients, reduced in a fixed order."""
+
+    @staticmethod
+    def forward(ctx, qkv, table, tau, H, W, window, shift, heads, scale):
+        ext = load_ext()
+        qkv = qkv.contiguous()
+        o, lse = ext.window_attn_fwd(qkv, H, W, window, shift, heads, scale, table, tau)
+        count_launch()
+        ctx.save_for_backward(qkv, lse, table, tau)
+        ctx.geom = (H, W, window, shift, heads, scale)
+        return o
+
+    @staticmethod
+    def backward(ctx, go):
+        ext = load_ext()
+        qkv, lse, table, tau = ctx.saved_tensors
+        dqkv, dtable, dtau = ext.window_attn_bwd(go.contiguous(), qkv, lse, *ctx.geom, table, tau)
+        count_launch(3)
+        return dqkv, dtable, (dtau if tau is not None else None), None, None, None, None, None, None
+
+
+def window_attention(qkv, *, H: int, W: int, window: int, shift: int, heads: int, scale: float, table, tau=None):
+    """Attention inside the ``window × window`` windows of an ``H × W`` map cyclically shifted by ``shift`` (Swin).
+
+    ``qkv`` ``[B, H·W, 3C]`` is the qkv projection of the tokens in image order (per token ``[3, heads, d]``); returns
+    the attention output ``[B, H·W, C]`` in image order.  Exactly ``roll(-shift)`` → window partition → attention →
+    window reverse → ``roll(+shift)``, with the score ``scale·q·k + table[relative_position_index, h]`` plus ``-100``
+    between tokens of different shifted regions (``shifted_window_mask``).  With ``tau`` (fp32 ``[heads]``) the scores
+    are cosine ones, ``tau_h·q̂·k̂`` (SwinV2; ``scale`` is unused).  ``table`` is fp32 ``[(2·window − 1)², heads]``.
+    Gradients flow to ``qkv``, ``table`` and ``tau``.  Needs :func:`window_attention_supported`."""
+    return _WindowAttnFn.apply(qkv, table, tau, int(H), int(W), int(window), int(shift), int(heads), float(scale))
+
+
+# --------------------------------------------------------------------------------------
 # KV-cache decoding: caches are [b, g, C, d] buffers (g = the key/value heads) (libai_b200.inference.kv_cache.StaticKVCache); ``cache_seqlens``
 # (int32 [b]) is the number of rows already held, ``kv_start`` (int32 [b]) the left padding of each sample
 # --------------------------------------------------------------------------------------
