@@ -21,6 +21,11 @@
 // j <= i + (Sk - Sq) (bottom-right alignment, as in decode attention).  A query without a visible key gets O = 0,
 // lse = 0 and dQ = 0, and adds nothing to dK / dV.
 //
+// Packed sequences (DOC instances, causal self-attention only): doc_start [B, S] gives the first key of each query's
+// document, so query i of sample b sees key j iff doc_start[b, i] <= j <= i (doc_start clamped to [0, i]: every query
+// sees itself).  Nothing assumes doc_start to be non-decreasing along a row: which key tiles a forward CTA loads and
+// which (key block, query block) visits the backward skips come from the minimum over the rows of the query block.
+//
 // Forward, one CTA per (batch, query head, 128-query block), 384 threads:
 //   warpgroup 0  TMA producer (one elected thread): Q once, then K/V tiles of 128 keys (double buffered); it gives
 //                its registers to the consumers (setmaxnreg)
@@ -51,6 +56,7 @@ struct AttnFwdParams {
   float scale;
   const int* kv_lens; // optional [B]: end of the visible keys per sample (right-padded batches)
   const int* kv_start;   // optional [B]: start of the visible keys per sample (left-padded batches)
+  const int* doc_start;  // [B, Sq] in the DOC instances: first key of each query's document
   // additive score bias (v2 kernel): dense bf16 [.., Sq, Sk] with (batch, head, query) strides in elements (0 = broadcast;
   // T5 relative-position bias, Swin/BERT style masks) or ALiBi slopes per head (bias = slope * (key - query - (Sk - Sq)))
   const __nv_bfloat16* bias;
@@ -88,6 +94,10 @@ template <int D>
 LB_DEVICE bool col_in_head(int c, int d) {
   return (D == 128 && c < 64) || c < d;
 }
+// first visible key of query row i (< S) of a packed sample: its doc_start, clamped to [0, i]
+LB_DEVICE int doc_begin(const int* doc_start, int S, int batch, int i) {
+  return min(max(doc_start[static_cast<size_t>(batch) * S + i], 0), i);
+}
 
 template <int D>
 struct AttnFwdCfg {
@@ -96,10 +106,11 @@ struct AttnFwdCfg {
   static constexpr int SMEM_BYTES = 5 * TILE_BYTES + 1024 + 256;   // Q + 2 x (K, V)
 };
 
-template <int D, int BIAS, bool DROP>
-__global__ void __launch_bounds__(ATT_FWD_THREADS, 1)
-attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_k,
-                const __grid_constant__ CUtensorMap tmap_v, AttnFwdParams p) {
+// the forward of one CTA; tmap_* and p are the kernel's __grid_constant__ parameters (inlined: no call in the kernel)
+template <int D, int BIAS, bool DROP, bool DOC>
+LB_DEVICE void attn_fwd_cta(const CUtensorMap& tmap_q, const CUtensorMap& tmap_k, const CUtensorMap& tmap_v,
+                            const AttnFwdParams& p) {
+  static_assert(!DOC || (BIAS == BIAS_NONE && !DROP), "packed sequences run without bias and dropout");
   using Cfg = AttnFwdCfg<D>;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -112,6 +123,7 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
   uint64_t* k_empty = bars + 3;  // 2
   uint64_t* v_full = bars + 5;   // 2
   uint64_t* v_empty = bars + 7;  // 2
+  int* doc_min = reinterpret_cast<int*>(bars + 9);   // 4 (DOC): per-warp minima of the block's document starts
 
   const int warp_idx = threadIdx.x / 32;
   // heavy (late) query blocks first: better tail behaviour under the causal mask
@@ -124,8 +136,12 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
   const int off = p.Sk - p.Sq;   // causal offset: query i sees keys j <= i + off
   // key tiles j0 .. j0 + nkv - 1 hold every key some row of this block can see; the others are not loaded
   const int key_end = p.causal ? min(kv_len, min(q0 + ATT_BM, p.Sq) + off) : kv_len;
-  const int j0 = kv_beg / ATT_BN;
-  const int nkv = max(0, (key_end + ATT_BN - 1) / ATT_BN - j0);
+  if constexpr (DOC) {   // warpgroup 0 reads one row each (rows past Sq repeat the last row)
+    if (warp_idx < 4) {
+      const int m = __reduce_min_sync(0xffffffffu, doc_begin(p.doc_start, p.Sq, batch, min(q0 + static_cast<int>(threadIdx.x), p.Sq - 1)));
+      if (threadIdx.x % 32 == 0) doc_min[warp_idx] = m;
+    }
+  }
 
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmap_q);
@@ -142,6 +158,9 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
     fence_proxy_async();
   }
   __syncthreads();
+  // the first tile holds the earliest key any row of the block sees
+  const int j0 = (DOC ? min(min(doc_min[0], doc_min[1]), min(doc_min[2], doc_min[3])) : kv_beg) / ATT_BN;
+  const int nkv = max(0, (key_end + ATT_BN - 1) / ATT_BN - j0);
 
   if (warp_idx < 4) {
     asm volatile("setmaxnreg.dec.sync.aligned.u32 24;\n" ::: "memory");
@@ -173,12 +192,14 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
   const int t = threadIdx.x % 128;
   const int r_loc = 64 * wg + 16 * (t / 32) + (t % 32) / 4;   // this thread's rows: r_loc and r_loc + 8
   const int cq = 2 * (t % 4);                                  // its columns inside every 8-column group: cq, cq + 1
-  // keys kv_beg + [0, vis_len) are visible to row h: one unsigned comparison of key - kv_beg per element tests both ends
-  int q_idx[2], vis_len[2];
+  // keys row_beg + [0, vis_len) are visible to row h: one unsigned comparison of key - row_beg per element tests both
+  // ends (row_beg = kv_beg, or the row's document start in the DOC instances)
+  int q_idx[2], vis_len[2], row_beg[2];
 #pragma unroll
   for (int h = 0; h < 2; ++h) {
     q_idx[h] = q0 + r_loc + 8 * h;
-    vis_len[h] = max(0, (p.causal ? min(kv_len, q_idx[h] + off + 1) : kv_len) - kv_beg);
+    row_beg[h] = DOC ? doc_begin(p.doc_start, p.Sq, batch, min(q_idx[h], p.Sq - 1)) : kv_beg;
+    vis_len[h] = max(0, (p.causal ? min(kv_len, q_idx[h] + off + 1) : kv_len) - row_beg[h]);
   }
   constexpr float LOG2E = 1.4426950408889634f;
   unsigned long long rng_seed = 0, rng_offset = 0;
@@ -229,7 +250,9 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
 
     // ---- scores in the log2 domain, masked
     const int kbase = j * ATT_BN, krel = kbase - kv_beg;
-    const bool need_mask = kbase < kv_beg || kbase + ATT_BN > kv_len || (p.causal && kbase + ATT_BN - 1 > q0 + off);
+    // (per thread in the DOC instances: a tile may start before one of its rows' documents only)
+    const bool need_mask = kbase < (DOC ? max(row_beg[0], row_beg[1]) : kv_beg) || kbase + ATT_BN > kv_len ||
+                           (p.causal && kbase + ATT_BN - 1 > q0 + off);
 #pragma unroll
     for (int jj = 0; jj < ATT_BN / 8; ++jj) {
 #pragma unroll
@@ -260,7 +283,8 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
         for (int h = 0; h < 2; ++h) {
 #pragma unroll
           for (int c = 0; c < 2; ++c)
-            if (static_cast<unsigned>(krel + 8 * jj + cq + c) >= static_cast<unsigned>(vis_len[h])) s[4 * jj + 2 * h + c] = -INFINITY;
+            if (static_cast<unsigned>((DOC ? kbase - row_beg[h] : krel) + 8 * jj + cq + c) >= static_cast<unsigned>(vis_len[h]))
+              s[4 * jj + 2 * h + c] = -INFINITY;
         }
       }
     }
@@ -341,6 +365,20 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
   }
 }
 
+template <int D, int BIAS, bool DROP>
+__global__ void __launch_bounds__(ATT_FWD_THREADS, 1)
+attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_k,
+                const __grid_constant__ CUtensorMap tmap_v, const __grid_constant__ AttnFwdParams p) {
+  attn_fwd_cta<D, BIAS, DROP, false>(tmap_q, tmap_k, tmap_v, p);
+}
+// packed sequences (doc_start): causal self-attention without bias or dropout
+template <int D>
+__global__ void __launch_bounds__(ATT_FWD_THREADS, 1)
+attn_fwd_doc_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_k,
+                    const __grid_constant__ CUtensorMap tmap_v, const __grid_constant__ AttnFwdParams p) {
+  attn_fwd_cta<D, BIAS_NONE, false, true>(tmap_q, tmap_k, tmap_v, p);
+}
+
 }  // namespace lb
 
 namespace {
@@ -366,11 +404,11 @@ bool make_q_tmap(CUtensorMap* m, const void* ptr, int B, int G, int r, int S, in
   return lb_host::make_tmap_bf16(m, ptr, 5, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B);
 }
 
-template <int D, int BIAS, bool DROP>
+template <int D, int BIAS, bool DROP, bool DOC = false>
 cudaError_t launch_fwd_t(const CUtensorMap& tq, const CUtensorMap& tk, const CUtensorMap& tv, const lb::AttnFwdParams& p,
                          cudaStream_t s) {
   using Cfg = lb::AttnFwdCfg<D>;
-  auto kern = lb::attn_fwd_kernel<D, BIAS, DROP>;
+  auto kern = DOC ? lb::attn_fwd_doc_kernel<D> : lb::attn_fwd_kernel<D, BIAS, DROP>;
   static bool configured = false;
   if (!configured) {
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES);
@@ -385,6 +423,7 @@ cudaError_t launch_fwd_t(const CUtensorMap& tq, const CUtensorMap& tk, const CUt
 template <int D>
 cudaError_t launch_fwd(const CUtensorMap& tq, const CUtensorMap& tk, const CUtensorMap& tv, const lb::AttnFwdParams& p,
                        cudaStream_t s) {
+  if (p.doc_start != nullptr) return launch_fwd_t<D, lb::BIAS_NONE, false, true>(tq, tk, tv, p, s);
   const int bias = p.bias != nullptr ? lb::BIAS_DENSE : (p.alibi_slopes != nullptr ? lb::BIAS_ALIBI : lb::BIAS_NONE);
   const bool drop = p.drop_thresh > 0;
   if (bias == lb::BIAS_NONE) return drop ? launch_fwd_t<D, lb::BIAS_NONE, true>(tq, tk, tv, p, s) : launch_fwd_t<D, lb::BIAS_NONE, false>(tq, tk, tv, p, s);
@@ -397,15 +436,20 @@ cudaError_t launch_fwd(const CUtensorMap& tq, const CUtensorMap& tk, const CUten
 // (optional, int32 [B], device): per-sample key window.
 // p_drop in [0, 1): attention dropout probability (quantised to 1/256 like the byte-threshold test of the kernel);
 // bias (optional, bf16): dense additive score bias with (batch, head, query-row) strides in elements, key stride 1;
-// alibi_slopes (optional, fp32 [A]).
+// alibi_slopes (optional, fp32 [A]); doc_start (optional, int32 [B, Sq], device): packed sequences, causal Sq == Sk
+// only, without kv_lens, kv_start, bias or dropout.
 extern "C" int lb_attn_fwd(const void* q, const void* k, const void* v, void* o, float* lse, int B, int A, int G, int Sq,
                            int Sk, int D, const long* q_strides, const long* k_strides, const long* v_strides, int causal,
-                           float scale, const int* kv_lens, const int* kv_start, const void* bias, const long* bias_strides,
-                           const float* alibi_slopes, float p_drop, const lb::RngArgs* rng, long long* rng_out, cudaStream_t s) {
+                           float scale, const int* kv_lens, const int* kv_start, const int* doc_start, const void* bias,
+                           const long* bias_strides, const float* alibi_slopes, float p_drop, const lb::RngArgs* rng,
+                           long long* rng_out, cudaStream_t s) {
   const int tile = head_dim_tile(D);
   if (tile == 0) return -1;
   if (Sq <= 0 || Sk <= 0) return -5;
   if (G <= 0 || A % G) return -4;
+  if (doc_start != nullptr && (!causal || Sq != Sk || kv_lens != nullptr || kv_start != nullptr || bias != nullptr ||
+                               alibi_slopes != nullptr || p_drop > 0.f))
+    return -6;
   for (int i = 0; i < 3; ++i)
     if ((q_strides[i] % 8) || (k_strides[i] % 8) || (v_strides[i] % 8)) return -3;
   if (q_strides[3] % 8) return -3;
@@ -427,6 +471,7 @@ extern "C" int lb_attn_fwd(const void* q, const void* k, const void* v, void* o,
   p.scale_log2 = scale * 1.4426950408889634f;
   p.kv_lens = kv_lens;
   p.kv_start = kv_start;
+  p.doc_start = doc_start;
   p.bias = reinterpret_cast<const __nv_bfloat16*>(bias);
   for (int i = 0; i < 3; ++i) p.bias_strides[i] = (bias != nullptr && bias_strides != nullptr) ? bias_strides[i] : 0;
   if (bias != nullptr && ((p.bias_strides[0] | p.bias_strides[1] | p.bias_strides[2]) % 8 || (reinterpret_cast<uintptr_t>(bias) & 15)))
@@ -448,6 +493,11 @@ extern "C" int lb_attn_fwd(const void* q, const void* k, const void* v, void* o,
 // Which query blocks a key block visits depends on the shapes only (Sq, Sk, causal): under the causal mask query block
 // i and key block kb meet iff 64 kb <= 64 i + 63 + (Sk - Sq).  Keys outside a sample's kv_start / kv_lens window are
 // masked element-wise, so every visit happens and the dQ ordering below counts the same visits on both sides.
+// Packed sequences (DOC): a visit in which every query row's document starts after the key block is skipped by the
+// producer (no Q / dO load) and the consumer (no MMA) alike, from the same minimum over the rows.  It does not touch
+// the dQ order counter: whether a visit is skipped is monotone in the key block (skipped blocks lie below every
+// contributing one), so a contributing key block waits for exactly the contributing blocks above it, and the
+// contributions land in decreasing key-block order.
 //   Sᵀ = K·Q_iᵀ , dPᵀ = V·dO_iᵀ                  (wgmma, registers)
 //   Pᵀ = exp(Sᵀ·scale − lse) , dSᵀ = Pᵀ ∘ (dPᵀ − δ) · scale
 //   dV += Pᵀ·dO_i , dK += dSᵀ·Q_i                 (A operands straight from the registers, accumulators stay in
@@ -489,6 +539,7 @@ struct AttnBwdParams {
   float scale, scale_log2;
   const int* kv_lens;   // optional [B]
   const int* kv_start;  // optional [B]
+  const int* doc_start; // [B, Sq] in the DOC instances
   // same additive bias / dropout description as the forward; `rng_state` = the (seed, offset) pair the forward used
   const __nv_bfloat16* bias;
   long bias_strides[3];
@@ -501,10 +552,20 @@ struct AttnBwdParams {
   SpinTimeout* timeout_rec;  // where a timed-out dq_order wait leaves its diagnostic (host-mapped)
 };
 
-template <int D, int BIAS, bool DROP>
+// DOC: true when no row of the query block [q0, q0 + 64) sees a key of the block [k0, k0 + 64), i.e. every row's
+// document starts after it.  Called by a whole warp; rows past Sq repeat the last row.
+LB_DEVICE bool doc_visit_empty(const int* doc_start, int S, int batch, int q0, int k0) {
+  const int lane = threadIdx.x % 32;
+  const int m = min(doc_begin(doc_start, S, batch, min(q0 + lane, S - 1)),
+                    doc_begin(doc_start, S, batch, min(q0 + 32 + lane, S - 1)));
+  return __reduce_min_sync(0xffffffffu, m) >= k0 + ATT_BWD_BN;
+}
+
+template <int D, int BIAS, bool DROP, bool DOC>
 __global__ void __launch_bounds__(ATT_BWD_THREADS, 1)
 attn_bwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_k,
                 const __grid_constant__ CUtensorMap tmap_v, const __grid_constant__ CUtensorMap tmap_do, AttnBwdParams p) {
+  static_assert(!DOC || (BIAS == BIAS_NONE && !DROP), "packed sequences run without bias and dropout");
   using Cfg = AttnBwdCfg<D>;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -548,24 +609,32 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
   __syncthreads();
 
   if (warp_idx == 4) {
-    if (elect_one()) {
+    const bool leader = elect_one();
+    if (leader) {
       mbar_arrive_expect_tx(kv_full, 2 * Cfg::TILE_BYTES);
 #pragma unroll
       for (int c = 0; c < Cfg::CHUNKS; ++c) {
         tma_load_4d(sK + c * (64 * 128), &tmap_k, kv_full, c * 64, k0, kv_head, batch);
         tma_load_4d(sV + c * (64 * 128), &tmap_v, kv_full, c * 64, k0, kv_head, batch);
       }
+    }
+    if (DOC || leader) {   // DOC: the whole warp takes the skip decisions, the leader loads
+      int ld = 0;          // visits loaded so far: the Q / dO ring position
       for (int step = 0; step < steps; ++step) {
         const int hi = step / iters;
-        const int st = step & 1;
         const int q0 = (i_begin + step - hi * iters) * ATT_BWD_BM;
-        mbar_wait(&qdo_empty[st], ((step >> 1) & 1) ^ 1);
+        if constexpr (DOC) {
+          if (doc_visit_empty(p.doc_start, p.Sq, batch, q0, k0) || !leader) continue;
+        }
+        const int st = ld & 1;
+        mbar_wait(&qdo_empty[st], ((ld >> 1) & 1) ^ 1);
         mbar_arrive_expect_tx(&qdo_full[st], 2 * Cfg::TILE_BYTES);
 #pragma unroll
         for (int c = 0; c < Cfg::CHUNKS; ++c) {
           tma_load_5d(sQ + st * Cfg::TILE_BYTES + c * (64 * 128), &tmap_q, &qdo_full[st], c * 64, q0, hi, kv_head, batch);
           tma_load_5d(sDO + st * Cfg::TILE_BYTES + c * (64 * 128), &tmap_do, &qdo_full[st], c * 64, q0, hi, kv_head, batch);
         }
+        ++ld;
       }
     }
     return;
@@ -596,6 +665,7 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
   }
   mbar_wait(kv_full, 0);
 
+  int ld = 0;   // visits loaded so far (the producer's ring position)
   for (int step = 0; step < steps; ++step) {
     const int hi = step / iters;
     const int it = step - hi * iters;
@@ -604,10 +674,17 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
     float slope2 = 0.f;
     if constexpr (BIAS == BIAS_ALIBI) slope2 = p.alibi_slopes[head] * LOG2E;
     const long bias_bh = batch * p.bias_strides[0] + head * p.bias_strides[1];
-    const int st = step & 1;
     const int q0 = (i_begin + it) * ATT_BWD_BM;
+    // DOC: a skipped visit leaves the dQ order counter alone.  Skipping is monotone in the key block (if kb is skipped,
+    // so is every kb' < kb of the same query block), so the key blocks above a contributing one all contribute and
+    // its wait for last_kb - kb_this counts exactly their additions.
+    if constexpr (DOC) {
+      if (doc_visit_empty(p.doc_start, p.Sq, batch, q0, k0)) continue;
+    }
+    const int st = ld & 1;
     const uint32_t q_addr = smem_u32(sQ + st * Cfg::TILE_BYTES), do_addr = smem_u32(sDO + st * Cfg::TILE_BYTES);
-    mbar_wait(&qdo_full[st], (step >> 1) & 1);
+    mbar_wait(&qdo_full[st], (ld >> 1) & 1);
+    ++ld;
     // ---- Sᵀ = K·Q_iᵀ, dPᵀ = V·dO_iᵀ (64 keys x 64 queries each)
     float sT[32], dpT[32];
     wgmma_fence();
@@ -638,6 +715,7 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
         const float lse2 = q_ok ? p.lse[bh * p.Sq + q_idx] * LOG2E : 0.f;
         const float delta_s = q_ok ? p.delta[bh * p.Sq + q_idx] * p.scale : 0.f;
         const int key_lim = !q_ok ? 0 : (p.causal ? min(kv_len, q_idx + off + 1) : kv_len);
+        const int key_lo = DOC && q_ok ? doc_begin(p.doc_start, p.Sq, batch, q_idx) : 0;   // the query's document
         uint4 rnd;
         if constexpr (DROP)   // both rows of this thread lie in the same 16-key group
           rnd = attn_dropout_bytes(static_cast<uint32_t>(q_idx), static_cast<uint32_t>((k0 + 16 * (t / 32)) >> 4),
@@ -654,7 +732,7 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
           } else if constexpr (BIAS == BIAS_ALIBI) {
             x = fmaf(slope2, static_cast<float>(kidx - q_idx - off), x);
           }
-          const float pv = kvis[h] < key_lim ? fast_exp2(x - lse2) : 0.f;
+          const float pv = kvis[h] < key_lim && (!DOC || kvis[h] >= key_lo) ? fast_exp2(x - lse2) : 0.f;
           float g = dpT[i], pd = pv;   // dP w.r.t. the dropped, rescaled P; what multiplied V in the forward
           if constexpr (DROP) {
             const bool keep = rnd_byte(rnd, (r_loc + 8 * h) & 15) >= p.drop_thresh;
@@ -847,11 +925,11 @@ int sm_count() {
   return n;
 }
 
-template <int D, int BIAS, bool DROP>
+template <int D, int BIAS, bool DROP, bool DOC = false>
 cudaError_t launch_bwd_t(const CUtensorMap& tq, const CUtensorMap& tk, const CUtensorMap& tv, const CUtensorMap& tdo,
                          const lb::AttnBwdParams& p, cudaStream_t s) {
   using Cfg = lb::AttnBwdCfg<D>;
-  auto kern = lb::attn_bwd_kernel<D, BIAS, DROP>;
+  auto kern = lb::attn_bwd_kernel<D, BIAS, DROP, DOC>;
   static bool configured = false;
   if (!configured) {
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES);
@@ -865,6 +943,7 @@ cudaError_t launch_bwd_t(const CUtensorMap& tq, const CUtensorMap& tk, const CUt
 template <int D>
 cudaError_t launch_bwd(const CUtensorMap& tq, const CUtensorMap& tk, const CUtensorMap& tv, const CUtensorMap& tdo,
                        const lb::AttnBwdParams& p, cudaStream_t s) {
+  if (p.doc_start != nullptr) return launch_bwd_t<D, lb::BIAS_NONE, false, true>(tq, tk, tv, tdo, p, s);
   const int bias = p.bias != nullptr ? lb::BIAS_DENSE : (p.alibi_slopes != nullptr ? lb::BIAS_ALIBI : lb::BIAS_NONE);
   const bool drop = p.drop_thresh > 0;
   if (bias == lb::BIAS_NONE) return drop ? launch_bwd_t<D, lb::BIAS_NONE, true>(tq, tk, tv, tdo, p, s) : launch_bwd_t<D, lb::BIAS_NONE, false>(tq, tk, tv, tdo, p, s);
@@ -880,13 +959,16 @@ extern "C" int lb_attn_bwd(const void* dout, const void* q, const void* k, const
                            const float* lse, void* dq, void* dk, void* dv, const long* dq_strides, const long* dkv_strides,
                            float* delta, float* dq_accum, int B, int A, int G, int Sq, int Sk, int D, const long* q_strides,
                            const long* k_strides, const long* v_strides, const long* do_strides, int causal, float scale,
-                           const int* kv_lens, const int* kv_start, const void* bias, const long* bias_strides,
-                           const float* alibi_slopes, float* dbias, float p_drop, const long long* rng_state,
-                           unsigned* dq_order, cudaStream_t s) {
+                           const int* kv_lens, const int* kv_start, const int* doc_start, const void* bias,
+                           const long* bias_strides, const float* alibi_slopes, float* dbias, float p_drop,
+                           const long long* rng_state, unsigned* dq_order, cudaStream_t s) {
   const int tile = head_dim_tile(D);
   if (tile == 0) return -1;
   if (Sq <= 0 || Sk <= 0) return -5;
   if (G <= 0 || A % G) return -4;
+  if (doc_start != nullptr && (!causal || Sq != Sk || kv_lens != nullptr || kv_start != nullptr || bias != nullptr ||
+                               alibi_slopes != nullptr || p_drop > 0.f))
+    return -6;
   const int r = A / G;
   for (int i = 0; i < 3; ++i)
     if ((q_strides[i] % 8) || (k_strides[i] % 8) || (v_strides[i] % 8) || (do_strides[i] % 8)) return -3;
@@ -931,6 +1013,7 @@ extern "C" int lb_attn_bwd(const void* dout, const void* q, const void* k, const
   p.scale_log2 = scale * 1.4426950408889634f;
   p.kv_lens = kv_lens;
   p.kv_start = kv_start;
+  p.doc_start = doc_start;
   p.bias = reinterpret_cast<const __nv_bfloat16*>(bias);
   for (int i = 0; i < 3; ++i) p.bias_strides[i] = (bias != nullptr && bias_strides != nullptr) ? bias_strides[i] : 0;
   p.alibi_slopes = bias != nullptr ? nullptr : alibi_slopes;

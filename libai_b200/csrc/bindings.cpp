@@ -38,7 +38,7 @@ int lb_swiglu_bwd(const void* gy, const void* gate, const void* up, void* dgate,
 int lb_swiglu_packed_fwd(const void* gu, void* y, long rows, long F, cudaStream_t s);
 int lb_swiglu_packed_bwd(const void* gy, const void* gu, void* dgu, long rows, long F, cudaStream_t s);
 int lb_rope_qkv(const void* x, const float* cosv, const float* sinv, void* y, long groups, int S, int G, int r, int D,
-                int pos_offset, int backward, cudaStream_t s);
+                int pos_offset, const int* positions, int npos, int backward, cudaStream_t s);
 int lb_rope(const void* x, const float* cosv, const float* sinv, void* y, long rows, int S, int D, int backward,
             cudaStream_t s);
 int lb_colsum_workspace_rows(int M, int N);
@@ -79,14 +79,16 @@ struct LbRngArgs {
 };
 int lb_attn_fwd(const void* q, const void* k, const void* v, void* o, float* lse, int B, int A, int G, int Sq, int Sk,
                 int D, const long* q_strides, const long* k_strides, const long* v_strides, int causal, float scale,
-                const int* kv_lens, const int* kv_start, const void* bias, const long* bias_strides,
-                const float* alibi_slopes, float p_drop, const LbRngArgs* rng, long long* rng_out, cudaStream_t s);
+                const int* kv_lens, const int* kv_start, const int* doc_start, const void* bias,
+                const long* bias_strides, const float* alibi_slopes, float p_drop, const LbRngArgs* rng,
+                long long* rng_out, cudaStream_t s);
 int lb_attn_bwd(const void* dout, const void* q, const void* k, const void* v, const void* o, const float* lse,
                 void* dq, void* dk, void* dv, const long* dq_strides, const long* dkv_strides, float* delta,
                 float* dq_accum, int B, int A, int G, int Sq, int Sk, int D, const long* q_strides, const long* k_strides,
                 const long* v_strides, const long* do_strides, int causal, float scale, const int* kv_lens,
-                const int* kv_start, const void* bias, const long* bias_strides, const float* alibi_slopes, float* dbias,
-                float p_drop, const long long* rng_state, unsigned* dq_order, cudaStream_t s);
+                const int* kv_start, const int* doc_start, const void* bias, const long* bias_strides,
+                const float* alibi_slopes, float* dbias, float p_drop, const long long* rng_state, unsigned* dq_order,
+                cudaStream_t s);
 int lb_bias_dropout_residual(const void* x, const void* bias, const void* res, void* y, long rows, int N, float p,
                              const LbRngArgs* rng, const long long* rng_in, long long* rng_out, cudaStream_t s);
 int lb_spin_timeout_report(char* buf, int n);
@@ -540,23 +542,37 @@ PackedQKV packed_qkv(const Tensor& qkv, const char* what) {
   return g;
 }
 
+// per-token int32 [B, S] tensor of a packed batch (rope positions, attention doc_start) → device pointer or nullptr
+const int* token_index(const c10::optional<Tensor>& t, const Tensor& like, int B, int S, const char* what) {
+  if (!(t.has_value() && t->defined())) return nullptr;
+  TORCH_CHECK(t->scalar_type() == at::kInt, what, ": int32 expected, got ", t->scalar_type());
+  TORCH_CHECK(t->dim() == 2 && t->size(0) == B && t->size(1) == S, what, ": [", B, ", ", S, "] expected, got shape ",
+              t->sizes());
+  TORCH_CHECK(t->is_cuda() && t->device() == like.device(), what, ": must be on ", like.device(), ", got ", t->device());
+  TORCH_CHECK(t->is_contiguous(), what, ": must be contiguous");
+  return t->data_ptr<int>();
+}
+
 // packed projection [b, s, a, 3d] or [b, s, g, r + 2, d]; rotates every q and k (v copied).  inplace=true rewrites qkv
-// itself.
+// itself.  positions (optional, int32 [b, s]): the position of every token (packed sequences), instead of
+// s + pos_offset; values outside the tables are clamped to them.
 Tensor rope_qkv(const Tensor& qkv, const Tensor& cosv, const Tensor& sinv, int64_t pos_offset, bool backward,
-                bool inplace) {
+                bool inplace, const c10::optional<Tensor>& positions) {
   c10::cuda::CUDAGuard guard(qkv.device());
   TORCH_CHECK(qkv.is_contiguous() && qkv.scalar_type() == at::kBFloat16, "rope_qkv: contiguous bf16 packed projection");
   const PackedQKV g = packed_qkv(qkv, "rope_qkv");
   const int S = g.S, D = g.D;
   TORCH_CHECK(D % 2 == 0, "rope_qkv: head dim must be even");
+  const int* pos = token_index(positions, qkv, g.B, S, "rope_qkv: positions");
   TORCH_CHECK(cosv.scalar_type() == at::kFloat && sinv.scalar_type() == at::kFloat && cosv.is_contiguous() &&
-                  sinv.is_contiguous() && cosv.size(0) >= S + pos_offset && cosv.size(1) == D &&
+                  sinv.is_contiguous() && cosv.size(0) >= (pos != nullptr ? 1 : S + pos_offset) && cosv.size(1) == D &&
                   sinv.sizes() == cosv.sizes(),
               "rope_qkv: cos/sin fp32 [>=S+offset, D]");
   TORCH_CHECK(cosv.device() == qkv.device() && sinv.device() == qkv.device(), "rope_qkv: cos/sin must be on qkv's device");
   Tensor y = inplace ? qkv : at::empty_like(qkv);
   check(lb_rope_qkv(qkv.data_ptr(), cosv.data_ptr<float>(), sinv.data_ptr<float>(), y.data_ptr(),
-                    qkv.numel() / ((g.r + 2) * D), S, g.G, g.r, D, (int)pos_offset, backward ? 1 : 0, cur_stream()),
+                    qkv.numel() / ((g.r + 2) * D), S, g.G, g.r, D, (int)pos_offset, pos, (int)cosv.size(0),
+                    backward ? 1 : 0, cur_stream()),
         "rope_qkv");
   return y;
 }
@@ -765,14 +781,28 @@ const int* key_bound(const c10::optional<Tensor>& t, const Tensor& q, int B, con
   return t->data_ptr<int>();
 }
 
+// doc_start (optional, int32 [B, S]): packed sequences, query i sees keys doc_start[b, i] <= j <= i (clamped to [0, i])
+const int* doc_starts(const c10::optional<Tensor>& doc_start, const Tensor& q, const QGeom& g, bool causal,
+                      bool other_masks, double p_drop, const char* what) {
+  const int* ds = token_index(doc_start, q, g.B, g.Sq, what);
+  TORCH_CHECK(ds == nullptr || (causal && g.Sq == g.Sk && !other_masks && p_drop == 0.0), what,
+              ": supported for causal self-attention (Sq == Sk) without kv_lens, kv_start, bias, ALiBi or dropout");
+  return ds;
+}
+
 // returns (o, lse, rng_state): rng_state int64[2] = (seed, offset) of the dropout mask (empty without dropout)
 std::tuple<Tensor, Tensor, Tensor> attn_fwd(const Tensor& q, const Tensor& k, const Tensor& v, bool causal, double scale,
                                             const c10::optional<Tensor>& kv_lens, const c10::optional<Tensor>& bias,
                                             const c10::optional<Tensor>& alibi_slopes, double p_drop, int64_t salt,
-                                            const c10::optional<Tensor>& kv_start) {
+                                            const c10::optional<Tensor>& kv_start, const c10::optional<Tensor>& doc_start) {
   c10::cuda::CUDAGuard guard(q.device());
   const QGeom g = q_geom(q, k, v, "attn_fwd");
   const int B = g.B, A = g.A, Sq = g.Sq, Sk = g.Sk, D = g.D;
+  const bool has_alibi = alibi_slopes.has_value() && alibi_slopes->defined();
+  const int* dst = doc_starts(doc_start, q, g, causal,
+                              (kv_lens.has_value() && kv_lens->defined()) || (kv_start.has_value() && kv_start->defined()) ||
+                                  (bias.has_value() && bias->defined()) || has_alibi,
+                              p_drop, "attn_fwd: doc_start");
   Tensor o = at::empty({B, Sq, A, D}, q.options());
   Tensor lse = at::empty({B, A, Sq}, q.options().dtype(at::kFloat));
   const long* qs = g.qs;
@@ -797,7 +827,7 @@ std::tuple<Tensor, Tensor, Tensor> attn_fwd(const Tensor& q, const Tensor& k, co
     rng_state = at::empty({0}, q.options().dtype(at::kLong));
   }
   check(lb_attn_fwd(q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(), lse.data_ptr<float>(), B, A, g.G, Sq, Sk, D, qs,
-                    ks, vs, causal ? 1 : 0, (float)scale, kvl, kvs, bd.ptr, bd.strides, slopes, (float)p_drop,
+                    ks, vs, causal ? 1 : 0, (float)scale, kvl, kvs, dst, bd.ptr, bd.strides, slopes, (float)p_drop,
                     drop ? &a : nullptr,
                     drop ? reinterpret_cast<long long*>(rng_state.data_ptr<int64_t>()) : nullptr, cur_stream()),
         "attn_fwd");
@@ -973,10 +1003,16 @@ std::tuple<Tensor, Tensor, Tensor, Tensor> attn_bwd(const Tensor& dout, const Te
                                             const c10::optional<Tensor>& kv_lens, const c10::optional<Tensor>& bias,
                                             const c10::optional<Tensor>& alibi_slopes, c10::optional<Tensor> dbias,
                                             double p_drop, const c10::optional<Tensor>& rng_state,
-                                            const c10::optional<Tensor>& kv_start) {
+                                            const c10::optional<Tensor>& kv_start,
+                                            const c10::optional<Tensor>& doc_start) {
   c10::cuda::CUDAGuard guard(q.device());
   const QGeom g = q_geom(q, k, v, "attn_bwd");
   const int B = g.B, A = g.A, G = g.G, Sq = g.Sq, Sk = g.Sk, D = g.D, r = A / G;
+  const int* dst = doc_starts(doc_start, q, g, causal,
+                              (kv_lens.has_value() && kv_lens->defined()) || (kv_start.has_value() && kv_start->defined()) ||
+                                  (bias.has_value() && bias->defined()) ||
+                                  (alibi_slopes.has_value() && alibi_slopes->defined()),
+                              p_drop, "attn_bwd: doc_start");
   // Sq == Sk: gradients are produced in the packed [B, S, G, r + 2, D] layout (r = 1: [B, S, A, 3, D]) so that the QKV
   // dgrad/wgrad GEMMs read them directly; dq comes back in q's shape (a copy only for a 4-D q with r > 1).
   // Sq != Sk: dq is [B, Sq, G, r, D] and dk, dv are packed as [B, Sk, G, 2, D]; the returned dqkv is empty.
@@ -1022,7 +1058,7 @@ std::tuple<Tensor, Tensor, Tensor, Tensor> attn_bwd(const Tensor& dout, const Te
   check(lb_attn_bwd(dout_c.data_ptr(), q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(), lse.data_ptr<float>(),
                     dq5.data_ptr(), dk.data_ptr(), dv.data_ptr(), dqs, dkvs, delta.data_ptr<float>(),
                     dq_acc.data_ptr<float>(), B, A, G, Sq, Sk, D, qs, ks, vs, ds, causal ? 1 : 0, (float)scale, kvl, kvs,
-                    bd.ptr, bd.strides,
+                    dst, bd.ptr, bd.strides,
                     (alibi_slopes.has_value() && alibi_slopes->defined()) ? alibi_slopes->data_ptr<float>() : nullptr, dbp,
                     (float)(has_rng ? p_drop : 0.0),
                     has_rng ? reinterpret_cast<const long long*>(rng_state->data_ptr<int64_t>()) : nullptr,
@@ -1174,13 +1210,13 @@ TORCH_LIBRARY(libai_b200, m) {
   m.def("swiglu_packed_bwd(Tensor gy, Tensor gu) -> Tensor", &swiglu_packed_bwd);
   m.def("dgrad_actgrad(Tensor gy, Tensor w, Tensor pre, int act, Tensor(a!)? bias_grad=None) -> Tensor", &dgrad_actgrad);
   m.def("rope(Tensor x, Tensor cos, Tensor sin, bool backward) -> Tensor", &rope);
-  m.def("rope_qkv(Tensor(a!) qkv, Tensor cos, Tensor sin, int pos_offset, bool backward, bool inplace) -> Tensor(a!)", &rope_qkv);
+  m.def("rope_qkv(Tensor(a!) qkv, Tensor cos, Tensor sin, int pos_offset, bool backward, bool inplace, Tensor? positions=None) -> Tensor(a!)", &rope_qkv);
   m.def("ce_stats(Tensor logits, Tensor labels, int vocab_start) -> (Tensor, Tensor, Tensor)", &ce_stats);
   m.def("ce_bwd(Tensor(a!) logits, Tensor labels, Tensor lse, Tensor gloss, int vocab_start) -> Tensor(a!)", &ce_bwd);
   m.def("fused_adamw(Tensor(a!) master, Tensor grad, Tensor(b!) m, Tensor(c!) v, Tensor? lp_out, Tensor scale, float lr, float b1, float b2, float eps, float wd, float bc1, float bc2, bool decoupled) -> ()", &fused_adamw);
   m.def("sqnorm(Tensor x) -> Tensor", &sqnorm);
-  m.def("attn_fwd(Tensor q, Tensor k, Tensor v, bool causal, float scale, Tensor? kv_lens, Tensor? bias=None, Tensor? alibi_slopes=None, float p_drop=0.0, int salt=0, Tensor? kv_start=None) -> (Tensor, Tensor, Tensor)", &attn_fwd);
-  m.def("attn_bwd(Tensor dout, Tensor q, Tensor k, Tensor v, Tensor o, Tensor lse, bool causal, float scale, Tensor? kv_lens, Tensor? bias=None, Tensor? alibi_slopes=None, Tensor(a!)? dbias=None, float p_drop=0.0, Tensor? rng_state=None, Tensor? kv_start=None) -> (Tensor, Tensor, Tensor, Tensor)", &attn_bwd);
+  m.def("attn_fwd(Tensor q, Tensor k, Tensor v, bool causal, float scale, Tensor? kv_lens, Tensor? bias=None, Tensor? alibi_slopes=None, float p_drop=0.0, int salt=0, Tensor? kv_start=None, Tensor? doc_start=None) -> (Tensor, Tensor, Tensor)", &attn_fwd);
+  m.def("attn_bwd(Tensor dout, Tensor q, Tensor k, Tensor v, Tensor o, Tensor lse, bool causal, float scale, Tensor? kv_lens, Tensor? bias=None, Tensor? alibi_slopes=None, Tensor(a!)? dbias=None, float p_drop=0.0, Tensor? rng_state=None, Tensor? kv_start=None, Tensor? doc_start=None) -> (Tensor, Tensor, Tensor, Tensor)", &attn_bwd);
   m.def("kv_append(Tensor qkv, Tensor(a!) k_cache, Tensor(b!) v_cache, Tensor cache_seqlens, Tensor? cos, Tensor? sin, bool write_q) -> Tensor", &kv_append);
   m.def("window_attn_fwd(Tensor qkv, int H, int W, int window, int shift, int heads, float scale, Tensor table, Tensor? tau) -> (Tensor, Tensor)", &window_attn_fwd);
   m.def("window_attn_bwd(Tensor dout, Tensor qkv, Tensor lse, int H, int W, int window, int shift, int heads, float scale, Tensor table, Tensor? tau) -> (Tensor, Tensor, Tensor)", &window_attn_bwd);

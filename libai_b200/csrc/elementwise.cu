@@ -228,11 +228,15 @@ __global__ void rope_kernel(const __nv_bfloat16* __restrict__ x, const float* __
 }
 
 // Rotary embedding on the grouped packed QKV projection [tokens(b*s), G, r + 2, D] (per K/V group q_0 .. q_{r-1}, k, v;
-// r = 1 is the per-head [q|k|v] layout): the r + 1 q/k slots are rotated with the position (s + pos_offset), v is
-// copied.  `y` may alias `x` (in-place, used by the backward).
+// r = 1 is the per-head [q|k|v] layout): the r + 1 q/k slots are rotated with the position (s + pos_offset), or with
+// positions[token] (int32 [tokens], packed sequences; clamped to the npos rows of the tables) when given, v is
+// copied.  `y` may alias `x` (in-place, used by the backward).  POS: positions given (a separate instance, so the
+// s + pos_offset instance compiles to the same arithmetic as kv_append_kernel, with which it is bit-identical).
+template <bool POS>
 __global__ void rope_qkv_kernel(const __nv_bfloat16* __restrict__ x, const float* __restrict__ cosv,
                                 const float* __restrict__ sinv, __nv_bfloat16* __restrict__ y, size_t groups, int S,
-                                int G, int r, int D, int pos_offset, int backward, int copy_v) {
+                                int G, int r, int D, int pos_offset, const int* __restrict__ positions, int npos,
+                                int backward, int copy_v) {
   const int half = D / 2;
   const int parts = copy_v ? r + 2 : r + 1;
   const size_t total = groups * parts * half;
@@ -247,7 +251,7 @@ __global__ void rope_qkv_kernel(const __nv_bfloat16* __restrict__ x, const float
       y[base + c + half] = x[base + c + half];
       continue;
     }
-    const int s = static_cast<int>((head / G) % S) + pos_offset;
+    const int s = POS ? min(max(positions[head / G], 0), npos - 1) : static_cast<int>((head / G) % S) + pos_offset;
     const float c1 = cosv[s * D + c], c2 = cosv[s * D + c + half];
     const float s1 = sinv[s * D + c], s2 = sinv[s * D + c + half];
     float y1, y2;
@@ -656,13 +660,19 @@ extern "C" int lb_rope(const void* x, const float* cosv, const float* sinv, void
                                                                      (size_t)rows, S, D, backward);
   return (int)cudaGetLastError();
 }
-// groups = tokens * G; r query heads per group
+// groups = tokens * G; r query heads per group; positions (optional, int32 [tokens]) replaces s + pos_offset, npos =
+// rows of the cos / sin tables
 extern "C" int lb_rope_qkv(const void* x, const float* cosv, const float* sinv, void* y, long groups, int S, int G, int r,
-                           int D, int pos_offset, int backward, cudaStream_t s) {
+                           int D, int pos_offset, const int* positions, int npos, int backward, cudaStream_t s) {
   if (groups == 0) return 0;
   const int copy_v = (x != y);
-  lb::rope_qkv_kernel<<<ew_grid((size_t)groups * (copy_v ? r + 2 : r + 1) * D / 2, 256), 256, 0, s>>>(
-      (const bf16*)x, cosv, sinv, (bf16*)y, (size_t)groups, S, G, r, D, pos_offset, backward, copy_v);
+  const dim3 grid = ew_grid((size_t)groups * (copy_v ? r + 2 : r + 1) * D / 2, 256);
+  if (positions != nullptr)
+    lb::rope_qkv_kernel<true><<<grid, 256, 0, s>>>((const bf16*)x, cosv, sinv, (bf16*)y, (size_t)groups, S, G, r, D,
+                                                   pos_offset, positions, npos, backward, copy_v);
+  else
+    lb::rope_qkv_kernel<false><<<grid, 256, 0, s>>>((const bf16*)x, cosv, sinv, (bf16*)y, (size_t)groups, S, G, r, D,
+                                                    pos_offset, positions, npos, backward, copy_v);
   return (int)cudaGetLastError();
 }
 // rows per block of the column-sum pass; the number of row blocks is the row count of its fp32 workspace [.., N]

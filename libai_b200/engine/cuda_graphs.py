@@ -15,8 +15,9 @@ AG→GEMM / GEMM→RS kernels keep their call counters, arrival targets and writ
 themselves, so a replay is indistinguishable from a fresh launch.
 
 Not captured: embedding, LM head + loss, optimizer, NCCL collectives.  Restrictions (checked): besides the hidden state a
-block may take model buffers as keyword tensors (RoPE tables — Llama) and a right-padded ``KeyPaddingMask`` (BERT,
-RoBERTa: its key lengths become a second graph input); no activation checkpointing.  Dropout inside captured blocks draws its Philox offset
+block may take model buffers as keyword tensors (RoPE tables — Llama), a right-padded ``KeyPaddingMask`` (BERT,
+RoBERTa: its key lengths become a second graph input) and the per-batch int32 ``position_ids`` / ``doc_start`` of a
+packed batch (Llama family: more graph inputs, read by the kernels on the device); no activation checkpointing.  Dropout inside captured blocks draws its Philox offset
 from a device counter that the dropout kernels advance (``ops/functional.py``), so replays produce fresh masks.
 """
 from __future__ import annotations
@@ -94,21 +95,28 @@ class BlockCallSpec:
     * ``const_kwargs`` – keyword tensors that are buffers of the model (RoPE cos/sin tables): the same storage on every
       call, so the captured kernels simply keep reading it;
     * ``key_lengths`` – the block takes a ``KeyPaddingMask`` as second positional argument (BERT / RoBERTa): its
-      per-sample key lengths (int32 ``[b]``) become a second *graph input*, copied into the static buffer on replay.
+      per-sample key lengths (int32 ``[b]``) become a second *graph input*, copied into the static buffer on replay;
+    * ``batch_kwargs`` – per-batch keyword tensors of a packed batch (``position_ids`` / ``doc_start``, int32
+      ``[b, s]``): further graph inputs, in this order after the key lengths.
     """
 
-    def __init__(self, const_kwargs=None, key_lengths: Optional[torch.Tensor] = None):
+    def __init__(self, const_kwargs=None, key_lengths: Optional[torch.Tensor] = None, batch_kwargs=None):
         self.const_kwargs = dict(const_kwargs or {})
         self.key_lengths = key_lengths
+        self.batch_kwargs = dict(batch_kwargs or {})
 
     @property
     def trivial(self) -> bool:
-        return not self.const_kwargs and self.key_lengths is None
+        return not self.const_kwargs and self.key_lengths is None and not self.batch_kwargs
 
     def matches(self, args, kwargs) -> bool:
         """Can this call be served by the captured graph?  (Otherwise the caller runs the eager block.)"""
         live = {k: v for k, v in kwargs.items() if v is not None}
+        per_batch = {k: live.pop(k) for k in list(live) if k in self.batch_kwargs}
         if set(live) != set(self.const_kwargs) or any(live[k] is not self.const_kwargs[k] for k in live):
+            return False
+        if set(per_batch) != set(self.batch_kwargs) or any(
+                v.shape != self.batch_kwargs[k].shape or v.dtype != self.batch_kwargs[k].dtype for k, v in per_batch.items()):
             return False
         if self.key_lengths is None:
             return len(args) == 0
@@ -119,8 +127,18 @@ class BlockCallSpec:
         m = args[0]
         return (isinstance(m, KeyPaddingMask) and m.lengths.shape == self.key_lengths.shape and m.is_prefix())
 
-    def graph_inputs(self, args):
-        return (args[0].lengths,) if self.key_lengths is not None else ()
+    def graph_inputs(self, args, kwargs=None):
+        lengths = (args[0].lengths,) if self.key_lengths is not None else ()
+        return lengths + tuple(kwargs[k] for k in self.batch_kwargs)
+
+    def call_kwargs(self, extra):
+        """Keyword arguments of a block call from the graph inputs after the hidden state (key lengths excluded)."""
+        return {**self.const_kwargs, **dict(zip(self.batch_kwargs, extra))}
+
+
+# per-batch keyword tensors a block may take inside a graph (packed batches of the Llama family); the kernels read them
+# on the device, so a replay only copies them into the captured static buffers
+BATCH_KWARGS = ("position_ids", "doc_start")
 
 
 def classify_block_call(model: nn.Module, args, kwargs) -> Optional[BlockCallSpec]:
@@ -128,9 +146,12 @@ def classify_block_call(model: nn.Module, args, kwargs) -> Optional[BlockCallSpe
     from libai_b200.layers.attention import KeyPaddingMask
 
     buffers = {id(b) for b in model.buffers()}
-    const = {}
+    const, per_batch = {}, {}
     for k, v in kwargs.items():
         if v is None:
+            continue
+        if k in BATCH_KWARGS and torch.is_tensor(v) and v.is_cuda and v.dtype == torch.int32:
+            per_batch[k] = v
             continue
         if not (torch.is_tensor(v) and id(v) in buffers):
             return None
@@ -139,9 +160,9 @@ def classify_block_call(model: nn.Module, args, kwargs) -> Optional[BlockCallSpe
     while args and args[-1] is None:
         args.pop()
     if not args:
-        return BlockCallSpec(const)
+        return BlockCallSpec(const, batch_kwargs=per_batch)
     if len(args) == 1 and isinstance(args[0], KeyPaddingMask) and args[0].is_prefix():
-        return BlockCallSpec(const, args[0].lengths)
+        return BlockCallSpec(const, args[0].lengths, per_batch)
     return None
 
 
@@ -154,18 +175,19 @@ class _EagerBlock:
         self.fn = block.forward
         self.spec = spec or BlockCallSpec()
 
-    def __call__(self, hidden, lengths=None):
-        if lengths is None:
-            return self.fn(hidden, **self.spec.const_kwargs)
+    def __call__(self, hidden, *extra):
+        if self.spec.key_lengths is None:
+            return self.fn(hidden, **self.spec.call_kwargs(extra))
         from libai_b200.layers.attention import KeyPaddingMask
 
-        return self.fn(hidden, KeyPaddingMask.from_lengths(lengths), **self.spec.const_kwargs)
+        return self.fn(hidden, KeyPaddingMask.from_lengths(extra[0]), **self.spec.call_kwargs(extra[1:]))
 
 
 def graph_blocks_multi_slot(blocks: Sequence[nn.Module], sample_hidden: torch.Tensor, n_slots: int, warmup_iters: int = 3,
                             spec: Optional[BlockCallSpec] = None) -> bool:
     spec = spec or BlockCallSpec()
-    extra = (spec.key_lengths.detach().clone(),) if spec.key_lengths is not None else ()
+    extra = ((spec.key_lengths.detach().clone(),) if spec.key_lengths is not None else ()) + tuple(
+        t.detach().clone() for t in spec.batch_kwargs.values())
     with torch.no_grad():
         n0 = ops.launch_count()
         _EagerBlock(blocks[0], spec)(sample_hidden.detach(), *extra)
@@ -194,7 +216,7 @@ def graph_blocks_multi_slot(blocks: Sequence[nn.Module], sample_hidden: torch.Te
                     and hidden.shape == sample_hidden.shape and spec.matches(args, kwargs)):
                 return _eager(hidden, *args, **kwargs)
             ops.count_launch(fwd_kernels + bwd_kernels)
-            return _slots[_CURRENT_SLOT % len(_slots)](hidden, *spec.graph_inputs(args))
+            return _slots[_CURRENT_SLOT % len(_slots)](hidden, *spec.graph_inputs(args, kwargs))
 
         block.forward = forward
     return True
@@ -249,7 +271,8 @@ def _enable_for_model(model: nn.Module, example_batch: dict, topo) -> bool:
     h.remove()
     spec = classify_block_call(model, shapes.get("args", ()), shapes.get("kwargs", {})) if torch.is_tensor(shapes.get("hidden")) else None
     if spec is None:
-        logger.warning("cuda graphs: blocks take arguments that are neither model buffers nor a right-padded key mask — not captured")
+        logger.warning("cuda graphs: blocks take arguments that are neither model buffers, a right-padded key mask nor "
+                       "packed-batch positions — not captured")
         return False
     try:
         if spec.trivial:

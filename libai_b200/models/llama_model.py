@@ -48,6 +48,14 @@ def rotary_tables(rotary_dim: int, seq_len: int, base: float = 10000.0, device=N
     return emb.cos().contiguous(), emb.sin().contiguous()
 
 
+def packed_positions(position_ids):
+    """int32 ``(position_ids, doc_start)`` of a packed batch: ``position_ids[b, i]`` is the index of token ``i`` inside
+    its document, so ``doc_start[b, i] = i - position_ids[b, i]`` is the first token of that document (the flash
+    kernels' per-query key window, see :func:`OF.visible_keys`)."""
+    pos = position_ids.to(torch.int32).contiguous()
+    return pos, (torch.arange(pos.shape[1], dtype=torch.int32, device=pos.device)[None] - pos).contiguous()
+
+
 class RotaryEmbedding(nn.Module):
     """``cos, sin = rope(x, seq_len)`` — fp32 tables ``[seq_len, dim]`` on ``x``'s device, cached up to the longest
     length requested (reference projects/Llama/llama.py:46-63 returns slices of tables the model owns; the attention
@@ -143,7 +151,9 @@ class LlamaAttention(nn.Module):
                              init_method=output_layer_init_method, layer_idx=layer_idx)
 
     def forward(self, hidden_states, attention_mask=None, past_key_value=None, cos_cached=None, sin_cached=None,
-                use_cache=False):
+                use_cache=False, position_ids=None, doc_start=None):
+        """``position_ids`` / ``doc_start`` (int32 ``[b, s]``, from :func:`packed_positions`): a packed batch, whose
+        rotary positions and causal attention restart at every document."""
         sp = dutil.get_dist_util().sequence_parallel and hidden_states.dim() == 2
         a, d, g = self.local_heads, self.head_size, self.local_kv_heads
         bsz, tgt_len = get_sp_shape() if sp else hidden_states.shape[:2]
@@ -155,12 +165,13 @@ class LlamaAttention(nn.Module):
             output = self.o_proj(context)
             return (output, past_key_value) if use_cache else output
         past_len = 0 if past_key_value is None else past_key_value[0].shape[2]
-        qkv = OF.apply_rotary_qkv(qkv, cos_cached, sin_cached, past_len)
+        qkv = OF.apply_rotary_qkv(qkv, cos_cached, sin_cached, past_len, position_ids)
         if (
             past_key_value is None and not use_cache and attention_mask is None
-            and OF.attention_qkvpacked_supported(qkv, None, 0.0, self.training)
+            and OF.attention_qkvpacked_supported(qkv, None, 0.0, self.training, doc_start)
         ):
-            context = OF.attention_qkvpacked(qkv, causal=True, scale=self.norm_factor).reshape(bsz, -1, a * d)
+            context = OF.attention_qkvpacked(qkv, causal=True, scale=self.norm_factor,
+                                             doc_start=doc_start).reshape(bsz, -1, a * d)
         else:
             query, key, value = (t.permute(0, 2, 1, 3) for t in OF.split_qkv(qkv))   # key, value: g heads
             if past_key_value is not None:
@@ -172,6 +183,10 @@ class LlamaAttention(nn.Module):
             mask = attention_mask
             if mask is None and not causal:  # decoding with a cache: every cached key is visible
                 mask = None
+            if doc_start is not None:   # packed sequences: causal within each document
+                mask = OF.visible_keys(query.shape[2], key.shape[2], causal=True, doc_start=doc_start,
+                                       device=query.device)
+                causal = False
             context = OF.attention(query, key, value, causal=causal, scale=self.norm_factor, mask=mask)
             context = context.transpose(1, 2).reshape(bsz, -1, a * d)
         if sp:
@@ -236,10 +251,12 @@ class LlamaDecoderLayer(nn.Module):
         self.mlp = LlamaMLP(hidden_size, intermediate_size, init_method, output_layer_init_method, layer_idx=layer_idx)
 
     def forward(self, hidden_states, attention_mask=None, past_key_value=None, cos_cached=None, sin_cached=None,
-                use_cache=False):
+                use_cache=False, position_ids=None, doc_start=None):
+        # (only a packed batch passes its positions: attention subclasses without packing keep their signature)
+        packed = {} if position_ids is None else dict(position_ids=position_ids, doc_start=doc_start)
         attn = self.self_attn(self.input_layernorm(hidden_states), attention_mask=attention_mask,
                               past_key_value=past_key_value, cos_cached=cos_cached, sin_cached=sin_cached,
-                              use_cache=use_cache)
+                              use_cache=use_cache, **packed)
         presents = None
         if use_cache:
             attn, presents = attn
@@ -288,7 +305,8 @@ class LlamaModel(nn.Module):
             return self.embed_tokens(input_ids, scatter_to_sequence_parallel=True)
         return self.embed_tokens(input_ids)
 
-    def forward(self, input_ids, attention_mask=None, past_key_values=None, use_cache=False, set_cache=None):
+    def forward(self, input_ids, attention_mask=None, past_key_values=None, use_cache=False, set_cache=None,
+                position_ids=None):
         if isinstance(past_key_values, StaticKVCache):
             # the layers append in place; the lengths advance once every layer has seen this step's tokens
             cache = past_key_values
@@ -301,11 +319,13 @@ class LlamaModel(nn.Module):
             cache.advance(input_ids.shape[1])
             return self.norm(hidden_states)
         presents = [] if use_cache else None
+        pos, doc = packed_positions(position_ids) if position_ids is not None else (None, None)
         hidden_states = self.embed(input_ids)
         past_key_values = past_key_values or [None] * len(self.layers)
         for layer, past in zip(self.layers, past_key_values):
             hidden_states = layer(hidden_states, attention_mask=attention_mask, past_key_value=past,
-                                  cos_cached=self.cos_cached, sin_cached=self.sin_cached, use_cache=use_cache)
+                                  cos_cached=self.cos_cached, sin_cached=self.sin_cached, use_cache=use_cache,
+                                  position_ids=pos, doc_start=doc)
             if use_cache:
                 hidden_states, present = hidden_states
                 presents.append(present)
@@ -390,7 +410,19 @@ class LlamaForCausalLM(nn.Module, PipelineStageMixin, Generator, KVCacheOwner):
         return self.model.layers
 
     def stage_layer_call(self, layer, hidden, batch):
-        return layer(hidden, cos_cached=self.model.cos_cached, sin_cached=self.model.sin_cached)
+        return layer(hidden, cos_cached=self.model.cos_cached, sin_cached=self.model.sin_cached,
+                     position_ids=batch.get("position_ids"), doc_start=batch.get("doc_start"))
+
+    def forward_stage(self, batch, hidden_in=None):
+        # a packed batch: the int32 positions and document starts are derived once per forward, for every block
+        if batch.get("position_ids") is not None and batch.get("doc_start") is None:
+            lo, hi = (int(x) for x in batch["position_ids"].aminmax())   # one host sync per forward, outside the blocks
+            if lo < 0 or hi >= self.model.cos_cached.shape[0]:
+                raise ValueError(f"position_ids must lie in [0, {self.model.cos_cached.shape[0]}) "
+                                 f"(max_position_embeddings), got [{lo}, {hi}]")
+            pos, doc = packed_positions(batch["position_ids"])
+            batch = {**batch, "position_ids": pos, "doc_start": doc}
+        return super().forward_stage(batch, hidden_in)
 
     def stage_post(self, hidden, labels=None, **_):
         logits = self.lm_head(self.model.norm(hidden))
@@ -405,9 +437,17 @@ class LlamaForCausalLM(nn.Module, PipelineStageMixin, Generator, KVCacheOwner):
             logits = logits.view(b, s, -1)
         return mappings.gather_from_tp(logits) if topo.tensor_parallel_size > 1 else logits
 
-    def forward(self, input_ids, attention_mask=None, labels=None, use_cache=False):
+    def forward(self, input_ids, attention_mask=None, labels=None, use_cache=False, position_ids=None):
+        """``position_ids`` (int ``[b, s]``): a packed batch (several documents per row, e.g. from
+        ``PackedSFTDataset``), each token's index inside its own document; attention and rotary positions restart at
+        every document.  A training / scoring input: not with ``attention_mask`` or the KV cache."""
+        if position_ids is not None and (use_cache or attention_mask is not None):
+            raise ValueError("position_ids (packed sequences) cannot be combined with attention_mask or use_cache")
         if not use_cache and attention_mask is None:
-            return self.forward_stage({"input_ids": input_ids, "labels": labels})
+            batch = {"input_ids": input_ids, "labels": labels}
+            if position_ids is not None:
+                batch["position_ids"] = position_ids
+            return self.forward_stage(batch)
         # generation / padded batches: explicit masks and the KV cache (single pipeline stage)
         if not use_cache:
             mask = None if attention_mask is None else self.casual_mask(input_ids, attention_mask=attention_mask)

@@ -585,14 +585,19 @@ def attention_ref(q, k, v, *, causal: bool, scale: float, mask=None, bias=None, 
     return torch.matmul(probs, v.float()).to(q.dtype)
 
 
-def visible_keys(sq: int, sk: int, *, causal: bool, kv_start=None, kv_lens=None, device=None):
+def visible_keys(sq: int, sk: int, *, causal: bool, kv_start=None, kv_lens=None, doc_start=None, device=None):
     """Boolean ``[b|1, 1, sq, sk]`` visibility of the flash kernels: key ``j`` is visible to query ``i`` of sample ``b``
     iff ``kv_start[b] <= j < max(1, kv_lens[b])`` (defaults ``0`` and ``sk``) and, when ``causal``,
-    ``j <= i + sk - sq`` (bottom-right alignment)."""
+    ``j <= i + sk - sq`` (bottom-right alignment).  ``doc_start`` (int ``[b, sq]``, packed sequences) adds
+    ``j >= doc_start[b, i]``, with ``doc_start`` clamped to ``[0, i]`` so that every query sees itself."""
     j = torch.arange(sk, device=device)
     vis = torch.ones(1, sq, sk, dtype=torch.bool, device=device)
     if causal:
         vis = vis & (j[None, :] <= torch.arange(sq, device=device)[:, None] + (sk - sq))[None]
+    if doc_start is not None:
+        i = torch.arange(sq, device=device)
+        beg = torch.minimum(doc_start.to(device=device, dtype=torch.long).clamp(min=0), i[None, :])
+        vis = vis & (j[None, None, :] >= beg[:, :, None])
     if kv_start is not None:
         vis = vis & (j[None, None, :] >= kv_start.to(device=device, dtype=torch.long)[:, None, None])
     if kv_lens is not None:
@@ -664,25 +669,25 @@ class _FlashAttnPackedFn(torch.autograd.Function):
     ``dqkv`` of the same layout – no slicing, no expanded K/V, no gradient accumulation kernels around the attention."""
 
     @staticmethod
-    def forward(ctx, qkv, causal, scale, kv_lens, p_drop=0.0, alibi_slopes=None):
+    def forward(ctx, qkv, causal, scale, kv_lens, p_drop=0.0, alibi_slopes=None, doc_start=None):
         ext = load_ext()
         q, k, v = _packed_views(qkv)
         o, lse, rng_state = ext.attn_fwd(q, k, v, causal, scale, kv_lens, None, alibi_slopes, p_drop,
-                                         tp_rng_salt(True) if p_drop > 0 else 0)
+                                         tp_rng_salt(True) if p_drop > 0 else 0, None, doc_start)
         count_launch()
-        ctx.save_for_backward(qkv, o, lse, kv_lens, rng_state, alibi_slopes)
+        ctx.save_for_backward(qkv, o, lse, kv_lens, rng_state, alibi_slopes, doc_start)
         ctx.causal, ctx.scale, ctx.p_drop = causal, scale, p_drop
         return o.permute(0, 2, 1, 3)  # [b, s, a, d] contiguous
 
     @staticmethod
     def backward(ctx, go):
         ext = load_ext()
-        qkv, o, lse, kv_lens, rng_state, slopes = ctx.saved_tensors
+        qkv, o, lse, kv_lens, rng_state, slopes, doc_start = ctx.saved_tensors
         q, k, v = _packed_views(qkv)
         _, _, _, dqkv = ext.attn_bwd(go.permute(0, 2, 1, 3), q, k, v, o, lse, ctx.causal, ctx.scale, kv_lens, None, slopes,
-                                     None, ctx.p_drop, rng_state if ctx.p_drop > 0 else None)
+                                     None, ctx.p_drop, rng_state if ctx.p_drop > 0 else None, None, doc_start)
         count_launch(3)
-        return dqkv.view(qkv.shape), None, None, None, None, None
+        return dqkv.view(qkv.shape), None, None, None, None, None, None
 
 
 def flash_head_dim_supported(d: int) -> bool:
@@ -691,25 +696,28 @@ def flash_head_dim_supported(d: int) -> bool:
     return d % 8 == 0 and 8 <= d <= 128
 
 
-def attention_qkvpacked_supported(qkv, mask, dropout_p, training) -> bool:
+def attention_qkvpacked_supported(qkv, mask, dropout_p, training, doc_start=None) -> bool:
     """True when :func:`attention_qkvpacked` runs the native flash kernels: a contiguous bf16 projection on the GPU
-    whose head dim :func:`flash_head_dim_supported` accepts, and no dense ``mask``."""
+    whose head dim :func:`flash_head_dim_supported` accepts, and no dense ``mask``; packed sequences (``doc_start``)
+    also need no attention dropout in training."""
     return (
         use_native(qkv)
         and qkv.dtype == torch.bfloat16
         and mask is None
         and flash_head_dim_supported(packed_head_dim(qkv))
         and qkv.is_contiguous()
+        and (doc_start is None or not (training and dropout_p > 0))
     )
 
 
 def attention_qkvpacked(qkv, *, causal: bool, scale: float, kv_lens=None, dropout_p: float = 0.0, training: bool = False,
-                        alibi_slopes=None):
+                        alibi_slopes=None, doc_start=None):
     """qkv ``[b, s, a, 3d]`` or grouped ``[b, s, g, r + 2, d]`` → context ``[b, s, a, d]``; ``kv_lens`` (int32 ``[b]``): valid keys per sample
     of a right-padded batch (keys beyond it are masked inside the kernel); ``dropout_p`` > 0 in training drops
-    attention probabilities inside the kernel (Philox, TP-rank salted)."""
+    attention probabilities inside the kernel (Philox, TP-rank salted).  ``doc_start`` (int32 ``[b, s]``, causal
+    only): packed sequences, query ``i`` sees the keys ``doc_start[b, i] <= j <= i`` (see :func:`visible_keys`)."""
     p = float(dropout_p) if training else 0.0
-    return _FlashAttnPackedFn.apply(qkv, causal, float(scale), kv_lens, p, alibi_slopes)
+    return _FlashAttnPackedFn.apply(qkv, causal, float(scale), kv_lens, p, alibi_slopes, doc_start)
 
 
 def attention_supported(q, k, mask=None, bias=None) -> bool:
@@ -1052,37 +1060,41 @@ class _RopeQKVFn(torch.autograd.Function):
     the backward rotates the packed ``dqkv`` of the attention kernel in place with the inverse rotation."""
 
     @staticmethod
-    def forward(ctx, qkv, cos, sin, pos_offset):
+    def forward(ctx, qkv, cos, sin, pos_offset, positions=None):
         ext = load_ext()
-        ctx.save_for_backward(cos, sin)
+        ctx.save_for_backward(cos, sin, positions)
         ctx.pos_offset = pos_offset
         count_launch()
-        return ext.rope_qkv(qkv, cos, sin, pos_offset, False, False)
+        return ext.rope_qkv(qkv, cos, sin, pos_offset, False, False, positions)
 
     @staticmethod
     def backward(ctx, g):
         ext = load_ext()
-        cos, sin = ctx.saved_tensors
+        cos, sin, positions = ctx.saved_tensors
         count_launch()
         g = g if g.is_contiguous() else g.contiguous()
-        return ext.rope_qkv(g, cos, sin, ctx.pos_offset, True, True), None, None, None
+        return ext.rope_qkv(g, cos, sin, ctx.pos_offset, True, True, positions), None, None, None, None
 
 
-def apply_rotary_qkv(qkv, cos, sin, pos_offset: int = 0):
+def apply_rotary_qkv(qkv, cos, sin, pos_offset: int = 0, position_ids=None):
     """qkv ``[b, s, a, 3d]`` (per-head ``[q|k|v]``) or grouped ``[b, s, g, r + 2, d]`` (per group ``q_0 .. q_{r-1}, k,
-    v``); cos/sin fp32 ``[max_pos, d]``; token ``i`` of the sequence uses position ``i + pos_offset``."""
+    v``); cos/sin fp32 ``[max_pos, d]``; token ``i`` of the sequence uses position ``i + pos_offset``, or
+    ``position_ids[b, i]`` (int32 ``[b, s]``, packed sequences; clamped to the tables) when given."""
     if use_native(qkv) and qkv.dtype == torch.bfloat16 and cos.dtype == torch.float32 and qkv.is_contiguous():
-        return _RopeQKVFn.apply(qkv, cos, sin, int(pos_offset))
+        return _RopeQKVFn.apply(qkv, cos, sin, int(pos_offset), position_ids)
     s_len = qkv.shape[1]
+    if position_ids is not None:   # [b, s, 1, d] (+ a group axis below)
+        idx = position_ids.to(device=cos.device, dtype=torch.long).clamp(0, cos.shape[0] - 1)
+        c, sn = cos[idx][:, :, None, :].to(qkv.dtype), sin[idx][:, :, None, :].to(qkv.dtype)
+    else:
+        c = cos[pos_offset : pos_offset + s_len, None, :].to(qkv.dtype)
+        sn = sin[pos_offset : pos_offset + s_len, None, :].to(qkv.dtype)
     if qkv.dim() == 5:
         r = qkv.shape[3] - 2
-        c = cos[pos_offset : pos_offset + s_len, None, None, :].to(qkv.dtype)
-        sn = sin[pos_offset : pos_offset + s_len, None, None, :].to(qkv.dtype)
+        c, sn = c.unsqueeze(-2), sn.unsqueeze(-2)
         qk = qkv[..., : r + 1, :]
         return torch.cat([qk * c + rotate_half(qk) * sn, qkv[..., r + 1 :, :]], dim=3)
     d = qkv.shape[-1] // 3
-    c = cos[pos_offset : pos_offset + s_len, None, :].to(qkv.dtype)
-    sn = sin[pos_offset : pos_offset + s_len, None, :].to(qkv.dtype)
     q, k, v = qkv[..., :d], qkv[..., d : 2 * d], qkv[..., 2 * d :]
     return torch.cat([q * c + rotate_half(q) * sn, k * c + rotate_half(k) * sn, v], dim=-1)
 

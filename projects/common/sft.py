@@ -2,6 +2,8 @@
 
 * ``SFTDataset`` — ``torch.save``-d list of ``{"input_ids", "labels"}`` produced by ``prepare_sft_corpus``
   (reference projects/Llama/dataset.py:8-22 and its copies in the sibling projects);
+* ``PackedSFTDataset`` — the same corpus packed several samples to a row, with per-document ``position_ids`` (the
+  Llama family attends and rotates per document, so no compute goes to padding between samples);
 * ``generate_prompt`` / ``prepare_sample`` / ``prepare_sft_corpus`` — Alpaca-style prompt construction, tokenisation,
   prompt masking (label −1 = ignored) and fixed-length padding (reference projects/Llama/utils/prepare_alpaca.py);
 * ``SentencePieceTokenizer`` — the minimal sentencepiece wrapper those projects use (reference
@@ -35,6 +37,78 @@ class SFTDataset(Dataset):
         return Instance(
             input_ids=DistTensorData(torch.as_tensor(item["input_ids"], dtype=torch.long)),
             labels=DistTensorData(torch.as_tensor(item["labels"], dtype=torch.long), placement_idx=-1),
+        )
+
+
+def sample_length(labels) -> int:
+    """Tokens of a prepared sample that matter for training: up to the input that predicts its last trainable label
+    (label > 0; ``SFTLoss`` ignores 0 and ``IGNORE_INDEX``), plus the token that label names, i.e. the last trainable
+    label's index + 2.  0 for a sample without a trainable label."""
+    idx = torch.nonzero(torch.as_tensor(labels) > 0).flatten()
+    return int(idx[-1]) + 2 if idx.numel() else 0
+
+
+def pack_samples(lengths, max_length: int) -> List[List[int]]:
+    """Sample indices per row: samples are taken in order and a row is closed when the next one does not fit, so the
+    packing is deterministic, keeps the corpus order and never splits a sample.  Samples of length 0 are dropped."""
+    rows, cur, used = [], [], 0
+    for i, n in enumerate(lengths):
+        if n == 0:
+            continue
+        if n > max_length:
+            raise ValueError(f"sample {i} has {n} tokens, more than max_length={max_length}")
+        if used + n > max_length:
+            rows.append(cur)
+            cur, used = [], 0
+        cur.append(i)
+        used += n
+    if cur:
+        rows.append(cur)
+    return rows
+
+
+class PackedSFTDataset(Dataset):
+    """The prepared SFT corpus of :class:`SFTDataset`, packed into rows of ``max_length`` tokens (``position_ids``
+    packing, as Hugging Face's ``position_ids`` collator, TRL's ``packing=True`` and Megatron's
+    ``reset_position_ids`` / ``reset_attention_mask``).  Each sample keeps its tokens up to
+    :func:`sample_length`; samples without a trainable label are dropped.  A row carries ``input_ids``, ``labels``
+    (``IGNORE_INDEX`` on the padding tail; a document's last token predicts nothing, so no label crosses a document
+    boundary) and ``position_ids``, which restart at 0 at every document; the padding tail counts as one more document.
+    ``fill_rate`` is the share of row tokens that belong to a sample."""
+
+    def __init__(self, path, max_length: int, tokenizer=None):
+        data = torch.load(path, weights_only=False) if isinstance(path, (str, os.PathLike)) else list(path)
+        self.max_length, self.tokenizer = int(max_length), tokenizer
+        pad_id = getattr(tokenizer, "pad_token_id", None)
+        pad_id = 0 if pad_id is None else int(pad_id)
+        lengths = [sample_length(item["labels"]) for item in data]
+        self.rows = []
+        for members in pack_samples(lengths, self.max_length):
+            ids = torch.full((self.max_length,), pad_id, dtype=torch.long)
+            labels = torch.full((self.max_length,), IGNORE_INDEX, dtype=torch.long)
+            pos = torch.zeros(self.max_length, dtype=torch.long)
+            at = 0
+            for i in members:
+                n = lengths[i]
+                ids[at : at + n] = torch.as_tensor(data[i]["input_ids"], dtype=torch.long)[:n]
+                lab = torch.as_tensor(data[i]["labels"], dtype=torch.long)[:n].clone()
+                lab[n - 1] = IGNORE_INDEX
+                labels[at : at + n] = lab
+                pos[at : at + n] = torch.arange(n)
+                at += n
+            pos[at:] = torch.arange(self.max_length - at)
+            self.rows.append((ids, labels, pos))
+        self.fill_rate = sum(lengths) / max(1, len(self.rows) * self.max_length)
+
+    def __len__(self):
+        return len(self.rows)
+
+    def __getitem__(self, index):
+        ids, labels, pos = self.rows[index]
+        return Instance(
+            input_ids=DistTensorData(ids),
+            labels=DistTensorData(labels, placement_idx=-1),
+            position_ids=DistTensorData(pos),
         )
 
 
