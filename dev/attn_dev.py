@@ -1,5 +1,6 @@
 """Attention kernel development loop: numerics against the fp32 reference on a few shapes, then CUDA-event timings of
-the benchmark shape (B8 H16 S1024 D64 causal) next to PyTorch SDPA (cuDNN / flash).  `python dev/attn_dev.py [--ncu]`
+the benchmark shape (B8 H16 S1024 D64 causal) next to PyTorch SDPA (cuDNN / flash); the backward is timed with its
+delta and dQ-convert kernels, under an L2 flush, and reported in TFLOP/s of its MMA work too.  `python dev/attn_dev.py [--ncu]`
 (--ncu: three launches of each kernel only, for `ncu -k regex:attn_`)."""
 import json
 import math
@@ -78,6 +79,13 @@ def main():
         "sdpa_fwd_ms": timeit(lambda: torch.nn.functional.scaled_dot_product_attention(qc, kc, vc, is_causal=True)),
         "sdpa_bwd_ms": timeit(lambda: torch.autograd.grad(og, (qc, kc, vc), gog, retain_graph=True)),
     }
+    # the backward's tensor-core work: 5 MMAs of 64 x 64 x D per (64-key, 64-query) block pair the causal mask keeps
+    nb = S // 64
+    bwd_flop = B * A * nb * (nb + 1) // 2 * 5 * 2 * 64 * 64 * D
+    out["speed"]["bwd_gflop"] = bwd_flop / 1e9
+    out["speed"]["bwd_tflops"] = bwd_flop / (out["speed"]["bwd_ms"] * 1e-3) / 1e12
+    props = torch.cuda.get_device_properties(0)
+    out["device"] = props.name
     od, lsed, std = ext.attn_fwd(q, k, v, True, 0.125, None, None, None, 0.1, 0)
     out["speed"]["fwd_ms_dropout0.1"] = timeit(lambda: ext.attn_fwd(q, k, v, True, 0.125, None, None, None, 0.1, 0))
     out["speed"]["bwd_ms_dropout0.1"] = timeit(lambda: ext.attn_bwd(go, q, k, v, od, lsed, True, 0.125, None, None, None, None, 0.1, std))

@@ -41,9 +41,8 @@ namespace lb {
 constexpr int ATT_BM = 128;   // queries per CTA (forward)
 constexpr int ATT_BN = 128;   // keys per tile (forward)
 constexpr int ATT_FWD_THREADS = 384;
-constexpr int ATT_BWD_BN = 64;   // keys per CTA (backward)
+constexpr int ATT_BWD_BN = 64;   // keys per consumer warpgroup (backward)
 constexpr int ATT_BWD_BM = 64;   // queries per step (backward)
-constexpr int ATT_BWD_THREADS = 160;
 
 struct AttnFwdParams {
   __nv_bfloat16* o;   // [B, Sq, A, d]
@@ -488,47 +487,80 @@ extern "C" int lb_attn_fwd(const void* q, const void* k, const void* v, void* o,
   return (int)e;
 }
 // =================================================================================================
-// Backward.  One CTA per (batch, K/V head, 64-key block); one consumer warpgroup loops over the r query heads of the
-// group and, for each, over the 64-query blocks that attend to it (warp 4 = TMA producer, Q / dO double buffered).
+// Backward.  One CTA per (batch, K/V head, NWG consecutive 64-key blocks).  Consumer warpgroup w (warpgroups 1 ..
+// NWG) owns key block kb = NWG * cta + w and loops over the r query heads of the group and, for each, over the
+// 64-query blocks that attend to it; warpgroup 0 holds the TMA producer (warp 0) and the dQ writer (warp 1).  With
+// NWG = 2 the producer warpgroup gives its registers to the consumers (setmaxnreg), and one warpgroup's exp / dS math
+// overlaps the other's wgmmas (attn_bwd_wgs says which instances run two).
 // Which query blocks a key block visits depends on the shapes only (Sq, Sk, causal): under the causal mask query block
 // i and key block kb meet iff 64 kb <= 64 i + 63 + (Sk - Sq).  Keys outside a sample's kv_start / kv_lens window are
 // masked element-wise, so every visit happens and the dQ ordering below counts the same visits on both sides.
-// Packed sequences (DOC): a visit in which every query row's document starts after the key block is skipped by the
-// producer (no Q / dO load) and the consumer (no MMA) alike, from the same minimum over the rows.  It does not touch
-// the dQ order counter: whether a visit is skipped is monotone in the key block (skipped blocks lie below every
-// contributing one), so a contributing key block waits for exactly the contributing blocks above it, and the
-// contributions land in decreasing key-block order.
+// The warpgroups of a CTA step through one sequence of (query head, query block) visits, from the first query block
+// its lowest key block meets; the producer loads Q_i, dO_i and the block's lse and δ once for all of them, and a
+// warpgroup whose key block does not meet query block i (a higher block under the causal mask) lets that visit pass
+// without an MMA.
+// Packed sequences (DOC): a visit in which every query row's document starts after the key block is skipped by its
+// warpgroup (no MMA), and by the producer (no Q / dO load) when every key block of the CTA skips it; skips are taken
+// from the same minimum over the rows everywhere.  A skipped visit does not touch the dQ order counter: whether a
+// visit is skipped is monotone in the key block (skipped blocks lie below every contributing one), so a contributing
+// key block waits for exactly the contributing blocks above it, and the contributions land in decreasing key-block
+// order.
 //   Sᵀ = K·Q_iᵀ , dPᵀ = V·dO_iᵀ                  (wgmma, registers)
 //   Pᵀ = exp(Sᵀ·scale − lse) , dSᵀ = Pᵀ ∘ (dPᵀ − δ) · scale
 //   dV += Pᵀ·dO_i , dK += dSᵀ·Q_i                 (A operands straight from the registers, accumulators stay in
 //                                                  registers for the whole CTA: the group's sum is formed in a fixed
 //                                                  order and written once, no atomics)
-//   dQ_i += dS·K                                  (dSᵀ through shared memory, read as a transposed A operand; fp32
-//                                                  red.add into dq_accum, key block after key block in decreasing
-//                                                  order: a per-(query head, query block) counter orders the CTAs, so
-//                                                  the sums are
-//                                                  deterministic.  CTA kb at step `it` needs what kb + 1 added at step
-//                                                  it - 1, so the CTAs do not stall each other, and the highest key
-//                                                  blocks are launched first so that a waiter's predecessor is resident)
-// Forward progress of that wait relies on the hardware dispatching the CTAs of a grid in increasing linear block index
-// (the waited-for CTA always has the lower index), the same assumption as FlashAttention-3's deterministic backward.
-// Should it ever fail, the bounded spin wait traps after its timeout instead of hanging.
+//   dQ_i += dS·K                                  (dSᵀ through shared memory, read as a transposed A operand; the fp32
+//                                                  partial goes to a shared staging buffer and the consumer moves on)
+// The dQ writer warp adds the staged partials to dq_accum (one cp.reduce.async.bulk add.f32 per partial), key block
+// after key block in decreasing order: a per-(query head, query block) counter in global memory orders the CTAs, and
+// within a CTA the writer takes the partials of a visit from the highest key block down, so every element of dq_accum
+// receives the same additions in the same order as with one key block per CTA, and the sums are deterministic.  Key block kb adds to query block
+// i once the counter shows the last_kb - kb blocks above it that visit i; the writer then fences its additions and
+// releases the counter.  Key block kb at step `it` needs what kb + 1 added at an earlier step, so the CTAs do not
+// stall each other, and the highest key blocks are launched first so that a waiter's predecessor is resident.
+// Forward progress of that wait relies on the hardware dispatching the CTAs of a grid in increasing linear block index:
+// a writer waits either for its own CTA's higher key block, whose partial it added itself just before, or for a CTA
+// of lower linear index, whose writer in turn waits only for lower indices (the same assumption as FlashAttention-3's
+// deterministic backward).  Inside a CTA nothing waits for the writer except a consumer whose staging buffers are all
+// full, so the writer's progress is all the consumers need.  Should the assumption ever fail, the bounded spin wait
+// traps after its timeout instead of hanging.
 // δ = rowsum(dO ∘ O) is produced by attn_delta_kernel, dq_accum is converted to bf16 afterwards.
 // =================================================================================================
 namespace lb {
 
-template <int D>
+// consumer warpgroups (64-key blocks) per CTA of an instance.  Two share the register file with the producer
+// warpgroup at 224 registers each (the producer keeps 56), which the dropout and head-dim-128 consumers exceed: those
+// keep one consumer warpgroup and all 255 registers.
+template <int D, int BIAS, bool DROP>
+constexpr int attn_bwd_wgs() {
+  return D == 64 && !DROP ? 2 : 1;
+}
+
+template <int D, int NWG>
 struct AttnBwdCfg {
   static constexpr int CHUNKS = D / 64;
-  static constexpr int TILE_BYTES = 64 * D * 2;   // 64 rows of K / V / Q / dO
-  static constexpr int DS_BYTES = 64 * 64 * 2;
-  static constexpr int SMEM_BYTES = 2 * TILE_BYTES /*K,V*/ + 4 * TILE_BYTES /*Q,dO x2*/ + DS_BYTES + 1024 + 256;
+  static constexpr int THREADS = 128 * (NWG + 1);
+  static constexpr int TILE_BYTES = 64 * D * 2;      // 64 rows of K / V / Q / dO
+  static constexpr int DS_BYTES = 64 * 64 * 2;       // one warpgroup's dSᵀ
+  static constexpr int DQ_BYTES = 64 * D * 4;        // one staged fp32 dQ partial
+  static constexpr int DQ_BUFS = 2;                  // staging buffers per warpgroup
+  static constexpr int ROW_BYTES = 2 * 64 * 4;       // lse and δ of a query block
+  static constexpr int BAR_BYTES = 512;
+  static constexpr int FIXED = 2 * NWG * TILE_BYTES /*K, V*/ + NWG * DS_BYTES + NWG * DQ_BUFS * DQ_BYTES;
+  static constexpr int STAGE_BYTES = 2 * TILE_BYTES /*Q, dO*/ + ROW_BYTES;
+  // as many Q / dO stages as the 227 KB of shared memory per block hold: 6 with two consumer warpgroups at D = 64,
+  // 10 with one, 3 at D = 128
+  static constexpr int STAGES = (227 * 1024 - 1024 - BAR_BYTES - FIXED) / STAGE_BYTES;
+  static constexpr int SMEM_BYTES = FIXED + STAGES * STAGE_BYTES + BAR_BYTES + 1024;
+  static_assert(STAGES >= 2, "the Q / dO ring needs two stages");
+  static_assert((1 + 2 * STAGES + 2 * NWG * DQ_BUFS) * 8 <= BAR_BYTES, "barriers");
 };
 
 struct AttnBwdParams {
   const float* lse;     // [B, A, Sq]
   const float* delta;   // [B, A, Sq]
-  float* dq_accum;      // [B, A, Sq, d] fp32
+  float* dq_accum;      // [B, A, query blocks] tiles of [64][D] fp32 (dq_tile_index)
   __nv_bfloat16* dk;    // strided [B, G, Sk, d] views
   __nv_bfloat16* dv;
   long g_strides[3];    // batch, head, seq strides (elements) of dk / dv
@@ -560,36 +592,61 @@ LB_DEVICE bool doc_visit_empty(const int* doc_start, int S, int batch, int q0, i
                     doc_begin(doc_start, S, batch, min(q0 + 32 + lane, S - 1)));
   return __reduce_min_sync(0xffffffffu, m) >= k0 + ATT_BWD_BN;
 }
+// first query block whose last row (64 i + 63) sees key block kb: floor((64 kb - (Sk - Sq)) / 64), at least 0 (C
+// division truncates a negative quotient towards 0, which the max turns into the same 0).  At most nq - 1, since
+// 64 kb <= Sk - 1.
+LB_DEVICE int bwd_first_qblock(const AttnBwdParams& p, int kb) {
+  return p.causal ? max(0, (kb * ATT_BWD_BN - (p.Sk - p.Sq)) / ATT_BWD_BM) : 0;
+}
+// dq_accum holds each (batch, query head, 64-query block) as one [64][D] fp32 tile, stored as the backward stages its
+// dQ partials so that the writer adds a partial with one bulk operation: row-major, the 16-byte chunks of a row
+// swizzled with the row (chunk c at c ^ (row % 8)), which keeps the consumers' fragment stores free of bank conflicts.
+// Rows past Sq and columns past d are padding: the accumulator holds B·A·⌈Sq/64⌉·64·D floats against B·A·Sq·d for
+// a dense one, e.g. 2.7x at d = 24 and 1.6x at d = 80 (both cleared by the delta kernel).  Returns the float index of
+// (row, col) inside a tile.
+template <int D>
+LB_DEVICE int dq_tile_index(int row, int col) {
+  return row * D + ((((col >> 2) ^ row) & 7) | ((col >> 2) & ~7)) * 4 + (col & 3);
+}
+// whether key block kb (of nkb) visits query block qb; called by a whole warp (DOC)
+template <bool DOC>
+LB_DEVICE bool bwd_visits(const AttnBwdParams& p, int batch, int nkb, int kb, int qb) {
+  if (kb >= nkb || qb < bwd_first_qblock(p, kb)) return false;
+  return !DOC || !doc_visit_empty(p.doc_start, p.Sq, batch, qb * ATT_BWD_BM, kb * ATT_BWD_BN);
+}
 
 template <int D, int BIAS, bool DROP, bool DOC>
-__global__ void __launch_bounds__(ATT_BWD_THREADS, 1)
+__global__ void __launch_bounds__(AttnBwdCfg<D, attn_bwd_wgs<D, BIAS, DROP>()>::THREADS, 1)
 attn_bwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_k,
                 const __grid_constant__ CUtensorMap tmap_v, const __grid_constant__ CUtensorMap tmap_do, AttnBwdParams p) {
   static_assert(!DOC || (BIAS == BIAS_NONE && !DROP), "packed sequences run without bias and dropout");
-  using Cfg = AttnBwdCfg<D>;
+  constexpr int NWG = attn_bwd_wgs<D, BIAS, DROP>();
+  using Cfg = AttnBwdCfg<D, NWG>;
+  constexpr int STAGES = Cfg::STAGES, DQ_BUFS = Cfg::DQ_BUFS;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* sK = smem;
-  uint8_t* sV = sK + Cfg::TILE_BYTES;
-  uint8_t* sQ = sV + Cfg::TILE_BYTES;      // 2 stages
-  uint8_t* sDO = sQ + 2 * Cfg::TILE_BYTES;  // 2 stages
-  uint8_t* sDS = sDO + 2 * Cfg::TILE_BYTES;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sDS + Cfg::DS_BYTES);
+  uint8_t* sK = smem;                               // NWG tiles
+  uint8_t* sV = sK + NWG * Cfg::TILE_BYTES;         // NWG tiles
+  uint8_t* sQ = sV + NWG * Cfg::TILE_BYTES;         // STAGES
+  uint8_t* sDO = sQ + STAGES * Cfg::TILE_BYTES;     // STAGES
+  uint8_t* sDS = sDO + STAGES * Cfg::TILE_BYTES;    // NWG
+  float* sDQ = reinterpret_cast<float*>(sDS + NWG * Cfg::DS_BYTES);   // NWG x DQ_BUFS partials [64][D], 16-byte swizzle
+  float* sRow = sDQ + NWG * DQ_BUFS * 64 * D;       // STAGES x {lse[64], δ[64]}
+  uint64_t* bars = reinterpret_cast<uint64_t*>(sRow + STAGES * 128);
   uint64_t* kv_full = bars;
-  uint64_t* qdo_full = bars + 1;    // 2
-  uint64_t* qdo_empty = bars + 3;   // 2
+  uint64_t* qdo_full = bars + 1;                    // STAGES
+  uint64_t* qdo_empty = qdo_full + STAGES;          // STAGES
+  uint64_t* dq_full = qdo_empty + STAGES;           // NWG x DQ_BUFS
+  uint64_t* dq_empty = dq_full + NWG * DQ_BUFS;     // NWG x DQ_BUFS
 
-  const int warp_idx = threadIdx.x / 32;
-  const int kv_blk = static_cast<int>(gridDim.x) - 1 - static_cast<int>(blockIdx.x);
+  const int warp_idx = threadIdx.x / 32, lane = threadIdx.x % 32;
+  const int cta = static_cast<int>(gridDim.x) - 1 - static_cast<int>(blockIdx.x);   // highest keys first
   const int kv_head = blockIdx.y, batch = blockIdx.z;
-  const int k0 = kv_blk * ATT_BWD_BN;
-  const int kv_len = p.kv_lens != nullptr ? max(1, min(p.Sk, p.kv_lens[batch])) : p.Sk;
-  const int kv_beg = p.kv_start != nullptr ? min(max(p.kv_start[batch], 0), p.Sk) : 0;
+  const int nkb = (p.Sk + ATT_BWD_BN - 1) / ATT_BWD_BN;
+  const int kb0 = NWG * cta;                        // the CTA's lowest key block
   const int off = p.Sk - p.Sq;
   const int nq = (p.Sq + ATT_BWD_BM - 1) / ATT_BWD_BM;
-  // first query block whose last row (64 i + 63) sees key k0: floor((k0 - off) / 64), at least 0 (C division truncates
-  // a negative quotient towards 0, which the max turns into the same 0).  It is at most nq - 1, since k0 <= Sk - 1.
-  const int i_begin = p.causal ? max(0, (k0 - off) / ATT_BWD_BM) : 0;
+  const int i_begin = bwd_first_qblock(p, kb0);
   const int iters = nq - i_begin;   // query blocks per query head
   const int steps = p.r * iters;    // step = (query head in group) * iters + query block - i_begin
 
@@ -599,48 +656,115 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
     tma_prefetch_desc(&tmap_v);
     tma_prefetch_desc(&tmap_do);
     mbar_init(kv_full, 1);
-    for (int i = 0; i < 2; ++i) {
+    for (int i = 0; i < STAGES; ++i) {
       mbar_init(&qdo_full[i], 1);
-      mbar_init(&qdo_empty[i], 128);
+      mbar_init(&qdo_empty[i], NWG * 128);
+    }
+    for (int i = 0; i < NWG * DQ_BUFS; ++i) {
+      mbar_init(&dq_full[i], 128);
+      mbar_init(&dq_empty[i], 1);
     }
     fence_barrier_init();
     fence_proxy_async();
   }
   __syncthreads();
 
-  if (warp_idx == 4) {
-    const bool leader = elect_one();
-    if (leader) {
-      mbar_arrive_expect_tx(kv_full, 2 * Cfg::TILE_BYTES);
+  if (warp_idx < 4) {
+    if constexpr (NWG == 2) asm volatile("setmaxnreg.dec.sync.aligned.u32 56;\n" ::: "memory");
+    if (warp_idx == 0) {   // ---- producer: K / V once, then Q_i, dO_i, lse_i, δ_i per visit some warpgroup makes
+      if (lane == 0) {
+        const int nblk = min(NWG, nkb - kb0);
+        mbar_arrive_expect_tx(kv_full, 2 * nblk * Cfg::TILE_BYTES);
+        for (int w = 0; w < nblk; ++w) {
 #pragma unroll
-      for (int c = 0; c < Cfg::CHUNKS; ++c) {
-        tma_load_4d(sK + c * (64 * 128), &tmap_k, kv_full, c * 64, k0, kv_head, batch);
-        tma_load_4d(sV + c * (64 * 128), &tmap_v, kv_full, c * 64, k0, kv_head, batch);
+          for (int c = 0; c < Cfg::CHUNKS; ++c) {
+            tma_load_4d(sK + w * Cfg::TILE_BYTES + c * (64 * 128), &tmap_k, kv_full, c * 64, (kb0 + w) * ATT_BWD_BN, kv_head, batch);
+            tma_load_4d(sV + w * Cfg::TILE_BYTES + c * (64 * 128), &tmap_v, kv_full, c * 64, (kb0 + w) * ATT_BWD_BN, kv_head, batch);
+          }
+        }
       }
-    }
-    if (DOC || leader) {   // DOC: the whole warp takes the skip decisions, the leader loads
-      int ld = 0;          // visits loaded so far: the Q / dO ring position
+      int ld = 0;   // visits loaded so far: the Q / dO ring position
       for (int step = 0; step < steps; ++step) {
         const int hi = step / iters;
-        const int q0 = (i_begin + step - hi * iters) * ATT_BWD_BM;
-        if constexpr (DOC) {
-          if (doc_visit_empty(p.doc_start, p.Sq, batch, q0, k0) || !leader) continue;
-        }
-        const int st = ld & 1;
-        mbar_wait(&qdo_empty[st], ((ld >> 1) & 1) ^ 1);
-        mbar_arrive_expect_tx(&qdo_full[st], 2 * Cfg::TILE_BYTES);
+        const int qb = i_begin + step - hi * iters;
+        bool need = false;
 #pragma unroll
-        for (int c = 0; c < Cfg::CHUNKS; ++c) {
-          tma_load_5d(sQ + st * Cfg::TILE_BYTES + c * (64 * 128), &tmap_q, &qdo_full[st], c * 64, q0, hi, kv_head, batch);
-          tma_load_5d(sDO + st * Cfg::TILE_BYTES + c * (64 * 128), &tmap_do, &qdo_full[st], c * 64, q0, hi, kv_head, batch);
+        for (int w = 0; w < NWG; ++w) need = need || bwd_visits<DOC>(p, batch, nkb, kb0 + w, qb);
+        if (!need) continue;
+        const int st = ld % STAGES;
+        mbar_wait(&qdo_empty[st], ((ld / STAGES) & 1) ^ 1);
+        const int q0 = qb * ATT_BWD_BM;
+        const size_t bh = static_cast<size_t>(batch) * p.A + kv_head * p.r + hi;
+        for (int i = lane; i < ATT_BWD_BM; i += 32) {   // rows past Sq are never read
+          const int q = min(q0 + i, p.Sq - 1);
+          sRow[st * 128 + i] = p.lse[bh * p.Sq + q];
+          sRow[st * 128 + 64 + i] = p.delta[bh * p.Sq + q];
+        }
+        __syncwarp();
+        if (lane == 0) {
+          mbar_arrive_expect_tx(&qdo_full[st], 2 * Cfg::TILE_BYTES);
+#pragma unroll
+          for (int c = 0; c < Cfg::CHUNKS; ++c) {
+            tma_load_5d(sQ + st * Cfg::TILE_BYTES + c * (64 * 128), &tmap_q, &qdo_full[st], c * 64, q0, hi, kv_head, batch);
+            tma_load_5d(sDO + st * Cfg::TILE_BYTES + c * (64 * 128), &tmap_do, &qdo_full[st], c * 64, q0, hi, kv_head, batch);
+          }
         }
         ++ld;
+      }
+    } else if (warp_idx == 1) {   // ---- dQ writer: the staged partials into dq_accum, in decreasing key-block order
+      int staged[NWG];
+#pragma unroll
+      for (int w = 0; w < NWG; ++w) staged[w] = 0;
+      for (int step = 0; step < steps; ++step) {
+        const int hi = step / iters;
+        const int qb = i_begin + step - hi * iters;
+        bool makes[NWG];
+#pragma unroll
+        for (int w = 0; w < NWG; ++w) makes[w] = bwd_visits<DOC>(p, batch, nkb, kb0 + w, qb);
+        if (lane == 0) {
+          const size_t blk = (static_cast<size_t>(batch) * p.A + kv_head * p.r + hi) * nq + qb;
+          unsigned* order = p.dq_order + blk;
+          // the key blocks above kb that visit query block qb: all of them, or under the causal mask
+          // kb' <= (64 qb + 63 + off) / 64 (a non-negative quotient, since kb visits qb)
+          const int last_kb = p.causal ? min(nkb - 1, (qb * ATT_BWD_BM + ATT_BWD_BM - 1 + off) / ATT_BWD_BN) : nkb - 1;
+          uint32_t landed = 0;   // partials of this visit added so far
+#pragma unroll
+          for (int w = NWG - 1; w >= 0; --w) {
+            if (!makes[w]) continue;
+            const int kb = kb0 + w, b = staged[w] % DQ_BUFS;
+            const uint32_t par = (staged[w] / DQ_BUFS) & 1;
+            ++staged[w];
+            // after the partial of the key block above, added by this thread, the counter is at this block's target
+            if (landed == 0) {
+              spin_wait_ge_gpu(order, static_cast<uint32_t>(last_kb - kb), 0, p.timeout_rec, /*what=*/5, kb);
+              asm volatile("fence.proxy.async.global;\n" ::: "memory");   // the acquire orders the bulk addition below
+            }
+            mbar_wait(&dq_full[w * DQ_BUFS + b], par);
+            bulk_reduce_add_f32(p.dq_accum + blk * (64 * D), sDQ + (w * DQ_BUFS + b) * (64 * D), 64 * D * 4);
+            tma_store_commit();
+            tma_store_wait<0>();   // performed: the next partial of this query block adds on top of it
+            mbar_arrive(&dq_empty[w * DQ_BUFS + b]);
+            ++landed;
+          }
+          if (landed) {
+            __threadfence();
+            asm volatile("red.release.gpu.global.add.u32 [%0], %1;\n" ::"l"(order), "r"(landed) : "memory");
+          }
+        }
+        __syncwarp();
       }
     }
     return;
   }
+  if constexpr (NWG == 2) asm volatile("setmaxnreg.inc.sync.aligned.u32 224;\n" ::: "memory");
 
-  const int t = threadIdx.x;                              // 0..127
+  // ---- consumer warpgroup w: key block kb0 + w
+  const int w = NWG == 1 ? 0 : warp_idx / 4 - 1;   // (a constant with one warpgroup: fewer address registers)
+  const int kb = kb0 + w;
+  const int k0 = kb * ATT_BWD_BN;
+  const int kv_len = p.kv_lens != nullptr ? max(1, min(p.Sk, p.kv_lens[batch])) : p.Sk;
+  const int kv_beg = p.kv_start != nullptr ? min(max(p.kv_start[batch], 0), p.Sk) : 0;
+  const int t = threadIdx.x % 128;
   const int r_loc = 16 * (t / 32) + (t % 32) / 4;         // fragment rows r_loc, r_loc + 8
   const int cq = 2 * (t % 4);
   constexpr float LOG2E = 1.4426950408889634f;
@@ -650,7 +774,9 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
     rng_offset = static_cast<unsigned long long>(p.rng_state[1]);
   }
   const float inv_scale = 1.0f / p.scale;
-  const uint32_t k_addr = smem_u32(sK), v_addr = smem_u32(sV), ds_addr = smem_u32(sDS);
+  const uint32_t k_addr = smem_u32(sK + w * Cfg::TILE_BYTES), v_addr = smem_u32(sV + w * Cfg::TILE_BYTES);
+  uint8_t* my_ds = sDS + w * Cfg::DS_BYTES;
+  const uint32_t ds_addr = smem_u32(my_ds);
   // this thread's key rows are fixed for the CTA: a row before kv_start is never visible, which folds into the one
   // comparison against key_lim per element (INT_MAX is never below it)
   int kvis[2];
@@ -665,158 +791,156 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
   }
   mbar_wait(kv_full, 0);
 
-  int ld = 0;   // visits loaded so far (the producer's ring position)
+  int ld = 0;       // visits loaded so far (the producer's ring position)
+  int staged = 0;   // dQ partials staged so far
   for (int step = 0; step < steps; ++step) {
     const int hi = step / iters;
     const int it = step - hi * iters;
-    const int head = kv_head * p.r + hi;   // query head
-    const size_t bh = static_cast<size_t>(batch) * p.A + head;
-    float slope2 = 0.f;
-    if constexpr (BIAS == BIAS_ALIBI) slope2 = p.alibi_slopes[head] * LOG2E;
-    const long bias_bh = batch * p.bias_strides[0] + head * p.bias_strides[1];
-    const int q0 = (i_begin + it) * ATT_BWD_BM;
-    // DOC: a skipped visit leaves the dQ order counter alone.  Skipping is monotone in the key block (if kb is skipped,
-    // so is every kb' < kb of the same query block), so the key blocks above a contributing one all contribute and
-    // its wait for last_kb - kb_this counts exactly their additions.
-    if constexpr (DOC) {
-      if (doc_visit_empty(p.doc_start, p.Sq, batch, q0, k0)) continue;
-    }
-    const int st = ld & 1;
-    const uint32_t q_addr = smem_u32(sQ + st * Cfg::TILE_BYTES), do_addr = smem_u32(sDO + st * Cfg::TILE_BYTES);
-    mbar_wait(&qdo_full[st], (ld >> 1) & 1);
+    const int qb = i_begin + it;
+    const bool mine = bwd_visits<DOC>(p, batch, nkb, kb, qb);
+    bool need = mine;
+#pragma unroll
+    for (int u = 0; u < NWG; ++u)
+      if (u != w) need = need || bwd_visits<DOC>(p, batch, nkb, kb0 + u, qb);
+    if (!need) continue;   // not loaded
+    const int st = ld % STAGES;
+    mbar_wait(&qdo_full[st], (ld / STAGES) & 1);
     ++ld;
-    // ---- Sᵀ = K·Q_iᵀ, dPᵀ = V·dO_iᵀ (64 keys x 64 queries each)
-    float sT[32], dpT[32];
-    wgmma_fence();
+    if (mine) {
+      const int head = kv_head * p.r + hi;   // query head
+      const size_t bh = static_cast<size_t>(batch) * p.A + head;
+      float slope2 = 0.f;
+      if constexpr (BIAS == BIAS_ALIBI) slope2 = p.alibi_slopes[head] * LOG2E;
+      const long bias_bh = batch * p.bias_strides[0] + head * p.bias_strides[1];
+      const int q0 = qb * ATT_BWD_BM;
+      const float* s_lse = sRow + st * 128;
+      const float* s_delta = s_lse + 64;
+      const uint32_t q_addr = smem_u32(sQ + st * Cfg::TILE_BYTES), do_addr = smem_u32(sDO + st * Cfg::TILE_BYTES);
+      // ---- Sᵀ = K·Q_iᵀ, dPᵀ = V·dO_iᵀ (64 keys x 64 queries each)
+      float sT[32], dpT[32];
+      wgmma_fence();
 #pragma unroll
-    for (int kk = 0; kk < D / 16; ++kk) {
-      const uint32_t off = (kk / 4) * (64 * 128) + (kk % 4) * 32;
-      wgmma_bf16_ss<64, 0, 0>(sT, make_smem_desc_sw128(k_addr + off, 0, 1024), make_smem_desc_sw128(q_addr + off, 0, 1024),
-                              kk > 0 ? 1u : 0u);
-    }
+      for (int kk = 0; kk < D / 16; ++kk) {
+        const uint32_t off = (kk / 4) * (64 * 128) + (kk % 4) * 32;
+        wgmma_bf16_ss<64, 0, 0>(sT, make_smem_desc_sw128(k_addr + off, 0, 1024), make_smem_desc_sw128(q_addr + off, 0, 1024),
+                                kk > 0 ? 1u : 0u);
+      }
 #pragma unroll
-    for (int kk = 0; kk < D / 16; ++kk) {
-      const uint32_t off = (kk / 4) * (64 * 128) + (kk % 4) * 32;
-      wgmma_bf16_ss<64, 0, 0>(dpT, make_smem_desc_sw128(v_addr + off, 0, 1024), make_smem_desc_sw128(do_addr + off, 0, 1024),
-                              kk > 0 ? 1u : 0u);
-    }
-    wgmma_commit();
-    wgmma_wait<0>();
-    wgmma_fence_regs(sT);
-    wgmma_fence_regs(dpT);
+      for (int kk = 0; kk < D / 16; ++kk) {
+        const uint32_t off = (kk / 4) * (64 * 128) + (kk % 4) * 32;
+        wgmma_bf16_ss<64, 0, 0>(dpT, make_smem_desc_sw128(v_addr + off, 0, 1024), make_smem_desc_sw128(do_addr + off, 0, 1024),
+                                kk > 0 ? 1u : 0u);
+      }
+      wgmma_commit();
+      wgmma_wait<0>();
+      wgmma_fence_regs(sT);
+      wgmma_fence_regs(dpT);
 
-    // ---- Pᵀ (as it multiplied V in the forward, i.e. dropped and rescaled) into sT, dSᵀ into dpT
+      // ---- Pᵀ (as it multiplied V in the forward, i.e. dropped and rescaled) into sT, dSᵀ into dpT
 #pragma unroll
-    for (int jj = 0; jj < 8; ++jj) {
+      for (int jj = 0; jj < 8; ++jj) {
 #pragma unroll
-      for (int c = 0; c < 2; ++c) {
-        const int q_idx = q0 + 8 * jj + cq + c;
-        const bool q_ok = q_idx < p.Sq;
-        const float lse2 = q_ok ? p.lse[bh * p.Sq + q_idx] * LOG2E : 0.f;
-        const float delta_s = q_ok ? p.delta[bh * p.Sq + q_idx] * p.scale : 0.f;
-        const int key_lim = !q_ok ? 0 : (p.causal ? min(kv_len, q_idx + off + 1) : kv_len);
-        const int key_lo = DOC && q_ok ? doc_begin(p.doc_start, p.Sq, batch, q_idx) : 0;   // the query's document
-        uint4 rnd;
-        if constexpr (DROP)   // both rows of this thread lie in the same 16-key group
-          rnd = attn_dropout_bytes(static_cast<uint32_t>(q_idx), static_cast<uint32_t>((k0 + 16 * (t / 32)) >> 4),
-                                   static_cast<uint32_t>(bh), rng_seed, rng_offset);
+        for (int c = 0; c < 2; ++c) {
+          const int q_idx = q0 + 8 * jj + cq + c;
+          const bool q_ok = q_idx < p.Sq;
+          const float lse2 = q_ok ? s_lse[8 * jj + cq + c] * LOG2E : 0.f;
+          const float delta_s = q_ok ? s_delta[8 * jj + cq + c] * p.scale : 0.f;
+          const int key_lim = !q_ok ? 0 : (p.causal ? min(kv_len, q_idx + off + 1) : kv_len);
+          const int key_lo = DOC && q_ok ? doc_begin(p.doc_start, p.Sq, batch, q_idx) : 0;   // the query's document
+          uint4 rnd;
+          if constexpr (DROP)   // both rows of this thread lie in the same 16-key group
+            rnd = attn_dropout_bytes(static_cast<uint32_t>(q_idx), static_cast<uint32_t>((k0 + 16 * (t / 32)) >> 4),
+                                     static_cast<uint32_t>(bh), rng_seed, rng_offset);
 #pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          const int kidx = k0 + r_loc + 8 * h;
-          const int i = 4 * jj + 2 * h + c;
-          float x = sT[i] * p.scale_log2;
-          long boff = 0;
-          if constexpr (BIAS == BIAS_DENSE) {
-            boff = bias_bh + static_cast<long>(min(q_idx, p.Sq - 1)) * p.bias_strides[2] + min(kidx, p.Sk - 1);
-            x = fmaf(__bfloat162float(p.bias[boff]), LOG2E, x);
-          } else if constexpr (BIAS == BIAS_ALIBI) {
-            x = fmaf(slope2, static_cast<float>(kidx - q_idx - off), x);
+          for (int h = 0; h < 2; ++h) {
+            const int kidx = k0 + r_loc + 8 * h;
+            const int i = 4 * jj + 2 * h + c;
+            float x = sT[i] * p.scale_log2;
+            long boff = 0;
+            if constexpr (BIAS == BIAS_DENSE) {
+              boff = bias_bh + static_cast<long>(min(q_idx, p.Sq - 1)) * p.bias_strides[2] + min(kidx, p.Sk - 1);
+              x = fmaf(__bfloat162float(p.bias[boff]), LOG2E, x);
+            } else if constexpr (BIAS == BIAS_ALIBI) {
+              x = fmaf(slope2, static_cast<float>(kidx - q_idx - off), x);
+            }
+            const float pv = kvis[h] < key_lim && (!DOC || kvis[h] >= key_lo) ? fast_exp2(x - lse2) : 0.f;
+            float g = dpT[i], pd = pv;   // dP w.r.t. the dropped, rescaled P; what multiplied V in the forward
+            if constexpr (DROP) {
+              const bool keep = rnd_byte(rnd, (r_loc + 8 * h) & 15) >= p.drop_thresh;
+              g = keep ? g * p.inv_keep : 0.f;
+              pd = keep ? pv * p.inv_keep : 0.f;
+            }
+            const float ds = pv * fmaf(g, p.scale, -delta_s);
+            if constexpr (BIAS == BIAS_DENSE) {
+              // d bias = P ∘ (dP − δ): fp32 reductions (broadcast dims sum over CTAs)
+              if (p.dbias != nullptr && q_ok && kidx < p.Sk) atomicAdd(p.dbias + boff, ds * inv_scale);
+            }
+            sT[i] = pd;
+            dpT[i] = ds;
           }
-          const float pv = kvis[h] < key_lim && (!DOC || kvis[h] >= key_lo) ? fast_exp2(x - lse2) : 0.f;
-          float g = dpT[i], pd = pv;   // dP w.r.t. the dropped, rescaled P; what multiplied V in the forward
-          if constexpr (DROP) {
-            const bool keep = rnd_byte(rnd, (r_loc + 8 * h) & 15) >= p.drop_thresh;
-            g = keep ? g * p.inv_keep : 0.f;
-            pd = keep ? pv * p.inv_keep : 0.f;
-          }
-          const float ds = pv * fmaf(g, p.scale, -delta_s);
-          if constexpr (BIAS == BIAS_DENSE) {
-            // d bias = P ∘ (dP − δ): fp32 reductions (broadcast dims sum over CTAs)
-            if (p.dbias != nullptr && q_ok && kidx < p.Sk) atomicAdd(p.dbias + boff, ds * inv_scale);
-          }
-          sT[i] = pd;
-          dpT[i] = ds;
         }
       }
-    }
-    uint32_t pa[4][4], da[4][4];
+      uint32_t pa[4][4], da[4][4];
 #pragma unroll
-    for (int g = 0; g < 4; ++g) {
-      acc_to_a_frag(&sT[8 * g], pa[g]);
-      acc_to_a_frag(&dpT[8 * g], da[g]);
-    }
-    // dSᵀ -> shared memory (64 key rows x 128 B, 128-byte swizzle) for the dQ product
-#pragma unroll
-    for (int jj = 0; jj < 8; ++jj) {
-#pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        const int row = r_loc + 8 * h;
-        *reinterpret_cast<uint32_t*>(sDS + row * 128 + ((jj ^ (row & 7)) << 4) + cq * 2) =
-            pack_bf16(dpT[4 * jj + 2 * h], dpT[4 * jj + 2 * h + 1]);
+      for (int g = 0; g < 4; ++g) {
+        acc_to_a_frag(&sT[8 * g], pa[g]);
+        acc_to_a_frag(&dpT[8 * g], da[g]);
       }
-    }
-    fence_proxy_async();
-    warpgroup_sync(0);
-    // ---- dV += Pᵀ·dO_i, dK += dSᵀ·Q_i (B operands: the [query, D] tiles read MN-major)
-    wgmma_fence();
+      // dSᵀ -> shared memory (64 key rows x 128 B, 128-byte swizzle) for the dQ product
 #pragma unroll
-    for (int kk = 0; kk < 4; ++kk)
-      wgmma_bf16_rs<D, 1>(dv, pa[kk], make_smem_desc_sw128(do_addr + kk * (16 * 128), 64 * 128, 1024), 1u);
+      for (int jj = 0; jj < 8; ++jj) {
 #pragma unroll
-    for (int kk = 0; kk < 4; ++kk)
-      wgmma_bf16_rs<D, 1>(dk, da[kk], make_smem_desc_sw128(q_addr + kk * (16 * 128), 64 * 128, 1024), 1u);
-    wgmma_commit();
-    // ---- dQ_i is accumulated by the key blocks in decreasing order: wait until the key blocks above this one that
-    // visit query block i (all of them, or under the causal mask kb <= (64 i + 63 + off) / 64, a non-negative quotient
-    // since this block visits i) have added theirs
-    const int q_blk = i_begin + it;
-    unsigned* order = p.dq_order + bh * nq + q_blk;
-    const int last_kb = p.causal ? min(static_cast<int>(gridDim.x) - 1, (q_blk * ATT_BWD_BM + ATT_BWD_BM - 1 + off) / ATT_BWD_BN)
-                                 : static_cast<int>(gridDim.x) - 1;
-    if (t == 0) spin_wait_ge_sys(order, static_cast<uint32_t>(last_kb - kv_blk), 0, p.timeout_rec, /*what=*/5, kv_blk);
-    warpgroup_sync(0);
-    // ---- dQ_i = dS·K, 64 columns at a time: A = dSᵀ read transposed, B = the K tile read MN-major
-#pragma unroll
-    for (int n = 0; n < D / 64; ++n) {
-      float dq[32];
+        for (int h = 0; h < 2; ++h) {
+          const int row = r_loc + 8 * h;
+          *reinterpret_cast<uint32_t*>(my_ds + row * 128 + ((jj ^ (row & 7)) << 4) + cq * 2) =
+              pack_bf16(dpT[4 * jj + 2 * h], dpT[4 * jj + 2 * h + 1]);
+        }
+      }
+      fence_proxy_async();
+      warpgroup_sync(w);
+      // ---- dV += Pᵀ·dO_i, dK += dSᵀ·Q_i (B operands: the [query, D] tiles read MN-major)
       wgmma_fence();
 #pragma unroll
       for (int kk = 0; kk < 4; ++kk)
-        wgmma_bf16_ss<64, 1, 1>(dq, make_smem_desc_sw128(ds_addr + kk * (16 * 128), 64 * 128, 1024),
-                                make_smem_desc_sw128(k_addr + n * (64 * 128) + kk * (16 * 128), 64 * 128, 1024),
-                                kk > 0 ? 1u : 0u);
+        wgmma_bf16_rs<D, 1>(dv, pa[kk], make_smem_desc_sw128(do_addr + kk * (16 * 128), 64 * 128, 1024), 1u);
+#pragma unroll
+      for (int kk = 0; kk < 4; ++kk)
+        wgmma_bf16_rs<D, 1>(dk, da[kk], make_smem_desc_sw128(q_addr + kk * (16 * 128), 64 * 128, 1024), 1u);
       wgmma_commit();
-      wgmma_wait<0>();
-      wgmma_fence_regs(dq);
+      // ---- dQ_i = dS·K, 64 columns at a time (A = dSᵀ read transposed, B = the K tile read MN-major), staged for the
+      // writer in the layout of a dq_accum tile
+      const int b = staged % DQ_BUFS;
+      const uint32_t dpar = (staged / DQ_BUFS) & 1;
+      ++staged;
+      float* stage = sDQ + (w * DQ_BUFS + b) * (64 * D);
 #pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        const int q_idx = q0 + r_loc + 8 * h;
-        if (q_idx < p.Sq) {
-          float* dq_row = p.dq_accum + (bh * p.Sq + q_idx) * p.d + n * 64;
+      for (int n = 0; n < D / 64; ++n) {
+        float dq[32];
+        wgmma_fence();
 #pragma unroll
-          for (int jj = 0; jj < 8; ++jj)
-            if (col_in_head<D>(n * 64 + 8 * jj, p.d))
-              asm volatile("red.global.add.v2.f32 [%0], {%1, %2};\n" ::"l"(dq_row + 8 * jj + cq), "f"(dq[4 * jj + 2 * h]),
-                           "f"(dq[4 * jj + 2 * h + 1])
-                           : "memory");
+        for (int kk = 0; kk < 4; ++kk)
+          wgmma_bf16_ss<64, 1, 1>(dq, make_smem_desc_sw128(ds_addr + kk * (16 * 128), 64 * 128, 1024),
+                                  make_smem_desc_sw128(k_addr + n * (64 * 128) + kk * (16 * 128), 64 * 128, 1024),
+                                  kk > 0 ? 1u : 0u);
+        wgmma_commit();
+        if (n == 0) mbar_wait(&dq_empty[w * DQ_BUFS + b], dpar ^ 1);
+        wgmma_wait<0>();
+        wgmma_fence_regs(dq);
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int row = r_loc + 8 * h;
+#pragma unroll
+          for (int jj = 0; jj < 8; ++jj) {
+            const int col = n * 64 + 8 * jj + cq;
+            *reinterpret_cast<float2*>(stage + dq_tile_index<D>(row, col)) = make_float2(dq[4 * jj + 2 * h], dq[4 * jj + 2 * h + 1]);
+          }
         }
       }
+      fence_proxy_async();   // the writer's bulk addition reads the tile through the async proxy
+      mbar_arrive(&dq_full[w * DQ_BUFS + b]);
+      wgmma_fence_regs(dv);
+      wgmma_fence_regs(dk);
     }
-    __threadfence();
-    warpgroup_sync(0);
-    if (t == 0) asm volatile("red.release.gpu.global.add.u32 [%0], 1;\n" ::"l"(order) : "memory");
-    wgmma_fence_regs(dv);
-    wgmma_fence_regs(dk);
     mbar_arrive(&qdo_empty[st]);
   }
 
@@ -879,33 +1003,38 @@ attn_delta_kernel(const __nv_bfloat16* __restrict__ dout, const __nv_bfloat16* _
   }
 }
 
-// dq (strided bf16, query head a = group a / r, slot a % r) = dq_accum (fp32 [B, A, S, D]); 8 elements per thread (two
-// 16-byte loads, one 16-byte store)
+// dq (strided bf16, query head a = group a / r, slot a % r) = dq_accum (tiles of [64][D] fp32, dq_tile_index); 8
+// columns per thread (two 16-byte loads, one 16-byte store)
+template <int D>
 __global__ void __launch_bounds__(256)
-attn_dq_convert_kernel(const float* __restrict__ acc, __nv_bfloat16* __restrict__ dq, int B, int A, int S, int D, int r,
+attn_dq_convert_kernel(const float* __restrict__ acc, __nv_bfloat16* __restrict__ dq, int B, int A, int S, int d, int r,
                        long sb, long sg, long si, long ss) {
-  const long nvec = static_cast<long>(B) * A * S * D / 8;
+  const int vpr = d / 8;   // 8-column groups per row
+  const long nvec = static_cast<long>(B) * A * S * vpr;
+  const long nq = (S + ATT_BWD_BM - 1) / ATT_BWD_BM;
   const long stride = static_cast<long>(gridDim.x) * blockDim.x;
   for (long i0 = blockIdx.x * static_cast<long>(blockDim.x) + threadIdx.x; i0 < nvec; i0 += 2 * stride) {
     float4 lo[2], hi[2];
+    long row[2];
+    int col[2];
 #pragma unroll
     for (int u = 0; u < 2; ++u) {
       const long i = i0 + u * stride;
+      row[u] = i / vpr;
+      col[u] = static_cast<int>(i - row[u] * vpr) * 8;
       if (i < nvec) {
-        lo[u] = reinterpret_cast<const float4*>(acc)[2 * i];
-        hi[u] = reinterpret_cast<const float4*>(acc)[2 * i + 1];
+        const int sq = static_cast<int>(row[u] % S);
+        const float* tile = acc + ((row[u] / S) * nq + sq / ATT_BWD_BM) * (ATT_BWD_BM * D);
+        lo[u] = *reinterpret_cast<const float4*>(tile + dq_tile_index<D>(sq % ATT_BWD_BM, col[u]));
+        hi[u] = *reinterpret_cast<const float4*>(tile + dq_tile_index<D>(sq % ATT_BWD_BM, col[u] + 4));
       }
     }
 #pragma unroll
     for (int u = 0; u < 2; ++u) {
-      const long i = i0 + u * stride;
-      if (i < nvec) {
-        const long e = i * 8;
-        const int d = static_cast<int>(e % D);
-        const long row = e / D;
-        const int sq = static_cast<int>(row % S), a = static_cast<int>((row / S) % A);
-        const long b = row / (static_cast<long>(S) * A);
-        *reinterpret_cast<uint4*>(dq + b * sb + (a / r) * sg + (a % r) * si + sq * ss + d) =
+      if (i0 + u * stride < nvec) {
+        const int sq = static_cast<int>(row[u] % S), a = static_cast<int>((row[u] / S) % A);
+        const long b = row[u] / (static_cast<long>(S) * A);
+        *reinterpret_cast<uint4*>(dq + b * sb + (a / r) * sg + (a % r) * si + sq * ss + col[u]) =
             make_uint4(pack_bf16(lo[u].x, lo[u].y), pack_bf16(lo[u].z, lo[u].w), pack_bf16(hi[u].x, hi[u].y), pack_bf16(hi[u].z, hi[u].w));
       }
     }
@@ -928,7 +1057,8 @@ int sm_count() {
 template <int D, int BIAS, bool DROP, bool DOC = false>
 cudaError_t launch_bwd_t(const CUtensorMap& tq, const CUtensorMap& tk, const CUtensorMap& tv, const CUtensorMap& tdo,
                          const lb::AttnBwdParams& p, cudaStream_t s) {
-  using Cfg = lb::AttnBwdCfg<D>;
+  constexpr int NWG = lb::attn_bwd_wgs<D, BIAS, DROP>();
+  using Cfg = lb::AttnBwdCfg<D, NWG>;
   auto kern = lb::attn_bwd_kernel<D, BIAS, DROP, DOC>;
   static bool configured = false;
   if (!configured) {
@@ -936,8 +1066,9 @@ cudaError_t launch_bwd_t(const CUtensorMap& tq, const CUtensorMap& tk, const CUt
     if (e != cudaSuccess) return e;
     configured = true;
   }
-  dim3 grid((p.Sk + lb::ATT_BWD_BN - 1) / lb::ATT_BWD_BN, p.A / p.r, p.B);
-  kern<<<grid, lb::ATT_BWD_THREADS, Cfg::SMEM_BYTES, s>>>(tq, tk, tv, tdo, p);
+  const int nkb = (p.Sk + lb::ATT_BWD_BN - 1) / lb::ATT_BWD_BN;   // 64-key blocks, NWG per CTA
+  dim3 grid((nkb + NWG - 1) / NWG, p.A / p.r, p.B);
+  kern<<<grid, Cfg::THREADS, Cfg::SMEM_BYTES, s>>>(tq, tk, tv, tdo, p);
   return cudaGetLastError();
 }
 template <int D>
@@ -951,6 +1082,10 @@ cudaError_t launch_bwd(const CUtensorMap& tq, const CUtensorMap& tk, const CUten
   return drop ? launch_bwd_t<D, lb::BIAS_ALIBI, true>(tq, tk, tv, tdo, p, s) : launch_bwd_t<D, lb::BIAS_ALIBI, false>(tq, tk, tv, tdo, p, s);
 }
 }  // namespace
+// floats of the backward's dQ accumulator (fp32 [64][tile] per batch, query head and 64-query block)
+extern "C" long lb_attn_bwd_accum_floats(int B, int A, int Sq, int D) {
+  return (long)B * A * ((Sq + lb::ATT_BWD_BM - 1) / lb::ATT_BWD_BM) * lb::ATT_BWD_BM * head_dim_tile(D);
+}
 // A query heads in G groups; q_strides = {batch, group, in-group, seq}, k/v_strides = {batch, head, seq} over the G K/V
 // heads, do_strides = {batch, head, seq} over the A query heads.  dq is written with dq_strides = {batch, group,
 // in-group, seq}, dk and dv with dkv_strides = {batch, head, seq} (for Sq == Sk the caller passes views of one packed
@@ -989,11 +1124,11 @@ extern "C" int lb_attn_bwd(const void* dout, const void* q, const void* k, const
     if (tile == 64)
       lb::attn_delta_kernel<64><<<(unsigned)blocks, 256, 0, s>>>((const __nv_bfloat16*)dout, (const __nv_bfloat16*)o, delta, B,
                                                                    A, Sq, D, do_strides[0], do_strides[1], do_strides[2],
-                                                                   reinterpret_cast<float4*>(dq_accum), rows * D / 4);
+                                                                   reinterpret_cast<float4*>(dq_accum), lb_attn_bwd_accum_floats(B, A, Sq, D) / 4);
     else
       lb::attn_delta_kernel<128><<<(unsigned)blocks, 256, 0, s>>>((const __nv_bfloat16*)dout, (const __nv_bfloat16*)o, delta, B,
                                                                     A, Sq, D, do_strides[0], do_strides[1], do_strides[2],
-                                                                    reinterpret_cast<float4*>(dq_accum), rows * D / 4);
+                                                                    reinterpret_cast<float4*>(dq_accum), lb_attn_bwd_accum_floats(B, A, Sq, D) / 4);
   }
   lb::AttnBwdParams p;
   p.lse = lse;
@@ -1030,7 +1165,8 @@ extern "C" int lb_attn_bwd(const void* dout, const void* q, const void* k, const
   const long nvec = rows * D / 8;
   int blocks = (int)((nvec + 511) / 512);
   if (blocks > sm_count() * 8) blocks = sm_count() * 8;
-  lb::attn_dq_convert_kernel<<<blocks, 256, 0, s>>>(dq_accum, (__nv_bfloat16*)dq, B, A, Sq, D, r, dq_strides[0],
-                                                    dq_strides[1], dq_strides[2], dq_strides[3]);
+  auto convert = tile == 64 ? lb::attn_dq_convert_kernel<64> : lb::attn_dq_convert_kernel<128>;
+  convert<<<blocks, 256, 0, s>>>(dq_accum, (__nv_bfloat16*)dq, B, A, Sq, D, r, dq_strides[0], dq_strides[1],
+                                 dq_strides[2], dq_strides[3]);
   return (int)cudaGetLastError();
 }

@@ -89,6 +89,7 @@ int lb_attn_bwd(const void* dout, const void* q, const void* k, const void* v, c
                 const int* kv_start, const int* doc_start, const void* bias, const long* bias_strides,
                 const float* alibi_slopes, float* dbias, float p_drop, const long long* rng_state, unsigned* dq_order,
                 cudaStream_t s);
+long lb_attn_bwd_accum_floats(int B, int A, int Sq, int D);
 int lb_bias_dropout_residual(const void* x, const void* bias, const void* res, void* y, long rows, int N, float p,
                              const LbRngArgs* rng, const long long* rng_in, long long* rng_out, cudaStream_t s);
 int lb_spin_timeout_report(char* buf, int n);
@@ -1032,7 +1033,8 @@ std::tuple<Tensor, Tensor, Tensor, Tensor> attn_bwd(const Tensor& dout, const Te
   const long dqs[4] = {dq5.stride(0), dq5.stride(1), dq5.stride(2), dq5.stride(3)};
   const long dkvs[3] = {dk.stride(0), dk.stride(1), dk.stride(2)};
   Tensor delta = at::empty({B, A, Sq}, q.options().dtype(at::kFloat));
-  Tensor dq_acc = at::empty({B, A, Sq, D}, q.options().dtype(at::kFloat));   // cleared by the delta kernel
+  // fp32 dQ tiles, cleared by the delta kernel
+  Tensor dq_acc = at::empty({lb_attn_bwd_accum_floats(B, A, Sq, D)}, q.options().dtype(at::kFloat));
   // per (batch, head, 64-query block): key blocks that have added their dQ contribution
   Tensor dq_order = at::zeros({B * A * ((Sq + 63) / 64)}, q.options().dtype(at::kInt));
   TORCH_CHECK(o.stride(3) == 1, "attn_bwd: o must have contiguous D");

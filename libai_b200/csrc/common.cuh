@@ -55,22 +55,33 @@ LB_DEVICE uint32_t ld_acquire_sys_u32(const uint32_t* a) {
   asm volatile("ld.acquire.sys.global.u32 %0, [%1];\n" : "=r"(v) : "l"(a) : "memory");
   return v;
 }
+LB_DEVICE uint32_t ld_acquire_gpu_u32(const uint32_t* a) {
+  uint32_t v;
+  asm volatile("ld.acquire.gpu.global.u32 %0, [%1];\n" : "=r"(v) : "l"(a) : "memory");
+  return v;
+}
+template <bool SYS>
+LB_DEVICE uint32_t ld_acquire_u32(const uint32_t* a) {
+  return SYS ? ld_acquire_sys_u32(a) : ld_acquire_gpu_u32(a);
+}
 constexpr unsigned long long kDefaultSpinTimeoutNs = 120ull * 1000ull * 1000ull * 1000ull;  // 2 min
-// wait until *addr >= target (wrap-safe signed distance); `what`/`who` only label the diagnostic written to `rec`
-// (may be null: then the waiter traps without a record)
-LB_DEVICE void spin_wait_ge_sys(const uint32_t* addr, uint32_t target, unsigned long long timeout_ns, SpinTimeout* rec,
-                                int what, int who) {
-  if (static_cast<int32_t>(ld_acquire_sys_u32(addr) - target) >= 0) return;
+// wait until *addr >= target (wrap-safe signed distance), polling with system-scope (SYS: flags written by a peer GPU)
+// or GPU-scope acquire loads; `what`/`who` only label the diagnostic written to `rec` (may be null: then the waiter
+// traps without a record)
+template <bool SYS>
+LB_DEVICE void spin_wait_ge(const uint32_t* addr, uint32_t target, unsigned long long timeout_ns, SpinTimeout* rec,
+                            int what, int who) {
+  if (static_cast<int32_t>(ld_acquire_u32<SYS>(addr) - target) >= 0) return;
   const unsigned long long t0 = globaltimer_ns();
   const unsigned long long budget = timeout_ns ? timeout_ns : kDefaultSpinTimeoutNs;
   uint32_t polls = 0;
-  while (static_cast<int32_t>(ld_acquire_sys_u32(addr) - target) < 0) {
+  while (static_cast<int32_t>(ld_acquire_u32<SYS>(addr) - target) < 0) {
     if ((++polls & 1023u) == 0 && globaltimer_ns() - t0 > budget) {
       if (rec != nullptr && atomicCAS(&rec->claimed, 0u, 1u) == 0u) {
         rec->kind = what;
         rec->who = who;
         rec->block = static_cast<int>(blockIdx.x);
-        rec->value = ld_acquire_sys_u32(addr);
+        rec->value = ld_acquire_u32<SYS>(addr);
         rec->target = target;
         rec->flag = reinterpret_cast<unsigned long long>(addr);
         __threadfence_system();
@@ -80,6 +91,14 @@ LB_DEVICE void spin_wait_ge_sys(const uint32_t* addr, uint32_t target, unsigned 
       asm volatile("trap;");
     }
   }
+}
+LB_DEVICE void spin_wait_ge_sys(const uint32_t* addr, uint32_t target, unsigned long long timeout_ns, SpinTimeout* rec,
+                                int what, int who) {
+  spin_wait_ge<true>(addr, target, timeout_ns, rec, what, who);
+}
+LB_DEVICE void spin_wait_ge_gpu(const uint32_t* addr, uint32_t target, unsigned long long timeout_ns, SpinTimeout* rec,
+                                int what, int who) {
+  spin_wait_ge<false>(addr, target, timeout_ns, rec, what, who);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -203,6 +222,13 @@ LB_DEVICE void tma_store_4d(const CUtensorMap* map, const void* smem_src, int32_
   asm volatile("cp.async.bulk.tensor.4d.global.shared::cta.bulk_group [%0, {%2, %3, %4, %5}], [%1];\n" ::"l"(
                    reinterpret_cast<uint64_t>(map)),
                "r"(smem_u32(smem_src)), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
+               : "memory");
+}
+// global[dst .. dst + bytes) += shared[src ..] (fp32 element-wise adds, one bulk operation; 16-byte aligned, bytes a
+// multiple of 16), bulk async group completion
+LB_DEVICE void bulk_reduce_add_f32(float* dst, const float* src, uint32_t bytes) {
+  asm volatile("cp.reduce.async.bulk.global.shared::cta.bulk_group.add.f32 [%0], [%1], %2;\n" ::"l"(dst),
+               "r"(smem_u32(src)), "r"(bytes)
                : "memory");
 }
 LB_DEVICE void tma_store_commit() { asm volatile("cp.async.bulk.commit_group;\n" ::: "memory"); }

@@ -101,11 +101,6 @@ LB_DEVICE uint4 ld_stream_u4(const uint4* p) {
                : "l"(p));
   return v;
 }
-LB_DEVICE uint32_t ld_acquire_gpu_u32(const uint32_t* a) {
-  uint32_t v;
-  asm volatile("ld.acquire.gpu.global.u32 %0, [%1];\n" : "=r"(v) : "l"(a) : "memory");
-  return v;
-}
 
 template <int BLOCK_N>
 struct StageCfg {
