@@ -35,6 +35,7 @@
 
 #include <cstdlib>
 #include <cstring>
+#include <type_traits>
 
 namespace lb {
 
@@ -419,72 +420,92 @@ cudaError_t launch_fwd_t(const CUtensorMap& tq, const CUtensorMap& tk, const CUt
   return cudaGetLastError();
 }
 
-template <int D>
-cudaError_t launch_fwd(const CUtensorMap& tq, const CUtensorMap& tk, const CUtensorMap& tv, const lb::AttnFwdParams& p,
-                       cudaStream_t s) {
-  if (p.doc_start != nullptr) return launch_fwd_t<D, lb::BIAS_NONE, false, true>(tq, tk, tv, p, s);
-  const int bias = p.bias != nullptr ? lb::BIAS_DENSE : (p.alibi_slopes != nullptr ? lb::BIAS_ALIBI : lb::BIAS_NONE);
-  const bool drop = p.drop_thresh > 0;
-  if (bias == lb::BIAS_NONE) return drop ? launch_fwd_t<D, lb::BIAS_NONE, true>(tq, tk, tv, p, s) : launch_fwd_t<D, lb::BIAS_NONE, false>(tq, tk, tv, p, s);
-  if (bias == lb::BIAS_DENSE) return drop ? launch_fwd_t<D, lb::BIAS_DENSE, true>(tq, tk, tv, p, s) : launch_fwd_t<D, lb::BIAS_DENSE, false>(tq, tk, tv, p, s);
-  return drop ? launch_fwd_t<D, lb::BIAS_ALIBI, true>(tq, tk, tv, p, s) : launch_fwd_t<D, lb::BIAS_ALIBI, false>(tq, tk, tv, p, s);
+// the launcher-level conditions both directions share: the tile width (64 or 128) of the head dim, or -1 (head dim),
+// -5 (empty sequence), -4 (A % G), -6 (doc_start outside causal self-attention), -3 (strides or bias not 16-byte
+// aligned)
+int check_attn_args(const lb::AttnArgs& a) {
+  const int tile = head_dim_tile(a.d);
+  if (tile == 0) return -1;
+  if (a.Sq <= 0 || a.Sk <= 0) return -5;
+  if (a.G <= 0 || a.A % a.G) return -4;
+  if (a.doc_start != nullptr && !lb::attn_doc_start_supported(a)) return -6;
+  for (int i = 0; i < 3; ++i)
+    if ((a.q_strides[i] % 8) || (a.k_strides[i] % 8) || (a.v_strides[i] % 8)) return -3;
+  if (a.q_strides[3] % 8) return -3;
+  if (a.bias != nullptr && ((a.bias_strides[0] | a.bias_strides[1] | a.bias_strides[2]) % 8 ||
+                            (reinterpret_cast<uintptr_t>(a.bias) & 15)))
+    return -3;
+  return tile;
+}
+
+// the fields AttnFwdParams and AttnBwdParams share (each keeps its own member order: the kernels sit at their register
+// limit, so the layout is part of their performance).  `dropout`: a dropout stream is given; a dense bias takes
+// precedence over ALiBi slopes.
+template <class P>
+void fill_score_params(P& p, const lb::AttnArgs& a, bool dropout) {
+  p.B = a.B;
+  p.A = a.A;
+  p.r = a.A / a.G;
+  p.Sq = a.Sq;
+  p.Sk = a.Sk;
+  p.d = a.d;
+  p.causal = a.causal;
+  p.scale = a.scale;
+  p.scale_log2 = a.scale * 1.4426950408889634f;
+  p.kv_lens = a.kv_lens;
+  p.kv_start = a.kv_start;
+  p.doc_start = a.doc_start;
+  p.bias = reinterpret_cast<const __nv_bfloat16*>(a.bias);
+  for (int i = 0; i < 3; ++i) p.bias_strides[i] = a.bias != nullptr ? a.bias_strides[i] : 0;
+  p.alibi_slopes = a.bias != nullptr ? nullptr : a.alibi_slopes;
+  // keep a key iff its random byte >= drop_thresh: p quantised to 1/256, a positive p drops at least 1/256
+  uint32_t thr = (uint32_t)(a.p_drop * 256.0f + 0.5f);
+  if (thr > 255u) thr = 255u;
+  p.drop_thresh = (a.p_drop > 0.f && dropout) ? (thr == 0 ? 1u : thr) : 0u;
+  p.inv_keep = 256.0f / (256.0f - (float)p.drop_thresh);
+}
+
+template <int V>
+using int_c = std::integral_constant<int, V>;
+template <bool V>
+using bool_c = std::integral_constant<bool, V>;
+// calls launch(D, BIAS, DROP, DOC) with the compile-time parameters of the kernel instance that runs p: the tile
+// width, the bias kind, dropout, and packed sequences (whose instances run without bias and dropout)
+template <class P, class F>
+cudaError_t launch_instance(int tile, const P& p, F&& launch) {
+  auto with_tile = [&](auto D) {
+    if (p.doc_start != nullptr) return launch(D, int_c<lb::BIAS_NONE>{}, bool_c<false>{}, bool_c<true>{});
+    auto with_bias = [&](auto BIAS) {
+      return p.drop_thresh > 0 ? launch(D, BIAS, bool_c<true>{}, bool_c<false>{})
+                               : launch(D, BIAS, bool_c<false>{}, bool_c<false>{});
+    };
+    if (p.bias == nullptr && p.alibi_slopes == nullptr) return with_bias(int_c<lb::BIAS_NONE>{});
+    if (p.bias != nullptr) return with_bias(int_c<lb::BIAS_DENSE>{});
+    return with_bias(int_c<lb::BIAS_ALIBI>{});
+  };
+  return tile == 64 ? with_tile(int_c<64>{}) : with_tile(int_c<128>{});
 }
 }  // namespace
-// A query heads in G groups (A % G == 0); Sq queries, Sk keys; head dim D a multiple of 8 in [8, 128]; q_strides =
-// {batch, group, in-group, seq}, k/v_strides = {batch, head, seq} over the G K/V heads (elements).  kv_lens / kv_start
-// (optional, int32 [B], device): per-sample key window.
-// p_drop in [0, 1): attention dropout probability (quantised to 1/256 like the byte-threshold test of the kernel);
-// bias (optional, bf16): dense additive score bias with (batch, head, query-row) strides in elements, key stride 1;
-// alibi_slopes (optional, fp32 [A]); doc_start (optional, int32 [B, Sq], device): packed sequences, causal Sq == Sk
-// only, without kv_lens, kv_start, bias or dropout.
-extern "C" int lb_attn_fwd(const void* q, const void* k, const void* v, void* o, float* lse, int B, int A, int G, int Sq,
-                           int Sk, int D, const long* q_strides, const long* k_strides, const long* v_strides, int causal,
-                           float scale, const int* kv_lens, const int* kv_start, const int* doc_start, const void* bias,
-                           const long* bias_strides, const float* alibi_slopes, float p_drop, const lb::RngArgs* rng,
-                           long long* rng_out, cudaStream_t s) {
-  const int tile = head_dim_tile(D);
-  if (tile == 0) return -1;
-  if (Sq <= 0 || Sk <= 0) return -5;
-  if (G <= 0 || A % G) return -4;
-  if (doc_start != nullptr && (!causal || Sq != Sk || kv_lens != nullptr || kv_start != nullptr || bias != nullptr ||
-                               alibi_slopes != nullptr || p_drop > 0.f))
-    return -6;
-  for (int i = 0; i < 3; ++i)
-    if ((q_strides[i] % 8) || (k_strides[i] % 8) || (v_strides[i] % 8)) return -3;
-  if (q_strides[3] % 8) return -3;
+// o [B, Sq, A, d], lse [B, A, Sq]; see launchers.h
+extern "C" int lb_attn_fwd(const lb::AttnArgs* a, const void* q, const void* k, const void* v, void* o, float* lse,
+                           const lb::RngArgs* rng, long long* rng_out, cudaStream_t s) {
+  const int tile = check_attn_args(*a);
+  if (tile < 0) return tile;
   CUtensorMap tq, tk, tv;
-  if (!make_q_tmap(&tq, q, B, G, A / G, Sq, D, q_strides, 128)) return -2;
-  if (!make_qkv_tmap(&tk, k, B, G, Sk, D, k_strides, 128)) return -2;
-  if (!make_qkv_tmap(&tv, v, B, G, Sk, D, v_strides, 128)) return -2;
+  if (!make_q_tmap(&tq, q, a->B, a->G, a->A / a->G, a->Sq, a->d, a->q_strides, 128)) return -2;
+  if (!make_qkv_tmap(&tk, k, a->B, a->G, a->Sk, a->d, a->k_strides, 128)) return -2;
+  if (!make_qkv_tmap(&tv, v, a->B, a->G, a->Sk, a->d, a->v_strides, 128)) return -2;
   lb::AttnFwdParams p;
   p.o = reinterpret_cast<__nv_bfloat16*>(o);
   p.lse = lse;
-  p.B = B;
-  p.A = A;
-  p.r = A / G;
-  p.Sq = Sq;
-  p.Sk = Sk;
-  p.d = D;
-  p.causal = causal;
-  p.scale = scale;
-  p.scale_log2 = scale * 1.4426950408889634f;
-  p.kv_lens = kv_lens;
-  p.kv_start = kv_start;
-  p.doc_start = doc_start;
-  p.bias = reinterpret_cast<const __nv_bfloat16*>(bias);
-  for (int i = 0; i < 3; ++i) p.bias_strides[i] = (bias != nullptr && bias_strides != nullptr) ? bias_strides[i] : 0;
-  if (bias != nullptr && ((p.bias_strides[0] | p.bias_strides[1] | p.bias_strides[2]) % 8 || (reinterpret_cast<uintptr_t>(bias) & 15)))
-    return -3;
-  p.alibi_slopes = bias != nullptr ? nullptr : alibi_slopes;
-  uint32_t thr = (uint32_t)(p_drop * 256.0f + 0.5f);
-  if (thr > 255u) thr = 255u;
-  p.drop_thresh = (p_drop > 0.f && rng != nullptr) ? (thr == 0 ? 1u : thr) : 0u;
-  p.inv_keep = 256.0f / (256.0f - (float)p.drop_thresh);
+  fill_score_params(p, *a, rng != nullptr);
   memset(&p.rng, 0, sizeof(p.rng));
   if (rng != nullptr) p.rng = *rng;
   p.rng_out = rng_out;
-  cudaError_t e = (tile == 64) ? launch_fwd<64>(tq, tk, tv, p, s) : launch_fwd<128>(tq, tk, tv, p, s);
-  return (int)e;
+  return (int)launch_instance(tile, p, [&](auto tile_c, auto bias, auto drop, auto doc) {
+    return launch_fwd_t<decltype(tile_c)::value, decltype(bias)::value, decltype(drop)::value, decltype(doc)::value>(
+        tq, tk, tv, p, s);
+  });
 }
 // =================================================================================================
 // Backward.  One CTA per (batch, K/V head, NWG consecutive 64-key blocks).  Consumer warpgroup w (warpgroups 1 ..
@@ -1044,16 +1065,6 @@ attn_dq_convert_kernel(const float* __restrict__ acc, __nv_bfloat16* __restrict_
 }  // namespace lb
 
 namespace {
-int sm_count() {
-  static int n = 0;
-  if (n == 0) {
-    int dev = 0;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-  }
-  return n;
-}
-
 template <int D, int BIAS, bool DROP, bool DOC = false>
 cudaError_t launch_bwd_t(const CUtensorMap& tq, const CUtensorMap& tk, const CUtensorMap& tv, const CUtensorMap& tdo,
                          const lb::AttnBwdParams& p, cudaStream_t s) {
@@ -1071,48 +1082,26 @@ cudaError_t launch_bwd_t(const CUtensorMap& tq, const CUtensorMap& tk, const CUt
   kern<<<grid, Cfg::THREADS, Cfg::SMEM_BYTES, s>>>(tq, tk, tv, tdo, p);
   return cudaGetLastError();
 }
-template <int D>
-cudaError_t launch_bwd(const CUtensorMap& tq, const CUtensorMap& tk, const CUtensorMap& tv, const CUtensorMap& tdo,
-                       const lb::AttnBwdParams& p, cudaStream_t s) {
-  if (p.doc_start != nullptr) return launch_bwd_t<D, lb::BIAS_NONE, false, true>(tq, tk, tv, tdo, p, s);
-  const int bias = p.bias != nullptr ? lb::BIAS_DENSE : (p.alibi_slopes != nullptr ? lb::BIAS_ALIBI : lb::BIAS_NONE);
-  const bool drop = p.drop_thresh > 0;
-  if (bias == lb::BIAS_NONE) return drop ? launch_bwd_t<D, lb::BIAS_NONE, true>(tq, tk, tv, tdo, p, s) : launch_bwd_t<D, lb::BIAS_NONE, false>(tq, tk, tv, tdo, p, s);
-  if (bias == lb::BIAS_DENSE) return drop ? launch_bwd_t<D, lb::BIAS_DENSE, true>(tq, tk, tv, tdo, p, s) : launch_bwd_t<D, lb::BIAS_DENSE, false>(tq, tk, tv, tdo, p, s);
-  return drop ? launch_bwd_t<D, lb::BIAS_ALIBI, true>(tq, tk, tv, tdo, p, s) : launch_bwd_t<D, lb::BIAS_ALIBI, false>(tq, tk, tv, tdo, p, s);
-}
 }  // namespace
 // floats of the backward's dQ accumulator (fp32 [64][tile] per batch, query head and 64-query block)
 extern "C" long lb_attn_bwd_accum_floats(int B, int A, int Sq, int D) {
   return (long)B * A * ((Sq + lb::ATT_BWD_BM - 1) / lb::ATT_BWD_BM) * lb::ATT_BWD_BM * head_dim_tile(D);
 }
-// A query heads in G groups; q_strides = {batch, group, in-group, seq}, k/v_strides = {batch, head, seq} over the G K/V
-// heads, do_strides = {batch, head, seq} over the A query heads.  dq is written with dq_strides = {batch, group,
-// in-group, seq}, dk and dv with dkv_strides = {batch, head, seq} (for Sq == Sk the caller passes views of one packed
-// [B, S, G, r + 2, D] gradient).
-extern "C" int lb_attn_bwd(const void* dout, const void* q, const void* k, const void* v, const void* o,
-                           const float* lse, void* dq, void* dk, void* dv, const long* dq_strides, const long* dkv_strides,
-                           float* delta, float* dq_accum, int B, int A, int G, int Sq, int Sk, int D, const long* q_strides,
-                           const long* k_strides, const long* v_strides, const long* do_strides, int causal, float scale,
-                           const int* kv_lens, const int* kv_start, const int* doc_start, const void* bias,
-                           const long* bias_strides, const float* alibi_slopes, float* dbias, float p_drop,
+// see launchers.h; for Sq == Sk the caller passes views of one packed [B, S, G, r + 2, D] gradient as dq, dk and dv
+extern "C" int lb_attn_bwd(const lb::AttnArgs* a, const void* dout, const long* do_strides, const void* q, const void* k,
+                           const void* v, const void* o, const float* lse, void* dq, void* dk, void* dv,
+                           const long* dq_strides, const long* dkv_strides, float* delta, float* dq_accum, float* dbias,
                            const long long* rng_state, unsigned* dq_order, cudaStream_t s) {
-  const int tile = head_dim_tile(D);
-  if (tile == 0) return -1;
-  if (Sq <= 0 || Sk <= 0) return -5;
-  if (G <= 0 || A % G) return -4;
-  if (doc_start != nullptr && (!causal || Sq != Sk || kv_lens != nullptr || kv_start != nullptr || bias != nullptr ||
-                               alibi_slopes != nullptr || p_drop > 0.f))
-    return -6;
-  const int r = A / G;
+  const int tile = check_attn_args(*a);
+  if (tile < 0) return tile;
+  const int B = a->B, A = a->A, G = a->G, Sq = a->Sq, Sk = a->Sk, D = a->d, r = A / G;
   for (int i = 0; i < 3; ++i)
-    if ((q_strides[i] % 8) || (k_strides[i] % 8) || (v_strides[i] % 8) || (do_strides[i] % 8)) return -3;
-  if (q_strides[3] % 8) return -3;
+    if (do_strides[i] % 8) return -3;
   const long do_strides4[4] = {do_strides[0], r * do_strides[1], do_strides[1], do_strides[2]};
   CUtensorMap tq, tk, tv, tdo;
-  if (!make_q_tmap(&tq, q, B, G, r, Sq, D, q_strides, 64)) return -2;
-  if (!make_qkv_tmap(&tk, k, B, G, Sk, D, k_strides, 64)) return -2;
-  if (!make_qkv_tmap(&tv, v, B, G, Sk, D, v_strides, 64)) return -2;
+  if (!make_q_tmap(&tq, q, B, G, r, Sq, D, a->q_strides, 64)) return -2;
+  if (!make_qkv_tmap(&tk, k, B, G, Sk, D, a->k_strides, 64)) return -2;
+  if (!make_qkv_tmap(&tv, v, B, G, Sk, D, a->v_strides, 64)) return -2;
   if (!make_q_tmap(&tdo, dout, B, G, r, Sq, D, do_strides4, 64)) return -2;
   const long rows = (long)B * A * Sq;
   {
@@ -1120,7 +1109,7 @@ extern "C" int lb_attn_bwd(const void* dout, const void* q, const void* k, const
     const long groups = (rows + 3) / 4;
     const long lpr = tile / 8;
     long blocks = (groups * lpr + 255) / 256;
-    if (blocks > sm_count() * 16L) blocks = sm_count() * 16L;
+    if (blocks > lb_host::num_sms() * 16L) blocks = lb_host::num_sms() * 16L;
     if (tile == 64)
       lb::attn_delta_kernel<64><<<(unsigned)blocks, 256, 0, s>>>((const __nv_bfloat16*)dout, (const __nv_bfloat16*)o, delta, B,
                                                                    A, Sq, D, do_strides[0], do_strides[1], do_strides[2],
@@ -1137,34 +1126,19 @@ extern "C" int lb_attn_bwd(const void* dout, const void* q, const void* k, const
   p.dk = (__nv_bfloat16*)dk;
   p.dv = (__nv_bfloat16*)dv;
   for (int i = 0; i < 3; ++i) p.g_strides[i] = dkv_strides[i];
-  p.B = B;
-  p.A = A;
-  p.r = r;
-  p.Sq = Sq;
-  p.Sk = Sk;
-  p.d = D;
-  p.causal = causal;
-  p.scale = scale;
-  p.scale_log2 = scale * 1.4426950408889634f;
-  p.kv_lens = kv_lens;
-  p.kv_start = kv_start;
-  p.doc_start = doc_start;
-  p.bias = reinterpret_cast<const __nv_bfloat16*>(bias);
-  for (int i = 0; i < 3; ++i) p.bias_strides[i] = (bias != nullptr && bias_strides != nullptr) ? bias_strides[i] : 0;
-  p.alibi_slopes = bias != nullptr ? nullptr : alibi_slopes;
-  p.dbias = bias != nullptr ? dbias : nullptr;
-  uint32_t thr = (uint32_t)(p_drop * 256.0f + 0.5f);
-  if (thr > 255u) thr = 255u;
-  p.drop_thresh = (p_drop > 0.f && rng_state != nullptr) ? (thr == 0 ? 1u : thr) : 0u;
-  p.inv_keep = 256.0f / (256.0f - (float)p.drop_thresh);
+  fill_score_params(p, *a, rng_state != nullptr);
+  p.dbias = a->bias != nullptr ? dbias : nullptr;
   p.rng_state = rng_state;
   p.dq_order = dq_order;
   p.timeout_rec = lb_host::spin_timeout_record(s);
-  cudaError_t e = (tile == 64) ? launch_bwd<64>(tq, tk, tv, tdo, p, s) : launch_bwd<128>(tq, tk, tv, tdo, p, s);
+  cudaError_t e = launch_instance(tile, p, [&](auto tile_c, auto bias, auto drop, auto doc) {
+    return launch_bwd_t<decltype(tile_c)::value, decltype(bias)::value, decltype(drop)::value, decltype(doc)::value>(
+        tq, tk, tv, tdo, p, s);
+  });
   if (e != cudaSuccess) return (int)e;
   const long nvec = rows * D / 8;
   int blocks = (int)((nvec + 511) / 512);
-  if (blocks > sm_count() * 8) blocks = sm_count() * 8;
+  if (blocks > lb_host::num_sms() * 8) blocks = lb_host::num_sms() * 8;
   auto convert = tile == 64 ? lb::attn_dq_convert_kernel<64> : lb::attn_dq_convert_kernel<128>;
   convert<<<blocks, 256, 0, s>>>(dq_accum, (__nv_bfloat16*)dq, B, A, Sq, D, r, dq_strides[0], dq_strides[1],
                                  dq_strides[2], dq_strides[3]);

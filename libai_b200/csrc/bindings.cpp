@@ -11,101 +11,7 @@
 
 #include <tuple>
 
-extern "C" {
-int lb_gemm_bf16(const void* a, const void* b, void* out, int M, int N, int K, int lda, int ldb, int ldo, int layout,
-                 int epi, const void* bias, int act, void* pre_out, int force_bn, int force_splits, cudaStream_t s);
-int lb_gemm_set_schedule(int schedule);
-int lb_norm_fwd(const void* x, const void* gamma, const void* beta, void* y, float* mean, float* rstd, int rows, int H,
-                float eps, int rms, int dtype, int wdtype, cudaStream_t s);
-int lb_gemm_bf16_bias_residual(const void* x, const void* w, void* out, int M, int N, int K, int lda, int ldb,
-                               const void* bias, const void* residual, cudaStream_t s);
-int lb_gemm_fp8(const void* xq, const void* wq, void* out, int M, int N, int K, const void* bias, int act, void* pre_out,
-                const void* residual, const float* deq_x, const float* deq_w, int force_bn, cudaStream_t s);
-int lb_quant_e4m3(const void* x, void* q, void* amax_scratch, float* deq, long n, cudaStream_t s);
-int lb_norm_bwd_workspace_rows(int rows);
-int lb_norm_bwd_supports_gadd(int H);
-int lb_norm_bwd(const void* gy, const void* x, const void* gamma, const float* mean, const float* rstd, void* gx,
-                float* dgamma, float* dbeta, float* workspace, int rows, int H, int rms, int dtype, int wdtype,
-                int accumulate, const void* gadd, cudaStream_t s);
-int lb_bias_act_fwd(const void* x, const void* bias, void* y, long rows, int N, int act, cudaStream_t s);
-int lb_gemm_bf16_actgrad(const void* a, const void* b, void* out, int M, int N, int K, int lda, int ldb, int ldo,
-                         int layout, int act, const void* pre_in, float* colsum, cudaStream_t stream);
-int lb_bias_act_bwd(const void* gy, const void* x, const void* bias, void* gx, long rows, int N, int act,
-                    cudaStream_t s);
-int lb_bias_residual(const void* x, const void* bias, const void* res, void* y, long rows, int N, cudaStream_t s);
-int lb_swiglu_fwd(const void* gate, const void* up, void* y, long n, cudaStream_t s);
-int lb_swiglu_bwd(const void* gy, const void* gate, const void* up, void* dgate, void* dup, long n, cudaStream_t s);
-int lb_swiglu_packed_fwd(const void* gu, void* y, long rows, long F, cudaStream_t s);
-int lb_swiglu_packed_bwd(const void* gy, const void* gu, void* dgu, long rows, long F, cudaStream_t s);
-int lb_rope_qkv(const void* x, const float* cosv, const float* sinv, void* y, long groups, int S, int G, int r, int D,
-                int pos_offset, const int* positions, int npos, int backward, cudaStream_t s);
-int lb_rope(const void* x, const float* cosv, const float* sinv, void* y, long rows, int S, int D, int backward,
-            cudaStream_t s);
-int lb_colsum_workspace_rows(int M, int N);
-int lb_colsum(const void* x, float* out, int M, int N, int accumulate, float* workspace, cudaStream_t s);
-int lb_embedding_fwd(const int64_t* ids, const void* table, void* out, long T, int H, long vocab_start, long rows, cudaStream_t s);
-int lb_embedding_bwd(const int64_t* sorted_ids, const int64_t* order, const void* gy, float* grad, long T, int H,
-                     long vocab_start, long rows, cudaStream_t s);
-int lb_ce_stats(const void* logits, const int64_t* labels, float* mx, float* se, float* tgt, int T, int V,
-                long vocab_start, int dtype, cudaStream_t s);
-int lb_ce_bwd(const void* logits, const int64_t* labels, const float* lse, const float* gloss, void* dlogits, int T,
-              int V, long vocab_start, int dtype, cudaStream_t s);
-int lb_adamw(float* master, const float* grad, float* m, float* v, void* lp_out, int lp_dtype, const float* scale, long n,
-             float lr, float b1, float b2, float eps, float wd, float bc1, float bc2, int decoupled, cudaStream_t s);
-int lb_sqnorm_workspace(long n);
-int lb_sqnorm(const float* x, float* out, long n, float* workspace, cudaStream_t s);
-int lb_gemm_bf16_comm(const void* a, const void* b, void* out, int M, int N, int K, int layout, int epi,
-                      const void* bias, int act, void* pre_out, const void* pre_in, float* colsum, int mode,
-                      int world, int rank, const long* peer_buf, const long* peer_flags, const long* peer_done,
-                      void* state, const void* local_shard, int fill_local, const void* residual, void* rs_out,
-                      long staging_parity_off, int n_comm, cudaStream_t stream);
-int lb_zero_reduce_scatter(const long* grad_ptrs, const long* flag_ptrs, float* red, float* sqnorm, long lo, long n,
-                           float scale, int world, int rank, unsigned epoch, long mc_grad, cudaStream_t s);
-int lb_zero_adam_allgather(float* master, const float* red, float* m, float* v, const long* param_ptrs,
-                           const long* flag_ptrs, unsigned* done_counter, const float* clip, long lo, long n, float lr,
-                           float b1, float b2, float eps, float wd, float bc1, float bc2, int decoupled, int world,
-                           int rank, unsigned epoch, long mc_param, cudaStream_t s);
-int lb_device_barrier(const long* flag_ptrs, int world, int rank, int slot, unsigned epoch, cudaStream_t s);
-int lb_p2p_allgather(const void* shard, const long* out_ptrs, const long* flag_ptrs, unsigned* done_counter,
-                     long nbytes, int world, int rank, unsigned epoch, cudaStream_t s);
-// mirror of lb::RngArgs (common.cuh)
-struct LbRngArgs {
-  unsigned long long seed_val, offset_val;
-  const long long* seed_ptr;
-  const long long* offset_ptr;
-  unsigned int offset_intragraph;
-  int captured;
-  unsigned long long salt;
-};
-int lb_attn_fwd(const void* q, const void* k, const void* v, void* o, float* lse, int B, int A, int G, int Sq, int Sk,
-                int D, const long* q_strides, const long* k_strides, const long* v_strides, int causal, float scale,
-                const int* kv_lens, const int* kv_start, const int* doc_start, const void* bias,
-                const long* bias_strides, const float* alibi_slopes, float p_drop, const LbRngArgs* rng,
-                long long* rng_out, cudaStream_t s);
-int lb_attn_bwd(const void* dout, const void* q, const void* k, const void* v, const void* o, const float* lse,
-                void* dq, void* dk, void* dv, const long* dq_strides, const long* dkv_strides, float* delta,
-                float* dq_accum, int B, int A, int G, int Sq, int Sk, int D, const long* q_strides, const long* k_strides,
-                const long* v_strides, const long* do_strides, int causal, float scale, const int* kv_lens,
-                const int* kv_start, const int* doc_start, const void* bias, const long* bias_strides,
-                const float* alibi_slopes, float* dbias, float p_drop, const long long* rng_state, unsigned* dq_order,
-                cudaStream_t s);
-long lb_attn_bwd_accum_floats(int B, int A, int Sq, int D);
-int lb_bias_dropout_residual(const void* x, const void* bias, const void* res, void* y, long rows, int N, float p,
-                             const LbRngArgs* rng, const long long* rng_in, long long* rng_out, cudaStream_t s);
-int lb_spin_timeout_report(char* buf, int n);
-int lb_decode_splits(int B, int blocks, int C, int D);
-int lb_decode_attn(const void* q, const long* q_strides, const void* k, const void* v, void* o, float* part_o,
-                   float* part_ml, const int* seqlens, const int* kv_start, int B, int Sq, int A, int G, int C, int D,
-                   float scale, int nsplit, cudaStream_t s);
-int lb_kv_append(const void* qkv, const float* cosv, const float* sinv, void* q_out, void* k_cache, void* v_cache,
-                 const int* seqlens, int B, int Sq, int G, int r, int C, int D, cudaStream_t s);
-int lb_window_attn_groups(int B, int H, int W, int ws, int heads);
-int lb_window_attn_fwd(const void* qkv, void* out, float* lse, const float* table, const float* tau, int B, int H, int W,
-                       int ws, int shift, int heads, int d, float scale, cudaStream_t s);
-int lb_window_attn_bwd(const void* dout, const void* qkv, const float* lse, const float* table,
-                       const float* tau, void* dqkv, float* dtable, float* dtau, float* dt_part, float* dtau_part, int B,
-                       int H, int W, int ws, int shift, int heads, int d, float scale, cudaStream_t s);
-}
+#include "launchers.h"
 
 namespace {
 
@@ -662,14 +568,14 @@ Tensor sqnorm(const Tensor& x) {
 // (seed, offset) of the default CUDA generator, advanced by `increment`; graph-capture aware (pointers + intra-graph
 // offset while capturing — PyTorch refreshes the pointed-to values before every replay).  `salt` != 0 decorrelates
 // tensor-parallel ranks in sharded regions.
-LbRngArgs next_rng(int64_t salt, uint64_t increment = 4) {
+lb::RngArgs next_rng(int64_t salt, uint64_t increment = 4) {
   auto gen = at::get_generator_or_default<at::CUDAGeneratorImpl>(c10::nullopt, at::cuda::detail::getDefaultCUDAGenerator());
   at::PhiloxCudaState st;
   {
     std::lock_guard<std::mutex> lock(gen->mutex_);
     st = gen->philox_cuda_state(increment);
   }
-  LbRngArgs a;
+  lb::RngArgs a;
   std::memset(&a, 0, sizeof(a));
   a.captured = st.captured_ ? 1 : 0;
   if (st.captured_) {
@@ -702,7 +608,7 @@ std::tuple<Tensor, Tensor> bias_dropout_residual(const Tensor& x, const c10::opt
     return std::make_tuple(y, *rng_state);
   }
   Tensor st = at::empty({2}, x.options().dtype(at::kLong));
-  LbRngArgs a = next_rng(salt);
+  lb::RngArgs a = next_rng(salt);
   check(lb_bias_dropout_residual(x.data_ptr(), bptr, rptr, y.data_ptr(), x.size(0), (int)x.size(1), (float)p, &a, nullptr,
                                  reinterpret_cast<long long*>(st.data_ptr<int64_t>()), cur_stream()),
         "bias_dropout_residual");
@@ -715,80 +621,88 @@ std::tuple<Tensor, Tensor> bias_dropout_residual(const Tensor& x, const c10::opt
 // (D contiguous).  Output o is allocated as [B, Sq, A, D] and returned as the [B, A, Sq, D] view, lse fp32 [B, A, Sq].
 // Key j is visible to query i of sample b iff kv_start[b] <= j < kv_lens[b] (defaults 0 and Sk) and, when causal,
 // j <= i + Sk - Sq.
-struct BiasDesc {
-  const void* ptr = nullptr;
-  long strides[3] = {0, 0, 0};
-};
-// bias [Bb, Ab, Sq, Sk] (Bb in {1, B}, Ab in {1, A}), bf16, key dimension contiguous; broadcast dims get stride 0
-BiasDesc bias_desc(const c10::optional<Tensor>& bias, int B, int A, int Sq, int Sk) {
-  BiasDesc d;
-  if (!(bias.has_value() && bias->defined())) return d;
-  const Tensor& b = *bias;
-  TORCH_CHECK(b.dim() == 4 && b.scalar_type() == at::kBFloat16 && b.stride(3) == 1 && b.size(2) == Sq && b.size(3) == Sk,
-              "attention bias: bf16 [B|1, A|1, Sq, Sk] with contiguous keys");
-  TORCH_CHECK((b.size(0) == 1 || b.size(0) == B) && (b.size(1) == 1 || b.size(1) == A), "attention bias: bad broadcast shape");
-  d.ptr = b.data_ptr();
-  d.strides[0] = b.size(0) == 1 ? 0 : b.stride(0);
-  d.strides[1] = b.size(1) == 1 ? 0 : b.stride(1);
-  d.strides[2] = b.stride(2);
-  return d;
-}
+bool given(const c10::optional<Tensor>& t) { return t.has_value() && t->defined(); }
 
-// shapes of an attention call: q [B, A, Sq, D] / [B, G, r, Sq, D] against k, v [B, G, Sk, D]; qs = q's {batch, group,
-// in-group, seq} strides
-struct QGeom {
-  int B, A, G, Sq, Sk, D;
-  long qs[4];
-};
-QGeom q_geom(const Tensor& q, const Tensor& k, const Tensor& v, const char* what) {
+// One flash-attention problem, validated: q, k, v as above, bf16 on one CUDA device; kv_lens / kv_start int32 [B];
+// doc_start int32 [B, Sq] (packed sequences); bias bf16 [B|1, A|1, Sq, Sk] with contiguous keys (broadcast dims get
+// stride 0); alibi_slopes fp32 [A]; p_drop in [0, 1).  `what` names the op in the error messages.
+lb::AttnArgs attn_args(const Tensor& q, const Tensor& k, const Tensor& v, bool causal, double scale,
+                       const c10::optional<Tensor>& kv_lens, const c10::optional<Tensor>& kv_start,
+                       const c10::optional<Tensor>& doc_start, const c10::optional<Tensor>& bias,
+                       const c10::optional<Tensor>& alibi_slopes, double p_drop, const char* what) {
   TORCH_CHECK(q.dim() == 4 || q.dim() == 5, what, ": q must be [B, A, S, D] or [B, G, r, S, D]");
   TORCH_CHECK(k.dim() == 4 && k.sizes() == v.sizes(), what, ": k, v must be [B, G, S, D] of one shape");
+  TORCH_CHECK(q.scalar_type() == at::kBFloat16 && k.scalar_type() == at::kBFloat16 && v.scalar_type() == at::kBFloat16,
+              what, ": q, k, v must be bf16, got ", q.scalar_type(), ", ", k.scalar_type(), ", ", v.scalar_type());
+  TORCH_CHECK(q.is_cuda() && k.device() == q.device() && v.device() == q.device(), what,
+              ": q, k, v must be on one CUDA device, got ", q.device(), ", ", k.device(), ", ", v.device());
   TORCH_CHECK(q.stride(-1) == 1 && k.stride(3) == 1 && v.stride(3) == 1, what, ": D must be contiguous");
-  QGeom g;
-  g.B = (int)q.size(0);
-  g.G = (int)k.size(1);
-  g.Sq = (int)q.size(-2);
-  g.Sk = (int)k.size(2);
-  g.D = (int)q.size(-1);
+  lb::AttnArgs a{};
+  a.B = (int)q.size(0);
+  a.G = (int)k.size(1);
+  a.Sq = (int)q.size(-2);
+  a.Sk = (int)k.size(2);
+  a.d = (int)q.size(-1);
   if (q.dim() == 4) {
-    g.A = (int)q.size(1);
-    TORCH_CHECK(g.G > 0 && g.A % g.G == 0, what, ": the query heads must be a multiple of the K/V heads");
-    const long r = g.A / g.G;
-    g.qs[0] = q.stride(0);
-    g.qs[1] = r * q.stride(1);
-    g.qs[2] = q.stride(1);
-    g.qs[3] = q.stride(2);
+    a.A = (int)q.size(1);
+    TORCH_CHECK(a.G > 0 && a.A % a.G == 0, what, ": the query heads must be a multiple of the K/V heads");
+    const long r = a.A / a.G;
+    a.q_strides[0] = q.stride(0);
+    a.q_strides[1] = r * q.stride(1);
+    a.q_strides[2] = q.stride(1);
+    a.q_strides[3] = q.stride(2);
   } else {
-    TORCH_CHECK(q.size(1) == g.G, what, ": grouped q [B, G, r, S, D] must have the K/V heads' G");
-    g.A = g.G * (int)q.size(2);
-    g.qs[0] = q.stride(0);
-    g.qs[1] = q.stride(1);
-    g.qs[2] = q.stride(2);
-    g.qs[3] = q.stride(3);
+    TORCH_CHECK(q.size(1) == a.G, what, ": grouped q [B, G, r, S, D] must have the K/V heads' G");
+    a.A = a.G * (int)q.size(2);
+    for (int i = 0; i < 4; ++i) a.q_strides[i] = q.stride(i);
   }
-  TORCH_CHECK(k.size(0) == g.B && k.size(3) == g.D, what, ": k, v do not match q");
-  TORCH_CHECK(g.D % 8 == 0 && g.D >= 8 && g.D <= 128, what, ": head dim must be a multiple of 8 in [8, 128], got ", g.D);
-  TORCH_CHECK(g.Sq >= 1 && g.Sk >= 1, what, ": empty query or key sequence");
-  return g;
-}
-
-// optional per-sample key bound (kv_lens: end, kv_start: start of the visible keys) → device pointer or nullptr
-const int* key_bound(const c10::optional<Tensor>& t, const Tensor& q, int B, const char* what) {
-  if (!(t.has_value() && t->defined())) return nullptr;
-  TORCH_CHECK(t->scalar_type() == at::kInt, what, ": int32 expected, got ", t->scalar_type());
-  TORCH_CHECK(t->numel() == B, what, ": ", B, " elements (one per sample) expected, got shape ", t->sizes());
-  TORCH_CHECK(t->is_cuda() && t->device() == q.device(), what, ": must be on ", q.device(), ", got ", t->device());
-  TORCH_CHECK(t->is_contiguous(), what, ": must be contiguous");
-  return t->data_ptr<int>();
-}
-
-// doc_start (optional, int32 [B, S]): packed sequences, query i sees keys doc_start[b, i] <= j <= i (clamped to [0, i])
-const int* doc_starts(const c10::optional<Tensor>& doc_start, const Tensor& q, const QGeom& g, bool causal,
-                      bool other_masks, double p_drop, const char* what) {
-  const int* ds = token_index(doc_start, q, g.B, g.Sq, what);
-  TORCH_CHECK(ds == nullptr || (causal && g.Sq == g.Sk && !other_masks && p_drop == 0.0), what,
-              ": supported for causal self-attention (Sq == Sk) without kv_lens, kv_start, bias, ALiBi or dropout");
-  return ds;
+  TORCH_CHECK(k.size(0) == a.B && k.size(3) == a.d, what, ": k, v do not match q");
+  TORCH_CHECK(a.d % 8 == 0 && a.d >= 8 && a.d <= 128, what, ": head dim must be a multiple of 8 in [8, 128], got ", a.d);
+  TORCH_CHECK(a.Sq >= 1 && a.Sk >= 1, what, ": empty query or key sequence");
+  for (int i = 0; i < 3; ++i) {
+    a.k_strides[i] = k.stride(i);
+    a.v_strides[i] = v.stride(i);
+  }
+  a.causal = causal;
+  a.scale = (float)scale;
+  // per-sample key bound (kv_lens: end, kv_start: start of the visible keys)
+  auto key_bound = [&](const c10::optional<Tensor>& t, const char* name) -> const int* {
+    if (!given(t)) return nullptr;
+    TORCH_CHECK(t->scalar_type() == at::kInt, what, ": ", name, ": int32 expected, got ", t->scalar_type());
+    TORCH_CHECK(t->numel() == a.B, what, ": ", name, ": ", a.B, " elements (one per sample) expected, got shape ",
+                t->sizes());
+    TORCH_CHECK(t->is_cuda() && t->device() == q.device(), what, ": ", name, ": must be on ", q.device(), ", got ",
+                t->device());
+    TORCH_CHECK(t->is_contiguous(), what, ": ", name, ": must be contiguous");
+    return t->data_ptr<int>();
+  };
+  a.kv_lens = key_bound(kv_lens, "kv_lens");
+  a.kv_start = key_bound(kv_start, "kv_start");
+  a.doc_start = token_index(doc_start, q, a.B, a.Sq, (std::string(what) + ": doc_start").c_str());
+  if (given(bias)) {
+    const Tensor& b = *bias;
+    TORCH_CHECK(b.dim() == 4 && b.scalar_type() == at::kBFloat16 && b.stride(3) == 1 && b.size(2) == a.Sq &&
+                    b.size(3) == a.Sk && b.device() == q.device(),
+                what, ": attention bias: bf16 [B|1, A|1, Sq, Sk] on q's device with contiguous keys");
+    TORCH_CHECK((b.size(0) == 1 || b.size(0) == a.B) && (b.size(1) == 1 || b.size(1) == a.A), what,
+                ": attention bias: bad broadcast shape");
+    a.bias = b.data_ptr();
+    a.bias_strides[0] = b.size(0) == 1 ? 0 : b.stride(0);
+    a.bias_strides[1] = b.size(1) == 1 ? 0 : b.stride(1);
+    a.bias_strides[2] = b.stride(2);
+  }
+  if (given(alibi_slopes)) {
+    const Tensor& s = *alibi_slopes;
+    TORCH_CHECK(s.scalar_type() == at::kFloat && s.numel() == a.A && s.device() == q.device() && s.is_contiguous(),
+                what, ": alibi_slopes: contiguous fp32 [A] on q's device");
+    a.alibi_slopes = s.data_ptr<float>();
+  }
+  TORCH_CHECK(p_drop < 1.0, "dropout probability must be in [0, 1)");
+  a.p_drop = (float)p_drop;
+  TORCH_CHECK(a.doc_start == nullptr || lb::attn_doc_start_supported(a), what,
+              ": doc_start: supported for causal self-attention (Sq == Sk) without kv_lens, kv_start, bias, ALiBi or "
+              "dropout");
+  return a;
 }
 
 // returns (o, lse, rng_state): rng_state int64[2] = (seed, offset) of the dropout mask (empty without dropout)
@@ -796,41 +710,18 @@ std::tuple<Tensor, Tensor, Tensor> attn_fwd(const Tensor& q, const Tensor& k, co
                                             const c10::optional<Tensor>& kv_lens, const c10::optional<Tensor>& bias,
                                             const c10::optional<Tensor>& alibi_slopes, double p_drop, int64_t salt,
                                             const c10::optional<Tensor>& kv_start, const c10::optional<Tensor>& doc_start) {
+  const lb::AttnArgs a =
+      attn_args(q, k, v, causal, scale, kv_lens, kv_start, doc_start, bias, alibi_slopes, p_drop, "attn_fwd");
   c10::cuda::CUDAGuard guard(q.device());
-  const QGeom g = q_geom(q, k, v, "attn_fwd");
-  const int B = g.B, A = g.A, Sq = g.Sq, Sk = g.Sk, D = g.D;
-  const bool has_alibi = alibi_slopes.has_value() && alibi_slopes->defined();
-  const int* dst = doc_starts(doc_start, q, g, causal,
-                              (kv_lens.has_value() && kv_lens->defined()) || (kv_start.has_value() && kv_start->defined()) ||
-                                  (bias.has_value() && bias->defined()) || has_alibi,
-                              p_drop, "attn_fwd: doc_start");
-  Tensor o = at::empty({B, Sq, A, D}, q.options());
-  Tensor lse = at::empty({B, A, Sq}, q.options().dtype(at::kFloat));
-  const long* qs = g.qs;
-  long ks[3] = {k.stride(0), k.stride(1), k.stride(2)};
-  long vs[3] = {v.stride(0), v.stride(1), v.stride(2)};
-  const int* kvl = key_bound(kv_lens, q, B, "attn_fwd: kv_lens");
-  const int* kvs = key_bound(kv_start, q, B, "attn_fwd: kv_start");
-  BiasDesc bd = bias_desc(bias, B, A, Sq, Sk);
-  const float* slopes = nullptr;
-  if (alibi_slopes.has_value() && alibi_slopes->defined()) {
-    TORCH_CHECK(alibi_slopes->scalar_type() == at::kFloat && alibi_slopes->numel() == A && alibi_slopes->is_cuda(), "alibi_slopes: fp32 cuda [A]");
-    slopes = alibi_slopes->data_ptr<float>();
-  }
-  Tensor rng_state;
-  LbRngArgs a;
+  Tensor o = at::empty({a.B, a.Sq, a.A, a.d}, q.options());
+  Tensor lse = at::empty({a.B, a.A, a.Sq}, q.options().dtype(at::kFloat));
   const bool drop = p_drop > 0.0;
-  if (drop) {
-    TORCH_CHECK(p_drop < 1.0, "dropout probability must be in [0, 1)");
-    rng_state = at::empty({2}, q.options().dtype(at::kLong));
-    a = next_rng(salt);
-  } else {
-    rng_state = at::empty({0}, q.options().dtype(at::kLong));
-  }
-  check(lb_attn_fwd(q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(), lse.data_ptr<float>(), B, A, g.G, Sq, Sk, D, qs,
-                    ks, vs, causal ? 1 : 0, (float)scale, kvl, kvs, dst, bd.ptr, bd.strides, slopes, (float)p_drop,
-                    drop ? &a : nullptr,
-                    drop ? reinterpret_cast<long long*>(rng_state.data_ptr<int64_t>()) : nullptr, cur_stream()),
+  Tensor rng_state = at::empty({drop ? 2 : 0}, q.options().dtype(at::kLong));
+  lb::RngArgs rng{};
+  if (drop) rng = next_rng(salt);
+  check(lb_attn_fwd(&a, q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(), lse.data_ptr<float>(),
+                    drop ? &rng : nullptr, drop ? reinterpret_cast<long long*>(rng_state.data_ptr<int64_t>()) : nullptr,
+                    cur_stream()),
         "attn_fwd");
   return std::make_tuple(o.permute({0, 2, 1, 3}), lse, rng_state);
 }
@@ -1006,14 +897,21 @@ std::tuple<Tensor, Tensor, Tensor, Tensor> attn_bwd(const Tensor& dout, const Te
                                             double p_drop, const c10::optional<Tensor>& rng_state,
                                             const c10::optional<Tensor>& kv_start,
                                             const c10::optional<Tensor>& doc_start) {
+  const lb::AttnArgs a =
+      attn_args(q, k, v, causal, scale, kv_lens, kv_start, doc_start, bias, alibi_slopes, p_drop, "attn_bwd");
   c10::cuda::CUDAGuard guard(q.device());
-  const QGeom g = q_geom(q, k, v, "attn_bwd");
-  const int B = g.B, A = g.A, G = g.G, Sq = g.Sq, Sk = g.Sk, D = g.D, r = A / G;
-  const int* dst = doc_starts(doc_start, q, g, causal,
-                              (kv_lens.has_value() && kv_lens->defined()) || (kv_start.has_value() && kv_start->defined()) ||
-                                  (bias.has_value() && bias->defined()) ||
-                                  (alibi_slopes.has_value() && alibi_slopes->defined()),
-                              p_drop, "attn_bwd: doc_start");
+  const int B = a.B, A = a.A, G = a.G, Sq = a.Sq, Sk = a.Sk, D = a.d, r = A / G;
+  TORCH_CHECK(o.scalar_type() == at::kBFloat16 && o.device() == q.device() && o.sizes() == at::IntArrayRef({B, A, Sq, D}) &&
+                  o.stride(3) == 1,
+              "attn_bwd: o must be the forward's bf16 [B, A, Sq, D] with contiguous D");
+  TORCH_CHECK(dout.device() == q.device() && dout.sizes() == o.sizes(), "attn_bwd: dout must be [B, A, Sq, D] on q's device");
+  TORCH_CHECK(lse.scalar_type() == at::kFloat && lse.device() == q.device() && lse.is_contiguous() &&
+                  lse.sizes() == at::IntArrayRef({B, A, Sq}),
+              "attn_bwd: lse must be the forward's contiguous fp32 [B, A, Sq]");
+  const bool drop = p_drop > 0.0;
+  TORCH_CHECK(!drop || (given(rng_state) && rng_state->scalar_type() == at::kLong && rng_state->numel() == 2 &&
+                        rng_state->is_contiguous() && rng_state->device() == q.device()),
+              "attn_bwd: p_drop > 0 needs the forward's rng_state, int64 [2] on q's device");
   // Sq == Sk: gradients are produced in the packed [B, S, G, r + 2, D] layout (r = 1: [B, S, A, 3, D]) so that the QKV
   // dgrad/wgrad GEMMs read them directly; dq comes back in q's shape (a copy only for a 4-D q with r > 1).
   // Sq != Sk: dq is [B, Sq, G, r, D] and dk, dv are packed as [B, Sk, G, 2, D]; the returned dqkv is empty.
@@ -1037,33 +935,23 @@ std::tuple<Tensor, Tensor, Tensor, Tensor> attn_bwd(const Tensor& dout, const Te
   Tensor dq_acc = at::empty({lb_attn_bwd_accum_floats(B, A, Sq, D)}, q.options().dtype(at::kFloat));
   // per (batch, head, 64-query block): key blocks that have added their dQ contribution
   Tensor dq_order = at::zeros({B * A * ((Sq + 63) / 64)}, q.options().dtype(at::kInt));
-  TORCH_CHECK(o.stride(3) == 1, "attn_bwd: o must have contiguous D");
   Tensor dout_c = dout;
-  if (dout.strides() != o.strides()) {  // bring dout into the [B, S, A, D]-backed layout of o
+  if (dout.strides() != o.strides() || dout.scalar_type() != at::kBFloat16) {   // into the [B, S, A, D]-backed layout of o
     dout_c = at::empty_strided(o.sizes(), o.strides(), o.options());
     dout_c.copy_(dout);
   }
-  const long* qs = g.qs;
-  long ks[3] = {k.stride(0), k.stride(1), k.stride(2)};
-  long vs[3] = {v.stride(0), v.stride(1), v.stride(2)};
-  long ds[3] = {dout_c.stride(0), dout_c.stride(1), dout_c.stride(2)};
-  BiasDesc bd = bias_desc(bias, B, A, Sq, Sk);
-  const int* kvl = key_bound(kv_lens, q, B, "attn_bwd: kv_lens");
-  const int* kvs = key_bound(kv_start, q, B, "attn_bwd: kv_start");
+  const long ds[3] = {dout_c.stride(0), dout_c.stride(1), dout_c.stride(2)};
   float* dbp = nullptr;
-  if (dbias.has_value() && dbias->defined()) {
-    TORCH_CHECK(bd.ptr != nullptr && dbias->scalar_type() == at::kFloat && dbias->sizes() == bias->sizes() &&
-                    dbias->strides() == bias->strides(), "attn_bwd: dbias must be fp32 with the shape/strides of bias");
+  if (given(dbias)) {
+    TORCH_CHECK(a.bias != nullptr && dbias->scalar_type() == at::kFloat && dbias->device() == q.device() &&
+                    dbias->sizes() == bias->sizes() && dbias->strides() == bias->strides(),
+                "attn_bwd: dbias must be fp32 with the shape/strides of bias");
     dbp = dbias->data_ptr<float>();
   }
-  const bool has_rng = p_drop > 0.0 && rng_state.has_value() && rng_state->defined() && rng_state->numel() == 2;
-  check(lb_attn_bwd(dout_c.data_ptr(), q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(), lse.data_ptr<float>(),
-                    dq5.data_ptr(), dk.data_ptr(), dv.data_ptr(), dqs, dkvs, delta.data_ptr<float>(),
-                    dq_acc.data_ptr<float>(), B, A, G, Sq, Sk, D, qs, ks, vs, ds, causal ? 1 : 0, (float)scale, kvl, kvs,
-                    dst, bd.ptr, bd.strides,
-                    (alibi_slopes.has_value() && alibi_slopes->defined()) ? alibi_slopes->data_ptr<float>() : nullptr, dbp,
-                    (float)(has_rng ? p_drop : 0.0),
-                    has_rng ? reinterpret_cast<const long long*>(rng_state->data_ptr<int64_t>()) : nullptr,
+  check(lb_attn_bwd(&a, dout_c.data_ptr(), ds, q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(),
+                    lse.data_ptr<float>(), dq5.data_ptr(), dk.data_ptr(), dv.data_ptr(), dqs, dkvs,
+                    delta.data_ptr<float>(), dq_acc.data_ptr<float>(), dbp,
+                    drop ? reinterpret_cast<const long long*>(rng_state->data_ptr<int64_t>()) : nullptr,
                     reinterpret_cast<unsigned*>(dq_order.data_ptr<int>()), cur_stream()),
         "attn_bwd");
   Tensor dq = q.dim() == 5 ? dq5 : dq5.reshape({B, A, Sq, D});   // after the kernel: for r > 1 this copies

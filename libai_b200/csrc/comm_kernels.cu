@@ -207,11 +207,8 @@ p2p_allgather_push_kernel(const uint4* __restrict__ shard, PeerPtrs outs, PeerPt
 
 namespace {
 int comm_grid(size_t work) {
-  int dev = 0, sms = 132;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   size_t need = (work + 255) / 256;
-  size_t cap = (size_t)sms * 4;
+  size_t cap = (size_t)lb_host::num_sms() * 4;
   return (int)(need < cap ? (need == 0 ? 1 : need) : cap);
 }
 lb::PeerPtrs to_peers(const long* ptrs, int world) {

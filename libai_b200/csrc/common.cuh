@@ -7,6 +7,7 @@
 #include <stdint.h>
 #include <stdio.h>
 
+#include "launchers.h"
 #include "wgmma.cuh"
 
 namespace lb {
@@ -109,14 +110,6 @@ LB_DEVICE void spin_wait_ge_gpu(const uint32_t* addr, uint32_t target, unsigned 
 // values before every replay) — so captured transformer blocks draw fresh masks on every replay.
 // `salt` distinguishes tensor-parallel ranks in sharded regions (0 in replicated regions: identical masks).
 // ---------------------------------------------------------------------------------------------
-struct RngArgs {
-  unsigned long long seed_val, offset_val;   // eager: the values
-  const long long* seed_ptr;                 // capture: where PyTorch keeps them
-  const long long* offset_ptr;
-  unsigned int offset_intragraph;
-  int captured;
-  unsigned long long salt;
-};
 LB_DEVICE void rng_resolve(const RngArgs& a, unsigned long long& seed, unsigned long long& offset) {
   if (a.captured) {
     seed = static_cast<unsigned long long>(*a.seed_ptr);
@@ -435,6 +428,8 @@ bool make_tmap_typed(CUtensorMap* out, CUtensorMapDataType dtype, const void* ba
                      const uint64_t* strides_bytes, const uint32_t* box, CUtensorMapSwizzle swizzle);
 bool make_tmap_bf16(CUtensorMap* out, const void* base, int rank, const uint64_t* dims, const uint64_t* strides_bytes,
                     const uint32_t* box, CUtensorMapSwizzle swizzle);
+// multiprocessors of the current device, queried once per process
+int num_sms();
 // the process-wide lb::SpinTimeout record (host-mapped pinned memory, allocated on first use); null when it does not
 // exist yet and `s` is being captured into a CUDA graph, or when the allocation failed
 lb::SpinTimeout* spin_timeout_record(cudaStream_t s);

@@ -350,16 +350,6 @@ __global__ void kv_append_kernel(const __nv_bfloat16* __restrict__ qkv, const fl
 }  // namespace lb
 
 namespace {
-int dec_sm_count() {
-  static int n = 0;
-  if (n == 0) {
-    int dev = 0;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-  }
-  return n;
-}
-
 // opts the kernel into its dynamic shared memory once; returns how many of its CTAs one SM holds (0 on error)
 template <int D>
 int configure_decode() {
@@ -390,7 +380,7 @@ cudaError_t launch_decode(const lb::dec::Params& p, int B, int nsplit, cudaStrea
 // G * ceil(r * Sq / 16) CTAs per sample and split.  Depends on the shapes only, never on the current lengths.
 extern "C" int lb_decode_splits(int B, int blocks, int C, int D) {
   const int resident = D == 64 ? configure_decode<64>() : configure_decode<128>();
-  int n = dec_sm_count() * (resident > 0 ? resident : 1) / (B * blocks);
+  int n = lb_host::num_sms() * (resident > 0 ? resident : 1) / (B * blocks);
   n = n < (C + 127) / 128 ? n : (C + 127) / 128;
   n = n < lb::dec::kMaxSplits ? n : lb::dec::kMaxSplits;
   return n > 1 ? n : 1;

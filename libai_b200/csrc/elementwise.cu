@@ -573,11 +573,8 @@ __global__ void __launch_bounds__(128) embedding_bwd_kernel(const int64_t* __res
 
 namespace {
 int ew_grid(size_t work, int block) {
-  int dev = 0, sms = 132;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   size_t need = (work + block - 1) / block;
-  size_t cap = (size_t)sms * 8;
+  size_t cap = (size_t)lb_host::num_sms() * 8;
   return (int)(need < cap ? (need == 0 ? 1 : need) : cap);
 }
 }  // namespace
@@ -678,11 +675,8 @@ extern "C" int lb_rope_qkv(const void* x, const float* cosv, const float* sinv, 
 // rows per block of the column-sum pass; the number of row blocks is the row count of its fp32 workspace [.., N]
 static int colsum_rows_per_block(int M, int N) {
   if (N % 8) return 128;
-  int dev = 0, sms = 0;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   const int col_blocks = (N + 255) / 256;
-  int row_blocks = (2 * sms + col_blocks - 1) / col_blocks;  // ~2 blocks per SM
+  int row_blocks = (2 * lb_host::num_sms() + col_blocks - 1) / col_blocks;  // ~2 blocks per SM
   if (row_blocks > (M + 63) / 64) row_blocks = (M + 63) / 64;
   if (row_blocks < 1) row_blocks = 1;
   return (M + row_blocks - 1) / row_blocks;

@@ -943,6 +943,16 @@ bool make_tmap_bf16(CUtensorMap* out, const void* base, int rank, const uint64_t
   return make_tmap_typed(out, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, base, rank, dims, strides_bytes, box, swizzle);
 }
 
+int num_sms() {
+  static const int n = [] {
+    int dev = 0, sms = 0;
+    cudaGetDevice(&dev);
+    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+    return sms;
+  }();
+  return n;
+}
+
 static lb::SpinTimeout* g_spin_timeout = nullptr;
 
 lb::SpinTimeout* spin_timeout_record(cudaStream_t s) {
@@ -981,16 +991,6 @@ extern "C" int lb_spin_timeout_report(char* buf, int n) {
 }
 
 namespace {
-
-int g_num_sms = 0;
-int num_sms() {
-  if (g_num_sms == 0) {
-    int dev = 0;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&g_num_sms, cudaDevAttrMultiProcessorCount, dev);
-  }
-  return g_num_sms;
-}
 
 // operand tensor map: K-major [rows, K] -> box {64, rows_box}; MN-major [K, cols] -> box {64, 64}
 bool operand_tmap(CUtensorMap* m, const void* ptr, bool mn_major, int rows_or_cols, int K, int ld, int block_mn) {
@@ -1093,7 +1093,7 @@ static int gemm_impl(const void* a, const void* b, void* out, int M, int N, int 
   if ((lda % 8) || (ldb % 8) || (N % 8) || (ldo % 4)) return -1;
   const bool a_mn = (layout == 2);
   const bool b_mn = (layout != 0);
-  const int sms = num_sms();
+  const int sms = lb_host::num_sms();
   const int m_blocks = (M + lb::BLOCK_M - 1) / lb::BLOCK_M;
   // ---- ping-pong schedule: bf16 output of NT / NN without a collective, 128 x 128 tiles.  Its epilogue goes through
   // TMA (16-byte aligned bases, ldo % 8 == 0); pre_out and pre_in share its staging buffer, so not both at once; the

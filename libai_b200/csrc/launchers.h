@@ -1,0 +1,136 @@
+// The native C boundary: every extern "C" kernel launcher of the extension, declared once.  Each .cu file sees these
+// declarations through common.cuh and bindings.cpp includes them, so a definition that disagrees with its declaration
+// fails to compile ("conflicting declaration of C function") instead of being called with the wrong arguments.
+// Host-only: no device code, so g++ compiles it as well as nvcc.
+#pragma once
+#include <cuda_runtime.h>
+#include <stdint.h>
+
+namespace lb {
+
+// (seed, offset) of the PyTorch CUDA generator for a dropout mask (see rng_resolve in common.cuh): the values in eager
+// mode, device pointers and an intra-graph offset while a CUDA graph is being captured; `salt` distinguishes
+// tensor-parallel ranks in sharded regions
+struct RngArgs {
+  unsigned long long seed_val, offset_val;   // eager: the values
+  const long long* seed_ptr;                 // capture: where PyTorch keeps them
+  const long long* offset_ptr;
+  unsigned int offset_intragraph;
+  int captured;
+  unsigned long long salt;
+};
+
+// One flash-attention problem, shared by lb_attn_fwd and lb_attn_bwd.  A query heads in G groups (query head h reads
+// K/V head h / (A / G)); Sq queries against Sk keys; head dim d a multiple of 8 in [8, 128].  Strides are in elements.
+// Key j is visible to query i of sample b iff kv_start[b] <= j < kv_lens[b] (defaults 0 and Sk) and, when causal,
+// j <= i + (Sk - Sq).
+struct AttnArgs {
+  int B, A, G, Sq, Sk, d;
+  long q_strides[4];   // {batch, group, in-group, seq}
+  long k_strides[3];   // {batch, head, seq} over the G K/V heads
+  long v_strides[3];
+  bool causal;
+  float scale;
+  const int* kv_lens;     // optional int32 [B]: end of the visible keys per sample
+  const int* kv_start;    // optional int32 [B]: start of the visible keys per sample
+  const int* doc_start;   // optional int32 [B, Sq]: packed sequences, query i sees keys doc_start[b, i] <= j <= i
+  const void* bias;       // optional bf16 additive score bias, key stride 1
+  long bias_strides[3];   // {batch, head, query} of bias, 0 for a broadcast dimension
+  const float* alibi_slopes;   // optional fp32 [A]; ignored when `bias` is given
+  float p_drop;           // attention dropout probability in [0, 1), quantised to 1/256
+};
+
+// packed sequences (doc_start) run as causal self-attention only, without kv_lens, kv_start, bias, ALiBi or dropout
+inline bool attn_doc_start_supported(const AttnArgs& a) {
+  return a.causal && a.Sq == a.Sk && a.kv_lens == nullptr && a.kv_start == nullptr && a.bias == nullptr &&
+         a.alibi_slopes == nullptr && !(a.p_drop > 0.f);
+}
+
+}  // namespace lb
+
+extern "C" {
+int lb_gemm_bf16(const void* a, const void* b, void* out, int M, int N, int K, int lda, int ldb, int ldo, int layout,
+                 int epi, const void* bias, int act, void* pre_out, int force_bn, int force_splits, cudaStream_t s);
+int lb_gemm_set_schedule(int schedule);
+int lb_norm_fwd(const void* x, const void* gamma, const void* beta, void* y, float* mean, float* rstd, int rows, int H,
+                float eps, int rms, int dtype, int wdtype, cudaStream_t s);
+int lb_gemm_bf16_bias_residual(const void* x, const void* w, void* out, int M, int N, int K, int lda, int ldb,
+                               const void* bias, const void* residual, cudaStream_t s);
+int lb_gemm_fp8(const void* xq, const void* wq, void* out, int M, int N, int K, const void* bias, int act, void* pre_out,
+                const void* residual, const float* deq_x, const float* deq_w, int force_bn, cudaStream_t s);
+int lb_quant_e4m3(const void* x, void* q, void* amax_scratch, float* deq, long n, cudaStream_t s);
+int lb_norm_bwd_workspace_rows(int rows);
+int lb_norm_bwd_supports_gadd(int H);
+int lb_norm_bwd(const void* gy, const void* x, const void* gamma, const float* mean, const float* rstd, void* gx,
+                float* dgamma, float* dbeta, float* workspace, int rows, int H, int rms, int dtype, int wdtype,
+                int accumulate, const void* gadd, cudaStream_t s);
+int lb_bias_act_fwd(const void* x, const void* bias, void* y, long rows, int N, int act, cudaStream_t s);
+int lb_gemm_bf16_actgrad(const void* a, const void* b, void* out, int M, int N, int K, int lda, int ldb, int ldo,
+                         int layout, int act, const void* pre_in, float* colsum, cudaStream_t stream);
+int lb_bias_act_bwd(const void* gy, const void* x, const void* bias, void* gx, long rows, int N, int act,
+                    cudaStream_t s);
+int lb_bias_residual(const void* x, const void* bias, const void* res, void* y, long rows, int N, cudaStream_t s);
+int lb_swiglu_fwd(const void* gate, const void* up, void* y, long n, cudaStream_t s);
+int lb_swiglu_bwd(const void* gy, const void* gate, const void* up, void* dgate, void* dup, long n, cudaStream_t s);
+int lb_swiglu_packed_fwd(const void* gu, void* y, long rows, long F, cudaStream_t s);
+int lb_swiglu_packed_bwd(const void* gy, const void* gu, void* dgu, long rows, long F, cudaStream_t s);
+int lb_rope_qkv(const void* x, const float* cosv, const float* sinv, void* y, long groups, int S, int G, int r, int D,
+                int pos_offset, const int* positions, int npos, int backward, cudaStream_t s);
+int lb_rope(const void* x, const float* cosv, const float* sinv, void* y, long rows, int S, int D, int backward,
+            cudaStream_t s);
+int lb_colsum_workspace_rows(int M, int N);
+int lb_colsum(const void* x, float* out, int M, int N, int accumulate, float* workspace, cudaStream_t s);
+int lb_embedding_fwd(const int64_t* ids, const void* table, void* out, long T, int H, long vocab_start, long rows, cudaStream_t s);
+int lb_embedding_bwd(const int64_t* sorted_ids, const int64_t* order, const void* gy, float* grad, long T, int H,
+                     long vocab_start, long rows, cudaStream_t s);
+int lb_ce_stats(const void* logits, const int64_t* labels, float* mx, float* se, float* tgt, int T, int V,
+                long vocab_start, int dtype, cudaStream_t s);
+int lb_ce_bwd(const void* logits, const int64_t* labels, const float* lse, const float* gloss, void* dlogits, int T,
+              int V, long vocab_start, int dtype, cudaStream_t s);
+int lb_adamw(float* master, const float* grad, float* m, float* v, void* lp_out, int lp_dtype, const float* scale, long n,
+             float lr, float b1, float b2, float eps, float wd, float bc1, float bc2, int decoupled, cudaStream_t s);
+int lb_sqnorm_workspace(long n);
+int lb_sqnorm(const float* x, float* out, long n, float* workspace, cudaStream_t s);
+int lb_gemm_bf16_comm(const void* a, const void* b, void* out, int M, int N, int K, int layout, int epi,
+                      const void* bias, int act, void* pre_out, const void* pre_in, float* colsum, int mode,
+                      int world, int rank, const long* peer_buf, const long* peer_flags, const long* peer_done,
+                      void* state, const void* local_shard, int fill_local, const void* residual, void* rs_out,
+                      long staging_parity_off, int n_comm, cudaStream_t stream);
+int lb_zero_reduce_scatter(const long* grad_ptrs, const long* flag_ptrs, float* red, float* sqnorm, long lo, long n,
+                           float scale, int world, int rank, unsigned epoch, long mc_grad, cudaStream_t s);
+int lb_zero_adam_allgather(float* master, const float* red, float* m, float* v, const long* param_ptrs,
+                           const long* flag_ptrs, unsigned* done_counter, const float* clip, long lo, long n, float lr,
+                           float b1, float b2, float eps, float wd, float bc1, float bc2, int decoupled, int world,
+                           int rank, unsigned epoch, long mc_param, cudaStream_t s);
+int lb_device_barrier(const long* flag_ptrs, int world, int rank, int slot, unsigned epoch, cudaStream_t s);
+int lb_p2p_allgather(const void* shard, const long* out_ptrs, const long* flag_ptrs, unsigned* done_counter,
+                     long nbytes, int world, int rank, unsigned epoch, cudaStream_t s);
+// forward: o [B, Sq, A, d] bf16, lse fp32 [B, A, Sq]; with dropout, `rng` is the stream and rng_out [2] receives the
+// (seed, offset) pair it resolved to, for the backward
+int lb_attn_fwd(const lb::AttnArgs* a, const void* q, const void* k, const void* v, void* o, float* lse,
+                const lb::RngArgs* rng, long long* rng_out, cudaStream_t s);
+// backward: dout with do_strides = {batch, head, seq} over the A query heads; dq written with dq_strides = {batch,
+// group, in-group, seq}, dk and dv with dkv_strides = {batch, head, seq}; delta fp32 [B, A, Sq] and dq_accum
+// (lb_attn_bwd_accum_floats) are workspaces, dq_order [B * A * ceil(Sq / 64)] zeroed by the caller; dbias (optional,
+// fp32, bias' strides) accumulates the bias gradient; rng_state = the forward's (seed, offset) under dropout
+int lb_attn_bwd(const lb::AttnArgs* a, const void* dout, const long* do_strides, const void* q, const void* k,
+                const void* v, const void* o, const float* lse, void* dq, void* dk, void* dv, const long* dq_strides,
+                const long* dkv_strides, float* delta, float* dq_accum, float* dbias, const long long* rng_state,
+                unsigned* dq_order, cudaStream_t s);
+long lb_attn_bwd_accum_floats(int B, int A, int Sq, int D);
+int lb_bias_dropout_residual(const void* x, const void* bias, const void* res, void* y, long rows, int N, float p,
+                             const lb::RngArgs* rng, const long long* rng_in, long long* rng_out, cudaStream_t s);
+int lb_spin_timeout_report(char* buf, int n);
+int lb_decode_splits(int B, int blocks, int C, int D);
+int lb_decode_attn(const void* q, const long* q_strides, const void* k, const void* v, void* o, float* part_o,
+                   float* part_ml, const int* seqlens, const int* kv_start, int B, int Sq, int A, int G, int C, int D,
+                   float scale, int nsplit, cudaStream_t s);
+int lb_kv_append(const void* qkv, const float* cosv, const float* sinv, void* q_out, void* k_cache, void* v_cache,
+                 const int* seqlens, int B, int Sq, int G, int r, int C, int D, cudaStream_t s);
+int lb_window_attn_groups(int B, int H, int W, int ws, int heads);
+int lb_window_attn_fwd(const void* qkv, void* out, float* lse, const float* table, const float* tau, int B, int H, int W,
+                       int ws, int shift, int heads, int d, float scale, cudaStream_t s);
+int lb_window_attn_bwd(const void* dout, const void* qkv, const float* lse, const float* table,
+                       const float* tau, void* dqkv, float* dtable, float* dtau, float* dt_part, float* dtau_part, int B,
+                       int H, int W, int ws, int shift, int heads, int d, float scale, cudaStream_t s);
+}

@@ -375,30 +375,21 @@ norm_bwd_colpart_generic(const T* __restrict__ gy, const T* __restrict__ x, cons
 }  // namespace lb
 
 namespace {
-int norm_sms() {
-  static int sms = 0;
-  if (sms == 0) {
-    int dev = 0;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-  }
-  return sms;
-}
 int norm_grid(int rows) {
   const int need = (rows + lb::NORM_WARPS - 1) / lb::NORM_WARPS;
-  const int cap = norm_sms() * 2;
+  const int cap = lb_host::num_sms() * 2;
   return need < cap ? need : cap;
 }
 // forward: 64 registers → four 8-warp blocks per SM
 int norm_fwd_grid(int rows) {
   const int need = (rows + lb::NORM_WARPS - 1) / lb::NORM_WARPS;
-  const int cap = norm_sms() * 4;
+  const int cap = lb_host::num_sms() * 4;
   return need < cap ? need : cap;
 }
 // bf16 backward: three 4-warp blocks per SM (one wave; every block leaves one row of column partials)
 int norm_bwd_bf16_grid(int rows) {
   const int need = (rows + lb::NORM_BWD_WARPS - 1) / lb::NORM_BWD_WARPS;
-  const int cap = norm_sms() * 3;
+  const int cap = lb_host::num_sms() * 3;
   return need < cap ? need : cap;
 }
 

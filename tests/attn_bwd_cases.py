@@ -2,7 +2,9 @@
 tests/golden/attn_bwd_parent.json.  The file was written by dev/attn_bwd_golden.py with the backward kernel as it was
 before the warp-specialised schedule (one consumer warpgroup per 64-key block), so every later schedule must reproduce
 those bytes exactly: the per-visit arithmetic and the order of every fp32 dQ addition are part of the kernel's
-contract.  Inputs come from a CPU torch.Generator, so they do not depend on the device's random number generator."""
+contract.  Inputs come from a CPU torch.Generator, so they do not depend on the device's random number generator.
+The forward's outputs are pinned the same way in tests/golden/attn_fwd_parent.json (dev/attn_bwd_golden.py
+--forward), written by the build before the launcher arguments were gathered into lb::AttnArgs."""
 import hashlib
 
 import torch
@@ -30,7 +32,15 @@ CASES = {
     # the attention shape of the GPT-2 medium training step
     "bench_b8_h16_s1024_d64": (8, 16, 16, 1024, 1024, 64, True, None),
 }
+# the forward's o / lse (and the rng_state it returns) are pinned in tests/golden/attn_fwd_parent.json for every case
+# above and these forward-only ones
+FWD_CASES = dict(CASES, **{
+    # the GPT-2 training step's attention with its dropout 0.1
+    "bench_b8_h16_s1024_d64_dropout": (8, 16, 16, 1024, 1024, 64, True, "dropout"),
+})
+FWD_GOLDEN = "tests/golden/attn_fwd_parent.json"
 DROPOUT_RNG_STATE = (0x5DEECE66D, 0x1234)   # (seed, offset) of the dropout stream
+FWD_DROPOUT_SEED = 0x2545F491   # torch.cuda.manual_seed before a forward with dropout
 
 
 def _randn(gen, *shape, scale=1.0):
@@ -39,7 +49,7 @@ def _randn(gen, *shape, scale=1.0):
 
 def make_inputs(name, device):
     """The arguments of ext.attn_fwd / ext.attn_bwd for one case, on `device`."""
-    B, A, G, Sq, Sk, d, causal, extra = CASES[name]
+    B, A, G, Sq, Sk, d, causal, extra = FWD_CASES[name]
     gen = torch.Generator().manual_seed(int.from_bytes(hashlib.sha256(name.encode()).digest()[:4], "little"))
     q = _randn(gen, B, A, Sq, d).to(device)
     k = _randn(gen, B, G, Sk, d).to(device)
@@ -90,6 +100,20 @@ def run_backward(ext, name, device):
     out = dict(dq=dq, dk=dk, dv=dv)
     if dbias is not None:
         out["dbias"] = dbias
+    return out
+
+
+def run_forward(ext, name, device):
+    """The forward with the case's masks, bias and dropout (drawn from the CUDA generator after
+    torch.cuda.manual_seed(FWD_DROPOUT_SEED)); returns o, lse and, with dropout, the rng_state it used."""
+    q, k, v, _, causal, scale, kw = make_inputs(name, device)
+    if kw["p"] > 0:
+        torch.cuda.manual_seed(FWD_DROPOUT_SEED)
+    o, lse, rng_state = ext.attn_fwd(q, k, v, causal, scale, kw["kv_lens"], kw["bias"], kw["alibi"], kw["p"], 0,
+                                     kw["kv_start"], kw["doc_start"])
+    out = dict(o=o, lse=lse)
+    if kw["p"] > 0:
+        out["rng_state"] = rng_state
     return out
 
 
