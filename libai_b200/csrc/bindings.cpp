@@ -484,6 +484,80 @@ Tensor rope_qkv(const Tensor& qkv, const Tensor& cosv, const Tensor& sinv, int64
   return y;
 }
 
+// ChatGLM rotary: the fused projection [b, s, (a + 2g) * d] <-> the packed layouts the attention kernels read (grouped
+// [b, s, g, a/g + 2, d] or per-head [b, s, a, 3d]).  `what` names the op in every error.
+struct GlmRotary {
+  int B, S, A, G, D;
+  const int* positions;
+};
+GlmRotary glm_rotary_args(const Tensor& t, int64_t B, int64_t S, int64_t heads, int64_t kv_heads, int64_t D,
+                          const Tensor& table, int64_t pos_offset, const c10::optional<Tensor>& position_ids,
+                          const char* what) {
+  TORCH_CHECK(t.scalar_type() == at::kBFloat16, what, ": bf16 input expected, got ", t.scalar_type());
+  TORCH_CHECK(t.is_cuda() && t.is_contiguous(), what, ": contiguous CUDA input expected");
+  TORCH_CHECK(heads > 0 && kv_heads > 0 && heads % kv_heads == 0, what, ": heads (", heads,
+              ") must be a positive multiple of kv_heads (", kv_heads, ")");
+  TORCH_CHECK(D > 0 && D % 4 == 0, what, ": head dim must be a positive multiple of 4, got ", D);
+  TORCH_CHECK(S > 0, what, ": empty sequence");
+  TORCH_CHECK(table.scalar_type() == at::kFloat && table.is_contiguous() && table.dim() == 3 && table.size(1) == D / 4 &&
+                  table.size(2) == 2,
+              what, ": table must be contiguous fp32 [P, d/4, 2] = [P, ", D / 4, ", 2], got ", table.scalar_type(), " ",
+              table.sizes());
+  TORCH_CHECK(table.device() == t.device(), what, ": table must be on ", t.device(), ", got ", table.device());
+  GlmRotary g{(int)B, (int)S, (int)heads, (int)kv_heads, (int)D, nullptr};
+  g.positions = token_index(position_ids, t, g.B, g.S, what);
+  const int64_t P = table.size(0);
+  if (g.positions != nullptr) {
+    // every sample takes the positions of the first row (one host sync)
+    const auto [lo, hi] = at::aminmax(position_ids->select(0, 0));
+    const int64_t mn = lo.item<int64_t>(), mx = hi.item<int64_t>();
+    TORCH_CHECK(mn >= 0 && mx < P, what, ": position_ids must lie in [0, ", P, "), got [", mn, ", ", mx, "]");
+  } else {
+    TORCH_CHECK(pos_offset >= 0 && pos_offset + S <= P, what, ": positions [", pos_offset, ", ", pos_offset + S,
+                ") exceed the table's ", P, " rows");
+  }
+  return g;
+}
+
+Tensor glm_rotary_qkv(const Tensor& mixed, int64_t heads, int64_t kv_heads, const Tensor& table, int64_t pos_offset,
+                      const c10::optional<Tensor>& position_ids, bool grouped) {
+  c10::cuda::CUDAGuard guard(mixed.device());
+  TORCH_CHECK(mixed.dim() == 3, "glm_rotary_qkv: fused projection [b, s, (a + 2g) * d] expected, got ", mixed.sizes());
+  TORCH_CHECK(heads > 0 && kv_heads > 0 && mixed.size(2) % (heads + 2 * kv_heads) == 0, "glm_rotary_qkv: last dim ",
+              mixed.size(2), " is not (heads + 2 * kv_heads) * d");
+  const int64_t B = mixed.size(0), S = mixed.size(1), D = mixed.size(2) / (heads + 2 * kv_heads);
+  const GlmRotary g =
+      glm_rotary_args(mixed, B, S, heads, kv_heads, D, table, pos_offset, position_ids, "glm_rotary_qkv");
+  Tensor out = grouped ? at::empty({B, S, kv_heads, heads / kv_heads + 2, D}, mixed.options())
+                       : at::empty({B, S, heads, 3 * D}, mixed.options());
+  check(lb_glm_rotary_qkv(mixed.data_ptr(), table.data_ptr<float>(), out.data_ptr(), B * S, g.S, g.A, g.G, g.D,
+                          (int)pos_offset, g.positions, grouped ? 1 : 0, 0, cur_stream()),
+        "glm_rotary_qkv");
+  return out;
+}
+
+// grad: the gradient of glm_rotary_qkv's output (its rank tells the layout) -> the gradient of the fused projection
+Tensor glm_rotary_qkv_bwd(const Tensor& grad, int64_t heads, int64_t kv_heads, const Tensor& table, int64_t pos_offset,
+                          const c10::optional<Tensor>& position_ids) {
+  c10::cuda::CUDAGuard guard(grad.device());
+  const bool grouped = grad.dim() == 5;
+  TORCH_CHECK(heads > 0 && kv_heads > 0 && heads % kv_heads == 0, "glm_rotary_qkv_bwd: heads (", heads,
+              ") must be a positive multiple of kv_heads (", kv_heads, ")");
+  TORCH_CHECK(grad.dim() == 4 || grad.dim() == 5, "glm_rotary_qkv_bwd: gradient [b, s, g, a/g + 2, d] or [b, s, a, 3d] "
+              "expected, got ", grad.sizes());
+  TORCH_CHECK((grouped && grad.size(2) == kv_heads && grad.size(3) == heads / kv_heads + 2) ||
+                  (grad.dim() == 4 && grad.size(2) == heads && grad.size(3) % 3 == 0),
+              "glm_rotary_qkv_bwd: gradient [b, s, g, a/g + 2, d] or [b, s, a, 3d] expected, got ", grad.sizes());
+  const int64_t B = grad.size(0), S = grad.size(1), D = grouped ? grad.size(4) : grad.size(3) / 3;
+  const GlmRotary g =
+      glm_rotary_args(grad, B, S, heads, kv_heads, D, table, pos_offset, position_ids, "glm_rotary_qkv_bwd");
+  Tensor dmixed = at::empty({B, S, (heads + 2 * kv_heads) * D}, grad.options());
+  check(lb_glm_rotary_qkv(grad.data_ptr(), table.data_ptr<float>(), dmixed.data_ptr(), B * S, g.S, g.A, g.G, g.D,
+                          (int)pos_offset, g.positions, grouped ? 1 : 0, 1, cur_stream()),
+        "glm_rotary_qkv_bwd");
+  return dmixed;
+}
+
 Tensor rope(const Tensor& x, const Tensor& cosv, const Tensor& sinv, bool backward) {
   c10::cuda::CUDAGuard guard(x.device());
   TORCH_CHECK(x.dim() == 4 && x.is_contiguous() && x.scalar_type() == at::kBFloat16, "rope: contiguous bf16 [b,a,s,d]");
@@ -1101,6 +1175,8 @@ TORCH_LIBRARY(libai_b200, m) {
   m.def("dgrad_actgrad(Tensor gy, Tensor w, Tensor pre, int act, Tensor(a!)? bias_grad=None) -> Tensor", &dgrad_actgrad);
   m.def("rope(Tensor x, Tensor cos, Tensor sin, bool backward) -> Tensor", &rope);
   m.def("rope_qkv(Tensor(a!) qkv, Tensor cos, Tensor sin, int pos_offset, bool backward, bool inplace, Tensor? positions=None) -> Tensor(a!)", &rope_qkv);
+  m.def("glm_rotary_qkv(Tensor mixed, int heads, int kv_heads, Tensor table, int pos_offset, Tensor? position_ids, bool grouped) -> Tensor", &glm_rotary_qkv);
+  m.def("glm_rotary_qkv_bwd(Tensor grad, int heads, int kv_heads, Tensor table, int pos_offset, Tensor? position_ids) -> Tensor", &glm_rotary_qkv_bwd);
   m.def("ce_stats(Tensor logits, Tensor labels, int vocab_start) -> (Tensor, Tensor, Tensor)", &ce_stats);
   m.def("ce_bwd(Tensor(a!) logits, Tensor labels, Tensor lse, Tensor gloss, int vocab_start) -> Tensor(a!)", &ce_bwd);
   m.def("fused_adamw(Tensor(a!) master, Tensor grad, Tensor(b!) m, Tensor(c!) v, Tensor? lp_out, Tensor scale, float lr, float b1, float b2, float eps, float wd, float bc1, float bc2, bool decoupled) -> ()", &fused_adamw);

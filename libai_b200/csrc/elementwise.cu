@@ -267,6 +267,106 @@ __global__ void rope_qkv_kernel(const __nv_bfloat16* __restrict__ x, const float
   }
 }
 
+// ChatGLM2/3 rotary ("GLM" convention) between the fused projection x [tokens(b*s), (A + 2G) * D] (all q heads, then
+// all k heads, then all v heads) and a packed attention layout:
+//   grouped  [tokens, G, r + 2, D]  (per K/V group q_0 .. q_{r-1}, k, v; r = A / G)
+//   per-head [tokens, A, 3, D]      (per query head [q_h | k_{h/r} | v_{h/r}]: K/V repeated r times)
+// The first D/2 channels of every q and k head rotate in interleaved pairs (2p, 2p + 1) by table[pos, p] = (cos, sin)
+// (fp32 [npos, D/4, 2]); the other channels and v are copied.  pos = positions[i] (int32, the sequence index i of the
+// token; one row shared by the batch) or i + pos_offset.  Every product is rounded on its own (no FMA contraction), so
+// the forward is bit-identical to the fp32 reference x0·c − x1·s, x1·c + x0·s rounded once to bf16.
+// One thread per output channel pair (D % 4 == 0, so a pair never straddles the rotated half).
+LB_DEVICE int glm_position(size_t token, int S, int pos_offset, const int* __restrict__ positions) {
+  const int i = static_cast<int>(token % S);
+  return positions != nullptr ? positions[i] : i + pos_offset;
+}
+
+// forward: one pass over the packed output
+__global__ void glm_rotary_pack_kernel(const __nv_bfloat16* __restrict__ x, const float* __restrict__ table,
+                                       __nv_bfloat16* __restrict__ y, size_t tokens, int S, int A, int G, int D,
+                                       int pos_offset, const int* __restrict__ positions, int grouped) {
+  const int pairs = D / 2, r = A / G;
+  const int slots = grouped ? G * (r + 2) : 3 * A;   // D-wide rows per token in the output
+  const size_t total = tokens * slots * pairs;
+  const size_t in_row = static_cast<size_t>(A + 2 * G) * D;
+  for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
+    const int p = static_cast<int>(i % pairs);
+    const int slot = static_cast<int>((i / pairs) % slots);
+    const size_t token = i / (static_cast<size_t>(pairs) * slots);
+    int col;   // source head column of x, in units of D: q heads [0, A), k heads [A, A + G), v heads [A + G, A + 2G)
+    if (grouped) {
+      const int grp = slot / (r + 2), j = slot % (r + 2);
+      col = j < r ? grp * r + j : (j == r ? A + grp : A + G + grp);
+    } else {
+      const int h = slot / 3, part = slot % 3;
+      col = part == 0 ? h : (part == 1 ? A + h / r : A + G + h / r);
+    }
+    const __nv_bfloat162 v2 =
+        *reinterpret_cast<const __nv_bfloat162*>(x + token * in_row + static_cast<size_t>(col) * D + 2 * p);
+    __nv_bfloat162 out = v2;
+    if (col < A + G && 2 * p < D / 2) {
+      const float2 cs = reinterpret_cast<const float2*>(table)[static_cast<size_t>(glm_position(token, S, pos_offset,
+                                                                                                positions)) * (D / 4) + p];
+      const float x0 = __low2float(v2), x1 = __high2float(v2);
+      const float y0 = __fsub_rn(__fmul_rn(x0, cs.x), __fmul_rn(x1, cs.y));
+      const float y1 = __fadd_rn(__fmul_rn(x1, cs.x), __fmul_rn(x0, cs.y));
+      out = __floats2bfloat162_rn(y0, y1);
+    }
+    *reinterpret_cast<__nv_bfloat162*>(y + i * 2) = out;
+  }
+}
+
+// backward: one pass over the gradient of x.  In the per-head layout the r copies of a K/V group's gradient are summed in
+// fp32 in increasing head order; the inverse rotation (dx0 = dy0·c + dy1·s, dx1 = dy1·c − dy0·s) follows in fp32 and the
+// result is rounded once.  Every element of dx is written exactly once.
+__global__ void glm_rotary_unpack_kernel(const __nv_bfloat16* __restrict__ dy, const float* __restrict__ table,
+                                         __nv_bfloat16* __restrict__ dx, size_t tokens, int S, int A, int G, int D,
+                                         int pos_offset, const int* __restrict__ positions, int grouped) {
+  const int pairs = D / 2, r = A / G;
+  const int cols = A + 2 * G;
+  const size_t total = tokens * cols * pairs;
+  const size_t out_row = static_cast<size_t>(grouped ? G * (r + 2) : 3 * A) * D;
+  for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
+    const int p = static_cast<int>(i % pairs);
+    const int col = static_cast<int>((i / pairs) % cols);
+    const size_t token = i / (static_cast<size_t>(pairs) * cols);
+    const __nv_bfloat16* row = dy + token * out_row + 2 * p;
+    float g0, g1;
+    if (col < A) {   // query head: one slot
+      const int slot = grouped ? (col / r) * (r + 2) + col % r : 3 * col;
+      const float2 v = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(row + static_cast<size_t>(slot) * D));
+      g0 = v.x;
+      g1 = v.y;
+    } else {
+      const int kv = col < A + G ? 0 : 1, grp = col - A - kv * G;
+      if (grouped) {
+        const float2 v = __bfloat1622float2(
+            *reinterpret_cast<const __nv_bfloat162*>(row + static_cast<size_t>(grp * (r + 2) + r + kv) * D));
+        g0 = v.x;
+        g1 = v.y;
+      } else {
+        g0 = 0.f;
+        g1 = 0.f;
+        for (int h = grp * r; h < grp * r + r; ++h) {
+          const float2 v =
+              __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(row + static_cast<size_t>(3 * h + 1 + kv) * D));
+          g0 = __fadd_rn(g0, v.x);
+          g1 = __fadd_rn(g1, v.y);
+        }
+      }
+    }
+    if (col < A + G && 2 * p < D / 2) {
+      const float2 cs = reinterpret_cast<const float2*>(table)[static_cast<size_t>(glm_position(token, S, pos_offset,
+                                                                                                positions)) * (D / 4) + p];
+      const float d0 = __fadd_rn(__fmul_rn(g0, cs.x), __fmul_rn(g1, cs.y));
+      const float d1 = __fsub_rn(__fmul_rn(g1, cs.x), __fmul_rn(g0, cs.y));
+      g0 = d0;
+      g1 = d1;
+    }
+    *reinterpret_cast<__nv_bfloat162*>(dx + i * 2) = __floats2bfloat162_rn(g0, g1);
+  }
+}
+
 // part[blockIdx.y, c] = sum over the block's rows of x[r, c]: block = 32 column lanes (8 columns each, 16-byte loads) x
 // 8 row stripes combined in shared memory.  The partials are summed in a fixed order by colsum_partials_kernel, so the
 // result does not depend on the order in which blocks finish.
@@ -670,6 +770,26 @@ extern "C" int lb_rope_qkv(const void* x, const float* cosv, const float* sinv, 
   else
     lb::rope_qkv_kernel<false><<<grid, 256, 0, s>>>((const bf16*)x, cosv, sinv, (bf16*)y, (size_t)groups, S, G, r, D,
                                                     pos_offset, positions, npos, backward, copy_v);
+  return (int)cudaGetLastError();
+}
+// forward (backward = 0): in = the fused projection [tokens, (A + 2G) * D], out = the packed layout (grouped [tokens, G,
+// A / G + 2, D] or per-head [tokens, A, 3D]); backward: in = the gradient of the packed layout, out = that of the fused
+// projection.  table fp32 [npos, D / 4, 2]; positions (optional, int32 [S]) replaces i + pos_offset.  The caller keeps
+// every position in [0, npos).
+extern "C" int lb_glm_rotary_qkv(const void* in, const float* table, void* out, long tokens, int S, int A, int G, int D,
+                                 int pos_offset, const int* positions, int grouped, int backward, cudaStream_t s) {
+  if (G <= 0 || A % G || D % 4 || S <= 0) return -1;
+  if (tokens == 0) return 0;
+  if (!backward) {
+    const size_t pairs = (size_t)tokens * (grouped ? (A / G + 2) * G : 3 * A) * (D / 2);
+    lb::glm_rotary_pack_kernel<<<ew_grid(pairs, 256), 256, 0, s>>>((const bf16*)in, table, (bf16*)out, (size_t)tokens,
+                                                                    S, A, G, D, pos_offset, positions, grouped);
+  } else {
+    const size_t pairs = (size_t)tokens * (A + 2 * G) * (D / 2);
+    lb::glm_rotary_unpack_kernel<<<ew_grid(pairs, 256), 256, 0, s>>>((const bf16*)in, table, (bf16*)out,
+                                                                      (size_t)tokens, S, A, G, D, pos_offset, positions,
+                                                                      grouped);
+  }
   return (int)cudaGetLastError();
 }
 // rows per block of the column-sum pass; the number of row blocks is the row count of its fp32 workspace [.., N]

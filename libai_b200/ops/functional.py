@@ -1099,6 +1099,84 @@ def apply_rotary_qkv(qkv, cos, sin, pos_offset: int = 0, position_ids=None):
     return torch.cat([q * c + rotate_half(q) * sn, k * c + rotate_half(k) * sn, v], dim=-1)
 
 
+# ChatGLM2/3 ("GLM") rotary: the first half of every head rotates in interleaved pairs by an fp32 ``[positions, d/4, 2]``
+# (cos, sin) table (reference projects/ChatGLM/chatglm.py ``RotaryEmbedding`` / ``apply_rotary_pos_emb``)
+def glm_rope_table(seq_len: int, rotary_dim: int, base: float = 10000.0, device=None):
+    """``[seq_len, rotary_dim/2, 2]`` (cos, sin) table; ``rotary_dim`` = half of the head dimension."""
+    theta = 1.0 / (base ** (torch.arange(0, rotary_dim, 2, dtype=torch.float32, device=device) / rotary_dim))
+    idx = torch.outer(torch.arange(seq_len, dtype=torch.float32, device=device), theta)
+    return torch.stack([idx.cos(), idx.sin()], dim=-1)
+
+
+def apply_glm_rotary(x: torch.Tensor, table: torch.Tensor) -> torch.Tensor:
+    """x ``[b, s, heads, d]``; rotates interleaved pairs of the first ``2·table.shape[-2]`` channels by the first ``s``
+    rows of ``table``, in fp32."""
+    b, s, h, d = x.shape
+    rot = table.shape[-2] * 2
+    xr, xp = x[..., :rot], x[..., rot:]
+    xr = xr.float().reshape(b, s, h, rot // 2, 2)
+    c = table[:s].view(1, s, 1, rot // 2, 2)
+    out = torch.stack([xr[..., 0] * c[..., 0] - xr[..., 1] * c[..., 1], xr[..., 1] * c[..., 0] + xr[..., 0] * c[..., 1]], -1)
+    return torch.cat([out.flatten(3).to(x.dtype), xp], dim=-1)
+
+
+def apply_glm_rotary_qkv_ref(mixed, *, heads: int, kv_heads: int, table, pos_offset: int = 0, position_ids=None,
+                             grouped: bool = False):
+    """:func:`apply_glm_rotary_qkv` in PyTorch: :func:`apply_glm_rotary` on q and k, then stacked (and, per-head,
+    repeated) into the packed layout."""
+    b, s, _ = mixed.shape
+    a, g = heads, kv_heads
+    d = mixed.shape[-1] // (a + 2 * g)
+    rope = table[position_ids[0].long()] if position_ids is not None else table[pos_offset : pos_offset + s]
+    q, k, v = mixed.split([a * d, g * d, g * d], dim=-1)
+    q = apply_glm_rotary(q.view(b, s, a, d), rope)
+    k = apply_glm_rotary(k.view(b, s, g, d), rope)
+    v = v.view(b, s, g, d)
+    if grouped:
+        return torch.cat([q.view(b, s, g, a // g, d), k.unsqueeze(3), v.unsqueeze(3)], dim=3)
+    return torch.cat([q, k.repeat_interleave(a // g, dim=2), v.repeat_interleave(a // g, dim=2)], dim=-1)
+
+
+class _GlmRotaryQKVFn(torch.autograd.Function):
+    """The GLM rotary pass from the fused projection to a packed layout; the backward sums the per-head K/V copies and
+    rotates back in one pass."""
+
+    @staticmethod
+    def forward(ctx, mixed, heads, kv_heads, table, pos_offset, position_ids, grouped):
+        ext = load_ext()
+        ctx.save_for_backward(table, position_ids)
+        ctx.geom = (heads, kv_heads, pos_offset)
+        count_launch()
+        return ext.glm_rotary_qkv(mixed, heads, kv_heads, table, pos_offset, position_ids, grouped)
+
+    @staticmethod
+    def backward(ctx, g):
+        ext = load_ext()
+        table, position_ids = ctx.saved_tensors
+        heads, kv_heads, pos_offset = ctx.geom
+        count_launch()
+        dmixed = ext.glm_rotary_qkv_bwd(g.contiguous(), heads, kv_heads, table, pos_offset, position_ids)
+        return dmixed, None, None, None, None, None, None
+
+
+def apply_glm_rotary_qkv(mixed, *, heads: int, kv_heads: int, table, pos_offset: int = 0, position_ids=None,
+                         grouped: bool = False):
+    """ChatGLM's fused projection ``mixed`` ``[b, s, (a + 2g)·d]`` (all ``a`` q heads, then the ``g`` k heads, then the
+    ``g`` v heads) → the packed layout the attention kernels read, q and k rotated by the GLM rotary (:func:`apply_glm_rotary`
+    with the fp32 ``table`` ``[P, d/4, 2]`` of :func:`glm_rope_table`): per-head ``[b, s, a, 3d]`` (query head ``h``
+    with copies of K/V group ``h // (a // g)``, for :func:`attention_qkvpacked`), or with ``grouped`` ``[b, s, g, a/g + 2,
+    d]`` (for :func:`kv_cache_append`).  Token ``i`` sits at position ``pos_offset + i``, or ``position_ids[0, i]``
+    (``[b, s]``; the first row serves the whole batch) when given.  The native kernel's forward is bit-identical to
+    :func:`apply_glm_rotary_qkv_ref`; its backward sums the K/V copies in fp32 and rounds once."""
+    if use_native(mixed) and mixed.dtype == torch.bfloat16 and table.dtype == torch.float32:
+        if position_ids is not None:
+            position_ids = position_ids.to(device=mixed.device, dtype=torch.int32).contiguous()
+        return _GlmRotaryQKVFn.apply(mixed.contiguous(), int(heads), int(kv_heads), table.contiguous(), int(pos_offset),
+                                     position_ids, bool(grouped))
+    return apply_glm_rotary_qkv_ref(mixed, heads=heads, kv_heads=kv_heads, table=table, pos_offset=pos_offset,
+                                    position_ids=position_ids, grouped=grouped)
+
+
 # --------------------------------------------------------------------------------------
 # fused softmax variants kept for exact-parity tests
 # --------------------------------------------------------------------------------------

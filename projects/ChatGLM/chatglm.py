@@ -13,16 +13,19 @@ Parallelism: data / pipeline parallel (the fused multi-query projection is not s
 from __future__ import annotations
 
 import math
-from typing import List, Optional
+from typing import NamedTuple, Optional
 
 import torch
 from torch import nn
 
 from libai_b200.inference.generator.generation_utils import Generator
+from libai_b200.inference.kv_cache import KVCacheLayer, KVCacheOwner, StaticKVCache, left_padding
 from libai_b200.layers import LayerNorm, Linear, RMSLayerNorm
 from libai_b200.layers._param import create_parameter
+from libai_b200.layers.attention import KeyPaddingMask
 from libai_b200.models.utils.weight_init import init_method_normal
 from libai_b200.ops import functional as OF
+from libai_b200.ops import use_native
 
 
 class PrefixEncoder(nn.Module):
@@ -43,22 +46,21 @@ class PrefixEncoder(nn.Module):
         return self.trans(tokens) if self.prefix_projection else tokens
 
 
-def rope_cache(seq_len: int, rotary_dim: int, base: float = 10000.0, device=None):
-    """``[seq, rotary_dim/2, 2]`` (cos, sin) table; ``rotary_dim`` = half of the head dimension."""
-    theta = 1.0 / (base ** (torch.arange(0, rotary_dim, 2, dtype=torch.float32, device=device) / rotary_dim))
-    idx = torch.outer(torch.arange(seq_len, dtype=torch.float32, device=device), theta)
-    return torch.stack([idx.cos(), idx.sin()], dim=-1)
+rope_cache = OF.glm_rope_table   # ``[seq, rotary_dim/2, 2]`` (cos, sin) table; ``rotary_dim`` = half of the head dim
+apply_rotary_pos_emb = OF.apply_glm_rotary   # x ``[b, s, heads, d]`` rotated by the first ``s`` rows of a table
 
 
-def apply_rotary_pos_emb(x: torch.Tensor, cache: torch.Tensor) -> torch.Tensor:
-    """x ``[b, s, heads, d]``; rotates interleaved pairs of the first ``2·cache.shape[-2]`` channels."""
-    b, s, h, d = x.shape
-    rot = cache.shape[-2] * 2
-    xr, xp = x[..., :rot], x[..., rot:]
-    xr = xr.float().reshape(b, s, h, rot // 2, 2)
-    c = cache[:s].view(1, s, 1, rot // 2, 2)
-    out = torch.stack([xr[..., 0] * c[..., 0] - xr[..., 1] * c[..., 1], xr[..., 1] * c[..., 0] + xr[..., 0] * c[..., 1]], -1)
-    return torch.cat([out.flatten(3).to(x.dtype), xp], dim=-1)
+class AttentionInputs(NamedTuple):
+    """What every layer's attention takes besides its hidden states, decided once per forward: the rotary table and
+    positions of the new tokens, and how keys are masked — ``mask`` (a dense ``[b, 1, q, k]`` visibility for the
+    reference math), ``kv_lens`` (right padding) or ``kv_start`` (left padding), none of them for plain causal."""
+
+    table: torch.Tensor
+    pos_offset: int = 0
+    position_ids: Optional[torch.Tensor] = None
+    mask: Optional[torch.Tensor] = None
+    kv_lens: Optional[torch.Tensor] = None
+    kv_start: Optional[torch.Tensor] = None
 
 
 class RotaryEmbedding(nn.Module):
@@ -75,18 +77,19 @@ class RotaryEmbedding(nn.Module):
 
 class CoreAttention(nn.Module):
     """Scaled-dot-product core on ``[b, heads, s, d]`` tensors → ``[b, s, heads·d]``: the flash kernel when no explicit
-    mask is given (causal for square scores), the masked reference math otherwise."""
+    mask is given (causal, bottom-right aligned when there are more keys than queries; ``kv_start`` = left padding),
+    the masked reference math otherwise."""
 
     def __init__(self, cfg=None, layer_number=1):
         super().__init__()
         self.layer_number = max(1, layer_number)
         self.attention_dropout = float(cfg.attention_dropout) if cfg is not None else 0.0
 
-    def forward(self, query_layer, key_layer, value_layer, attention_mask=None):
+    def forward(self, query_layer, key_layer, value_layer, attention_mask=None, kv_start=None):
         b, a, s, d = query_layer.shape
-        causal = attention_mask is None and s == key_layer.shape[2]
-        ctx = OF.attention(query_layer, key_layer, value_layer, causal=causal, scale=1.0 / math.sqrt(d),
-                           mask=attention_mask, dropout_p=self.attention_dropout, training=self.training)
+        ctx = OF.attention(query_layer, key_layer, value_layer, causal=attention_mask is None, scale=1.0 / math.sqrt(d),
+                           mask=attention_mask, dropout_p=self.attention_dropout, training=self.training,
+                           kv_start=kv_start)
         return ctx.transpose(1, 2).reshape(b, s, a * d)
 
 
@@ -105,24 +108,50 @@ class SelfAttention(nn.Module):
                             layer_idx=layer_number - 1)
         self.attention_dropout = cfg.attention_dropout
         self.core_attention = CoreAttention(cfg, layer_number)
+        # what a StaticKVCache sizes itself by (KVCacheOwner): the cache holds the g key/value heads
+        self.head_size, self.local_heads, self.local_kv_heads = self.d, self.heads, self.groups
 
-    def forward(self, hidden, attention_mask, rotary_pos_emb, kv_cache=None, use_cache=True):
+    def forward(self, hidden, inputs: AttentionInputs, kv_cache=None):
+        """``kv_cache``: this layer's :class:`KVCacheLayer` (cached generation), or the P-tuning prefix ``(k, v)``
+        (``[b, g, pre, d]`` each, never rotated), or None."""
         b, s, _ = hidden.shape
         a, g, d = self.heads, self.groups, self.d
         mixed = self.query_key_value(hidden)
-        q, k, v = mixed.split([a * d, g * d, g * d], dim=-1)
-        q, k, v = q.view(b, s, a, d), k.view(b, s, g, d), v.view(b, s, g, d)
-        if rotary_pos_emb is not None:
-            q, k = apply_rotary_pos_emb(q, rotary_pos_emb), apply_rotary_pos_emb(k, rotary_pos_emb)
-        q, k, v = q.transpose(1, 2), k.transpose(1, 2), v.transpose(1, 2)  # [b, heads, s, d]
-        if kv_cache is not None:
-            k = torch.cat((kv_cache[0].type_as(k), k), dim=2)
-            v = torch.cat((kv_cache[1].type_as(v), v), dim=2)
-        new_cache = (k, v) if use_cache else None
-        if g != a:  # multi-query: every group of a/g query heads shares one KV head
-            k = k.repeat_interleave(a // g, dim=1)
-            v = v.repeat_interleave(a // g, dim=1)
-        return self.dense(self.core_attention(q, k, v, attention_mask)), new_cache
+        if isinstance(kv_cache, KVCacheLayer):
+            return self.dense(self._cached_attention(mixed, inputs, kv_cache).reshape(b, s, a * d))
+        # per-head [b, s, a, 3d]: every query head with its own copy of its group's K/V (multi-query attention)
+        qkv = OF.apply_glm_rotary_qkv(mixed, heads=a, kv_heads=g, table=inputs.table, pos_offset=inputs.pos_offset,
+                                      position_ids=inputs.position_ids)
+        if kv_cache is None and inputs.mask is None and inputs.kv_start is None and OF.attention_qkvpacked_supported(
+                qkv, None, self.attention_dropout, self.training):
+            ctx = OF.attention_qkvpacked(qkv, causal=True, scale=1.0 / math.sqrt(d), kv_lens=inputs.kv_lens,
+                                         dropout_p=self.attention_dropout, training=self.training)
+            return self.dense(ctx.reshape(b, s, a * d))
+        q, k, v = (t.transpose(1, 2) for t in OF.split_qkv(qkv))   # [b, a, s, d] views
+        if kv_cache is not None:   # P-tuning v2: the prefix keys / values go in front of the tokens'
+            k = torch.cat((kv_cache[0].repeat_interleave(a // g, dim=1).type_as(k), k), dim=2)
+            v = torch.cat((kv_cache[1].repeat_interleave(a // g, dim=1).type_as(v), v), dim=2)
+        return self.dense(self.core_attention(q, k, v, inputs.mask, kv_start=inputs.kv_start))
+
+    def _cached_attention(self, mixed, inputs: AttentionInputs, cache: KVCacheLayer):
+        """GLM rotary into the grouped layout, append to the layer's cache, then attention over it → ``[b, s, a, d]``.
+        Once the cache holds rows (a P-tuning prefix, an earlier step), the new tokens go to :func:`OF.decode_attention`
+        (the split-KV kernel up to 16 tokens, the causal flash kernel over the cache window beyond); the prefill of an
+        empty cache runs the flash kernel (``cache.kv_start`` carries left padding), and a dense ``inputs.mask`` the
+        reference math."""
+        a, g, d = self.heads, self.groups, self.d
+        qkv = OF.apply_glm_rotary_qkv(mixed, heads=a, kv_heads=g, table=inputs.table, pos_offset=inputs.pos_offset,
+                                      position_ids=inputs.position_ids, grouped=True)
+        past, scale = cache.length, 1.0 / math.sqrt(d)
+        q = OF.kv_cache_append(qkv, cache.k, cache.v, cache.seqlens)
+        if past > 0 and inputs.mask is None:
+            return OF.decode_attention(q, cache.k, cache.v, cache.seqlens, cache.kv_start, scale=scale, past=past)
+        L = past + qkv.shape[1]
+        query, key, value = q.permute(0, 2, 1, 3), cache.k[:, :, :L], cache.v[:, :, :L]
+        causal = inputs.mask is None
+        kv_start = cache.kv_start if causal and OF.attention_supported(query, key) else None
+        ctx = OF.attention(query, key, value, causal=causal, scale=scale, mask=inputs.mask, kv_start=kv_start)
+        return ctx.transpose(1, 2)
 
 
 class MLP(nn.Module):
@@ -151,15 +180,14 @@ class GLMBlock(nn.Module):
         self.post_attention_layernorm = norm(cfg.hidden_size, eps=cfg.layernorm_epsilon, layer_idx=self.layer_idx)
         self.mlp = MLP(cfg, self.layer_idx)
 
-    def forward(self, hidden, attention_mask, rotary_pos_emb, kv_cache=None, use_cache=True):
+    def forward(self, hidden, inputs: AttentionInputs, kv_cache=None):
         ln = self.input_layernorm(hidden)
-        attn, kv_cache = self.self_attention(ln, attention_mask, rotary_pos_emb, kv_cache=kv_cache, use_cache=use_cache)
+        attn = self.self_attention(ln, inputs, kv_cache=kv_cache)
         residual = ln if self.apply_residual_connection_post_layernorm else hidden
         x = residual + torch.nn.functional.dropout(attn, p=self.hidden_dropout, training=self.training)
         ln2 = self.post_attention_layernorm(x)
         residual = ln2 if self.apply_residual_connection_post_layernorm else x
-        out = residual + torch.nn.functional.dropout(self.mlp(ln2), p=self.hidden_dropout, training=self.training)
-        return out, kv_cache
+        return residual + torch.nn.functional.dropout(self.mlp(ln2), p=self.hidden_dropout, training=self.training)
 
 
 class GLMTransformer(nn.Module):
@@ -171,15 +199,14 @@ class GLMTransformer(nn.Module):
             norm = RMSLayerNorm if cfg.rmsnorm else LayerNorm
             self.final_layernorm = norm(cfg.hidden_size, eps=cfg.layernorm_epsilon, layer_idx=-1)
 
-    def forward(self, hidden, attention_mask, rotary_pos_emb, kv_caches=None, use_cache=True):
+    def forward(self, hidden, inputs: AttentionInputs, kv_caches=None):
+        """``kv_caches``: one entry per layer (see :meth:`SelfAttention.forward`), or None."""
         kv_caches = kv_caches or [None] * self.num_layers
-        presents = []
         for layer, cache in zip(self.layers, kv_caches):
-            hidden, present = layer(hidden, attention_mask, rotary_pos_emb, kv_cache=cache, use_cache=use_cache)
-            presents.append(present)
+            hidden = layer(hidden, inputs, kv_cache=cache)
         if self.post_layer_norm:
             hidden = self.final_layernorm(hidden)
-        return hidden, (presents if use_cache else None)
+        return hidden
 
 
 class EmbeddingLayer(nn.Module):
@@ -245,42 +272,92 @@ class ChatGLMModel(nn.Module, ChatGLMPreTrainedModel):
             mask = mask & padding_mask.bool()[:, None, None, :k]
         return mask
 
-    def forward(self, input_ids, position_ids=None, attention_mask=None, past_key_values=None, use_cache=False):
+    def _flash_attention(self, hidden) -> bool:
+        """True when the layers' attention runs the flash kernels (see :func:`OF.attention_supported`), which take
+        right / left padding as ``kv_lens`` / ``kv_start`` instead of a dense mask."""
+        return use_native(hidden) and hidden.dtype == torch.bfloat16 and OF.flash_head_dim_supported(self.kv_channels)
+
+    def forward(self, input_ids, position_ids=None, attention_mask=None, past_key_values=None):
+        """``past_key_values``: the :class:`StaticKVCache` of cached generation (appended to in place), or None.
+        ``attention_mask`` ``[b, past + s]``: 1 = token, 0 = padding.  ``position_ids`` ``[b, s]``: the rotary positions
+        of the tokens (the first row serves the batch); by default they continue from the cache."""
         b, q = input_ids.shape
         hidden = self.embedding(input_ids)
-        if self.pre_seq_len is not None and past_key_values is None:
-            past_key_values = self.get_prompt(b, input_ids.device, hidden.dtype)
-        past_len = 0 if not past_key_values or past_key_values[0] is None else past_key_values[0][0].shape[2]
         if self._rope is None or self._rope.device != input_ids.device or self._rope.shape[0] < self.seq_length:
             self._rope = rope_cache(self.seq_length, self.rotary_dim, device=input_ids.device)
-        rope_offset = past_len - (self.pre_seq_len or 0) if self.pre_seq_len is not None else past_len
-        if position_ids is not None:
-            rope = self._rope[position_ids[0]]
-        else:
-            rope = self._rope[max(rope_offset, 0) : max(rope_offset, 0) + q]
-        mask = self.get_masks(input_ids, past_len, attention_mask)
-        hidden, presents = self.encoder(hidden, mask, rope, kv_caches=past_key_values, use_cache=use_cache)
-        return hidden, presents
+        pre = self.pre_seq_len or 0
+        flash = self._flash_attention(hidden)
+        if isinstance(past_key_values, StaticKVCache):
+            cache = past_key_values
+            if cache.length == 0:   # prefill: the P-tuning prefix rows first, then the prompt's padding
+                padded = attention_mask is not None and not bool(attention_mask.all())
+                if pre:
+                    for i, (k, v) in enumerate(self.get_prompt(b, input_ids.device, hidden.dtype)):
+                        if i in cache.owned:
+                            cache.k[i][:, :, :pre] = k
+                            cache.v[i][:, :, :pre] = v
+                    cache.advance(pre)
+                if padded:
+                    kv_start = left_padding(attention_mask) if not pre else None
+                    cache.dense_mask = kv_start is None
+                    if kv_start is not None:
+                        cache.kv_start.copy_(kv_start)
+                # the flash kernel reads a left-padded prompt's padding from cache.kv_start; the reference math and
+                # every step of a mask kv_start cannot express take the dense mask
+                dense = padded and (cache.dense_mask or not flash)
+            else:
+                dense = cache.dense_mask
+            past = cache.length
+            inputs = AttentionInputs(self._rope, past - pre, position_ids,
+                                     mask=self.get_masks(input_ids, past, attention_mask) if dense else None)
+            hidden = self.encoder(hidden, inputs, kv_caches=[cache.layer(i) for i in range(self.num_layers)])
+            cache.advance(q)
+            return hidden
+        padded = attention_mask is not None and not bool(attention_mask.all())
+        inputs = AttentionInputs(self._rope, 0, position_ids)
+        if not flash or (padded and pre):
+            inputs = inputs._replace(mask=self.get_masks(input_ids, pre, attention_mask if padded else None))
+        elif padded:
+            keys = KeyPaddingMask(attention_mask)
+            kv_start = None if keys.is_prefix() else left_padding(attention_mask)
+            if keys.is_prefix():
+                inputs = inputs._replace(kv_lens=keys.lengths)
+            elif kv_start is not None:
+                inputs = inputs._replace(kv_start=kv_start)
+            else:   # neither a right- nor a left-padded batch
+                inputs = inputs._replace(mask=self.get_masks(input_ids, 0, attention_mask))
+        prefix = self.get_prompt(b, input_ids.device, hidden.dtype) if pre else None
+        return self.encoder(hidden, inputs, kv_caches=prefix)
 
 
-class ChatGLMForConditionalGeneration(nn.Module, ChatGLMPreTrainedModel, Generator):
+class ChatGLMForConditionalGeneration(nn.Module, ChatGLMPreTrainedModel, Generator, KVCacheOwner):
     def __init__(self, cfg):
         super().__init__()
         self.cfg = cfg
         self.transformer = ChatGLMModel(cfg)
-        self.past_key_values: List = [None] * cfg.num_layers
+        self.kv_cache: Optional[StaticKVCache] = None
+        self.past_length = 0
         if cfg.get("lora_enable", False):
             from projects.ChatGLM.lora.lora_model import LoraModel
 
             self.transformer = LoraModel(self.transformer, cfg.lora_cfg, "default")
 
+    @property
+    def glm(self) -> ChatGLMModel:
+        """The transformer, unwrapped from a :class:`LoraModel`."""
+        return self.transformer if isinstance(self.transformer, ChatGLMModel) else self.transformer.model
+
     def forward(self, input_ids, position_ids=None, attention_mask=None, labels=None, use_cache=False):
-        past = self.past_key_values if use_cache and self.past_key_values[0] is not None else None
-        hidden, presents = self.transformer(input_ids, position_ids, attention_mask, past, use_cache)
+        cache = None
         if use_cache:
-            self.set_cache(presents)
-        model = self.transformer.model if hasattr(self.transformer, "model") else self.transformer
-        logits = model.output_layer(hidden)
+            pre = self.glm.pre_seq_len or 0
+            cache = self._prepare_cache(input_ids, max_positions=self.glm.seq_length + pre)
+            if cache.length == 0:
+                cache.reserve(pre + input_ids.shape[1])
+        hidden = self.transformer(input_ids, position_ids, attention_mask, cache)
+        if cache is not None:
+            self.past_length = cache.length
+        logits = self.glm.output_layer(hidden)
         if labels is not None:
             shift_logits = logits[:, :-1].float().reshape(-1, logits.shape[-1])
             shift_labels = labels[:, 1:].reshape(-1)
@@ -288,13 +365,22 @@ class ChatGLMForConditionalGeneration(nn.Module, ChatGLMPreTrainedModel, Generat
             return {"loss": loss}
         return {"logits": logits}
 
-    def set_cache(self, past_key_values):
-        self.past_key_values = [None] * self.cfg.num_layers if past_key_values is None else list(past_key_values)
+    # ---- KV cache (KVCacheOwner) ----------------------------------------------------------------
+    def _cache_attention_modules(self):
+        return [layer.self_attention for layer in self.glm.encoder.layers]
+
+    def allocate_kv_cache(self, batch: int, max_length: int) -> StaticKVCache:
+        # the cache also holds the P-tuning prefix rows
+        return super().allocate_kv_cache(batch, max_length + (self.glm.pre_seq_len or 0))
 
     def prepare_inputs_for_generation(self, input_ids, past=None, attention_mask=None, use_cache=None, **kwargs):
+        """With a warm cache only the newest token is fed; the padding mask always covers cache + new tokens."""
         if past is not None and use_cache:
             input_ids = input_ids[:, -1:]
-        return {"input_ids": input_ids, "attention_mask": attention_mask, "use_cache": bool(use_cache)}
+        out = {"input_ids": input_ids, "use_cache": bool(use_cache)}
+        if attention_mask is not None and not bool(attention_mask.all()):
+            out["attention_mask"] = attention_mask
+        return out
 
     def process_response(self, output, history):
         content = ""
