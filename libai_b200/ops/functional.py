@@ -135,7 +135,9 @@ class _LinearFn(torch.autograd.Function):
         x2 = x.reshape(-1, x.shape[-1])
         if not x2.is_contiguous():
             x2 = x2.contiguous()
-        need_pre = act not in (None, "none") and (x.requires_grad or w.requires_grad)
+        # the backward runs whenever any input needs a gradient, and every gradient (the bias' alone included) goes
+        # through the activation backward, which reads the pre-activation
+        need_pre = act not in (None, "none") and any(ctx.needs_input_grad[:3])
         y, pre = _linear_fwd_any(ext, x2, w, bias, _ACT_IDS[act], need_pre)
         ctx.act = act
         ctx.has_bias = bias is not None
@@ -1057,7 +1059,8 @@ def apply_rotary(x, cos, sin):
 class _RopeQKVFn(torch.autograd.Function):
     """Rotary embedding on every q and k of the packed projection (``[b, s, a, 3d]`` or ``[b, s, g, r + 2, d]``) in one
     pass (v copied);
-    the backward rotates the packed ``dqkv`` of the attention kernel in place with the inverse rotation."""
+    the backward applies the inverse rotation to the packed ``dqkv`` into a new tensor: the incoming gradient may be
+    the caller's own tensor or one autograd also hands to another branch, so it is never overwritten."""
 
     @staticmethod
     def forward(ctx, qkv, cos, sin, pos_offset, positions=None):
@@ -1073,7 +1076,7 @@ class _RopeQKVFn(torch.autograd.Function):
         cos, sin, positions = ctx.saved_tensors
         count_launch()
         g = g if g.is_contiguous() else g.contiguous()
-        return ext.rope_qkv(g, cos, sin, ctx.pos_offset, True, True, positions), None, None, None, None
+        return ext.rope_qkv(g, cos, sin, ctx.pos_offset, True, False, positions), None, None, None, None
 
 
 def apply_rotary_qkv(qkv, cos, sin, pos_offset: int = 0, position_ids=None):
