@@ -852,9 +852,10 @@ Tensor kv_append(const Tensor& qkv, const Tensor& k_cache, const Tensor& v_cache
 
 // q [B, Sq, A, D] (any strides with D contiguous, e.g. a view of the packed projection) against the caches [B, G, C, D]
 // (query head h reads cache head h / (A / G)); query i of sample b sees keys kv_start[b] .. cache_seqlens[b] + i.
-// Returns o [B, Sq, A, D] contiguous.  splits = 0: automatic.
+// Returns o [B, Sq, A, D] contiguous.  splits = 0: automatic.  alibi_slopes (fp32 [A]): ALiBi, each visible score gets
+// slope_h * (j - cache_seqlens[b] - i).
 Tensor decode_attn(const Tensor& q, const Tensor& k_cache, const Tensor& v_cache, const Tensor& cache_seqlens,
-                   const Tensor& kv_start, double scale, int64_t splits) {
+                   const Tensor& kv_start, double scale, int64_t splits, const c10::optional<Tensor>& alibi_slopes) {
   c10::cuda::CUDAGuard guard(q.device());
   check_cache(k_cache, v_cache, "decode_attn");
   const int B = (int)k_cache.size(0), G = (int)k_cache.size(1), C = (int)k_cache.size(2), D = (int)k_cache.size(3);
@@ -868,6 +869,15 @@ Tensor decode_attn(const Tensor& q, const Tensor& k_cache, const Tensor& v_cache
               q.stride(2) % 8 == 0, "decode_attn: q must be 16-byte aligned with strides that are multiples of 8");
   check_lengths(cache_seqlens, B, "decode_attn: cache_seqlens");
   check_lengths(kv_start, B, "decode_attn: kv_start");
+  const float* slopes = nullptr;
+  if (given(alibi_slopes)) {
+    const Tensor& s = *alibi_slopes;
+    TORCH_CHECK(s.scalar_type() == at::kFloat && s.dim() == 1 && s.size(0) == A && s.device() == q.device() &&
+                    s.is_contiguous(),
+                "decode_attn: alibi_slopes: contiguous fp32 [A] on q's device, got ", s.scalar_type(), " ", s.sizes(),
+                " on ", s.device());
+    slopes = s.data_ptr<float>();
+  }
   const int row_blocks = ((A / G) * Sq + 15) / 16;   // (query head, token) rows of one cache head, 16 per CTA
   const int nsplit = splits > 0 ? (int)std::min<int64_t>(splits, 32) : lb_decode_splits(B, G * row_blocks, C, D);
   Tensor o = at::empty({B, Sq, A, D}, q.options());
@@ -879,8 +889,8 @@ Tensor decode_attn(const Tensor& q, const Tensor& k_cache, const Tensor& v_cache
   long qs[3] = {q.stride(0), q.stride(1), q.stride(2)};
   check(lb_decode_attn(q.data_ptr(), qs, k_cache.data_ptr(), v_cache.data_ptr(), o.data_ptr(),
                        nsplit > 1 ? part_o.data_ptr<float>() : nullptr, nsplit > 1 ? part_ml.data_ptr<float>() : nullptr,
-                       cache_seqlens.data_ptr<int>(), kv_start.data_ptr<int>(), B, Sq, A, G, C, D, (float)scale, nsplit,
-                       cur_stream()),
+                       cache_seqlens.data_ptr<int>(), kv_start.data_ptr<int>(), slopes, B, Sq, A, G, C, D, (float)scale,
+                       nsplit, cur_stream()),
         "decode_attn");
   return o;
 }
@@ -1186,6 +1196,6 @@ TORCH_LIBRARY(libai_b200, m) {
   m.def("kv_append(Tensor qkv, Tensor(a!) k_cache, Tensor(b!) v_cache, Tensor cache_seqlens, Tensor? cos, Tensor? sin, bool write_q) -> Tensor", &kv_append);
   m.def("window_attn_fwd(Tensor qkv, int H, int W, int window, int shift, int heads, float scale, Tensor table, Tensor? tau) -> (Tensor, Tensor)", &window_attn_fwd);
   m.def("window_attn_bwd(Tensor dout, Tensor qkv, Tensor lse, int H, int W, int window, int shift, int heads, float scale, Tensor table, Tensor? tau) -> (Tensor, Tensor, Tensor)", &window_attn_bwd);
-  m.def("decode_attn(Tensor q, Tensor k_cache, Tensor v_cache, Tensor cache_seqlens, Tensor kv_start, float scale, int splits=0) -> Tensor", &decode_attn);
+  m.def("decode_attn(Tensor q, Tensor k_cache, Tensor v_cache, Tensor cache_seqlens, Tensor kv_start, float scale, int splits=0, Tensor? alibi_slopes=None) -> Tensor", &decode_attn);
   m.def("bias_dropout_residual(Tensor x, Tensor? bias, Tensor? res, float p, int salt, Tensor? rng_state=None) -> (Tensor, Tensor)", &bias_dropout_residual);
 }

@@ -28,253 +28,18 @@
 //   (TMA tensor-map) tiles, while mma.sync's M = 16 matches Sq exactly and reads plain row-major tiles.
 //   Lengths are read on the device and the grid depends only on (B, G, r, Sq, splits): one captured launch replays correctly
 //   after cache_seqlens has been bumped on the device.
+//   ALiBi (BLOOM): with alibi_slopes (fp32 [A]) every visible score gets slope_h·(j − (cache_seqlens[b] + i)), which is
+//   the flash kernel's slope·(j − i − (Sk − Sq)) with Sk = cache_seqlens[b] + Sq, so a continuation scores the same
+//   through either kernel.  The kernel template lives in decode_attention_sm90.cuh; its ALiBi instances are compiled in
+//   decode_attention_alibi_sm90.cu.
 //   Known limit (docs/source/tutorials/get_started/Benchmark.md, "Decoding"): at large batches the kernel tops out near
 //   the same rate of key rows per second at both head dims (about 2.1 TB/s at 128, 1.0 TB/s at 64 on an H100), which
 //   points to the one bulk copy per row, not to HBM (not confirmed with a profiler).  Whole-tile TMA tensor-map loads
 //   with a 128-byte swizzle (and the matching XOR in the ldmatrix addresses) are the planned change.
-#include "common.cuh"
+#include "decode_attention_sm90.cuh"
 
 namespace lb {
 namespace dec {
-
-constexpr int kTile = 64;                  // keys per pipeline stage
-constexpr int kWarps = 4;                  // consumer warps, 16 keys of every tile each
-constexpr int kThreads = (kWarps + 1) * 32;
-constexpr int kMaxQ = 16;                  // rows of the m16n8k16 MMA: (query head, new token) pairs
-constexpr int kMaxSplits = 32;
-
-template <int D>
-struct Cfg {
-  static constexpr int kRow = D + 8;                       // padded smem row (elements): rows start 4 banks apart
-  static constexpr int kStages = D == 128 ? 3 : 4;         // 104 / 74 KB: two or three CTAs per SM
-  static constexpr int kStageElems = 2 * kTile * kRow;     // K tile, then V tile
-  static constexpr int kRingBytes = kStages * kStageElems * 2;
-  static constexpr int kMergeBytes = kWarps * kMaxQ * (D + 2) * 4;   // per-warp O, m, l for the merge
-  static constexpr int kSmem = (kRingBytes > kMergeBytes ? kRingBytes : kMergeBytes) + 2 * kStages * 8;
-};
-
-struct Params {
-  const __nv_bfloat16* q;      // [B, Sq, A, D] view: strides below (elements), D contiguous
-  long q_sb, q_si, q_sh;
-  const __nv_bfloat16* k;      // [B, G, C, D] contiguous
-  const __nv_bfloat16* v;
-  __nv_bfloat16* o;            // [B, Sq, A, D] contiguous
-  float* part_o;               // [B, G, splits, r * Sq, D] (splits > 1)
-  float2* part_ml;             // [B, G, splits, r * Sq]: (max, sum) in log2 units
-  const int* seqlens;          // [B]
-  const int* kv_start;         // [B]
-  int A, G, C, Sq;
-  int rows;                    // r * Sq
-  int row_blocks;              // ceil(rows / 16)
-  float scale_log2;
-};
-
-LB_DEVICE void bulk_load(void* dst, const void* src, uint32_t bytes, uint64_t* bar) {
-  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];\n" ::"r"(
-                   smem_u32(dst)),
-               "l"(src), "r"(bytes), "r"(smem_u32(bar))
-               : "memory");
-}
-template <int D>
-__global__ void __launch_bounds__(kThreads) decode_attn_kernel(const Params p) {
-  using C = Cfg<D>;
-  extern __shared__ __align__(128) unsigned char smem[];
-  __nv_bfloat16* ring = reinterpret_cast<__nv_bfloat16*>(smem);
-  uint64_t* full = reinterpret_cast<uint64_t*>(smem + (C::kRingBytes > C::kMergeBytes ? C::kRingBytes : C::kMergeBytes));
-  uint64_t* empty = full + C::kStages;
-
-  const int split = blockIdx.x, nsplit = gridDim.x, b = blockIdx.z;
-  const int kvh = blockIdx.y / p.row_blocks;                  // cache head
-  const int row0 = (blockIdx.y - kvh * p.row_blocks) * kMaxQ; // first (query head in group, token) row of this CTA
-  const int nrows = min(kMaxQ, p.rows - row0);
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const long head_off = ((long)b * p.G + kvh) * p.C * D;
-  const int len = p.seqlens[b];
-  const int lo = max(p.kv_start[b], 0);
-  const int hi = min(len + p.Sq, p.C);   // exclusive; the cache object keeps len + Sq <= C, this only guards memory
-  const int ntiles = hi > lo ? (hi - lo + kTile - 1) / kTile : 0;
-  const int per = (ntiles + nsplit - 1) / nsplit;
-  const int t0 = split * per;
-  const int my = max(0, min(ntiles, t0 + per) - t0);
-
-  if (threadIdx.x == 0) {
-    for (int s = 0; s < C::kStages; ++s) {
-      mbar_init(&full[s], 1);
-      mbar_init(&empty[s], kWarps);
-    }
-    fence_barrier_init();
-  }
-  __syncthreads();
-
-  // merge state of the consumer warps (rows r0 and r0 + 8 of the 16 query rows)
-  float o[D / 8][4];
-  float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};
-#pragma unroll
-  for (int n = 0; n < D / 8; ++n) o[n][0] = o[n][1] = o[n][2] = o[n][3] = 0.f;
-  const int r0 = lane >> 2, c0 = (lane & 3) * 2;
-
-  if (warp == kWarps) {
-    // producer: rows past the window repeat its last row (finite data; those keys get zero weight)
-    const __nv_bfloat16* kg = p.k + head_off;
-    const __nv_bfloat16* vg = p.v + head_off;
-    for (int t = 0; t < my; ++t) {
-      const int st = t % C::kStages;
-      if (t >= C::kStages) mbar_wait(&empty[st], ((t / C::kStages) & 1) ^ 1);
-      if (lane == 0) mbar_arrive_expect_tx(&full[st], 2 * kTile * D * 2);
-      __syncwarp();
-      __nv_bfloat16* sk = ring + st * C::kStageElems;
-      __nv_bfloat16* sv = sk + kTile * C::kRow;
-      const int base = lo + (t0 + t) * kTile;
-#pragma unroll
-      for (int r = lane; r < kTile; r += 32) {
-        const long row = min(base + r, hi - 1);
-        bulk_load(sk + r * C::kRow, kg + row * D, D * 2, &full[st]);
-        bulk_load(sv + r * C::kRow, vg + row * D, D * 2, &full[st]);
-      }
-    }
-  } else if (my > 0) {
-    // Q fragments (A operand, rows = (query head, new token) pairs; rows past the last pair are zero), loaded once.
-    // lim: the last visible key of each of this thread's two rows (causal among the new tokens)
-    uint32_t qf[D / 16][4];
-    int lim[2];
-    {
-      const int hr = kvh * (p.rows / p.Sq);   // first query head of the group
-      const bool v0 = r0 < nrows, v1 = r0 + 8 < nrows;
-      const int t0 = (row0 + r0) % p.Sq, t1 = (row0 + r0 + 8) % p.Sq;
-      lim[0] = len + t0;
-      lim[1] = len + t1;
-      const __nv_bfloat16* qb = p.q + (long)b * p.q_sb + c0;
-      const uint32_t* q0 = reinterpret_cast<const uint32_t*>(
-          qb + (long)t0 * p.q_si + (long)(hr + (row0 + r0) / p.Sq) * p.q_sh);
-      const uint32_t* q1 = reinterpret_cast<const uint32_t*>(
-          qb + (long)t1 * p.q_si + (long)(hr + (row0 + r0 + 8) / p.Sq) * p.q_sh);
-#pragma unroll
-      for (int ks = 0; ks < D / 16; ++ks) {
-        qf[ks][0] = v0 ? q0[ks * 8] : 0u;
-        qf[ks][1] = v1 ? q1[ks * 8] : 0u;
-        qf[ks][2] = v0 ? q0[ks * 8 + 4] : 0u;
-        qf[ks][3] = v1 ? q1[ks * 8 + 4] : 0u;
-      }
-    }
-    const int kw = warp * 16;
-    // ldmatrix lane addresses: K (non-transposed: keys = rows of the B fragment), V (transposed)
-    const int k_row = kw + (lane & 7) + ((lane >> 4) << 3), k_col = ((lane >> 3) & 1) * 8;
-    const int v_row = kw + (lane & 7) + (((lane >> 3) & 1) << 3), v_col = (lane >> 4) * 8;
-    for (int t = 0; t < my; ++t) {
-      const int st = t % C::kStages;
-      mbar_wait(&full[st], (t / C::kStages) & 1);
-      const __nv_bfloat16* sk = ring + st * C::kStageElems;
-      const __nv_bfloat16* sv = sk + kTile * C::kRow;
-      float s[2][4] = {{0.f, 0.f, 0.f, 0.f}, {0.f, 0.f, 0.f, 0.f}};
-#pragma unroll
-      for (int ks = 0; ks < D / 16; ++ks) {
-        uint32_t bk[4];
-        ldsm_x4(bk, sk + k_row * C::kRow + ks * 16 + k_col);
-        mma_bf16(s[0], qf[ks], bk[0], bk[1]);
-        mma_bf16(s[1], qf[ks], bk[2], bk[3]);
-      }
-      // mask + online softmax (log2 domain); the two rows of this thread are r0 and r0 + 8
-      const int key0 = lo + (t0 + t) * kTile + kw + c0;
-      float mx[2] = {-INFINITY, -INFINITY};
-#pragma unroll
-      for (int n = 0; n < 2; ++n)
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          const int key = key0 + n * 8 + (j & 1);
-          const bool vis = key < hi && key <= lim[j >> 1];
-          s[n][j] = vis ? s[n][j] * p.scale_log2 : -INFINITY;
-          mx[j >> 1] = fmaxf(mx[j >> 1], s[n][j]);
-        }
-      float alpha[2], base[2];
-#pragma unroll
-      for (int r = 0; r < 2; ++r) {
-        mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 1));
-        mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 2));
-        const float mn = fmaxf(m[r], mx[r]);
-        base[r] = mn == -INFINITY ? 0.f : mn;
-        alpha[r] = fast_exp2(m[r] - base[r]);
-        m[r] = mn;
-        l[r] *= alpha[r];
-      }
-      uint32_t pa[4];
-#pragma unroll
-      for (int n = 0; n < 2; ++n) {
-        const float p0 = fast_exp2(s[n][0] - base[0]), p1 = fast_exp2(s[n][1] - base[0]);
-        const float p2 = fast_exp2(s[n][2] - base[1]), p3 = fast_exp2(s[n][3] - base[1]);
-        l[0] += p0 + p1;
-        l[1] += p2 + p3;
-        pa[2 * n] = pack_bf16(p0, p1);
-        pa[2 * n + 1] = pack_bf16(p2, p3);
-      }
-#pragma unroll
-      for (int n = 0; n < D / 8; ++n) {
-        o[n][0] *= alpha[0];
-        o[n][1] *= alpha[0];
-        o[n][2] *= alpha[1];
-        o[n][3] *= alpha[1];
-      }
-#pragma unroll
-      for (int j = 0; j < D / 16; ++j) {
-        uint32_t bv[4];
-        ldsm_x4_t(bv, sv + v_row * C::kRow + j * 16 + v_col);
-        mma_bf16(o[2 * j], pa, bv[0], bv[1]);
-        mma_bf16(o[2 * j + 1], pa, bv[2], bv[3]);
-      }
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&empty[st]);
-    }
-#pragma unroll
-    for (int r = 0; r < 2; ++r) {
-      l[r] += __shfl_xor_sync(0xffffffffu, l[r], 1);
-      l[r] += __shfl_xor_sync(0xffffffffu, l[r], 2);
-    }
-  }
-  __syncthreads();   // every stage has been consumed: the ring becomes the merge buffer
-
-  float* mo = reinterpret_cast<float*>(smem);                 // [warp][16][D]
-  float* mm = mo + kWarps * kMaxQ * D;                        // [warp][16]
-  float* ml = mm + kWarps * kMaxQ;                            // [warp][16]
-  if (warp < kWarps) {
-    float* w = mo + warp * kMaxQ * D;
-#pragma unroll
-    for (int n = 0; n < D / 8; ++n) {
-      *reinterpret_cast<float2*>(w + r0 * D + n * 8 + c0) = make_float2(o[n][0], o[n][1]);
-      *reinterpret_cast<float2*>(w + (r0 + 8) * D + n * 8 + c0) = make_float2(o[n][2], o[n][3]);
-    }
-    if ((lane & 3) == 0) {
-      mm[warp * kMaxQ + r0] = m[0];
-      mm[warp * kMaxQ + r0 + 8] = m[1];
-      ml[warp * kMaxQ + r0] = l[0];
-      ml[warp * kMaxQ + r0 + 8] = l[1];
-    }
-  }
-  __syncthreads();
-
-  const long bg = (long)b * p.G + kvh;
-  for (int e = threadIdx.x; e < nrows * D; e += kThreads) {
-    const int i = e / D, d = e % D;   // row row0 + i: query head kvh * r + (row0 + i) / Sq, token (row0 + i) % Sq
-    float M = -INFINITY;
-#pragma unroll
-    for (int w = 0; w < kWarps; ++w) M = fmaxf(M, mm[w * kMaxQ + i]);
-    const float base = M == -INFINITY ? 0.f : M;
-    float L = 0.f, O = 0.f;
-#pragma unroll
-    for (int w = 0; w < kWarps; ++w) {
-      const float f = fast_exp2(mm[w * kMaxQ + i] - base);
-      L += ml[w * kMaxQ + i] * f;
-      O += mo[(w * kMaxQ + i) * D + d] * f;
-    }
-    if (nsplit == 1) {
-      const int row = row0 + i, tok = row % p.Sq;
-      const int h = kvh * (p.rows / p.Sq) + row / p.Sq;
-      p.o[(((long)b * p.Sq + tok) * p.A + h) * D + d] = __float2bfloat16(L > 0.f ? O / L : 0.f);
-    } else {
-      const long row = (bg * nsplit + split) * p.rows + row0 + i;
-      p.part_o[row * D + d] = O;
-      if (d == 0) p.part_ml[row] = make_float2(M, L);
-    }
-  }
-}
 
 // o[b, i, h, :] from the per-split partials, summed in split order; one CTA per (cache head, row block, sample)
 template <int D>
@@ -350,26 +115,11 @@ __global__ void kv_append_kernel(const __nv_bfloat16* __restrict__ qkv, const fl
 }  // namespace lb
 
 namespace {
-// opts the kernel into its dynamic shared memory once; returns how many of its CTAs one SM holds (0 on error)
 template <int D>
-int configure_decode() {
-  static int resident = 0;
-  if (resident == 0) {
-    using Cfg = lb::dec::Cfg<D>;
-    auto kern = lb::dec::decode_attn_kernel<D>;
-    if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmem) != cudaSuccess ||
-        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&resident, kern, lb::dec::kThreads, Cfg::kSmem) != cudaSuccess)
-      resident = 0;
-  }
-  return resident;
-}
-
-template <int D>
-cudaError_t launch_decode(const lb::dec::Params& p, int B, int nsplit, cudaStream_t s) {
-  using Cfg = lb::dec::Cfg<D>;
-  auto kern = lb::dec::decode_attn_kernel<D>;
-  if (configure_decode<D>() == 0) return cudaErrorInvalidConfiguration;   // the shared memory opt-in failed
-  kern<<<dim3(nsplit, p.G * p.row_blocks, B), lb::dec::kThreads, Cfg::kSmem, s>>>(p);
+cudaError_t launch_decode(const lb::dec::Params& p, int B, int nsplit, bool alibi, cudaStream_t s) {
+  cudaError_t e = alibi ? lb::dec::launch_decode_attn_alibi(p, D, B, nsplit, s)
+                        : lb::dec::launch_decode_attn<D, false>(p, B, nsplit, s);
+  if (e != cudaSuccess) return e;
   if (nsplit > 1) lb::dec::decode_combine_kernel<D><<<dim3(p.G * p.row_blocks, B), 128, 0, s>>>(p, nsplit);
   return cudaGetLastError();
 }
@@ -379,7 +129,8 @@ cudaError_t launch_decode(const lb::dec::Params& p, int B, int nsplit, cudaStrea
 // one wave (a second, partial wave would only add a tail), at most one split per 128 keys of the capacity.  `blocks` =
 // G * ceil(r * Sq / 16) CTAs per sample and split.  Depends on the shapes only, never on the current lengths.
 extern "C" int lb_decode_splits(int B, int blocks, int C, int D) {
-  const int resident = D == 64 ? configure_decode<64>() : configure_decode<128>();
+  // (the ALiBi instances hold as many CTAs per SM: the same shared memory, and registers that do not limit it)
+  const int resident = D == 64 ? lb::dec::configure_decode<64, false>() : lb::dec::configure_decode<128, false>();
   int n = lb_host::num_sms() * (resident > 0 ? resident : 1) / (B * blocks);
   n = n < (C + 127) / 128 ? n : (C + 127) / 128;
   n = n < lb::dec::kMaxSplits ? n : lb::dec::kMaxSplits;
@@ -387,8 +138,9 @@ extern "C" int lb_decode_splits(int B, int blocks, int C, int D) {
 }
 
 extern "C" int lb_decode_attn(const void* q, const long* q_strides, const void* k, const void* v, void* o,
-                              float* part_o, float* part_ml, const int* seqlens, const int* kv_start, int B, int Sq,
-                              int A, int G, int C, int D, float scale, int nsplit, cudaStream_t s) {
+                              float* part_o, float* part_ml, const int* seqlens, const int* kv_start,
+                              const float* alibi_slopes, int B, int Sq, int A, int G, int C, int D, float scale,
+                              int nsplit, cudaStream_t s) {
   if (B == 0 || A == 0) return 0;
   if (G <= 0 || A % G) return -4;
   lb::dec::Params p;
@@ -410,7 +162,9 @@ extern "C" int lb_decode_attn(const void* q, const long* q_strides, const void* 
   p.rows = (A / G) * Sq;
   p.row_blocks = (p.rows + lb::dec::kMaxQ - 1) / lb::dec::kMaxQ;
   p.scale_log2 = scale * 1.4426950408889634f;
-  cudaError_t e = D == 64 ? launch_decode<64>(p, B, nsplit, s) : launch_decode<128>(p, B, nsplit, s);
+  p.alibi_slopes = alibi_slopes;
+  const bool alibi = alibi_slopes != nullptr;
+  cudaError_t e = D == 64 ? launch_decode<64>(p, B, nsplit, alibi, s) : launch_decode<128>(p, B, nsplit, alibi, s);
   return (int)e;
 }
 

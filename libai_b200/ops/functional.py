@@ -872,39 +872,46 @@ def kv_cache_append_ref(qkv, k_cache, v_cache, cache_seqlens, cos=None, sin=None
 
 
 def decode_attention(q, k_cache, v_cache, cache_seqlens, kv_start, *, scale: float, splits: int = 0,
-                     past: Optional[int] = None):
+                     past: Optional[int] = None, alibi_slopes=None):
     """Attention of ``q [b, s, a, d]`` (new tokens, already appended to the caches; any strides with d contiguous) over
     the caches ``[b, g, C, d]`` (query head ``h`` reads cache head ``h // (a // g)``): query ``i`` of sample ``b`` sees exactly the keys ``kv_start[b] <= j <= cache_seqlens[b] + i``.  Returns
     ``[b, s, a, d]`` contiguous; a query without a visible key gets zeros.  The native kernel takes up to 16 new tokens
     and reads lengths on the device (no host sync; one CUDA-graph capture replays after the lengths change); ``splits``
     > 0 fixes its number of key-range splits.  ``past`` (host int): the rows every sample held before these tokens
     (``cache_seqlens`` all equal to it, as in a :class:`~libai_b200.inference.kv_cache.StaticKVCache`); with it, more
-    than 16 new tokens run the causal flash kernel over the cache window ``[:past + s]`` (chunked prefill)."""
+    than 16 new tokens run the causal flash kernel over the cache window ``[:past + s]`` (chunked prefill).
+    ``alibi_slopes`` (fp32 ``[a]``, on q's device): ALiBi, every visible score gets ``slope_h·(j − cache_seqlens[b] − i)``
+    — the flash kernel's ``slope·(j − i − (sk − sq))`` over the cache window, so both paths score alike."""
     if _decode_native(q, k_cache):
         if q.shape[1] <= 16:
             ext = load_ext()
-            o = ext.decode_attn(q, k_cache, v_cache, cache_seqlens, kv_start, float(scale), int(splits))
+            o = ext.decode_attn(q, k_cache, v_cache, cache_seqlens, kv_start, float(scale), int(splits), alibi_slopes)
             count_launch(2)
             return o
         if past is not None:
             L = past + q.shape[1]
             o = attention(q.permute(0, 2, 1, 3), k_cache[:, :, :L], v_cache[:, :, :L], causal=True, scale=scale,
-                          kv_start=kv_start)
+                          kv_start=kv_start, alibi_slopes=alibi_slopes)
             return o.transpose(1, 2)   # the kernel's [b, s, a, d] output
-    return decode_attention_ref(q, k_cache, v_cache, cache_seqlens, kv_start, scale=scale)
+    return decode_attention_ref(q, k_cache, v_cache, cache_seqlens, kv_start, scale=scale, alibi_slopes=alibi_slopes)
 
 
-def decode_attention_ref(q, k_cache, v_cache, cache_seqlens, kv_start, *, scale: float):
+def decode_attention_ref(q, k_cache, v_cache, cache_seqlens, kv_start, *, scale: float, alibi_slopes=None):
     """:func:`attention_ref` over the window ``[:L]`` of the caches (``L = max(cache_seqlens) + s``) with the mask built
-    from ``kv_start`` and causality among the new tokens."""
+    from ``kv_start`` and causality among the new tokens, and the ALiBi bias ``slope_h·(j − (cache_seqlens[b] + i))``
+    when ``alibi_slopes`` is given."""
     s_len = q.shape[1]
     lens = cache_seqlens.long()
     L = int(lens.max()) + s_len
     j = torch.arange(L, device=q.device)[None, None, :]
     i = torch.arange(s_len, device=q.device)[None, :, None]
     visible = (j >= kv_start.long()[:, None, None]) & (j <= lens[:, None, None] + i)          # [b, s, L]
+    bias = None
+    if alibi_slopes is not None:
+        rel = (j - (lens[:, None, None] + i)).float()                                          # [b, s, L]
+        bias = alibi_slopes.float()[None, :, None, None] * rel[:, None]                        # [b, a, s, L]
     o = attention_ref(q.permute(0, 2, 1, 3), k_cache[:, :, :L], v_cache[:, :, :L], causal=False, scale=scale,
-                      mask=visible[:, None])
+                      mask=visible[:, None], bias=bias)
     o = o.masked_fill(~visible.any(-1)[:, None, :, None], 0)
     return o.permute(0, 2, 1, 3).contiguous()
 

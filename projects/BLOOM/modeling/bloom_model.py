@@ -6,19 +6,27 @@ slope × key position counted over the attention mask), ``BloomAttention`` (fuse
 ``baddbmm(alibi, q, kᵀ, beta=1, alpha=1/sqrt(d))``), ``BloomModel`` (:29-255) with embedding LayerNorm and a
 final ``ln_f``, ``BloomForCausalLM`` (:258-420) with the generation hooks.  Names follow the HF checkpoint layout
 (``word_embeddings``, ``h.N.self_attention.query_key_value`` …) so the loader is a prefix strip.
+
+The kernels evaluate ALiBi from the slopes as ``slope·(j − i − (sk − sq))``.  For a left- or right-padded row that
+differs from the bias above (key position counted over the mask) by a constant along each query row, which softmax
+ignores, so the flash and decode kernels compute BLOOM's attention exactly with ``kv_start`` / ``kv_lens``.
 """
 from __future__ import annotations
 
 import math
+from typing import NamedTuple, Optional
 
 import torch
 from torch import nn
 
 from libai_b200.config import configurable
 from libai_b200.inference.generator.generation_utils import Generator
+from libai_b200.inference.kv_cache import KVCacheLayer, KVCacheOwner, StaticKVCache, left_padding
 from libai_b200.layers import LayerNorm, Linear, LMLogits, ParallelCrossEntropyLoss, VocabEmbedding
+from libai_b200.layers.attention import KeyPaddingMask
 from libai_b200.models.utils.weight_init import init_method_normal
 from libai_b200.ops import functional as OF
+from libai_b200.ops import use_native
 from libai_b200.parallel import mappings
 from libai_b200.utils import distributed as dutil
 
@@ -40,37 +48,70 @@ def build_alibi_tensor(attention_mask: torch.Tensor, num_heads: int, dtype=torch
     return (alibi_slopes(num_heads).to(attention_mask.device)[None, :, None, None] * pos).to(dtype)
 
 
+class AttentionInputs(NamedTuple):
+    """What every layer's attention takes besides its hidden states, decided once per forward: the slopes of all heads
+    (fp32 ``[n_head]``), and how keys are masked.  ``bias`` + ``mask`` (a dense ALiBi ``[b, heads, 1, k]`` and a
+    dense ``[b, 1, q, k]`` visibility) select the reference math; otherwise attention is causal with the slopes,
+    ``kv_lens`` carrying right padding and ``kv_start`` left padding (in cached generation: ``cache.kv_start``)."""
+
+    slopes: torch.Tensor
+    bias: Optional[torch.Tensor] = None
+    mask: Optional[torch.Tensor] = None
+    kv_lens: Optional[torch.Tensor] = None
+    kv_start: Optional[torch.Tensor] = None
+
+
 class BloomAttention(nn.Module):
     def __init__(self, hidden_size, n_head, hidden_dropout, attention_dropout, init_method, layer_idx):
         super().__init__()
         topo = dutil.get_dist_util()
         self.num_heads, self.head_dim = n_head, hidden_size // n_head
         self.local_heads = n_head // topo.tensor_parallel_size
+        self.head_size = self.head_dim   # what a StaticKVCache sizes itself by (KVCacheOwner)
         self.query_key_value = Linear(hidden_size, 3 * hidden_size, bias=True, parallel="col", init_method=init_method, layer_idx=layer_idx)
         self.dense = Linear(hidden_size, hidden_size, bias=True, parallel="row", init_method=init_method, layer_idx=layer_idx)
         self.attention_dropout, self.hidden_dropout = attention_dropout, nn.Dropout(hidden_dropout)
 
-    def forward(self, hidden, residual, alibi, mask, layer_past=None, use_cache=False):
-        b = hidden.shape[0]
+    def forward(self, hidden, residual, inputs: AttentionInputs, cache: Optional[KVCacheLayer] = None):
+        b, s = hidden.shape[:2]
         a, d = self.local_heads, self.head_dim
-        qkv = self.query_key_value(hidden).view(b, -1, a, 3 * d).permute(0, 2, 1, 3)
-        q, k, v = qkv[..., :d], qkv[..., d : 2 * d], qkv[..., 2 * d :]
-        if layer_past is not None:
-            k = torch.cat((layer_past[0].type_as(k), k), dim=2)
-            v = torch.cat((layer_past[1].type_as(v), v), dim=2)
-        present = (k, v) if use_cache else None
-        topo = dutil.get_dist_util()
-        if alibi.dim() == 1:
-            # unpadded batch without a KV cache: ALiBi slopes + causal mask are evaluated inside the flash kernel
-            slopes = alibi[topo.tp_rank * a : (topo.tp_rank + 1) * a] if alibi.shape[0] != a else alibi
-            ctx = OF.attention(q, k, v, causal=True, scale=1.0 / math.sqrt(d), alibi_slopes=slopes.contiguous(),
-                               dropout_p=self.attention_dropout, training=self.training)
+        rank = dutil.get_dist_util().tp_rank
+        slopes = inputs.slopes[rank * a : (rank + 1) * a]   # this rank's heads (a contiguous view)
+        bias = None if inputs.bias is None else inputs.bias[:, rank * a : (rank + 1) * a]
+        qkv = self.query_key_value(hidden).view(b, s, a, 3 * d)   # per-head [q|k|v]: the MHA packed layout
+        if cache is not None:
+            ctx = self._cached_attention(qkv, inputs, cache, slopes, bias)
         else:
-            bias = alibi[:, topo.tp_rank * a : (topo.tp_rank + 1) * a] if alibi.shape[1] != a else alibi
-            ctx = OF.attention(q, k, v, causal=False, scale=1.0 / math.sqrt(d), mask=mask, bias=bias,
-                               dropout_p=self.attention_dropout, training=self.training)
-        out = self.dense(ctx.transpose(1, 2).reshape(b, -1, a * d))
-        return residual + self.hidden_dropout(out), present
+            q, k, v = (t.transpose(1, 2) for t in OF.split_qkv(qkv))   # [b, a, s, d] views
+            if bias is None:
+                ctx = OF.attention(q, k, v, causal=True, scale=1.0 / math.sqrt(d), alibi_slopes=slopes,
+                                   kv_lens=inputs.kv_lens, kv_start=inputs.kv_start,
+                                   dropout_p=self.attention_dropout, training=self.training)
+            else:
+                ctx = OF.attention(q, k, v, causal=False, scale=1.0 / math.sqrt(d), mask=inputs.mask, bias=bias,
+                                   dropout_p=self.attention_dropout, training=self.training)
+            ctx = ctx.transpose(1, 2)
+        out = self.dense(ctx.reshape(b, s, a * d))
+        return residual + self.hidden_dropout(out)
+
+    def _cached_attention(self, qkv, inputs: AttentionInputs, cache: KVCacheLayer, slopes, bias):
+        """Append k, v to the layer's cache, then attention over it → ``[b, s, a, d]``.  Steps after the prefill go to
+        :func:`OF.decode_attention` with the slopes (the split-KV kernel up to 16 new tokens, the causal flash kernel
+        over the cache window beyond; ``cache.kv_start`` carries left padding); the prefill runs the flash kernel over
+        the cache window, and a dense ``inputs.mask`` the reference math."""
+        past, scale = cache.length, 1.0 / math.sqrt(self.head_dim)
+        q = OF.kv_cache_append(qkv, cache.k, cache.v, cache.seqlens)
+        if past > 0 and bias is None:
+            return OF.decode_attention(q, cache.k, cache.v, cache.seqlens, cache.kv_start, scale=scale, past=past,
+                                       alibi_slopes=slopes)
+        L = past + qkv.shape[1]
+        query, key, value = q.permute(0, 2, 1, 3), cache.k[:, :, :L], cache.v[:, :, :L]
+        if bias is not None:
+            ctx = OF.attention(query, key, value, causal=False, scale=scale, mask=inputs.mask, bias=bias)
+        else:   # prefill of an unpadded or left-padded prompt
+            kv_start = cache.kv_start if OF.attention_supported(query, key) else None
+            ctx = OF.attention(query, key, value, causal=True, scale=scale, alibi_slopes=slopes, kv_start=kv_start)
+        return ctx.transpose(1, 2)
 
 
 class BloomMLP(nn.Module):
@@ -95,11 +136,11 @@ class BloomBlock(nn.Module):
         self.mlp = BloomMLP(hidden_size, hidden_dropout, init_method, layer_idx)
         self.post_ln_residual = apply_residual_connection_post_layernorm
 
-    def forward(self, hidden, alibi, mask, layer_past=None, use_cache=False):
+    def forward(self, hidden, inputs: AttentionInputs, cache: Optional[KVCacheLayer] = None):
         ln = self.input_layernorm(hidden)
-        attn, present = self.self_attention(ln, ln if self.post_ln_residual else hidden, alibi, mask, layer_past, use_cache)
+        attn = self.self_attention(ln, ln if self.post_ln_residual else hidden, inputs, cache)
         ln2 = self.post_attention_layernorm(attn)
-        return self.mlp(ln2, ln2 if self.post_ln_residual else attn), present
+        return self.mlp(ln2, ln2 if self.post_ln_residual else attn)
 
 
 class BloomModel(nn.Module):
@@ -109,6 +150,7 @@ class BloomModel(nn.Module):
                  hidden_dropout=0.0, attention_dropout=0.0, amp_enabled=False, layer_norm_epsilon=1e-12, cfg=None):
         super().__init__()
         self.cfg, self.n_head, self.hidden_layers = cfg, n_head, hidden_layers
+        self.head_dim = hidden_size // n_head
         init_method = init_method_normal(initializer_range)
         self.word_embeddings = VocabEmbedding(vocab_size, hidden_size, padding_idx=padding_idx, init_method=init_method,
                                               amp_enabled=amp_enabled)
@@ -118,6 +160,8 @@ class BloomModel(nn.Module):
                        apply_residual_connection_post_layernorm, init_method, layer_idx=i)
             for i in range(hidden_layers)])
         self.ln_f = LayerNorm(hidden_size, eps=layer_norm_epsilon, layer_idx=-1)
+        # the slopes of all heads (each tensor-parallel rank reads its own); not a checkpoint entry
+        self.register_buffer("alibi_slopes", alibi_slopes(n_head), persistent=False)
 
     @classmethod
     def from_config(cls, cfg):
@@ -127,29 +171,61 @@ class BloomModel(nn.Module):
         out["cfg"] = cfg
         return out
 
-    def forward(self, input_ids, attention_mask=None, past_key_values=None, use_cache=False):
+    def _dense_inputs(self, slopes, input_ids, past: int, attention_mask) -> AttentionInputs:
+        """The reference math's inputs: HF's ALiBi (key positions counted over the mask) and the causal padding mask."""
         b, q = input_ids.shape
-        past_key_values = past_key_values or [None] * len(self.h)
-        past_len = 0 if past_key_values[0] is None else past_key_values[0][0].shape[2]
-        k = past_len + q
+        k = past + q
+        if attention_mask is None:
+            attention_mask = torch.ones(b, k, dtype=torch.long, device=input_ids.device)
+        causal = torch.ones(k, k, dtype=torch.bool, device=input_ids.device).tril()[k - q :]
+        mask = causal[None, None] & attention_mask.bool()[:, None, None, :]
+        return AttentionInputs(slopes, bias=build_alibi_tensor(attention_mask, self.n_head, torch.float32), mask=mask)
+
+    def forward(self, input_ids, attention_mask=None, past_key_values=None):
+        """``past_key_values``: the :class:`StaticKVCache` of cached generation (appended to in place), or None.
+        ``attention_mask`` ``[b, past + s]``: 1 = token, 0 = padding."""
         hidden = self.word_embeddings_layernorm(self.word_embeddings(input_ids))
-        if attention_mask is None and past_len == 0 and not use_cache and input_ids.is_cuda:
-            # no padding, no cache: hand the blocks the per-head slopes only (1-D `alibi` selects the in-kernel path)
-            alibi, mask = alibi_slopes(self.n_head).to(input_ids.device), None
-        else:
-            if attention_mask is None:
-                attention_mask = torch.ones(b, k, dtype=torch.long, device=input_ids.device)
-            alibi = build_alibi_tensor(attention_mask, self.n_head, torch.float32)
-            causal = torch.ones(k, k, dtype=torch.bool, device=input_ids.device).tril()[k - q :]
-            mask = causal[None, None] & attention_mask.bool()[:, None, None, :]
-        presents = []
-        for block, past in zip(self.h, past_key_values):
-            hidden, present = block(hidden, alibi, mask, past, use_cache)
-            presents.append(present)
-        return self.ln_f(hidden), (presents if use_cache else None)
+        if self.alibi_slopes.device != hidden.device or self.alibi_slopes.dtype != torch.float32:
+            # a model placed on the GPU or cast (``.to(torch.bfloat16)`` casts buffers too): the kernels take fp32
+            self.alibi_slopes = alibi_slopes(self.n_head).to(hidden.device)
+        slopes = self.alibi_slopes
+        # the flash kernels take right / left padding as kv_lens / kv_start instead of a dense mask
+        flash = use_native(hidden) and hidden.dtype == torch.bfloat16 and OF.flash_head_dim_supported(self.head_dim)
+        padded = attention_mask is not None and not bool(attention_mask.all())
+        if isinstance(past_key_values, StaticKVCache):
+            cache = past_key_values
+            past = cache.length
+            if past == 0 and padded:
+                kv_start = left_padding(attention_mask)
+                cache.dense_mask = kv_start is None
+                if kv_start is not None:
+                    cache.kv_start.copy_(kv_start)
+            # the flash kernel reads a left-padded prompt's padding from cache.kv_start; the reference math and every
+            # step of a mask kv_start cannot express take the dense mask
+            dense = padded and (cache.dense_mask or (past == 0 and not flash))
+            inputs = self._dense_inputs(slopes, input_ids, past, attention_mask) if dense else AttentionInputs(slopes)
+            for i, block in enumerate(self.h):
+                hidden = block(hidden, inputs, cache.layer(i))
+            cache.advance(input_ids.shape[1])
+            return self.ln_f(hidden)
+        inputs = AttentionInputs(slopes)
+        if padded and flash:
+            keys = KeyPaddingMask(attention_mask)
+            kv_start = None if keys.is_prefix() else left_padding(attention_mask)
+            if keys.is_prefix():
+                inputs = inputs._replace(kv_lens=keys.lengths)
+            elif kv_start is not None:
+                inputs = inputs._replace(kv_start=kv_start)
+            else:   # neither a right- nor a left-padded batch
+                inputs = self._dense_inputs(slopes, input_ids, 0, attention_mask)
+        elif padded or not hidden.is_cuda:
+            inputs = self._dense_inputs(slopes, input_ids, 0, attention_mask)
+        for block in self.h:
+            hidden = block(hidden, inputs)
+        return self.ln_f(hidden)
 
 
-class BloomForCausalLM(nn.Module, Generator):
+class BloomForCausalLM(nn.Module, Generator, KVCacheOwner):
     @configurable
     def __init__(self, cfg=None, **kwargs):
         super().__init__()
@@ -157,17 +233,18 @@ class BloomForCausalLM(nn.Module, Generator):
         self.transformer = BloomModel(cfg=cfg, **kwargs) if cfg is None else BloomModel(cfg)
         self.lm_head = LMLogits(self.transformer.word_embeddings.num_embeddings, bias=False)
         self.loss = ParallelCrossEntropyLoss()
-        self.past_key_values = [None] * self.transformer.hidden_layers
+        self.kv_cache: Optional[StaticKVCache] = None
+        self.past_length = 0
 
     @classmethod
     def from_config(cls, cfg):
         return {"cfg": cfg}
 
     def forward(self, input_ids, attention_mask=None, labels=None, use_cache=False):
-        hidden, presents = self.transformer(input_ids, attention_mask,
-                                            self.past_key_values if use_cache else None, use_cache)
-        if use_cache:
-            self.set_cache(presents)
+        cache = self._prepare_cache(input_ids) if use_cache else None
+        hidden = self.transformer(input_ids, attention_mask, cache)
+        if cache is not None:
+            self.past_length = cache.length
         logits = self.lm_head(hidden, self.transformer.word_embeddings.weight)
         if labels is not None:
             shift = self.loss(logits[:, :-1].contiguous(), labels[:, 1:].contiguous())
@@ -176,10 +253,15 @@ class BloomForCausalLM(nn.Module, Generator):
             logits = mappings.gather_from_tp(logits)
         return {"logits": logits}
 
-    def set_cache(self, past_key_values):
-        self.past_key_values = [None] * self.transformer.hidden_layers if past_key_values is None else list(past_key_values)
+    # ---- KV cache (KVCacheOwner) ----------------------------------------------------------------
+    def _cache_attention_modules(self):
+        return [block.self_attention for block in self.transformer.h]
 
     def prepare_inputs_for_generation(self, input_ids, past=None, attention_mask=None, use_cache=None, **kwargs):
+        """With a warm cache only the newest token is fed; the padding mask always covers cache + new tokens."""
         if past is not None and use_cache:
             input_ids = input_ids[:, -1:]
-        return {"input_ids": input_ids, "attention_mask": attention_mask, "use_cache": bool(use_cache)}
+        out = {"input_ids": input_ids, "use_cache": bool(use_cache)}
+        if attention_mask is not None and not bool(attention_mask.all()):
+            out["attention_mask"] = attention_mask
+        return out
