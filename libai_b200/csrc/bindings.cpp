@@ -853,9 +853,12 @@ Tensor kv_append(const Tensor& qkv, const Tensor& k_cache, const Tensor& v_cache
 // q [B, Sq, A, D] (any strides with D contiguous, e.g. a view of the packed projection) against the caches [B, G, C, D]
 // (query head h reads cache head h / (A / G)); query i of sample b sees keys kv_start[b] .. cache_seqlens[b] + i.
 // Returns o [B, Sq, A, D] contiguous.  splits = 0: automatic.  alibi_slopes (fp32 [A]): ALiBi, each visible score gets
-// slope_h * (j - cache_seqlens[b] - i).
+// slope_h * (j - cache_seqlens[b] - i).  rel_bias (fp32 [A, R]): T5's relative-position bias, each visible score gets
+// rel_bias[h, min(cache_seqlens[b] + i - j, R - 1)].  causal = false: every query sees kv_start[b] <= j < cache_seqlens[b]
+// (cross-attention; the new tokens are not in this cache), without a bias.
 Tensor decode_attn(const Tensor& q, const Tensor& k_cache, const Tensor& v_cache, const Tensor& cache_seqlens,
-                   const Tensor& kv_start, double scale, int64_t splits, const c10::optional<Tensor>& alibi_slopes) {
+                   const Tensor& kv_start, double scale, int64_t splits, const c10::optional<Tensor>& alibi_slopes,
+                   const c10::optional<Tensor>& rel_bias, bool causal) {
   c10::cuda::CUDAGuard guard(q.device());
   check_cache(k_cache, v_cache, "decode_attn");
   const int B = (int)k_cache.size(0), G = (int)k_cache.size(1), C = (int)k_cache.size(2), D = (int)k_cache.size(3);
@@ -878,6 +881,21 @@ Tensor decode_attn(const Tensor& q, const Tensor& k_cache, const Tensor& v_cache
                 " on ", s.device());
     slopes = s.data_ptr<float>();
   }
+  const float* rel = nullptr;
+  int R = 0;
+  if (given(rel_bias)) {
+    const Tensor& r = *rel_bias;
+    TORCH_CHECK(r.scalar_type() == at::kFloat && r.dim() == 2 && r.size(0) == A && r.size(1) >= 1 &&
+                    r.device() == q.device() && r.is_contiguous(),
+                "decode_attn: rel_bias: contiguous fp32 [A, R] with R >= 1 on q's device, got ", r.scalar_type(), " ",
+                r.sizes(), " on ", r.device());
+    TORCH_CHECK(r.size(1) <= INT32_MAX, "decode_attn: rel_bias: R fits in int32");
+    TORCH_CHECK(slopes == nullptr, "decode_attn: alibi_slopes or rel_bias, not both");
+    rel = r.data_ptr<float>();
+    R = (int)r.size(1);
+  }
+  TORCH_CHECK(causal || (slopes == nullptr && rel == nullptr),
+              "decode_attn: causal=False takes no score bias (neither alibi_slopes nor rel_bias)");
   const int row_blocks = ((A / G) * Sq + 15) / 16;   // (query head, token) rows of one cache head, 16 per CTA
   const int nsplit = splits > 0 ? (int)std::min<int64_t>(splits, 32) : lb_decode_splits(B, G * row_blocks, C, D);
   Tensor o = at::empty({B, Sq, A, D}, q.options());
@@ -889,8 +907,8 @@ Tensor decode_attn(const Tensor& q, const Tensor& k_cache, const Tensor& v_cache
   long qs[3] = {q.stride(0), q.stride(1), q.stride(2)};
   check(lb_decode_attn(q.data_ptr(), qs, k_cache.data_ptr(), v_cache.data_ptr(), o.data_ptr(),
                        nsplit > 1 ? part_o.data_ptr<float>() : nullptr, nsplit > 1 ? part_ml.data_ptr<float>() : nullptr,
-                       cache_seqlens.data_ptr<int>(), kv_start.data_ptr<int>(), slopes, B, Sq, A, G, C, D, (float)scale,
-                       nsplit, cur_stream()),
+                       cache_seqlens.data_ptr<int>(), kv_start.data_ptr<int>(), slopes, rel, R, causal, B, Sq, A, G, C, D,
+                       (float)scale, nsplit, cur_stream()),
         "decode_attn");
   return o;
 }
@@ -1196,6 +1214,6 @@ TORCH_LIBRARY(libai_b200, m) {
   m.def("kv_append(Tensor qkv, Tensor(a!) k_cache, Tensor(b!) v_cache, Tensor cache_seqlens, Tensor? cos, Tensor? sin, bool write_q) -> Tensor", &kv_append);
   m.def("window_attn_fwd(Tensor qkv, int H, int W, int window, int shift, int heads, float scale, Tensor table, Tensor? tau) -> (Tensor, Tensor)", &window_attn_fwd);
   m.def("window_attn_bwd(Tensor dout, Tensor qkv, Tensor lse, int H, int W, int window, int shift, int heads, float scale, Tensor table, Tensor? tau) -> (Tensor, Tensor, Tensor)", &window_attn_bwd);
-  m.def("decode_attn(Tensor q, Tensor k_cache, Tensor v_cache, Tensor cache_seqlens, Tensor kv_start, float scale, int splits=0, Tensor? alibi_slopes=None) -> Tensor", &decode_attn);
+  m.def("decode_attn(Tensor q, Tensor k_cache, Tensor v_cache, Tensor cache_seqlens, Tensor kv_start, float scale, int splits=0, Tensor? alibi_slopes=None, Tensor? rel_bias=None, bool causal=True) -> Tensor", &decode_attn);
   m.def("bias_dropout_residual(Tensor x, Tensor? bias, Tensor? res, float p, int salt, Tensor? rng_state=None) -> (Tensor, Tensor)", &bias_dropout_residual);
 }

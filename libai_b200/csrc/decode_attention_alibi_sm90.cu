@@ -6,7 +6,8 @@ namespace lb {
 namespace dec {
 
 cudaError_t launch_decode_attn_alibi(const Params& p, int D, int B, int nsplit, cudaStream_t s) {
-  return D == 64 ? launch_decode_attn<64, true>(p, B, nsplit, s) : launch_decode_attn<128, true>(p, B, nsplit, s);
+  return D == 64 ? launch_decode_attn<64, Score::kAlibi>(p, B, nsplit, s)
+                 : launch_decode_attn<128, Score::kAlibi>(p, B, nsplit, s);
 }
 
 }  // namespace dec

@@ -1,5 +1,6 @@
-// The split-KV decode attention kernel (documented in decode_attention_sm90.cu) and its launch.  Two translation units
-// instantiate it: decode_attention_sm90.cu without a score bias, decode_attention_alibi_sm90.cu with ALiBi slopes.
+// The split-KV decode attention kernel (documented in decode_attention_sm90.cu) and its launch.  Three translation units
+// instantiate it: decode_attention_sm90.cu without a score bias, decode_attention_alibi_sm90.cu with ALiBi slopes and
+// decode_attention_t5_sm90.cu with T5's relative-position bias or a non-causal key window.
 #pragma once
 #include "common.cuh"
 
@@ -36,8 +37,13 @@ struct Params {
   int rows;                    // r * Sq
   int row_blocks;              // ceil(rows / 16)
   float scale_log2;
-  const float* alibi_slopes;   // [A] (ALIBI instances only)
+  int R;                       // Score::kRelBias: columns of the bias (in former padding: the layout is unchanged)
+  const float* bias;           // Score::kAlibi: the slopes [A]; Score::kRelBias: the relative bias [A, R]
 };
+
+// What a visible score gets besides q·k·scale, and which keys are visible.  kNone, kAlibi, kRelBias: query i of sample b
+// sees kv_start[b] <= j <= cache_seqlens[b] + i (causal); kWindow: every query sees kv_start[b] <= j < cache_seqlens[b].
+enum class Score { kNone, kAlibi, kRelBias, kWindow };
 
 LB_DEVICE void bulk_load(void* dst, const void* src, uint32_t bytes, uint64_t* bar) {
   asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];\n" ::"r"(
@@ -45,8 +51,9 @@ LB_DEVICE void bulk_load(void* dst, const void* src, uint32_t bytes, uint64_t* b
                "l"(src), "r"(bytes), "r"(smem_u32(bar))
                : "memory");
 }
-template <int D, bool ALIBI>
-__global__ void __launch_bounds__(kThreads) decode_attn_kernel(const Params p) {
+template <int D, Score S>
+__device__ __forceinline__ void decode_attn_body(const Params& p) {
+  constexpr bool ALIBI = S == Score::kAlibi;
   using C = Cfg<D>;
   extern __shared__ __align__(128) unsigned char smem[];
   __nv_bfloat16* ring = reinterpret_cast<__nv_bfloat16*>(smem);
@@ -61,7 +68,8 @@ __global__ void __launch_bounds__(kThreads) decode_attn_kernel(const Params p) {
   const long head_off = ((long)b * p.G + kvh) * p.C * D;
   const int len = p.seqlens[b];
   const int lo = max(p.kv_start[b], 0);
-  const int hi = min(len + p.Sq, p.C);   // exclusive; the cache object keeps len + Sq <= C, this only guards memory
+  // exclusive; the cache object keeps len + Sq <= C, this only guards memory
+  const int hi = S == Score::kWindow ? min(len, p.C) : min(len + p.Sq, p.C);
   const int ntiles = hi > lo ? (hi - lo + kTile - 1) / kTile : 0;
   const int per = (ntiles + nsplit - 1) / nsplit;
   const int t0 = split * per;
@@ -104,20 +112,26 @@ __global__ void __launch_bounds__(kThreads) decode_attn_kernel(const Params p) {
     }
   } else if (my > 0) {
     // Q fragments (A operand, rows = (query head, new token) pairs; rows past the last pair are zero), loaded once.
-    // lim: the last visible key of each of this thread's two rows (causal among the new tokens)
+    // lim: the last visible key of each of this thread's two rows (causal among the new tokens; the whole window
+    // for kWindow)
     uint32_t qf[D / 16][4];
     int lim[2];
     float slope2[2] = {0.f, 0.f};   // ALiBi slope of each row's query head, times log2(e)
+    const float* rb[2] = {nullptr, nullptr};   // kRelBias: the bias row of each row's query head
     {
       const int hr = kvh * (p.rows / p.Sq);   // first query head of the group
       const bool v0 = r0 < nrows, v1 = r0 + 8 < nrows;
       const int t0 = (row0 + r0) % p.Sq, t1 = (row0 + r0 + 8) % p.Sq;
-      lim[0] = len + t0;
-      lim[1] = len + t1;
+      lim[0] = S == Score::kWindow ? hi - 1 : len + t0;
+      lim[1] = S == Score::kWindow ? hi - 1 : len + t1;
+      if constexpr (S == Score::kRelBias) {   // rows past the last pair read head 0's row (their scores are unused)
+        rb[0] = p.bias + (v0 ? (long)(hr + (row0 + r0) / p.Sq) * p.R : 0);
+        rb[1] = p.bias + (v1 ? (long)(hr + (row0 + r0 + 8) / p.Sq) * p.R : 0);
+      }
       if constexpr (ALIBI) {
         constexpr float kLog2e = 1.4426950408889634f;
-        slope2[0] = v0 ? p.alibi_slopes[hr + (row0 + r0) / p.Sq] * kLog2e : 0.f;
-        slope2[1] = v1 ? p.alibi_slopes[hr + (row0 + r0 + 8) / p.Sq] * kLog2e : 0.f;
+        slope2[0] = v0 ? p.bias[hr + (row0 + r0) / p.Sq] * kLog2e : 0.f;
+        slope2[1] = v1 ? p.bias[hr + (row0 + r0 + 8) / p.Sq] * kLog2e : 0.f;
       }
       const __nv_bfloat16* qb = p.q + (long)b * p.q_sb + c0;
       const uint32_t* q0 = reinterpret_cast<const uint32_t*>(
@@ -158,11 +172,18 @@ __global__ void __launch_bounds__(kThreads) decode_attn_kernel(const Params p) {
         for (int j = 0; j < 4; ++j) {
           const int key = key0 + n * 8 + (j & 1);
           const bool vis = key < hi && key <= lim[j >> 1];
-          if constexpr (ALIBI)   // key − lim is a non-positive integer of at most the capacity: exact in fp32
+          if constexpr (ALIBI) {   // key − lim is a non-positive integer of at most the capacity: exact in fp32
             s[n][j] = vis ? fmaf(slope2[j >> 1], static_cast<float>(key - lim[j >> 1]), s[n][j] * p.scale_log2)
                           : -INFINITY;
-          else
+          } else if constexpr (S == Score::kRelBias) {
+            // bias of the distance lim − key = cache_seqlens[b] + i − j, constant from R − 1 on; a few hundred bytes
+            // per head, read through L1 (the clamp below 0 only keeps the address of an invisible key in the row)
+            constexpr float kLog2e = 1.4426950408889634f;
+            const float bias = __ldg(rb[j >> 1] + min(max(lim[j >> 1] - key, 0), p.R - 1));
+            s[n][j] = vis ? fmaf(bias, kLog2e, s[n][j] * p.scale_log2) : -INFINITY;
+          } else {
             s[n][j] = vis ? s[n][j] * p.scale_log2 : -INFINITY;
+          }
           mx[j >> 1] = fmaxf(mx[j >> 1], s[n][j]);
         }
       float alpha[2], base[2];
@@ -256,12 +277,31 @@ __global__ void __launch_bounds__(kThreads) decode_attn_kernel(const Params p) {
   }
 }
 
-// opts the kernel into its dynamic shared memory once; returns how many of its CTAs one SM holds (0 on error)
 template <int D, bool ALIBI>
+__global__ void __launch_bounds__(kThreads) decode_attn_kernel(const Params p) {
+  decode_attn_body<D, ALIBI ? Score::kAlibi : Score::kNone>(p);
+}
+
+// S = kRelBias or kWindow (decode_attention_t5_sm90.cu)
+template <int D, Score S>
+__global__ void __launch_bounds__(kThreads) decode_attn_t5_kernel(const Params p) {
+  decode_attn_body<D, S>(p);
+}
+
+template <int D, Score S>
+constexpr auto decode_kernel() {
+  if constexpr (S == Score::kNone || S == Score::kAlibi)
+    return decode_attn_kernel<D, S == Score::kAlibi>;
+  else
+    return decode_attn_t5_kernel<D, S>;
+}
+
+// opts the kernel into its dynamic shared memory once; returns how many of its CTAs one SM holds (0 on error)
+template <int D, Score S>
 int configure_decode() {
   static int resident = 0;
   if (resident == 0) {
-    auto kern = decode_attn_kernel<D, ALIBI>;
+    auto kern = decode_kernel<D, S>();
     if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg<D>::kSmem) != cudaSuccess ||
         cudaOccupancyMaxActiveBlocksPerMultiprocessor(&resident, kern, kThreads, Cfg<D>::kSmem) != cudaSuccess)
       resident = 0;
@@ -270,15 +310,17 @@ int configure_decode() {
 }
 
 // the attention kernel over the (split) key ranges; the partials of nsplit > 1 are reduced by decode_combine_kernel
-template <int D, bool ALIBI>
+template <int D, Score S>
 cudaError_t launch_decode_attn(const Params& p, int B, int nsplit, cudaStream_t s) {
-  if (configure_decode<D, ALIBI>() == 0) return cudaErrorInvalidConfiguration;   // the shared memory opt-in failed
-  decode_attn_kernel<D, ALIBI><<<dim3(nsplit, p.G * p.row_blocks, B), kThreads, Cfg<D>::kSmem, s>>>(p);
+  if (configure_decode<D, S>() == 0) return cudaErrorInvalidConfiguration;   // the shared memory opt-in failed
+  decode_kernel<D, S>()<<<dim3(nsplit, p.G * p.row_blocks, B), kThreads, Cfg<D>::kSmem, s>>>(p);
   return cudaGetLastError();
 }
 
 // the ALIBI instances (decode_attention_alibi_sm90.cu); D is 64 or 128
 cudaError_t launch_decode_attn_alibi(const Params& p, int D, int B, int nsplit, cudaStream_t s);
+// the T5 instances (decode_attention_t5_sm90.cu): S is kRelBias or kWindow, D is 64 or 128
+cudaError_t launch_decode_attn_t5(const Params& p, Score S, int D, int B, int nsplit, cudaStream_t s);
 
 }  // namespace dec
 }  // namespace lb

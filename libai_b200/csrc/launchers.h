@@ -128,8 +128,9 @@ int lb_bias_dropout_residual(const void* x, const void* bias, const void* res, v
 int lb_spin_timeout_report(char* buf, int n);
 int lb_decode_splits(int B, int blocks, int C, int D);
 int lb_decode_attn(const void* q, const long* q_strides, const void* k, const void* v, void* o, float* part_o,
-                   float* part_ml, const int* seqlens, const int* kv_start, const float* alibi_slopes, int B, int Sq,
-                   int A, int G, int C, int D, float scale, int nsplit, cudaStream_t s);
+                   float* part_ml, const int* seqlens, const int* kv_start, const float* alibi_slopes,
+                   const float* rel_bias, int R, bool causal, int B, int Sq, int A, int G, int C, int D, float scale,
+                   int nsplit, cudaStream_t s);
 int lb_kv_append(const void* qkv, const float* cosv, const float* sinv, void* q_out, void* k_cache, void* v_cache,
                  const int* seqlens, int B, int Sq, int G, int r, int C, int D, cudaStream_t s);
 int lb_window_attn_groups(int B, int H, int W, int ws, int heads);

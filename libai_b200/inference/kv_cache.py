@@ -10,7 +10,7 @@ left padding included), which sizes the windows and decides when the buffers mus
 """
 from __future__ import annotations
 
-from typing import Iterable, List, Optional
+from typing import Iterable, List, Optional, Tuple
 
 import torch
 
@@ -26,6 +26,21 @@ def left_padding(attention_mask: torch.Tensor) -> Optional[torch.Tensor]:
     if not bool((m[:, -1] == 1).all()):
         return None
     return (m.shape[1] - m.to(torch.int32).sum(dim=1)).to(torch.int32)
+
+
+def padding_window(attention_mask: torch.Tensor) -> Optional[Tuple[torch.Tensor, torch.Tensor]]:
+    """``(kv_start, kv_end)`` (int32 ``[b]``) of a 2-D padding mask whose rows are each one run of ones — "ones, then
+    zeros" (right padding), "zeros, then ones" (left padding) or all ones: the keys ``kv_start[b] <= j < kv_end[b]``.
+    None for any other mask (a row with a hole, or without a one).  One small host sync."""
+    m = attention_mask.to(torch.int32)
+    n = m.shape[1]
+    j = torch.arange(n, dtype=torch.int32, device=m.device)[None, :]
+    ones = m.sum(dim=1, dtype=torch.int32)
+    start = torch.where(m > 0, j, n).amin(dim=1)
+    end = torch.where(m > 0, j + 1, 0).amax(dim=1)
+    if not bool(((m == 0) | (m == 1)).all() & (ones > 0).all() & (end - start == ones).all()):
+        return None
+    return start.to(torch.int32), end.to(torch.int32)
 
 
 class KVCacheLayer:

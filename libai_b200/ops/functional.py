@@ -872,7 +872,7 @@ def kv_cache_append_ref(qkv, k_cache, v_cache, cache_seqlens, cos=None, sin=None
 
 
 def decode_attention(q, k_cache, v_cache, cache_seqlens, kv_start, *, scale: float, splits: int = 0,
-                     past: Optional[int] = None, alibi_slopes=None):
+                     past: Optional[int] = None, alibi_slopes=None, rel_bias=None, causal: bool = True):
     """Attention of ``q [b, s, a, d]`` (new tokens, already appended to the caches; any strides with d contiguous) over
     the caches ``[b, g, C, d]`` (query head ``h`` reads cache head ``h // (a // g)``): query ``i`` of sample ``b`` sees exactly the keys ``kv_start[b] <= j <= cache_seqlens[b] + i``.  Returns
     ``[b, s, a, d]`` contiguous; a query without a visible key gets zeros.  The native kernel takes up to 16 new tokens
@@ -881,35 +881,58 @@ def decode_attention(q, k_cache, v_cache, cache_seqlens, kv_start, *, scale: flo
     (``cache_seqlens`` all equal to it, as in a :class:`~libai_b200.inference.kv_cache.StaticKVCache`); with it, more
     than 16 new tokens run the causal flash kernel over the cache window ``[:past + s]`` (chunked prefill).
     ``alibi_slopes`` (fp32 ``[a]``, on q's device): ALiBi, every visible score gets ``slope_h·(j − cache_seqlens[b] − i)``
-    — the flash kernel's ``slope·(j − i − (sk − sq))`` over the cache window, so both paths score alike."""
+    — the flash kernel's ``slope·(j − i − (sk − sq))`` over the cache window, so both paths score alike.
+    ``rel_bias`` (fp32 ``[a, R]``, contiguous, on q's device): T5's relative-position bias, every visible score gets
+    ``rel_bias[h, min(cache_seqlens[b] + i − j, R − 1)]``; longer ``past=`` continuations run the flash kernel with the
+    dense bias it expands to.
+    ``causal=False`` (cross-attention, no bias): every query sees ``kv_start[b] <= j < cache_seqlens[b]`` — a cache the
+    new tokens are not in; more than 16 tokens run the rectangular flash kernel over that window (whose end, like
+    :func:`attention`'s ``kv_lens``, is at least 1)."""
     if _decode_native(q, k_cache):
         if q.shape[1] <= 16:
             ext = load_ext()
-            o = ext.decode_attn(q, k_cache, v_cache, cache_seqlens, kv_start, float(scale), int(splits), alibi_slopes)
+            extra = () if rel_bias is None and causal else (rel_bias, bool(causal))
+            o = ext.decode_attn(q, k_cache, v_cache, cache_seqlens, kv_start, float(scale), int(splits), alibi_slopes,
+                                *extra)
             count_launch(2)
             return o
+        if not causal:
+            o = attention(q.permute(0, 2, 1, 3), k_cache, v_cache, causal=False, scale=scale, kv_start=kv_start,
+                          kv_lens=cache_seqlens)
+            return o.transpose(1, 2)
         if past is not None:
             L = past + q.shape[1]
+            bias = None
+            if rel_bias is not None:   # [1, a, s, L]: query past + i, key j
+                dist = torch.arange(past, L, device=q.device)[:, None] - torch.arange(L, device=q.device)[None, :]
+                bias = rel_bias[:, dist.clamp(0, rel_bias.shape[1] - 1)].to(torch.bfloat16)[None]
             o = attention(q.permute(0, 2, 1, 3), k_cache[:, :, :L], v_cache[:, :, :L], causal=True, scale=scale,
-                          kv_start=kv_start, alibi_slopes=alibi_slopes)
+                          kv_start=kv_start, alibi_slopes=alibi_slopes, bias=bias)
             return o.transpose(1, 2)   # the kernel's [b, s, a, d] output
-    return decode_attention_ref(q, k_cache, v_cache, cache_seqlens, kv_start, scale=scale, alibi_slopes=alibi_slopes)
+    return decode_attention_ref(q, k_cache, v_cache, cache_seqlens, kv_start, scale=scale, alibi_slopes=alibi_slopes,
+                                rel_bias=rel_bias, causal=causal)
 
 
-def decode_attention_ref(q, k_cache, v_cache, cache_seqlens, kv_start, *, scale: float, alibi_slopes=None):
+def decode_attention_ref(q, k_cache, v_cache, cache_seqlens, kv_start, *, scale: float, alibi_slopes=None,
+                         rel_bias=None, causal: bool = True):
     """:func:`attention_ref` over the window ``[:L]`` of the caches (``L = max(cache_seqlens) + s``) with the mask built
     from ``kv_start`` and causality among the new tokens, and the ALiBi bias ``slope_h·(j − (cache_seqlens[b] + i))``
-    when ``alibi_slopes`` is given."""
+    when ``alibi_slopes`` is given, or T5's ``rel_bias[h, min(cache_seqlens[b] + i − j, R − 1)]`` when ``rel_bias`` is.
+    ``causal=False``: every query sees ``kv_start[b] <= j < cache_seqlens[b]`` (``L = max(cache_seqlens)``)."""
     s_len = q.shape[1]
     lens = cache_seqlens.long()
-    L = int(lens.max()) + s_len
+    L = int(lens.max()) + (s_len if causal else 0)
     j = torch.arange(L, device=q.device)[None, None, :]
     i = torch.arange(s_len, device=q.device)[None, :, None]
-    visible = (j >= kv_start.long()[:, None, None]) & (j <= lens[:, None, None] + i)          # [b, s, L]
+    end = lens[:, None, None] + i if causal else lens[:, None, None] - 1
+    visible = (j >= kv_start.long()[:, None, None]) & (j <= end)                              # [b, s, L]
     bias = None
     if alibi_slopes is not None:
         rel = (j - (lens[:, None, None] + i)).float()                                          # [b, s, L]
         bias = alibi_slopes.float()[None, :, None, None] * rel[:, None]                        # [b, a, s, L]
+    if rel_bias is not None:
+        dist = (lens[:, None, None] + i - j).clamp(0, rel_bias.shape[1] - 1)                   # [b, s, L]
+        bias = rel_bias[:, dist].permute(1, 0, 2, 3)                                           # [b, a, s, L]
     o = attention_ref(q.permute(0, 2, 1, 3), k_cache[:, :, :L], v_cache[:, :, :L], causal=False, scale=scale,
                       mask=visible[:, None], bias=bias)
     o = o.masked_fill(~visible.any(-1)[:, None, :, None], 0)

@@ -6,16 +6,24 @@ bucketed relative position bias owned by the first layer of each stack and share
 (attention_layer.py:268-345), ReLU MLP for ``model_type="t5"`` / gated-GELU (``wi_0``, ``wi_1``) for ``"mt5"``
 (mlp_layer.py), shared or separate LM head (``tie_word_embeddings`` rescales by ``hidden_size**-0.5``).
 Parameter names follow the reference project so its loader mapping applies.
+
+Cached generation (one pipeline stage) decodes from two preallocated :class:`StaticKVCache` objects: the decoder
+self-attention's, appended to at every step, and the cross-attention's, which holds every decoder layer's projection of
+the encoder states from the first step on.  The decoder's relative-position bias only depends on the distance
+``p − j >= 0`` between query and key and is constant from ``MAX_DISTANCE`` on, so the decode kernel takes it as one
+``[heads, MAX_DISTANCE + 1]`` vector per forward.
 """
 from __future__ import annotations
 
 import math
+from typing import Optional
 
 import torch
 from torch import nn
 
 from libai_b200.config import configurable
 from libai_b200.inference.generator.generation_utils import Generator
+from libai_b200.inference.kv_cache import KVCacheLayer, KVCacheOwner, StaticKVCache, padding_window
 from libai_b200.layers import Linear, LMLogits, ParallelCrossEntropyLoss, RMSLayerNorm, VocabEmbedding
 from libai_b200.layers._param import create_parameter
 from libai_b200.models.utils.weight_init import init_method_normal, scaled_init_method_normal
@@ -34,7 +42,10 @@ class MT5Embedding(nn.Module):
         return self.embedding_dropout(self.word_embeddings(input_ids))
 
 
-def relative_position_bucket(relative_position, bidirectional=True, num_buckets=32, max_distance=128):
+MAX_DISTANCE = 128   # T5's bucketing saturates at this distance
+
+
+def relative_position_bucket(relative_position, bidirectional=True, num_buckets=32, max_distance=MAX_DISTANCE):
     """T5 bucketing: half of the buckets are exact offsets, the other half log-spaced up to ``max_distance``."""
     buckets = torch.zeros_like(relative_position)
     if bidirectional:
@@ -85,7 +96,18 @@ class T5Attention(nn.Module):
         bucket = relative_position_bucket(mem - ctx, bidirectional=not self.is_decoder, num_buckets=self.num_buckets)
         return self.relative_attention_bias[bucket].permute(2, 0, 1).unsqueeze(0)  # [1, a, q, k]
 
-    def forward(self, hidden, mask=None, encoder_states=None, past_key_value=None, position_bias=None, use_cache=False):
+    def relative_bias_vector(self):
+        """fp32 ``[a, MAX_DISTANCE + 1]``: the decoder's bias at distance ``p − j = 0 .. MAX_DISTANCE`` (this rank's
+        heads); unidirectional buckets saturate at ``num_buckets − 1`` from ``MAX_DISTANCE`` on, so the last column holds
+        for every longer distance (the decode kernel clamps the distance to it)."""
+        dist = torch.arange(MAX_DISTANCE + 1, device=self.relative_attention_bias.device)
+        bucket = relative_position_bucket(-dist, bidirectional=False, num_buckets=self.num_buckets)
+        return self.relative_attention_bias[bucket].t().float().contiguous()
+
+    def forward(self, hidden, mask=None, encoder_states=None, past_key_value=None, position_bias=None, use_cache=False,
+                cache: Optional[KVCacheLayer] = None):
+        if cache is not None:
+            return self._cached_forward(hidden, mask, cache, position_bias)
         b = hidden.shape[0]
         a, d = self.local_heads, self.head_size
         if self.is_cross_attention:
@@ -118,6 +140,43 @@ class T5Attention(nn.Module):
                            training=self.training)
         out = self.dropout(self.dense(ctx.transpose(1, 2).reshape(b, -1, a * d)))
         return out, position_bias, present
+
+    def _cached_forward(self, hidden, mask, cache: KVCacheLayer, position_bias):
+        """Attention of the new tokens over the layer's cache.  Self-attention appends k, v first and, without a
+        ``mask``, runs :func:`OF.decode_attention` with the relative-bias vector (built by the first layer, then handed
+        down as ``position_bias``).  Cross-attention reads the cache of the encoder projection: without a ``mask``
+        through the non-causal decode window ``cache.kv_start <= j < cache.seqlens``.  A ``mask`` (decoder padding, an
+        encoder mask with holes) keeps the dense bias with the mask folded in, as without the cache."""
+        b, s = hidden.shape[:2]
+        a, d = self.local_heads, self.head_size
+        if self.is_cross_attention:
+            q = self.query(hidden).view(b, s, a, d)
+            if mask is None:
+                ctx = OF.decode_attention(q, cache.k, cache.v, cache.seqlens, cache.kv_start, scale=1.0, causal=False)
+            else:
+                L = mask.shape[-1]
+                if position_bias is None:
+                    position_bias = torch.zeros(1, a, s, L, device=hidden.device, dtype=hidden.dtype)
+                    position_bias = position_bias + (1.0 - mask.to(position_bias.dtype)) * -10000.0
+                ctx = OF.attention(q.transpose(1, 2), cache.k[:, :, :L], cache.v[:, :, :L], causal=False, scale=1.0,
+                                   bias=position_bias).transpose(1, 2)
+        else:
+            past = cache.length
+            q = OF.kv_cache_append(self.query_key_value(hidden).view(b, s, a, 3 * d), cache.k, cache.v, cache.seqlens)
+            if mask is None:
+                if position_bias is None:
+                    position_bias = self.relative_bias_vector()
+                ctx = OF.decode_attention(q, cache.k, cache.v, cache.seqlens, cache.kv_start, scale=1.0, past=past,
+                                          rel_bias=position_bias)
+            else:
+                L = past + s
+                if position_bias is None:
+                    position_bias = self.compute_bias(s, L, hidden.device)
+                    position_bias = position_bias + (1.0 - mask.to(position_bias.dtype)) * -10000.0
+                ctx = OF.attention(q.transpose(1, 2), cache.k[:, :, :L], cache.v[:, :, :L], causal=False, scale=1.0,
+                                   bias=position_bias).transpose(1, 2)
+        out = self.dropout(self.dense(ctx.reshape(b, s, a * d)))
+        return out, position_bias, None
 
 
 class T5MLP(nn.Module):
@@ -168,17 +227,21 @@ class TransformerLayer(nn.Module):
         self.mlp = mlp_cls(hidden_size, ffn_hidden_size, output_dropout_prob, init_method, output_layer_init_method, layer_idx)
 
     def forward(self, hidden, attention_mask=None, encoder_states=None, encoder_attention_mask=None, past_key_value=None,
-                position_bias=None, encoder_decoder_position_bias=None, use_cache=False):
+                position_bias=None, encoder_decoder_position_bias=None, use_cache=False,
+                cache: Optional[KVCacheLayer] = None, cross_cache: Optional[KVCacheLayer] = None):
+        """``cache`` / ``cross_cache``: the layer's self- and cross-attention caches of cached generation (then
+        ``past_key_value`` and ``use_cache`` are unused and no ``present`` is returned)."""
         self_past = past_key_value[:2] if past_key_value is not None else None
         cross_past = past_key_value[2:] if past_key_value is not None and len(past_key_value) == 4 else None
         out, position_bias, present = self.self_attention(self.input_layernorm(hidden), attention_mask,
                                                           past_key_value=self_past, position_bias=position_bias,
-                                                          use_cache=use_cache)
+                                                          use_cache=use_cache, cache=cache)
         hidden = hidden + out
         if self.is_decoder:
             out, encoder_decoder_position_bias, cross_present = self.cross_attention(
                 self.post_attention_layernorm(hidden), encoder_attention_mask, encoder_states=encoder_states,
-                past_key_value=cross_past, position_bias=encoder_decoder_position_bias, use_cache=use_cache)
+                past_key_value=cross_past, position_bias=encoder_decoder_position_bias, use_cache=use_cache,
+                cache=cross_cache)
             hidden = hidden + out
             hidden = hidden + self.mlp(self.post_cross_attention_layernorm(hidden))
             if use_cache:
@@ -200,7 +263,7 @@ def _extend(mask, causal_len=None):
     return mask
 
 
-class MT5Model(nn.Module, Generator):
+class MT5Model(nn.Module, Generator, KVCacheOwner):
     @configurable
     def __init__(self, vocab_size, hidden_size, hidden_layers, num_attention_heads, head_size, intermediate_size,
                  embedding_dropout_prob, hidden_dropout_prob, attention_probs_dropout_prob, relative_attention_num_buckets,
@@ -228,9 +291,11 @@ class MT5Model(nn.Module, Generator):
 
         self.encoder = stack(False, 0)
         self.decoder = stack(True, hidden_layers)
-        self.past_key_values = [None] * hidden_layers
+        self.past_key_values = [None] * hidden_layers   # the tuple cache of pipeline-parallel inference
         self.encoder_states = None
         self.past_length = 0
+        self.kv_cache: Optional[StaticKVCache] = None      # decoder self-attention (KVCacheOwner)
+        self.cross_cache: Optional[StaticKVCache] = None   # the encoder projection of every decoder layer
         self.tie_word_embeddings = bool(cfg.get("tie_word_embeddings", model_type != "mt5")) if cfg is not None else model_type != "mt5"
         if model_type == "mt5":
             self.lm_head = Linear(hidden_size, vocab_size, bias=False, parallel="col", init_method=init_method,
@@ -349,14 +414,16 @@ class MT5Model(nn.Module, Generator):
         if dutil.get_dist_util().pipeline_parallel_size > 1 and not torch.is_grad_enabled():
             return self._forward_pipelined(encoder_input_ids, decoder_input_ids, encoder_attn_mask, decoder_attn_mask,
                                            encoder_decoder_attn_mask, use_cache, only_encoder)
-        if use_cache and self.encoder_states is not None:
-            encoder_states = self.encoder_states
-        else:
-            self.set_cache(None, None)
-            encoder_states = self.encode(encoder_input_ids, encoder_attn_mask)
+        if use_cache and only_encoder and self.encoder_states is not None:
+            return self.encoder_states
+        if use_cache and not only_encoder:
+            return self._forward_cached(encoder_input_ids, decoder_input_ids, encoder_attn_mask, decoder_attn_mask,
+                                        encoder_decoder_attn_mask)
+        self.set_cache(None, None)
+        encoder_states = self.encode(encoder_input_ids, encoder_attn_mask)
         if only_encoder:
             return encoder_states
-        past_len = self.past_key_values[0][0].shape[2] if use_cache and self.past_key_values[0] is not None else 0
+        past_len = 0
         q_len = decoder_input_ids.shape[1]
         causal = torch.ones(past_len + q_len, past_len + q_len, dtype=torch.bool, device=decoder_input_ids.device).tril()
         dec_mask = causal[past_len:][None, None]
@@ -368,14 +435,13 @@ class MT5Model(nn.Module, Generator):
         if cross_mask is not None and cross_mask.shape[-2] > 1:
             cross_mask = cross_mask[..., -q_len:, :]
         hidden = self.embedding(decoder_input_ids)
-        presents, bias, cross_bias = [], None, None
-        for layer, past in zip(self.decoder.layers, self.past_key_values):
-            hidden, bias, cross_bias, present = layer(hidden, dec_mask, encoder_states, cross_mask, past_key_value=past,
-                                                      position_bias=bias, encoder_decoder_position_bias=cross_bias,
-                                                      use_cache=use_cache)
-            presents.append(present)
-        if use_cache:
-            self.set_cache(encoder_states, presents)
+        bias, cross_bias = None, None
+        for layer in self.decoder.layers:
+            hidden, bias, cross_bias = layer(hidden, dec_mask, encoder_states, cross_mask, position_bias=bias,
+                                             encoder_decoder_position_bias=cross_bias)[:3]
+        return {"logits": self._logits(hidden)}
+
+    def _logits(self, hidden):
         hidden = self.decoder.final_layernorm(hidden)
         if self.tie_word_embeddings:
             hidden = hidden * (self.hidden_size ** -0.5)
@@ -385,17 +451,105 @@ class MT5Model(nn.Module, Generator):
             logits = self.lm_head(hidden, self.embedding.word_embeddings.weight)
         if not self.training and dutil.get_dist_util().tensor_parallel_size > 1:
             logits = mappings.gather_from_tp(logits)
-        return {"logits": logits}
+        return logits
+
+    # ---- cached generation on the StaticKVCache (one pipeline stage) -------------------------------
+    def _forward_cached(self, encoder_input_ids, decoder_input_ids, encoder_attn_mask, decoder_attn_mask,
+                        encoder_decoder_attn_mask):
+        """The decoder over the preallocated caches.  The first step (an empty cache) runs the encoder and writes each
+        decoder layer's projection of its states into ``cross_cache``, once.  Without a decoder mask that has padding,
+        self-attention runs the decode kernels with the relative-bias vector; a 2-D encoder mask whose rows are one
+        run of ones (left or right padding) becomes the cross cache's key window, any other one stays a dense mask."""
+        cache = self._prepare_cache(decoder_input_ids)
+        past, q_len = cache.length, decoder_input_ids.shape[1]
+        cross_mask = encoder_decoder_attn_mask if encoder_decoder_attn_mask is not None else encoder_attn_mask
+        if past == 0:
+            # the mask's window first: its host sync then waits for no encoder work, and the decoder's launches keep
+            # overlapping the encoder on the device
+            window = padding_window(cross_mask) if cross_mask is not None and cross_mask.dim() == 2 else None
+            self.encoder_states = self.encode(encoder_input_ids, encoder_attn_mask)
+            self._fill_cross_cache(self.encoder_states, cross_mask is not None and window is None, window)
+        self_mask = None
+        extra = _extend(decoder_attn_mask)
+        if extra is not None and extra.shape[-1] == past + q_len and not bool(extra.all()):
+            causal = torch.ones(past + q_len, past + q_len, dtype=torch.bool, device=decoder_input_ids.device).tril()
+            self_mask = causal[past:][None, None] & (extra[..., -q_len:, :] if extra.shape[-2] > 1 else extra)
+        if self.cross_cache.dense_mask:
+            cross_mask = _extend(cross_mask)
+            if cross_mask.shape[-2] > 1:
+                cross_mask = cross_mask[..., -q_len:, :]
+        else:
+            cross_mask = None
+        hidden, bias, cross_bias = self.embedding(decoder_input_ids), None, None
+        for i, layer in enumerate(self.decoder.layers):
+            hidden, bias, cross_bias, _ = layer(hidden, self_mask, encoder_attention_mask=cross_mask,
+                                                position_bias=bias, encoder_decoder_position_bias=cross_bias,
+                                                cache=cache.layer(i), cross_cache=self.cross_cache.layer(i))
+        cache.advance(q_len)
+        self.past_length = cache.length
+        return {"logits": self._logits(hidden)}
+
+    def _fill_cross_cache(self, encoder_states, dense_mask: bool, window):
+        b, S = encoder_states.shape[:2]
+        attn = self.decoder.layers[0].cross_attention
+        a, d = attn.local_heads, attn.head_size
+        c = self.cross_cache
+        if c is None or not c.matches(b, encoder_states.dtype, encoder_states.device) or c.capacity < S:
+            c = StaticKVCache(len(self.decoder.layers), b, a, d, S, encoder_states.dtype, encoder_states.device)
+        c.reset()
+        c.dense_mask = dense_mask
+        if window is None:
+            c.seqlens.fill_(S)
+        else:
+            c.kv_start.copy_(window[0])
+            c.seqlens.copy_(window[1])
+        c.length = S
+        for i, layer in enumerate(self.decoder.layers):
+            kv = layer.cross_attention.key_value(encoder_states).view(b, S, a, 2 * d).transpose(1, 2)
+            c.k[i][:, :, :S] = kv[..., :d]
+            c.v[i][:, :, :S] = kv[..., d:]
+        self.cross_cache = c
 
     # ---- generation support ---------------------------------------------------------------------
+    def _cache_attention_modules(self):
+        return [layer.self_attention for layer in self.decoder.layers]
+
+    def allocate_kv_cache(self, batch: int, max_length: int):
+        """The decoder self-attention cache (one pipeline stage; pipeline-parallel inference keeps its tuple cache)."""
+        if dutil.get_dist_util().pipeline_parallel_size > 1:
+            return None
+        return super().allocate_kv_cache(batch, max_length)
+
+    @property
+    def past_key_values(self):
+        return self.kv_cache if self.kv_cache is not None else self._tuple_cache
+
+    @past_key_values.setter
+    def past_key_values(self, value):
+        self._tuple_cache = value
+
     def set_cache(self, encoder_states, past_key_values):
         self.encoder_states = encoder_states
+        if isinstance(past_key_values, StaticKVCache):
+            self.kv_cache, self.past_length = past_key_values, past_key_values.length
+            return
+        if past_key_values is None and self.kv_cache is not None:
+            self.kv_cache.reset()
         self.past_length = 0 if past_key_values is None else past_key_values[0][0].shape[2]
-        self.past_key_values = [None] * len(self.decoder.layers) if past_key_values is None else list(past_key_values)
+        self._tuple_cache = [None] * len(self.decoder.layers) if past_key_values is None else list(past_key_values)
 
     def _reorder_cache(self, past, beam_idx):
         if past is None:
             return None
+        if isinstance(past, StaticKVCache):
+            # Only the self-attention cache is gathered.  The cross cache and the encoder states stay as they are:
+            # _expand_inputs_for_generation gives every beam of a sample the same encoder inputs, and for a sample
+            # still decoding BeamSearchScorer.process picks beam_idx among that sample's own beams, so its rows keep
+            # their own encoder keys.  A finished sample's beam_idx entries are 0 (its out_indices are never set): its
+            # rows take sample 0's self cache, as in HF, while keeping their own cross rows.  Those rows only ever emit
+            # pad_token_id from then on, so which keys they attend to changes no output.
+            past.reorder_(beam_idx)
+            return past
         if self.encoder_states is not None:
             self.encoder_states = self.encoder_states.index_select(0, beam_idx.to(self.encoder_states.device))
         return [None if layer is None else tuple(t.index_select(0, beam_idx.to(t.device)) for t in layer) for layer in past]
