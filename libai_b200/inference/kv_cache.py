@@ -14,6 +14,7 @@ from typing import Iterable, List, Optional, Tuple
 
 import torch
 
+from libai_b200.ops import functional as OF
 from libai_b200.utils import distributed as dutil
 
 
@@ -28,19 +29,51 @@ def left_padding(attention_mask: torch.Tensor) -> Optional[torch.Tensor]:
     return (m.shape[1] - m.to(torch.int32).sum(dim=1)).to(torch.int32)
 
 
-def padding_window(attention_mask: torch.Tensor) -> Optional[Tuple[torch.Tensor, torch.Tensor]]:
-    """``(kv_start, kv_end)`` (int32 ``[b]``) of a 2-D padding mask whose rows are each one run of ones — "ones, then
-    zeros" (right padding), "zeros, then ones" (left padding) or all ones: the keys ``kv_start[b] <= j < kv_end[b]``.
-    None for any other mask (a row with a hole, or without a one).  One small host sync."""
+def _ones_runs(attention_mask: torch.Tensor):
+    """On the device, for a 2-D padding mask: whether it is 0/1, and per row the index of the first one, one past the
+    last one, and the number of ones (int32 ``[b]``; a row without a one has ``start = n``, ``end = 0``)."""
     m = attention_mask.to(torch.int32)
     n = m.shape[1]
     j = torch.arange(n, dtype=torch.int32, device=m.device)[None, :]
     ones = m.sum(dim=1, dtype=torch.int32)
     start = torch.where(m > 0, j, n).amin(dim=1)
     end = torch.where(m > 0, j + 1, 0).amax(dim=1)
-    if not bool(((m == 0) | (m == 1)).all() & (ones > 0).all() & (end - start == ones).all()):
+    return ((m == 0) | (m == 1)).all(), start, end, ones
+
+
+def padding_window(attention_mask: torch.Tensor) -> Optional[Tuple[torch.Tensor, torch.Tensor]]:
+    """``(kv_start, kv_end)`` (int32 ``[b]``) of a 2-D padding mask whose rows are each one run of ones — "ones, then
+    zeros" (right padding), "zeros, then ones" (left padding) or all ones: the keys ``kv_start[b] <= j < kv_end[b]``.
+    None for any other mask (a row with a hole, or without a one).  One small host sync."""
+    binary, start, end, ones = _ones_runs(attention_mask)
+    if not bool(binary & (ones > 0).all() & (end - start == ones).all()):
         return None
     return start.to(torch.int32), end.to(torch.int32)
+
+
+def _padding_sides(attention_mask: torch.Tensor) -> Tuple[bool, bool, torch.Tensor, torch.Tensor]:
+    """``(right, left, start, ones)`` of a 2-D 0/1 padding mask, with one small host sync: ``right`` when every row is
+    "ones, then zeros" (all zeros included), ``left`` when every row is "zeros, then ones" with at least one one (an
+    all-ones mask is both), and per row the index of the first one and the number of ones (int32 ``[b]``)."""
+    binary, start, end, ones = _ones_runs(attention_mask)
+    run = end - start == ones   # the row's ones are contiguous (never for a row without a one)
+    right = binary & ((run & (start == 0)) | (ones == 0)).all()
+    left = binary & (run & (end == attention_mask.shape[1])).all()
+    right, left = torch.stack((right, left)).tolist()
+    return right, left, start, ones
+
+
+def padding_bounds(attention_mask: torch.Tensor) -> Optional[Tuple[Optional[torch.Tensor], Optional[torch.Tensor]]]:
+    """How the flash kernels take a padded 2-D mask without a dense one: ``(kv_lens, None)`` when every row is right
+    padded ("ones, then zeros"; an all-zero row gets ``kv_lens = 0``, which the kernels clamp to 1), else
+    ``(None, kv_start)`` when every row is left padded ("zeros, then ones"), both int32 ``[b]``; None for any other mask
+    (a hole, padding on both sides, or left and right padded rows together).  One small host sync."""
+    right, left, start, ones = _padding_sides(attention_mask)
+    if right:
+        return ones, None
+    if left:
+        return None, start
+    return None
 
 
 class KVCacheLayer:
@@ -71,6 +104,44 @@ class KVCacheLayer:
     def length(self) -> int:
         return self.cache.length
 
+    def append(self, qkv: torch.Tensor, cos=None, sin=None) -> torch.Tensor:
+        """Write k, v of the packed projection ``qkv`` (per-head ``[b, s, a, 3d]`` or grouped ``[b, s, g, r + 2, d]``) at
+        rows ``seqlens[b] + i`` (:func:`OF.kv_cache_append`, rotated by ``cos/sin`` when given); returns q ``[b, s, a,
+        d]``.  A per-head projection without rotary hands q back as its strided view: nothing needs writing."""
+        if cos is None and qkv.dim() == 4:
+            OF.kv_cache_append(qkv, self.k, self.v, self.seqlens, return_q=False)
+            return qkv[..., : qkv.shape[-1] // 3]
+        return OF.kv_cache_append(qkv, self.k, self.v, self.seqlens, cos, sin)
+
+    def attend(self, q: torch.Tensor, *, scale: float, causal: bool = True, mask=None, bias=None, alibi_slopes=None,
+               rel_bias=None, dropout_p: float = 0.0, training: bool = False) -> torch.Tensor:
+        """Attention of the new tokens' ``q`` ``[b, s, a, d]`` over the cache → ``[b, s, a, d]``.  ``causal``: the new
+        tokens were appended this step (self-attention); ``causal=False``: the cache is a fixed window the queries all
+        see (cross-attention).  The rows held before this step (``length``) are the same for every layer: the model
+        advances the cache after its last layer.
+
+        - a dense 0/1 ``mask`` or additive ``bias`` (the model folded its padding into it): :func:`OF.attention` over
+          the window ``[:length + s]`` (causal) or ``[:length]``, non-causal;
+        - the causal prefill of an empty cache without ``rel_bias``: the flash kernel over ``[:s]``, the prompt's left
+          padding in ``kv_start``;
+        - anything else: :func:`OF.decode_attention` (the split-KV kernel up to 16 new tokens, the flash kernel over
+          the cache window beyond)."""
+        past = self.length
+        if mask is not None or bias is not None:
+            L = past + q.shape[1] if causal else past
+            ctx = OF.attention(q.transpose(1, 2), self.k[:, :, :L], self.v[:, :, :L], causal=False, scale=scale,
+                               mask=mask, bias=bias, dropout_p=dropout_p, training=training)
+            return ctx.transpose(1, 2)
+        if causal and past == 0 and rel_bias is None:
+            s_len = q.shape[1]
+            query, key = q.transpose(1, 2), self.k[:, :, :s_len]
+            kv_start = self.kv_start if OF.attention_supported(query, key) else None
+            ctx = OF.attention(query, key, self.v[:, :, :s_len], causal=True, scale=scale, alibi_slopes=alibi_slopes,
+                               kv_start=kv_start, dropout_p=dropout_p, training=training)
+            return ctx.transpose(1, 2)
+        return OF.decode_attention(q, self.k, self.v, self.seqlens, self.kv_start, scale=scale, past=past,
+                                   alibi_slopes=alibi_slopes, rel_bias=rel_bias, causal=causal)
+
 
 class StaticKVCache:
     def __init__(self, num_layers: int, batch: int, heads: int, head_dim: int, capacity: int,
@@ -98,6 +169,50 @@ class StaticKVCache:
 
     def matches(self, batch: int, dtype, device) -> bool:
         return self.batch == batch and self.dtype == dtype and self.device == torch.device(device)
+
+    def flash_attention(self) -> bool:
+        """True when :func:`OF.attention` over the buffers runs the flash kernels, which take a left-padded prompt's
+        padding from ``kv_start``; the reference math needs a dense mask for it."""
+        k = self.k[self.owned[0]]
+        return OF.attention_supported(k, k)
+
+    def step_needs_dense_mask(self, attention_mask: Optional[torch.Tensor], *, flash: bool,
+                              kv_start_ok: bool = True) -> bool:
+        """The padding policy of a decoder-only model's step, called once before its layers: True when the layers must
+        take ``attention_mask`` (``[b, length + s]``, 1 = token) as a dense mask.  The prefill of an empty cache
+        classifies the prompt's padding: a left-padded 2-D mask goes to ``kv_start`` (unless ``kv_start_ok`` is False,
+        e.g. when rows precede the prompt), any other padding sets ``dense_mask`` for every later step; the prefill
+        itself needs the dense mask for such padding, and for any padding when the attention is not ``flash``.  Later
+        steps need it when ``dense_mask`` is set, without a host sync."""
+        if self.length > 0:
+            return attention_mask is not None and self.dense_mask
+        if attention_mask is None:
+            return False
+        if attention_mask.dim() == 2:
+            right, left, start, _ = _padding_sides(attention_mask)
+            padded, in_kv_start = not (right and left), left and kv_start_ok
+            if in_kv_start:
+                self.kv_start.copy_(start)
+        else:
+            padded, in_kv_start = not bool(attention_mask.all()), False
+        self.dense_mask = padded and not in_kv_start
+        return padded and (self.dense_mask or not flash)
+
+    def fill(self, kv: Iterable[Tuple[torch.Tensor, torch.Tensor]], S: int,
+             window: Optional[Tuple[torch.Tensor, torch.Tensor]] = None) -> None:
+        """Hold a fixed window of ``S`` rows (e.g. the encoder projection a decoder cross-attends to): ``kv`` yields
+        ``(k, v)`` ``[b, heads, S, d]`` of every layer, and each sample sees the rows ``kv_start[b] <= j < end[b]`` of
+        ``window = (kv_start, end)`` (int32 ``[b]``), or all ``S``.  Read with ``attend(causal=False)``."""
+        self.reset()
+        if window is None:
+            self.seqlens.fill_(S)
+        else:
+            self.kv_start.copy_(window[0])
+            self.seqlens.copy_(window[1])
+        self.length = S
+        for i, (k, v) in enumerate(kv):
+            self.k[i][:, :, :S] = k
+            self.v[i][:, :, :S] = v
 
     def reserve(self, n: int) -> None:
         """Make room for ``n`` more rows: the buffers are reallocated at twice their capacity (or more, when needed) and
@@ -177,6 +292,15 @@ class KVCacheOwner:
                              f"and the current length is {c.length + s_len}.")
         c.reserve(s_len)
         return c
+
+    def prepare_inputs_for_generation(self, input_ids, past=None, attention_mask=None, use_cache=None, **kwargs):
+        """With a warm cache only the newest token is fed; the padding mask always covers cache + new tokens."""
+        if past is not None and use_cache:
+            input_ids = input_ids[:, -1:]
+        out = {"input_ids": input_ids, "use_cache": bool(use_cache)}
+        if attention_mask is not None and not bool(attention_mask.all()):
+            out["attention_mask"] = attention_mask
+        return out
 
     def set_cache(self, past_key_values):
         """``None`` empties the cache (its buffers are kept); a :class:`StaticKVCache` becomes the model's cache."""

@@ -184,7 +184,14 @@ class MultiheadAttention(nn.Module):
                 output, bias = self.dense(context)
                 return OF.bias_dropout_add(output, bias, residual, self.output_dropout_prob, self.training)
             if isinstance(past_key_value, KVCacheLayer):
-                context = self._cached_attention(qkv_packed, attention_mask, past_key_value).reshape(bsz, -1, a * d)
+                if self.attn_mask_type != AttnMaskType.causal:
+                    raise ValueError("a KVCacheLayer decodes causal self-attention only")
+                if isinstance(attention_mask, KeyPaddingMask):
+                    attention_mask = attention_mask.dense()
+                q = past_key_value.append(qkv_packed)
+                context = past_key_value.attend(q, scale=self.softmax_scale, mask=attention_mask,
+                                                dropout_p=self.attention_dropout_prob, training=self.training)
+                context = context.reshape(bsz, -1, a * d)
                 if sp and hidden_states.dim() == 2:
                     context = context.reshape(-1, a * d)
                 output, bias = self.dense(context)
@@ -227,27 +234,6 @@ class MultiheadAttention(nn.Module):
         if use_cache:
             return output, past_key_value
         return output
-
-    def _cached_attention(self, qkv, attention_mask, cache):
-        """Self-attention with a :class:`KVCacheLayer`: append k, v in place, then :func:`OF.decode_attention` for the
-        steps after the prefill (split-KV kernel for bf16 with head dim 64 / 128 and up to 16 new tokens, the causal
-        flash kernel over the cache window for longer continuations) or the usual dispatch on views of the cache →
-        ``[b, s, a, d]``."""
-        d = self.head_size
-        past, s_len = cache.length, qkv.shape[1]
-        OF.kv_cache_append(qkv, cache.k, cache.v, cache.seqlens, return_q=False)
-        q = qkv[..., :d]
-        if past > 0 and attention_mask is None and self.attn_mask_type == AttnMaskType.causal:
-            return OF.decode_attention(q, cache.k, cache.v, cache.seqlens, cache.kv_start, scale=self.softmax_scale,
-                                       past=past)
-        if isinstance(attention_mask, KeyPaddingMask):
-            attention_mask = attention_mask.dense()
-        L = past + s_len
-        context = OF.attention(q.permute(0, 2, 1, 3), cache.k[:, :, :L], cache.v[:, :, :L],
-                               causal=self.attn_mask_type == AttnMaskType.causal and attention_mask is None,
-                               scale=self.softmax_scale, mask=attention_mask, dropout_p=self.attention_dropout_prob,
-                               training=self.training)
-        return context.transpose(1, 2)
 
     def extra_repr(self) -> str:
         return "hidden_size={}, num_heads={}, is_cross_attention={}".format(

@@ -19,7 +19,7 @@ vocab-parallel cross entropy (the reference replicates ``lm_head``).
 from __future__ import annotations
 
 import math
-from typing import List, Optional, Tuple
+from typing import List, Tuple
 
 import torch
 from torch import nn
@@ -34,7 +34,7 @@ from libai_b200.parallel import mappings
 from libai_b200.utils import distributed as dutil
 
 from libai_b200.inference.generator.generation_utils import Generator
-from libai_b200.inference.kv_cache import KVCacheLayer, KVCacheOwner, StaticKVCache, left_padding
+from libai_b200.inference.kv_cache import KVCacheLayer, KVCacheOwner, StaticKVCache
 
 from .utils.pipeline_model import PipelineStageMixin
 from .utils.weight_init import init_method_normal, scaled_init_method_normal
@@ -160,7 +160,8 @@ class LlamaAttention(nn.Module):
         qkv = self.query_key_value(hidden_states)
         qkv = qkv.view(bsz, -1, a, 3 * d) if g == a else qkv.view(bsz, -1, g, a // g + 2, d)
         if isinstance(past_key_value, KVCacheLayer):
-            context = self._cached_attention(qkv, attention_mask, past_key_value, cos_cached, sin_cached)
+            q = past_key_value.append(qkv, cos_cached, sin_cached)
+            context = past_key_value.attend(q, scale=self.norm_factor, mask=attention_mask)
             context = context.reshape(-1, a * d) if sp else context.reshape(bsz, -1, a * d)
             output = self.o_proj(context)
             return (output, past_key_value) if use_cache else output
@@ -193,26 +194,6 @@ class LlamaAttention(nn.Module):
             context = context.reshape(-1, a * d)
         output = self.o_proj(context)
         return (output, past_key_value) if use_cache else output
-
-    def _cached_attention(self, qkv, attention_mask, cache, cos, sin):
-        """Rotary + append into the layer's cache, then attention over it → ``[b, s, a, d]``.  Steps after the prefill
-        (padding carried by ``cache.kv_start``) go to :func:`OF.decode_attention`: the split-KV kernel for bf16 with head
-        dim 64 / 128 and up to 16 new tokens, the causal flash kernel over the cache window for longer continuations,
-        the reference math otherwise.  The prefill runs the usual dispatch on views of the cache: the flash kernel for
-        a causal prompt, left padding included (``cache.kv_start``), and the reference math for a dense
-        ``attention_mask``."""
-        past, s_len = cache.length, qkv.shape[1]
-        q = OF.kv_cache_append(qkv, cache.k, cache.v, cache.seqlens, cos, sin)
-        if past > 0 and attention_mask is None:
-            return OF.decode_attention(q, cache.k, cache.v, cache.seqlens, cache.kv_start, scale=self.norm_factor,
-                                       past=past)
-        L = past + s_len
-        query, key, value = q.permute(0, 2, 1, 3), cache.k[:, :, :L], cache.v[:, :, :L]
-        causal = attention_mask is None   # prefill of an unpadded or left-padded prompt
-        kv_start = cache.kv_start if causal and OF.attention_supported(query, key) else None
-        context = OF.attention(query, key, value, causal=causal, scale=self.norm_factor, mask=attention_mask,
-                               kv_start=kv_start)
-        return context.transpose(1, 2)
 
 
 class CasualMask(nn.Module):
@@ -361,7 +342,7 @@ class SFTLoss(nn.Module):
         return {"lm_loss": (loss * keep).sum() / keep.sum().clamp(min=1.0)}
 
 
-class LlamaForCausalLM(nn.Module, PipelineStageMixin, Generator, KVCacheOwner):
+class LlamaForCausalLM(nn.Module, PipelineStageMixin, KVCacheOwner, Generator):
 
     # `train.dist.sequence_parallel = "auto"` resolves to True for this model (token-sharded activations between
     # the tensor-parallel blocks are handled by its embeddings / heads)
@@ -387,8 +368,6 @@ class LlamaForCausalLM(nn.Module, PipelineStageMixin, Generator, KVCacheOwner):
         self.lm_head = Linear(hidden_size, vocab_size, bias=False, parallel="col",
                               init_method=init_method_normal(initializer_range), layer_idx=-1)
         self.loss_func = SFTLoss()
-        self.kv_cache: Optional[StaticKVCache] = None
-        self.past_length = 0
 
     @classmethod
     def from_config(cls, cfg):
@@ -456,17 +435,8 @@ class LlamaForCausalLM(nn.Module, PipelineStageMixin, Generator, KVCacheOwner):
             cache = self._prepare_cache(input_ids, max_positions=self.model.cos_cached.shape[0])
             self.past_length = past = cache.length
             mask = None
-            if attention_mask is not None:
-                if past == 0:
-                    kv_start = left_padding(attention_mask) if attention_mask.dim() == 2 else None
-                    cache.dense_mask = kv_start is None
-                    if kv_start is not None:
-                        cache.kv_start.copy_(kv_start)
-                # the flash kernel reads a left-padded prompt's padding from cache.kv_start; the reference math and
-                # every step of a mask kv_start cannot express take the dense mask
-                c_k = cache.k[cache.owned[0]]
-                if cache.dense_mask or (past == 0 and not OF.attention_supported(c_k, c_k)):
-                    mask = self.casual_mask(input_ids, past_length=past, attention_mask=attention_mask)
+            if cache.step_needs_dense_mask(attention_mask, flash=cache.flash_attention()):
+                mask = self.casual_mask(input_ids, past_length=past, attention_mask=attention_mask)
             output = self.model(input_ids, attention_mask=mask, past_key_values=cache)
             self.past_length = cache.length
         logits = self.lm_head(output)
@@ -477,15 +447,6 @@ class LlamaForCausalLM(nn.Module, PipelineStageMixin, Generator, KVCacheOwner):
     # ---- KV cache (KVCacheOwner) ----------------------------------------------------------------
     def _cache_attention_modules(self):
         return [layer.self_attn for layer in self.model.layers]
-
-    def prepare_inputs_for_generation(self, input_ids, past=None, attention_mask=None, use_cache=None, **kwargs):
-        """With a warm cache only the newest token is fed; the padding mask always covers cache + new tokens."""
-        if past is not None and use_cache:
-            input_ids = input_ids[:, -1:]
-        out = {"input_ids": input_ids, "use_cache": bool(use_cache)}
-        if attention_mask is not None and not bool(attention_mask.all()):
-            out["attention_mask"] = attention_mask
-        return out
 
     @staticmethod
     def set_pipeline_stage_id(model):

@@ -21,9 +21,8 @@ from torch import nn
 
 from libai_b200.config import configurable
 from libai_b200.inference.generator.generation_utils import Generator
-from libai_b200.inference.kv_cache import KVCacheLayer, KVCacheOwner, StaticKVCache, left_padding
+from libai_b200.inference.kv_cache import KVCacheLayer, KVCacheOwner, StaticKVCache, padding_bounds
 from libai_b200.layers import LayerNorm, Linear, LMLogits, ParallelCrossEntropyLoss, VocabEmbedding
-from libai_b200.layers.attention import KeyPaddingMask
 from libai_b200.models.utils.weight_init import init_method_normal
 from libai_b200.ops import functional as OF
 from libai_b200.ops import use_native
@@ -80,7 +79,8 @@ class BloomAttention(nn.Module):
         bias = None if inputs.bias is None else inputs.bias[:, rank * a : (rank + 1) * a]
         qkv = self.query_key_value(hidden).view(b, s, a, 3 * d)   # per-head [q|k|v]: the MHA packed layout
         if cache is not None:
-            ctx = self._cached_attention(qkv, inputs, cache, slopes, bias)
+            ctx = cache.attend(cache.append(qkv), scale=1.0 / math.sqrt(d), mask=inputs.mask, bias=bias,
+                               alibi_slopes=slopes)
         else:
             q, k, v = (t.transpose(1, 2) for t in OF.split_qkv(qkv))   # [b, a, s, d] views
             if bias is None:
@@ -93,25 +93,6 @@ class BloomAttention(nn.Module):
             ctx = ctx.transpose(1, 2)
         out = self.dense(ctx.reshape(b, s, a * d))
         return residual + self.hidden_dropout(out)
-
-    def _cached_attention(self, qkv, inputs: AttentionInputs, cache: KVCacheLayer, slopes, bias):
-        """Append k, v to the layer's cache, then attention over it → ``[b, s, a, d]``.  Steps after the prefill go to
-        :func:`OF.decode_attention` with the slopes (the split-KV kernel up to 16 new tokens, the causal flash kernel
-        over the cache window beyond; ``cache.kv_start`` carries left padding); the prefill runs the flash kernel over
-        the cache window, and a dense ``inputs.mask`` the reference math."""
-        past, scale = cache.length, 1.0 / math.sqrt(self.head_dim)
-        q = OF.kv_cache_append(qkv, cache.k, cache.v, cache.seqlens)
-        if past > 0 and bias is None:
-            return OF.decode_attention(q, cache.k, cache.v, cache.seqlens, cache.kv_start, scale=scale, past=past,
-                                       alibi_slopes=slopes)
-        L = past + qkv.shape[1]
-        query, key, value = q.permute(0, 2, 1, 3), cache.k[:, :, :L], cache.v[:, :, :L]
-        if bias is not None:
-            ctx = OF.attention(query, key, value, causal=False, scale=scale, mask=inputs.mask, bias=bias)
-        else:   # prefill of an unpadded or left-padded prompt
-            kv_start = cache.kv_start if OF.attention_supported(query, key) else None
-            ctx = OF.attention(query, key, value, causal=True, scale=scale, alibi_slopes=slopes, kv_start=kv_start)
-        return ctx.transpose(1, 2)
 
 
 class BloomMLP(nn.Module):
@@ -189,35 +170,22 @@ class BloomModel(nn.Module):
             # a model placed on the GPU or cast (``.to(torch.bfloat16)`` casts buffers too): the kernels take fp32
             self.alibi_slopes = alibi_slopes(self.n_head).to(hidden.device)
         slopes = self.alibi_slopes
-        # the flash kernels take right / left padding as kv_lens / kv_start instead of a dense mask
-        flash = use_native(hidden) and hidden.dtype == torch.bfloat16 and OF.flash_head_dim_supported(self.head_dim)
-        padded = attention_mask is not None and not bool(attention_mask.all())
         if isinstance(past_key_values, StaticKVCache):
             cache = past_key_values
-            past = cache.length
-            if past == 0 and padded:
-                kv_start = left_padding(attention_mask)
-                cache.dense_mask = kv_start is None
-                if kv_start is not None:
-                    cache.kv_start.copy_(kv_start)
-            # the flash kernel reads a left-padded prompt's padding from cache.kv_start; the reference math and every
-            # step of a mask kv_start cannot express take the dense mask
-            dense = padded and (cache.dense_mask or (past == 0 and not flash))
-            inputs = self._dense_inputs(slopes, input_ids, past, attention_mask) if dense else AttentionInputs(slopes)
+            dense = cache.step_needs_dense_mask(attention_mask, flash=cache.flash_attention())
+            inputs = self._dense_inputs(slopes, input_ids, cache.length, attention_mask) if dense else \
+                AttentionInputs(slopes)
             for i, block in enumerate(self.h):
                 hidden = block(hidden, inputs, cache.layer(i))
             cache.advance(input_ids.shape[1])
             return self.ln_f(hidden)
+        # the flash kernels take right / left padding as kv_lens / kv_start instead of a dense mask
+        flash = use_native(hidden) and hidden.dtype == torch.bfloat16 and OF.flash_head_dim_supported(self.head_dim)
+        padded = attention_mask is not None and not bool(attention_mask.all())
         inputs = AttentionInputs(slopes)
-        if padded and flash:
-            keys = KeyPaddingMask(attention_mask)
-            kv_start = None if keys.is_prefix() else left_padding(attention_mask)
-            if keys.is_prefix():
-                inputs = inputs._replace(kv_lens=keys.lengths)
-            elif kv_start is not None:
-                inputs = inputs._replace(kv_start=kv_start)
-            else:   # neither a right- nor a left-padded batch
-                inputs = self._dense_inputs(slopes, input_ids, 0, attention_mask)
+        bounds = padding_bounds(attention_mask) if padded and flash else None
+        if bounds is not None:
+            inputs = inputs._replace(kv_lens=bounds[0], kv_start=bounds[1])
         elif padded or not hidden.is_cuda:
             inputs = self._dense_inputs(slopes, input_ids, 0, attention_mask)
         for block in self.h:
@@ -225,7 +193,7 @@ class BloomModel(nn.Module):
         return self.ln_f(hidden)
 
 
-class BloomForCausalLM(nn.Module, Generator, KVCacheOwner):
+class BloomForCausalLM(nn.Module, KVCacheOwner, Generator):
     @configurable
     def __init__(self, cfg=None, **kwargs):
         super().__init__()
@@ -233,8 +201,6 @@ class BloomForCausalLM(nn.Module, Generator, KVCacheOwner):
         self.transformer = BloomModel(cfg=cfg, **kwargs) if cfg is None else BloomModel(cfg)
         self.lm_head = LMLogits(self.transformer.word_embeddings.num_embeddings, bias=False)
         self.loss = ParallelCrossEntropyLoss()
-        self.kv_cache: Optional[StaticKVCache] = None
-        self.past_length = 0
 
     @classmethod
     def from_config(cls, cfg):
@@ -256,12 +222,3 @@ class BloomForCausalLM(nn.Module, Generator, KVCacheOwner):
     # ---- KV cache (KVCacheOwner) ----------------------------------------------------------------
     def _cache_attention_modules(self):
         return [block.self_attention for block in self.transformer.h]
-
-    def prepare_inputs_for_generation(self, input_ids, past=None, attention_mask=None, use_cache=None, **kwargs):
-        """With a warm cache only the newest token is fed; the padding mask always covers cache + new tokens."""
-        if past is not None and use_cache:
-            input_ids = input_ids[:, -1:]
-        out = {"input_ids": input_ids, "use_cache": bool(use_cache)}
-        if attention_mask is not None and not bool(attention_mask.all()):
-            out["attention_mask"] = attention_mask
-        return out

@@ -19,10 +19,9 @@ import torch
 from torch import nn
 
 from libai_b200.inference.generator.generation_utils import Generator
-from libai_b200.inference.kv_cache import KVCacheLayer, KVCacheOwner, StaticKVCache, left_padding
+from libai_b200.inference.kv_cache import KVCacheLayer, KVCacheOwner, StaticKVCache, padding_bounds
 from libai_b200.layers import LayerNorm, Linear, RMSLayerNorm
 from libai_b200.layers._param import create_parameter
-from libai_b200.layers.attention import KeyPaddingMask
 from libai_b200.models.utils.weight_init import init_method_normal
 from libai_b200.ops import functional as OF
 from libai_b200.ops import use_native
@@ -117,8 +116,11 @@ class SelfAttention(nn.Module):
         b, s, _ = hidden.shape
         a, g, d = self.heads, self.groups, self.d
         mixed = self.query_key_value(hidden)
-        if isinstance(kv_cache, KVCacheLayer):
-            return self.dense(self._cached_attention(mixed, inputs, kv_cache).reshape(b, s, a * d))
+        if isinstance(kv_cache, KVCacheLayer):   # GLM rotary into the grouped layout the cache appends from
+            qkv = OF.apply_glm_rotary_qkv(mixed, heads=a, kv_heads=g, table=inputs.table, pos_offset=inputs.pos_offset,
+                                          position_ids=inputs.position_ids, grouped=True)
+            ctx = kv_cache.attend(kv_cache.append(qkv), scale=1.0 / math.sqrt(d), mask=inputs.mask)
+            return self.dense(ctx.reshape(b, s, a * d))
         # per-head [b, s, a, 3d]: every query head with its own copy of its group's K/V (multi-query attention)
         qkv = OF.apply_glm_rotary_qkv(mixed, heads=a, kv_heads=g, table=inputs.table, pos_offset=inputs.pos_offset,
                                       position_ids=inputs.position_ids)
@@ -132,26 +134,6 @@ class SelfAttention(nn.Module):
             k = torch.cat((kv_cache[0].repeat_interleave(a // g, dim=1).type_as(k), k), dim=2)
             v = torch.cat((kv_cache[1].repeat_interleave(a // g, dim=1).type_as(v), v), dim=2)
         return self.dense(self.core_attention(q, k, v, inputs.mask, kv_start=inputs.kv_start))
-
-    def _cached_attention(self, mixed, inputs: AttentionInputs, cache: KVCacheLayer):
-        """GLM rotary into the grouped layout, append to the layer's cache, then attention over it → ``[b, s, a, d]``.
-        Once the cache holds rows (a P-tuning prefix, an earlier step), the new tokens go to :func:`OF.decode_attention`
-        (the split-KV kernel up to 16 tokens, the causal flash kernel over the cache window beyond); the prefill of an
-        empty cache runs the flash kernel (``cache.kv_start`` carries left padding), and a dense ``inputs.mask`` the
-        reference math."""
-        a, g, d = self.heads, self.groups, self.d
-        qkv = OF.apply_glm_rotary_qkv(mixed, heads=a, kv_heads=g, table=inputs.table, pos_offset=inputs.pos_offset,
-                                      position_ids=inputs.position_ids, grouped=True)
-        past, scale = cache.length, 1.0 / math.sqrt(d)
-        q = OF.kv_cache_append(qkv, cache.k, cache.v, cache.seqlens)
-        if past > 0 and inputs.mask is None:
-            return OF.decode_attention(q, cache.k, cache.v, cache.seqlens, cache.kv_start, scale=scale, past=past)
-        L = past + qkv.shape[1]
-        query, key, value = q.permute(0, 2, 1, 3), cache.k[:, :, :L], cache.v[:, :, :L]
-        causal = inputs.mask is None
-        kv_start = cache.kv_start if causal and OF.attention_supported(query, key) else None
-        ctx = OF.attention(query, key, value, causal=causal, scale=scale, mask=inputs.mask, kv_start=kv_start)
-        return ctx.transpose(1, 2)
 
 
 class MLP(nn.Module):
@@ -286,27 +268,16 @@ class ChatGLMModel(nn.Module, ChatGLMPreTrainedModel):
         if self._rope is None or self._rope.device != input_ids.device or self._rope.shape[0] < self.seq_length:
             self._rope = rope_cache(self.seq_length, self.rotary_dim, device=input_ids.device)
         pre = self.pre_seq_len or 0
-        flash = self._flash_attention(hidden)
         if isinstance(past_key_values, StaticKVCache):
             cache = past_key_values
-            if cache.length == 0:   # prefill: the P-tuning prefix rows first, then the prompt's padding
-                padded = attention_mask is not None and not bool(attention_mask.all())
-                if pre:
-                    for i, (k, v) in enumerate(self.get_prompt(b, input_ids.device, hidden.dtype)):
-                        if i in cache.owned:
-                            cache.k[i][:, :, :pre] = k
-                            cache.v[i][:, :, :pre] = v
-                    cache.advance(pre)
-                if padded:
-                    kv_start = left_padding(attention_mask) if not pre else None
-                    cache.dense_mask = kv_start is None
-                    if kv_start is not None:
-                        cache.kv_start.copy_(kv_start)
-                # the flash kernel reads a left-padded prompt's padding from cache.kv_start; the reference math and
-                # every step of a mask kv_start cannot express take the dense mask
-                dense = padded and (cache.dense_mask or not flash)
-            else:
-                dense = cache.dense_mask
+            # the prompt's padding sits behind the P-tuning prefix rows, where kv_start cannot describe it
+            dense = cache.step_needs_dense_mask(attention_mask, flash=cache.flash_attention(), kv_start_ok=not pre)
+            if cache.length == 0 and pre:   # prefill: the prefix rows first
+                for i, (k, v) in enumerate(self.get_prompt(b, input_ids.device, hidden.dtype)):
+                    if i in cache.owned:
+                        cache.k[i][:, :, :pre] = k
+                        cache.v[i][:, :, :pre] = v
+                cache.advance(pre)
             past = cache.length
             inputs = AttentionInputs(self._rope, past - pre, position_ids,
                                      mask=self.get_masks(input_ids, past, attention_mask) if dense else None)
@@ -315,28 +286,23 @@ class ChatGLMModel(nn.Module, ChatGLMPreTrainedModel):
             return hidden
         padded = attention_mask is not None and not bool(attention_mask.all())
         inputs = AttentionInputs(self._rope, 0, position_ids)
-        if not flash or (padded and pre):
+        if not self._flash_attention(hidden) or (padded and pre):
             inputs = inputs._replace(mask=self.get_masks(input_ids, pre, attention_mask if padded else None))
         elif padded:
-            keys = KeyPaddingMask(attention_mask)
-            kv_start = None if keys.is_prefix() else left_padding(attention_mask)
-            if keys.is_prefix():
-                inputs = inputs._replace(kv_lens=keys.lengths)
-            elif kv_start is not None:
-                inputs = inputs._replace(kv_start=kv_start)
-            else:   # neither a right- nor a left-padded batch
+            bounds = padding_bounds(attention_mask)
+            if bounds is None:   # neither a right- nor a left-padded batch
                 inputs = inputs._replace(mask=self.get_masks(input_ids, 0, attention_mask))
+            else:
+                inputs = inputs._replace(kv_lens=bounds[0], kv_start=bounds[1])
         prefix = self.get_prompt(b, input_ids.device, hidden.dtype) if pre else None
         return self.encoder(hidden, inputs, kv_caches=prefix)
 
 
-class ChatGLMForConditionalGeneration(nn.Module, ChatGLMPreTrainedModel, Generator, KVCacheOwner):
+class ChatGLMForConditionalGeneration(nn.Module, ChatGLMPreTrainedModel, KVCacheOwner, Generator):
     def __init__(self, cfg):
         super().__init__()
         self.cfg = cfg
         self.transformer = ChatGLMModel(cfg)
-        self.kv_cache: Optional[StaticKVCache] = None
-        self.past_length = 0
         if cfg.get("lora_enable", False):
             from projects.ChatGLM.lora.lora_model import LoraModel
 
@@ -372,15 +338,6 @@ class ChatGLMForConditionalGeneration(nn.Module, ChatGLMPreTrainedModel, Generat
     def allocate_kv_cache(self, batch: int, max_length: int) -> StaticKVCache:
         # the cache also holds the P-tuning prefix rows
         return super().allocate_kv_cache(batch, max_length + (self.glm.pre_seq_len or 0))
-
-    def prepare_inputs_for_generation(self, input_ids, past=None, attention_mask=None, use_cache=None, **kwargs):
-        """With a warm cache only the newest token is fed; the padding mask always covers cache + new tokens."""
-        if past is not None and use_cache:
-            input_ids = input_ids[:, -1:]
-        out = {"input_ids": input_ids, "use_cache": bool(use_cache)}
-        if attention_mask is not None and not bool(attention_mask.all()):
-            out["attention_mask"] = attention_mask
-        return out
 
     def process_response(self, output, history):
         content = ""

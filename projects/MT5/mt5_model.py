@@ -107,7 +107,29 @@ class T5Attention(nn.Module):
     def forward(self, hidden, mask=None, encoder_states=None, past_key_value=None, position_bias=None, use_cache=False,
                 cache: Optional[KVCacheLayer] = None):
         if cache is not None:
-            return self._cached_forward(hidden, mask, cache, position_bias)
+            # Attention of the new tokens over the layer's cache.  Self-attention appends k, v first and, without a
+            # mask, takes the relative-bias vector (built by the first layer, then handed down as position_bias).
+            # Cross-attention reads the cache of the encoder projection, without a mask through its window.  A mask
+            # (decoder padding, an encoder mask with holes) keeps the dense bias with the mask folded in.
+            b, s = hidden.shape[:2]
+            a, d = self.local_heads, self.head_size
+            causal = not self.is_cross_attention
+            if causal:
+                q = cache.append(self.query_key_value(hidden).view(b, s, a, 3 * d))
+            else:
+                q = self.query(hidden).view(b, s, a, d)
+            if mask is None:
+                if causal and position_bias is None:
+                    position_bias = self.relative_bias_vector()
+                ctx = cache.attend(q, scale=1.0, causal=causal, rel_bias=position_bias)
+            else:
+                if position_bias is None:
+                    L = mask.shape[-1]
+                    position_bias = self.compute_bias(s, L, hidden.device) if causal else \
+                        torch.zeros(1, a, s, L, device=hidden.device, dtype=hidden.dtype)
+                    position_bias = position_bias + (1.0 - mask.to(position_bias.dtype)) * -10000.0
+                ctx = cache.attend(q, scale=1.0, causal=causal, bias=position_bias)
+            return self.dropout(self.dense(ctx.reshape(b, s, a * d))), position_bias, None
         b = hidden.shape[0]
         a, d = self.local_heads, self.head_size
         if self.is_cross_attention:
@@ -140,43 +162,6 @@ class T5Attention(nn.Module):
                            training=self.training)
         out = self.dropout(self.dense(ctx.transpose(1, 2).reshape(b, -1, a * d)))
         return out, position_bias, present
-
-    def _cached_forward(self, hidden, mask, cache: KVCacheLayer, position_bias):
-        """Attention of the new tokens over the layer's cache.  Self-attention appends k, v first and, without a
-        ``mask``, runs :func:`OF.decode_attention` with the relative-bias vector (built by the first layer, then handed
-        down as ``position_bias``).  Cross-attention reads the cache of the encoder projection: without a ``mask``
-        through the non-causal decode window ``cache.kv_start <= j < cache.seqlens``.  A ``mask`` (decoder padding, an
-        encoder mask with holes) keeps the dense bias with the mask folded in, as without the cache."""
-        b, s = hidden.shape[:2]
-        a, d = self.local_heads, self.head_size
-        if self.is_cross_attention:
-            q = self.query(hidden).view(b, s, a, d)
-            if mask is None:
-                ctx = OF.decode_attention(q, cache.k, cache.v, cache.seqlens, cache.kv_start, scale=1.0, causal=False)
-            else:
-                L = mask.shape[-1]
-                if position_bias is None:
-                    position_bias = torch.zeros(1, a, s, L, device=hidden.device, dtype=hidden.dtype)
-                    position_bias = position_bias + (1.0 - mask.to(position_bias.dtype)) * -10000.0
-                ctx = OF.attention(q.transpose(1, 2), cache.k[:, :, :L], cache.v[:, :, :L], causal=False, scale=1.0,
-                                   bias=position_bias).transpose(1, 2)
-        else:
-            past = cache.length
-            q = OF.kv_cache_append(self.query_key_value(hidden).view(b, s, a, 3 * d), cache.k, cache.v, cache.seqlens)
-            if mask is None:
-                if position_bias is None:
-                    position_bias = self.relative_bias_vector()
-                ctx = OF.decode_attention(q, cache.k, cache.v, cache.seqlens, cache.kv_start, scale=1.0, past=past,
-                                          rel_bias=position_bias)
-            else:
-                L = past + s
-                if position_bias is None:
-                    position_bias = self.compute_bias(s, L, hidden.device)
-                    position_bias = position_bias + (1.0 - mask.to(position_bias.dtype)) * -10000.0
-                ctx = OF.attention(q.transpose(1, 2), cache.k[:, :, :L], cache.v[:, :, :L], causal=False, scale=1.0,
-                                   bias=position_bias).transpose(1, 2)
-        out = self.dropout(self.dense(ctx.reshape(b, s, a * d)))
-        return out, position_bias, None
 
 
 class T5MLP(nn.Module):
@@ -293,8 +278,6 @@ class MT5Model(nn.Module, Generator, KVCacheOwner):
         self.decoder = stack(True, hidden_layers)
         self.past_key_values = [None] * hidden_layers   # the tuple cache of pipeline-parallel inference
         self.encoder_states = None
-        self.past_length = 0
-        self.kv_cache: Optional[StaticKVCache] = None      # decoder self-attention (KVCacheOwner)
         self.cross_cache: Optional[StaticKVCache] = None   # the encoder projection of every decoder layer
         self.tie_word_embeddings = bool(cfg.get("tie_word_embeddings", model_type != "mt5")) if cfg is not None else model_type != "mt5"
         if model_type == "mt5":
@@ -496,18 +479,10 @@ class MT5Model(nn.Module, Generator, KVCacheOwner):
         c = self.cross_cache
         if c is None or not c.matches(b, encoder_states.dtype, encoder_states.device) or c.capacity < S:
             c = StaticKVCache(len(self.decoder.layers), b, a, d, S, encoder_states.dtype, encoder_states.device)
-        c.reset()
+        kv = (layer.cross_attention.key_value(encoder_states).view(b, S, a, 2 * d).transpose(1, 2).split(d, dim=-1)
+              for layer in self.decoder.layers)
+        c.fill(kv, S, window)
         c.dense_mask = dense_mask
-        if window is None:
-            c.seqlens.fill_(S)
-        else:
-            c.kv_start.copy_(window[0])
-            c.seqlens.copy_(window[1])
-        c.length = S
-        for i, layer in enumerate(self.decoder.layers):
-            kv = layer.cross_attention.key_value(encoder_states).view(b, S, a, 2 * d).transpose(1, 2)
-            c.k[i][:, :, :S] = kv[..., :d]
-            c.v[i][:, :, :S] = kv[..., d:]
         self.cross_cache = c
 
     # ---- generation support ---------------------------------------------------------------------

@@ -16,8 +16,6 @@ class GPTModel(core.GPTModel, Generator, KVCacheOwner):
     def __init__(self, *args, cfg=None, **kwargs):
         super().__init__(*args, **kwargs)
         self.cfg = cfg
-        self.kv_cache = None
-        self.past_length = 0
 
     @classmethod
     def from_config(cls, cfg):
