@@ -803,9 +803,10 @@ std::tuple<Tensor, Tensor, Tensor> attn_fwd(const Tensor& q, const Tensor& k, co
 // ---- KV-cache decoding ------------------------------------------------------------------------------
 // The cache capacity C (rows per head) cannot be checked against the device-side lengths without a host sync: the
 // caller (libai_b200.inference.kv_cache.StaticKVCache) guarantees cache_seqlens[b] + Sq <= C before every call.
-void check_cache(const Tensor& k_cache, const Tensor& v_cache, const char* what) {
-  TORCH_CHECK(k_cache.is_cuda() && k_cache.scalar_type() == at::kBFloat16 && v_cache.scalar_type() == at::kBFloat16,
-              what, ": bf16 CUDA cache expected");
+void check_cache(const Tensor& k_cache, const Tensor& v_cache, const char* what,
+                 at::ScalarType dtype = at::kBFloat16) {
+  TORCH_CHECK(k_cache.is_cuda() && k_cache.scalar_type() == dtype && v_cache.scalar_type() == dtype, what, ": ",
+              dtype, " CUDA cache expected, got ", k_cache.scalar_type(), " and ", v_cache.scalar_type());
   TORCH_CHECK(k_cache.dim() == 4 && k_cache.sizes() == v_cache.sizes() && k_cache.is_contiguous() && v_cache.is_contiguous(),
               what, ": K and V caches must be contiguous [B, G, C, D] of the same shape");
   TORCH_CHECK(k_cache.size(3) == 64 || k_cache.size(3) == 128, what, ": head dim must be 64 or 128");
@@ -815,6 +816,19 @@ void check_cache(const Tensor& k_cache, const Tensor& v_cache, const char* what)
 void check_lengths(const Tensor& t, int64_t B, const char* what) {
   TORCH_CHECK(t.is_cuda() && t.scalar_type() == at::kInt && t.dim() == 1 && t.size(0) == B && t.is_contiguous(), what,
               ": int32 CUDA [B] expected");
+}
+// the row scales of an FP8 (E4M3) cache [B, G, C, D]: contiguous fp32 [B, G, C] on `device`, C a multiple of 4 (the
+// decode kernel loads the scales of a tile from a 16-byte boundary)
+void check_scales(const c10::optional<Tensor>& scale, const Tensor& cache, const c10::Device& device,
+                  const char* what) {
+  TORCH_CHECK(given(scale), what, ": an FP8 cache needs k_scale and v_scale");
+  const Tensor& t = *scale;
+  TORCH_CHECK(t.scalar_type() == at::kFloat && t.dim() == 3 && t.size(0) == cache.size(0) &&
+                  t.size(1) == cache.size(1) && t.size(2) == cache.size(2) && t.is_contiguous() && t.device() == device,
+              what, ": scales: contiguous fp32 [B, G, C] on q's device expected, got ", t.scalar_type(), " ", t.sizes(),
+              " on ", t.device());
+  TORCH_CHECK(cache.size(2) % 4 == 0 && reinterpret_cast<uintptr_t>(t.data_ptr()) % 16 == 0, what,
+              ": an FP8 cache's capacity must be a multiple of 4 and its scales 16-byte aligned");
 }
 
 // k, v of the packed projection qkv ([B, Sq, A, 3D] or grouped [B, Sq, G, r + 2, D]) go to rows cache_seqlens[b] + i
@@ -850,17 +864,63 @@ Tensor kv_append(const Tensor& qkv, const Tensor& k_cache, const Tensor& v_cache
   return q_out;
 }
 
+// kv_append into an FP8 (E4M3) cache with row scales k_scale, v_scale (fp32 [B, G, C]): q (returned when write_q) and
+// the bf16 k row before quantization are those of kv_append; each k and v row x is stored as the bytes
+// e4m3_rn_satfinite(x / s) with s = amax|x| / 448 (1 for a zero row).
+Tensor kv_append_fp8(const Tensor& qkv, const Tensor& k_cache, const Tensor& v_cache, const Tensor& k_scale,
+                     const Tensor& v_scale, const Tensor& cache_seqlens, const c10::optional<Tensor>& cosv,
+                     const c10::optional<Tensor>& sinv, bool write_q) {
+  c10::cuda::CUDAGuard guard(qkv.device());
+  check_cache(k_cache, v_cache, "kv_append_fp8", at::kFloat8_e4m3fn);
+  check_scales(k_scale, k_cache, qkv.device(), "kv_append_fp8: k_scale");
+  check_scales(v_scale, v_cache, qkv.device(), "kv_append_fp8: v_scale");
+  const int B = (int)k_cache.size(0), G = (int)k_cache.size(1), C = (int)k_cache.size(2), D = (int)k_cache.size(3);
+  TORCH_CHECK(qkv.is_cuda() && qkv.scalar_type() == at::kBFloat16 && qkv.is_contiguous(),
+              "kv_append_fp8: contiguous bf16 packed projection expected");
+  const PackedQKV g = packed_qkv(qkv, "kv_append_fp8");
+  TORCH_CHECK(g.B == B && g.G == G && g.D == D, "kv_append_fp8: qkv does not match the cache");
+  const int Sq = g.S, A = G * g.r;
+  TORCH_CHECK(Sq >= 1 && Sq <= C, "kv_append_fp8: 1 <= Sq <= capacity");
+  check_lengths(cache_seqlens, B, "kv_append_fp8: cache_seqlens");
+  const float* cp = nullptr;
+  const float* sp = nullptr;
+  if (cosv.has_value() && cosv->defined()) {
+    TORCH_CHECK(sinv.has_value() && sinv->defined(), "kv_append_fp8: cos and sin go together");
+    TORCH_CHECK(cosv->scalar_type() == at::kFloat && sinv->scalar_type() == at::kFloat && cosv->is_contiguous() &&
+                sinv->is_contiguous() && cosv->dim() == 2 && cosv->size(1) == D && cosv->sizes() == sinv->sizes() &&
+                cosv->is_cuda(), "kv_append_fp8: cos/sin fp32 contiguous [positions, D]");
+    cp = cosv->data_ptr<float>();
+    sp = sinv->data_ptr<float>();
+  }
+  Tensor q_out = write_q ? at::empty({B, Sq, A, D}, qkv.options()) : at::empty({0}, qkv.options());
+  check(lb_kv_append_fp8(qkv.data_ptr(), cp, sp, write_q ? q_out.data_ptr() : nullptr, k_cache.data_ptr(),
+                         v_cache.data_ptr(), k_scale.data_ptr<float>(), v_scale.data_ptr<float>(),
+                         cache_seqlens.data_ptr<int>(), B, Sq, G, g.r, C, D, cur_stream()),
+        "kv_append_fp8");
+  return q_out;
+}
+
 // q [B, Sq, A, D] (any strides with D contiguous, e.g. a view of the packed projection) against the caches [B, G, C, D]
 // (query head h reads cache head h / (A / G)); query i of sample b sees keys kv_start[b] .. cache_seqlens[b] + i.
 // Returns o [B, Sq, A, D] contiguous.  splits = 0: automatic.  alibi_slopes (fp32 [A]): ALiBi, each visible score gets
 // slope_h * (j - cache_seqlens[b] - i).  rel_bias (fp32 [A, R]): T5's relative-position bias, each visible score gets
 // rel_bias[h, min(cache_seqlens[b] + i - j, R - 1)].  causal = false: every query sees kv_start[b] <= j < cache_seqlens[b]
-// (cross-attention; the new tokens are not in this cache), without a bias.
+// (cross-attention; the new tokens are not in this cache), without a bias.  k_scale, v_scale (fp32 [B, G, C]): the row
+// scales of FP8 (E4M3) caches, required for those and rejected otherwise; the scores and outputs are those over the
+// dequantized rows float(e) * s.
 Tensor decode_attn(const Tensor& q, const Tensor& k_cache, const Tensor& v_cache, const Tensor& cache_seqlens,
                    const Tensor& kv_start, double scale, int64_t splits, const c10::optional<Tensor>& alibi_slopes,
-                   const c10::optional<Tensor>& rel_bias, bool causal) {
+                   const c10::optional<Tensor>& rel_bias, bool causal, const c10::optional<Tensor>& k_scale,
+                   const c10::optional<Tensor>& v_scale) {
   c10::cuda::CUDAGuard guard(q.device());
-  check_cache(k_cache, v_cache, "decode_attn");
+  const bool fp8 = k_cache.scalar_type() == at::kFloat8_e4m3fn;
+  check_cache(k_cache, v_cache, "decode_attn", fp8 ? at::kFloat8_e4m3fn : at::kBFloat16);
+  if (fp8) {
+    check_scales(k_scale, k_cache, q.device(), "decode_attn: k_scale");
+    check_scales(v_scale, v_cache, q.device(), "decode_attn: v_scale");
+  } else {
+    TORCH_CHECK(!given(k_scale) && !given(v_scale), "decode_attn: k_scale and v_scale belong to an FP8 cache");
+  }
   const int B = (int)k_cache.size(0), G = (int)k_cache.size(1), C = (int)k_cache.size(2), D = (int)k_cache.size(3);
   TORCH_CHECK(q.is_cuda() && q.scalar_type() == at::kBFloat16 && q.dim() == 4 && q.stride(3) == 1,
               "decode_attn: bf16 q [B, Sq, A, D] with D contiguous expected");
@@ -897,7 +957,7 @@ Tensor decode_attn(const Tensor& q, const Tensor& k_cache, const Tensor& v_cache
   TORCH_CHECK(causal || (slopes == nullptr && rel == nullptr),
               "decode_attn: causal=False takes no score bias (neither alibi_slopes nor rel_bias)");
   const int row_blocks = ((A / G) * Sq + 15) / 16;   // (query head, token) rows of one cache head, 16 per CTA
-  const int nsplit = splits > 0 ? (int)std::min<int64_t>(splits, 32) : lb_decode_splits(B, G * row_blocks, C, D);
+  const int nsplit = splits > 0 ? (int)std::min<int64_t>(splits, 32) : lb_decode_splits(B, G * row_blocks, C, D, fp8);
   Tensor o = at::empty({B, Sq, A, D}, q.options());
   Tensor part_o, part_ml;
   if (nsplit > 1) {
@@ -907,8 +967,9 @@ Tensor decode_attn(const Tensor& q, const Tensor& k_cache, const Tensor& v_cache
   long qs[3] = {q.stride(0), q.stride(1), q.stride(2)};
   check(lb_decode_attn(q.data_ptr(), qs, k_cache.data_ptr(), v_cache.data_ptr(), o.data_ptr(),
                        nsplit > 1 ? part_o.data_ptr<float>() : nullptr, nsplit > 1 ? part_ml.data_ptr<float>() : nullptr,
-                       cache_seqlens.data_ptr<int>(), kv_start.data_ptr<int>(), slopes, rel, R, causal, B, Sq, A, G, C, D,
-                       (float)scale, nsplit, cur_stream()),
+                       cache_seqlens.data_ptr<int>(), kv_start.data_ptr<int>(), slopes, rel, R, causal,
+                       fp8 ? k_scale->data_ptr<float>() : nullptr, fp8 ? v_scale->data_ptr<float>() : nullptr, B, Sq, A,
+                       G, C, D, (float)scale, nsplit, cur_stream()),
         "decode_attn");
   return o;
 }
@@ -1212,8 +1273,9 @@ TORCH_LIBRARY(libai_b200, m) {
   m.def("attn_fwd(Tensor q, Tensor k, Tensor v, bool causal, float scale, Tensor? kv_lens, Tensor? bias=None, Tensor? alibi_slopes=None, float p_drop=0.0, int salt=0, Tensor? kv_start=None, Tensor? doc_start=None) -> (Tensor, Tensor, Tensor)", &attn_fwd);
   m.def("attn_bwd(Tensor dout, Tensor q, Tensor k, Tensor v, Tensor o, Tensor lse, bool causal, float scale, Tensor? kv_lens, Tensor? bias=None, Tensor? alibi_slopes=None, Tensor(a!)? dbias=None, float p_drop=0.0, Tensor? rng_state=None, Tensor? kv_start=None, Tensor? doc_start=None) -> (Tensor, Tensor, Tensor, Tensor)", &attn_bwd);
   m.def("kv_append(Tensor qkv, Tensor(a!) k_cache, Tensor(b!) v_cache, Tensor cache_seqlens, Tensor? cos, Tensor? sin, bool write_q) -> Tensor", &kv_append);
+  m.def("kv_append_fp8(Tensor qkv, Tensor(a!) k_cache, Tensor(b!) v_cache, Tensor(c!) k_scale, Tensor(d!) v_scale, Tensor cache_seqlens, Tensor? cos, Tensor? sin, bool write_q) -> Tensor", &kv_append_fp8);
   m.def("window_attn_fwd(Tensor qkv, int H, int W, int window, int shift, int heads, float scale, Tensor table, Tensor? tau) -> (Tensor, Tensor)", &window_attn_fwd);
   m.def("window_attn_bwd(Tensor dout, Tensor qkv, Tensor lse, int H, int W, int window, int shift, int heads, float scale, Tensor table, Tensor? tau) -> (Tensor, Tensor, Tensor)", &window_attn_bwd);
-  m.def("decode_attn(Tensor q, Tensor k_cache, Tensor v_cache, Tensor cache_seqlens, Tensor kv_start, float scale, int splits=0, Tensor? alibi_slopes=None, Tensor? rel_bias=None, bool causal=True) -> Tensor", &decode_attn);
+  m.def("decode_attn(Tensor q, Tensor k_cache, Tensor v_cache, Tensor cache_seqlens, Tensor kv_start, float scale, int splits=0, Tensor? alibi_slopes=None, Tensor? rel_bias=None, bool causal=True, Tensor? k_scale=None, Tensor? v_scale=None) -> Tensor", &decode_attn);
   m.def("bias_dropout_residual(Tensor x, Tensor? bias, Tensor? res, float p, int salt, Tensor? rng_state=None) -> (Tensor, Tensor)", &bias_dropout_residual);
 }

@@ -1,0 +1,159 @@
+// FP8 (E4M3) KV caches: the quantizing cache append, and the instances of the split-KV decode attention kernel for
+// every score kind at head dims 64 and 128.  Kept in their own translation unit so that the objects of the bf16
+// kernels hold exactly the kernels they held before them.  The format, the scale folding and the shared-memory layout are described
+// at Cfg8 and decode_attn_body in decode_attention_sm90.cuh; the partials go through the same decode_combine_kernel.
+#include "decode_attention_sm90.cuh"
+
+namespace lb {
+namespace dec {
+
+// IEEE round-to-nearest division, also under --use_fast_math (no flush of subnormals)
+__device__ __forceinline__ float div_rn(float a, float b) {
+  float r;
+  asm("div.rn.f32 %0, %1, %2;" : "=f"(r) : "f"(a), "f"(b));
+  return r;
+}
+
+// one row of an FP8 cache: the scale s = amax / 448 (1 for a zero row) and the bytes e4m3_rn_satfinite(x / s) of the
+// bf16 values x[p], x[p + 1] (columns lane * 2 + 64 * p' and D / 2 past them, see kv_append_fp8_kernel)
+template <int P>
+__device__ __forceinline__ void quantize_row(const float (&x)[2 * P], uint8_t* row, float* scale, int lane) {
+  float amax = 0.f;
+#pragma unroll
+  for (int e = 0; e < 2 * P; ++e) amax = fmaxf(amax, fabsf(x[e]));
+  amax = warp_max(amax);
+  const float s = amax == 0.f ? 1.f : div_rn(amax, 448.f);
+#pragma unroll
+  for (int e = 0; e < 2 * P; ++e)
+    row[(e & 1) * (P * 32) + (e >> 1) * 32 + lane] =
+        __nv_cvt_float_to_fp8(div_rn(x[e], s), __NV_SATFINITE, __NV_E4M3);
+  if (lane == 0) *scale = s;
+}
+
+// the FP8 cache append: one warp per (b, i, group); lane c < D/2 handles the pairs (c + 32 p, c + 32 p + D/2) of the
+// r q rows and of k (rotated with the expressions of kv_append_kernel, so q and the bf16 k row are bit-identical to
+// its output) and of v, then each of the k and v rows is quantized (quantize_row) at row cache_seqlens[b] + i
+template <int D>
+__global__ void __launch_bounds__(256) kv_append_fp8_kernel(
+    const __nv_bfloat16* __restrict__ qkv, const float* __restrict__ cosv, const float* __restrict__ sinv,
+    __nv_bfloat16* __restrict__ q_out, uint8_t* __restrict__ kc, uint8_t* __restrict__ vc, float* __restrict__ ks,
+    float* __restrict__ vs, const int* __restrict__ seqlens, int B, int Sq, int G, int r, int C) {
+  constexpr int half = D / 2, P = half / 32;
+  const int lane = threadIdx.x & 31;
+  const size_t total = (size_t)B * Sq * G;
+  const size_t stride = ((size_t)gridDim.x * blockDim.x) >> 5;
+  for (size_t grp = (blockIdx.x * (size_t)blockDim.x + threadIdx.x) >> 5; grp < total; grp += stride) {
+    const int g = static_cast<int>(grp % G);
+    const int i = static_cast<int>((grp / G) % Sq);
+    const int b = static_cast<int>(grp / ((size_t)G * Sq));
+    const int pos = seqlens[b] + i;
+    const size_t in = grp * (r + 2) * D;
+    const size_t crow = ((size_t)b * G + g) * C + pos;
+    float c1[P], c2[P], s1[P], s2[P];
+#pragma unroll
+    for (int p = 0; p < P; ++p) {
+      const int c = lane + 32 * p;
+      c1[p] = 1.f, c2[p] = 1.f, s1[p] = 0.f, s2[p] = 0.f;
+      if (cosv != nullptr) {
+        c1[p] = cosv[pos * D + c], c2[p] = cosv[pos * D + c + half];
+        s1[p] = sinv[pos * D + c], s2[p] = sinv[pos * D + c + half];
+      }
+    }
+    float kx[2 * P], vx[2 * P];   // the bf16 k and v values of this lane: [2p] column c, [2p + 1] column c + D/2
+    for (int j = 0; j <= r; ++j) {   // slots 0 .. r - 1: q of query head g * r + j; slot r: k
+      const size_t src = in + (size_t)j * D;
+#pragma unroll
+      for (int p = 0; p < P; ++p) {
+        const int c = lane + 32 * p;
+        const float x1 = __bfloat162float(qkv[src + c]), x2 = __bfloat162float(qkv[src + c + half]);
+        float y1 = x1, y2 = x2;
+        if (cosv != nullptr) {
+          y1 = x1 * c1[p] - x2 * s1[p];
+          y2 = x2 * c2[p] + x1 * s2[p];
+        }
+        if (j == r) {
+          kx[2 * p] = __bfloat162float(__float2bfloat16(y1));
+          kx[2 * p + 1] = __bfloat162float(__float2bfloat16(y2));
+        } else if (q_out != nullptr) {
+          const size_t qrow = (grp * r + j) * D;
+          q_out[qrow + c] = __float2bfloat16(y1);
+          q_out[qrow + c + half] = __float2bfloat16(y2);
+        }
+      }
+    }
+#pragma unroll
+    for (int p = 0; p < P; ++p) {
+      vx[2 * p] = __bfloat162float(qkv[in + (size_t)(r + 1) * D + lane + 32 * p]);
+      vx[2 * p + 1] = __bfloat162float(qkv[in + (size_t)(r + 1) * D + lane + 32 * p + half]);
+    }
+    quantize_row<P>(kx, kc + crow * D, ks + crow, lane);
+    quantize_row<P>(vx, vc + crow * D, vs + crow, lane);
+  }
+}
+
+template <int D, Score S>
+__global__ void __launch_bounds__(kThreads) decode_attn_fp8_kernel(const Params p, const float* k_scale,
+                                                                   const float* v_scale) {
+  decode_attn_body<D, S, true>(p, k_scale, v_scale);
+}
+
+template <int D, Score S>
+int configure_decode_fp8() {
+  static int resident = 0;
+  if (resident == 0) {
+    auto kern = decode_attn_fp8_kernel<D, S>;
+    if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg8<D>::kSmem) != cudaSuccess ||
+        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&resident, kern, kThreads, Cfg8<D>::kSmem) != cudaSuccess)
+      resident = 0;
+  }
+  return resident;
+}
+
+template <int D, Score S>
+cudaError_t launch_fp8(const Params& p, const float* k_scale, const float* v_scale, int B, int nsplit,
+                       cudaStream_t s) {
+  if (configure_decode_fp8<D, S>() == 0) return cudaErrorInvalidConfiguration;   // the shared memory opt-in failed
+  decode_attn_fp8_kernel<D, S><<<dim3(nsplit, p.G * p.row_blocks, B), kThreads, Cfg8<D>::kSmem, s>>>(p, k_scale,
+                                                                                                      v_scale);
+  return cudaGetLastError();
+}
+
+template <int D>
+cudaError_t launch_fp8(const Params& p, const float* k_scale, const float* v_scale, Score S, int B, int nsplit,
+                       cudaStream_t s) {
+  switch (S) {
+    case Score::kNone: return launch_fp8<D, Score::kNone>(p, k_scale, v_scale, B, nsplit, s);
+    case Score::kAlibi: return launch_fp8<D, Score::kAlibi>(p, k_scale, v_scale, B, nsplit, s);
+    case Score::kRelBias: return launch_fp8<D, Score::kRelBias>(p, k_scale, v_scale, B, nsplit, s);
+    default: return launch_fp8<D, Score::kWindow>(p, k_scale, v_scale, B, nsplit, s);
+  }
+}
+
+cudaError_t launch_decode_attn_fp8(const Params& p, const float* k_scale, const float* v_scale, Score S, int D, int B,
+                                   int nsplit, cudaStream_t s) {
+  return D == 64 ? launch_fp8<64>(p, k_scale, v_scale, S, B, nsplit, s)
+                 : launch_fp8<128>(p, k_scale, v_scale, S, B, nsplit, s);
+}
+
+// (the other score kinds hold as many CTAs per SM: the same shared memory, and registers that do not limit it)
+int decode_fp8_resident(int D) {
+  return D == 64 ? configure_decode_fp8<64, Score::kNone>() : configure_decode_fp8<128, Score::kNone>();
+}
+
+}  // namespace dec
+}  // namespace lb
+
+extern "C" int lb_kv_append_fp8(const void* qkv, const float* cosv, const float* sinv, void* q_out, void* k_cache,
+                                void* v_cache, float* k_scale, float* v_scale, const int* seqlens, int B, int Sq, int G,
+                                int r, int C, int D, cudaStream_t s) {
+  const size_t warps = (size_t)B * Sq * G;
+  if (warps == 0) return 0;
+  if (D != 64 && D != 128) return -4;
+  const int threads = 256;
+  const int blocks = (int)((warps * 32 + threads - 1) / threads < 4096 ? (warps * 32 + threads - 1) / threads : 4096);
+  auto kern = D == 64 ? lb::dec::kv_append_fp8_kernel<64> : lb::dec::kv_append_fp8_kernel<128>;
+  kern<<<blocks, threads, 0, s>>>(static_cast<const __nv_bfloat16*>(qkv), cosv, sinv,
+                                  static_cast<__nv_bfloat16*>(q_out), static_cast<uint8_t*>(k_cache),
+                                  static_cast<uint8_t*>(v_cache), k_scale, v_scale, seqlens, B, Sq, G, r, C);
+  return (int)cudaGetLastError();
+}

@@ -37,6 +37,9 @@
 //   cache_seqlens[b], the new tokens not being in that cache.
 //   The kernel template lives in decode_attention_sm90.cuh; its ALiBi instances are compiled in
 //   decode_attention_alibi_sm90.cu and its T5 instances in decode_attention_t5_sm90.cu.
+//   FP8 (E4M3) caches (decode_attention_fp8_sm90.cu, with their quantizing append): K, V bytes with one fp32 scale per
+//   row; every score kind at both head dims, one bulk copy per tile and array, the scales folded into the scores and
+//   probabilities (Cfg8 and decode_attn_body in decode_attention_sm90.cuh).
 //   Known limit (docs/source/tutorials/get_started/Benchmark.md, "Decoding"): at large batches the kernel tops out near
 //   the same rate of key rows per second at both head dims (about 2.1 TB/s at 128, 1.0 TB/s at 64 on an H100), which
 //   points to the one bulk copy per row, not to HBM (not confirmed with a profiler).  Whole-tile TMA tensor-map loads
@@ -121,11 +124,13 @@ __global__ void kv_append_kernel(const __nv_bfloat16* __restrict__ qkv, const fl
 
 namespace {
 template <int D>
-cudaError_t launch_decode(const lb::dec::Params& p, int B, int nsplit, lb::dec::Score score, cudaStream_t s) {
+cudaError_t launch_decode(const lb::dec::Params& p, const float* k_scale, const float* v_scale, int B, int nsplit,
+                          lb::dec::Score score, cudaStream_t s) {
   using lb::dec::Score;
-  cudaError_t e = score == Score::kAlibi  ? lb::dec::launch_decode_attn_alibi(p, D, B, nsplit, s)
-                  : score == Score::kNone ? lb::dec::launch_decode_attn<D, Score::kNone>(p, B, nsplit, s)
-                                          : lb::dec::launch_decode_attn_t5(p, score, D, B, nsplit, s);
+  cudaError_t e = k_scale != nullptr      ? lb::dec::launch_decode_attn_fp8(p, k_scale, v_scale, score, D, B, nsplit, s)
+                  : score == Score::kAlibi ? lb::dec::launch_decode_attn_alibi(p, D, B, nsplit, s)
+                  : score == Score::kNone  ? lb::dec::launch_decode_attn<D, Score::kNone>(p, B, nsplit, s)
+                                           : lb::dec::launch_decode_attn_t5(p, score, D, B, nsplit, s);
   if (e != cudaSuccess) return e;
   if (nsplit > 1) lb::dec::decode_combine_kernel<D><<<dim3(p.G * p.row_blocks, B), 128, 0, s>>>(p, nsplit);
   return cudaGetLastError();
@@ -134,12 +139,14 @@ cudaError_t launch_decode(const lb::dec::Params& p, int B, int nsplit, lb::dec::
 
 // Number of key-range splits per (sample, cache head, row block): as many as fill the resident CTA slots of the GPU in
 // one wave (a second, partial wave would only add a tail), at most one split per 128 keys of the capacity.  `blocks` =
-// G * ceil(r * Sq / 16) CTAs per sample and split.  Depends on the shapes only, never on the current lengths.
-extern "C" int lb_decode_splits(int B, int blocks, int C, int D) {
+// G * ceil(r * Sq / 16) CTAs per sample and split, of the FP8 instances when `fp8`.  Depends on the shapes only, never
+// on the current lengths.
+extern "C" int lb_decode_splits(int B, int blocks, int C, int D, bool fp8) {
   // (the ALiBi and T5 instances hold as many CTAs per SM: the same shared memory, and registers that do not limit it)
   using lb::dec::Score;
-  const int resident =
-      D == 64 ? lb::dec::configure_decode<64, Score::kNone>() : lb::dec::configure_decode<128, Score::kNone>();
+  const int resident = fp8        ? lb::dec::decode_fp8_resident(D)
+                       : D == 64 ? lb::dec::configure_decode<64, Score::kNone>()
+                                 : lb::dec::configure_decode<128, Score::kNone>();
   int n = lb_host::num_sms() * (resident > 0 ? resident : 1) / (B * blocks);
   n = n < (C + 127) / 128 ? n : (C + 127) / 128;
   n = n < lb::dec::kMaxSplits ? n : lb::dec::kMaxSplits;
@@ -148,12 +155,14 @@ extern "C" int lb_decode_splits(int B, int blocks, int C, int D) {
 
 extern "C" int lb_decode_attn(const void* q, const long* q_strides, const void* k, const void* v, void* o,
                               float* part_o, float* part_ml, const int* seqlens, const int* kv_start,
-                              const float* alibi_slopes, const float* rel_bias, int R, bool causal, int B, int Sq,
-                              int A, int G, int C, int D, float scale, int nsplit, cudaStream_t s) {
+                              const float* alibi_slopes, const float* rel_bias, int R, bool causal,
+                              const float* k_scale, const float* v_scale, int B, int Sq, int A, int G, int C, int D,
+                              float scale, int nsplit, cudaStream_t s) {
   if (B == 0 || A == 0) return 0;
   if (G <= 0 || A % G) return -4;
   // the four kinds: no bias or ALiBi or T5's relative bias (causal), no bias (non-causal)
   if ((alibi_slopes != nullptr) + (rel_bias != nullptr) + !causal > 1 || (rel_bias != nullptr && R < 1)) return -5;
+  if ((k_scale != nullptr) != (v_scale != nullptr) || (k_scale != nullptr && C % 4)) return -6;
   lb::dec::Params p;
   p.q = static_cast<const __nv_bfloat16*>(q);
   p.q_sb = q_strides[0];
@@ -180,7 +189,8 @@ extern "C" int lb_decode_attn(const void* q, const long* q_strides, const void* 
                       : rel_bias != nullptr   ? Score::kRelBias
                       : !causal               ? Score::kWindow
                                               : Score::kNone;
-  cudaError_t e = D == 64 ? launch_decode<64>(p, B, nsplit, score, s) : launch_decode<128>(p, B, nsplit, score, s);
+  cudaError_t e = D == 64 ? launch_decode<64>(p, k_scale, v_scale, B, nsplit, score, s)
+                          : launch_decode<128>(p, k_scale, v_scale, B, nsplit, score, s);
   return (int)e;
 }
 

@@ -1,7 +1,13 @@
-// The split-KV decode attention kernel (documented in decode_attention_sm90.cu) and its launch.  Three translation units
-// instantiate it: decode_attention_sm90.cu without a score bias, decode_attention_alibi_sm90.cu with ALiBi slopes and
-// decode_attention_t5_sm90.cu with T5's relative-position bias or a non-causal key window.
+// The split-KV decode attention kernel (documented in decode_attention_sm90.cu) and its launch.  Four translation units
+// instantiate it: decode_attention_sm90.cu without a score bias, decode_attention_alibi_sm90.cu with ALiBi slopes,
+// decode_attention_t5_sm90.cu with T5's relative-position bias or a non-causal key window, and
+// decode_attention_fp8_sm90.cu every score kind over an FP8 (E4M3) cache.
 #pragma once
+#include <cuda_fp16.h>
+#include <cuda_fp8.h>
+
+#include <type_traits>
+
 #include "common.cuh"
 
 namespace lb {
@@ -20,6 +26,23 @@ struct Cfg {
   static constexpr int kStageElems = 2 * kTile * kRow;     // K tile, then V tile
   static constexpr int kRingBytes = kStages * kStageElems * 2;
   static constexpr int kMergeBytes = kWarps * kMaxQ * (D + 2) * 4;   // per-warp O, m, l for the merge
+  static constexpr int kSmem = (kRingBytes > kMergeBytes ? kRingBytes : kMergeBytes) + 2 * kStages * 8;
+};
+
+// FP8 (E4M3) caches: K, V bytes [B, G, C, D] and one fp32 scale per row, [B, G, C] (C a multiple of 4, so every
+// 4-row group of scales is 16-byte aligned).  A stage holds the window rows of one 64-key tile, each array loaded with
+// one bulk copy: K, V, and their scales from the 16-byte boundary at or below the tile's first row.  Each consumer
+// warp widens its own 16 keys of K and V to bf16 (exact) into a padded staging area of its own, read by the same
+// ldmatrix code as the bf16 ring.  Four / six stages: 100 / 69 KB, two / three CTAs per SM at D = 128 / 64.
+template <int D>
+struct Cfg8 {
+  static constexpr int kRow = D + 8;                                  // padded bf16 staging row (elements)
+  static constexpr int kStages = D == 128 ? 4 : 6;
+  static constexpr int kScales = kTile + 4;                           // floats of one scale array in a stage
+  static constexpr int kStageBytes = 2 * kTile * D + 2 * kScales * 4;  // K, V bytes, then K, V scales
+  static constexpr int kStagingBytes = kWarps * 2 * 16 * kRow * 2;    // per consumer warp: 16 keys of K, then of V
+  static constexpr int kRingBytes = kStages * kStageBytes + kStagingBytes;
+  static constexpr int kMergeBytes = Cfg<D>::kMergeBytes;
   static constexpr int kSmem = (kRingBytes > kMergeBytes ? kRingBytes : kMergeBytes) + 2 * kStages * 8;
 };
 
@@ -51,10 +74,23 @@ LB_DEVICE void bulk_load(void* dst, const void* src, uint32_t bytes, uint64_t* b
                "l"(src), "r"(bytes), "r"(smem_u32(bar))
                : "memory");
 }
-template <int D, Score S>
-__device__ __forceinline__ void decode_attn_body(const Params& p) {
+// e4m3 pair (low byte first) -> bf16 pair, exactly (every e4m3 value is an f16 and a bf16)
+LB_DEVICE uint32_t e4m3x2_to_bf16x2(uint16_t x) {
+  const __half2_raw h = __nv_cvt_fp8x2_to_halfraw2(static_cast<__nv_fp8x2_storage_t>(x), __NV_E4M3);
+  const float2 f = __half22float2(*reinterpret_cast<const __half2*>(&h));
+  return pack_bf16(f.x, f.y);
+}
+LB_DEVICE uint2 e4m3x4_to_bf16x4(uint32_t x) {
+  return make_uint2(e4m3x2_to_bf16x2(static_cast<uint16_t>(x)), e4m3x2_to_bf16x2(static_cast<uint16_t>(x >> 16)));
+}
+
+// FP8: p.k / p.v point at the E4M3 bytes and k_scale / v_scale at their row scales; key j's score is
+// scale·s^k_j·(q·ê_j), and P·V runs on P_j·s^v_j while the softmax sums P_j.
+template <int D, Score S, bool FP8 = false>
+__device__ __forceinline__ void decode_attn_body(const Params& p, const float* k_scale = nullptr,
+                                                 const float* v_scale = nullptr) {
   constexpr bool ALIBI = S == Score::kAlibi;
-  using C = Cfg<D>;
+  using C = std::conditional_t<FP8, Cfg8<D>, Cfg<D>>;
   extern __shared__ __align__(128) unsigned char smem[];
   __nv_bfloat16* ring = reinterpret_cast<__nv_bfloat16*>(smem);
   uint64_t* full = reinterpret_cast<uint64_t*>(smem + (C::kRingBytes > C::kMergeBytes ? C::kRingBytes : C::kMergeBytes));
@@ -92,22 +128,42 @@ __device__ __forceinline__ void decode_attn_body(const Params& p) {
   const int r0 = lane >> 2, c0 = (lane & 3) * 2;
 
   if (warp == kWarps) {
-    // producer: rows past the window repeat its last row (finite data; those keys get zero weight)
-    const __nv_bfloat16* kg = p.k + head_off;
-    const __nv_bfloat16* vg = p.v + head_off;
-    for (int t = 0; t < my; ++t) {
-      const int st = t % C::kStages;
-      if (t >= C::kStages) mbar_wait(&empty[st], ((t / C::kStages) & 1) ^ 1);
-      if (lane == 0) mbar_arrive_expect_tx(&full[st], 2 * kTile * D * 2);
-      __syncwarp();
-      __nv_bfloat16* sk = ring + st * C::kStageElems;
-      __nv_bfloat16* sv = sk + kTile * C::kRow;
-      const int base = lo + (t0 + t) * kTile;
-#pragma unroll
-      for (int r = lane; r < kTile; r += 32) {
-        const long row = min(base + r, hi - 1);
-        bulk_load(sk + r * C::kRow, kg + row * D, D * 2, &full[st]);
-        bulk_load(sv + r * C::kRow, vg + row * D, D * 2, &full[st]);
+    if constexpr (FP8) {
+      // producer: the window rows of each tile (clipped at hi) and their scales; nothing past the window is copied
+      const uint8_t* kg = reinterpret_cast<const uint8_t*>(p.k) + head_off;
+      const uint8_t* vg = reinterpret_cast<const uint8_t*>(p.v) + head_off;
+      const long srow = ((long)b * p.G + kvh) * p.C;
+      const int soff = lo & 3;   // first row of every tile past its 16-byte scale boundary
+      for (int t = 0; t < my && lane == 0; ++t) {
+        const int st = t % C::kStages;
+        if (t >= C::kStages) mbar_wait(&empty[st], ((t / C::kStages) & 1) ^ 1);
+        const int base = lo + (t0 + t) * kTile;
+        const int n = min(kTile, hi - base), ns = (soff + n + 3) & ~3;
+        unsigned char* sk = smem + st * C::kStageBytes;
+        mbar_arrive_expect_tx(&full[st], 2 * n * D + 2 * ns * 4);
+        bulk_load(sk, kg + (long)base * D, n * D, &full[st]);
+        bulk_load(sk + kTile * D, vg + (long)base * D, n * D, &full[st]);
+        bulk_load(sk + 2 * kTile * D, k_scale + srow + base - soff, ns * 4, &full[st]);
+        bulk_load(sk + 2 * kTile * D + C::kScales * 4, v_scale + srow + base - soff, ns * 4, &full[st]);
+      }
+    } else {
+      // producer: rows past the window repeat its last row (finite data; those keys get zero weight)
+      const __nv_bfloat16* kg = p.k + head_off;
+      const __nv_bfloat16* vg = p.v + head_off;
+      for (int t = 0; t < my; ++t) {
+        const int st = t % C::kStages;
+        if (t >= C::kStages) mbar_wait(&empty[st], ((t / C::kStages) & 1) ^ 1);
+        if (lane == 0) mbar_arrive_expect_tx(&full[st], 2 * kTile * D * 2);
+        __syncwarp();
+        __nv_bfloat16* sk = ring + st * C::kStageElems;
+        __nv_bfloat16* sv = sk + kTile * C::kRow;
+        const int base = lo + (t0 + t) * kTile;
+  #pragma unroll
+        for (int r = lane; r < kTile; r += 32) {
+          const long row = min(base + r, hi - 1);
+          bulk_load(sk + r * C::kRow, kg + row * D, D * 2, &full[st]);
+          bulk_load(sv + r * C::kRow, vg + row * D, D * 2, &full[st]);
+        }
       }
     }
   } else if (my > 0) {
@@ -147,14 +203,59 @@ __device__ __forceinline__ void decode_attn_body(const Params& p) {
       }
     }
     const int kw = warp * 16;
+    const int kr = FP8 ? 0 : kw;   // the first of this warp's keys among the rows ldmatrix reads (FP8: its staging)
     // ldmatrix lane addresses: K (non-transposed: keys = rows of the B fragment), V (transposed)
-    const int k_row = kw + (lane & 7) + ((lane >> 4) << 3), k_col = ((lane >> 3) & 1) * 8;
-    const int v_row = kw + (lane & 7) + (((lane >> 3) & 1) << 3), v_col = (lane >> 4) * 8;
+    const int k_row = kr + (lane & 7) + ((lane >> 4) << 3), k_col = ((lane >> 3) & 1) * 8;
+    const int v_row = kr + (lane & 7) + (((lane >> 3) & 1) << 3), v_col = (lane >> 4) * 8;
     for (int t = 0; t < my; ++t) {
       const int st = t % C::kStages;
       mbar_wait(&full[st], (t / C::kStages) & 1);
-      const __nv_bfloat16* sk = ring + st * C::kStageElems;
-      const __nv_bfloat16* sv = sk + kTile * C::kRow;
+      const __nv_bfloat16* sk;
+      const __nv_bfloat16* sv;
+      float ksc[2][2], vsc[2][2];   // FP8: the scales of this thread's keys kw + n * 8 + c0 + e (0 past the window)
+      if constexpr (FP8) {
+        const unsigned char* stage = smem + st * C::kStageBytes;
+        __nv_bfloat16* stg = reinterpret_cast<__nv_bfloat16*>(smem + C::kStages * C::kStageBytes) +
+                             warp * 2 * 16 * C::kRow;
+        const int first = lo + (t0 + t) * kTile + kw;   // this warp's first key
+        __syncwarp();   // the previous tile's ldmatrix reads of the staging area are done
+        // widen 16 bytes per lane and step: rows past the window become zeros (the bytes there were not copied)
+#pragma unroll
+        for (int c = lane; c < D; c += 32) {   // 16 rows of D / 16 chunks
+          const int r = c / (D / 16), col = (c % (D / 16)) * 16;
+          const bool in = first + r < hi;
+          const uint4 kx = in ? *reinterpret_cast<const uint4*>(stage + (kw + r) * D + col) : make_uint4(0, 0, 0, 0);
+          const uint4 vx = in ? *reinterpret_cast<const uint4*>(stage + kTile * D + (kw + r) * D + col)
+                              : make_uint4(0, 0, 0, 0);
+          uint4* dk = reinterpret_cast<uint4*>(stg + r * C::kRow + col);
+          uint4* dv = reinterpret_cast<uint4*>(stg + (16 + r) * C::kRow + col);
+          const uint2 k0 = e4m3x4_to_bf16x4(kx.x), k1 = e4m3x4_to_bf16x4(kx.y), k2 = e4m3x4_to_bf16x4(kx.z),
+                      k3 = e4m3x4_to_bf16x4(kx.w);
+          dk[0] = make_uint4(k0.x, k0.y, k1.x, k1.y);
+          dk[1] = make_uint4(k2.x, k2.y, k3.x, k3.y);
+          const uint2 v0 = e4m3x4_to_bf16x4(vx.x), v1 = e4m3x4_to_bf16x4(vx.y), v2 = e4m3x4_to_bf16x4(vx.z),
+                      v3 = e4m3x4_to_bf16x4(vx.w);
+          dv[0] = make_uint4(v0.x, v0.y, v1.x, v1.y);
+          dv[1] = make_uint4(v2.x, v2.y, v3.x, v3.y);
+        }
+        const float* ks = reinterpret_cast<const float*>(stage + 2 * kTile * D) + (lo & 3) + kw;
+        const float* vs = ks + C::kScales;
+#pragma unroll
+        for (int n = 0; n < 2; ++n)
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            const int k = n * 8 + c0 + e;
+            ksc[n][e] = first + k < hi ? ks[k] : 0.f;
+            vsc[n][e] = first + k < hi ? vs[k] : 0.f;
+          }
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&empty[st]);   // this warp is done with the stage: the producer may refill it
+        sk = stg;
+        sv = stg + 16 * C::kRow;
+      } else {
+        sk = ring + st * C::kStageElems;
+        sv = sk + kTile * C::kRow;
+      }
       float s[2][4] = {{0.f, 0.f, 0.f, 0.f}, {0.f, 0.f, 0.f, 0.f}};
 #pragma unroll
       for (int ks = 0; ks < D / 16; ++ks) {
@@ -172,6 +273,7 @@ __device__ __forceinline__ void decode_attn_body(const Params& p) {
         for (int j = 0; j < 4; ++j) {
           const int key = key0 + n * 8 + (j & 1);
           const bool vis = key < hi && key <= lim[j >> 1];
+          if constexpr (FP8) s[n][j] *= ksc[n][j & 1];
           if constexpr (ALIBI) {   // key − lim is a non-positive integer of at most the capacity: exact in fp32
             s[n][j] = vis ? fmaf(slope2[j >> 1], static_cast<float>(key - lim[j >> 1]), s[n][j] * p.scale_log2)
                           : -INFINITY;
@@ -204,8 +306,13 @@ __device__ __forceinline__ void decode_attn_body(const Params& p) {
         const float p2 = fast_exp2(s[n][2] - base[1]), p3 = fast_exp2(s[n][3] - base[1]);
         l[0] += p0 + p1;
         l[1] += p2 + p3;
-        pa[2 * n] = pack_bf16(p0, p1);
-        pa[2 * n + 1] = pack_bf16(p2, p3);
+        if constexpr (FP8) {
+          pa[2 * n] = pack_bf16(p0 * vsc[n][0], p1 * vsc[n][1]);
+          pa[2 * n + 1] = pack_bf16(p2 * vsc[n][0], p3 * vsc[n][1]);
+        } else {
+          pa[2 * n] = pack_bf16(p0, p1);
+          pa[2 * n + 1] = pack_bf16(p2, p3);
+        }
       }
 #pragma unroll
       for (int n = 0; n < D / 8; ++n) {
@@ -221,8 +328,10 @@ __device__ __forceinline__ void decode_attn_body(const Params& p) {
         mma_bf16(o[2 * j], pa, bv[0], bv[1]);
         mma_bf16(o[2 * j + 1], pa, bv[2], bv[3]);
       }
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&empty[st]);
+      if constexpr (!FP8) {
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&empty[st]);
+      }
     }
 #pragma unroll
     for (int r = 0; r < 2; ++r) {
@@ -321,6 +430,11 @@ cudaError_t launch_decode_attn(const Params& p, int B, int nsplit, cudaStream_t 
 cudaError_t launch_decode_attn_alibi(const Params& p, int D, int B, int nsplit, cudaStream_t s);
 // the T5 instances (decode_attention_t5_sm90.cu): S is kRelBias or kWindow, D is 64 or 128
 cudaError_t launch_decode_attn_t5(const Params& p, Score S, int D, int B, int nsplit, cudaStream_t s);
+// the FP8 instances (decode_attention_fp8_sm90.cu): every score kind, D is 64 or 128
+cudaError_t launch_decode_attn_fp8(const Params& p, const float* k_scale, const float* v_scale, Score S, int D, int B,
+                                   int nsplit, cudaStream_t s);
+// CTAs per SM of the FP8 instances at head dim D (0 when the shared memory opt-in failed)
+int decode_fp8_resident(int D);
 
 }  // namespace dec
 }  // namespace lb

@@ -126,13 +126,18 @@ long lb_attn_bwd_accum_floats(int B, int A, int Sq, int D);
 int lb_bias_dropout_residual(const void* x, const void* bias, const void* res, void* y, long rows, int N, float p,
                              const lb::RngArgs* rng, const long long* rng_in, long long* rng_out, cudaStream_t s);
 int lb_spin_timeout_report(char* buf, int n);
-int lb_decode_splits(int B, int blocks, int C, int D);
+int lb_decode_splits(int B, int blocks, int C, int D, bool fp8);
+// k_scale, v_scale (fp32 [B, G, C], C a multiple of 4): k and v are an FP8 (E4M3) cache with these row scales
 int lb_decode_attn(const void* q, const long* q_strides, const void* k, const void* v, void* o, float* part_o,
                    float* part_ml, const int* seqlens, const int* kv_start, const float* alibi_slopes,
-                   const float* rel_bias, int R, bool causal, int B, int Sq, int A, int G, int C, int D, float scale,
-                   int nsplit, cudaStream_t s);
+                   const float* rel_bias, int R, bool causal, const float* k_scale, const float* v_scale, int B, int Sq,
+                   int A, int G, int C, int D, float scale, int nsplit, cudaStream_t s);
 int lb_kv_append(const void* qkv, const float* cosv, const float* sinv, void* q_out, void* k_cache, void* v_cache,
                  const int* seqlens, int B, int Sq, int G, int r, int C, int D, cudaStream_t s);
+// lb_kv_append into an FP8 (E4M3) cache: each k and v row is stored as bytes [B, G, C, D] and an fp32 scale [B, G, C]
+int lb_kv_append_fp8(const void* qkv, const float* cosv, const float* sinv, void* q_out, void* k_cache, void* v_cache,
+                     float* k_scale, float* v_scale, const int* seqlens, int B, int Sq, int G, int r, int C, int D,
+                     cudaStream_t s);
 int lb_window_attn_groups(int B, int H, int W, int ws, int heads);
 int lb_window_attn_fwd(const void* qkv, void* out, float* lse, const float* table, const float* tau, int B, int H, int W,
                        int ws, int shift, int heads, int d, float scale, cudaStream_t s);

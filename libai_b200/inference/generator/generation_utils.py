@@ -22,7 +22,7 @@ import torch
 from libai_b200.utils import distributed as dutil
 import torch.distributed as dist
 
-from ..kv_cache import StaticKVCache
+from ..kv_cache import KVCacheOwner, StaticKVCache
 from .generation_beam_search import BeamScorer, BeamSearchScorer
 from .generation_logits_processor import (
     EncoderNoRepeatNGramLogitsProcessor,
@@ -58,7 +58,17 @@ _DEFAULTS = dict(
     num_return_sequences=1, output_scores=False, use_cache=True, bos_token_id=None, eos_token_id=None,
     pad_token_id=None, decoder_start_token_id=None, forced_bos_token_id=None, forced_eos_token_id=None,
     remove_invalid_values=False, exponential_decay_length_penalty=None, chunk_size_feed_forward=0,
+    kv_cache_dtype=None,
 )
+
+
+def _kv_cache_dtype(value):
+    """``generate(kv_cache_dtype=...)``: None (the weights' dtype), or ``"fp8"`` / ``torch.float8_e4m3fn``."""
+    if value is None or value == torch.float8_e4m3fn:
+        return value
+    if isinstance(value, str) and value.lower() == "fp8":
+        return torch.float8_e4m3fn
+    raise ValueError(f"kv_cache_dtype must be None, 'fp8' or torch.float8_e4m3fn, got {value!r}")
 
 
 class Generator:
@@ -483,7 +493,16 @@ class Generator:
                  num_beam_groups=None, diversity_penalty=None, prefix_allowed_tokens_fn=None, logits_processor=None,
                  renormalize_logits=None, stopping_criteria=None, constraints=None, output_scores=None,
                  forced_bos_token_id=None, forced_eos_token_id=None, remove_invalid_values=None,
-                 exponential_decay_length_penalty=None, **model_kwargs):
+                 exponential_decay_length_penalty=None, kv_cache_dtype=None, **model_kwargs):
+        """``kv_cache_dtype`` (default: the model cfg's ``kv_cache_dtype``): ``"fp8"`` or ``torch.float8_e4m3fn`` holds
+        the preallocated KV cache as E4M3 rows with per-row scales
+        (:class:`~libai_b200.inference.kv_cache.StaticKVCache`) for this call: about half the memory, and of the bytes
+        each decoding step reads, for 8-bit keys and values.
+        None keeps the weights' dtype.  A model that does not decode on a ``StaticKVCache`` raises ``ValueError``."""
+        kv_cache_dtype = _kv_cache_dtype(self._pick(kv_cache_dtype, "kv_cache_dtype"))
+        if kv_cache_dtype is not None and not isinstance(self, KVCacheOwner):
+            raise ValueError(f"kv_cache_dtype={kv_cache_dtype}: {type(self).__name__} does not decode on a "
+                             "StaticKVCache")
         self._validate_model_kwargs(model_kwargs.copy())
         logits_processor = logits_processor if logits_processor is not None else LogitsProcessorList()
         stopping_criteria = stopping_criteria if stopping_criteria is not None else StoppingCriteriaList()
@@ -561,15 +580,19 @@ class Generator:
             renormalize_logits=renormalize_logits,
         )
         stopping_criteria = self._get_stopping_criteria(max_length, max_time, stopping_criteria)
-        # models with a preallocated cache size it once for every sequence the search runs
-        allocate = getattr(self, "allocate_kv_cache", None)
-        if allocate is not None and model_kwargs.get("use_cache") and stopping_criteria.max_length is not None:
-            rows = batch_size * (num_beams if is_beam else num_return_sequences if is_sample else 1)
-            allocate(rows, stopping_criteria.max_length)
-
+        saved_kv_cache_dtype = getattr(self, "kv_cache_dtype", None)
         was_training = self.training
         self.eval()
         try:
+            if kv_cache_dtype is not None:   # the cache format of this call (allocate_kv_cache reads it)
+                self.kv_cache_dtype = kv_cache_dtype
+            # models with a preallocated cache size it once for every sequence the search runs
+            allocate = getattr(self, "allocate_kv_cache", None)
+            if allocate is not None and model_kwargs.get("use_cache") and stopping_criteria.max_length is not None:
+                rows = batch_size * (num_beams if is_beam else num_return_sequences if is_sample else 1)
+                if allocate(rows, stopping_criteria.max_length) is None and kv_cache_dtype is not None:
+                    raise ValueError(f"kv_cache_dtype={kv_cache_dtype}: {type(self).__name__} keeps a tuple cache "
+                                     "here (pipeline-parallel inference), not a StaticKVCache")
             if is_greedy:
                 if num_return_sequences > 1:
                     raise ValueError(f"num_return_sequences has to be 1, but is {num_return_sequences} when doing greedy search.")
@@ -601,3 +624,5 @@ class Generator:
             raise NotImplementedError("beam sampling is not supported (neither is it in the reference)")
         finally:
             self.train(was_training)
+            if kv_cache_dtype is not None:
+                self.kv_cache_dtype = saved_kv_cache_dtype

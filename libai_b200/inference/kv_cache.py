@@ -7,6 +7,11 @@ rank's local ones).  New tokens are written in place at rows ``seqlens[b] + i``
 step copies nothing but the new rows.  ``seqlens`` and ``kv_start`` (the left padding of each sample) are int32 device
 tensors read inside the kernels; ``length`` is their host-side mirror (every sample holds the same number of rows, the
 left padding included), which sizes the windows and decides when the buffers must grow.
+
+With ``kv_dtype=torch.float8_e4m3fn`` the K and V buffers hold E4M3 bytes and each row has an fp32 scale,
+``k_scale`` / ``v_scale`` ``[batch, heads, capacity]`` (the format of :func:`OF.kv_cache_quantize_ref`): about half the
+bytes of a bf16 cache, at the accuracy of a per-row 8-bit float.  Every attention over such a cache is the attention
+over its dequantized rows.  It is a user's choice (``generate(kv_cache_dtype="fp8")``), never made for them.
 """
 from __future__ import annotations
 
@@ -93,6 +98,14 @@ class KVCacheLayer:
         return self.cache.v[self.idx]
 
     @property
+    def k_scale(self) -> Optional[torch.Tensor]:
+        return self.cache.k_scale[self.idx]
+
+    @property
+    def v_scale(self) -> Optional[torch.Tensor]:
+        return self.cache.v_scale[self.idx]
+
+    @property
     def seqlens(self) -> torch.Tensor:
         return self.cache.seqlens
 
@@ -108,10 +121,18 @@ class KVCacheLayer:
         """Write k, v of the packed projection ``qkv`` (per-head ``[b, s, a, 3d]`` or grouped ``[b, s, g, r + 2, d]``) at
         rows ``seqlens[b] + i`` (:func:`OF.kv_cache_append`, rotated by ``cos/sin`` when given); returns q ``[b, s, a,
         d]``.  A per-head projection without rotary hands q back as its strided view: nothing needs writing."""
+        scales = {} if self.k_scale is None else {"k_scale": self.k_scale, "v_scale": self.v_scale}
         if cos is None and qkv.dim() == 4:
-            OF.kv_cache_append(qkv, self.k, self.v, self.seqlens, return_q=False)
+            OF.kv_cache_append(qkv, self.k, self.v, self.seqlens, return_q=False, **scales)
             return qkv[..., : qkv.shape[-1] // 3]
-        return OF.kv_cache_append(qkv, self.k, self.v, self.seqlens, cos, sin)
+        return OF.kv_cache_append(qkv, self.k, self.v, self.seqlens, cos, sin, **scales)
+
+    def window(self, L: int, dtype) -> Tuple[torch.Tensor, torch.Tensor]:
+        """K and V rows ``[:L]``: views of the buffers, or of an FP8 cache its rows dequantized to ``dtype``."""
+        if self.k_scale is None:
+            return self.k[:, :, :L], self.v[:, :, :L]
+        return (OF.kv_cache_dequant(self.k[:, :, :L], self.k_scale[:, :, :L], dtype),
+                OF.kv_cache_dequant(self.v[:, :, :L], self.v_scale[:, :, :L], dtype))
 
     def attend(self, q: torch.Tensor, *, scale: float, causal: bool = True, mask=None, bias=None, alibi_slopes=None,
                rel_bias=None, dropout_p: float = 0.0, training: bool = False) -> torch.Tensor:
@@ -125,35 +146,49 @@ class KVCacheLayer:
         - the causal prefill of an empty cache without ``rel_bias``: the flash kernel over ``[:s]``, the prompt's left
           padding in ``kv_start``;
         - anything else: :func:`OF.decode_attention` (the split-KV kernel up to 16 new tokens, the flash kernel over
-          the cache window beyond)."""
+          the cache window beyond).
+
+        The first two read an FP8 cache's window dequantized to q's dtype; the decode kernel reads its bytes."""
         past = self.length
         if mask is not None or bias is not None:
             L = past + q.shape[1] if causal else past
-            ctx = OF.attention(q.transpose(1, 2), self.k[:, :, :L], self.v[:, :, :L], causal=False, scale=scale,
-                               mask=mask, bias=bias, dropout_p=dropout_p, training=training)
+            k, v = self.window(L, q.dtype)
+            ctx = OF.attention(q.transpose(1, 2), k, v, causal=False, scale=scale, mask=mask, bias=bias,
+                               dropout_p=dropout_p, training=training)
             return ctx.transpose(1, 2)
         if causal and past == 0 and rel_bias is None:
-            s_len = q.shape[1]
-            query, key = q.transpose(1, 2), self.k[:, :, :s_len]
+            query, (key, value) = q.transpose(1, 2), self.window(q.shape[1], q.dtype)
             kv_start = self.kv_start if OF.attention_supported(query, key) else None
-            ctx = OF.attention(query, key, self.v[:, :, :s_len], causal=True, scale=scale, alibi_slopes=alibi_slopes,
+            ctx = OF.attention(query, key, value, causal=True, scale=scale, alibi_slopes=alibi_slopes,
                                kv_start=kv_start, dropout_p=dropout_p, training=training)
             return ctx.transpose(1, 2)
+        scales = {} if self.k_scale is None else {"k_scale": self.k_scale, "v_scale": self.v_scale}
         return OF.decode_attention(q, self.k, self.v, self.seqlens, self.kv_start, scale=scale, past=past,
-                                   alibi_slopes=alibi_slopes, rel_bias=rel_bias, causal=causal)
+                                   alibi_slopes=alibi_slopes, rel_bias=rel_bias, causal=causal, **scales)
 
 
 class StaticKVCache:
+    """``dtype``: the dtype of the projections the cache serves; ``kv_dtype``: what the buffers hold (default
+    ``dtype``; ``torch.float8_e4m3fn``: E4M3 rows with fp32 row scales, the capacity then a multiple of 4)."""
+
     def __init__(self, num_layers: int, batch: int, heads: int, head_dim: int, capacity: int,
-                 dtype=torch.bfloat16, device=None, layers: Optional[Iterable[int]] = None):
+                 dtype=torch.bfloat16, device=None, layers: Optional[Iterable[int]] = None, kv_dtype=None):
         self.num_layers, self.batch, self.heads, self.head_dim = num_layers, batch, heads, head_dim
         self.dtype, self.device = dtype, torch.device(device) if device is not None else torch.device("cpu")
+        self.kv_dtype = dtype if kv_dtype is None else kv_dtype
+        if self.kv_dtype not in (dtype, torch.float8_e4m3fn):
+            raise ValueError(f"kv_dtype must be the projections' {dtype} or torch.float8_e4m3fn, got {kv_dtype}")
+        self.fp8 = self.kv_dtype == torch.float8_e4m3fn
         self.owned = sorted(range(num_layers) if layers is None else layers)
-        self.capacity = max(int(capacity), 1)
+        self.capacity = self._rounded(max(int(capacity), 1))
         self.k: List[Optional[torch.Tensor]] = [None] * num_layers
         self.v: List[Optional[torch.Tensor]] = [None] * num_layers
+        self.k_scale: List[Optional[torch.Tensor]] = [None] * num_layers   # FP8: the row scales
+        self.v_scale: List[Optional[torch.Tensor]] = [None] * num_layers
         for i in self.owned:
             self.k[i], self.v[i] = self._buffer(self.capacity), self._buffer(self.capacity)
+            if self.fp8:
+                self.k_scale[i], self.v_scale[i] = self._scales(self.capacity), self._scales(self.capacity)
         self.seqlens = torch.zeros(batch, dtype=torch.int32, device=self.device)
         self.kv_start = torch.zeros(batch, dtype=torch.int32, device=self.device)
         self.length = 0
@@ -161,20 +196,44 @@ class StaticKVCache:
 
     def _buffer(self, capacity):
         # uninitialised: the attention reads rows below the current length only (the decode kernel repeats the last
-        # row of the window to fill its last tile), and every such row has been written by an append
-        return torch.empty(self.batch, self.heads, capacity, self.head_dim, dtype=self.dtype, device=self.device)
+        # row of the window to fill its last tile; over an FP8 cache it zeroes them), and every such row has been
+        # written by an append
+        return torch.empty(self.batch, self.heads, capacity, self.head_dim, dtype=self.kv_dtype, device=self.device)
+
+    def _scales(self, capacity):
+        return torch.empty(self.batch, self.heads, capacity, dtype=torch.float32, device=self.device)
+
+    def _rounded(self, capacity: int) -> int:
+        # the decode kernel loads the scales of a tile from a 16-byte boundary of their row
+        return -(-capacity // 4) * 4 if self.fp8 else capacity
 
     def layer(self, i: int) -> KVCacheLayer:
         return KVCacheLayer(self, i)
 
-    def matches(self, batch: int, dtype, device) -> bool:
-        return self.batch == batch and self.dtype == dtype and self.device == torch.device(device)
+    def matches(self, batch: int, dtype, device, kv_dtype=None) -> bool:
+        """Whether this cache serves ``batch`` sequences of ``dtype`` projections on ``device`` and holds ``kv_dtype``
+        rows (default ``dtype``)."""
+        return (self.batch == batch and self.dtype == dtype and self.device == torch.device(device)
+                and self.kv_dtype == (dtype if kv_dtype is None else kv_dtype))
 
     def flash_attention(self) -> bool:
-        """True when :func:`OF.attention` over the buffers runs the flash kernels, which take a left-padded prompt's
-        padding from ``kv_start``; the reference math needs a dense mask for it."""
+        """True when :func:`OF.attention` over the buffers (an FP8 cache's dequantized to ``dtype``) runs the flash
+        kernels, which take a left-padded prompt's padding from ``kv_start``; the reference math needs a dense mask for
+        it."""
         k = self.k[self.owned[0]]
+        if self.fp8:
+            k = torch.empty((self.batch, self.heads, 1, self.head_dim), dtype=self.dtype, device=self.device)
         return OF.attention_supported(k, k)
+
+    def write_rows(self, i: int, k: torch.Tensor, v: torch.Tensor, row0: int = 0) -> None:
+        """Write ``k``, ``v`` ``[batch, heads, n, head_dim]`` at rows ``row0 .. row0 + n`` of layer ``i`` (an FP8 cache
+        quantizes them by :func:`OF.kv_cache_quantize_ref`).  The lengths are the caller's to advance."""
+        n = k.shape[2]
+        for buf, scale, x in ((self.k, self.k_scale, k), (self.v, self.v_scale, v)):
+            if self.fp8:
+                buf[i][:, :, row0 : row0 + n], scale[i][:, :, row0 : row0 + n] = OF.kv_cache_quantize_ref(x)
+            else:
+                buf[i][:, :, row0 : row0 + n] = x
 
     def step_needs_dense_mask(self, attention_mask: Optional[torch.Tensor], *, flash: bool,
                               kv_start_ok: bool = True) -> bool:
@@ -211,8 +270,7 @@ class StaticKVCache:
             self.seqlens.copy_(window[1])
         self.length = S
         for i, (k, v) in enumerate(kv):
-            self.k[i][:, :, :S] = k
-            self.v[i][:, :, :S] = v
+            self.write_rows(i, k, v)
 
     def reserve(self, n: int) -> None:
         """Make room for ``n`` more rows: the buffers are reallocated at twice their capacity (or more, when needed) and
@@ -220,10 +278,13 @@ class StaticKVCache:
         need = self.length + n
         if need <= self.capacity:
             return
-        cap = max(2 * self.capacity, need)
+        cap = self._rounded(max(2 * self.capacity, need))
         for i in self.owned:
-            for bufs in (self.k, self.v):
-                new = self._buffer(cap)
+            for bufs, alloc in ((self.k, self._buffer), (self.v, self._buffer), (self.k_scale, self._scales),
+                                (self.v_scale, self._scales)):
+                if bufs[i] is None:
+                    continue
+                new = alloc(cap)
                 new[:, :, : self.length] = bufs[i][:, :, : self.length]
                 bufs[i] = new
         self.capacity = cap
@@ -238,8 +299,9 @@ class StaticKVCache:
         idx = beam_idx.to(device=self.device, dtype=torch.long)
         L = self.length
         for i in self.owned:
-            for buf in (self.k[i], self.v[i]):
-                buf[:, :, :L] = buf[:, :, :L].index_select(0, idx)
+            for buf in (self.k[i], self.v[i], self.k_scale[i], self.v_scale[i]):
+                if buf is not None:
+                    buf[:, :, :L] = buf[:, :, :L].index_select(0, idx)
         self.seqlens.copy_(self.seqlens.index_select(0, idx))
         self.kv_start.copy_(self.kv_start.index_select(0, idx))
 
@@ -258,6 +320,8 @@ class KVCacheOwner:
 
     kv_cache: Optional[StaticKVCache] = None
     past_length = 0
+    kv_cache_dtype = None   # what the cache holds: None = the weights' dtype; torch.float8_e4m3fn = FP8 rows
+
 
     def _cache_attention_modules(self) -> list:
         raise NotImplementedError
@@ -274,9 +338,10 @@ class KVCacheOwner:
         owned = [i for i in range(len(mods)) if topo.owns_layer(i)]   # this pipeline stage's layers
         w = mods[0].query_key_value.weight
         c = self.kv_cache
-        if c is None or not c.matches(batch, w.dtype, w.device) or c.capacity < max_length:
+        if c is None or not c.matches(batch, w.dtype, w.device, self.kv_cache_dtype) or c.capacity < max_length:
             heads = getattr(mods[0], "local_kv_heads", mods[0].local_heads)
-            c = StaticKVCache(len(mods), batch, heads, mods[0].head_size, max_length, w.dtype, w.device, owned)
+            c = StaticKVCache(len(mods), batch, heads, mods[0].head_size, max_length, w.dtype, w.device, owned,
+                              self.kv_cache_dtype)
         c.reset()
         self.kv_cache, self.past_length = c, 0
         return c

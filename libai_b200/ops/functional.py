@@ -829,33 +829,69 @@ def window_attention(qkv, *, H: int, W: int, window: int, shift: int, heads: int
 # (int32 [b]) is the number of rows already held, ``kv_start`` (int32 [b]) the left padding of each sample
 # --------------------------------------------------------------------------------------
 def _decode_native(x, k_cache) -> bool:
-    """The decode kernels take bf16 projections and caches with head dim 64 or 128; other dtypes and head dims run the
-    reference math (as :func:`attention` does)."""
+    """The decode kernels take bf16 projections and bf16 or FP8 (E4M3, with row scales) caches with head dim 64 or
+    128; other dtypes and head dims run the reference math (as :func:`attention` does)."""
     return (
         use_native(x)
         and x.dtype == torch.bfloat16
-        and k_cache.dtype == torch.bfloat16
+        and k_cache.dtype in (torch.bfloat16, torch.float8_e4m3fn)
         and k_cache.shape[-1] in (64, 128)
     )
 
 
-def kv_cache_append(qkv, k_cache, v_cache, cache_seqlens, cos=None, sin=None, return_q: bool = True):
+# FP8 (E4M3) caches hold each row x (the bf16 row a bf16 cache would hold) as the bytes e4m3_rn_satfinite(x / s) and
+# the fp32 scale s = amax|x| / 448 (1 for a zero row), ``k_scale`` / ``v_scale`` [b, g, C]; a row reads back as
+# float(e)·s.  The decode kernel folds the scales into its scores and probabilities; every other path attends over the
+# window dequantized to the projection's dtype.
+E4M3_MAX = 448.0
+
+
+def kv_cache_quantize_ref(x):
+    """``(e, s)``: the E4M3 bytes (``float8_e4m3fn``, ``x``'s shape) and fp32 row scales (``x.shape[:-1]``) of the rows
+    of ``x`` by the rule above — bit for bit what the append kernel stores for the same bf16 rows."""
+    xf = x.float()
+    amax = xf.abs().amax(dim=-1)
+    # (a tensor divisor: PyTorch's CUDA division by a Python scalar multiplies by its rounded reciprocal)
+    s = torch.where(amax == 0, torch.ones_like(amax), amax / torch.full_like(amax, E4M3_MAX))
+    return (xf / s[..., None]).to(torch.float8_e4m3fn), s
+
+
+def kv_cache_dequant(e, s, dtype=torch.bfloat16):
+    """The rows ``float(e)·s`` of FP8 bytes ``e`` and their scales ``s``, rounded to ``dtype``."""
+    return (e.float() * s[..., None]).to(dtype)
+
+
+def _check_scales(k_cache, k_scale, v_scale):
+    if k_cache.dtype == torch.float8_e4m3fn:
+        if k_scale is None or v_scale is None:
+            raise ValueError("an FP8 cache needs k_scale and v_scale")
+    elif k_scale is not None or v_scale is not None:
+        raise ValueError(f"k_scale and v_scale belong to an FP8 cache, not a {k_cache.dtype} one")
+
+
+def kv_cache_append(qkv, k_cache, v_cache, cache_seqlens, cos=None, sin=None, return_q: bool = True, k_scale=None,
+                    v_scale=None):
     """Write k, v of the packed projection ``qkv`` (``[b, s, a, 3d]``, or grouped ``[b, s, g, r + 2, d]``) into rows
     ``cache_seqlens[b] + i`` of the caches ``[b, g, C, d]``.  With
     ``cos/sin`` (fp32 ``[positions, d]``) q and k are first rotated at those positions, exactly as
     :func:`apply_rotary_qkv` with ``pos_offset = cache_seqlens[b]`` does.  Returns q ``[b, s, a, d]`` (rotated when the
-    tables are given) when ``return_q``, else None."""
+    tables are given) when ``return_q``, else None.  FP8 caches (``float8_e4m3fn``) take their row scales ``k_scale``,
+    ``v_scale`` (fp32 ``[b, g, C]``) and store each row quantized (:func:`kv_cache_quantize_ref`)."""
+    _check_scales(k_cache, k_scale, v_scale)
     if _decode_native(qkv, k_cache) and (cos is None or cos.dtype == torch.float32):
         ext = load_ext()
-        q = ext.kv_append(qkv if qkv.is_contiguous() else qkv.contiguous(), k_cache, v_cache, cache_seqlens, cos, sin,
-                          bool(return_q))
+        qkv = qkv if qkv.is_contiguous() else qkv.contiguous()
+        if k_scale is not None:
+            q = ext.kv_append_fp8(qkv, k_cache, v_cache, k_scale, v_scale, cache_seqlens, cos, sin, bool(return_q))
+        else:
+            q = ext.kv_append(qkv, k_cache, v_cache, cache_seqlens, cos, sin, bool(return_q))
         count_launch()
         return q if return_q else None
-    q = kv_cache_append_ref(qkv, k_cache, v_cache, cache_seqlens, cos, sin)
+    q = kv_cache_append_ref(qkv, k_cache, v_cache, cache_seqlens, cos, sin, k_scale, v_scale)
     return q if return_q else None
 
 
-def kv_cache_append_ref(qkv, k_cache, v_cache, cache_seqlens, cos=None, sin=None):
+def kv_cache_append_ref(qkv, k_cache, v_cache, cache_seqlens, cos=None, sin=None, k_scale=None, v_scale=None):
     s_len = qkv.shape[1]
     q, k, v = split_qkv(qkv)
     starts = [int(x) for x in cache_seqlens.tolist()]
@@ -866,13 +902,17 @@ def kv_cache_append_ref(qkv, k_cache, v_cache, cache_seqlens, cos=None, sin=None
         q = q * c + rotate_half(q) * sn
         k = k * c + rotate_half(k) * sn
     for b, st in enumerate(starts):
-        k_cache[b, :, st : st + s_len] = k[b].transpose(0, 1)
-        v_cache[b, :, st : st + s_len] = v[b].transpose(0, 1)
+        for cache, scale, x in ((k_cache, k_scale, k[b]), (v_cache, v_scale, v[b])):
+            if scale is None:
+                cache[b, :, st : st + s_len] = x.transpose(0, 1)
+            else:
+                cache[b, :, st : st + s_len], scale[b, :, st : st + s_len] = kv_cache_quantize_ref(x.transpose(0, 1))
     return q
 
 
 def decode_attention(q, k_cache, v_cache, cache_seqlens, kv_start, *, scale: float, splits: int = 0,
-                     past: Optional[int] = None, alibi_slopes=None, rel_bias=None, causal: bool = True):
+                     past: Optional[int] = None, alibi_slopes=None, rel_bias=None, causal: bool = True, k_scale=None,
+                     v_scale=None):
     """Attention of ``q [b, s, a, d]`` (new tokens, already appended to the caches; any strides with d contiguous) over
     the caches ``[b, g, C, d]`` (query head ``h`` reads cache head ``h // (a // g)``): query ``i`` of sample ``b`` sees exactly the keys ``kv_start[b] <= j <= cache_seqlens[b] + i``.  Returns
     ``[b, s, a, d]`` contiguous; a query without a visible key gets zeros.  The native kernel takes up to 16 new tokens
@@ -887,15 +927,29 @@ def decode_attention(q, k_cache, v_cache, cache_seqlens, kv_start, *, scale: flo
     dense bias it expands to.
     ``causal=False`` (cross-attention, no bias): every query sees ``kv_start[b] <= j < cache_seqlens[b]`` — a cache the
     new tokens are not in; more than 16 tokens run the rectangular flash kernel over that window (whose end, like
-    :func:`attention`'s ``kv_lens``, is at least 1)."""
-    if _decode_native(q, k_cache):
-        if q.shape[1] <= 16:
-            ext = load_ext()
-            extra = () if rel_bias is None and causal else (rel_bias, bool(causal))
-            o = ext.decode_attn(q, k_cache, v_cache, cache_seqlens, kv_start, float(scale), int(splits), alibi_slopes,
-                                *extra)
-            count_launch(2)
-            return o
+    :func:`attention`'s ``kv_lens``, is at least 1).
+    FP8 caches (``float8_e4m3fn``) take their row scales ``k_scale``, ``v_scale`` (fp32 ``[b, g, C]``); the attention is
+    that over the dequantized rows.  The decode kernel reads the bytes; every other path dequantizes the window to
+    q's dtype first (:func:`kv_cache_dequant`)."""
+    _check_scales(k_cache, k_scale, v_scale)
+    native = _decode_native(q, k_cache)
+    if native and q.shape[1] <= 16:
+        ext = load_ext()
+        extra = () if rel_bias is None and causal else (rel_bias, bool(causal))
+        if k_scale is not None:
+            extra = (rel_bias, bool(causal), k_scale, v_scale)
+        o = ext.decode_attn(q, k_cache, v_cache, cache_seqlens, kv_start, float(scale), int(splits), alibi_slopes,
+                            *extra)
+        count_launch(2)
+        return o
+    if k_scale is not None:
+        if past is not None:
+            L = past + q.shape[1] if causal else past
+        else:
+            L = k_cache.shape[2] if native else int(cache_seqlens.max()) + (q.shape[1] if causal else 0)
+        k_cache = kv_cache_dequant(k_cache[:, :, :L], k_scale[:, :, :L], q.dtype)
+        v_cache = kv_cache_dequant(v_cache[:, :, :L], v_scale[:, :, :L], q.dtype)
+    if native:
         if not causal:
             o = attention(q.permute(0, 2, 1, 3), k_cache, v_cache, causal=False, scale=scale, kv_start=kv_start,
                           kv_lens=cache_seqlens)
@@ -914,14 +968,19 @@ def decode_attention(q, k_cache, v_cache, cache_seqlens, kv_start, *, scale: flo
 
 
 def decode_attention_ref(q, k_cache, v_cache, cache_seqlens, kv_start, *, scale: float, alibi_slopes=None,
-                         rel_bias=None, causal: bool = True):
+                         rel_bias=None, causal: bool = True, k_scale=None, v_scale=None):
     """:func:`attention_ref` over the window ``[:L]`` of the caches (``L = max(cache_seqlens) + s``) with the mask built
     from ``kv_start`` and causality among the new tokens, and the ALiBi bias ``slope_h·(j − (cache_seqlens[b] + i))``
     when ``alibi_slopes`` is given, or T5's ``rel_bias[h, min(cache_seqlens[b] + i − j, R − 1)]`` when ``rel_bias`` is.
-    ``causal=False``: every query sees ``kv_start[b] <= j < cache_seqlens[b]`` (``L = max(cache_seqlens)``)."""
+    ``causal=False``: every query sees ``kv_start[b] <= j < cache_seqlens[b]`` (``L = max(cache_seqlens)``).  FP8
+    caches with ``k_scale`` / ``v_scale``: over the window dequantized to q's dtype."""
+    _check_scales(k_cache, k_scale, v_scale)
     s_len = q.shape[1]
     lens = cache_seqlens.long()
     L = int(lens.max()) + (s_len if causal else 0)
+    if k_scale is not None:
+        k_cache = kv_cache_dequant(k_cache[:, :, :L], k_scale[:, :, :L], q.dtype)
+        v_cache = kv_cache_dequant(v_cache[:, :, :L], v_scale[:, :, :L], q.dtype)
     j = torch.arange(L, device=q.device)[None, None, :]
     i = torch.arange(s_len, device=q.device)[None, :, None]
     end = lens[:, None, None] + i if causal else lens[:, None, None] - 1

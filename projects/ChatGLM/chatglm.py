@@ -275,8 +275,7 @@ class ChatGLMModel(nn.Module, ChatGLMPreTrainedModel):
             if cache.length == 0 and pre:   # prefill: the prefix rows first
                 for i, (k, v) in enumerate(self.get_prompt(b, input_ids.device, hidden.dtype)):
                     if i in cache.owned:
-                        cache.k[i][:, :, :pre] = k
-                        cache.v[i][:, :, :pre] = v
+                        cache.write_rows(i, k, v)
                 cache.advance(pre)
             past = cache.length
             inputs = AttentionInputs(self._rope, past - pre, position_ids,

@@ -477,8 +477,11 @@ class MT5Model(nn.Module, Generator, KVCacheOwner):
         attn = self.decoder.layers[0].cross_attention
         a, d = attn.local_heads, attn.head_size
         c = self.cross_cache
-        if c is None or not c.matches(b, encoder_states.dtype, encoder_states.device) or c.capacity < S:
-            c = StaticKVCache(len(self.decoder.layers), b, a, d, S, encoder_states.dtype, encoder_states.device)
+        kv_dtype = self.kv_cache_dtype   # the same format as the self-attention cache
+        if (c is None or not c.matches(b, encoder_states.dtype, encoder_states.device, kv_dtype)
+                or c.capacity < S):
+            c = StaticKVCache(len(self.decoder.layers), b, a, d, S, encoder_states.dtype, encoder_states.device,
+                              kv_dtype=kv_dtype)
         kv = (layer.cross_attention.key_value(encoder_states).view(b, S, a, 2 * d).transpose(1, 2).split(d, dim=-1)
               for layer in self.decoder.layers)
         c.fill(kv, S, window)
