@@ -154,6 +154,64 @@ std::tuple<Tensor, Tensor> linear_fwd(const Tensor& x, const Tensor& w, const c1
   return std::make_tuple(y, pre.defined() ? pre : at::empty({0}, x.options()));
 }
 
+// FP8 (E4M3) weights with per-output-channel scales: w [N, K] float8_e4m3fn and w_scale fp32 [N] on x's device,
+// contiguous and 16-byte aligned, K % 16 == 0
+void check_fp8_weight(const Tensor& x, const Tensor& w, const Tensor& w_scale, const char* what) {
+  TORCH_CHECK(w.scalar_type() == at::kFloat8_e4m3fn && w.dim() == 2 && w.is_contiguous() && w.device() == x.device(),
+              what, ": w must be a contiguous float8_e4m3fn [N, K] tensor on x's device, got ", w.scalar_type(), " ",
+              w.sizes(), " on ", w.device());
+  TORCH_CHECK(w.size(0) >= 1 && w.size(1) >= 16 && w.size(1) % 16 == 0, what, ": K must be a positive multiple of 16, got ",
+              w.sizes());
+  TORCH_CHECK(w.size(0) <= INT32_MAX && w.size(1) <= INT32_MAX, what, ": N and K must fit in int32");
+  TORCH_CHECK(reinterpret_cast<uintptr_t>(w.data_ptr()) % 16 == 0, what, ": w must be 16-byte aligned");
+  TORCH_CHECK(w_scale.scalar_type() == at::kFloat && w_scale.dim() == 1 && w_scale.size(0) == w.size(0) &&
+                  w_scale.is_contiguous() && w_scale.device() == x.device(),
+              what, ": w_scale must be a contiguous fp32 [N] tensor on x's device, got ", w_scale.scalar_type(), " ",
+              w_scale.sizes(), " on ", w_scale.device());
+}
+
+// y [M, N] = act((x [M, K] · float(w)ᵀ) · w_scale + bias): the weight-streaming kernel for 1 <= M <= 64 (x bf16
+// contiguous and 16-byte aligned, bias bf16 [N] or None, act one of the ACT_* ids without the residual add)
+Tensor linear_fp8w(const Tensor& x, const Tensor& w, const Tensor& w_scale, const c10::optional<Tensor>& bias,
+                   int64_t act) {
+  TORCH_CHECK(x.is_cuda() && x.scalar_type() == at::kBFloat16 && x.dim() == 2 && x.is_contiguous(),
+              "linear_fp8w: x must be a contiguous bf16 CUDA tensor [M, K], got ", x.scalar_type(), " ", x.sizes(),
+              " on ", x.device());
+  check_fp8_weight(x, w, w_scale, "linear_fp8w");
+  const int64_t M = x.size(0), K = x.size(1), N = w.size(0);
+  TORCH_CHECK(w.size(1) == K, "linear_fp8w: x [M, K] and w [N, K] disagree on K: ", x.sizes(), " vs ", w.sizes());
+  TORCH_CHECK(M >= 1 && M <= 64, "linear_fp8w: 1 <= M <= 64 rows, got ", M);
+  TORCH_CHECK(reinterpret_cast<uintptr_t>(x.data_ptr()) % 16 == 0, "linear_fp8w: x must be 16-byte aligned");
+  TORCH_CHECK(act >= 0 && act <= 5, "linear_fp8w: act must be an activation id in [0, 5], got ", act);
+  const void* bias_ptr = nullptr;
+  if (bias.has_value() && bias->defined()) {
+    TORCH_CHECK(bias->scalar_type() == at::kBFloat16 && bias->dim() == 1 && bias->size(0) == N &&
+                    bias->is_contiguous() && bias->device() == x.device(),
+                "linear_fp8w: bias must be a contiguous bf16 [N] tensor on x's device");
+    bias_ptr = bias->data_ptr();
+  }
+  c10::cuda::CUDAGuard guard(x.device());
+  Tensor y = at::empty({M, N}, x.options());
+  const long ws = lb_linear_fp8w_workspace((int)M, (int)N, (int)K);
+  Tensor part = ws > 0 ? at::empty({ws}, x.options().dtype(at::kFloat)) : Tensor();
+  check(lb_linear_fp8w(x.data_ptr(), w.data_ptr(), w_scale.data_ptr<float>(), bias_ptr, y.data_ptr(),
+                       ws > 0 ? part.data_ptr<float>() : nullptr, (int)M, (int)N, (int)K, (int)act, cur_stream()),
+        "linear_fp8w");
+  return y;
+}
+
+// bf16 [N, K] = bf16_rn(float(w) · w_scale[:, None]) (the weight the prefill GEMM of an FP8 linear multiplies)
+Tensor dequant_e4m3_rows(const Tensor& w, const Tensor& w_scale) {
+  TORCH_CHECK(w.is_cuda(), "dequant_e4m3_rows: w must be a CUDA tensor");
+  check_fp8_weight(w, w, w_scale, "dequant_e4m3_rows");
+  c10::cuda::CUDAGuard guard(w.device());
+  Tensor out = at::empty(w.sizes(), w.options().dtype(at::kBFloat16));
+  check(lb_dequant_e4m3_rows(w.data_ptr(), w_scale.data_ptr<float>(), out.data_ptr(), (long)w.size(0), (int)w.size(1),
+                             cur_stream()),
+        "dequant_e4m3_rows");
+  return out;
+}
+
 // per-tensor E4M3 quantisation of a contiguous bf16 tensor: returns (q [same shape, float8_e4m3fn], deq fp32 [1]) with
 // x ≈ q * deq (deq = amax / 448); two kernels, no host synchronisation
 std::tuple<Tensor, Tensor> quantize_e4m3(const Tensor& x) {
@@ -1249,6 +1307,8 @@ TORCH_LIBRARY(libai_b200, m) {
   m.def("gemm_schedule(int schedule) -> int", &gemm_schedule);
   m.def("linear_fwd(Tensor x, Tensor w, Tensor? bias, int act, bool need_pre) -> (Tensor, Tensor)", &linear_fwd);
   m.def("quantize_e4m3(Tensor x) -> (Tensor, Tensor)", &quantize_e4m3);
+  m.def("linear_fp8w(Tensor x, Tensor w, Tensor w_scale, Tensor? bias, int act) -> Tensor", &linear_fp8w);
+  m.def("dequant_e4m3_rows(Tensor w, Tensor w_scale) -> Tensor", &dequant_e4m3_rows);
   m.def("linear_fp8_fwd(Tensor xq, Tensor wq, Tensor deq_x, Tensor deq_w, Tensor? bias, int act, bool need_pre, Tensor? residual=None, int bn=0) -> (Tensor, Tensor)", &linear_fp8_fwd);
   m.def("act_bwd(Tensor gy, Tensor pre, int act) -> Tensor", &act_bwd);
   m.def("colsum(Tensor x, Tensor(a!)? accum=None) -> Tensor", &colsum);

@@ -3,6 +3,8 @@
 #pragma once
 #include <cuda.h>
 #include <cuda_bf16.h>
+#include <cuda_fp16.h>
+#include <cuda_fp8.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdio.h>
@@ -297,6 +299,15 @@ LB_DEVICE float2 unpack_bf16(uint32_t u) {
   // a bf16 is the upper half of an fp32: one shift for the low element, one mask for the high one (the intrinsic
   // compiled to PRMT + IMAD for the high half)
   return make_float2(__uint_as_float(u << 16), __uint_as_float(u & 0xffff0000u));
+}
+// e4m3 pair (low byte first) -> bf16 pair, exactly (every e4m3 value is an f16 and a bf16)
+LB_DEVICE uint32_t e4m3x2_to_bf16x2(uint16_t x) {
+  const __half2_raw h = __nv_cvt_fp8x2_to_halfraw2(static_cast<__nv_fp8x2_storage_t>(x), __NV_E4M3);
+  const float2 f = __half22float2(*reinterpret_cast<const __half2*>(&h));
+  return pack_bf16(f.x, f.y);
+}
+LB_DEVICE uint2 e4m3x4_to_bf16x4(uint32_t x) {
+  return make_uint2(e4m3x2_to_bf16x2(static_cast<uint16_t>(x)), e4m3x2_to_bf16x2(static_cast<uint16_t>(x >> 16)));
 }
 
 // one Adam step of one element, shared by fused_adamw and the ZeRO update: g = grad * scale (+ wd * p when the weight

@@ -3,9 +3,6 @@
 // decode_attention_t5_sm90.cu with T5's relative-position bias or a non-causal key window, and
 // decode_attention_fp8_sm90.cu every score kind over an FP8 (E4M3) cache.
 #pragma once
-#include <cuda_fp16.h>
-#include <cuda_fp8.h>
-
 #include <type_traits>
 
 #include "common.cuh"
@@ -73,15 +70,6 @@ LB_DEVICE void bulk_load(void* dst, const void* src, uint32_t bytes, uint64_t* b
                    smem_u32(dst)),
                "l"(src), "r"(bytes), "r"(smem_u32(bar))
                : "memory");
-}
-// e4m3 pair (low byte first) -> bf16 pair, exactly (every e4m3 value is an f16 and a bf16)
-LB_DEVICE uint32_t e4m3x2_to_bf16x2(uint16_t x) {
-  const __half2_raw h = __nv_cvt_fp8x2_to_halfraw2(static_cast<__nv_fp8x2_storage_t>(x), __NV_E4M3);
-  const float2 f = __half22float2(*reinterpret_cast<const __half2*>(&h));
-  return pack_bf16(f.x, f.y);
-}
-LB_DEVICE uint2 e4m3x4_to_bf16x4(uint32_t x) {
-  return make_uint2(e4m3x2_to_bf16x2(static_cast<uint16_t>(x)), e4m3x2_to_bf16x2(static_cast<uint16_t>(x >> 16)));
 }
 
 // FP8: p.k / p.v point at the E4M3 bytes and k_scale / v_scale at their row scales; key j's score is

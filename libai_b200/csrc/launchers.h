@@ -138,6 +138,14 @@ int lb_kv_append(const void* qkv, const float* cosv, const float* sinv, void* q_
 int lb_kv_append_fp8(const void* qkv, const float* cosv, const float* sinv, void* q_out, void* k_cache, void* v_cache,
                      float* k_scale, float* v_scale, const int* seqlens, int B, int Sq, int G, int r, int C, int D,
                      cudaStream_t s);
+// y [M, N] bf16 = act((x [M, K] bf16 · float(w [N, K] E4M3)ᵀ) · w_scale [N] + bias [N]) with 1 <= M <= 64 and
+// K % 16 == 0; bias (bf16 [N]) may be null.  part: an fp32 workspace of lb_linear_fp8w_workspace(M, N, K) floats (null
+// when that is 0).
+long lb_linear_fp8w_workspace(int M, int N, int K);
+int lb_linear_fp8w(const void* x, const void* w, const float* w_scale, const void* bias, void* y, float* part, int M,
+                   int N, int K, int act, cudaStream_t s);
+// out [rows, K] bf16 = bf16_rn(float(w [rows, K] E4M3) · scale[row]), K % 16 == 0
+int lb_dequant_e4m3_rows(const void* w, const float* scale, void* out, long rows, int K, cudaStream_t s);
 int lb_window_attn_groups(int B, int H, int W, int ws, int heads);
 int lb_window_attn_fwd(const void* qkv, void* out, float* lse, const float* table, const float* tau, int B, int H, int W,
                        int ws, int shift, int heads, int d, float scale, cudaStream_t s);

@@ -24,7 +24,11 @@ logger = logging.getLogger(__name__)
 class BasePipeline(metaclass=ABCMeta):
     def __init__(self, config_file, data_parallel=None, tensor_parallel=None, pipeline_parallel=None,
                  pipeline_stage_id=None, pipeline_num_layers=None, model_path=None, mode="libai", device=None,
-                 **kwargs):
+                 weight_dtype=None, **kwargs):
+        """``weight_dtype``: None keeps the weights as placed; ``"fp8"`` converts the model's linear layers to FP8
+        (E4M3) weights with per-channel scales after placing it (:func:`libai_b200.inference.quantize_weights_fp8_`)."""
+        if weight_dtype not in (None, "fp8"):
+            raise ValueError(f"weight_dtype={weight_dtype!r}: None or 'fp8'")
         self.cfg = LazyConfig.load(config_file) if isinstance(config_file, (str, Path)) else config_file
         self.update_cfg(data_parallel, tensor_parallel, pipeline_parallel, pipeline_stage_id, pipeline_num_layers)
         self.device = device or ("cuda" if torch.cuda.is_available() else "cpu")
@@ -43,6 +47,10 @@ class BasePipeline(metaclass=ABCMeta):
 
         self.model = self.load_pretrain_weight(self.cfg.model, self.model_path, mode=mode)
         self.model = self._place(self.model).eval()
+        if weight_dtype == "fp8":
+            from libai_b200.inference import quantize_weights_fp8_
+
+            quantize_weights_fp8_(self.model)
         self.tokenizer = self.build_tokenizer(self.cfg)
         self._preprocess_params, self._forward_params, self._postprocess_params = self._parse_parameters(**kwargs)
 

@@ -336,11 +336,14 @@ class KVCacheOwner:
         mods = self._cache_attention_modules()
         topo = dutil.get_dist_util()
         owned = [i for i in range(len(mods)) if topo.owns_layer(i)]   # this pipeline stage's layers
-        w = mods[0].query_key_value.weight
+        qkv = mods[0].query_key_value
+        w = qkv.weight
+        # the activations' dtype: a Linear1D with FP8 weights keeps it apart (LoRA wrappers have no compute_dtype)
+        dtype = getattr(qkv, "compute_dtype", None) or w.dtype
         c = self.kv_cache
-        if c is None or not c.matches(batch, w.dtype, w.device, self.kv_cache_dtype) or c.capacity < max_length:
+        if c is None or not c.matches(batch, dtype, w.device, self.kv_cache_dtype) or c.capacity < max_length:
             heads = getattr(mods[0], "local_kv_heads", mods[0].local_heads)
-            c = StaticKVCache(len(mods), batch, heads, mods[0].head_size, max_length, w.dtype, w.device, owned,
+            c = StaticKVCache(len(mods), batch, heads, mods[0].head_size, max_length, dtype, w.device, owned,
                               self.kv_cache_dtype)
         c.reset()
         self.kv_cache, self.past_length = c, 0

@@ -14,6 +14,9 @@ Communication (explicit, instead of SBP boxing):
 
 On H100 the sequence-parallel pairs run as single fused kernels (AG→GEMM, GEMM→RS over NVLink
 peer memory, ``libai_b200/ops/comm_gemm.py``) when ``train.dist.fused_tp_comm`` is on.
+
+For inference, ``quantize_fp8_`` turns the layer's weight into FP8 (E4M3) bytes with one fp32 scale per output
+channel of this rank's shard; the forward then runs ``OF.linear_fp8w`` inside the same TP mappings.
 """
 from __future__ import annotations
 
@@ -27,7 +30,12 @@ from libai_b200.utils import distributed as dutil
 from ._param import create_parameter, xavier_normal_, zeros_
 
 
+_FP8_SOURCE_DTYPES = (torch.bfloat16, torch.float16, torch.float32)
+
+
 class Linear1D(nn.Module):
+    compute_dtype = None   # FP8 weights: the dtype of the inputs, outputs and bias (the weight's dtype before)
+
     def __init__(
         self,
         in_features,
@@ -62,6 +70,50 @@ class Linear1D(nn.Module):
             # added after the reduce-scatter, i.e. on token shards: its gradient is partial per TP rank
             self.bias.sequence_parallel = dutil.get_dist_util().sequence_parallel
 
+    @property
+    def fp8(self) -> bool:
+        """The weight is FP8 (E4M3) bytes with row scales ``weight_scale`` (:meth:`quantize_fp8_`)."""
+        return self.weight.dtype == torch.float8_e4m3fn
+
+    @torch.no_grad()
+    def quantize_fp8_(self):
+        """Replace the weight ``[out_local, in_local]`` by its FP8 (E4M3) bytes and the fp32 scales ``weight_scale``
+        ``[out_local]``, one per output channel: ``s = amax|w_n| / 448`` (1 for an all-zero row), bytes
+        ``e4m3_rn_satfinite(w / s)`` (``OF.kv_cache_quantize_ref``); the weight reads back as ``float(e)·s``.  The bias
+        and the activations keep the weight's former dtype (``compute_dtype``).  For inference only; a second call is a
+        no-op."""
+        if self.fp8:
+            return self
+        w = self.weight
+        if w.dtype not in _FP8_SOURCE_DTYPES:
+            raise TypeError(f"quantize_fp8_: a {w.dtype} weight (bf16, fp16 or fp32 expected)")
+        e, s = OF.kv_cache_quantize_ref(w)
+        self.compute_dtype = w.dtype
+        self.weight = nn.Parameter(e, requires_grad=False)
+        self.weight_scale = nn.Parameter(s, requires_grad=False)
+        return self
+
+    def _apply(self, fn, recurse=True):
+        """Dtype casts (``.to(dtype)``, ``.bfloat16()``, ``.half()``, ``.float()``) leave FP8 bytes and their fp32
+        scales as they are and change ``compute_dtype`` (and the bias) instead; device moves move them."""
+        if not self.fp8:
+            return super()._apply(fn, recurse)
+        probe = fn(torch.empty(0, dtype=self.compute_dtype, device=self.weight.device))
+        order = list(self._parameters)
+        held = {k: self._parameters.pop(k) for k in ("weight", "weight_scale")}
+        try:
+            super()._apply(fn, recurse)
+        finally:
+            rest = dict(self._parameters)
+            self._parameters.clear()
+            self._parameters.update({k: held[k] if k in held else rest[k] for k in order})
+        for k, p in held.items():
+            if p.device != probe.device:
+                self._parameters[k] = nn.Parameter(p.detach().to(probe.device), requires_grad=False)
+        if probe.is_floating_point():
+            self.compute_dtype = probe.dtype
+        return self
+
     def fused_bias_residual(self, x, residual):
         """Row-parallel fast path of the block-output projections under fused tensor parallelism:
         ``reduce_scatter(x @ Wᵀ) + bias + residual`` in ONE kernel (bias and residual are added by the reduce phase of
@@ -83,19 +135,24 @@ class Linear1D(nn.Module):
                 return (y, self.bias) if self.skip_bias_add else y
         if self.parallel == "col":
             x = mappings.gather_from_sp(x) if sp else mappings.copy_to_tp(x)
-            y = OF.linear(x, self.weight, bias_now, act)
+            y = self._gemm(x, bias_now, act)
         elif self.parallel == "row":
-            y = OF.linear(x, self.weight, None, None)
+            y = self._gemm(x, None, None)
             y = mappings.reduce_scatter_to_sp(y) if sp else mappings.reduce_from_tp(y)
             if bias_now is not None:
                 y = y + bias_now.to(y.dtype)
             if act is not None:
                 y = OF._act_ref(y, act)
         else:
-            y = OF.linear(x, self.weight, bias_now, act)
+            y = self._gemm(x, bias_now, act)
         if self.skip_bias_add:
             return y, self.bias
         return y
+
+    def _gemm(self, x, bias, act):
+        if self.fp8:
+            return OF.linear_fp8w(x, self.weight, self.weight_scale, bias, act)
+        return OF.linear(x, self.weight, bias, act)
 
     def _forward_fused(self, x, bias_now, act, topo, residual=None):
         """AG->GEMM / GEMM->RS with the collective inside the wgmma kernel (None = shape unsupported)."""
@@ -118,8 +175,9 @@ class Linear1D(nn.Module):
         return comm_gemm.row_parallel_linear(x2.contiguous(), self.weight, bias_now, residual, topo.tp_group)
 
     def extra_repr(self) -> str:
-        return "in_features={}, out_features={}, bias={}, parallel={}".format(
-            self.in_features, self.out_features, self.bias is not None, self.parallel
+        return "in_features={}, out_features={}, bias={}, parallel={}{}".format(
+            self.in_features, self.out_features, self.bias is not None, self.parallel,
+            f", weight=fp8 (compute_dtype={self.compute_dtype})" if self.fp8 else "",
         )
 
 

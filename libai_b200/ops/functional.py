@@ -175,8 +175,17 @@ class _LinearFn(torch.autograd.Function):
         return gx, gw, gb, None
 
 
+def reject_fp8_weight(what: str, *weights) -> None:
+    """FP8 (E4M3) weights read back only with their row scales, which the bf16 GEMM entries do not take: they raise
+    instead of multiplying the bytes unscaled (:func:`linear_fp8w` is the entry for such weights)."""
+    for w in weights:
+        if w is not None and w.dtype == torch.float8_e4m3fn:
+            raise TypeError(f"{what}: float8_e4m3fn weight; FP8 weights take OF.linear_fp8w with their row scales")
+
+
 def linear(x, w, bias=None, act: Optional[str] = None):
     """``act(x @ w.T + bias)``; ``w`` is ``[out, in]``."""
+    reject_fp8_weight("linear", w)
     if use_native(x, w) and _gemm_ok(x, w):
         return _LinearFn.apply(x, w, bias, act)
     y = F.linear(x, w.to(x.dtype) if w.dtype != x.dtype else w, None if bias is None else bias.to(x.dtype))
@@ -255,6 +264,7 @@ class _MLPFn(torch.autograd.Function):
 def mlp(x, w1, b1, w2, act: str = "gelu", b2=None, residual=None):
     """``act(x @ w1ᵀ + b1) @ w2ᵀ``; with ``residual`` also ``+ b2 + residual`` in the second GEMM's epilogue
     (without it the second bias is left to the fused bias+dropout+residual op)."""
+    reject_fp8_weight("mlp", w1, w2)
     if use_native(x, w1) and _gemm_ok(x, w1) and _gemm_ok(x.new_empty(1, w1.shape[0]), w2):
         if residual is not None:
             return _MLPFn.apply(x, w1, b1, w2, act, b2, residual)
@@ -304,10 +314,58 @@ class _LinearResidualFn(torch.autograd.Function):
 
 def linear_bias_residual(x, w, bias, residual):
     """``x @ wᵀ + bias + residual`` (output projection of a block, dropout-free)."""
+    reject_fp8_weight("linear_bias_residual", w)
     if use_native(x, w) and _gemm_ok(x, w) and residual is not None and residual.dtype == torch.bfloat16:
         return _LinearResidualFn.apply(x, w, bias, residual)
     y = linear(x, w, bias)
     return y if residual is None else y + residual
+
+
+# --------------------------------------------------------------------------------------
+# FP8 (E4M3) weights for inference: ``w`` [N, K] float8_e4m3fn with one fp32 scale per output channel, ``w_scale``
+# [N] (:func:`kv_cache_quantize_ref` per row, see ``Linear1D.quantize_fp8_``); the weight reads back as float(e)·s
+# --------------------------------------------------------------------------------------
+# Up to this many rows (tokens) run the weight-streaming kernel; more dequantize the weight to bf16 and run the bf16 GEMM.
+# 64 is the most the kernel takes: it was faster than dequantize + GEMM at every M of the sweep up to 64
+# (dev/fp8_weights_bench.py, Kernels.md "FP8 weights")
+FP8W_KERNEL_MAX_M = 64
+
+
+def linear_fp8w_ref(x, w, w_scale, bias=None, act: Optional[str] = None):
+    """``act(x @ (float(w)·w_scale[:, None])ᵀ + bias)`` in fp32, rounded to x's dtype."""
+    y = F.linear(x.float(), w.float() * w_scale.float()[:, None], None if bias is None else bias.float())
+    return _act_ref(y, act).to(x.dtype)
+
+
+def linear_fp8w(x, w, w_scale, bias=None, act: Optional[str] = None):
+    """``act(x @ (float(w)·w_scale[:, None])ᵀ + bias)`` for FP8 weights ``w`` [N, K] (float8_e4m3fn) with fp32 row
+    scales ``w_scale`` [N]; returns x's dtype.  On the GPU with bf16 x (K % 16 == 0): up to ``FP8W_KERNEL_MAX_M``
+    rows run the weight-streaming kernel (fp32 accumulation, scale, bias and activation on the fp32 sum), more rows
+    dequantize the weight to bf16 (``bf16_rn(float(e)·s)``, a temporary of the caching allocator) and run the bf16 GEMM
+    with its bias/activation epilogue.  Other inputs (CPU, fp32 or fp16 x, other shapes) run :func:`linear_fp8w_ref`.
+    Inference only: a call that would need a gradient raises."""
+    if torch.is_grad_enabled() and (x.requires_grad or (bias is not None and bias.requires_grad)):
+        raise RuntimeError("FP8 weights are for inference: run the model under torch.no_grad() (and without inputs "
+                           "that require a gradient)")
+    N, K = w.shape
+    x2 = x.reshape(-1, K)
+    M = x2.shape[0]
+    if (use_native(x) and x.dtype == torch.bfloat16 and w.is_cuda and w.is_contiguous() and K % 16 == 0 and M >= 1
+            and (bias is None or bias.dtype == torch.bfloat16)):
+        ext = load_ext()
+        x2 = x2.contiguous()
+        b = None if bias is None else bias.contiguous()
+        if x2.data_ptr() % 16 == 0 and w.data_ptr() % 16 == 0:
+            if M <= FP8W_KERNEL_MAX_M:
+                y = ext.linear_fp8w(x2, w, w_scale, b, _ACT_IDS[act])
+                count_launch(2)   # the kernel, and the sum over its K ranges
+                return y.view(*x.shape[:-1], N)
+            if N % 8 == 0:
+                wb = ext.dequant_e4m3_rows(w, w_scale)
+                y, _ = ext.linear_fwd(x2, wb, b, _ACT_IDS[act], False)
+                count_launch(2)
+                return y.view(*x.shape[:-1], N)
+    return linear_fp8w_ref(x, w, w_scale, bias, act)
 
 
 def matmul_nt(a, b):
