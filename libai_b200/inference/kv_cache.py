@@ -136,10 +136,10 @@ class KVCacheLayer:
 
     def attend(self, q: torch.Tensor, *, scale: float, causal: bool = True, mask=None, bias=None, alibi_slopes=None,
                rel_bias=None, dropout_p: float = 0.0, training: bool = False) -> torch.Tensor:
-        """Attention of the new tokens' ``q`` ``[b, s, a, d]`` over the cache → ``[b, s, a, d]``.  ``causal``: the new
-        tokens were appended this step (self-attention); ``causal=False``: the cache is a fixed window the queries all
-        see (cross-attention).  The rows held before this step (``length``) are the same for every layer: the model
-        advances the cache after its last layer.
+        """Attention of the new tokens' ``q`` ``[b, s, a, d]`` over the cache → ``[b, s, a, d]``, contiguous.
+        ``causal``: the new tokens were appended this step (self-attention); ``causal=False``: the cache is a fixed
+        window the queries all see (cross-attention).  The rows held before this step (``length``) are the same for
+        every layer: the model advances the cache after its last layer.
 
         - a dense 0/1 ``mask`` or additive ``bias`` (the model folded its padding into it): :func:`OF.attention` over
           the window ``[:length + s]`` (causal) or ``[:length]``, non-causal;
@@ -155,7 +155,7 @@ class KVCacheLayer:
             k, v = self.window(L, q.dtype)
             ctx = OF.attention(q.transpose(1, 2), k, v, causal=False, scale=scale, mask=mask, bias=bias,
                                dropout_p=dropout_p, training=training)
-            return ctx.transpose(1, 2)
+            return ctx.transpose(1, 2).contiguous()   # the reference math's [b, a, s, d] output is not
         if causal and past == 0 and rel_bias is None:
             query, (key, value) = q.transpose(1, 2), self.window(q.shape[1], q.dtype)
             kv_start = self.kv_start if OF.attention_supported(query, key) else None

@@ -988,7 +988,13 @@ def decode_attention(q, k_cache, v_cache, cache_seqlens, kv_start, *, scale: flo
     :func:`attention`'s ``kv_lens``, is at least 1).
     FP8 caches (``float8_e4m3fn``) take their row scales ``k_scale``, ``v_scale`` (fp32 ``[b, g, C]``); the attention is
     that over the dequantized rows.  The decode kernel reads the bytes; every other path dequantizes the window to
-    q's dtype first (:func:`kv_cache_dequant`)."""
+    q's dtype first (:func:`kv_cache_dequant`).
+    Rows read: the decode kernel reads no row at or past a sample's window end (``cache_seqlens[b] + s``, or
+    ``cache_seqlens[b]`` for cross-attention); the flash kernel reads the window ``[:past + s]`` (``[:past]`` for
+    cross-attention; without ``past``, any row of the capacity); the reference math reads ``[:max(cache_seqlens) + s]``
+    and zeroes the value rows a sample cannot see.  So rows past the window may hold anything, NaN included (an
+    uninitialised cache), while invisible rows inside it (before ``kv_start[b]``, or in cross-attention from
+    ``cache_seqlens[b]`` to ``past``) may be loaded with weight zero and must be finite, as the appends leave them."""
     _check_scales(k_cache, k_scale, v_scale)
     native = _decode_native(q, k_cache)
     if native and q.shape[1] <= 16:
@@ -1009,6 +1015,8 @@ def decode_attention(q, k_cache, v_cache, cache_seqlens, kv_start, *, scale: flo
         v_cache = kv_cache_dequant(v_cache[:, :, :L], v_scale[:, :, :L], q.dtype)
     if native:
         if not causal:
+            if past is not None:   # the kernel loads whole key tiles: rows past the window must not enter P·V
+                k_cache, v_cache = k_cache[:, :, :past], v_cache[:, :, :past]
             o = attention(q.permute(0, 2, 1, 3), k_cache, v_cache, causal=False, scale=scale, kv_start=kv_start,
                           kv_lens=cache_seqlens)
             return o.transpose(1, 2)
@@ -1043,6 +1051,9 @@ def decode_attention_ref(q, k_cache, v_cache, cache_seqlens, kv_start, *, scale:
     i = torch.arange(s_len, device=q.device)[None, :, None]
     end = lens[:, None, None] + i if causal else lens[:, None, None] - 1
     visible = (j >= kv_start.long()[:, None, None]) & (j <= end)                              # [b, s, L]
+    # a masked score gets probability 0, but 0 · NaN is NaN: a shorter sample's rows past its own window end (never
+    # written) must not reach P @ V
+    v_cache = torch.where(visible.any(1)[:, None, :, None], v_cache[:, :, :L], 0)
     bias = None
     if alibi_slopes is not None:
         rel = (j - (lens[:, None, None] + i)).float()                                          # [b, s, L]

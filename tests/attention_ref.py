@@ -136,13 +136,16 @@ def _bias_head(bias, alibi, b, h, Sq, Sk, device):
 
 
 # ------------------------------------------------------------------------------------------------------------ forward
-def attention_fwd_ref(q, k, v, *, scale, vis, bias=None, alibi=None, keep=None, inv_keep=1.0, tile=64):
+def attention_fwd_ref(q, k, v, *, scale, vis, bias=None, alibi=None, keep=None, inv_keep=1.0, tile=64,
+                      eta_extra=None):
     """Reference O [B, A, Sq, D] and lse [B, A, Sq] with their bounds, as ((o, o_bound), (lse, lse_bound)).
 
     q [B, A, Sq, D]; k, v [B, G, Sk, D] (query head h reads K/V head h / (A / G)); vis: bool [B|1, 1|A, Sq, Sk]
     (``OF.visible_keys``); bias: dense [B|1, A|1, Sq, Sk] or ``alibi`` slopes [A]; keep: bool [B, A, Sq, Sk] and its
     ``inv_keep``.  A row without a visible key has O = 0 and lse = 0, with a zero bound.  ``tile``: the smallest number
-    of keys after which a kernel rescales its running sums (64 in decode, 128 in the flash forward)."""
+    of keys after which a kernel rescales its running sums (64 in decode, 128 in the flash forward).  ``eta_extra``
+    (fp64 [B|1, A|1, Sq, Sk], or a number): a relative error of each unnormalised probability beyond the kernel's own
+    roundings, e.g. from inputs the kernel saw rounded where the reference holds them exact."""
     B, A, Sq, D = q.shape
     G, Sk = k.shape[1], k.shape[2]
     r = A // G
@@ -175,6 +178,10 @@ def attention_fwd_ref(q, k, v, *, scale, vis, bias=None, alibi=None, keep=None, 
             #     the n_resc running-max differences, each 2^-24 of a value below |z| + M (log2 e / ln 2 absorbed in 2^3);
             #   (n_resc + 2) EX2_APPROX: its own ex2.approx and the ex2.approx of every rescale applied to it
             eta = scale * dS + 2.0 ** -21 * (n_resc + 2) * (z.abs() + M) + (n_resc + 2) * EX2_APPROX
+            if eta_extra is not None:
+                ex = eta_extra if not torch.is_tensor(eta_extra) else \
+                    eta_extra[min(b, eta_extra.shape[0] - 1), min(h, eta_extra.shape[1] - 1)].to(dev)
+                eta = eta + ex
             eta = torch.where(vm, eta, torch.zeros_like(eta))
             eta_max = eta.max(-1, keepdim=True).values
             # O = N / l with N = sum_j T_j V_j: each term of N carries eta, its bf16 rounding 2^-8 and the fp32 sum over

@@ -60,6 +60,51 @@ def test_kernel_matches_fp64(ext, M, K, epi):
     assert bool((err <= tol).all()), float((err - tol).max())
 
 
+def _split_of(N, K):
+    """(splits, range) of ``split_of`` in linear_fp8w_sm90.cu: 64-row blocks, ranges of at least 256 columns in 64-column
+    steps, enough splits for 4 · 132 CTAs."""
+    row_blocks = -(-N // 64)
+    splits = min(max(-(-528 // row_blocks), 1), -(-K // 256))
+    rng = -(-(-(-K // splits)) // 64) * 64
+    return -(-K // rng), rng
+
+
+# (N, K) -> (splits, range): the paths test_kernel_matches_fp64 does not reach
+SPLIT_SHAPES = {
+    (37888, 3584): (1, 3584),   # the direct-write epilogue at a real K (Qwen2-7B's packed gate/up projection)
+    (200, 208): (1, 256),       # direct write, K % 64 = 16
+    (200, 224): (1, 256),       # K % 64 = 32
+    (200, 240): (1, 256),       # K % 64 = 48
+    (4096, 4128): (9, 512),     # the last split holds 32 columns
+    (63, 1040): (5, 256),       # the last split holds 16 columns; one partial row block
+    (1, 4096): (16, 256),       # fewer than 16 weight rows: lanes without a valid row
+    (8, 4096): (16, 256),
+}
+
+
+@pytest.mark.parametrize("NK", list(SPLIT_SHAPES), ids=[f"N{n}_K{k}" for n, k in SPLIT_SHAPES])
+@pytest.mark.parametrize("epi", [(False, None), (True, "silu")], ids=["plain", "bias_silu"])
+def test_kernel_split_shapes_match_fp64(ext, NK, epi):
+    N, K = NK
+    assert _split_of(N, K) == SPLIT_SHAPES[NK]
+    bias, act = epi
+    x, e, s, b = _case(64, N, K, bias, seed=N + K)
+    full = ext.linear_fp8w(x, e, s, b, ACT[act])
+    for M in (1, 9, 33, 64):
+        y = full if M == 64 else ext.linear_fp8w(x[:M].contiguous(), e, s, b, ACT[act])
+        assert y.dtype == torch.bfloat16 and y.shape == (M, N)
+        ref, mag = _ref64(x[:M], e, s, b, act)
+        # the tolerance of test_kernel_matches_fp64
+        err = (y.double() - ref).abs()
+        tol = 2.0 ** -8 * ref.abs() + 2e-6 * mag * (1 + K / 1024) + 1e-5
+        assert bool((err <= tol).all()), (M, float((err - tol).max()))
+        if NK == (37888, 3584):   # batch invariance on the direct-write path, at the first and the last rows
+            assert torch.equal(y, full[:M]), M
+            tail = ext.linear_fp8w(x[64 - M :].contiguous(), e, s, b, ACT[act])
+            assert torch.equal(tail, full[64 - M :]), M
+        del ref, mag
+
+
 def test_kernel_is_deterministic_graph_safe_and_batch_invariant(ext):
     N, K = 4096 + 40, 4096
     x, e, s, b = _case(64, N, K, True, seed=5)
