@@ -39,40 +39,150 @@ int dtype_code(const Tensor& t) {
   TORCH_CHECK(false, "libai_b200: unsupported dtype ", t.scalar_type());
 }
 
+
+bool given(const c10::optional<Tensor>& t) { return t.has_value() && t->defined(); }
+
+// ---- argument checks ------------------------------------------------------------------------------------
+// The kernels get raw pointers, so every tensor argument of an op is checked by one call that states its dtype, its
+// sizes (kAny: a free dimension), its layout and, where the kernel vector-loads it, its alignment.  Those rules run
+// first, for every argument; guard() then requires every argument on the first one's device and that device to be a
+// CUDA device, and returns the guard for it.  The guard and every allocation come after the checks, and no check
+// syncs the host or allocates.
+constexpr int64_t kAny = -1;
+constexpr at::ScalarType kAnyDtype = at::ScalarType::Undefined;
+enum class Layout { Contiguous, LastDimContiguous, Strided };
+
+// one dtype, or either of two (kAnyDtype: any)
+struct Dtypes {
+  Dtypes(at::ScalarType t) : a(t), b(t) {}
+  Dtypes(at::ScalarType t, at::ScalarType u) : a(t), b(u) {}
+  at::ScalarType a, b;
+};
+
+const char* dtype_name(at::ScalarType t) {
+  switch (t) {
+    case at::kBFloat16: return "bf16";
+    case at::kHalf: return "fp16";
+    case at::kFloat: return "fp32";
+    case at::kDouble: return "fp64";
+    case at::kInt: return "int32";
+    case at::kLong: return "int64";
+    case at::kFloat8_e4m3fn: return "float8_e4m3fn";
+    default: return c10::toString(t);
+  }
+}
+
+struct Rule {
+  Dtypes dtypes;
+  at::IntArrayRef sizes;
+  Layout layout;
+  int align;
+};
+std::ostream& operator<<(std::ostream& os, const Rule& r) {
+  if (r.align != 0) os << r.align << "-byte aligned ";
+  if (r.layout == Layout::Contiguous) os << "contiguous ";
+  if (r.dtypes.a != kAnyDtype) os << dtype_name(r.dtypes.a) << " ";
+  if (r.dtypes.b != r.dtypes.a) os << "or " << dtype_name(r.dtypes.b) << " ";
+  os << "[";
+  for (size_t i = 0; i < r.sizes.size(); ++i) {
+    if (i > 0) os << ", ";
+    if (r.sizes[i] == kAny) os << "*";
+    else os << r.sizes[i];
+  }
+  os << "]";
+  if (r.layout == Layout::LastDimContiguous) os << " with a contiguous last dim";
+  return os;
+}
+struct Got {
+  const Tensor& t;
+};
+std::ostream& operator<<(std::ostream& os, const Got& g) {
+  return os << dtype_name(g.t.scalar_type()) << " " << g.t.sizes() << " on " << g.t.device();
+}
+
+class Args {
+ public:
+  explicit Args(const char* op) : op_(op) {}
+  const char* op() const { return op_; }
+
+  // Checks one argument now and its device in guard().  The first argument checked is the reference: the op runs on
+  // its device.
+  const Tensor& operator()(const char* name, const Tensor& t, Dtypes dtypes, at::IntArrayRef sizes,
+                           Layout layout = Layout::Contiguous, int align = 0) {
+    const Rule rule{dtypes, sizes, layout, align};
+    TORCH_CHECK(fits(t, rule), op_, ": ", name, " must be ", rule, ", got ", Got{t});
+    TORCH_INTERNAL_ASSERT(n_ < kMaxArgs, op_, ": too many tensor arguments");
+    seen_[n_++] = {name, &t};
+    return t;
+  }
+  // an optional argument: its data pointer, or nullptr for None
+  template <typename T = const void>
+  T* opt(const char* name, const c10::optional<Tensor>& t, Dtypes dtypes, at::IntArrayRef sizes,
+         Layout layout = Layout::Contiguous, int align = 0) {
+    if (!given(t)) return nullptr;
+    return static_cast<T*>((*this)(name, *t, dtypes, sizes, layout, align).data_ptr());
+  }
+
+  c10::cuda::CUDAGuard guard() const {
+    const auto& [ref_name, ref] = seen_[0];
+    for (int i = 1; i < n_; ++i)
+      TORCH_CHECK(seen_[i].second->device() == ref->device(), op_, ": ", seen_[i].first, " must be on ", ref_name,
+                  "'s device ", ref->device(), ", got ", Got{*seen_[i].second});
+    TORCH_CHECK(ref->is_cuda(), op_, ": ", ref_name, " must be a CUDA tensor, got ", Got{*ref});
+    return c10::cuda::CUDAGuard(ref->device());
+  }
+
+ private:
+  static bool fits(const Tensor& t, const Rule& r) {
+    if (r.dtypes.a != kAnyDtype && t.scalar_type() != r.dtypes.a && t.scalar_type() != r.dtypes.b) return false;
+    if (t.dim() != (int64_t)r.sizes.size()) return false;
+    for (int64_t i = 0; i < t.dim(); ++i)
+      if (r.sizes[i] != kAny && t.size(i) != r.sizes[i]) return false;
+    if (r.layout == Layout::Contiguous && !t.is_contiguous()) return false;
+    if (r.layout == Layout::LastDimContiguous && t.dim() > 0 && t.stride(-1) != 1) return false;
+    return r.align == 0 || reinterpret_cast<uintptr_t>(t.data_ptr()) % r.align == 0;
+  }
+
+  static constexpr int kMaxArgs = 16;
+  const char* op_;
+  std::pair<const char*, const Tensor*> seen_[kMaxArgs];
+  int n_ = 0;
+};
+
 // ---- GEMM -----------------------------------------------------------------------------------------
-// layout 0: a[M,K] b[N,K]; 1: a[M,K] b[K,N]; 2: a[K,M] b[K,N].  Returns out (allocated when not given).
+struct GemmDims {
+  int64_t M, N, K;
+};
+// the bf16 operands of layout 0: a [M, K] b [N, K]; 1: a [M, K] b [K, N]; 2: a [K, M] b [K, N] (row-major, any row
+// stride)
+GemmDims gemm_operands(Args& args, const Tensor& a, const Tensor& b, int64_t layout) {
+  TORCH_CHECK(layout >= 0 && layout <= 2, args.op(), ": layout must be 0, 1 or 2, got ", layout);
+  args("a", a, at::kBFloat16, {kAny, kAny}, Layout::LastDimContiguous);
+  GemmDims d;
+  d.M = layout == 2 ? a.size(1) : a.size(0);
+  d.K = layout == 2 ? a.size(0) : a.size(1);
+  if (layout == 0) args("b", b, at::kBFloat16, {kAny, d.K}, Layout::LastDimContiguous);
+  else args("b", b, at::kBFloat16, {d.K, kAny}, Layout::LastDimContiguous);
+  d.N = layout == 0 ? b.size(0) : b.size(1);
+  return d;
+}
+
+// Returns out (allocated when not given).
 Tensor gemm(const Tensor& a, const Tensor& b, int64_t layout, const c10::optional<Tensor>& bias,
             const c10::optional<Tensor>& out_opt, bool accumulate, at::ScalarType out_dtype) {
-  TORCH_CHECK(a.is_cuda() && b.is_cuda() && a.dim() == 2 && b.dim() == 2, "gemm: 2-D CUDA tensors expected");
-  TORCH_CHECK(a.scalar_type() == at::kBFloat16 && b.scalar_type() == at::kBFloat16, "gemm: bf16 operands expected");
-  TORCH_CHECK(a.stride(1) == 1 && b.stride(1) == 1, "gemm: operands must be row-major");
-  c10::cuda::CUDAGuard guard(a.device());
-  int64_t M, N, K;
-  if (layout == 0) { M = a.size(0); K = a.size(1); N = b.size(0); TORCH_CHECK(b.size(1) == K, "gemm NT: K mismatch"); }
-  else if (layout == 1) { M = a.size(0); K = a.size(1); N = b.size(1); TORCH_CHECK(b.size(0) == K, "gemm NN: K mismatch"); }
-  else { K = a.size(0); M = a.size(1); N = b.size(1); TORCH_CHECK(b.size(0) == K, "gemm TN: K mismatch"); }
-  Tensor out;
-  int epi;
-  if (out_opt.has_value()) {
-    out = out_opt.value();
-    TORCH_CHECK(out.dim() == 2 && out.size(0) == M && out.size(1) == N && out.stride(1) == 1, "gemm: bad out shape");
-  } else {
-    auto opts = a.options().dtype(out_dtype);
-    out = (accumulate || (layout == 2 && out_dtype == at::kFloat)) ? at::zeros({M, N}, opts) : at::empty({M, N}, opts);
-  }
-  if (out.scalar_type() == at::kBFloat16) {
-    TORCH_CHECK(!accumulate, "gemm: accumulate needs an fp32 output");
-    epi = 0;
-  } else {
-    TORCH_CHECK(out.scalar_type() == at::kFloat, "gemm: out must be bf16 or fp32");
-    // a freshly zeroed wgrad output takes the accumulating epilogue too; a given `out` is added to only on request
-    epi = (accumulate || (layout == 2 && !out_opt.has_value())) ? 2 : 1;
-  }
-  const void* bias_ptr = nullptr;
-  if (bias.has_value() && bias->defined()) {
-    TORCH_CHECK(epi == 0 && bias->scalar_type() == at::kBFloat16 && bias->numel() == N, "gemm: bias must be bf16 [N]");
-    bias_ptr = bias->data_ptr();
-  }
+  Args args("gemm");
+  const auto [M, N, K] = gemm_operands(args, a, b, layout);
+  const void* bias_ptr = args.opt("bias", bias, at::kBFloat16, {N});
+  args.opt("out", out_opt, {at::kBFloat16, at::kFloat}, {M, N}, Layout::LastDimContiguous);
+  const at::ScalarType odt = given(out_opt) ? out_opt->scalar_type() : out_dtype;
+  TORCH_CHECK(odt == at::kBFloat16 || odt == at::kFloat, "gemm: out must be bf16 or fp32");
+  TORCH_CHECK(odt == at::kFloat || !accumulate, "gemm: accumulate needs an fp32 output");
+  // a freshly zeroed wgrad output takes the accumulating epilogue too; a given `out` is added to only on request
+  const int epi = odt == at::kBFloat16 ? 0 : (accumulate || (layout == 2 && !given(out_opt))) ? 2 : 1;
+  TORCH_CHECK(bias_ptr == nullptr || epi == 0, "gemm: a bias needs a bf16 output");
+  const auto guard = args.guard();
+  const auto opts = a.options().dtype(odt);
+  const Tensor out = given(out_opt) ? *out_opt : epi == 2 ? at::zeros({M, N}, opts) : at::empty({M, N}, opts);
   check(lb_gemm_bf16(a.data_ptr(), b.data_ptr(), out.data_ptr(), (int)M, (int)N, (int)K, (int)a.stride(0),
                      (int)b.stride(0), (int)out.stride(0), (int)layout, epi, bias_ptr, 0, nullptr, 0, 0, cur_stream()),
         "gemm");
@@ -84,20 +194,15 @@ Tensor gemm(const Tensor& a, const Tensor& b, int64_t layout, const c10::optiona
 // With `bias_grad` (fp32 [N], e.g. the bias' slice of main_grad) the column sums of the result are accumulated into it
 // by the GEMM epilogue.
 Tensor dgrad_actgrad(const Tensor& gy, const Tensor& w, const Tensor& pre, int64_t act, const c10::optional<Tensor>& bias_grad) {
-  TORCH_CHECK(gy.is_cuda() && gy.dim() == 2 && w.dim() == 2 && pre.dim() == 2, "dgrad_actgrad: 2-D CUDA tensors");
-  TORCH_CHECK(gy.scalar_type() == at::kBFloat16 && w.scalar_type() == at::kBFloat16 && pre.scalar_type() == at::kBFloat16,
-              "dgrad_actgrad: bf16 expected");
-  TORCH_CHECK(gy.stride(1) == 1 && w.stride(1) == 1 && pre.is_contiguous(), "dgrad_actgrad: row-major operands");
-  const int64_t M = gy.size(0), K = gy.size(1), N = w.size(1);
-  TORCH_CHECK(w.size(0) == K && pre.size(0) == M && pre.size(1) == N, "dgrad_actgrad: shape mismatch");
-  c10::cuda::CUDAGuard guard(gy.device());
+  Args args("dgrad_actgrad");
+  args("gy", gy, at::kBFloat16, {kAny, kAny}, Layout::LastDimContiguous);
+  const int64_t M = gy.size(0), K = gy.size(1);
+  args("w", w, at::kBFloat16, {K, kAny}, Layout::LastDimContiguous);
+  const int64_t N = w.size(1);
+  args("pre", pre, at::kBFloat16, {M, N});
+  float* colsum = args.opt<float>("bias_grad", bias_grad, at::kFloat, {N});
+  const auto guard = args.guard();
   Tensor out = at::empty({M, N}, gy.options());
-  float* colsum = nullptr;
-  if (bias_grad.has_value() && bias_grad->defined()) {
-    TORCH_CHECK(bias_grad->scalar_type() == at::kFloat && bias_grad->is_contiguous() && bias_grad->numel() == N && bias_grad->is_cuda(),
-                "dgrad_actgrad: bias_grad must be a contiguous fp32 CUDA tensor [N]");
-    colsum = bias_grad->data_ptr<float>();
-  }
   check(lb_gemm_bf16_actgrad(gy.data_ptr(), w.data_ptr(), out.data_ptr(), (int)M, (int)N, (int)K, (int)gy.stride(0),
                              (int)w.stride(0), (int)N, 1, (int)act, pre.data_ptr(), nullptr, cur_stream()),
         "dgrad_actgrad");
@@ -110,21 +215,21 @@ Tensor dgrad_actgrad(const Tensor& gy, const Tensor& w, const Tensor& pre, int64
   return out;
 }
 
+// x [M, K] and w [N, K] of a forward GEMM (bf16, row-major with any row stride); returns (M, N, K)
+GemmDims linear_operands(Args& args, const Tensor& x, const Tensor& w) {
+  args("x", x, at::kBFloat16, {kAny, kAny}, Layout::LastDimContiguous);
+  args("w", w, at::kBFloat16, {kAny, x.size(1)}, Layout::LastDimContiguous);
+  return {x.size(0), w.size(0), x.size(1)};
+}
+
 // y = x @ w^T + bias + residual (one kernel)
 Tensor linear_bias_residual(const Tensor& x, const Tensor& w, const c10::optional<Tensor>& bias, const Tensor& residual) {
-  TORCH_CHECK(x.is_cuda() && x.dim() == 2 && w.dim() == 2 && x.size(1) == w.size(1), "linear_bias_residual: shape mismatch");
-  TORCH_CHECK(x.scalar_type() == at::kBFloat16 && w.scalar_type() == at::kBFloat16 && residual.scalar_type() == at::kBFloat16,
-              "linear_bias_residual: bf16 expected");
-  TORCH_CHECK(x.stride(1) == 1 && w.stride(1) == 1 && residual.is_contiguous(), "linear_bias_residual: row-major operands");
-  const int64_t M = x.size(0), K = x.size(1), N = w.size(0);
-  TORCH_CHECK(residual.dim() == 2 && residual.size(0) == M && residual.size(1) == N, "linear_bias_residual: residual must be [M, N]");
-  c10::cuda::CUDAGuard guard(x.device());
+  Args args("linear_bias_residual");
+  const auto [M, N, K] = linear_operands(args, x, w);
+  const void* bias_ptr = args.opt("bias", bias, at::kBFloat16, {N});
+  args("residual", residual, at::kBFloat16, {M, N});
+  const auto guard = args.guard();
   Tensor y = at::empty({M, N}, x.options());
-  const void* bias_ptr = nullptr;
-  if (bias.has_value() && bias->defined()) {
-    TORCH_CHECK(bias->scalar_type() == at::kBFloat16 && bias->numel() == N, "linear_bias_residual: bias must be bf16 [N]");
-    bias_ptr = bias->data_ptr();
-  }
   check(lb_gemm_bf16_bias_residual(x.data_ptr(), w.data_ptr(), y.data_ptr(), (int)M, (int)N, (int)K, (int)x.stride(0),
                                    (int)w.stride(0), bias_ptr, residual.data_ptr(), cur_stream()),
         "linear_bias_residual");
@@ -134,19 +239,13 @@ Tensor linear_bias_residual(const Tensor& x, const Tensor& w, const c10::optiona
 // y = act(x @ w^T + bias); optionally also returns the pre-activation (for backward)
 std::tuple<Tensor, Tensor> linear_fwd(const Tensor& x, const Tensor& w, const c10::optional<Tensor>& bias, int64_t act,
                                       bool need_pre) {
-  TORCH_CHECK(x.is_cuda() && x.dim() == 2 && w.dim() == 2 && x.size(1) == w.size(1), "linear_fwd: shape mismatch");
-  TORCH_CHECK(x.scalar_type() == at::kBFloat16 && w.scalar_type() == at::kBFloat16, "linear_fwd: bf16 expected");
-  TORCH_CHECK(x.stride(1) == 1 && w.stride(1) == 1, "linear_fwd: row-major operands expected");
-  c10::cuda::CUDAGuard guard(x.device());
-  const int64_t M = x.size(0), K = x.size(1), N = w.size(0);
+  Args args("linear_fwd");
+  const auto [M, N, K] = linear_operands(args, x, w);
+  const void* bias_ptr = args.opt("bias", bias, at::kBFloat16, {N});
+  const auto guard = args.guard();
   Tensor y = at::empty({M, N}, x.options());
   Tensor pre;
   if (need_pre && act != 0) pre = at::empty({M, N}, x.options());
-  const void* bias_ptr = nullptr;
-  if (bias.has_value() && bias->defined()) {
-    TORCH_CHECK(bias->scalar_type() == at::kBFloat16 && bias->numel() == N, "linear_fwd: bias must be bf16 [N]");
-    bias_ptr = bias->data_ptr();
-  }
   check(lb_gemm_bf16(x.data_ptr(), w.data_ptr(), y.data_ptr(), (int)M, (int)N, (int)K, (int)x.stride(0),
                      (int)w.stride(0), (int)N, 0, 0, bias_ptr, (int)act, pre.defined() ? pre.data_ptr() : nullptr, 0, 0,
                      cur_stream()),
@@ -154,43 +253,29 @@ std::tuple<Tensor, Tensor> linear_fwd(const Tensor& x, const Tensor& w, const c1
   return std::make_tuple(y, pre.defined() ? pre : at::empty({0}, x.options()));
 }
 
-// FP8 (E4M3) weights with per-output-channel scales: w [N, K] float8_e4m3fn and w_scale fp32 [N] on x's device,
-// contiguous and 16-byte aligned, K % 16 == 0
-void check_fp8_weight(const Tensor& x, const Tensor& w, const Tensor& w_scale, const char* what) {
-  TORCH_CHECK(w.scalar_type() == at::kFloat8_e4m3fn && w.dim() == 2 && w.is_contiguous() && w.device() == x.device(),
-              what, ": w must be a contiguous float8_e4m3fn [N, K] tensor on x's device, got ", w.scalar_type(), " ",
-              w.sizes(), " on ", w.device());
-  TORCH_CHECK(w.size(0) >= 1 && w.size(1) >= 16 && w.size(1) % 16 == 0, what, ": K must be a positive multiple of 16, got ",
-              w.sizes());
-  TORCH_CHECK(w.size(0) <= INT32_MAX && w.size(1) <= INT32_MAX, what, ": N and K must fit in int32");
-  TORCH_CHECK(reinterpret_cast<uintptr_t>(w.data_ptr()) % 16 == 0, what, ": w must be 16-byte aligned");
-  TORCH_CHECK(w_scale.scalar_type() == at::kFloat && w_scale.dim() == 1 && w_scale.size(0) == w.size(0) &&
-                  w_scale.is_contiguous() && w_scale.device() == x.device(),
-              what, ": w_scale must be a contiguous fp32 [N] tensor on x's device, got ", w_scale.scalar_type(), " ",
-              w_scale.sizes(), " on ", w_scale.device());
+// FP8 (E4M3) weights with per-output-channel scales: w float8_e4m3fn [N, K] (16-byte aligned, K % 16 == 0) and
+// w_scale fp32 [N]
+void fp8_weight_args(Args& args, const Tensor& w, const Tensor& w_scale) {
+  args("w", w, at::kFloat8_e4m3fn, {kAny, kAny}, Layout::Contiguous, 16);
+  TORCH_CHECK(w.size(0) >= 1 && w.size(1) >= 16 && w.size(1) % 16 == 0, args.op(),
+              ": K must be a positive multiple of 16, got ", w.sizes());
+  TORCH_CHECK(w.size(0) <= INT32_MAX && w.size(1) <= INT32_MAX, args.op(), ": N and K must fit in int32");
+  args("w_scale", w_scale, at::kFloat, {w.size(0)});
 }
 
 // y [M, N] = act((x [M, K] · float(w)ᵀ) · w_scale + bias): the weight-streaming kernel for 1 <= M <= 64 (x bf16
 // contiguous and 16-byte aligned, bias bf16 [N] or None, act one of the ACT_* ids without the residual add)
 Tensor linear_fp8w(const Tensor& x, const Tensor& w, const Tensor& w_scale, const c10::optional<Tensor>& bias,
                    int64_t act) {
-  TORCH_CHECK(x.is_cuda() && x.scalar_type() == at::kBFloat16 && x.dim() == 2 && x.is_contiguous(),
-              "linear_fp8w: x must be a contiguous bf16 CUDA tensor [M, K], got ", x.scalar_type(), " ", x.sizes(),
-              " on ", x.device());
-  check_fp8_weight(x, w, w_scale, "linear_fp8w");
+  Args args("linear_fp8w");
+  args("x", x, at::kBFloat16, {kAny, kAny}, Layout::Contiguous, 16);
+  fp8_weight_args(args, w, w_scale);
   const int64_t M = x.size(0), K = x.size(1), N = w.size(0);
   TORCH_CHECK(w.size(1) == K, "linear_fp8w: x [M, K] and w [N, K] disagree on K: ", x.sizes(), " vs ", w.sizes());
   TORCH_CHECK(M >= 1 && M <= 64, "linear_fp8w: 1 <= M <= 64 rows, got ", M);
-  TORCH_CHECK(reinterpret_cast<uintptr_t>(x.data_ptr()) % 16 == 0, "linear_fp8w: x must be 16-byte aligned");
   TORCH_CHECK(act >= 0 && act <= 5, "linear_fp8w: act must be an activation id in [0, 5], got ", act);
-  const void* bias_ptr = nullptr;
-  if (bias.has_value() && bias->defined()) {
-    TORCH_CHECK(bias->scalar_type() == at::kBFloat16 && bias->dim() == 1 && bias->size(0) == N &&
-                    bias->is_contiguous() && bias->device() == x.device(),
-                "linear_fp8w: bias must be a contiguous bf16 [N] tensor on x's device");
-    bias_ptr = bias->data_ptr();
-  }
-  c10::cuda::CUDAGuard guard(x.device());
+  const void* bias_ptr = args.opt("bias", bias, at::kBFloat16, {N});
+  const auto guard = args.guard();
   Tensor y = at::empty({M, N}, x.options());
   const long ws = lb_linear_fp8w_workspace((int)M, (int)N, (int)K);
   Tensor part = ws > 0 ? at::empty({ws}, x.options().dtype(at::kFloat)) : Tensor();
@@ -202,9 +287,9 @@ Tensor linear_fp8w(const Tensor& x, const Tensor& w, const Tensor& w_scale, cons
 
 // bf16 [N, K] = bf16_rn(float(w) · w_scale[:, None]) (the weight the prefill GEMM of an FP8 linear multiplies)
 Tensor dequant_e4m3_rows(const Tensor& w, const Tensor& w_scale) {
-  TORCH_CHECK(w.is_cuda(), "dequant_e4m3_rows: w must be a CUDA tensor");
-  check_fp8_weight(w, w, w_scale, "dequant_e4m3_rows");
-  c10::cuda::CUDAGuard guard(w.device());
+  Args args("dequant_e4m3_rows");
+  fp8_weight_args(args, w, w_scale);
+  const auto guard = args.guard();
   Tensor out = at::empty(w.sizes(), w.options().dtype(at::kBFloat16));
   check(lb_dequant_e4m3_rows(w.data_ptr(), w_scale.data_ptr<float>(), out.data_ptr(), (long)w.size(0), (int)w.size(1),
                              cur_stream()),
@@ -215,8 +300,9 @@ Tensor dequant_e4m3_rows(const Tensor& w, const Tensor& w_scale) {
 // per-tensor E4M3 quantisation of a contiguous bf16 tensor: returns (q [same shape, float8_e4m3fn], deq fp32 [1]) with
 // x ≈ q * deq (deq = amax / 448); two kernels, no host synchronisation
 std::tuple<Tensor, Tensor> quantize_e4m3(const Tensor& x) {
-  TORCH_CHECK(x.is_cuda() && x.is_contiguous() && x.scalar_type() == at::kBFloat16, "quantize_e4m3: contiguous bf16 CUDA tensor");
-  c10::cuda::CUDAGuard guard(x.device());
+  Args args("quantize_e4m3");
+  args("x", x, at::kBFloat16, x.sizes(), Layout::Contiguous, 16);
+  const auto guard = args.guard();
   Tensor q = at::empty(x.sizes(), x.options().dtype(at::kFloat8_e4m3fn));
   Tensor scratch = at::zeros({2}, x.options().dtype(at::kFloat));   // [0] = dequantisation scale, [1] = amax bits (zeroed)
   check(lb_quant_e4m3(x.data_ptr(), q.data_ptr(), scratch.data_ptr<float>() + 1, scratch.data_ptr<float>(), (long)x.numel(),
@@ -232,31 +318,21 @@ std::tuple<Tensor, Tensor> linear_fp8_fwd(const Tensor& xq, const Tensor& wq, co
                                           const c10::optional<Tensor>& bias, int64_t act, bool want_pre,
                                           const c10::optional<Tensor>& residual, int64_t bn) {
   TORCH_CHECK(bn == 0 || bn == 64 || bn == 128 || bn == 192 || bn == 256, "linear_fp8_fwd: bn must be 0, 64, 128, 192 or 256");
-  const bool has_res = residual.has_value() && residual->defined();
-  TORCH_CHECK(!has_res || (act == 0 && !want_pre),
+  TORCH_CHECK(!given(residual) || (act == 0 && !want_pre),
               "linear_fp8_fwd: a residual epilogue takes no activation and no pre-activation copy");
-  TORCH_CHECK(xq.is_cuda() && xq.dim() == 2 && wq.dim() == 2 && xq.size(1) == wq.size(1), "linear_fp8_fwd: shape mismatch");
-  TORCH_CHECK(xq.scalar_type() == at::kFloat8_e4m3fn && wq.scalar_type() == at::kFloat8_e4m3fn, "linear_fp8_fwd: e4m3 operands");
-  TORCH_CHECK(xq.is_contiguous() && wq.is_contiguous(), "linear_fp8_fwd: contiguous operands");
-  TORCH_CHECK(deq_x.scalar_type() == at::kFloat && deq_w.scalar_type() == at::kFloat && deq_x.is_cuda() && deq_w.is_cuda(),
-              "linear_fp8_fwd: fp32 device scales");
+  Args args("linear_fp8_fwd");
+  args("xq", xq, at::kFloat8_e4m3fn, {kAny, kAny});
+  args("wq", wq, at::kFloat8_e4m3fn, {kAny, xq.size(1)});
+  args("deq_x", deq_x, at::kFloat, {1});
+  args("deq_w", deq_w, at::kFloat, {1});
   const int64_t M = xq.size(0), K = xq.size(1), N = wq.size(0);
   TORCH_CHECK(K % 16 == 0 && N % 8 == 0, "linear_fp8_fwd: K % 16 == 0 and N % 8 == 0 required");
-  c10::cuda::CUDAGuard guard(xq.device());
+  const void* bias_ptr = args.opt("bias", bias, at::kBFloat16, {N});
+  const void* res_ptr = args.opt("residual", residual, at::kBFloat16, {M, N});
+  const auto guard = args.guard();
   auto opts = xq.options().dtype(at::kBFloat16);
   Tensor y = at::empty({M, N}, opts);
   Tensor pre = want_pre ? at::empty({M, N}, opts) : Tensor();
-  const void* bias_ptr = nullptr;
-  if (bias.has_value() && bias->defined()) {
-    TORCH_CHECK(bias->scalar_type() == at::kBFloat16 && bias->numel() == N, "linear_fp8_fwd: bias must be bf16 [N]");
-    bias_ptr = bias->data_ptr();
-  }
-  const void* res_ptr = nullptr;
-  if (residual.has_value() && residual->defined()) {
-    TORCH_CHECK(residual->scalar_type() == at::kBFloat16 && residual->is_contiguous() && residual->numel() == M * N,
-                "linear_fp8_fwd: residual must be contiguous bf16 [M, N]");
-    res_ptr = residual->data_ptr();
-  }
   check(lb_gemm_fp8(xq.data_ptr(), wq.data_ptr(), y.data_ptr(), (int)M, (int)N, (int)K, bias_ptr, (int)act,
                     pre.defined() ? pre.data_ptr() : nullptr, res_ptr, deq_x.data_ptr<float>(), deq_w.data_ptr<float>(),
                     (int)bn, cur_stream()),
@@ -266,11 +342,9 @@ std::tuple<Tensor, Tensor> linear_fp8_fwd(const Tensor& xq, const Tensor& wq, co
 
 // raw entry used by tests / autotuning: explicit tile-N and split-K
 Tensor gemm_tuned(const Tensor& a, const Tensor& b, int64_t layout, int64_t bn, int64_t splits, bool fp32_out) {
-  c10::cuda::CUDAGuard guard(a.device());
-  int64_t M, N, K;
-  if (layout == 0) { M = a.size(0); K = a.size(1); N = b.size(0); }
-  else if (layout == 1) { M = a.size(0); K = a.size(1); N = b.size(1); }
-  else { K = a.size(0); M = a.size(1); N = b.size(1); }
+  Args args("gemm_tuned");
+  const auto [M, N, K] = gemm_operands(args, a, b, layout);
+  const auto guard = args.guard();
   const bool atomic = splits != 1;
   Tensor out = atomic ? at::zeros({M, N}, a.options().dtype(at::kFloat))
                       : at::empty({M, N}, a.options().dtype(fp32_out ? at::kFloat : at::kBFloat16));
@@ -291,7 +365,10 @@ int64_t gemm_schedule(int64_t schedule) {
 
 // gx = gy * act'(pre)
 Tensor act_bwd(const Tensor& gy, const Tensor& pre, int64_t act) {
-  c10::cuda::CUDAGuard guard(gy.device());
+  Args args("act_bwd");
+  args("gy", gy, at::kBFloat16, {kAny, kAny}, Layout::Contiguous, 16);
+  args("pre", pre, at::kBFloat16, gy.sizes(), Layout::Contiguous, 16);
+  const auto guard = args.guard();
   Tensor gx = at::empty_like(gy);
   check(lb_bias_act_bwd(gy.data_ptr(), pre.data_ptr(), nullptr, gx.data_ptr(), gy.size(0), (int)gy.size(1), (int)act,
                         cur_stream()),
@@ -299,13 +376,12 @@ Tensor act_bwd(const Tensor& gy, const Tensor& pre, int64_t act) {
   return gx;
 }
 
-// column sums of a bf16 [M, N] tensor.  With `accum` (fp32 [N], e.g. a bias' slice of the flat main-grad buffer) the
-// sums are added into it and an empty tensor is returned; otherwise a fresh bf16 [N] tensor.
 // embedding lookup on a (vocabulary shard of a) bf16 table; ids int64 (any shape) -> [ids.numel(), H]
 Tensor embedding_fwd(const Tensor& ids, const Tensor& table, int64_t vocab_start) {
-  c10::cuda::CUDAGuard guard(table.device());
-  TORCH_CHECK(ids.scalar_type() == at::kLong && ids.is_contiguous() && ids.is_cuda(), "embedding_fwd: contiguous int64 CUDA ids");
-  TORCH_CHECK(table.dim() == 2 && table.is_contiguous() && table.scalar_type() == at::kBFloat16, "embedding_fwd: contiguous bf16 table");
+  Args args("embedding_fwd");
+  args("table", table, at::kBFloat16, {kAny, kAny}, Layout::Contiguous, 16);
+  args("ids", ids, at::kLong, ids.sizes());
+  const auto guard = args.guard();
   const int64_t T = ids.numel(), H = table.size(1);
   Tensor out = at::empty({T, H}, table.options());
   check(lb_embedding_fwd(ids.data_ptr<int64_t>(), table.data_ptr(), out.data_ptr(), (long)T, (int)H, (long)vocab_start,
@@ -315,14 +391,11 @@ Tensor embedding_fwd(const Tensor& ids, const Tensor& table, int64_t vocab_start
 }
 // grad[ids - vocab_start] += gy   (grad: the parameter's fp32 main-grad view, same shape as the table)
 void embedding_bwd(const Tensor& ids, const Tensor& gy, Tensor grad, int64_t vocab_start) {
-  c10::cuda::CUDAGuard guard(gy.device());
-  TORCH_CHECK(ids.scalar_type() == at::kLong && ids.is_contiguous(), "embedding_bwd: contiguous int64 ids");
-  TORCH_CHECK(gy.is_cuda() && ids.device() == gy.device() && grad.device() == gy.device(),
-              "embedding_bwd: ids, gy and grad must be on one CUDA device");
-  TORCH_CHECK(gy.dim() == 2 && gy.is_contiguous() && gy.scalar_type() == at::kBFloat16 && gy.size(0) == ids.numel(),
-              "embedding_bwd: gy must be contiguous bf16 [ids.numel(), H]");
-  TORCH_CHECK(grad.dim() == 2 && grad.is_contiguous() && grad.scalar_type() == at::kFloat && grad.size(1) == gy.size(1),
-              "embedding_bwd: grad must be contiguous fp32 [rows, H]");
+  Args args("embedding_bwd");
+  args("gy", gy, at::kBFloat16, {ids.numel(), kAny}, Layout::Contiguous, 16);
+  args("ids", ids, at::kLong, ids.sizes());
+  args("grad", grad, at::kFloat, {kAny, gy.size(1)}, Layout::Contiguous, 16);
+  const auto guard = args.guard();
   const auto sorted = at::sort(ids.reshape({-1}), /*stable=*/true, /*dim=*/0, /*descending=*/false);
   check(lb_embedding_bwd(std::get<0>(sorted).data_ptr<int64_t>(), std::get<1>(sorted).data_ptr<int64_t>(), gy.data_ptr(),
                          grad.data_ptr<float>(), (long)ids.numel(), (int)gy.size(1), (long)vocab_start, (long)grad.size(0),
@@ -330,32 +403,28 @@ void embedding_bwd(const Tensor& ids, const Tensor& gy, Tensor grad, int64_t voc
         "embedding_bwd");
 }
 
+// column sums of a bf16 [M, N] tensor.  With `accum` (fp32 [N], e.g. a bias' slice of the flat main-grad buffer) the
+// sums are added into it and an empty tensor is returned; otherwise a fresh bf16 [N] tensor.
 Tensor colsum(const Tensor& x, const c10::optional<Tensor>& accum) {
-  c10::cuda::CUDAGuard guard(x.device());
-  TORCH_CHECK(x.dim() == 2 && x.is_contiguous() && x.scalar_type() == at::kBFloat16, "colsum: contiguous bf16 [M,N]");
-  if (accum.has_value() && accum->defined()) {
-    TORCH_CHECK(accum->scalar_type() == at::kFloat && accum->numel() == x.size(1) && accum->is_contiguous(),
-                "colsum: accum must be contiguous fp32 [N]");
-    Tensor ws = at::empty({(int64_t)lb_colsum_workspace_rows((int)x.size(0), (int)x.size(1)) * x.size(1)},
-                          x.options().dtype(at::kFloat));
-    check(lb_colsum(x.data_ptr(), accum->data_ptr<float>(), (int)x.size(0), (int)x.size(1), 1, ws.data_ptr<float>(),
-                    cur_stream()),
-          "colsum");
-    return at::empty({0}, x.options());
-  }
-  Tensor out = at::empty({x.size(1)}, x.options().dtype(at::kFloat));
-  Tensor ws = at::empty({(int64_t)lb_colsum_workspace_rows((int)x.size(0), (int)x.size(1)) * x.size(1)},
-                        x.options().dtype(at::kFloat));
-  check(lb_colsum(x.data_ptr(), out.data_ptr<float>(), (int)x.size(0), (int)x.size(1), 0, ws.data_ptr<float>(), cur_stream()),
+  Args args("colsum");
+  args("x", x, at::kBFloat16, {kAny, kAny});
+  const int64_t M = x.size(0), N = x.size(1);
+  float* acc = args.opt<float>("accum", accum, at::kFloat, {N});
+  const auto guard = args.guard();
+  Tensor out = acc != nullptr ? Tensor() : at::empty({N}, x.options().dtype(at::kFloat));
+  Tensor ws = at::empty({(int64_t)lb_colsum_workspace_rows((int)M, (int)N) * N}, x.options().dtype(at::kFloat));
+  check(lb_colsum(x.data_ptr(), acc != nullptr ? acc : out.data_ptr<float>(), (int)M, (int)N, acc != nullptr ? 1 : 0,
+                  ws.data_ptr<float>(), cur_stream()),
         "colsum");
-  return out.to(at::kBFloat16);
+  return acc != nullptr ? at::empty({0}, x.options()) : out.to(at::kBFloat16);
 }
 
 // ---- norms ----------------------------------------------------------------------------------------
 // The kernels read H elements of γ (and β) with no bounds of their own and are built for the (x, γ) dtype pairs
 // (bf16, bf16), (bf16, fp32) and (fp32, fp32).
-void check_norm_params(const char* what, const Tensor& x, const Tensor& gamma, const Tensor* beta) {
-  TORCH_CHECK(x.is_cuda() && x.dim() == 2 && x.is_contiguous(), what, ": x must be a contiguous CUDA tensor [rows, H]");
+void norm_args(Args& args, const Tensor& x, const Tensor& gamma, const Tensor* beta) {
+  const char* what = args.op();
+  args("x", x, {at::kBFloat16, at::kFloat}, {kAny, kAny});
   const bool pair_ok = (x.scalar_type() == at::kBFloat16 &&
                         (gamma.scalar_type() == at::kBFloat16 || gamma.scalar_type() == at::kFloat)) ||
                        (x.scalar_type() == at::kFloat && gamma.scalar_type() == at::kFloat);
@@ -372,14 +441,14 @@ void check_norm_params(const char* what, const Tensor& x, const Tensor& gamma, c
 
 std::tuple<Tensor, Tensor, Tensor> norm_fwd(const Tensor& x, const Tensor& gamma, const c10::optional<Tensor>& beta,
                                             double eps, bool rms) {
-  c10::cuda::CUDAGuard guard(x.device());
-  const bool has_beta = beta.has_value() && beta->defined();
-  check_norm_params("norm_fwd", x, gamma, has_beta ? &beta.value() : nullptr);
+  Args args("norm_fwd");
+  norm_args(args, x, gamma, given(beta) ? &beta.value() : nullptr);
+  const auto guard = args.guard();
   const int rows = (int)x.size(0), H = (int)x.size(1);
   Tensor y = at::empty_like(x);
   Tensor mean = rms ? at::empty({0}, x.options().dtype(at::kFloat)) : at::empty({rows}, x.options().dtype(at::kFloat));
   Tensor rstd = at::empty({rows}, x.options().dtype(at::kFloat));
-  const void* b = has_beta ? beta->data_ptr() : nullptr;
+  const void* b = given(beta) ? beta->data_ptr() : nullptr;
   check(lb_norm_fwd(x.data_ptr(), gamma.data_ptr(), b, y.data_ptr(), rms ? nullptr : mean.data_ptr<float>(),
                     rstd.data_ptr<float>(), rows, H, (float)eps, rms ? 1 : 0, dtype_code(x), dtype_code(gamma),
                     cur_stream()),
@@ -392,74 +461,88 @@ std::tuple<Tensor, Tensor, Tensor> norm_bwd(const Tensor& gy, const Tensor& x, c
                                             const c10::optional<Tensor>& dgamma_accum,
                                             const c10::optional<Tensor>& dbeta_accum,
                                             const c10::optional<Tensor>& gadd) {
-  c10::cuda::CUDAGuard guard(x.device());
-  check_norm_params("norm_bwd", x, gamma, nullptr);
-  TORCH_CHECK(gy.sizes() == x.sizes() && gy.scalar_type() == x.scalar_type() && gy.is_contiguous() &&
-                  gy.device() == x.device(),
-              "norm_bwd: gy must be contiguous with x's shape, dtype and device");
+  Args args("norm_bwd");
+  norm_args(args, x, gamma, nullptr);
   const int rows = (int)x.size(0), H = (int)x.size(1);
-  TORCH_CHECK(rstd.numel() == rows && (rms || mean.numel() == rows), "norm_bwd: mean / rstd must hold one value per row");
+  args("gy", gy, x.scalar_type(), x.sizes());
+  if (!rms) args("mean", mean, at::kFloat, {rows});
+  args("rstd", rstd, at::kFloat, {rows});
+  // accumulate mode: dgamma / dbeta are added straight into the fp32 main-grad slices of the parameters
+  const bool acc = given(dgamma_accum);
+  if (acc) {
+    args("dgamma_accum", *dgamma_accum, at::kFloat, {H});
+    TORCH_CHECK(!has_bias || given(dbeta_accum), "norm_bwd: dbeta_accum must be given with dgamma_accum when has_bias");
+    if (has_bias) args("dbeta_accum", *dbeta_accum, at::kFloat, {H});
+  }
+  // optional gradient of the skip connection around this norm: added to gx inside the kernel when supported
+  args.opt("gadd", gadd, kAnyDtype, x.sizes(), Layout::Strided);
+  const bool fuse_add = given(gadd) && lb_norm_bwd_supports_gadd(H) && gadd->is_contiguous() &&
+                        gadd->scalar_type() == x.scalar_type();
+  const auto guard = args.guard();
   Tensor gx = at::empty_like(x);
   auto fopt = x.options().dtype(at::kFloat);
-  // accumulate mode: dgamma / dbeta are added straight into the fp32 main-grad slices of the parameters
-  const bool acc = dgamma_accum.has_value() && dgamma_accum->defined();
-  if (acc) {
-    TORCH_CHECK(dgamma_accum->scalar_type() == at::kFloat && dgamma_accum->numel() == H && dgamma_accum->is_contiguous(),
-                "norm_bwd: dgamma_accum must be contiguous fp32 [H]");
-    TORCH_CHECK(!has_bias || (dbeta_accum.has_value() && dbeta_accum->defined() &&
-                              dbeta_accum->scalar_type() == at::kFloat && dbeta_accum->numel() == H &&
-                              dbeta_accum->is_contiguous()),
-                "norm_bwd: dbeta_accum must be contiguous fp32 [H]");
-  }
   Tensor dgamma = acc ? dgamma_accum.value() : at::empty({H}, fopt);
   Tensor dbeta = !has_bias ? at::empty({0}, fopt) : (acc ? dbeta_accum.value() : at::empty({H}, fopt));
   const int wrows = lb_norm_bwd_workspace_rows(rows);
   Tensor ws = at::empty({2 * (int64_t)wrows * H}, fopt);
-  // optional gradient of the skip connection around this norm: added to gx inside the kernel when supported
-  const bool has_add = gadd.has_value() && gadd->defined();
-  const bool fuse_add = has_add && lb_norm_bwd_supports_gadd(H) && gadd->is_contiguous() && gadd->scalar_type() == x.scalar_type();
   check(lb_norm_bwd(gy.data_ptr(), x.data_ptr(), gamma.data_ptr(), rms ? nullptr : mean.data_ptr<float>(),
                     rstd.data_ptr<float>(), gx.data_ptr(), dgamma.data_ptr<float>(),
                     has_bias ? dbeta.data_ptr<float>() : nullptr, ws.data_ptr<float>(), rows, H, rms ? 1 : 0,
                     dtype_code(x), dtype_code(gamma), acc ? 1 : 0, fuse_add ? gadd->data_ptr() : nullptr, cur_stream()),
         "norm_bwd");
-  if (has_add && !fuse_add) gx.add_(gadd->to(gx.scalar_type()));
+  if (given(gadd) && !fuse_add) gx.add_(gadd->to(gx.scalar_type()));
   if (acc) return std::make_tuple(gx, at::empty({0}, fopt), at::empty({0}, fopt));
   return std::make_tuple(gx, dgamma, dbeta);
 }
 
 // ---- elementwise ------------------------------------------------------------------------------------
+// The kernels load 8 bf16 values at a time from every operand: each is 16-byte aligned and, but for the [N] bias,
+// contiguous [rows, N] (N % 8 == 0, which the launchers check).
 Tensor bias_act_fwd(const Tensor& x, const c10::optional<Tensor>& bias, int64_t act) {
-  c10::cuda::CUDAGuard guard(x.device());
+  Args args("bias_act_fwd");
+  args("x", x, at::kBFloat16, {kAny, kAny}, Layout::Contiguous, 16);
+  const void* b = args.opt("bias", bias, at::kBFloat16, {x.size(1)}, Layout::Contiguous, 16);
+  const auto guard = args.guard();
   Tensor y = at::empty_like(x);
-  const void* b = (bias.has_value() && bias->defined()) ? bias->data_ptr() : nullptr;
   check(lb_bias_act_fwd(x.data_ptr(), b, y.data_ptr(), x.size(0), (int)x.size(1), (int)act, cur_stream()), "bias_act_fwd");
   return y;
 }
 Tensor bias_act_bwd(const Tensor& gy, const Tensor& x, const c10::optional<Tensor>& bias, int64_t act) {
-  c10::cuda::CUDAGuard guard(x.device());
+  Args args("bias_act_bwd");
+  args("x", x, at::kBFloat16, {kAny, kAny}, Layout::Contiguous, 16);
+  args("gy", gy, at::kBFloat16, x.sizes(), Layout::Contiguous, 16);
+  const void* b = args.opt("bias", bias, at::kBFloat16, {x.size(1)}, Layout::Contiguous, 16);
+  const auto guard = args.guard();
   Tensor gx = at::empty_like(x);
-  const void* b = (bias.has_value() && bias->defined()) ? bias->data_ptr() : nullptr;
   check(lb_bias_act_bwd(gy.data_ptr(), x.data_ptr(), b, gx.data_ptr(), x.size(0), (int)x.size(1), (int)act, cur_stream()),
         "bias_act_bwd");
   return gx;
 }
 Tensor bias_residual_fwd(const Tensor& x, const c10::optional<Tensor>& bias, const c10::optional<Tensor>& res) {
-  c10::cuda::CUDAGuard guard(x.device());
+  Args args("bias_residual_fwd");
+  args("x", x, at::kBFloat16, {kAny, kAny}, Layout::Contiguous, 16);
+  const void* b = args.opt("bias", bias, at::kBFloat16, {x.size(1)}, Layout::Contiguous, 16);
+  const void* r = args.opt("res", res, at::kBFloat16, x.sizes(), Layout::Contiguous, 16);
+  const auto guard = args.guard();
   Tensor y = at::empty_like(x);
-  const void* b = (bias.has_value() && bias->defined()) ? bias->data_ptr() : nullptr;
-  const void* r = (res.has_value() && res->defined()) ? res->data_ptr() : nullptr;
   check(lb_bias_residual(x.data_ptr(), b, r, y.data_ptr(), x.size(0), (int)x.size(1), cur_stream()), "bias_residual");
   return y;
 }
 Tensor swiglu_fwd(const Tensor& gate, const Tensor& up) {
-  c10::cuda::CUDAGuard guard(gate.device());
+  Args args("swiglu_fwd");
+  args("gate", gate, at::kBFloat16, gate.sizes(), Layout::Contiguous, 16);
+  args("up", up, at::kBFloat16, gate.sizes(), Layout::Contiguous, 16);
+  const auto guard = args.guard();
   Tensor y = at::empty_like(gate);
   check(lb_swiglu_fwd(gate.data_ptr(), up.data_ptr(), y.data_ptr(), gate.numel(), cur_stream()), "swiglu_fwd");
   return y;
 }
 std::tuple<Tensor, Tensor> swiglu_bwd(const Tensor& gy, const Tensor& gate, const Tensor& up) {
-  c10::cuda::CUDAGuard guard(gate.device());
+  Args args("swiglu_bwd");
+  args("gate", gate, at::kBFloat16, gate.sizes(), Layout::Contiguous, 16);
+  args("up", up, at::kBFloat16, gate.sizes(), Layout::Contiguous, 16);
+  args("gy", gy, at::kBFloat16, gate.sizes(), Layout::Contiguous, 16);
+  const auto guard = args.guard();
   Tensor dg = at::empty_like(gate), du = at::empty_like(up);
   check(lb_swiglu_bwd(gy.data_ptr(), gate.data_ptr(), up.data_ptr(), dg.data_ptr(), du.data_ptr(), gate.numel(),
                       cur_stream()),
@@ -467,18 +550,23 @@ std::tuple<Tensor, Tensor> swiglu_bwd(const Tensor& gy, const Tensor& gate, cons
   return std::make_tuple(dg, du);
 }
 // gu [T, 2F] = [gate | up] (one GEMM against the stacked gate / up weights) -> silu(gate) * up  [T, F]
+void swiglu_packed_args(Args& args, const Tensor& gu) {
+  args("gu", gu, at::kBFloat16, {kAny, kAny}, Layout::Contiguous, 16);
+  TORCH_CHECK(gu.size(1) % 16 == 0, args.op(), ": gu [T, 2F] needs F % 8 == 0, got ", gu.sizes());
+}
 Tensor swiglu_packed_fwd(const Tensor& gu) {
-  c10::cuda::CUDAGuard guard(gu.device());
-  TORCH_CHECK(gu.dim() == 2 && gu.is_contiguous() && gu.scalar_type() == at::kBFloat16 && gu.size(1) % 16 == 0,
-              "swiglu_packed_fwd: contiguous bf16 [T, 2F] with F % 8 == 0");
+  Args args("swiglu_packed_fwd");
+  swiglu_packed_args(args, gu);
+  const auto guard = args.guard();
   Tensor y = at::empty({gu.size(0), gu.size(1) / 2}, gu.options());
   check(lb_swiglu_packed_fwd(gu.data_ptr(), y.data_ptr(), gu.size(0), gu.size(1) / 2, cur_stream()), "swiglu_packed_fwd");
   return y;
 }
 Tensor swiglu_packed_bwd(const Tensor& gy, const Tensor& gu) {
-  c10::cuda::CUDAGuard guard(gu.device());
-  TORCH_CHECK(gy.is_contiguous() && gu.is_contiguous() && gy.dim() == 2 && gu.size(1) == 2 * gy.size(1) &&
-                  gy.scalar_type() == at::kBFloat16, "swiglu_packed_bwd: gy [T, F], gu [T, 2F] contiguous bf16");
+  Args args("swiglu_packed_bwd");
+  swiglu_packed_args(args, gu);
+  args("gy", gy, at::kBFloat16, {gu.size(0), gu.size(1) / 2}, Layout::Contiguous, 16);
+  const auto guard = args.guard();
   Tensor dgu = at::empty_like(gu);
   check(lb_swiglu_packed_bwd(gy.data_ptr(), gu.data_ptr(), dgu.data_ptr(), gu.size(0), gy.size(1), cur_stream()),
         "swiglu_packed_bwd");
@@ -507,15 +595,12 @@ PackedQKV packed_qkv(const Tensor& qkv, const char* what) {
   return g;
 }
 
-// per-token int32 [B, S] tensor of a packed batch (rope positions, attention doc_start) → device pointer or nullptr
-const int* token_index(const c10::optional<Tensor>& t, const Tensor& like, int B, int S, const char* what) {
-  if (!(t.has_value() && t->defined())) return nullptr;
-  TORCH_CHECK(t->scalar_type() == at::kInt, what, ": int32 expected, got ", t->scalar_type());
-  TORCH_CHECK(t->dim() == 2 && t->size(0) == B && t->size(1) == S, what, ": [", B, ", ", S, "] expected, got shape ",
-              t->sizes());
-  TORCH_CHECK(t->is_cuda() && t->device() == like.device(), what, ": must be on ", like.device(), ", got ", t->device());
-  TORCH_CHECK(t->is_contiguous(), what, ": must be contiguous");
-  return t->data_ptr<int>();
+// the cos / sin tables of a rotary embedding: fp32 [>= min_rows, D] of one shape
+void rope_tables(Args& args, const Tensor& cosv, const Tensor& sinv, int64_t min_rows, int64_t D) {
+  args("cos/sin", cosv, at::kFloat, {kAny, D});
+  args("cos/sin", sinv, at::kFloat, cosv.sizes());
+  TORCH_CHECK(cosv.size(0) >= min_rows, args.op(), ": cos/sin must have at least ", min_rows, " rows, got ",
+              cosv.sizes());
 }
 
 // packed projection [b, s, a, 3d] or [b, s, g, r + 2, d]; rotates every q and k (v copied).  inplace=true rewrites qkv
@@ -523,17 +608,14 @@ const int* token_index(const c10::optional<Tensor>& t, const Tensor& like, int B
 // s + pos_offset; values outside the tables are clamped to them.
 Tensor rope_qkv(const Tensor& qkv, const Tensor& cosv, const Tensor& sinv, int64_t pos_offset, bool backward,
                 bool inplace, const c10::optional<Tensor>& positions) {
-  c10::cuda::CUDAGuard guard(qkv.device());
-  TORCH_CHECK(qkv.is_contiguous() && qkv.scalar_type() == at::kBFloat16, "rope_qkv: contiguous bf16 packed projection");
+  Args args("rope_qkv");
+  args("qkv", qkv, at::kBFloat16, qkv.sizes());
   const PackedQKV g = packed_qkv(qkv, "rope_qkv");
   const int S = g.S, D = g.D;
   TORCH_CHECK(D % 2 == 0, "rope_qkv: head dim must be even");
-  const int* pos = token_index(positions, qkv, g.B, S, "rope_qkv: positions");
-  TORCH_CHECK(cosv.scalar_type() == at::kFloat && sinv.scalar_type() == at::kFloat && cosv.is_contiguous() &&
-                  sinv.is_contiguous() && cosv.size(0) >= (pos != nullptr ? 1 : S + pos_offset) && cosv.size(1) == D &&
-                  sinv.sizes() == cosv.sizes(),
-              "rope_qkv: cos/sin fp32 [>=S+offset, D]");
-  TORCH_CHECK(cosv.device() == qkv.device() && sinv.device() == qkv.device(), "rope_qkv: cos/sin must be on qkv's device");
+  const int* pos = args.opt<const int>("positions", positions, at::kInt, {g.B, S});
+  rope_tables(args, cosv, sinv, pos != nullptr ? 1 : S + pos_offset, D);
+  const auto guard = args.guard();
   Tensor y = inplace ? qkv : at::empty_like(qkv);
   check(lb_rope_qkv(qkv.data_ptr(), cosv.data_ptr<float>(), sinv.data_ptr<float>(), y.data_ptr(),
                     qkv.numel() / ((g.r + 2) * D), S, g.G, g.r, D, (int)pos_offset, pos, (int)cosv.size(0),
@@ -543,49 +625,50 @@ Tensor rope_qkv(const Tensor& qkv, const Tensor& cosv, const Tensor& sinv, int64
 }
 
 // ChatGLM rotary: the fused projection [b, s, (a + 2g) * d] <-> the packed layouts the attention kernels read (grouped
-// [b, s, g, a/g + 2, d] or per-head [b, s, a, 3d]).  `what` names the op in every error.
+// [b, s, g, a/g + 2, d] or per-head [b, s, a, 3d]).  `name` names the input in the errors.
 struct GlmRotary {
   int B, S, A, G, D;
   const int* positions;
 };
-GlmRotary glm_rotary_args(const Tensor& t, int64_t B, int64_t S, int64_t heads, int64_t kv_heads, int64_t D,
-                          const Tensor& table, int64_t pos_offset, const c10::optional<Tensor>& position_ids,
-                          const char* what) {
+GlmRotary glm_rotary_args(Args& args, const char* name, const Tensor& t, int64_t B, int64_t S, int64_t heads,
+                          int64_t kv_heads, int64_t D, const Tensor& table, int64_t pos_offset,
+                          const c10::optional<Tensor>& position_ids) {
+  const char* what = args.op();
   TORCH_CHECK(t.scalar_type() == at::kBFloat16, what, ": bf16 input expected, got ", t.scalar_type());
-  TORCH_CHECK(t.is_cuda() && t.is_contiguous(), what, ": contiguous CUDA input expected");
+  TORCH_CHECK(t.is_contiguous(), what, ": contiguous input expected");
+  args(name, t, at::kBFloat16, t.sizes());
   TORCH_CHECK(heads > 0 && kv_heads > 0 && heads % kv_heads == 0, what, ": heads (", heads,
               ") must be a positive multiple of kv_heads (", kv_heads, ")");
   TORCH_CHECK(D > 0 && D % 4 == 0, what, ": head dim must be a positive multiple of 4, got ", D);
   TORCH_CHECK(S > 0, what, ": empty sequence");
-  TORCH_CHECK(table.scalar_type() == at::kFloat && table.is_contiguous() && table.dim() == 3 && table.size(1) == D / 4 &&
-                  table.size(2) == 2,
-              what, ": table must be contiguous fp32 [P, d/4, 2] = [P, ", D / 4, ", 2], got ", table.scalar_type(), " ",
-              table.sizes());
-  TORCH_CHECK(table.device() == t.device(), what, ": table must be on ", t.device(), ", got ", table.device());
+  args("table", table, at::kFloat, {kAny, D / 4, 2});
+  TORCH_CHECK(!given(position_ids) || position_ids->scalar_type() == at::kInt, what, ": int32 position_ids expected, got ",
+              position_ids->scalar_type());
   GlmRotary g{(int)B, (int)S, (int)heads, (int)kv_heads, (int)D, nullptr};
-  g.positions = token_index(position_ids, t, g.B, g.S, what);
+  g.positions = args.opt<const int>("position_ids", position_ids, at::kInt, {B, S});
   const int64_t P = table.size(0);
-  if (g.positions != nullptr) {
-    // every sample takes the positions of the first row (one host sync)
-    const auto [lo, hi] = at::aminmax(position_ids->select(0, 0));
-    const int64_t mn = lo.item<int64_t>(), mx = hi.item<int64_t>();
-    TORCH_CHECK(mn >= 0 && mx < P, what, ": position_ids must lie in [0, ", P, "), got [", mn, ", ", mx, "]");
-  } else {
-    TORCH_CHECK(pos_offset >= 0 && pos_offset + S <= P, what, ": positions [", pos_offset, ", ", pos_offset + S,
-                ") exceed the table's ", P, " rows");
-  }
+  TORCH_CHECK(g.positions != nullptr || (pos_offset >= 0 && pos_offset + S <= P), what, ": positions [", pos_offset,
+              ", ", pos_offset + S, ") exceed the table's ", P, " rows");
   return g;
+}
+// every sample takes the positions of the first row (one host sync, after the other checks)
+void check_glm_positions(const char* what, const c10::optional<Tensor>& position_ids, int64_t P) {
+  if (!given(position_ids)) return;
+  const auto [lo, hi] = at::aminmax(position_ids->select(0, 0));
+  const int64_t mn = lo.item<int64_t>(), mx = hi.item<int64_t>();
+  TORCH_CHECK(mn >= 0 && mx < P, what, ": position_ids must lie in [0, ", P, "), got [", mn, ", ", mx, "]");
 }
 
 Tensor glm_rotary_qkv(const Tensor& mixed, int64_t heads, int64_t kv_heads, const Tensor& table, int64_t pos_offset,
                       const c10::optional<Tensor>& position_ids, bool grouped) {
-  c10::cuda::CUDAGuard guard(mixed.device());
   TORCH_CHECK(mixed.dim() == 3, "glm_rotary_qkv: fused projection [b, s, (a + 2g) * d] expected, got ", mixed.sizes());
   TORCH_CHECK(heads > 0 && kv_heads > 0 && mixed.size(2) % (heads + 2 * kv_heads) == 0, "glm_rotary_qkv: last dim ",
               mixed.size(2), " is not (heads + 2 * kv_heads) * d");
   const int64_t B = mixed.size(0), S = mixed.size(1), D = mixed.size(2) / (heads + 2 * kv_heads);
-  const GlmRotary g =
-      glm_rotary_args(mixed, B, S, heads, kv_heads, D, table, pos_offset, position_ids, "glm_rotary_qkv");
+  Args args("glm_rotary_qkv");
+  const GlmRotary g = glm_rotary_args(args, "mixed", mixed, B, S, heads, kv_heads, D, table, pos_offset, position_ids);
+  const auto guard = args.guard();
+  check_glm_positions("glm_rotary_qkv", position_ids, table.size(0));
   Tensor out = grouped ? at::empty({B, S, kv_heads, heads / kv_heads + 2, D}, mixed.options())
                        : at::empty({B, S, heads, 3 * D}, mixed.options());
   check(lb_glm_rotary_qkv(mixed.data_ptr(), table.data_ptr<float>(), out.data_ptr(), B * S, g.S, g.A, g.G, g.D,
@@ -597,7 +680,6 @@ Tensor glm_rotary_qkv(const Tensor& mixed, int64_t heads, int64_t kv_heads, cons
 // grad: the gradient of glm_rotary_qkv's output (its rank tells the layout) -> the gradient of the fused projection
 Tensor glm_rotary_qkv_bwd(const Tensor& grad, int64_t heads, int64_t kv_heads, const Tensor& table, int64_t pos_offset,
                           const c10::optional<Tensor>& position_ids) {
-  c10::cuda::CUDAGuard guard(grad.device());
   const bool grouped = grad.dim() == 5;
   TORCH_CHECK(heads > 0 && kv_heads > 0 && heads % kv_heads == 0, "glm_rotary_qkv_bwd: heads (", heads,
               ") must be a positive multiple of kv_heads (", kv_heads, ")");
@@ -607,8 +689,10 @@ Tensor glm_rotary_qkv_bwd(const Tensor& grad, int64_t heads, int64_t kv_heads, c
                   (grad.dim() == 4 && grad.size(2) == heads && grad.size(3) % 3 == 0),
               "glm_rotary_qkv_bwd: gradient [b, s, g, a/g + 2, d] or [b, s, a, 3d] expected, got ", grad.sizes());
   const int64_t B = grad.size(0), S = grad.size(1), D = grouped ? grad.size(4) : grad.size(3) / 3;
-  const GlmRotary g =
-      glm_rotary_args(grad, B, S, heads, kv_heads, D, table, pos_offset, position_ids, "glm_rotary_qkv_bwd");
+  Args args("glm_rotary_qkv_bwd");
+  const GlmRotary g = glm_rotary_args(args, "grad", grad, B, S, heads, kv_heads, D, table, pos_offset, position_ids);
+  const auto guard = args.guard();
+  check_glm_positions("glm_rotary_qkv_bwd", position_ids, table.size(0));
   Tensor dmixed = at::empty({B, S, (heads + 2 * kv_heads) * D}, grad.options());
   check(lb_glm_rotary_qkv(grad.data_ptr(), table.data_ptr<float>(), dmixed.data_ptr(), B * S, g.S, g.A, g.G, g.D,
                           (int)pos_offset, g.positions, grouped ? 1 : 0, 1, cur_stream()),
@@ -617,14 +701,11 @@ Tensor glm_rotary_qkv_bwd(const Tensor& grad, int64_t heads, int64_t kv_heads, c
 }
 
 Tensor rope(const Tensor& x, const Tensor& cosv, const Tensor& sinv, bool backward) {
-  c10::cuda::CUDAGuard guard(x.device());
-  TORCH_CHECK(x.dim() == 4 && x.is_contiguous() && x.scalar_type() == at::kBFloat16, "rope: contiguous bf16 [b,a,s,d]");
+  Args args("rope");
+  args("x", x, at::kBFloat16, {kAny, kAny, kAny, kAny});
   const int S = (int)x.size(2), D = (int)x.size(3);
-  TORCH_CHECK(cosv.scalar_type() == at::kFloat && sinv.scalar_type() == at::kFloat && cosv.is_contiguous() &&
-                  sinv.is_contiguous() && cosv.dim() == 2 && cosv.size(0) >= S && cosv.size(1) == D &&
-                  sinv.sizes() == cosv.sizes(),
-              "rope: cos/sin fp32 contiguous [>=S, D] of one shape");
-  TORCH_CHECK(cosv.device() == x.device() && sinv.device() == x.device(), "rope: cos/sin must be on x's device");
+  rope_tables(args, cosv, sinv, S, D);
+  const auto guard = args.guard();
   Tensor y = at::empty_like(x);
   check(lb_rope(x.data_ptr(), cosv.data_ptr<float>(), sinv.data_ptr<float>(), y.data_ptr(), x.numel() / D, S, D,
                 backward ? 1 : 0, cur_stream()),
@@ -633,9 +714,15 @@ Tensor rope(const Tensor& x, const Tensor& cosv, const Tensor& sinv, bool backwa
 }
 
 // ---- cross entropy ------------------------------------------------------------------------------------
+// logits bf16 or fp32 [T, V], labels int64 [T]
+void ce_args(Args& args, const Tensor& logits, const Tensor& labels) {
+  args("logits", logits, {at::kBFloat16, at::kFloat}, {kAny, kAny});
+  args("labels", labels, at::kLong, {logits.size(0)});
+}
 std::tuple<Tensor, Tensor, Tensor> ce_stats(const Tensor& logits, const Tensor& labels, int64_t vocab_start) {
-  c10::cuda::CUDAGuard guard(logits.device());
-  TORCH_CHECK(logits.dim() == 2 && logits.is_contiguous() && labels.scalar_type() == at::kLong, "ce_stats: bad args");
+  Args args("ce_stats");
+  ce_args(args, logits, labels);
+  const auto guard = args.guard();
   const int T = (int)logits.size(0), V = (int)logits.size(1);
   auto fopt = logits.options().dtype(at::kFloat);
   Tensor mx = at::empty({T}, fopt), se = at::empty({T}, fopt), tgt = at::empty({T}, fopt);
@@ -645,8 +732,12 @@ std::tuple<Tensor, Tensor, Tensor> ce_stats(const Tensor& logits, const Tensor& 
   return std::make_tuple(mx, se, tgt);
 }
 Tensor ce_bwd(const Tensor& logits, const Tensor& labels, const Tensor& lse, const Tensor& gloss, int64_t vocab_start) {
-  c10::cuda::CUDAGuard guard(logits.device());
+  Args args("ce_bwd");
+  ce_args(args, logits, labels);
   const int T = (int)logits.size(0), V = (int)logits.size(1);
+  args("lse", lse, at::kFloat, {T});
+  args("gloss", gloss, at::kFloat, {T});
+  const auto guard = args.guard();
   // in place: the saved logits buffer becomes dlogits (no second [T, V] allocation)
   Tensor d = logits;
   check(lb_ce_bwd(logits.data_ptr(), labels.data_ptr<int64_t>(), lse.data_ptr<float>(), gloss.data_ptr<float>(),
@@ -660,36 +751,25 @@ void fused_adamw(Tensor master, const Tensor& grad, Tensor m, Tensor v, const c1
                  const Tensor& scale, double lr, double b1, double b2, double eps, double wd, double bc1, double bc2,
                  bool decoupled) {
   // float4 loads and stores over master.numel() elements of every buffer
-  const auto dev = master.device();
-  for (const Tensor* t : {static_cast<const Tensor*>(&master), &grad, static_cast<const Tensor*>(&m),
-                          static_cast<const Tensor*>(&v)}) {
-    TORCH_CHECK(t->is_cuda() && t->device() == dev && t->scalar_type() == at::kFloat && t->is_contiguous() &&
-                    t->numel() == master.numel(),
-                "fused_adamw: master, grad, m and v must be contiguous fp32 tensors of one size on one CUDA device");
-    TORCH_CHECK(reinterpret_cast<uintptr_t>(t->data_ptr()) % 16 == 0, "fused_adamw: buffers must be 16-byte aligned");
-  }
+  Args args("fused_adamw");
+  args("master", master, at::kFloat, master.sizes(), Layout::Contiguous, 16);
+  args("grad", grad, at::kFloat, master.sizes(), Layout::Contiguous, 16);
+  args("m", m, at::kFloat, master.sizes(), Layout::Contiguous, 16);
+  args("v", v, at::kFloat, master.sizes(), Layout::Contiguous, 16);
   TORCH_CHECK(master.numel() % 4 == 0, "fused_adamw: numel must be a multiple of 4");
-  TORCH_CHECK(scale.is_cuda() && scale.device() == dev && scale.scalar_type() == at::kFloat && scale.numel() == 1,
-              "fused_adamw: scale must be a one-element fp32 tensor on the buffers' device");
-  void* lp = nullptr;
-  int lp_dtype = 0;
-  if (lp_out.has_value() && lp_out->defined()) {
-    TORCH_CHECK(lp_out->scalar_type() == at::kBFloat16 || lp_out->scalar_type() == at::kHalf,
-                "fused_adamw: lp_out must be bf16 or fp16");
-    TORCH_CHECK(lp_out->is_cuda() && lp_out->device() == dev && lp_out->is_contiguous() &&
-                    lp_out->numel() == master.numel() && reinterpret_cast<uintptr_t>(lp_out->data_ptr()) % 8 == 0,
-                "fused_adamw: lp_out must be contiguous, 8-byte aligned, of master's size and on its device");
-    lp = lp_out->data_ptr();
-    lp_dtype = lp_out->scalar_type() == at::kHalf ? 1 : 0;
-  }
-  c10::cuda::CUDAGuard guard(dev);
+  args("scale", scale, at::kFloat, {1});
+  void* lp = args.opt<void>("lp_out", lp_out, {at::kBFloat16, at::kHalf}, master.sizes(), Layout::Contiguous, 8);
+  const int lp_dtype = lp != nullptr && lp_out->scalar_type() == at::kHalf ? 1 : 0;
+  const auto guard = args.guard();
   check(lb_adamw(master.data_ptr<float>(), grad.data_ptr<float>(), m.data_ptr<float>(), v.data_ptr<float>(), lp, lp_dtype,
                  scale.data_ptr<float>(), master.numel(), (float)lr, (float)b1, (float)b2, (float)eps, (float)wd,
                  (float)bc1, (float)bc2, decoupled ? 1 : 0, cur_stream()),
         "fused_adamw");
 }
 Tensor sqnorm(const Tensor& x) {
-  c10::cuda::CUDAGuard guard(x.device());
+  Args args("sqnorm");
+  args("x", x, at::kFloat, x.sizes(), Layout::Contiguous, 16);
+  const auto guard = args.guard();
   Tensor out = at::zeros({1}, x.options().dtype(at::kFloat));
   Tensor ws = at::empty({(int64_t)lb_sqnorm_workspace(x.numel())}, x.options().dtype(at::kFloat));
   check(lb_sqnorm(x.data_ptr<float>(), out.data_ptr<float>(), x.numel(), ws.data_ptr<float>(), cur_stream()), "sqnorm");
@@ -722,20 +802,23 @@ lb::RngArgs next_rng(int64_t salt, uint64_t increment = 4) {
   return a;
 }
 
+
 // y = residual + dropout(x + bias, p); returns (y, rng_state int64[2]) — the backward is the same op on the output
 // gradient with `rng_state` passed back in (bias = residual = None)
 std::tuple<Tensor, Tensor> bias_dropout_residual(const Tensor& x, const c10::optional<Tensor>& bias,
                                                  const c10::optional<Tensor>& res, double p, int64_t salt,
                                                  const c10::optional<Tensor>& rng_state) {
-  c10::cuda::CUDAGuard guard(x.device());
-  TORCH_CHECK(x.is_cuda() && x.scalar_type() == at::kBFloat16 && x.is_contiguous() && x.dim() == 2, "bias_dropout_residual: bf16 contiguous 2-D");
+  Args args("bias_dropout_residual");
+  args("x", x, at::kBFloat16, {kAny, kAny}, Layout::Contiguous, 16);
+  const void* bptr = args.opt("bias", bias, at::kBFloat16, {x.size(1)}, Layout::Contiguous, 16);
+  const void* rptr = args.opt("res", res, at::kBFloat16, x.sizes(), Layout::Contiguous, 16);
+  const auto* rng_in = args.opt<const long long>("rng_state", rng_state, at::kLong, {2});
   TORCH_CHECK(p >= 0.0 && p < 1.0, "dropout probability must be in [0, 1)");
+  const auto guard = args.guard();
   Tensor y = at::empty_like(x);
-  const void* bptr = (bias.has_value() && bias->defined()) ? bias->data_ptr() : nullptr;
-  const void* rptr = (res.has_value() && res->defined()) ? res->data_ptr() : nullptr;
-  if (rng_state.has_value() && rng_state->defined()) {
+  if (rng_in != nullptr) {
     check(lb_bias_dropout_residual(x.data_ptr(), bptr, rptr, y.data_ptr(), x.size(0), (int)x.size(1), (float)p, nullptr,
-                                   reinterpret_cast<const long long*>(rng_state->data_ptr<int64_t>()), nullptr, cur_stream()),
+                                   rng_in, nullptr, cur_stream()),
           "bias_dropout_residual");
     return std::make_tuple(y, *rng_state);
   }
@@ -753,22 +836,19 @@ std::tuple<Tensor, Tensor> bias_dropout_residual(const Tensor& x, const c10::opt
 // (D contiguous).  Output o is allocated as [B, Sq, A, D] and returned as the [B, A, Sq, D] view, lse fp32 [B, A, Sq].
 // Key j is visible to query i of sample b iff kv_start[b] <= j < kv_lens[b] (defaults 0 and Sk) and, when causal,
 // j <= i + Sk - Sq.
-bool given(const c10::optional<Tensor>& t) { return t.has_value() && t->defined(); }
 
-// One flash-attention problem, validated: q, k, v as above, bf16 on one CUDA device; kv_lens / kv_start int32 [B];
-// doc_start int32 [B, Sq] (packed sequences); bias bf16 [B|1, A|1, Sq, Sk] with contiguous keys (broadcast dims get
-// stride 0); alibi_slopes fp32 [A]; p_drop in [0, 1).  `what` names the op in the error messages.
-lb::AttnArgs attn_args(const Tensor& q, const Tensor& k, const Tensor& v, bool causal, double scale,
+// One flash-attention problem, validated: q, k, v as above, bf16; kv_lens / kv_start int32 [B]; doc_start int32
+// [B, Sq] (packed sequences); bias bf16 [B|1, A|1, Sq, Sk] with contiguous keys (broadcast dims get stride 0);
+// alibi_slopes fp32 [A]; p_drop in [0, 1).
+lb::AttnArgs attn_args(Args& args, const Tensor& q, const Tensor& k, const Tensor& v, bool causal, double scale,
                        const c10::optional<Tensor>& kv_lens, const c10::optional<Tensor>& kv_start,
                        const c10::optional<Tensor>& doc_start, const c10::optional<Tensor>& bias,
-                       const c10::optional<Tensor>& alibi_slopes, double p_drop, const char* what) {
+                       const c10::optional<Tensor>& alibi_slopes, double p_drop) {
+  const char* what = args.op();
   TORCH_CHECK(q.dim() == 4 || q.dim() == 5, what, ": q must be [B, A, S, D] or [B, G, r, S, D]");
-  TORCH_CHECK(k.dim() == 4 && k.sizes() == v.sizes(), what, ": k, v must be [B, G, S, D] of one shape");
-  TORCH_CHECK(q.scalar_type() == at::kBFloat16 && k.scalar_type() == at::kBFloat16 && v.scalar_type() == at::kBFloat16,
-              what, ": q, k, v must be bf16, got ", q.scalar_type(), ", ", k.scalar_type(), ", ", v.scalar_type());
-  TORCH_CHECK(q.is_cuda() && k.device() == q.device() && v.device() == q.device(), what,
-              ": q, k, v must be on one CUDA device, got ", q.device(), ", ", k.device(), ", ", v.device());
-  TORCH_CHECK(q.stride(-1) == 1 && k.stride(3) == 1 && v.stride(3) == 1, what, ": D must be contiguous");
+  args("q", q, at::kBFloat16, q.sizes(), Layout::LastDimContiguous);
+  args("k", k, at::kBFloat16, {q.size(0), kAny, kAny, q.size(-1)}, Layout::LastDimContiguous);
+  args("v", v, at::kBFloat16, k.sizes(), Layout::LastDimContiguous);
   lb::AttnArgs a{};
   a.B = (int)q.size(0);
   a.G = (int)k.size(1);
@@ -788,7 +868,6 @@ lb::AttnArgs attn_args(const Tensor& q, const Tensor& k, const Tensor& v, bool c
     a.A = a.G * (int)q.size(2);
     for (int i = 0; i < 4; ++i) a.q_strides[i] = q.stride(i);
   }
-  TORCH_CHECK(k.size(0) == a.B && k.size(3) == a.d, what, ": k, v do not match q");
   TORCH_CHECK(a.d % 8 == 0 && a.d >= 8 && a.d <= 128, what, ": head dim must be a multiple of 8 in [8, 128], got ", a.d);
   TORCH_CHECK(a.Sq >= 1 && a.Sk >= 1, what, ": empty query or key sequence");
   for (int i = 0; i < 3; ++i) {
@@ -798,24 +877,11 @@ lb::AttnArgs attn_args(const Tensor& q, const Tensor& k, const Tensor& v, bool c
   a.causal = causal;
   a.scale = (float)scale;
   // per-sample key bound (kv_lens: end, kv_start: start of the visible keys)
-  auto key_bound = [&](const c10::optional<Tensor>& t, const char* name) -> const int* {
-    if (!given(t)) return nullptr;
-    TORCH_CHECK(t->scalar_type() == at::kInt, what, ": ", name, ": int32 expected, got ", t->scalar_type());
-    TORCH_CHECK(t->numel() == a.B, what, ": ", name, ": ", a.B, " elements (one per sample) expected, got shape ",
-                t->sizes());
-    TORCH_CHECK(t->is_cuda() && t->device() == q.device(), what, ": ", name, ": must be on ", q.device(), ", got ",
-                t->device());
-    TORCH_CHECK(t->is_contiguous(), what, ": ", name, ": must be contiguous");
-    return t->data_ptr<int>();
-  };
-  a.kv_lens = key_bound(kv_lens, "kv_lens");
-  a.kv_start = key_bound(kv_start, "kv_start");
-  a.doc_start = token_index(doc_start, q, a.B, a.Sq, (std::string(what) + ": doc_start").c_str());
+  a.kv_lens = args.opt<const int>("kv_lens", kv_lens, at::kInt, {a.B});
+  a.kv_start = args.opt<const int>("kv_start", kv_start, at::kInt, {a.B});
+  a.doc_start = args.opt<const int>("doc_start", doc_start, at::kInt, {a.B, a.Sq});
   if (given(bias)) {
-    const Tensor& b = *bias;
-    TORCH_CHECK(b.dim() == 4 && b.scalar_type() == at::kBFloat16 && b.stride(3) == 1 && b.size(2) == a.Sq &&
-                    b.size(3) == a.Sk && b.device() == q.device(),
-                what, ": attention bias: bf16 [B|1, A|1, Sq, Sk] on q's device with contiguous keys");
+    const Tensor& b = args("bias", *bias, at::kBFloat16, {kAny, kAny, a.Sq, a.Sk}, Layout::LastDimContiguous);
     TORCH_CHECK((b.size(0) == 1 || b.size(0) == a.B) && (b.size(1) == 1 || b.size(1) == a.A), what,
                 ": attention bias: bad broadcast shape");
     a.bias = b.data_ptr();
@@ -823,12 +889,7 @@ lb::AttnArgs attn_args(const Tensor& q, const Tensor& k, const Tensor& v, bool c
     a.bias_strides[1] = b.size(1) == 1 ? 0 : b.stride(1);
     a.bias_strides[2] = b.stride(2);
   }
-  if (given(alibi_slopes)) {
-    const Tensor& s = *alibi_slopes;
-    TORCH_CHECK(s.scalar_type() == at::kFloat && s.numel() == a.A && s.device() == q.device() && s.is_contiguous(),
-                what, ": alibi_slopes: contiguous fp32 [A] on q's device");
-    a.alibi_slopes = s.data_ptr<float>();
-  }
+  a.alibi_slopes = args.opt<const float>("alibi_slopes", alibi_slopes, at::kFloat, {a.A});
   TORCH_CHECK(p_drop < 1.0, "dropout probability must be in [0, 1)");
   a.p_drop = (float)p_drop;
   TORCH_CHECK(a.doc_start == nullptr || lb::attn_doc_start_supported(a), what,
@@ -842,9 +903,9 @@ std::tuple<Tensor, Tensor, Tensor> attn_fwd(const Tensor& q, const Tensor& k, co
                                             const c10::optional<Tensor>& kv_lens, const c10::optional<Tensor>& bias,
                                             const c10::optional<Tensor>& alibi_slopes, double p_drop, int64_t salt,
                                             const c10::optional<Tensor>& kv_start, const c10::optional<Tensor>& doc_start) {
-  const lb::AttnArgs a =
-      attn_args(q, k, v, causal, scale, kv_lens, kv_start, doc_start, bias, alibi_slopes, p_drop, "attn_fwd");
-  c10::cuda::CUDAGuard guard(q.device());
+  Args args("attn_fwd");
+  const lb::AttnArgs a = attn_args(args, q, k, v, causal, scale, kv_lens, kv_start, doc_start, bias, alibi_slopes, p_drop);
+  const auto guard = args.guard();
   Tensor o = at::empty({a.B, a.Sq, a.A, a.d}, q.options());
   Tensor lse = at::empty({a.B, a.A, a.Sq}, q.options().dtype(at::kFloat));
   const bool drop = p_drop > 0.0;
@@ -859,103 +920,64 @@ std::tuple<Tensor, Tensor, Tensor> attn_fwd(const Tensor& q, const Tensor& k, co
 }
 
 // ---- KV-cache decoding ------------------------------------------------------------------------------
-// The cache capacity C (rows per head) cannot be checked against the device-side lengths without a host sync: the
-// caller (libai_b200.inference.kv_cache.StaticKVCache) guarantees cache_seqlens[b] + Sq <= C before every call.
-void check_cache(const Tensor& k_cache, const Tensor& v_cache, const char* what,
-                 at::ScalarType dtype = at::kBFloat16) {
-  TORCH_CHECK(k_cache.is_cuda() && k_cache.scalar_type() == dtype && v_cache.scalar_type() == dtype, what, ": ",
-              dtype, " CUDA cache expected, got ", k_cache.scalar_type(), " and ", v_cache.scalar_type());
-  TORCH_CHECK(k_cache.dim() == 4 && k_cache.sizes() == v_cache.sizes() && k_cache.is_contiguous() && v_cache.is_contiguous(),
-              what, ": K and V caches must be contiguous [B, G, C, D] of the same shape");
-  TORCH_CHECK(k_cache.size(3) == 64 || k_cache.size(3) == 128, what, ": head dim must be 64 or 128");
-  TORCH_CHECK(reinterpret_cast<uintptr_t>(k_cache.data_ptr()) % 16 == 0 &&
-              reinterpret_cast<uintptr_t>(v_cache.data_ptr()) % 16 == 0, what, ": caches must be 16-byte aligned");
-}
-void check_lengths(const Tensor& t, int64_t B, const char* what) {
-  TORCH_CHECK(t.is_cuda() && t.scalar_type() == at::kInt && t.dim() == 1 && t.size(0) == B && t.is_contiguous(), what,
-              ": int32 CUDA [B] expected");
-}
-// the row scales of an FP8 (E4M3) cache [B, G, C, D]: contiguous fp32 [B, G, C] on `device`, C a multiple of 4 (the
-// decode kernel loads the scales of a tile from a 16-byte boundary)
-void check_scales(const c10::optional<Tensor>& scale, const Tensor& cache, const c10::Device& device,
-                  const char* what) {
-  TORCH_CHECK(given(scale), what, ": an FP8 cache needs k_scale and v_scale");
-  const Tensor& t = *scale;
-  TORCH_CHECK(t.scalar_type() == at::kFloat && t.dim() == 3 && t.size(0) == cache.size(0) &&
-                  t.size(1) == cache.size(1) && t.size(2) == cache.size(2) && t.is_contiguous() && t.device() == device,
-              what, ": scales: contiguous fp32 [B, G, C] on q's device expected, got ", t.scalar_type(), " ", t.sizes(),
-              " on ", t.device());
-  TORCH_CHECK(cache.size(2) % 4 == 0 && reinterpret_cast<uintptr_t>(t.data_ptr()) % 16 == 0, what,
-              ": an FP8 cache's capacity must be a multiple of 4 and its scales 16-byte aligned");
+// K and V caches [B, G, C, D], bf16 or (with row scales k_scale, v_scale fp32 [B, G, C]) FP8 (E4M3), D 64 or 128.  An
+// FP8 cache's capacity is a multiple of 4: the decode kernel loads the scales of a tile from a 16-byte boundary.  The
+// capacity C cannot be checked against the device-side lengths without a host sync: the caller
+// (libai_b200.inference.kv_cache.StaticKVCache) guarantees cache_seqlens[b] + Sq <= C before every call.
+void cache_args(Args& args, const Tensor& k_cache, const Tensor& v_cache, const Tensor* k_scale, const Tensor* v_scale,
+                at::IntArrayRef sizes) {
+  const at::ScalarType dtype = k_scale != nullptr ? at::kFloat8_e4m3fn : at::kBFloat16;
+  args("k_cache", k_cache, dtype, sizes, Layout::Contiguous, 16);
+  args("v_cache", v_cache, dtype, k_cache.sizes(), Layout::Contiguous, 16);
+  TORCH_CHECK(k_cache.size(3) == 64 || k_cache.size(3) == 128, args.op(), ": head dim must be 64 or 128");
+  if (k_scale != nullptr) {
+    TORCH_CHECK(k_cache.size(2) % 4 == 0, args.op(), ": an FP8 cache's capacity must be a multiple of 4");
+    args("k_scale", *k_scale, at::kFloat, k_cache.sizes().slice(0, 3), Layout::Contiguous, 16);
+    args("v_scale", *v_scale, at::kFloat, k_cache.sizes().slice(0, 3), Layout::Contiguous, 16);
+  }
 }
 
 // k, v of the packed projection qkv ([B, Sq, A, 3D] or grouped [B, Sq, G, r + 2, D]) go to rows cache_seqlens[b] + i
 // of the caches [B, G, C, D]; with cos/sin (fp32 [>= positions, D]) q and k are rotated first.  Returns the (rotated) q
-// as [B, Sq, G * r, D] when write_q, else empty.
-Tensor kv_append(const Tensor& qkv, const Tensor& k_cache, const Tensor& v_cache, const Tensor& cache_seqlens,
-                 const c10::optional<Tensor>& cosv, const c10::optional<Tensor>& sinv, bool write_q) {
-  c10::cuda::CUDAGuard guard(qkv.device());
-  check_cache(k_cache, v_cache, "kv_append");
-  const int B = (int)k_cache.size(0), G = (int)k_cache.size(1), C = (int)k_cache.size(2), D = (int)k_cache.size(3);
-  TORCH_CHECK(qkv.is_cuda() && qkv.scalar_type() == at::kBFloat16 && qkv.is_contiguous(),
-              "kv_append: contiguous bf16 packed projection expected");
-  const PackedQKV g = packed_qkv(qkv, "kv_append");
-  TORCH_CHECK(g.B == B && g.G == G && g.D == D, "kv_append: qkv does not match the cache");
-  const int Sq = g.S, A = G * g.r;
-  TORCH_CHECK(Sq >= 1 && Sq <= C, "kv_append: 1 <= Sq <= capacity");
-  check_lengths(cache_seqlens, B, "kv_append: cache_seqlens");
-  const float* cp = nullptr;
-  const float* sp = nullptr;
-  if (cosv.has_value() && cosv->defined()) {
-    TORCH_CHECK(sinv.has_value() && sinv->defined(), "kv_append: cos and sin go together");
-    TORCH_CHECK(cosv->scalar_type() == at::kFloat && sinv->scalar_type() == at::kFloat && cosv->is_contiguous() &&
-                sinv->is_contiguous() && cosv->dim() == 2 && cosv->size(1) == D && cosv->sizes() == sinv->sizes() &&
-                cosv->is_cuda(), "kv_append: cos/sin fp32 contiguous [positions, D]");
-    // like the capacity, the rows of the tables (positions up to cache_seqlens[b] + Sq - 1) are the caller's guarantee
-    cp = cosv->data_ptr<float>();
-    sp = sinv->data_ptr<float>();
-  }
+// as [B, Sq, G * r, D] when write_q, else empty.  With k_scale and v_scale the caches are FP8 (E4M3): the bf16 k row
+// before quantization is that of a bf16 cache, and each k and v row x is stored as the bytes e4m3_rn_satfinite(x / s)
+// with s = amax|x| / 448 (1 for a zero row).
+Tensor kv_append_any(const char* op, const Tensor& qkv, const Tensor& k_cache, const Tensor& v_cache,
+                     const Tensor* k_scale, const Tensor* v_scale, const Tensor& cache_seqlens,
+                     const c10::optional<Tensor>& cosv, const c10::optional<Tensor>& sinv, bool write_q) {
+  Args args(op);
+  args("qkv", qkv, at::kBFloat16, qkv.sizes());
+  const PackedQKV g = packed_qkv(qkv, op);
+  cache_args(args, k_cache, v_cache, k_scale, v_scale, {g.B, g.G, kAny, g.D});
+  const int B = g.B, G = g.G, C = (int)k_cache.size(2), D = g.D, Sq = g.S, A = G * g.r;
+  TORCH_CHECK(Sq >= 1 && Sq <= C, op, ": 1 <= Sq <= capacity");
+  args("cache_seqlens", cache_seqlens, at::kInt, {B});
+  TORCH_CHECK(given(cosv) == given(sinv), op, ": cos and sin go together");
+  // like the capacity, the rows of the tables (positions up to cache_seqlens[b] + Sq - 1) are the caller's guarantee
+  if (given(cosv)) rope_tables(args, *cosv, *sinv, 0, D);
+  const auto guard = args.guard();
   Tensor q_out = write_q ? at::empty({B, Sq, A, D}, qkv.options()) : at::empty({0}, qkv.options());
-  check(lb_kv_append(qkv.data_ptr(), cp, sp, write_q ? q_out.data_ptr() : nullptr, k_cache.data_ptr(),
-                     v_cache.data_ptr(), cache_seqlens.data_ptr<int>(), B, Sq, G, g.r, C, D, cur_stream()),
-        "kv_append");
+  const float* cp = given(cosv) ? cosv->data_ptr<float>() : nullptr;
+  const float* sp = given(sinv) ? sinv->data_ptr<float>() : nullptr;
+  void* qp = write_q ? q_out.data_ptr() : nullptr;
+  if (k_scale != nullptr)
+    check(lb_kv_append_fp8(qkv.data_ptr(), cp, sp, qp, k_cache.data_ptr(), v_cache.data_ptr(), k_scale->data_ptr<float>(),
+                           v_scale->data_ptr<float>(), cache_seqlens.data_ptr<int>(), B, Sq, G, g.r, C, D, cur_stream()),
+          op);
+  else
+    check(lb_kv_append(qkv.data_ptr(), cp, sp, qp, k_cache.data_ptr(), v_cache.data_ptr(), cache_seqlens.data_ptr<int>(),
+                       B, Sq, G, g.r, C, D, cur_stream()),
+          op);
   return q_out;
 }
-
-// kv_append into an FP8 (E4M3) cache with row scales k_scale, v_scale (fp32 [B, G, C]): q (returned when write_q) and
-// the bf16 k row before quantization are those of kv_append; each k and v row x is stored as the bytes
-// e4m3_rn_satfinite(x / s) with s = amax|x| / 448 (1 for a zero row).
+Tensor kv_append(const Tensor& qkv, const Tensor& k_cache, const Tensor& v_cache, const Tensor& cache_seqlens,
+                 const c10::optional<Tensor>& cosv, const c10::optional<Tensor>& sinv, bool write_q) {
+  return kv_append_any("kv_append", qkv, k_cache, v_cache, nullptr, nullptr, cache_seqlens, cosv, sinv, write_q);
+}
 Tensor kv_append_fp8(const Tensor& qkv, const Tensor& k_cache, const Tensor& v_cache, const Tensor& k_scale,
                      const Tensor& v_scale, const Tensor& cache_seqlens, const c10::optional<Tensor>& cosv,
                      const c10::optional<Tensor>& sinv, bool write_q) {
-  c10::cuda::CUDAGuard guard(qkv.device());
-  check_cache(k_cache, v_cache, "kv_append_fp8", at::kFloat8_e4m3fn);
-  check_scales(k_scale, k_cache, qkv.device(), "kv_append_fp8: k_scale");
-  check_scales(v_scale, v_cache, qkv.device(), "kv_append_fp8: v_scale");
-  const int B = (int)k_cache.size(0), G = (int)k_cache.size(1), C = (int)k_cache.size(2), D = (int)k_cache.size(3);
-  TORCH_CHECK(qkv.is_cuda() && qkv.scalar_type() == at::kBFloat16 && qkv.is_contiguous(),
-              "kv_append_fp8: contiguous bf16 packed projection expected");
-  const PackedQKV g = packed_qkv(qkv, "kv_append_fp8");
-  TORCH_CHECK(g.B == B && g.G == G && g.D == D, "kv_append_fp8: qkv does not match the cache");
-  const int Sq = g.S, A = G * g.r;
-  TORCH_CHECK(Sq >= 1 && Sq <= C, "kv_append_fp8: 1 <= Sq <= capacity");
-  check_lengths(cache_seqlens, B, "kv_append_fp8: cache_seqlens");
-  const float* cp = nullptr;
-  const float* sp = nullptr;
-  if (cosv.has_value() && cosv->defined()) {
-    TORCH_CHECK(sinv.has_value() && sinv->defined(), "kv_append_fp8: cos and sin go together");
-    TORCH_CHECK(cosv->scalar_type() == at::kFloat && sinv->scalar_type() == at::kFloat && cosv->is_contiguous() &&
-                sinv->is_contiguous() && cosv->dim() == 2 && cosv->size(1) == D && cosv->sizes() == sinv->sizes() &&
-                cosv->is_cuda(), "kv_append_fp8: cos/sin fp32 contiguous [positions, D]");
-    cp = cosv->data_ptr<float>();
-    sp = sinv->data_ptr<float>();
-  }
-  Tensor q_out = write_q ? at::empty({B, Sq, A, D}, qkv.options()) : at::empty({0}, qkv.options());
-  check(lb_kv_append_fp8(qkv.data_ptr(), cp, sp, write_q ? q_out.data_ptr() : nullptr, k_cache.data_ptr(),
-                         v_cache.data_ptr(), k_scale.data_ptr<float>(), v_scale.data_ptr<float>(),
-                         cache_seqlens.data_ptr<int>(), B, Sq, G, g.r, C, D, cur_stream()),
-        "kv_append_fp8");
-  return q_out;
+  return kv_append_any("kv_append_fp8", qkv, k_cache, v_cache, &k_scale, &v_scale, cache_seqlens, cosv, sinv, write_q);
 }
 
 // q [B, Sq, A, D] (any strides with D contiguous, e.g. a view of the packed projection) against the caches [B, G, C, D]
@@ -970,35 +992,22 @@ Tensor decode_attn(const Tensor& q, const Tensor& k_cache, const Tensor& v_cache
                    const Tensor& kv_start, double scale, int64_t splits, const c10::optional<Tensor>& alibi_slopes,
                    const c10::optional<Tensor>& rel_bias, bool causal, const c10::optional<Tensor>& k_scale,
                    const c10::optional<Tensor>& v_scale) {
-  c10::cuda::CUDAGuard guard(q.device());
+  Args args("decode_attn");
+  args("q", q, at::kBFloat16, {kAny, kAny, kAny, kAny}, Layout::LastDimContiguous, 16);
+  TORCH_CHECK(q.stride(0) % 8 == 0 && q.stride(1) % 8 == 0 && q.stride(2) % 8 == 0,
+              "decode_attn: q must be 16-byte aligned with strides that are multiples of 8");
   const bool fp8 = k_cache.scalar_type() == at::kFloat8_e4m3fn;
-  check_cache(k_cache, v_cache, "decode_attn", fp8 ? at::kFloat8_e4m3fn : at::kBFloat16);
-  if (fp8) {
-    check_scales(k_scale, k_cache, q.device(), "decode_attn: k_scale");
-    check_scales(v_scale, v_cache, q.device(), "decode_attn: v_scale");
-  } else {
-    TORCH_CHECK(!given(k_scale) && !given(v_scale), "decode_attn: k_scale and v_scale belong to an FP8 cache");
-  }
+  TORCH_CHECK(!fp8 || (given(k_scale) && given(v_scale)), "decode_attn: an FP8 cache needs k_scale and v_scale");
+  TORCH_CHECK(fp8 || (!given(k_scale) && !given(v_scale)), "decode_attn: k_scale and v_scale belong to an FP8 cache");
+  cache_args(args, k_cache, v_cache, fp8 ? &*k_scale : nullptr, fp8 ? &*v_scale : nullptr,
+             {q.size(0), kAny, kAny, q.size(3)});
   const int B = (int)k_cache.size(0), G = (int)k_cache.size(1), C = (int)k_cache.size(2), D = (int)k_cache.size(3);
-  TORCH_CHECK(q.is_cuda() && q.scalar_type() == at::kBFloat16 && q.dim() == 4 && q.stride(3) == 1,
-              "decode_attn: bf16 q [B, Sq, A, D] with D contiguous expected");
-  const int A = (int)q.size(2);
-  TORCH_CHECK(q.size(0) == B && A % G == 0 && q.size(3) == D, "decode_attn: q does not match the cache");
-  const int Sq = (int)q.size(1);
+  const int Sq = (int)q.size(1), A = (int)q.size(2);
+  TORCH_CHECK(A % G == 0, "decode_attn: the query heads must be a multiple of the cache heads");
   TORCH_CHECK(Sq >= 1 && Sq <= 16, "decode_attn: 1 <= Sq <= 16 new queries");
-  TORCH_CHECK(reinterpret_cast<uintptr_t>(q.data_ptr()) % 16 == 0 && q.stride(0) % 8 == 0 && q.stride(1) % 8 == 0 &&
-              q.stride(2) % 8 == 0, "decode_attn: q must be 16-byte aligned with strides that are multiples of 8");
-  check_lengths(cache_seqlens, B, "decode_attn: cache_seqlens");
-  check_lengths(kv_start, B, "decode_attn: kv_start");
-  const float* slopes = nullptr;
-  if (given(alibi_slopes)) {
-    const Tensor& s = *alibi_slopes;
-    TORCH_CHECK(s.scalar_type() == at::kFloat && s.dim() == 1 && s.size(0) == A && s.device() == q.device() &&
-                    s.is_contiguous(),
-                "decode_attn: alibi_slopes: contiguous fp32 [A] on q's device, got ", s.scalar_type(), " ", s.sizes(),
-                " on ", s.device());
-    slopes = s.data_ptr<float>();
-  }
+  args("cache_seqlens", cache_seqlens, at::kInt, {B});
+  args("kv_start", kv_start, at::kInt, {B});
+  const float* slopes = args.opt<const float>("alibi_slopes", alibi_slopes, at::kFloat, {A});
   const float* rel = nullptr;
   int R = 0;
   if (given(rel_bias)) {
@@ -1014,6 +1023,7 @@ Tensor decode_attn(const Tensor& q, const Tensor& k_cache, const Tensor& v_cache
   }
   TORCH_CHECK(causal || (slopes == nullptr && rel == nullptr),
               "decode_attn: causal=False takes no score bias (neither alibi_slopes nor rel_bias)");
+  const auto guard = args.guard();
   const int row_blocks = ((A / G) * Sq + 15) / 16;   // (query head, token) rows of one cache head, 16 per CTA
   const int nsplit = splits > 0 ? (int)std::min<int64_t>(splits, 32) : lb_decode_splits(B, G * row_blocks, C, D, fp8);
   Tensor o = at::empty({B, Sq, A, D}, q.options());
@@ -1035,11 +1045,10 @@ Tensor decode_attn(const Tensor& q, const Tensor& k_cache, const Tensor& v_cache
 // ---- shifted-window attention -----------------------------------------------------------------------
 // qkv [B, H*W, 3*C] in image order (per token [3, heads, d]), an H x W map of ws x ws windows cyclically shifted by
 // `shift`; table fp32 [(2ws - 1)^2, heads]; tau fp32 [heads] selects cosine attention (SwinV2).  Returns the head dim.
-int64_t check_window_args(const Tensor& qkv, int64_t H, int64_t W, int64_t ws, int64_t shift, int64_t heads,
-                          const Tensor& table, const c10::optional<Tensor>& tau, const char* what) {
-  TORCH_CHECK(qkv.is_cuda() && qkv.scalar_type() == at::kBFloat16 && qkv.dim() == 3 && qkv.is_contiguous(), what,
-              ": contiguous bf16 CUDA qkv [B, H*W, 3*C] expected");
-  TORCH_CHECK(reinterpret_cast<uintptr_t>(qkv.data_ptr()) % 16 == 0, what, ": qkv must be 16-byte aligned");
+int64_t window_args(Args& args, const Tensor& qkv, int64_t H, int64_t W, int64_t ws, int64_t shift, int64_t heads,
+                    const Tensor& table, const c10::optional<Tensor>& tau) {
+  const char* what = args.op();
+  args("qkv", qkv, at::kBFloat16, {kAny, kAny, kAny}, Layout::Contiguous, 16);
   TORCH_CHECK(heads >= 1 && heads <= 65535 && qkv.size(2) % (3 * heads) == 0, what, ": qkv width ", qkv.size(2),
               " is not 3 * heads * d for ", heads, " heads");
   const int64_t d = qkv.size(2) / (3 * heads);
@@ -1051,24 +1060,21 @@ int64_t check_window_args(const Tensor& qkv, int64_t H, int64_t W, int64_t ws, i
   TORCH_CHECK(qkv.size(1) == H * W, what, ": qkv has ", qkv.size(1), " tokens, the map ", H * W);
   TORCH_CHECK(qkv.size(0) * H * W <= INT32_MAX, what, ": more than 2^31 - 1 tokens");
   TORCH_CHECK(shift >= 0 && shift < ws, what, ": shift ", shift, " not supported (supported: 0 <= shift < window)");
-  TORCH_CHECK(table.is_cuda() && table.scalar_type() == at::kFloat && table.is_contiguous() && table.dim() == 2 &&
-                  table.size(0) == (2 * ws - 1) * (2 * ws - 1) && table.size(1) == heads,
-              what, ": table must be contiguous fp32 CUDA [(2 * window - 1)^2, heads]");
-  if (tau.has_value() && tau->defined())
-    TORCH_CHECK(tau->is_cuda() && tau->scalar_type() == at::kFloat && tau->is_contiguous() && tau->numel() == heads,
-                what, ": tau must be contiguous fp32 CUDA [heads]");
+  args("table", table, at::kFloat, {(2 * ws - 1) * (2 * ws - 1), heads});
+  args.opt("tau", tau, at::kFloat, {heads});
   return d;
 }
 
 std::tuple<Tensor, Tensor> window_attn_fwd(const Tensor& qkv, int64_t H, int64_t W, int64_t window, int64_t shift,
                                            int64_t heads, double scale, const Tensor& table,
                                            const c10::optional<Tensor>& tau) {
-  c10::cuda::CUDAGuard guard(qkv.device());
-  const int64_t d = check_window_args(qkv, H, W, window, shift, heads, table, tau, "window_attn_fwd");
+  Args args("window_attn_fwd");
+  const int64_t d = window_args(args, qkv, H, W, window, shift, heads, table, tau);
+  const auto guard = args.guard();
   const int64_t B = qkv.size(0), nwin = B * (H / window) * (W / window);
   Tensor o = at::empty({B, H * W, heads * d}, qkv.options());
   Tensor lse = at::empty({nwin, heads, window * window}, qkv.options().dtype(at::kFloat));
-  const bool cos = tau.has_value() && tau->defined();
+  const bool cos = given(tau);
   check(lb_window_attn_fwd(qkv.data_ptr(), o.data_ptr(), lse.data_ptr<float>(), table.data_ptr<float>(),
                            cos ? tau->data_ptr<float>() : nullptr, (int)B, (int)H, (int)W, (int)window, (int)shift,
                            (int)heads, (int)d, (float)scale, cur_stream()),
@@ -1080,17 +1086,13 @@ std::tuple<Tensor, Tensor> window_attn_fwd(const Tensor& qkv, int64_t H, int64_t
 std::tuple<Tensor, Tensor, Tensor> window_attn_bwd(const Tensor& dout, const Tensor& qkv, const Tensor& lse, int64_t H, int64_t W, int64_t window,
                                                    int64_t shift, int64_t heads, double scale, const Tensor& table,
                                                    const c10::optional<Tensor>& tau) {
-  c10::cuda::CUDAGuard guard(qkv.device());
-  const int64_t d = check_window_args(qkv, H, W, window, shift, heads, table, tau, "window_attn_bwd");
+  Args args("window_attn_bwd");
+  const int64_t d = window_args(args, qkv, H, W, window, shift, heads, table, tau);
   const int64_t B = qkv.size(0), N = window * window, nwin = B * (H / window) * (W / window);
-  TORCH_CHECK(dout.is_cuda() && dout.scalar_type() == at::kBFloat16 && dout.is_contiguous() &&
-                  dout.sizes() == at::IntArrayRef({B, H * W, heads * d}) &&
-                  reinterpret_cast<uintptr_t>(dout.data_ptr()) % 16 == 0,
-              "window_attn_bwd: dout must be a contiguous 16-byte aligned bf16 [B, H*W, C]");
-  TORCH_CHECK(lse.is_cuda() && lse.scalar_type() == at::kFloat && lse.is_contiguous() &&
-                  lse.sizes() == at::IntArrayRef({nwin, heads, N}),
-              "window_attn_bwd: lse must be the forward's fp32 [windows, heads, window^2]");
-  const bool cos = tau.has_value() && tau->defined();
+  args("dout", dout, at::kBFloat16, {B, H * W, heads * d}, Layout::Contiguous, 16);
+  args("lse", lse, at::kFloat, {nwin, heads, N});
+  const auto guard = args.guard();
+  const bool cos = given(tau);
   const int G = lb_window_attn_groups((int)B, (int)H, (int)W, (int)window, (int)heads);
   Tensor dqkv = at::empty_like(qkv);
   Tensor dtable = at::empty_like(table);
@@ -1118,21 +1120,22 @@ std::tuple<Tensor, Tensor, Tensor, Tensor> attn_bwd(const Tensor& dout, const Te
                                             double p_drop, const c10::optional<Tensor>& rng_state,
                                             const c10::optional<Tensor>& kv_start,
                                             const c10::optional<Tensor>& doc_start) {
-  const lb::AttnArgs a =
-      attn_args(q, k, v, causal, scale, kv_lens, kv_start, doc_start, bias, alibi_slopes, p_drop, "attn_bwd");
-  c10::cuda::CUDAGuard guard(q.device());
+  Args args("attn_bwd");
+  const lb::AttnArgs a = attn_args(args, q, k, v, causal, scale, kv_lens, kv_start, doc_start, bias, alibi_slopes, p_drop);
   const int B = a.B, A = a.A, G = a.G, Sq = a.Sq, Sk = a.Sk, D = a.d, r = A / G;
-  TORCH_CHECK(o.scalar_type() == at::kBFloat16 && o.device() == q.device() && o.sizes() == at::IntArrayRef({B, A, Sq, D}) &&
-                  o.stride(3) == 1,
-              "attn_bwd: o must be the forward's bf16 [B, A, Sq, D] with contiguous D");
-  TORCH_CHECK(dout.device() == q.device() && dout.sizes() == o.sizes(), "attn_bwd: dout must be [B, A, Sq, D] on q's device");
-  TORCH_CHECK(lse.scalar_type() == at::kFloat && lse.device() == q.device() && lse.is_contiguous() &&
-                  lse.sizes() == at::IntArrayRef({B, A, Sq}),
-              "attn_bwd: lse must be the forward's contiguous fp32 [B, A, Sq]");
+  args("o", o, at::kBFloat16, {B, A, Sq, D}, Layout::LastDimContiguous);
+  args("dout", dout, kAnyDtype, {B, A, Sq, D}, Layout::Strided);
+  args("lse", lse, at::kFloat, {B, A, Sq});
   const bool drop = p_drop > 0.0;
-  TORCH_CHECK(!drop || (given(rng_state) && rng_state->scalar_type() == at::kLong && rng_state->numel() == 2 &&
-                        rng_state->is_contiguous() && rng_state->device() == q.device()),
-              "attn_bwd: p_drop > 0 needs the forward's rng_state, int64 [2] on q's device");
+  TORCH_CHECK(!drop || given(rng_state), "attn_bwd: p_drop > 0 needs the forward's rng_state");
+  const auto* rng_in = drop ? args.opt<const long long>("rng_state", rng_state, at::kLong, {2}) : nullptr;
+  float* dbp = nullptr;
+  if (given(dbias)) {
+    TORCH_CHECK(given(bias), "attn_bwd: dbias needs bias");
+    dbp = args.opt<float>("dbias", dbias, at::kFloat, bias->sizes(), Layout::Strided);
+    TORCH_CHECK(dbias->strides() == bias->strides(), "attn_bwd: dbias must have the strides of bias");
+  }
+  const auto guard = args.guard();
   // Sq == Sk: gradients are produced in the packed [B, S, G, r + 2, D] layout (r = 1: [B, S, A, 3, D]) so that the QKV
   // dgrad/wgrad GEMMs read them directly; dq comes back in q's shape (a copy only for a 4-D q with r > 1).
   // Sq != Sk: dq is [B, Sq, G, r, D] and dk, dv are packed as [B, Sk, G, 2, D]; the returned dqkv is empty.
@@ -1162,17 +1165,9 @@ std::tuple<Tensor, Tensor, Tensor, Tensor> attn_bwd(const Tensor& dout, const Te
     dout_c.copy_(dout);
   }
   const long ds[3] = {dout_c.stride(0), dout_c.stride(1), dout_c.stride(2)};
-  float* dbp = nullptr;
-  if (given(dbias)) {
-    TORCH_CHECK(a.bias != nullptr && dbias->scalar_type() == at::kFloat && dbias->device() == q.device() &&
-                    dbias->sizes() == bias->sizes() && dbias->strides() == bias->strides(),
-                "attn_bwd: dbias must be fp32 with the shape/strides of bias");
-    dbp = dbias->data_ptr<float>();
-  }
   check(lb_attn_bwd(&a, dout_c.data_ptr(), ds, q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(),
                     lse.data_ptr<float>(), dq5.data_ptr(), dk.data_ptr(), dv.data_ptr(), dqs, dkvs,
-                    delta.data_ptr<float>(), dq_acc.data_ptr<float>(), dbp,
-                    drop ? reinterpret_cast<const long long*>(rng_state->data_ptr<int64_t>()) : nullptr,
+                    delta.data_ptr<float>(), dq_acc.data_ptr<float>(), dbp, rng_in,
                     reinterpret_cast<unsigned*>(dq_order.data_ptr<int>()), cur_stream()),
         "attn_bwd");
   Tensor dq = q.dim() == 5 ? dq5 : dq5.reshape({B, A, Sq, D});   // after the kernel: for r > 1 this copies
@@ -1182,7 +1177,7 @@ std::tuple<Tensor, Tensor, Tensor, Tensor> attn_bwd(const Tensor& dout, const Te
 // ---- fused collectives ---------------------------------------------------------------------------------------
 std::vector<long> to_longs(at::IntArrayRef v) { return std::vector<long>(v.begin(), v.end()); }
 
-const void* opt_ptr(const c10::optional<Tensor>& t) { return (t.has_value() && t->defined()) ? t->data_ptr() : nullptr; }
+const void* opt_ptr(const c10::optional<Tensor>& t) { return given(t) ? t->data_ptr() : nullptr; }
 
 // all-gather -> GEMM: y [M, N] = epilogue(all_gather(shard) @ op(w)); `gathered` is the local symmetric buffer [M, K]
 // whose remote rows the peers' copy CTAs fill during the kernel.  Epilogue: + bias, activation (returning the
@@ -1202,7 +1197,7 @@ std::tuple<Tensor, Tensor> ag_gemm(const Tensor& gathered, const Tensor& shard, 
   auto pb = to_longs(peer_buf), pf = to_longs(peer_flags), pd = to_longs(peer_done);
   Tensor out = at::empty({M, N}, gathered.options());
   Tensor pre = need_pre ? at::empty({M, N}, gathered.options()) : Tensor();
-  float* cs = (colsum.has_value() && colsum->defined()) ? colsum->data_ptr<float>() : nullptr;
+  float* cs = given(colsum) ? colsum->data_ptr<float>() : nullptr;
   check(lb_gemm_bf16_comm(gathered.data_ptr(), w.data_ptr(), out.data_ptr(), (int)M, (int)N, (int)K, (int)layout, 0,
                           opt_ptr(bias), (int)act, need_pre ? pre.data_ptr() : nullptr, opt_ptr(pre_in), cs, 1, (int)world,
                           (int)rank, pb.data(), pf.data(), pd.data(), state.data_ptr(), shard.data_ptr(), fill_local ? 1 : 0,
