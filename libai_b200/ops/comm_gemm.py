@@ -21,7 +21,8 @@ from typing import Dict, Tuple
 import torch
 
 from libai_b200.ops import count_launch, load_ext
-from libai_b200.ops.functional import _ACT_IDS, _bias_grad, reject_fp8_weight
+from libai_b200.ops import functional as OF
+from libai_b200.ops.functional import _ACT_IDS, reject_fp8_weight
 from libai_b200.parallel.symm_mem import CommWorkspace, get_workspace
 
 _BM = 128
@@ -191,25 +192,16 @@ def gemm_rs(x: torch.Tensor, w: torch.Tensor, bias, residual, group, layout: int
 
 
 def _wgrad_ag(gy, x_shard, w, group):
-    """dW of a column-parallel weight: fp32 accumulate into ``w.main_grad`` when the optimizer provides it."""
-    main_grad = getattr(w, "main_grad", None)
-    if main_grad is not None and main_grad.dtype == torch.float32 and main_grad.is_contiguous():
+    """dW of a column-parallel weight with the all-gather of ``x_shard`` inside the wgrad kernel; the destination
+    follows :func:`functional._weight_grad`'s rule."""
+    main_grad = OF._main_grad(w)
+    if main_grad is not None:
         ag_wgrad(gy, x_shard, main_grad, True, group)
         w.grad_added_to_main_grad = True
         return None
     out = torch.empty(w.shape, dtype=torch.float32, device=w.device)
     ag_wgrad(gy, x_shard, out, False, group)
     return out.to(w.dtype)
-
-
-def _wgrad_plain(ext, gy_full, x, w):
-    count_launch()
-    main_grad = getattr(w, "main_grad", None)
-    if main_grad is not None:
-        ext.gemm(gy_full, x, 2, None, main_grad, True, torch.float32)
-        w.grad_added_to_main_grad = True
-        return None
-    return ext.gemm(gy_full, x, 2, None, None, False, torch.float32).to(w.dtype)
 
 
 # --------------------------------------------------------------------------------------------------
@@ -222,7 +214,8 @@ class ColumnParallelLinearFused(torch.autograd.Function):
     @staticmethod
     def forward(ctx, x_shard, w, bias, act, group):
         has_act = act not in (None, "none")
-        need_pre = has_act and (x_shard.requires_grad or w.requires_grad)
+        # every gradient, the bias' alone included, goes through the activation backward, which reads the pre-activation
+        need_pre = has_act and any(ctx.needs_input_grad[:3])
         y, pre, gathered = ag_gemm(x_shard, w, bias, act if has_act else None, group, need_pre=need_pre)
         x_full = None
         if _SAVE_GATHERED and ctx.needs_input_grad[1]:
@@ -243,9 +236,9 @@ class ColumnParallelLinearFused(torch.autograd.Function):
         if ctx.needs_input_grad[0]:
             gx = gemm_rs(gy, w, None, None, ctx.group, layout=1)  # dy [M, N_loc] · W [N_loc, K]
         if ctx.needs_input_grad[1]:
-            gw = _wgrad_plain(ext, gy, x_full, w) if x_full is not None else _wgrad_ag(gy, x_shard, w, ctx.group)
-        if ctx.bias_param is not None and ctx.needs_input_grad[2]:
-            gb = _bias_grad(ext, gy, ctx.bias_param)
+            gw = OF._weight_grad(ext, gy, x_full, w) if x_full is not None else _wgrad_ag(gy, x_shard, w, ctx.group)
+        if ctx.needs_input_grad[2]:
+            gb = OF._bias_grad(ext, gy, ctx.bias_param)
         return gx, gw, gb, None, None
 
 
@@ -269,9 +262,9 @@ class RowParallelLinearFused(torch.autograd.Function):
         need_w = ctx.needs_input_grad[1]
         gx, _, gy_full = ag_gemm(gy_shard, w, None, None, ctx.group, layout=1, fill_local=need_w)  # dy_full [M, N] · W [N, K_loc]
         if need_w:
-            gw = _wgrad_plain(ext, gy_full, x, w)
-        if ctx.bias_param is not None and ctx.needs_input_grad[2]:
-            gb = _bias_grad(ext, gy_shard, ctx.bias_param)  # partial over token shards: summed over TP by sync_gradients
+            gw = OF._weight_grad(ext, gy_full, x, w)
+        if ctx.needs_input_grad[2]:
+            gb = OF._bias_grad(ext, gy_shard, ctx.bias_param)  # partial over token shards: summed over TP by sync_gradients
         return (gx if ctx.needs_input_grad[0] else None), gw, gb, (gy_shard if ctx.has_res else None), None
 
 
@@ -297,26 +290,22 @@ class TPMLPFused(torch.autograd.Function):
         x_shard, w1, w2, pre, h, x_full = ctx.saved_tensors
         gy_shard = gy_shard.contiguous()
         b1, b2 = ctx.b1, ctx.b2
-        fused_gb1 = None
-        if b1 is not None and ctx.needs_input_grad[2]:
-            mg = getattr(b1, "main_grad", None)
-            if mg is not None and mg.dtype == torch.float32 and mg.is_contiguous() and mg.data_ptr() % 16 == 0:
-                fused_gb1 = mg
+        fused_gb1 = OF._fused_bias_grad_target(b1) if ctx.needs_input_grad[2] else None
         need_w2 = ctx.needs_input_grad[3]
         # dpre = (all_gather(dy_shard) · W2) ⊙ act'(pre)   [+ column sums → b1.main_grad]
         dpre, _, gy_full = ag_gemm(gy_shard, w2, None, ctx.act, ctx.group, layout=1, pre_in=pre, colsum=fused_gb1,
                                    fill_local=need_w2)
-        gw2 = _wgrad_plain(ext, gy_full, h, w2) if need_w2 else None
-        gb2 = _bias_grad(ext, gy_shard, b2) if (b2 is not None and ctx.needs_input_grad[4]) else None
+        gw2 = OF._weight_grad(ext, gy_full, h, w2) if need_w2 else None
+        gb2 = OF._bias_grad(ext, gy_shard, b2) if ctx.needs_input_grad[4] else None
         gx = gemm_rs(dpre, w1, None, None, ctx.group, layout=1) if ctx.needs_input_grad[0] else None
         gw1 = None
         if ctx.needs_input_grad[1]:
-            gw1 = _wgrad_plain(ext, dpre, x_full, w1) if x_full is not None else _wgrad_ag(dpre, x_shard, w1, ctx.group)
+            gw1 = OF._weight_grad(ext, dpre, x_full, w1) if x_full is not None else _wgrad_ag(dpre, x_shard, w1, ctx.group)
         gb1 = None
         if fused_gb1 is not None:
             b1.grad_added_to_main_grad = True
-        elif b1 is not None and ctx.needs_input_grad[2]:
-            gb1 = _bias_grad(ext, dpre, b1)
+        elif ctx.needs_input_grad[2]:
+            gb1 = OF._bias_grad(ext, dpre, b1)
         return gx, gw1, gb1, gw2, gb2, (gy_shard if ctx.has_res else None), None, None
 
 

@@ -111,37 +111,66 @@ def _linear_fwd_any(ext, x2, w, bias, act_id, need_pre, residual=None):
     return ext.linear_fwd(x2, w, bias, act_id, need_pre)
 
 
+def _main_grad(p):
+    """``p.main_grad`` when it is an fp32 contiguous tensor (the optimizers' slice of their flat gradient buffer), else
+    None.  A native backward accumulates a parameter's gradient into this tensor and sets
+    ``p.grad_added_to_main_grad``, or, without it, returns the gradient to autograd in ``p``'s dtype; CUDA-graph
+    capture and ``sync_gradients`` rely on that choice."""
+    mg = getattr(p, "main_grad", None)
+    return mg if mg is not None and mg.dtype == torch.float32 and mg.is_contiguous() else None
+
+
+def _fused_bias_grad_target(bias):
+    """Where a dgrad GEMM epilogue may add the column sums of its result as ``bias``' gradient: ``_main_grad(bias)``
+    when ``ops.fused_bias_grad()`` is on and that slice is 16-byte aligned (the tensor-parallel epilogue adds into it
+    with vector reductions), else None."""
+    if not ops.fused_bias_grad():
+        return None
+    mg = _main_grad(bias)
+    return mg if mg is not None and mg.data_ptr() % 16 == 0 else None
+
+
 def _bias_grad(ext, g2, bias):
     """Column sums of ``g2`` as the gradient of ``bias``: accumulated straight into ``bias.main_grad`` (fp32 slice of
     the optimizer's flat gradient buffer) when the parameter owns one – no temporary, no bf16 round trip, no
     per-parameter add kernel later – otherwise returned as a tensor for autograd."""
     count_launch()
-    main_grad = getattr(bias, "main_grad", None)
-    if main_grad is not None and main_grad.dtype == torch.float32:
+    main_grad = _main_grad(bias)
+    if main_grad is not None:
         ext.colsum(g2, main_grad)
         bias.grad_added_to_main_grad = True
         return None
     return ext.colsum(g2).to(bias.dtype)
 
 
+def _weight_grad(ext, g, x, w):
+    """``gᵀ · x`` as the gradient of ``w``: a ``TN`` split-K GEMM accumulating in fp32 straight into ``w.main_grad``
+    when the parameter owns one (gradient-accumulation fusion), otherwise returned to autograd in ``w``'s dtype."""
+    count_launch()
+    main_grad = _main_grad(w)
+    if main_grad is not None:
+        ext.gemm(g, x, 2, None, main_grad, True, torch.float32)
+        w.grad_added_to_main_grad = True
+        return None
+    return ext.gemm(g, x, 2, None, None, False, torch.float32).to(w.dtype)
+
+
 class _LinearFn(torch.autograd.Function):
-    """Native linear: fwd ``NT`` GEMM with fused bias/activation epilogue, dgrad ``NN`` GEMM,
-    wgrad ``TN`` split-K GEMM accumulating in fp32 straight into ``weight.main_grad`` when the
-    parameter owns one (gradient-accumulation fusion)."""
+    """Native linear: fwd ``NT`` GEMM with fused bias/activation epilogue, dgrad ``NN`` GEMM, wgrad through
+    :func:`_weight_grad`.  With ``residual`` (no activation) the epilogue also adds it, and its gradient is ``gy``."""
 
     @staticmethod
-    def forward(ctx, x, w, bias, act):
+    def forward(ctx, x, w, bias, act, residual=None):
         ext = load_ext()
-        x2 = x.reshape(-1, x.shape[-1])
-        if not x2.is_contiguous():
-            x2 = x2.contiguous()
+        x2 = x.reshape(-1, x.shape[-1]).contiguous()
         # the backward runs whenever any input needs a gradient, and every gradient (the bias' alone included) goes
         # through the activation backward, which reads the pre-activation
         need_pre = act not in (None, "none") and any(ctx.needs_input_grad[:3])
-        y, pre = _linear_fwd_any(ext, x2, w, bias, _ACT_IDS[act], need_pre)
+        res2 = None if residual is None else residual.reshape(-1, w.shape[0]).contiguous()
+        y, pre = _linear_fwd_any(ext, x2, w, bias, _ACT_IDS[act], need_pre, res2)
         ctx.act = act
-        ctx.has_bias = bias is not None
         ctx.bias_param = bias
+        ctx.has_res = residual is not None
         ctx.save_for_backward(x2, w, pre if need_pre else None)
         ctx.x_shape = x.shape
         return y.view(*x.shape[:-1], w.shape[0])
@@ -150,9 +179,7 @@ class _LinearFn(torch.autograd.Function):
     def backward(ctx, gy):
         ext = load_ext()
         x2, w, pre = ctx.saved_tensors
-        g2 = gy.reshape(-1, gy.shape[-1])
-        if not g2.is_contiguous():
-            g2 = g2.contiguous()
+        g2 = gy.reshape(-1, gy.shape[-1]).contiguous()
         if ctx.act not in (None, "none"):
             g2 = ext.act_bwd(g2, pre, _ACT_IDS[ctx.act])
             count_launch()
@@ -162,17 +189,10 @@ class _LinearFn(torch.autograd.Function):
             count_launch()
             gx = gx.view(ctx.x_shape)
         if ctx.needs_input_grad[1]:
-            main_grad = getattr(w, "main_grad", None)
-            if main_grad is not None:
-                ext.gemm(g2, x2, 2, None, main_grad, True, torch.float32)  # TN accumulate
-                gw = None
-                w.grad_added_to_main_grad = True
-            else:
-                gw = ext.gemm(g2, x2, 2, None, None, False, torch.float32).to(w.dtype)
-            count_launch()
-        if ctx.has_bias and ctx.needs_input_grad[2]:
+            gw = _weight_grad(ext, g2, x2, w)
+        if ctx.needs_input_grad[2]:
             gb = _bias_grad(ext, g2, ctx.bias_param)
-        return gx, gw, gb, None
+        return gx, gw, gb, None, (gy if ctx.has_res else None)
 
 
 def reject_fp8_weight(what: str, *weights) -> None:
@@ -201,9 +221,7 @@ class _MLPFn(torch.autograd.Function):
     @staticmethod
     def forward(ctx, x, w1, b1, w2, act, b2=None, residual=None):
         ext = load_ext()
-        x2 = x.reshape(-1, x.shape[-1])
-        if not x2.is_contiguous():
-            x2 = x2.contiguous()
+        x2 = x.reshape(-1, x.shape[-1]).contiguous()
         h, pre = _linear_fwd_any(ext, x2, w1, b1, _ACT_IDS[act], True)
         # with a residual, the second bias and the block's residual add ride in the epilogue of the second GEMM
         res2 = residual.reshape(-1, w2.shape[0]).contiguous() if residual is not None else None
@@ -211,7 +229,6 @@ class _MLPFn(torch.autograd.Function):
         ctx.act = act
         ctx.save_for_backward(x2, w1, w2, pre, h)
         ctx.x_shape = x.shape
-        ctx.has_bias = b1 is not None
         ctx.bias_param = b1
         ctx.bias2_param = b2
         ctx.has_res = residual is not None
@@ -221,36 +238,20 @@ class _MLPFn(torch.autograd.Function):
     def backward(ctx, gy):
         ext = load_ext()
         x2, w1, w2, pre, h = ctx.saved_tensors
-        g2 = gy.reshape(-1, gy.shape[-1])
-        if not g2.is_contiguous():
-            g2 = g2.contiguous()
+        g2 = gy.reshape(-1, gy.shape[-1]).contiguous()
         # bias gradient of the first linear = column sums of dpre, accumulated into b1.main_grad by the dgrad call (a
         # column-sum pass with a fixed summation order, launched right behind the GEMM)
         b1 = ctx.bias_param
-        fused_gb1 = None
-        if ctx.has_bias and ctx.needs_input_grad[2] and ops.fused_bias_grad():
-            mg = getattr(b1, "main_grad", None)
-            if mg is not None and mg.dtype == torch.float32 and mg.is_contiguous():
-                fused_gb1 = mg
+        fused_gb1 = _fused_bias_grad_target(b1) if ctx.needs_input_grad[2] else None
         dpre = ext.dgrad_actgrad(g2, w2, pre, _ACT_IDS[ctx.act], fused_gb1)
         count_launch()
-
-        def wgrad(g, inp, w):
-            main_grad = getattr(w, "main_grad", None)
-            count_launch()
-            if main_grad is not None:
-                ext.gemm(g, inp, 2, None, main_grad, True, torch.float32)
-                w.grad_added_to_main_grad = True
-                return None
-            return ext.gemm(g, inp, 2, None, None, False, torch.float32).to(w.dtype)
-
-        gw2 = wgrad(g2, h, w2) if ctx.needs_input_grad[3] else None
-        gw1 = wgrad(dpre, x2, w1) if ctx.needs_input_grad[1] else None
+        gw2 = _weight_grad(ext, g2, h, w2) if ctx.needs_input_grad[3] else None
+        gw1 = _weight_grad(ext, dpre, x2, w1) if ctx.needs_input_grad[1] else None
         gb1 = None
         if fused_gb1 is not None:
             b1.grad_added_to_main_grad = True
-        elif ctx.has_bias and ctx.needs_input_grad[2]:
-            gb1 = _bias_grad(ext, dpre, ctx.bias_param)
+        elif ctx.needs_input_grad[2]:
+            gb1 = _bias_grad(ext, dpre, b1)
         gx = None
         if ctx.needs_input_grad[0]:
             gx = ext.gemm(dpre, w1, 1, None, None, False, torch.bfloat16).view(ctx.x_shape)
@@ -273,50 +274,11 @@ def mlp(x, w1, b1, w2, act: str = "gelu", b2=None, residual=None):
     return y if residual is None else y + residual
 
 
-class _LinearResidualFn(torch.autograd.Function):
-    """``x @ wᵀ + bias + residual`` with bias and residual added in the GEMM epilogue."""
-
-    @staticmethod
-    def forward(ctx, x, w, bias, residual):
-        ext = load_ext()
-        x2 = x.reshape(-1, x.shape[-1])
-        if not x2.is_contiguous():
-            x2 = x2.contiguous()
-        y, _ = _linear_fwd_any(ext, x2, w, bias, 0, False, residual.reshape(-1, w.shape[0]).contiguous())
-        ctx.bias_param = bias
-        ctx.save_for_backward(x2, w)
-        ctx.x_shape = x.shape
-        return y.view(*x.shape[:-1], w.shape[0])
-
-    @staticmethod
-    def backward(ctx, gy):
-        ext = load_ext()
-        x2, w = ctx.saved_tensors
-        g2 = gy.reshape(-1, gy.shape[-1])
-        if not g2.is_contiguous():
-            g2 = g2.contiguous()
-        gx = gw = gb = None
-        if ctx.needs_input_grad[0]:
-            gx = ext.gemm(g2, w, 1, None, None, False, torch.bfloat16).view(ctx.x_shape)
-            count_launch()
-        if ctx.needs_input_grad[1]:
-            main_grad = getattr(w, "main_grad", None)
-            if main_grad is not None:
-                ext.gemm(g2, x2, 2, None, main_grad, True, torch.float32)
-                w.grad_added_to_main_grad = True
-            else:
-                gw = ext.gemm(g2, x2, 2, None, None, False, torch.float32).to(w.dtype)
-            count_launch()
-        if ctx.bias_param is not None and ctx.needs_input_grad[2]:
-            gb = _bias_grad(ext, g2, ctx.bias_param)
-        return gx, gw, gb, gy
-
-
 def linear_bias_residual(x, w, bias, residual):
     """``x @ wᵀ + bias + residual`` (output projection of a block, dropout-free)."""
     reject_fp8_weight("linear_bias_residual", w)
     if use_native(x, w) and _gemm_ok(x, w) and residual is not None and residual.dtype == torch.bfloat16:
-        return _LinearResidualFn.apply(x, w, bias, residual)
+        return _LinearFn.apply(x, w, bias, None, residual)
     y = linear(x, w, bias)
     return y if residual is None else y + residual
 
@@ -405,9 +367,9 @@ class _LayerNormFn(torch.autograd.Function):
         g2 = gy.reshape(-1, gy.shape[-1]).contiguous()
         gadd = None if gskip is None else gskip.reshape(-1, gskip.shape[-1]).contiguous()
         count_launch(2)
-        wg = getattr(weight, "main_grad", None)
-        bg = getattr(ctx.bias_param, "main_grad", None) if ctx.has_bias else None
-        if wg is not None and wg.dtype == torch.float32 and (not ctx.has_bias or bg is not None):
+        wg = _main_grad(weight)
+        bg = _main_grad(ctx.bias_param) if ctx.has_bias else None
+        if wg is not None and (not ctx.has_bias or bg is not None):
             # dγ / dβ are reduced straight into the fp32 main-grad slices (one kernel for both)
             gx, _, _ = ext.norm_bwd(g2, x2, weight, mean, rstd, ctx.rms, ctx.has_bias, wg, bg, gadd)
             weight.grad_added_to_main_grad = True
@@ -1157,8 +1119,8 @@ class _EmbeddingFn(torch.autograd.Function):
         g2 = gy.reshape(-1, gy.shape[-1]).contiguous()
         ext = load_ext()
         count_launch()
-        main_grad = getattr(table, "main_grad", None)
-        if main_grad is not None and main_grad.dtype == torch.float32:
+        main_grad = _main_grad(table)
+        if main_grad is not None:
             ext.embedding_bwd(flat, g2, main_grad, ctx.vocab_start)
             table.grad_added_to_main_grad = True
             return None, None, None

@@ -19,6 +19,7 @@ from typing import Optional, Tuple
 import torch
 
 from libai_b200.ops import count_launch, load_ext
+from libai_b200.ops import functional as OF
 from libai_b200.ops.functional import reject_fp8_weight
 
 _ENABLED = os.environ.get("LIBAI_B200_FUSED_GATE_UP", "1") == "1"
@@ -45,17 +46,17 @@ def fused_gate_up_views(wg: torch.Tensor, wu: torch.Tensor) -> Optional[Tuple[to
         return None
     f, k = wg.shape
     w = torch.as_strided(wg.detach(), (2 * f, k), (k, 1))
-    g1, g2 = getattr(wg, "main_grad", None), getattr(wu, "main_grad", None)
+    g1, g2 = OF._main_grad(wg), OF._main_grad(wu)
     mg = None
-    if g1 is not None and g2 is not None and g1.dtype == torch.float32 and _adjacent(g1, g2):
+    if g1 is not None and g2 is not None and _adjacent(g1, g2):
         mg = torch.as_strided(g1, (2 * f, k), (k, 1))
     return w, mg
 
 
-def _finish_wgrad(wg, wu, mg, out):
-    """Bookkeeping after the fused wgrad: gradients already sit in ``main_grad`` (return ``None`` to autograd), or split
-    the freshly computed ``[2F, K]`` fp32 gradient between the two parameters."""
-    if mg is not None:
+def _gate_up_grads(wg, wu, out):
+    """Autograd's gradients of the gate and up weights after the ``[2F, K]`` wgrad: ``None`` for both when it
+    accumulated into the fused ``main_grad`` view (``out`` is None), else the halves of its fresh fp32 result."""
+    if out is None:
         wg.grad_added_to_main_grad = True
         wu.grad_added_to_main_grad = True
         return None, None
@@ -70,9 +71,7 @@ class GatedMLPFn(torch.autograd.Function):
     def forward(ctx, x, wg, wu, wd):
         ext = load_ext()
         w, _ = fused_gate_up_views(wg, wu)
-        x2 = x.reshape(-1, x.shape[-1])
-        if not x2.is_contiguous():
-            x2 = x2.contiguous()
+        x2 = x.reshape(-1, x.shape[-1]).contiguous()
         gu = ext.gemm(x2, w, 0, None, None, False, torch.bfloat16)
         h = ext.swiglu_packed_fwd(gu)
         y = ext.gemm(h, wd, 0, None, None, False, torch.bfloat16)
@@ -87,29 +86,20 @@ class GatedMLPFn(torch.autograd.Function):
         x2, gu, h = ctx.saved_tensors
         wg, wu, wd = ctx.params
         w, mg = fused_gate_up_views(wg, wu)
-        g2 = gy.reshape(-1, gy.shape[-1])
-        if not g2.is_contiguous():
-            g2 = g2.contiguous()
+        g2 = gy.reshape(-1, gy.shape[-1]).contiguous()
         dh = ext.gemm(g2, wd, 1, None, None, False, torch.bfloat16)
-        gwd = None
-        if ctx.needs_input_grad[3]:
-            md = getattr(wd, "main_grad", None)
-            if md is not None:
-                ext.gemm(g2, h, 2, None, md, True, torch.float32)
-                wd.grad_added_to_main_grad = True
-            else:
-                gwd = ext.gemm(g2, h, 2, None, None, False, torch.float32).to(wd.dtype)
-            count_launch()
+        gwd = OF._weight_grad(ext, g2, h, wd) if ctx.needs_input_grad[3] else None
         dgu = ext.swiglu_packed_bwd(dh, gu)
         gx = ext.gemm(dgu, w, 1, None, None, False, torch.bfloat16).view(*gy.shape[:-1], x2.shape[1]) if ctx.needs_input_grad[0] else None
         gwg = gwu = None
         if ctx.needs_input_grad[1] or ctx.needs_input_grad[2]:
+            out = None
             if mg is not None:
                 ext.gemm(dgu, x2, 2, None, mg, True, torch.float32)
-                gwg, gwu = _finish_wgrad(wg, wu, mg, None)
             else:
-                gwg, gwu = _finish_wgrad(wg, wu, None, ext.gemm(dgu, x2, 2, None, None, False, torch.float32))
+                out = ext.gemm(dgu, x2, 2, None, None, False, torch.float32)
             count_launch()
+            gwg, gwu = _gate_up_grads(wg, wu, out)
         count_launch(3)
         return gx, gwg, gwu, gwd
 
@@ -143,19 +133,19 @@ class TPGatedMLPFused(torch.autograd.Function):
         gy_shard = gy_shard.contiguous()
         need_wd = ctx.needs_input_grad[3]
         dh, _, gy_full = comm_gemm.ag_gemm(gy_shard, wd, None, None, ctx.group, layout=1, fill_local=need_wd)
-        gwd = comm_gemm._wgrad_plain(ext, gy_full, h, wd) if need_wd else None
+        gwd = OF._weight_grad(ext, gy_full, h, wd) if need_wd else None
         dgu = ext.swiglu_packed_bwd(dh, gu)
         count_launch()
         gx = comm_gemm.gemm_rs(dgu, w, None, None, ctx.group, layout=1) if ctx.needs_input_grad[0] else None
         gwg = gwu = None
         if ctx.needs_input_grad[1] or ctx.needs_input_grad[2]:
+            out = None
             if mg is not None:
                 comm_gemm.ag_wgrad(dgu, x_shard, mg, True, ctx.group)
-                gwg, gwu = _finish_wgrad(wg, wu, mg, None)
             else:
                 out = torch.empty(w.shape, dtype=torch.float32, device=w.device)
                 comm_gemm.ag_wgrad(dgu, x_shard, out, False, ctx.group)
-                gwg, gwu = _finish_wgrad(wg, wu, None, out)
+            gwg, gwu = _gate_up_grads(wg, wu, out)
         return gx, gwg, gwu, gwd, (gy_shard if ctx.has_res else None), None
 
 

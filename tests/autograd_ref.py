@@ -1,5 +1,6 @@
 """fp64 references, with per-element bounds, of the linear-layer autograd wrappers in ``libai_b200.ops.functional``
-(``linear`` and ``mlp``): forward output and every gradient, from the exact bf16 inputs and upstream gradient.
+(``linear`` and ``mlp``) and ``libai_b200.ops.gated_mlp``: forward output and every gradient, from the exact bf16
+inputs and upstream gradient.  The tensor-parallel nodes of ``ops/comm_gemm.py`` on one rank compute the same.
 
 The bounds carry each kernel's error forward to first order, with the constants of ``tests/dense_ref.py``:
 
@@ -102,5 +103,41 @@ def mlp_ref(x, w1, b1, w2, gy, act, b2=None, residual=None):
     out["gb1"] = (dpre.sum(0), (M + 8) * R.ACC * dpre.abs().sum(0) + e_dpre.sum(0) + R.FLUSH)
     out["gw2"] = (G.t() @ h, G.abs().t() @ (M * R.ACC * h.abs() + e_h) + R.FLUSH)
     out["gb2"] = (G.sum(0), (M + 8) * R.ACC * G.abs().sum(0) + R.FLUSH)
+    out["gres"] = (G, torch.zeros_like(G))
+    return out
+
+
+def gated_mlp_ref(x, wg, wu, wd, gy, residual=None):
+    """``(silu(x @ wg^T) * (x @ wu^T)) @ wd^T (+ residual)`` of the gated MLP: y, gx, gwg, gwu, gwd, gres.  The gate and
+    up projections are stored in bf16, the SwiGLU reads them and stores h and its two gradients in bf16."""
+    X, Wg, Wu, Wd, G = x.double(), wg.double(), wu.double(), wd.double(), gy.double()
+    M, K = X.shape
+    Fh, N = Wg.shape[0], Wd.shape[0]
+    gate, up = X @ Wg.t(), X @ Wu.t()
+    s = torch.sigmoid(gate)
+    silu, dsilu = gate * s, s * (1 + gate * (1 - s))
+    rel = R.EXPF_APPROX * (1 + gate.abs())
+    e_g = U8 * gate.abs() + K * R.ACC * (X.abs() @ Wg.abs().t())
+    e_u = U8 * up.abs() + K * R.ACC * (X.abs() @ Wu.abs().t())
+    h = silu * up
+    e_h = U8 * h.abs() + R.ACT_LIPSCHITZ * up.abs() * e_g + silu.abs() * e_u + h.abs() * rel
+    y = h @ Wd.t()
+    e_y = Fh * R.ACC * (h.abs() @ Wd.abs().t()) + e_h @ Wd.abs().t()
+    if residual is not None:
+        y = y + residual.double()
+        e_y = e_y + 2.0 ** -23 * y.abs()
+    out = {"y": (y, U8 * y.abs() + e_y + R.FLUSH)}
+    dh = G @ Wd
+    e_dh = U8 * dh.abs() + N * R.ACC * (G.abs() @ Wd.abs())
+    dgate, dup = dh * up * dsilu, dh * silu
+    e_dgate = (U8 * dgate.abs() + (up * dsilu).abs() * e_dh + (dh * dsilu).abs() * e_u + 0.5 * (dh * up).abs() * e_g
+               + (dh * up).abs() * s * (1 - s) * (1 + 2 * gate.abs()) * rel)
+    e_dup = U8 * dup.abs() + silu.abs() * e_dh + R.ACT_LIPSCHITZ * dh.abs() * e_g + dup.abs() * rel
+    gx = dgate @ Wg + dup @ Wu
+    out["gx"] = (gx, U8 * gx.abs() + (2 * Fh * R.ACC * dgate.abs() + e_dgate) @ Wg.abs()
+                 + (2 * Fh * R.ACC * dup.abs() + e_dup) @ Wu.abs() + R.FLUSH)
+    out["gwg"] = (dgate.t() @ X, (M * R.ACC * dgate.abs() + e_dgate).t() @ X.abs() + R.FLUSH)
+    out["gwu"] = (dup.t() @ X, (M * R.ACC * dup.abs() + e_dup).t() @ X.abs() + R.FLUSH)
+    out["gwd"] = (G.t() @ h, G.abs().t() @ (M * R.ACC * h.abs() + e_h) + R.FLUSH)
     out["gres"] = (G, torch.zeros_like(G))
     return out

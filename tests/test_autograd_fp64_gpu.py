@@ -170,25 +170,43 @@ def test_mlp(epilogue, fused_bias_grad):
 
 
 @pytest.mark.parametrize("has_bias", [True, False])
-def test_linear_bias_residual(has_bias):
+@pytest.mark.parametrize("grad_to", ["autograd", "main_grad"])
+def test_linear_bias_residual(grad_to, has_bias):
+    """With ``grad_to="main_grad"`` the weight and bias own fp32 main_grad slices, and the three upstream layouts
+    accumulate into them as three micro-batches would."""
     B, S, K, N = 2, 101, 72, 136
     x0, w0, b0, r0 = rand(B, S, K, seed=1), rand(N, K, seed=2, scale=0.3), rand(N, seed=3), rand(B, S, N, seed=4)
+    if grad_to == "main_grad":
+        params = [nn.Parameter(w0.clone())] + ([nn.Parameter(b0.clone())] if has_bias else [])
+        _, bases = flat_params(*params, seed=70)
+        w, b = params[0], (params[1] if has_bias else None)
+        sums = {"gw": [], "gb": []}
     for layout, gy in upstream((B, S, N), seed=40):
-        x, w, r = x0.clone().requires_grad_(), w0.clone().requires_grad_(), r0.clone().requires_grad_()
-        b = b0.clone().requires_grad_() if has_bias else None
+        x, r = x0.clone().requires_grad_(), r0.clone().requires_grad_()
+        if grad_to == "autograd":
+            w = w0.clone().requires_grad_()
+            b = b0.clone().requires_grad_() if has_bias else None
         y = OF.linear_bias_residual(x, w, b, r)
-        assert type(y.grad_fn).__name__ == "_LinearResidualFnBackward"
+        assert type(y.grad_fn).__name__ == "_LinearFnBackward"
         y.backward(gy)
-        what = f"linear_bias_residual bias={has_bias} gy={layout}"
+        what = f"linear_bias_residual {grad_to} bias={has_bias} gy={layout}"
         ref = AR.linear_ref(x0.reshape(-1, K), w0, b0 if has_bias else None, gy.reshape(-1, N), None)
         yr = ref["y"][0] + r0.reshape(-1, N).double()
         # the bound of x @ w^T + bias, plus the residual's fp32 add and the bf16 rounding of the sum
         R.check(y.reshape(-1, N), yr, ref["y"][1] + (U8 + 2.0 ** -23) * yr.abs(), what + " y")
         R.check(x.grad.reshape(-1, K), *ref["gx"], what + " gx")
-        as_grad(w, *ref["gw"], what + " gw")
-        if has_bias:
-            as_grad(b, *ref["gb"], what + " gb")
+        if grad_to == "autograd":
+            as_grad(w, *ref["gw"], what + " gw")
+            if has_bias:
+                as_grad(b, *ref["gb"], what + " gb")
+        else:
+            sums["gw"].append(ref["gw"])
+            sums["gb"].append(ref["gb"])
         assert torch.equal(r.grad, gy.contiguous()), what + " the residual's gradient is gy itself"
+    if grad_to == "main_grad":
+        for p, base, k in zip(params, bases, ("gw", "gb")):
+            assert p.grad is None and p.grad_added_to_main_grad, f"linear_bias_residual {k} did not go to main_grad"
+            R.check(p.main_grad, *accumulated(base, sums[k]), f"linear_bias_residual bias={has_bias} {k} main_grad")
 
 
 # -------------------------------------------------------------------------------------------------------------- norms
@@ -996,26 +1014,28 @@ def test_block_check_rejects_scaled_bias_gradient(monkeypatch):
     _expect_rejected(monkeypatch, "bias gradient * (1 + 2^-5)")
 
 
-def test_function_checks_reject_scaled_bias_gradient(monkeypatch):
+def test_linear_checks_reject_scaled_bias_gradient(monkeypatch):
+    """The scaled bias gradient is caught whether it returns to autograd or accumulates into main_grad."""
     monkeypatch.setattr(OF, "_bias_grad", _scaled_bias_grad)
     with pytest.raises(R.Mismatch, match="gb"):
         test_linear("gelu", "b")
-    with pytest.raises(R.Mismatch, match="gb"):
-        test_linear_bias_residual(True)
+    for grad_to in ("autograd", "main_grad"):
+        with pytest.raises(R.Mismatch, match="gb"):
+            test_linear_bias_residual(grad_to=grad_to, has_bias=True)
 
 
-def test_block_check_rejects_scaled_weight_gradient(monkeypatch):
-    """The attention output projection's weight gradient off by a factor (1 + 2^-5)."""
-    orig = OF._LinearResidualFn.backward
+def test_block_check_rejects_scaled_attention_weight_gradients(monkeypatch):
+    """The attention projections' weight gradients off by a factor (1 + 2^-5)."""
+    orig = OF._LinearFn.backward
 
     def wrong(ctx, gy):
-        _, w = ctx.saved_tensors
+        w = ctx.saved_tensors[1]
         before = w.main_grad.clone()
         out = orig(ctx, gy)
         w.main_grad.add_((w.main_grad - before) * 2.0 ** -5)
         return out
 
-    monkeypatch.setattr(OF._LinearResidualFn, "backward", staticmethod(wrong))
+    monkeypatch.setattr(OF._LinearFn, "backward", staticmethod(wrong))
     _expect_rejected(monkeypatch, "weight gradient * (1 + 2^-5)")
 
 
@@ -1046,12 +1066,12 @@ def test_block_check_rejects_dropped_skip_gradient(monkeypatch):
     _expect_rejected(monkeypatch, "LayerNorm backward without gadd")
 
 
-def test_block_check_rejects_main_grad_added_twice(monkeypatch):
-    orig = OF._LinearResidualFn.backward
+def test_block_check_rejects_linear_main_grad_added_twice(monkeypatch):
+    orig = OF._LinearFn.backward
     seen = []
 
     def wrong(ctx, gy):
-        x2, w = ctx.saved_tensors
+        w = ctx.saved_tensors[1]
         before = w.main_grad.clone() if getattr(w, "main_grad", None) is not None else None
         out = orig(ctx, gy)
         if before is not None and not seen:            # the first micro-batch's wgrad lands twice
@@ -1059,7 +1079,7 @@ def test_block_check_rejects_main_grad_added_twice(monkeypatch):
             w.main_grad.add_(w.main_grad - before)
         return out
 
-    monkeypatch.setattr(OF._LinearResidualFn, "backward", staticmethod(wrong))
+    monkeypatch.setattr(OF._LinearFn, "backward", staticmethod(wrong))
     _expect_rejected(monkeypatch, "one micro-batch's main_grad added twice")
 
 
