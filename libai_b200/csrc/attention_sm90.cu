@@ -21,6 +21,12 @@
 // j <= i + (Sk - Sq) (bottom-right alignment, as in decode attention).  A query without a visible key gets O = 0,
 // lse = 0 and dQ = 0, and adds nothing to dK / dV.
 //
+// Prefix LM (PREFIX instances, causal only, without bias or doc_start): prefix_lens [B] makes the first prefix_lens[b]
+// keys visible to every query, so the causal condition becomes j <= i + (Sk - Sq) or j < prefix_lens[b] (GLM: a
+// bidirectional context followed by a causal generated part).  A row's key limit is max(i + Sk - Sq + 1, prefix),
+// clipped to kv_lens; with a prefix of 0 the instances compute what the causal kernel does, with a prefix >= Sk what
+// the non-causal one does, bit for bit.
+//
 // Packed sequences (DOC instances, causal self-attention only): doc_start [B, S] gives the first key of each query's
 // document, so query i of sample b sees key j iff doc_start[b, i] <= j <= i (doc_start clamped to [0, i]: every query
 // sees itself).  Nothing assumes doc_start to be non-decreasing along a row: which key tiles a forward CTA loads and
@@ -67,6 +73,8 @@ struct AttnFwdParams {
   float inv_keep;
   RngArgs rng;
   long long* rng_out;   // [2]: the (seed, offset) pair used, for the backward
+  const int* prefix_lens;   // [B] in the PREFIX instances: keys below it are visible to every query (last: the older
+                            // members keep their offsets)
 };
 
 enum AttnBias : int { BIAS_NONE = 0, BIAS_DENSE = 1, BIAS_ALIBI = 2 };
@@ -107,10 +115,11 @@ struct AttnFwdCfg {
 };
 
 // the forward of one CTA; tmap_* and p are the kernel's __grid_constant__ parameters (inlined: no call in the kernel)
-template <int D, int BIAS, bool DROP, bool DOC>
+template <int D, int BIAS, bool DROP, bool DOC, bool PREFIX = false>
 LB_DEVICE void attn_fwd_cta(const CUtensorMap& tmap_q, const CUtensorMap& tmap_k, const CUtensorMap& tmap_v,
                             const AttnFwdParams& p) {
   static_assert(!DOC || (BIAS == BIAS_NONE && !DROP), "packed sequences run without bias and dropout");
+  static_assert(!PREFIX || (BIAS == BIAS_NONE && !DOC), "a prefix runs without bias and packed sequences");
   using Cfg = AttnFwdCfg<D>;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -134,8 +143,11 @@ LB_DEVICE void attn_fwd_cta(const CUtensorMap& tmap_q, const CUtensorMap& tmap_k
   const int kv_len = p.kv_lens != nullptr ? max(1, min(p.Sk, p.kv_lens[batch])) : p.Sk;
   const int kv_beg = p.kv_start != nullptr ? min(max(p.kv_start[batch], 0), p.Sk) : 0;
   const int off = p.Sk - p.Sq;   // causal offset: query i sees keys j <= i + off
+  // keys below `pre` are visible to every row (PREFIX; 0 otherwise)
+  const int pre = PREFIX ? min(max(p.prefix_lens[batch], 0), p.Sk) : 0;
   // key tiles j0 .. j0 + nkv - 1 hold every key some row of this block can see; the others are not loaded
-  const int key_end = p.causal ? min(kv_len, min(q0 + ATT_BM, p.Sq) + off) : kv_len;
+  const int key_end = p.causal ? min(kv_len, PREFIX ? max(min(q0 + ATT_BM, p.Sq) + off, pre) : min(q0 + ATT_BM, p.Sq) + off)
+                               : kv_len;
   if constexpr (DOC) {   // warpgroup 0 reads one row each (rows past Sq repeat the last row)
     if (warp_idx < 4) {
       const int m = __reduce_min_sync(0xffffffffu, doc_begin(p.doc_start, p.Sq, batch, min(q0 + static_cast<int>(threadIdx.x), p.Sq - 1)));
@@ -199,7 +211,8 @@ LB_DEVICE void attn_fwd_cta(const CUtensorMap& tmap_q, const CUtensorMap& tmap_k
   for (int h = 0; h < 2; ++h) {
     q_idx[h] = q0 + r_loc + 8 * h;
     row_beg[h] = DOC ? doc_begin(p.doc_start, p.Sq, batch, min(q_idx[h], p.Sq - 1)) : kv_beg;
-    vis_len[h] = max(0, (p.causal ? min(kv_len, q_idx[h] + off + 1) : kv_len) - row_beg[h]);
+    vis_len[h] = max(0, (p.causal ? min(kv_len, PREFIX ? max(q_idx[h] + off + 1, pre) : q_idx[h] + off + 1) : kv_len) -
+                            row_beg[h]);
   }
   constexpr float LOG2E = 1.4426950408889634f;
   unsigned long long rng_seed = 0, rng_offset = 0;
@@ -251,8 +264,9 @@ LB_DEVICE void attn_fwd_cta(const CUtensorMap& tmap_q, const CUtensorMap& tmap_k
     // ---- scores in the log2 domain, masked
     const int kbase = j * ATT_BN, krel = kbase - kv_beg;
     // (per thread in the DOC instances: a tile may start before one of its rows' documents only)
+    // (PREFIX: a tile inside the prefix is visible to every row whatever the causal bound)
     const bool need_mask = kbase < (DOC ? max(row_beg[0], row_beg[1]) : kv_beg) || kbase + ATT_BN > kv_len ||
-                           (p.causal && kbase + ATT_BN - 1 > q0 + off);
+                           (p.causal && kbase + ATT_BN - 1 > q0 + off && (!PREFIX || kbase + ATT_BN > pre));
 #pragma unroll
     for (int jj = 0; jj < ATT_BN / 8; ++jj) {
 #pragma unroll
@@ -378,6 +392,13 @@ attn_fwd_doc_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_con
                     const __grid_constant__ CUtensorMap tmap_v, const __grid_constant__ AttnFwdParams p) {
   attn_fwd_cta<D, BIAS_NONE, false, true>(tmap_q, tmap_k, tmap_v, p);
 }
+// prefix LM (prefix_lens): causal attention without bias, with or without dropout
+template <int D, bool DROP>
+__global__ void __launch_bounds__(ATT_FWD_THREADS, 1)
+attn_fwd_prefix_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_k,
+                       const __grid_constant__ CUtensorMap tmap_v, const __grid_constant__ AttnFwdParams p) {
+  attn_fwd_cta<D, BIAS_NONE, DROP, false, true>(tmap_q, tmap_k, tmap_v, p);
+}
 
 }  // namespace lb
 
@@ -404,11 +425,11 @@ bool make_q_tmap(CUtensorMap* m, const void* ptr, int B, int G, int r, int S, in
   return lb_host::make_tmap_bf16(m, ptr, 5, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B);
 }
 
-template <int D, int BIAS, bool DROP, bool DOC = false>
+template <int D, int BIAS, bool DROP, bool DOC, bool PREFIX>
 cudaError_t launch_fwd_t(const CUtensorMap& tq, const CUtensorMap& tk, const CUtensorMap& tv, const lb::AttnFwdParams& p,
                          cudaStream_t s) {
   using Cfg = lb::AttnFwdCfg<D>;
-  auto kern = DOC ? lb::attn_fwd_doc_kernel<D> : lb::attn_fwd_kernel<D, BIAS, DROP>;
+  auto kern = DOC ? lb::attn_fwd_doc_kernel<D> : PREFIX ? lb::attn_fwd_prefix_kernel<D, DROP> : lb::attn_fwd_kernel<D, BIAS, DROP>;
   static bool configured = false;
   if (!configured) {
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES);
@@ -421,14 +442,15 @@ cudaError_t launch_fwd_t(const CUtensorMap& tq, const CUtensorMap& tk, const CUt
 }
 
 // the launcher-level conditions both directions share: the tile width (64 or 128) of the head dim, or -1 (head dim),
-// -5 (empty sequence), -4 (A % G), -6 (doc_start outside causal self-attention), -3 (strides or bias not 16-byte
-// aligned)
+// -5 (empty sequence), -4 (A % G), -6 (doc_start outside causal self-attention), -7 (prefix_lens without the causal
+// mask, or with bias, ALiBi or doc_start), -3 (strides or bias not 16-byte aligned)
 int check_attn_args(const lb::AttnArgs& a) {
   const int tile = head_dim_tile(a.d);
   if (tile == 0) return -1;
   if (a.Sq <= 0 || a.Sk <= 0) return -5;
   if (a.G <= 0 || a.A % a.G) return -4;
   if (a.doc_start != nullptr && !lb::attn_doc_start_supported(a)) return -6;
+  if (a.prefix_lens != nullptr && !lb::attn_prefix_supported(a)) return -7;
   for (int i = 0; i < 3; ++i)
     if ((a.q_strides[i] % 8) || (a.k_strides[i] % 8) || (a.v_strides[i] % 8)) return -3;
   if (a.q_strides[3] % 8) return -3;
@@ -455,6 +477,7 @@ void fill_score_params(P& p, const lb::AttnArgs& a, bool dropout) {
   p.kv_lens = a.kv_lens;
   p.kv_start = a.kv_start;
   p.doc_start = a.doc_start;
+  p.prefix_lens = a.prefix_lens;
   p.bias = reinterpret_cast<const __nv_bfloat16*>(a.bias);
   for (int i = 0; i < 3; ++i) p.bias_strides[i] = a.bias != nullptr ? a.bias_strides[i] : 0;
   p.alibi_slopes = a.bias != nullptr ? nullptr : a.alibi_slopes;
@@ -469,15 +492,19 @@ template <int V>
 using int_c = std::integral_constant<int, V>;
 template <bool V>
 using bool_c = std::integral_constant<bool, V>;
-// calls launch(D, BIAS, DROP, DOC) with the compile-time parameters of the kernel instance that runs p: the tile
-// width, the bias kind, dropout, and packed sequences (whose instances run without bias and dropout)
+// calls launch(D, BIAS, DROP, DOC, PREFIX) with the compile-time parameters of the kernel instance that runs p: the
+// tile width, the bias kind, dropout, packed sequences (whose instances run without bias and dropout) and a prefix
+// (whose instances run without bias)
 template <class P, class F>
 cudaError_t launch_instance(int tile, const P& p, F&& launch) {
   auto with_tile = [&](auto D) {
-    if (p.doc_start != nullptr) return launch(D, int_c<lb::BIAS_NONE>{}, bool_c<false>{}, bool_c<true>{});
+    if (p.doc_start != nullptr) return launch(D, int_c<lb::BIAS_NONE>{}, bool_c<false>{}, bool_c<true>{}, bool_c<false>{});
+    if (p.prefix_lens != nullptr)
+      return p.drop_thresh > 0 ? launch(D, int_c<lb::BIAS_NONE>{}, bool_c<true>{}, bool_c<false>{}, bool_c<true>{})
+                               : launch(D, int_c<lb::BIAS_NONE>{}, bool_c<false>{}, bool_c<false>{}, bool_c<true>{});
     auto with_bias = [&](auto BIAS) {
-      return p.drop_thresh > 0 ? launch(D, BIAS, bool_c<true>{}, bool_c<false>{})
-                               : launch(D, BIAS, bool_c<false>{}, bool_c<false>{});
+      return p.drop_thresh > 0 ? launch(D, BIAS, bool_c<true>{}, bool_c<false>{}, bool_c<false>{})
+                               : launch(D, BIAS, bool_c<false>{}, bool_c<false>{}, bool_c<false>{});
     };
     if (p.bias == nullptr && p.alibi_slopes == nullptr) return with_bias(int_c<lb::BIAS_NONE>{});
     if (p.bias != nullptr) return with_bias(int_c<lb::BIAS_DENSE>{});
@@ -502,9 +529,9 @@ extern "C" int lb_attn_fwd(const lb::AttnArgs* a, const void* q, const void* k, 
   memset(&p.rng, 0, sizeof(p.rng));
   if (rng != nullptr) p.rng = *rng;
   p.rng_out = rng_out;
-  return (int)launch_instance(tile, p, [&](auto tile_c, auto bias, auto drop, auto doc) {
-    return launch_fwd_t<decltype(tile_c)::value, decltype(bias)::value, decltype(drop)::value, decltype(doc)::value>(
-        tq, tk, tv, p, s);
+  return (int)launch_instance(tile, p, [&](auto tile_c, auto bias, auto drop, auto doc, auto prefix) {
+    return launch_fwd_t<decltype(tile_c)::value, decltype(bias)::value, decltype(drop)::value, decltype(doc)::value,
+                        decltype(prefix)::value>(tq, tk, tv, p, s);
   });
 }
 // =================================================================================================
@@ -516,6 +543,15 @@ extern "C" int lb_attn_fwd(const lb::AttnArgs* a, const void* q, const void* k, 
 // Which query blocks a key block visits depends on the shapes only (Sq, Sk, causal): under the causal mask query block
 // i and key block kb meet iff 64 kb <= 64 i + 63 + (Sk - Sq).  Keys outside a sample's kv_start / kv_lens window are
 // masked element-wise, so every visit happens and the dQ ordering below counts the same visits on both sides.
+// Prefix LM (PREFIX): query block i and key block kb of sample b meet iff 64 kb <= 64 i + 63 + (Sk - Sq) or
+// 64 kb < prefix_lens[b] (the shapes and that one number per sample).  A key block inside the prefix meets every query
+// block, so a CTA whose lowest key block lies in the prefix starts its visits at query block 0.  Meeting stays monotone
+// in the key block (if kb meets i, every lower key block does), so the dQ counter rule below keeps its form: key block
+// kb adds to query block i after exactly last_kb - kb additions, where last_kb = min(nkb - 1, max(the causal last
+// block (64 i + 63 + Sk - Sq) / 64, ceil(min(prefix_lens[b], Sk) / 64) - 1)).  Keys outside kv_start / kv_lens stay
+// masked element-wise, with every visit made.  Forward progress rests on the same dispatch-order assumption as
+// without a prefix (below): a waiter only waits for higher key blocks, which live in its own CTA or in CTAs of lower
+// linear index.
 // The warpgroups of a CTA step through one sequence of (query head, query block) visits, from the first query block
 // its lowest key block meets; the producer loads Q_i, dO_i and the block's lse and δ once for all of them, and a
 // warpgroup whose key block does not meet query block i (a higher block under the causal mask) lets that visit pass
@@ -603,6 +639,7 @@ struct AttnBwdParams {
   const long long* rng_state;
   unsigned* dq_order;   // [B * A * query blocks]: key blocks whose dQ contribution has landed (zeroed by the caller)
   SpinTimeout* timeout_rec;  // where a timed-out dq_order wait leaves its diagnostic (host-mapped)
+  const int* prefix_lens;    // [B] in the PREFIX instances (last: the older members keep their offsets)
 };
 
 // DOC: true when no row of the query block [q0, q0 + 64) sees a key of the block [k0, k0 + 64), i.e. every row's
@@ -615,8 +652,10 @@ LB_DEVICE bool doc_visit_empty(const int* doc_start, int S, int batch, int q0, i
 }
 // first query block whose last row (64 i + 63) sees key block kb: floor((64 kb - (Sk - Sq)) / 64), at least 0 (C
 // division truncates a negative quotient towards 0, which the max turns into the same 0).  At most nq - 1, since
-// 64 kb <= Sk - 1.
-LB_DEVICE int bwd_first_qblock(const AttnBwdParams& p, int kb) {
+// 64 kb <= Sk - 1.  PREFIX: 0 for a key block that starts inside the prefix `pre` (every query sees it).
+template <bool PREFIX>
+LB_DEVICE int bwd_first_qblock(const AttnBwdParams& p, int kb, int pre) {
+  if (PREFIX && kb * ATT_BWD_BN < pre) return 0;
   return p.causal ? max(0, (kb * ATT_BWD_BN - (p.Sk - p.Sq)) / ATT_BWD_BM) : 0;
 }
 // dq_accum holds each (batch, query head, 64-query block) as one [64][D] fp32 tile, stored as the backward stages its
@@ -630,17 +669,18 @@ LB_DEVICE int dq_tile_index(int row, int col) {
   return row * D + ((((col >> 2) ^ row) & 7) | ((col >> 2) & ~7)) * 4 + (col & 3);
 }
 // whether key block kb (of nkb) visits query block qb; called by a whole warp (DOC)
-template <bool DOC>
-LB_DEVICE bool bwd_visits(const AttnBwdParams& p, int batch, int nkb, int kb, int qb) {
-  if (kb >= nkb || qb < bwd_first_qblock(p, kb)) return false;
+template <bool DOC, bool PREFIX>
+LB_DEVICE bool bwd_visits(const AttnBwdParams& p, int batch, int nkb, int kb, int qb, int pre) {
+  if (kb >= nkb || qb < bwd_first_qblock<PREFIX>(p, kb, pre)) return false;
   return !DOC || !doc_visit_empty(p.doc_start, p.Sq, batch, qb * ATT_BWD_BM, kb * ATT_BWD_BN);
 }
 
-template <int D, int BIAS, bool DROP, bool DOC>
-__global__ void __launch_bounds__(AttnBwdCfg<D, attn_bwd_wgs<D, BIAS, DROP>()>::THREADS, 1)
-attn_bwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_k,
-                const __grid_constant__ CUtensorMap tmap_v, const __grid_constant__ CUtensorMap tmap_do, AttnBwdParams p) {
+// the backward of one CTA; the tensor maps and p are the kernel's parameters (inlined: no call in the kernel)
+template <int D, int BIAS, bool DROP, bool DOC, bool PREFIX>
+LB_DEVICE void attn_bwd_cta(const CUtensorMap& tmap_q, const CUtensorMap& tmap_k, const CUtensorMap& tmap_v,
+                            const CUtensorMap& tmap_do, const AttnBwdParams& p) {
   static_assert(!DOC || (BIAS == BIAS_NONE && !DROP), "packed sequences run without bias and dropout");
+  static_assert(!PREFIX || (BIAS == BIAS_NONE && !DOC), "a prefix runs without bias and packed sequences");
   constexpr int NWG = attn_bwd_wgs<D, BIAS, DROP>();
   using Cfg = AttnBwdCfg<D, NWG>;
   constexpr int STAGES = Cfg::STAGES, DQ_BUFS = Cfg::DQ_BUFS;
@@ -667,7 +707,8 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
   const int kb0 = NWG * cta;                        // the CTA's lowest key block
   const int off = p.Sk - p.Sq;
   const int nq = (p.Sq + ATT_BWD_BM - 1) / ATT_BWD_BM;
-  const int i_begin = bwd_first_qblock(p, kb0);
+  const int pre = PREFIX ? min(max(p.prefix_lens[batch], 0), p.Sk) : 0;   // keys every query sees
+  const int i_begin = bwd_first_qblock<PREFIX>(p, kb0, pre);
   const int iters = nq - i_begin;   // query blocks per query head
   const int steps = p.r * iters;    // step = (query head in group) * iters + query block - i_begin
 
@@ -710,7 +751,7 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
         const int qb = i_begin + step - hi * iters;
         bool need = false;
 #pragma unroll
-        for (int w = 0; w < NWG; ++w) need = need || bwd_visits<DOC>(p, batch, nkb, kb0 + w, qb);
+        for (int w = 0; w < NWG; ++w) need = need || bwd_visits<DOC, PREFIX>(p, batch, nkb, kb0 + w, qb, pre);
         if (!need) continue;
         const int st = ld % STAGES;
         mbar_wait(&qdo_empty[st], ((ld / STAGES) & 1) ^ 1);
@@ -741,13 +782,15 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
         const int qb = i_begin + step - hi * iters;
         bool makes[NWG];
 #pragma unroll
-        for (int w = 0; w < NWG; ++w) makes[w] = bwd_visits<DOC>(p, batch, nkb, kb0 + w, qb);
+        for (int w = 0; w < NWG; ++w) makes[w] = bwd_visits<DOC, PREFIX>(p, batch, nkb, kb0 + w, qb, pre);
         if (lane == 0) {
           const size_t blk = (static_cast<size_t>(batch) * p.A + kv_head * p.r + hi) * nq + qb;
           unsigned* order = p.dq_order + blk;
           // the key blocks above kb that visit query block qb: all of them, or under the causal mask
-          // kb' <= (64 qb + 63 + off) / 64 (a non-negative quotient, since kb visits qb)
-          const int last_kb = p.causal ? min(nkb - 1, (qb * ATT_BWD_BM + ATT_BWD_BM - 1 + off) / ATT_BWD_BN) : nkb - 1;
+          // kb' <= (64 qb + 63 + off) / 64 (a non-negative quotient, since kb visits qb) or, with a prefix, the blocks
+          // that start inside it
+          int last_kb = p.causal ? min(nkb - 1, (qb * ATT_BWD_BM + ATT_BWD_BM - 1 + off) / ATT_BWD_BN) : nkb - 1;
+          if (PREFIX && p.causal) last_kb = min(nkb - 1, max(last_kb, (pre + ATT_BWD_BN - 1) / ATT_BWD_BN - 1));
           uint32_t landed = 0;   // partials of this visit added so far
 #pragma unroll
           for (int w = NWG - 1; w >= 0; --w) {
@@ -818,11 +861,11 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
     const int hi = step / iters;
     const int it = step - hi * iters;
     const int qb = i_begin + it;
-    const bool mine = bwd_visits<DOC>(p, batch, nkb, kb, qb);
+    const bool mine = bwd_visits<DOC, PREFIX>(p, batch, nkb, kb, qb, pre);
     bool need = mine;
 #pragma unroll
     for (int u = 0; u < NWG; ++u)
-      if (u != w) need = need || bwd_visits<DOC>(p, batch, nkb, kb0 + u, qb);
+      if (u != w) need = need || bwd_visits<DOC, PREFIX>(p, batch, nkb, kb0 + u, qb, pre);
     if (!need) continue;   // not loaded
     const int st = ld % STAGES;
     mbar_wait(&qdo_full[st], (ld / STAGES) & 1);
@@ -866,7 +909,7 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
           const bool q_ok = q_idx < p.Sq;
           const float lse2 = q_ok ? s_lse[8 * jj + cq + c] * LOG2E : 0.f;
           const float delta_s = q_ok ? s_delta[8 * jj + cq + c] * p.scale : 0.f;
-          const int key_lim = !q_ok ? 0 : (p.causal ? min(kv_len, q_idx + off + 1) : kv_len);
+          const int key_lim = !q_ok ? 0 : (p.causal ? min(kv_len, PREFIX ? max(q_idx + off + 1, pre) : q_idx + off + 1) : kv_len);
           const int key_lo = DOC && q_ok ? doc_begin(p.doc_start, p.Sq, batch, q_idx) : 0;   // the query's document
           uint4 rnd;
           if constexpr (DROP)   // both rows of this thread lie in the same 16-key group
@@ -980,6 +1023,21 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
   }
 }
 
+template <int D, int BIAS, bool DROP, bool DOC>
+__global__ void __launch_bounds__(AttnBwdCfg<D, attn_bwd_wgs<D, BIAS, DROP>()>::THREADS, 1)
+attn_bwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_k,
+                const __grid_constant__ CUtensorMap tmap_v, const __grid_constant__ CUtensorMap tmap_do, AttnBwdParams p) {
+  attn_bwd_cta<D, BIAS, DROP, DOC, false>(tmap_q, tmap_k, tmap_v, tmap_do, p);
+}
+// prefix LM (prefix_lens): causal attention without bias, with or without dropout
+template <int D, bool DROP>
+__global__ void __launch_bounds__(AttnBwdCfg<D, attn_bwd_wgs<D, BIAS_NONE, DROP>()>::THREADS, 1)
+attn_bwd_prefix_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_k,
+                       const __grid_constant__ CUtensorMap tmap_v, const __grid_constant__ CUtensorMap tmap_do,
+                       AttnBwdParams p) {
+  attn_bwd_cta<D, BIAS_NONE, DROP, false, true>(tmap_q, tmap_k, tmap_v, tmap_do, p);
+}
+
 // delta[b, a, s] = sum_d dO[b, a, s, d] * O[b, a, s, d] over the head dim d <= D
 // D / 8 lanes per row (lanes past d add zeros), 16-byte loads; rows are visited in (b, s, a) order = memory order of the
 // [b, s, a, d] tensors, so a warp reads contiguous bytes per tensor, and every thread keeps 4 rows (8 loads) in flight.
@@ -1065,12 +1123,12 @@ attn_dq_convert_kernel(const float* __restrict__ acc, __nv_bfloat16* __restrict_
 }  // namespace lb
 
 namespace {
-template <int D, int BIAS, bool DROP, bool DOC = false>
+template <int D, int BIAS, bool DROP, bool DOC, bool PREFIX>
 cudaError_t launch_bwd_t(const CUtensorMap& tq, const CUtensorMap& tk, const CUtensorMap& tv, const CUtensorMap& tdo,
                          const lb::AttnBwdParams& p, cudaStream_t s) {
   constexpr int NWG = lb::attn_bwd_wgs<D, BIAS, DROP>();
   using Cfg = lb::AttnBwdCfg<D, NWG>;
-  auto kern = lb::attn_bwd_kernel<D, BIAS, DROP, DOC>;
+  auto kern = PREFIX ? lb::attn_bwd_prefix_kernel<D, DROP> : lb::attn_bwd_kernel<D, BIAS, DROP, DOC>;
   static bool configured = false;
   if (!configured) {
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES);
@@ -1131,9 +1189,9 @@ extern "C" int lb_attn_bwd(const lb::AttnArgs* a, const void* dout, const long* 
   p.rng_state = rng_state;
   p.dq_order = dq_order;
   p.timeout_rec = lb_host::spin_timeout_record(s);
-  cudaError_t e = launch_instance(tile, p, [&](auto tile_c, auto bias, auto drop, auto doc) {
-    return launch_bwd_t<decltype(tile_c)::value, decltype(bias)::value, decltype(drop)::value, decltype(doc)::value>(
-        tq, tk, tv, tdo, p, s);
+  cudaError_t e = launch_instance(tile, p, [&](auto tile_c, auto bias, auto drop, auto doc, auto prefix) {
+    return launch_bwd_t<decltype(tile_c)::value, decltype(bias)::value, decltype(drop)::value, decltype(doc)::value,
+                        decltype(prefix)::value>(tq, tk, tv, tdo, p, s);
   });
   if (e != cudaSuccess) return (int)e;
   const long nvec = rows * D / 8;

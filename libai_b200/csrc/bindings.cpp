@@ -835,15 +835,16 @@ std::tuple<Tensor, Tensor> bias_dropout_residual(const Tensor& x, const c10::opt
 // head h reads K/V head h / r) and head dim D a multiple of 8 in [8, 128]; views with arbitrary batch/head/seq strides
 // (D contiguous).  Output o is allocated as [B, Sq, A, D] and returned as the [B, A, Sq, D] view, lse fp32 [B, A, Sq].
 // Key j is visible to query i of sample b iff kv_start[b] <= j < kv_lens[b] (defaults 0 and Sk) and, when causal,
-// j <= i + Sk - Sq.
+// j <= i + Sk - Sq or j < prefix_lens[b].
 
-// One flash-attention problem, validated: q, k, v as above, bf16; kv_lens / kv_start int32 [B]; doc_start int32
-// [B, Sq] (packed sequences); bias bf16 [B|1, A|1, Sq, Sk] with contiguous keys (broadcast dims get stride 0);
+// One flash-attention problem, validated: q, k, v as above, bf16; kv_lens / kv_start / prefix_lens int32 [B]; doc_start
+// int32 [B, Sq] (packed sequences); bias bf16 [B|1, A|1, Sq, Sk] with contiguous keys (broadcast dims get stride 0);
 // alibi_slopes fp32 [A]; p_drop in [0, 1).
 lb::AttnArgs attn_args(Args& args, const Tensor& q, const Tensor& k, const Tensor& v, bool causal, double scale,
                        const c10::optional<Tensor>& kv_lens, const c10::optional<Tensor>& kv_start,
                        const c10::optional<Tensor>& doc_start, const c10::optional<Tensor>& bias,
-                       const c10::optional<Tensor>& alibi_slopes, double p_drop) {
+                       const c10::optional<Tensor>& alibi_slopes, double p_drop,
+                       const c10::optional<Tensor>& prefix_lens) {
   const char* what = args.op();
   TORCH_CHECK(q.dim() == 4 || q.dim() == 5, what, ": q must be [B, A, S, D] or [B, G, r, S, D]");
   args("q", q, at::kBFloat16, q.sizes(), Layout::LastDimContiguous);
@@ -880,6 +881,7 @@ lb::AttnArgs attn_args(Args& args, const Tensor& q, const Tensor& k, const Tenso
   a.kv_lens = args.opt<const int>("kv_lens", kv_lens, at::kInt, {a.B});
   a.kv_start = args.opt<const int>("kv_start", kv_start, at::kInt, {a.B});
   a.doc_start = args.opt<const int>("doc_start", doc_start, at::kInt, {a.B, a.Sq});
+  a.prefix_lens = args.opt<const int>("prefix_lens", prefix_lens, at::kInt, {a.B});
   if (given(bias)) {
     const Tensor& b = args("bias", *bias, at::kBFloat16, {kAny, kAny, a.Sq, a.Sk}, Layout::LastDimContiguous);
     TORCH_CHECK((b.size(0) == 1 || b.size(0) == a.B) && (b.size(1) == 1 || b.size(1) == a.A), what,
@@ -895,6 +897,9 @@ lb::AttnArgs attn_args(Args& args, const Tensor& q, const Tensor& k, const Tenso
   TORCH_CHECK(a.doc_start == nullptr || lb::attn_doc_start_supported(a), what,
               ": doc_start: supported for causal self-attention (Sq == Sk) without kv_lens, kv_start, bias, ALiBi or "
               "dropout");
+  TORCH_CHECK(a.prefix_lens == nullptr || lb::attn_prefix_supported(a), what,
+              ": prefix_lens: supported for causal attention, with kv_lens, kv_start, grouped-query heads and dropout, "
+              "without bias, ALiBi or doc_start");
   return a;
 }
 
@@ -902,9 +907,11 @@ lb::AttnArgs attn_args(Args& args, const Tensor& q, const Tensor& k, const Tenso
 std::tuple<Tensor, Tensor, Tensor> attn_fwd(const Tensor& q, const Tensor& k, const Tensor& v, bool causal, double scale,
                                             const c10::optional<Tensor>& kv_lens, const c10::optional<Tensor>& bias,
                                             const c10::optional<Tensor>& alibi_slopes, double p_drop, int64_t salt,
-                                            const c10::optional<Tensor>& kv_start, const c10::optional<Tensor>& doc_start) {
+                                            const c10::optional<Tensor>& kv_start, const c10::optional<Tensor>& doc_start,
+                                            const c10::optional<Tensor>& prefix_lens) {
   Args args("attn_fwd");
-  const lb::AttnArgs a = attn_args(args, q, k, v, causal, scale, kv_lens, kv_start, doc_start, bias, alibi_slopes, p_drop);
+  const lb::AttnArgs a = attn_args(args, q, k, v, causal, scale, kv_lens, kv_start, doc_start, bias, alibi_slopes, p_drop,
+                                   prefix_lens);
   const auto guard = args.guard();
   Tensor o = at::empty({a.B, a.Sq, a.A, a.d}, q.options());
   Tensor lse = at::empty({a.B, a.A, a.Sq}, q.options().dtype(at::kFloat));
@@ -1119,9 +1126,11 @@ std::tuple<Tensor, Tensor, Tensor, Tensor> attn_bwd(const Tensor& dout, const Te
                                             const c10::optional<Tensor>& alibi_slopes, c10::optional<Tensor> dbias,
                                             double p_drop, const c10::optional<Tensor>& rng_state,
                                             const c10::optional<Tensor>& kv_start,
-                                            const c10::optional<Tensor>& doc_start) {
+                                            const c10::optional<Tensor>& doc_start,
+                                            const c10::optional<Tensor>& prefix_lens) {
   Args args("attn_bwd");
-  const lb::AttnArgs a = attn_args(args, q, k, v, causal, scale, kv_lens, kv_start, doc_start, bias, alibi_slopes, p_drop);
+  const lb::AttnArgs a = attn_args(args, q, k, v, causal, scale, kv_lens, kv_start, doc_start, bias, alibi_slopes, p_drop,
+                                   prefix_lens);
   const int B = a.B, A = a.A, G = a.G, Sq = a.Sq, Sk = a.Sk, D = a.d, r = A / G;
   args("o", o, at::kBFloat16, {B, A, Sq, D}, Layout::LastDimContiguous);
   args("dout", dout, kAnyDtype, {B, A, Sq, D}, Layout::Strided);
@@ -1325,8 +1334,8 @@ TORCH_LIBRARY(libai_b200, m) {
   m.def("ce_bwd(Tensor(a!) logits, Tensor labels, Tensor lse, Tensor gloss, int vocab_start) -> Tensor(a!)", &ce_bwd);
   m.def("fused_adamw(Tensor(a!) master, Tensor grad, Tensor(b!) m, Tensor(c!) v, Tensor? lp_out, Tensor scale, float lr, float b1, float b2, float eps, float wd, float bc1, float bc2, bool decoupled) -> ()", &fused_adamw);
   m.def("sqnorm(Tensor x) -> Tensor", &sqnorm);
-  m.def("attn_fwd(Tensor q, Tensor k, Tensor v, bool causal, float scale, Tensor? kv_lens, Tensor? bias=None, Tensor? alibi_slopes=None, float p_drop=0.0, int salt=0, Tensor? kv_start=None, Tensor? doc_start=None) -> (Tensor, Tensor, Tensor)", &attn_fwd);
-  m.def("attn_bwd(Tensor dout, Tensor q, Tensor k, Tensor v, Tensor o, Tensor lse, bool causal, float scale, Tensor? kv_lens, Tensor? bias=None, Tensor? alibi_slopes=None, Tensor(a!)? dbias=None, float p_drop=0.0, Tensor? rng_state=None, Tensor? kv_start=None, Tensor? doc_start=None) -> (Tensor, Tensor, Tensor, Tensor)", &attn_bwd);
+  m.def("attn_fwd(Tensor q, Tensor k, Tensor v, bool causal, float scale, Tensor? kv_lens, Tensor? bias=None, Tensor? alibi_slopes=None, float p_drop=0.0, int salt=0, Tensor? kv_start=None, Tensor? doc_start=None, Tensor? prefix_lens=None) -> (Tensor, Tensor, Tensor)", &attn_fwd);
+  m.def("attn_bwd(Tensor dout, Tensor q, Tensor k, Tensor v, Tensor o, Tensor lse, bool causal, float scale, Tensor? kv_lens, Tensor? bias=None, Tensor? alibi_slopes=None, Tensor(a!)? dbias=None, float p_drop=0.0, Tensor? rng_state=None, Tensor? kv_start=None, Tensor? doc_start=None, Tensor? prefix_lens=None) -> (Tensor, Tensor, Tensor, Tensor)", &attn_bwd);
   m.def("kv_append(Tensor qkv, Tensor(a!) k_cache, Tensor(b!) v_cache, Tensor cache_seqlens, Tensor? cos, Tensor? sin, bool write_q) -> Tensor", &kv_append);
   m.def("kv_append_fp8(Tensor qkv, Tensor(a!) k_cache, Tensor(b!) v_cache, Tensor(c!) k_scale, Tensor(d!) v_scale, Tensor cache_seqlens, Tensor? cos, Tensor? sin, bool write_q) -> Tensor", &kv_append_fp8);
   m.def("window_attn_fwd(Tensor qkv, int H, int W, int window, int shift, int heads, float scale, Tensor table, Tensor? tau) -> (Tensor, Tensor)", &window_attn_fwd);

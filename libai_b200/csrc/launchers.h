@@ -23,7 +23,7 @@ struct RngArgs {
 // One flash-attention problem, shared by lb_attn_fwd and lb_attn_bwd.  A query heads in G groups (query head h reads
 // K/V head h / (A / G)); Sq queries against Sk keys; head dim d a multiple of 8 in [8, 128].  Strides are in elements.
 // Key j is visible to query i of sample b iff kv_start[b] <= j < kv_lens[b] (defaults 0 and Sk) and, when causal,
-// j <= i + (Sk - Sq).
+// j <= i + (Sk - Sq) or j < prefix_lens[b] (prefix LM: the first prefix_lens[b] keys are visible to every query).
 struct AttnArgs {
   int B, A, G, Sq, Sk, d;
   long q_strides[4];   // {batch, group, in-group, seq}
@@ -38,12 +38,19 @@ struct AttnArgs {
   long bias_strides[3];   // {batch, head, query} of bias, 0 for a broadcast dimension
   const float* alibi_slopes;   // optional fp32 [A]; ignored when `bias` is given
   float p_drop;           // attention dropout probability in [0, 1), quantised to 1/256
+  const int* prefix_lens; // optional int32 [B] (causal only): keys j < prefix_lens[b] are visible to every query
 };
 
 // packed sequences (doc_start) run as causal self-attention only, without kv_lens, kv_start, bias, ALiBi or dropout
 inline bool attn_doc_start_supported(const AttnArgs& a) {
   return a.causal && a.Sq == a.Sk && a.kv_lens == nullptr && a.kv_start == nullptr && a.bias == nullptr &&
          a.alibi_slopes == nullptr && !(a.p_drop > 0.f);
+}
+
+// a prefix (prefix_lens) runs with the causal mask only, combined with kv_start, kv_lens, grouped-query heads and
+// dropout, without bias, ALiBi or doc_start
+inline bool attn_prefix_supported(const AttnArgs& a) {
+  return a.causal && a.bias == nullptr && a.alibi_slopes == nullptr && a.doc_start == nullptr;
 }
 
 }  // namespace lb

@@ -135,7 +135,7 @@ class KVCacheLayer:
                 OF.kv_cache_dequant(self.v[:, :, :L], self.v_scale[:, :, :L], dtype))
 
     def attend(self, q: torch.Tensor, *, scale: float, causal: bool = True, mask=None, bias=None, alibi_slopes=None,
-               rel_bias=None, dropout_p: float = 0.0, training: bool = False) -> torch.Tensor:
+               rel_bias=None, dropout_p: float = 0.0, training: bool = False, prefix_lens=None) -> torch.Tensor:
         """Attention of the new tokens' ``q`` ``[b, s, a, d]`` over the cache → ``[b, s, a, d]``, contiguous.
         ``causal``: the new tokens were appended this step (self-attention); ``causal=False``: the cache is a fixed
         window the queries all see (cross-attention).  The rows held before this step (``length``) are the same for
@@ -144,12 +144,19 @@ class KVCacheLayer:
         - a dense 0/1 ``mask`` or additive ``bias`` (the model folded its padding into it): :func:`OF.attention` over
           the window ``[:length + s]`` (causal) or ``[:length]``, non-causal;
         - the causal prefill of an empty cache without ``rel_bias``: the flash kernel over ``[:s]``, the prompt's left
-          padding in ``kv_start``;
+          padding in ``kv_start``; ``prefix_lens`` (int32 ``[b]``, a prefix LM's context width) makes the first
+          ``prefix_lens[b]`` rows visible to every new token.  Only this branch takes a prefix: every cached row is
+          visible to a later token, so later steps need none, and any other call with ``prefix_lens`` raises
+          ``ValueError``;
         - anything else: :func:`OF.decode_attention` (the split-KV kernel up to 16 new tokens, the flash kernel over
           the cache window beyond).
 
         The first two read an FP8 cache's window dequantized to q's dtype; the decode kernel reads its bytes."""
         past = self.length
+        if prefix_lens is not None and (past > 0 or not causal or mask is not None or bias is not None
+                                        or alibi_slopes is not None or rel_bias is not None):
+            raise ValueError("prefix_lens: only the causal prefill of an empty cache, without mask, bias, ALiBi or "
+                             "rel_bias, takes a prefix")
         if mask is not None or bias is not None:
             L = past + q.shape[1] if causal else past
             k, v = self.window(L, q.dtype)
@@ -158,9 +165,9 @@ class KVCacheLayer:
             return ctx.transpose(1, 2).contiguous()   # the reference math's [b, a, s, d] output is not
         if causal and past == 0 and rel_bias is None:
             query, (key, value) = q.transpose(1, 2), self.window(q.shape[1], q.dtype)
-            kv_start = self.kv_start if OF.attention_supported(query, key) else None
+            kv_start = self.kv_start if prefix_lens is not None or OF.attention_supported(query, key) else None
             ctx = OF.attention(query, key, value, causal=True, scale=scale, alibi_slopes=alibi_slopes,
-                               kv_start=kv_start, dropout_p=dropout_p, training=training)
+                               kv_start=kv_start, dropout_p=dropout_p, training=training, prefix_lens=prefix_lens)
             return ctx.transpose(1, 2)
         scales = {} if self.k_scale is None else {"k_scale": self.k_scale, "v_scale": self.v_scale}
         return OF.decode_attention(q, self.k, self.v, self.seqlens, self.kv_start, scale=scale, past=past,

@@ -607,15 +607,22 @@ def attention_ref(q, k, v, *, causal: bool, scale: float, mask=None, bias=None, 
     return torch.matmul(probs, v.float()).to(q.dtype)
 
 
-def visible_keys(sq: int, sk: int, *, causal: bool, kv_start=None, kv_lens=None, doc_start=None, device=None):
+def visible_keys(sq: int, sk: int, *, causal: bool, kv_start=None, kv_lens=None, doc_start=None, prefix_lens=None,
+                 device=None):
     """Boolean ``[b|1, 1, sq, sk]`` visibility of the flash kernels: key ``j`` is visible to query ``i`` of sample ``b``
     iff ``kv_start[b] <= j < max(1, kv_lens[b])`` (defaults ``0`` and ``sk``) and, when ``causal``,
-    ``j <= i + sk - sq`` (bottom-right alignment).  ``doc_start`` (int ``[b, sq]``, packed sequences) adds
+    ``j <= i + sk - sq`` (bottom-right alignment) or ``j < prefix_lens[b]`` (int ``[b]``, causal only: a prefix LM's
+    bidirectional context, counted in key coordinates).  ``doc_start`` (int ``[b, sq]``, packed sequences) adds
     ``j >= doc_start[b, i]``, with ``doc_start`` clamped to ``[0, i]`` so that every query sees itself."""
+    if prefix_lens is not None and not causal:
+        raise ValueError("prefix_lens needs causal=True")
     j = torch.arange(sk, device=device)
     vis = torch.ones(1, sq, sk, dtype=torch.bool, device=device)
     if causal:
-        vis = vis & (j[None, :] <= torch.arange(sq, device=device)[:, None] + (sk - sq))[None]
+        c = (j[None, :] <= torch.arange(sq, device=device)[:, None] + (sk - sq))[None]
+        if prefix_lens is not None:
+            c = c | (j[None, None, :] < prefix_lens.to(device=device, dtype=torch.long)[:, None, None])
+        vis = vis & c
     if doc_start is not None:
         i = torch.arange(sq, device=device)
         beg = torch.minimum(doc_start.to(device=device, dtype=torch.long).clamp(min=0), i[None, :])
@@ -651,17 +658,18 @@ def _prep_bias(bias, q):
 
 class _FlashAttnFn(torch.autograd.Function):
     """Flash attention on ``[b, a, sq, d]`` / ``[b, g, sk, d]`` views with optional additive bias (dense or ALiBi
-    slopes), per-sample key windows (``kv_start`` / ``kv_lens``) and Philox dropout on the probabilities — all inside
-    the wgmma kernels."""
+    slopes), per-sample key windows (``kv_start`` / ``kv_lens``), a prefix-LM prefix (``prefix_lens``) and Philox
+    dropout on the probabilities — all inside the wgmma kernels."""
 
     @staticmethod
-    def forward(ctx, q, k, v, causal, scale, bias, alibi_slopes, p_drop, kv_lens, kv_start=None):
+    def forward(ctx, q, k, v, causal, scale, bias, alibi_slopes, p_drop, kv_lens, kv_start=None, prefix_lens=None):
         ext = load_ext()
         b = _prep_bias(bias, q)
+        ctx.prefix = {} if prefix_lens is None else {"prefix_lens": prefix_lens}
         o, lse, rng_state = ext.attn_fwd(q, k, v, causal, scale, kv_lens, b, alibi_slopes, p_drop,
-                                         tp_rng_salt(True) if p_drop > 0 else 0, kv_start)
+                                         tp_rng_salt(True) if p_drop > 0 else 0, kv_start, **ctx.prefix)
         count_launch()
-        ctx.save_for_backward(q, k, v, o, lse, b, alibi_slopes, rng_state, kv_lens, kv_start)
+        ctx.save_for_backward(q, k, v, o, lse, b, alibi_slopes, rng_state, kv_lens, kv_start, prefix_lens)
         ctx.causal, ctx.scale, ctx.p_drop = causal, scale, p_drop
         ctx.bias_shape = None if bias is None else (bias.shape, bias.dtype)
         return o
@@ -669,20 +677,21 @@ class _FlashAttnFn(torch.autograd.Function):
     @staticmethod
     def backward(ctx, go):
         ext = load_ext()
-        q, k, v, o, lse, b, slopes, rng_state, kv_lens, kv_start = ctx.saved_tensors
+        q, k, v, o, lse, b, slopes, rng_state, kv_lens, kv_start, prefix_lens = ctx.saved_tensors
+        prefix = {} if prefix_lens is None else {"prefix_lens": prefix_lens}
         dbias = None
         if b is not None and ctx.needs_input_grad[5]:
             dbias = torch.zeros(b.shape, dtype=torch.float32, device=b.device)
             if dbias.stride() != b.stride():
                 dbias = torch.empty_strided(b.shape, b.stride(), dtype=torch.float32, device=b.device).zero_()
         dq, dk, dv, _ = ext.attn_bwd(go, q, k, v, o, lse, ctx.causal, ctx.scale, kv_lens, b, slopes, dbias, ctx.p_drop,
-                                     rng_state if ctx.p_drop > 0 else None, kv_start)
+                                     rng_state if ctx.p_drop > 0 else None, kv_start, **prefix)
         count_launch(3)
         gb = None
         if dbias is not None:
             shape, dtype = ctx.bias_shape
             gb = dbias.to(dtype).reshape(shape)
-        return dq, dk, dv, None, None, gb, None, None, None, None
+        return dq, dk, dv, None, None, gb, None, None, None, None, None
 
 
 class _FlashAttnPackedFn(torch.autograd.Function):
@@ -757,7 +766,8 @@ def attention_supported(q, k, mask=None, bias=None) -> bool:
 
 
 def attention(q, k, v, *, causal: bool = False, scale: Optional[float] = None, mask=None, bias=None,
-              dropout_p: float = 0.0, training: bool = False, alibi_slopes=None, kv_lens=None, kv_start=None):
+              dropout_p: float = 0.0, training: bool = False, alibi_slopes=None, kv_lens=None, kv_start=None,
+              prefix_lens=None):
     """Softmax attention of q ``[b, a, sq, d]`` over k, v ``[b, g, sk, d]`` (``g = a`` or, grouped-query, a divisor of
     ``a``; ``sq`` and ``sk`` independent).  Key ``j`` is visible to query ``i`` of sample ``b`` iff
     ``kv_start[b] <= j < kv_lens[b]`` (int32 ``[b]`` device tensors, defaults ``0`` and ``sk``; ``kv_lens`` is clamped to
@@ -765,15 +775,22 @@ def attention(q, k, v, *, causal: bool = False, scale: Optional[float] = None, m
     gets zeros.  The native flash kernels (see :func:`attention_supported`) handle this masking, an additive score bias
     (dense ``[b|1, a|1, sq, sk]`` — T5 relative positions — or ``alibi_slopes`` ``[a]``, ``slope·(j − i − (sk − sq))``)
     and dropout on the probabilities; arbitrary dense 0/1 masks use the reference math.  The reference applies
-    ``kv_lens`` only together with ``kv_start``."""
+    ``kv_lens`` only together with ``kv_start`` or ``prefix_lens``.
+
+    ``prefix_lens`` (int32 ``[b]`` device tensor, ``causal`` only, without ``bias`` or ``alibi_slopes``): a prefix LM,
+    key ``j`` is also visible to every query when ``j < prefix_lens[b]`` (GLM's bidirectional context, counted in key
+    coordinates).  The reference math builds the same rule densely (:func:`visible_keys`)."""
     if scale is None:
         scale = 1.0 / math.sqrt(q.shape[-1])
+    if prefix_lens is not None and (not causal or bias is not None or alibi_slopes is not None):
+        raise ValueError("prefix_lens needs causal=True and combines with neither bias nor alibi_slopes")
     if attention_supported(q, k, mask, bias):
         # strided [b, a, s, d] views of the packed QKV projection are consumed directly (TMA strides)
         return _FlashAttnFn.apply(q, k, v, causal, float(scale), bias, alibi_slopes,
-                                  float(dropout_p) if training else 0.0, kv_lens, kv_start)
-    if kv_start is not None:
-        vis = visible_keys(q.shape[-2], k.shape[-2], causal=causal, kv_start=kv_start, kv_lens=kv_lens, device=q.device)
+                                  float(dropout_p) if training else 0.0, kv_lens, kv_start, prefix_lens)
+    if kv_start is not None or prefix_lens is not None:
+        vis = visible_keys(q.shape[-2], k.shape[-2], causal=causal, kv_start=kv_start, kv_lens=kv_lens,
+                           prefix_lens=prefix_lens, device=q.device)
         if mask is not None:
             vis = vis & mask.bool()
         o = attention(q, k, v, causal=False, scale=scale, mask=vis, bias=bias, dropout_p=dropout_p, training=training,

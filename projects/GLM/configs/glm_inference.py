@@ -14,7 +14,7 @@ cfg = DictConfig(
         num_beam_groups=1, diversity_penalty=0.0, temperature=1.0, top_k=50, top_p=1.0, typical_p=1.0,
         repetition_penalty=1.0, length_penalty=1.0, no_repeat_ngram_size=0, encoder_no_repeat_ngram_size=0,
         num_return_sequences=1, chunk_size_feed_forward=0, output_scores=False, forced_bos_token_id=None,
-        forced_eos_token_id=None, remove_invalid_values=False, exponential_decay_length_penalty=None, use_cache=False,
+        forced_eos_token_id=None, remove_invalid_values=False, exponential_decay_length_penalty=None, use_cache=True,
         pad_token_id=50000, eos_token_id=50007, bos_token_id=None, sep_token_id=None, decoder_start_token_id=None,
     )
 )
