@@ -700,19 +700,6 @@ Tensor glm_rotary_qkv_bwd(const Tensor& grad, int64_t heads, int64_t kv_heads, c
   return dmixed;
 }
 
-Tensor rope(const Tensor& x, const Tensor& cosv, const Tensor& sinv, bool backward) {
-  Args args("rope");
-  args("x", x, at::kBFloat16, {kAny, kAny, kAny, kAny});
-  const int S = (int)x.size(2), D = (int)x.size(3);
-  rope_tables(args, cosv, sinv, S, D);
-  const auto guard = args.guard();
-  Tensor y = at::empty_like(x);
-  check(lb_rope(x.data_ptr(), cosv.data_ptr<float>(), sinv.data_ptr<float>(), y.data_ptr(), x.numel() / D, S, D,
-                backward ? 1 : 0, cur_stream()),
-        "rope");
-  return y;
-}
-
 // ---- cross entropy ------------------------------------------------------------------------------------
 // logits bf16 or fp32 [T, V], labels int64 [T]
 void ce_args(Args& args, const Tensor& logits, const Tensor& labels) {
@@ -1326,7 +1313,6 @@ TORCH_LIBRARY(libai_b200, m) {
   m.def("swiglu_packed_fwd(Tensor gu) -> Tensor", &swiglu_packed_fwd);
   m.def("swiglu_packed_bwd(Tensor gy, Tensor gu) -> Tensor", &swiglu_packed_bwd);
   m.def("dgrad_actgrad(Tensor gy, Tensor w, Tensor pre, int act, Tensor(a!)? bias_grad=None) -> Tensor", &dgrad_actgrad);
-  m.def("rope(Tensor x, Tensor cos, Tensor sin, bool backward) -> Tensor", &rope);
   m.def("rope_qkv(Tensor(a!) qkv, Tensor cos, Tensor sin, int pos_offset, bool backward, bool inplace, Tensor? positions=None) -> Tensor(a!)", &rope_qkv);
   m.def("glm_rotary_qkv(Tensor mixed, int heads, int kv_heads, Tensor table, int pos_offset, Tensor? position_ids, bool grouped) -> Tensor", &glm_rotary_qkv);
   m.def("glm_rotary_qkv_bwd(Tensor grad, int heads, int kv_heads, Tensor table, int pos_offset, Tensor? position_ids) -> Tensor", &glm_rotary_qkv_bwd);

@@ -310,6 +310,22 @@ LB_DEVICE uint2 e4m3x4_to_bf16x4(uint32_t x) {
   return make_uint2(e4m3x2_to_bf16x2(static_cast<uint16_t>(x)), e4m3x2_to_bf16x2(static_cast<uint16_t>(x >> 16)));
 }
 
+// Rotary embedding in the rotate-half convention: the channel pair (x1, x2) = (c, c + D/2) of a head at position pos,
+// with c1, c2 = cos[pos, c], cos[pos, c + D/2] and s1, s2 the same of sin (fp32 tables [P, D]).  The backward applies
+// the transposed rotation.  Every rotate-half kernel rotates through this one helper, so they agree bit for bit.
+struct RopePair {
+  float c1, c2, s1, s2;
+  LB_DEVICE static RopePair load(const float* __restrict__ cosv, const float* __restrict__ sinv, int pos, int c,
+                                 int D) {
+    const int half = D / 2;
+    return {cosv[pos * D + c], cosv[pos * D + c + half], sinv[pos * D + c], sinv[pos * D + c + half]};
+  }
+  LB_DEVICE float2 rotate(float x1, float x2, bool backward) const {
+    return backward ? make_float2(x1 * c1 + x2 * s2, x2 * c2 - x1 * s1)
+                    : make_float2(x1 * c1 - x2 * s1, x2 * c2 + x1 * s2);
+  }
+};
+
 // one Adam step of one element, shared by fused_adamw and the ZeRO update: g = grad * scale (+ wd * p when the weight
 // decay is coupled), fp32 moments m, v, bias corrections bc1, bc2; decoupled weight decay adds wd * p to the update
 LB_DEVICE void adam_element(float& p, float& m, float& v, float grad, float scale, float lr, float b1, float b2, float eps,

@@ -31,8 +31,8 @@ __device__ __forceinline__ void quantize_row(const float (&x)[2 * P], uint8_t* r
 }
 
 // the FP8 cache append: one warp per (b, i, group); lane c < D/2 handles the pairs (c + 32 p, c + 32 p + D/2) of the
-// r q rows and of k (rotated with the expressions of kv_append_kernel, so q and the bf16 k row are bit-identical to
-// its output) and of v, then each of the k and v rows is quantized (quantize_row) at row cache_seqlens[b] + i
+// r q rows and of k (rotated, RopePair) and of v, then each of the k and v rows is quantized (quantize_row) at row
+// cache_seqlens[b] + i
 template <int D>
 __global__ void __launch_bounds__(256) kv_append_fp8_kernel(
     const __nv_bfloat16* __restrict__ qkv, const float* __restrict__ cosv, const float* __restrict__ sinv,
@@ -49,15 +49,11 @@ __global__ void __launch_bounds__(256) kv_append_fp8_kernel(
     const int pos = seqlens[b] + i;
     const size_t in = grp * (r + 2) * D;
     const size_t crow = ((size_t)b * G + g) * C + pos;
-    float c1[P], c2[P], s1[P], s2[P];
+    RopePair t[P];
 #pragma unroll
     for (int p = 0; p < P; ++p) {
-      const int c = lane + 32 * p;
-      c1[p] = 1.f, c2[p] = 1.f, s1[p] = 0.f, s2[p] = 0.f;
-      if (cosv != nullptr) {
-        c1[p] = cosv[pos * D + c], c2[p] = cosv[pos * D + c + half];
-        s1[p] = sinv[pos * D + c], s2[p] = sinv[pos * D + c + half];
-      }
+      t[p] = RopePair{1.f, 1.f, 0.f, 0.f};
+      if (cosv != nullptr) t[p] = RopePair::load(cosv, sinv, pos, lane + 32 * p, D);
     }
     float kx[2 * P], vx[2 * P];   // the bf16 k and v values of this lane: [2p] column c, [2p + 1] column c + D/2
     for (int j = 0; j <= r; ++j) {   // slots 0 .. r - 1: q of query head g * r + j; slot r: k
@@ -66,18 +62,14 @@ __global__ void __launch_bounds__(256) kv_append_fp8_kernel(
       for (int p = 0; p < P; ++p) {
         const int c = lane + 32 * p;
         const float x1 = __bfloat162float(qkv[src + c]), x2 = __bfloat162float(qkv[src + c + half]);
-        float y1 = x1, y2 = x2;
-        if (cosv != nullptr) {
-          y1 = x1 * c1[p] - x2 * s1[p];
-          y2 = x2 * c2[p] + x1 * s2[p];
-        }
+        const float2 y = cosv != nullptr ? t[p].rotate(x1, x2, false) : make_float2(x1, x2);
         if (j == r) {
-          kx[2 * p] = __bfloat162float(__float2bfloat16(y1));
-          kx[2 * p + 1] = __bfloat162float(__float2bfloat16(y2));
+          kx[2 * p] = __bfloat162float(__float2bfloat16(y.x));
+          kx[2 * p + 1] = __bfloat162float(__float2bfloat16(y.y));
         } else if (q_out != nullptr) {
           const size_t qrow = (grp * r + j) * D;
-          q_out[qrow + c] = __float2bfloat16(y1);
-          q_out[qrow + c + half] = __float2bfloat16(y2);
+          q_out[qrow + c] = __float2bfloat16(y.x);
+          q_out[qrow + c + half] = __float2bfloat16(y.y);
         }
       }
     }

@@ -4,9 +4,9 @@
 // [B, Sq, G, r + 2, D] with q_0 .. q_{r-1}, k, v per group (r = 1: per-head [q|k|v]), and the caches hold the G heads.
 //
 // lb_kv_append: one pass over the packed projection.  q and k are rotated with the fp32 cos/sin tables in the
-//   rotate-half convention of rope_qkv_kernel (same expressions, so the rotated values are bit-identical), k and v are
-//   written into the layer's cache K, V [B, G, C, D] at rows cache_seqlens[b] + i, and the rotated q goes to
-//   q_out [B, Sq, A, D].  Without tables (GPT-2) the values are copied unrotated.
+//   rotate-half convention (RopePair, as rope_qkv_kernel rotates them), k and v are written into the layer's cache
+//   K, V [B, G, C, D] at rows cache_seqlens[b] + i, and the rotated q goes to q_out [B, Sq, A, D].  Without tables
+//   (GPT-2) the values are copied unrotated.
 //
 // lb_decode_attn: o [B, Sq, A, D] for 1 <= Sq <= 16 new queries per (sample, head).  Query i of sample b sees exactly the
 //   keys j with kv_start[b] <= j <= cache_seqlens[b] + i (kv_start = left padding, cache_seqlens = length before this
@@ -75,8 +75,7 @@ __global__ void __launch_bounds__(128) decode_combine_kernel(const Params p, int
   }
 }
 
-// one thread per (b, i, group, c < D/2): the r q pairs and the k pair (c, c + D/2) rotated exactly like rope_qkv_kernel,
-// v copied
+// one thread per (b, i, group, c < D/2): the r q pairs and the k pair (c, c + D/2) rotated (RopePair), v copied
 __global__ void kv_append_kernel(const __nv_bfloat16* __restrict__ qkv, const float* __restrict__ cosv,
                                  const float* __restrict__ sinv, __nv_bfloat16* __restrict__ q_out,
                                  __nv_bfloat16* __restrict__ kc, __nv_bfloat16* __restrict__ vc,
@@ -92,26 +91,19 @@ __global__ void kv_append_kernel(const __nv_bfloat16* __restrict__ qkv, const fl
     const int pos = seqlens[b] + i;
     const size_t in = grp * (r + 2) * D;
     const size_t crow = (((size_t)b * G + g) * C + pos) * D;
-    float c1 = 1.f, c2 = 1.f, s1 = 0.f, s2 = 0.f;
-    if (cosv != nullptr) {
-      c1 = cosv[pos * D + c], c2 = cosv[pos * D + c + half];
-      s1 = sinv[pos * D + c], s2 = sinv[pos * D + c + half];
-    }
+    RopePair t{1.f, 1.f, 0.f, 0.f};
+    if (cosv != nullptr) t = RopePair::load(cosv, sinv, pos, c, D);
     for (int j = 0; j <= r; ++j) {   // slots 0 .. r - 1: q of query head g * r + j; slot r: k
       const size_t src = in + (size_t)j * D;
       const float x1 = __bfloat162float(qkv[src + c]), x2 = __bfloat162float(qkv[src + c + half]);
-      float y1 = x1, y2 = x2;
-      if (cosv != nullptr) {
-        y1 = x1 * c1 - x2 * s1;
-        y2 = x2 * c2 + x1 * s2;
-      }
+      const float2 y = cosv != nullptr ? t.rotate(x1, x2, false) : make_float2(x1, x2);
       if (j == r) {
-        kc[crow + c] = __float2bfloat16(y1);
-        kc[crow + c + half] = __float2bfloat16(y2);
+        kc[crow + c] = __float2bfloat16(y.x);
+        kc[crow + c + half] = __float2bfloat16(y.y);
       } else if (q_out != nullptr) {
         const size_t qrow = (grp * r + j) * D;    // [B, Sq, A, D] with A = G * r
-        q_out[qrow + c] = __float2bfloat16(y1);
-        q_out[qrow + c + half] = __float2bfloat16(y2);
+        q_out[qrow + c] = __float2bfloat16(y.x);
+        q_out[qrow + c + half] = __float2bfloat16(y.y);
       }
     }
     vc[crow + c] = qkv[in + (size_t)(r + 1) * D + c];

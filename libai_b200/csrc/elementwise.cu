@@ -200,38 +200,10 @@ __global__ void swiglu_bwd_kernel(const __nv_bfloat16* __restrict__ gy, const __
   }
 }
 
-// RoPE ("rotate_half" convention): x [B, A, S, D] contiguous, cos/sin fp32 [S, D]
-//   fwd: y = x*cos + rot(x)*sin, rot(x) = cat(-x2, x1);   bwd: gx = g*cos + rot^T(g*sin) = g*cos - rot(g*sin) ... (below)
-__global__ void rope_kernel(const __nv_bfloat16* __restrict__ x, const float* __restrict__ cosv,
-                            const float* __restrict__ sinv, __nv_bfloat16* __restrict__ y, size_t rows, int S, int D,
-                            int backward) {
-  const int half = D / 2;
-  const size_t total = rows * half;
-  for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
-    const size_t row = i / half;
-    const int c = static_cast<int>(i % half);
-    const int s = static_cast<int>(row % S);
-    const float x1 = __bfloat162float(x[row * D + c]), x2 = __bfloat162float(x[row * D + c + half]);
-    const float c1 = cosv[s * D + c], c2 = cosv[s * D + c + half];
-    const float s1 = sinv[s * D + c], s2 = sinv[s * D + c + half];
-    float y1, y2;
-    if (!backward) {
-      y1 = x1 * c1 - x2 * s1;
-      y2 = x2 * c2 + x1 * s2;
-    } else {
-      y1 = x1 * c1 + x2 * s2;
-      y2 = x2 * c2 - x1 * s1;
-    }
-    y[row * D + c] = __float2bfloat16(y1);
-    y[row * D + c + half] = __float2bfloat16(y2);
-  }
-}
-
-// Rotary embedding on the grouped packed QKV projection [tokens(b*s), G, r + 2, D] (per K/V group q_0 .. q_{r-1}, k, v;
-// r = 1 is the per-head [q|k|v] layout): the r + 1 q/k slots are rotated with the position (s + pos_offset), or with
-// positions[token] (int32 [tokens], packed sequences; clamped to the npos rows of the tables) when given, v is
-// copied.  `y` may alias `x` (in-place, used by the backward).  POS: positions given (a separate instance, so the
-// s + pos_offset instance compiles to the same arithmetic as kv_append_kernel, with which it is bit-identical).
+// Rotary embedding (RopePair) on the grouped packed QKV projection [tokens(b*s), G, r + 2, D] (per K/V group q_0 ..
+// q_{r-1}, k, v; r = 1 is the per-head [q|k|v] layout): the r + 1 q/k slots are rotated with the position
+// (s + pos_offset), or with positions[token] (int32 [tokens], packed sequences; clamped to the npos rows of the tables)
+// when given, v is copied.  `y` may alias `x` (in-place, used by the backward).  POS: positions given.
 template <bool POS>
 __global__ void rope_qkv_kernel(const __nv_bfloat16* __restrict__ x, const float* __restrict__ cosv,
                                 const float* __restrict__ sinv, __nv_bfloat16* __restrict__ y, size_t groups, int S,
@@ -252,18 +224,9 @@ __global__ void rope_qkv_kernel(const __nv_bfloat16* __restrict__ x, const float
       continue;
     }
     const int s = POS ? min(max(positions[head / G], 0), npos - 1) : static_cast<int>((head / G) % S) + pos_offset;
-    const float c1 = cosv[s * D + c], c2 = cosv[s * D + c + half];
-    const float s1 = sinv[s * D + c], s2 = sinv[s * D + c + half];
-    float y1, y2;
-    if (!backward) {
-      y1 = x1 * c1 - x2 * s1;
-      y2 = x2 * c2 + x1 * s2;
-    } else {
-      y1 = x1 * c1 + x2 * s2;
-      y2 = x2 * c2 - x1 * s1;
-    }
-    y[base + c] = __float2bfloat16(y1);
-    y[base + c + half] = __float2bfloat16(y2);
+    const float2 rot = RopePair::load(cosv, sinv, s, c, D).rotate(x1, x2, backward);
+    y[base + c] = __float2bfloat16(rot.x);
+    y[base + c + half] = __float2bfloat16(rot.y);
   }
 }
 
@@ -748,13 +711,6 @@ extern "C" int lb_swiglu_packed_bwd(const void* gy, const void* gu, void* dgu, l
   if (rows == 0) return 0;
   lb::swiglu_packed_bwd_kernel<<<ew_grid(rows * F / 8, 256), 256, 0, s>>>((const bf16*)gy, (const bf16*)gu, (bf16*)dgu,
                                                                          (size_t)rows, (size_t)(F / 8));
-  return (int)cudaGetLastError();
-}
-extern "C" int lb_rope(const void* x, const float* cosv, const float* sinv, void* y, long rows, int S, int D,
-                       int backward, cudaStream_t s) {
-  if (rows == 0) return 0;
-  lb::rope_kernel<<<ew_grid((size_t)rows * D / 2, 256), 256, 0, s>>>((const bf16*)x, cosv, sinv, (bf16*)y,
-                                                                     (size_t)rows, S, D, backward);
   return (int)cudaGetLastError();
 }
 // groups = tokens * G; r query heads per group; positions (optional, int32 [tokens]) replaces s + pos_offset, npos =

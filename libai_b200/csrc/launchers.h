@@ -83,8 +83,6 @@ int lb_swiglu_packed_fwd(const void* gu, void* y, long rows, long F, cudaStream_
 int lb_swiglu_packed_bwd(const void* gy, const void* gu, void* dgu, long rows, long F, cudaStream_t s);
 int lb_rope_qkv(const void* x, const float* cosv, const float* sinv, void* y, long groups, int S, int G, int r, int D,
                 int pos_offset, const int* positions, int npos, int backward, cudaStream_t s);
-int lb_rope(const void* x, const float* cosv, const float* sinv, void* y, long rows, int S, int D, int backward,
-            cudaStream_t s);
 // ChatGLM rotary between the fused projection [tokens, (A + 2G) * D] and a packed layout (grouped [tokens, G, A/G + 2,
 // D] or per-head [tokens, A, 3D]): forward packs (in = fused, out = packed), backward unpacks the gradient (in =
 // packed, out = fused); table fp32 [npos, D/4, 2], positions optional int32 [S]

@@ -26,7 +26,7 @@ from torch import nn
 
 from libai_b200.config import configurable
 from libai_b200.layers import Linear, RMSLayerNorm, VocabEmbedding
-from libai_b200.layers._param import xavier_normal_
+from libai_b200.layers._param import param_device, xavier_normal_
 from libai_b200.layers.attention import AttnMaskType
 from libai_b200.layers.embedding import get_sp_shape, set_sp_shape
 from libai_b200.ops import functional as OF
@@ -274,7 +274,8 @@ class LlamaModel(nn.Module):
         self._set_cos_sin_cache(hidden_size // num_attention_heads, max_position_embeddings, base=rope_base)
 
     def _set_cos_sin_cache(self, rotary_dim, seq_len, base=10000, dtype=None, layer_idx=0):
-        cos, sin = rotary_tables(rotary_dim, seq_len, base)
+        # computed on the CPU (the same values on every device), held where the parameters are
+        cos, sin = (t.to(param_device()) for t in rotary_tables(rotary_dim, seq_len, base))
         self.register_buffer("cos_cached", cos, persistent=False)
         self.register_buffer("sin_cached", sin, persistent=False)
 
@@ -291,8 +292,6 @@ class LlamaModel(nn.Module):
         if isinstance(past_key_values, StaticKVCache):
             # the layers append in place; the lengths advance once every layer has seen this step's tokens
             cache = past_key_values
-            if self.cos_cached.device != input_ids.device:   # tables built on the CPU for a model built on the GPU
-                self.cos_cached, self.sin_cached = self.cos_cached.to(input_ids.device), self.sin_cached.to(input_ids.device)
             hidden_states = self.embed(input_ids)
             for i, layer in enumerate(self.layers):
                 hidden_states = layer(hidden_states, attention_mask=attention_mask, past_key_value=cache.layer(i),

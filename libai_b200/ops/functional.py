@@ -930,14 +930,11 @@ def kv_cache_append(qkv, k_cache, v_cache, cache_seqlens, cos=None, sin=None, re
 
 def kv_cache_append_ref(qkv, k_cache, v_cache, cache_seqlens, cos=None, sin=None, k_scale=None, v_scale=None):
     s_len = qkv.shape[1]
-    q, k, v = split_qkv(qkv)
     starts = [int(x) for x in cache_seqlens.tolist()]
     if cos is not None:
         pos = torch.tensor(starts, device=cos.device)[:, None] + torch.arange(s_len, device=cos.device)[None]
-        c = cos[pos][:, :, None, :].to(qkv.dtype)
-        sn = sin[pos][:, :, None, :].to(qkv.dtype)
-        q = q * c + rotate_half(q) * sn
-        k = k * c + rotate_half(k) * sn
+        qkv = _rotary_qkv_ref(qkv, cos, sin, position_ids=pos)
+    q, k, v = split_qkv(qkv)
     for b, st in enumerate(starts):
         for cache, scale, x in ((k_cache, k_scale, k[b]), (v_cache, v_scale, v[b])):
             if scale is None:
@@ -1166,33 +1163,6 @@ def rotate_half(x):
     return torch.cat((-x2, x1), dim=-1)
 
 
-class _RopeFn(torch.autograd.Function):
-    @staticmethod
-    def forward(ctx, x, cos, sin):
-        ext = load_ext()
-        ctx.save_for_backward(cos, sin)
-        count_launch()
-        return ext.rope(x.contiguous(), cos, sin, False)
-
-    @staticmethod
-    def backward(ctx, g):
-        ext = load_ext()
-        cos, sin = ctx.saved_tensors
-        count_launch()
-        return ext.rope(g.contiguous(), cos, sin, True), None, None
-
-
-def apply_rotary(x, cos, sin):
-    """x ``[b, a, s, d]``; cos/sin ``[s, d]`` (HF "rotate_half" convention; reference
-    projects/Llama/llama.py:31-43)."""
-    if use_native(x) and x.dtype == torch.bfloat16 and cos.dtype == torch.float32:
-        return _RopeFn.apply(x, cos, sin)
-    c = cos[None, None].to(x.dtype)
-    s = sin[None, None].to(x.dtype)
-    return x * c + rotate_half(x) * s
-
-
-
 class _RopeQKVFn(torch.autograd.Function):
     """Rotary embedding on every q and k of the packed projection (``[b, s, a, 3d]`` or ``[b, s, g, r + 2, d]``) in one
     pass (v copied);
@@ -1222,6 +1192,11 @@ def apply_rotary_qkv(qkv, cos, sin, pos_offset: int = 0, position_ids=None):
     ``position_ids[b, i]`` (int32 ``[b, s]``, packed sequences; clamped to the tables) when given."""
     if use_native(qkv) and qkv.dtype == torch.bfloat16 and cos.dtype == torch.float32 and qkv.is_contiguous():
         return _RopeQKVFn.apply(qkv, cos, sin, int(pos_offset), position_ids)
+    return _rotary_qkv_ref(qkv, cos, sin, pos_offset, position_ids)
+
+
+def _rotary_qkv_ref(qkv, cos, sin, pos_offset=0, position_ids=None):
+    """The reference math of :func:`apply_rotary_qkv` (reference projects/Llama/llama.py:31-43)."""
     s_len = qkv.shape[1]
     if position_ids is not None:   # [b, s, 1, d] (+ a group axis below)
         idx = position_ids.to(device=cos.device, dtype=torch.long).clamp(0, cos.shape[0] - 1)

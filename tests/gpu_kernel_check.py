@@ -460,26 +460,6 @@ def main():
 
     record("accumulating colsum / norm_bwd", accum_grads)
 
-    def rope():
-        from libai_b200.ops.functional import rotate_half
-
-        x = torch.randn(2, 4, 128, 64, device="cuda").bfloat16()
-        pos = torch.arange(128, device="cuda").float()
-        inv = 1.0 / (10000 ** (torch.arange(0, 64, 2, device="cuda").float() / 64))
-        fr = torch.outer(pos, inv)
-        emb = torch.cat([fr, fr], -1)
-        cos, sin = emb.cos().contiguous(), emb.sin().contiguous()
-        y = ext.rope(x, cos, sin, False)
-        xf = x.float().requires_grad_(True)
-        ref = xf * cos + rotate_half(xf) * sin
-        gy = torch.randn_like(ref)
-        ref.backward(gy)
-        gx = ext.rope(gy.bfloat16(), cos, sin, True)
-        e = [rel_err(y, ref), rel_err(gx, xf.grad)]
-        return {"ok": max(e) < 2e-2, "errs": e}
-
-    record("rope", rope)
-
     def rope_qkv():
         from libai_b200.ops.functional import rotate_half
 
@@ -500,6 +480,29 @@ def main():
         return {"ok": max(e) < 2e-2, "errs": e}
 
     record("rope_qkv packed", rope_qkv)
+
+    def rope_qkv_positions():
+        from libai_b200.ops.functional import rotate_half
+
+        b, sq, g, r, d = 2, 96, 2, 4, 128
+        qkv = torch.randn(b, sq, g, r + 2, d, device="cuda").bfloat16()
+        inv = 1.0 / (10000 ** (torch.arange(0, d, 2, device="cuda").float() / d))
+        fr = torch.outer(torch.arange(sq, device="cuda").float(), inv)
+        emb = torch.cat([fr, fr], -1)
+        cos, sin = emb.cos().contiguous(), emb.sin().contiguous()
+        pos = torch.randint(0, sq, (b, sq), device="cuda", dtype=torch.int32)
+        y = ext.rope_qkv(qkv, cos, sin, 0, False, False, pos)
+        c, s_ = cos[pos.long()][:, :, None, None], sin[pos.long()][:, :, None, None]
+        qf = qkv.float().requires_grad_(True)
+        qk = qf[..., :r + 1, :]
+        ref = torch.cat([qk * c + rotate_half(qk) * s_, qf[..., r + 1:, :]], 3)
+        gy = torch.randn_like(ref)
+        ref.backward(gy)
+        gx = ext.rope_qkv(gy.bfloat16(), cos, sin, 0, True, False, pos)
+        e = [rel_err(y, ref.detach()), rel_err(gx, qf.grad)]
+        return {"ok": max(e) < 2e-2, "errs": e}
+
+    record("rope_qkv grouped, per-token positions (fwd + bwd)", rope_qkv_positions)
 
     # ------------------------------------------------------------------ cross entropy
     def ce():

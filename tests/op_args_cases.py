@@ -154,13 +154,12 @@ def cases(dev):
         _c("swiglu_packed_fwd", dict(gu=r(16, 128)), ["gu:dtype=float32", "gu:misalign", "gu:noncontig"], [(16, 64)]),
         _c("swiglu_packed_bwd", dict(gy=r(16, 64), gu=r(16, 128)),
            ["gy:short", "gy:dtype=float32", "gy:device"], [(16, 128)]),
-        _c("rope", dict(x=r(1, 2, 16, 64), cos=r(16, 64, dtype=F32), sin=r(16, 64, dtype=F32), backward=False),
-           ["x:noncontig", ("sin:short", "rope: cos/sin"), ("sin:dtype=float64", "rope: cos/sin"),
-            ("cos:device", "rope: cos/sin must be on")], [(1, 2, 16, 64)]),
         _c("rope_qkv", dict(qkv=r(1, 16, 2, 192), cos=r(16, 64, dtype=F32), sin=r(16, 64, dtype=F32), pos_offset=0,
                             backward=False, inplace=False, positions=ar(16).view(1, 16)),
-           ["qkv:dtype=float32", "positions:dtype=int64", "positions:narrow", "positions:device",
-            ("cos:device", "rope_qkv: cos/sin must be on")], [(1, 16, 2, 192)]),
+           ["qkv:dtype=float32", "qkv:noncontig", "positions:dtype=int64", "positions:narrow", "positions:device",
+            ("cos:narrow", "rope_qkv: cos/sin"), ("sin:short", "rope_qkv: cos/sin"),
+            ("sin:dtype=float64", "rope_qkv: cos/sin"), ("cos:device", "rope_qkv: cos/sin must be on")],
+           [(1, 16, 2, 192)]),
         _c("glm_rotary_qkv", dict(mixed=r(1, 8, 512), heads=4, kv_heads=2, table=r(16, 16, 2, dtype=F32),
                                   pos_offset=0, position_ids=ar(8).view(1, 8), grouped=False),
            [("mixed:noncontig", "glm_rotary_qkv: contiguous"), "table:dtype=float64", "table:device",

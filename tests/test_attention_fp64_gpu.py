@@ -338,28 +338,6 @@ def rotate(x, cos, sin, backward):
     return rope_ref(xd[..., :h], xd[..., h:], c[..., :h], c[..., h:], s[..., :h], s[..., h:], backward)
 
 
-@pytest.mark.parametrize("D", [64, 128])
-@pytest.mark.parametrize("backward", [False, True])
-def test_rope_per_element(ext, D, backward):
-    B, A, S = 2, 3, 77
-    x = rand(B, A, S, D, seed=61, scale=4.0)
-    cos, sin = tables(S + 40, D)
-    y = ext.rope(x, cos, sin, backward)
-    ref, bnd = rotate(x, cos[:S], sin[:S], backward)
-    check(y, ref, bnd, f"rope D={D} backward={backward}")
-
-
-def test_rope_rejects_bad_tables(ext):
-    x = rand(1, 2, 16, 64, seed=62)
-    cos, sin = tables(16, 64)
-    with pytest.raises(RuntimeError, match="cos/sin"):
-        ext.rope(x, cos, sin[:8].contiguous(), False)           # sin has fewer rows than positions
-    with pytest.raises(RuntimeError, match="cos/sin"):
-        ext.rope(x, cos, sin.double(), False)
-    with pytest.raises(RuntimeError, match="device"):
-        ext.rope(x, cos.cpu(), sin.cpu(), False)
-
-
 @pytest.mark.parametrize("r", [1, 4])
 @pytest.mark.parametrize("backward", [False, True])
 def test_rope_qkv_per_element(ext, r, backward):

@@ -603,19 +603,6 @@ def rotate(x, cos, sin, backward):
     return ref, U8 * ref.abs() + (1 + U8) * 2.0 ** -22 * torch.cat([m1, m2], -1) + R.FLUSH
 
 
-def test_apply_rotary():
-    B, A, S, D = 2, 3, 77, 64
-    cos, sin = rope_tables(S, D)
-    x0 = rand(B, A, S, D, seed=1, scale=4.0)
-    for layout, gy in upstream((B, A, S, D), seed=10):
-        x = x0.clone().requires_grad_()
-        y = OF.apply_rotary(x, cos, sin)
-        assert type(y.grad_fn).__name__ == "_RopeFnBackward"
-        y.backward(gy)
-        R.check(y, *rotate(x0, cos, sin, False), f"apply_rotary gy={layout} y")
-        R.check(x.grad, *rotate(gy, cos, sin, True), f"apply_rotary gy={layout} gx")
-
-
 @pytest.mark.parametrize("positions", ["offset", "position_ids"])
 @pytest.mark.parametrize("r", [1, 4])
 def test_apply_rotary_qkv(r, positions):

@@ -199,9 +199,30 @@ def test_gqa_llama_generate_runs_native_decode(head_dim, monkeypatch):
     assert rel_err(steps, ref) < 3e-2, rel_err(steps, ref)
 
 
+def test_llama_built_on_the_gpu_trains_through_forward_stage(monkeypatch):
+    """A model built under ``param_defaults(device=...)`` holds its rotary tables on that device, so a training step
+    through ``forward_stage`` (the blocks' path in the trainer and the pipeline schedules) rotates on the native
+    kernel without being moved first."""
+    from libai_b200 import ops
+
+    def refuse(*a, **k):
+        raise AssertionError("the reference rotary must not run on the native path")
+
+    monkeypatch.setenv("LIBAI_B200_IMPL", "native")
+    monkeypatch.setattr(OF, "rotate_half", refuse)
+    model = _gqa_llama(128).train()
+    ids = torch.randint(3, 512, (2, 128), device=DEV, generator=torch.Generator(device=DEV).manual_seed(5))
+    ops.reset_launch_count()
+    loss = model.forward_stage({"input_ids": ids, "labels": ids})["lm_loss"]
+    loss.backward()
+    assert ops.launch_count() > 0
+    assert torch.isfinite(loss)
+    assert all(torch.isfinite(p.grad).all() for p in model.parameters())
+
+
 def test_gqa_llama_training_is_bit_identical_run_to_run():
     def run():
-        model = _gqa_llama(128).to(DEV).train()   # (moves the rotary tables, which are built on the CPU)
+        model = _gqa_llama(128).train()
         opt = torch.optim.SGD(model.parameters(), lr=0.05)
         g = torch.Generator(device=DEV).manual_seed(7)
         losses = []

@@ -62,6 +62,21 @@ def test_append_rope_matches_apply_rotary_qkv():
     assert torch.equal(c.v[0][:, :, 4:7], want[..., 16:].transpose(1, 2))
 
 
+def test_llama_rotary_tables_are_built_where_the_parameters_are(monkeypatch):
+    """The training blocks, the uncached forward and cached decoding all read the model's cos / sin buffers, so they
+    must be on the parameters' device from the start (``meta`` stands in for a GPU here)."""
+    from libai_b200.layers._param import param_defaults
+    from libai_b200.models import LlamaForCausalLM
+    from libai_b200.utils import distributed as dutil
+
+    monkeypatch.setenv("LIBAI_B200_SKIP_INIT", "1")   # the initialisers draw from a torch.Generator, which meta lacks
+    dutil.reset_dist_util()
+    with param_defaults(device="meta"):
+        model = LlamaForCausalLM(DictConfig(LLAMA))
+    assert model.model.embed_tokens.weight.device.type == "meta"
+    assert model.model.cos_cached.device.type == "meta" and model.model.sin_cached.device.type == "meta"
+
+
 def test_growth_keeps_contents():
     c, _ = _filled_cache(cap=6)
     before = [t[:, :, :5].clone() for t in c.k + c.v]
