@@ -659,27 +659,36 @@ void check_glm_positions(const char* what, const c10::optional<Tensor>& position
   TORCH_CHECK(mn >= 0 && mx < P, what, ": position_ids must lie in [0, ", P, "), got [", mn, ", ", mx, "]");
 }
 
+// pos_base (optional, int32 [>= 1], not with position_ids): token i sits at pos_base[0] + pos_offset + i, read on the
+// device (a decoding step's cache length, e.g. cache_seqlens; a captured step then replays at the current length).
+// Like the lengths of kv_append, those positions are the caller's guarantee.
 Tensor glm_rotary_qkv(const Tensor& mixed, int64_t heads, int64_t kv_heads, const Tensor& table, int64_t pos_offset,
-                      const c10::optional<Tensor>& position_ids, bool grouped) {
+                      const c10::optional<Tensor>& position_ids, bool grouped, const c10::optional<Tensor>& pos_base) {
   TORCH_CHECK(mixed.dim() == 3, "glm_rotary_qkv: fused projection [b, s, (a + 2g) * d] expected, got ", mixed.sizes());
   TORCH_CHECK(heads > 0 && kv_heads > 0 && mixed.size(2) % (heads + 2 * kv_heads) == 0, "glm_rotary_qkv: last dim ",
               mixed.size(2), " is not (heads + 2 * kv_heads) * d");
+  TORCH_CHECK(!(given(pos_base) && given(position_ids)),
+              "glm_rotary_qkv: position_ids and pos_base exclude each other");
   const int64_t B = mixed.size(0), S = mixed.size(1), D = mixed.size(2) / (heads + 2 * kv_heads);
   Args args("glm_rotary_qkv");
-  const GlmRotary g = glm_rotary_args(args, "mixed", mixed, B, S, heads, kv_heads, D, table, pos_offset, position_ids);
+  // (the host-side range check of pos_offset does not apply to a device-side base)
+  const GlmRotary g = glm_rotary_args(args, "mixed", mixed, B, S, heads, kv_heads, D, table,
+                                      given(pos_base) ? 0 : pos_offset, position_ids);
+  const int* base = args.opt<const int>("pos_base", pos_base, at::kInt, {kAny});
+  TORCH_CHECK(base == nullptr || pos_base->numel() >= 1, "glm_rotary_qkv: pos_base must hold at least one element");
   const auto guard = args.guard();
   check_glm_positions("glm_rotary_qkv", position_ids, table.size(0));
   Tensor out = grouped ? at::empty({B, S, kv_heads, heads / kv_heads + 2, D}, mixed.options())
                        : at::empty({B, S, heads, 3 * D}, mixed.options());
   check(lb_glm_rotary_qkv(mixed.data_ptr(), table.data_ptr<float>(), out.data_ptr(), B * S, g.S, g.A, g.G, g.D,
-                          (int)pos_offset, g.positions, grouped ? 1 : 0, 0, cur_stream()),
+                          (int)pos_offset, g.positions, base, grouped ? 1 : 0, 0, cur_stream()),
         "glm_rotary_qkv");
   return out;
 }
 
 // grad: the gradient of glm_rotary_qkv's output (its rank tells the layout) -> the gradient of the fused projection
 Tensor glm_rotary_qkv_bwd(const Tensor& grad, int64_t heads, int64_t kv_heads, const Tensor& table, int64_t pos_offset,
-                          const c10::optional<Tensor>& position_ids) {
+                          const c10::optional<Tensor>& position_ids, const c10::optional<Tensor>& pos_base) {
   const bool grouped = grad.dim() == 5;
   TORCH_CHECK(heads > 0 && kv_heads > 0 && heads % kv_heads == 0, "glm_rotary_qkv_bwd: heads (", heads,
               ") must be a positive multiple of kv_heads (", kv_heads, ")");
@@ -688,14 +697,19 @@ Tensor glm_rotary_qkv_bwd(const Tensor& grad, int64_t heads, int64_t kv_heads, c
   TORCH_CHECK((grouped && grad.size(2) == kv_heads && grad.size(3) == heads / kv_heads + 2) ||
                   (grad.dim() == 4 && grad.size(2) == heads && grad.size(3) % 3 == 0),
               "glm_rotary_qkv_bwd: gradient [b, s, g, a/g + 2, d] or [b, s, a, 3d] expected, got ", grad.sizes());
+  TORCH_CHECK(!(given(pos_base) && given(position_ids)),
+              "glm_rotary_qkv_bwd: position_ids and pos_base exclude each other");
   const int64_t B = grad.size(0), S = grad.size(1), D = grouped ? grad.size(4) : grad.size(3) / 3;
   Args args("glm_rotary_qkv_bwd");
-  const GlmRotary g = glm_rotary_args(args, "grad", grad, B, S, heads, kv_heads, D, table, pos_offset, position_ids);
+  const GlmRotary g = glm_rotary_args(args, "grad", grad, B, S, heads, kv_heads, D, table,
+                                      given(pos_base) ? 0 : pos_offset, position_ids);
+  const int* base = args.opt<const int>("pos_base", pos_base, at::kInt, {kAny});
+  TORCH_CHECK(base == nullptr || pos_base->numel() >= 1, "glm_rotary_qkv_bwd: pos_base must hold at least one element");
   const auto guard = args.guard();
   check_glm_positions("glm_rotary_qkv_bwd", position_ids, table.size(0));
   Tensor dmixed = at::empty({B, S, (heads + 2 * kv_heads) * D}, grad.options());
   check(lb_glm_rotary_qkv(grad.data_ptr(), table.data_ptr<float>(), dmixed.data_ptr(), B * S, g.S, g.A, g.G, g.D,
-                          (int)pos_offset, g.positions, grouped ? 1 : 0, 1, cur_stream()),
+                          (int)pos_offset, g.positions, base, grouped ? 1 : 0, 1, cur_stream()),
         "glm_rotary_qkv_bwd");
   return dmixed;
 }
@@ -1314,8 +1328,8 @@ TORCH_LIBRARY(libai_b200, m) {
   m.def("swiglu_packed_bwd(Tensor gy, Tensor gu) -> Tensor", &swiglu_packed_bwd);
   m.def("dgrad_actgrad(Tensor gy, Tensor w, Tensor pre, int act, Tensor(a!)? bias_grad=None) -> Tensor", &dgrad_actgrad);
   m.def("rope_qkv(Tensor(a!) qkv, Tensor cos, Tensor sin, int pos_offset, bool backward, bool inplace, Tensor? positions=None) -> Tensor(a!)", &rope_qkv);
-  m.def("glm_rotary_qkv(Tensor mixed, int heads, int kv_heads, Tensor table, int pos_offset, Tensor? position_ids, bool grouped) -> Tensor", &glm_rotary_qkv);
-  m.def("glm_rotary_qkv_bwd(Tensor grad, int heads, int kv_heads, Tensor table, int pos_offset, Tensor? position_ids) -> Tensor", &glm_rotary_qkv_bwd);
+  m.def("glm_rotary_qkv(Tensor mixed, int heads, int kv_heads, Tensor table, int pos_offset, Tensor? position_ids, bool grouped, Tensor? pos_base=None) -> Tensor", &glm_rotary_qkv);
+  m.def("glm_rotary_qkv_bwd(Tensor grad, int heads, int kv_heads, Tensor table, int pos_offset, Tensor? position_ids, Tensor? pos_base=None) -> Tensor", &glm_rotary_qkv_bwd);
   m.def("ce_stats(Tensor logits, Tensor labels, int vocab_start) -> (Tensor, Tensor, Tensor)", &ce_stats);
   m.def("ce_bwd(Tensor(a!) logits, Tensor labels, Tensor lse, Tensor gloss, int vocab_start) -> Tensor(a!)", &ce_bwd);
   m.def("fused_adamw(Tensor(a!) master, Tensor grad, Tensor(b!) m, Tensor(c!) v, Tensor? lp_out, Tensor scale, float lr, float b1, float b2, float eps, float wd, float bc1, float bc2, bool decoupled) -> ()", &fused_adamw);

@@ -236,18 +236,23 @@ __global__ void rope_qkv_kernel(const __nv_bfloat16* __restrict__ x, const float
 //   per-head [tokens, A, 3, D]      (per query head [q_h | k_{h/r} | v_{h/r}]: K/V repeated r times)
 // The first D/2 channels of every q and k head rotate in interleaved pairs (2p, 2p + 1) by table[pos, p] = (cos, sin)
 // (fp32 [npos, D/4, 2]); the other channels and v are copied.  pos = positions[i] (int32, the sequence index i of the
-// token; one row shared by the batch) or i + pos_offset.  Every product is rounded on its own (no FMA contraction), so
-// the forward is bit-identical to the fp32 reference x0·c − x1·s, x1·c + x0·s rounded once to bf16.
+// token; one row shared by the batch), or i + pos_offset (+ pos_base[0] when given: an offset read on the device, so a
+// CUDA graph of a decoding step replays at the cache's current length).  Every product is rounded on its own (no FMA
+// contraction), so the forward is bit-identical to the fp32 reference x0·c − x1·s, x1·c + x0·s rounded once to
+// bf16.
 // One thread per output channel pair (D % 4 == 0, so a pair never straddles the rotated half).
-LB_DEVICE int glm_position(size_t token, int S, int pos_offset, const int* __restrict__ positions) {
+LB_DEVICE int glm_position(size_t token, int S, int pos_offset, const int* __restrict__ positions,
+                           const int* __restrict__ pos_base) {
   const int i = static_cast<int>(token % S);
-  return positions != nullptr ? positions[i] : i + pos_offset;
+  if (positions != nullptr) return positions[i];
+  return i + pos_offset + (pos_base != nullptr ? *pos_base : 0);
 }
 
 // forward: one pass over the packed output
 __global__ void glm_rotary_pack_kernel(const __nv_bfloat16* __restrict__ x, const float* __restrict__ table,
                                        __nv_bfloat16* __restrict__ y, size_t tokens, int S, int A, int G, int D,
-                                       int pos_offset, const int* __restrict__ positions, int grouped) {
+                                       int pos_offset, const int* __restrict__ positions,
+                                       const int* __restrict__ pos_base, int grouped) {
   const int pairs = D / 2, r = A / G;
   const int slots = grouped ? G * (r + 2) : 3 * A;   // D-wide rows per token in the output
   const size_t total = tokens * slots * pairs;
@@ -268,8 +273,8 @@ __global__ void glm_rotary_pack_kernel(const __nv_bfloat16* __restrict__ x, cons
         *reinterpret_cast<const __nv_bfloat162*>(x + token * in_row + static_cast<size_t>(col) * D + 2 * p);
     __nv_bfloat162 out = v2;
     if (col < A + G && 2 * p < D / 2) {
-      const float2 cs = reinterpret_cast<const float2*>(table)[static_cast<size_t>(glm_position(token, S, pos_offset,
-                                                                                                positions)) * (D / 4) + p];
+      const int pos = glm_position(token, S, pos_offset, positions, pos_base);
+      const float2 cs = reinterpret_cast<const float2*>(table)[static_cast<size_t>(pos) * (D / 4) + p];
       const float x0 = __low2float(v2), x1 = __high2float(v2);
       const float y0 = __fsub_rn(__fmul_rn(x0, cs.x), __fmul_rn(x1, cs.y));
       const float y1 = __fadd_rn(__fmul_rn(x1, cs.x), __fmul_rn(x0, cs.y));
@@ -284,7 +289,8 @@ __global__ void glm_rotary_pack_kernel(const __nv_bfloat16* __restrict__ x, cons
 // result is rounded once.  Every element of dx is written exactly once.
 __global__ void glm_rotary_unpack_kernel(const __nv_bfloat16* __restrict__ dy, const float* __restrict__ table,
                                          __nv_bfloat16* __restrict__ dx, size_t tokens, int S, int A, int G, int D,
-                                         int pos_offset, const int* __restrict__ positions, int grouped) {
+                                         int pos_offset, const int* __restrict__ positions,
+                                         const int* __restrict__ pos_base, int grouped) {
   const int pairs = D / 2, r = A / G;
   const int cols = A + 2 * G;
   const size_t total = tokens * cols * pairs;
@@ -319,8 +325,8 @@ __global__ void glm_rotary_unpack_kernel(const __nv_bfloat16* __restrict__ dy, c
       }
     }
     if (col < A + G && 2 * p < D / 2) {
-      const float2 cs = reinterpret_cast<const float2*>(table)[static_cast<size_t>(glm_position(token, S, pos_offset,
-                                                                                                positions)) * (D / 4) + p];
+      const int pos = glm_position(token, S, pos_offset, positions, pos_base);
+      const float2 cs = reinterpret_cast<const float2*>(table)[static_cast<size_t>(pos) * (D / 4) + p];
       const float d0 = __fadd_rn(__fmul_rn(g0, cs.x), __fmul_rn(g1, cs.y));
       const float d1 = __fsub_rn(__fmul_rn(g1, cs.x), __fmul_rn(g0, cs.y));
       g0 = d0;
@@ -730,21 +736,24 @@ extern "C" int lb_rope_qkv(const void* x, const float* cosv, const float* sinv, 
 }
 // forward (backward = 0): in = the fused projection [tokens, (A + 2G) * D], out = the packed layout (grouped [tokens, G,
 // A / G + 2, D] or per-head [tokens, A, 3D]); backward: in = the gradient of the packed layout, out = that of the fused
-// projection.  table fp32 [npos, D / 4, 2]; positions (optional, int32 [S]) replaces i + pos_offset.  The caller keeps
-// every position in [0, npos).
+// projection.  table fp32 [npos, D / 4, 2]; positions (optional, int32 [S]) replaces i + pos_offset; pos_base
+// (optional, int32) adds its first element to i + pos_offset.  The caller keeps every position in
+// [0, npos).
 extern "C" int lb_glm_rotary_qkv(const void* in, const float* table, void* out, long tokens, int S, int A, int G, int D,
-                                 int pos_offset, const int* positions, int grouped, int backward, cudaStream_t s) {
+                                 int pos_offset, const int* positions, const int* pos_base, int grouped, int backward,
+                                 cudaStream_t s) {
   if (G <= 0 || A % G || D % 4 || S <= 0) return -1;
   if (tokens == 0) return 0;
   if (!backward) {
     const size_t pairs = (size_t)tokens * (grouped ? (A / G + 2) * G : 3 * A) * (D / 2);
     lb::glm_rotary_pack_kernel<<<ew_grid(pairs, 256), 256, 0, s>>>((const bf16*)in, table, (bf16*)out, (size_t)tokens,
-                                                                    S, A, G, D, pos_offset, positions, grouped);
+                                                                    S, A, G, D, pos_offset, positions, pos_base,
+                                                                    grouped);
   } else {
     const size_t pairs = (size_t)tokens * (A + 2 * G) * (D / 2);
     lb::glm_rotary_unpack_kernel<<<ew_grid(pairs, 256), 256, 0, s>>>((const bf16*)in, table, (bf16*)out,
                                                                       (size_t)tokens, S, A, G, D, pos_offset, positions,
-                                                                      grouped);
+                                                                      pos_base, grouped);
   }
   return (int)cudaGetLastError();
 }

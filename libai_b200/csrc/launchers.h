@@ -85,9 +85,11 @@ int lb_rope_qkv(const void* x, const float* cosv, const float* sinv, void* y, lo
                 int pos_offset, const int* positions, int npos, int backward, cudaStream_t s);
 // ChatGLM rotary between the fused projection [tokens, (A + 2G) * D] and a packed layout (grouped [tokens, G, A/G + 2,
 // D] or per-head [tokens, A, 3D]): forward packs (in = fused, out = packed), backward unpacks the gradient (in =
-// packed, out = fused); table fp32 [npos, D/4, 2], positions optional int32 [S]
+// packed, out = fused); table fp32 [npos, D/4, 2], positions optional int32 [S], pos_base optional int32 (its first
+// element is added to i + pos_offset on the device)
 int lb_glm_rotary_qkv(const void* in, const float* table, void* out, long tokens, int S, int A, int G, int D,
-                      int pos_offset, const int* positions, int grouped, int backward, cudaStream_t s);
+                      int pos_offset, const int* positions, const int* pos_base, int grouped, int backward,
+                      cudaStream_t s);
 int lb_colsum_workspace_rows(int M, int N);
 int lb_colsum(const void* x, float* out, int M, int N, int accumulate, float* workspace, cudaStream_t s);
 int lb_embedding_fwd(const int64_t* ids, const void* table, void* out, long T, int H, long vocab_start, long rows, cudaStream_t s);

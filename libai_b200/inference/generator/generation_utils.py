@@ -22,6 +22,7 @@ import torch
 from libai_b200.utils import distributed as dutil
 import torch.distributed as dist
 
+from .. import decode_graph
 from ..kv_cache import KVCacheOwner, StaticKVCache
 from .generation_beam_search import BeamScorer, BeamSearchScorer
 from .generation_logits_processor import (
@@ -58,7 +59,7 @@ _DEFAULTS = dict(
     num_return_sequences=1, output_scores=False, use_cache=True, bos_token_id=None, eos_token_id=None,
     pad_token_id=None, decoder_start_token_id=None, forced_bos_token_id=None, forced_eos_token_id=None,
     remove_invalid_values=False, exponential_decay_length_penalty=None, chunk_size_feed_forward=0,
-    kv_cache_dtype=None,
+    kv_cache_dtype=None, decode_graphs=False,
 )
 
 
@@ -69,6 +70,13 @@ def _kv_cache_dtype(value):
     if isinstance(value, str) and value.lower() == "fp8":
         return torch.float8_e4m3fn
     raise ValueError(f"kv_cache_dtype must be None, 'fp8' or torch.float8_e4m3fn, got {value!r}")
+
+
+def _decode_graphs(value) -> bool:
+    """``generate(decode_graphs=...)``: a bool."""
+    if not isinstance(value, bool):
+        raise ValueError(f"decode_graphs must be True or False, got {value!r}")
+    return value
 
 
 class Generator:
@@ -361,6 +369,17 @@ class Generator:
         inputs = self.prepare_inputs_for_generation(input_ids, **model_kwargs)
         return inputs
 
+    # the decode graphs of the running generate() call (decode_graph.DecodeCall), None when its steps run eagerly
+    _decode_graphs = None
+
+    def _decode_step(self, input_ids, model_kwargs):
+        """One step of the model: replayed from a CUDA graph when ``generate(decode_graphs=True)`` asked for it and the
+        step is eligible (:mod:`libai_b200.inference.decode_graph`), else eager."""
+        inputs = self._model_inputs(input_ids, model_kwargs)
+        if self._decode_graphs is not None:
+            return decode_graph.step(self, inputs, self._decode_graphs)
+        return self(**inputs)
+
     @torch.no_grad()
     def greedy_search(self, input_ids, logits_processor=None, stopping_criteria=None, max_length=None,
                       pad_token_id=None, eos_token_id=None, is_encoder_decoder=False, output_scores=False,
@@ -375,7 +394,7 @@ class Generator:
         scores = () if output_scores else None
         unfinished = torch.ones(input_ids.shape[0], dtype=torch.long, device=input_ids.device)
         while True:
-            outputs = self(**self._model_inputs(input_ids, model_kwargs))
+            outputs = self._decode_step(input_ids, model_kwargs)
             next_scores = logits_processor(input_ids, self._step_logits(outputs))
             if output_scores:
                 scores += (next_scores,)
@@ -408,7 +427,7 @@ class Generator:
         scores = () if output_scores else None
         unfinished = torch.ones(input_ids.shape[0], dtype=torch.long, device=input_ids.device)
         while True:
-            outputs = self(**self._model_inputs(input_ids, model_kwargs))
+            outputs = self._decode_step(input_ids, model_kwargs)
             next_scores = logits_warper(input_ids, logits_processor(input_ids, self._step_logits(outputs)))
             if output_scores:
                 scores += (next_scores,)
@@ -450,7 +469,7 @@ class Generator:
         beam_scores[:, 1:] = -1e9  # all beams start identical: only the first one may spawn continuations
         beam_scores = beam_scores.view(-1)
         while True:
-            outputs = self(**self._model_inputs(input_ids, model_kwargs))
+            outputs = self._decode_step(input_ids, model_kwargs)
             logprobs = torch.log_softmax(self._step_logits(outputs), dim=-1)
             processed = logits_processor(input_ids, logprobs)
             next_scores = processed + beam_scores[:, None]
@@ -493,16 +512,26 @@ class Generator:
                  num_beam_groups=None, diversity_penalty=None, prefix_allowed_tokens_fn=None, logits_processor=None,
                  renormalize_logits=None, stopping_criteria=None, constraints=None, output_scores=None,
                  forced_bos_token_id=None, forced_eos_token_id=None, remove_invalid_values=None,
-                 exponential_decay_length_penalty=None, kv_cache_dtype=None, **model_kwargs):
+                 exponential_decay_length_penalty=None, kv_cache_dtype=None, decode_graphs=None, **model_kwargs):
         """``kv_cache_dtype`` (default: the model cfg's ``kv_cache_dtype``): ``"fp8"`` or ``torch.float8_e4m3fn`` holds
         the preallocated KV cache as E4M3 rows with per-row scales
         (:class:`~libai_b200.inference.kv_cache.StaticKVCache`) for this call: about half the memory, and of the bytes
         each decoding step reads, for 8-bit keys and values.
-        None keeps the weights' dtype.  A model that does not decode on a ``StaticKVCache`` raises ``ValueError``."""
+        None keeps the weights' dtype.  A model that does not decode on a ``StaticKVCache`` raises ``ValueError``.
+
+        ``decode_graphs`` (default: the model cfg's ``decode_graphs``, else False): True replays the cached decode steps
+        from a CUDA graph, one graph launch per step (:mod:`libai_b200.inference.decode_graph`), with the tokens of
+        eager decoding.  The first decode step of a new batch or cache runs eagerly and the next is captured; the
+        graph holds a private memory pool while the cache lives, and Python hooks on modules do not run in a replayed
+        step.  Steps the graph cannot reproduce run eagerly (logged once per reason).  A model that does not decode on
+        a ``StaticKVCache`` raises ``ValueError``."""
         kv_cache_dtype = _kv_cache_dtype(self._pick(kv_cache_dtype, "kv_cache_dtype"))
         if kv_cache_dtype is not None and not isinstance(self, KVCacheOwner):
             raise ValueError(f"kv_cache_dtype={kv_cache_dtype}: {type(self).__name__} does not decode on a "
                              "StaticKVCache")
+        decode_graphs = _decode_graphs(self._pick(decode_graphs, "decode_graphs"))
+        if decode_graphs and not isinstance(self, KVCacheOwner):
+            raise ValueError(f"decode_graphs=True: {type(self).__name__} does not decode on a StaticKVCache")
         self._validate_model_kwargs(model_kwargs.copy())
         logits_processor = logits_processor if logits_processor is not None else LogitsProcessorList()
         stopping_criteria = stopping_criteria if stopping_criteria is not None else StoppingCriteriaList()
@@ -586,6 +615,8 @@ class Generator:
         try:
             if kv_cache_dtype is not None:   # the cache format of this call (allocate_kv_cache reads it)
                 self.kv_cache_dtype = kv_cache_dtype
+            if decode_graphs:
+                self._decode_graphs = decode_graph.DecodeCall()
             # models with a preallocated cache size it once for every sequence the search runs
             allocate = getattr(self, "allocate_kv_cache", None)
             if allocate is not None and model_kwargs.get("use_cache") and stopping_criteria.max_length is not None:
@@ -626,3 +657,5 @@ class Generator:
             self.train(was_training)
             if kv_cache_dtype is not None:
                 self.kv_cache_dtype = saved_kv_cache_dtype
+            if decode_graphs:
+                del self._decode_graphs   # back to the class's None

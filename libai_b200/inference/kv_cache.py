@@ -328,7 +328,8 @@ class KVCacheOwner:
     kv_cache: Optional[StaticKVCache] = None
     past_length = 0
     kv_cache_dtype = None   # what the cache holds: None = the weights' dtype; torch.float8_e4m3fn = FP8 rows
-
+    # the rows a step may reach (the last _prepare_cache's max_positions): a replayed decode graph checks it instead
+    max_cache_positions: Optional[int] = None
 
     def _cache_attention_modules(self) -> list:
         raise NotImplementedError
@@ -352,6 +353,7 @@ class KVCacheOwner:
             heads = getattr(mods[0], "local_kv_heads", mods[0].local_heads)
             c = StaticKVCache(len(mods), batch, heads, mods[0].head_size, max_length, dtype, w.device, owned,
                               self.kv_cache_dtype)
+            self._decode_graph = None   # a decode graph of the old cache (and its memory pool) goes with it
         c.reset()
         self.kv_cache, self.past_length = c, 0
         return c
@@ -362,6 +364,7 @@ class KVCacheOwner:
         c = self.kv_cache
         if c is None or (c.length == 0 and c.batch != bsz):
             c = self.allocate_kv_cache(bsz, s_len)
+        self.max_cache_positions = max_positions
         if max_positions is not None and c.length + s_len > max_positions:
             raise ValueError(f"The maximum supported length is {max_positions}, "
                              f"and the current length is {c.length + s_len}.")

@@ -61,9 +61,12 @@ class GPTEmbedding(nn.Module):
         self.dropout = Dropout(embedding_dropout_prob)
         self.max_seq_length = max_seq_length
 
-    def forward(self, input_ids, past_length=0):
+    def forward(self, input_ids, past_length=0, position_ids=None):
+        """``position_ids`` (int64 ``[s]``, shared by the batch): the positions of the tokens, by default
+        ``past_length + i``; a cached step derives them from its cache's lengths on the device."""
         bsz, seq_length = input_ids.shape
-        position_ids = torch.arange(past_length, past_length + seq_length, device=input_ids.device)
+        if position_ids is None:
+            position_ids = torch.arange(past_length, past_length + seq_length, device=input_ids.device)
         token_embeds = self.token_embeddings(input_ids)
         position_embeds = self.position_embeddings(position_ids)
         x = self.dropout(token_embeds + position_embeds.unsqueeze(0))

@@ -1236,13 +1236,16 @@ def apply_glm_rotary(x: torch.Tensor, table: torch.Tensor) -> torch.Tensor:
 
 
 def apply_glm_rotary_qkv_ref(mixed, *, heads: int, kv_heads: int, table, pos_offset: int = 0, position_ids=None,
-                             grouped: bool = False):
+                             grouped: bool = False, pos_base=None):
     """:func:`apply_glm_rotary_qkv` in PyTorch: :func:`apply_glm_rotary` on q and k, then stacked (and, per-head,
     repeated) into the packed layout."""
     b, s, _ = mixed.shape
     a, g = heads, kv_heads
     d = mixed.shape[-1] // (a + 2 * g)
-    rope = table[position_ids[0].long()] if position_ids is not None else table[pos_offset : pos_offset + s]
+    if pos_base is not None:
+        rope = table[pos_base[0].long() + pos_offset + torch.arange(s, device=table.device)]
+    else:
+        rope = table[position_ids[0].long()] if position_ids is not None else table[pos_offset : pos_offset + s]
     q, k, v = mixed.split([a * d, g * d, g * d], dim=-1)
     q = apply_glm_rotary(q.view(b, s, a, d), rope)
     k = apply_glm_rotary(k.view(b, s, g, d), rope)
@@ -1257,39 +1260,44 @@ class _GlmRotaryQKVFn(torch.autograd.Function):
     rotates back in one pass."""
 
     @staticmethod
-    def forward(ctx, mixed, heads, kv_heads, table, pos_offset, position_ids, grouped):
+    def forward(ctx, mixed, heads, kv_heads, table, pos_offset, position_ids, grouped, pos_base):
         ext = load_ext()
-        ctx.save_for_backward(table, position_ids)
+        ctx.save_for_backward(table, position_ids, pos_base)
         ctx.geom = (heads, kv_heads, pos_offset)
         count_launch()
-        return ext.glm_rotary_qkv(mixed, heads, kv_heads, table, pos_offset, position_ids, grouped)
+        return ext.glm_rotary_qkv(mixed, heads, kv_heads, table, pos_offset, position_ids, grouped, pos_base)
 
     @staticmethod
     def backward(ctx, g):
         ext = load_ext()
-        table, position_ids = ctx.saved_tensors
+        table, position_ids, pos_base = ctx.saved_tensors
         heads, kv_heads, pos_offset = ctx.geom
         count_launch()
-        dmixed = ext.glm_rotary_qkv_bwd(g.contiguous(), heads, kv_heads, table, pos_offset, position_ids)
-        return dmixed, None, None, None, None, None, None
+        dmixed = ext.glm_rotary_qkv_bwd(g.contiguous(), heads, kv_heads, table, pos_offset, position_ids, pos_base)
+        return dmixed, None, None, None, None, None, None, None
 
 
 def apply_glm_rotary_qkv(mixed, *, heads: int, kv_heads: int, table, pos_offset: int = 0, position_ids=None,
-                         grouped: bool = False):
+                         grouped: bool = False, pos_base=None):
     """ChatGLM's fused projection ``mixed`` ``[b, s, (a + 2g)·d]`` (all ``a`` q heads, then the ``g`` k heads, then the
     ``g`` v heads) → the packed layout the attention kernels read, q and k rotated by the GLM rotary (:func:`apply_glm_rotary`
     with the fp32 ``table`` ``[P, d/4, 2]`` of :func:`glm_rope_table`): per-head ``[b, s, a, 3d]`` (query head ``h``
     with copies of K/V group ``h // (a // g)``, for :func:`attention_qkvpacked`), or with ``grouped`` ``[b, s, g, a/g + 2,
     d]`` (for :func:`kv_cache_append`).  Token ``i`` sits at position ``pos_offset + i``, or ``position_ids[0, i]``
     (``[b, s]``; the first row serves the whole batch) when given.  The native kernel's forward is bit-identical to
-    :func:`apply_glm_rotary_qkv_ref`; its backward sums the K/V copies in fp32 and rounds once."""
+    :func:`apply_glm_rotary_qkv_ref`; its backward sums the K/V copies in fp32 and rounds once.
+    ``pos_base`` (int32 ``[>= 1]``, not with ``position_ids``): token ``i`` sits at ``pos_base[0] + pos_offset + i``,
+    read on the device, forward and backward.  A cached step passes its cache's lengths, so that the step holds no
+    host-side position and a CUDA graph of it replays at the cache's current length."""
+    if pos_base is not None and position_ids is not None:
+        raise ValueError("position_ids and pos_base exclude each other")
     if use_native(mixed) and mixed.dtype == torch.bfloat16 and table.dtype == torch.float32:
         if position_ids is not None:
             position_ids = position_ids.to(device=mixed.device, dtype=torch.int32).contiguous()
         return _GlmRotaryQKVFn.apply(mixed.contiguous(), int(heads), int(kv_heads), table.contiguous(), int(pos_offset),
-                                     position_ids, bool(grouped))
+                                     position_ids, bool(grouped), pos_base)
     return apply_glm_rotary_qkv_ref(mixed, heads=heads, kv_heads=kv_heads, table=table, pos_offset=pos_offset,
-                                    position_ids=position_ids, grouped=grouped)
+                                    position_ids=position_ids, grouped=grouped, pos_base=pos_base)
 
 
 # --------------------------------------------------------------------------------------

@@ -52,7 +52,9 @@ apply_rotary_pos_emb = OF.apply_glm_rotary   # x ``[b, s, heads, d]`` rotated by
 class AttentionInputs(NamedTuple):
     """What every layer's attention takes besides its hidden states, decided once per forward: the rotary table and
     positions of the new tokens, and how keys are masked — ``mask`` (a dense ``[b, 1, q, k]`` visibility for the
-    reference math), ``kv_lens`` (right padding) or ``kv_start`` (left padding), none of them for plain causal."""
+    reference math), ``kv_lens`` (right padding) or ``kv_start`` (left padding), none of them for plain causal.
+    ``pos_base`` (int32 device tensor): the new tokens sit at ``pos_base[0] + pos_offset + i`` (a cached step reads its
+    positions from the cache's lengths)."""
 
     table: torch.Tensor
     pos_offset: int = 0
@@ -60,6 +62,7 @@ class AttentionInputs(NamedTuple):
     mask: Optional[torch.Tensor] = None
     kv_lens: Optional[torch.Tensor] = None
     kv_start: Optional[torch.Tensor] = None
+    pos_base: Optional[torch.Tensor] = None
 
 
 class RotaryEmbedding(nn.Module):
@@ -118,7 +121,7 @@ class SelfAttention(nn.Module):
         mixed = self.query_key_value(hidden)
         if isinstance(kv_cache, KVCacheLayer):   # GLM rotary into the grouped layout the cache appends from
             qkv = OF.apply_glm_rotary_qkv(mixed, heads=a, kv_heads=g, table=inputs.table, pos_offset=inputs.pos_offset,
-                                          position_ids=inputs.position_ids, grouped=True)
+                                          position_ids=inputs.position_ids, grouped=True, pos_base=inputs.pos_base)
             ctx = kv_cache.attend(kv_cache.append(qkv), scale=1.0 / math.sqrt(d), mask=inputs.mask)
             return self.dense(ctx.reshape(b, s, a * d))
         # per-head [b, s, a, 3d]: every query head with its own copy of its group's K/V (multi-query attention)
@@ -278,8 +281,11 @@ class ChatGLMModel(nn.Module, ChatGLMPreTrainedModel):
                         cache.write_rows(i, k, v)
                 cache.advance(pre)
             past = cache.length
-            inputs = AttentionInputs(self._rope, past - pre, position_ids,
-                                     mask=self.get_masks(input_ids, past, attention_mask) if dense else None)
+            # the default positions continue from the cache: seqlens (every sample's rows, the prefix's included)
+            # minus the prefix, read on the device
+            inputs = AttentionInputs(self._rope, -pre, position_ids,
+                                     mask=self.get_masks(input_ids, past, attention_mask) if dense else None,
+                                     pos_base=cache.seqlens if position_ids is None else None)
             hidden = self.encoder(hidden, inputs, kv_caches=[cache.layer(i) for i in range(self.num_layers)])
             cache.advance(q)
             return hidden

@@ -241,8 +241,8 @@ class GLMModel(nn.Module):
         b, q = input_ids.shape
         mem_len = memory_states[0].shape[1] if memory_states is not None else 0
         past = kv_cache.length if kv_cache is not None else mem_len
-        if attention_mask is None:
-            attention_mask = torch.tensor(q, device=input_ids.device)
+        if attention_mask is None:   # (a fill on the device: a cached step copies nothing from the host)
+            attention_mask = torch.full((), q, dtype=torch.long, device=input_ids.device)
         hidden = self.embeddings(input_ids, position_ids)
         # the prefix-LM rule where the kernels run: every uncached call, and the prefill of a cache (a later step
         # sees every cached row, unless the prefill needed the dense mask)

@@ -38,13 +38,15 @@ class AdapterAttention(LlamaAttention):
         bsz = hidden_states.shape[0]
         # queries need the same rotary phase as in the main path
         qkv = self.query_key_value(hidden_states).view(bsz, -1, a, 3 * d)
-        if past_key_value is None:
-            past_len = 0
-        elif isinstance(past_key_value, KVCacheLayer):
-            past_len = past_key_value.length   # rows before this step: the lengths advance after the last layer
-        else:
+        past_len, positions = 0, None
+        if isinstance(past_key_value, KVCacheLayer):
+            # the cache's rows before this step (the lengths advance after the last layer), read on the device: a
+            # cached step holds no host-side position, so a CUDA graph of it replays at the current length
+            s = hidden_states.shape[1]
+            positions = past_key_value.seqlens[:, None] + torch.arange(s, dtype=torch.int32, device=qkv.device)
+        elif past_key_value is not None:
             past_len = past_key_value[0].shape[2]
-        q = OF.apply_rotary_qkv(qkv, cos_cached, sin_cached, past_len)[..., :d].permute(0, 2, 1, 3)
+        q = OF.apply_rotary_qkv(qkv, cos_cached, sin_cached, past_len, positions)[..., :d].permute(0, 2, 1, 3)
         akv = self.query_key_value(self.adapter.to(hidden_states.dtype)).view(1, -1, a, 3 * d).permute(0, 2, 1, 3)
         ak, av = akv[..., d : 2 * d], akv[..., 2 * d :]
         scores = torch.matmul(q.float(), ak.float().transpose(-1, -2)) * self.norm_factor

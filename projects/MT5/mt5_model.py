@@ -482,6 +482,7 @@ class MT5Model(nn.Module, Generator, KVCacheOwner):
                 or c.capacity < S):
             c = StaticKVCache(len(self.decoder.layers), b, a, d, S, encoder_states.dtype, encoder_states.device,
                               kv_dtype=kv_dtype)
+            self._decode_graph = None   # a decode graph of the old cross cache (and its memory pool) goes with it
         kv = (layer.cross_attention.key_value(encoder_states).view(b, S, a, 2 * d).transpose(1, 2).split(d, dim=-1)
               for layer in self.decoder.layers)
         c.fill(kv, S, window)

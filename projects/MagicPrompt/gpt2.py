@@ -1,5 +1,6 @@
 """GPT-2 with a KV cache and ``generate`` (reference projects/MagicPrompt/gpt2.py: the library GPT-2 extended with
 ``past_key_values`` / ``use_cache`` and the ``Generator`` mixin for prompt completion)."""
+import torch
 from torch import nn
 
 from libai_b200.config import configurable
@@ -27,8 +28,10 @@ class GPTModel(core.GPTModel, Generator, KVCacheOwner):
         if not use_cache and self.training:
             return {"logits": super().forward(input_ids)}
         cache = self._prepare_cache(input_ids) if use_cache else None
-        past_len = cache.length if use_cache else 0
-        hidden = self.embeddings(input_ids, past_len)
+        # a cached step reads its positions from the cache's lengths on the device (every sample holds as many rows)
+        positions = cache.seqlens[:1].long() + torch.arange(input_ids.shape[1], device=input_ids.device) \
+            if use_cache else None
+        hidden = self.embeddings(input_ids, position_ids=positions)
         for i, layer in enumerate(self.transformer.layers):
             # causal prefill, then decoding steps over the cache (every cached token is visible)
             hidden = layer(hidden, None, past_key_value=cache.layer(i) if use_cache else None)
