@@ -68,6 +68,7 @@ const char* dtype_name(at::ScalarType t) {
     case at::kInt: return "int32";
     case at::kLong: return "int64";
     case at::kFloat8_e4m3fn: return "float8_e4m3fn";
+    case at::kByte: return "uint8";
     default: return c10::toString(t);
   }
 }
@@ -294,6 +295,54 @@ Tensor dequant_e4m3_rows(const Tensor& w, const Tensor& w_scale) {
   check(lb_dequant_e4m3_rows(w.data_ptr(), w_scale.data_ptr<float>(), out.data_ptr(), (long)w.size(0), (int)w.size(1),
                              cur_stream()),
         "dequant_e4m3_rows");
+  return out;
+}
+
+// Group-wise INT4 weights: w uint8 [N, K/2] (two 4-bit values per byte, 16-byte aligned), w_scale bf16 and w_zero uint8
+// [N, K/128], K % 128 == 0; returns (N, K)
+std::pair<int64_t, int64_t> int4_weight_args(Args& args, const Tensor& w, const Tensor& w_scale, const Tensor& w_zero) {
+  args("w", w, at::kByte, {kAny, kAny}, Layout::Contiguous, 16);
+  const int64_t N = w.size(0), K = 2 * w.size(1);
+  TORCH_CHECK(N >= 1 && K >= 128 && K % 128 == 0, args.op(), ": w [N, K/2] needs K a positive multiple of 128, got ",
+              w.sizes());
+  TORCH_CHECK(N <= INT32_MAX && K <= INT32_MAX, args.op(), ": N and K must fit in int32");
+  args("w_scale", w_scale, at::kBFloat16, {N, K / 128});
+  args("w_zero", w_zero, at::kByte, {N, K / 128});
+  return {N, K};
+}
+
+// y [M, N] = act(x [M, K] · Ŵᵀ + bias), Ŵ = bf16_rn((q − w_zero) · w_scale) per group of 128 columns: the
+// weight-streaming kernel for 1 <= M <= 64 (x bf16 contiguous and 16-byte aligned, bias bf16 [N] or None, act one of
+// the ACT_* ids without the residual add)
+Tensor linear_int4w(const Tensor& x, const Tensor& w, const Tensor& w_scale, const Tensor& w_zero,
+                    const c10::optional<Tensor>& bias, int64_t act) {
+  Args args("linear_int4w");
+  args("x", x, at::kBFloat16, {kAny, kAny}, Layout::Contiguous, 16);
+  const auto [N, K] = int4_weight_args(args, w, w_scale, w_zero);
+  const int64_t M = x.size(0);
+  TORCH_CHECK(x.size(1) == K, "linear_int4w: x [M, K] and w [N, K/2] disagree on K: ", x.sizes(), " vs ", w.sizes());
+  TORCH_CHECK(M >= 1 && M <= 64, "linear_int4w: 1 <= M <= 64 rows, got ", M);
+  TORCH_CHECK(act >= 0 && act <= 5, "linear_int4w: act must be an activation id in [0, 5], got ", act);
+  const void* bias_ptr = args.opt("bias", bias, at::kBFloat16, {N});
+  const auto guard = args.guard();
+  Tensor y = at::empty({M, N}, x.options());
+  const long ws = lb_linear_int4w_workspace((int)M, (int)N, (int)K);
+  Tensor part = ws > 0 ? at::empty({ws}, x.options().dtype(at::kFloat)) : Tensor();
+  check(lb_linear_int4w(x.data_ptr(), w.data_ptr(), w_scale.data_ptr(), w_zero.data_ptr(), bias_ptr, y.data_ptr(),
+                        ws > 0 ? part.data_ptr<float>() : nullptr, (int)M, (int)N, (int)K, (int)act, cur_stream()),
+        "linear_int4w");
+  return y;
+}
+
+// bf16 [N, K] = Ŵ (the weight the prefill GEMM of an INT4 linear multiplies)
+Tensor dequant_int4_rows(const Tensor& w, const Tensor& w_scale, const Tensor& w_zero) {
+  Args args("dequant_int4_rows");
+  const auto [N, K] = int4_weight_args(args, w, w_scale, w_zero);
+  const auto guard = args.guard();
+  Tensor out = at::empty({N, K}, w.options().dtype(at::kBFloat16));
+  check(lb_dequant_int4_rows(w.data_ptr(), w_scale.data_ptr(), w_zero.data_ptr(), out.data_ptr(), (long)N, (int)K,
+                             cur_stream()),
+        "dequant_int4_rows");
   return out;
 }
 
@@ -1314,6 +1363,9 @@ TORCH_LIBRARY(libai_b200, m) {
   m.def("quantize_e4m3(Tensor x) -> (Tensor, Tensor)", &quantize_e4m3);
   m.def("linear_fp8w(Tensor x, Tensor w, Tensor w_scale, Tensor? bias, int act) -> Tensor", &linear_fp8w);
   m.def("dequant_e4m3_rows(Tensor w, Tensor w_scale) -> Tensor", &dequant_e4m3_rows);
+  m.def("linear_int4w(Tensor x, Tensor w, Tensor w_scale, Tensor w_zero, Tensor? bias, int act) -> Tensor",
+        &linear_int4w);
+  m.def("dequant_int4_rows(Tensor w, Tensor w_scale, Tensor w_zero) -> Tensor", &dequant_int4_rows);
   m.def("linear_fp8_fwd(Tensor xq, Tensor wq, Tensor deq_x, Tensor deq_w, Tensor? bias, int act, bool need_pre, Tensor? residual=None, int bn=0) -> (Tensor, Tensor)", &linear_fp8_fwd);
   m.def("act_bwd(Tensor gy, Tensor pre, int act) -> Tensor", &act_bwd);
   m.def("colsum(Tensor x, Tensor(a!)? accum=None) -> Tensor", &colsum);

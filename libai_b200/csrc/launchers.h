@@ -153,6 +153,16 @@ int lb_linear_fp8w(const void* x, const void* w, const float* w_scale, const voi
                    int N, int K, int act, cudaStream_t s);
 // out [rows, K] bf16 = bf16_rn(float(w [rows, K] E4M3) · scale[row]), K % 16 == 0
 int lb_dequant_e4m3_rows(const void* w, const float* scale, void* out, long rows, int K, cudaStream_t s);
+// y [M, N] bf16 = act(x [M, K] bf16 · Ŵᵀ + bias [N]) with Ŵ[n, k] = bf16_rn((q[n, k] − zero[n, k/128]) · scale[n, k/128]):
+// w uint8 [N, K/2] holds q two per byte (column 2j in the low nibble of byte j), scale bf16 and zero uint8 [N, K/128].
+// 1 <= M <= 64, K % 128 == 0; bias may be null.  part: an fp32 workspace of lb_linear_int4w_workspace(M, N, K) floats
+// (null when that is 0).
+long lb_linear_int4w_workspace(int M, int N, int K);
+int lb_linear_int4w(const void* x, const void* w, const void* w_scale, const void* w_zero, const void* bias, void* y,
+                    float* part, int M, int N, int K, int act, cudaStream_t s);
+// out [rows, K] bf16 = Ŵ of lb_linear_int4w, K % 128 == 0
+int lb_dequant_int4_rows(const void* w, const void* w_scale, const void* w_zero, void* out, long rows, int K,
+                         cudaStream_t s);
 int lb_window_attn_groups(int B, int H, int W, int ws, int heads);
 int lb_window_attn_fwd(const void* qkv, void* out, float* lse, const float* table, const float* tau, int B, int H, int W,
                        int ws, int shift, int heads, int d, float scale, cudaStream_t s);

@@ -11,53 +11,16 @@
 // 16-byte loads of x its B operands.  Every sum runs over the same K positions, in a fixed order.  The loads of the
 // next steps are in flight while the current ones are multiplied.
 //
-// A CTA is 4 warps = 64 weight rows over one K range.  The number of K ranges (splits) is chosen from (N, K) alone, so
-// that about 4 · 132 CTAs are in flight even at N = 4096; with more than one range the fp32 partials go to a workspace
-// and linear_fp8w_combine sums them in range order.  Neither the splits nor any summation order depend on M: a token's
-// output row is the same bits whether it is computed alone or among 63 others.  The per-row scale, the bias and the
-// activation are applied once, to the finished fp32 sum.
-#include "common.cuh"
+// The split policy, the streaming load, the epilogue and the sum over the K ranges are weight_stream.cuh's.  The
+// per-row scale, the bias and the activation are applied once, to the finished fp32 sum.
+#include "weight_stream.cuh"
 
 namespace lb {
 namespace fp8w {
 
-constexpr int kWarps = 4;
-constexpr int kThreads = kWarps * 32;
-constexpr int kRows = kWarps * 16;     // weight rows per CTA
+using namespace wstream;
+
 constexpr int kStep = 64;              // K columns per warp step: 16 bytes of each row per lane of a quad
-constexpr int kMinRange = 256;         // K columns of a range at least
-constexpr int kTargetCtas = 4 * 132;   // CTAs to keep in flight: four per SM of an H100 SXM
-
-struct Split {
-  int splits, range;   // range: K columns per split (a multiple of kStep; the last split may hold fewer)
-};
-
-inline Split split_of(int N, int K) {
-  const int row_blocks = (N + kRows - 1) / kRows;
-  const int max_splits = (K + kMinRange - 1) / kMinRange;
-  const int want = (kTargetCtas + row_blocks - 1) / row_blocks;
-  const int splits = want < 1 ? 1 : (want > max_splits ? max_splits : want);
-  const int range = ((K + splits - 1) / splits + kStep - 1) / kStep * kStep;
-  return {(K + range - 1) / range, range};
-}
-
-// 16 bytes that are read once: no L1 allocation, and the rest of the 256-byte L2 block is prefetched (the next steps
-// of the same rows read it)
-LB_DEVICE uint4 ld_stream(const void* p) {
-  uint4 r;
-  asm("ld.global.nc.L1::no_allocate.L2::256B.v4.u32 {%0, %1, %2, %3}, [%4];\n"
-      : "=r"(r.x), "=r"(r.y), "=r"(r.z), "=r"(r.w)
-      : "l"(p));
-  return r;
-}
-
-LB_DEVICE uint32_t word(const uint4& v, int j) { return j == 0 ? v.x : j == 1 ? v.y : j == 2 ? v.z : v.w; }
-
-LB_DEVICE float epilogue(float acc, int n, const float* scale, const __nv_bfloat16* bias, int act) {
-  float v = acc * scale[n];
-  if (bias != nullptr) v += __bfloat162float(bias[n]);
-  return act_fwd(v, act);
-}
 
 // NT: n8 tiles of tokens (M <= 8 * NT); U: steps whose weight loads are issued together
 template <int NT, int U>
@@ -135,21 +98,10 @@ __global__ void __launch_bounds__(kThreads) linear_fp8w_kernel(const __nv_bfloat
       const int tok = t * 8 + 2 * q + (e & 1), n = row + (e >> 1) * 8;
       if (tok >= M || n >= N) continue;
       if (gridDim.y == 1)
-        y[(long)tok * N + n] = __float2bfloat16(epilogue(acc[t][e], n, scale, bias, act));
+        y[(long)tok * N + n] = __float2bfloat16(epilogue<true>(acc[t][e], n, scale, bias, act));
       else
         part[((long)blockIdx.y * M + tok) * N + n] = acc[t][e];
     }
-}
-
-// y = epilogue(sum over the splits of part [splits, M, N]), summed in split order
-__global__ void linear_fp8w_combine(const float* __restrict__ part, const float* __restrict__ scale,
-                                    const __nv_bfloat16* __restrict__ bias, __nv_bfloat16* __restrict__ y, int MN,
-                                    int N, int splits, int act) {
-  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < MN; i += gridDim.x * blockDim.x) {
-    float s = 0.f;
-    for (int p = 0; p < splits; ++p) s += part[(long)p * MN + i];
-    y[i] = __float2bfloat16(epilogue(s, i % N, scale, bias, act));
-  }
 }
 
 // out [rows, K] bf16 = bf16_rn(float(w) · scale[row]); 16 weight bytes per thread and step
@@ -180,16 +132,13 @@ __global__ void dequant_e4m3_rows(const uint8_t* __restrict__ w, const float* __
 template <int NT, int U>
 cudaError_t launch(const void* x, const void* w, const float* scale, const void* bias, void* y, float* part, int M,
                    int N, int K, int act, cudaStream_t s) {
-  const Split sp = split_of(N, K);
+  const Split sp = split_of(N, K, kStep);
   linear_fp8w_kernel<NT, U><<<dim3((N + kRows - 1) / kRows, sp.splits), kThreads, 0, s>>>(
       static_cast<const __nv_bfloat16*>(x), static_cast<const uint8_t*>(w), scale,
       static_cast<const __nv_bfloat16*>(bias), static_cast<__nv_bfloat16*>(y), part, M, N, K, sp.range, act);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess || sp.splits == 1) return e;
-  const int MN = M * N, blocks = (MN + 255) / 256;
-  linear_fp8w_combine<<<blocks, 256, 0, s>>>(part, scale, static_cast<const __nv_bfloat16*>(bias),
-                                             static_cast<__nv_bfloat16*>(y), MN, N, sp.splits, act);
-  return cudaGetLastError();
+  return launch_combine<true>(part, scale, bias, y, M, N, sp.splits, act, s);
 }
 
 }  // namespace fp8w
@@ -198,7 +147,7 @@ cudaError_t launch(const void* x, const void* w, const float* scale, const void*
 extern "C" {
 
 long lb_linear_fp8w_workspace(int M, int N, int K) {
-  const lb::fp8w::Split sp = lb::fp8w::split_of(N, K);
+  const lb::wstream::Split sp = lb::wstream::split_of(N, K, lb::fp8w::kStep);
   return sp.splits > 1 ? (long)sp.splits * M * N : 0;
 }
 

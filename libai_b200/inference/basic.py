@@ -26,9 +26,11 @@ class BasePipeline(metaclass=ABCMeta):
                  pipeline_stage_id=None, pipeline_num_layers=None, model_path=None, mode="libai", device=None,
                  weight_dtype=None, **kwargs):
         """``weight_dtype``: None keeps the weights as placed; ``"fp8"`` converts the model's linear layers to FP8
-        (E4M3) weights with per-channel scales after placing it (:func:`libai_b200.inference.quantize_weights_fp8_`)."""
-        if weight_dtype not in (None, "fp8"):
-            raise ValueError(f"weight_dtype={weight_dtype!r}: None or 'fp8'")
+        (E4M3) weights with per-channel scales after placing it (:func:`libai_b200.inference.quantize_weights_fp8_`),
+        ``"int4"`` to INT4 weights with a scale and zero point per group of 128 input columns
+        (:func:`libai_b200.inference.quantize_weights_int4_`)."""
+        if weight_dtype not in (None, "fp8", "int4"):
+            raise ValueError(f"weight_dtype={weight_dtype!r}: None, 'fp8' or 'int4'")
         self.cfg = LazyConfig.load(config_file) if isinstance(config_file, (str, Path)) else config_file
         self.update_cfg(data_parallel, tensor_parallel, pipeline_parallel, pipeline_stage_id, pipeline_num_layers)
         self.device = device or ("cuda" if torch.cuda.is_available() else "cpu")
@@ -51,6 +53,10 @@ class BasePipeline(metaclass=ABCMeta):
             from libai_b200.inference import quantize_weights_fp8_
 
             quantize_weights_fp8_(self.model)
+        elif weight_dtype == "int4":
+            from libai_b200.inference import quantize_weights_int4_
+
+            quantize_weights_int4_(self.model)
         self.tokenizer = self.build_tokenizer(self.cfg)
         self._preprocess_params, self._forward_params, self._postprocess_params = self._parse_parameters(**kwargs)
 

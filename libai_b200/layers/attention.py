@@ -174,7 +174,7 @@ class MultiheadAttention(nn.Module):
                     context = context.reshape(-1, a * d)
                 topo = dutil.get_dist_util()
                 if (residual is not None and topo.tensor_parallel_size == 1 and context.dtype == torch.bfloat16
-                        and not getattr(self.dense, "fp8", False) and (self.output_dropout_prob == 0.0 or not self.training)):
+                        and not getattr(self.dense, "quantized", False) and (self.output_dropout_prob == 0.0 or not self.training)):
                     # bias + residual in the epilogue of the output projection
                     return OF.linear_bias_residual(context, self.dense.weight, self.dense.bias, residual)
                 if residual is not None and (self.output_dropout_prob == 0.0 or not self.training):

@@ -16,7 +16,8 @@ On H100 the sequence-parallel pairs run as single fused kernels (AG→GEMM, GEMM
 peer memory, ``libai_b200/ops/comm_gemm.py``) when ``train.dist.fused_tp_comm`` is on.
 
 For inference, ``quantize_fp8_`` turns the layer's weight into FP8 (E4M3) bytes with one fp32 scale per output
-channel of this rank's shard; the forward then runs ``OF.linear_fp8w`` inside the same TP mappings.
+channel of this rank's shard, and ``quantize_int4_`` into packed 4-bit values with a scale and zero point per row and
+group of 128 input columns; the forward then runs ``OF.linear_fp8w`` or ``OF.linear_int4w`` inside the same TP mappings.
 """
 from __future__ import annotations
 
@@ -34,7 +35,7 @@ _FP8_SOURCE_DTYPES = (torch.bfloat16, torch.float16, torch.float32)
 
 
 class Linear1D(nn.Module):
-    compute_dtype = None   # FP8 weights: the dtype of the inputs, outputs and bias (the weight's dtype before)
+    compute_dtype = None   # FP8 or INT4 weights: the dtype of the inputs, outputs and bias (the weight's dtype before)
 
     def __init__(
         self,
@@ -75,6 +76,17 @@ class Linear1D(nn.Module):
         """The weight is FP8 (E4M3) bytes with row scales ``weight_scale`` (:meth:`quantize_fp8_`)."""
         return self.weight.dtype == torch.float8_e4m3fn
 
+    @property
+    def int4(self) -> bool:
+        """The weight is packed INT4 values with group scales ``weight_scale`` and zeros ``weight_zero``
+        (:meth:`quantize_int4_`)."""
+        return self.weight.dtype == torch.uint8
+
+    @property
+    def quantized(self) -> bool:
+        """The weight is FP8 or INT4: only ``OF.linear_fp8w`` / ``OF.linear_int4w`` read it, never a bf16 GEMM."""
+        return self.fp8 or self.int4
+
     @torch.no_grad()
     def quantize_fp8_(self):
         """Replace the weight ``[out_local, in_local]`` by its FP8 (E4M3) bytes and the fp32 scales ``weight_scale``
@@ -85,7 +97,7 @@ class Linear1D(nn.Module):
         if self.fp8:
             return self
         w = self.weight
-        if w.dtype not in _FP8_SOURCE_DTYPES:
+        if self.int4 or w.dtype not in _FP8_SOURCE_DTYPES:
             raise TypeError(f"quantize_fp8_: a {w.dtype} weight (bf16, fp16 or fp32 expected)")
         e, s = OF.kv_cache_quantize_ref(w)
         self.compute_dtype = w.dtype
@@ -93,14 +105,33 @@ class Linear1D(nn.Module):
         self.weight_scale = nn.Parameter(s, requires_grad=False)
         return self
 
+    @torch.no_grad()
+    def quantize_int4_(self):
+        """Replace the weight ``[out_local, in_local]`` (``in_local % 128 == 0``, finite) by its 4-bit values packed two
+        per byte (uint8 ``[out_local, in_local / 2]``), with a bf16 scale ``weight_scale`` and a uint8 zero point
+        ``weight_zero`` ``[out_local, in_local / 128]`` per row and group of 128 columns (``OF.int4_quantize_ref``); the
+        weight reads back as ``bf16_rn((q − z) · s)``.  The bias and the activations keep the weight's former dtype
+        (``compute_dtype``).  For inference only; a second call is a no-op."""
+        if self.int4:
+            return self
+        w = self.weight
+        if self.fp8 or w.dtype not in _FP8_SOURCE_DTYPES:
+            raise TypeError(f"quantize_int4_: a {w.dtype} weight (bf16, fp16 or fp32 expected)")
+        q, s, z = OF.int4_quantize_ref(w)
+        self.compute_dtype = w.dtype
+        self.weight = nn.Parameter(q, requires_grad=False)
+        self.weight_scale = nn.Parameter(s, requires_grad=False)
+        self.weight_zero = nn.Parameter(z, requires_grad=False)
+        return self
+
     def _apply(self, fn, recurse=True):
-        """Dtype casts (``.to(dtype)``, ``.bfloat16()``, ``.half()``, ``.float()``) leave FP8 bytes and their fp32
-        scales as they are and change ``compute_dtype`` (and the bias) instead; device moves move them."""
-        if not self.fp8:
+        """Dtype casts (``.to(dtype)``, ``.bfloat16()``, ``.half()``, ``.float()``) leave FP8 or INT4 bytes and their
+        scales (and zeros) as they are and change ``compute_dtype`` (and the bias) instead; device moves move them."""
+        if not self.quantized:
             return super()._apply(fn, recurse)
         probe = fn(torch.empty(0, dtype=self.compute_dtype, device=self.weight.device))
         order = list(self._parameters)
-        held = {k: self._parameters.pop(k) for k in ("weight", "weight_scale")}
+        held = {k: self._parameters.pop(k) for k in ("weight", "weight_scale", "weight_zero") if k in self._parameters}
         try:
             super()._apply(fn, recurse)
         finally:
@@ -152,6 +183,8 @@ class Linear1D(nn.Module):
     def _gemm(self, x, bias, act):
         if self.fp8:
             return OF.linear_fp8w(x, self.weight, self.weight_scale, bias, act)
+        if self.int4:
+            return OF.linear_int4w(x, self.weight, self.weight_scale, self.weight_zero, bias, act)
         return OF.linear(x, self.weight, bias, act)
 
     def _forward_fused(self, x, bias_now, act, topo, residual=None):
@@ -177,7 +210,8 @@ class Linear1D(nn.Module):
     def extra_repr(self) -> str:
         return "in_features={}, out_features={}, bias={}, parallel={}{}".format(
             self.in_features, self.out_features, self.bias is not None, self.parallel,
-            f", weight=fp8 (compute_dtype={self.compute_dtype})" if self.fp8 else "",
+            f", weight={'fp8' if self.fp8 else 'int4 (group 128)'} (compute_dtype={self.compute_dtype})"
+            if self.quantized else "",
         )
 
 

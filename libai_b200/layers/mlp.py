@@ -48,9 +48,9 @@ class MLP(nn.Module):
     def forward(self, hidden_states, residual=None):
         """Returns ``residual + dropout(mlp(x))`` when ``residual`` is given (fused epilogue)."""
         topo = dutil.get_dist_util()
-        # FP8 weights take the per-Linear path: OF.mlp and the fused TP kernels multiply bf16 weights only
-        fp8 = getattr(self.dense_h_to_4h, "fp8", False) or getattr(self.dense_4h_to_h, "fp8", False)
-        if not topo.sequence_parallel and not topo.fused_tp_comm and not fp8:
+        # FP8 and INT4 weights take the per-Linear path: OF.mlp and the fused TP kernels multiply bf16 weights only
+        quantized = getattr(self.dense_h_to_4h, "quantized", False) or getattr(self.dense_4h_to_h, "quantized", False)
+        if not topo.sequence_parallel and not topo.fused_tp_comm and not quantized:
             # both GEMMs in one autograd node: GELU' runs in the epilogue of the second layer's dgrad
             x = mappings.copy_to_tp(hidden_states)
             if (residual is not None and topo.tensor_parallel_size == 1
@@ -62,7 +62,7 @@ class MLP(nn.Module):
             out = OF.mlp(x, self.dense_h_to_4h.weight, self.dense_h_to_4h.bias, self.dense_4h_to_h.weight, "gelu")
             out, bias = mappings.reduce_from_tp(out), self.dense_4h_to_h.bias
         else:
-            if (topo.fused_tp_comm and not fp8 and hidden_states.is_cuda and hidden_states.dtype == torch.bfloat16
+            if (topo.fused_tp_comm and not quantized and hidden_states.is_cuda and hidden_states.dtype == torch.bfloat16
                     and hidden_states.dim() == 2 and (self.output_dropout_prob == 0.0 or not self.training)):
                 # both linears + their collectives + bias/GELU/bias/residual as one autograd node (ops/comm_gemm.py)
                 from libai_b200.ops import comm_gemm, use_native

@@ -22,7 +22,7 @@ import torch
 
 from libai_b200.ops import count_launch, load_ext
 from libai_b200.ops import functional as OF
-from libai_b200.ops.functional import _ACT_IDS, reject_fp8_weight
+from libai_b200.ops.functional import _ACT_IDS, reject_quantized_weight
 from libai_b200.parallel.symm_mem import CommWorkspace, get_workspace
 
 _BM = 128
@@ -133,7 +133,7 @@ def ag_gemm(x_shard: torch.Tensor, w: torch.Tensor, bias, act, group, layout: in
     ``layout`` 0: w is ``[N, K]``; 1: w is ``[K, N]``.  Epilogue: ``+ bias`` then ``act`` (``pre`` = the pre-activation
     when ``need_pre``), or with ``pre_in``: ``· act'(pre_in)`` (dgrad fused with the activation backward) and optional
     fp32 column sums into ``colsum``.  ``x_full`` (the local gathered buffer) is complete only with ``fill_local``."""
-    reject_fp8_weight("comm_gemm.ag_gemm", w)
+    reject_quantized_weight("comm_gemm.ag_gemm", w)
     ext = load_ext()
     st = _state(group)
     rows, K = x_shard.shape
@@ -175,7 +175,7 @@ def ag_wgrad(gy: torch.Tensor, x_shard: torch.Tensor, out: torch.Tensor, accumul
 
 def gemm_rs(x: torch.Tensor, w: torch.Tensor, bias, residual, group, layout: int = 0):
     """``reduce_scatter(x @ op(w)) (+ bias) (+ residual)`` → ``[M / world, N]``."""
-    reject_fp8_weight("comm_gemm.gemm_rs", w)
+    reject_quantized_weight("comm_gemm.gemm_rs", w)
     ext = load_ext()
     st = _state(group)
     M = x.shape[0]
@@ -310,15 +310,15 @@ class TPMLPFused(torch.autograd.Function):
 
 
 def column_parallel_linear(x_shard, w, bias, act, group):
-    reject_fp8_weight("comm_gemm.column_parallel_linear", w)
+    reject_quantized_weight("comm_gemm.column_parallel_linear", w)
     return ColumnParallelLinearFused.apply(x_shard, w, bias, act, group)
 
 
 def row_parallel_linear(x, w, bias, residual, group):
-    reject_fp8_weight("comm_gemm.row_parallel_linear", w)
+    reject_quantized_weight("comm_gemm.row_parallel_linear", w)
     return RowParallelLinearFused.apply(x, w, bias, residual, group)
 
 
 def tp_mlp(x_shard, w1, b1, w2, b2, residual, act, group):
-    reject_fp8_weight("comm_gemm.tp_mlp", w1, w2)
+    reject_quantized_weight("comm_gemm.tp_mlp", w1, w2)
     return TPMLPFused.apply(x_shard, w1, b1, w2, b2, residual, act, group)

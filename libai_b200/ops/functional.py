@@ -195,17 +195,21 @@ class _LinearFn(torch.autograd.Function):
         return gx, gw, gb, None, (gy if ctx.has_res else None)
 
 
-def reject_fp8_weight(what: str, *weights) -> None:
-    """FP8 (E4M3) weights read back only with their row scales, which the bf16 GEMM entries do not take: they raise
-    instead of multiplying the bytes unscaled (:func:`linear_fp8w` is the entry for such weights)."""
+def reject_quantized_weight(what: str, *weights) -> None:
+    """FP8 (E4M3) weights read back only with their row scales, and packed INT4 weights (uint8) only with their group
+    scales and zeros, which the bf16 GEMM entries do not take: they raise instead of multiplying the bytes
+    (:func:`linear_fp8w` and :func:`linear_int4w` are the entries for such weights)."""
     for w in weights:
         if w is not None and w.dtype == torch.float8_e4m3fn:
             raise TypeError(f"{what}: float8_e4m3fn weight; FP8 weights take OF.linear_fp8w with their row scales")
+        if w is not None and w.dtype == torch.uint8:
+            raise TypeError(f"{what}: packed INT4 (uint8) weight; INT4 weights take OF.linear_int4w with their group "
+                            "scales and zeros")
 
 
 def linear(x, w, bias=None, act: Optional[str] = None):
     """``act(x @ w.T + bias)``; ``w`` is ``[out, in]``."""
-    reject_fp8_weight("linear", w)
+    reject_quantized_weight("linear", w)
     if use_native(x, w) and _gemm_ok(x, w):
         return _LinearFn.apply(x, w, bias, act)
     y = F.linear(x, w.to(x.dtype) if w.dtype != x.dtype else w, None if bias is None else bias.to(x.dtype))
@@ -265,7 +269,7 @@ class _MLPFn(torch.autograd.Function):
 def mlp(x, w1, b1, w2, act: str = "gelu", b2=None, residual=None):
     """``act(x @ w1ᵀ + b1) @ w2ᵀ``; with ``residual`` also ``+ b2 + residual`` in the second GEMM's epilogue
     (without it the second bias is left to the fused bias+dropout+residual op)."""
-    reject_fp8_weight("mlp", w1, w2)
+    reject_quantized_weight("mlp", w1, w2)
     if use_native(x, w1) and _gemm_ok(x, w1) and _gemm_ok(x.new_empty(1, w1.shape[0]), w2):
         if residual is not None:
             return _MLPFn.apply(x, w1, b1, w2, act, b2, residual)
@@ -276,7 +280,7 @@ def mlp(x, w1, b1, w2, act: str = "gelu", b2=None, residual=None):
 
 def linear_bias_residual(x, w, bias, residual):
     """``x @ wᵀ + bias + residual`` (output projection of a block, dropout-free)."""
-    reject_fp8_weight("linear_bias_residual", w)
+    reject_quantized_weight("linear_bias_residual", w)
     if use_native(x, w) and _gemm_ok(x, w) and residual is not None and residual.dtype == torch.bfloat16:
         return _LinearFn.apply(x, w, bias, None, residual)
     y = linear(x, w, bias)
@@ -328,6 +332,88 @@ def linear_fp8w(x, w, w_scale, bias=None, act: Optional[str] = None):
                 count_launch(2)
                 return y.view(*x.shape[:-1], N)
     return linear_fp8w_ref(x, w, w_scale, bias, act)
+
+
+# --------------------------------------------------------------------------------------
+# Group-wise INT4 weights for inference: ``w`` [N, K/2] uint8 holds the 4-bit values q two per byte (column 2j in the low
+# nibble of byte j), ``w_scale`` [N, K/128] bf16 and ``w_zero`` [N, K/128] uint8 one scale s and zero point z per row and
+# group of 128 columns (:func:`int4_quantize_ref`, see ``Linear1D.quantize_int4_``).  The weight reads back as
+# Ŵ[n, k] = bf16_rn((q[n, k] − z[n, k/128]) · s[n, k/128]): q − z is an integer in [−15, 15] and s has an 8-bit
+# significand, so the product is exact in fp32 and Ŵ is one rounding, the same bits in the kernel, the dequantize kernel
+# and :func:`int4_dequant_ref`.
+# --------------------------------------------------------------------------------------
+INT4_GROUP = 128
+# Up to this many rows (tokens) run the weight-streaming kernel; more dequantize the weight to bf16 and run the bf16 GEMM.
+# 64 is the most the kernel takes: it was faster than dequantize + GEMM at every M of the sweep up to 64
+# (dev/int4_weights_bench.py, Kernels.md "INT4 weights")
+INT4W_KERNEL_MAX_M = 64
+
+
+def int4_quantize_ref(w):
+    """``(weight, weight_scale, weight_zero)`` of ``w`` [N, K] (K % 128 == 0, finite): round to nearest per row and
+    group of 128 columns, in fp32 on ``w``'s device.  With ``lo = min(0, min w)`` and ``hi = max(0, max w)`` of a group,
+    ``s = bf16_rn((hi − lo) / 15)`` (1 if that is zero or subnormal), ``z = clamp(round(−lo / s), 0, 15)`` and
+    ``q = clamp(round(w / s) + z, 0, 15)``, rounding half to even.  Returns q packed two per byte (uint8 [N, K/2]),
+    s (bf16 [N, K/128]) and z (uint8 [N, K/128])."""
+    if w.dim() != 2 or w.shape[1] % INT4_GROUP != 0:
+        raise ValueError(f"int4_quantize_ref: a [N, K] weight with K % {INT4_GROUP} == 0, got {tuple(w.shape)}")
+    if not bool(torch.isfinite(w).all()):
+        raise ValueError("int4_quantize_ref: the weight has a non-finite value")
+    N, K = w.shape
+    g = w.float().view(N, K // INT4_GROUP, INT4_GROUP)
+    lo = g.amin(-1).clamp(max=0.0)
+    hi = g.amax(-1).clamp(min=0.0)
+    s = ((hi - lo) / 15).to(torch.bfloat16).float()
+    s = torch.where(s < torch.finfo(torch.float32).tiny, torch.ones_like(s), s)   # zero or subnormal
+    z = torch.clamp(torch.round(-lo / s), 0, 15)
+    q = torch.clamp(torch.round(g / s[..., None]) + z[..., None], 0, 15).to(torch.uint8).view(N, K)
+    return q[:, 0::2] | (q[:, 1::2] << 4), s.to(torch.bfloat16), z.to(torch.uint8)
+
+
+def int4_dequant_ref(w, w_scale, w_zero):
+    """Ŵ = bf16_rn((q − z) · s) as bf16 [N, K] of a packed INT4 weight (:func:`int4_quantize_ref`)."""
+    N = w.shape[0]
+    q = torch.stack([w & 15, w >> 4], dim=-1).view(N, -1, INT4_GROUP).float()
+    wf = (q - w_zero.float()[..., None]) * w_scale.float()[..., None]
+    return wf.view(N, -1).to(torch.bfloat16)
+
+
+def linear_int4w_ref(x, w, w_scale, w_zero, bias=None, act: Optional[str] = None):
+    """``act(x @ Ŵᵀ + bias)`` in fp32, rounded to x's dtype."""
+    wf = int4_dequant_ref(w, w_scale, w_zero).float()
+    y = F.linear(x.float(), wf, None if bias is None else bias.float())
+    return _act_ref(y, act).to(x.dtype)
+
+
+def linear_int4w(x, w, w_scale, w_zero, bias=None, act: Optional[str] = None):
+    """``act(x @ Ŵᵀ + bias)`` for a packed INT4 weight ``w`` [N, K/2] (uint8) with bf16 group scales ``w_scale`` and uint8
+    zero points ``w_zero`` [N, K/128]; returns x's dtype.  On the GPU with bf16 x: up to ``INT4W_KERNEL_MAX_M`` rows run
+    the weight-streaming kernel (fp32 accumulation, bias and activation on the fp32 sum), more rows dequantize the
+    weight to bf16 Ŵ (a temporary of the caching allocator) and run the bf16 GEMM with its bias/activation epilogue.
+    Other inputs (CPU, fp32 or fp16 x) run :func:`linear_int4w_ref`.  Inference only: a call that would need a gradient
+    raises."""
+    if torch.is_grad_enabled() and (x.requires_grad or (bias is not None and bias.requires_grad)):
+        raise RuntimeError("INT4 weights are for inference: run the model under torch.no_grad() (and without inputs "
+                           "that require a gradient)")
+    N, K = w.shape[0], 2 * w.shape[1]
+    x2 = x.reshape(-1, K)
+    M = x2.shape[0]
+    if (use_native(x) and x.dtype == torch.bfloat16 and w.is_cuda and K % INT4_GROUP == 0 and M >= 1
+            and all(t.is_contiguous() for t in (w, w_scale, w_zero)) and (bias is None or bias.dtype == torch.bfloat16)):
+        ext = load_ext()
+        x2 = x2.contiguous()
+        b = None if bias is None else bias.contiguous()
+        if x2.data_ptr() % 16 == 0 and w.data_ptr() % 16 == 0:
+            if M <= INT4W_KERNEL_MAX_M:
+                y = ext.linear_int4w(x2, w, w_scale, w_zero, b, _ACT_IDS[act])
+                count_launch(2)   # the kernel, and the sum over its K ranges
+                return y.view(*x.shape[:-1], N)
+            if N % 8 == 0:
+                wb = ext.dequant_int4_rows(w, w_scale, w_zero)
+                y, _ = ext.linear_fwd(x2, wb, b, _ACT_IDS[act], False)
+                count_launch(2)
+                return y.view(*x.shape[:-1], N)
+    return linear_int4w_ref(x, w, w_scale, w_zero, bias, act)
 
 
 def matmul_nt(a, b):

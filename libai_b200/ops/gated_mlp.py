@@ -20,7 +20,7 @@ import torch
 
 from libai_b200.ops import count_launch, load_ext
 from libai_b200.ops import functional as OF
-from libai_b200.ops.functional import reject_fp8_weight
+from libai_b200.ops.functional import reject_quantized_weight
 
 _ENABLED = os.environ.get("LIBAI_B200_FUSED_GATE_UP", "1") == "1"
 
@@ -150,10 +150,10 @@ class TPGatedMLPFused(torch.autograd.Function):
 
 
 def gated_mlp(x, wg, wu, wd):
-    reject_fp8_weight("gated_mlp", wg, wu, wd)
+    reject_quantized_weight("gated_mlp", wg, wu, wd)
     return GatedMLPFn.apply(x, wg, wu, wd)
 
 
 def tp_gated_mlp(x_shard, wg, wu, wd, residual, group):
-    reject_fp8_weight("tp_gated_mlp", wg, wu, wd)
+    reject_quantized_weight("tp_gated_mlp", wg, wu, wd)
     return TPGatedMLPFused.apply(x_shard, wg, wu, wd, residual, group)
