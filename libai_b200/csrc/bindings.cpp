@@ -346,6 +346,29 @@ Tensor dequant_int4_rows(const Tensor& w, const Tensor& w_scale, const Tensor& w
   return out;
 }
 
+// One speculative-decoding iteration's greedy acceptance (speculative_sm90.cu): logits bf16 or fp32 [b, R, V]
+// (contiguous), draft int64 [b, R - 1], unfinished int64 [b] (updated in place); eos < 0: no EOS.  Returns out int64
+// [b, 2R + 3]: the argmaxes, the emitted tokens, a_b, n and the updated unfinished.  The kernel's block counter is one
+// more element of out's allocation, zeroed on the stream before the launch.
+Tensor spec_accept(const Tensor& logits, const Tensor& draft, Tensor unfinished, int64_t eos, int64_t pad) {
+  Args args("spec_accept");
+  args("logits", logits, Dtypes(at::kBFloat16, at::kFloat), {kAny, kAny, kAny});
+  const int64_t B = logits.size(0), R = logits.size(1), V = logits.size(2);
+  TORCH_CHECK(B >= 1 && R >= 1 && R <= 16 && V >= 1 && V <= INT32_MAX, "spec_accept: logits [b, k + 1, V] needs b >= 1, ",
+              "1 <= k + 1 <= 16 and V >= 1, got ", logits.sizes());
+  args("draft", draft, at::kLong, {B, R - 1});
+  args("unfinished", unfinished, at::kLong, {B});
+  const auto guard = args.guard();
+  const int64_t cols = 2 * R + 3;
+  Tensor buf = at::empty({B * cols + 1}, draft.options());
+  int64_t* out = buf.data_ptr<int64_t>();
+  check(lb_spec_accept(logits.data_ptr(), logits.scalar_type() == at::kFloat ? 1 : 0, draft.data_ptr<int64_t>(),
+                       unfinished.data_ptr<int64_t>(), out, reinterpret_cast<unsigned int*>(out + B * cols), (int)B,
+                       (int)R, (int)V, (long long)eos, (long long)pad, cur_stream()),
+        "spec_accept");
+  return buf.narrow(0, 0, B * cols).view({B, cols});
+}
+
 // per-tensor E4M3 quantisation of a contiguous bf16 tensor: returns (q [same shape, float8_e4m3fn], deq fp32 [1]) with
 // x ≈ q * deq (deq = amax / 448); two kernels, no host synchronisation
 std::tuple<Tensor, Tensor> quantize_e4m3(const Tensor& x) {
@@ -1366,6 +1389,7 @@ TORCH_LIBRARY(libai_b200, m) {
   m.def("linear_int4w(Tensor x, Tensor w, Tensor w_scale, Tensor w_zero, Tensor? bias, int act) -> Tensor",
         &linear_int4w);
   m.def("dequant_int4_rows(Tensor w, Tensor w_scale, Tensor w_zero) -> Tensor", &dequant_int4_rows);
+  m.def("spec_accept(Tensor logits, Tensor draft, Tensor(a!) unfinished, int eos, int pad) -> Tensor", &spec_accept);
   m.def("linear_fp8_fwd(Tensor xq, Tensor wq, Tensor deq_x, Tensor deq_w, Tensor? bias, int act, bool need_pre, Tensor? residual=None, int bn=0) -> (Tensor, Tensor)", &linear_fp8_fwd);
   m.def("act_bwd(Tensor gy, Tensor pre, int act) -> Tensor", &act_bwd);
   m.def("colsum(Tensor x, Tensor(a!)? accum=None) -> Tensor", &colsum);

@@ -163,6 +163,11 @@ int lb_linear_int4w(const void* x, const void* w, const void* w_scale, const voi
 // out [rows, K] bf16 = Ŵ of lb_linear_int4w, K % 128 == 0
 int lb_dequant_int4_rows(const void* w, const void* w_scale, const void* w_zero, void* out, long rows, int K,
                          cudaStream_t s);
+// Greedy acceptance of one speculative-decoding iteration (speculative_sm90.cu): logits [B, R, V] bf16 (logits_fp32 = 0)
+// or fp32, draft int64 [B, R - 1], unfinished int64 [B] (updated in place), out int64 [B, 2R + 3]; counter: a uint32 of
+// this launch's own, zeroed on the stream before the kernel.  eos < 0: no EOS.
+int lb_spec_accept(const void* logits, int logits_fp32, const int64_t* draft, int64_t* unfinished, int64_t* out,
+                   unsigned int* counter, int B, int R, int V, long long eos, long long pad, cudaStream_t s);
 int lb_window_attn_groups(int B, int H, int W, int ws, int heads);
 int lb_window_attn_fwd(const void* qkv, void* out, float* lse, const float* table, const float* tau, int B, int H, int W,
                        int ws, int shift, int heads, int d, float scale, cudaStream_t s);

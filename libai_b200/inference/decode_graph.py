@@ -9,7 +9,8 @@ Capture protocol (:class:`DecodeGraph`): a step is first run eagerly (a real ste
 one-time setup: extension load, ``cudaFuncSetAttribute``, driver entry points); the next one is captured, which runs
 its Python once but no kernel, so every host-side effect of the captured Python (``cache.length``, the model's
 ``past_length``) is rolled back; that step and every later one are then replayed, and after each replay the host
-mirrors advance by one row.  The device-side ``seqlens.add_`` of ``StaticKVCache.advance`` is inside the graph, so after
+mirrors advance by the step's rows: one, or ``tokens`` for a step that opts in to more (a speculative verify step,
+``step(..., tokens=k + 1)``).  The device-side ``seqlens.add_`` of ``StaticKVCache.advance`` is inside the graph, so after
 every step the cache rows, ``seqlens``, ``kv_start`` and the host mirror are what eager decoding leaves, bit for bit.
 
 A graph is kept per model and keyed by the batch, the caches' buffer addresses, capacity and KV dtype, the weights'
@@ -40,6 +41,8 @@ STATIC_INPUTS = ("input_ids", "decoder_input_ids", "position_ids")
 # inputs a cached step provably ignores while no cache needs a dense mask: padding masks (kv_start holds a left-padded
 # prompt's padding) and an encoder-decoder model's encoder inputs (its cross cache holds their projection)
 IGNORED_INPUTS = ("attention_mask", "encoder_input_ids", "encoder_attn_mask", "encoder_decoder_attn_mask")
+# the most new tokens a replayed step takes: the split-KV decode kernel's limit (OF.decode_attention)
+MAX_TOKENS = 16
 
 
 class DecodeCall:
@@ -78,8 +81,9 @@ def _signature(inputs: Dict):
     return tuple(sig)
 
 
-def fallback_reason(model, inputs: Dict) -> Optional[str]:
-    """Why this decode step (the cache is not empty) cannot replay a graph, or None when it can."""
+def fallback_reason(model, inputs: Dict, tokens: int = 1) -> Optional[str]:
+    """Why this decode step (the cache is not empty) of ``tokens`` new tokens cannot replay a graph, or None when it
+    can."""
     cache = model.kv_cache
     if cache.device.type != "cuda":
         return "the cache is not on a CUDA device"
@@ -89,14 +93,14 @@ def fallback_reason(model, inputs: Dict) -> Optional[str]:
     if not (use_native(cache.seqlens) and cache.dtype == torch.bfloat16 and cache.head_dim in (64, 128)):
         return "the step does not run the native bf16 kernels"
     ids = inputs.get("decoder_input_ids", inputs.get("input_ids"))
-    if not torch.is_tensor(ids) or ids.dim() != 2 or ids.shape[1] != 1:
-        return "more than one new token"
+    if not torch.is_tensor(ids) or ids.dim() != 2 or ids.shape[1] != tokens:
+        return "more than one new token" if tokens == 1 else f"not {tokens} new tokens"
     if any(c.dense_mask for c in _caches(model)):
         return "the prompt's padding needs a dense mask"
-    if cache.length + 1 > cache.capacity:
+    if cache.length + tokens > cache.capacity:
         return "the cache must grow"
     limit = model.max_cache_positions
-    if limit is not None and cache.length + 1 > limit:
+    if limit is not None and cache.length + tokens > limit:
         return "the step passes the model's maximum length"
     for k, v in inputs.items():
         if torch.is_tensor(v) and k not in STATIC_INPUTS and k not in IGNORED_INPUTS:
@@ -108,8 +112,9 @@ class DecodeGraph:
     """The CUDA graph of one decode step of ``model`` on its current cache(s): static input buffers, the captured graph
     and its outputs.  :meth:`step` runs the eager warm-up step, captures, and replays."""
 
-    def __init__(self, key, inputs: Dict):
+    def __init__(self, key, inputs: Dict, tokens: int = 1):
         self.key = key
+        self.tokens = tokens       # the new tokens (cache rows) of one step
         self.static = {k: v.clone() for k, v in inputs.items() if k in STATIC_INPUTS and torch.is_tensor(v)}
         self.graph: Optional[torch.cuda.CUDAGraph] = None
         self.outputs = None
@@ -153,8 +158,8 @@ class DecodeGraph:
             for c, n in zip(caches, lengths):
                 c.length = n
             model.past_length = past
-        if advanced != 1:
-            raise RuntimeError(f"the captured step advanced the cache by {advanced} rows, not 1")
+        if advanced != self.tokens:
+            raise RuntimeError(f"the captured step advanced the cache by {advanced} rows, not {self.tokens}")
         self.graph, self.outputs = graph, outputs
         self.capture_ms = (time.perf_counter() - t0) * 1e3
 
@@ -164,7 +169,7 @@ class DecodeGraph:
         self.graph.replay()
         ops.count_launch(self.launches)
         cache = model.kv_cache
-        cache.length += 1
+        cache.length += self.tokens
         model.past_length = cache.length
         # the graph's outputs are overwritten by the next replay: hand out copies
         return {k: v.clone() if torch.is_tensor(v) else v for k, v in self.outputs.items()}
@@ -178,13 +183,17 @@ def _eager(model, inputs: Dict, call: DecodeCall, reason: str, level=logging.INF
     return model(**inputs)
 
 
-def step(model, inputs: Dict, call: DecodeCall):
+def step(model, inputs: Dict, call: DecodeCall, tokens: int = 1):
     """One cached step of ``model`` (``model(**inputs)``): replayed from the model's :class:`DecodeGraph` when the step
-    is eligible, else eager (the prefill, and each :func:`fallback_reason` or failed capture, logged once per call)."""
+    is eligible, else eager (the prefill, and each :func:`fallback_reason` or failed capture, logged once per call).
+    ``tokens``: the new tokens of the step the graph captures and replays, 1 to 16 (a speculative verify step takes
+    k + 1); a step with another number of new tokens runs eagerly."""
+    if not 1 <= tokens <= MAX_TOKENS:
+        raise ValueError(f"tokens: a decode graph replays steps of 1 to {MAX_TOKENS} new tokens, got {tokens}")
     cache = getattr(model, "kv_cache", None)
     if not isinstance(cache, StaticKVCache) or cache.length == 0 or not inputs.get("use_cache"):
         return model(**inputs)
-    reason = fallback_reason(model, inputs)
+    reason = fallback_reason(model, inputs) if tokens == 1 else fallback_reason(model, inputs, tokens)
     if reason is not None:
         return _eager(model, inputs, call, reason)
     if call.weights is None:
@@ -193,7 +202,7 @@ def step(model, inputs: Dict, call: DecodeCall):
     graph = current_graph(model)
     if graph is None or graph.key != key:
         model._decode_graph = None   # the old graph and its memory pool go first
-        graph = model._decode_graph = DecodeGraph(key, inputs)
+        graph = model._decode_graph = DecodeGraph(key, inputs, tokens)
     return graph.step(model, inputs, call)
 
 

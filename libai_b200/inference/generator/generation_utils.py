@@ -19,6 +19,7 @@ from typing import Callable, Dict, Iterable, List, Optional, Tuple, Union
 
 import torch
 
+from libai_b200.ops import functional as OF
 from libai_b200.utils import distributed as dutil
 import torch.distributed as dist
 
@@ -59,8 +60,19 @@ _DEFAULTS = dict(
     num_return_sequences=1, output_scores=False, use_cache=True, bos_token_id=None, eos_token_id=None,
     pad_token_id=None, decoder_start_token_id=None, forced_bos_token_id=None, forced_eos_token_id=None,
     remove_invalid_values=False, exponential_decay_length_penalty=None, chunk_size_feed_forward=0,
-    kv_cache_dtype=None, decode_graphs=False,
+    kv_cache_dtype=None, decode_graphs=False, assistant_model=None, num_assistant_tokens=None,
+    prompt_lookup_num_tokens=None, max_matching_ngram_size=None,
 )
+# generate()'s arguments for the logits processors speculative decoding refuses, by processor
+_PROCESSOR_ARGS = {
+    HammingDiversityLogitsProcessor: "diversity_penalty", RepetitionPenaltyLogitsProcessor: "repetition_penalty",
+    NoRepeatNGramLogitsProcessor: "no_repeat_ngram_size", EncoderNoRepeatNGramLogitsProcessor: "encoder_no_repeat_ngram_size",
+    MinLengthLogitsProcessor: "min_length", PrefixConstrainedLogitsProcessor: "prefix_allowed_tokens_fn",
+    ForcedBOSTokenLogitsProcessor: "forced_bos_token_id", ForcedEOSTokenLogitsProcessor: "forced_eos_token_id",
+    InfNanRemoveLogitsProcessor: "remove_invalid_values", ExponentialDecayLengthPenalty: "exponential_decay_length_penalty",
+    NormalizationLogitsProcessor: "renormalize_logits",
+}
+MAX_SPECULATIVE_TOKENS = 15   # k: a verify step of k + 1 tokens stays within the split-KV decode kernel's 16
 
 
 def _kv_cache_dtype(value):
@@ -70,6 +82,25 @@ def _kv_cache_dtype(value):
     if isinstance(value, str) and value.lower() == "fp8":
         return torch.float8_e4m3fn
     raise ValueError(f"kv_cache_dtype must be None, 'fp8' or torch.float8_e4m3fn, got {value!r}")
+
+
+def prompt_lookup(seq: List[int], k: int, max_ngram: int) -> List[int]:
+    """Prompt-lookup proposals for one sample (HF's rule): for n from ``max_ngram`` down to 1, the earliest earlier
+    occurrence of the last n tokens of ``seq`` that has at least one following token; up to ``k`` of the tokens that
+    follow it, padded to ``k`` by repeating the last one (the last token of ``seq`` when nothing matches).  The filler
+    only costs acceptance: greedy acceptance keeps only tokens the target chooses itself."""
+    L = len(seq)
+    out: List[int] = []
+    for n in range(min(max_ngram, L - 1), 0, -1):
+        tail = seq[L - n :]
+        for i in range(L - n):   # i + n < L: the occurrence has a following token
+            if seq[i : i + n] == tail:
+                out = seq[i + n : i + n + k]
+                break
+        if out:
+            break
+    fill = out[-1] if out else seq[-1]
+    return out + [fill] * (k - len(out))
 
 
 def _decode_graphs(value) -> bool:
@@ -502,6 +533,197 @@ class Generator:
             return result["sequences"], result["sequence_scores"], scores
         return result["sequences"]
 
+    # a decoder-only model whose cached step takes ``{"input_ids": [b, s], "use_cache": True}`` for any s (positions and
+    # padding from its StaticKVCache): it can verify speculative proposals, and serve as a draft
+    speculative_decoding = False
+
+    def _verify_step(self, block):
+        """One cached step of the target on ``block`` ``[b, k + 1]`` (a graph of k + 1 tokens when graphs are on)."""
+        inputs = {"input_ids": block, "use_cache": True}
+        if self._decode_graphs is not None:
+            return decode_graph.step(self, inputs, self._decode_graphs, tokens=block.shape[1])
+        return self(**inputs)
+
+    @staticmethod
+    def _all_logits(outputs):
+        return (outputs["logits"] if "logits" in outputs else outputs["prediction_scores"]).contiguous()
+
+    @torch.no_grad()
+    def speculative_search(self, input_ids, assistant_model=None, num_assistant_tokens=4, prompt_lookup_num_tokens=None,
+                           max_matching_ngram_size=2, stopping_criteria=None, pad_token_id=None, eos_token_id=None,
+                           output_scores=False, **model_kwargs):
+        """Greedy speculative decoding: proposals from ``assistant_model`` (a draft model, ``num_assistant_tokens`` per
+        iteration) or from prompt lookup (``prompt_lookup_num_tokens``, :func:`prompt_lookup`), verified in one cached
+        step of this model.
+
+        One iteration, x the last emitted token: propose d_1 .. d_k; run the target on ``[x, d_1 .. d_k]``; accept, per
+        sample, the longest prefix of the proposals equal to the target's argmaxes; advance the whole batch by the
+        minimum n over its unfinished samples and emit the target's tokens t_1 .. t_{n+1} (:func:`OF.spec_accept`, one
+        readback per iteration).  The output follows ``greedy_search`` (its shape, EOS padding and stops, one fp32
+        score row per emitted token).  Each token equals plain greedy's whenever the verify step's argmax equals the
+        single-token step's: the two differ only in rounding (other split ranges in the decode attention, another M
+        in the GEMMs), so the output is greedy decoding up to rounding, not bit for bit.
+
+        A sample that emits EOS inside a block, with n past its EOS, is fed the proposals that follow its EOS in that
+        block where greedy feeds pad tokens: its cache holds their rows, and its score rows differ from greedy's from
+        that position on, in every later iteration too (its tokens are pad either way).  A finished sample's later
+        proposals are pad tokens.
+
+        After every iteration each cache holds the rows of the sequence minus its last token, as greedy leaves them
+        (but for the rows after a finished sample's EOS, above):
+        the target drops the rows past the accepted tokens (``StaticKVCache.rollback``); the draft, which only takes
+        single-token steps, rolls back too, or, when all k were accepted, feeds d_k at the start of the next
+        iteration.  Both caches hold ``max_length + k`` rows (``generate`` sizes them).  Near a model's maximum
+        positions k shrinks so that no step writes past them; those steps run eagerly under decode graphs."""
+        stopping_criteria = stopping_criteria if stopping_criteria is not None else StoppingCriteriaList()
+        draft = assistant_model
+        k = num_assistant_tokens if draft is not None else prompt_lookup_num_tokens
+        max_length = stopping_criteria.max_length
+        b, dev = input_ids.shape[0], input_ids.device
+        scores = () if output_scores else None
+
+        outputs = self._decode_step(input_ids, model_kwargs)
+        cache = self.kv_cache
+        if cache.dense_mask:
+            raise ValueError("attention_mask: speculative decoding needs padding that the cache's kv_start holds "
+                             "(left padding); this prompt needs a dense mask")
+        rows = self._all_logits(outputs)[:, -1:].contiguous()
+        # rows a cache holds besides the sequence's (ChatGLM's P-tuning prefix)
+        extra = cache.length - input_ids.shape[1]
+        draft_kwargs = {"past": None, "use_cache": True}
+        if draft is not None:
+            mask = model_kwargs.get("attention_mask")
+            draft_out = draft._decode_step(input_ids, {"use_cache": True, **({} if mask is None else
+                                                                            {"attention_mask": mask})})
+            if draft._all_logits(draft_out).shape[-1] != rows.shape[-1]:
+                raise ValueError(f"assistant_model: its logits are {draft._all_logits(draft_out).shape[-1]} wide, the "
+                                 f"target's {rows.shape[-1]}")
+            if draft.kv_cache.dense_mask:
+                raise ValueError("attention_mask: the assistant's cache needs a dense mask for this prompt")
+            draft_kwargs["past"] = draft.kv_cache
+            draft_extra = draft.kv_cache.length - input_ids.shape[1]
+        history = staging = None
+        if draft is None:
+            history = input_ids.tolist()
+            if dev.type == "cuda":   # prompt-lookup proposals reach the device by an asynchronous copy from pinned memory
+                staging = torch.empty(b * k, dtype=input_ids.dtype, pin_memory=True)
+        proposals = input_ids.new_empty(b, 0)
+        unfinished = torch.ones(b, dtype=torch.long, device=dev)
+        host_unfinished = [1] * b
+        while True:
+            R = rows.shape[1]
+            res = OF.spec_accept(rows, proposals, unfinished, eos_token_id, pad_token_id)
+            host = res.tolist()   # the iteration's one readback
+            n = host[0][2 * R + 1]
+            count = n + 1
+            if max_length is not None:
+                count = min(count, max(max_length - input_ids.shape[1], 1))   # greedy emits one token at least
+            if eos_token_id is not None:   # greedy stops at the first position where every sample is finished
+                live = list(host_unfinished)
+                for j in range(count):
+                    live = [u and int(host[i][R + j] != eos_token_id) for i, u in enumerate(live)]
+                    if not any(live):
+                        count = j + 1
+                        break
+            input_ids = torch.cat([input_ids, res[:, R : R + count]], dim=-1)
+            if output_scores:
+                scores += tuple(rows[:, j].float() for j in range(count))
+            if history is not None:
+                for i in range(b):
+                    history[i].extend(host[i][R : R + count])
+            host_unfinished = [row[2 * R + 2] for row in host]
+            if not any(host_unfinished) or count < n + 1 or stopping_criteria(input_ids, scores):
+                break
+
+            # both caches back to the invariant: the rows of the sequence minus its last token
+            L = input_ids.shape[1]
+            cache.rollback(cache.length - (L - 1 + extra))
+            self.past_length = cache.length
+            kk = k
+            if self.max_cache_positions is not None:   # the verify step writes k + 1 rows
+                kk = min(kk, self.max_cache_positions - cache.length - 1)
+            if draft is not None:
+                dc, held = draft.kv_cache, L - 1 + draft_extra
+                if dc.length > held:
+                    dc.rollback(dc.length - held)
+                    draft.past_length = dc.length
+                elif dc.length == held - 1:   # every proposal was accepted: the draft lacks the row of d_k
+                    draft._decode_step(input_ids[:, L - 2 : L - 1], draft_kwargs)
+                if draft.max_cache_positions is not None:   # the draft writes k rows
+                    kk = min(kk, draft.max_cache_positions - dc.length)
+            kk = max(kk, 0)
+
+            x = input_ids[:, -1:]
+            if draft is not None:
+                tok, props = x, []
+                for _ in range(kk):
+                    tok = self._all_logits(draft._decode_step(tok, draft_kwargs))[:, -1].argmax(dim=-1, keepdim=True)
+                    props.append(tok)
+                proposals = torch.cat(props, dim=1) if props else input_ids.new_empty(b, 0)
+            else:
+                proposals = torch.tensor([prompt_lookup(h, kk, max_matching_ngram_size) for h in history],
+                                         dtype=input_ids.dtype).view(b, kk)
+                if staging is not None:
+                    # the previous iteration's copy out of the buffer ended before its readback returned
+                    proposals = staging[: b * kk].view(b, kk).copy_(proposals)
+                proposals = proposals.to(dev, non_blocking=True)
+            if eos_token_id is not None:   # a finished sample is fed pad tokens, as greedy feeds it
+                proposals = proposals.masked_fill(unfinished[:, None] == 0, pad_token_id)
+            rows = self._all_logits(self._verify_step(torch.cat([x, proposals], dim=1)))
+        self._reset_cache()
+        if draft is not None:
+            draft._reset_cache()
+        return (input_ids, scores) if output_scores else input_ids
+
+    def _speculative_args(self, draft, num_assistant_tokens, prompt_lookup_num_tokens, max_matching_ngram_size,
+                          do_sample, num_beams, num_return_sequences, processors, custom_criteria, is_enc_dec,
+                          max_length, model_kwargs):
+        """Check a speculative ``generate()`` call; returns ``(k, max_matching_ngram_size)``."""
+        if draft is not None and prompt_lookup_num_tokens is not None:
+            raise ValueError("assistant_model and prompt_lookup_num_tokens: give one proposer, not both")
+        name = "assistant_model" if draft is not None else "prompt_lookup_num_tokens"
+        k = (4 if num_assistant_tokens is None else num_assistant_tokens) if draft is not None \
+            else prompt_lookup_num_tokens
+        arg = "num_assistant_tokens" if draft is not None else "prompt_lookup_num_tokens"
+        if isinstance(k, bool) or not isinstance(k, int) or not 1 <= k <= MAX_SPECULATIVE_TOKENS:
+            raise ValueError(f"{arg} must be an int in [1, {MAX_SPECULATIVE_TOKENS}], got {k!r}")
+        ngram = 2 if max_matching_ngram_size is None else max_matching_ngram_size
+        if draft is None and (isinstance(ngram, bool) or not isinstance(ngram, int) or ngram < 1):
+            raise ValueError(f"max_matching_ngram_size must be a positive int, got {ngram!r}")
+        if do_sample:
+            raise ValueError(f"{name}: speculative decoding is greedy; do_sample=True is not supported")
+        if num_beams != 1:
+            raise ValueError(f"{name}: speculative decoding is greedy; num_beams={num_beams} is not supported")
+        if num_return_sequences != 1:
+            raise ValueError(f"{name}: num_return_sequences={num_return_sequences} is not supported")
+        if processors:
+            names = sorted({_PROCESSOR_ARGS.get(type(p), "logits_processor") for p in processors})
+            raise ValueError(f"{name}: speculative decoding applies no logits processor; drop {', '.join(names)}")
+        if custom_criteria:
+            raise ValueError(f"{name}: custom stopping_criteria are not supported (max_length and max_time are)")
+        if not model_kwargs.get("use_cache"):
+            raise ValueError(f"{name}: speculative decoding runs on the KV cache; use_cache=False is not supported")
+        if max_length is None:
+            raise ValueError(f"{name}: speculative decoding sizes both caches from max_length; give max_length or "
+                             "max_new_tokens")
+        topo = dutil.get_dist_util()
+        if topo.tensor_parallel_size > 1 or topo.pipeline_parallel_size > 1:
+            raise ValueError(f"{name}: tensor- or pipeline-parallel inference is not supported")
+        for role, m in (("the model", self), ("assistant_model", draft)):
+            if m is None:
+                continue
+            cls = type(m).__name__
+            if not (isinstance(m, KVCacheOwner) and isinstance(m, Generator)) or not m.speculative_decoding or \
+                    bool(m._gcfg("is_encoder_decoder")) or (m is self and is_enc_dec):
+                raise ValueError(f"{name}: {role} ({cls}) is not a decoder-only model that speculative decoding "
+                                 "supports (encoder-decoder and GLM models are not)")
+        if draft is not None:
+            if draft is self:
+                raise ValueError("assistant_model must be another model than the one generating: each owns one cache")
+            if draft._device() != self._device():
+                raise ValueError(f"assistant_model is on {draft._device()}, the model on {self._device()}")
+        return k, ngram
+
     # ------------------------------------------------------------------ entry point
     @torch.no_grad()
     def generate(self, inputs=None, max_length=None, min_length=None, do_sample=None, early_stopping=None,
@@ -512,7 +734,9 @@ class Generator:
                  num_beam_groups=None, diversity_penalty=None, prefix_allowed_tokens_fn=None, logits_processor=None,
                  renormalize_logits=None, stopping_criteria=None, constraints=None, output_scores=None,
                  forced_bos_token_id=None, forced_eos_token_id=None, remove_invalid_values=None,
-                 exponential_decay_length_penalty=None, kv_cache_dtype=None, decode_graphs=None, **model_kwargs):
+                 exponential_decay_length_penalty=None, kv_cache_dtype=None, decode_graphs=None, assistant_model=None,
+                 num_assistant_tokens=None, prompt_lookup_num_tokens=None, max_matching_ngram_size=None,
+                 **model_kwargs):
         """``kv_cache_dtype`` (default: the model cfg's ``kv_cache_dtype``): ``"fp8"`` or ``torch.float8_e4m3fn`` holds
         the preallocated KV cache as E4M3 rows with per-row scales
         (:class:`~libai_b200.inference.kv_cache.StaticKVCache`) for this call: about half the memory, and of the bytes
@@ -524,7 +748,15 @@ class Generator:
         eager decoding.  The first decode step of a new batch or cache runs eagerly and the next is captured; the
         graph holds a private memory pool while the cache lives, and Python hooks on modules do not run in a replayed
         step.  Steps the graph cannot reproduce run eagerly (logged once per reason).  A model that does not decode on
-        a ``StaticKVCache`` raises ``ValueError``."""
+        a ``StaticKVCache`` raises ``ValueError``.
+
+        Speculative decoding (:meth:`speculative_search`), greedy only: ``assistant_model`` (a second decoder-only
+        model on the same device, with the same logits width; ``num_assistant_tokens`` proposals per iteration, 1 to
+        15, default 4) or ``prompt_lookup_num_tokens`` (1 to 15 proposals from the sequence itself, matching n-grams of
+        up to ``max_matching_ngram_size`` tokens, default 2), not both.  ``kv_cache_dtype`` applies to this model, the
+        assistant's cfg sets its own; ``decode_graphs`` applies to both.  Sampling, beams, ``num_return_sequences > 1``,
+        logits processors, custom stopping criteria, encoder-decoder and GLM models, tensor or pipeline parallelism and
+        a prompt whose padding needs a dense mask raise ``ValueError``."""
         kv_cache_dtype = _kv_cache_dtype(self._pick(kv_cache_dtype, "kv_cache_dtype"))
         if kv_cache_dtype is not None and not isinstance(self, KVCacheOwner):
             raise ValueError(f"kv_cache_dtype={kv_cache_dtype}: {type(self).__name__} does not decode on a "
@@ -608,22 +840,46 @@ class Generator:
             exponential_decay_length_penalty=exponential_decay_length_penalty, logits_processor=logits_processor,
             renormalize_logits=renormalize_logits,
         )
+        custom_criteria = bool(stopping_criteria)
         stopping_criteria = self._get_stopping_criteria(max_length, max_time, stopping_criteria)
+        draft = assistant_model
+        speculative = draft is not None or prompt_lookup_num_tokens is not None
+        spec_k = 0
+        if speculative:
+            spec_k, max_matching_ngram_size = self._speculative_args(
+                draft, num_assistant_tokens, prompt_lookup_num_tokens, max_matching_ngram_size, do_sample, num_beams,
+                num_return_sequences, logits_processor, custom_criteria, is_enc_dec, stopping_criteria.max_length,
+                model_kwargs)
         saved_kv_cache_dtype = getattr(self, "kv_cache_dtype", None)
         was_training = self.training
         self.eval()
+        if draft is not None:
+            draft_state = (draft.training, getattr(draft, "kv_cache_dtype", None))
+            draft.eval()
         try:
             if kv_cache_dtype is not None:   # the cache format of this call (allocate_kv_cache reads it)
                 self.kv_cache_dtype = kv_cache_dtype
             if decode_graphs:
                 self._decode_graphs = decode_graph.DecodeCall()
+            if draft is not None:
+                draft.kv_cache_dtype = _kv_cache_dtype(draft._gcfg("kv_cache_dtype")) or draft_state[1]
+                if decode_graphs:
+                    draft._decode_graphs = decode_graph.DecodeCall()
+                # a verify step appends k + 1 rows and keeps n + 1 of them: room for k more than the output
+                draft.allocate_kv_cache(batch_size, stopping_criteria.max_length + spec_k)
             # models with a preallocated cache size it once for every sequence the search runs
             allocate = getattr(self, "allocate_kv_cache", None)
             if allocate is not None and model_kwargs.get("use_cache") and stopping_criteria.max_length is not None:
                 rows = batch_size * (num_beams if is_beam else num_return_sequences if is_sample else 1)
-                if allocate(rows, stopping_criteria.max_length) is None and kv_cache_dtype is not None:
+                if allocate(rows, stopping_criteria.max_length + spec_k) is None and kv_cache_dtype is not None:
                     raise ValueError(f"kv_cache_dtype={kv_cache_dtype}: {type(self).__name__} keeps a tuple cache "
                                      "here (pipeline-parallel inference), not a StaticKVCache")
+            if speculative:
+                return self.speculative_search(
+                    input_ids, assistant_model=draft, num_assistant_tokens=spec_k,
+                    prompt_lookup_num_tokens=spec_k if draft is None else None,
+                    max_matching_ngram_size=max_matching_ngram_size, stopping_criteria=stopping_criteria,
+                    pad_token_id=pad_token_id, eos_token_id=eos_token_id, output_scores=output_scores, **model_kwargs)
             if is_greedy:
                 if num_return_sequences > 1:
                     raise ValueError(f"num_return_sequences has to be 1, but is {num_return_sequences} when doing greedy search.")
@@ -659,3 +915,8 @@ class Generator:
                 self.kv_cache_dtype = saved_kv_cache_dtype
             if decode_graphs:
                 del self._decode_graphs   # back to the class's None
+            if draft is not None:
+                draft.train(draft_state[0])
+                draft.kv_cache_dtype = draft_state[1]
+                if decode_graphs:
+                    del draft._decode_graphs

@@ -301,6 +301,16 @@ class StaticKVCache:
         self.seqlens.add_(n)
         self.length += n
 
+    def rollback(self, n: int) -> None:
+        """Drop the last ``n`` rows of every sample (on the device in place, and in the host mirror): a speculative
+        verify step's rows past the accepted tokens.  Rows at or past ``seqlens`` are never read (an FP8 cache's
+        included), so nothing is cleared; the next append overwrites them."""
+        if not 0 <= n <= self.length:
+            raise ValueError(f"rollback: 0 <= n <= length ({self.length}), got {n}")
+        if n:
+            self.seqlens.sub_(n)
+            self.length -= n
+
     def reorder_(self, beam_idx: torch.Tensor) -> None:
         """Gather the samples along the batch dimension in place (beam search)."""
         idx = beam_idx.to(device=self.device, dtype=torch.long)

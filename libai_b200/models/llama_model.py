@@ -342,6 +342,7 @@ class SFTLoss(nn.Module):
 
 
 class LlamaForCausalLM(nn.Module, PipelineStageMixin, KVCacheOwner, Generator):
+    speculative_decoding = True
 
     # `train.dist.sequence_parallel = "auto"` resolves to True for this model (token-sharded activations between
     # the tensor-parallel blocks are handled by its embeddings / heads)

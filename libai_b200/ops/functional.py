@@ -416,6 +416,61 @@ def linear_int4w(x, w, w_scale, w_zero, bias=None, act: Optional[str] = None):
     return linear_int4w_ref(x, w, w_scale, w_zero, bias, act)
 
 
+# --------------------------------------------------------------------------------------
+# speculative decoding: greedy acceptance of one iteration (Generator.speculative_search)
+# --------------------------------------------------------------------------------------
+def spec_accept_ref(logits, draft, unfinished, eos: Optional[int] = None, pad: Optional[int] = None):
+    """The PyTorch mirror of :func:`spec_accept` (same outputs, ``unfinished`` updated in place)."""
+    b, R, _ = logits.shape
+    k = R - 1
+    t = logits.argmax(dim=-1)   # the first of equal maxima
+    match = (draft == t[:, :k]).long()
+    a = match.cumprod(dim=1).sum(dim=1) if k > 0 else torch.zeros(b, dtype=torch.long, device=logits.device)
+    live = unfinished != 0
+    if eos is not None:
+        upto = torch.arange(R, device=logits.device)[None, :] <= a[:, None]
+        live_a = torch.where(((t == eos) & upto).any(dim=1), k, a)
+    else:
+        live_a = a
+    n = int(live_a[live].min()) if bool(live.any()) else k
+    e = t.clone()
+    u = unfinished.clone()
+    for j in range(R):
+        if j > n:
+            e[:, j] = -1
+        elif eos is not None:
+            e[:, j] = torch.where(u != 0, t[:, j], pad)
+            u = u * (e[:, j] != eos).long()
+    unfinished.copy_(u)
+    nn_ = torch.full((b, 1), n, dtype=torch.long, device=logits.device)
+    return torch.cat([t, e, a[:, None], nn_, u[:, None]], dim=1)
+
+
+def spec_accept(logits, draft, unfinished, eos: Optional[int] = None, pad: Optional[int] = None):
+    """Greedy acceptance of one speculative-decoding iteration, in one launch of the sm_90a kernel on the GPU.
+
+    ``logits`` ``[b, k + 1, V]`` (bf16 or fp32, read in place): the verify step's rows after ``x, d_1 .. d_k``;
+    ``draft`` int64 ``[b, k]``: the proposals; ``unfinished`` int64 ``[b]``, updated in place.  With ``t_j`` the argmax
+    of row j (the lowest index among equal maxima, for finite or −inf logits):
+
+    - ``a_b``: the length of the longest prefix with ``draft[b, j] == t_j``;
+    - ``n``: the minimum of ``a_b`` over the samples unfinished on entry, a sample that emits ``eos`` among
+      ``t_0 .. t_{a_b}`` counting as k; k when none is unfinished;
+    - ``e_j``: ``t_j`` for ``j <= n`` while the sample is unfinished, ``pad`` once it is (emitting ``eos`` finishes it),
+      −1 for ``j > n``.  ``eos=None``: no EOS (``pad`` unused).
+
+    Returns int64 ``[b, 2(k + 1) + 3]``: columns ``[0, k + 1)`` t, ``[k + 1, 2(k + 1))`` e, then ``a_b``, ``n`` and the
+    updated ``unfinished``: everything the host needs, in one readback.  CPU tensors run :func:`spec_accept_ref`."""
+    if eos is not None and pad is None:
+        raise ValueError("spec_accept: eos needs a pad token")
+    if not use_native(logits):
+        return spec_accept_ref(logits, draft, unfinished, eos, pad)
+    out = load_ext().spec_accept(logits, draft, unfinished, -1 if eos is None else int(eos),
+                                 0 if pad is None else int(pad))
+    count_launch(1)
+    return out
+
+
 def matmul_nt(a, b):
     """``a @ b.T`` without autograd bookkeeping beyond PyTorch's (used by LM head on ref path)."""
     return linear(a, b)

@@ -194,6 +194,8 @@ class BloomModel(nn.Module):
 
 
 class BloomForCausalLM(nn.Module, KVCacheOwner, Generator):
+    speculative_decoding = True
+
     @configurable
     def __init__(self, cfg=None, **kwargs):
         super().__init__()

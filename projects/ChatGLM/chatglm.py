@@ -304,6 +304,8 @@ class ChatGLMModel(nn.Module, ChatGLMPreTrainedModel):
 
 
 class ChatGLMForConditionalGeneration(nn.Module, ChatGLMPreTrainedModel, KVCacheOwner, Generator):
+    speculative_decoding = True
+
     def __init__(self, cfg):
         super().__init__()
         self.cfg = cfg

@@ -13,6 +13,8 @@ from libai_b200.utils import distributed as dutil
 
 
 class GPTModel(core.GPTModel, Generator, KVCacheOwner):
+    speculative_decoding = True
+
     @configurable
     def __init__(self, *args, cfg=None, **kwargs):
         super().__init__(*args, **kwargs)
