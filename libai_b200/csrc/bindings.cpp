@@ -3,6 +3,7 @@
 // python ABI dependency).
 #include <ATen/cuda/CUDAContext.h>
 #include <ATen/cuda/CUDAGeneratorImpl.h>
+#include <cmath>
 #include <cstring>
 #include <mutex>
 #include <c10/cuda/CUDAGuard.h>
@@ -366,6 +367,72 @@ Tensor spec_accept(const Tensor& logits, const Tensor& draft, Tensor unfinished,
                        unfinished.data_ptr<int64_t>(), out, reinterpret_cast<unsigned int*>(out + B * cols), (int)B,
                        (int)R, (int)V, (long long)eos, (long long)pad, cur_stream()),
         "spec_accept");
+  return buf.narrow(0, 0, B * cols).view({B, cols});
+}
+
+// The warp arguments of speculative sampling: temperature > 0 (finite), top_k >= 0 (0: off), 0 < top_p <= 1.
+static void check_warp(const char* op, double temperature, int64_t top_k, double top_p) {
+  TORCH_CHECK(std::isfinite(temperature) && temperature > 0, op, ": temperature must be a finite float > 0, got ",
+              temperature);
+  TORCH_CHECK(top_k >= 0 && top_k <= INT32_MAX, op, ": top_k must be >= 0 (0: off), got ", top_k);
+  TORCH_CHECK(top_p > 0 && top_p <= 1, op, ": top_p must be in (0, 1], got ", top_p);
+}
+
+// One draft step of speculative sampling (speculative_sm90.cu): logits bf16 or fp32 [b, V] (contiguous) is kept in
+// q[:, j] (q [b, K, V], the same dtype) and proposals[:, j] (int64 [b, J]) is drawn from its warped distribution with
+// the uniforms u[:, j] (fp32 [b, J]).
+void spec_sample(const Tensor& logits, Tensor q, int64_t j, const Tensor& u, Tensor proposals, double temperature,
+                 int64_t top_k, double top_p) {
+  Args args("spec_sample");
+  args("logits", logits, Dtypes(at::kBFloat16, at::kFloat), {kAny, kAny});
+  const int64_t B = logits.size(0), V = logits.size(1);
+  TORCH_CHECK(B >= 1 && V >= 1 && V <= INT32_MAX, "spec_sample: logits [b, V] needs b >= 1 and V >= 1, got ",
+              logits.sizes());
+  args("q", q, logits.scalar_type(), {B, kAny, V});
+  args("proposals", proposals, at::kLong, {B, kAny});
+  const int64_t K = q.size(1), J = proposals.size(1);
+  args("u", u, at::kFloat, {B, J});
+  TORCH_CHECK(j >= 0 && j < K && j < J, "spec_sample: column j = ", j, " must be below q's ", K, " and proposals' ", J);
+  check_warp("spec_sample", temperature, top_k, top_p);
+  const auto guard = args.guard();
+  check(lb_spec_sample(logits.data_ptr(), q.data_ptr(), logits.scalar_type() == at::kFloat ? 1 : 0, u.data_ptr<float>(),
+                       proposals.data_ptr<int64_t>(), (int)B, (int)V, (int)K, (int)J, (int)j, (float)temperature,
+                       (int)top_k, (float)top_p, cur_stream()),
+        "spec_sample");
+}
+
+// One speculative-sampling iteration's acceptance (speculative_sm90.cu): logits bf16 or fp32 [b, R, V], q bf16 or
+// fp32 [b, K, V] (the draft's rows, K >= R - 1), draft int64 [b, R - 1], u fp32 [b, R, 2], unfinished int64 [b]
+// (updated in place), scores (optional) fp32 [b, R, V], written with the target's warped logits.  Returns out int64
+// [b, 2R + 3] laid out as spec_accept's.  The per-row decisions and the block counter live past out in its allocation.
+Tensor spec_accept_sample(const Tensor& logits, const Tensor& q, const Tensor& draft, const Tensor& u,
+                          Tensor unfinished, double temperature, int64_t top_k, double top_p, int64_t eos, int64_t pad,
+                          c10::optional<Tensor> scores) {
+  Args args("spec_accept_sample");
+  args("logits", logits, Dtypes(at::kBFloat16, at::kFloat), {kAny, kAny, kAny});
+  const int64_t B = logits.size(0), R = logits.size(1), V = logits.size(2);
+  TORCH_CHECK(B >= 1 && R >= 1 && R <= 16 && V >= 1 && V <= INT32_MAX, "spec_accept_sample: logits [b, k + 1, V] ",
+              "needs b >= 1, 1 <= k + 1 <= 16 and V >= 1, got ", logits.sizes());
+  args("q", q, Dtypes(at::kBFloat16, at::kFloat), {B, kAny, V});
+  TORCH_CHECK(q.size(1) >= R - 1, "spec_accept_sample: q holds ", q.size(1), " draft rows, the iteration needs ", R - 1);
+  args("draft", draft, at::kLong, {B, R - 1});
+  args("u", u, at::kFloat, {B, R, 2});
+  args("unfinished", unfinished, at::kLong, {B});
+  float* scores_ptr = args.opt<float>("scores", scores, at::kFloat, {B, R, V});
+  check_warp("spec_accept_sample", temperature, top_k, top_p);
+  const auto guard = args.guard();
+  const int64_t cols = 2 * R + 3;
+  // out, then B·R int32 decisions (B·R / 2 + 1 int64 slots) and the counter
+  Tensor buf = at::empty({B * cols + (B * R) / 2 + 2}, draft.options());
+  int64_t* out = buf.data_ptr<int64_t>();
+  int* accepted = reinterpret_cast<int*>(out + B * cols);
+  unsigned int* counter = reinterpret_cast<unsigned int*>(out + B * cols + (B * R) / 2 + 1);
+  check(lb_spec_accept_sample(logits.data_ptr(), logits.scalar_type() == at::kFloat ? 1 : 0, q.data_ptr(),
+                              q.scalar_type() == at::kFloat ? 1 : 0, draft.data_ptr<int64_t>(), u.data_ptr<float>(),
+                              unfinished.data_ptr<int64_t>(), out, accepted, counter, scores_ptr, (int)B, (int)R,
+                              (int)V, (int)q.size(1), (float)temperature, (int)top_k, (float)top_p, (long long)eos,
+                              (long long)pad, cur_stream()),
+        "spec_accept_sample");
   return buf.narrow(0, 0, B * cols).view({B, cols});
 }
 
@@ -1390,6 +1457,10 @@ TORCH_LIBRARY(libai_b200, m) {
         &linear_int4w);
   m.def("dequant_int4_rows(Tensor w, Tensor w_scale, Tensor w_zero) -> Tensor", &dequant_int4_rows);
   m.def("spec_accept(Tensor logits, Tensor draft, Tensor(a!) unfinished, int eos, int pad) -> Tensor", &spec_accept);
+  m.def("spec_sample(Tensor logits, Tensor(a!) q, int j, Tensor u, Tensor(b!) proposals, float temperature, int top_k, "
+        "float top_p) -> ()", &spec_sample);
+  m.def("spec_accept_sample(Tensor logits, Tensor q, Tensor draft, Tensor u, Tensor(a!) unfinished, float temperature, "
+        "int top_k, float top_p, int eos, int pad, Tensor(b!)? scores=None) -> Tensor", &spec_accept_sample);
   m.def("linear_fp8_fwd(Tensor xq, Tensor wq, Tensor deq_x, Tensor deq_w, Tensor? bias, int act, bool need_pre, Tensor? residual=None, int bn=0) -> (Tensor, Tensor)", &linear_fp8_fwd);
   m.def("act_bwd(Tensor gy, Tensor pre, int act) -> Tensor", &act_bwd);
   m.def("colsum(Tensor x, Tensor(a!)? accum=None) -> Tensor", &colsum);

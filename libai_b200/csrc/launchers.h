@@ -168,6 +168,19 @@ int lb_dequant_int4_rows(const void* w, const void* w_scale, const void* w_zero,
 // this launch's own, zeroed on the stream before the kernel.  eos < 0: no EOS.
 int lb_spec_accept(const void* logits, int logits_fp32, const int64_t* draft, int64_t* unfinished, int64_t* out,
                    unsigned int* counter, int B, int R, int V, long long eos, long long pad, cudaStream_t s);
+// Speculative sampling (speculative_sm90.cu, the warp rule of sampling.cuh).  lb_spec_sample, after draft step j:
+// logits [B, V] (bf16, or fp32 with fp32 = 1) is copied to qbuf[:, j] ([B, K, V], the same dtype) and
+// proposals[:, j] ([B, J] int64) is drawn from its warped distribution with u[:, j] ([B, J] fp32).
+int lb_spec_sample(const void* logits, void* qbuf, int fp32, const float* u, int64_t* proposals, int B, int V, int K,
+                   int J, int j, float temperature, int top_k, float top_p, cudaStream_t s);
+// The acceptance of one speculative-sampling iteration: logits [B, R, V], qbuf [B, K, V] (K >= R - 1; each bf16 or
+// fp32), draft int64 [B, R - 1], u fp32 [B, R, 2], unfinished int64 [B] (updated in place), out int64 [B, 2R + 3] as
+// lb_spec_accept's; accepted: B·R ints of scratch; counter: a uint32 of this launch's own; scores: fp32 [B, R, V] or
+// null.  eos < 0: no EOS.
+int lb_spec_accept_sample(const void* logits, int logits_fp32, const void* qbuf, int q_fp32, const int64_t* draft,
+                          const float* u, int64_t* unfinished, int64_t* out, int* accepted, unsigned int* counter,
+                          float* scores, int B, int R, int V, int K, float temperature, int top_k, float top_p,
+                          long long eos, long long pad, cudaStream_t s);
 int lb_window_attn_groups(int B, int H, int W, int ws, int heads);
 int lb_window_attn_fwd(const void* qkv, void* out, float* lse, const float* table, const float* tau, int B, int H, int W,
                        int ws, int shift, int heads, int d, float scale, cudaStream_t s);

@@ -143,3 +143,188 @@ int lb_spec_accept(const void* logits, int logits_fp32, const int64_t* draft, in
 }
 
 }  // extern "C"
+
+// ------------------------------------------------------------------------------------------------------------------
+// Speculative sampling (Leviathan et al. 2023; Chen et al. 2023): the draft samples its proposals from its warped
+// distribution q, the target accepts d with probability min(1, p(d) / q(d)) and replaces the first rejected proposal
+// by a draw from norm(max(0, p − q)).  The warp rule (temperature, top-k, top-p, fixed-point masses, the inverse-CDF
+// pick) is sampling.cuh's, one CTA per row.
+//
+// spec_sample: after draft step j, per sample b: q_j[b] = the step's logits row, kept in qbuf[b, j] (q itself is never
+// materialised), and d_{j+1} = pick(floor(u[b, j] · Σe)) over q_j's masses, written to proposals[b, j].
+//
+// spec_accept_sample, phase 1, one CTA per row (b, j) of the verify step's logits [B, R, V] (R = k + 1):
+//   accept_j = u[b, j, 0] · q_j(d_{j+1}) < p_j(d_{j+1})                         (j < k, in fp64 from the masses)
+//   c_j      = pick(floor(u[b, j, 1] · Σr)) over r_i = 2^40 · max(0, p_j(i) − q_j(i)), rounded (j < k, Σr > 0);
+//              pick over p_j's masses when Σr = 0 or j = k (the bonus token)
+// phase 2, the last CTA (the counter pattern of spec_accept): a_b = the first rejected j (k if none); t_j = d_{j+1}
+// for j < a_b, else c_j; then n, e and unfinished as spec_accept defines them from t.  scores (optional, fp32
+// [B, R, V]): the target's warped logits, z on the kept set and −inf elsewhere.
+#include "sampling.cuh"
+
+namespace lb {
+namespace spec {
+
+using samp::Row;
+using samp::Warped;
+
+template <typename T>
+__global__ void __launch_bounds__(samp::kThreads, 1) sample_kernel(const T* __restrict__ logits, T* __restrict__ qbuf,
+                                                                const float* __restrict__ u,
+                                                                int64_t* __restrict__ proposals, int V, int K, int J,
+                                                                int j, float temperature, int top_k, float top_p) {
+  __shared__ samp::Shared sh;
+  const int b = blockIdx.x;
+  const T* x = logits + (size_t)b * V;
+  T* q = qbuf + ((size_t)b * K + j) * V;
+  for (int i = threadIdx.x; i < V; i += samp::kThreads) q[i] = x[i];
+  const Row<T> row{x, temperature};
+  const Warped w = samp::warp_row(row, V, top_k, top_p, sh);
+  const int d = samp::pick([row, w](int i) { return samp::mass_of(row, w, i); }, V,
+                           samp::draw(u[(size_t)b * J + j], w.total), sh);
+  if (threadIdx.x == 0) proposals[(size_t)b * J + j] = d;
+}
+
+template <typename TP, typename TQ>
+__global__ void __launch_bounds__(samp::kThreads, 1) accept_sample_kernel(
+    const TP* __restrict__ logits, const TQ* __restrict__ qbuf, const int64_t* __restrict__ draft,
+    const float* __restrict__ u, int64_t* __restrict__ unfinished, int64_t* __restrict__ out, int* __restrict__ accepted,
+    unsigned int* __restrict__ counter, float* __restrict__ scores, int B, int R, int V, int K, float temperature,
+    int top_k, float top_p, long long eos, long long pad) {
+  __shared__ samp::Shared sh;
+  __shared__ bool s_last;
+  __shared__ int s_n;
+  const int row_id = blockIdx.x;   // b * R + j
+  const int b = row_id / R, j = row_id % R, k = R - 1;
+  const int cols = 2 * R + 3;
+  const Row<TP> p_row{logits + (size_t)row_id * V, temperature};
+  const Warped pw = samp::warp_row(p_row, V, top_k, top_p, sh);
+  const float u0 = u[(size_t)row_id * 2], u1 = u[(size_t)row_id * 2 + 1];
+  int cand;
+  if (j < k) {
+    const Row<TQ> q_row{qbuf + ((size_t)b * K + j) * V, temperature};
+    const Warped qw = samp::warp_row(q_row, V, top_k, top_p, sh);
+    const double inv_p = 1.0 / (double)pw.total, inv_q = 1.0 / (double)qw.total;
+    if (threadIdx.x == 0) {
+      const int64_t d = draft[(size_t)b * k + j];
+      bool acc = false;
+      if (d >= 0 && d < V) {
+        const double pd = (double)samp::mass_of(p_row, pw, (int)d) * inv_p;
+        const double qd = (double)samp::mass_of(q_row, qw, (int)d) * inv_q;
+        acc = (double)u0 * qd < pd;
+      }
+      accepted[row_id] = acc;
+    }
+    auto resid = [&](int i) {
+      const double r = (double)samp::mass_of(p_row, pw, i) * inv_p - (double)samp::mass_of(q_row, qw, i) * inv_q;
+      return r > 0.0 ? __double2ull_rn(r * samp::kOneD) : 0ull;
+    };
+    unsigned long long s = 0;
+    for (int i = threadIdx.x; i < V; i += samp::kThreads) s += resid(i);
+    const unsigned long long total = samp::block_sum(s, sh);
+    if (total > 0)
+      cand = samp::pick(resid, V, samp::draw(u1, total), sh);
+    else
+      cand = samp::pick([&](int i) { return samp::mass_of(p_row, pw, i); }, V, samp::draw(u1, pw.total), sh);
+  } else {
+    if (threadIdx.x == 0) accepted[row_id] = 0;
+    cand = samp::pick([&](int i) { return samp::mass_of(p_row, pw, i); }, V, samp::draw(u1, pw.total), sh);
+  }
+  if (scores != nullptr) {
+    float* o = scores + (size_t)row_id * V;
+    for (int i = threadIdx.x; i < V; i += samp::kThreads) {
+      const float z = p_row.z(i);
+      o[i] = samp::key_of(z) >= pw.keep ? z : -INFINITY;
+    }
+  }
+  if (threadIdx.x == 0) {
+    out[(size_t)b * cols + j] = cand;
+    __threadfence();
+    s_last = atomicAdd(counter, 1u) == (unsigned)(gridDim.x - 1);
+  }
+  __syncthreads();
+  if (!s_last) return;
+
+  // phase 2: the last block sees every row's decision and candidate
+  __threadfence();
+  if (threadIdx.x == 0) s_n = k;
+  __syncthreads();
+  for (int bb = threadIdx.x; bb < B; bb += samp::kThreads) {
+    volatile int64_t* t = out + (size_t)bb * cols;
+    const volatile int* acc = accepted + (size_t)bb * R;
+    int a = 0;
+    while (a < k && acc[a]) ++a;
+    for (int jj = 0; jj < a; ++jj) t[jj] = draft[(size_t)bb * k + jj];
+    out[(size_t)bb * cols + 2 * R] = a;
+    if (unfinished[bb] != 0) {
+      bool ends = false;
+      for (int jj = 0; jj <= a && eos >= 0; ++jj) ends |= t[jj] == eos;
+      atomicMin(&s_n, ends ? k : a);
+    }
+  }
+  __syncthreads();
+  const int n = s_n;
+  for (int bb = threadIdx.x; bb < B; bb += samp::kThreads) {
+    int64_t* o = out + (size_t)bb * cols;
+    const volatile int64_t* t = o;
+    int64_t uf = unfinished[bb];
+    for (int jj = 0; jj < R; ++jj) {
+      int64_t e = -1;
+      if (jj <= n) {
+        e = t[jj];
+        if (eos >= 0) {
+          if (uf == 0) e = pad;
+          if (e == eos) uf = 0;
+        }
+      }
+      o[R + jj] = e;
+    }
+    o[2 * R + 1] = n;
+    o[2 * R + 2] = uf;
+    unfinished[bb] = uf;
+  }
+}
+
+}  // namespace spec
+}  // namespace lb
+
+extern "C" {
+
+int lb_spec_sample(const void* logits, void* qbuf, int fp32, const float* u, int64_t* proposals, int B, int V, int K,
+                   int J, int j, float temperature, int top_k, float top_p, cudaStream_t s) {
+  using namespace lb::spec;
+  if (B < 1 || V < 1 || K < 1 || J < 1 || j < 0 || j >= K || j >= J) return static_cast<int>(cudaErrorInvalidValue);
+  if (fp32)
+    sample_kernel<float><<<B, lb::samp::kThreads, 0, s>>>(static_cast<const float*>(logits), static_cast<float*>(qbuf),
+                                                          u, proposals, V, K, J, j, temperature, top_k, top_p);
+  else
+    sample_kernel<__nv_bfloat16><<<B, lb::samp::kThreads, 0, s>>>(
+        static_cast<const __nv_bfloat16*>(logits), static_cast<__nv_bfloat16*>(qbuf), u, proposals, V, K, J, j,
+        temperature, top_k, top_p);
+  return static_cast<int>(cudaGetLastError());
+}
+
+int lb_spec_accept_sample(const void* logits, int logits_fp32, const void* qbuf, int q_fp32, const int64_t* draft,
+                          const float* u, int64_t* unfinished, int64_t* out, int* accepted, unsigned int* counter,
+                          float* scores, int B, int R, int V, int K, float temperature, int top_k, float top_p,
+                          long long eos, long long pad, cudaStream_t s) {
+  using namespace lb::spec;
+  if (B < 1 || R < 1 || V < 1 || K < R - 1 || (long long)B * R > 0x7fffffffLL)
+    return static_cast<int>(cudaErrorInvalidValue);
+  const cudaError_t e = cudaMemsetAsync(counter, 0, sizeof(unsigned int), s);
+  if (e != cudaSuccess) return static_cast<int>(e);
+  const unsigned grid = (unsigned)(B * R);
+  constexpr int nt = lb::samp::kThreads;
+#define LB_ACCEPT_SAMPLE(TP, TQ)                                                                                       \
+  accept_sample_kernel<TP, TQ><<<grid, nt, 0, s>>>(static_cast<const TP*>(logits), static_cast<const TQ*>(qbuf), draft, \
+                                                   u, unfinished, out, accepted, counter, scores, B, R, V, K,           \
+                                                   temperature, top_k, top_p, eos, pad)
+  if (logits_fp32 && q_fp32) LB_ACCEPT_SAMPLE(float, float);
+  else if (logits_fp32) LB_ACCEPT_SAMPLE(float, __nv_bfloat16);
+  else if (q_fp32) LB_ACCEPT_SAMPLE(__nv_bfloat16, float);
+  else LB_ACCEPT_SAMPLE(__nv_bfloat16, __nv_bfloat16);
+#undef LB_ACCEPT_SAMPLE
+  return static_cast<int>(cudaGetLastError());
+}
+
+}  // extern "C"

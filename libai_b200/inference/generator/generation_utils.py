@@ -551,10 +551,11 @@ class Generator:
     @torch.no_grad()
     def speculative_search(self, input_ids, assistant_model=None, num_assistant_tokens=4, prompt_lookup_num_tokens=None,
                            max_matching_ngram_size=2, stopping_criteria=None, pad_token_id=None, eos_token_id=None,
-                           output_scores=False, **model_kwargs):
-        """Greedy speculative decoding: proposals from ``assistant_model`` (a draft model, ``num_assistant_tokens`` per
+                           output_scores=False, warp=None, **model_kwargs):
+        """Speculative decoding: proposals from ``assistant_model`` (a draft model, ``num_assistant_tokens`` per
         iteration) or from prompt lookup (``prompt_lookup_num_tokens``, :func:`prompt_lookup`), verified in one cached
-        step of this model.
+        step of this model.  Greedy, or speculative sampling with ``warp=(temperature, top_k, top_p)`` (a draft model
+        only; below).
 
         One iteration, x the last emitted token: propose d_1 .. d_k; run the target on ``[x, d_1 .. d_k]``; accept, per
         sample, the longest prefix of the proposals equal to the target's argmaxes; advance the whole batch by the
@@ -574,13 +575,28 @@ class Generator:
         the target drops the rows past the accepted tokens (``StaticKVCache.rollback``); the draft, which only takes
         single-token steps, rolls back too, or, when all k were accepted, feeds d_k at the start of the next
         iteration.  Both caches hold ``max_length + k`` rows (``generate`` sizes them).  Near a model's maximum
-        positions k shrinks so that no step writes past them; those steps run eagerly under decode graphs."""
+        positions k shrinks so that no step writes past them; those steps run eagerly under decode graphs.
+
+        Speculative sampling (``warp`` given; Leviathan et al. 2023, Chen et al. 2023): p and q are the target's and
+        the draft's distributions under one warp rule (temperature, top-k, top-p: :func:`OF.spec_warp_ref`).  After
+        each of its k single-token steps the draft samples d_{j+1} ~ q_j on the device (:func:`OF.spec_sample`, uniforms
+        ``[b, k]`` from ``torch.rand``) and keeps its logits row; after the verify step :func:`OF.spec_accept_sample`
+        accepts d_{j+1} with probability min(1, p_j/q_j) and replaces the first rejected one by a draw from
+        norm(max(0, p_j − q_j)), or draws a bonus token from p_k when all are accepted (uniforms ``[b, k + 1, 2]``).
+        The batch advances by the same n and the caches roll back as above.  Every emitted token is distributed as p
+        given its prefix, whatever the draft is.  Each iteration draws a fixed number of uniforms from the default
+        generator, so ``torch.manual_seed`` reproduces a call, eagerly or under decode graphs.  ``output_scores``
+        holds the target's warped logits (z on the kept set, −inf elsewhere), as ``multinomial_sample`` reports them."""
         stopping_criteria = stopping_criteria if stopping_criteria is not None else StoppingCriteriaList()
         draft = assistant_model
         k = num_assistant_tokens if draft is not None else prompt_lookup_num_tokens
         max_length = stopping_criteria.max_length
         b, dev = input_ids.shape[0], input_ids.device
         scores = () if output_scores else None
+        sample = warp is not None
+        if sample and draft is None:
+            raise ValueError("do_sample: speculative sampling needs an assistant_model (prompt lookup has no proposal "
+                             "distribution)")
 
         outputs = self._decode_step(input_ids, model_kwargs)
         cache = self.kv_cache
@@ -602,6 +618,8 @@ class Generator:
                 raise ValueError("attention_mask: the assistant's cache needs a dense mask for this prompt")
             draft_kwargs["past"] = draft.kv_cache
             draft_extra = draft.kv_cache.length - input_ids.shape[1]
+            if sample:   # the draft's logits rows of an iteration, from which the acceptance recomputes q
+                qbuf = torch.empty(b, k, rows.shape[-1], dtype=draft._all_logits(draft_out).dtype, device=dev)
         history = staging = None
         if draft is None:
             history = input_ids.tolist()
@@ -612,7 +630,13 @@ class Generator:
         host_unfinished = [1] * b
         while True:
             R = rows.shape[1]
-            res = OF.spec_accept(rows, proposals, unfinished, eos_token_id, pad_token_id)
+            if sample:
+                u = torch.rand(b, R, 2, device=dev)
+                warped = torch.empty(rows.shape, dtype=torch.float32, device=dev) if output_scores else None
+                res = OF.spec_accept_sample(rows, qbuf, proposals, u, unfinished, *warp, eos_token_id, pad_token_id,
+                                            warped)
+            else:
+                res = OF.spec_accept(rows, proposals, unfinished, eos_token_id, pad_token_id)
             host = res.tolist()   # the iteration's one readback
             n = host[0][2 * R + 1]
             count = n + 1
@@ -627,7 +651,7 @@ class Generator:
                         break
             input_ids = torch.cat([input_ids, res[:, R : R + count]], dim=-1)
             if output_scores:
-                scores += tuple(rows[:, j].float() for j in range(count))
+                scores += tuple(warped[:, j] if sample else rows[:, j].float() for j in range(count))
             if history is not None:
                 for i in range(b):
                     history[i].extend(host[i][R : R + count])
@@ -654,7 +678,14 @@ class Generator:
             kk = max(kk, 0)
 
             x = input_ids[:, -1:]
-            if draft is not None:
+            if sample:
+                ud = torch.rand(b, kk, device=dev)
+                proposals, tok = input_ids.new_empty(b, kk), x
+                for j in range(kk):
+                    step = self._all_logits(draft._decode_step(tok, draft_kwargs))[:, -1]
+                    OF.spec_sample(step, qbuf, j, ud, proposals, *warp)
+                    tok = proposals[:, j : j + 1].contiguous()
+            elif draft is not None:
                 tok, props = x, []
                 for _ in range(kk):
                     tok = self._all_logits(draft._decode_step(tok, draft_kwargs))[:, -1].argmax(dim=-1, keepdim=True)
@@ -677,8 +708,9 @@ class Generator:
 
     def _speculative_args(self, draft, num_assistant_tokens, prompt_lookup_num_tokens, max_matching_ngram_size,
                           do_sample, num_beams, num_return_sequences, processors, custom_criteria, is_enc_dec,
-                          max_length, model_kwargs):
-        """Check a speculative ``generate()`` call; returns ``(k, max_matching_ngram_size)``."""
+                          max_length, model_kwargs, temperature=None, top_k=None, top_p=None, typical_p=None):
+        """Check a speculative ``generate()`` call; returns ``(k, max_matching_ngram_size, warp)``, warp the
+        ``(temperature, top_k, top_p)`` of speculative sampling (None when greedy)."""
         if draft is not None and prompt_lookup_num_tokens is not None:
             raise ValueError("assistant_model and prompt_lookup_num_tokens: give one proposer, not both")
         name = "assistant_model" if draft is not None else "prompt_lookup_num_tokens"
@@ -690,12 +722,28 @@ class Generator:
         ngram = 2 if max_matching_ngram_size is None else max_matching_ngram_size
         if draft is None and (isinstance(ngram, bool) or not isinstance(ngram, int) or ngram < 1):
             raise ValueError(f"max_matching_ngram_size must be a positive int, got {ngram!r}")
-        if do_sample:
-            raise ValueError(f"{name}: speculative decoding is greedy; do_sample=True is not supported")
+        if do_sample and draft is None:
+            raise ValueError(f"{name}: do_sample=True needs an assistant_model; prompt lookup has no proposal "
+                             "distribution to sample from")
         if num_beams != 1:
-            raise ValueError(f"{name}: speculative decoding is greedy; num_beams={num_beams} is not supported")
-        if num_return_sequences != 1:
-            raise ValueError(f"{name}: num_return_sequences={num_return_sequences} is not supported")
+            raise ValueError(f"{name}: speculative decoding does not search beams; num_beams={num_beams} is not "
+                             "supported")
+        if num_return_sequences != 1 and not do_sample:
+            raise ValueError(f"{name}: num_return_sequences={num_return_sequences} needs do_sample=True")
+        warp = None
+        if do_sample:
+            # the warpers multinomial_sample would apply, validated by their classes; the kernels apply the same rule
+            self._get_logits_warper(top_k, top_p, typical_p, temperature, num_beams)
+            typical_p = self._pick(typical_p, "typical_p")
+            if typical_p is not None and typical_p < 1.0:
+                raise ValueError(f"{name}: speculative sampling applies temperature, top_k and top_p; "
+                                 f"typical_p={typical_p} is not supported")
+            temperature, top_k, top_p = (self._pick(v, key) for v, key in ((temperature, "temperature"),
+                                                                            (top_k, "top_k"), (top_p, "top_p")))
+            top_p = 1.0 if top_p is None or top_p >= 1.0 else float(top_p)
+            if not top_p > 0:
+                raise ValueError(f"{name}: speculative sampling needs top_p > 0, got {top_p}")
+            warp = (1.0 if temperature is None else float(temperature), 0 if top_k is None else int(top_k), top_p)
         if processors:
             names = sorted({_PROCESSOR_ARGS.get(type(p), "logits_processor") for p in processors})
             raise ValueError(f"{name}: speculative decoding applies no logits processor; drop {', '.join(names)}")
@@ -722,7 +770,7 @@ class Generator:
                 raise ValueError("assistant_model must be another model than the one generating: each owns one cache")
             if draft._device() != self._device():
                 raise ValueError(f"assistant_model is on {draft._device()}, the model on {self._device()}")
-        return k, ngram
+        return k, ngram, warp
 
     # ------------------------------------------------------------------ entry point
     @torch.no_grad()
@@ -750,13 +798,17 @@ class Generator:
         step.  Steps the graph cannot reproduce run eagerly (logged once per reason).  A model that does not decode on
         a ``StaticKVCache`` raises ``ValueError``.
 
-        Speculative decoding (:meth:`speculative_search`), greedy only: ``assistant_model`` (a second decoder-only
+        Speculative decoding (:meth:`speculative_search`): ``assistant_model`` (a second decoder-only
         model on the same device, with the same logits width; ``num_assistant_tokens`` proposals per iteration, 1 to
         15, default 4) or ``prompt_lookup_num_tokens`` (1 to 15 proposals from the sequence itself, matching n-grams of
         up to ``max_matching_ngram_size`` tokens, default 2), not both.  ``kv_cache_dtype`` applies to this model, the
-        assistant's cfg sets its own; ``decode_graphs`` applies to both.  Sampling, beams, ``num_return_sequences > 1``,
-        logits processors, custom stopping criteria, encoder-decoder and GLM models, tensor or pipeline parallelism and
-        a prompt whose padding needs a dense mask raise ``ValueError``."""
+        assistant's cfg sets its own; ``decode_graphs`` applies to both.  Greedy, or with ``do_sample=True`` and an
+        ``assistant_model``, speculative sampling: ``temperature``, ``top_k`` and ``top_p`` (``generate()``'s defaults,
+        so top-k 50) warp both models' logits, and the output follows the target's warped distribution exactly;
+        ``num_return_sequences`` expands the inputs as ``multinomial_sample`` does.  Beams, ``typical_p < 1``,
+        ``do_sample`` with prompt lookup, ``num_return_sequences > 1`` without sampling, logits processors (including
+        ``renormalize_logits``), custom stopping criteria, encoder-decoder and GLM models, tensor or pipeline
+        parallelism and a prompt whose padding needs a dense mask raise ``ValueError``."""
         kv_cache_dtype = _kv_cache_dtype(self._pick(kv_cache_dtype, "kv_cache_dtype"))
         if kv_cache_dtype is not None and not isinstance(self, KVCacheOwner):
             raise ValueError(f"kv_cache_dtype={kv_cache_dtype}: {type(self).__name__} does not decode on a "
@@ -844,12 +896,12 @@ class Generator:
         stopping_criteria = self._get_stopping_criteria(max_length, max_time, stopping_criteria)
         draft = assistant_model
         speculative = draft is not None or prompt_lookup_num_tokens is not None
-        spec_k = 0
+        spec_k, spec_warp = 0, None
         if speculative:
-            spec_k, max_matching_ngram_size = self._speculative_args(
+            spec_k, max_matching_ngram_size, spec_warp = self._speculative_args(
                 draft, num_assistant_tokens, prompt_lookup_num_tokens, max_matching_ngram_size, do_sample, num_beams,
                 num_return_sequences, logits_processor, custom_criteria, is_enc_dec, stopping_criteria.max_length,
-                model_kwargs)
+                model_kwargs, temperature=temperature, top_k=top_k, top_p=top_p, typical_p=typical_p)
         saved_kv_cache_dtype = getattr(self, "kv_cache_dtype", None)
         was_training = self.training
         self.eval()
@@ -866,7 +918,8 @@ class Generator:
                 if decode_graphs:
                     draft._decode_graphs = decode_graph.DecodeCall()
                 # a verify step appends k + 1 rows and keeps n + 1 of them: room for k more than the output
-                draft.allocate_kv_cache(batch_size, stopping_criteria.max_length + spec_k)
+                draft.allocate_kv_cache(batch_size * (num_return_sequences if is_sample else 1),
+                                        stopping_criteria.max_length + spec_k)
             # models with a preallocated cache size it once for every sequence the search runs
             allocate = getattr(self, "allocate_kv_cache", None)
             if allocate is not None and model_kwargs.get("use_cache") and stopping_criteria.max_length is not None:
@@ -875,11 +928,15 @@ class Generator:
                     raise ValueError(f"kv_cache_dtype={kv_cache_dtype}: {type(self).__name__} keeps a tuple cache "
                                      "here (pipeline-parallel inference), not a StaticKVCache")
             if speculative:
+                if is_sample:   # as multinomial_sample expands them
+                    input_ids, model_kwargs = self._expand_inputs_for_generation(
+                        input_ids, expand_size=num_return_sequences, is_encoder_decoder=is_enc_dec, **model_kwargs)
                 return self.speculative_search(
                     input_ids, assistant_model=draft, num_assistant_tokens=spec_k,
                     prompt_lookup_num_tokens=spec_k if draft is None else None,
                     max_matching_ngram_size=max_matching_ngram_size, stopping_criteria=stopping_criteria,
-                    pad_token_id=pad_token_id, eos_token_id=eos_token_id, output_scores=output_scores, **model_kwargs)
+                    pad_token_id=pad_token_id, eos_token_id=eos_token_id, output_scores=output_scores, warp=spec_warp,
+                    **model_kwargs)
             if is_greedy:
                 if num_return_sequences > 1:
                     raise ValueError(f"num_return_sequences has to be 1, but is {num_return_sequences} when doing greedy search.")

@@ -433,6 +433,13 @@ def spec_accept_ref(logits, draft, unfinished, eos: Optional[int] = None, pad: O
     else:
         live_a = a
     n = int(live_a[live].min()) if bool(live.any()) else k
+    return _spec_emit(t, a, n, unfinished, eos, pad)
+
+
+def _spec_emit(t, a, n: int, unfinished, eos, pad):
+    """The emitted tokens e of one speculative iteration from its tokens t [b, R], a_b and n (``unfinished`` updated in
+    place): the ``[b, 2R + 3]`` output of :func:`spec_accept` and :func:`spec_accept_sample`."""
+    b, R = t.shape
     e = t.clone()
     u = unfinished.clone()
     for j in range(R):
@@ -442,7 +449,7 @@ def spec_accept_ref(logits, draft, unfinished, eos: Optional[int] = None, pad: O
             e[:, j] = torch.where(u != 0, t[:, j], pad)
             u = u * (e[:, j] != eos).long()
     unfinished.copy_(u)
-    nn_ = torch.full((b, 1), n, dtype=torch.long, device=logits.device)
+    nn_ = torch.full((b, 1), n, dtype=torch.long, device=t.device)
     return torch.cat([t, e, a[:, None], nn_, u[:, None]], dim=1)
 
 
@@ -467,6 +474,182 @@ def spec_accept(logits, draft, unfinished, eos: Optional[int] = None, pad: Optio
         return spec_accept_ref(logits, draft, unfinished, eos, pad)
     out = load_ext().spec_accept(logits, draft, unfinished, -1 if eos is None else int(eos),
                                  0 if pad is None else int(pad))
+    count_launch(1)
+    return out
+
+
+# --------------------------------------------------------------------------------------
+# speculative sampling: the warp rule, the draft's draws and the acceptance of one iteration
+# --------------------------------------------------------------------------------------
+# the fp32 margin within which the mirrors flag a decision as a boundary case: the kernels compute the masses from
+# fp32 exponentials and 2^-40 fixed-point sums, the mirrors in fp64, so a decision this close may go either way
+SPEC_SAMPLE_MARGIN = 1e-5
+
+
+def _f32(x: float) -> float:
+    return float(torch.tensor(x, dtype=torch.float32))
+
+
+def _warp64(logits, temperature: float, top_k: int, top_p: float):
+    """The warp rule on rows ``logits [..., V]``: ``(z, keep, p, gap)``.  z: the fp32 ``logits / T``; keep: the final
+    kept set; p: fp64 probabilities on it (0 elsewhere); gap: per row, the distance of the nearest top-p mass above a
+    token to ``top_p`` (inf when top-p is off)."""
+    x = logits.float()
+    T = torch.tensor(_f32(temperature), dtype=torch.float64, device=x.device)
+    z = (x.double() / T).float()   # fp32 division, correctly rounded (fp64 quotient of fp32 operands, rounded once)
+    V = z.shape[-1]
+    keep = torch.ones_like(z, dtype=torch.bool)
+    if 0 < top_k < V:
+        kth = z.topk(top_k, dim=-1).values[..., -1:]
+        keep = z >= kth
+    zmax = z.amax(dim=-1, keepdim=True)
+    z64 = z.double()
+    e = torch.where(z == zmax, torch.ones_like(z64), torch.exp(z64 - zmax.double())) * keep
+    gap = torch.full(z.shape[:-1], float("inf"), dtype=torch.float64, device=z.device)
+    tp = _f32(top_p)
+    if tp < 1.0:
+        pi = e / e.sum(dim=-1, keepdim=True)
+        zs, idx = z.masked_fill(~keep, float("-inf")).sort(dim=-1, descending=True)
+        ps = pi.gather(-1, idx)
+        excl = ps.cumsum(dim=-1) - ps
+        # the mass strictly above a token: the exclusive sum at the first token of its tie group
+        first = torch.searchsorted((-zs).contiguous(), (-zs).contiguous(), right=False).clamp(max=V - 1)
+        above = torch.empty_like(excl).scatter_(-1, idx, excl.gather(-1, first))
+        gap = (above - tp).abs().masked_fill(~keep, float("inf")).amin(dim=-1)
+        keep = keep & (above <= tp)
+        e = e * keep
+    return z, keep, e / e.sum(dim=-1, keepdim=True), gap
+
+
+def spec_warp_ref(logits, temperature: float = 1.0, top_k: int = 0, top_p: float = 1.0):
+    """The warp rule of speculative sampling on rows ``logits [..., V]`` (bf16 or fp32), as fp32 warped logits: z on
+    the kept set, −inf elsewhere.
+
+    - ``z = logit / T``, an fp32 division (``TemperatureLogitsWarper``);
+    - top-k (``k' = min(top_k, V)``, off when 0): keep ``z >=`` the k'-th largest z, counting duplicates
+      (``TopKLogitsWarper``);
+    - top-p (off when >= 1): with π the softmax of the kept z, keep token i iff the mass of kept tokens with z strictly
+      greater than ``z_i`` is ``<= top_p``.  This is ``TopPLogitsWarper`` except on ties at the boundary: there
+      ``TopPLogitsWarper`` keeps those of the tied tokens its (unstable) sort puts first, this rule keeps every one.
+
+    p is the softmax over the final kept set.  ``temperature`` and ``top_p`` are taken as fp32, as the kernels take
+    them."""
+    z, keep, _, _ = _warp64(logits, temperature, top_k, top_p)
+    return z.masked_fill(~keep, float("-inf"))
+
+
+def _pick64(w, u):
+    """Inverse CDF in index order on fp64 weights ``w [n, V]`` with uniforms ``u [n]``: the smallest i whose inclusive
+    prefix sum exceeds ``u · Σw``; and whether ``u · Σw`` lies within the margin of a step of the CDF."""
+    total = w.sum(dim=-1)
+    target = u.double() * total
+    cum = w.cumsum(dim=-1)
+    idx = torch.searchsorted(cum, target[:, None], right=True).clamp(max=w.shape[-1] - 1)[:, 0]
+    upper = cum.gather(-1, idx[:, None])[:, 0]
+    lower = torch.where(idx > 0, cum.gather(-1, (idx - 1).clamp(min=0)[:, None])[:, 0], torch.zeros_like(total))
+    near = torch.minimum(target - lower, upper - target) <= SPEC_SAMPLE_MARGIN * total
+    return idx, near
+
+
+def spec_sample_ref(logits, q, j: int, u, proposals, temperature: float = 1.0, top_k: int = 0, top_p: float = 1.0,
+                    flags: bool = False):
+    """The fp64 PyTorch mirror of :func:`spec_sample`; ``flags=True`` also returns, per sample, whether the draw lies
+    within :data:`SPEC_SAMPLE_MARGIN` of a boundary (a step of the CDF, or a top-p mass)."""
+    q[:, j].copy_(logits)
+    _, _, p, gap = _warp64(logits, temperature, top_k, top_p)
+    d, near = _pick64(p, u[:, j])
+    proposals[:, j] = d
+    if flags:
+        return near | (gap <= SPEC_SAMPLE_MARGIN)
+
+
+def spec_sample(logits, q, j: int, u, proposals, temperature: float = 1.0, top_k: int = 0, top_p: float = 1.0):
+    """One draft step of speculative sampling, in one launch of the sm_90a kernel on the GPU: keeps the draft's logits
+    row ``logits [b, V]`` (bf16 or fp32) in ``q[:, j]`` (``q [b, K, V]``, the same dtype; q itself is never
+    materialised) and draws ``proposals[:, j]`` (int64 ``[b, J]``) from its warped distribution (:func:`spec_warp_ref`)
+    by inverse CDF in index order with the uniforms ``u[:, j]`` (fp32 ``[b, J]``), without a host sync.  CPU tensors
+    run :func:`spec_sample_ref`."""
+    if not use_native(logits):
+        spec_sample_ref(logits, q, j, u, proposals, temperature, top_k, top_p)
+        return
+    load_ext().spec_sample(logits, q, int(j), u, proposals, float(temperature), int(top_k), float(top_p))
+    count_launch(1)
+
+
+def spec_accept_sample_ref(logits, q, draft, u, unfinished, temperature: float = 1.0, top_k: int = 0,
+                           top_p: float = 1.0, eos: Optional[int] = None, pad: Optional[int] = None, scores=None,
+                           flags: bool = False):
+    """The fp64 PyTorch mirror of :func:`spec_accept_sample` (same outputs, ``unfinished`` and ``scores`` written in
+    place).  ``flags=True`` also returns a bool ``[b, k + 1]``: the decisions of row j (its acceptance and its
+    candidate) lie within :data:`SPEC_SAMPLE_MARGIN` of a boundary: a top-p mass of p_j or q_j, ``u · q`` against p, a
+    step of the CDF, or a residual mass near 0."""
+    b, R, V = logits.shape
+    k = R - 1
+    z, keep, p, gap = _warp64(logits, temperature, top_k, top_p)
+    near = gap <= SPEC_SAMPLE_MARGIN
+    if scores is not None:
+        scores.copy_(z.masked_fill(~keep, float("-inf")))
+    u0, u1 = u[..., 0].double(), u[..., 1]
+    cand_w = p.clone()
+    a = torch.zeros(b, dtype=torch.long, device=logits.device)
+    if k > 0:
+        _, _, qq, gap_q = _warp64(q[:, :k], temperature, top_k, top_p)
+        d = draft.clamp(0, V - 1)[..., None]
+        pd, qd = p[:, :k].gather(-1, d)[..., 0], qq.gather(-1, d)[..., 0]
+        acc = (u0[:, :k] * qd < pd) & (draft >= 0) & (draft < V)
+        near[:, :k] |= (gap_q <= SPEC_SAMPLE_MARGIN) | ((u0[:, :k] * qd - pd).abs() <= SPEC_SAMPLE_MARGIN * (pd + qd))
+        r = (p[:, :k] - qq).clamp(min=0)
+        rs = r.sum(dim=-1, keepdim=True)
+        near[:, :k] |= (rs[..., 0] > 0) & (rs[..., 0] <= SPEC_SAMPLE_MARGIN)
+        cand_w[:, :k] = torch.where(rs > 0, r, p[:, :k])
+        a = acc.long().cumprod(dim=1).sum(dim=1)
+    cand, near_pick = _pick64(cand_w.reshape(b * R, V), u1.reshape(b * R))
+    cand = cand.view(b, R)
+    near |= near_pick.view(b, R)
+    t = cand.clone()
+    if k > 0:
+        t[:, :k] = torch.where(torch.arange(k, device=t.device)[None, :] < a[:, None], draft, cand[:, :k])
+    live = unfinished != 0
+    if eos is not None:
+        upto = torch.arange(R, device=t.device)[None, :] <= a[:, None]
+        live_a = torch.where(((t == eos) & upto).any(dim=1), k, a)
+    else:
+        live_a = a
+    n = int(live_a[live].min()) if bool(live.any()) else k
+    out = _spec_emit(t, a, n, unfinished, eos, pad)
+    return (out, near) if flags else out
+
+
+def spec_accept_sample(logits, q, draft, u, unfinished, temperature: float = 1.0, top_k: int = 0, top_p: float = 1.0,
+                       eos: Optional[int] = None, pad: Optional[int] = None, scores=None):
+    """The acceptance of one speculative-sampling iteration, in one launch of the sm_90a kernel on the GPU.
+
+    ``logits [b, k + 1, V]``: the verify step's rows after ``x, d_1 .. d_k`` (p_j warped from row j); ``q [b, K, V]``
+    (K >= k): the draft's rows, q_j warped from ``q[:, j]`` by the same rule (:func:`spec_warp_ref`), so the q that
+    accepts a proposal is the q it was drawn from, bit for bit; ``draft`` int64 ``[b, k]``: d_1 .. d_k; ``u`` fp32
+    ``[b, k + 1, 2]``: uniforms; ``unfinished`` int64 ``[b]``, updated in place.  Per sample and row j:
+
+    - accept_j: ``u[b, j, 0] · q_j(d_{j+1}) < p_j(d_{j+1})`` (j < k);
+    - the candidate c_j, drawn with ``u[b, j, 1]`` by inverse CDF in index order from norm(max(0, p_j − q_j)) for
+      j < k (from p_j when that mass is 0), from p_k for j = k (the bonus token);
+    - ``a_b``: the first rejected j (k if none); ``t_j = d_{j+1}`` for ``j < a_b``, else c_j;
+    - n, e and ``unfinished`` from t as :func:`spec_accept` defines them.
+
+    Returns int64 ``[b, 2(k + 1) + 3]`` laid out as :func:`spec_accept`'s.  ``scores`` (optional, fp32 ``[b, k + 1,
+    V]``): written with the target's warped logits (z on the kept set, −inf elsewhere).
+
+    Why the batch rule is unbiased.  A sample's token at position j is emitted iff j <= n, and whether it reaches j
+    depends only on its own acceptances before j and on the other samples, never on its own token at j.  Given its
+    prefix, that token is d_{j+1} ~ q_j accepted with probability min(1, p_j/q_j), or on the first rejection a draw
+    from norm(max(0, p_j − q_j)): together distributed as p_j (Leviathan et al. 2023, appendix A.1); at j = a_b with no
+    rejection it is the bonus draw from p_j.  So every emitted token is distributed as p given its prefix, whatever
+    the draft is.  CPU tensors run :func:`spec_accept_sample_ref`."""
+    if eos is not None and pad is None:
+        raise ValueError("spec_accept_sample: eos needs a pad token")
+    if not use_native(logits):
+        return spec_accept_sample_ref(logits, q, draft, u, unfinished, temperature, top_k, top_p, eos, pad, scores)
+    out = load_ext().spec_accept_sample(logits, q, draft, u, unfinished, float(temperature), int(top_k), float(top_p),
+                                        -1 if eos is None else int(eos), 0 if pad is None else int(pad), scores)
     count_launch(1)
     return out
 
