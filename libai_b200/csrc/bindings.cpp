@@ -347,27 +347,48 @@ Tensor dequant_int4_rows(const Tensor& w, const Tensor& w_scale, const Tensor& w
   return out;
 }
 
-// One speculative-decoding iteration's greedy acceptance (speculative_sm90.cu): logits bf16 or fp32 [b, R, V]
-// (contiguous), draft int64 [b, R - 1], unfinished int64 [b] (updated in place); eos < 0: no EOS.  Returns out int64
-// [b, 2R + 3]: the argmaxes, the emitted tokens, a_b, n and the updated unfinished.  The kernel's block counter is one
-// more element of out's allocation, zeroed on the stream before the launch.
-Tensor spec_accept(const Tensor& logits, const Tensor& draft, Tensor unfinished, int64_t eos, int64_t pad) {
-  Args args("spec_accept");
+// The verify step's arguments of both acceptance ops: logits bf16 or fp32 [b, R, V] (contiguous, R = k + 1 <= 16),
+// draft int64 [b, R - 1] and unfinished int64 [b].  Returns (b, R, V).
+std::tuple<int64_t, int64_t, int64_t> spec_verify_args(Args& args, const Tensor& logits, const Tensor& draft,
+                                                       const Tensor& unfinished) {
   args("logits", logits, Dtypes(at::kBFloat16, at::kFloat), {kAny, kAny, kAny});
   const int64_t B = logits.size(0), R = logits.size(1), V = logits.size(2);
-  TORCH_CHECK(B >= 1 && R >= 1 && R <= 16 && V >= 1 && V <= INT32_MAX, "spec_accept: logits [b, k + 1, V] needs b >= 1, ",
-              "1 <= k + 1 <= 16 and V >= 1, got ", logits.sizes());
+  TORCH_CHECK(B >= 1 && R >= 1 && R <= 16 && V >= 1 && V <= INT32_MAX, args.op(), ": logits [b, k + 1, V] needs ",
+              "b >= 1, 1 <= k + 1 <= 16 and V >= 1, got ", logits.sizes());
   args("draft", draft, at::kLong, {B, R - 1});
   args("unfinished", unfinished, at::kLong, {B});
+  return {B, R, V};
+}
+
+// The output of both acceptance ops, out int64 [b, 2R + 3], followed in its allocation by `scratch` int32 entries for
+// the kernel and its block counter, which the launcher zeroes on the stream.
+struct SpecOut {
+  Tensor out;
+  int64_t* data;
+  int* scratch;   // nullptr when scratch = 0
+  unsigned int* counter;
+};
+SpecOut spec_out(const Tensor& like, int64_t B, int64_t R, int64_t scratch) {
+  const int64_t n = B * (2 * R + 3), words = (scratch + 1) / 2;
+  Tensor buf = at::empty({n + words + 1}, like.options().dtype(at::kLong));
+  int64_t* data = buf.data_ptr<int64_t>();
+  return {buf.narrow(0, 0, n).view({B, 2 * R + 3}), data, scratch > 0 ? reinterpret_cast<int*>(data + n) : nullptr,
+          reinterpret_cast<unsigned int*>(data + n + words)};
+}
+
+// One speculative-decoding iteration's greedy acceptance (speculative_sm90.cu): logits bf16 or fp32 [b, R, V]
+// (contiguous), draft int64 [b, R - 1], unfinished int64 [b] (updated in place); eos < 0: no EOS.  Returns out int64
+// [b, 2R + 3]: the argmaxes, the emitted tokens, a_b, n and the updated unfinished.
+Tensor spec_accept(const Tensor& logits, const Tensor& draft, Tensor unfinished, int64_t eos, int64_t pad) {
+  Args args("spec_accept");
+  const auto [B, R, V] = spec_verify_args(args, logits, draft, unfinished);
   const auto guard = args.guard();
-  const int64_t cols = 2 * R + 3;
-  Tensor buf = at::empty({B * cols + 1}, draft.options());
-  int64_t* out = buf.data_ptr<int64_t>();
+  const SpecOut o = spec_out(draft, B, R, 0);
   check(lb_spec_accept(logits.data_ptr(), logits.scalar_type() == at::kFloat ? 1 : 0, draft.data_ptr<int64_t>(),
-                       unfinished.data_ptr<int64_t>(), out, reinterpret_cast<unsigned int*>(out + B * cols), (int)B,
-                       (int)R, (int)V, (long long)eos, (long long)pad, cur_stream()),
+                       unfinished.data_ptr<int64_t>(), o.data, o.counter, (int)B, (int)R, (int)V, (long long)eos,
+                       (long long)pad, cur_stream()),
         "spec_accept");
-  return buf.narrow(0, 0, B * cols).view({B, cols});
+  return o.out;
 }
 
 // The warp arguments of speculative sampling: temperature > 0 (finite), top_k >= 0 (0: off), 0 < top_p <= 1.
@@ -404,36 +425,26 @@ void spec_sample(const Tensor& logits, Tensor q, int64_t j, const Tensor& u, Ten
 // One speculative-sampling iteration's acceptance (speculative_sm90.cu): logits bf16 or fp32 [b, R, V], q bf16 or
 // fp32 [b, K, V] (the draft's rows, K >= R - 1), draft int64 [b, R - 1], u fp32 [b, R, 2], unfinished int64 [b]
 // (updated in place), scores (optional) fp32 [b, R, V], written with the target's warped logits.  Returns out int64
-// [b, 2R + 3] laid out as spec_accept's.  The per-row decisions and the block counter live past out in its allocation.
+// [b, 2R + 3] laid out as spec_accept's; the kernel keeps the per-row decisions in out's scratch.
 Tensor spec_accept_sample(const Tensor& logits, const Tensor& q, const Tensor& draft, const Tensor& u,
                           Tensor unfinished, double temperature, int64_t top_k, double top_p, int64_t eos, int64_t pad,
                           c10::optional<Tensor> scores) {
   Args args("spec_accept_sample");
-  args("logits", logits, Dtypes(at::kBFloat16, at::kFloat), {kAny, kAny, kAny});
-  const int64_t B = logits.size(0), R = logits.size(1), V = logits.size(2);
-  TORCH_CHECK(B >= 1 && R >= 1 && R <= 16 && V >= 1 && V <= INT32_MAX, "spec_accept_sample: logits [b, k + 1, V] ",
-              "needs b >= 1, 1 <= k + 1 <= 16 and V >= 1, got ", logits.sizes());
+  const auto [B, R, V] = spec_verify_args(args, logits, draft, unfinished);
   args("q", q, Dtypes(at::kBFloat16, at::kFloat), {B, kAny, V});
   TORCH_CHECK(q.size(1) >= R - 1, "spec_accept_sample: q holds ", q.size(1), " draft rows, the iteration needs ", R - 1);
-  args("draft", draft, at::kLong, {B, R - 1});
   args("u", u, at::kFloat, {B, R, 2});
-  args("unfinished", unfinished, at::kLong, {B});
   float* scores_ptr = args.opt<float>("scores", scores, at::kFloat, {B, R, V});
   check_warp("spec_accept_sample", temperature, top_k, top_p);
   const auto guard = args.guard();
-  const int64_t cols = 2 * R + 3;
-  // out, then B·R int32 decisions (B·R / 2 + 1 int64 slots) and the counter
-  Tensor buf = at::empty({B * cols + (B * R) / 2 + 2}, draft.options());
-  int64_t* out = buf.data_ptr<int64_t>();
-  int* accepted = reinterpret_cast<int*>(out + B * cols);
-  unsigned int* counter = reinterpret_cast<unsigned int*>(out + B * cols + (B * R) / 2 + 1);
+  const SpecOut o = spec_out(draft, B, R, B * R);
   check(lb_spec_accept_sample(logits.data_ptr(), logits.scalar_type() == at::kFloat ? 1 : 0, q.data_ptr(),
                               q.scalar_type() == at::kFloat ? 1 : 0, draft.data_ptr<int64_t>(), u.data_ptr<float>(),
-                              unfinished.data_ptr<int64_t>(), out, accepted, counter, scores_ptr, (int)B, (int)R,
-                              (int)V, (int)q.size(1), (float)temperature, (int)top_k, (float)top_p, (long long)eos,
-                              (long long)pad, cur_stream()),
+                              unfinished.data_ptr<int64_t>(), o.data, o.scratch, o.counter, scores_ptr, (int)B,
+                              (int)R, (int)V, (int)q.size(1), (float)temperature, (int)top_k, (float)top_p,
+                              (long long)eos, (long long)pad, cur_stream()),
         "spec_accept_sample");
-  return buf.narrow(0, 0, B * cols).view({B, cols});
+  return o.out;
 }
 
 // per-tensor E4M3 quantisation of a contiguous bf16 tensor: returns (q [same shape, float8_e4m3fn], deq fp32 [1]) with

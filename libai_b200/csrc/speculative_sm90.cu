@@ -16,10 +16,14 @@
 //
 // Phase 1 is one block per row: a strided scan of V and a block reduction of (value, index) pairs.  The pair order
 // (larger value, then smaller index) is a total order on finite and −inf values, so the result does not depend on
-// the order of the comparisons: the reduction is deterministic.  V needs no alignment (scalar, coalesced loads).  The
-// last block to finish runs phase 2 over the b·R argmaxes.  It finds that it is last through a counter that the launcher
-// zeroes on the stream before the kernel (cudaMemsetAsync): every launch has its own, so launches on other streams
-// never share one and a launch that did not complete leaves nothing behind.
+// the order of the comparisons: the reduction is deterministic.  V needs no alignment (scalar, coalesced loads).
+//
+// Phase 2 (emit(), shared with spec_accept_sample) runs in the last block to finish, over the b·R tokens t in
+// out[:, 0:R) and a predicate that says whether row (b, j)'s proposal is accepted (here draft[b, j] == t_j): it
+// computes a_b, writes draft[b, j] over t_j for j < a_b (for greedy acceptance the value already there), then n, e and
+// the updated unfinished.  The block finds that it is last through a counter that the launcher zeroes on the stream
+// before the kernel (cudaMemsetAsync): every launch has its own, so launches on other streams never share one and a
+// launch that did not complete leaves nothing behind.
 #include <climits>
 
 #include "common.cuh"
@@ -35,6 +39,65 @@ __device__ __forceinline__ float load(const float* p) { return *p; }
 // (v, i) beats (w, j): a larger value, or an equal one at a smaller index
 __device__ __forceinline__ bool beats(float v, int i, float w, int j) { return v > w || (v == w && i < j); }
 
+// Called by every thread once thread 0 has written its block's results: whether this block is the last of the launch
+// to finish, in which case every block's results are visible to it.
+__device__ __forceinline__ bool last_block(unsigned int* counter) {
+  __shared__ bool s_last;
+  if (threadIdx.x == 0) {
+    __threadfence();
+    s_last = atomicAdd(counter, 1u) == gridDim.x - 1;
+  }
+  __syncthreads();
+  if (!s_last) return false;
+  __threadfence();
+  return true;
+}
+
+// Phase 2 of both acceptance kernels, in the last block, from the tokens t in out[:, 0:R) and accepted(b, j), whether
+// row j's proposal draft[b, j] is accepted (j < k).
+template <typename Accepted>
+__device__ __forceinline__ void emit(Accepted accepted, const int64_t* __restrict__ draft,
+                                     int64_t* __restrict__ unfinished, int64_t* out, int B, int R, long long eos,
+                                     long long pad) {
+  __shared__ int s_n;
+  const int k = R - 1, cols = 2 * R + 3;
+  if (threadIdx.x == 0) s_n = k;
+  __syncthreads();
+  for (int b = threadIdx.x; b < B; b += blockDim.x) {
+    volatile int64_t* t = out + (size_t)b * cols;
+    int a = 0;
+    while (a < k && accepted(b, a)) ++a;
+    for (int j = 0; j < a; ++j) t[j] = draft[(size_t)b * k + j];
+    t[2 * R] = a;
+    if (unfinished[b] != 0) {
+      bool ends = false;
+      for (int j = 0; j <= a && eos >= 0; ++j) ends |= t[j] == eos;
+      atomicMin(&s_n, ends ? k : a);
+    }
+  }
+  __syncthreads();
+  const int n = s_n;
+  for (int b = threadIdx.x; b < B; b += blockDim.x) {
+    int64_t* o = out + (size_t)b * cols;
+    const volatile int64_t* t = o;
+    int64_t u = unfinished[b];
+    for (int j = 0; j < R; ++j) {
+      int64_t e = -1;
+      if (j <= n) {
+        e = t[j];
+        if (eos >= 0) {
+          if (u == 0) e = pad;
+          if (e == eos) u = 0;
+        }
+      }
+      o[R + j] = e;
+    }
+    o[2 * R + 1] = n;
+    o[2 * R + 2] = u;
+    unfinished[b] = u;
+  }
+}
+
 template <typename T>
 __global__ void __launch_bounds__(kThreads) accept_kernel(const T* __restrict__ logits, const int64_t* __restrict__ draft,
                                                           int64_t* __restrict__ unfinished, int64_t* __restrict__ out,
@@ -42,8 +105,6 @@ __global__ void __launch_bounds__(kThreads) accept_kernel(const T* __restrict__ 
                                                           long long eos, long long pad) {
   __shared__ float s_val[kThreads / 32];
   __shared__ int s_idx[kThreads / 32];
-  __shared__ bool s_last;
-  __shared__ int s_n;
   const int row = blockIdx.x;   // b * R + j
   const int cols = 2 * R + 3;
   const T* p = logits + (size_t)row * V;
@@ -72,53 +133,14 @@ __global__ void __launch_bounds__(kThreads) accept_kernel(const T* __restrict__ 
       const int j = __shfl_xor_sync(0xffffffffu, idx, off);
       if (beats(w, j, best, idx)) best = w, idx = j;
     }
-    if (lane == 0) {
-      // a row of −inf only: every index ties, the lowest is 0 (as torch.argmax); idx is INT_MAX only when V == 0
-      out[(size_t)(row / R) * cols + row % R] = idx == INT_MAX ? 0 : idx;
-      __threadfence();
-      s_last = atomicAdd(counter, 1u) == (unsigned)(gridDim.x - 1);
-    }
+    // a row of −inf only: every index ties, the lowest is 0 (as torch.argmax); idx is INT_MAX only when V == 0
+    if (lane == 0) out[(size_t)(row / R) * cols + row % R] = idx == INT_MAX ? 0 : idx;
   }
-  __syncthreads();
-  if (!s_last) return;
-
-  // phase 2: the last block sees every row's argmax
-  __threadfence();
+  if (!last_block(counter)) return;
+  const volatile int64_t* t = out;
   const int k = R - 1;
-  if (threadIdx.x == 0) s_n = k;
-  __syncthreads();
-  for (int b = threadIdx.x; b < B; b += kThreads) {
-    const volatile int64_t* t = out + (size_t)b * cols;
-    int a = 0;
-    while (a < k && draft[(size_t)b * k + a] == t[a]) ++a;
-    out[(size_t)b * cols + 2 * R] = a;
-    if (unfinished[b] != 0) {
-      bool ends = false;
-      for (int j = 0; j <= a && eos >= 0; ++j) ends |= t[j] == eos;
-      atomicMin(&s_n, ends ? k : a);
-    }
-  }
-  __syncthreads();
-  const int n = s_n;
-  for (int b = threadIdx.x; b < B; b += kThreads) {
-    int64_t* o = out + (size_t)b * cols;
-    const volatile int64_t* t = o;
-    int64_t u = unfinished[b];
-    for (int j = 0; j < R; ++j) {
-      int64_t e = -1;
-      if (j <= n) {
-        e = t[j];
-        if (eos >= 0) {
-          if (u == 0) e = pad;
-          if (e == eos) u = 0;
-        }
-      }
-      o[R + j] = e;
-    }
-    o[2 * R + 1] = n;
-    o[2 * R + 2] = u;
-    unfinished[b] = u;
-  }
+  emit([=](int b, int j) { return draft[(size_t)b * k + j] == t[(size_t)b * cols + j]; }, draft, unfinished, out, B,
+       R, eos, pad);
 }
 
 }  // namespace spec
@@ -157,9 +179,9 @@ int lb_spec_accept(const void* logits, int logits_fp32, const int64_t* draft, in
 //   accept_j = u[b, j, 0] · q_j(d_{j+1}) < p_j(d_{j+1})                         (j < k, in fp64 from the masses)
 //   c_j      = pick(floor(u[b, j, 1] · Σr)) over r_i = 2^40 · max(0, p_j(i) − q_j(i)), rounded (j < k, Σr > 0);
 //              pick over p_j's masses when Σr = 0 or j = k (the bonus token)
-// phase 2, the last CTA (the counter pattern of spec_accept): a_b = the first rejected j (k if none); t_j = d_{j+1}
-// for j < a_b, else c_j; then n, e and unfinished as spec_accept defines them from t.  scores (optional, fp32
-// [B, R, V]): the target's warped logits, z on the kept set and −inf elsewhere.
+// phase 2, spec_accept's emit() over t_j = c_j and accepted(b, j) = accept_j: a_b = the first rejected j (k if none);
+// t_j = d_{j+1} for j < a_b; then n, e and unfinished from t.  scores (optional, fp32 [B, R, V]): the target's warped
+// logits, z on the kept set and −inf elsewhere.
 #include "sampling.cuh"
 
 namespace lb {
@@ -192,8 +214,6 @@ __global__ void __launch_bounds__(samp::kThreads, 1) accept_sample_kernel(
     unsigned int* __restrict__ counter, float* __restrict__ scores, int B, int R, int V, int K, float temperature,
     int top_k, float top_p, long long eos, long long pad) {
   __shared__ samp::Shared sh;
-  __shared__ bool s_last;
-  __shared__ int s_n;
   const int row_id = blockIdx.x;   // b * R + j
   const int b = row_id / R, j = row_id % R, k = R - 1;
   const int cols = 2 * R + 3;
@@ -237,52 +257,10 @@ __global__ void __launch_bounds__(samp::kThreads, 1) accept_sample_kernel(
       o[i] = samp::key_of(z) >= pw.keep ? z : -INFINITY;
     }
   }
-  if (threadIdx.x == 0) {
-    out[(size_t)b * cols + j] = cand;
-    __threadfence();
-    s_last = atomicAdd(counter, 1u) == (unsigned)(gridDim.x - 1);
-  }
-  __syncthreads();
-  if (!s_last) return;
-
-  // phase 2: the last block sees every row's decision and candidate
-  __threadfence();
-  if (threadIdx.x == 0) s_n = k;
-  __syncthreads();
-  for (int bb = threadIdx.x; bb < B; bb += samp::kThreads) {
-    volatile int64_t* t = out + (size_t)bb * cols;
-    const volatile int* acc = accepted + (size_t)bb * R;
-    int a = 0;
-    while (a < k && acc[a]) ++a;
-    for (int jj = 0; jj < a; ++jj) t[jj] = draft[(size_t)bb * k + jj];
-    out[(size_t)bb * cols + 2 * R] = a;
-    if (unfinished[bb] != 0) {
-      bool ends = false;
-      for (int jj = 0; jj <= a && eos >= 0; ++jj) ends |= t[jj] == eos;
-      atomicMin(&s_n, ends ? k : a);
-    }
-  }
-  __syncthreads();
-  const int n = s_n;
-  for (int bb = threadIdx.x; bb < B; bb += samp::kThreads) {
-    int64_t* o = out + (size_t)bb * cols;
-    const volatile int64_t* t = o;
-    int64_t uf = unfinished[bb];
-    for (int jj = 0; jj < R; ++jj) {
-      int64_t e = -1;
-      if (jj <= n) {
-        e = t[jj];
-        if (eos >= 0) {
-          if (uf == 0) e = pad;
-          if (e == eos) uf = 0;
-        }
-      }
-      o[R + jj] = e;
-    }
-    o[2 * R + 1] = n;
-    o[2 * R + 2] = uf;
-    unfinished[bb] = uf;
-  }
+  if (threadIdx.x == 0) out[(size_t)b * cols + j] = cand;
+  if (!last_block(counter)) return;
+  const volatile int* acc = accepted;
+  emit([=](int bb, int jj) { return acc[(size_t)bb * R + jj] != 0; }, draft, unfinished, out, B, R, eos, pad);
 }
 
 }  // namespace spec

@@ -12,6 +12,7 @@ every rank runs the same search; sampled tokens are broadcast from rank 0 so the
 """
 from __future__ import annotations
 
+import contextlib
 import inspect
 import logging
 import warnings
@@ -108,6 +109,26 @@ def _decode_graphs(value) -> bool:
     if not isinstance(value, bool):
         raise ValueError(f"decode_graphs must be True or False, got {value!r}")
     return value
+
+
+@contextlib.contextmanager
+def _call_state(model, kv_cache_dtype, decode_graphs: bool):
+    """A model's state for one ``generate()`` call, restored when it ends: eval mode, the call's cache format when it
+    gives one (``allocate_kv_cache`` reads it) and, with ``decode_graphs``, its decode graphs."""
+    was_training, saved_kv_cache_dtype = model.training, getattr(model, "kv_cache_dtype", None)
+    model.eval()
+    try:
+        if kv_cache_dtype is not None:
+            model.kv_cache_dtype = kv_cache_dtype
+        if decode_graphs:
+            model._decode_graphs = decode_graph.DecodeCall()
+        yield
+    finally:
+        model.train(was_training)
+        if kv_cache_dtype is not None:
+            model.kv_cache_dtype = saved_kv_cache_dtype
+        if decode_graphs:
+            del model._decode_graphs   # back to the class's None
 
 
 class Generator:
@@ -420,29 +441,9 @@ class Generator:
         if max_length is not None:
             warnings.warn("`max_length` is deprecated here; use `stopping_criteria=[MaxLengthCriteria(...)]`", UserWarning)
             stopping_criteria = validate_stopping_criteria(stopping_criteria, max_length)
-        pad_token_id = self._pick(pad_token_id, "pad_token_id")
-        eos_token_id = self._pick(eos_token_id, "eos_token_id")
-        scores = () if output_scores else None
-        unfinished = torch.ones(input_ids.shape[0], dtype=torch.long, device=input_ids.device)
-        while True:
-            outputs = self._decode_step(input_ids, model_kwargs)
-            next_scores = logits_processor(input_ids, self._step_logits(outputs))
-            if output_scores:
-                scores += (next_scores,)
-            next_tokens = torch.argmax(next_scores, dim=-1)
-            if eos_token_id is not None:
-                if pad_token_id is None:
-                    raise ValueError("If `eos_token_id` is defined, make sure that `pad_token_id` is defined.")
-                next_tokens = next_tokens * unfinished + pad_token_id * (1 - unfinished)
-            next_tokens = self._sync_tokens(next_tokens)
-            input_ids = torch.cat([input_ids, next_tokens[:, None]], dim=-1)
-            model_kwargs = self._update_model_kwargs_for_generation(outputs, model_kwargs, is_encoder_decoder)
-            if eos_token_id is not None:
-                unfinished = unfinished * (next_tokens != eos_token_id).long()
-            if unfinished.max() == 0 or stopping_criteria(input_ids, scores):
-                break
-        self._reset_cache()
-        return (input_ids, scores) if output_scores else input_ids
+        return self._token_loop(input_ids, lambda s: torch.argmax(s, dim=-1), logits_processor, LogitsProcessorList(),
+                                stopping_criteria, pad_token_id, eos_token_id, is_encoder_decoder, output_scores,
+                                model_kwargs)
 
     @torch.no_grad()
     def multinomial_sample(self, input_ids, logits_processor=None, stopping_criteria=None, logits_warper=None,
@@ -453,6 +454,15 @@ class Generator:
         if max_length is not None:
             stopping_criteria = validate_stopping_criteria(stopping_criteria, max_length)
         logits_warper = logits_warper if logits_warper is not None else LogitsProcessorList()
+        return self._token_loop(input_ids,
+                                lambda s: torch.multinomial(torch.softmax(s, dim=-1), num_samples=1).squeeze(1),
+                                logits_processor, logits_warper, stopping_criteria, pad_token_id, eos_token_id,
+                                is_encoder_decoder, output_scores, model_kwargs)
+
+    def _token_loop(self, input_ids, pick, logits_processor, logits_warper, stopping_criteria, pad_token_id,
+                    eos_token_id, is_encoder_decoder, output_scores, model_kwargs):
+        """The loop of ``greedy_search`` and ``multinomial_sample``: one token per step, ``pick`` of the processed and
+        warped logits, until every sample has emitted EOS or ``stopping_criteria`` stops."""
         pad_token_id = self._pick(pad_token_id, "pad_token_id")
         eos_token_id = self._pick(eos_token_id, "eos_token_id")
         scores = () if output_scores else None
@@ -462,8 +472,7 @@ class Generator:
             next_scores = logits_warper(input_ids, logits_processor(input_ids, self._step_logits(outputs)))
             if output_scores:
                 scores += (next_scores,)
-            probs = torch.softmax(next_scores, dim=-1)
-            next_tokens = torch.multinomial(probs, num_samples=1).squeeze(1)
+            next_tokens = pick(next_scores)
             if eos_token_id is not None:
                 if pad_token_id is None:
                     raise ValueError("If `eos_token_id` is defined, make sure that `pad_token_id` is defined.")
@@ -604,8 +613,9 @@ class Generator:
             raise ValueError("attention_mask: speculative decoding needs padding that the cache's kv_start holds "
                              "(left padding); this prompt needs a dense mask")
         rows = self._all_logits(outputs)[:, -1:].contiguous()
-        # rows a cache holds besides the sequence's (ChatGLM's P-tuning prefix)
-        extra = cache.length - input_ids.shape[1]
+        # per model: the rows its cache holds besides the sequence's (ChatGLM's P-tuning prefix), and the rows an
+        # iteration's steps write besides the k proposals (the verify step's x)
+        models = [(self, cache.length - input_ids.shape[1], 1)]
         draft_kwargs = {"past": None, "use_cache": True}
         if draft is not None:
             mask = model_kwargs.get("attention_mask")
@@ -617,7 +627,7 @@ class Generator:
             if draft.kv_cache.dense_mask:
                 raise ValueError("attention_mask: the assistant's cache needs a dense mask for this prompt")
             draft_kwargs["past"] = draft.kv_cache
-            draft_extra = draft.kv_cache.length - input_ids.shape[1]
+            models.append((draft, draft.kv_cache.length - input_ids.shape[1], 0))
             if sample:   # the draft's logits rows of an iteration, from which the acceptance recomputes q
                 qbuf = torch.empty(b, k, rows.shape[-1], dtype=draft._all_logits(draft_out).dtype, device=dev)
         history = staging = None
@@ -659,38 +669,33 @@ class Generator:
             if not any(host_unfinished) or count < n + 1 or stopping_criteria(input_ids, scores):
                 break
 
-            # both caches back to the invariant: the rows of the sequence minus its last token
+            # both caches back to the invariant: the rows of the sequence minus its last token; then k, so that no
+            # step writes past a model's maximum positions
             L = input_ids.shape[1]
-            cache.rollback(cache.length - (L - 1 + extra))
-            self.past_length = cache.length
             kk = k
-            if self.max_cache_positions is not None:   # the verify step writes k + 1 rows
-                kk = min(kk, self.max_cache_positions - cache.length - 1)
-            if draft is not None:
-                dc, held = draft.kv_cache, L - 1 + draft_extra
-                if dc.length > held:
-                    dc.rollback(dc.length - held)
-                    draft.past_length = dc.length
-                elif dc.length == held - 1:   # every proposal was accepted: the draft lacks the row of d_k
+            for m, m_extra, more in models:
+                c, held = m.kv_cache, L - 1 + m_extra
+                if c.length < held:   # every proposal was accepted: the draft lacks the row of d_k
                     draft._decode_step(input_ids[:, L - 2 : L - 1], draft_kwargs)
-                if draft.max_cache_positions is not None:   # the draft writes k rows
-                    kk = min(kk, draft.max_cache_positions - dc.length)
+                else:
+                    c.rollback(c.length - held)
+                    m.past_length = c.length
+                if m.max_cache_positions is not None:
+                    kk = min(kk, m.max_cache_positions - c.length - more)
             kk = max(kk, 0)
 
             x = input_ids[:, -1:]
-            if sample:
-                ud = torch.rand(b, kk, device=dev)
+            if draft is not None:
+                if sample:
+                    ud = torch.rand(b, kk, device=dev)
                 proposals, tok = input_ids.new_empty(b, kk), x
                 for j in range(kk):
                     step = self._all_logits(draft._decode_step(tok, draft_kwargs))[:, -1]
-                    OF.spec_sample(step, qbuf, j, ud, proposals, *warp)
+                    if sample:
+                        OF.spec_sample(step, qbuf, j, ud, proposals, *warp)
+                    else:
+                        proposals[:, j] = step.argmax(dim=-1)
                     tok = proposals[:, j : j + 1].contiguous()
-            elif draft is not None:
-                tok, props = x, []
-                for _ in range(kk):
-                    tok = self._all_logits(draft._decode_step(tok, draft_kwargs))[:, -1].argmax(dim=-1, keepdim=True)
-                    props.append(tok)
-                proposals = torch.cat(props, dim=1) if props else input_ids.new_empty(b, 0)
             else:
                 proposals = torch.tensor([prompt_lookup(h, kk, max_matching_ngram_size) for h in history],
                                          dtype=input_ids.dtype).view(b, kk)
@@ -902,31 +907,21 @@ class Generator:
                 draft, num_assistant_tokens, prompt_lookup_num_tokens, max_matching_ngram_size, do_sample, num_beams,
                 num_return_sequences, logits_processor, custom_criteria, is_enc_dec, stopping_criteria.max_length,
                 model_kwargs, temperature=temperature, top_k=top_k, top_p=top_p, typical_p=typical_p)
-        saved_kv_cache_dtype = getattr(self, "kv_cache_dtype", None)
-        was_training = self.training
-        self.eval()
-        if draft is not None:
-            draft_state = (draft.training, getattr(draft, "kv_cache_dtype", None))
-            draft.eval()
-        try:
-            if kv_cache_dtype is not None:   # the cache format of this call (allocate_kv_cache reads it)
-                self.kv_cache_dtype = kv_cache_dtype
-            if decode_graphs:
-                self._decode_graphs = decode_graph.DecodeCall()
-            if draft is not None:
-                draft.kv_cache_dtype = _kv_cache_dtype(draft._gcfg("kv_cache_dtype")) or draft_state[1]
-                if decode_graphs:
-                    draft._decode_graphs = decode_graph.DecodeCall()
-                # a verify step appends k + 1 rows and keeps n + 1 of them: room for k more than the output
-                draft.allocate_kv_cache(batch_size * (num_return_sequences if is_sample else 1),
-                                        stopping_criteria.max_length + spec_k)
-            # models with a preallocated cache size it once for every sequence the search runs
-            allocate = getattr(self, "allocate_kv_cache", None)
-            if allocate is not None and model_kwargs.get("use_cache") and stopping_criteria.max_length is not None:
-                rows = batch_size * (num_beams if is_beam else num_return_sequences if is_sample else 1)
-                if allocate(rows, stopping_criteria.max_length + spec_k) is None and kv_cache_dtype is not None:
-                    raise ValueError(f"kv_cache_dtype={kv_cache_dtype}: {type(self).__name__} keeps a tuple cache "
-                                     "here (pipeline-parallel inference), not a StaticKVCache")
+        with contextlib.ExitStack() as call:
+            call.enter_context(_call_state(self, kv_cache_dtype, decode_graphs))
+            models = [self]
+            if draft is not None:   # the assistant's cfg sets its cache format
+                call.enter_context(_call_state(draft, _kv_cache_dtype(draft._gcfg("kv_cache_dtype")), decode_graphs))
+                models.insert(0, draft)
+            # models with a preallocated cache size it once for every sequence the search runs; a verify step appends
+            # k + 1 rows and keeps n + 1 of them: room for k more than the output
+            rows = batch_size * (num_beams if is_beam else num_return_sequences if is_sample else 1)
+            for m in models:
+                allocate = getattr(m, "allocate_kv_cache", None)
+                if allocate is not None and model_kwargs.get("use_cache") and stopping_criteria.max_length is not None:
+                    if allocate(rows, stopping_criteria.max_length + spec_k) is None and kv_cache_dtype is not None:
+                        raise ValueError(f"kv_cache_dtype={kv_cache_dtype}: {type(m).__name__} keeps a tuple cache "
+                                         "here (pipeline-parallel inference), not a StaticKVCache")
             if speculative:
                 if is_sample:   # as multinomial_sample expands them
                     input_ids, model_kwargs = self._expand_inputs_for_generation(
@@ -966,14 +961,3 @@ class Generator:
                                         eos_token_id=eos_token_id, is_encoder_decoder=is_enc_dec,
                                         output_scores=output_scores, **model_kwargs)
             raise NotImplementedError("beam sampling is not supported (neither is it in the reference)")
-        finally:
-            self.train(was_training)
-            if kv_cache_dtype is not None:
-                self.kv_cache_dtype = saved_kv_cache_dtype
-            if decode_graphs:
-                del self._decode_graphs   # back to the class's None
-            if draft is not None:
-                draft.train(draft_state[0])
-                draft.kv_cache_dtype = draft_state[1]
-                if decode_graphs:
-                    del draft._decode_graphs

@@ -426,20 +426,21 @@ def spec_accept_ref(logits, draft, unfinished, eos: Optional[int] = None, pad: O
     t = logits.argmax(dim=-1)   # the first of equal maxima
     match = (draft == t[:, :k]).long()
     a = match.cumprod(dim=1).sum(dim=1) if k > 0 else torch.zeros(b, dtype=torch.long, device=logits.device)
+    return _spec_emit(t, a, unfinished, eos, pad)
+
+
+def _spec_emit(t, a, unfinished, eos, pad):
+    """n and the emitted tokens e of one speculative iteration from its tokens t [b, R] and a_b (``unfinished``
+    updated in place): the ``[b, 2R + 3]`` output of :func:`spec_accept` and :func:`spec_accept_sample`."""
+    b, R = t.shape
+    k = R - 1
     live = unfinished != 0
     if eos is not None:
-        upto = torch.arange(R, device=logits.device)[None, :] <= a[:, None]
+        upto = torch.arange(R, device=t.device)[None, :] <= a[:, None]
         live_a = torch.where(((t == eos) & upto).any(dim=1), k, a)
     else:
         live_a = a
     n = int(live_a[live].min()) if bool(live.any()) else k
-    return _spec_emit(t, a, n, unfinished, eos, pad)
-
-
-def _spec_emit(t, a, n: int, unfinished, eos, pad):
-    """The emitted tokens e of one speculative iteration from its tokens t [b, R], a_b and n (``unfinished`` updated in
-    place): the ``[b, 2R + 3]`` output of :func:`spec_accept` and :func:`spec_accept_sample`."""
-    b, R = t.shape
     e = t.clone()
     u = unfinished.clone()
     for j in range(R):
@@ -609,14 +610,7 @@ def spec_accept_sample_ref(logits, q, draft, u, unfinished, temperature: float =
     t = cand.clone()
     if k > 0:
         t[:, :k] = torch.where(torch.arange(k, device=t.device)[None, :] < a[:, None], draft, cand[:, :k])
-    live = unfinished != 0
-    if eos is not None:
-        upto = torch.arange(R, device=t.device)[None, :] <= a[:, None]
-        live_a = torch.where(((t == eos) & upto).any(dim=1), k, a)
-    else:
-        live_a = a
-    n = int(live_a[live].min()) if bool(live.any()) else k
-    out = _spec_emit(t, a, n, unfinished, eos, pad)
+    out = _spec_emit(t, a, unfinished, eos, pad)
     return (out, near) if flags else out
 
 
