@@ -1099,15 +1099,24 @@ void cache_args(Args& args, const Tensor& k_cache, const Tensor& v_cache, const 
 // of the caches [B, G, C, D]; with cos/sin (fp32 [>= positions, D]) q and k are rotated first.  Returns the (rotated) q
 // as [B, Sq, G * r, D] when write_q, else empty.  With k_scale and v_scale the caches are FP8 (E4M3): the bf16 k row
 // before quantization is that of a bf16 cache, and each k and v row x is stored as the bytes e4m3_rn_satfinite(x / s)
-// with s = amax|x| / 448 (1 for a zero row).
+// with s = amax|x| / 448 (1 for a zero row).  With a block table (int32 [B, max_pages]) the caches are paged: pools of
+// 64-row pages [P, G, 64, D] (scales [P, G, 64]), logical row j of sample b at row j % 64 of page table[b][j / 64];
+// like the lengths, page ids in [0, P) for the rows written are the caller's guarantee.
 Tensor kv_append_any(const char* op, const Tensor& qkv, const Tensor& k_cache, const Tensor& v_cache,
                      const Tensor* k_scale, const Tensor* v_scale, const Tensor& cache_seqlens,
-                     const c10::optional<Tensor>& cosv, const c10::optional<Tensor>& sinv, bool write_q) {
+                     const c10::optional<Tensor>& cosv, const c10::optional<Tensor>& sinv, bool write_q,
+                     const Tensor* table = nullptr) {
   Args args(op);
   args("qkv", qkv, at::kBFloat16, qkv.sizes());
   const PackedQKV g = packed_qkv(qkv, op);
-  cache_args(args, k_cache, v_cache, k_scale, v_scale, {g.B, g.G, kAny, g.D});
-  const int B = g.B, G = g.G, C = (int)k_cache.size(2), D = g.D, Sq = g.S, A = G * g.r;
+  if (table != nullptr)
+    cache_args(args, k_cache, v_cache, k_scale, v_scale, {kAny, g.G, 64, g.D});
+  else
+    cache_args(args, k_cache, v_cache, k_scale, v_scale, {g.B, g.G, kAny, g.D});
+  if (table != nullptr) args("block_table", *table, at::kInt, {g.B, kAny});
+  const int max_pages = table != nullptr ? (int)table->size(1) : 0;
+  const int B = g.B, G = g.G, C = table != nullptr ? max_pages * 64 : (int)k_cache.size(2), D = g.D, Sq = g.S,
+            A = G * g.r;
   TORCH_CHECK(Sq >= 1 && Sq <= C, op, ": 1 <= Sq <= capacity");
   args("cache_seqlens", cache_seqlens, at::kInt, {B});
   TORCH_CHECK(given(cosv) == given(sinv), op, ": cos and sin go together");
@@ -1118,9 +1127,19 @@ Tensor kv_append_any(const char* op, const Tensor& qkv, const Tensor& k_cache, c
   const float* cp = given(cosv) ? cosv->data_ptr<float>() : nullptr;
   const float* sp = given(sinv) ? sinv->data_ptr<float>() : nullptr;
   void* qp = write_q ? q_out.data_ptr() : nullptr;
-  if (k_scale != nullptr)
+  const int* tp = table != nullptr ? table->data_ptr<int>() : nullptr;
+  if (k_scale != nullptr && table != nullptr)
+    check(lb_kv_append_fp8_paged(qkv.data_ptr(), cp, sp, qp, k_cache.data_ptr(), v_cache.data_ptr(),
+                                 k_scale->data_ptr<float>(), v_scale->data_ptr<float>(), cache_seqlens.data_ptr<int>(),
+                                 tp, max_pages, B, Sq, G, g.r, D, cur_stream()),
+          op);
+  else if (k_scale != nullptr)
     check(lb_kv_append_fp8(qkv.data_ptr(), cp, sp, qp, k_cache.data_ptr(), v_cache.data_ptr(), k_scale->data_ptr<float>(),
                            v_scale->data_ptr<float>(), cache_seqlens.data_ptr<int>(), B, Sq, G, g.r, C, D, cur_stream()),
+          op);
+  else if (table != nullptr)
+    check(lb_kv_append_paged(qkv.data_ptr(), cp, sp, qp, k_cache.data_ptr(), v_cache.data_ptr(),
+                             cache_seqlens.data_ptr<int>(), tp, max_pages, B, Sq, G, g.r, D, cur_stream()),
           op);
   else
     check(lb_kv_append(qkv.data_ptr(), cp, sp, qp, k_cache.data_ptr(), v_cache.data_ptr(), cache_seqlens.data_ptr<int>(),
@@ -1137,6 +1156,52 @@ Tensor kv_append_fp8(const Tensor& qkv, const Tensor& k_cache, const Tensor& v_c
                      const c10::optional<Tensor>& sinv, bool write_q) {
   return kv_append_any("kv_append_fp8", qkv, k_cache, v_cache, &k_scale, &v_scale, cache_seqlens, cosv, sinv, write_q);
 }
+Tensor kv_append_paged(const Tensor& qkv, const Tensor& k_pool, const Tensor& v_pool, const Tensor& block_table,
+                       const Tensor& cache_seqlens, const c10::optional<Tensor>& cosv,
+                       const c10::optional<Tensor>& sinv, bool write_q) {
+  return kv_append_any("kv_append_paged", qkv, k_pool, v_pool, nullptr, nullptr, cache_seqlens, cosv, sinv, write_q,
+                       &block_table);
+}
+Tensor kv_append_fp8_paged(const Tensor& qkv, const Tensor& k_pool, const Tensor& v_pool, const Tensor& k_scale,
+                           const Tensor& v_scale, const Tensor& block_table, const Tensor& cache_seqlens,
+                           const c10::optional<Tensor>& cosv, const c10::optional<Tensor>& sinv, bool write_q) {
+  return kv_append_any("kv_append_fp8_paged", qkv, k_pool, v_pool, &k_scale, &v_scale, cache_seqlens, cosv, sinv,
+                       write_q, &block_table);
+}
+
+// Copies page src to page dst of every array of `arrays` (the K and V pools, and the FP8 scales, of every layer of a
+// paged cache: contiguous, on one device, with the same number of pages P and pages of a multiple of 16 bytes) for
+// each row (src, dst) of `pairs` (int32 [n, 2], on the host, ids in [0, P): checked here).  One launch.
+void kv_page_copy(at::TensorList arrays, const Tensor& pairs) {
+  TORCH_CHECK(pairs.device().is_cpu() && pairs.scalar_type() == at::kInt && pairs.dim() == 2 && pairs.size(1) == 2,
+              "kv_page_copy: pairs must be a host int32 [n, 2] tensor, got ", Got{pairs});
+  TORCH_CHECK(!arrays.empty(), "kv_page_copy: no arrays");
+  const int64_t n = pairs.size(0), P = arrays[0].size(0), A = (int64_t)arrays.size();
+  TORCH_CHECK(A <= 65535, "kv_page_copy: at most 65535 arrays");
+  std::vector<long> desc(2 * n + 2 * A);
+  const Tensor pc = pairs.contiguous();
+  const int* pp = pc.data_ptr<int>();
+  for (int64_t i = 0; i < 2 * n; ++i) {
+    TORCH_CHECK(pp[i] >= 0 && pp[i] < P, "kv_page_copy: page ids must be in [0, ", P, "), got ", pp[i]);
+    desc[i] = pp[i];
+  }
+  for (int64_t a = 0; a < A; ++a) {
+    const Tensor& t = arrays[a];
+    TORCH_CHECK(t.is_cuda() && t.is_contiguous() && t.dim() >= 2 && t.size(0) == P && t.device() == arrays[0].device(),
+                "kv_page_copy: every array must be a contiguous CUDA tensor of ", P, " pages on ", arrays[0].device(),
+                ", got ", Got{t});
+    const int64_t bytes = t.numel() / P * t.element_size();
+    TORCH_CHECK(bytes % 16 == 0 && reinterpret_cast<uintptr_t>(t.data_ptr()) % 16 == 0,
+                "kv_page_copy: pages must be multiples of 16 bytes, 16-byte aligned");
+    desc[2 * n + 2 * a] = reinterpret_cast<long>(t.data_ptr());
+    desc[2 * n + 2 * a + 1] = bytes;
+  }
+  if (n == 0) return;
+  const c10::cuda::CUDAGuard guard(arrays[0].device());
+  Tensor d = at::from_blob(desc.data(), {(int64_t)desc.size()}, at::kLong)
+                 .to(arrays[0].device(), /*non_blocking=*/false, /*copy=*/true);
+  check(lb_kv_page_copy(reinterpret_cast<const long*>(d.data_ptr()), (int)n, (int)A, cur_stream()), "kv_page_copy");
+}
 
 // q [B, Sq, A, D] (any strides with D contiguous, e.g. a view of the packed projection) against the caches [B, G, C, D]
 // (query head h reads cache head h / (A / G)); query i of sample b sees keys kv_start[b] .. cache_seqlens[b] + i.
@@ -1146,23 +1211,33 @@ Tensor kv_append_fp8(const Tensor& qkv, const Tensor& k_cache, const Tensor& v_c
 // (cross-attention; the new tokens are not in this cache), without a bias.  k_scale, v_scale (fp32 [B, G, C]): the row
 // scales of FP8 (E4M3) caches, required for those and rejected otherwise; the scores and outputs are those over the
 // dequantized rows float(e) * s.
-Tensor decode_attn(const Tensor& q, const Tensor& k_cache, const Tensor& v_cache, const Tensor& cache_seqlens,
-                   const Tensor& kv_start, double scale, int64_t splits, const c10::optional<Tensor>& alibi_slopes,
-                   const c10::optional<Tensor>& rel_bias, bool causal, const c10::optional<Tensor>& k_scale,
-                   const c10::optional<Tensor>& v_scale) {
-  Args args("decode_attn");
+// With a block table (int32 [B, max_pages]) the caches are paged (see kv_append_any; no rel_bias, causal only): the
+// kernel runs the same tiles as over a contiguous cache of capacity max_pages * 64, and the same splits.
+Tensor decode_attn_any(const char* op, const Tensor& q, const Tensor& k_cache, const Tensor& v_cache,
+                       const Tensor& cache_seqlens, const Tensor& kv_start, double scale, int64_t splits,
+                       const c10::optional<Tensor>& alibi_slopes, const c10::optional<Tensor>& rel_bias, bool causal,
+                       const c10::optional<Tensor>& k_scale, const c10::optional<Tensor>& v_scale,
+                       const Tensor* table) {
+  Args args(op);
   args("q", q, at::kBFloat16, {kAny, kAny, kAny, kAny}, Layout::LastDimContiguous, 16);
   TORCH_CHECK(q.stride(0) % 8 == 0 && q.stride(1) % 8 == 0 && q.stride(2) % 8 == 0,
-              "decode_attn: q must be 16-byte aligned with strides that are multiples of 8");
+              op, ": q must be 16-byte aligned with strides that are multiples of 8");
   const bool fp8 = k_cache.scalar_type() == at::kFloat8_e4m3fn;
-  TORCH_CHECK(!fp8 || (given(k_scale) && given(v_scale)), "decode_attn: an FP8 cache needs k_scale and v_scale");
-  TORCH_CHECK(fp8 || (!given(k_scale) && !given(v_scale)), "decode_attn: k_scale and v_scale belong to an FP8 cache");
-  cache_args(args, k_cache, v_cache, fp8 ? &*k_scale : nullptr, fp8 ? &*v_scale : nullptr,
-             {q.size(0), kAny, kAny, q.size(3)});
-  const int B = (int)k_cache.size(0), G = (int)k_cache.size(1), C = (int)k_cache.size(2), D = (int)k_cache.size(3);
+  TORCH_CHECK(!fp8 || (given(k_scale) && given(v_scale)), op, ": an FP8 cache needs k_scale and v_scale");
+  TORCH_CHECK(fp8 || (!given(k_scale) && !given(v_scale)), op, ": k_scale and v_scale belong to an FP8 cache");
+  if (table != nullptr)
+    cache_args(args, k_cache, v_cache, fp8 ? &*k_scale : nullptr, fp8 ? &*v_scale : nullptr,
+               {kAny, kAny, 64, q.size(3)});
+  else
+    cache_args(args, k_cache, v_cache, fp8 ? &*k_scale : nullptr, fp8 ? &*v_scale : nullptr,
+               {q.size(0), kAny, kAny, q.size(3)});
+  if (table != nullptr) args("block_table", *table, at::kInt, {q.size(0), kAny});
+  const int max_pages = table != nullptr ? (int)table->size(1) : 0;
+  const int B = (int)q.size(0), G = (int)k_cache.size(1), D = (int)k_cache.size(3);
+  const int C = table != nullptr ? max_pages * 64 : (int)k_cache.size(2);
   const int Sq = (int)q.size(1), A = (int)q.size(2);
-  TORCH_CHECK(A % G == 0, "decode_attn: the query heads must be a multiple of the cache heads");
-  TORCH_CHECK(Sq >= 1 && Sq <= 16, "decode_attn: 1 <= Sq <= 16 new queries");
+  TORCH_CHECK(A % G == 0, op, ": the query heads must be a multiple of the cache heads");
+  TORCH_CHECK(Sq >= 1 && Sq <= 16, op, ": 1 <= Sq <= 16 new queries");
   args("cache_seqlens", cache_seqlens, at::kInt, {B});
   args("kv_start", kv_start, at::kInt, {B});
   const float* slopes = args.opt<const float>("alibi_slopes", alibi_slopes, at::kFloat, {A});
@@ -1172,15 +1247,16 @@ Tensor decode_attn(const Tensor& q, const Tensor& k_cache, const Tensor& v_cache
     const Tensor& r = *rel_bias;
     TORCH_CHECK(r.scalar_type() == at::kFloat && r.dim() == 2 && r.size(0) == A && r.size(1) >= 1 &&
                     r.device() == q.device() && r.is_contiguous(),
-                "decode_attn: rel_bias: contiguous fp32 [A, R] with R >= 1 on q's device, got ", r.scalar_type(), " ",
+                op, ": rel_bias: contiguous fp32 [A, R] with R >= 1 on q's device, got ", r.scalar_type(), " ",
                 r.sizes(), " on ", r.device());
-    TORCH_CHECK(r.size(1) <= INT32_MAX, "decode_attn: rel_bias: R fits in int32");
-    TORCH_CHECK(slopes == nullptr, "decode_attn: alibi_slopes or rel_bias, not both");
+    TORCH_CHECK(r.size(1) <= INT32_MAX, op, ": rel_bias: R fits in int32");
+    TORCH_CHECK(slopes == nullptr, op, ": alibi_slopes or rel_bias, not both");
     rel = r.data_ptr<float>();
     R = (int)r.size(1);
   }
   TORCH_CHECK(causal || (slopes == nullptr && rel == nullptr),
-              "decode_attn: causal=False takes no score bias (neither alibi_slopes nor rel_bias)");
+              op, ": causal=False takes no score bias (neither alibi_slopes nor rel_bias)");
+  TORCH_CHECK(table == nullptr || (rel == nullptr && causal), op, ": a paged cache takes no rel_bias and no causal=False");
   const auto guard = args.guard();
   const int row_blocks = ((A / G) * Sq + 15) / 16;   // (query head, token) rows of one cache head, 16 per CTA
   const int nsplit = splits > 0 ? (int)std::min<int64_t>(splits, 32) : lb_decode_splits(B, G * row_blocks, C, D, fp8);
@@ -1194,10 +1270,26 @@ Tensor decode_attn(const Tensor& q, const Tensor& k_cache, const Tensor& v_cache
   check(lb_decode_attn(q.data_ptr(), qs, k_cache.data_ptr(), v_cache.data_ptr(), o.data_ptr(),
                        nsplit > 1 ? part_o.data_ptr<float>() : nullptr, nsplit > 1 ? part_ml.data_ptr<float>() : nullptr,
                        cache_seqlens.data_ptr<int>(), kv_start.data_ptr<int>(), slopes, rel, R, causal,
-                       fp8 ? k_scale->data_ptr<float>() : nullptr, fp8 ? v_scale->data_ptr<float>() : nullptr, B, Sq, A,
-                       G, C, D, (float)scale, nsplit, cur_stream()),
-        "decode_attn");
+                       fp8 ? k_scale->data_ptr<float>() : nullptr, fp8 ? v_scale->data_ptr<float>() : nullptr,
+                       table != nullptr ? table->data_ptr<int>() : nullptr, max_pages, B, Sq, A, G, C, D, (float)scale,
+                       nsplit, cur_stream()),
+        op);
   return o;
+}
+
+Tensor decode_attn(const Tensor& q, const Tensor& k_cache, const Tensor& v_cache, const Tensor& cache_seqlens,
+                   const Tensor& kv_start, double scale, int64_t splits, const c10::optional<Tensor>& alibi_slopes,
+                   const c10::optional<Tensor>& rel_bias, bool causal, const c10::optional<Tensor>& k_scale,
+                   const c10::optional<Tensor>& v_scale) {
+  return decode_attn_any("decode_attn", q, k_cache, v_cache, cache_seqlens, kv_start, scale, splits, alibi_slopes,
+                         rel_bias, causal, k_scale, v_scale, nullptr);
+}
+Tensor decode_attn_paged(const Tensor& q, const Tensor& k_pool, const Tensor& v_pool, const Tensor& block_table,
+                         const Tensor& cache_seqlens, const Tensor& kv_start, double scale, int64_t splits,
+                         const c10::optional<Tensor>& alibi_slopes, const c10::optional<Tensor>& k_scale,
+                         const c10::optional<Tensor>& v_scale) {
+  return decode_attn_any("decode_attn_paged", q, k_pool, v_pool, cache_seqlens, kv_start, scale, splits, alibi_slopes,
+                         c10::nullopt, true, k_scale, v_scale, &block_table);
 }
 
 // ---- shifted-window attention -----------------------------------------------------------------------
@@ -1498,6 +1590,10 @@ TORCH_LIBRARY(libai_b200, m) {
   m.def("kv_append_fp8(Tensor qkv, Tensor(a!) k_cache, Tensor(b!) v_cache, Tensor(c!) k_scale, Tensor(d!) v_scale, Tensor cache_seqlens, Tensor? cos, Tensor? sin, bool write_q) -> Tensor", &kv_append_fp8);
   m.def("window_attn_fwd(Tensor qkv, int H, int W, int window, int shift, int heads, float scale, Tensor table, Tensor? tau) -> (Tensor, Tensor)", &window_attn_fwd);
   m.def("window_attn_bwd(Tensor dout, Tensor qkv, Tensor lse, int H, int W, int window, int shift, int heads, float scale, Tensor table, Tensor? tau) -> (Tensor, Tensor, Tensor)", &window_attn_bwd);
+  m.def("kv_append_paged(Tensor qkv, Tensor(a!) k_pool, Tensor(b!) v_pool, Tensor block_table, Tensor cache_seqlens, Tensor? cos, Tensor? sin, bool write_q) -> Tensor", &kv_append_paged);
+  m.def("kv_append_fp8_paged(Tensor qkv, Tensor(a!) k_pool, Tensor(b!) v_pool, Tensor(c!) k_scale, Tensor(d!) v_scale, Tensor block_table, Tensor cache_seqlens, Tensor? cos, Tensor? sin, bool write_q) -> Tensor", &kv_append_fp8_paged);
+  m.def("kv_page_copy(Tensor(a!)[] arrays, Tensor pairs) -> ()", &kv_page_copy);
+  m.def("decode_attn_paged(Tensor q, Tensor k_pool, Tensor v_pool, Tensor block_table, Tensor cache_seqlens, Tensor kv_start, float scale, int splits=0, Tensor? alibi_slopes=None, Tensor? k_scale=None, Tensor? v_scale=None) -> Tensor", &decode_attn_paged);
   m.def("decode_attn(Tensor q, Tensor k_cache, Tensor v_cache, Tensor cache_seqlens, Tensor kv_start, float scale, int splits=0, Tensor? alibi_slopes=None, Tensor? rel_bias=None, bool causal=True, Tensor? k_scale=None, Tensor? v_scale=None) -> Tensor", &decode_attn);
   m.def("bias_dropout_residual(Tensor x, Tensor? bias, Tensor? res, float p, int salt, Tensor? rng_state=None) -> (Tensor, Tensor)", &bias_dropout_residual);
 }

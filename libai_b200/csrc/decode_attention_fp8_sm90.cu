@@ -7,29 +7,6 @@
 namespace lb {
 namespace dec {
 
-// IEEE round-to-nearest division, also under --use_fast_math (no flush of subnormals)
-__device__ __forceinline__ float div_rn(float a, float b) {
-  float r;
-  asm("div.rn.f32 %0, %1, %2;" : "=f"(r) : "f"(a), "f"(b));
-  return r;
-}
-
-// one row of an FP8 cache: the scale s = amax / 448 (1 for a zero row) and the bytes e4m3_rn_satfinite(x / s) of the
-// bf16 values x[p], x[p + 1] (columns lane * 2 + 64 * p' and D / 2 past them, see kv_append_fp8_kernel)
-template <int P>
-__device__ __forceinline__ void quantize_row(const float (&x)[2 * P], uint8_t* row, float* scale, int lane) {
-  float amax = 0.f;
-#pragma unroll
-  for (int e = 0; e < 2 * P; ++e) amax = fmaxf(amax, fabsf(x[e]));
-  amax = warp_max(amax);
-  const float s = amax == 0.f ? 1.f : div_rn(amax, 448.f);
-#pragma unroll
-  for (int e = 0; e < 2 * P; ++e)
-    row[(e & 1) * (P * 32) + (e >> 1) * 32 + lane] =
-        __nv_cvt_float_to_fp8(div_rn(x[e], s), __NV_SATFINITE, __NV_E4M3);
-  if (lane == 0) *scale = s;
-}
-
 // the FP8 cache append: one warp per (b, i, group); lane c < D/2 handles the pairs (c + 32 p, c + 32 p + D/2) of the
 // r q rows and of k (rotated, RopePair) and of v, then each of the k and v rows is quantized (quantize_row) at row
 // cache_seqlens[b] + i
@@ -38,49 +15,7 @@ __global__ void __launch_bounds__(256) kv_append_fp8_kernel(
     const __nv_bfloat16* __restrict__ qkv, const float* __restrict__ cosv, const float* __restrict__ sinv,
     __nv_bfloat16* __restrict__ q_out, uint8_t* __restrict__ kc, uint8_t* __restrict__ vc, float* __restrict__ ks,
     float* __restrict__ vs, const int* __restrict__ seqlens, int B, int Sq, int G, int r, int C) {
-  constexpr int half = D / 2, P = half / 32;
-  const int lane = threadIdx.x & 31;
-  const size_t total = (size_t)B * Sq * G;
-  const size_t stride = ((size_t)gridDim.x * blockDim.x) >> 5;
-  for (size_t grp = (blockIdx.x * (size_t)blockDim.x + threadIdx.x) >> 5; grp < total; grp += stride) {
-    const int g = static_cast<int>(grp % G);
-    const int i = static_cast<int>((grp / G) % Sq);
-    const int b = static_cast<int>(grp / ((size_t)G * Sq));
-    const int pos = seqlens[b] + i;
-    const size_t in = grp * (r + 2) * D;
-    const size_t crow = ((size_t)b * G + g) * C + pos;
-    RopePair t[P];
-#pragma unroll
-    for (int p = 0; p < P; ++p) {
-      t[p] = RopePair{1.f, 1.f, 0.f, 0.f};
-      if (cosv != nullptr) t[p] = RopePair::load(cosv, sinv, pos, lane + 32 * p, D);
-    }
-    float kx[2 * P], vx[2 * P];   // the bf16 k and v values of this lane: [2p] column c, [2p + 1] column c + D/2
-    for (int j = 0; j <= r; ++j) {   // slots 0 .. r - 1: q of query head g * r + j; slot r: k
-      const size_t src = in + (size_t)j * D;
-#pragma unroll
-      for (int p = 0; p < P; ++p) {
-        const int c = lane + 32 * p;
-        const float x1 = __bfloat162float(qkv[src + c]), x2 = __bfloat162float(qkv[src + c + half]);
-        const float2 y = cosv != nullptr ? t[p].rotate(x1, x2, false) : make_float2(x1, x2);
-        if (j == r) {
-          kx[2 * p] = __bfloat162float(__float2bfloat16(y.x));
-          kx[2 * p + 1] = __bfloat162float(__float2bfloat16(y.y));
-        } else if (q_out != nullptr) {
-          const size_t qrow = (grp * r + j) * D;
-          q_out[qrow + c] = __float2bfloat16(y.x);
-          q_out[qrow + c + half] = __float2bfloat16(y.y);
-        }
-      }
-    }
-#pragma unroll
-    for (int p = 0; p < P; ++p) {
-      vx[2 * p] = __bfloat162float(qkv[in + (size_t)(r + 1) * D + lane + 32 * p]);
-      vx[2 * p + 1] = __bfloat162float(qkv[in + (size_t)(r + 1) * D + lane + 32 * p + half]);
-    }
-    quantize_row<P>(kx, kc + crow * D, ks + crow, lane);
-    quantize_row<P>(vx, vc + crow * D, vs + crow, lane);
-  }
+  kv_append_fp8_body<D, false>(qkv, cosv, sinv, q_out, kc, vc, ks, vs, seqlens, nullptr, 0, B, Sq, G, r, C);
 }
 
 template <int D, Score S>

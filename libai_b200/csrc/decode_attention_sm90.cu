@@ -37,6 +37,8 @@
 //   cache_seqlens[b], the new tokens not being in that cache.
 //   The kernel template lives in decode_attention_sm90.cuh; its ALiBi instances are compiled in
 //   decode_attention_alibi_sm90.cu and its T5 instances in decode_attention_t5_sm90.cu.
+//   Paged caches (decode_attention_paged_sm90.cu, with their appends): pools of 64-row pages and a block table per
+//   sample; the same tiles, so the same output bit for bit.
 //   FP8 (E4M3) caches (decode_attention_fp8_sm90.cu, with their quantizing append): K, V bytes with one fp32 scale per
 //   row; every score kind at both head dims, one bulk copy per tile and array, the scales folded into the scores and
 //   probabilities (Cfg8 and decode_attn_body in decode_attention_sm90.cuh).
@@ -80,35 +82,7 @@ __global__ void kv_append_kernel(const __nv_bfloat16* __restrict__ qkv, const fl
                                  const float* __restrict__ sinv, __nv_bfloat16* __restrict__ q_out,
                                  __nv_bfloat16* __restrict__ kc, __nv_bfloat16* __restrict__ vc,
                                  const int* __restrict__ seqlens, int B, int Sq, int G, int r, int C, int D) {
-  const int half = D / 2;
-  const size_t total = (size_t)B * Sq * G * half;
-  for (size_t idx = blockIdx.x * (size_t)blockDim.x + threadIdx.x; idx < total; idx += (size_t)gridDim.x * blockDim.x) {
-    const int c = static_cast<int>(idx % half);
-    const size_t grp = idx / half;               // (b * Sq + i) * G + g
-    const int g = static_cast<int>(grp % G);
-    const int i = static_cast<int>((grp / G) % Sq);
-    const int b = static_cast<int>(grp / ((size_t)G * Sq));
-    const int pos = seqlens[b] + i;
-    const size_t in = grp * (r + 2) * D;
-    const size_t crow = (((size_t)b * G + g) * C + pos) * D;
-    RopePair t{1.f, 1.f, 0.f, 0.f};
-    if (cosv != nullptr) t = RopePair::load(cosv, sinv, pos, c, D);
-    for (int j = 0; j <= r; ++j) {   // slots 0 .. r - 1: q of query head g * r + j; slot r: k
-      const size_t src = in + (size_t)j * D;
-      const float x1 = __bfloat162float(qkv[src + c]), x2 = __bfloat162float(qkv[src + c + half]);
-      const float2 y = cosv != nullptr ? t.rotate(x1, x2, false) : make_float2(x1, x2);
-      if (j == r) {
-        kc[crow + c] = __float2bfloat16(y.x);
-        kc[crow + c + half] = __float2bfloat16(y.y);
-      } else if (q_out != nullptr) {
-        const size_t qrow = (grp * r + j) * D;    // [B, Sq, A, D] with A = G * r
-        q_out[qrow + c] = __float2bfloat16(y.x);
-        q_out[qrow + c + half] = __float2bfloat16(y.y);
-      }
-    }
-    vc[crow + c] = qkv[in + (size_t)(r + 1) * D + c];
-    vc[crow + c + half] = qkv[in + (size_t)(r + 1) * D + c + half];
-  }
+  kv_append_body<false>(qkv, cosv, sinv, q_out, kc, vc, seqlens, nullptr, 0, B, Sq, G, r, C, D);
 }
 
 }  // namespace dec
@@ -116,10 +90,12 @@ __global__ void kv_append_kernel(const __nv_bfloat16* __restrict__ qkv, const fl
 
 namespace {
 template <int D>
-cudaError_t launch_decode(const lb::dec::Params& p, const float* k_scale, const float* v_scale, int B, int nsplit,
-                          lb::dec::Score score, cudaStream_t s) {
+cudaError_t launch_decode(const lb::dec::Params& p, const float* k_scale, const float* v_scale, const int* block_table,
+                          int max_pages, int B, int nsplit, lb::dec::Score score, cudaStream_t s) {
   using lb::dec::Score;
-  cudaError_t e = k_scale != nullptr      ? lb::dec::launch_decode_attn_fp8(p, k_scale, v_scale, score, D, B, nsplit, s)
+  cudaError_t e = block_table != nullptr ? lb::dec::launch_decode_attn_paged(p, k_scale, v_scale, block_table,
+                                                                             max_pages, score, D, B, nsplit, s)
+                  : k_scale != nullptr     ? lb::dec::launch_decode_attn_fp8(p, k_scale, v_scale, score, D, B, nsplit, s)
                   : score == Score::kAlibi ? lb::dec::launch_decode_attn_alibi(p, D, B, nsplit, s)
                   : score == Score::kNone  ? lb::dec::launch_decode_attn<D, Score::kNone>(p, B, nsplit, s)
                                            : lb::dec::launch_decode_attn_t5(p, score, D, B, nsplit, s);
@@ -148,8 +124,8 @@ extern "C" int lb_decode_splits(int B, int blocks, int C, int D, bool fp8) {
 extern "C" int lb_decode_attn(const void* q, const long* q_strides, const void* k, const void* v, void* o,
                               float* part_o, float* part_ml, const int* seqlens, const int* kv_start,
                               const float* alibi_slopes, const float* rel_bias, int R, bool causal,
-                              const float* k_scale, const float* v_scale, int B, int Sq, int A, int G, int C, int D,
-                              float scale, int nsplit, cudaStream_t s) {
+                              const float* k_scale, const float* v_scale, const int* block_table, int max_pages, int B,
+                              int Sq, int A, int G, int C, int D, float scale, int nsplit, cudaStream_t s) {
   if (B == 0 || A == 0) return 0;
   if (G <= 0 || A % G) return -4;
   // the four kinds: no bias or ALiBi or T5's relative bias (causal), no bias (non-causal)
@@ -181,8 +157,8 @@ extern "C" int lb_decode_attn(const void* q, const long* q_strides, const void* 
                       : rel_bias != nullptr   ? Score::kRelBias
                       : !causal               ? Score::kWindow
                                               : Score::kNone;
-  cudaError_t e = D == 64 ? launch_decode<64>(p, k_scale, v_scale, B, nsplit, score, s)
-                          : launch_decode<128>(p, k_scale, v_scale, B, nsplit, score, s);
+  cudaError_t e = D == 64 ? launch_decode<64>(p, k_scale, v_scale, block_table, max_pages, B, nsplit, score, s)
+                          : launch_decode<128>(p, k_scale, v_scale, block_table, max_pages, B, nsplit, score, s);
   return (int)e;
 }
 

@@ -74,9 +74,15 @@ LB_DEVICE void bulk_load(void* dst, const void* src, uint32_t bytes, uint64_t* b
 
 // FP8: p.k / p.v point at the E4M3 bytes and k_scale / v_scale at their row scales; key j's score is
 // scale·s^k_j·(q·ê_j), and P·V runs on P_j·s^v_j while the softmax sums P_j.
-template <int D, Score S, bool FP8 = false>
+// PAGED (decode_attention_paged_sm90.cu): p.k, p.v (and the FP8 scales) are pools of pages [P, G, kTile, D]
+// ([P, G, kTile]), logical row j of sample b is row j % kTile of page block_table[b * max_pages + j / kTile], and
+// p.C = max_pages * kTile.  Only the producer's addresses change: the tiles still start at kv_start[b], not at page
+// boundaries, so every sum runs in the order of the contiguous kernel and the result is bit-identical to it over the
+// same logical rows.  (The table is not a field of Params: a larger Params changes the code of every other instance.)
+template <int D, Score S, bool FP8 = false, bool PAGED = false>
 __device__ __forceinline__ void decode_attn_body(const Params& p, const float* k_scale = nullptr,
-                                                 const float* v_scale = nullptr) {
+                                                 const float* v_scale = nullptr, const int* block_table = nullptr,
+                                                 int max_pages = 0) {
   constexpr bool ALIBI = S == Score::kAlibi;
   using C = std::conditional_t<FP8, Cfg8<D>, Cfg<D>>;
   extern __shared__ __align__(128) unsigned char smem[];
@@ -129,10 +135,34 @@ __device__ __forceinline__ void decode_attn_body(const Params& p, const float* k
         const int n = min(kTile, hi - base), ns = (soff + n + 3) & ~3;
         unsigned char* sk = smem + st * C::kStageBytes;
         mbar_arrive_expect_tx(&full[st], 2 * n * D + 2 * ns * 4);
-        bulk_load(sk, kg + (long)base * D, n * D, &full[st]);
-        bulk_load(sk + kTile * D, vg + (long)base * D, n * D, &full[st]);
-        bulk_load(sk + 2 * kTile * D, k_scale + srow + base - soff, ns * 4, &full[st]);
-        bulk_load(sk + 2 * kTile * D + C::kScales * 4, v_scale + srow + base - soff, ns * 4, &full[st]);
+        if constexpr (PAGED) {
+          // A tile spans at most two pages: one piece of each array per page.  The scales start at the 4-row boundary
+          // base - soff, in the page of base (page boundaries are multiples of 4 rows), and end at the 4-row boundary
+          // at or past base + n, which passes the page boundary only when the rows do: every piece of bytes and of
+          // scales starts and ends on a 16-byte boundary, as in the contiguous layout.
+          const int* table = block_table + (long)b * max_pages;
+          for (int r = base - soff; r < base - soff + ns;) {
+            const int end = min((r / kTile + 1) * kTile, base - soff + ns);
+            const long pg = ((long)table[r / kTile] * p.G + kvh) * kTile;
+            const int b0 = max(r, base), b1 = min(end, base + n);   // the rows of the piece
+            if (b1 > b0) {
+              bulk_load(sk + (b0 - base) * D, reinterpret_cast<const uint8_t*>(p.k) + (pg + b0 % kTile) * D,
+                        (b1 - b0) * D, &full[st]);
+              bulk_load(sk + kTile * D + (b0 - base) * D,
+                        reinterpret_cast<const uint8_t*>(p.v) + (pg + b0 % kTile) * D, (b1 - b0) * D, &full[st]);
+            }
+            const int s0 = r - (base - soff);
+            bulk_load(sk + 2 * kTile * D + s0 * 4, k_scale + pg + r % kTile, (end - r) * 4, &full[st]);
+            bulk_load(sk + 2 * kTile * D + C::kScales * 4 + s0 * 4, v_scale + pg + r % kTile, (end - r) * 4,
+                      &full[st]);
+            r = end;
+          }
+        } else {
+          bulk_load(sk, kg + (long)base * D, n * D, &full[st]);
+          bulk_load(sk + kTile * D, vg + (long)base * D, n * D, &full[st]);
+          bulk_load(sk + 2 * kTile * D, k_scale + srow + base - soff, ns * 4, &full[st]);
+          bulk_load(sk + 2 * kTile * D + C::kScales * 4, v_scale + srow + base - soff, ns * 4, &full[st]);
+        }
       }
     } else {
       // producer: rows past the window repeat its last row (finite data; those keys get zero weight)
@@ -149,8 +179,15 @@ __device__ __forceinline__ void decode_attn_body(const Params& p, const float* k
   #pragma unroll
         for (int r = lane; r < kTile; r += 32) {
           const long row = min(base + r, hi - 1);
-          bulk_load(sk + r * C::kRow, kg + row * D, D * 2, &full[st]);
-          bulk_load(sv + r * C::kRow, vg + row * D, D * 2, &full[st]);
+          if constexpr (PAGED) {
+            const long at = (((long)block_table[(long)b * max_pages + row / kTile] * p.G + kvh) * kTile +
+                             row % kTile) * D;
+            bulk_load(sk + r * C::kRow, p.k + at, D * 2, &full[st]);
+            bulk_load(sv + r * C::kRow, p.v + at, D * 2, &full[st]);
+          } else {
+            bulk_load(sk + r * C::kRow, kg + row * D, D * 2, &full[st]);
+            bulk_load(sv + r * C::kRow, vg + row * D, D * 2, &full[st]);
+          }
         }
       }
     }
@@ -374,6 +411,129 @@ __device__ __forceinline__ void decode_attn_body(const Params& p, const float* k
   }
 }
 
+// The row of a cache that holds logical row pos of sample b, cache head g: [B, G, C, D] caches, or (PAGED) pools of
+// pages [P, G, kTile, D] through the block table [B, max_pages]
+template <bool PAGED>
+__device__ __forceinline__ size_t cache_row(const int* table, int max_pages, int b, int g, int G, int C, int pos) {
+  if constexpr (PAGED)
+    return ((size_t)table[(size_t)b * max_pages + pos / kTile] * G + g) * kTile + pos % kTile;
+  else
+    return ((size_t)b * G + g) * C + pos;
+}
+
+// the bf16 cache append (kv_append_kernel, and its paged instance): one thread per (b, i, group, c < D/2)
+template <bool PAGED>
+__device__ __forceinline__ void kv_append_body(const __nv_bfloat16* __restrict__ qkv, const float* __restrict__ cosv,
+                                               const float* __restrict__ sinv, __nv_bfloat16* __restrict__ q_out,
+                                               __nv_bfloat16* __restrict__ kc, __nv_bfloat16* __restrict__ vc,
+                                               const int* __restrict__ seqlens, const int* __restrict__ table,
+                                               int max_pages, int B, int Sq, int G, int r, int C, int D) {
+  const int half = D / 2;
+  const size_t total = (size_t)B * Sq * G * half;
+  for (size_t idx = blockIdx.x * (size_t)blockDim.x + threadIdx.x; idx < total; idx += (size_t)gridDim.x * blockDim.x) {
+    const int c = static_cast<int>(idx % half);
+    const size_t grp = idx / half;               // (b * Sq + i) * G + g
+    const int g = static_cast<int>(grp % G);
+    const int i = static_cast<int>((grp / G) % Sq);
+    const int b = static_cast<int>(grp / ((size_t)G * Sq));
+    const int pos = seqlens[b] + i;
+    const size_t in = grp * (r + 2) * D;
+    const size_t crow = cache_row<PAGED>(table, max_pages, b, g, G, C, pos) * D;
+    RopePair t{1.f, 1.f, 0.f, 0.f};
+    if (cosv != nullptr) t = RopePair::load(cosv, sinv, pos, c, D);
+    for (int j = 0; j <= r; ++j) {   // slots 0 .. r - 1: q of query head g * r + j; slot r: k
+      const size_t src = in + (size_t)j * D;
+      const float x1 = __bfloat162float(qkv[src + c]), x2 = __bfloat162float(qkv[src + c + half]);
+      const float2 y = cosv != nullptr ? t.rotate(x1, x2, false) : make_float2(x1, x2);
+      if (j == r) {
+        kc[crow + c] = __float2bfloat16(y.x);
+        kc[crow + c + half] = __float2bfloat16(y.y);
+      } else if (q_out != nullptr) {
+        const size_t qrow = (grp * r + j) * D;    // [B, Sq, A, D] with A = G * r
+        q_out[qrow + c] = __float2bfloat16(y.x);
+        q_out[qrow + c + half] = __float2bfloat16(y.y);
+      }
+    }
+    vc[crow + c] = qkv[in + (size_t)(r + 1) * D + c];
+    vc[crow + c + half] = qkv[in + (size_t)(r + 1) * D + c + half];
+  }
+}
+
+// IEEE round-to-nearest division, also under --use_fast_math (no flush of subnormals)
+__device__ __forceinline__ float div_rn(float a, float b) {
+  float r;
+  asm("div.rn.f32 %0, %1, %2;" : "=f"(r) : "f"(a), "f"(b));
+  return r;
+}
+
+// one row of an FP8 cache: the scale s = amax / 448 (1 for a zero row) and the bytes e4m3_rn_satfinite(x / s) of the
+// bf16 values x[p], x[p + 1] (columns lane * 2 + 64 * p' and D / 2 past them, see kv_append_fp8_kernel)
+template <int P>
+__device__ __forceinline__ void quantize_row(const float (&x)[2 * P], uint8_t* row, float* scale, int lane) {
+  float amax = 0.f;
+#pragma unroll
+  for (int e = 0; e < 2 * P; ++e) amax = fmaxf(amax, fabsf(x[e]));
+  amax = warp_max(amax);
+  const float s = amax == 0.f ? 1.f : div_rn(amax, 448.f);
+#pragma unroll
+  for (int e = 0; e < 2 * P; ++e)
+    row[(e & 1) * (P * 32) + (e >> 1) * 32 + lane] =
+        __nv_cvt_float_to_fp8(div_rn(x[e], s), __NV_SATFINITE, __NV_E4M3);
+  if (lane == 0) *scale = s;
+}
+
+// the FP8 cache append (kv_append_fp8_kernel, and its paged instance); see kv_append_fp8_kernel
+template <int D, bool PAGED>
+__device__ __forceinline__ void kv_append_fp8_body(
+    const __nv_bfloat16* __restrict__ qkv, const float* __restrict__ cosv, const float* __restrict__ sinv,
+    __nv_bfloat16* __restrict__ q_out, uint8_t* __restrict__ kc, uint8_t* __restrict__ vc, float* __restrict__ ks,
+    float* __restrict__ vs, const int* __restrict__ seqlens, const int* __restrict__ table, int max_pages, int B,
+    int Sq, int G, int r, int C) {
+  constexpr int half = D / 2, P = half / 32;
+  const int lane = threadIdx.x & 31;
+  const size_t total = (size_t)B * Sq * G;
+  const size_t stride = ((size_t)gridDim.x * blockDim.x) >> 5;
+  for (size_t grp = (blockIdx.x * (size_t)blockDim.x + threadIdx.x) >> 5; grp < total; grp += stride) {
+    const int g = static_cast<int>(grp % G);
+    const int i = static_cast<int>((grp / G) % Sq);
+    const int b = static_cast<int>(grp / ((size_t)G * Sq));
+    const int pos = seqlens[b] + i;
+    const size_t in = grp * (r + 2) * D;
+    const size_t crow = cache_row<PAGED>(table, max_pages, b, g, G, C, pos);
+    RopePair t[P];
+#pragma unroll
+    for (int p = 0; p < P; ++p) {
+      t[p] = RopePair{1.f, 1.f, 0.f, 0.f};
+      if (cosv != nullptr) t[p] = RopePair::load(cosv, sinv, pos, lane + 32 * p, D);
+    }
+    float kx[2 * P], vx[2 * P];   // the bf16 k and v values of this lane: [2p] column c, [2p + 1] column c + D/2
+    for (int j = 0; j <= r; ++j) {   // slots 0 .. r - 1: q of query head g * r + j; slot r: k
+      const size_t src = in + (size_t)j * D;
+#pragma unroll
+      for (int p = 0; p < P; ++p) {
+        const int c = lane + 32 * p;
+        const float x1 = __bfloat162float(qkv[src + c]), x2 = __bfloat162float(qkv[src + c + half]);
+        const float2 y = cosv != nullptr ? t[p].rotate(x1, x2, false) : make_float2(x1, x2);
+        if (j == r) {
+          kx[2 * p] = __bfloat162float(__float2bfloat16(y.x));
+          kx[2 * p + 1] = __bfloat162float(__float2bfloat16(y.y));
+        } else if (q_out != nullptr) {
+          const size_t qrow = (grp * r + j) * D;
+          q_out[qrow + c] = __float2bfloat16(y.x);
+          q_out[qrow + c + half] = __float2bfloat16(y.y);
+        }
+      }
+    }
+#pragma unroll
+    for (int p = 0; p < P; ++p) {
+      vx[2 * p] = __bfloat162float(qkv[in + (size_t)(r + 1) * D + lane + 32 * p]);
+      vx[2 * p + 1] = __bfloat162float(qkv[in + (size_t)(r + 1) * D + lane + 32 * p + half]);
+    }
+    quantize_row<P>(kx, kc + crow * D, ks + crow, lane);
+    quantize_row<P>(vx, vc + crow * D, vs + crow, lane);
+  }
+}
+
 template <int D, bool ALIBI>
 __global__ void __launch_bounds__(kThreads) decode_attn_kernel(const Params p) {
   decode_attn_body<D, ALIBI ? Score::kAlibi : Score::kNone>(p);
@@ -423,6 +583,10 @@ cudaError_t launch_decode_attn_fp8(const Params& p, const float* k_scale, const 
                                    int nsplit, cudaStream_t s);
 // CTAs per SM of the FP8 instances at head dim D (0 when the shared memory opt-in failed)
 int decode_fp8_resident(int D);
+// the paged instances (decode_attention_paged_sm90.cu): S is kNone or kAlibi, bf16 or (k_scale given) FP8, D 64 or 128
+cudaError_t launch_decode_attn_paged(const Params& p, const float* k_scale, const float* v_scale,
+                                     const int* block_table, int max_pages, Score S, int D, int B, int nsplit,
+                                     cudaStream_t s);
 
 }  // namespace dec
 }  // namespace lb

@@ -134,17 +134,31 @@ int lb_bias_dropout_residual(const void* x, const void* bias, const void* res, v
                              const lb::RngArgs* rng, const long long* rng_in, long long* rng_out, cudaStream_t s);
 int lb_spin_timeout_report(char* buf, int n);
 int lb_decode_splits(int B, int blocks, int C, int D, bool fp8);
-// k_scale, v_scale (fp32 [B, G, C], C a multiple of 4): k and v are an FP8 (E4M3) cache with these row scales
+// k_scale, v_scale (fp32 [B, G, C], C a multiple of 4): k and v are an FP8 (E4M3) cache with these row scales.
+// block_table (int32 [B, max_pages], or null): k, v (and the scales) are pools of 64-row pages [P, G, 64, D]
+// ([P, G, 64]) and C = max_pages * 64; no score bias or ALiBi only
 int lb_decode_attn(const void* q, const long* q_strides, const void* k, const void* v, void* o, float* part_o,
                    float* part_ml, const int* seqlens, const int* kv_start, const float* alibi_slopes,
-                   const float* rel_bias, int R, bool causal, const float* k_scale, const float* v_scale, int B, int Sq,
-                   int A, int G, int C, int D, float scale, int nsplit, cudaStream_t s);
+                   const float* rel_bias, int R, bool causal, const float* k_scale, const float* v_scale,
+                   const int* block_table, int max_pages, int B, int Sq, int A, int G, int C, int D, float scale,
+                   int nsplit, cudaStream_t s);
 int lb_kv_append(const void* qkv, const float* cosv, const float* sinv, void* q_out, void* k_cache, void* v_cache,
                  const int* seqlens, int B, int Sq, int G, int r, int C, int D, cudaStream_t s);
 // lb_kv_append into an FP8 (E4M3) cache: each k and v row is stored as bytes [B, G, C, D] and an fp32 scale [B, G, C]
 int lb_kv_append_fp8(const void* qkv, const float* cosv, const float* sinv, void* q_out, void* k_cache, void* v_cache,
                      float* k_scale, float* v_scale, const int* seqlens, int B, int Sq, int G, int r, int C, int D,
                      cudaStream_t s);
+// lb_kv_append and lb_kv_append_fp8 into paged caches: pools [P, G, 64, D] (scales [P, G, 64]), logical row
+// seqlens[b] + i at row (seqlens[b] + i) % 64 of page block_table[b][(seqlens[b] + i) / 64]
+int lb_kv_append_paged(const void* qkv, const float* cosv, const float* sinv, void* q_out, void* k_pool, void* v_pool,
+                       const int* seqlens, const int* block_table, int max_pages, int B, int Sq, int G, int r, int D,
+                       cudaStream_t s);
+int lb_kv_append_fp8_paged(const void* qkv, const float* cosv, const float* sinv, void* q_out, void* k_pool,
+                           void* v_pool, float* k_scale, float* v_scale, const int* seqlens, const int* block_table,
+                           int max_pages, int B, int Sq, int G, int r, int D, cudaStream_t s);
+// desc (device int64): npairs (src, dst) page pairs, then per array its address and page bytes (a multiple of 16);
+// copies page src to page dst of every array
+int lb_kv_page_copy(const long* desc, int npairs, int narrays, cudaStream_t s);
 // y [M, N] bf16 = act((x [M, K] bf16 · float(w [N, K] E4M3)ᵀ) · w_scale [N] + bias [N]) with 1 <= M <= 64 and
 // K % 16 == 0; bias (bf16 [N]) may be null.  part: an fp32 workspace of lb_linear_fp8w_workspace(M, N, K) floats (null
 // when that is 0).

@@ -16,7 +16,9 @@ every step the cache rows, ``seqlens``, ``kv_start`` and the host mirror are wha
 A graph is kept per model and keyed by the batch, the caches' buffer addresses, capacity and KV dtype, the weights'
 addresses and the step's input signature; a new key captures again and frees the old graph's memory pool.  A model
 that allocates a new cache drops its graph at once, so a replaced cache's buffers are not kept alive by it.  Beam
-search's in-place ``StaticKVCache.reorder_`` keeps the key.  A step the graph cannot reproduce runs eagerly, with the
+search's in-place ``StaticKVCache.reorder_`` keeps the key, and so does a :class:`PagedKVCache`'s reorder, which
+rewrites its block table in place; such a cache maps the pages of a step's rows before the capture and before every
+replay.  A step the graph cannot reproduce runs eagerly, with the
 same tokens and one log line per reason (:func:`fallback_reason`), and so does every step of a key whose capture
 failed.
 """
@@ -32,7 +34,7 @@ from libai_b200 import ops
 from libai_b200.ops import use_native
 from libai_b200.utils import distributed as dutil
 
-from .kv_cache import StaticKVCache
+from .kv_cache import PagedKVCache, StaticKVCache
 
 logger = logging.getLogger(__name__)
 
@@ -62,8 +64,11 @@ def _caches(model):
 
 def _cache_key(c: StaticKVCache):
     # addresses, not the object: the graph reads and writes these buffers and nothing else of the cache, and a key
-    # that held the cache would keep a replaced one's buffers alive
+    # that held the cache would keep a replaced one's buffers alive (a paged cache: its pools and block table, which
+    # a reorder rewrites in place)
     buffers = [t for bufs in (c.k, c.v, c.k_scale, c.v_scale) for t in bufs if t is not None]
+    if isinstance(c, PagedKVCache):
+        buffers.append(c.block_table)
     return (c.batch, c.capacity, c.kv_dtype, tuple(t.data_ptr() for t in buffers), c.seqlens.data_ptr(),
             c.kv_start.data_ptr())
 
@@ -138,6 +143,8 @@ class DecodeGraph:
         return self.replay(model, inputs)
 
     def _capture(self, model, inputs: Dict):
+        # a paged cache maps (and copies on write) the pages of the step's rows now: the captured step must not
+        model.kv_cache.reserve(self.tokens)
         caches = _caches(model)
         lengths, past = [c.length for c in caches], model.past_length
         call = {**inputs, **self.static}
@@ -166,6 +173,8 @@ class DecodeGraph:
     def replay(self, model, inputs: Dict):
         for k, v in self.static.items():
             v.copy_(inputs[k])
+        # a replayed step runs no Python: the pages of its rows are mapped first (a contiguous cache has its rows)
+        model.kv_cache.reserve(self.tokens)
         self.graph.replay()
         ops.count_launch(self.launches)
         cache = model.kv_cache

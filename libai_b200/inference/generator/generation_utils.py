@@ -25,7 +25,7 @@ from libai_b200.utils import distributed as dutil
 import torch.distributed as dist
 
 from .. import decode_graph
-from ..kv_cache import KVCacheOwner, StaticKVCache
+from ..kv_cache import KVCacheOwner, PagedKVCache, StaticKVCache
 from .generation_beam_search import BeamScorer, BeamSearchScorer
 from .generation_logits_processor import (
     EncoderNoRepeatNGramLogitsProcessor,
@@ -62,7 +62,7 @@ _DEFAULTS = dict(
     pad_token_id=None, decoder_start_token_id=None, forced_bos_token_id=None, forced_eos_token_id=None,
     remove_invalid_values=False, exponential_decay_length_penalty=None, chunk_size_feed_forward=0,
     kv_cache_dtype=None, decode_graphs=False, assistant_model=None, num_assistant_tokens=None,
-    prompt_lookup_num_tokens=None, max_matching_ngram_size=None,
+    prompt_lookup_num_tokens=None, max_matching_ngram_size=None, paged_kv_cache=False,
 )
 # generate()'s arguments for the logits processors speculative decoding refuses, by processor
 _PROCESSOR_ARGS = {
@@ -111,10 +111,18 @@ def _decode_graphs(value) -> bool:
     return value
 
 
+def _paged_kv_cache(value) -> bool:
+    """``generate(paged_kv_cache=...)``: a bool."""
+    if not isinstance(value, bool):
+        raise ValueError(f"paged_kv_cache must be True or False, got {value!r}")
+    return value
+
+
 @contextlib.contextmanager
-def _call_state(model, kv_cache_dtype, decode_graphs: bool):
+def _call_state(model, kv_cache_dtype, decode_graphs: bool, paging=None):
     """A model's state for one ``generate()`` call, restored when it ends: eval mode, the call's cache format when it
-    gives one (``allocate_kv_cache`` reads it) and, with ``decode_graphs``, its decode graphs."""
+    gives one (``allocate_kv_cache`` reads it: ``kv_cache_dtype``, and ``paging`` = (sequences per prompt, prompt
+    length) for a paged cache) and, with ``decode_graphs``, its decode graphs."""
     was_training, saved_kv_cache_dtype = model.training, getattr(model, "kv_cache_dtype", None)
     model.eval()
     try:
@@ -122,6 +130,8 @@ def _call_state(model, kv_cache_dtype, decode_graphs: bool):
             model.kv_cache_dtype = kv_cache_dtype
         if decode_graphs:
             model._decode_graphs = decode_graph.DecodeCall()
+        if paging is not None:
+            model.kv_cache_paging = paging
         yield
     finally:
         model.train(was_training)
@@ -129,6 +139,8 @@ def _call_state(model, kv_cache_dtype, decode_graphs: bool):
             model.kv_cache_dtype = saved_kv_cache_dtype
         if decode_graphs:
             del model._decode_graphs   # back to the class's None
+        if paging is not None:
+            del model.kv_cache_paging
 
 
 class Generator:
@@ -467,8 +479,9 @@ class Generator:
         eos_token_id = self._pick(eos_token_id, "eos_token_id")
         scores = () if output_scores else None
         unfinished = torch.ones(input_ids.shape[0], dtype=torch.long, device=input_ids.device)
+        first = model_kwargs.pop("_first_step", None)   # the outputs of a shared prefill (_shared_prefill)
         while True:
-            outputs = self._decode_step(input_ids, model_kwargs)
+            outputs, first = (self._decode_step(input_ids, model_kwargs) if first is None else first), None
             next_scores = logits_warper(input_ids, logits_processor(input_ids, self._step_logits(outputs)))
             if output_scores:
                 scores += (next_scores,)
@@ -508,8 +521,9 @@ class Generator:
         beam_scores = torch.zeros((batch_size, num_beams), dtype=torch.float32, device=input_ids.device)
         beam_scores[:, 1:] = -1e9  # all beams start identical: only the first one may spawn continuations
         beam_scores = beam_scores.view(-1)
+        first = model_kwargs.pop("_first_step", None)   # the outputs of a shared prefill (_shared_prefill)
         while True:
-            outputs = self._decode_step(input_ids, model_kwargs)
+            outputs, first = (self._decode_step(input_ids, model_kwargs) if first is None else first), None
             logprobs = torch.log_softmax(self._step_logits(outputs), dim=-1)
             processed = logits_processor(input_ids, logprobs)
             next_scores = processed + beam_scores[:, None]
@@ -541,6 +555,22 @@ class Generator:
         if output_scores:
             return result["sequences"], result["sequence_scores"], scores
         return result["sequences"]
+
+    def _shared_prefill(self, input_ids, n: int, model_kwargs):
+        """The prefill of the ``b`` prompts once, on a paged cache, which then forks into ``n`` sequences per prompt
+        (:meth:`PagedKVCache.fork`).  Other per-sequence inputs given for all ``b * n`` sequences (GLM's positions) are
+        taken once per prompt.  Returns the expanded ``input_ids`` and ``model_kwargs`` of the decoding loop, whose
+        ``_first_step`` holds the prefill's last logits, each prompt's row repeated for its ``n`` sequences."""
+        b = input_ids.shape[0]
+        once = {k: v[::n] if torch.is_tensor(v) and v.dim() > 0 and v.shape[0] == b * n else v
+                for k, v in model_kwargs.items()}
+        outputs = self._decode_step(input_ids, once)
+        self.kv_cache.fork(n)
+        key = "logits" if "logits" in outputs else "prediction_scores"
+        first = {key: outputs[key][:, -1:].repeat_interleave(n, dim=0)}
+        input_ids, model_kwargs = self._expand_inputs_for_generation(input_ids, expand_size=n, **model_kwargs)
+        model_kwargs["_first_step"] = first
+        return input_ids, model_kwargs
 
     # a decoder-only model whose cached step takes ``{"input_ids": [b, s], "use_cache": True}`` for any s (positions and
     # padding from its StaticKVCache): it can verify speculative proposals, and serve as a draft
@@ -789,7 +819,7 @@ class Generator:
                  forced_bos_token_id=None, forced_eos_token_id=None, remove_invalid_values=None,
                  exponential_decay_length_penalty=None, kv_cache_dtype=None, decode_graphs=None, assistant_model=None,
                  num_assistant_tokens=None, prompt_lookup_num_tokens=None, max_matching_ngram_size=None,
-                 **model_kwargs):
+                 paged_kv_cache=None, **model_kwargs):
         """``kv_cache_dtype`` (default: the model cfg's ``kv_cache_dtype``): ``"fp8"`` or ``torch.float8_e4m3fn`` holds
         the preallocated KV cache as E4M3 rows with per-row scales
         (:class:`~libai_b200.inference.kv_cache.StaticKVCache`) for this call: about half the memory, and of the bytes
@@ -813,8 +843,27 @@ class Generator:
         ``num_return_sequences`` expands the inputs as ``multinomial_sample`` does.  Beams, ``typical_p < 1``,
         ``do_sample`` with prompt lookup, ``num_return_sequences > 1`` without sampling, logits processors (including
         ``renormalize_logits``), custom stopping criteria, encoder-decoder and GLM models, tensor or pipeline
-        parallelism and a prompt whose padding needs a dense mask raise ``ValueError``."""
+        parallelism and a prompt whose padding needs a dense mask raise ``ValueError``.
+
+        ``paged_kv_cache`` (default: the model cfg's ``paged_kv_cache``, else False): True holds the cache in 64-row
+        pages (:class:`~libai_b200.inference.kv_cache.PagedKVCache`), with the tokens of the contiguous cache.  Beam
+        search, and sampling with ``num_return_sequences > 1``, then prefill each prompt once and fork its cache into
+        the beams or samples, which share the prompt's pages; a beam reorder rewrites block tables instead of copying
+        the cache.  Greedy search and single-sequence sampling run on pages without a fork.  Encoder-decoder models
+        (T5/mT5) and models without a preallocated cache, tensor or pipeline parallelism, and speculative decoding
+        raise ``ValueError``."""
         kv_cache_dtype = _kv_cache_dtype(self._pick(kv_cache_dtype, "kv_cache_dtype"))
+        paged = _paged_kv_cache(self._pick(paged_kv_cache, "paged_kv_cache"))
+        if paged:
+            if not isinstance(self, KVCacheOwner) or self._gcfg("is_encoder_decoder"):
+                raise ValueError(f"paged_kv_cache=True: {type(self).__name__} is not a decoder-only model with a "
+                                 "preallocated KV cache")
+            topo = dutil.get_dist_util()
+            if topo.tensor_parallel_size > 1 or topo.pipeline_parallel_size > 1:
+                raise ValueError("paged_kv_cache=True: tensor- and pipeline-parallel inference keep contiguous caches")
+            if assistant_model is not None or prompt_lookup_num_tokens is not None:
+                raise ValueError("paged_kv_cache=True: speculative decoding (assistant_model, prompt_lookup_num_tokens) "
+                                 "runs on contiguous caches")
         if kv_cache_dtype is not None and not isinstance(self, KVCacheOwner):
             raise ValueError(f"kv_cache_dtype={kv_cache_dtype}: {type(self).__name__} does not decode on a "
                              "StaticKVCache")
@@ -907,15 +956,18 @@ class Generator:
                 draft, num_assistant_tokens, prompt_lookup_num_tokens, max_matching_ngram_size, do_sample, num_beams,
                 num_return_sequences, logits_processor, custom_criteria, is_enc_dec, stopping_criteria.max_length,
                 model_kwargs, temperature=temperature, top_k=top_k, top_p=top_p, typical_p=typical_p)
+        # sequences per prompt: a paged cache forks into them after one prefill per prompt
+        fork = num_beams if is_beam else num_return_sequences if is_sample else 1
         with contextlib.ExitStack() as call:
-            call.enter_context(_call_state(self, kv_cache_dtype, decode_graphs))
+            call.enter_context(_call_state(self, kv_cache_dtype, decode_graphs,
+                                           (fork, input_ids_seq_length) if paged else None))
             models = [self]
             if draft is not None:   # the assistant's cfg sets its cache format
                 call.enter_context(_call_state(draft, _kv_cache_dtype(draft._gcfg("kv_cache_dtype")), decode_graphs))
                 models.insert(0, draft)
             # models with a preallocated cache size it once for every sequence the search runs; a verify step appends
             # k + 1 rows and keeps n + 1 of them: room for k more than the output
-            rows = batch_size * (num_beams if is_beam else num_return_sequences if is_sample else 1)
+            rows = batch_size * (1 if paged else fork)
             for m in models:
                 allocate = getattr(m, "allocate_kv_cache", None)
                 if allocate is not None and model_kwargs.get("use_cache") and stopping_criteria.max_length is not None:
@@ -939,10 +991,14 @@ class Generator:
                                           stopping_criteria=stopping_criteria, pad_token_id=pad_token_id,
                                           eos_token_id=eos_token_id, is_encoder_decoder=is_enc_dec,
                                           output_scores=output_scores, **model_kwargs)
+            shared = fork > 1 and model_kwargs.get("use_cache") and isinstance(self.kv_cache, PagedKVCache)
             if is_sample:
                 warper = self._get_logits_warper(top_k, top_p, typical_p, temperature, num_beams, renormalize_logits)
-                input_ids, model_kwargs = self._expand_inputs_for_generation(
-                    input_ids, expand_size=num_return_sequences, is_encoder_decoder=is_enc_dec, **model_kwargs)
+                if shared:
+                    input_ids, model_kwargs = self._shared_prefill(input_ids, fork, model_kwargs)
+                else:
+                    input_ids, model_kwargs = self._expand_inputs_for_generation(
+                        input_ids, expand_size=num_return_sequences, is_encoder_decoder=is_enc_dec, **model_kwargs)
                 return self.multinomial_sample(input_ids, logits_processor=logits_processor, logits_warper=warper,
                                                stopping_criteria=stopping_criteria, pad_token_id=pad_token_id,
                                                eos_token_id=eos_token_id, is_encoder_decoder=is_enc_dec,
@@ -954,8 +1010,11 @@ class Generator:
                     raise ValueError("`max_length` needs to be a stopping_criteria for now.")
                 scorer = BeamSearchScorer(batch_size=batch_size, num_beams=num_beams, length_penalty=length_penalty,
                                           do_early_stopping=early_stopping, num_beam_hyps_to_keep=num_return_sequences)
-                input_ids, model_kwargs = self._expand_inputs_for_generation(
-                    input_ids, expand_size=num_beams, is_encoder_decoder=is_enc_dec, **model_kwargs)
+                if shared:
+                    input_ids, model_kwargs = self._shared_prefill(input_ids, fork, model_kwargs)
+                else:
+                    input_ids, model_kwargs = self._expand_inputs_for_generation(
+                        input_ids, expand_size=num_beams, is_encoder_decoder=is_enc_dec, **model_kwargs)
                 return self.beam_search(input_ids, scorer, logits_processor=logits_processor,
                                         stopping_criteria=stopping_criteria, pad_token_id=pad_token_id,
                                         eos_token_id=eos_token_id, is_encoder_decoder=is_enc_dec,

@@ -12,6 +12,10 @@ With ``kv_dtype=torch.float8_e4m3fn`` the K and V buffers hold E4M3 bytes and ea
 ``k_scale`` / ``v_scale`` ``[batch, heads, capacity]`` (the format of :func:`OF.kv_cache_quantize_ref`): about half the
 bytes of a bf16 cache, at the accuracy of a per-row 8-bit float.  Every attention over such a cache is the attention
 over its dequantized rows.  It is a user's choice (``generate(kv_cache_dtype="fp8")``), never made for them.
+
+``PagedKVCache`` holds the same logical rows in pages of 64 (``generate(paged_kv_cache=True)``): the sequences of one
+prompt (beams, or ``num_return_sequences`` samples) share its prompt's pages, and a beam reorder rewrites block tables
+instead of copying the cache.
 """
 from __future__ import annotations
 
@@ -117,15 +121,20 @@ class KVCacheLayer:
     def length(self) -> int:
         return self.cache.length
 
+    @property
+    def pages(self) -> dict:
+        """The block table of a paged cache's kernels ({} for contiguous buffers)."""
+        return {}
+
     def append(self, qkv: torch.Tensor, cos=None, sin=None) -> torch.Tensor:
         """Write k, v of the packed projection ``qkv`` (per-head ``[b, s, a, 3d]`` or grouped ``[b, s, g, r + 2, d]``) at
         rows ``seqlens[b] + i`` (:func:`OF.kv_cache_append`, rotated by ``cos/sin`` when given); returns q ``[b, s, a,
         d]``.  A per-head projection without rotary hands q back as its strided view: nothing needs writing."""
         scales = {} if self.k_scale is None else {"k_scale": self.k_scale, "v_scale": self.v_scale}
         if cos is None and qkv.dim() == 4:
-            OF.kv_cache_append(qkv, self.k, self.v, self.seqlens, return_q=False, **scales)
+            OF.kv_cache_append(qkv, self.k, self.v, self.seqlens, return_q=False, **scales, **self.pages)
             return qkv[..., : qkv.shape[-1] // 3]
-        return OF.kv_cache_append(qkv, self.k, self.v, self.seqlens, cos, sin, **scales)
+        return OF.kv_cache_append(qkv, self.k, self.v, self.seqlens, cos, sin, **scales, **self.pages)
 
     def window(self, L: int, dtype) -> Tuple[torch.Tensor, torch.Tensor]:
         """K and V rows ``[:L]``: views of the buffers, or of an FP8 cache its rows dequantized to ``dtype``."""
@@ -171,7 +180,7 @@ class KVCacheLayer:
             return ctx.transpose(1, 2)
         scales = {} if self.k_scale is None else {"k_scale": self.k_scale, "v_scale": self.v_scale}
         return OF.decode_attention(q, self.k, self.v, self.seqlens, self.kv_start, scale=scale, past=past,
-                                   alibi_slopes=alibi_slopes, rel_bias=rel_bias, causal=causal, **scales)
+                                   alibi_slopes=alibi_slopes, rel_bias=rel_bias, causal=causal, **scales, **self.pages)
 
 
 class StaticKVCache:
@@ -329,6 +338,221 @@ class StaticKVCache:
         self.dense_mask = False
 
 
+class PagedKVCacheLayer(KVCacheLayer):
+    """A layer of a :class:`PagedKVCache`: the kernels take the block table; ``window`` gathers the logical rows."""
+
+    __slots__ = ()
+
+    @property
+    def pages(self) -> dict:
+        return {"block_table": self.cache.block_table}
+
+    def window(self, L: int, dtype) -> Tuple[torch.Tensor, torch.Tensor]:
+        t = self.cache.block_table
+        k, v = OF.kv_pages_gather(self.k, t, L), OF.kv_pages_gather(self.v, t, L)
+        if self.k_scale is None:
+            return k, v
+        return (OF.kv_cache_dequant(k, OF.kv_pages_gather(self.k_scale, t, L), dtype),
+                OF.kv_cache_dequant(v, OF.kv_pages_gather(self.v_scale, t, L), dtype))
+
+
+class PagedKVCache(StaticKVCache):
+    """The logical rows of a :class:`StaticKVCache` in pages of ``PAGE_ROWS`` = 64 rows (one key tile of the decode
+    kernel), for generation that runs several sequences per prompt.
+
+    Each owned layer has a K and a V pool ``[num_pages, heads, 64, head_dim]`` (an FP8 cache: E4M3 bytes, with fp32
+    row scales ``[num_pages, heads, 64]`` per pool, quantized as in a contiguous cache), and one block table, int32
+    ``[batch, max_pages]`` on the device, serves every layer: logical row ``j`` of sequence ``b`` is row ``j % 64`` of
+    page ``block_table[b, j // 64]``.  Its host mirror, a reference count per page and a free list live on the host.
+    ``seqlens``, ``kv_start`` and ``length`` are logical rows, as in a contiguous cache; ``capacity`` is
+    ``max_pages * 64``.
+
+    - ``batch`` prompts are prefilled once, then :meth:`fork` makes each of them ``fork`` sequences that share its
+      pages.  A page two sequences share is never written: :meth:`reserve` maps the pages of the rows a step will
+      write and gives a sequence whose page there is shared its own copy first (copy on write).  Only the last, partly
+      filled page of a sequence can be written while shared, so a full page is never copied.
+    - :meth:`reorder_` (beam search) builds the new table rows from the parents' on the host, returns the pages nobody
+      references to the free list and writes the table to the device in one copy.
+    - The pool is sized once, for the whole call: with ``S = prompt_len // 64`` full prompt pages,
+      ``num_pages = batch * S + batch * fork * (max_pages - S)`` — the shared prompt pages once per prompt, and every
+      other page once per sequence.  That bounds the distinct pages referenced at any time, copies on write included
+      (a copy replaces a reference to a shared page), so generating up to ``capacity`` rows allocates nothing after the
+      fork.  With ``fork >= 2`` the pool is smaller than a contiguous cache for the same call whenever
+      ``(fork - 1) * S * 64 > fork * (max_pages * 64 - capacity)``.
+    """
+
+    def __init__(self, num_layers: int, batch: int, heads: int, head_dim: int, capacity: int,
+                 dtype=torch.bfloat16, device=None, layers: Optional[Iterable[int]] = None, kv_dtype=None, *,
+                 fork: int = 1, prompt_len: int = 0):
+        self.num_layers, self.heads, self.head_dim = num_layers, heads, head_dim
+        self.dtype, self.device = dtype, torch.device(device) if device is not None else torch.device("cpu")
+        self.kv_dtype = dtype if kv_dtype is None else kv_dtype
+        if self.kv_dtype not in (dtype, torch.float8_e4m3fn):
+            raise ValueError(f"kv_dtype must be the projections' {dtype} or torch.float8_e4m3fn, got {kv_dtype}")
+        if fork < 1:
+            raise ValueError(f"fork must be >= 1, got {fork}")
+        self.fp8 = self.kv_dtype == torch.float8_e4m3fn
+        self.owned = sorted(range(num_layers) if layers is None else layers)
+        self.prompts, self.fork_n, self.rows = batch, fork, batch * fork
+        P = OF.PAGE_ROWS
+        self.max_pages = -(-max(int(capacity), 1) // P)
+        self.capacity = self.max_pages * P
+        shared = min(max(int(prompt_len), 0) // P, self.max_pages)
+        self.num_pages = batch * shared + self.rows * (self.max_pages - shared)
+        self.k: List[Optional[torch.Tensor]] = [None] * num_layers
+        self.v: List[Optional[torch.Tensor]] = [None] * num_layers
+        self.k_scale: List[Optional[torch.Tensor]] = [None] * num_layers
+        self.v_scale: List[Optional[torch.Tensor]] = [None] * num_layers
+        for i in self.owned:
+            # uninitialised, as a contiguous cache's buffers: the kernels read the rows of a sequence's window only
+            self.k[i], self.v[i] = (torch.empty(self.num_pages, heads, P, head_dim, dtype=self.kv_dtype,
+                                                device=self.device) for _ in range(2))
+            if self.fp8:
+                self.k_scale[i], self.v_scale[i] = (torch.empty(self.num_pages, heads, P, dtype=torch.float32,
+                                                                device=self.device) for _ in range(2))
+        self._seqlens = torch.zeros(self.rows, dtype=torch.int32, device=self.device)
+        self._kv_start = torch.zeros(self.rows, dtype=torch.int32, device=self.device)
+        self._table = torch.full((self.rows, self.max_pages), -1, dtype=torch.int32, device=self.device)
+        self.reset()
+
+    def layer(self, i: int) -> KVCacheLayer:
+        return PagedKVCacheLayer(self, i)
+
+    def _views(self, batch: int) -> None:
+        # views of the full-size tensors: their addresses (which a decode graph reads) do not change at the fork
+        self.batch = batch
+        self.seqlens, self.kv_start = self._seqlens[:batch], self._kv_start[:batch]
+        self.block_table = self._table[:batch]
+
+    def arrays(self) -> List[torch.Tensor]:
+        """Every pool (K, V and the FP8 scales of every owned layer): what a page copy copies."""
+        return [t for i in self.owned for t in (self.k[i], self.v[i], self.k_scale[i], self.v_scale[i])
+                if t is not None]
+
+    def _write_table(self) -> None:
+        self._table.copy_(torch.tensor(self.host_table, dtype=torch.int32))
+
+    def _alloc(self) -> int:
+        if not self.free:
+            raise RuntimeError("PagedKVCache: out of pages (the pool is sized for the call it was allocated for)")
+        p = self.free.pop()
+        self.refs[p] = 1
+        return p
+
+    def _release(self, p: int) -> None:
+        self.refs[p] -= 1
+        if self.refs[p] == 0:
+            self.free.append(p)
+
+    def flash_attention(self) -> bool:
+        k = torch.empty((self.batch, self.heads, 1, self.head_dim), dtype=self.dtype, device=self.device)
+        return OF.attention_supported(k, k)
+
+    def write_rows(self, i: int, k: torch.Tensor, v: torch.Tensor, row0: int = 0) -> None:
+        """As :meth:`StaticKVCache.write_rows`, into the pages of the rows (mapped by :meth:`reserve` first)."""
+        n = k.shape[2]
+        rows = torch.arange(row0, row0 + n, device=self.device)[None].expand(self.batch, n)
+        ids = OF._page_ids(self.block_table, rows, self.num_pages)
+        off = rows % OF.PAGE_ROWS
+        for pool, scale, x in ((self.k, self.k_scale, k), (self.v, self.v_scale, v)):
+            x = x.transpose(1, 2)   # [batch, n, heads, d]
+            if self.fp8:
+                pool[i][ids, :, off], scale[i][ids, :, off] = OF.kv_cache_quantize_ref(x)
+            else:
+                pool[i][ids, :, off] = x
+
+    def fill(self, kv, S: int, window=None) -> None:
+        raise NotImplementedError("PagedKVCache holds self-attention rows only (no fixed cross-attention window)")
+
+    def reserve(self, n: int) -> None:
+        """Map the pages of rows ``length .. length + n`` of every sequence and make each of them the sequence's own: a
+        shared page is copied first (one page copy launch for every layer).  The pool is never reallocated."""
+        need = self.length + n
+        if need > self.capacity:
+            raise ValueError(f"PagedKVCache holds up to {self.capacity} rows per sequence, {need} needed")
+        P = OF.PAGE_ROWS
+        copies, changed = [], False
+        for slot in range(self.length // P, -(-need // P)):
+            for row in self.host_table[: self.batch]:
+                if slot >= self.mapped:
+                    row[slot], changed = self._alloc(), True
+                elif self.refs[row[slot]] > 1:
+                    new = self._alloc()
+                    copies.append((row[slot], new))
+                    self.refs[row[slot]] -= 1
+                    row[slot], changed = new, True
+        self.mapped = max(self.mapped, -(-need // P))
+        if copies:
+            OF.kv_page_copy(self.arrays(), copies)
+        if changed:
+            self._write_table()
+
+    def _unmap_from(self, slot: int) -> None:
+        # every sequence's pages from `slot` on go back (the rows there are no longer held)
+        for row in self.host_table[: self.batch]:
+            for s in range(slot, self.mapped):
+                self._release(row[s])
+                row[s] = -1
+        self.mapped = min(self.mapped, slot)
+
+    def rollback(self, n: int) -> None:
+        super().rollback(n)
+        slot = -(-self.length // OF.PAGE_ROWS)
+        if slot < self.mapped:
+            self._unmap_from(slot)
+            self._write_table()
+
+    def fork(self, n: int) -> None:
+        """After the prefill of the ``batch`` prompts: each prompt becomes ``n`` sequences (prompt ``p``'s are rows
+        ``p * n .. p * n + n - 1``, the order of ``generate``'s expanded inputs) sharing its pages; ``seqlens``,
+        ``kv_start`` and the dense-mask flag carry over."""
+        if n < 1 or self.batch * n > self.rows:
+            raise ValueError(f"fork: {self.batch} prompts x {n} exceed the {self.rows} sequences this cache holds")
+        if n == 1:
+            return
+        b = self.batch
+        self.host_table = [list(self.host_table[p]) for p in range(b) for _ in range(n)] + \
+            self.host_table[b * n:]
+        for row in self.host_table[: b * n : n]:
+            for page in row[: self.mapped]:
+                self.refs[page] += n - 1
+        seqlens, kv_start = self.seqlens.repeat_interleave(n), self.kv_start.repeat_interleave(n)
+        self._views(b * n)
+        self.seqlens.copy_(seqlens)
+        self.kv_start.copy_(kv_start)
+        self._write_table()
+
+    def reorder_(self, beam_idx: torch.Tensor) -> None:
+        """Sequence ``i`` continues sequence ``beam_idx[i]``: its table row becomes the parent's (one host sync); pages
+        no sequence references any more return to the free list.  No page is copied here: a shared last page is copied
+        when a sequence next writes to it (:meth:`reserve`)."""
+        idx = [int(i) for i in beam_idx.tolist()]
+        old = self.host_table
+        self.host_table = [list(old[i]) for i in idx] + old[self.batch:]
+        refs = [0] * self.num_pages
+        for row in self.host_table[: self.batch]:
+            for page in row[: self.mapped]:
+                refs[page] += 1
+        self.free += [p for p in range(self.num_pages) if self.refs[p] > 0 and refs[p] == 0]
+        self.refs = refs
+        self._write_table()
+        dev = beam_idx.to(device=self.device, dtype=torch.long)
+        self.seqlens.copy_(self.seqlens.index_select(0, dev))
+        self.kv_start.copy_(self.kv_start.index_select(0, dev))
+
+    def reset(self) -> None:
+        self._views(self.prompts)
+        self._seqlens.zero_()
+        self._kv_start.zero_()
+        self.length = 0
+        self.dense_mask = False
+        self.host_table = [[-1] * self.max_pages for _ in range(self.rows)]
+        self.refs = [0] * self.num_pages
+        self.free = list(range(self.num_pages - 1, -1, -1))   # pages are taken from the end: 0, 1, 2, ...
+        self.mapped = 0   # the page slots mapped in every sequence's row
+        self._write_table()
+
+
 class KVCacheOwner:
     """The model side of a :class:`StaticKVCache` for decoder-only models: ``generate`` sizes it through
     ``allocate_kv_cache``, ``set_cache`` / ``past_key_values`` / ``past_length`` keep the generator's cache protocol.
@@ -338,6 +562,9 @@ class KVCacheOwner:
     kv_cache: Optional[StaticKVCache] = None
     past_length = 0
     kv_cache_dtype = None   # what the cache holds: None = the weights' dtype; torch.float8_e4m3fn = FP8 rows
+    # a paged cache for the next allocate_kv_cache: (sequences per prompt, prompt length), set by generate(); None = a
+    # contiguous StaticKVCache
+    kv_cache_paging: Optional[Tuple[int, int]] = None
     # the rows a step may reach (the last _prepare_cache's max_positions): a replayed decode graph checks it instead
     max_cache_positions: Optional[int] = None
 
@@ -359,8 +586,14 @@ class KVCacheOwner:
         # the activations' dtype: a Linear1D with FP8 weights keeps it apart (LoRA wrappers have no compute_dtype)
         dtype = getattr(qkv, "compute_dtype", None) or w.dtype
         c = self.kv_cache
-        if c is None or not c.matches(batch, dtype, w.device, self.kv_cache_dtype) or c.capacity < max_length:
-            heads = getattr(mods[0], "local_kv_heads", mods[0].local_heads)
+        heads = getattr(mods[0], "local_kv_heads", mods[0].local_heads)
+        if self.kv_cache_paging is not None:   # sized for this call: a new pool every time
+            fork, prompt_len = self.kv_cache_paging
+            self.kv_cache = self._decode_graph = None   # the old cache (and a graph on it) go first
+            c = PagedKVCache(len(mods), batch, heads, mods[0].head_size, max_length, dtype, w.device, owned,
+                             self.kv_cache_dtype, fork=fork, prompt_len=prompt_len)
+        elif (c is None or isinstance(c, PagedKVCache) or not c.matches(batch, dtype, w.device, self.kv_cache_dtype)
+              or c.capacity < max_length):
             c = StaticKVCache(len(mods), batch, heads, mods[0].head_size, max_length, dtype, w.device, owned,
                               self.kv_cache_dtype)
             self._decode_graph = None   # a decode graph of the old cache (and its memory pool) goes with it

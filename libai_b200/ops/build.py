@@ -25,7 +25,7 @@ NVCC = os.path.join(CUDA_HOME, "bin", "nvcc")
 CU_SOURCES = ["gemm_sm90.cu", "norm.cu", "elementwise.cu", "attention_sm90.cu", "comm_kernels.cu",
               "decode_attention_sm90.cu", "decode_attention_alibi_sm90.cu", "decode_attention_t5_sm90.cu",
               "decode_attention_fp8_sm90.cu", "window_attention_sm90.cu", "linear_fp8w_sm90.cu",
-              "linear_int4w_sm90.cu", "speculative_sm90.cu"]
+              "linear_int4w_sm90.cu", "speculative_sm90.cu", "decode_attention_paged_sm90.cu"]
 CPP_SOURCES = ["bindings.cpp", "symm_mem.cpp"]
 
 NVCC_FLAGS = [

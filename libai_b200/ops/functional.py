@@ -1225,34 +1225,94 @@ def _check_scales(k_cache, k_scale, v_scale):
 
 
 def kv_cache_append(qkv, k_cache, v_cache, cache_seqlens, cos=None, sin=None, return_q: bool = True, k_scale=None,
-                    v_scale=None):
+                    v_scale=None, block_table=None):
     """Write k, v of the packed projection ``qkv`` (``[b, s, a, 3d]``, or grouped ``[b, s, g, r + 2, d]``) into rows
     ``cache_seqlens[b] + i`` of the caches ``[b, g, C, d]``.  With
     ``cos/sin`` (fp32 ``[positions, d]``) q and k are first rotated at those positions, exactly as
     :func:`apply_rotary_qkv` with ``pos_offset = cache_seqlens[b]`` does.  Returns q ``[b, s, a, d]`` (rotated when the
     tables are given) when ``return_q``, else None.  FP8 caches (``float8_e4m3fn``) take their row scales ``k_scale``,
-    ``v_scale`` (fp32 ``[b, g, C]``) and store each row quantized (:func:`kv_cache_quantize_ref`)."""
+    ``v_scale`` (fp32 ``[b, g, C]``) and store each row quantized (:func:`kv_cache_quantize_ref`).
+    ``block_table`` (int32 ``[b, max_pages]``): the caches are paged, pools ``[P, g, 64, d]`` (scales ``[P, g, 64]``)
+    whose logical row ``j`` of sample ``b`` is row ``j % 64`` of page ``block_table[b, j // 64]``
+    (:class:`~libai_b200.inference.kv_cache.PagedKVCache`); the bytes and scales written are those of a contiguous
+    cache.  Page ids in ``[0, P)`` for the rows written are the caller's guarantee (the reference path checks them)."""
     _check_scales(k_cache, k_scale, v_scale)
     if _decode_native(qkv, k_cache) and (cos is None or cos.dtype == torch.float32):
         ext = load_ext()
         qkv = qkv if qkv.is_contiguous() else qkv.contiguous()
-        if k_scale is not None:
+        if block_table is not None and k_scale is not None:
+            q = ext.kv_append_fp8_paged(qkv, k_cache, v_cache, k_scale, v_scale, block_table, cache_seqlens, cos, sin,
+                                        bool(return_q))
+        elif block_table is not None:
+            q = ext.kv_append_paged(qkv, k_cache, v_cache, block_table, cache_seqlens, cos, sin, bool(return_q))
+        elif k_scale is not None:
             q = ext.kv_append_fp8(qkv, k_cache, v_cache, k_scale, v_scale, cache_seqlens, cos, sin, bool(return_q))
         else:
             q = ext.kv_append(qkv, k_cache, v_cache, cache_seqlens, cos, sin, bool(return_q))
         count_launch()
         return q if return_q else None
-    q = kv_cache_append_ref(qkv, k_cache, v_cache, cache_seqlens, cos, sin, k_scale, v_scale)
+    pages = {} if block_table is None else {"block_table": block_table}
+    q = kv_cache_append_ref(qkv, k_cache, v_cache, cache_seqlens, cos, sin, k_scale, v_scale, **pages)
     return q if return_q else None
 
 
-def kv_cache_append_ref(qkv, k_cache, v_cache, cache_seqlens, cos=None, sin=None, k_scale=None, v_scale=None):
+PAGE_ROWS = 64   # the rows of a page of a paged cache: one key tile of the decode kernel
+
+
+def _page_ids(block_table, rows, num_pages):
+    """The page ids ``[b, n]`` of the logical rows ``rows`` (long ``[b, n]``), checked to be in ``[0, num_pages)``."""
+    ids = block_table.long().gather(1, rows // PAGE_ROWS)
+    if bool(((ids < 0) | (ids >= num_pages)).any()):
+        raise ValueError(f"block_table: a row in use maps to a page outside [0, {num_pages})")
+    return ids
+
+
+def kv_pages_gather(pool, block_table, L: int):
+    """The logical rows ``[:L]`` of a paged cache's pool ``[P, g, 64, ...]`` (bytes, or scales ``[P, g, 64]``) through
+    ``block_table`` ``[b, max_pages]``, contiguous: ``[b, g, L, ...]``.  Every row below ``L`` must be mapped."""
+    rows = torch.arange(L, device=block_table.device)[None].expand(block_table.shape[0], L)
+    ids = _page_ids(block_table, rows, pool.shape[0]).to(pool.device)
+    off = (rows % PAGE_ROWS).to(pool.device)
+    return pool[ids, :, off].transpose(1, 2)   # [b, L, g, ...] -> [b, g, L, ...]
+
+
+def kv_page_copy(arrays, pairs):
+    """Copy page ``src`` to page ``dst`` of every array in ``arrays`` (pools ``[P, ...]``: the K and V pools, and the
+    FP8 scales, of every layer of a paged cache) for each ``(src, dst)`` of ``pairs`` (a list, or int32 ``[n, 2]``).
+    One launch on the GPU."""
+    pairs = torch.as_tensor(pairs, dtype=torch.int32).reshape(-1, 2).cpu()
+    if pairs.shape[0] == 0:
+        return
+    P = arrays[0].shape[0]
+    if bool(((pairs < 0) | (pairs >= P)).any()):
+        raise ValueError(f"kv_page_copy: page ids must be in [0, {P})")
+    if use_native(arrays[0]):
+        load_ext().kv_page_copy(list(arrays), pairs)
+        count_launch()
+        return
+    src, dst = pairs[:, 0].long(), pairs[:, 1].long()
+    for t in arrays:
+        t[dst.to(t.device)] = t[src.to(t.device)]
+
+
+def kv_cache_append_ref(qkv, k_cache, v_cache, cache_seqlens, cos=None, sin=None, k_scale=None, v_scale=None,
+                        block_table=None):
     s_len = qkv.shape[1]
     starts = [int(x) for x in cache_seqlens.tolist()]
     if cos is not None:
         pos = torch.tensor(starts, device=cos.device)[:, None] + torch.arange(s_len, device=cos.device)[None]
         qkv = _rotary_qkv_ref(qkv, cos, sin, position_ids=pos)
     q, k, v = split_qkv(qkv)
+    if block_table is not None:   # [b, s, g, d] rows scattered to their pages
+        rows = torch.tensor(starts, device=block_table.device)[:, None] + torch.arange(s_len, device=block_table.device)
+        ids = _page_ids(block_table, rows, k_cache.shape[0]).to(k_cache.device)
+        off = (rows % PAGE_ROWS).to(k_cache.device)
+        for cache, scale, x in ((k_cache, k_scale, k), (v_cache, v_scale, v)):
+            if scale is None:
+                cache[ids, :, off] = x.to(cache.dtype)
+            else:
+                cache[ids, :, off], scale[ids, :, off] = kv_cache_quantize_ref(x)
+        return q
     for b, st in enumerate(starts):
         for cache, scale, x in ((k_cache, k_scale, k[b]), (v_cache, v_scale, v[b])):
             if scale is None:
@@ -1264,7 +1324,7 @@ def kv_cache_append_ref(qkv, k_cache, v_cache, cache_seqlens, cos=None, sin=None
 
 def decode_attention(q, k_cache, v_cache, cache_seqlens, kv_start, *, scale: float, splits: int = 0,
                      past: Optional[int] = None, alibi_slopes=None, rel_bias=None, causal: bool = True, k_scale=None,
-                     v_scale=None):
+                     v_scale=None, block_table=None):
     """Attention of ``q [b, s, a, d]`` (new tokens, already appended to the caches; any strides with d contiguous) over
     the caches ``[b, g, C, d]`` (query head ``h`` reads cache head ``h // (a // g)``): query ``i`` of sample ``b`` sees exactly the keys ``kv_start[b] <= j <= cache_seqlens[b] + i``.  Returns
     ``[b, s, a, d]`` contiguous; a query without a visible key gets zeros.  The native kernel takes up to 16 new tokens
@@ -1291,6 +1351,17 @@ def decode_attention(q, k_cache, v_cache, cache_seqlens, kv_start, *, scale: flo
     ``cache_seqlens[b]`` to ``past``) may be loaded with weight zero and must be finite, as the appends leave them."""
     _check_scales(k_cache, k_scale, v_scale)
     native = _decode_native(q, k_cache)
+    if block_table is not None:
+        if rel_bias is not None or not causal:
+            raise ValueError("block_table: a paged cache takes no rel_bias and no causal=False")
+        if native and q.shape[1] <= 16:
+            o = load_ext().decode_attn_paged(q, k_cache, v_cache, block_table, cache_seqlens, kv_start, float(scale),
+                                             int(splits), alibi_slopes, k_scale, v_scale)
+            count_launch(2)
+            return o
+        return decode_attention_paged_ref(q, k_cache, v_cache, block_table, cache_seqlens, kv_start, scale=scale,
+                                          splits=splits, past=past, alibi_slopes=alibi_slopes, k_scale=k_scale,
+                                          v_scale=v_scale)
     if native and q.shape[1] <= 16:
         ext = load_ext()
         extra = () if rel_bias is None and causal else (rel_bias, bool(causal))
@@ -1325,6 +1396,20 @@ def decode_attention(q, k_cache, v_cache, cache_seqlens, kv_start, *, scale: flo
             return o.transpose(1, 2)   # the kernel's [b, s, a, d] output
     return decode_attention_ref(q, k_cache, v_cache, cache_seqlens, kv_start, scale=scale, alibi_slopes=alibi_slopes,
                                 rel_bias=rel_bias, causal=causal)
+
+
+def decode_attention_paged_ref(q, k_pool, v_pool, block_table, cache_seqlens, kv_start, *, scale: float, splits=0,
+                               past: Optional[int] = None, alibi_slopes=None, k_scale=None, v_scale=None):
+    """:func:`decode_attention` over a paged cache by its logical rows: the rows ``[:L]`` gathered through the table
+    (``L = past + s`` with ``past``, else ``max(cache_seqlens) + s``) into contiguous caches, then the contiguous call
+    (the flash kernel beyond 16 new tokens on the GPU, the reference math on the CPU)."""
+    L = past + q.shape[1] if past is not None else int(cache_seqlens.max()) + q.shape[1]
+    k, v = kv_pages_gather(k_pool, block_table, L), kv_pages_gather(v_pool, block_table, L)
+    scales = {}
+    if k_scale is not None:
+        scales = {"k_scale": kv_pages_gather(k_scale, block_table, L), "v_scale": kv_pages_gather(v_scale, block_table, L)}
+    return decode_attention(q, k, v, cache_seqlens, kv_start, scale=scale, splits=splits, past=past,
+                            alibi_slopes=alibi_slopes, **scales)
 
 
 def decode_attention_ref(q, k_cache, v_cache, cache_seqlens, kv_start, *, scale: float, alibi_slopes=None,
