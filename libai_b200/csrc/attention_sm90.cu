@@ -32,6 +32,9 @@
 // sees itself).  Nothing assumes doc_start to be non-decreasing along a row: which key tiles a forward CTA loads and
 // which (key block, query block) visits the backward skips come from the minimum over the rows of the query block.
 //
+// Paged K/V (PAGED instances, forward only, causal, no bias or ALiBi, D = 64 and 128): the keys are the logical rows of
+// a paged KV cache, read through its block table; each 128-key tile is two 64-row pages (see AttnPages).
+//
 // Forward, one CTA per (batch, query head, 128-query block), 384 threads:
 //   warpgroup 0  TMA producer (one elected thread): Q once, then K/V tiles of 128 keys (double buffered); it gives
 //                its registers to the consumers (setmaxnreg)
@@ -114,10 +117,46 @@ struct AttnFwdCfg {
   static constexpr int SMEM_BYTES = 5 * TILE_BYTES + 1024 + 256;   // Q + 2 x (K, V)
 };
 
-// the forward of one CTA; tmap_* and p are the kernel's __grid_constant__ parameters (inlined: no call in the kernel)
-template <int D, int BIAS, bool DROP, bool DOC, bool PREFIX = false>
+// Paged K/V (PAGED instances, attn_fwd_paged_kernel): the keys are the logical rows [0, Sk) of pools [P, G, 64, D],
+// row j of sample b being row j % 64 of page table[b * max_pages + j / 64].  tmap_k / tmap_v cover the pools as
+// {D, 64, G, P}; tail_k / tail_v the same pools with only the first Sk % 64 rows of each page (Sk % 64 != 0).
+constexpr int ATT_PAGE_ROWS = 64;   // a key tile (ATT_BN) is two pages
+struct AttnPages {
+  const int* table;   // [B, max_pages]
+  int max_pages;
+  int num_pages;      // P
+};
+// The coordinates (row, page) of the box that fills page slot `slot` of sample `batch`, and whether it reads the tail
+// map.  A slot at or past the window end, or whose table entry is not a page of the pool, gets a box wholly below the
+// page's 64 rows: TMA fills it with zeros, as the contiguous kernel's rows past Sk, reads no memory and still counts the
+// box's bytes, so no V row outside the window (uninitialised, or another sequence's, NaN included) reaches P·V.  The
+// rows of the last, partial page past Sk read through the tail map, whose row extent ends at Sk % 64, so they are
+// zero-filled too.
+LB_DEVICE void attn_page_box(const AttnPages& pg, int batch, int slot, int Sk, int& row, int& page, bool& tail) {
+  const int rows = Sk - slot * ATT_PAGE_ROWS;
+  row = ATT_PAGE_ROWS;
+  page = 0;
+  tail = false;
+  if (rows > 0) {
+    const int id = pg.table[static_cast<size_t>(batch) * pg.max_pages + slot];
+    if (id >= 0 && id < pg.num_pages) {
+      row = 0;
+      page = id;
+      tail = rows < ATT_PAGE_ROWS;
+    }
+  }
+}
+
+// the forward of one CTA; tmap_* and p are the kernel's __grid_constant__ parameters (inlined: no call in the kernel).
+// PAGED: K/V through the block table `pages` (tail: the maps tail_k, tail_v; see AttnPages); only the producer's
+// addresses change, so the shared-memory tiles, and the output, are those of the contiguous kernel over the gathered
+// rows [0, Sk).
+template <int D, int BIAS, bool DROP, bool DOC, bool PREFIX = false, bool PAGED = false>
 LB_DEVICE void attn_fwd_cta(const CUtensorMap& tmap_q, const CUtensorMap& tmap_k, const CUtensorMap& tmap_v,
-                            const AttnFwdParams& p) {
+                            const AttnFwdParams& p, const CUtensorMap* tail_k = nullptr,
+                            const CUtensorMap* tail_v = nullptr, const AttnPages* pages = nullptr) {
+  static_assert(!PAGED || (!DROP && !DOC && !PREFIX && BIAS != BIAS_DENSE), "paged K/V: no dropout, dense bias, "
+                "packed sequences or prefix");
   static_assert(!DOC || (BIAS == BIAS_NONE && !DROP), "packed sequences run without bias and dropout");
   static_assert(!PREFIX || (BIAS == BIAS_NONE && !DOC), "a prefix runs without bias and packed sequences");
   using Cfg = AttnFwdCfg<D>;
@@ -184,16 +223,41 @@ LB_DEVICE void attn_fwd_cta(const CUtensorMap& tmap_q, const CUtensorMap& tmap_k
       for (int it = 0; it < nkv; ++it) {
         const int j = j0 + it, b = it & 1;
         const uint32_t par = ((it >> 1) & 1) ^ 1;
-        mbar_wait(&k_empty[b], par);
-        mbar_arrive_expect_tx(&k_full[b], Cfg::TILE_BYTES);
+        if constexpr (PAGED) {
+          // page slot 2j + h fills rows 64h .. 64h + 63 of the tile: one 64-row box per page and 64-column chunk, at
+          // a 1024-byte (8-row) boundary, so the 128B swizzle lays the rows out as one 128-row box does
+          int row[2], page[2];
+          bool tail[2];
 #pragma unroll
-        for (int c = 0; c < Cfg::CHUNKS; ++c)
-          tma_load_4d(sK + b * Cfg::TILE_BYTES + c * (ATT_BN * 128), &tmap_k, &k_full[b], c * 64, j * ATT_BN, kv_head, batch);
-        mbar_wait(&v_empty[b], par);
-        mbar_arrive_expect_tx(&v_full[b], Cfg::TILE_BYTES);
+          for (int h = 0; h < 2; ++h) attn_page_box(*pages, batch, 2 * j + h, p.Sk, row[h], page[h], tail[h]);
+          mbar_wait(&k_empty[b], par);
+          mbar_arrive_expect_tx(&k_full[b], Cfg::TILE_BYTES);
 #pragma unroll
-        for (int c = 0; c < Cfg::CHUNKS; ++c)
-          tma_load_4d(sV + b * Cfg::TILE_BYTES + c * (ATT_BN * 128), &tmap_v, &v_full[b], c * 64, j * ATT_BN, kv_head, batch);
+          for (int h = 0; h < 2; ++h)
+#pragma unroll
+            for (int c = 0; c < Cfg::CHUNKS; ++c)
+              tma_load_4d(sK + b * Cfg::TILE_BYTES + c * (ATT_BN * 128) + h * (ATT_PAGE_ROWS * 128),
+                          tail[h] ? tail_k : &tmap_k, &k_full[b], c * 64, row[h], kv_head, page[h]);
+          mbar_wait(&v_empty[b], par);
+          mbar_arrive_expect_tx(&v_full[b], Cfg::TILE_BYTES);
+#pragma unroll
+          for (int h = 0; h < 2; ++h)
+#pragma unroll
+            for (int c = 0; c < Cfg::CHUNKS; ++c)
+              tma_load_4d(sV + b * Cfg::TILE_BYTES + c * (ATT_BN * 128) + h * (ATT_PAGE_ROWS * 128),
+                          tail[h] ? tail_v : &tmap_v, &v_full[b], c * 64, row[h], kv_head, page[h]);
+        } else {
+          mbar_wait(&k_empty[b], par);
+          mbar_arrive_expect_tx(&k_full[b], Cfg::TILE_BYTES);
+#pragma unroll
+          for (int c = 0; c < Cfg::CHUNKS; ++c)
+            tma_load_4d(sK + b * Cfg::TILE_BYTES + c * (ATT_BN * 128), &tmap_k, &k_full[b], c * 64, j * ATT_BN, kv_head, batch);
+          mbar_wait(&v_empty[b], par);
+          mbar_arrive_expect_tx(&v_full[b], Cfg::TILE_BYTES);
+#pragma unroll
+          for (int c = 0; c < Cfg::CHUNKS; ++c)
+            tma_load_4d(sV + b * Cfg::TILE_BYTES + c * (ATT_BN * 128), &tmap_v, &v_full[b], c * 64, j * ATT_BN, kv_head, batch);
+        }
       }
     }
     return;
@@ -399,6 +463,15 @@ attn_fwd_prefix_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_
                        const __grid_constant__ CUtensorMap tmap_v, const __grid_constant__ AttnFwdParams p) {
   attn_fwd_cta<D, BIAS_NONE, DROP, false, true>(tmap_q, tmap_k, tmap_v, p);
 }
+// paged K/V (AttnPages): causal attention of the new tokens over a paged cache, without bias or with ALiBi
+template <int D, int BIAS>
+__global__ void __launch_bounds__(ATT_FWD_THREADS, 1)
+attn_fwd_paged_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_k,
+                      const __grid_constant__ CUtensorMap tmap_v, const __grid_constant__ AttnFwdParams p,
+                      const __grid_constant__ CUtensorMap tail_k, const __grid_constant__ CUtensorMap tail_v,
+                      const __grid_constant__ AttnPages pages) {
+  attn_fwd_cta<D, BIAS, false, false, false, true>(tmap_q, tmap_k, tmap_v, p, &tail_k, &tail_v, &pages);
+}
 
 }  // namespace lb
 
@@ -533,6 +606,58 @@ extern "C" int lb_attn_fwd(const lb::AttnArgs* a, const void* q, const void* k, 
     return launch_fwd_t<decltype(tile_c)::value, decltype(bias)::value, decltype(drop)::value, decltype(doc)::value,
                         decltype(prefix)::value>(tq, tk, tv, p, s);
   });
+}
+
+namespace {
+template <int D, int BIAS>
+cudaError_t launch_fwd_paged_t(const CUtensorMap (&maps)[5], const lb::AttnFwdParams& p, const lb::AttnPages& pages,
+                               cudaStream_t s) {
+  using Cfg = lb::AttnFwdCfg<D>;
+  auto kern = lb::attn_fwd_paged_kernel<D, BIAS>;
+  static bool configured = false;
+  if (!configured) {
+    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES);
+    if (e != cudaSuccess) return e;
+    configured = true;
+  }
+  dim3 grid((p.Sq + lb::ATT_BM - 1) / lb::ATT_BM, p.A, p.B);
+  kern<<<grid, lb::ATT_FWD_THREADS, Cfg::SMEM_BYTES, s>>>(maps[0], maps[1], maps[2], p, maps[3], maps[4], pages);
+  return cudaGetLastError();
+}
+}  // namespace
+// o [B, Sq, A, d], lse [B, A, Sq] over the paged pools [num_pages, G, 64, d]; see launchers.h.  Returns -8 for a problem
+// the paged instances do not run (d not 64 or 128, not causal, kv_lens, dense bias, doc_start, prefix_lens, dropout)
+// and -9 when the block table has fewer than Sk / 64 slots.
+extern "C" int lb_attn_fwd_paged(const lb::AttnArgs* a, const void* q, const void* k_pool, const void* v_pool,
+                                 int num_pages, const int* block_table, int max_pages, void* o, float* lse,
+                                 cudaStream_t s) {
+  const int tile = check_attn_args(*a);
+  if (tile < 0) return tile;
+  if (a->d != tile || !a->causal || a->kv_lens != nullptr || a->bias != nullptr || a->doc_start != nullptr ||
+      a->prefix_lens != nullptr || a->p_drop > 0.f)
+    return -8;
+  if (num_pages <= 0 || (long)max_pages * lb::ATT_PAGE_ROWS < a->Sk) return -9;
+  const int P = lb::ATT_PAGE_ROWS, tail_rows = a->Sk % P == 0 ? P : a->Sk % P;
+  const long pool_strides[3] = {(long)a->G * P * a->d, (long)P * a->d, a->d};   // {page, head, row}
+  CUtensorMap maps[5];   // q, k, v, tail_k, tail_v
+  if (!make_q_tmap(&maps[0], q, a->B, a->G, a->A / a->G, a->Sq, a->d, a->q_strides, 128)) return -2;
+  if (!make_qkv_tmap(&maps[1], k_pool, num_pages, a->G, P, a->d, pool_strides, P)) return -2;
+  if (!make_qkv_tmap(&maps[2], v_pool, num_pages, a->G, P, a->d, pool_strides, P)) return -2;
+  if (!make_qkv_tmap(&maps[3], k_pool, num_pages, a->G, tail_rows, a->d, pool_strides, P)) return -2;
+  if (!make_qkv_tmap(&maps[4], v_pool, num_pages, a->G, tail_rows, a->d, pool_strides, P)) return -2;
+  lb::AttnFwdParams p;
+  fill_score_params(p, *a, false);
+  p.o = reinterpret_cast<__nv_bfloat16*>(o);
+  p.lse = lse;
+  memset(&p.rng, 0, sizeof(p.rng));
+  p.rng_out = nullptr;
+  const lb::AttnPages pages{block_table, max_pages, num_pages};
+  const bool alibi = p.alibi_slopes != nullptr;
+  if (tile == 64)
+    return (int)(alibi ? launch_fwd_paged_t<64, lb::BIAS_ALIBI>(maps, p, pages, s)
+                       : launch_fwd_paged_t<64, lb::BIAS_NONE>(maps, p, pages, s));
+  return (int)(alibi ? launch_fwd_paged_t<128, lb::BIAS_ALIBI>(maps, p, pages, s)
+                     : launch_fwd_paged_t<128, lb::BIAS_NONE>(maps, p, pages, s));
 }
 // =================================================================================================
 // Backward.  One CTA per (batch, K/V head, NWG consecutive 64-key blocks).  Consumer warpgroup w (warpgroups 1 ..

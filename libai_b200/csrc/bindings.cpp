@@ -1077,6 +1077,52 @@ std::tuple<Tensor, Tensor, Tensor> attn_fwd(const Tensor& q, const Tensor& k, co
   return std::make_tuple(o.permute({0, 2, 1, 3}), lse, rng_state);
 }
 
+// Causal flash attention of q [B, Sq, A, D] (the new tokens, appended already; any strides with D contiguous) over the
+// logical rows [0, past + Sq) of a paged cache: contiguous bf16 pools [P, G, 64, D] (D 64 or 128, A a multiple of G)
+// read through block_table int32 [B, max_pages] (max_pages * 64 >= past + Sq).  kv_start int32 [B] (left padding) and
+// alibi_slopes fp32 [A] as in attn_fwd.  The table entries of those rows are the caller's guarantee (an entry outside
+// [0, P) reads as zero rows).  Returns o [B, Sq, A, D] contiguous.
+Tensor attn_fwd_paged(const Tensor& q, const Tensor& k_pool, const Tensor& v_pool, const Tensor& block_table,
+                      int64_t past, double scale, const c10::optional<Tensor>& kv_start,
+                      const c10::optional<Tensor>& alibi_slopes) {
+  Args args("attn_fwd_paged");
+  args("q", q, at::kBFloat16, {kAny, kAny, kAny, kAny}, Layout::LastDimContiguous, 16);
+  const int64_t D = q.size(3);
+  TORCH_CHECK(D == 64 || D == 128, "attn_fwd_paged: head dim must be 64 or 128, got ", D);
+  args("k_pool", k_pool, at::kBFloat16, {kAny, kAny, 64, D});
+  args("v_pool", v_pool, at::kBFloat16, k_pool.sizes());
+  args("block_table", block_table, at::kInt, {q.size(0), kAny});
+  lb::AttnArgs a{};
+  a.B = (int)q.size(0);
+  a.Sq = (int)q.size(1);
+  a.A = (int)q.size(2);
+  a.G = (int)k_pool.size(1);
+  a.d = (int)D;
+  TORCH_CHECK(a.G > 0 && a.A % a.G == 0, "attn_fwd_paged: the query heads must be a multiple of the K/V heads");
+  TORCH_CHECK(k_pool.size(0) >= 1 && k_pool.size(0) <= INT32_MAX, "attn_fwd_paged: 1 <= pages <= INT32_MAX");
+  TORCH_CHECK(past >= 0 && a.Sq >= 1 && past + a.Sq <= block_table.size(1) * 64, "attn_fwd_paged: the rows [0, past + ",
+              "Sq) must fit the block table's ", block_table.size(1), " pages, got past = ", past, ", Sq = ", a.Sq);
+  a.Sk = (int)(past + a.Sq);
+  const long r = a.A / a.G;
+  a.q_strides[0] = q.stride(0);
+  a.q_strides[1] = r * q.stride(2);
+  a.q_strides[2] = q.stride(2);
+  a.q_strides[3] = q.stride(1);
+  for (int i = 0; i < 3; ++i) a.k_strides[i] = a.v_strides[i] = k_pool.stride(i);
+  a.causal = true;
+  a.scale = (float)scale;
+  a.kv_start = args.opt<const int>("kv_start", kv_start, at::kInt, {a.B});
+  a.alibi_slopes = args.opt<const float>("alibi_slopes", alibi_slopes, at::kFloat, {a.A});
+  const auto guard = args.guard();
+  Tensor o = at::empty({a.B, a.Sq, a.A, a.d}, q.options());
+  Tensor lse = at::empty({a.B, a.A, a.Sq}, q.options().dtype(at::kFloat));
+  check(lb_attn_fwd_paged(&a, q.data_ptr(), k_pool.data_ptr(), v_pool.data_ptr(), (int)k_pool.size(0),
+                          block_table.data_ptr<int>(), (int)block_table.size(1), o.data_ptr(), lse.data_ptr<float>(),
+                          cur_stream()),
+        "attn_fwd_paged");
+  return o;
+}
+
 // ---- KV-cache decoding ------------------------------------------------------------------------------
 // K and V caches [B, G, C, D], bf16 or (with row scales k_scale, v_scale fp32 [B, G, C]) FP8 (E4M3), D 64 or 128.  An
 // FP8 cache's capacity is a multiple of 4: the decode kernel loads the scales of a tile from a 16-byte boundary.  The
@@ -1586,6 +1632,7 @@ TORCH_LIBRARY(libai_b200, m) {
   m.def("sqnorm(Tensor x) -> Tensor", &sqnorm);
   m.def("attn_fwd(Tensor q, Tensor k, Tensor v, bool causal, float scale, Tensor? kv_lens, Tensor? bias=None, Tensor? alibi_slopes=None, float p_drop=0.0, int salt=0, Tensor? kv_start=None, Tensor? doc_start=None, Tensor? prefix_lens=None) -> (Tensor, Tensor, Tensor)", &attn_fwd);
   m.def("attn_bwd(Tensor dout, Tensor q, Tensor k, Tensor v, Tensor o, Tensor lse, bool causal, float scale, Tensor? kv_lens, Tensor? bias=None, Tensor? alibi_slopes=None, Tensor(a!)? dbias=None, float p_drop=0.0, Tensor? rng_state=None, Tensor? kv_start=None, Tensor? doc_start=None, Tensor? prefix_lens=None) -> (Tensor, Tensor, Tensor, Tensor)", &attn_bwd);
+  m.def("attn_fwd_paged(Tensor q, Tensor k_pool, Tensor v_pool, Tensor block_table, int past, float scale, Tensor? kv_start=None, Tensor? alibi_slopes=None) -> Tensor", &attn_fwd_paged);
   m.def("kv_append(Tensor qkv, Tensor(a!) k_cache, Tensor(b!) v_cache, Tensor cache_seqlens, Tensor? cos, Tensor? sin, bool write_q) -> Tensor", &kv_append);
   m.def("kv_append_fp8(Tensor qkv, Tensor(a!) k_cache, Tensor(b!) v_cache, Tensor(c!) k_scale, Tensor(d!) v_scale, Tensor cache_seqlens, Tensor? cos, Tensor? sin, bool write_q) -> Tensor", &kv_append_fp8);
   m.def("window_attn_fwd(Tensor qkv, int H, int W, int window, int shift, int heads, float scale, Tensor table, Tensor? tau) -> (Tensor, Tensor)", &window_attn_fwd);

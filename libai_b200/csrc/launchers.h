@@ -121,6 +121,13 @@ int lb_p2p_allgather(const void* shard, const long* out_ptrs, const long* flag_p
 // (seed, offset) pair it resolved to, for the backward
 int lb_attn_fwd(const lb::AttnArgs* a, const void* q, const void* k, const void* v, void* o, float* lse,
                 const lb::RngArgs* rng, long long* rng_out, cudaStream_t s);
+// the forward over a paged cache: q (a->q_strides) holds the Sq new tokens, appended already; k_pool and v_pool are
+// contiguous bf16 pools [num_pages, G, 64, d] (d = 64 or 128) whose logical row j of sample b is row j % 64 of page
+// block_table[b * max_pages + j / 64], and the keys are the rows [0, a->Sk) (Sk = past + Sq), causal, with kv_start and
+// ALiBi slopes (no kv_lens, dense bias, doc_start, prefix_lens or dropout).  Rows at or past Sk, and table entries
+// outside [0, num_pages), are never read: they count as zero rows.  o [B, Sq, A, d] bf16, lse fp32 [B, A, Sq].
+int lb_attn_fwd_paged(const lb::AttnArgs* a, const void* q, const void* k_pool, const void* v_pool, int num_pages,
+                      const int* block_table, int max_pages, void* o, float* lse, cudaStream_t s);
 // backward: dout with do_strides = {batch, head, seq} over the A query heads; dq written with dq_strides = {batch,
 // group, in-group, seq}, dk and dv with dkv_strides = {batch, head, seq}; delta fp32 [B, A, Sq] and dq_accum
 // (lb_attn_bwd_accum_floats) are workspaces, dq_order [B * A * ceil(Sq / 64)] zeroed by the caller; dbias (optional,

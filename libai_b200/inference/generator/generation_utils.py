@@ -62,7 +62,7 @@ _DEFAULTS = dict(
     pad_token_id=None, decoder_start_token_id=None, forced_bos_token_id=None, forced_eos_token_id=None,
     remove_invalid_values=False, exponential_decay_length_penalty=None, chunk_size_feed_forward=0,
     kv_cache_dtype=None, decode_graphs=False, assistant_model=None, num_assistant_tokens=None,
-    prompt_lookup_num_tokens=None, max_matching_ngram_size=None, paged_kv_cache=False,
+    prompt_lookup_num_tokens=None, max_matching_ngram_size=None, paged_kv_cache=False, prefix_cache_tokens=0,
 )
 # generate()'s arguments for the logits processors speculative decoding refuses, by processor
 _PROCESSOR_ARGS = {
@@ -115,6 +115,13 @@ def _paged_kv_cache(value) -> bool:
     """``generate(paged_kv_cache=...)``: a bool."""
     if not isinstance(value, bool):
         raise ValueError(f"paged_kv_cache must be True or False, got {value!r}")
+    return value
+
+
+def _prefix_cache_tokens(value) -> int:
+    """``generate(prefix_cache_tokens=...)``: an int >= 0."""
+    if isinstance(value, bool) or not isinstance(value, int) or value < 0:
+        raise ValueError(f"prefix_cache_tokens must be an int >= 0, got {value!r}")
     return value
 
 
@@ -497,6 +504,9 @@ class Generator:
                 unfinished = unfinished * (next_tokens != eos_token_id).long()
             if unfinished.max() == 0 or stopping_criteria(input_ids, scores):
                 break
+        cache = getattr(self, "kv_cache", None)
+        if isinstance(cache, PagedKVCache) and cache.fork_n == 1:   # the rows fed: prompt and generated tokens
+            cache.insert(input_ids, model_kwargs.get("attention_mask"))
         self._reset_cache()
         return (input_ids, scores) if output_scores else input_ids
 
@@ -556,15 +566,18 @@ class Generator:
             return result["sequences"], result["sequence_scores"], scores
         return result["sequences"]
 
-    def _shared_prefill(self, input_ids, n: int, model_kwargs):
+    def _shared_prefill(self, input_ids, n: int, model_kwargs, hit: int = 0):
         """The prefill of the ``b`` prompts once, on a paged cache, which then forks into ``n`` sequences per prompt
         (:meth:`PagedKVCache.fork`).  Other per-sequence inputs given for all ``b * n`` sequences (GLM's positions) are
-        taken once per prompt.  Returns the expanded ``input_ids`` and ``model_kwargs`` of the decoding loop, whose
-        ``_first_step`` holds the prefill's last logits, each prompt's row repeated for its ``n`` sequences."""
+        taken once per prompt.  ``hit``: the prompts' first ``hit`` pages are mapped from the prefix index already
+        (:meth:`PagedKVCache.lookup`), so only the tokens after them are fed; the prompt's full pages are then indexed.
+        Returns the expanded ``input_ids`` and ``model_kwargs`` of the decoding loop, whose ``_first_step`` holds the
+        prefill's last logits, each prompt's row repeated for its ``n`` sequences."""
         b = input_ids.shape[0]
         once = {k: v[::n] if torch.is_tensor(v) and v.dim() > 0 and v.shape[0] == b * n else v
                 for k, v in model_kwargs.items()}
-        outputs = self._decode_step(input_ids, once)
+        outputs = self._decode_step(input_ids[:, hit * OF.PAGE_ROWS :], once)
+        self.kv_cache.insert(input_ids, once.get("attention_mask"))
         self.kv_cache.fork(n)
         key = "logits" if "logits" in outputs else "prediction_scores"
         first = {key: outputs[key][:, -1:].repeat_interleave(n, dim=0)}
@@ -575,6 +588,8 @@ class Generator:
     # a decoder-only model whose cached step takes ``{"input_ids": [b, s], "use_cache": True}`` for any s (positions and
     # padding from its StaticKVCache): it can verify speculative proposals, and serve as a draft
     speculative_decoding = False
+    # generate(prefix_cache_tokens=...): a model whose cached rows depend only on the tokens before them
+    prefix_caching = True
 
     def _verify_step(self, block):
         """One cached step of the target on ``block`` ``[b, k + 1]`` (a graph of k + 1 tokens when graphs are on)."""
@@ -819,7 +834,7 @@ class Generator:
                  forced_bos_token_id=None, forced_eos_token_id=None, remove_invalid_values=None,
                  exponential_decay_length_penalty=None, kv_cache_dtype=None, decode_graphs=None, assistant_model=None,
                  num_assistant_tokens=None, prompt_lookup_num_tokens=None, max_matching_ngram_size=None,
-                 paged_kv_cache=None, **model_kwargs):
+                 paged_kv_cache=None, prefix_cache_tokens=None, **model_kwargs):
         """``kv_cache_dtype`` (default: the model cfg's ``kv_cache_dtype``): ``"fp8"`` or ``torch.float8_e4m3fn`` holds
         the preallocated KV cache as E4M3 rows with per-row scales
         (:class:`~libai_b200.inference.kv_cache.StaticKVCache`) for this call: about half the memory, and of the bytes
@@ -851,19 +866,40 @@ class Generator:
         the beams or samples, which share the prompt's pages; a beam reorder rewrites block tables instead of copying
         the cache.  Greedy search and single-sequence sampling run on pages without a fork.  Encoder-decoder models
         (T5/mT5) and models without a preallocated cache, tensor or pipeline parallelism, and speculative decoding
-        raise ``ValueError``."""
+        raise ``ValueError``.
+
+        ``prefix_cache_tokens`` (default: the model cfg's ``prefix_cache_tokens``, else 0 = off): N > 0 keeps up to N
+        tokens (rounded up to 64-row pages) of K/V pages across calls, on a paged cache (it implies
+        ``paged_kv_cache=True``; an explicit ``paged_kv_cache=False`` raises ``ValueError``).  A call whose prompts all
+        start with cached pages maps them and prefills only the rest (at least one token); ``kv_cache.reused_rows``
+        counts the rows taken.  A page is keyed by the tokens and padding mask of its rows and of every row before it,
+        so a left-padded prompt matches prompts with the same padding.  After the prefill the prompt's full pages are
+        cached; after a greedy or single-sample call also those of its generated tokens, so the next chat turn reuses its
+        previous answer.  The pool and its index are kept while later calls fit the pool (batch, sequences per prompt,
+        length and cache format), and are cleared when a parameter or the KV dtype changes, or by
+        ``clear_prefix_cache()``.  The first tokens' logits are not bitwise those of a full prefill (the GEMMs see
+        another number of rows).  Prompts whose padding needs a dense mask, and caches with rows before the prompt
+        (ChatGLM's P-tuning), are neither looked up nor cached.  The cases ``paged_kv_cache`` refuses, and GLM (whose
+        prefix-LM prompt attends bidirectionally), raise ``ValueError``."""
         kv_cache_dtype = _kv_cache_dtype(self._pick(kv_cache_dtype, "kv_cache_dtype"))
-        paged = _paged_kv_cache(self._pick(paged_kv_cache, "paged_kv_cache"))
+        prefix_tokens = _prefix_cache_tokens(self._pick(prefix_cache_tokens, "prefix_cache_tokens"))
+        if prefix_tokens > 0 and paged_kv_cache is False:
+            raise ValueError("prefix_cache_tokens > 0 holds the cache in pages: it cannot run with paged_kv_cache=False")
+        paged = prefix_tokens > 0 or _paged_kv_cache(self._pick(paged_kv_cache, "paged_kv_cache"))
         if paged:
+            what = "prefix_cache_tokens > 0" if prefix_tokens > 0 else "paged_kv_cache=True"
             if not isinstance(self, KVCacheOwner) or self._gcfg("is_encoder_decoder"):
-                raise ValueError(f"paged_kv_cache=True: {type(self).__name__} is not a decoder-only model with a "
+                raise ValueError(f"{what}: {type(self).__name__} is not a decoder-only model with a "
                                  "preallocated KV cache")
             topo = dutil.get_dist_util()
             if topo.tensor_parallel_size > 1 or topo.pipeline_parallel_size > 1:
-                raise ValueError("paged_kv_cache=True: tensor- and pipeline-parallel inference keep contiguous caches")
+                raise ValueError(f"{what}: tensor- and pipeline-parallel inference keep contiguous caches")
             if assistant_model is not None or prompt_lookup_num_tokens is not None:
-                raise ValueError("paged_kv_cache=True: speculative decoding (assistant_model, prompt_lookup_num_tokens) "
+                raise ValueError(f"{what}: speculative decoding (assistant_model, prompt_lookup_num_tokens) "
                                  "runs on contiguous caches")
+            if prefix_tokens > 0 and not self.prefix_caching:
+                raise ValueError(f"prefix_cache_tokens > 0: {type(self).__name__}'s cached rows depend on later "
+                                 "tokens (a bidirectional prompt), so they cannot be reused")
         if kv_cache_dtype is not None and not isinstance(self, KVCacheOwner):
             raise ValueError(f"kv_cache_dtype={kv_cache_dtype}: {type(self).__name__} does not decode on a "
                              "StaticKVCache")
@@ -960,7 +996,7 @@ class Generator:
         fork = num_beams if is_beam else num_return_sequences if is_sample else 1
         with contextlib.ExitStack() as call:
             call.enter_context(_call_state(self, kv_cache_dtype, decode_graphs,
-                                           (fork, input_ids_seq_length) if paged else None))
+                                           (fork, input_ids_seq_length, prefix_tokens) if paged else None))
             models = [self]
             if draft is not None:   # the assistant's cfg sets its cache format
                 call.enter_context(_call_state(draft, _kv_cache_dtype(draft._gcfg("kv_cache_dtype")), decode_graphs))
@@ -984,18 +1020,29 @@ class Generator:
                     max_matching_ngram_size=max_matching_ngram_size, stopping_criteria=stopping_criteria,
                     pad_token_id=pad_token_id, eos_token_id=eos_token_id, output_scores=output_scores, warp=spec_warp,
                     **model_kwargs)
+            # the prefix index: map the prompts' cached pages, then prefill the rest once (_shared_prefill)
+            hit, prefix = 0, prefix_tokens > 0 and model_kwargs.get("use_cache") and isinstance(self.kv_cache,
+                                                                                                PagedKVCache)
+            if prefix:
+                cache = self.kv_cache
+                if self.cache_rows_before_prompt:
+                    cache.prefix_ok = False
+                else:
+                    hit = cache.lookup(input_ids, model_kwargs.get("attention_mask"))
             if is_greedy:
                 if num_return_sequences > 1:
                     raise ValueError(f"num_return_sequences has to be 1, but is {num_return_sequences} when doing greedy search.")
+                if prefix:
+                    input_ids, model_kwargs = self._shared_prefill(input_ids, 1, model_kwargs, hit)
                 return self.greedy_search(input_ids, logits_processor=logits_processor,
                                           stopping_criteria=stopping_criteria, pad_token_id=pad_token_id,
                                           eos_token_id=eos_token_id, is_encoder_decoder=is_enc_dec,
                                           output_scores=output_scores, **model_kwargs)
-            shared = fork > 1 and model_kwargs.get("use_cache") and isinstance(self.kv_cache, PagedKVCache)
+            shared = (fork > 1 or prefix) and model_kwargs.get("use_cache") and isinstance(self.kv_cache, PagedKVCache)
             if is_sample:
                 warper = self._get_logits_warper(top_k, top_p, typical_p, temperature, num_beams, renormalize_logits)
                 if shared:
-                    input_ids, model_kwargs = self._shared_prefill(input_ids, fork, model_kwargs)
+                    input_ids, model_kwargs = self._shared_prefill(input_ids, fork, model_kwargs, hit)
                 else:
                     input_ids, model_kwargs = self._expand_inputs_for_generation(
                         input_ids, expand_size=num_return_sequences, is_encoder_decoder=is_enc_dec, **model_kwargs)
@@ -1011,7 +1058,7 @@ class Generator:
                 scorer = BeamSearchScorer(batch_size=batch_size, num_beams=num_beams, length_penalty=length_penalty,
                                           do_early_stopping=early_stopping, num_beam_hyps_to_keep=num_return_sequences)
                 if shared:
-                    input_ids, model_kwargs = self._shared_prefill(input_ids, fork, model_kwargs)
+                    input_ids, model_kwargs = self._shared_prefill(input_ids, fork, model_kwargs, hit)
                 else:
                     input_ids, model_kwargs = self._expand_inputs_for_generation(
                         input_ids, expand_size=num_beams, is_encoder_decoder=is_enc_dec, **model_kwargs)

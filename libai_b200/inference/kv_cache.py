@@ -19,12 +19,15 @@ instead of copying the cache.
 """
 from __future__ import annotations
 
+import logging
 from typing import Iterable, List, Optional, Tuple
 
 import torch
 
 from libai_b200.ops import functional as OF
 from libai_b200.utils import distributed as dutil
+
+logger = logging.getLogger(__name__)
 
 
 def left_padding(attention_mask: torch.Tensor) -> Optional[torch.Tensor]:
@@ -347,6 +350,18 @@ class PagedKVCacheLayer(KVCacheLayer):
     def pages(self) -> dict:
         return {"block_table": self.cache.block_table}
 
+    def attend(self, q: torch.Tensor, *, scale: float, causal: bool = True, mask=None, bias=None, alibi_slopes=None,
+               rel_bias=None, dropout_p: float = 0.0, training: bool = False, prefix_lens=None) -> torch.Tensor:
+        """As :meth:`KVCacheLayer.attend`; the causal prefill of an empty bf16 cache (no mask, bias, ``rel_bias``,
+        prefix or dropout) runs the paged flash kernel (:func:`OF.attention_paged`), which reads the pages in place
+        and computes what the flash kernel computes over the gathered window."""
+        if (causal and self.length == 0 and mask is None and bias is None and rel_bias is None and prefix_lens is None
+                and not (training and dropout_p > 0) and OF.attention_paged_supported(q, self.k)):
+            return OF.attention_paged(q, self.k, self.v, self.cache.block_table, 0, self.kv_start, scale=scale,
+                                      alibi_slopes=alibi_slopes)
+        return super().attend(q, scale=scale, causal=causal, mask=mask, bias=bias, alibi_slopes=alibi_slopes,
+                              rel_bias=rel_bias, dropout_p=dropout_p, training=training, prefix_lens=prefix_lens)
+
     def window(self, L: int, dtype) -> Tuple[torch.Tensor, torch.Tensor]:
         t = self.cache.block_table
         k, v = OF.kv_pages_gather(self.k, t, L), OF.kv_pages_gather(self.v, t, L)
@@ -383,7 +398,7 @@ class PagedKVCache(StaticKVCache):
 
     def __init__(self, num_layers: int, batch: int, heads: int, head_dim: int, capacity: int,
                  dtype=torch.bfloat16, device=None, layers: Optional[Iterable[int]] = None, kv_dtype=None, *,
-                 fork: int = 1, prompt_len: int = 0):
+                 fork: int = 1, prompt_len: int = 0, prefix_tokens: int = 0):
         self.num_layers, self.heads, self.head_dim = num_layers, heads, head_dim
         self.dtype, self.device = dtype, torch.device(device) if device is not None else torch.device("cpu")
         self.kv_dtype = dtype if kv_dtype is None else kv_dtype
@@ -398,7 +413,17 @@ class PagedKVCache(StaticKVCache):
         self.max_pages = -(-max(int(capacity), 1) // P)
         self.capacity = self.max_pages * P
         shared = min(max(int(prompt_len), 0) // P, self.max_pages)
-        self.num_pages = batch * shared + self.rows * (self.max_pages - shared)
+        # the prefix index's budget: extra pages, so the start of a call never evicts
+        self.prefix_pages = -(-max(int(prefix_tokens), 0) // P)
+        self.num_pages = batch * shared + self.rows * (self.max_pages - shared) + self.prefix_pages
+        self._used = {}       # cached page -> the tick it was last looked up or inserted at
+        self._index = {}      # (parent page or -1, ((token, mask), ... 64)) -> page
+        self._entry = {}      # cached page -> its key
+        self._children = {}   # cached page -> the cached pages that continue it
+        self._tick = 0
+        self.reused_rows = 0  # the rows the last prefill took from the index
+        self.prefix_ok = False   # the call's prompt may be looked up and inserted
+        self.index_owner = None  # what the index is valid for (the weights), set by KVCacheOwner
         self.k: List[Optional[torch.Tensor]] = [None] * num_layers
         self.v: List[Optional[torch.Tensor]] = [None] * num_layers
         self.k_scale: List[Optional[torch.Tensor]] = [None] * num_layers
@@ -529,7 +554,7 @@ class PagedKVCache(StaticKVCache):
         idx = [int(i) for i in beam_idx.tolist()]
         old = self.host_table
         self.host_table = [list(old[i]) for i in idx] + old[self.batch:]
-        refs = [0] * self.num_pages
+        refs = self._index_refs()
         for row in self.host_table[: self.batch]:
             for page in row[: self.mapped]:
                 refs[page] += 1
@@ -547,10 +572,134 @@ class PagedKVCache(StaticKVCache):
         self.length = 0
         self.dense_mask = False
         self.host_table = [[-1] * self.max_pages for _ in range(self.rows)]
-        self.refs = [0] * self.num_pages
-        self.free = list(range(self.num_pages - 1, -1, -1))   # pages are taken from the end: 0, 1, 2, ...
+        self.refs = self._index_refs()   # the prefix index keeps its pages
+        # pages are taken from the end: 0, 1, 2, ...
+        self.free = [p for p in range(self.num_pages - 1, -1, -1) if self.refs[p] == 0]
         self.mapped = 0   # the page slots mapped in every sequence's row
         self._write_table()
+
+    # ---- prefix index -------------------------------------------------------------------------------------------
+    # A full page is immutable once written (only a sequence's last, partly filled page is ever written, and a shared
+    # one is copied first), so a later call can map it into its table instead of computing its rows again.  A page's
+    # key is its parent page (-1 for the first) and the (token id, mask) of its 64 rows: rows with the same key hold
+    # the same K/V for the same weights and cache format, whatever the call.  The index holds one reference per page.
+
+    def _index_refs(self) -> List[int]:
+        refs = [0] * self.num_pages
+        for page in getattr(self, "_entry", {}):
+            refs[page] = 1
+        return refs
+
+    @staticmethod
+    def _page_keys(ids: List[int], mask: List[int], pages: int):
+        P = OF.PAGE_ROWS
+        return [tuple(zip(ids[j * P : (j + 1) * P], mask[j * P : (j + 1) * P])) for j in range(pages)]
+
+    @staticmethod
+    def _rows(input_ids: torch.Tensor, attention_mask: Optional[torch.Tensor]):
+        ids = input_ids.tolist()
+        mask = [[1] * len(r) for r in ids] if attention_mask is None else attention_mask.to(torch.int64).tolist()
+        return ids, mask
+
+    def cached_pages(self) -> int:
+        return len(self._entry)
+
+    def fits(self, batch: int, fork: int, prompt_len: int, capacity: int, prefix_tokens: int, dtype, device,
+             kv_dtype) -> bool:
+        """Whether a call of ``batch`` prompts forked ``fork`` times, with ``prompt_len``-token prompts and up to
+        ``capacity`` rows, runs on this pool with a prefix budget of ``prefix_tokens``: the pool, and its index, are
+        then kept."""
+        P = OF.PAGE_ROWS
+        shared = min(max(int(prompt_len), 0) // P, self.max_pages)
+        need = batch * shared + batch * fork * (self.max_pages - shared) + self.prefix_pages
+        return (self.prompts == batch and self.fork_n == fork and self.max_pages * P >= capacity
+                and self.prefix_pages == -(-int(prefix_tokens) // P) and need <= self.num_pages
+                and self.dtype == dtype and self.device == torch.device(device)
+                and self.kv_dtype == (dtype if kv_dtype is None else kv_dtype))
+
+    def clear_prefix_index(self) -> None:
+        """Drop every cached page (a page a sequence still maps keeps that sequence's reference)."""
+        for page in list(self._entry):
+            del self._index[self._entry.pop(page)]
+            self._release(page)
+        self._children = {}
+
+    def lookup(self, input_ids: torch.Tensor, attention_mask: Optional[torch.Tensor]) -> int:
+        """Before the prefill of the ``batch`` prompts ``input_ids`` ``[batch, s]`` on the empty cache: map the longest
+        run of cached pages every prompt starts with, at most ``(s - 1) // 64`` (at least one token is prefilled, for the
+        first logits), into every row, and set the lengths and ``kv_start`` (the prompt's left padding) as if those rows
+        had been prefilled.  Returns the pages taken; ``reused_rows`` counts their rows.  A prompt whose padding needs a
+        dense mask is neither looked up nor inserted (``prefix_ok``)."""
+        if self.length != 0 or input_ids.shape[0] != self.batch:
+            raise ValueError("lookup: the prompts of an empty cache, one per row")
+        self.reused_rows = 0
+        start = None
+        if attention_mask is not None:
+            start = left_padding(attention_mask)
+        self.prefix_ok = self.prefix_pages > 0 and (attention_mask is None or start is not None)
+        if not self.prefix_ok:
+            return 0
+        s = input_ids.shape[1]
+        ids, mask = self._rows(input_ids, attention_mask)
+        chains = []
+        for b in range(self.batch):
+            parent, chain = -1, []
+            for key in self._page_keys(ids[b], mask[b], (s - 1) // OF.PAGE_ROWS):
+                page = self._index.get((parent, key))
+                if page is None:
+                    break
+                chain.append(page)
+                parent = page
+            chains.append(chain)
+        hit = min(len(c) for c in chains)
+        if hit == 0:
+            return 0
+        self._tick += 1
+        for b, chain in enumerate(chains):
+            for j, page in enumerate(chain[:hit]):
+                self.host_table[b][j] = page
+                self.refs[page] += 1
+                self._used[page] = self._tick
+        rows = hit * OF.PAGE_ROWS
+        self.mapped, self.length, self.reused_rows = hit, rows, rows
+        self.seqlens.fill_(rows)
+        if start is not None:
+            self.kv_start.copy_(start)
+        self._write_table()
+        return hit
+
+    def insert(self, input_ids: torch.Tensor, attention_mask: Optional[torch.Tensor]) -> None:
+        """Index the full pages of every sequence's rows ``[:L]`` (``L = input_ids.shape[1] <= length``: the tokens
+        fed, with their mask), then evict least-recently-used leaves (pages no cached page continues) down to the
+        budget.  Nothing for a call whose prompt is not ``prefix_ok``."""
+        if not self.prefix_ok:
+            return
+        L = min(input_ids.shape[1], self.length)
+        ids, mask = self._rows(input_ids[:, :L], None if attention_mask is None else attention_mask[:, :L])
+        self._tick += 1
+        for b in range(self.batch):
+            parent = -1
+            for j, key in enumerate(self._page_keys(ids[b], mask[b], L // OF.PAGE_ROWS)):
+                page = self._index.get((parent, key))
+                if page is None:
+                    page = self.host_table[b][j]
+                    if page in self._entry:   # cached under another key: cannot happen for an immutable page
+                        break
+                    self._index[(parent, key)], self._entry[page] = page, (parent, key)
+                    self._children[page] = 0
+                    if parent >= 0:
+                        self._children[parent] += 1
+                    self.refs[page] += 1
+                self._used[page] = self._tick
+                parent = page
+        while len(self._entry) > self.prefix_pages:
+            leaf = min((p for p, n in self._children.items() if n == 0), key=lambda p: self._used[p])
+            parent, _ = self._entry.pop(leaf)
+            del self._index[(parent, _)]
+            del self._children[leaf]
+            if parent >= 0:
+                self._children[parent] -= 1
+            self._release(leaf)
 
 
 class KVCacheOwner:
@@ -562,9 +711,9 @@ class KVCacheOwner:
     kv_cache: Optional[StaticKVCache] = None
     past_length = 0
     kv_cache_dtype = None   # what the cache holds: None = the weights' dtype; torch.float8_e4m3fn = FP8 rows
-    # a paged cache for the next allocate_kv_cache: (sequences per prompt, prompt length), set by generate(); None = a
-    # contiguous StaticKVCache
-    kv_cache_paging: Optional[Tuple[int, int]] = None
+    # a paged cache for the next allocate_kv_cache: (sequences per prompt, prompt length, prefix index budget in
+    # tokens), set by generate(); None = a contiguous StaticKVCache
+    kv_cache_paging: Optional[Tuple[int, int, int]] = None
     # the rows a step may reach (the last _prepare_cache's max_positions): a replayed decode graph checks it instead
     max_cache_positions: Optional[int] = None
 
@@ -587,11 +736,20 @@ class KVCacheOwner:
         dtype = getattr(qkv, "compute_dtype", None) or w.dtype
         c = self.kv_cache
         heads = getattr(mods[0], "local_kv_heads", mods[0].local_heads)
-        if self.kv_cache_paging is not None:   # sized for this call: a new pool every time
-            fork, prompt_len = self.kv_cache_paging
-            self.kv_cache = self._decode_graph = None   # the old cache (and a graph on it) go first
-            c = PagedKVCache(len(mods), batch, heads, mods[0].head_size, max_length, dtype, w.device, owned,
-                             self.kv_cache_dtype, fork=fork, prompt_len=prompt_len)
+        if self.kv_cache_paging is not None:
+            fork, prompt_len, prefix_tokens = self.kv_cache_paging
+            if not (prefix_tokens > 0 and isinstance(c, PagedKVCache)
+                    and c.fits(batch, fork, prompt_len, max_length, prefix_tokens, dtype, w.device, self.kv_cache_dtype)):
+                if prefix_tokens > 0 and isinstance(c, PagedKVCache) and c.cached_pages():
+                    logger.info("prefix cache: this call does not fit the paged pool; a new pool starts empty")
+                # sized for this call: the old cache (and a graph on it) go first
+                self.kv_cache = self._decode_graph = c = None
+                c = PagedKVCache(len(mods), batch, heads, mods[0].head_size, max_length, dtype, w.device, owned,
+                                 self.kv_cache_dtype, fork=fork, prompt_len=prompt_len, prefix_tokens=prefix_tokens)
+            weights = self._prefix_cache_weights()
+            if c.index_owner != weights:   # the index holds K/V of other weights
+                c.clear_prefix_index()
+                c.index_owner = weights
         elif (c is None or isinstance(c, PagedKVCache) or not c.matches(batch, dtype, w.device, self.kv_cache_dtype)
               or c.capacity < max_length):
             c = StaticKVCache(len(mods), batch, heads, mods[0].head_size, max_length, dtype, w.device, owned,
@@ -600,6 +758,18 @@ class KVCacheOwner:
         c.reset()
         self.kv_cache, self.past_length = c, 0
         return c
+
+    def _prefix_cache_weights(self) -> tuple:
+        # every parameter's storage and version: load_state_dict, in-place updates and weight quantization change them
+        return tuple((p.data_ptr(), p._version) for p in self.parameters())
+
+    # rows a step writes before the prompt's (ChatGLM's P-tuning prefix): such a cache takes no prefix index
+    cache_rows_before_prompt = 0
+
+    def clear_prefix_cache(self) -> None:
+        """Empty the prefix index of the model's paged cache (``generate(prefix_cache_tokens=...)``)."""
+        if isinstance(self.kv_cache, PagedKVCache):
+            self.kv_cache.clear_prefix_index()
 
     def _prepare_cache(self, input_ids, max_positions: Optional[int] = None) -> StaticKVCache:
         """The cache for this step's ``input_ids`` ``[b, s]``: allocated for a new batch, grown to fit ``s`` more rows."""

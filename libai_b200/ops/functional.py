@@ -1331,7 +1331,8 @@ def decode_attention(q, k_cache, v_cache, cache_seqlens, kv_start, *, scale: flo
     and reads lengths on the device (no host sync; one CUDA-graph capture replays after the lengths change); ``splits``
     > 0 fixes its number of key-range splits.  ``past`` (host int): the rows every sample held before these tokens
     (``cache_seqlens`` all equal to it, as in a :class:`~libai_b200.inference.kv_cache.StaticKVCache`); with it, more
-    than 16 new tokens run the causal flash kernel over the cache window ``[:past + s]`` (chunked prefill).
+    than 16 new tokens run the causal flash kernel over the cache window ``[:past + s]`` (chunked prefill); over a paged
+    bf16 cache (``block_table``) that kernel reads the pages in place (:func:`attention_paged`).
     ``alibi_slopes`` (fp32 ``[a]``, on q's device): ALiBi, every visible score gets ``slope_h·(j − cache_seqlens[b] − i)``
     — the flash kernel's ``slope·(j − i − (sk − sq))`` over the cache window, so both paths score alike.
     ``rel_bias`` (fp32 ``[a, R]``, contiguous, on q's device): T5's relative-position bias, every visible score gets
@@ -1359,6 +1360,9 @@ def decode_attention(q, k_cache, v_cache, cache_seqlens, kv_start, *, scale: flo
                                              int(splits), alibi_slopes, k_scale, v_scale)
             count_launch(2)
             return o
+        if native and k_scale is None and past is not None:
+            return attention_paged(q, k_cache, v_cache, block_table, past, kv_start, scale=scale,
+                                   alibi_slopes=alibi_slopes)
         return decode_attention_paged_ref(q, k_cache, v_cache, block_table, cache_seqlens, kv_start, scale=scale,
                                           splits=splits, past=past, alibi_slopes=alibi_slopes, k_scale=k_scale,
                                           v_scale=v_scale)
@@ -1396,6 +1400,27 @@ def decode_attention(q, k_cache, v_cache, cache_seqlens, kv_start, *, scale: flo
             return o.transpose(1, 2)   # the kernel's [b, s, a, d] output
     return decode_attention_ref(q, k_cache, v_cache, cache_seqlens, kv_start, scale=scale, alibi_slopes=alibi_slopes,
                                 rel_bias=rel_bias, causal=causal)
+
+
+def attention_paged_supported(q, k_pool) -> bool:
+    """True when :func:`attention_paged` runs: bf16 projections on the GPU over a bf16 pool of head dim 64 or 128 (the
+    decode kernels' caches, FP8 excepted)."""
+    return _decode_native(q, k_pool) and k_pool.dtype == torch.bfloat16
+
+
+def attention_paged(q, k_pool, v_pool, block_table, past: int, kv_start=None, *, scale: float, alibi_slopes=None):
+    """Causal flash attention of the new tokens ``q [b, s, a, d]`` (appended already; any strides with d contiguous)
+    over the logical rows ``[:past + s]`` of a paged cache's bf16 pools ``[P, g, 64, d]``, read in place through
+    ``block_table`` ``[b, max_pages]``; ``kv_start`` (int32 ``[b]``) and ``alibi_slopes`` as in :func:`attention`.
+    Returns ``[b, s, a, d]`` contiguous, bit for bit the flash kernel over the gathered rows
+    (``kv_pages_gather(pool, block_table, past + s)``).  Rows at or past ``past + s`` are never read, so they may hold
+    anything.  One launch, no host sync; the sm_90a kernel only (see :func:`attention_paged_supported`)."""
+    if not attention_paged_supported(q, k_pool):
+        raise RuntimeError("attention_paged: needs bf16 q and pools with head dim 64 or 128 on the GPU, with the native "
+                           "extension")
+    o = load_ext().attn_fwd_paged(q, k_pool, v_pool, block_table, int(past), float(scale), kv_start, alibi_slopes)
+    count_launch()
+    return o
 
 
 def decode_attention_paged_ref(q, k_pool, v_pool, block_table, cache_seqlens, kv_start, *, scale: float, splits=0,

@@ -342,6 +342,10 @@ class ChatGLMForConditionalGeneration(nn.Module, ChatGLMPreTrainedModel, KVCache
     def _cache_attention_modules(self):
         return [layer.self_attention for layer in self.glm.encoder.layers]
 
+    @property
+    def cache_rows_before_prompt(self) -> int:
+        return self.glm.pre_seq_len or 0
+
     def allocate_kv_cache(self, batch: int, max_length: int) -> StaticKVCache:
         # the cache also holds the P-tuning prefix rows
         return super().allocate_kv_cache(batch, max_length + (self.glm.pre_seq_len or 0))

@@ -312,6 +312,9 @@ class GLMForConditionalGeneration(nn.Module, KVCacheOwner, Generator):
     """``use_cache=True`` decodes on a :class:`StaticKVCache` (``generate(kv_cache_dtype="fp8")`` holds it in FP8);
     ``use_cache=False`` carries the hidden-state memories through ``memory_states`` / ``past_key_values``."""
 
+    # the prefix-LM prompt attends bidirectionally: a row's K/V depend on later tokens, so no page can be reused
+    prefix_caching = False
+
     @configurable
     def __init__(self, cfg=None, **kwargs):
         super().__init__()
