@@ -114,10 +114,11 @@ def expect(q, k64, v64, *, scale, vis, bias=None, alibi=None, tile, eta_extra=No
 
 
 class Recorder:
-    """The extension with every call recorded.  Attention calls are described: ``("decode_attn", fp8)`` and
-    ``("attn_fwd", bias, alibi, kv_start, key rows, key dtype)`` (the first three: whether the argument was given)."""
+    """The extension with every call recorded.  Attention calls are described: ``("decode_attn", fp8)``,
+    ``("attn_fwd", bias, alibi, kv_start, key rows, key dtype)`` (the first three: whether the argument was given), and
+    over a paged cache ``("decode_attn_paged", fp8)`` and ``("attn_fwd_paged", alibi, past)``."""
 
-    APPENDS = ("kv_append", "kv_append_fp8")
+    APPENDS = ("kv_append", "kv_append_fp8", "kv_append_paged", "kv_append_fp8_paged")
 
     def __init__(self, ext):
         self.ext, self.calls = ext, []
@@ -134,6 +135,10 @@ class Recorder:
                 kv_start = a[10] if len(a) > 10 else k.get("kv_start")
                 self.calls.append(("attn_fwd", a[6] is not None, a[7] is not None, kv_start is not None,
                                    a[1].shape[-2], a[1].dtype))
+            elif name == "decode_attn_paged":   # (q, k, v, table, seqlens, kv_start, scale, splits, alibi, k_scale, ..)
+                self.calls.append(("decode_attn_paged", a[9] is not None))
+            elif name == "attn_fwd_paged":      # (q, k, v, table, past, scale, kv_start, alibi)
+                self.calls.append(("attn_fwd_paged", a[7] is not None, int(a[4])))
             else:
                 self.calls.append((name,))
             return fn(*a, **k)
