@@ -35,6 +35,10 @@
 // Paged K/V (PAGED instances, forward only, causal, no bias or ALiBi, D = 64 and 128): the keys are the logical rows of
 // a paged KV cache, read through its block table; each 128-key tile is two 64-row pages (see AttnPages).
 //
+// Ragged paged K/V (RAGGED instances, attn_fwd_paged_varlen_kernel): N sequences packed along the token axis, each with
+// its own rows already held and its own block-table row; one CTA per (128-query tile of a sequence, query head), the
+// tiles listed by the host (see AttnRagged).
+//
 // Forward, one CTA per (batch, query head, 128-query block), 384 threads:
 //   warpgroup 0  TMA producer (one elected thread): Q once, then K/V tiles of 128 keys (double buffered); it gives
 //                its registers to the consumers (setmaxnreg)
@@ -147,16 +151,35 @@ LB_DEVICE void attn_page_box(const AttnPages& pg, int batch, int slot, int Sk, i
   }
 }
 
+// Ragged paged K/V (RAGGED instances): sequence n owns the query rows cu_q[n] .. cu_q[n + 1] of a packed q [T, A, D]
+// and holds past[n] rows before them in block-table row n; its query i sees its logical rows [0, past[n] + i].  A
+// tile is (n, 128-query block of n), listed heaviest first by the host, which knows every length.  Each CTA runs the
+// paged forward of its sequence alone (Sq = its length, Sk = past + Sq), so its output is that of the PAGED kernel
+// called on the sequence by itself, bit for bit.
+struct AttnRagged {
+  const int* cu_q;    // [N + 1]
+  const int* past;    // [N]
+  const int2* tiles;  // [n_tiles]: (sequence, query block)
+};
+
 // the forward of one CTA; tmap_* and p are the kernel's __grid_constant__ parameters (inlined: no call in the kernel).
 // PAGED: K/V through the block table `pages` (tail: the maps tail_k, tail_v; see AttnPages); only the producer's
 // addresses change, so the shared-memory tiles, and the output, are those of the contiguous kernel over the gathered
 // rows [0, Sk).
-template <int D, int BIAS, bool DROP, bool DOC, bool PREFIX = false, bool PAGED = false>
+// RAGGED (with PAGED; see AttnRagged): p, pages are the sequence's own (p.o, p.lse and the table at its rows), q_blk its
+// query block and q_row its first row in q.  One tail map cannot end at every sequence's window, so the tail maps are
+// the full ones and the last page's rows past Sk arrive as they are in the pool (anything, NaN included).  Their
+// scores are masked by assignment, so K needs nothing; V's rows at or past Sk in the window's last tile are zeroed in
+// shared memory before P·V (the consumers' generic stores, a proxy fence, then a barrier of the 256 consumer threads),
+// so that tile holds what the tail map would have loaded.
+template <int D, int BIAS, bool DROP, bool DOC, bool PREFIX = false, bool PAGED = false, bool RAGGED = false>
 LB_DEVICE void attn_fwd_cta(const CUtensorMap& tmap_q, const CUtensorMap& tmap_k, const CUtensorMap& tmap_v,
                             const AttnFwdParams& p, const CUtensorMap* tail_k = nullptr,
-                            const CUtensorMap* tail_v = nullptr, const AttnPages* pages = nullptr) {
+                            const CUtensorMap* tail_v = nullptr, const AttnPages* pages = nullptr, int rg_blk = 0,
+                            int rg_row = 0) {
   static_assert(!PAGED || (!DROP && !DOC && !PREFIX && BIAS != BIAS_DENSE), "paged K/V: no dropout, dense bias, "
                 "packed sequences or prefix");
+  static_assert(!RAGGED || PAGED, "ragged sequences read paged K/V");
   static_assert(!DOC || (BIAS == BIAS_NONE && !DROP), "packed sequences run without bias and dropout");
   static_assert(!PREFIX || (BIAS == BIAS_NONE && !DOC), "a prefix runs without bias and packed sequences");
   using Cfg = AttnFwdCfg<D>;
@@ -175,8 +198,8 @@ LB_DEVICE void attn_fwd_cta(const CUtensorMap& tmap_q, const CUtensorMap& tmap_k
 
   const int warp_idx = threadIdx.x / 32;
   // heavy (late) query blocks first: better tail behaviour under the causal mask
-  const int q_blk = static_cast<int>(gridDim.x) - 1 - static_cast<int>(blockIdx.x);
-  const int head = blockIdx.y, batch = blockIdx.z;
+  const int q_blk = RAGGED ? rg_blk : static_cast<int>(gridDim.x) - 1 - static_cast<int>(blockIdx.x);
+  const int head = blockIdx.y, batch = RAGGED ? 0 : blockIdx.z;
   const int kv_head = head / p.r;
   const int q0 = q_blk * ATT_BM;
   const int kv_len = p.kv_lens != nullptr ? max(1, min(p.Sk, p.kv_lens[batch])) : p.Sk;
@@ -219,7 +242,8 @@ LB_DEVICE void attn_fwd_cta(const CUtensorMap& tmap_q, const CUtensorMap& tmap_k
       mbar_arrive_expect_tx(q_full, Cfg::TILE_BYTES);
 #pragma unroll
       for (int c = 0; c < Cfg::CHUNKS; ++c)
-        tma_load_5d(sQ + c * (ATT_BM * 128), &tmap_q, q_full, c * 64, q0, head - kv_head * p.r, kv_head, batch);
+        tma_load_5d(sQ + c * (ATT_BM * 128), &tmap_q, q_full, c * 64, RAGGED ? rg_row + q0 : q0, head - kv_head * p.r,
+                    kv_head, batch);
       for (int it = 0; it < nkv; ++it) {
         const int j = j0 + it, b = it & 1;
         const uint32_t par = ((it >> 1) & 1) ^ 1;
@@ -412,6 +436,19 @@ LB_DEVICE void attn_fwd_cta(const CUtensorMap& tmap_q, const CUtensorMap& tmap_k
     }
     // ---- O += P·V_j
     mbar_wait(&v_full[b], par);
+    if constexpr (RAGGED) {
+      // the window's last tile: rows kv_len - kbase .. 127 of every 64-column chunk (the 128B swizzle permutes the
+      // 16-byte pieces inside a row, so a chunk's rows from r0 on are one contiguous range)
+      const int r0 = kv_len - kbase;
+      if (r0 < ATT_BN) {
+        for (int c = 0; c < Cfg::CHUNKS; ++c) {
+          uint4* z = reinterpret_cast<uint4*>(sV + b * Cfg::TILE_BYTES + c * (ATT_BN * 128) + r0 * 128);
+          for (int e = threadIdx.x - 128; e < (ATT_BN - r0) * 8; e += 256) z[e] = make_uint4(0u, 0u, 0u, 0u);
+        }
+        fence_proxy_async();   // the generic stores, before the wgmma reads the tile through the async proxy
+        asm volatile("bar.sync 1, 256;\n" ::: "memory");
+      }
+    }
     const uint32_t v_addr = smem_u32(sV + b * Cfg::TILE_BYTES);
     wgmma_fence();
 #pragma unroll
@@ -471,6 +508,26 @@ attn_fwd_paged_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_c
                       const __grid_constant__ CUtensorMap tail_k, const __grid_constant__ CUtensorMap tail_v,
                       const __grid_constant__ AttnPages pages) {
   attn_fwd_cta<D, BIAS, false, false, false, true>(tmap_q, tmap_k, tmap_v, p, &tail_k, &tail_v, &pages);
+}
+// ragged paged K/V (AttnRagged): the sequences of one packed q, each causal over its own pages, without bias or with
+// ALiBi; p holds the shapes shared by every sequence (A, d, r, scale, slopes), p.o [T, A, d] and p.lse [T * A], whose
+// sequence n part is [A, Sq_n] at A * cu_q[n]; pages.table is [N, max_pages]
+template <int D, int BIAS>
+__global__ void __launch_bounds__(ATT_FWD_THREADS, 1)
+attn_fwd_paged_varlen_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_k,
+                             const __grid_constant__ CUtensorMap tmap_v, const __grid_constant__ AttnFwdParams p,
+                             const __grid_constant__ AttnPages pages, const __grid_constant__ AttnRagged rg) {
+  const int2 tile = rg.tiles[blockIdx.x];
+  const int n = tile.x, row0 = rg.cu_q[n];
+  AttnFwdParams sp = p;
+  sp.Sq = rg.cu_q[n + 1] - row0;
+  sp.Sk = rg.past[n] + sp.Sq;
+  sp.o = p.o + static_cast<size_t>(row0) * p.A * p.d;
+  sp.lse = p.lse + static_cast<size_t>(row0) * p.A;
+  AttnPages pg = pages;
+  pg.table = pages.table + static_cast<size_t>(n) * pages.max_pages;
+  attn_fwd_cta<D, BIAS, false, false, false, true, true>(tmap_q, tmap_k, tmap_v, sp, &tmap_k, &tmap_v, &pg, tile.y,
+                                                         row0);
 }
 
 }  // namespace lb
@@ -658,6 +715,61 @@ extern "C" int lb_attn_fwd_paged(const lb::AttnArgs* a, const void* q, const voi
                        : launch_fwd_paged_t<64, lb::BIAS_NONE>(maps, p, pages, s));
   return (int)(alibi ? launch_fwd_paged_t<128, lb::BIAS_ALIBI>(maps, p, pages, s)
                      : launch_fwd_paged_t<128, lb::BIAS_NONE>(maps, p, pages, s));
+}
+
+namespace {
+template <int D, int BIAS>
+cudaError_t launch_fwd_paged_varlen_t(const CUtensorMap (&maps)[3], const lb::AttnFwdParams& p,
+                                      const lb::AttnPages& pages, const lb::AttnRagged& rg, int n_tiles,
+                                      cudaStream_t s) {
+  using Cfg = lb::AttnFwdCfg<D>;
+  auto kern = lb::attn_fwd_paged_varlen_kernel<D, BIAS>;
+  static bool configured = false;
+  if (!configured) {
+    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES);
+    if (e != cudaSuccess) return e;
+    configured = true;
+  }
+  kern<<<dim3(n_tiles, p.A), lb::ATT_FWD_THREADS, Cfg::SMEM_BYTES, s>>>(maps[0], maps[1], maps[2], p, pages, rg);
+  return cudaGetLastError();
+}
+}  // namespace
+// o [T, A, d] and lse [T * A] of the N ragged sequences of q [T, A, d] (a->B = 1, a->Sq = T) over the paged pools
+// [num_pages, G, 64, d]; see launchers.h.  Returns -8 for a problem the paged instances do not run (as
+// lb_attn_fwd_paged, kv_start included) and -9 for an empty pool or table.
+extern "C" int lb_attn_fwd_paged_varlen(const lb::AttnArgs* a, const void* q, const void* k_pool, const void* v_pool,
+                                        int num_pages, const int* block_table, int max_pages, const int* cu_q,
+                                        const int* past, const int* tiles, int n_tiles, void* o, float* lse,
+                                        cudaStream_t s) {
+  lb::AttnArgs full = *a;
+  full.Sk = a->Sq;   // check_attn_args looks at the shapes of q; the key windows are per sequence
+  const int tile = check_attn_args(full);
+  if (tile < 0) return tile;
+  if (a->B != 1 || a->d != tile || !a->causal || a->kv_lens != nullptr || a->kv_start != nullptr ||
+      a->bias != nullptr || a->doc_start != nullptr || a->prefix_lens != nullptr || a->p_drop > 0.f)
+    return -8;
+  if (num_pages <= 0 || max_pages <= 0) return -9;
+  if (n_tiles == 0) return 0;
+  const int P = lb::ATT_PAGE_ROWS;
+  const long pool_strides[3] = {(long)a->G * P * a->d, (long)P * a->d, a->d};   // {page, head, row}
+  CUtensorMap maps[3];   // q, k, v
+  if (!make_q_tmap(&maps[0], q, 1, a->G, a->A / a->G, a->Sq, a->d, a->q_strides, 128)) return -2;
+  if (!make_qkv_tmap(&maps[1], k_pool, num_pages, a->G, P, a->d, pool_strides, P)) return -2;
+  if (!make_qkv_tmap(&maps[2], v_pool, num_pages, a->G, P, a->d, pool_strides, P)) return -2;
+  lb::AttnFwdParams p;
+  fill_score_params(p, full, false);
+  p.o = reinterpret_cast<__nv_bfloat16*>(o);
+  p.lse = lse;
+  memset(&p.rng, 0, sizeof(p.rng));
+  p.rng_out = nullptr;
+  const lb::AttnPages pages{block_table, max_pages, num_pages};
+  const lb::AttnRagged rg{cu_q, past, reinterpret_cast<const int2*>(tiles)};
+  const bool alibi = p.alibi_slopes != nullptr;
+  if (tile == 64)
+    return (int)(alibi ? launch_fwd_paged_varlen_t<64, lb::BIAS_ALIBI>(maps, p, pages, rg, n_tiles, s)
+                       : launch_fwd_paged_varlen_t<64, lb::BIAS_NONE>(maps, p, pages, rg, n_tiles, s));
+  return (int)(alibi ? launch_fwd_paged_varlen_t<128, lb::BIAS_ALIBI>(maps, p, pages, rg, n_tiles, s)
+                     : launch_fwd_paged_varlen_t<128, lb::BIAS_NONE>(maps, p, pages, rg, n_tiles, s));
 }
 // =================================================================================================
 // Backward.  One CTA per (batch, K/V head, NWG consecutive 64-key blocks).  Consumer warpgroup w (warpgroups 1 ..

@@ -1123,6 +1123,59 @@ Tensor attn_fwd_paged(const Tensor& q, const Tensor& k_pool, const Tensor& v_poo
   return o;
 }
 
+// The causal flash attention of N ragged sequences packed in q [T, A, D] (any strides with D contiguous) over their
+// logical rows of a paged cache's bf16 pools [P, G, 64, D]: sequence n owns the rows cu_q[n] .. cu_q[n + 1] of q and
+// holds past[n] rows before them in row n of block_table int32 [N, max_pages] (cu_q int32 [N + 1], past int32 [N]).
+// tiles int32 [n_tiles, 2] lists (n, 128-query block) once for every block of every sequence (built on the host, which
+// knows the lengths).  Those device values are the caller's guarantee: cu_q non-decreasing from 0 to at most T,
+// past[n] + Sq_n <= max_pages * 64, and the table entries of the rows each sequence reads (an entry outside [0, P)
+// reads as zero rows).  alibi_slopes fp32 [A] as in attn_fwd.  Returns o [T, A, D]; rows of no sequence are left
+// uninitialised.
+Tensor attn_fwd_paged_varlen(const Tensor& q, const Tensor& k_pool, const Tensor& v_pool, const Tensor& block_table,
+                             const Tensor& cu_q, const Tensor& past, const Tensor& tiles, double scale,
+                             const c10::optional<Tensor>& alibi_slopes) {
+  Args args("attn_fwd_paged_varlen");
+  args("q", q, at::kBFloat16, {kAny, kAny, kAny}, Layout::LastDimContiguous, 16);
+  const int64_t D = q.size(2);
+  TORCH_CHECK(D == 64 || D == 128, "attn_fwd_paged_varlen: head dim must be 64 or 128, got ", D);
+  args("k_pool", k_pool, at::kBFloat16, {kAny, kAny, 64, D});
+  args("v_pool", v_pool, at::kBFloat16, k_pool.sizes());
+  args("block_table", block_table, at::kInt, {kAny, kAny});
+  const int64_t N = block_table.size(0);
+  args("cu_q", cu_q, at::kInt, {N + 1});
+  args("past", past, at::kInt, {N});
+  args("tiles", tiles, at::kInt, {kAny, 2}, Layout::Contiguous, 8);
+  lb::AttnArgs a{};
+  a.B = 1;
+  a.Sq = (int)q.size(0);
+  a.A = (int)q.size(1);
+  a.G = (int)k_pool.size(1);
+  a.d = (int)D;
+  TORCH_CHECK(a.G > 0 && a.A % a.G == 0, "attn_fwd_paged_varlen: the query heads must be a multiple of the K/V heads");
+  TORCH_CHECK(k_pool.size(0) >= 1 && k_pool.size(0) <= INT32_MAX, "attn_fwd_paged_varlen: 1 <= pages <= INT32_MAX");
+  TORCH_CHECK(a.Sq >= 1 && N >= 1 && block_table.size(1) >= 1, "attn_fwd_paged_varlen: at least one token, one "
+              "sequence and one table column");
+  TORCH_CHECK(tiles.size(0) <= INT32_MAX / 2, "attn_fwd_paged_varlen: too many tiles");
+  const long r = a.A / a.G;
+  a.q_strides[0] = (long)q.size(0) * q.stride(0);
+  a.q_strides[1] = r * q.stride(1);
+  a.q_strides[2] = q.stride(1);
+  a.q_strides[3] = q.stride(0);
+  for (int i = 0; i < 3; ++i) a.k_strides[i] = a.v_strides[i] = k_pool.stride(i);
+  a.causal = true;
+  a.scale = (float)scale;
+  a.alibi_slopes = args.opt<const float>("alibi_slopes", alibi_slopes, at::kFloat, {a.A});
+  const auto guard = args.guard();
+  Tensor o = at::empty({a.Sq, a.A, a.d}, q.options());
+  Tensor lse = at::empty({(int64_t)a.Sq * a.A}, q.options().dtype(at::kFloat));
+  check(lb_attn_fwd_paged_varlen(&a, q.data_ptr(), k_pool.data_ptr(), v_pool.data_ptr(), (int)k_pool.size(0),
+                                 block_table.data_ptr<int>(), (int)block_table.size(1), cu_q.data_ptr<int>(),
+                                 past.data_ptr<int>(), tiles.data_ptr<int>(), (int)tiles.size(0), o.data_ptr(),
+                                 lse.data_ptr<float>(), cur_stream()),
+        "attn_fwd_paged_varlen");
+  return o;
+}
+
 // ---- KV-cache decoding ------------------------------------------------------------------------------
 // K and V caches [B, G, C, D], bf16 or (with row scales k_scale, v_scale fp32 [B, G, C]) FP8 (E4M3), D 64 or 128.  An
 // FP8 cache's capacity is a multiple of 4: the decode kernel loads the scales of a tile from a 16-byte boundary.  The
@@ -1213,6 +1266,39 @@ Tensor kv_append_fp8_paged(const Tensor& qkv, const Tensor& k_pool, const Tensor
                            const c10::optional<Tensor>& cosv, const c10::optional<Tensor>& sinv, bool write_q) {
   return kv_append_any("kv_append_fp8_paged", qkv, k_pool, v_pool, &k_scale, &v_scale, cache_seqlens, cosv, sinv,
                        write_q, &block_table);
+}
+
+// k, v of the packed projection qkv [1, T, A, 3D] or [1, T, G, r + 2, D] of N ragged sequences go to their pages: token
+// t of sequence n (cu_q[n] <= t < cu_q[n + 1]) to logical row past[n] + t - cu_q[n] of row n of block_table int32
+// [N, max_pages], rotated at that position with cos/sin; bf16 pools [P, G, 64, D].  Like the lengths of
+// kv_append_paged, cu_q (int32 [N + 1], from 0 to T, non-decreasing), past (int32 [N]) and the page ids of the rows
+// written are the caller's guarantee.  Returns q [1, T, G * r, D] when write_q, else empty.
+Tensor kv_append_paged_varlen(const Tensor& qkv, const Tensor& k_pool, const Tensor& v_pool, const Tensor& block_table,
+                              const Tensor& cu_q, const Tensor& past, const c10::optional<Tensor>& cosv,
+                              const c10::optional<Tensor>& sinv, bool write_q) {
+  const char* op = "kv_append_paged_varlen";
+  Args args(op);
+  args("qkv", qkv, at::kBFloat16, qkv.sizes());
+  const PackedQKV g = packed_qkv(qkv, op);
+  TORCH_CHECK(g.B == 1, op, ": the sequences are packed along dim 1 of a batch of 1, got batch ", g.B);
+  cache_args(args, k_pool, v_pool, nullptr, nullptr, {kAny, g.G, 64, g.D});
+  args("block_table", block_table, at::kInt, {kAny, kAny});
+  const int64_t N = block_table.size(0);
+  TORCH_CHECK(N >= 1 && N <= INT32_MAX && block_table.size(1) >= 1, op, ": at least one sequence and table column");
+  args("cu_q", cu_q, at::kInt, {N + 1});
+  args("past", past, at::kInt, {N});
+  TORCH_CHECK(given(cosv) == given(sinv), op, ": cos and sin go together");
+  if (given(cosv)) rope_tables(args, *cosv, *sinv, 0, g.D);
+  const auto guard = args.guard();
+  const int T = g.S, A = g.G * g.r;
+  Tensor q_out = write_q ? at::empty({1, T, A, g.D}, qkv.options()) : at::empty({0}, qkv.options());
+  check(lb_kv_append_paged_varlen(qkv.data_ptr(), given(cosv) ? cosv->data_ptr<float>() : nullptr,
+                                  given(sinv) ? sinv->data_ptr<float>() : nullptr,
+                                  write_q ? q_out.data_ptr() : nullptr, k_pool.data_ptr(), v_pool.data_ptr(),
+                                  cu_q.data_ptr<int>(), past.data_ptr<int>(), (int)N, block_table.data_ptr<int>(),
+                                  (int)block_table.size(1), T, g.G, g.r, g.D, cur_stream()),
+        op);
+  return q_out;
 }
 
 // Copies page src to page dst of every array of `arrays` (the K and V pools, and the FP8 scales, of every layer of a
@@ -1633,6 +1719,8 @@ TORCH_LIBRARY(libai_b200, m) {
   m.def("attn_fwd(Tensor q, Tensor k, Tensor v, bool causal, float scale, Tensor? kv_lens, Tensor? bias=None, Tensor? alibi_slopes=None, float p_drop=0.0, int salt=0, Tensor? kv_start=None, Tensor? doc_start=None, Tensor? prefix_lens=None) -> (Tensor, Tensor, Tensor)", &attn_fwd);
   m.def("attn_bwd(Tensor dout, Tensor q, Tensor k, Tensor v, Tensor o, Tensor lse, bool causal, float scale, Tensor? kv_lens, Tensor? bias=None, Tensor? alibi_slopes=None, Tensor(a!)? dbias=None, float p_drop=0.0, Tensor? rng_state=None, Tensor? kv_start=None, Tensor? doc_start=None, Tensor? prefix_lens=None) -> (Tensor, Tensor, Tensor, Tensor)", &attn_bwd);
   m.def("attn_fwd_paged(Tensor q, Tensor k_pool, Tensor v_pool, Tensor block_table, int past, float scale, Tensor? kv_start=None, Tensor? alibi_slopes=None) -> Tensor", &attn_fwd_paged);
+  m.def("attn_fwd_paged_varlen(Tensor q, Tensor k_pool, Tensor v_pool, Tensor block_table, Tensor cu_q, Tensor past, Tensor tiles, float scale, Tensor? alibi_slopes=None) -> Tensor", &attn_fwd_paged_varlen);
+  m.def("kv_append_paged_varlen(Tensor qkv, Tensor(a!) k_pool, Tensor(b!) v_pool, Tensor block_table, Tensor cu_q, Tensor past, Tensor? cos, Tensor? sin, bool write_q) -> Tensor", &kv_append_paged_varlen);
   m.def("kv_append(Tensor qkv, Tensor(a!) k_cache, Tensor(b!) v_cache, Tensor cache_seqlens, Tensor? cos, Tensor? sin, bool write_q) -> Tensor", &kv_append);
   m.def("kv_append_fp8(Tensor qkv, Tensor(a!) k_cache, Tensor(b!) v_cache, Tensor(c!) k_scale, Tensor(d!) v_scale, Tensor cache_seqlens, Tensor? cos, Tensor? sin, bool write_q) -> Tensor", &kv_append_fp8);
   m.def("window_attn_fwd(Tensor qkv, int H, int W, int window, int shift, int heads, float scale, Tensor table, Tensor? tau) -> (Tensor, Tensor)", &window_attn_fwd);

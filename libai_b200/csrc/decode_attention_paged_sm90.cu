@@ -14,7 +14,8 @@
 //   per row as before (only the address changes); FP8 issues one bulk copy per page piece and array, at most two.
 //   Instances: no score bias and ALiBi, bf16 and FP8, D = 64 and 128.
 // appends: kv_append_body / kv_append_fp8_body with the row address taken through the table; bytes and scales are
-//   those of the contiguous appends.
+//   those of the contiguous appends.  The ragged bf16 append (kv_append_body's RAGGED flag) writes the tokens of N
+//   sequences packed along one axis, each at its own rows; its bytes are those of the paged append per sequence.
 // page copy: the (src, dst) page pairs of every array of a list (K, V and the FP8 scales of every layer) in one
 //   launch.
 #include "decode_attention_sm90.cuh"
@@ -70,6 +71,16 @@ __global__ void kv_append_paged_kernel(const __nv_bfloat16* __restrict__ qkv, co
   kv_append_body<true>(qkv, cosv, sinv, q_out, kc, vc, seqlens, table, max_pages, B, Sq, G, r, kTile, D);
 }
 
+// the append of N ragged sequences packed along the token axis (kv_append_body's RAGGED flag)
+__global__ void kv_append_paged_varlen_kernel(const __nv_bfloat16* __restrict__ qkv, const float* __restrict__ cosv,
+                                              const float* __restrict__ sinv, __nv_bfloat16* __restrict__ q_out,
+                                              __nv_bfloat16* __restrict__ kc, __nv_bfloat16* __restrict__ vc,
+                                              const int* __restrict__ cu_q, const int* __restrict__ past, int nseq,
+                                              const int* __restrict__ table, int max_pages, int T, int G, int r,
+                                              int D) {
+  kv_append_body<true, true>(qkv, cosv, sinv, q_out, kc, vc, past, table, max_pages, 1, T, G, r, kTile, D, cu_q, nseq);
+}
+
 template <int D>
 __global__ void __launch_bounds__(256) kv_append_fp8_paged_kernel(
     const __nv_bfloat16* __restrict__ qkv, const float* __restrict__ cosv, const float* __restrict__ sinv,
@@ -105,6 +116,21 @@ extern "C" int lb_kv_append_paged(const void* qkv, const float* cosv, const floa
       static_cast<const __nv_bfloat16*>(qkv), cosv, sinv, static_cast<__nv_bfloat16*>(q_out),
       static_cast<__nv_bfloat16*>(k_pool), static_cast<__nv_bfloat16*>(v_pool), seqlens, block_table, max_pages, B, Sq,
       G, r, D);
+  return (int)cudaGetLastError();
+}
+
+extern "C" int lb_kv_append_paged_varlen(const void* qkv, const float* cosv, const float* sinv, void* q_out,
+                                         void* k_pool, void* v_pool, const int* cu_q, const int* past, int nseq,
+                                         const int* block_table, int max_pages, int T, int G, int r, int D,
+                                         cudaStream_t s) {
+  const size_t total = (size_t)T * G * (D / 2);
+  if (total == 0 || nseq == 0) return 0;
+  const int threads = 256;
+  const int blocks = (int)((total + threads - 1) / threads < 4096 ? (total + threads - 1) / threads : 4096);
+  lb::dec::kv_append_paged_varlen_kernel<<<blocks, threads, 0, s>>>(
+      static_cast<const __nv_bfloat16*>(qkv), cosv, sinv, static_cast<__nv_bfloat16*>(q_out),
+      static_cast<__nv_bfloat16*>(k_pool), static_cast<__nv_bfloat16*>(v_pool), cu_q, past, nseq, block_table,
+      max_pages, T, G, r, D);
   return (int)cudaGetLastError();
 }
 

@@ -421,13 +421,17 @@ __device__ __forceinline__ size_t cache_row(const int* table, int max_pages, int
     return ((size_t)b * G + g) * C + pos;
 }
 
-// the bf16 cache append (kv_append_kernel, and its paged instance): one thread per (b, i, group, c < D/2)
-template <bool PAGED>
+// the bf16 cache append (kv_append_kernel, and its paged instances): one thread per (b, i, group, c < D/2).
+// RAGGED (paged, B = 1): token i belongs to the sequence n with cu_q[n] <= i < cu_q[n + 1] (nseq sequences, found by
+// binary search) and goes to its logical row seqlens[n] + i - cu_q[n] through table row n.
+template <bool PAGED, bool RAGGED = false>
 __device__ __forceinline__ void kv_append_body(const __nv_bfloat16* __restrict__ qkv, const float* __restrict__ cosv,
                                                const float* __restrict__ sinv, __nv_bfloat16* __restrict__ q_out,
                                                __nv_bfloat16* __restrict__ kc, __nv_bfloat16* __restrict__ vc,
                                                const int* __restrict__ seqlens, const int* __restrict__ table,
-                                               int max_pages, int B, int Sq, int G, int r, int C, int D) {
+                                               int max_pages, int B, int Sq, int G, int r, int C, int D,
+                                               const int* __restrict__ cu_q = nullptr, int nseq = 0) {
+  static_assert(!RAGGED || PAGED, "ragged sequences append to pages");
   const int half = D / 2;
   const size_t total = (size_t)B * Sq * G * half;
   for (size_t idx = blockIdx.x * (size_t)blockDim.x + threadIdx.x; idx < total; idx += (size_t)gridDim.x * blockDim.x) {
@@ -436,9 +440,20 @@ __device__ __forceinline__ void kv_append_body(const __nv_bfloat16* __restrict__
     const int g = static_cast<int>(grp % G);
     const int i = static_cast<int>((grp / G) % Sq);
     const int b = static_cast<int>(grp / ((size_t)G * Sq));
-    const int pos = seqlens[b] + i;
+    int seq = b, pos;
+    if constexpr (RAGGED) {
+      int lo = 0, hi = nseq - 1;   // the last n with cu_q[n] <= i
+      while (lo < hi) {
+        const int mid = (lo + hi + 1) / 2;
+        if (cu_q[mid] <= i) lo = mid; else hi = mid - 1;
+      }
+      seq = lo;
+      pos = seqlens[seq] + i - cu_q[seq];
+    } else {
+      pos = seqlens[b] + i;
+    }
     const size_t in = grp * (r + 2) * D;
-    const size_t crow = cache_row<PAGED>(table, max_pages, b, g, G, C, pos) * D;
+    const size_t crow = cache_row<PAGED>(table, max_pages, seq, g, G, C, pos) * D;
     RopePair t{1.f, 1.f, 0.f, 0.f};
     if (cosv != nullptr) t = RopePair::load(cosv, sinv, pos, c, D);
     for (int j = 0; j <= r; ++j) {   // slots 0 .. r - 1: q of query head g * r + j; slot r: k

@@ -128,6 +128,16 @@ int lb_attn_fwd(const lb::AttnArgs* a, const void* q, const void* k, const void*
 // outside [0, num_pages), are never read: they count as zero rows.  o [B, Sq, A, d] bf16, lse fp32 [B, A, Sq].
 int lb_attn_fwd_paged(const lb::AttnArgs* a, const void* q, const void* k_pool, const void* v_pool, int num_pages,
                       const int* block_table, int max_pages, void* o, float* lse, cudaStream_t s);
+// the forward of N ragged sequences over a paged cache: q [T, A, d] (a->B = 1, a->Sq = T, a->q_strides) packs them,
+// sequence n owning rows cu_q[n] .. cu_q[n + 1] and holding past[n] rows before them in table row n
+// (block_table [N, max_pages]); its query i sees its logical rows [0, past[n] + i], causal, with ALiBi slopes (no
+// kv_start, kv_lens, dense bias, doc_start, prefix_lens or dropout).  tiles int32 [n_tiles, 2]: (n, 128-query block),
+// one CTA per tile and query head.  Each sequence's output is lb_attn_fwd_paged's on that sequence alone, bit for bit;
+// rows past its window, and table entries outside [0, num_pages), never reach P·V.  o [T, A, d] bf16 (rows of no
+// sequence are not written), lse fp32 [T * A] (sequence n's [A, Sq_n] at A * cu_q[n]).
+int lb_attn_fwd_paged_varlen(const lb::AttnArgs* a, const void* q, const void* k_pool, const void* v_pool,
+                             int num_pages, const int* block_table, int max_pages, const int* cu_q, const int* past,
+                             const int* tiles, int n_tiles, void* o, float* lse, cudaStream_t s);
 // backward: dout with do_strides = {batch, head, seq} over the A query heads; dq written with dq_strides = {batch,
 // group, in-group, seq}, dk and dv with dkv_strides = {batch, head, seq}; delta fp32 [B, A, Sq] and dq_accum
 // (lb_attn_bwd_accum_floats) are workspaces, dq_order [B * A * ceil(Sq / 64)] zeroed by the caller; dbias (optional,
@@ -160,6 +170,12 @@ int lb_kv_append_fp8(const void* qkv, const float* cosv, const float* sinv, void
 int lb_kv_append_paged(const void* qkv, const float* cosv, const float* sinv, void* q_out, void* k_pool, void* v_pool,
                        const int* seqlens, const int* block_table, int max_pages, int B, int Sq, int G, int r, int D,
                        cudaStream_t s);
+// lb_kv_append_paged for N ragged sequences packed along Sq (B = 1): token t of sequence n (cu_q[n] <= t <
+// cu_q[n + 1], int32 [N + 1] on the device) goes to logical row past[n] + t - cu_q[n] of table row n, rotated at that
+// position; bf16 pools only
+int lb_kv_append_paged_varlen(const void* qkv, const float* cosv, const float* sinv, void* q_out, void* k_pool,
+                              void* v_pool, const int* cu_q, const int* past, int nseq, const int* block_table,
+                              int max_pages, int T, int G, int r, int D, cudaStream_t s);
 int lb_kv_append_fp8_paged(const void* qkv, const float* cosv, const float* sinv, void* q_out, void* k_pool,
                            void* v_pool, float* k_scale, float* v_scale, const int* seqlens, const int* block_table,
                            int max_pages, int B, int Sq, int G, int r, int D, cudaStream_t s);

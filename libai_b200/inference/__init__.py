@@ -1,5 +1,7 @@
 import torch
 
+from .engine import GenerationEngine, RequestOutput  # noqa: F401
+
 
 def quantize_weights_fp8_(model, exclude=("lm_head", "output_layer")):
     """Convert, in place, every ``Linear1D`` of ``model`` whose qualified name does not end with one of ``exclude`` to

@@ -590,6 +590,9 @@ class Generator:
     speculative_decoding = False
     # generate(prefix_cache_tokens=...): a model whose cached rows depend only on the tokens before them
     prefix_caching = True
+    # GenerationEngine (continuous batching): a model whose cached step takes positions only from the cache's
+    # per-sequence lengths, with continuous_batching_logits and continuous_batching_max_length
+    continuous_batching = False
 
     def _verify_step(self, block):
         """One cached step of the target on ``block`` ``[b, k + 1]`` (a graph of k + 1 tokens when graphs are on)."""

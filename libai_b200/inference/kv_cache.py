@@ -88,6 +88,101 @@ def padding_bounds(attention_mask: torch.Tensor) -> Optional[Tuple[Optional[torc
     return None
 
 
+class PrefixIndex:
+    """The prefix index of a paged cache: full pages of 64 rows kept after the sequences that wrote them, so that a later
+    prompt starting with the same tokens maps them instead of computing their rows again.
+
+    A full page is immutable once written, so rows with the same key hold the same K/V for the same weights and cache
+    format, whatever the call.  A page's key is its parent page (-1 for the first) and the (token id, mask) of its 64
+    rows.  The index holds one reference per page: the cache that owns the pool counts it, and takes it back for the
+    pages :meth:`evict` and :meth:`clear` return.  Eviction takes the least-recently-used leaf (a page no cached page
+    continues), so a cached chain is always a prefix of what was inserted."""
+
+    def __init__(self):
+        self.pages = {}      # (parent page or -1, ((token, mask), ... 64)) -> page
+        self.keys = {}       # cached page -> its key
+        self.children = {}   # cached page -> the number of cached pages that continue it
+        self.used = {}       # cached page -> the tick it was last looked up or inserted at
+        self.tick = 0
+
+    def __len__(self) -> int:
+        return len(self.keys)
+
+    def __contains__(self, page: int) -> bool:
+        return page in self.keys
+
+    @staticmethod
+    def page_keys(ids: List[int], mask: List[int], pages: int):
+        P = OF.PAGE_ROWS
+        return [tuple(zip(ids[j * P : (j + 1) * P], mask[j * P : (j + 1) * P])) for j in range(pages)]
+
+    def chain(self, keys) -> List[int]:
+        """The cached pages of the longest run of ``keys`` (from the first page on) the index holds."""
+        parent, chain = -1, []
+        for key in keys:
+            page = self.pages.get((parent, key))
+            if page is None:
+                break
+            chain.append(page)
+            parent = page
+        return chain
+
+    def touch(self, pages: Iterable[int]) -> None:
+        """Mark ``pages`` used now (one tick for all of them)."""
+        self.tick += 1
+        for page in pages:
+            self.used[page] = self.tick
+
+    def insert(self, rows) -> List[int]:
+        """Index the pages of ``rows``, pairs ``(keys, table_row)``: page ``j`` of a row, under ``keys[j]``, is
+        ``table_row[j]`` unless the index holds that key already.  One tick for all rows.  Returns the pages added,
+        each of which the index now holds a reference to."""
+        self.tick += 1
+        added = []
+        for keys, table_row in rows:
+            parent = -1
+            for j, key in enumerate(keys):
+                page = self.pages.get((parent, key))
+                if page is None:
+                    page = table_row[j]
+                    if page in self.keys:   # cached under another key: cannot happen for an immutable page
+                        break
+                    self.pages[(parent, key)], self.keys[page] = page, (parent, key)
+                    self.children[page] = 0
+                    if parent >= 0:
+                        self.children[parent] += 1
+                    added.append(page)
+                self.used[page] = self.tick
+                parent = page
+        return added
+
+    def pop_leaf(self, evictable=None) -> Optional[int]:
+        """Drop the least-recently-used leaf (among those ``evictable(page)`` accepts) and return it, or None."""
+        leaves = [p for p, n in self.children.items() if n == 0 and (evictable is None or evictable(p))]
+        if not leaves:
+            return None
+        leaf = min(leaves, key=lambda p: self.used[p])
+        parent, key = self.keys.pop(leaf)
+        del self.pages[(parent, key)]
+        del self.children[leaf]
+        if parent >= 0:
+            self.children[parent] -= 1
+        return leaf
+
+    def evict(self, budget: int) -> List[int]:
+        """Drop least-recently-used leaves down to ``budget`` pages; returns them."""
+        out = []
+        while len(self.keys) > budget:
+            out.append(self.pop_leaf())
+        return out
+
+    def clear(self) -> List[int]:
+        """Drop every page; returns them."""
+        out = list(self.keys)
+        self.pages, self.keys, self.children = {}, {}, {}
+        return out
+
+
 class KVCacheLayer:
     """The cache of one layer, handed to its attention module in place of the ``(key, value)`` tuple."""
 
@@ -416,11 +511,7 @@ class PagedKVCache(StaticKVCache):
         # the prefix index's budget: extra pages, so the start of a call never evicts
         self.prefix_pages = -(-max(int(prefix_tokens), 0) // P)
         self.num_pages = batch * shared + self.rows * (self.max_pages - shared) + self.prefix_pages
-        self._used = {}       # cached page -> the tick it was last looked up or inserted at
-        self._index = {}      # (parent page or -1, ((token, mask), ... 64)) -> page
-        self._entry = {}      # cached page -> its key
-        self._children = {}   # cached page -> the cached pages that continue it
-        self._tick = 0
+        self._prefix = PrefixIndex()
         self.reused_rows = 0  # the rows the last prefill took from the index
         self.prefix_ok = False   # the call's prompt may be looked up and inserted
         self.index_owner = None  # what the index is valid for (the weights), set by KVCacheOwner
@@ -578,22 +669,25 @@ class PagedKVCache(StaticKVCache):
         self.mapped = 0   # the page slots mapped in every sequence's row
         self._write_table()
 
-    # ---- prefix index -------------------------------------------------------------------------------------------
-    # A full page is immutable once written (only a sequence's last, partly filled page is ever written, and a shared
-    # one is copied first), so a later call can map it into its table instead of computing its rows again.  A page's
-    # key is its parent page (-1 for the first) and the (token id, mask) of its 64 rows: rows with the same key hold
-    # the same K/V for the same weights and cache format, whatever the call.  The index holds one reference per page.
+    # ---- prefix index (PrefixIndex) -------------------------------------------------------------------------------
+    # Only a sequence's last, partly filled page is ever written, and a shared one is copied first, so a full page is
+    # immutable and a later call can map it.
+
+    _page_keys = staticmethod(PrefixIndex.page_keys)
+
+    @property
+    def _index(self) -> dict:
+        return self._prefix.pages
+
+    @property
+    def _entry(self) -> dict:
+        return self._prefix.keys
 
     def _index_refs(self) -> List[int]:
         refs = [0] * self.num_pages
-        for page in getattr(self, "_entry", {}):
+        for page in self._entry:
             refs[page] = 1
         return refs
-
-    @staticmethod
-    def _page_keys(ids: List[int], mask: List[int], pages: int):
-        P = OF.PAGE_ROWS
-        return [tuple(zip(ids[j * P : (j + 1) * P], mask[j * P : (j + 1) * P])) for j in range(pages)]
 
     @staticmethod
     def _rows(input_ids: torch.Tensor, attention_mask: Optional[torch.Tensor]):
@@ -619,10 +713,8 @@ class PagedKVCache(StaticKVCache):
 
     def clear_prefix_index(self) -> None:
         """Drop every cached page (a page a sequence still maps keeps that sequence's reference)."""
-        for page in list(self._entry):
-            del self._index[self._entry.pop(page)]
+        for page in self._prefix.clear():
             self._release(page)
-        self._children = {}
 
     def lookup(self, input_ids: torch.Tensor, attention_mask: Optional[torch.Tensor]) -> int:
         """Before the prefill of the ``batch`` prompts ``input_ids`` ``[batch, s]`` on the empty cache: map the longest
@@ -641,25 +733,16 @@ class PagedKVCache(StaticKVCache):
             return 0
         s = input_ids.shape[1]
         ids, mask = self._rows(input_ids, attention_mask)
-        chains = []
-        for b in range(self.batch):
-            parent, chain = -1, []
-            for key in self._page_keys(ids[b], mask[b], (s - 1) // OF.PAGE_ROWS):
-                page = self._index.get((parent, key))
-                if page is None:
-                    break
-                chain.append(page)
-                parent = page
-            chains.append(chain)
+        chains = [self._prefix.chain(self._page_keys(ids[b], mask[b], (s - 1) // OF.PAGE_ROWS))
+                  for b in range(self.batch)]
         hit = min(len(c) for c in chains)
         if hit == 0:
             return 0
-        self._tick += 1
+        self._prefix.touch(page for chain in chains for page in chain[:hit])
         for b, chain in enumerate(chains):
             for j, page in enumerate(chain[:hit]):
                 self.host_table[b][j] = page
                 self.refs[page] += 1
-                self._used[page] = self._tick
         rows = hit * OF.PAGE_ROWS
         self.mapped, self.length, self.reused_rows = hit, rows, rows
         self.seqlens.fill_(rows)
@@ -676,30 +759,257 @@ class PagedKVCache(StaticKVCache):
             return
         L = min(input_ids.shape[1], self.length)
         ids, mask = self._rows(input_ids[:, :L], None if attention_mask is None else attention_mask[:, :L])
-        self._tick += 1
-        for b in range(self.batch):
-            parent = -1
-            for j, key in enumerate(self._page_keys(ids[b], mask[b], L // OF.PAGE_ROWS)):
-                page = self._index.get((parent, key))
+        for page in self._prefix.insert((self._page_keys(ids[b], mask[b], L // OF.PAGE_ROWS), self.host_table[b])
+                                        for b in range(self.batch)):
+            self.refs[page] += 1
+        for page in self._prefix.evict(self.prefix_pages):
+            self._release(page)
+
+
+class RaggedPagedKVCacheLayer(KVCacheLayer):
+    """A layer of a :class:`RaggedPagedKVCache`: the ragged append, then the decode rows through the split-KV decode
+    kernel and the prompt chunks through the ragged paged flash prefill."""
+
+    __slots__ = ()
+
+    def append(self, qkv: torch.Tensor, cos=None, sin=None) -> torch.Tensor:
+        c = self.cache
+        return OF.kv_cache_append_paged_varlen(qkv, self.k, self.v, c.table, c.cu_q, c.past, cos, sin)
+
+    def attend(self, q: torch.Tensor, *, scale: float, causal: bool = True, mask=None, bias=None, alibi_slopes=None,
+               rel_bias=None, dropout_p: float = 0.0, training: bool = False, prefix_lens=None) -> torch.Tensor:
+        """The attention of the step's ``q`` ``[1, T, a, d]``, each token over its own sequence's rows → ``[1, T, a, d]``.
+        Causal self-attention only (with or without ALiBi)."""
+        if (not causal or mask is not None or bias is not None or rel_bias is not None or prefix_lens is not None
+                or (training and dropout_p > 0)):
+            raise ValueError("RaggedPagedKVCache: causal self-attention without mask, bias, rel_bias, prefix or "
+                             "dropout only")
+        c = self.cache
+        if not OF.attention_paged_supported(q, self.k):   # the reference math, every sequence alike
+            return OF.attention_paged_varlen(q[0], self.k, self.v, c.table, c.cu_q, c.past, scale=scale,
+                                             alibi_slopes=alibi_slopes)[None]
+        mb = c.max_batch
+        out = OF.decode_attention(q[0, :mb, None], self.k, self.v, c.past[:mb], c.kv_start, scale=scale,
+                                  alibi_slopes=alibi_slopes, block_table=c.table[:mb])
+        out = out.view(1, mb, *q.shape[2:])
+        if c.chunks == 0:
+            return out
+        pre = OF.attention_paged_varlen(q[0, mb:], self.k, self.v, c.table[mb:], c.cu_c, c.past[mb:], c.tiles,
+                                        scale=scale, alibi_slopes=alibi_slopes)
+        return torch.cat((out, pre[None]), dim=1)
+
+
+class RaggedPagedKVCache(StaticKVCache):
+    """The KV cache of continuous batching (:class:`~libai_b200.inference.engine.GenerationEngine`): up to
+    ``max_batch`` sequences (slots) of their own lengths, whose tokens of one step are packed into one forward over
+    ``[1, T]``.  A model's cached step runs on it unchanged: ``layer(i).append`` / ``attend`` and ``advance`` are those
+    of a :class:`StaticKVCache` of batch 1.
+
+    - Each owned layer has a K and a V pool ``[num_pages + 1, heads, 64, head_dim]`` in the format of a
+      :class:`PagedKVCache`; the last page is the **sink**, which idle decode rows write and read (their outputs are
+      discarded).  Every other page is the scheduler's: :meth:`alloc` and :meth:`release` keep a reference count per
+      page and a free list, and the prefix index (:class:`PrefixIndex`) holds one reference per cached page.
+    - A step's tokens are the ``max_batch`` decode rows, one per slot in slot order, then the prompt chunks.  Its
+      descriptor (:meth:`write_step`), written to the device in one copy, holds the token ids, ``cu_q`` (the
+      sequences' token offsets: the decode rows are sequences of one token), ``past`` (the rows each holds), one
+      block-table row per sequence (a decode row of a slot that is not decoding maps the sink, with ``past`` 0), the
+      chunks' own offsets ``cu_c`` and the prefill's tile list.  The buffers have fixed addresses, so a decode graph
+      replays a step of decode rows after its descriptor is rewritten.
+    - ``length`` counts the tokens of the current step once :meth:`advance` ran (what a decode graph checks); the
+      per-sequence lengths are the scheduler's, written into each step's descriptor.  :meth:`reserve` does nothing:
+      the pages are mapped at admission.
+    """
+
+    def __init__(self, num_layers: int, max_batch: int, heads: int, head_dim: int, num_pages: int, max_pages: int,
+                 max_tokens: int, dtype=torch.bfloat16, device=None, layers: Optional[Iterable[int]] = None):
+        self.num_layers, self.heads, self.head_dim = num_layers, heads, head_dim
+        self.dtype, self.kv_dtype = dtype, dtype
+        self.device = torch.device(device) if device is not None else torch.device("cpu")
+        self.fp8 = False
+        self.owned = sorted(range(num_layers) if layers is None else layers)
+        self.max_batch, self.max_pages, self.max_tokens = max_batch, max_pages, max_tokens
+        self.num_pages, self.sink = num_pages, num_pages
+        self.batch, self.capacity, self.length, self.dense_mask = 1, max_pages * OF.PAGE_ROWS, 0, False
+        P = OF.PAGE_ROWS
+        self.k: List[Optional[torch.Tensor]] = [None] * num_layers
+        self.v: List[Optional[torch.Tensor]] = [None] * num_layers
+        self.k_scale: List[Optional[torch.Tensor]] = [None] * num_layers
+        self.v_scale: List[Optional[torch.Tensor]] = [None] * num_layers
+        for i in self.owned:
+            # uninitialised: the kernels read the rows of each sequence's window only
+            self.k[i], self.v[i] = (torch.empty(num_pages + 1, heads, P, head_dim, dtype=dtype, device=self.device)
+                                    for _ in range(2))
+        self.refs = [0] * num_pages
+        self.free = list(range(num_pages - 1, -1, -1))   # pages are taken from the end: 0, 1, 2, ...
+        self.prefix = PrefixIndex()
+        self.index_owner = None
+        # the descriptor: offsets (int32 elements) of its parts in one buffer
+        nseq, self.max_tiles = 2 * max_batch, max_tokens // 128 + max_batch
+        sizes = (("ids", max_tokens), ("cu_q", nseq + 1), ("past", nseq), ("table", nseq * max_pages),
+                 ("cu_c", max_batch + 1), ("tiles", 2 * self.max_tiles), ("rows", 2 * max_batch))
+        self._off, n = {}, 0
+        for name, size in sizes:
+            n += n % 2   # the tiles are read as int2
+            self._off[name] = (n, size)
+            n += size
+        pin = self.device.type == "cuda"
+        self._host = torch.zeros(n, dtype=torch.int32, pin_memory=pin)
+        self._desc = torch.zeros(n, dtype=torch.int32, device=self.device)
+        # the host buffer is rewritten only once the previous step's copy out of it has run: a step that samples no
+        # token (prompt chunks that end no prompt) has no host sync of its own
+        self._copied = torch.cuda.Event() if pin else None
+        self.kv_start = torch.zeros(max_batch, dtype=torch.int32, device=self.device)
+        self.seqlens = self._part(self._desc, "past")[:max_batch]
+        self._views(max_batch, 0, 0, 0)
+
+    def _part(self, buf: torch.Tensor, name: str) -> torch.Tensor:
+        o, n = self._off[name]
+        return buf[o : o + n]
+
+    def _views(self, T: int, nseq: int, chunks: int, tiles: int) -> None:
+        d = self._desc
+        self.T, self.chunks = T, chunks
+        nseq = max(nseq, self.max_batch)
+        self.ids = self._part(d, "ids")[:T]
+        self.cu_q = self._part(d, "cu_q")[: nseq + 1]
+        self.past = self._part(d, "past")[:nseq]
+        self.table = self._part(d, "table")[: nseq * self.max_pages].view(nseq, self.max_pages)
+        self.cu_c = self._part(d, "cu_c")[: chunks + 1]
+        self.tiles = self._part(d, "tiles")[: 2 * tiles].view(tiles, 2)
+
+    def layer(self, i: int) -> KVCacheLayer:
+        return RaggedPagedKVCacheLayer(self, i)
+
+    def write_step(self, decode, chunks, rows=()) -> Tuple[torch.Tensor, torch.Tensor]:
+        """Write the descriptor of a step to the device (one copy) and return its token ids ``[1, T]`` (int64) and
+        ``rows`` (the token rows whose logits are sampled; int32), both on the device.  ``decode``: per slot ``None``
+        (not decoding) or ``(token, past, pages)``; ``chunks``: the prompt chunks ``(tokens, past, pages)``.  ``pages``
+        lists a sequence's table row (its pages in order)."""
+        mb, mp = self.max_batch, self.max_pages
+        if self._copied is not None:
+            self._copied.synchronize()
+        h = self._host.numpy()   # the pinned buffer, written in place
+        ids, cu, past, cu_c, tiles, sample = (self._part(h, n) for n in ("ids", "cu_q", "past", "cu_c", "tiles",
+                                                                          "rows"))
+        table = self._part(h, "table").reshape(-1, mp)
+        lens = [len(c[0]) for c in chunks]
+        nseq, T = mb + len(chunks), mb + sum(lens)
+        if len(decode) != mb or len(chunks) > mb or T > self.max_tokens:
+            raise ValueError(f"a step holds {mb} decode rows, at most {mb} chunks and {self.max_tokens} tokens")
+        table[:nseq] = -1
+        for n, d in enumerate(decode):
+            if d is None:
+                ids[n], past[n], table[n, 0] = 0, 0, self.sink
+            else:
+                ids[n], past[n] = d[0], d[1]
+                table[n, : len(d[2])] = d[2]
+        t = mb
+        for k, (tok, pst, pages) in enumerate(chunks):
+            ids[t : t + len(tok)] = tok
+            past[mb + k] = pst
+            table[mb + k, : len(pages)] = pages
+            t += len(tok)
+        cu[: mb + 1] = range(mb + 1)
+        cu_c[0] = 0
+        cu_c[1 : len(chunks) + 1] = _cumsum(lens)
+        cu[mb + 1 : nseq + 1] = [mb + x for x in _cumsum(lens)]
+        tl = OF.varlen_tiles(lens, [c[1] for c in chunks]).numpy()
+        tiles[: tl.size] = tl.reshape(-1)
+        sample[: len(rows)] = rows
+        self._desc.copy_(self._host, non_blocking=True)
+        if self._copied is not None:
+            self._copied.record()
+        self._views(T, nseq, len(chunks), tl.shape[0])
+        self.length = 0
+        return self.ids.long()[None], self._part(self._desc, "rows")[: len(rows)]
+
+    # ---- pages ----------------------------------------------------------------------------------------------------
+    def index_only(self, exclude=()) -> int:
+        """The pages only the prefix index holds (free on demand), not counting ``exclude``."""
+        return sum(1 for p in self.prefix.keys if self.refs[p] == 1 and p not in exclude)
+
+    def available(self, exclude=()) -> int:
+        return len(self.free) + self.index_only(exclude)
+
+    def alloc(self, n: int) -> List[int]:
+        """``n`` pages of the free list, evicting least-recently-used index-only pages as needed."""
+        out = []
+        for _ in range(n):
+            if not self.free:
+                page = self.prefix.pop_leaf(lambda p: self.refs[p] == 1)
                 if page is None:
-                    page = self.host_table[b][j]
-                    if page in self._entry:   # cached under another key: cannot happen for an immutable page
-                        break
-                    self._index[(parent, key)], self._entry[page] = page, (parent, key)
-                    self._children[page] = 0
-                    if parent >= 0:
-                        self._children[parent] += 1
-                    self.refs[page] += 1
-                self._used[page] = self._tick
-                parent = page
-        while len(self._entry) > self.prefix_pages:
-            leaf = min((p for p, n in self._children.items() if n == 0), key=lambda p: self._used[p])
-            parent, _ = self._entry.pop(leaf)
-            del self._index[(parent, _)]
-            del self._children[leaf]
-            if parent >= 0:
-                self._children[parent] -= 1
-            self._release(leaf)
+                    raise RuntimeError("RaggedPagedKVCache: out of pages")
+                self.release([page])
+            page = self.free.pop()
+            self.refs[page] = 1
+            out.append(page)
+        return out
+
+    def retain(self, pages: Iterable[int]) -> None:
+        for p in pages:
+            self.refs[p] += 1
+
+    def release(self, pages: Iterable[int]) -> None:
+        for p in pages:
+            self.refs[p] -= 1
+            if self.refs[p] == 0:
+                self.free.append(p)
+
+    def lookup(self, tokens: List[int]) -> List[int]:
+        """The cached pages a prompt of ``tokens`` starts with, at most ``(len - 1) // 64``, mapped by reference (and
+        marked used)."""
+        keys = PrefixIndex.page_keys(tokens, [1] * len(tokens), (len(tokens) - 1) // OF.PAGE_ROWS)
+        chain = self.prefix.chain(keys)
+        if chain:
+            self.prefix.touch(chain)
+            self.retain(chain)
+        return chain
+
+    def peek(self, tokens: List[int]) -> List[int]:
+        """:meth:`lookup` without taking the pages."""
+        keys = PrefixIndex.page_keys(tokens, [1] * len(tokens), (len(tokens) - 1) // OF.PAGE_ROWS)
+        return self.prefix.chain(keys)
+
+    def insert(self, tokens: List[int], pages: List[int]) -> None:
+        """Index the full pages of a sequence's fed ``tokens`` (its rows), held in ``pages``."""
+        full = len(tokens) // OF.PAGE_ROWS
+        self.retain(self.prefix.insert([(PrefixIndex.page_keys(tokens, [1] * len(tokens), full), pages)]))
+
+    def clear_prefix_index(self) -> None:
+        self.release(self.prefix.clear())
+
+    # ---- the StaticKVCache protocol of a model's cached step --------------------------------------------------------
+    def flash_attention(self) -> bool:
+        return OF.attention_paged_supported(torch.empty(1, dtype=self.dtype, device=self.device), self.k[self.owned[0]])
+
+    def advance(self, n: int) -> None:
+        self.length += n
+
+    def reserve(self, n: int) -> None:
+        return None
+
+    def reset(self) -> None:
+        self.length = 0
+
+    def write_rows(self, i, k, v, row0=0):
+        raise NotImplementedError("RaggedPagedKVCache: rows are written by the ragged append")
+
+    def fill(self, kv, S: int, window=None) -> None:
+        raise NotImplementedError("RaggedPagedKVCache holds self-attention rows only")
+
+    def rollback(self, n: int) -> None:
+        raise NotImplementedError("RaggedPagedKVCache: no rollback")
+
+    def reorder_(self, beam_idx) -> None:
+        raise NotImplementedError("RaggedPagedKVCache: no reorder")
+
+
+def _cumsum(xs) -> List[int]:
+    out, t = [], 0
+    for x in xs:
+        t += x
+        out.append(t)
+    return out
 
 
 class KVCacheOwner:

@@ -343,6 +343,7 @@ class SFTLoss(nn.Module):
 
 class LlamaForCausalLM(nn.Module, PipelineStageMixin, KVCacheOwner, Generator):
     speculative_decoding = True
+    continuous_batching = True
 
     # `train.dist.sequence_parallel = "auto"` resolves to True for this model (token-sharded activations between
     # the tensor-parallel blocks are handled by its embeddings / heads)
@@ -447,6 +448,15 @@ class LlamaForCausalLM(nn.Module, PipelineStageMixin, KVCacheOwner, Generator):
     # ---- KV cache (KVCacheOwner) ----------------------------------------------------------------
     def _cache_attention_modules(self):
         return [layer.self_attn for layer in self.model.layers]
+
+    def continuous_batching_logits(self, input_ids, cache):
+        """The logits ``[1, T, vocab]`` of one step of a ``GenerationEngine``: ``input_ids`` ``[1, T]`` on its
+        ``RaggedPagedKVCache``, whose append rotates each token at its own sequence's position."""
+        return self.lm_head(self.model(input_ids, past_key_values=cache))
+
+    def continuous_batching_max_length(self):
+        """The positions of the rotary tables: the longest sequence a ``GenerationEngine`` runs."""
+        return self.model.cos_cached.shape[0]
 
     @staticmethod
     def set_pipeline_stage_id(model):

@@ -1423,6 +1423,87 @@ def attention_paged(q, k_pool, v_pool, block_table, past: int, kv_start=None, *,
     return o
 
 
+def varlen_tiles(q_lens, past=None) -> torch.Tensor:
+    """The tile list of :func:`attention_paged_varlen` for sequences of ``q_lens`` new tokens after ``past`` rows each
+    (default 0): int32 ``[n, 2]`` on the host, ``(sequence, 128-query block)`` for every block of every sequence, the
+    blocks that see the most keys (``past`` plus the block's last query) first."""
+    past = [0] * len(q_lens) if past is None else [int(p) for p in past]
+    tiles = [(n, blk) for n, s in enumerate(q_lens) for blk in range(-(-int(s) // 128))]
+    tiles.sort(key=lambda t: -(past[t[0]] + min(128 * (t[1] + 1), int(q_lens[t[0]]))))
+    return torch.tensor(tiles, dtype=torch.int32).reshape(-1, 2)
+
+
+def attention_paged_varlen(q, k_pool, v_pool, block_table, cu_q, past, tiles=None, *, scale: float,
+                           alibi_slopes=None):
+    """Causal attention of ``N`` ragged sequences packed in ``q [T, a, d]`` over their rows of a paged cache's pools
+    ``[P, g, 64, d]``: sequence ``n`` owns rows ``cu_q[n] .. cu_q[n + 1]`` of q (int32 ``[N + 1]``, from 0 to T) and
+    holds ``past[n]`` rows (int32 ``[N]``) before them in row ``n`` of ``block_table`` ``[N, max_pages]``; its query
+    ``i`` sees its logical rows ``[0, past[n] + i]``.  ``alibi_slopes`` as in :func:`attention`.  Returns ``[T, a, d]``.
+
+    On the GPU (bf16, head dim 64 or 128) one launch of the ragged paged flash kernel, one CTA per (128-query tile of
+    a sequence, query head) of ``tiles`` (int32 ``[n, 2]`` on q's device, :func:`varlen_tiles`; built here, with a host
+    sync, when None); each sequence's rows are bit for bit those of :func:`attention_paged` on that sequence alone.
+    Rows of a page past a sequence's window never reach P·V, whatever they hold.  Elsewhere the reference math per
+    sequence (:func:`attention_paged_varlen_ref`)."""
+    if attention_paged_supported(q, k_pool):
+        if tiles is None:
+            tiles = varlen_tiles(cu_q.diff().tolist(), past.tolist()).to(q.device)
+        o = load_ext().attn_fwd_paged_varlen(q, k_pool, v_pool, block_table, cu_q, past, tiles, float(scale),
+                                             alibi_slopes)
+        count_launch()
+        return o
+    return attention_paged_varlen_ref(q, k_pool, v_pool, block_table, cu_q, past, scale=scale,
+                                      alibi_slopes=alibi_slopes)
+
+
+def attention_paged_varlen_ref(q, k_pool, v_pool, block_table, cu_q, past, *, scale: float, alibi_slopes=None):
+    """:func:`attention_paged_varlen` by the reference math: per sequence, its rows ``[:past[n] + s_n]`` gathered
+    through its table row, then :func:`attention_ref` (causal, bottom-right aligned, with the ALiBi bias
+    ``slope_h·(j − past[n] − i)``)."""
+    cu, pa = [int(x) for x in cu_q.tolist()], [int(x) for x in past.tolist()]
+    o = torch.zeros_like(q)
+    for n in range(len(pa)):
+        s = cu[n + 1] - cu[n]
+        if s == 0:
+            continue
+        L = pa[n] + s
+        k = kv_pages_gather(k_pool, block_table[n : n + 1], L)
+        v = kv_pages_gather(v_pool, block_table[n : n + 1], L)
+        qn = q[cu[n] : cu[n + 1]].transpose(0, 1)[None]   # [1, a, s, d]
+        bias = None
+        if alibi_slopes is not None:
+            dist = torch.arange(L, device=q.device)[None, :] - torch.arange(pa[n], L, device=q.device)[:, None]
+            bias = (alibi_slopes.float().to(q.device)[:, None, None] * dist[None].float())[None]
+        o[cu[n] : cu[n + 1]] = attention_ref(qn, k.to(q.dtype), v.to(q.dtype), causal=True, scale=scale,
+                                             bias=bias)[0].transpose(0, 1)
+    return o
+
+
+def kv_cache_append_paged_varlen(qkv, k_pool, v_pool, block_table, cu_q, past, cos=None, sin=None):
+    """Write k, v of the packed projection ``qkv`` (``[1, T, a, 3d]`` or ``[1, T, g, r + 2, d]``) of ``N`` ragged
+    sequences into a paged cache's pools ``[P, g, 64, d]``: token ``t`` of sequence ``n`` (``cu_q[n] <= t < cu_q[n +
+    1]``, int32 ``[N + 1]`` from 0 to T) at its logical row ``past[n] + t − cu_q[n]`` of row ``n`` of ``block_table``
+    ``[N, max_pages]``, q and k rotated at that position by ``cos/sin`` when given.  Returns q ``[1, T, a, d]``.  On
+    the GPU one launch of the ragged bf16 append, whose bytes are :func:`kv_cache_append`'s per sequence; elsewhere
+    :func:`kv_cache_append_ref` per sequence."""
+    if attention_paged_supported(qkv, k_pool) and (cos is None or cos.dtype == torch.float32):
+        qkv = qkv if qkv.is_contiguous() else qkv.contiguous()
+        q = load_ext().kv_append_paged_varlen(qkv, k_pool, v_pool, block_table, cu_q, past, cos, sin, True)
+        count_launch()
+        return q
+    return kv_cache_append_paged_varlen_ref(qkv, k_pool, v_pool, block_table, cu_q, past, cos, sin)
+
+
+def kv_cache_append_paged_varlen_ref(qkv, k_pool, v_pool, block_table, cu_q, past, cos=None, sin=None):
+    cu, pa = [int(x) for x in cu_q.tolist()], past.to(torch.int32)
+    qs = []
+    for n in range(len(cu) - 1):
+        if cu[n + 1] > cu[n]:
+            qs.append(kv_cache_append_ref(qkv[:, cu[n] : cu[n + 1]], k_pool, v_pool, pa[n : n + 1], cos, sin,
+                                          block_table=block_table[n : n + 1]))
+    return torch.cat(qs, dim=1)
+
+
 def decode_attention_paged_ref(q, k_pool, v_pool, block_table, cache_seqlens, kv_start, *, scale: float, splits=0,
                                past: Optional[int] = None, alibi_slopes=None, k_scale=None, v_scale=None):
     """:func:`decode_attention` over a paged cache by its logical rows: the rows ``[:L]`` gathered through the table

@@ -195,6 +195,7 @@ class BloomModel(nn.Module):
 
 class BloomForCausalLM(nn.Module, KVCacheOwner, Generator):
     speculative_decoding = True
+    continuous_batching = True
 
     @configurable
     def __init__(self, cfg=None, **kwargs):
@@ -224,3 +225,11 @@ class BloomForCausalLM(nn.Module, KVCacheOwner, Generator):
     # ---- KV cache (KVCacheOwner) ----------------------------------------------------------------
     def _cache_attention_modules(self):
         return [block.self_attention for block in self.transformer.h]
+
+    def continuous_batching_logits(self, input_ids, cache):
+        """The logits ``[1, T, vocab]`` of one step of a ``GenerationEngine`` on its ``RaggedPagedKVCache``: ALiBi
+        scores each key by its distance inside its own sequence."""
+        return self.lm_head(self.transformer(input_ids, None, cache), self.transformer.word_embeddings.weight)
+
+    def continuous_batching_max_length(self):
+        return None   # ALiBi: no position table

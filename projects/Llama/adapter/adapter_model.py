@@ -57,6 +57,9 @@ class AdapterAttention(LlamaAttention):
 
 
 class LlamaForCausalLM(_BaseLlama):
+    # the adapter's query rotary takes its positions from a StaticKVCache's per-sample seqlens
+    continuous_batching = False
+
     @configurable
     def __init__(self, *args, adapter_len=10, adapter_layer=30, cfg=None, **kwargs):
         super().__init__(*args, **kwargs)  # (without `cfg`: the base initialiser would re-enter from_config)
