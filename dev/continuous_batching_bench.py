@@ -16,6 +16,13 @@ start of the run), peak memory, and the kernel launches of a decode-only engine 
 prefill against one ``attention_paged`` launch per sequence on a ragged batch (8 sequences, q_len in [1, 512], past in
 [0, 4096]), outputs checked bit for bit.  One JSON document goes to stdout (and ``--out``); the card's name and power
 limit are read in the same launch.
+
+``--kv-cache-dtype fp8`` runs the mixed workload on the engine only, eagerly, in three arms: the bf16 engine as above
+(``max_batch`` 32, 1,300 pages), FP8 pools of the same bytes (``max_batch`` 64, 2,521 pages: a page of K and V over 32
+layers is 33.55 MB in bf16 and 17.30 MB in E4M3 with its fp32 row scales), and FP8 at ``max_batch`` 32 with 1,300
+pages, which isolates the decode kernels from admission.  Its kernel-level pair is the FP8 ragged prefill against the
+bf16 ragged prefill on the same batch, the FP8 output checked bit for bit against the bf16 kernel over the dequantized
+pools.
 """
 import argparse
 import json
@@ -92,12 +99,13 @@ def _static(model, work, max_batch, graphs):
     return total, lat, ttft
 
 
-def _engine(model, work, max_batch, graphs, prefix=False):
+def _engine(model, work, max_batch, graphs, prefix=False, num_pages=1300, kv_cache_dtype=None):
     model.kv_cache = model._decode_graph = None   # the static arm's cache and graph
     torch.cuda.empty_cache()
-    # 1,300 pages of 64 rows: 41.6 GB of K/V at this shape, beside the 13.5 GB of weights
-    e = GenerationEngine(model, max_batch=max_batch, max_tokens_per_step=2048, num_pages=1300,
-                         prefix_caching=prefix, decode_graphs=graphs)
+    # by default 1,300 pages of 64 rows: 41.6 GB of bf16 K/V at this shape (22.5 GB in FP8), beside the 13.5 GB of
+    # weights; 2,521 FP8 pages take the bytes of 1,300 bf16 ones
+    e = GenerationEngine(model, max_batch=max_batch, max_tokens_per_step=2048, num_pages=num_pages,
+                         prefix_caching=prefix, decode_graphs=graphs, kv_cache_dtype=kv_cache_dtype)
     t0 = time.perf_counter()
     ids = [e.add_request(p, m) for p, m in work]
     for r in e.requests.values():
@@ -127,7 +135,7 @@ def _arm(name, fn, useful):
     return res
 
 
-def _kernel(reps=20):
+def _kernel(reps=20, fp8=False):
     rng = random.Random(0)
     q_lens = [rng.randint(1, 512) for _ in range(8)]
     past = [rng.randint(0, 4096) for _ in range(8)]
@@ -150,14 +158,26 @@ def _kernel(reps=20):
     def ragged():
         return OF.attention_paged_varlen(q, k, v, table, cu, pa, tiles, scale=D ** -0.5)
 
-    def per_seq():
-        return [OF.attention_paged(q[None, c[n] : c[n + 1]], k, v, table[n : n + 1], past[n], scale=D ** -0.5)
-                for n in range(8)]
+    if fp8:
+        (k8, ks), (v8, vs) = OF.kv_cache_quantize_ref(k), OF.kv_cache_quantize_ref(v)
+        kd, vd = OF.kv_cache_dequant(k8, ks), OF.kv_cache_dequant(v8, vs)
 
-    o, refs = ragged(), per_seq()
-    equal = all(torch.equal(o[c[n] : c[n + 1]], refs[n][0]) for n in range(8))
+        def ragged_fp8():
+            return OF.attention_paged_varlen(q, k8, v8, table, cu, pa, tiles, scale=D ** -0.5, k_scale=ks,
+                                             v_scale=vs)
+
+        equal = torch.equal(ragged_fp8(), OF.attention_paged_varlen(q, kd, vd, table, cu, pa, tiles, scale=D ** -0.5))
+        pair = (("fp8", ragged_fp8), ("bf16", ragged))
+    else:
+        def per_seq():
+            return [OF.attention_paged(q[None, c[n] : c[n + 1]], k, v, table[n : n + 1], past[n], scale=D ** -0.5)
+                    for n in range(8)]
+
+        o, refs = ragged(), per_seq()
+        equal = all(torch.equal(o[c[n] : c[n + 1]], refs[n][0]) for n in range(8))
+        pair = (("ragged", ragged), ("per_sequence", per_seq))
     times = {}
-    for name, fn in (("ragged", ragged), ("per_sequence", per_seq)) * 2:
+    for name, fn in pair * 2:
         fn()
         s, e = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         s.record()
@@ -166,8 +186,8 @@ def _kernel(reps=20):
         e.record()
         torch.cuda.synchronize()
         times[name] = s.elapsed_time(e) / reps
-    res = {"kernel": "ragged_prefill", "q_lens": q_lens, "past": past, "bit_equal": equal,
-           "ragged_ms": times["ragged"], "per_sequence_ms": times["per_sequence"]}
+    res = {"kernel": "ragged_prefill_fp8" if fp8 else "ragged_prefill", "q_lens": q_lens, "past": past,
+           "bit_equal": equal, **{f"{name}_ms": t for name, t in times.items()}}
     print(json.dumps(res), flush=True)
     return res
 
@@ -180,6 +200,7 @@ def main():
     ap.add_argument("--out", default=None)
     # the two workloads take minutes each at the default size: one launch can run either
     ap.add_argument("--workload", choices=("mixed", "shared", "both"), default="both")
+    ap.add_argument("--kv-cache-dtype", choices=("bf16", "fp8"), default="bf16")
     args = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("continuous_batching_bench needs a GPU")
@@ -187,7 +208,26 @@ def main():
                                          device_type="cuda")))
     ops.load_ext(required=True)
     doc = {"card": _card(), "requests": args.requests, "max_batch": args.max_batch, "layers": args.layers,
-           "workload": args.workload}
+           "workload": args.workload, "kv_cache_dtype": args.kv_cache_dtype}
+    if args.kv_cache_dtype == "fp8":
+        doc["workload"] = "mixed"
+        doc["kernel"] = _kernel(fp8=True)
+        model = _model(args.layers)
+        work = _workload(args.requests, 0)
+        useful = sum(m for _, m in work)
+        # (name, max_batch, num_pages, kv_cache_dtype)
+        fp8_arms = (("engine_bf16", 32, 1300, None), ("engine_fp8_same_bytes", 64, 2521, "fp8"),
+                    ("engine_fp8", 32, 1300, "fp8"))
+        for _, mb, pages, kv in fp8_arms:   # warm-up
+            _engine(model, work[:4], mb, False, num_pages=pages, kv_cache_dtype=kv)
+        doc["arms"] = [_arm(name, lambda: _engine(model, work, mb, False, num_pages=pages, kv_cache_dtype=kv), useful)
+                       for name, mb, pages, kv in fp8_arms]
+        text = json.dumps(doc, indent=1)
+        if args.out:
+            Path(args.out).parent.mkdir(parents=True, exist_ok=True)
+            Path(args.out).write_text(text)
+        print(text)
+        return
     if args.workload != "shared":
         doc["kernel"] = _kernel()
     model = _model(args.layers)

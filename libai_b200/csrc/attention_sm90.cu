@@ -39,6 +39,9 @@
 // its own rows already held and its own block-table row; one CTA per (128-query tile of a sequence, query head), the
 // tiles listed by the host (see AttnRagged).
 //
+// FP8 ragged paged K/V (RAGGED FP8 instances, attn_fwd_paged_varlen_fp8_kernel): the same over E4M3 pools with fp32 row
+// scales; the producer warpgroup dequantizes the pages into the bf16 tiles (see AttnFp8Pages).
+//
 // Forward, one CTA per (batch, query head, 128-query block), 384 threads:
 //   warpgroup 0  TMA producer (one elected thread): Q once, then K/V tiles of 128 keys (double buffered); it gives
 //                its registers to the consumers (setmaxnreg)
@@ -119,6 +122,8 @@ struct AttnFwdCfg {
   static constexpr int CHUNKS = D / 64;                    // 64-element (128B) chunks of a row
   static constexpr int TILE_BYTES = ATT_BN * D * 2;        // one Q / K / V tile
   static constexpr int SMEM_BYTES = 5 * TILE_BYTES + 1024 + 256;   // Q + 2 x (K, V)
+  // the FP8 instances' staging buffer after the barriers: K and V bytes of one key tile, and their scales
+  static constexpr int FP8_SMEM_BYTES = SMEM_BYTES + 2 * ATT_BN * D + 2 * ATT_BN * 4;
 };
 
 // Paged K/V (PAGED instances, attn_fwd_paged_kernel): the keys are the logical rows [0, Sk) of pools [P, G, 64, D],
@@ -162,6 +167,114 @@ struct AttnRagged {
   const int2* tiles;  // [n_tiles]: (sequence, query block)
 };
 
+// FP8 ragged paged K/V (RAGGED FP8 instances): pools of E4M3 bytes [P, G, 64, D] and fp32 row scales [P, G, 64].  No
+// TMA reads them: the producer warpgroup's 128 threads copy a tile's window rows of both pools (cp.async, 16 bytes each)
+// and their scales into one staging buffer, then write each element as bf16_rn(float(e) * s) into the K / V tile, laid
+// out exactly as the 128B-swizzled TMA box lays out a bf16 page, with zeros for rows at or past the window and for
+// pages whose table entry is outside the pool (what the bf16 kernel's tail map and out-of-page boxes load).  So the
+// tiles, and the output, are those of the bf16 RAGGED kernel over the dequantized pools, bit for bit.
+struct AttnFp8Pages {
+  const uint8_t* k;
+  const uint8_t* v;
+  const float* k_scale;
+  const float* v_scale;
+  int G;
+};
+// the rows of page slot `slot` (of a RAGGED sequence, whose table row pg.table is) inside the window [0, Sk), 0 when
+// there are none or the entry is outside the pool; `page` its id
+LB_DEVICE int attn_page_rows(const AttnPages& pg, int slot, int Sk, int& page) {
+  const int rows = Sk - slot * ATT_PAGE_ROWS;
+  page = 0;
+  if (rows <= 0) return 0;
+  const int id = pg.table[slot];
+  if (id < 0 || id >= pg.num_pages) return 0;
+  page = id;
+  return min(rows, ATT_PAGE_ROWS);
+}
+// shared-memory accesses by shared-space address (smem_u32): the tile pointers are computed through an integer, from
+// which the compiler cannot tell the space, and the producer has no registers for generic addressing
+LB_DEVICE void cp_async16(uint32_t dst, const void* src) {
+  asm volatile("cp.async.cg.shared.global [%0], [%1], 16;\n" ::"r"(dst), "l"(src) : "memory");
+}
+LB_DEVICE void cp_async4(uint32_t dst, const void* src) {
+  asm volatile("cp.async.ca.shared.global [%0], [%1], 4;\n" ::"r"(dst), "l"(src) : "memory");
+}
+LB_DEVICE void cp_async_commit() { asm volatile("cp.async.commit_group;\n" ::: "memory"); }
+template <int N>
+LB_DEVICE void cp_async_wait() { asm volatile("cp.async.wait_group %0;\n" ::"n"(N) : "memory"); }
+LB_DEVICE void sts128(uint32_t a, uint32_t x, uint32_t y, uint32_t z, uint32_t w) {
+  asm volatile("st.shared.v4.u32 [%0], {%1, %2, %3, %4};\n" ::"r"(a), "r"(x), "r"(y), "r"(z), "r"(w) : "memory");
+}
+LB_DEVICE void sts32(uint32_t a, uint32_t x) { asm volatile("st.shared.u32 [%0], %1;\n" ::"r"(a), "r"(x) : "memory"); }
+LB_DEVICE uint2 lds64(uint32_t a) {
+  uint2 v;
+  asm volatile("ld.shared.v2.u32 {%0, %1}, [%2];\n" : "=r"(v.x), "=r"(v.y) : "r"(a) : "memory");
+  return v;
+}
+LB_DEVICE float lds32f(uint32_t a) {
+  float v;
+  asm volatile("ld.shared.f32 %0, [%1];\n" : "=f"(v) : "r"(a) : "memory");
+  return v;
+}
+// the producer warpgroup's barrier (the consumers' is 1)
+LB_DEVICE void producer_sync() { asm volatile("bar.sync 2, 128;\n" ::: "memory"); }
+// IEEE round-to-nearest product, also under --use_fast_math (no flush of subnormal products)
+LB_DEVICE float mul_rn(float a, float b) {
+  float r;
+  asm("mul.rn.f32 %0, %1, %2;" : "=f"(r) : "f"(a), "f"(b));
+  return r;
+}
+// the two E4M3 bytes of x's low half, dequantized with scale s: bf16_rn(float(e) * s) each, low byte first
+LB_DEVICE uint32_t e4m3x2_dequant(uint32_t x, float s) {
+  const __half2_raw h = __nv_cvt_fp8x2_to_halfraw2(static_cast<__nv_fp8x2_storage_t>(x & 0xffffu), __NV_E4M3);
+  const float2 f = __half22float2(*reinterpret_cast<const __half2*>(&h));
+  return pack_bf16(mul_rn(f.x, s), mul_rn(f.y, s));
+}
+// thread t (of 128) stages its part of one pool's key tile j (page slots 2j and 2j + 1 of the sequence's table row)
+// into st [128, D] bytes and st_s [128] scales (shared addresses), as one commit group: the window rows' bytes and
+// scales by cp.async, zero bytes and a zero scale for every other row (which then dequantize to +0, the bits of TMA's
+// zero fill)
+template <int D>
+LB_DEVICE void fp8_tile_stage(uint32_t st, uint32_t st_s, const uint8_t* pool, const float* scale, const AttnPages& pg,
+                              int j, int Sk, int G, int kv_head, int t) {
+  constexpr int PIECES = D / 16;   // 16-byte pieces of a row
+  int page0, page1;
+  const int n0 = attn_page_rows(pg, 2 * j, Sk, page0), n1 = attn_page_rows(pg, 2 * j + 1, Sk, page1);
+#pragma unroll 1
+  for (int i = 0; i < ATT_BN * PIECES / 128; ++i) {
+    const int e = t + 128 * i;
+    const int row = e / PIECES, h = row / ATT_PAGE_ROWS, rr = row % ATT_PAGE_ROWS;
+    if (rr < (h ? n1 : n0))
+      cp_async16(st + e * 16, pool + ((static_cast<size_t>(h ? page1 : page0) * G + kv_head) * ATT_PAGE_ROWS + rr) * D +
+                                  (e % PIECES) * 16);
+    else
+      sts128(st + e * 16, 0u, 0u, 0u, 0u);
+  }
+  const int h = t / ATT_PAGE_ROWS, rr = t % ATT_PAGE_ROWS;   // thread t: the scale of row t
+  if (rr < (h ? n1 : n0))
+    cp_async4(st_s + 4 * t, scale + (static_cast<size_t>(h ? page1 : page0) * G + kv_head) * ATT_PAGE_ROWS + rr);
+  else
+    sts32(st_s + 4 * t, 0u);
+  cp_async_commit();
+}
+// thread t writes its part of the bf16 tile (2 x 64-row pages, CHUNKS 64-column boxes; shared address `tile`) from the
+// staged rows, one 16-byte unit (8 columns) at a time
+template <int D>
+LB_DEVICE void fp8_tile_fill(uint32_t tile, uint32_t st, uint32_t st_s, int t) {
+  constexpr int UNITS = D / 8;   // 16-byte bf16 units of a row
+#pragma unroll 1
+  for (int i = 0; i < ATT_BN * UNITS / 128; ++i) {
+    const int e = t + 128 * i;
+    const int row = e / UNITS, c = e % UNITS;
+    const uint2 x = lds64(st + e * 8);
+    const float s = lds32f(st_s + 4 * row);
+    // columns 8c .. 8c + 7: unit c % 8 of row `row` of 64-column box c / 8, at its 128B-swizzled place (unit u of
+    // row r at u ^ (r % 8))
+    sts128(tile + (c / 8) * (ATT_BN * 128) + row * 128 + (((c % 8) ^ (row % 8)) * 16), e4m3x2_dequant(x.x, s),
+           e4m3x2_dequant(x.x >> 16, s), e4m3x2_dequant(x.y, s), e4m3x2_dequant(x.y >> 16, s));
+  }
+}
+
 // the forward of one CTA; tmap_* and p are the kernel's __grid_constant__ parameters (inlined: no call in the kernel).
 // PAGED: K/V through the block table `pages` (tail: the maps tail_k, tail_v; see AttnPages); only the producer's
 // addresses change, so the shared-memory tiles, and the output, are those of the contiguous kernel over the gathered
@@ -172,14 +285,18 @@ struct AttnRagged {
 // scores are masked by assignment, so K needs nothing; V's rows at or past Sk in the window's last tile are zeroed in
 // shared memory before P·V (the consumers' generic stores, a proxy fence, then a barrier of the 256 consumer threads),
 // so that tile holds what the tail map would have loaded.
-template <int D, int BIAS, bool DROP, bool DOC, bool PREFIX = false, bool PAGED = false, bool RAGGED = false>
+// FP8 (with RAGGED; see AttnFp8Pages): K/V come from the FP8 pools `f8`, dequantized by the producer warpgroup; the
+// tiles hold zeros past the window, so V needs no zeroing, and tmap_k / tmap_v are not read.
+template <int D, int BIAS, bool DROP, bool DOC, bool PREFIX = false, bool PAGED = false, bool RAGGED = false,
+          bool FP8 = false>
 LB_DEVICE void attn_fwd_cta(const CUtensorMap& tmap_q, const CUtensorMap& tmap_k, const CUtensorMap& tmap_v,
                             const AttnFwdParams& p, const CUtensorMap* tail_k = nullptr,
                             const CUtensorMap* tail_v = nullptr, const AttnPages* pages = nullptr, int rg_blk = 0,
-                            int rg_row = 0) {
+                            int rg_row = 0, const AttnFp8Pages* f8 = nullptr) {
   static_assert(!PAGED || (!DROP && !DOC && !PREFIX && BIAS != BIAS_DENSE), "paged K/V: no dropout, dense bias, "
                 "packed sequences or prefix");
   static_assert(!RAGGED || PAGED, "ragged sequences read paged K/V");
+  static_assert(!FP8 || RAGGED, "FP8 pools are read by the ragged instances");
   static_assert(!DOC || (BIAS == BIAS_NONE && !DROP), "packed sequences run without bias and dropout");
   static_assert(!PREFIX || (BIAS == BIAS_NONE && !DOC), "a prefix runs without bias and packed sequences");
   using Cfg = AttnFwdCfg<D>;
@@ -237,6 +354,48 @@ LB_DEVICE void attn_fwd_cta(const CUtensorMap& tmap_q, const CUtensorMap& tmap_k
   const int nkv = max(0, (key_end + ATT_BN - 1) / ATT_BN - j0);
 
   if (warp_idx < 4) {
+    if constexpr (FP8) {
+      // the TMA producer's 24 registers: the consumers' setmaxnreg.inc to 240 takes exactly the registers the
+      // producer warpgroup releases from the kernel's 168 (128 * 24 + 256 * 240 = 168 * 384), so the 128 threads
+      // filling tiles must fit in 24 as well
+      asm volatile("setmaxnreg.dec.sync.aligned.u32 24;\n" ::: "memory");
+      if (warp_idx == 0 && elect_one()) {
+        mbar_arrive_expect_tx(q_full, Cfg::TILE_BYTES);
+#pragma unroll
+        for (int c = 0; c < Cfg::CHUNKS; ++c)
+          tma_load_5d(sQ + c * (ATT_BM * 128), &tmap_q, q_full, c * 64, rg_row + q0, head - kv_head * p.r, kv_head, 0);
+      }
+      const int t = threadIdx.x;
+      // staging: K bytes [128, D], V bytes [128, D], K scales [128], V scales [128]
+      const uint32_t st_k = smem_u32(bars) + 256, st_v = st_k + ATT_BN * D;
+      const uint32_t ss_k = st_v + ATT_BN * D, ss_v = ss_k + ATT_BN * 4;
+      // each half of the staging buffer is refilled with the next tile as soon as it has been read, so the copies
+      // land while the other half is dequantized and the consumers run
+      if (nkv > 0) {
+        fp8_tile_stage<D>(st_k, ss_k, f8->k, f8->k_scale, *pages, j0, p.Sk, f8->G, kv_head, t);
+        fp8_tile_stage<D>(st_v, ss_v, f8->v, f8->v_scale, *pages, j0, p.Sk, f8->G, kv_head, t);
+      }
+      for (int it = 0; it < nkv; ++it) {
+        const int j = j0 + it, b = it & 1;
+        const uint32_t par = ((it >> 1) & 1) ^ 1;
+        cp_async_wait<1>();   // this thread's K copies (its V copies may be in flight)
+        producer_sync();      // everyone's
+        mbar_wait(&k_empty[b], par);
+        fp8_tile_fill<D>(smem_u32(sK) + b * Cfg::TILE_BYTES, st_k, ss_k, t);
+        fence_proxy_async();   // the generic stores, before the wgmma reads the tile through the async proxy
+        cp_async_wait<0>();
+        producer_sync();       // the K tile written, every V copy landed, the K staging free
+        if (t == 0) mbar_arrive(&k_full[b]);
+        if (it + 1 < nkv) fp8_tile_stage<D>(st_k, ss_k, f8->k, f8->k_scale, *pages, j + 1, p.Sk, f8->G, kv_head, t);
+        mbar_wait(&v_empty[b], par);
+        fp8_tile_fill<D>(smem_u32(sV) + b * Cfg::TILE_BYTES, st_v, ss_v, t);
+        fence_proxy_async();
+        producer_sync();       // the V tile written, the V staging free
+        if (t == 0) mbar_arrive(&v_full[b]);
+        if (it + 1 < nkv) fp8_tile_stage<D>(st_v, ss_v, f8->v, f8->v_scale, *pages, j + 1, p.Sk, f8->G, kv_head, t);
+      }
+      return;
+    }
     asm volatile("setmaxnreg.dec.sync.aligned.u32 24;\n" ::: "memory");
     if (warp_idx == 0 && elect_one()) {
       mbar_arrive_expect_tx(q_full, Cfg::TILE_BYTES);
@@ -436,7 +595,7 @@ LB_DEVICE void attn_fwd_cta(const CUtensorMap& tmap_q, const CUtensorMap& tmap_k
     }
     // ---- O += P·V_j
     mbar_wait(&v_full[b], par);
-    if constexpr (RAGGED) {
+    if constexpr (RAGGED && !FP8) {
       // the window's last tile: rows kv_len - kbase .. 127 of every 64-column chunk (the 128B swizzle permutes the
       // 16-byte pieces inside a row, so a chunk's rows from r0 on are one contiguous range)
       const int r0 = kv_len - kbase;
@@ -528,6 +687,24 @@ attn_fwd_paged_varlen_kernel(const __grid_constant__ CUtensorMap tmap_q, const _
   pg.table = pages.table + static_cast<size_t>(n) * pages.max_pages;
   attn_fwd_cta<D, BIAS, false, false, false, true, true>(tmap_q, tmap_k, tmap_v, sp, &tmap_k, &tmap_v, &pg, tile.y,
                                                          row0);
+}
+// attn_fwd_paged_varlen_kernel over FP8 pools (AttnFp8Pages): the same tiles, shapes and outputs
+template <int D, int BIAS>
+__global__ void __launch_bounds__(ATT_FWD_THREADS, 1)
+attn_fwd_paged_varlen_fp8_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ AttnFwdParams p,
+                                 const __grid_constant__ AttnPages pages, const __grid_constant__ AttnRagged rg,
+                                 const __grid_constant__ AttnFp8Pages f8) {
+  const int2 tile = rg.tiles[blockIdx.x];
+  const int n = tile.x, row0 = rg.cu_q[n];
+  AttnFwdParams sp = p;
+  sp.Sq = rg.cu_q[n + 1] - row0;
+  sp.Sk = rg.past[n] + sp.Sq;
+  sp.o = p.o + static_cast<size_t>(row0) * p.A * p.d;
+  sp.lse = p.lse + static_cast<size_t>(row0) * p.A;
+  AttnPages pg = pages;
+  pg.table = pages.table + static_cast<size_t>(n) * pages.max_pages;
+  attn_fwd_cta<D, BIAS, false, false, false, true, true, true>(tmap_q, tmap_q, tmap_q, sp, nullptr, nullptr, &pg,
+                                                               tile.y, row0, &f8);
 }
 
 }  // namespace lb
@@ -734,13 +911,11 @@ cudaError_t launch_fwd_paged_varlen_t(const CUtensorMap (&maps)[3], const lb::At
   return cudaGetLastError();
 }
 }  // namespace
-// o [T, A, d] and lse [T * A] of the N ragged sequences of q [T, A, d] (a->B = 1, a->Sq = T) over the paged pools
-// [num_pages, G, 64, d]; see launchers.h.  Returns -8 for a problem the paged instances do not run (as
-// lb_attn_fwd_paged, kv_start included) and -9 for an empty pool or table.
-extern "C" int lb_attn_fwd_paged_varlen(const lb::AttnArgs* a, const void* q, const void* k_pool, const void* v_pool,
-                                        int num_pages, const int* block_table, int max_pages, const int* cu_q,
-                                        const int* past, const int* tiles, int n_tiles, void* o, float* lse,
-                                        cudaStream_t s) {
+namespace {
+// what both ragged launchers share: the checks of q, the problem and the pool, q's tensor map and the parameters.
+// Returns the tile width, 0 when there is nothing to launch, or the launcher's error code.
+int varlen_setup(const lb::AttnArgs* a, const void* q, int num_pages, int max_pages, int n_tiles, void* o, float* lse,
+                 CUtensorMap& tq, lb::AttnFwdParams& p) {
   lb::AttnArgs full = *a;
   full.Sk = a->Sq;   // check_attn_args looks at the shapes of q; the key windows are per sequence
   const int tile = check_attn_args(full);
@@ -750,18 +925,30 @@ extern "C" int lb_attn_fwd_paged_varlen(const lb::AttnArgs* a, const void* q, co
     return -8;
   if (num_pages <= 0 || max_pages <= 0) return -9;
   if (n_tiles == 0) return 0;
-  const int P = lb::ATT_PAGE_ROWS;
-  const long pool_strides[3] = {(long)a->G * P * a->d, (long)P * a->d, a->d};   // {page, head, row}
-  CUtensorMap maps[3];   // q, k, v
-  if (!make_q_tmap(&maps[0], q, 1, a->G, a->A / a->G, a->Sq, a->d, a->q_strides, 128)) return -2;
-  if (!make_qkv_tmap(&maps[1], k_pool, num_pages, a->G, P, a->d, pool_strides, P)) return -2;
-  if (!make_qkv_tmap(&maps[2], v_pool, num_pages, a->G, P, a->d, pool_strides, P)) return -2;
-  lb::AttnFwdParams p;
+  if (!make_q_tmap(&tq, q, 1, a->G, a->A / a->G, a->Sq, a->d, a->q_strides, 128)) return -2;
   fill_score_params(p, full, false);
   p.o = reinterpret_cast<__nv_bfloat16*>(o);
   p.lse = lse;
   memset(&p.rng, 0, sizeof(p.rng));
   p.rng_out = nullptr;
+  return tile;
+}
+}  // namespace
+// o [T, A, d] and lse [T * A] of the N ragged sequences of q [T, A, d] (a->B = 1, a->Sq = T) over the paged pools
+// [num_pages, G, 64, d]; see launchers.h.  Returns -8 for a problem the paged instances do not run (as
+// lb_attn_fwd_paged, kv_start included) and -9 for an empty pool or table.
+extern "C" int lb_attn_fwd_paged_varlen(const lb::AttnArgs* a, const void* q, const void* k_pool, const void* v_pool,
+                                        int num_pages, const int* block_table, int max_pages, const int* cu_q,
+                                        const int* past, const int* tiles, int n_tiles, void* o, float* lse,
+                                        cudaStream_t s) {
+  CUtensorMap maps[3];   // q, k, v
+  lb::AttnFwdParams p;
+  const int tile = varlen_setup(a, q, num_pages, max_pages, n_tiles, o, lse, maps[0], p);
+  if (tile <= 0) return tile;
+  const int P = lb::ATT_PAGE_ROWS;
+  const long pool_strides[3] = {(long)a->G * P * a->d, (long)P * a->d, a->d};   // {page, head, row}
+  if (!make_qkv_tmap(&maps[1], k_pool, num_pages, a->G, P, a->d, pool_strides, P)) return -2;
+  if (!make_qkv_tmap(&maps[2], v_pool, num_pages, a->G, P, a->d, pool_strides, P)) return -2;
   const lb::AttnPages pages{block_table, max_pages, num_pages};
   const lb::AttnRagged rg{cu_q, past, reinterpret_cast<const int2*>(tiles)};
   const bool alibi = p.alibi_slopes != nullptr;
@@ -770,6 +957,49 @@ extern "C" int lb_attn_fwd_paged_varlen(const lb::AttnArgs* a, const void* q, co
                        : launch_fwd_paged_varlen_t<64, lb::BIAS_NONE>(maps, p, pages, rg, n_tiles, s));
   return (int)(alibi ? launch_fwd_paged_varlen_t<128, lb::BIAS_ALIBI>(maps, p, pages, rg, n_tiles, s)
                      : launch_fwd_paged_varlen_t<128, lb::BIAS_NONE>(maps, p, pages, rg, n_tiles, s));
+}
+
+namespace {
+template <int D, int BIAS>
+cudaError_t launch_fwd_paged_varlen_fp8_t(const CUtensorMap& tq, const lb::AttnFwdParams& p,
+                                          const lb::AttnPages& pages, const lb::AttnRagged& rg,
+                                          const lb::AttnFp8Pages& f8, int n_tiles, cudaStream_t s) {
+  using Cfg = lb::AttnFwdCfg<D>;
+  auto kern = lb::attn_fwd_paged_varlen_fp8_kernel<D, BIAS>;
+  static bool configured = false;
+  if (!configured) {
+    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::FP8_SMEM_BYTES);
+    if (e != cudaSuccess) return e;
+    configured = true;
+  }
+  kern<<<dim3(n_tiles, p.A), lb::ATT_FWD_THREADS, Cfg::FP8_SMEM_BYTES, s>>>(tq, p, pages, rg, f8);
+  return cudaGetLastError();
+}
+}  // namespace
+// lb_attn_fwd_paged_varlen over FP8 pools; see launchers.h.  Returns the codes of lb_attn_fwd_paged_varlen, and -3
+// for pools or scales not 16-byte aligned.
+extern "C" int lb_attn_fwd_paged_varlen_fp8(const lb::AttnArgs* a, const void* q, const void* k_pool,
+                                            const void* v_pool, const float* k_scale, const float* v_scale,
+                                            int num_pages, const int* block_table, int max_pages, const int* cu_q,
+                                            const int* past, const int* tiles, int n_tiles, void* o, float* lse,
+                                            cudaStream_t s) {
+  if (((reinterpret_cast<uintptr_t>(k_pool) | reinterpret_cast<uintptr_t>(v_pool) |
+        reinterpret_cast<uintptr_t>(k_scale) | reinterpret_cast<uintptr_t>(v_scale)) & 15))
+    return -3;
+  CUtensorMap tq;
+  lb::AttnFwdParams p;
+  const int tile = varlen_setup(a, q, num_pages, max_pages, n_tiles, o, lse, tq, p);
+  if (tile <= 0) return tile;
+  const lb::AttnPages pages{block_table, max_pages, num_pages};
+  const lb::AttnRagged rg{cu_q, past, reinterpret_cast<const int2*>(tiles)};
+  const lb::AttnFp8Pages f8{static_cast<const uint8_t*>(k_pool), static_cast<const uint8_t*>(v_pool), k_scale, v_scale,
+                            a->G};
+  const bool alibi = p.alibi_slopes != nullptr;
+  if (tile == 64)
+    return (int)(alibi ? launch_fwd_paged_varlen_fp8_t<64, lb::BIAS_ALIBI>(tq, p, pages, rg, f8, n_tiles, s)
+                       : launch_fwd_paged_varlen_fp8_t<64, lb::BIAS_NONE>(tq, p, pages, rg, f8, n_tiles, s));
+  return (int)(alibi ? launch_fwd_paged_varlen_fp8_t<128, lb::BIAS_ALIBI>(tq, p, pages, rg, f8, n_tiles, s)
+                     : launch_fwd_paged_varlen_fp8_t<128, lb::BIAS_NONE>(tq, p, pages, rg, f8, n_tiles, s));
 }
 // =================================================================================================
 // Backward.  One CTA per (batch, K/V head, NWG consecutive 64-key blocks).  Consumer warpgroup w (warpgroups 1 ..

@@ -1131,15 +1131,26 @@ Tensor attn_fwd_paged(const Tensor& q, const Tensor& k_pool, const Tensor& v_poo
 // past[n] + Sq_n <= max_pages * 64, and the table entries of the rows each sequence reads (an entry outside [0, P)
 // reads as zero rows).  alibi_slopes fp32 [A] as in attn_fwd.  Returns o [T, A, D]; rows of no sequence are left
 // uninitialised.
-Tensor attn_fwd_paged_varlen(const Tensor& q, const Tensor& k_pool, const Tensor& v_pool, const Tensor& block_table,
-                             const Tensor& cu_q, const Tensor& past, const Tensor& tiles, double scale,
-                             const c10::optional<Tensor>& alibi_slopes) {
-  Args args("attn_fwd_paged_varlen");
+// With k_scale and v_scale (fp32 [P, G, 64], contiguous) the pools are FP8 (E4M3, contiguous, 16-byte aligned): each
+// sequence's output is the bf16 op's over the dequantized pools bf16_rn(float(e) * s), bit for bit, whatever the pools
+// hold outside the windows.
+Tensor attn_fwd_paged_varlen_any(const char* op, const Tensor& q, const Tensor& k_pool, const Tensor& v_pool,
+                                 const Tensor* k_scale, const Tensor* v_scale, const Tensor& block_table,
+                                 const Tensor& cu_q, const Tensor& past, const Tensor& tiles, double scale,
+                                 const c10::optional<Tensor>& alibi_slopes) {
+  Args args(op);
   args("q", q, at::kBFloat16, {kAny, kAny, kAny}, Layout::LastDimContiguous, 16);
   const int64_t D = q.size(2);
-  TORCH_CHECK(D == 64 || D == 128, "attn_fwd_paged_varlen: head dim must be 64 or 128, got ", D);
-  args("k_pool", k_pool, at::kBFloat16, {kAny, kAny, 64, D});
-  args("v_pool", v_pool, at::kBFloat16, k_pool.sizes());
+  TORCH_CHECK(D == 64 || D == 128, op, ": head dim must be 64 or 128, got ", D);
+  if (k_scale != nullptr) {
+    args("k_pool", k_pool, at::kFloat8_e4m3fn, {kAny, kAny, 64, D}, Layout::Contiguous, 16);
+    args("v_pool", v_pool, at::kFloat8_e4m3fn, k_pool.sizes(), Layout::Contiguous, 16);
+    args("k_scale", *k_scale, at::kFloat, k_pool.sizes().slice(0, 3), Layout::Contiguous, 16);
+    args("v_scale", *v_scale, at::kFloat, k_pool.sizes().slice(0, 3), Layout::Contiguous, 16);
+  } else {
+    args("k_pool", k_pool, at::kBFloat16, {kAny, kAny, 64, D});
+    args("v_pool", v_pool, at::kBFloat16, k_pool.sizes());
+  }
   args("block_table", block_table, at::kInt, {kAny, kAny});
   const int64_t N = block_table.size(0);
   args("cu_q", cu_q, at::kInt, {N + 1});
@@ -1151,11 +1162,11 @@ Tensor attn_fwd_paged_varlen(const Tensor& q, const Tensor& k_pool, const Tensor
   a.A = (int)q.size(1);
   a.G = (int)k_pool.size(1);
   a.d = (int)D;
-  TORCH_CHECK(a.G > 0 && a.A % a.G == 0, "attn_fwd_paged_varlen: the query heads must be a multiple of the K/V heads");
-  TORCH_CHECK(k_pool.size(0) >= 1 && k_pool.size(0) <= INT32_MAX, "attn_fwd_paged_varlen: 1 <= pages <= INT32_MAX");
-  TORCH_CHECK(a.Sq >= 1 && N >= 1 && block_table.size(1) >= 1, "attn_fwd_paged_varlen: at least one token, one "
-              "sequence and one table column");
-  TORCH_CHECK(tiles.size(0) <= INT32_MAX / 2, "attn_fwd_paged_varlen: too many tiles");
+  TORCH_CHECK(a.G > 0 && a.A % a.G == 0, op, ": the query heads must be a multiple of the K/V heads");
+  TORCH_CHECK(k_pool.size(0) >= 1 && k_pool.size(0) <= INT32_MAX, op, ": 1 <= pages <= INT32_MAX");
+  TORCH_CHECK(a.Sq >= 1 && N >= 1 && block_table.size(1) >= 1, op, ": at least one token, one sequence and one table "
+              "column");
+  TORCH_CHECK(tiles.size(0) <= INT32_MAX / 2, op, ": too many tiles");
   const long r = a.A / a.G;
   a.q_strides[0] = (long)q.size(0) * q.stride(0);
   a.q_strides[1] = r * q.stride(1);
@@ -1168,12 +1179,33 @@ Tensor attn_fwd_paged_varlen(const Tensor& q, const Tensor& k_pool, const Tensor
   const auto guard = args.guard();
   Tensor o = at::empty({a.Sq, a.A, a.d}, q.options());
   Tensor lse = at::empty({(int64_t)a.Sq * a.A}, q.options().dtype(at::kFloat));
-  check(lb_attn_fwd_paged_varlen(&a, q.data_ptr(), k_pool.data_ptr(), v_pool.data_ptr(), (int)k_pool.size(0),
-                                 block_table.data_ptr<int>(), (int)block_table.size(1), cu_q.data_ptr<int>(),
-                                 past.data_ptr<int>(), tiles.data_ptr<int>(), (int)tiles.size(0), o.data_ptr(),
-                                 lse.data_ptr<float>(), cur_stream()),
-        "attn_fwd_paged_varlen");
+  const int P = (int)k_pool.size(0), mp = (int)block_table.size(1), n_tiles = (int)tiles.size(0);
+  if (k_scale != nullptr)
+    check(lb_attn_fwd_paged_varlen_fp8(&a, q.data_ptr(), k_pool.data_ptr(), v_pool.data_ptr(),
+                                       k_scale->data_ptr<float>(), v_scale->data_ptr<float>(), P,
+                                       block_table.data_ptr<int>(), mp, cu_q.data_ptr<int>(), past.data_ptr<int>(),
+                                       tiles.data_ptr<int>(), n_tiles, o.data_ptr(), lse.data_ptr<float>(),
+                                       cur_stream()),
+          op);
+  else
+    check(lb_attn_fwd_paged_varlen(&a, q.data_ptr(), k_pool.data_ptr(), v_pool.data_ptr(), P,
+                                   block_table.data_ptr<int>(), mp, cu_q.data_ptr<int>(), past.data_ptr<int>(),
+                                   tiles.data_ptr<int>(), n_tiles, o.data_ptr(), lse.data_ptr<float>(), cur_stream()),
+          op);
   return o;
+}
+Tensor attn_fwd_paged_varlen(const Tensor& q, const Tensor& k_pool, const Tensor& v_pool, const Tensor& block_table,
+                             const Tensor& cu_q, const Tensor& past, const Tensor& tiles, double scale,
+                             const c10::optional<Tensor>& alibi_slopes) {
+  return attn_fwd_paged_varlen_any("attn_fwd_paged_varlen", q, k_pool, v_pool, nullptr, nullptr, block_table, cu_q,
+                                   past, tiles, scale, alibi_slopes);
+}
+Tensor attn_fwd_paged_varlen_fp8(const Tensor& q, const Tensor& k_pool, const Tensor& v_pool, const Tensor& k_scale,
+                                 const Tensor& v_scale, const Tensor& block_table, const Tensor& cu_q,
+                                 const Tensor& past, const Tensor& tiles, double scale,
+                                 const c10::optional<Tensor>& alibi_slopes) {
+  return attn_fwd_paged_varlen_any("attn_fwd_paged_varlen_fp8", q, k_pool, v_pool, &k_scale, &v_scale, block_table,
+                                   cu_q, past, tiles, scale, alibi_slopes);
 }
 
 // ---- KV-cache decoding ------------------------------------------------------------------------------
@@ -1273,15 +1305,15 @@ Tensor kv_append_fp8_paged(const Tensor& qkv, const Tensor& k_pool, const Tensor
 // [N, max_pages], rotated at that position with cos/sin; bf16 pools [P, G, 64, D].  Like the lengths of
 // kv_append_paged, cu_q (int32 [N + 1], from 0 to T, non-decreasing), past (int32 [N]) and the page ids of the rows
 // written are the caller's guarantee.  Returns q [1, T, G * r, D] when write_q, else empty.
-Tensor kv_append_paged_varlen(const Tensor& qkv, const Tensor& k_pool, const Tensor& v_pool, const Tensor& block_table,
-                              const Tensor& cu_q, const Tensor& past, const c10::optional<Tensor>& cosv,
-                              const c10::optional<Tensor>& sinv, bool write_q) {
-  const char* op = "kv_append_paged_varlen";
+Tensor kv_append_paged_varlen_any(const char* op, const Tensor& qkv, const Tensor& k_pool, const Tensor& v_pool,
+                                  const Tensor* k_scale, const Tensor* v_scale, const Tensor& block_table,
+                                  const Tensor& cu_q, const Tensor& past, const c10::optional<Tensor>& cosv,
+                                  const c10::optional<Tensor>& sinv, bool write_q) {
   Args args(op);
   args("qkv", qkv, at::kBFloat16, qkv.sizes());
   const PackedQKV g = packed_qkv(qkv, op);
   TORCH_CHECK(g.B == 1, op, ": the sequences are packed along dim 1 of a batch of 1, got batch ", g.B);
-  cache_args(args, k_pool, v_pool, nullptr, nullptr, {kAny, g.G, 64, g.D});
+  cache_args(args, k_pool, v_pool, k_scale, v_scale, {kAny, g.G, 64, g.D});
   args("block_table", block_table, at::kInt, {kAny, kAny});
   const int64_t N = block_table.size(0);
   TORCH_CHECK(N >= 1 && N <= INT32_MAX && block_table.size(1) >= 1, op, ": at least one sequence and table column");
@@ -1292,13 +1324,36 @@ Tensor kv_append_paged_varlen(const Tensor& qkv, const Tensor& k_pool, const Ten
   const auto guard = args.guard();
   const int T = g.S, A = g.G * g.r;
   Tensor q_out = write_q ? at::empty({1, T, A, g.D}, qkv.options()) : at::empty({0}, qkv.options());
-  check(lb_kv_append_paged_varlen(qkv.data_ptr(), given(cosv) ? cosv->data_ptr<float>() : nullptr,
-                                  given(sinv) ? sinv->data_ptr<float>() : nullptr,
-                                  write_q ? q_out.data_ptr() : nullptr, k_pool.data_ptr(), v_pool.data_ptr(),
-                                  cu_q.data_ptr<int>(), past.data_ptr<int>(), (int)N, block_table.data_ptr<int>(),
-                                  (int)block_table.size(1), T, g.G, g.r, g.D, cur_stream()),
-        op);
+  const float* cp = given(cosv) ? cosv->data_ptr<float>() : nullptr;
+  const float* sp = given(sinv) ? sinv->data_ptr<float>() : nullptr;
+  void* qp = write_q ? q_out.data_ptr() : nullptr;
+  if (k_scale != nullptr)
+    check(lb_kv_append_fp8_paged_varlen(qkv.data_ptr(), cp, sp, qp, k_pool.data_ptr(), v_pool.data_ptr(),
+                                        k_scale->data_ptr<float>(), v_scale->data_ptr<float>(), cu_q.data_ptr<int>(),
+                                        past.data_ptr<int>(), (int)N, block_table.data_ptr<int>(),
+                                        (int)block_table.size(1), T, g.G, g.r, g.D, cur_stream()),
+          op);
+  else
+    check(lb_kv_append_paged_varlen(qkv.data_ptr(), cp, sp, qp, k_pool.data_ptr(), v_pool.data_ptr(),
+                                    cu_q.data_ptr<int>(), past.data_ptr<int>(), (int)N, block_table.data_ptr<int>(),
+                                    (int)block_table.size(1), T, g.G, g.r, g.D, cur_stream()),
+          op);
   return q_out;
+}
+Tensor kv_append_paged_varlen(const Tensor& qkv, const Tensor& k_pool, const Tensor& v_pool, const Tensor& block_table,
+                              const Tensor& cu_q, const Tensor& past, const c10::optional<Tensor>& cosv,
+                              const c10::optional<Tensor>& sinv, bool write_q) {
+  return kv_append_paged_varlen_any("kv_append_paged_varlen", qkv, k_pool, v_pool, nullptr, nullptr, block_table, cu_q,
+                                    past, cosv, sinv, write_q);
+}
+// kv_append_paged_varlen into FP8 (E4M3) pools with row scales k_scale, v_scale fp32 [P, G, 64]: each sequence's
+// bytes, scales and q are kv_append_fp8_paged's on that sequence alone
+Tensor kv_append_fp8_paged_varlen(const Tensor& qkv, const Tensor& k_pool, const Tensor& v_pool, const Tensor& k_scale,
+                                  const Tensor& v_scale, const Tensor& block_table, const Tensor& cu_q,
+                                  const Tensor& past, const c10::optional<Tensor>& cosv,
+                                  const c10::optional<Tensor>& sinv, bool write_q) {
+  return kv_append_paged_varlen_any("kv_append_fp8_paged_varlen", qkv, k_pool, v_pool, &k_scale, &v_scale,
+                                    block_table, cu_q, past, cosv, sinv, write_q);
 }
 
 // Copies page src to page dst of every array of `arrays` (the K and V pools, and the FP8 scales, of every layer of a
@@ -1720,6 +1775,8 @@ TORCH_LIBRARY(libai_b200, m) {
   m.def("attn_bwd(Tensor dout, Tensor q, Tensor k, Tensor v, Tensor o, Tensor lse, bool causal, float scale, Tensor? kv_lens, Tensor? bias=None, Tensor? alibi_slopes=None, Tensor(a!)? dbias=None, float p_drop=0.0, Tensor? rng_state=None, Tensor? kv_start=None, Tensor? doc_start=None, Tensor? prefix_lens=None) -> (Tensor, Tensor, Tensor, Tensor)", &attn_bwd);
   m.def("attn_fwd_paged(Tensor q, Tensor k_pool, Tensor v_pool, Tensor block_table, int past, float scale, Tensor? kv_start=None, Tensor? alibi_slopes=None) -> Tensor", &attn_fwd_paged);
   m.def("attn_fwd_paged_varlen(Tensor q, Tensor k_pool, Tensor v_pool, Tensor block_table, Tensor cu_q, Tensor past, Tensor tiles, float scale, Tensor? alibi_slopes=None) -> Tensor", &attn_fwd_paged_varlen);
+  m.def("attn_fwd_paged_varlen_fp8(Tensor q, Tensor k_pool, Tensor v_pool, Tensor k_scale, Tensor v_scale, Tensor block_table, Tensor cu_q, Tensor past, Tensor tiles, float scale, Tensor? alibi_slopes=None) -> Tensor", &attn_fwd_paged_varlen_fp8);
+  m.def("kv_append_fp8_paged_varlen(Tensor qkv, Tensor(a!) k_pool, Tensor(b!) v_pool, Tensor(c!) k_scale, Tensor(d!) v_scale, Tensor block_table, Tensor cu_q, Tensor past, Tensor? cos, Tensor? sin, bool write_q) -> Tensor", &kv_append_fp8_paged_varlen);
   m.def("kv_append_paged_varlen(Tensor qkv, Tensor(a!) k_pool, Tensor(b!) v_pool, Tensor block_table, Tensor cu_q, Tensor past, Tensor? cos, Tensor? sin, bool write_q) -> Tensor", &kv_append_paged_varlen);
   m.def("kv_append(Tensor qkv, Tensor(a!) k_cache, Tensor(b!) v_cache, Tensor cache_seqlens, Tensor? cos, Tensor? sin, bool write_q) -> Tensor", &kv_append);
   m.def("kv_append_fp8(Tensor qkv, Tensor(a!) k_cache, Tensor(b!) v_cache, Tensor(c!) k_scale, Tensor(d!) v_scale, Tensor cache_seqlens, Tensor? cos, Tensor? sin, bool write_q) -> Tensor", &kv_append_fp8);

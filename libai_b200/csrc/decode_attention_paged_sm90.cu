@@ -14,8 +14,9 @@
 //   per row as before (only the address changes); FP8 issues one bulk copy per page piece and array, at most two.
 //   Instances: no score bias and ALiBi, bf16 and FP8, D = 64 and 128.
 // appends: kv_append_body / kv_append_fp8_body with the row address taken through the table; bytes and scales are
-//   those of the contiguous appends.  The ragged bf16 append (kv_append_body's RAGGED flag) writes the tokens of N
-//   sequences packed along one axis, each at its own rows; its bytes are those of the paged append per sequence.
+//   those of the contiguous appends.  The ragged appends (the RAGGED flag of kv_append_body and kv_append_fp8_body)
+//   write the tokens of N sequences packed along one axis, each at its own rows; their bytes (and FP8 scales) are
+//   those of the paged append per sequence.
 // page copy: the (src, dst) page pairs of every array of a list (K, V and the FP8 scales of every layer) in one
 //   launch.
 #include "decode_attention_sm90.cuh"
@@ -90,6 +91,17 @@ __global__ void __launch_bounds__(256) kv_append_fp8_paged_kernel(
   kv_append_fp8_body<D, true>(qkv, cosv, sinv, q_out, kc, vc, ks, vs, seqlens, table, max_pages, B, Sq, G, r, kTile);
 }
 
+// the FP8 append of N ragged sequences packed along the token axis (kv_append_fp8_body's RAGGED flag)
+template <int D>
+__global__ void __launch_bounds__(256) kv_append_fp8_paged_varlen_kernel(
+    const __nv_bfloat16* __restrict__ qkv, const float* __restrict__ cosv, const float* __restrict__ sinv,
+    __nv_bfloat16* __restrict__ q_out, uint8_t* __restrict__ kc, uint8_t* __restrict__ vc, float* __restrict__ ks,
+    float* __restrict__ vs, const int* __restrict__ cu_q, const int* __restrict__ past, int nseq,
+    const int* __restrict__ table, int max_pages, int T, int G, int r) {
+  kv_append_fp8_body<D, true, true>(qkv, cosv, sinv, q_out, kc, vc, ks, vs, past, table, max_pages, 1, T, G, r, kTile,
+                                    cu_q, nseq);
+}
+
 // one CTA per (pair, array): the page src of array a to its page dst, 16 bytes per thread and step
 __global__ void __launch_bounds__(256) kv_page_copy_kernel(const long* __restrict__ desc, int npairs) {
   // desc: npairs (src, dst) pairs, then per array its address and its page bytes (a multiple of 16)
@@ -148,6 +160,23 @@ extern "C" int lb_kv_append_fp8_paged(const void* qkv, const float* cosv, const 
                                   static_cast<__nv_bfloat16*>(q_out), static_cast<uint8_t*>(k_pool),
                                   static_cast<uint8_t*>(v_pool), k_scale, v_scale, seqlens, block_table, max_pages, B,
                                   Sq, G, r);
+  return (int)cudaGetLastError();
+}
+
+extern "C" int lb_kv_append_fp8_paged_varlen(const void* qkv, const float* cosv, const float* sinv, void* q_out,
+                                             void* k_pool, void* v_pool, float* k_scale, float* v_scale,
+                                             const int* cu_q, const int* past, int nseq, const int* block_table,
+                                             int max_pages, int T, int G, int r, int D, cudaStream_t s) {
+  const size_t warps = (size_t)T * G;
+  if (warps == 0 || nseq == 0) return 0;
+  if (D != 64 && D != 128) return -4;
+  const int threads = 256;
+  const int blocks = (int)((warps * 32 + threads - 1) / threads < 4096 ? (warps * 32 + threads - 1) / threads : 4096);
+  auto kern = D == 64 ? lb::dec::kv_append_fp8_paged_varlen_kernel<64> : lb::dec::kv_append_fp8_paged_varlen_kernel<128>;
+  kern<<<blocks, threads, 0, s>>>(static_cast<const __nv_bfloat16*>(qkv), cosv, sinv,
+                                  static_cast<__nv_bfloat16*>(q_out), static_cast<uint8_t*>(k_pool),
+                                  static_cast<uint8_t*>(v_pool), k_scale, v_scale, cu_q, past, nseq, block_table,
+                                  max_pages, T, G, r);
   return (int)cudaGetLastError();
 }
 

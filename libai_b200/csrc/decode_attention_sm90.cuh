@@ -497,13 +497,15 @@ __device__ __forceinline__ void quantize_row(const float (&x)[2 * P], uint8_t* r
   if (lane == 0) *scale = s;
 }
 
-// the FP8 cache append (kv_append_fp8_kernel, and its paged instance); see kv_append_fp8_kernel
-template <int D, bool PAGED>
+// the FP8 cache append (kv_append_fp8_kernel, and its paged instances); see kv_append_fp8_kernel.
+// RAGGED (paged, B = 1): token i goes to its sequence's row as in kv_append_body's RAGGED instance.
+template <int D, bool PAGED, bool RAGGED = false>
 __device__ __forceinline__ void kv_append_fp8_body(
     const __nv_bfloat16* __restrict__ qkv, const float* __restrict__ cosv, const float* __restrict__ sinv,
     __nv_bfloat16* __restrict__ q_out, uint8_t* __restrict__ kc, uint8_t* __restrict__ vc, float* __restrict__ ks,
     float* __restrict__ vs, const int* __restrict__ seqlens, const int* __restrict__ table, int max_pages, int B,
-    int Sq, int G, int r, int C) {
+    int Sq, int G, int r, int C, const int* __restrict__ cu_q = nullptr, int nseq = 0) {
+  static_assert(!RAGGED || PAGED, "ragged sequences append to pages");
   constexpr int half = D / 2, P = half / 32;
   const int lane = threadIdx.x & 31;
   const size_t total = (size_t)B * Sq * G;
@@ -512,9 +514,20 @@ __device__ __forceinline__ void kv_append_fp8_body(
     const int g = static_cast<int>(grp % G);
     const int i = static_cast<int>((grp / G) % Sq);
     const int b = static_cast<int>(grp / ((size_t)G * Sq));
-    const int pos = seqlens[b] + i;
+    int seq = b, pos;
+    if constexpr (RAGGED) {
+      int lo = 0, hi = nseq - 1;   // the last n with cu_q[n] <= i
+      while (lo < hi) {
+        const int mid = (lo + hi + 1) / 2;
+        if (cu_q[mid] <= i) lo = mid; else hi = mid - 1;
+      }
+      seq = lo;
+      pos = seqlens[seq] + i - cu_q[seq];
+    } else {
+      pos = seqlens[b] + i;
+    }
     const size_t in = grp * (r + 2) * D;
-    const size_t crow = cache_row<PAGED>(table, max_pages, b, g, G, C, pos);
+    const size_t crow = cache_row<PAGED>(table, max_pages, seq, g, G, C, pos);
     RopePair t[P];
 #pragma unroll
     for (int p = 0; p < P; ++p) {

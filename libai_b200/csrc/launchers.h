@@ -138,6 +138,13 @@ int lb_attn_fwd_paged(const lb::AttnArgs* a, const void* q, const void* k_pool, 
 int lb_attn_fwd_paged_varlen(const lb::AttnArgs* a, const void* q, const void* k_pool, const void* v_pool,
                              int num_pages, const int* block_table, int max_pages, const int* cu_q, const int* past,
                              const int* tiles, int n_tiles, void* o, float* lse, cudaStream_t s);
+// lb_attn_fwd_paged_varlen over FP8 (E4M3) pools [num_pages, G, 64, d] with fp32 row scales k_scale, v_scale
+// [num_pages, G, 64] (16-byte aligned): the keys and values are the rows bf16_rn(float(e) * s), so each sequence's
+// output is lb_attn_fwd_paged_varlen's over the dequantized pools, bit for bit
+int lb_attn_fwd_paged_varlen_fp8(const lb::AttnArgs* a, const void* q, const void* k_pool, const void* v_pool,
+                                 const float* k_scale, const float* v_scale, int num_pages, const int* block_table,
+                                 int max_pages, const int* cu_q, const int* past, const int* tiles, int n_tiles,
+                                 void* o, float* lse, cudaStream_t s);
 // backward: dout with do_strides = {batch, head, seq} over the A query heads; dq written with dq_strides = {batch,
 // group, in-group, seq}, dk and dv with dkv_strides = {batch, head, seq}; delta fp32 [B, A, Sq] and dq_accum
 // (lb_attn_bwd_accum_floats) are workspaces, dq_order [B * A * ceil(Sq / 64)] zeroed by the caller; dbias (optional,
@@ -179,6 +186,11 @@ int lb_kv_append_paged_varlen(const void* qkv, const float* cosv, const float* s
 int lb_kv_append_fp8_paged(const void* qkv, const float* cosv, const float* sinv, void* q_out, void* k_pool,
                            void* v_pool, float* k_scale, float* v_scale, const int* seqlens, const int* block_table,
                            int max_pages, int B, int Sq, int G, int r, int D, cudaStream_t s);
+// lb_kv_append_paged_varlen into FP8 pools [P, G, 64, D] with scales [P, G, 64]
+int lb_kv_append_fp8_paged_varlen(const void* qkv, const float* cosv, const float* sinv, void* q_out, void* k_pool,
+                                  void* v_pool, float* k_scale, float* v_scale, const int* cu_q, const int* past,
+                                  int nseq, const int* block_table, int max_pages, int T, int G, int r, int D,
+                                  cudaStream_t s);
 // desc (device int64): npairs (src, dst) page pairs, then per array its address and page bytes (a multiple of 16);
 // copies page src to page dst of every array
 int lb_kv_page_copy(const long* desc, int npairs, int narrays, cudaStream_t s);

@@ -24,6 +24,10 @@ Scheduling rules:
   (a parameter's ``data_ptr()`` or ``_version``), as ``generate()``'s is.
 - ``decode_graphs``: a step without prompt chunks replays one CUDA graph (:class:`~.decode_graph.DecodeGraph`) of
   ``max_batch`` decode rows, whose inputs are the cache's descriptor buffers; steps with chunks run eagerly.
+- ``kv_cache_dtype="fp8"``: the pools hold E4M3 rows with fp32 row scales (the format of ``generate(kv_cache_dtype=
+  "fp8")``), about half the bytes of bf16 pages, so the same memory admits about twice the requests.  The ragged FP8
+  append writes the rows; the decode rows run the paged FP8 decode kernel and the chunks the FP8 ragged prefill, both
+  over the dequantized rows.  Chunked prefill, prefix caching and decode graphs work as on bf16 pools.
 
 Supported models are those whose class sets ``continuous_batching = True`` (their cached step takes positions only
 from the cache's per-sequence lengths): the Llama family and BLOOM.  The model's own ``kv_cache`` and decode graph are
@@ -47,6 +51,7 @@ from .generator.generation_logits_processor import (
     TopKLogitsWarper,
     TopPLogitsWarper,
 )
+from .generator.generation_utils import _kv_cache_dtype
 from .kv_cache import RaggedPagedKVCache
 
 
@@ -93,17 +98,20 @@ class GenerationEngine:
     """Continuous batching for a model with ``continuous_batching = True`` (see the module docstring).
 
     ``num_pages``: the pool's pages of 64 rows per layer (default: room for ``max_batch`` sequences of the model's
-    maximum length, or of 2,048 tokens for a model without one).  Sampling is engine-wide: greedy, or with
+    maximum length, or of 2,048 tokens for a model without one).  ``kv_cache_dtype``: None (the weights' dtype), or
+    ``"fp8"`` / ``torch.float8_e4m3fn`` for FP8 (E4M3) pools.  Sampling is engine-wide: greedy, or with
     ``do_sample`` temperature / top-k / top-p through ``generate()``'s logits warpers."""
 
     def __init__(self, model, max_batch: int = 32, max_tokens_per_step: int = 2048, num_pages: Optional[int] = None,
                  prefix_caching: bool = False, decode_graphs: bool = False, do_sample: bool = False,
-                 temperature: float = 1.0, top_k: int = 0, top_p: float = 1.0):
+                 temperature: float = 1.0, top_k: int = 0, top_p: float = 1.0, kv_cache_dtype=None):
         if not getattr(type(model), "continuous_batching", False):
             raise ValueError(f"{type(model).__name__} does not support continuous batching (its cached step does not "
                              "take positions from the cache's per-sequence lengths)")
         if getattr(model, "kv_cache_dtype", None) is not None:
-            raise ValueError("continuous batching runs on a bf16 (the weights' dtype) KV cache, not FP8")
+            raise ValueError("the engine's KV dtype is its own kv_cache_dtype argument (e.g. 'fp8' for an FP8 cache), "
+                             "not the model's kv_cache_dtype attribute, which generate() sets")
+        kv_dtype = _kv_cache_dtype(kv_cache_dtype)
         topo = dutil.get_dist_util()
         if topo.tensor_parallel_size > 1 or topo.pipeline_parallel_size > 1:
             raise ValueError("continuous batching does not run under tensor or pipeline parallelism")
@@ -125,7 +133,7 @@ class GenerationEngine:
         self.model, self.max_batch, self.max_tokens = model, max_batch, max_tokens_per_step
         self.prefix_caching, self.decode_graphs = prefix_caching, decode_graphs
         self.cache = RaggedPagedKVCache(len(mods), max_batch, heads, mods[0].head_size, num_pages, max_pages,
-                                        max_tokens_per_step, dtype, w.device)
+                                        max_tokens_per_step, dtype, w.device, kv_dtype=kv_dtype)
         self._forward = _Forward(model, self.cache)
         self.do_sample = do_sample
         self.warpers = LogitsProcessorList()

@@ -774,7 +774,8 @@ class RaggedPagedKVCacheLayer(KVCacheLayer):
 
     def append(self, qkv: torch.Tensor, cos=None, sin=None) -> torch.Tensor:
         c = self.cache
-        return OF.kv_cache_append_paged_varlen(qkv, self.k, self.v, c.table, c.cu_q, c.past, cos, sin)
+        return OF.kv_cache_append_paged_varlen(qkv, self.k, self.v, c.table, c.cu_q, c.past, cos, sin, self.k_scale,
+                                               self.v_scale)
 
     def attend(self, q: torch.Tensor, *, scale: float, causal: bool = True, mask=None, bias=None, alibi_slopes=None,
                rel_bias=None, dropout_p: float = 0.0, training: bool = False, prefix_lens=None) -> torch.Tensor:
@@ -785,17 +786,18 @@ class RaggedPagedKVCacheLayer(KVCacheLayer):
             raise ValueError("RaggedPagedKVCache: causal self-attention without mask, bias, rel_bias, prefix or "
                              "dropout only")
         c = self.cache
-        if not OF.attention_paged_supported(q, self.k):   # the reference math, every sequence alike
+        scales = {"k_scale": self.k_scale, "v_scale": self.v_scale}
+        if not c.flash_attention():   # the reference math, every sequence alike
             return OF.attention_paged_varlen(q[0], self.k, self.v, c.table, c.cu_q, c.past, scale=scale,
-                                             alibi_slopes=alibi_slopes)[None]
+                                             alibi_slopes=alibi_slopes, **scales)[None]
         mb = c.max_batch
         out = OF.decode_attention(q[0, :mb, None], self.k, self.v, c.past[:mb], c.kv_start, scale=scale,
-                                  alibi_slopes=alibi_slopes, block_table=c.table[:mb])
+                                  alibi_slopes=alibi_slopes, block_table=c.table[:mb], **scales)
         out = out.view(1, mb, *q.shape[2:])
         if c.chunks == 0:
             return out
         pre = OF.attention_paged_varlen(q[0, mb:], self.k, self.v, c.table[mb:], c.cu_c, c.past[mb:], c.tiles,
-                                        scale=scale, alibi_slopes=alibi_slopes)
+                                        scale=scale, alibi_slopes=alibi_slopes, **scales)
         return torch.cat((out, pre[None]), dim=1)
 
 
@@ -807,8 +809,11 @@ class RaggedPagedKVCache(StaticKVCache):
 
     - Each owned layer has a K and a V pool ``[num_pages + 1, heads, 64, head_dim]`` in the format of a
       :class:`PagedKVCache`; the last page is the **sink**, which idle decode rows write and read (their outputs are
-      discarded).  Every other page is the scheduler's: :meth:`alloc` and :meth:`release` keep a reference count per
-      page and a free list, and the prefix index (:class:`PrefixIndex`) holds one reference per cached page.
+      discarded).  With ``kv_dtype=torch.float8_e4m3fn`` the pools hold E4M3 bytes and each layer has fp32 row scales
+      ``k_scale`` / ``v_scale`` ``[num_pages + 1, heads, 64]`` (``fp8`` is set): the ragged FP8 append writes them, and
+      the decode rows and prompt chunks attend over the dequantized rows.  Every other page is the scheduler's:
+      :meth:`alloc` and :meth:`release` keep a reference count per page and a free list, and the prefix index
+      (:class:`PrefixIndex`) holds one reference per cached page.
     - A step's tokens are the ``max_batch`` decode rows, one per slot in slot order, then the prompt chunks.  Its
       descriptor (:meth:`write_step`), written to the device in one copy, holds the token ids, ``cu_q`` (the
       sequences' token offsets: the decode rows are sequences of one token), ``past`` (the rows each holds), one
@@ -821,11 +826,15 @@ class RaggedPagedKVCache(StaticKVCache):
     """
 
     def __init__(self, num_layers: int, max_batch: int, heads: int, head_dim: int, num_pages: int, max_pages: int,
-                 max_tokens: int, dtype=torch.bfloat16, device=None, layers: Optional[Iterable[int]] = None):
+                 max_tokens: int, dtype=torch.bfloat16, device=None, layers: Optional[Iterable[int]] = None,
+                 kv_dtype=None):
         self.num_layers, self.heads, self.head_dim = num_layers, heads, head_dim
-        self.dtype, self.kv_dtype = dtype, dtype
+        self.dtype = dtype
+        self.kv_dtype = dtype if kv_dtype is None else kv_dtype
+        if self.kv_dtype not in (dtype, torch.float8_e4m3fn):
+            raise ValueError(f"kv_dtype must be the projections' {dtype} or torch.float8_e4m3fn, got {kv_dtype}")
         self.device = torch.device(device) if device is not None else torch.device("cpu")
-        self.fp8 = False
+        self.fp8 = self.kv_dtype == torch.float8_e4m3fn
         self.owned = sorted(range(num_layers) if layers is None else layers)
         self.max_batch, self.max_pages, self.max_tokens = max_batch, max_pages, max_tokens
         self.num_pages, self.sink = num_pages, num_pages
@@ -837,8 +846,11 @@ class RaggedPagedKVCache(StaticKVCache):
         self.v_scale: List[Optional[torch.Tensor]] = [None] * num_layers
         for i in self.owned:
             # uninitialised: the kernels read the rows of each sequence's window only
-            self.k[i], self.v[i] = (torch.empty(num_pages + 1, heads, P, head_dim, dtype=dtype, device=self.device)
-                                    for _ in range(2))
+            self.k[i], self.v[i] = (torch.empty(num_pages + 1, heads, P, head_dim, dtype=self.kv_dtype,
+                                                device=self.device) for _ in range(2))
+            if self.fp8:
+                self.k_scale[i], self.v_scale[i] = (torch.empty(num_pages + 1, heads, P, dtype=torch.float32,
+                                                                device=self.device) for _ in range(2))
         self.refs = [0] * num_pages
         self.free = list(range(num_pages - 1, -1, -1))   # pages are taken from the end: 0, 1, 2, ...
         self.prefix = PrefixIndex()
@@ -980,7 +992,9 @@ class RaggedPagedKVCache(StaticKVCache):
 
     # ---- the StaticKVCache protocol of a model's cached step --------------------------------------------------------
     def flash_attention(self) -> bool:
-        return OF.attention_paged_supported(torch.empty(1, dtype=self.dtype, device=self.device), self.k[self.owned[0]])
+        """Whether the native kernels run: the decode rows through the paged decode kernel, the prompt chunks through
+        the ragged paged flash prefill (bf16 or FP8 pools)."""
+        return OF._decode_native(torch.empty(1, dtype=self.dtype, device=self.device), self.k[self.owned[0]])
 
     def advance(self, n: int) -> None:
         self.length += n

@@ -1434,7 +1434,7 @@ def varlen_tiles(q_lens, past=None) -> torch.Tensor:
 
 
 def attention_paged_varlen(q, k_pool, v_pool, block_table, cu_q, past, tiles=None, *, scale: float,
-                           alibi_slopes=None):
+                           alibi_slopes=None, k_scale=None, v_scale=None):
     """Causal attention of ``N`` ragged sequences packed in ``q [T, a, d]`` over their rows of a paged cache's pools
     ``[P, g, 64, d]``: sequence ``n`` owns rows ``cu_q[n] .. cu_q[n + 1]`` of q (int32 ``[N + 1]``, from 0 to T) and
     holds ``past[n]`` rows (int32 ``[N]``) before them in row ``n`` of ``block_table`` ``[N, max_pages]``; its query
@@ -1444,22 +1444,36 @@ def attention_paged_varlen(q, k_pool, v_pool, block_table, cu_q, past, tiles=Non
     a sequence, query head) of ``tiles`` (int32 ``[n, 2]`` on q's device, :func:`varlen_tiles`; built here, with a host
     sync, when None); each sequence's rows are bit for bit those of :func:`attention_paged` on that sequence alone.
     Rows of a page past a sequence's window never reach P·V, whatever they hold.  Elsewhere the reference math per
-    sequence (:func:`attention_paged_varlen_ref`)."""
-    if attention_paged_supported(q, k_pool):
+    sequence (:func:`attention_paged_varlen_ref`).
+
+    FP8 pools (``float8_e4m3fn``) take their row scales ``k_scale``, ``v_scale`` (fp32 ``[P, g, 64]``); the attention
+    is that over the dequantized rows (:func:`kv_cache_dequant`).  On the GPU the FP8 instances of the same kernel
+    dequantize the pages in shared memory, and each sequence's rows are bit for bit this op's over the bf16 pools
+    ``kv_cache_dequant(pool, scale)``."""
+    _check_scales(k_pool, k_scale, v_scale)
+    fp8 = k_scale is not None
+    if _decode_native(q, k_pool):
         if tiles is None:
             tiles = varlen_tiles(cu_q.diff().tolist(), past.tolist()).to(q.device)
-        o = load_ext().attn_fwd_paged_varlen(q, k_pool, v_pool, block_table, cu_q, past, tiles, float(scale),
-                                             alibi_slopes)
+        ext = load_ext()
+        if fp8:
+            o = ext.attn_fwd_paged_varlen_fp8(q, k_pool, v_pool, k_scale, v_scale, block_table, cu_q, past, tiles,
+                                              float(scale), alibi_slopes)
+        else:
+            o = ext.attn_fwd_paged_varlen(q, k_pool, v_pool, block_table, cu_q, past, tiles, float(scale),
+                                          alibi_slopes)
         count_launch()
         return o
     return attention_paged_varlen_ref(q, k_pool, v_pool, block_table, cu_q, past, scale=scale,
-                                      alibi_slopes=alibi_slopes)
+                                      alibi_slopes=alibi_slopes, k_scale=k_scale, v_scale=v_scale)
 
 
-def attention_paged_varlen_ref(q, k_pool, v_pool, block_table, cu_q, past, *, scale: float, alibi_slopes=None):
+def attention_paged_varlen_ref(q, k_pool, v_pool, block_table, cu_q, past, *, scale: float, alibi_slopes=None,
+                               k_scale=None, v_scale=None):
     """:func:`attention_paged_varlen` by the reference math: per sequence, its rows ``[:past[n] + s_n]`` gathered
-    through its table row, then :func:`attention_ref` (causal, bottom-right aligned, with the ALiBi bias
-    ``slope_h·(j − past[n] − i)``)."""
+    through its table row (and dequantized to q's dtype for FP8 pools), then :func:`attention_ref` (causal,
+    bottom-right aligned, with the ALiBi bias ``slope_h·(j − past[n] − i)``)."""
+    _check_scales(k_pool, k_scale, v_scale)
     cu, pa = [int(x) for x in cu_q.tolist()], [int(x) for x in past.tolist()]
     o = torch.zeros_like(q)
     for n in range(len(pa)):
@@ -1469,6 +1483,9 @@ def attention_paged_varlen_ref(q, k_pool, v_pool, block_table, cu_q, past, *, sc
         L = pa[n] + s
         k = kv_pages_gather(k_pool, block_table[n : n + 1], L)
         v = kv_pages_gather(v_pool, block_table[n : n + 1], L)
+        if k_scale is not None:
+            k = kv_cache_dequant(k, kv_pages_gather(k_scale, block_table[n : n + 1], L), q.dtype)
+            v = kv_cache_dequant(v, kv_pages_gather(v_scale, block_table[n : n + 1], L), q.dtype)
         qn = q[cu[n] : cu[n + 1]].transpose(0, 1)[None]   # [1, a, s, d]
         bias = None
         if alibi_slopes is not None:
@@ -1479,28 +1496,38 @@ def attention_paged_varlen_ref(q, k_pool, v_pool, block_table, cu_q, past, *, sc
     return o
 
 
-def kv_cache_append_paged_varlen(qkv, k_pool, v_pool, block_table, cu_q, past, cos=None, sin=None):
+def kv_cache_append_paged_varlen(qkv, k_pool, v_pool, block_table, cu_q, past, cos=None, sin=None, k_scale=None,
+                                 v_scale=None):
     """Write k, v of the packed projection ``qkv`` (``[1, T, a, 3d]`` or ``[1, T, g, r + 2, d]``) of ``N`` ragged
     sequences into a paged cache's pools ``[P, g, 64, d]``: token ``t`` of sequence ``n`` (``cu_q[n] <= t < cu_q[n +
     1]``, int32 ``[N + 1]`` from 0 to T) at its logical row ``past[n] + t − cu_q[n]`` of row ``n`` of ``block_table``
     ``[N, max_pages]``, q and k rotated at that position by ``cos/sin`` when given.  Returns q ``[1, T, a, d]``.  On
-    the GPU one launch of the ragged bf16 append, whose bytes are :func:`kv_cache_append`'s per sequence; elsewhere
-    :func:`kv_cache_append_ref` per sequence."""
-    if attention_paged_supported(qkv, k_pool) and (cos is None or cos.dtype == torch.float32):
+    the GPU one launch of the ragged append, whose bytes are :func:`kv_cache_append`'s per sequence; elsewhere
+    :func:`kv_cache_append_ref` per sequence.  FP8 pools (``float8_e4m3fn``) take their row scales ``k_scale``,
+    ``v_scale`` (fp32 ``[P, g, 64]``) and store each row quantized, bytes and scales those of :func:`kv_cache_append`
+    per sequence."""
+    _check_scales(k_pool, k_scale, v_scale)
+    if _decode_native(qkv, k_pool) and (cos is None or cos.dtype == torch.float32):
         qkv = qkv if qkv.is_contiguous() else qkv.contiguous()
-        q = load_ext().kv_append_paged_varlen(qkv, k_pool, v_pool, block_table, cu_q, past, cos, sin, True)
+        ext = load_ext()
+        if k_scale is not None:
+            q = ext.kv_append_fp8_paged_varlen(qkv, k_pool, v_pool, k_scale, v_scale, block_table, cu_q, past, cos,
+                                               sin, True)
+        else:
+            q = ext.kv_append_paged_varlen(qkv, k_pool, v_pool, block_table, cu_q, past, cos, sin, True)
         count_launch()
         return q
-    return kv_cache_append_paged_varlen_ref(qkv, k_pool, v_pool, block_table, cu_q, past, cos, sin)
+    return kv_cache_append_paged_varlen_ref(qkv, k_pool, v_pool, block_table, cu_q, past, cos, sin, k_scale, v_scale)
 
 
-def kv_cache_append_paged_varlen_ref(qkv, k_pool, v_pool, block_table, cu_q, past, cos=None, sin=None):
+def kv_cache_append_paged_varlen_ref(qkv, k_pool, v_pool, block_table, cu_q, past, cos=None, sin=None, k_scale=None,
+                                     v_scale=None):
     cu, pa = [int(x) for x in cu_q.tolist()], past.to(torch.int32)
     qs = []
     for n in range(len(cu) - 1):
         if cu[n + 1] > cu[n]:
             qs.append(kv_cache_append_ref(qkv[:, cu[n] : cu[n + 1]], k_pool, v_pool, pa[n : n + 1], cos, sin,
-                                          block_table=block_table[n : n + 1]))
+                                          k_scale, v_scale, block_table=block_table[n : n + 1]))
     return torch.cat(qs, dim=1)
 
 
